@@ -11,7 +11,13 @@ process so that the driver's records cover them:
   configs[3]  LMPC Monte-Carlo rollouts, 8192 controllers per GPU, device-resident closed loop, pooled safe-set exchange with
               one NCCL all-gather per lap (benchmarks/rollout_mc.py).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--config 1|2|3]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--config 1|2|3] [--dump-outputs DIR]
+
+`--dump-outputs DIR` writes, after the timed steps, what each leg that runs computed last, as DIR/<name>.npy in float64 (rank 0;
+under 16 MB): the last timed configs[1] step (xPred, uPred, status, iters, resid), the last timed configs[2] step (lmpc_*: the
+shifted predictions, terminal point, applied input and solver report), the end state of the configs[3] closed loop (rollout_*) and,
+with --impl reference, the last timed pass of the CPU arm (reference_z, reference_status, reference_iters).  Inputs are seeded, so
+two builds run with the same arguments can be compared output for output.
 
 Under torchrun (N > 1) every rank owns its own batch on its own GPU (weak scaling; instances are independent — SURVEY §8e);
 timing is CUDA events on the launching stream, max over ranks.  `--impl reference` times the CPU oracle
@@ -50,6 +56,7 @@ FLOPS_PER_ITER = 12 * 2 * (288 + 216 + 126 + 72 + 36 + 48) + 4 * 12 * 2 * 126 + 
 FLOPS_PER_ITER_LMPC = FLOPS_PER_ITER + 2 * 48 * (21 + 6 * 6) + 2000       # + simplex terminal block (W assembly, recoveries)
 # fp64 tensor-core instructions issued per iteration: 12 stages x (11 factor + 4 corrector gradient + 2 x 4 forward)
 DMMA_PER_ITER = 12 * (11 + 4 + 8) + 2 * 6 + 2 * 2     # sweeps per stage + stage-gradient / right-hand-side tiles of 8 stages
+HBM_DATASHEET_GBS = 3350.0   # H100 SXM data sheet (HBM3); the roofline uses MEASURED_PEAKS.json's hbm_gbs when the host provides it
 
 
 def dist_env():
@@ -60,7 +67,7 @@ def dist_env():
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -130,13 +137,16 @@ def oracle_problem_set(nsample, seed=1):
     return patP, patA, Px, np.stack(qs), Ax, np.stack(ls), np.stack(us)
 
 
-def oracle_pass(prob, nthreads):
-    """One pass of the CPU arm over the sample: (seconds, solved, mean ADMM iterations)."""
+def oracle_pass(prob, nthreads, outputs=None):
+    """One pass of the CPU arm over the sample: (seconds, solved, mean ADMM iterations).  outputs: None, or a dict that receives
+    the pass's solutions z[nsample, 126] (OSQP decision vector), status and ADMM iterations."""
     from oracle import osqp_port
     patP, patA, Px, q, Ax, l, u = prob
     t0 = time.perf_counter()
-    _, infos, _ = osqp_port.solve_batch(patP, patA, Px, q, Ax, l, u, nthreads=nthreads)
+    z, infos, _ = osqp_port.solve_batch(patP, patA, Px, q, Ax, l, u, nthreads=nthreads)
     dt = time.perf_counter() - t0
+    if outputs is not None:
+        outputs.update(z=z, status=np.array([i["status"] for i in infos]), iters=np.array([i["iters"] for i in infos]))
     return dt, sum(1 for i in infos if i["status"] == 1), float(np.mean([i["iters"] for i in infos]))
 
 
@@ -229,10 +239,12 @@ def run_reference(args):
     n, _ = cpu_threads()
     for _ in range(args.warmup):
         oracle_pass(prob, n)
+    outputs = {}
     t0 = time.perf_counter()
-    for _ in range(args.steps):
-        oracle_pass(prob, n)
+    for i in range(args.steps):
+        oracle_pass(prob, n, outputs if i == args.steps - 1 else None)
     dt = time.perf_counter() - t0
+    dump_outputs(args.dump_outputs, outputs, prefix="reference_")
     arm = cpu_arm(prob)
     val = CPU_SAMPLE * args.steps / dt
     print(json.dumps({
@@ -304,7 +316,7 @@ def leg_config1(args, rank, world, local, dev):
     d_st = torch.zeros(B, dtype=torch.int32, device=dev)
     d_it = torch.zeros(B, dtype=torch.int32, device=dev)
     d_rs = torch.zeros(B, 3, dtype=torch.float64, device=dev)
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)   # > 50 MB L2 of the H100
     torch.cuda.synchronize()
 
     def step_dev():
@@ -341,6 +353,7 @@ def leg_config1(args, rank, world, local, dev):
     step_ms = [a.elapsed_time(b) for a, b in ev]
     total_ms = _max_over_ranks(sum(step_ms), dev, world)
     status, iters, resid = d_st.cpu().numpy(), d_it.cpu().numpy(), d_rs.cpu().numpy()
+    outputs = dict(xPred=d_xP.cpu().numpy(), uPred=d_uP.cpu().numpy(), status=status, iters=iters, resid=resid)
     # nvidia-smi polling takes driver locks that stall cudaMemcpyAsync enqueues: the sampler covers the device-timed region
     # only and is stopped before the host-timed leg (measured: 2.6-3.4 M/s with it running, 3.9 M/s without)
     clocks = sampler.stop() if rank == 0 else None
@@ -376,7 +389,7 @@ def leg_config1(args, rank, world, local, dev):
     late = solver.late_accepts
     solver.close()
     return dict(B=B, total_ms=total_ms, step_ms=step_ms, launches=int(launches), status=status, iters=iters, resid=resid, clocks=clocks,
-                e2e_s=e2e_s, h2d=int(h_x0.nbytes + h_u.nbytes + h_abc.nbytes),
+                outputs=outputs, e2e_s=e2e_s, h2d=int(h_x0.nbytes + h_u.nbytes + h_abc.nbytes),
                 d2h=int(sum(out[k].nbytes for k in ("xPred", "uPred", "slack", "status", "iters", "resid"))), late=late)
 
 
@@ -422,6 +435,9 @@ def leg_config2(args, rank, world, local, dev, steps=None, with_e2e=True):
     torch.cuda.synchronize()
     step_ms = [a.elapsed_time(b) for a, b in ev]
     tot = _max_over_ranks(sum(step_ms), dev, world)
+    # what a caller of step_dev reads back: the shifted predictions, the terminal point, the applied input, the solver report
+    outputs = {k: v for k, v in c.get_state().items() if k != "timeStep"}
+    outputs.update(c.step_results())
     # per-kernel durations (CUDA events between the four launches of one step, L2 flushed, median of a few steps)
     kms = []
     for _ in range(5):
@@ -454,13 +470,22 @@ def leg_config2(args, rank, world, local, dev, steps=None, with_e2e=True):
     late = c.late_accepts
     c.close()
     return dict(B=B, steps=steps, total_ms=tot, launches=int(launches), kernel_ms=[float(v) for v in kms], ok=ok, iters=res["iters"],
-                rows_model=rows_model, rows_ss=rows_ss, e2e=e2e, data=data, late=late)
+                rows_model=rows_model, rows_ss=rows_ss, e2e=e2e, data=data, late=late, outputs=outputs)
+
+
+def dump_outputs(dirname, outputs, prefix=""):
+    """DIR/<prefix><name>.npy in float64 (integer status / iteration arrays widened exactly)."""
+    if not dirname:
+        return
+    os.makedirs(dirname, exist_ok=True)
+    for k, v in outputs.items():
+        np.save(os.path.join(dirname, prefix + k + ".npy"), np.ascontiguousarray(v, dtype=np.float64))
 
 
 def config2_block(r, world, probe, peaks):
     """JSON block of the configs[2] leg with per-kernel rooflines."""
     B = r["B"]
-    hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
+    hbm_peak = float(peaks.get("hbm_gbs", HBM_DATASHEET_GBS))
     k1, k2, qp, sh = r["kernel_ms"]
     k1_bytes = B * r["rows_model"] * 64.0                      # one pass over the used laps: x (48 B) + u (16 B) per stored row
     k2_bytes = B * r["rows_ss"] * 48.0                         # one pass over the states of the numSS_it fastest laps
@@ -509,7 +534,7 @@ def run_gpu(args):
         kern_ms = float(np.mean(r1["step_ms"]))                 # one kernel per step: launch duration == step duration
         tflops = float(np.sum(iters + 1)) * FLOPS_PER_ITER / (kern_ms * 1e-3) / 1e12
         issued = float(np.sum(iters + 1)) * DMMA_PER_ITER * 512 / (kern_ms * 1e-3) / 1e12
-        hbm_peak = float(peaks.get("hbm_gbs", 6650.0))
+        hbm_peak = float(peaks.get("hbm_gbs", HBM_DATASHEET_GBS))
         hbm_ach = B * ALGO_BYTES_PER_SOLVE / (kern_ms * 1e-3) / 1e9
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
@@ -536,14 +561,18 @@ def run_gpu(args):
                          "issued_tflops": issued, "issued_frac": issued / probe["dmma_tflops"], "fp64_probe": probe,
                          "hbm": {"achieved": hbm_ach, "peak": hbm_peak, "unit": "GB/s", "frac": hbm_ach / hbm_peak,
                                  "algorithmic_bytes_per_solve": ALGO_BYTES_PER_SOLVE,
-                                 "peak_source": "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6.65 TB/s"}},
+                                 "peak_source": "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "H100 SXM data sheet, 3.35 TB/s"}},
         }
+        dump_outputs(args.dump_outputs, r1["outputs"])
     # ---- the other BASELINE configurations, same process, all ranks (weak scaling: every rank its own batch)
     if not args.headline_only:
-        r2 = leg_config2(args, rank, world, local, dev, steps=max(3, min(args.steps, 10)))
+        r2 = leg_config2(args, rank, world, local, dev)
         from benchmarks import rollout_mc
-        r3 = rollout_mc.run(batch=args.rollout_batch, laps=3, mode="pooled", share=2, local=local)
+        final = {}
+        r3 = rollout_mc.run(batch=args.rollout_batch, laps=3, mode="pooled", share=2, local=local, final=final)
         if rank == 0:
+            dump_outputs(args.dump_outputs, r2["outputs"], prefix="lmpc_")
+            dump_outputs(args.dump_outputs, final, prefix="rollout_")
             r3["workload"] = ("configs[3]: LMPC Monte-Carlo rollouts, %d controllers per GPU x %d GPUs, device-resident closed loop (main.py's "
                               "PID lap -> seeding -> 3 LMPC laps), pooled safe-set exchange: one NCCL all-gather per lap" % (args.rollout_batch, world))
             line["configs"] = {"configs[2]": config2_block(r2, world, probe, peaks), "configs[3]": r3}
@@ -571,6 +600,7 @@ def run_lmpc_steps(args):
     r = leg_config2(args, rank, world, local, dev)
     clocks = sampler.stop() if rank == 0 else None
     if rank == 0:
+        dump_outputs(args.dump_outputs, r["outputs"], prefix="lmpc_")
         blk = config2_block(r, world, _native.probe_fp64(local), _peaks())
         ms = blk["ms_per_step"]
         line = {"metric": METRIC, "value": blk["value"], "unit": UNIT, "n_gpus": world, "steps": r["steps"], "warmup": max(args.warmup, 3),
@@ -596,8 +626,10 @@ def run_rollouts(args):
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     torch.cuda.set_device(local)
-    r = rollout_mc.run(batch=args.rollout_batch, laps=3, mode="pooled", share=2, local=local)
+    final = {}
+    r = rollout_mc.run(batch=args.rollout_batch, laps=3, mode="pooled", share=2, local=local, final=final)
     if rank == 0:
+        dump_outputs(args.dump_outputs, final, prefix="rollout_")
         print(json.dumps({"metric": "LMPC closed-loop controller steps/sec (configs[3])", "value": r["controller_steps_per_s"], "unit": "steps/s",
                           "n_gpus": world, "steps": r["closed_loop_steps"], "warmup": 0, "ms_per_step": r["ms_total"] / r["closed_loop_steps"],
                           "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f64", "data": "synthetic",
@@ -650,7 +682,11 @@ def main():
                          "1 = configs[1] only; 2 = batch=4096 full LMPC steps as its own line; 3 = Monte-Carlo rollouts as its own line")
     ap.add_argument("--batch", type=int, default=BATCH)
     ap.add_argument("--rollout-batch", type=int, default=8192, help="controllers per GPU of the configs[3] leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the timed legs computed last as DIR/<name>.npy (float64): configs[1] (no prefix), configs[2] (lmpc_), configs[3] end state (rollout_), --impl reference (reference_)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
     cpu_threads()                 # read the affinity mask before any OpenMP runtime pins this thread
     if args.config == 1:
         args.headline_only = True

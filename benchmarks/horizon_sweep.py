@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""BASELINE.json configs[4]: horizon sweep N in {6,12,24,48}, batch=16384 LTV-MPC QPs on one B200.
+"""BASELINE.json configs[4]: horizon sweep N in {6,12,24,48}, batch=16384 LTV-MPC QPs on one H100.
 
 Reports, per horizon: solves/s (device-resident inputs, CUDA events on the launching stream), interior-point
 iterations to (r_prim, r_dual <= 1e-8, gap <= 1e-11) and, on a 64-instance sample, the iterations the OSQP-algorithm

@@ -35,8 +35,10 @@ from racinglmpc_b200 import workloads, sharding, reference_params as rp      # n
 from racinglmpc_b200.controller import BatchedController                      # noqa: E402
 
 
-def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, poll=8, max_steps=0, seed=1234, local=None, warm=False):
-    """One Monte-Carlo run on this rank's GPU (torch.distributed may or may not be initialised).  Returns a dict (all ranks)."""
+def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, poll=8, max_steps=0, seed=1234, local=None, warm=False,
+        final=None):
+    """One Monte-Carlo run on this rank's GPU (torch.distributed may or may not be initialised).  Returns a dict (all ranks).
+    final: None, or a dict that receives the closed loop's end state (rollout_state) and the last step's solver report (step_results)."""
     rank = dist.get_rank() if dist.is_initialized() else 0
     world = dist.get_world_size() if dist.is_initialized() else 1
     local = int(os.environ.get("LOCAL_RANK", 0)) if local is None else local
@@ -124,6 +126,9 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
            "ipm_iters_mean_sampled": it_sum / max(it_n, 1), "ipm_iters_max_sampled": it_max,
            "instances_with_flags_rank0": int((flags_or != 0).sum()), "flag_bits_rank0": int(np.bitwise_or.reduce(flags_or)),
            "unsolved_steps_rank0": int(unsolved.sum()), "late_accepts_rank0": c.late_accepts}
+    if final is not None:
+        final.update(c.rollout_state())
+        final.update(c.step_results())
     c.close()
     return out
 

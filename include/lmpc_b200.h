@@ -1,4 +1,4 @@
-/* include/lmpc_b200.h — C ABI of liblmpc_b200.so (B200 / sm_100a batched LMPC hot path).
+/* include/lmpc_b200.h — C ABI of liblmpc_b200.so (H100 / sm_90a batched LMPC hot path).
  *
  * The reference (urosolia/RacingLMPC) is pure Python and has no FFI; its drop-in boundary is the
  * duck-typed controller protocol  solve(x0) / addPoint(x,u) / addTrajectory(x,u,x_glob)  with results
@@ -22,7 +22,7 @@ extern "C" {
 #define LMPC_OK 0
 #define LMPC_E_INVALID -1      /* bad argument / unsupported size                     */
 #define LMPC_E_CUDA -2         /* CUDA runtime error (lmpc_last_error() has the text) */
-#define LMPC_E_NODEVICE -3     /* no sm_100-class device available                    */
+#define LMPC_E_NODEVICE -3     /* no sm_90 (H100-class) device available              */
 #define LMPC_E_STATE -4        /* call sequence error (e.g. solve before addTrajectory) */
 
 /* per-instance solver status written to status[] (racinglmpc_b200/csrc/ftocp_pdip.cuh) */
@@ -96,7 +96,8 @@ long long lmpc_late_accepts(lmpc_handle* h);
  * (/sys/bus/pci/devices/<bus id>/numa_node; an anonymous mapping bound with mbind(MPOL_PREFERRED), touched, then pinned with
  * cudaHostRegister), which is what a single DMA stream needs to run at link rate on a multi-socket host; zero-filled.
  * lmpc_host_numa_node: that node, -1 = unknown / switched off with LMPC_B200_NUMA=off (LMPC_B200_NUMA=<n> forces node n).
- * lmpc_host_page_nodes: node of n (<= 64) evenly sampled pages of a block (diagnostics).  Plain pinned or pageable arrays remain
+ * lmpc_host_page_nodes: node of n (<= 64) evenly sampled pages of a block (diagnostics; -1 = unknown, on hosts that forbid the
+ * move_pages query).  Plain pinned or pageable arrays remain
  * valid arguments of every entry point. */
 int lmpc_host_alloc(int device, size_t bytes, void** out);
 int lmpc_host_free(void* p);

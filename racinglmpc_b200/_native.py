@@ -1,6 +1,6 @@
 """ctypes binding of liblmpc_b200.so (C ABI: include/lmpc_b200.h).
 
-There is NO fallback: if the library is missing or no B200-class device is present, importing the
+There is NO fallback: if the library is missing or no H100-class (sm_90) device is present, importing the
 controllers works but constructing one raises (the product path never routes through the CPU oracle).
 """
 import ctypes as C
@@ -46,7 +46,7 @@ def lib():
         return _LIB
     if not os.path.exists(_SO):
         raise NativeError("racinglmpc_b200: %s not found — run `python -c \"import __graft_entry__ as g; g.build()\"` "
-                          "(nvcc, sm_100a).  There is no CPU fallback." % _SO)
+                          "(nvcc, sm_90a).  There is no CPU fallback." % _SO)
     L = C.CDLL(_SO)
     L.lmpc_last_error.restype = C.c_char_p
     L.lmpc_device_count.restype = C.c_int

@@ -1,16 +1,18 @@
-"""In-tree build of liblmpc_b200.so (nvcc, sm_100a only).  No JIT cache: the .so sits next to this
-file so that it travels with the repository snapshot to the GPU box."""
+"""In-tree build of liblmpc_b200.so (nvcc, sm_90a only).  No JIT cache: the .so sits next to this
+file, inside the package, so that the package imports from the repository tree."""
 import os
+import shutil
 import subprocess
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "csrc", "lmpc_b200.cu")
 DEPS = [SRC] + [os.path.join(HERE, "csrc", f) for f in ("ftocp_pdip.cuh", "safeset.cuh", "lapbooks.cuh", "probe.cuh")] + \
-       [os.path.join(HERE, "..", "include", "lmpc_b200.h")]
+       [os.path.join(HERE, "..", "include", "lmpc_b200.h"), os.path.abspath(__file__)]   # this file holds the architecture flags
 OUT = os.path.join(HERE, "liblmpc_b200.so")
-NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
-         "-Xcompiler", "-fPIC", "-shared", "-ccbin", "/usr/bin/g++"]
+CUDA_HOME = os.environ.get("CUDA_HOME", "/usr/local/cuda")
+NVCC = os.environ.get("NVCC", os.path.join(CUDA_HOME, "bin", "nvcc"))
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]      # H100 (Hopper); the kernels use sm_90 PTX (cp.async.bulk, mbarrier)
+FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC", "-shared"]
 
 
 def stale():
@@ -23,7 +25,8 @@ def stale():
 def build_native(force=False, verbose=False):
     if not force and not stale():
         return OUT
-    cmd = [NVCC] + FLAGS + (["-Xptxas", "-v"] if verbose else []) + ["-o", OUT, SRC]
+    cxx = shutil.which("g++")
+    cmd = [NVCC] + FLAGS + (["-ccbin", cxx] if cxx else []) + (["-Xptxas", "-v"] if verbose else []) + ["-o", OUT, SRC]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError("nvcc failed:\n" + r.stdout)

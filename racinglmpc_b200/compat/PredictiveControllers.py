@@ -5,7 +5,7 @@ liblmpc_b200.so through racinglmpc_b200.controller (one instance of the batched 
 Reference call sites this satisfies: Simulator.sim (SysModel.py:34-38: ``solve(x)``, ``uPred[0,:]``,
 ``addPoint(x,u)``), main.py:76-120 (parameter assignment, ``addTrajectory``, ``Qfun[it][0]``) and plot.py
 (``SS, uSS, SS_glob, Qfun, LapTime, it, N, numSS_Points, xStoredPredTraj, SSStoredPredTraj``).
-There is no CPU fallback: without the CUDA library / a B200 the constructors raise.
+There is no CPU fallback: without the CUDA library / an H100 the constructors raise.
 """
 import datetime
 import os

@@ -1,4 +1,4 @@
-// racinglmpc_b200/csrc/lmpc_b200.cu — kernels + C ABI (include/lmpc_b200.h) for sm_100a.
+// racinglmpc_b200/csrc/lmpc_b200.cu — kernels + C ABI (include/lmpc_b200.h) for sm_90a (H100).
 //
 // K3/K4/K5 of SURVEY §2.3 fused in one kernel: one warp (= one 32-thread CTA) per FTOCP instance.
 //   load   : stage model (A_k,B_k,C_k) and the selected safe set are staged into shared memory with
@@ -6,7 +6,8 @@
 //   solve  : racinglmpc_b200/csrc/ftocp_pdip.cuh (Mehrotra PDIP + Riccati, fp64, all in smem/registers)
 //   unpack : xPred/uPred/lambd/slack + zt = Succ_SS lam, zt_u = Succ_uSS lam
 //            (PredictiveControllers.py:364-384), coalesced stores
-// No tensor cores: the largest contraction is 6x6x8 in fp64 (tcgen05 has no f64 kind) — see DESIGN.md.
+// Tensor cores only through the warp-level fp64 MMA (mma.sync.m8n8k4.f64): the largest contraction is 6x6x8 in fp64 and
+// wgmma has no f64 type — see DESIGN.md.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string.h>
@@ -15,6 +16,7 @@
 #include <string>
 #include <new>
 #include <ctype.h>
+#include <errno.h>
 #include <unistd.h>
 #include <sys/syscall.h>
 #include <sys/mman.h>
@@ -443,10 +445,10 @@ int lmpc_host_numa_node(int device) {
     if (e && isdigit((unsigned char)e[0]) && strcmp(e, "auto")) return atoi(e);
     return gpu_numa_node(device);
 }
-// Measured on the bench hosts (tools/numa_probe.py, profiles/r2h_numa_probe.json): one stream reads such a block at 55 GB/s from
-// either NUMA node, but cudaHostAlloc / torch.pin_memory() buffers -- whose pages the driver allocates, ignoring the caller's
-// memory policy -- at 19-29 GB/s (writes: 55 GB/s both ways).  The placement itself made no difference on these hosts; it is kept
-// because it costs nothing and two-socket hosts with a slower inter-socket link exist.
+// Why a registered anonymous mapping rather than cudaHostAlloc: the driver allocates cudaHostAlloc / torch.pin_memory() pages
+// itself, ignoring the caller's memory policy, and on some two-socket hosts a single DMA stream reads such buffers well below link
+// rate (tools/numa_probe.py measures both allocators on a given host).  The node placement costs nothing and matters on hosts
+// with a slow inter-socket link.
 static std::mutex g_host_mu;
 static std::map<void*, size_t> g_host_blocks;      // base -> mapped bytes
 int lmpc_host_alloc(int device, size_t bytes, void** out) {
@@ -499,8 +501,10 @@ int lmpc_host_page_nodes(const void* p, size_t bytes, int n, int* nodes_out) {
     void* pages[64];
     const size_t ps = 4096, np = bytes / ps > 0 ? bytes / ps : 1;
     for (int i = 0; i < n; ++i) pages[i] = (void*)(((uintptr_t)p & ~(uintptr_t)(ps - 1)) + (np * i / n) * ps);
-    if (syscall(SYS_move_pages, 0, (unsigned long)n, pages, nullptr, nodes_out, 0) != 0)
-        return fail(LMPC_E_STATE, "move_pages query failed");
+    if (syscall(SYS_move_pages, 0, (unsigned long)n, pages, nullptr, nodes_out, 0) != 0) {
+        if (errno != EPERM && errno != ENOSYS) return fail(LMPC_E_STATE, "move_pages query failed");
+        for (int i = 0; i < n; ++i) nodes_out[i] = -1;             // the host forbids the query (e.g. a container's syscall filter)
+    }
     return LMPC_OK;
 #else
     return fail(LMPC_E_STATE, "move_pages is not available");
@@ -518,7 +522,7 @@ int lmpc_create(const lmpc_params* p, int batch, int device, lmpc_handle** out) 
     if (device < 0 || device >= ndev) return fail(LMPC_E_INVALID, "bad device index");
     cudaDeviceProp prop;
     CK(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) return fail(LMPC_E_NODEVICE, "liblmpc_b200 is built for sm_100a only");
+    if (prop.major != 9 || prop.minor != 0) return fail(LMPC_E_NODEVICE, "liblmpc_b200 is built for sm_90a (H100) only");
     lmpc_handle* h = new (std::nothrow) lmpc_handle();
     if (!h) return fail(LMPC_E_INVALID, "out of host memory");
     memset(h, 0, sizeof(*h));

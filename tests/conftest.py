@@ -10,7 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "tests", "support")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu on a machine that has one)")
 
 
 @pytest.fixture(scope="session")

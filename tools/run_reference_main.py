@@ -5,7 +5,7 @@ driven by the drop-in modules of this repository.
 main.py imports its controllers by module name from `fnc/controller` (main.py:24-31), so putting a directory with modules named
 `PredictiveControllers` / `PredictiveModel` earlier on sys.path swaps the implementation.  Two back ends:
 
-  b200     racinglmpc_b200/compat  (ctypes -> liblmpc_b200.so -> CUDA kernels; needs a B200)
+  b200     racinglmpc_b200/compat  (ctypes -> liblmpc_b200.so -> CUDA kernels; needs an H100)
   oracle   tests/support/oracle_compat  (the oracle: reference arithmetic + OSQP-algorithm port at 1e-9; CPU)
 
 Everything else main.py imports (Simulator, Map, PID, Regression, initControllerParameters, plot) is the reference's own code.

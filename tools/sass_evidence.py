@@ -2,7 +2,7 @@
 """tools/sass_evidence.py > profiles/<round>_sass_evidence.md — instruction mix per kernel of the in-tree liblmpc_b200.so
 (cuobjdump -sass): the mnemonics that show what the kernels are built on (DMMA = fp64 tensor-core MMA, UBLKCP = 1-D bulk
 async copy (TMA), REDUX/CREDUX = warp reductions, DFMA/DADD/DMUL = fp64 pipe, MUFU.RSQ64H/RCP64H = the approximations the custom
-rsqrt / reciprocal refine) and what they are NOT (UTMALDG / UTCxMMA / LDTM: no tiled TMA, no tcgen05 -- there is no fp64 kind)."""
+rsqrt / reciprocal refine) and what they are NOT (UTMALDG / HGMMA: no tiled TMA, no wgmma -- it has no fp64 type)."""
 import collections, os, re, subprocess, sys
 root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 so = os.path.join(root, "racinglmpc_b200", "liblmpc_b200.so")
@@ -17,7 +17,7 @@ for line in txt.split("\n"):
     m = re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(?:@!?U?P\d+\s+)?([A-Z0-9_.]+)", line)
     if m and kern:
         mix[kern][m.group(1)] += 1
-keys = ["DMMA", "UBLKCP", "REDUX", "CREDUX", "DFMA", "DADD", "DMUL", "MUFU.RSQ64H", "MUFU.RCP64H", "SHFL", "LDS", "STS", "LDG", "BAR", "UTMALDG", "UTCHMMA", "LDTM"]
+keys = ["DMMA", "UBLKCP", "REDUX", "CREDUX", "DFMA", "DADD", "DMUL", "MUFU.RSQ64H", "MUFU.RCP64H", "SHFL", "LDS", "STS", "LDG", "BAR", "UTMALDG", "HGMMA"]
 print("# SASS instruction mix of liblmpc_b200.so (static counts, `cuobjdump -sass`), arch %s\n" % ", ".join(arch))
 print("| kernel | instructions | " + " | ".join(keys) + " |")
 print("|---|---|" + "---|" * len(keys))
