@@ -247,11 +247,14 @@ struct Work {
     alignas(16) double ru[N][2];      // input-stationarity residual
 #if LMPC_MMA
     // ---- tensor-core formulation of the sweeps: cost-to-go Hessian / gradient live in register fragments; per stage only the
-    //      barrier weights, the stage gradients, the feedback gain, the inverse input Hessian and the feed-forward term are kept
+    //      barrier weights, the stage gradients, the feedback gain (or the closed-loop rows built from it), the inverse input
+    //      Hessian and the feed-forward term are kept
     static_assert(NCX + NCU <= 6, "barrier weights of one stage must fit six entries of one 8-vector");
     alignas(16) double Wd[N][8];    // (Dt[0..NCX) | d2[0..NCU) | 0.. | input-rate weights at 6,7): diagonal of the stage's Fa' W Fa term
     alignas(16) double gv[N][16];   // row 0: stage gradient incl. the eliminated rows' right-hand side; row 1: -(stage gradient)
-    alignas(16) double Kst[N][16];  // K = -Suu^-1 [Sux | -diag(dR2)]  (2 x 8, row major): u_k = K (x_k, u_{k-1}) + f
+    // K = -Suu^-1 [Sux | -diag(dR2)]  (2 x 8, row major): u_k = K (x_k, u_{k-1}) + f.  Closed-loop sweeps (M == 0): K_k A~_{k-1}
+    // instead, rows 6,7 of Phi_k = [A_{k-1} B_{k-1}; K_k A~_{k-1}], which maps (x, u)_{k-1} to (x, u)_k - (0, f_k); Kst[0] unused
+    alignas(16) double Kst[N][16];
     alignas(16) double Sinv[N][4];  // Suu^-1 = (s00, s01, s11, -)
     alignas(16) double fst[N][2];   // f = -Suu^-1 g0 for the current right-hand side
     alignas(16) double tN[8];       // Qf2 x_N + qxN + yT  (= -costate at the end of the horizon)
@@ -1002,7 +1005,16 @@ struct Pdip {
     //   gradient  c_k = M'(A~' c + g_k),   f_k = -Suu^-1 (A~' c + g_k)_u,        g_k = stage gradient + eliminated-row terms,
     //   where c = (cost-to-go gradient) - (costate, 0): the costate recursion pi_k = A' pi - gst_x drops out of the solve and is
     //   only carried (row 1) in the factorising sweep to report the input-stationarity residual ru = gst_u - B' pi.
-    // forward:  (x_k, u_k) = M w_k + (0, f_k),  w_{k+1} = A~ (x_k, u_k).
+    // forward (open loop, M > 0):  (x_k, u_k) = M w_k + (0, f_k),  w_{k+1} = A~ (x_k, u_k).
+    // Closed loop (M == 0): the vector sweeps run on the stage variables z_k = (x_k, u_k) with Phi_k = M_k A~_{k-1} (k >= 1),
+    // one 8 x 8 x 8 product per stage; its rows 0..5 are [A B]_{k-1} as staged, rows 6,7 = K_k A~_{k-1} are stored (Kst):
+    //   backward:  h_{N-1} = A~'_{N-1} c_N + g_{N-1},  h_{k-1} = Phi_k' h_k + g_{k-1}   (h_k = A~' c_{k+1} + g_k, c_k = M' h_k)
+    //   forward:   z_0 = (0, f_0),  z_k = Phi_k z_{k-1} + (0, f_k),  x_N = [A B]_{N-1} z_{N-1}.
+    // Both forms solve the same system; they round differently.  On MPC-type QPs the closed-loop solutions agree with the
+    // open-loop ones to rounding and take the same iterations.  The LMPC terminal block (covariance form, degenerate simplex)
+    // amplifies any reordering of the sweep arithmetic to ~1e-10 in the solution and an iteration more or less on some QPs, and
+    // closed-loop LMPC roll-outs are chaotic, so a kernel with a safe set keeps the open-loop sweeps and its results.
+    static constexpr bool CLOSED = (M == 0);
     struct Frag { double a, b; };
 
     static LMPC_HD void dmma(double& d0, double& d1, double a, double b, double c0, double c1) {
@@ -1061,8 +1073,13 @@ struct Pdip {
         int r, q;
         Off at_a, at_b; int at_step;   // D layout of A~' : (A~[2q][r], A~[2q+1][r]); per-stage step
         Off af; int af_step;           // D layout of A~  : (A~[r][2q], A~[r][2q+1]) as one 16-byte load
+        // open loop (M > 0)
         Off mf; int mf_step;           // D layout of M   : rows 6,7 = K (from Kst), identity elsewhere
         Off mt_a, mt_b; int mt_step;   // D layout of M'  : (M[2q][r], M[2q+1][r]); q == 3 -> (K0[r], K1[r])
+        // closed loop (M == 0): Phi_k (k >= 1) at Phi_1 + (k - 1) * step; rows / columns 0..5 from the stage model of k - 1,
+        // 6,7 from Kst[k]
+        Off pf; int pf_step;           // D layout of Phi : (Phi[r][2q], Phi[r][2q+1]); r >= 6 -> one 16-byte load from Kst
+        Off pt_a, pt_b; int pt_step;   // D layout of Phi': (Phi[2q][r], Phi[2q+1][r]); q == 3 -> (Kst[0][r], Kst[1][r])
         Off cst;                       // the constant block (1,0 | 0,1 | 0,0)
     };
     // base address of the stage model as the sweeps see it.  STREAM: a global pointer made opaque, so that the compiler treats
@@ -1101,7 +1118,7 @@ struct Pdip {
         return lane;
     }
     static LMPC_HD LaneMap lane_map(const W& w, int lane) {
-        LaneMap m;
+        LaneMap m{};
         m.r = lane >> 2;
         m.q = lane & 3;
         const int r = m.r, q = m.q;
@@ -1123,10 +1140,17 @@ struct Pdip {
         }
         if (r < 6) { m.af = abc0 + ((q < 3) ? r * 6 + 2 * q : 36 + 2 * r); m.af_step = stg; }
         else { m.af = cst0 + ((q == 3) ? ((r == 6) ? 0 : 2) : 4); m.af_step = 0; }
-        if (r >= 6) { m.mf = kst0 + (r - 6) * 8 + 2 * q; m.mf_step = 16; }
-        else { m.mf = cst0 + ((r == 2 * q) ? 0 : ((r == 2 * q + 1) ? 2 : 4)); m.mf_step = 0; }
-        if (q == 3) { m.mt_a = kst0 + r; m.mt_b = kst0 + 8 + r; m.mt_step = 16; }
-        else { m.mt_a = cst0 + ((r == 2 * q) ? 0 : 1); m.mt_b = cst0 + ((r == 2 * q + 1) ? 0 : 1); m.mt_step = 0; }
+        if constexpr (CLOSED) {
+            if (r < 6) { m.pf = m.af; m.pf_step = stg; }
+            else { m.pf = kst0 + 16 + (r - 6) * 8 + 2 * q; m.pf_step = 16; }
+            if (q < 3) { m.pt_a = m.at_a; m.pt_b = m.at_b; m.pt_step = stg; }
+            else { m.pt_a = kst0 + 16 + r; m.pt_b = kst0 + 24 + r; m.pt_step = 16; }
+        } else {
+            if (r >= 6) { m.mf = kst0 + (r - 6) * 8 + 2 * q; m.mf_step = 16; }
+            else { m.mf = cst0 + ((r == 2 * q) ? 0 : ((r == 2 * q + 1) ? 2 : 4)); m.mf_step = 0; }
+            if (q == 3) { m.mt_a = kst0 + r; m.mt_b = kst0 + 8 + r; m.mt_step = 16; }
+            else { m.mt_a = cst0 + ((r == 2 * q) ? 0 : 1); m.mt_b = cst0 + ((r == 2 * q + 1) ? 0 : 1); m.mt_step = 0; }
+        }
         return m;
     }
 
@@ -1265,7 +1289,10 @@ struct Pdip {
         const double m_keep = (r < 6 && q < 3) ? 1.0 : 0.0;                   // entries of Sxx
         const double m_q01 = (q < 2) ? 1.0 : 0.0, m_q3 = (q == 3) ? 1.0 : 0.0;
         const double m_ru = (lane == 7) ? 0.0 : 1.0;                          // the costate has no input part
-        const Frag Id = Frag{(q < 3 && r == 2 * q) ? 1.0 : 0.0, (q < 3 && r == 2 * q + 1) ? 1.0 : 0.0};   // M' for q < 3
+        const Frag Id = Frag{(q < 3 && r == 2 * q) ? 1.0 : 0.0, (q < 3 && r == 2 * q + 1) ? 1.0 : 0.0};   // M' for q < 3 (open loop)
+        // closed loop: K in the D layout of M (lane (r >= 6, q): K[r-6][2q], K[r-6][2q+1]): column j of W sits in the lanes 4j..4j+3, and
+        // the lanes with odd q hand out row 1, those with even q row 0
+        const int k_src = 8 * q + (r & 1);
 
         // terminal cost-to-go
         Frag Pf{0.0, 0.0};
@@ -1273,7 +1300,7 @@ struct Pdip {
             Pf.a = c.Qf2[r * 6 + 2 * q] + (LMPC ? w.Wi[(r * 6 + 2 * q) % TMW] : 0.0);
             Pf.b = c.Qf2[r * 6 + 2 * q + 1] + (LMPC ? w.Wi[(r * 6 + 2 * q + 1) % TMW] : 0.0);
         }
-        Frag Vf = terminal_vec<true>(w, c1, r, q);
+        Frag Vf = terminal_vec<true>(w, c1, r, q);      // row vectors of stage k+1: c_N first, then c_{k+1} / (closed loop) h_{k+1}
         bool bad = false;
         // running pointers (stage N-1 first); lanes without a role in a load / store point at the zero constants / a dump slot
         const double* pa = base + lm.at_a + (N - 1) * lm.at_step;
@@ -1286,9 +1313,10 @@ struct Pdip {
         double* pfs = &w.fst[N - 1][0];
         double* pru = &w.ru[N - 1][0];
         Frag At{*pa, *pb_}, Gn = ld2(pg), Wn = ld2(pw);
+        Frag PhT = At;                 // closed loop: D layout of the map of the row vectors, A~'_{N-1} first, then Phi_{k+1}'
 LMPC_SWEEP_UNROLL
         for (int k = N - 1; k >= 0; --k) {
-            const Frag AtF = At, g = Gn, wd = Wn;
+            const Frag AtF = At, g = Gn, wd = Wn, PT = PhT;
             {   // prefetch the next stage's operands (k == 0 re-reads stage 0: no branch, nothing out of bounds)
                 const int st = (k > 0) ? 1 : 0;
                 pa -= st * lm.at_step; pb_ -= st * lm.at_step; pw -= st * 8; pg -= st * g_step;
@@ -1301,8 +1329,8 @@ LMPC_SWEEP_UNROLL
             // ---- S = A~' P A~ + H
             const Frag Gp = prod(AtF, Pf);                 // A~' P   (P symmetric: its D layout is also its transposed layout)
             const Frag S = prod_add(Gp, AtF, Hf);
-            // ---- row vectors: A~' c + g (row 0), A~' pi - gst (row 1); rows 2..7 stay 0
-            const Frag Tv = prod(Vf, AtF);
+            // ---- row vectors: h_k = A~' c + g (= Phi_{k+1}' h_{k+1} + g) (row 0), A~' pi - gst (row 1); rows 2..7 stay 0
+            const Frag Tv = prod(Vf, CLOSED ? PT : AtF);
             const Frag Hraw{Tv.a + g.a, Tv.b + g.b};
             if (lane == 7) st2(pru, -Hraw.a, -Hraw.b);      // ru = gst_u - B' pi
             const Frag Hv{Hraw.a * m_ru, Hraw.b * m_ru};
@@ -1321,7 +1349,7 @@ LMPC_SWEEP_UNROLL
             y1 = fma(m_x, y1, y1c);
             const double w0r = fma(s00, y0, s01 * y1);
             const double w1r = fma(s01, y0, s11 * y1);
-            if (q == 0) { pk[0] = -w0r; pk[8] = -w1r; }
+            const double wq = (q & 1) ? w1r : w0r;
             // ---- feed-forward term f = -Suu^-1 h_u (h_u sits in lane 3)
             if (lane == 3) {
                 st2(psi, s00, s01);
@@ -1329,9 +1357,21 @@ LMPC_SWEEP_UNROLL
                 st2(pfs, -fma(s00, Hv.a, s01 * Hv.b), -fma(s01, Hv.a, s11 * Hv.b));
             }
             // ---- cost-to-go Hessian of stage k as one MMA (summation index 0,1 used: rows of Y and W)
-            dmma(Pf.a, Pf.b, -((q & 1) ? y1 : y0), m_q01 * ((q & 1) ? w1r : w0r), m_keep * S.a, m_keep * S.b);
-            // ---- c_k = M' h (row 0); the costate passes through the identity part (row 1)
-            Vf = prod(Hv, Frag{fma(-m_q3, w0r, Id.a), fma(-m_q3, w1r, Id.b)});
+            dmma(Pf.a, Pf.b, -((q & 1) ? y1 : y0), m_q01 * wq, m_keep * S.a, m_keep * S.b);
+            if constexpr (CLOSED) {
+                // ---- Phi_k' = A~'_{k-1} M_k' (At holds A~_{k-1}; at k == 0 a product that is never read): only the q == 3
+                //      columns (K_k A~_{k-1})' differ from A~'_{k-1}; they are stored for the vector sweeps.  Off the Riccati chain.
+                const Frag WA = prod(At, Frag{bcast(wq, k_src), bcast(wq, k_src + 4)});     // W = -K
+                const Frag KA{-WA.a, -WA.b};
+                if (q == 3) { pk[0] = KA.a; pk[8] = KA.b; }
+                PhT = (q == 3) ? KA : At;
+                // ---- the row vectors go on in h-form: the costate passes through Phi (its input part is zero, row 1)
+                Vf = Hv;
+            } else {
+                if (q == 0) { pk[0] = -w0r; pk[8] = -w1r; }
+                // ---- c_k = M' h (row 0); the costate passes through the identity part (row 1)
+                Vf = prod(Hv, Frag{fma(-m_q3, w0r, Id.a), fma(-m_q3, w1r, Id.b)});
+            }
             pk -= 16; psi -= 4; pfs -= 2; pru -= 2;
         }
         if (bad && lane == 0) w.flag = ST_NUMERICAL;
@@ -1341,8 +1381,97 @@ LMPC_SWEEP_UNROLL
         return wmax_nn(ru_max);
     }
 
-    // Gradient-only backward sweep for a new right-hand side (corrector / recentring): c_k = M'(A~'c + g_k), f_k.
-    static LMPC_HD void backward_rhs(W& w, const FtocpConst& c, const double* c1) {
+    // Closed-loop gradient-only backward sweep for a new right-hand side (corrector / recentring): h_{k-1} = Phi_k' h_k + g_{k-1}, f_k.
+    static LMPC_HD void backward_rhs_closed(W& w, const FtocpConst& c, const double* c1) {
+        const int lane = sweep_lane();
+        const LaneMap lm = lane_map(w, lane);
+        const int r = lm.r, q = lm.q;
+        const double* base = sweep_base(w);
+        Frag Hv = terminal_vec<false>(w, c1, r, q);    // c_N, then h_{k+1}
+        // Phi_{N-1}', Phi_{N-2}', ..., Phi_1' in turn; the pointer stays at stage 1 once there (no read out of bounds)
+        const double* pa = base + lm.pt_a + (N - 2) * lm.pt_step;
+        const double* pb_ = base + lm.pt_b + (N - 2) * lm.pt_step;
+        const double* pg = (lane < 4) ? &w.gv[N - 1][2 * lane] : &w.cst[4];
+        const int g_step = (lane < 4) ? 16 : 0;
+        const double* psi = &w.Sinv[N - 1][0];
+        double* pfs = &w.fst[N - 1][0];
+        Frag Pt{base[lm.at_a + (N - 1) * lm.at_step], base[lm.at_b + (N - 1) * lm.at_step]};   // A~'_{N-1}: c_N enters through A~
+        Frag Gn = ld2(pg), Sn = ld2(psi);
+        Frag Pt2 = Pt;                 // STREAM: the model comes from L2, so its fragments are fetched two stages ahead
+        if constexpr (STREAM) { Pt2 = Frag{*pa, *pb_}; pa -= lm.pt_step; pb_ -= lm.pt_step; }
+        double S2n = psi[2];
+LMPC_SWEEP_UNROLL
+        for (int k = N - 1; k >= 0; --k) {
+            const Frag PT = Pt, g = Gn, s0 = Sn;
+            const double s11 = S2n;
+            {   // prefetch the next stage's operands off the dependent chain (k == 0 re-reads stage 0 / Phi_1')
+                const int st = (k > 0) ? 1 : 0;
+                pg -= st * g_step; psi -= st * 4;
+                if constexpr (STREAM) {
+                    Pt = Pt2;
+                    Pt2 = Frag{*pa, *pb_};                 // Phi_{k-1}'
+                    const int s2 = (k > 2) ? 1 : 0;
+                    pa -= s2 * lm.pt_step; pb_ -= s2 * lm.pt_step;
+                } else {
+                    Pt = Frag{*pa, *pb_};                  // Phi_k'
+                    const int s1 = (k > 1) ? 1 : 0;
+                    pa -= s1 * lm.pt_step; pb_ -= s1 * lm.pt_step;
+                }
+                Gn = ld2(pg);
+                Sn = ld2(psi);
+                S2n = psi[2];
+            }
+            Hv = prod_add(Hv, PT, g);                      // h_k (row 0; other rows 0)
+            if (lane == 3) st2(pfs, -fma(s0.a, Hv.a, s0.b * Hv.b), -fma(s0.b, Hv.a, s11 * Hv.b));
+            pfs -= 2;
+        }
+        wsync();
+    }
+
+    // Closed-loop forward sweep on the stage variables: z_0 = (0, f_0), z_k = Phi_k z_{k-1} + (0, f_k), dx_N = [A B]_{N-1} z_{N-1}.
+    static LMPC_HD void forward_closed(W& w) {
+        const int lane = sweep_lane();
+        const LaneMap lm = lane_map(w, lane);
+        const double* base = sweep_base(w);
+        const double* pp = base + lm.pf;               // Phi_1
+        const double* pc = (lane == 3) ? &w.fst[0][0] : &w.cst[4];
+        const int c_step = (lane == 3) ? 2 : 0;
+        // one store per stage: lanes 0..2 write dx_k, lane 3 writes du_k
+        double* po = (lane < 3) ? &w.dx[2 * lane] : &w.du[0];
+        const int o_step = (lane < 3) ? 6 : 2;
+        Frag Z = ld2(pc);                             // row 0: (dx_0 | du_0) = (0 | f_0)
+        pc += c_step;
+        Frag Pf = ld2(pp), Cf = ld2(pc);
+        Frag Pf2 = Pf;                 // STREAM: two stages ahead (see backward_rhs)
+        if constexpr (STREAM) { pp += ((N > 2) ? 1 : 0) * lm.pf_step; Pf2 = ld2(pp); }
+LMPC_SWEEP_UNROLL
+        for (int k = 1; k < N; ++k) {
+            const Frag PF = Pf, CF = Cf;
+            {   // prefetch the next stage's operands off the dependent chain (the last stage re-reads itself)
+                const int st = (k + 1 < N) ? 1 : 0;
+                pc += st * c_step;
+                if constexpr (STREAM) {
+                    pp += ((k + 2 < N) ? 1 : 0) * lm.pf_step;
+                    Pf = Pf2;
+                    Pf2 = ld2(pp);
+                } else {
+                    pp += st * lm.pf_step;
+                    Pf = ld2(pp);
+                }
+                Cf = ld2(pc);
+            }
+            if (lane < 4) st2(po, Z.a, Z.b);               // z_{k-1}
+            po += o_step;
+            Z = prod_add(Z, PF, CF);                       // row 0: (dx_k | du_k)
+        }
+        if (lane < 4) st2(po, Z.a, Z.b);
+        const Frag X = prod(Z, ld2(base + lm.af + (N - 1) * lm.af_step));     // row 0: (dx_N | du_{N-1})
+        if (lane < 3) st2(&w.dx[N * 6 + 2 * lane], X.a, X.b);
+        wsync();
+    }
+
+    // Open-loop gradient-only backward sweep for a new right-hand side (corrector / recentring): c_k = M'(A~'c + g_k), f_k.
+    static LMPC_HD void backward_rhs_open(W& w, const FtocpConst& c, const double* c1) {
         const int lane = sweep_lane();
         const LaneMap lm = lane_map(w, lane);
         const int r = lm.r, q = lm.q;
@@ -1391,8 +1520,8 @@ LMPC_SWEEP_UNROLL
         wsync();
     }
 
-    // Forward sweep: (dx_k, du_k) = M w_k + (0, f_k), w_{k+1} = A~ (dx_k, du_k), from w_0 = 0.
-    static LMPC_HD void forward(W& w) {
+    // Open-loop forward sweep: (dx_k, du_k) = M w_k + (0, f_k), w_{k+1} = A~ (dx_k, du_k), from w_0 = 0.
+    static LMPC_HD void forward_open(W& w) {
         const int lane = sweep_lane();
         const LaneMap lm = lane_map(w, lane);
         const double* base = sweep_base(w);
@@ -1431,6 +1560,15 @@ LMPC_SWEEP_UNROLL
         }
         if (lane < 3) st2(&w.dx[N * 6 + 2 * lane], Wf.a, Wf.b);
         wsync();
+    }
+
+    static LMPC_HD void backward_rhs(W& w, const FtocpConst& c, const double* c1) {
+        if constexpr (CLOSED) backward_rhs_closed(w, c, c1);
+        else backward_rhs_open(w, c, c1);
+    }
+    static LMPC_HD void forward(W& w) {
+        if constexpr (CLOSED) forward_closed(w);
+        else forward_open(w);
     }
 
     // Model roll-out of a starting point with the inputs in w.u: (x_{k+1} | u_k) = A~ (x_k | u_k) + (C_k | 0)
