@@ -36,9 +36,11 @@ from racinglmpc_b200.controller import BatchedController                      # 
 
 
 def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, poll=8, max_steps=0, seed=1234, local=None, warm=False,
-        final=None):
+        final=None, param_sets=None):
     """One Monte-Carlo run on this rank's GPU (torch.distributed may or may not be initialised).  Returns a dict (all ranks).
-    final: None, or a dict that receives the closed loop's end state (rollout_state) and the last step's solver report (step_results)."""
+    final: None, or a dict that receives the closed loop's end state (rollout_state) and the last step's solver report (step_results).
+    param_sets: None, or (params, index, QterminalSlack) handed to BatchedController.set_param_sets after construction (a
+    parameter sweep over the batch; the result then holds per-set lap statistics under "per_set_rank0")."""
     rank = dist.get_rank() if dist.is_initialized() else 0
     world = dist.get_world_size() if dist.is_initialized() else 1
     local = int(os.environ.get("LOCAL_RANK", 0)) if local is None else local
@@ -48,6 +50,8 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     numSS_it, numSS_Points, _, _, Qts, par = rp.lmpc_params(N)
     c = BatchedController(par, B, workloads.track_seg_table(), rp.TRACK_LENGTH, trToUse=4, numSS_Points=numSS_Points,
                           numSS_it=numSS_it, QterminalSlack=Qts, device=local, Tmax=1280, ss_cap=7, model_cap=5, warm_start=warm)
+    if param_sets is not None:
+        c.set_param_sets(*param_sets)
     stream = torch.cuda.ExternalStream(c.stream, device=dev)
     x0 = np.tile(np.array([0.5, 0, 0, 0, 0, 0.0]), (B, 1))
     # ---- main.py:65-66 + 99-110 on the device: every controller drives its OWN PID lap (the full 100 s) and is seeded with it
@@ -126,11 +130,25 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
            "ipm_iters_mean_sampled": it_sum / max(it_n, 1), "ipm_iters_max_sampled": it_max,
            "instances_with_flags_rank0": int((flags_or != 0).sum()), "flag_bits_rank0": int(np.bitwise_or.reduce(flags_or)),
            "unsolved_steps_rank0": int(unsolved.sum()), "late_accepts_rank0": c.late_accepts}
+    if param_sets is not None:
+        idx = np.asarray(param_sets[1]).reshape(B)
+        out["per_set_rank0"] = [_set_stats(bk, flags_or, unsolved, idx == k, laps) for k in range(len(param_sets[0]))]
     if final is not None:
         final.update(c.rollout_state())
         final.update(c.step_results())
     c.close()
     return out
+
+
+def _set_stats(bk, flags_or, unsolved, sel, laps):
+    """Lap lengths (mean / min per LMPC lap), unsolved steps and flagged controllers of the controllers `sel` of one parameter set."""
+    laps_out = []
+    for r in range(laps):
+        m = sel & (bk["lap_n"] > r)
+        a = bk["lap_hist"][m, r]
+        laps_out.append({"lap": r + 1, "n": int(m.sum()), "mean": float(a.mean()) if a.size else 0.0, "min": int(a.min()) if a.size else 0})
+    return {"controllers": int(sel.sum()), "laps": laps_out, "unsolved_steps": int(unsolved[sel].sum()),
+            "instances_with_flags": int((flags_or[sel] != 0).sum())}
 
 
 def main():

@@ -80,8 +80,26 @@ typedef struct lmpc_handle lmpc_handle;
 const char* lmpc_last_error(void);
 int lmpc_device_count(void);
 
-/* One handle = `batch` independent controllers with identical parameters on one device. */
+/* One handle = `batch` independent controllers on one device, created with identical parameters (see lmpc_set_param_sets for
+ * parameter sweeps in one batch). */
 int lmpc_create(const lmpc_params* p, int batch, int device, lmpc_handle** out);
+/* Per-controller QP parameters (parameter sweeps in one batch; no reference counterpart: the reference runs one controller).
+ * sets[nsets] are full lmpc_params; controller b solves its QPs with sets[set_of_instance[b]] (host array [batch]).  Applies to every
+ * QP the handle solves: the _host / _host_async / _dev entry points, lmpc_step_* and lmpc_rollout_step.  nsets == 0 (sets,
+ * set_of_instance NULL) returns the handle to the parameters it was created with.
+ *   - 1 <= nsets <= batch, every index in [0, nsets).
+ *   - Every set equals the handle's parameters in N, ncx, ncu, numSS_Points, numSS_it and warm_start; all other fields (weights,
+ *     xRef, Fx/bx, Fu/bu, QterminalSlack, tolerances, max_iter) may differ.  Each set is checked and converted as lmpc_create does
+ *     it (bu > 0, invertible QterminalSlack when numSS_Points > 0, values <= 0 select the default tolerances).
+ *   - Any failed check returns LMPC_E_INVALID and leaves the handle as it was.
+ *   - The call synchronises the handle's streams before it replaces the table: batches enqueued earlier (e.g. through the _async
+ *     entry points) complete with the parameters they were enqueued with.
+ *   - It invalidates the warm-start records (lmpc_params.warm_start): the next solve of every controller starts cold.
+ *   - The pooled safe-set exchange (lmpc_pool_*, lmpc_ss_import_laps_dev) still hands laps between all controllers whatever their
+ *     set; a clean sweep (each tuning learning from its own laps only) runs in the independent mode.
+ * A handle with sets installed launches a QP kernel variant that stages the instance's parameter record (1 776 B) in shared
+ * memory next to its stage model (DESIGN.md, "Per-controller parameters"); handles without sets launch the uniform kernel. */
+int lmpc_set_param_sets(lmpc_handle* h, const lmpc_params* sets, int nsets, const int* set_of_instance);
 int lmpc_destroy(lmpc_handle* h);
 int lmpc_sync(lmpc_handle* h);
 void* lmpc_stream(lmpc_handle* h);            /* cudaStream_t the handle enqueues on */

@@ -59,6 +59,7 @@ def lib():
     L.lmpc_kernel_launches.restype = C.c_longlong
     L.lmpc_late_accepts.argtypes = [_vp]
     L.lmpc_late_accepts.restype = C.c_longlong
+    L.lmpc_set_param_sets.argtypes = [_vp, C.POINTER(Params), C.c_int, _vp]
     ll = C.c_longlong
     for name in ("lmpc_solve_mpc_host", "lmpc_solve_mpc_dev"):
         getattr(L, name).argtypes = [_vp, _vp, _vp, _vp, ll, ll, _vp, _vp, _vp, _vp, _vp, _vp]
@@ -247,3 +248,38 @@ def make_params(p, numSS_Points=0, numSS_it=0, QterminalSlack=None, eps_res=0.0,
     q.eps_res, q.eps_gap, q.max_iter, q.eps_step = float(eps_res), float(eps_gap), int(max_iter), float(eps_step)
     q.warm_start = 1 if warm_start else 0
     return q
+
+
+def make_param_sets(base, params, index, batch, numSS_Points=0, numSS_it=0, QterminalSlack=None):
+    """Per-controller parameters for ``lmpc_set_param_sets``: K MPCParams-like objects ``params``, the set of every controller
+    ``index[batch]`` and ``QterminalSlack`` (None: the base's, or one 6x6 matrix per set).  ``base`` is the handle's own ``Params``;
+    the interior-point settings (tolerances, max_iter, warm_start) are taken from it.  Each set is converted by ``make_params``.
+    Raises ValueError where the library would refuse: an index of the wrong length or out of range, or a set that differs from
+    the base in N, the rows of Fx or Fu, slacks or n/d.  Returns (ctypes array Params * K, int32 index array)."""
+    if index is None:
+        raise ValueError("index is required: one set number per controller (%d)" % batch)
+    params = list(params)
+    K = len(params)
+    if not 1 <= K <= batch:
+        raise ValueError("need 1 .. batch (= %d) parameter sets, got %d" % (batch, K))
+    idx = np.ascontiguousarray(np.asarray(index).reshape(-1), dtype=np.int32)
+    if idx.shape[0] != batch or not np.array_equal(idx, np.asarray(index).reshape(-1)):
+        raise ValueError("index must hold one integer set number per controller (%d)" % batch)
+    if idx.min() < 0 or idx.max() >= K:
+        raise ValueError("set index out of range [0, %d)" % K)
+    if QterminalSlack is None:
+        qts = [np.ctypeslib.as_array(base.QterminalSlack).reshape(6, 6).copy()] * K
+    else:
+        qts = list(QterminalSlack)
+        if len(qts) != K:
+            raise ValueError("QterminalSlack needs one matrix per set (%d)" % K)
+    out = (Params * K)()
+    for k, (p, q) in enumerate(zip(params, qts)):
+        s = make_params(p, numSS_Points, numSS_it, q, base.eps_res, base.eps_gap, base.max_iter, base.eps_step, bool(base.warm_start))
+        if (s.N, s.ncx, s.ncu) != (base.N, base.ncx, base.ncu):
+            raise ValueError("set %d: N / rows of Fx / rows of Fu (%d, %d, %d) differ from the handle's (%d, %d, %d)"
+                             % (k, s.N, s.ncx, s.ncu, base.N, base.ncx, base.ncu))
+        if (s.numSS_Points, s.numSS_it) != (base.numSS_Points, base.numSS_it):
+            raise ValueError("set %d: numSS_Points / numSS_it differ from the handle's" % k)
+        out[k] = s
+    return out, idx

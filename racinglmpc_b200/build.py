@@ -6,7 +6,8 @@ import subprocess
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "csrc", "lmpc_b200.cu")
-DEPS = [SRC] + [os.path.join(HERE, "csrc", f) for f in ("ftocp_pdip.cuh", "safeset.cuh", "lapbooks.cuh", "probe.cuh")] + \
+SRCS = [SRC, os.path.join(HERE, "csrc", "ftocp_sets.cu")]      # the QP kernel for per-controller parameters (ftocp_launch.cuh)
+DEPS = SRCS + [os.path.join(HERE, "csrc", f) for f in ("ftocp_pdip.cuh", "ftocp_launch.cuh", "safeset.cuh", "lapbooks.cuh", "probe.cuh")] + \
        [os.path.join(HERE, "..", "include", "lmpc_b200.h"), os.path.abspath(__file__)]   # this file holds the architecture flags
 OUT = os.path.join(HERE, "liblmpc_b200.so")
 CUDA_HOME = os.environ.get("CUDA_HOME", "/usr/local/cuda")
@@ -26,7 +27,7 @@ def build_native(force=False, verbose=False):
     if not force and not stale():
         return OUT
     cxx = shutil.which("g++")
-    cmd = [NVCC] + FLAGS + (["-ccbin", cxx] if cxx else []) + (["-Xptxas", "-v"] if verbose else []) + ["-o", OUT, SRC]
+    cmd = [NVCC] + FLAGS + (["-ccbin", cxx] if cxx else []) + (["-Xptxas", "-v"] if verbose else []) + ["-o", OUT] + SRCS
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError("nvcc failed:\n" + r.stdout)

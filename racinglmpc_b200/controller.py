@@ -87,6 +87,20 @@ class BatchedController:
         """QPs accepted at the 1e-6 safety-net tolerance instead of eps_res / eps_gap since creation (expected 0)."""
         return int(self._lib.lmpc_late_accepts(self._h))
 
+    def set_param_sets(self, params, index=None, QterminalSlack=None):
+        """Per-controller QP parameters (a parameter sweep in one batch): controller b solves with ``params[index[b]]`` (objects
+        with the reference's MPCParams field names; every field but N and the constraint row counts may differ) and, for LMPC,
+        ``QterminalSlack[index[b]]`` (None: the handle's).  ``index`` is required with ``params``.  ``params=None`` (no index)
+        returns to the parameters the handle was created with.
+        Waits for work already enqueued; warm-start records start over."""
+        if params is None:
+            if index is not None:
+                raise ValueError("params=None reverts to the handle's own parameters and takes no index")
+            nat.check(self._lib.lmpc_set_param_sets(self._h, None, 0, None))
+            return
+        sets, idx = nat.make_param_sets(self._p, params, index, self.B, self._p.numSS_Points, self.numSS_it, QterminalSlack)
+        nat.check(self._lib.lmpc_set_param_sets(self._h, sets, len(sets), nat.ptr(idx)))
+
     # ------------------------------------------------------------------ PredictiveModel.addTrajectory
     def model_add_trajectory(self, inst, x, u):
         """PredictiveModel.py:35-46: keep laps sorted by length; only the trToUse fastest are ever read."""

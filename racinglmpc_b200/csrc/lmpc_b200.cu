@@ -21,6 +21,7 @@
 #include <sys/syscall.h>
 #include <sys/mman.h>
 #include <map>
+#include <vector>
 #include <mutex>
 
 #include "../../include/lmpc_b200.h"
@@ -28,64 +29,9 @@
 #include "safeset.cuh"
 #include "lapbooks.cuh"
 #include "probe.cuh"
+#include "ftocp_launch.cuh"
 
 using namespace lmpc;
-
-// ------------------------------------------------------------------------------------------------
-// device helpers: mbarrier + bulk async copy (PTX ISA: cp.async.bulk, sm_90+)
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
-                 "l"(src), "r"(bytes), "r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t done = 0;
-    while (!done) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(done)
-            : "r"(smem_u32(bar)), "r"(parity)
-            : "memory");
-    }
-}
-
-struct FtocpArgs {
-    int batch;
-    const double* x0;     // [B,6]
-    const double* uOld;   // [B,2]
-    const double* abc;    // stage model
-    long long abc_inst_stride, abc_stage_stride;   // doubles
-    const double* SS;     // [B,6,M]
-    const double* Qfun;   // [B,M]
-    const double* SuccSS; // [B,6,M] or null
-    const double* SuccU;  // [B,2,M] or null
-    double* xPred;        // [B,N+1,6]
-    double* uPred;        // [B,N,2]
-    double* slack;        // [B,N*NCX] or null
-    double* lambd;        // [B,M] or null
-    double* slackT;       // [B,6] or null
-    double* zt;           // [B,6] or null
-    double* ztu;          // [B,2] or null
-    int* status;
-    int* iters;
-    double* resid;        // [B,3]
-    unsigned long long* late;   // counter of instances accepted by the late-acceptance rule (ftocp_pdip.cuh), or null
-    double* warm;         // [B][warm_stride] warm-start records (ftocp_pdip.cuh), or null = cold start
-    int* warm_valid;      // [B]
-    long long warm_stride;
-};
 
 template <int N, int M, int NCX, int NCU>
 struct KernelSmem {
@@ -93,24 +39,11 @@ struct KernelSmem {
     alignas(8) uint64_t bar;
 };
 
-// resident CTAs (= warps) per SM the register allocation is held to: horizons up to 14 are bounded by registers and shared
-// memory alike; longer horizons by shared memory only
 #define LMPC_HOST_SLOTS 4              // buffer sets (batches in flight) of the asynchronous host entry points
 #ifndef LMPC_STEP_SPLIT_DEFAULT
 #define LMPC_STEP_SPLIT_DEFAULT 1     // instance ranges of the pipelined device-resident step (1 = one launch sequence)
 #endif
-#ifndef LMPC_LB_MPC
-#define LMPC_LB_MPC 16
-#endif
-#ifndef LMPC_LB_LMPC
-#define LMPC_LB_LMPC 12
-#endif
-// what shared memory allows (about 992 B per stage + 3.5 KB for a safe set + 1 KB reserved per CTA), capped by the register target
-constexpr int ftocp_min_blocks(int N, int M) {
-    const int by_smem = 227 * 1024 / ((lmpc::stream_model(N) ? 560 : 992) * N + (M > 0 ? 74 * M : 0) + 448 + 1024);
-    const int by_regs = M > 0 ? LMPC_LB_LMPC : LMPC_LB_MPC;
-    return by_smem < 1 ? 1 : (by_smem < by_regs ? by_smem : by_regs);
-}
+
 template <int N, int M, int NCX, int NCU>
 __global__ void __launch_bounds__(32, ftocp_min_blocks(N, M)) ftocp_kernel(const __grid_constant__ FtocpConst c, const FtocpArgs a) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -232,6 +165,9 @@ struct lmpc_handle {
     int* d_warm_valid;
     long long warm_stride;
     int warm_mode;
+    // per-controller parameters (lmpc_set_param_sets): table FtocpConstRec[nsets] and set index [batch]; null = uniform handle
+    FtocpConstRec* d_sets;
+    int* d_set_idx;
     // further buffer sets of the asynchronous host entry points (slots 1 .. LMPC_HOST_SLOTS - 1; each allocated on first use)
     struct HostBufs {
         double *x0, *uOld, *abc, *SS, *Qfun, *SuccSS, *SuccU, *xPred, *uPred, *slack, *lambd, *slackT, *zt, *ztu, *resid;
@@ -279,6 +215,8 @@ static bool inv6(const double* A, double* Ai) {
 }
 
 static int build_const(const lmpc_params& p, FtocpConst& c) {
+    for (int j = 0; j < p.ncu; ++j)
+        if (!(p.bu[j] > 0.0)) return fail(LMPC_E_INVALID, "bu must be positive (u = 0 strictly feasible)");
     memset(&c, 0, sizeof(c));
     for (int i = 0; i < 36; ++i) { c.Q2[i] = 2.0 * p.Q[i]; c.Qf2[i] = 2.0 * p.Qf[i]; }
     for (int i = 0; i < 4; ++i) c.R2[i] = 2.0 * p.R[i];
@@ -318,21 +256,15 @@ static int configure_t(cudaStream_t) {
 
 template <int N, int M>
 static int launch_t(lmpc_handle* h, const FtocpArgs& a, cudaStream_t st) {
-    using KS = KernelSmem<N, M, 2, 4>;
-    ftocp_kernel<N, M, 2, 4><<<a.batch, 32, sizeof(KS), st>>>(h->c, a);
-    CK(cudaGetLastError());
+    if (h->d_sets)     // the handle has per-controller parameters: every instance reads its own row (ftocp_sets.cu)
+        CK(ftocp_sets_launch(N, M, h->d_sets, a, st));
+    else {
+        ftocp_kernel<N, M, 2, 4><<<a.batch, 32, sizeof(KernelSmem<N, M, 2, 4>), st>>>(h->c, a);
+        CK(cudaGetLastError());
+    }
     h->launches += 1;
     return LMPC_OK;
 }
-
-// The supported (horizon, safe-set size) grid: one instantiation of the solver per pair.
-// Horizons 4..48 with and without the reference's 48-point safe set (initControllerParameters.py:43-44), and other safe-set
-// sizes (numSS_it x even points per lap) at the reference's and BASELINE's horizons.
-#define LMPC_FOR_EACH_CASE(X) \
-    X(4, 0) X(6, 0) X(8, 0) X(10, 0) X(12, 0) X(14, 0) X(16, 0) X(20, 0) X(24, 0) X(32, 0) X(48, 0) \
-    X(4, 48) X(6, 48) X(8, 48) X(10, 48) X(12, 48) X(14, 48) X(16, 48) X(20, 48) X(24, 48) X(32, 48) X(48, 48) \
-    X(12, 24) X(12, 32) X(12, 64) X(12, 96) X(14, 24) X(14, 32) X(14, 64) X(14, 96)
-#define LMPC_GRID_TEXT "N in {4,6,8,10,12,14,16,20,24,32,48} with numSS_Points in {0,48}; N in {12,14} also with numSS_Points in {24,32,64,96}"
 
 static int launch(lmpc_handle* h, const FtocpArgs& a, bool lmpc_mode, cudaStream_t st) {
     const int N = h->N, M = lmpc_mode ? h->M : 0;
@@ -353,6 +285,7 @@ static int configure(int N, int M) {
     const bool have_m = (M == 0) || (hit == 2);
     if (hit == 0 || !have_m)
         return fail(LMPC_E_INVALID, "unsupported (N, numSS_Points): built for " LMPC_GRID_TEXT);
+    CK(ftocp_sets_configure(N, M));      // the variant lmpc_set_param_sets switches to
     return LMPC_OK;
 }
 
@@ -515,8 +448,9 @@ int lmpc_create(const lmpc_params* p, int batch, int device, lmpc_handle** out) 
     if (!p || !out || batch <= 0) return fail(LMPC_E_INVALID, "null argument or batch <= 0");
     if (p->ncx != 2 || p->ncu != 4)
         return fail(LMPC_E_INVALID, "this build supports ncx == 2 lane rows and ncu == 4 input rows (the reference's values)");
-    for (int j = 0; j < p->ncu; ++j)
-        if (!(p->bu[j] > 0.0)) return fail(LMPC_E_INVALID, "bu must be positive (u = 0 strictly feasible)");
+    FtocpConst c;
+    int rc = build_const(*p, c);
+    if (rc != LMPC_OK) return rc;
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return fail(LMPC_E_NODEVICE, "no CUDA device");
     if (device < 0 || device >= ndev) return fail(LMPC_E_INVALID, "bad device index");
@@ -531,8 +465,8 @@ int lmpc_create(const lmpc_params* p, int batch, int device, lmpc_handle** out) 
     h->device = device;
     h->N = p->N;
     h->M = p->numSS_Points;
-    int rc = build_const(*p, h->c);
-    if (rc == LMPC_OK) rc = create_device_side(h);
+    h->c = c;
+    rc = create_device_side(h);
     if (rc != LMPC_OK) {             // nothing of a half-built handle survives (zero-initialised: freeing what was never allocated is safe)
         const std::string msg = g_err;
         lmpc_destroy(h);
@@ -558,6 +492,8 @@ int lmpc_destroy(lmpc_handle* h) {
     cudaFree(h->d_status);
     cudaFree(h->d_iters);
     cudaFree(h->d_late);
+    cudaFree(h->d_sets);
+    cudaFree(h->d_set_idx);
     if (h->stream) cudaStreamDestroy(h->stream);
     for (int i = 0; i < 4 * LMPC_HOST_SLOTS; ++i) if (h->cstream[i]) cudaStreamDestroy(h->cstream[i]);
     if (h->ev_fork) cudaEventDestroy(h->ev_fork);
@@ -584,6 +520,54 @@ long long lmpc_late_accepts(lmpc_handle* h) {
     return (long long)v;
 }
 long long lmpc_kernel_launches(lmpc_handle* h) { return h ? h->launches : 0; }
+
+// Per-controller parameters: every set goes through build_const (the conversion lmpc_create uses), then the table replaces the
+// previous one once the handle's streams are idle.  Nothing about the handle changes unless every check passes.
+int lmpc_set_param_sets(lmpc_handle* h, const lmpc_params* sets, int nsets, const int* set_of_instance) {
+    if (!h) return fail(LMPC_E_INVALID, "null handle");
+    if (nsets < 0 || nsets > h->batch) return fail(LMPC_E_INVALID, "lmpc_set_param_sets: nsets must be 0 .. batch");
+    if ((nsets == 0) != (sets == nullptr) || (nsets == 0) != (set_of_instance == nullptr))
+        return fail(LMPC_E_INVALID, "lmpc_set_param_sets: nsets == 0 goes with NULL sets and set_of_instance, nsets >= 1 with both");
+    std::vector<FtocpConstRec> rows(nsets);
+    for (int k = 0; k < nsets; ++k) {
+        const lmpc_params& s = sets[k];
+        if (s.N != h->p.N || s.ncx != h->p.ncx || s.ncu != h->p.ncu || s.numSS_Points != h->p.numSS_Points ||
+            s.numSS_it != h->p.numSS_it || s.warm_start != h->p.warm_start)
+            return fail(LMPC_E_INVALID, "lmpc_set_param_sets: set " + std::to_string(k) +
+                                            " differs from the handle in N, ncx, ncu, numSS_Points, numSS_it or warm_start");
+        const int rc = build_const(s, rows[k].c);
+        if (rc != LMPC_OK) return fail(rc, "lmpc_set_param_sets: set " + std::to_string(k) + ": " + g_err);
+    }
+    for (int b = 0; b < (nsets ? h->batch : 0); ++b)
+        if (set_of_instance[b] < 0 || set_of_instance[b] >= nsets)
+            return fail(LMPC_E_INVALID, "lmpc_set_param_sets: set index of instance " + std::to_string(b) + " out of range");
+    CK(cudaSetDevice(h->device));
+    // batches already enqueued (the _async entry points, the device-resident step) finish with the parameters they were enqueued with
+    CK(cudaStreamSynchronize(h->stream));
+    for (int i = 0; i < 4 * LMPC_HOST_SLOTS; ++i) CK(cudaStreamSynchronize(h->cstream[i]));
+    FtocpConstRec* tab = nullptr;
+    int* idx = nullptr;
+    if (nsets > 0) {
+        cudaError_t e = cudaMalloc((void**)&tab, sizeof(FtocpConstRec) * nsets);
+        if (e == cudaSuccess) e = cudaMalloc((void**)&idx, sizeof(int) * h->batch);
+        if (e == cudaSuccess) e = cudaMemcpy(tab, rows.data(), sizeof(FtocpConstRec) * nsets, cudaMemcpyHostToDevice);
+        if (e == cudaSuccess) e = cudaMemcpy(idx, set_of_instance, sizeof(int) * h->batch, cudaMemcpyHostToDevice);
+        if (e != cudaSuccess) {
+            cudaFree(tab); cudaFree(idx);
+            return fail(LMPC_E_CUDA, std::string("lmpc_set_param_sets: ") + cudaGetErrorString(e));
+        }
+    }
+    cudaFree(h->d_sets);
+    cudaFree(h->d_set_idx);
+    h->d_sets = tab;
+    h->d_set_idx = idx;
+    // a warm-start record belongs to the QP it was taken from
+    if (h->d_warm_valid) {
+        CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * h->batch, h->stream));
+        CK(cudaStreamSynchronize(h->stream));
+    }
+    return LMPC_OK;
+}
 
 static int check_align(const void* p, const char* what) {
     if (((uintptr_t)p) & 15) return fail(LMPC_E_INVALID, std::string(what) + " must be 16-byte aligned");
@@ -612,6 +596,7 @@ int lmpc_solve_lmpc_dev(lmpc_handle* h, const double* x0, const double* uOld, co
     a.late = h->d_late;
     a.warm = nullptr; a.warm_valid = nullptr; a.warm_stride = 0;    // caller-supplied QPs start cold; the controllers of the
                                                                     // device-resident step carry warm-start records (step_range)
+    a.set_idx = h->d_set_idx;
     return launch(h, a, lm, h->stream);
 }
 
@@ -718,6 +703,7 @@ static int enqueue_host_solve_impl(lmpc_handle* h, int slot, const double* x0, c
         a.status = hb.status + lo; a.iters = hb.iters + lo; a.resid = hb.resid + lo * 3;
         a.late = h->d_late;
         a.warm = nullptr; a.warm_valid = nullptr; a.warm_stride = 0;
+        a.set_idx = h->d_set_idx ? h->d_set_idx + lo : nullptr;
         if (trace) cudaEventRecord(h->tev[ci][0], s);
         int rc = launch(h, a, lm, s);
         if (rc != LMPC_OK) return rc;
@@ -1178,6 +1164,7 @@ static int step_range(lmpc_handle* h, int mode, const double* x0_dev, cudaEvent_
     a.late = h->d_late;
     a.warm = nullptr; a.warm_valid = nullptr; a.warm_stride = 0;
     if (h->d_warm) { a.warm = h->d_warm + lo * h->warm_stride; a.warm_valid = h->d_warm_valid + lo; a.warm_stride = h->warm_stride; }
+    a.set_idx = h->d_set_idx ? h->d_set_idx + lo : nullptr;
     if ((rc = launch(h, a, lm, st)) != LMPC_OK) return rc;
     if (ev) CK(cudaEventRecord(ev[3], st));
     ShiftArgs sa;
