@@ -3,8 +3,8 @@
 
 Leg 1, QP throughput: the configs[1] workload (4096 LTV-MPC QPs, N = 12) solved through the device entry point by three handles,
 timed in alternating rounds in the same process (CUDA events, L2 flushed between timed launches as in bench.py):
-  uniform   the handle's own parameters (ftocp_kernel: parameters in the constant bank);
-  one_set   the same parameters installed as the only set (ftocp_sets_kernel: the pure cost of the variant);
+  uniform   the handle's own parameters (ftocp_kernel<..., false>: parameters in the constant bank);
+  one_set   the same parameters installed as the only set (ftocp_kernel<..., true>: the pure cost of the variant);
   sweep16   16 sets varying Qslack, dR, xRef[0] and the lane bound bx, interleaved over the batch.  The tunings take different
             numbers of interior-point iterations, so this arm is not a pure overhead figure.
 Leg 2, closed-loop sweep: benchmarks/rollout_mc.run in independent mode with a 4 Qslack x 4 dR grid of LMPC tunings over the batch

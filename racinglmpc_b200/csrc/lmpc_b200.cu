@@ -33,97 +33,10 @@
 
 using namespace lmpc;
 
-template <int N, int M, int NCX, int NCU>
-struct KernelSmem {
-    Work<N, M, NCX, NCU> w;
-    alignas(8) uint64_t bar;
-};
-
 #define LMPC_HOST_SLOTS 4              // buffer sets (batches in flight) of the asynchronous host entry points
 #ifndef LMPC_STEP_SPLIT_DEFAULT
 #define LMPC_STEP_SPLIT_DEFAULT 1     // instance ranges of the pipelined device-resident step (1 = one launch sequence)
 #endif
-
-template <int N, int M, int NCX, int NCU>
-__global__ void __launch_bounds__(32, ftocp_min_blocks(N, M)) ftocp_kernel(const __grid_constant__ FtocpConst c, const FtocpArgs a) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    using KS = KernelSmem<N, M, NCX, NCU>;
-    KS& ks = *reinterpret_cast<KS*>(smem_raw);
-    auto& w = ks.w;
-    const int b = blockIdx.x;
-    if (b >= a.batch) return;
-    const int lane = threadIdx.x;
-
-    // ---- stage the instance's model into shared memory (TMA 1-D bulk copies) ----
-    if (lane == 0) {
-        mbar_init(&ks.bar, 1);
-        constexpr bool STREAM = Work<N, M, NCX, NCU>::STREAM;   // long horizons read the stage model in place (ftocp_pdip.cuh)
-        uint32_t bytes = (STREAM ? 0 : N * 54 * 8) + (M > 0 ? (6 * M + M) * 8 : 0);
-        mbar_expect_tx(&ks.bar, bytes);
-        const double* src = a.abc + (long long)b * a.abc_inst_stride;
-        w.gabc = src;
-        w.gstage = (int)a.abc_stage_stride;
-        if (STREAM) {
-        } else if (a.abc_stage_stride == 54) {
-            bulk_g2s(&w.ABC[0][0], src, N * 54 * 8, &ks.bar);
-        } else {
-            for (int k = 0; k < N; ++k) bulk_g2s(&w.ABC[k][0], src + (long long)k * a.abc_stage_stride, 54 * 8, &ks.bar);
-        }
-        if (M > 0) {
-            bulk_g2s(&w.SS[0], a.SS + (long long)b * 6 * M, 6 * M * 8, &ks.bar);
-            bulk_g2s(&w.Qfun[0], a.Qfun + (long long)b * M, M * 8, &ks.bar);
-        }
-    }
-    double x0[6];
-#pragma unroll
-    for (int i = 0; i < 6; ++i) x0[i] = a.x0[(long long)b * 6 + i];
-    if (lane < 2) w.uOld[lane] = a.uOld[(long long)b * 2 + lane];
-    __syncwarp();
-    mbar_wait(&ks.bar, 0);
-
-    // ---- solve ----
-    SolveInfo info;
-    Pdip<N, M, NCX, NCU>::solve(w, c, x0, info, (M > 0) ? w.d4i : nullptr, a.slack ? a.slack + (long long)b * N * NCX : nullptr,
-                                a.warm ? a.warm + (long long)b * a.warm_stride : nullptr, a.warm ? a.warm_valid + b : nullptr);
-
-    // ---- unpack (PC.py:364-384) ----
-    for (int e = lane; e < (N + 1) * 6; e += 32) a.xPred[(long long)b * (N + 1) * 6 + e] = w.x[e];
-    for (int e = lane; e < N * 2; e += 32) a.uPred[(long long)b * N * 2 + e] = w.u[e];
-    if (M > 0) {
-        const double* lam = w.d4i;   // solve() left lambda here
-        if (a.lambd)
-            for (int e = lane; e < M; e += 32) a.lambd[(long long)b * M + e] = lam[e];
-        for (int e = lane; e < 14; e += 32) {
-            double v = 0.0;
-            if (e < 6) {           // slackTerminal = SS lam - x_N
-                if (a.slackT) {
-                    for (int l = 0; l < M; ++l) v += w.SS[e * M + l] * lam[l];
-                    a.slackT[(long long)b * 6 + e] = v - w.x[N * 6 + e];
-                }
-            } else if (e < 12) {   // zt = Succ_SS lam
-                if (a.zt && a.SuccSS) {
-                    const double* S = a.SuccSS + ((long long)b * 6 + (e - 6)) * M;
-                    for (int l = 0; l < M; ++l) v += S[l] * lam[l];
-                    a.zt[(long long)b * 6 + (e - 6)] = v;
-                }
-            } else {               // zt_u = Succ_uSS lam
-                if (a.ztu && a.SuccU) {
-                    const double* S = a.SuccU + ((long long)b * 2 + (e - 12)) * M;
-                    for (int l = 0; l < M; ++l) v += S[l] * lam[l];
-                    a.ztu[(long long)b * 2 + (e - 12)] = v;
-                }
-            }
-        }
-    }
-    if (lane == 0) {
-        a.status[b] = info.status;
-        a.iters[b] = info.iters;
-        a.resid[(long long)b * 3 + 0] = info.r_prim;
-        a.resid[(long long)b * 3 + 1] = info.r_dual;
-        a.resid[(long long)b * 3 + 2] = info.gap;
-        if (info.late && a.late) atomicAdd(a.late, 1ull);
-    }
-}
 
 // ------------------------------------------------------------------------------------------------
 // host side
@@ -138,6 +51,14 @@ static int fail(int code, const std::string& msg) {
         cudaError_t e_ = (call);                                                                        \
         if (e_ != cudaSuccess) return fail(LMPC_E_CUDA, std::string(#call) + ": " + cudaGetErrorString(e_)); \
     } while (0)
+
+// The QP kernel's inputs and outputs for one whole batch: [B,6] x0, [B,2] uOld, [B,N,54] abc, [B,6,M] SS, [B,M] Qfun, [B,6,M]
+// SuccSS, [B,2,M] SuccU, [B,N+1,6] xPred, [B,N,2] uPred, [B,N*2] slack, [B,M] lambd, [B,6] slackT, [B,6] zt, [B,2] ztu,
+// [B,3] resid, [B] status, [B] iters (M = 1 for handles without a safe set)
+struct QpBufs {
+    double *x0, *uOld, *abc, *SS, *Qfun, *SuccSS, *SuccU, *xPred, *uPred, *slack, *lambd, *slackT, *zt, *ztu, *resid;
+    int *status, *iters;
+};
 
 struct lmpc_handle {
     lmpc_params p;
@@ -155,10 +76,9 @@ struct lmpc_handle {
     bool trace_on;
     cudaEvent_t tev[4][3], t0ev;
     long long launches;
-    // device buffers used by the *_host entry points
-    double *d_x0, *d_uOld, *d_abc, *d_SS, *d_Qfun, *d_SuccSS, *d_SuccU;
-    double *d_xPred, *d_uPred, *d_slack, *d_lambd, *d_slackT, *d_zt, *d_ztu, *d_resid;
-    int *d_status, *d_iters;
+    // QP buffer sets, one per slot of the *_host entry points.  hb[0] is allocated at creation and is also the device-resident
+    // step's (K1 writes its abc, K2 its safe set, the QP kernel its outputs; lmpc_device_buffer); hb[1..] on first use.
+    QpBufs hb[LMPC_HOST_SLOTS];
     unsigned long long* d_late;
     // warm-start records of the controllers of the device-resident step (lmpc_params.warm_start; allocated with the store)
     double* d_warm;
@@ -168,12 +88,6 @@ struct lmpc_handle {
     // per-controller parameters (lmpc_set_param_sets): table FtocpConstRec[nsets] and set index [batch]; null = uniform handle
     FtocpConstRec* d_sets;
     int* d_set_idx;
-    // further buffer sets of the asynchronous host entry points (slots 1 .. LMPC_HOST_SLOTS - 1; each allocated on first use)
-    struct HostBufs {
-        double *x0, *uOld, *abc, *SS, *Qfun, *SuccSS, *SuccU, *xPred, *uPred, *slack, *lambd, *slackT, *zt, *ztu, *resid;
-        int *status, *iters;
-    } hbx[LMPC_HOST_SLOTS - 1];
-    bool has_hbx[LMPC_HOST_SLOTS - 1];
     // lap stores + controller state (lmpc_store_create)
     bool has_store;
     ModelConst mc;
@@ -250,7 +164,8 @@ static int build_const(const lmpc_params& p, FtocpConst& c) {
 
 template <int N, int M>
 static int configure_t(cudaStream_t) {
-    CK(cudaFuncSetAttribute(ftocp_kernel<N, M, 2, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(KernelSmem<N, M, 2, 4>)));
+    CK(cudaFuncSetAttribute(ftocp_kernel<N, M, 2, 4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            (int)sizeof(KernelSmem<N, M, 2, 4, false>)));
     return LMPC_OK;
 }
 
@@ -259,7 +174,7 @@ static int launch_t(lmpc_handle* h, const FtocpArgs& a, cudaStream_t st) {
     if (h->d_sets)     // the handle has per-controller parameters: every instance reads its own row (ftocp_sets.cu)
         CK(ftocp_sets_launch(N, M, h->d_sets, a, st));
     else {
-        ftocp_kernel<N, M, 2, 4><<<a.batch, 32, sizeof(KernelSmem<N, M, 2, 4>), st>>>(h->c, a);
+        ftocp_kernel<N, M, 2, 4, false><<<a.batch, 32, sizeof(KernelSmem<N, M, 2, 4, false>), st>>>(h->c, a);
         CK(cudaGetLastError());
     }
     h->launches += 1;
@@ -315,12 +230,54 @@ static void free_rollout(lmpc_handle* h) {
     h->has_rollout = false;
 }
 
-static void free_hbx(lmpc_handle* h, int i) {
-    lmpc_handle::HostBufs& q = h->hbx[i];
+static void free_qp_bufs(QpBufs& q) {
     free_null(q.x0); free_null(q.uOld); free_null(q.abc); free_null(q.SS); free_null(q.Qfun); free_null(q.SuccSS); free_null(q.SuccU);
     free_null(q.xPred); free_null(q.uPred); free_null(q.slack); free_null(q.lambd); free_null(q.slackT); free_null(q.zt); free_null(q.ztu);
     free_null(q.resid); free_null(q.status); free_null(q.iters);
-    h->has_hbx[i] = false;
+}
+
+// Buffer set `slot` of the handle, allocated on first use (x0 != null: allocated); null (and g_err set) if the allocation failed,
+// which leaves nothing behind
+static QpBufs* qp_bufs(lmpc_handle* h, int slot) {
+    QpBufs& q = h->hb[slot];
+    if (!q.x0) {
+        const size_t B = h->batch, N = h->N, M = h->M > 0 ? h->M : 1;
+        cudaError_t e = cudaSuccess;
+        auto alloc = [&](auto*& p, size_t count) { if (e == cudaSuccess) e = cudaMalloc((void**)&p, sizeof(*p) * count); };
+        alloc(q.x0, B * 6); alloc(q.uOld, B * 2); alloc(q.abc, B * N * 54);
+        alloc(q.SS, B * 6 * M); alloc(q.Qfun, B * M); alloc(q.SuccSS, B * 6 * M); alloc(q.SuccU, B * 2 * M);
+        alloc(q.xPred, B * (N + 1) * 6); alloc(q.uPred, B * N * 2); alloc(q.slack, B * N * 2);
+        alloc(q.lambd, B * M); alloc(q.slackT, B * 6); alloc(q.zt, B * 6); alloc(q.ztu, B * 2);
+        alloc(q.resid, B * 3); alloc(q.status, B); alloc(q.iters, B);
+        if (e != cudaSuccess) {
+            free_qp_bufs(q);
+            fail(LMPC_E_CUDA, std::string("cudaMalloc of QP buffer set ") + std::to_string(slot) + ": " + cudaGetErrorString(e));
+            return nullptr;
+        }
+    }
+    return &q;
+}
+
+// which of the QP kernel's optional inputs and outputs a caller wants (qp_args); the safe-set ones only count on LMPC-type QPs
+enum : unsigned { QP_SUCC_SS = 1, QP_SUCC_U = 2, QP_SLACK = 4, QP_LAMBD = 8, QP_SLACKT = 16, QP_ZT = 32, QP_ZTU = 64, QP_ALL = 127 };
+
+// Kernel arguments for the whole batch held in q (per-instance model, strides (N*54, 54)); what the caller does not want stays null,
+// which the kernel skips
+static FtocpArgs qp_args(const lmpc_handle* h, const QpBufs& q, bool lm, unsigned want) {
+    if (!lm) want &= QP_SLACK;
+    FtocpArgs a = {};
+    a.batch = h->batch;
+    a.x0 = q.x0; a.uOld = q.uOld; a.abc = q.abc;
+    a.abc_inst_stride = (long long)h->N * 54; a.abc_stage_stride = 54;
+    a.SS = lm ? q.SS : nullptr; a.Qfun = lm ? q.Qfun : nullptr;
+    a.SuccSS = (want & QP_SUCC_SS) ? q.SuccSS : nullptr; a.SuccU = (want & QP_SUCC_U) ? q.SuccU : nullptr;
+    a.xPred = q.xPred; a.uPred = q.uPred; a.slack = (want & QP_SLACK) ? q.slack : nullptr;
+    a.lambd = (want & QP_LAMBD) ? q.lambd : nullptr; a.slackT = (want & QP_SLACKT) ? q.slackT : nullptr;
+    a.zt = (want & QP_ZT) ? q.zt : nullptr; a.ztu = (want & QP_ZTU) ? q.ztu : nullptr;
+    a.status = q.status; a.iters = q.iters; a.resid = q.resid;
+    a.late = h->d_late;
+    a.set_idx = h->d_set_idx;
+    return a;
 }
 
 static int create_device_side(lmpc_handle* h) {
@@ -333,14 +290,8 @@ static int create_device_side(lmpc_handle* h) {
     for (int i = 0; i < 4; ++i) CK(cudaEventCreateWithFlags(&h->ev_join[i], cudaEventDisableTiming));
     h->step_split = LMPC_STEP_SPLIT_DEFAULT;
     if (const char* e = getenv("LMPC_B200_STEP_SPLIT")) { const int v = atoi(e); if (v >= 1 && v <= 4) h->step_split = v; }   // tuning knob
-    const size_t B = h->batch, N = h->N, M = h->M > 0 ? h->M : 1;
-#define DALLOC(ptr, count) CK(cudaMalloc((void**)&h->ptr, sizeof(*h->ptr) * (count)))
-    DALLOC(d_x0, B * 6); DALLOC(d_uOld, B * 2); DALLOC(d_abc, B * N * 54);
-    DALLOC(d_SS, B * 6 * M); DALLOC(d_Qfun, B * M); DALLOC(d_SuccSS, B * 6 * M); DALLOC(d_SuccU, B * 2 * M);
-    DALLOC(d_xPred, B * (N + 1) * 6); DALLOC(d_uPred, B * N * 2); DALLOC(d_slack, B * N * 2);
-    DALLOC(d_lambd, B * M); DALLOC(d_slackT, B * 6); DALLOC(d_zt, B * 6); DALLOC(d_ztu, B * 2);
-    DALLOC(d_resid, B * 3); DALLOC(d_status, B); DALLOC(d_iters, B); DALLOC(d_late, 1);
-#undef DALLOC
+    if (!qp_bufs(h, 0)) return LMPC_E_CUDA;
+    CK(cudaMalloc((void**)&h->d_late, sizeof(unsigned long long)));
     CK(cudaMemset(h->d_late, 0, sizeof(unsigned long long)));
     return LMPC_OK;
 }
@@ -485,12 +436,7 @@ int lmpc_destroy(lmpc_handle* h) {
     // every pointer freed here is either a live allocation or still null (handle memory is zero-initialised)
     free_rollout(h);
     free_store(h);
-    for (int i = 0; i < LMPC_HOST_SLOTS - 1; ++i) free_hbx(h, i);
-    double* dbl[] = {h->d_x0, h->d_uOld, h->d_abc, h->d_SS, h->d_Qfun, h->d_SuccSS, h->d_SuccU, h->d_xPred, h->d_uPred,
-                     h->d_slack, h->d_lambd, h->d_slackT, h->d_zt, h->d_ztu, h->d_resid};
-    for (double* q : dbl) cudaFree(q);
-    cudaFree(h->d_status);
-    cudaFree(h->d_iters);
+    for (QpBufs& q : h->hb) free_qp_bufs(q);
     cudaFree(h->d_late);
     cudaFree(h->d_sets);
     cudaFree(h->d_set_idx);
@@ -586,7 +532,8 @@ int lmpc_solve_lmpc_dev(lmpc_handle* h, const double* x0, const double* uOld, co
     if ((rc = check_align(abc, "abc")) != LMPC_OK) return rc;
     if (lm && ((rc = check_align(SS_sel, "SS_sel")) != LMPC_OK || (rc = check_align(Qfun_sel, "Qfun_sel")) != LMPC_OK)) return rc;
     CK(cudaSetDevice(h->device));
-    FtocpArgs a;
+    FtocpArgs a = {};   // no warm-start records: caller-supplied QPs start cold; the controllers of the device-resident step
+                        // carry warm-start records (step_range)
     a.batch = h->batch;
     a.x0 = x0; a.uOld = uOld; a.abc = abc;
     a.abc_inst_stride = abc_inst_stride; a.abc_stage_stride = abc_stage_stride;
@@ -594,8 +541,6 @@ int lmpc_solve_lmpc_dev(lmpc_handle* h, const double* x0, const double* uOld, co
     a.xPred = xPred; a.uPred = uPred; a.slack = slack; a.lambd = lambd; a.slackT = slackTerminal;
     a.zt = zt; a.ztu = zt_u; a.status = status; a.iters = iters; a.resid = resid;
     a.late = h->d_late;
-    a.warm = nullptr; a.warm_valid = nullptr; a.warm_stride = 0;    // caller-supplied QPs start cold; the controllers of the
-                                                                    // device-resident step carry warm-start records (step_range)
     a.set_idx = h->d_set_idx;
     return launch(h, a, lm, h->stream);
 }
@@ -605,30 +550,6 @@ int lmpc_solve_mpc_dev(lmpc_handle* h, const double* x0, const double* uOld, con
                        double* resid) {
     return lmpc_solve_lmpc_dev(h, x0, uOld, abc, abc_inst_stride, abc_stage_stride, nullptr, nullptr, nullptr, nullptr, xPred,
                                uPred, slack, nullptr, nullptr, nullptr, nullptr, status, iters, resid);
-}
-
-static int host_bufs(lmpc_handle* h, int slot, lmpc_handle::HostBufs& b) {
-    if (slot == 0) {
-        b = {h->d_x0, h->d_uOld, h->d_abc, h->d_SS, h->d_Qfun, h->d_SuccSS, h->d_SuccU, h->d_xPred, h->d_uPred, h->d_slack,
-             h->d_lambd, h->d_slackT, h->d_zt, h->d_ztu, h->d_resid, h->d_status, h->d_iters};
-        return LMPC_OK;
-    }
-    const int xi = slot - 1;
-    if (!h->has_hbx[xi]) {
-        const size_t B = h->batch, N = h->N, M = h->M > 0 ? h->M : 1;
-        lmpc_handle::HostBufs& q = h->hbx[xi];
-#define DA1(ptr, count) do { if (cudaMalloc((void**)&q.ptr, sizeof(*q.ptr) * (count)) != cudaSuccess) { free_hbx(h, xi); \
-                              return fail(LMPC_E_CUDA, "cudaMalloc of a further host-path buffer set failed"); } } while (0)
-        DA1(x0, B * 6); DA1(uOld, B * 2); DA1(abc, B * N * 54);
-        DA1(SS, B * 6 * M); DA1(Qfun, B * M); DA1(SuccSS, B * 6 * M); DA1(SuccU, B * 2 * M);
-        DA1(xPred, B * (N + 1) * 6); DA1(uPred, B * N * 2); DA1(slack, B * N * 2);
-        DA1(lambd, B * M); DA1(slackT, B * 6); DA1(zt, B * 6); DA1(ztu, B * 2);
-        DA1(resid, B * 3); DA1(status, B); DA1(iters, B);
-#undef DA1
-        h->has_hbx[xi] = true;
-    }
-    b = h->hbx[xi];
-    return LMPC_OK;
 }
 
 // Enqueue one host-buffer solve on buffer set / stream group `slot` (0 .. LMPC_HOST_SLOTS - 1) WITHOUT waiting for it.
@@ -644,8 +565,9 @@ static int enqueue_host_solve_impl(lmpc_handle* h, int slot, const double* x0, c
     CK(cudaSetDevice(h->device));
     const size_t B = h->batch, N = h->N, M = h->M > 0 ? h->M : 1;
     const size_t D = sizeof(double);
-    lmpc_handle::HostBufs hb;
-    { int rcb = host_bufs(h, slot, hb); if (rcb) return rcb; }
+    const QpBufs* q = qp_bufs(h, slot);
+    if (!q) return LMPC_E_CUDA;
+    const QpBufs& hb = *q;
     cudaStream_t* cs = h->cstream + 4 * slot;
     long long dis, dss;
     bool per_inst = false;
@@ -676,6 +598,10 @@ static int enqueue_host_solve_impl(lmpc_handle* h, int slot, const double* x0, c
         cudaEventRecord(h->t0ev, cs[0]);
     }
     h->trace_on = trace;
+    FtocpArgs all = qp_args(h, hb, lm, (Succ_SS ? QP_SUCC_SS : 0) | (Succ_uSS ? QP_SUCC_U : 0) | (slack ? QP_SLACK : 0) |
+                                       (lambd ? QP_LAMBD : 0) | (slackTerminal ? QP_SLACKT : 0) | (zt ? QP_ZT : 0) |
+                                       (zt_u ? QP_ZTU : 0));
+    all.abc_inst_stride = dis; all.abc_stage_stride = dss;
     for (int ci = 0; ci < nchunk; ++ci) {
         const size_t lo = B * ci / nchunk, hi = B * (ci + 1) / nchunk, nb = hi - lo;
         cudaStream_t s = cs[ci];
@@ -688,24 +614,8 @@ static int enqueue_host_solve_impl(lmpc_handle* h, int slot, const double* x0, c
             if (Succ_SS) CK(cudaMemcpyAsync(hb.SuccSS + lo * 6 * M, Succ_SS + lo * 6 * M, nb * 6 * M * D, cudaMemcpyHostToDevice, s));
             if (Succ_uSS) CK(cudaMemcpyAsync(hb.SuccU + lo * 2 * M, Succ_uSS + lo * 2 * M, nb * 2 * M * D, cudaMemcpyHostToDevice, s));
         }
-        FtocpArgs a;
-        a.batch = (int)nb;
-        a.x0 = hb.x0 + lo * 6; a.uOld = hb.uOld + lo * 2;
-        a.abc = per_inst ? hb.abc + lo * N * 54 : hb.abc;
-        a.abc_inst_stride = dis; a.abc_stage_stride = dss;
-        a.SS = lm ? hb.SS + lo * 6 * M : nullptr; a.Qfun = lm ? hb.Qfun + lo * M : nullptr;
-        a.SuccSS = (lm && Succ_SS) ? hb.SuccSS + lo * 6 * M : nullptr; a.SuccU = (lm && Succ_uSS) ? hb.SuccU + lo * 2 * M : nullptr;
-        a.xPred = hb.xPred + lo * (N + 1) * 6; a.uPred = hb.uPred + lo * N * 2;
-        a.slack = slack ? hb.slack + lo * N * 2 : nullptr;
-        a.lambd = (lm && lambd) ? hb.lambd + lo * M : nullptr;
-        a.slackT = (lm && slackTerminal) ? hb.slackT + lo * 6 : nullptr;
-        a.zt = (lm && zt) ? hb.zt + lo * 6 : nullptr; a.ztu = (lm && zt_u) ? hb.ztu + lo * 2 : nullptr;
-        a.status = hb.status + lo; a.iters = hb.iters + lo; a.resid = hb.resid + lo * 3;
-        a.late = h->d_late;
-        a.warm = nullptr; a.warm_valid = nullptr; a.warm_stride = 0;
-        a.set_idx = h->d_set_idx ? h->d_set_idx + lo : nullptr;
         if (trace) cudaEventRecord(h->tev[ci][0], s);
-        int rc = launch(h, a, lm, s);
+        int rc = launch(h, all.range((int)lo, (int)nb, (int)N, h->M), lm, s);
         if (rc != LMPC_OK) return rc;
         if (trace) cudaEventRecord(h->tev[ci][1], s);
         CK(cudaMemcpyAsync(xPred + lo * (N + 1) * 6, hb.xPred + lo * (N + 1) * 6, nb * (N + 1) * 6 * D, cudaMemcpyDeviceToHost, s));
@@ -1060,7 +970,7 @@ static int launch_k1(lmpc_handle* h, int b0 = 0, int nb = -1, cudaStream_t st = 
     a.batch = h->batch; a.N = h->N; a.b0 = b0;
     a.wpb = h->N < 12 ? h->N : 12;
     a.pts_stride = k1_pts_stride(h->mc.trToUse);
-    a.xLin = h->d_xLin; a.uLin = h->d_uLin; a.pool = h->mdl; a.used = h->d_used; a.abc = h->d_abc; a.status = h->d_flags;
+    a.xLin = h->d_xLin; a.uLin = h->d_uLin; a.pool = h->mdl; a.used = h->d_used; a.abc = h->hb[0].abc; a.status = h->d_flags;
     dim3 grid(nb, (h->N + a.wpb - 1) / a.wpb);
     size_t smem = sizeof(float) * 5 * K1_TILE + sizeof(double) * (size_t)a.pts_stride * a.wpb;
     knn_ltv_regress_kernel<<<grid, 32 * a.wpb, smem, st>>>(h->mc, a);
@@ -1077,7 +987,7 @@ static int launch_k2(lmpc_handle* h, const double* d_x0, int b0 = 0, int nb = -1
     a.TrackLength = h->mc.TrackLength;
     a.x0 = d_x0; a.zt = h->d_ztState; a.pool = h->ss; a.sel = h->d_sel; a.is_prev = h->d_isprev;
     a.timeStep = h->d_timeStep; a.has_pred = h->d_hasPred; a.xPred = h->d_xPredPrev;
-    a.SS_sel = h->d_SS; a.Qfun_sel = h->d_Qfun; a.Succ_SS = h->d_SuccSS; a.Succ_uSS = h->d_SuccU;
+    a.SS_sel = h->hb[0].SS; a.Qfun_sel = h->hb[0].Qfun; a.Succ_SS = h->hb[0].SuccSS; a.Succ_uSS = h->hb[0].SuccU;
     a.zt_fixed = h->d_ztFixed; a.status = h->d_flags; a.min_index = h->d_minidx;
     ss_select_kernel<<<nb, 32 * a.numSS_it, 0, st>>>(a);
     CK(cudaGetLastError());
@@ -1092,7 +1002,7 @@ int lmpc_identify_host(lmpc_handle* h, double* abc_out, int* flags) {
     CK(cudaMemsetAsync(h->d_flags, 0, sizeof(int) * h->batch, h->stream));
     rc = launch_k1(h);
     if (rc) return rc;
-    if (abc_out) CK(cudaMemcpyAsync(abc_out, h->d_abc, sizeof(double) * h->batch * h->N * 54, cudaMemcpyDeviceToHost, h->stream));
+    if (abc_out) CK(cudaMemcpyAsync(abc_out, h->hb[0].abc, sizeof(double) * h->batch * h->N * 54, cudaMemcpyDeviceToHost, h->stream));
     if (flags) CK(cudaMemcpyAsync(flags, h->d_flags, sizeof(int) * h->batch, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     return LMPC_OK;
@@ -1106,14 +1016,14 @@ int lmpc_select_host(lmpc_handle* h, const double* x0, double* SS_sel, double* Q
     CK(cudaSetDevice(h->device));
     const size_t B = h->batch, M = h->M, D = sizeof(double);
     cudaStream_t s = h->stream;
-    CK(cudaMemcpyAsync(h->d_x0, x0, B * 6 * D, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(h->hb[0].x0, x0, B * 6 * D, cudaMemcpyHostToDevice, s));
     CK(cudaMemsetAsync(h->d_flags, 0, sizeof(int) * B, s));
-    rc = launch_k2(h, h->d_x0);
+    rc = launch_k2(h, h->hb[0].x0);
     if (rc) return rc;
-    if (SS_sel) CK(cudaMemcpyAsync(SS_sel, h->d_SS, B * 6 * M * D, cudaMemcpyDeviceToHost, s));
-    if (Qfun_sel) CK(cudaMemcpyAsync(Qfun_sel, h->d_Qfun, B * M * D, cudaMemcpyDeviceToHost, s));
-    if (Succ_SS) CK(cudaMemcpyAsync(Succ_SS, h->d_SuccSS, B * 6 * M * D, cudaMemcpyDeviceToHost, s));
-    if (Succ_uSS) CK(cudaMemcpyAsync(Succ_uSS, h->d_SuccU, B * 2 * M * D, cudaMemcpyDeviceToHost, s));
+    if (SS_sel) CK(cudaMemcpyAsync(SS_sel, h->hb[0].SS, B * 6 * M * D, cudaMemcpyDeviceToHost, s));
+    if (Qfun_sel) CK(cudaMemcpyAsync(Qfun_sel, h->hb[0].Qfun, B * M * D, cudaMemcpyDeviceToHost, s));
+    if (Succ_SS) CK(cudaMemcpyAsync(Succ_SS, h->hb[0].SuccSS, B * 6 * M * D, cudaMemcpyDeviceToHost, s));
+    if (Succ_uSS) CK(cudaMemcpyAsync(Succ_uSS, h->hb[0].SuccU, B * 2 * M * D, cudaMemcpyDeviceToHost, s));
     if (min_index) CK(cudaMemcpyAsync(min_index, h->d_minidx, B * h->p.numSS_it * sizeof(int), cudaMemcpyDeviceToHost, s));
     if (flags) CK(cudaMemcpyAsync(flags, h->d_flags, B * sizeof(int), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
@@ -1145,31 +1055,20 @@ int lmpc_step_profile(lmpc_handle* h, int mode, const double* x0_dev, float* ms4
 struct StepTail { const double* xc; SimArgs sim; };
 static int step_range(lmpc_handle* h, int mode, const double* x0_dev, cudaEvent_t* ev, int b0, int nb, cudaStream_t st, const StepTail* tail) {
     int rc;
-    const size_t N = h->N, M = h->M > 0 ? h->M : 1, lo = b0;
     const bool lm = mode == 1;
+    const QpBufs& q = h->hb[0];
     if ((rc = launch_k1(h, b0, nb, st)) != LMPC_OK) return rc;                       // PC.py:117
     if (ev) CK(cudaEventRecord(ev[1], st));
     if (lm && (rc = launch_k2(h, x0_dev, b0, nb, st)) != LMPC_OK) return rc;         // PC.py:121
     if (ev) CK(cudaEventRecord(ev[2], st));
-    FtocpArgs a;                                                                     // PC.py:124-125
-    a.batch = nb;
-    a.x0 = x0_dev + lo * 6; a.uOld = h->d_OldInput + lo * 2;
-    a.abc = h->d_abc + lo * N * 54; a.abc_inst_stride = (long long)N * 54; a.abc_stage_stride = 54;
-    a.SS = lm ? h->d_SS + lo * 6 * M : nullptr; a.Qfun = lm ? h->d_Qfun + lo * M : nullptr;
-    a.SuccSS = lm ? h->d_SuccSS + lo * 6 * M : nullptr; a.SuccU = lm ? h->d_SuccU + lo * 2 * M : nullptr;
-    a.xPred = h->d_xPred + lo * (N + 1) * 6; a.uPred = h->d_uPred + lo * N * 2; a.slack = h->d_slack + lo * N * 2;
-    a.lambd = lm ? h->d_lambd + lo * M : nullptr; a.slackT = lm ? h->d_slackT + lo * 6 : nullptr;
-    a.zt = lm ? h->d_zt + lo * 6 : nullptr; a.ztu = lm ? h->d_ztu + lo * 2 : nullptr;
-    a.status = h->d_status + lo; a.iters = h->d_iters + lo; a.resid = h->d_resid + lo * 3;
-    a.late = h->d_late;
-    a.warm = nullptr; a.warm_valid = nullptr; a.warm_stride = 0;
-    if (h->d_warm) { a.warm = h->d_warm + lo * h->warm_stride; a.warm_valid = h->d_warm_valid + lo; a.warm_stride = h->warm_stride; }
-    a.set_idx = h->d_set_idx ? h->d_set_idx + lo : nullptr;
-    if ((rc = launch(h, a, lm, st)) != LMPC_OK) return rc;
+    FtocpArgs a = qp_args(h, q, lm, QP_ALL);                                         // PC.py:124-125
+    a.x0 = x0_dev; a.uOld = h->d_OldInput;
+    if (h->d_warm) { a.warm = h->d_warm; a.warm_valid = h->d_warm_valid; a.warm_stride = h->warm_stride; }
+    if ((rc = launch(h, a.range(b0, nb, h->N, h->M), lm, st)) != LMPC_OK) return rc;
     if (ev) CK(cudaEventRecord(ev[3], st));
     ShiftArgs sa;
     sa.batch = h->batch; sa.N = h->N; sa.lmpc = mode; sa.b0 = b0;
-    sa.xPred = h->d_xPred; sa.uPred = h->d_uPred; sa.zt_in = h->d_zt; sa.ztu_in = h->d_ztu;
+    sa.xPred = q.xPred; sa.uPred = q.uPred; sa.zt_in = q.zt; sa.ztu_in = q.ztu;
     sa.xLin = h->d_xLin; sa.uLin = h->d_uLin; sa.zt = h->d_ztState; sa.OldInput = h->d_OldInput; sa.xPredPrev = h->d_xPredPrev;
     sa.timeStep = h->d_timeStep; sa.has_pred = h->d_hasPred;
     shift_state_kernel<<<nb, 64, 0, st>>>(sa);                                       // PC.py:129-137
@@ -1178,7 +1077,7 @@ static int step_range(lmpc_handle* h, int mode, const double* x0_dev, cudaEvent_
     if (ev) CK(cudaEventRecord(ev[4], st));
     if (tail) {
         if (lm) {                                                                    // SysModel.py:38 -> PC.py:466-476
-            ss_add_point_kernel<<<(nb + 127) / 128, 128, 0, st>>>(b0 + nb, h->ss, h->d_prevslot, tail->xc, h->d_uPred, (long long)h->N * 2,
+            ss_add_point_kernel<<<(nb + 127) / 128, 128, 0, st>>>(b0 + nb, h->ss, h->d_prevslot, tail->xc, q.uPred, (long long)h->N * 2,
                                                                   h->mc.TrackLength, h->d_flags, nullptr, b0);
             CK(cudaGetLastError());
             h->launches += 1;
@@ -1236,20 +1135,20 @@ int lmpc_step_host(lmpc_handle* h, int mode, const double* x0, double* xPred, do
     CK(cudaSetDevice(h->device));
     const size_t B = h->batch, N = h->N, M = h->M > 0 ? h->M : 1, D = sizeof(double);
     cudaStream_t s = h->stream;
-    CK(cudaMemcpyAsync(h->d_x0, x0, B * 6 * D, cudaMemcpyHostToDevice, s));
-    rc = lmpc_step_dev(h, mode, h->d_x0);
+    CK(cudaMemcpyAsync(h->hb[0].x0, x0, B * 6 * D, cudaMemcpyHostToDevice, s));
+    rc = lmpc_step_dev(h, mode, h->hb[0].x0);
     if (rc) return rc;
-    if (xPred) CK(cudaMemcpyAsync(xPred, h->d_xPred, B * (N + 1) * 6 * D, cudaMemcpyDeviceToHost, s));
-    if (uPred) CK(cudaMemcpyAsync(uPred, h->d_uPred, B * N * 2 * D, cudaMemcpyDeviceToHost, s));
+    if (xPred) CK(cudaMemcpyAsync(xPred, h->hb[0].xPred, B * (N + 1) * 6 * D, cudaMemcpyDeviceToHost, s));
+    if (uPred) CK(cudaMemcpyAsync(uPred, h->hb[0].uPred, B * N * 2 * D, cudaMemcpyDeviceToHost, s));
     if (mode == 1) {
-        if (lambd) CK(cudaMemcpyAsync(lambd, h->d_lambd, B * M * D, cudaMemcpyDeviceToHost, s));
-        if (zt) CK(cudaMemcpyAsync(zt, h->d_zt, B * 6 * D, cudaMemcpyDeviceToHost, s));
-        if (zt_u) CK(cudaMemcpyAsync(zt_u, h->d_ztu, B * 2 * D, cudaMemcpyDeviceToHost, s));
-        if (SS_sel) CK(cudaMemcpyAsync(SS_sel, h->d_SS, B * 6 * M * D, cudaMemcpyDeviceToHost, s));
+        if (lambd) CK(cudaMemcpyAsync(lambd, h->hb[0].lambd, B * M * D, cudaMemcpyDeviceToHost, s));
+        if (zt) CK(cudaMemcpyAsync(zt, h->hb[0].zt, B * 6 * D, cudaMemcpyDeviceToHost, s));
+        if (zt_u) CK(cudaMemcpyAsync(zt_u, h->hb[0].ztu, B * 2 * D, cudaMemcpyDeviceToHost, s));
+        if (SS_sel) CK(cudaMemcpyAsync(SS_sel, h->hb[0].SS, B * 6 * M * D, cudaMemcpyDeviceToHost, s));
     }
-    if (status) CK(cudaMemcpyAsync(status, h->d_status, B * sizeof(int), cudaMemcpyDeviceToHost, s));
-    if (iters) CK(cudaMemcpyAsync(iters, h->d_iters, B * sizeof(int), cudaMemcpyDeviceToHost, s));
-    if (resid) CK(cudaMemcpyAsync(resid, h->d_resid, B * 3 * D, cudaMemcpyDeviceToHost, s));
+    if (status) CK(cudaMemcpyAsync(status, h->hb[0].status, B * sizeof(int), cudaMemcpyDeviceToHost, s));
+    if (iters) CK(cudaMemcpyAsync(iters, h->hb[0].iters, B * sizeof(int), cudaMemcpyDeviceToHost, s));
+    if (resid) CK(cudaMemcpyAsync(resid, h->hb[0].resid, B * 3 * D, cudaMemcpyDeviceToHost, s));
     if (flags) CK(cudaMemcpyAsync(flags, h->d_flags, B * sizeof(int), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     return LMPC_OK;
@@ -1270,9 +1169,9 @@ int lmpc_step_results(lmpc_handle* h, int* status, int* iters, double* resid, in
     if (rc) return rc;
     CK(cudaSetDevice(h->device));
     const size_t B = h->batch;
-    if (status) CK(cudaMemcpyAsync(status, h->d_status, sizeof(int) * B, cudaMemcpyDeviceToHost, h->stream));
-    if (iters) CK(cudaMemcpyAsync(iters, h->d_iters, sizeof(int) * B, cudaMemcpyDeviceToHost, h->stream));
-    if (resid) CK(cudaMemcpyAsync(resid, h->d_resid, sizeof(double) * B * 3, cudaMemcpyDeviceToHost, h->stream));
+    if (status) CK(cudaMemcpyAsync(status, h->hb[0].status, sizeof(int) * B, cudaMemcpyDeviceToHost, h->stream));
+    if (iters) CK(cudaMemcpyAsync(iters, h->hb[0].iters, sizeof(int) * B, cudaMemcpyDeviceToHost, h->stream));
+    if (resid) CK(cudaMemcpyAsync(resid, h->hb[0].resid, sizeof(double) * B * 3, cudaMemcpyDeviceToHost, h->stream));
     if (flags) CK(cudaMemcpyAsync(flags, h->d_flags, sizeof(int) * B, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     return LMPC_OK;
@@ -1280,11 +1179,12 @@ int lmpc_step_results(lmpc_handle* h, int* status, int* iters, double* resid, in
 
 void* lmpc_device_buffer(lmpc_handle* h, const char* name) {
     if (!h || !name) return nullptr;
+    const QpBufs& q = h->hb[0];
     struct { const char* n; void* p; } tab[] = {
-        {"xPred", h->d_xPred}, {"uPred", h->d_uPred}, {"lambd", h->d_lambd}, {"zt", h->d_zt}, {"zt_u", h->d_ztu},
-        {"abc", h->d_abc}, {"SS_sel", h->d_SS}, {"Qfun_sel", h->d_Qfun}, {"Succ_SS", h->d_SuccSS}, {"Succ_uSS", h->d_SuccU},
-        {"status", h->d_status}, {"iters", h->d_iters}, {"resid", h->d_resid}, {"flags", h->d_flags}, {"xLin", h->d_xLin},
-        {"uLin", h->d_uLin}, {"x0", h->d_x0}, {"slack", h->d_slack}, {"slackT", h->d_slackT}, {"OldInput", h->d_OldInput}, {"abc_lti", h->has_rollout ? h->d_abc_lti : nullptr}};
+        {"xPred", q.xPred}, {"uPred", q.uPred}, {"lambd", q.lambd}, {"zt", q.zt}, {"zt_u", q.ztu},
+        {"abc", q.abc}, {"SS_sel", q.SS}, {"Qfun_sel", q.Qfun}, {"Succ_SS", q.SuccSS}, {"Succ_uSS", q.SuccU},
+        {"status", q.status}, {"iters", q.iters}, {"resid", q.resid}, {"flags", h->d_flags}, {"xLin", h->d_xLin},
+        {"uLin", h->d_uLin}, {"x0", q.x0}, {"slack", q.slack}, {"slackT", q.slackT}, {"OldInput", h->d_OldInput}, {"abc_lti", h->has_rollout ? h->d_abc_lti : nullptr}};
     for (auto& e : tab) if (strcmp(e.n, name) == 0) return e.p;
     return nullptr;
 }
@@ -1375,16 +1275,17 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
     int rc = need_rollout(h);
     if (rc) return rc;
     CK(cudaSetDevice(h->device));
+    const QpBufs& q = h->hb[0];
     const double* xc = h->d_rx[h->cur];
     if (z_host) CK(cudaMemcpyAsync(h->d_z, z_host, sizeof(double) * h->batch * 3, cudaMemcpyHostToDevice, h->stream));
     StepTail tail;
     tail.xc = xc;
     SimArgs& sa = tail.sim;
-    sa.batch = h->batch; sa.x = xc; sa.xg = h->d_rg[h->cur]; sa.u = h->d_uPred; sa.u_stride = (long long)h->N * 2;
+    sa.batch = h->batch; sa.x = xc; sa.xg = h->d_rg[h->cur]; sa.u = q.uPred; sa.u_stride = (long long)h->N * 2;
     sa.z = z_host ? h->d_z : nullptr; sa.seed = seed; sa.step = h->sim_step;
     sa.xn = h->d_rx[h->cur ^ 1]; sa.xgn = h->d_rg[h->cur ^ 1];
     sa.cl_x = h->d_clx; sa.cl_u = h->d_clu; sa.cl_len = h->d_cllen; sa.Tcl = h->Tcl; sa.done = h->d_done; sa.active = nullptr;
-    sa.flags = h->d_flags; sa.status = h->d_status; sa.health = h->d_health;
+    sa.flags = h->d_flags; sa.status = q.status; sa.health = h->d_health;
     // the trace of the chosen controllers reads the step's results and the state before dynModel: it has to sit between the
     // solve and the simulator, so a traced batch runs the simulator for the whole batch after it
     const bool fused_tail = !h->has_trace && mode != 2;
@@ -1392,22 +1293,21 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
         CK(cudaMemsetAsync(h->d_flags, 0, sizeof(int) * h->batch, h->stream));
         // LTI MPC with the per-instance model identified by lmpc_rollout_sysid (main.py:72-80); like the reference's LTI
         // controller it never refreshes the input-rate reference (OldInput keeps its initial value, PC.py:113-115)
-        rc = lmpc_solve_mpc_dev(h, xc, h->d_OldInput, h->d_abc_lti, 54, 0, h->d_xPred, h->d_uPred, h->d_slack, h->d_status, h->d_iters,
-                                h->d_resid);
+        rc = lmpc_solve_mpc_dev(h, xc, h->d_OldInput, h->d_abc_lti, 54, 0, q.xPred, q.uPred, q.slack, q.status, q.iters, q.resid);
     } else {
         rc = step_dev_impl(h, mode, xc, nullptr, fused_tail ? &tail : nullptr);
     }
     if (rc) return rc;
     if (!fused_tail) {
         if (mode == 1) {
-            ss_add_point_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->batch, h->ss, h->d_prevslot, xc, h->d_uPred,
+            ss_add_point_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->batch, h->ss, h->d_prevslot, xc, q.uPred,
                                                                                 (long long)h->N * 2, h->mc.TrackLength, h->d_flags, nullptr, 0);
             CK(cudaGetLastError());
             h->launches += 1;
         }
         if (h->has_trace) {
-            trace_step_kernel<<<h->tr.n, 128, 0, h->stream>>>(h->tr, xc, h->d_rg[h->cur], h->d_uPred, (long long)h->N * 2, h->d_xPred,
-                                                            mode == 1 ? h->d_SS : nullptr, h->has_books ? h->bk.lap_n : nullptr);
+            trace_step_kernel<<<h->tr.n, 128, 0, h->stream>>>(h->tr, xc, h->d_rg[h->cur], q.uPred, (long long)h->N * 2, q.xPred,
+                                                            mode == 1 ? q.SS : nullptr, h->has_books ? h->bk.lap_n : nullptr);
             CK(cudaGetLastError());
             h->launches += 1;
         }
@@ -1432,10 +1332,10 @@ int lmpc_rollout_pid_step(lmpc_handle* h, double vt, const double* z_pid_host, c
     if (z_sim_host) CK(cudaMemcpyAsync(h->d_z, z_sim_host, sizeof(double) * h->batch * 3, cudaMemcpyHostToDevice, h->stream));
     PidArgs pa;
     pa.batch = h->batch; pa.x = xc; pa.vt = vt; pa.z = z_pid_host ? h->d_zpid : nullptr; pa.seed = seed; pa.step = h->sim_step;
-    pa.u = h->d_uPred; pa.u_stride = (long long)h->N * 2;
+    pa.u = h->hb[0].uPred; pa.u_stride = (long long)h->N * 2;
     pid_input_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(pa);
     SimArgs sa;
-    sa.batch = h->batch; sa.x = xc; sa.xg = h->d_rg[h->cur]; sa.u = h->d_uPred; sa.u_stride = (long long)h->N * 2;
+    sa.batch = h->batch; sa.x = xc; sa.xg = h->d_rg[h->cur]; sa.u = h->hb[0].uPred; sa.u_stride = (long long)h->N * 2;
     sa.z = z_sim_host ? h->d_z : nullptr; sa.seed = seed; sa.step = h->sim_step;
     sa.xn = h->d_rx[h->cur ^ 1]; sa.xgn = h->d_rg[h->cur ^ 1];
     sa.cl_x = h->d_clx; sa.cl_u = h->d_clu; sa.cl_len = h->d_cllen; sa.Tcl = h->Tcl; sa.done = h->d_done; sa.active = nullptr;

@@ -126,31 +126,3 @@ def test_index_is_required_with_params():
     with pytest.raises(ValueError):
         nat.make_param_sets(_base(), [rp.mpc_params(N)], None, B)
 
-
-def _kernel_body(path, name):
-    """Text of a __global__ kernel's body (after its opening line) up to its closing brace."""
-    import os
-    src = open(os.path.join(os.path.dirname(__file__), "..", "racinglmpc_b200", "csrc", path)).read()
-    i = src.index(" " + name + "(")
-    i = src.index("{\n", i) + 2
-    return src[i:src.index("\n}\n", i) + 1]
-
-
-def test_sets_kernel_is_the_uniform_kernel_plus_its_three_edits():
-    """ftocp_sets_kernel (ftocp_sets.cu) is kept textually separate from ftocp_kernel (lmpc_b200.cu) so that the uniform kernel's
-    code stays as it is; this pins the two together: applying the variant's three documented edits to the uniform kernel's body
-    gives the variant's body exactly, so a change to either that is not made to both fails here (at every horizon, not only at the
-    ones the GPU bit-identity tests run)."""
-    uni = _kernel_body("lmpc_b200.cu", "ftocp_kernel")
-    sets = _kernel_body("ftocp_sets.cu", "ftocp_sets_kernel")
-    edits = [
-        ("    using KS = KernelSmem<N, M, NCX, NCU>;\n", "    using KS = KernelSmemSets<N, M, NCX, NCU>;\n"),
-        ("(M > 0 ? (6 * M + M) * 8 : 0);\n        mbar_expect_tx(&ks.bar, bytes);\n",
-         "(M > 0 ? (6 * M + M) * 8 : 0) + (uint32_t)sizeof(FtocpConstRec);\n        mbar_expect_tx(&ks.bar, bytes);\n"
-         "        bulk_g2s(&ks.c, table + a.set_idx[b], sizeof(FtocpConstRec), &ks.bar);\n"),
-        ("    // ---- solve ----\n    SolveInfo info;\n", "    // ---- solve ----\n    const FtocpConst& c = ks.c.c;\n    SolveInfo info;\n"),
-    ]
-    for old, new in edits:
-        assert uni.count(old) == 1, old
-        uni = uni.replace(old, new)
-    assert uni == sets

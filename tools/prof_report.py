@@ -7,7 +7,7 @@ racinglmpc_b200/csrc/ftocp_pdip.cuh.  This is how the per-phase shares quoted in
 Needs a writable /tmp/cub scratch directory."""
 import os; os.makedirs("/tmp/cub", exist_ok=True)
 import re, csv, collections, subprocess, sys, os
-rep=sys.argv[1]; func=sys.argv[2]  # e.g. _Z12ftocp_kernelILi12ELi0ELi2ELi4EE
+rep=sys.argv[1]; func=sys.argv[2]  # e.g. _Z12ftocp_kernelILi12ELi0ELi2ELi4ELb0EE
 os.system('ncu -i %s --page raw --csv 2>/dev/null > /tmp/raw.csv'%rep)
 os.system('ncu -i %s --page source --csv 2>/dev/null > /tmp/src.csv'%rep)
 rows=list(csv.reader(open('/tmp/raw.csv'))); hdr=rows[0]; units=rows[1]; vals=rows[2]
