@@ -36,11 +36,15 @@ from racinglmpc_b200.controller import BatchedController                      # 
 
 
 def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, poll=8, max_steps=0, seed=1234, local=None, warm=False,
-        final=None, param_sets=None):
+        final=None, param_sets=None, vehicle_sets=None, books=None):
     """One Monte-Carlo run on this rank's GPU (torch.distributed may or may not be initialised).  Returns a dict (all ranks).
     final: None, or a dict that receives the closed loop's end state (rollout_state) and the last step's solver report (step_results).
+    books: None, or a dict that receives the lap books (books) and the health counters (flags_or, unsolved).
     param_sets: None, or (params, index, QterminalSlack) handed to BatchedController.set_param_sets after construction (a
-    parameter sweep over the batch; the result then holds per-set lap statistics under "per_set_rank0")."""
+    parameter sweep over the batch; the result then holds per-set lap statistics under "per_set_rank0").
+    vehicle_sets: None, or (vehicles, index) handed to BatchedController.set_vehicles (a sweep over the plant, PID lap included; the
+    result then holds per-vehicle lap statistics under "per_vehicle_rank0").  The pooled mode still exchanges laps between
+    controllers whatever their car, so plant sweeps run in the independent mode."""
     rank = dist.get_rank() if dist.is_initialized() else 0
     world = dist.get_world_size() if dist.is_initialized() else 1
     local = int(os.environ.get("LOCAL_RANK", 0)) if local is None else local
@@ -52,6 +56,8 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
                           numSS_it=numSS_it, QterminalSlack=Qts, device=local, Tmax=1280, ss_cap=7, model_cap=5, warm_start=warm)
     if param_sets is not None:
         c.set_param_sets(*param_sets)
+    if vehicle_sets is not None:
+        c.set_vehicles(*vehicle_sets)
     stream = torch.cuda.ExternalStream(c.stream, device=dev)
     x0 = np.tile(np.array([0.5, 0, 0, 0, 0, 0.0]), (B, 1))
     # ---- main.py:65-66 + 99-110 on the device: every controller drives its OWN PID lap (the full 100 s) and is seeded with it
@@ -133,15 +139,20 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     if param_sets is not None:
         idx = np.asarray(param_sets[1]).reshape(B)
         out["per_set_rank0"] = [_set_stats(bk, flags_or, unsolved, idx == k, laps) for k in range(len(param_sets[0]))]
+    if vehicle_sets is not None:
+        idx = np.asarray(vehicle_sets[1]).reshape(B)
+        out["per_vehicle_rank0"] = [_set_stats(bk, flags_or, unsolved, idx == k, laps) for k in range(len(vehicle_sets[0]))]
     if final is not None:
         final.update(c.rollout_state())
         final.update(c.step_results())
+    if books is not None:
+        books.update(bk, flags_or=flags_or, unsolved=unsolved)
     c.close()
     return out
 
 
 def _set_stats(bk, flags_or, unsolved, sel, laps):
-    """Lap lengths (mean / min per LMPC lap), unsolved steps and flagged controllers of the controllers `sel` of one parameter set."""
+    """Lap lengths (mean / min per LMPC lap), unsolved steps and flagged controllers of the controllers `sel` of one parameter set or vehicle."""
     laps_out = []
     for r in range(laps):
         m = sel & (bk["lap_n"] > r)

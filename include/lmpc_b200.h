@@ -269,6 +269,25 @@ int lmpc_rollout_get_health(lmpc_handle* h, int* flags_or, int* unsolved_steps);
  *   regression model (the caller's lap books must say the same: lmpc_ss_set_selection / lmpc_model_set_used), xLin/uLin/zt/
  *   OldInput/timeStep are initialised as LMPC.__init__/addTrajectory do, the record restarts. */
 int lmpc_rollout_pid_step(lmpc_handle* h, double vt, const double* z_pid_host, const double* z_sim_host, unsigned long long seed);
+
+/* Vehicle of the device simulator: the ten constants of Simulator.dynModel (SysModel.py:61-70). */
+typedef struct lmpc_vehicle_params {
+    double m, lf, lr, Iz;         /* mass, CoG to front / rear axle, yaw inertia: 1.98, 0.125, 0.125, 0.024 */
+    double Df, Cf, Bf;            /* front Pacejka: Fyf = Df sin(Cf atan(Bf alpha_f)); 0.8 * m * 9.81 / 2.0, 1.25, 1.0 */
+    double Dr, Cr, Br;            /* rear, the same form */
+} lmpc_vehicle_params;
+/* Per-controller vehicles (Monte-Carlo over the plant; no reference counterpart: the reference simulates one car).  Controller b is
+ * simulated with sets[set_of_instance[b]] (host arrays) by every later lmpc_rollout_step (modes 0, 1, 2) and lmpc_rollout_pid_step,
+ * so the PID lap that seeds both stores, the LTI sysid and the learned models all see that controller's own car.  nsets == 0
+ * (sets, set_of_instance NULL) returns to the reference vehicle, which every handle starts with.
+ *   - 1 <= nsets <= batch, every index in [0, nsets); m, Iz, lf, lr > 0 and all ten values finite.
+ *   - Any failed check returns LMPC_E_INVALID and leaves the handle as it was.
+ *   - The call synchronises the handle's streams before it replaces the table.
+ *   - The vehicle index is independent of the parameter-set index of lmpc_set_param_sets (crossed designs work).  The QP entry
+ *     points, the noise model, dt and the 1 ms sub-step are unchanged.
+ *   - The pooled safe-set exchange (lmpc_pool_*, lmpc_ss_import_laps_dev) still hands laps between all controllers whatever their
+ *     car; a lap another car drove is not a feasible trajectory of this one, so clean plant sweeps run in the independent mode. */
+int lmpc_rollout_set_vehicles(lmpc_handle* h, const lmpc_vehicle_params* sets, int nsets, const int* set_of_instance);
 int lmpc_rollout_sysid(lmpc_handle* h, double lamb, double* abc_host, int* flags_host);
 int lmpc_rollout_seed_from_record(lmpc_handle* h, int copies, int ss_slot0, int model_slot0);
 int lmpc_rollout_get_lap(lmpc_handle* h, int inst, int* T, double* x, double* u);              /* closed-loop record   */
@@ -347,6 +366,7 @@ int lmpc_probe_fp64(int device, double* out8);
 
 int lmpc_sizeof_params(void);
 int lmpc_sizeof_model_params(void);
+int lmpc_sizeof_vehicle_params(void);
 
 #ifdef __cplusplus
 }

@@ -29,6 +29,11 @@ class ModelParams(C.Structure):
                 ("seg", C.c_double * (MAX_SEG * 3)), ("TrackLength", C.c_double)]
 
 
+class VehicleParams(C.Structure):
+    """lmpc_vehicle_params: the ten constants of Simulator.dynModel (SysModel.py:61-70)."""
+    _fields_ = [(f, C.c_double) for f in ("m", "lf", "lr", "Iz", "Df", "Cf", "Bf", "Dr", "Cr", "Br")]
+
+
 class NativeError(RuntimeError):
     pass
 
@@ -95,6 +100,7 @@ def lib():
     L.lmpc_rollout_step.argtypes = [_vp, C.c_int, _vp, C.c_ulonglong]
     L.lmpc_rollout_get_health.argtypes = [_vp, _vp, _vp]
     L.lmpc_rollout_pid_step.argtypes = [_vp, C.c_double, _vp, _vp, C.c_ulonglong]
+    L.lmpc_rollout_set_vehicles.argtypes = [_vp, C.POINTER(VehicleParams), C.c_int, _vp]
     L.lmpc_rollout_sysid.argtypes = [_vp, C.c_double, _vp, _vp]
     L.lmpc_rollout_seed_from_record.argtypes = [_vp, C.c_int, C.c_int, C.c_int]
     L.lmpc_rollout_get_lap.argtypes = [_vp, C.c_int, ip, _vp, _vp]
@@ -120,8 +126,10 @@ def lib():
     L.lmpc_host_page_nodes.argtypes = [_vp, C.c_size_t, C.c_int, _vp]
     L.lmpc_sizeof_params.restype = C.c_int
     L.lmpc_sizeof_model_params.restype = C.c_int
+    L.lmpc_sizeof_vehicle_params.restype = C.c_int
     assert L.lmpc_sizeof_params() == C.sizeof(Params), "lmpc_params ABI mismatch"
     assert L.lmpc_sizeof_model_params() == C.sizeof(ModelParams), "lmpc_model_params ABI mismatch"
+    assert L.lmpc_sizeof_vehicle_params() == C.sizeof(VehicleParams), "lmpc_vehicle_params ABI mismatch"
     _LIB = L
     return L
 
@@ -250,23 +258,30 @@ def make_params(p, numSS_Points=0, numSS_it=0, QterminalSlack=None, eps_res=0.0,
     return q
 
 
+def _set_index(index, K, batch, what):
+    """The index rules of the per-controller tables (lmpc_set_param_sets, lmpc_rollout_set_vehicles): 1 <= K <= batch rows and
+    one integer row number in [0, K) per controller.  Returns the index as a contiguous int32 array; raises ValueError."""
+    if index is None:
+        raise ValueError("index is required: one set number per controller (%d)" % batch)
+    if not 1 <= K <= batch:
+        raise ValueError("need 1 .. batch (= %d) %s, got %d" % (batch, what, K))
+    idx = np.ascontiguousarray(np.asarray(index).reshape(-1), dtype=np.int32)
+    if idx.shape[0] != batch or not np.array_equal(idx, np.asarray(index).reshape(-1)):
+        raise ValueError("index must hold one integer set number per controller (%d)" % batch)
+    if idx.min() < 0 or idx.max() >= K:
+        raise ValueError("set index out of range [0, %d)" % K)
+    return idx
+
+
 def make_param_sets(base, params, index, batch, numSS_Points=0, numSS_it=0, QterminalSlack=None):
     """Per-controller parameters for ``lmpc_set_param_sets``: K MPCParams-like objects ``params``, the set of every controller
     ``index[batch]`` and ``QterminalSlack`` (None: the base's, or one 6x6 matrix per set).  ``base`` is the handle's own ``Params``;
     the interior-point settings (tolerances, max_iter, warm_start) are taken from it.  Each set is converted by ``make_params``.
     Raises ValueError where the library would refuse: an index of the wrong length or out of range, or a set that differs from
     the base in N, the rows of Fx or Fu, slacks or n/d.  Returns (ctypes array Params * K, int32 index array)."""
-    if index is None:
-        raise ValueError("index is required: one set number per controller (%d)" % batch)
     params = list(params)
     K = len(params)
-    if not 1 <= K <= batch:
-        raise ValueError("need 1 .. batch (= %d) parameter sets, got %d" % (batch, K))
-    idx = np.ascontiguousarray(np.asarray(index).reshape(-1), dtype=np.int32)
-    if idx.shape[0] != batch or not np.array_equal(idx, np.asarray(index).reshape(-1)):
-        raise ValueError("index must hold one integer set number per controller (%d)" % batch)
-    if idx.min() < 0 or idx.max() >= K:
-        raise ValueError("set index out of range [0, %d)" % K)
+    idx = _set_index(index, K, batch, "parameter sets")
     if QterminalSlack is None:
         qts = [np.ctypeslib.as_array(base.QterminalSlack).reshape(6, 6).copy()] * K
     else:
@@ -282,4 +297,26 @@ def make_param_sets(base, params, index, batch, numSS_Points=0, numSS_it=0, Qter
         if (s.numSS_Points, s.numSS_it) != (base.numSS_Points, base.numSS_it):
             raise ValueError("set %d: numSS_Points / numSS_it differ from the handle's" % k)
         out[k] = s
+    return out, idx
+
+
+VEHICLE_FIELDS = tuple(f for f, _ in VehicleParams._fields_)
+
+
+def make_vehicle_sets(vehicles, index, batch):
+    """Per-controller vehicles for ``lmpc_rollout_set_vehicles``: K objects ``vehicles`` with the reference's field names (m, lf,
+    lr, Iz, Df, Cf, Bf, Dr, Cr, Br; e.g. reference_params.VehicleParams) and the vehicle of every controller ``index[batch]``.
+    Raises ValueError where the library would refuse: the index rules of ``make_param_sets``, a non-positive m, Iz, lf or lr,
+    or a value that is not finite.  Returns (ctypes array VehicleParams * K, int32 index array)."""
+    vehicles = list(vehicles)
+    K = len(vehicles)
+    idx = _set_index(index, K, batch, "vehicles")
+    out = (VehicleParams * K)()
+    for k, v in enumerate(vehicles):
+        vals = [float(getattr(v, f)) for f in VEHICLE_FIELDS]
+        if not all(np.isfinite(vals)):
+            raise ValueError("vehicle %d: every value must be finite" % k)
+        if min(v.m, v.Iz, v.lf, v.lr) <= 0:
+            raise ValueError("vehicle %d: m, Iz, lf and lr must be positive" % k)
+        out[k] = VehicleParams(*vals)
     return out, idx

@@ -101,6 +101,19 @@ class BatchedController:
         sets, idx = nat.make_param_sets(self._p, params, index, self.B, self._p.numSS_Points, self.numSS_it, QterminalSlack)
         nat.check(self._lib.lmpc_set_param_sets(self._h, sets, len(sets), nat.ptr(idx)))
 
+    def set_vehicles(self, vehicles, index=None):
+        """Per-controller vehicles of the device simulator (a Monte-Carlo over the plant in one batch): controller b is driven
+        with ``vehicles[index[b]]`` (objects with the reference's ten field names, e.g. reference_params.VehicleParams) by every
+        later ``rollout_step`` and ``rollout_pid_step``.  ``index`` is required with ``vehicles``.  ``vehicles=None`` (no index)
+        returns to the reference vehicle.  Independent of ``set_param_sets``.  Waits for work already enqueued."""
+        if vehicles is None:
+            if index is not None:
+                raise ValueError("vehicles=None reverts to the reference vehicle and takes no index")
+            nat.check(self._lib.lmpc_rollout_set_vehicles(self._h, None, 0, None))
+            return
+        sets, idx = nat.make_vehicle_sets(vehicles, index, self.B)
+        nat.check(self._lib.lmpc_rollout_set_vehicles(self._h, sets, len(sets), nat.ptr(idx)))
+
     # ------------------------------------------------------------------ PredictiveModel.addTrajectory
     def model_add_trajectory(self, inst, x, u):
         """PredictiveModel.py:35-46: keep laps sorted by length; only the trToUse fastest are ever read."""

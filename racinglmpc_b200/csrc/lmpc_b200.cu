@@ -100,6 +100,10 @@ struct lmpc_handle {
     unsigned long long sim_step;
     double *d_rx[2], *d_rg[2], *d_clx, *d_clu, *d_z, *d_zpid, *d_abc_lti;
     int *d_cllen, *d_done, cur;
+    // vehicles of the simulator (lmpc_rollout_set_vehicles): table lmpc_vehicle_params[nsets] and vehicle index [batch]; without
+    // sets a one-row table holding the reference vehicle and a null index (allocated at creation)
+    lmpc_vehicle_params* d_veh;
+    int* d_veh_idx;
     // device lap books (lapbooks.cuh): slot tables of both pools, lap history, exchange scratch
     LapBooks bk;
     int *d_bkbuf, *d_poolidx, *d_stats;
@@ -160,6 +164,58 @@ static int build_const(const lmpc_params& p, FtocpConst& c) {
     c.d4_min = 1e-6;
     c.max_iter = p.max_iter > 0 ? p.max_iter : 40;
     return LMPC_OK;
+}
+
+// Per-controller tables (lmpc_set_param_sets, lmpc_rollout_set_vehicles): `nsets` rows and one row index per controller.
+// The argument rules both calls share: 0 <= nsets <= batch, nsets == 0 exactly when both arrays are NULL, every index in range.
+static int check_set_index(const lmpc_handle* h, const char* who, const void* sets, int nsets, const int* set_of_instance) {
+    const std::string w(who);
+    if (nsets < 0 || nsets > h->batch) return fail(LMPC_E_INVALID, w + ": nsets must be 0 .. batch");
+    if ((nsets == 0) != (sets == nullptr) || (nsets == 0) != (set_of_instance == nullptr))
+        return fail(LMPC_E_INVALID, w + ": nsets == 0 goes with NULL sets and set_of_instance, nsets >= 1 with both");
+    for (int b = 0; b < (nsets ? h->batch : 0); ++b)
+        if (set_of_instance[b] < 0 || set_of_instance[b] >= nsets)
+            return fail(LMPC_E_INVALID, w + ": set index of instance " + std::to_string(b) + " out of range");
+    return LMPC_OK;
+}
+
+// Once the handle's streams are idle, replace the table *tab by rows[nrows] (none when nrows == 0) and the index *idx by
+// set_of_instance[batch] (none when it is NULL).  The handle keeps its old table unless every allocation and copy succeeds.
+template <typename T>
+static int swap_table(lmpc_handle* h, const char* who, const T* rows, int nrows, const int* set_of_instance, T** tab, int** idx) {
+    CK(cudaSetDevice(h->device));
+    // batches already enqueued (the _async entry points, the device-resident step) finish with the table they were enqueued with
+    CK(cudaStreamSynchronize(h->stream));
+    for (int i = 0; i < 4 * LMPC_HOST_SLOTS; ++i) CK(cudaStreamSynchronize(h->cstream[i]));
+    T* t = nullptr;
+    int* ix = nullptr;
+    cudaError_t e = cudaSuccess;
+    if (nrows > 0) {
+        e = cudaMalloc((void**)&t, sizeof(T) * nrows);
+        if (e == cudaSuccess) e = cudaMemcpy(t, rows, sizeof(T) * nrows, cudaMemcpyHostToDevice);
+    }
+    if (e == cudaSuccess && set_of_instance) {
+        e = cudaMalloc((void**)&ix, sizeof(int) * h->batch);
+        if (e == cudaSuccess) e = cudaMemcpy(ix, set_of_instance, sizeof(int) * h->batch, cudaMemcpyHostToDevice);
+    }
+    if (e != cudaSuccess) {
+        cudaFree(t); cudaFree(ix);
+        return fail(LMPC_E_CUDA, std::string(who) + ": " + cudaGetErrorString(e));
+    }
+    cudaFree(*tab);
+    cudaFree(*idx);
+    *tab = t;
+    *idx = ix;
+    return LMPC_OK;
+}
+
+// Simulator.dynModel's vehicle (SysModel.py:61-70), D in the reference's operation order
+static lmpc_vehicle_params reference_vehicle() {
+    lmpc_vehicle_params v;
+    v.m = 1.98; v.lf = 0.125; v.lr = 0.125; v.Iz = 0.024;
+    v.Df = 0.8 * v.m * 9.81 / 2.0; v.Cf = 1.25; v.Bf = 1.0;
+    v.Dr = 0.8 * v.m * 9.81 / 2.0; v.Cr = 1.25; v.Br = 1.0;
+    return v;
 }
 
 template <int N, int M>
@@ -293,7 +349,8 @@ static int create_device_side(lmpc_handle* h) {
     if (!qp_bufs(h, 0)) return LMPC_E_CUDA;
     CK(cudaMalloc((void**)&h->d_late, sizeof(unsigned long long)));
     CK(cudaMemset(h->d_late, 0, sizeof(unsigned long long)));
-    return LMPC_OK;
+    const lmpc_vehicle_params ref = reference_vehicle();
+    return swap_table(h, "lmpc_create", &ref, 1, nullptr, &h->d_veh, &h->d_veh_idx);
 }
 
 extern "C" {
@@ -440,6 +497,8 @@ int lmpc_destroy(lmpc_handle* h) {
     cudaFree(h->d_late);
     cudaFree(h->d_sets);
     cudaFree(h->d_set_idx);
+    cudaFree(h->d_veh);
+    cudaFree(h->d_veh_idx);
     if (h->stream) cudaStreamDestroy(h->stream);
     for (int i = 0; i < 4 * LMPC_HOST_SLOTS; ++i) if (h->cstream[i]) cudaStreamDestroy(h->cstream[i]);
     if (h->ev_fork) cudaEventDestroy(h->ev_fork);
@@ -471,9 +530,8 @@ long long lmpc_kernel_launches(lmpc_handle* h) { return h ? h->launches : 0; }
 // previous one once the handle's streams are idle.  Nothing about the handle changes unless every check passes.
 int lmpc_set_param_sets(lmpc_handle* h, const lmpc_params* sets, int nsets, const int* set_of_instance) {
     if (!h) return fail(LMPC_E_INVALID, "null handle");
-    if (nsets < 0 || nsets > h->batch) return fail(LMPC_E_INVALID, "lmpc_set_param_sets: nsets must be 0 .. batch");
-    if ((nsets == 0) != (sets == nullptr) || (nsets == 0) != (set_of_instance == nullptr))
-        return fail(LMPC_E_INVALID, "lmpc_set_param_sets: nsets == 0 goes with NULL sets and set_of_instance, nsets >= 1 with both");
+    int rc = check_set_index(h, "lmpc_set_param_sets", sets, nsets, set_of_instance);
+    if (rc != LMPC_OK) return rc;
     std::vector<FtocpConstRec> rows(nsets);
     for (int k = 0; k < nsets; ++k) {
         const lmpc_params& s = sets[k];
@@ -481,32 +539,10 @@ int lmpc_set_param_sets(lmpc_handle* h, const lmpc_params* sets, int nsets, cons
             s.numSS_it != h->p.numSS_it || s.warm_start != h->p.warm_start)
             return fail(LMPC_E_INVALID, "lmpc_set_param_sets: set " + std::to_string(k) +
                                             " differs from the handle in N, ncx, ncu, numSS_Points, numSS_it or warm_start");
-        const int rc = build_const(s, rows[k].c);
+        rc = build_const(s, rows[k].c);
         if (rc != LMPC_OK) return fail(rc, "lmpc_set_param_sets: set " + std::to_string(k) + ": " + g_err);
     }
-    for (int b = 0; b < (nsets ? h->batch : 0); ++b)
-        if (set_of_instance[b] < 0 || set_of_instance[b] >= nsets)
-            return fail(LMPC_E_INVALID, "lmpc_set_param_sets: set index of instance " + std::to_string(b) + " out of range");
-    CK(cudaSetDevice(h->device));
-    // batches already enqueued (the _async entry points, the device-resident step) finish with the parameters they were enqueued with
-    CK(cudaStreamSynchronize(h->stream));
-    for (int i = 0; i < 4 * LMPC_HOST_SLOTS; ++i) CK(cudaStreamSynchronize(h->cstream[i]));
-    FtocpConstRec* tab = nullptr;
-    int* idx = nullptr;
-    if (nsets > 0) {
-        cudaError_t e = cudaMalloc((void**)&tab, sizeof(FtocpConstRec) * nsets);
-        if (e == cudaSuccess) e = cudaMalloc((void**)&idx, sizeof(int) * h->batch);
-        if (e == cudaSuccess) e = cudaMemcpy(tab, rows.data(), sizeof(FtocpConstRec) * nsets, cudaMemcpyHostToDevice);
-        if (e == cudaSuccess) e = cudaMemcpy(idx, set_of_instance, sizeof(int) * h->batch, cudaMemcpyHostToDevice);
-        if (e != cudaSuccess) {
-            cudaFree(tab); cudaFree(idx);
-            return fail(LMPC_E_CUDA, std::string("lmpc_set_param_sets: ") + cudaGetErrorString(e));
-        }
-    }
-    cudaFree(h->d_sets);
-    cudaFree(h->d_set_idx);
-    h->d_sets = tab;
-    h->d_set_idx = idx;
+    if ((rc = swap_table(h, "lmpc_set_param_sets", rows.data(), nsets, set_of_instance, &h->d_sets, &h->d_set_idx)) != LMPC_OK) return rc;
     // a warm-start record belongs to the QP it was taken from
     if (h->d_warm_valid) {
         CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * h->batch, h->stream));
@@ -718,6 +754,7 @@ int lmpc_solve_mpc_host(lmpc_handle* h, const double* x0, const double* uOld, co
 // ================================================================================================
 int lmpc_sizeof_params(void) { return (int)sizeof(lmpc_params); }
 int lmpc_sizeof_model_params(void) { return (int)sizeof(lmpc_model_params); }
+int lmpc_sizeof_vehicle_params(void) { return (int)sizeof(lmpc_vehicle_params); }
 
 static int store_create_impl(lmpc_handle* h, const lmpc_model_params* mp, int ss_cap, int model_cap, int Tmax);
 int lmpc_store_create(lmpc_handle* h, const lmpc_model_params* mp, int ss_cap, int model_cap, int Tmax) {
@@ -1286,6 +1323,7 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
     sa.xn = h->d_rx[h->cur ^ 1]; sa.xgn = h->d_rg[h->cur ^ 1];
     sa.cl_x = h->d_clx; sa.cl_u = h->d_clu; sa.cl_len = h->d_cllen; sa.Tcl = h->Tcl; sa.done = h->d_done; sa.active = nullptr;
     sa.flags = h->d_flags; sa.status = q.status; sa.health = h->d_health;
+    sa.veh = h->d_veh; sa.veh_idx = h->d_veh_idx;
     // the trace of the chosen controllers reads the step's results and the state before dynModel: it has to sit between the
     // solve and the simulator, so a traced batch runs the simulator for the whole batch after it
     const bool fused_tail = !h->has_trace && mode != 2;
@@ -1340,6 +1378,7 @@ int lmpc_rollout_pid_step(lmpc_handle* h, double vt, const double* z_pid_host, c
     sa.xn = h->d_rx[h->cur ^ 1]; sa.xgn = h->d_rg[h->cur ^ 1];
     sa.cl_x = h->d_clx; sa.cl_u = h->d_clu; sa.cl_len = h->d_cllen; sa.Tcl = h->Tcl; sa.done = h->d_done; sa.active = nullptr;
     sa.flags = nullptr; sa.status = nullptr; sa.health = nullptr;
+    sa.veh = h->d_veh; sa.veh_idx = h->d_veh_idx;
     sim_step_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->mc, sa);
     CK(cudaGetLastError());
     h->launches += 2;
@@ -1347,6 +1386,29 @@ int lmpc_rollout_pid_step(lmpc_handle* h, double vt, const double* z_pid_host, c
     h->sim_step += 1;
     if (z_pid_host || z_sim_host) CK(cudaStreamSynchronize(h->stream));   // pageable host arrays of the caller
     return LMPC_OK;
+}
+
+// Per-controller vehicles: every set is checked, then the table replaces the previous one once the handle's streams are idle.
+// Nothing about the handle changes unless every check passes.
+int lmpc_rollout_set_vehicles(lmpc_handle* h, const lmpc_vehicle_params* sets, int nsets, const int* set_of_instance) {
+    static const char* who = "lmpc_rollout_set_vehicles";
+    if (!h) return fail(LMPC_E_INVALID, "null handle");
+    int rc = check_set_index(h, who, sets, nsets, set_of_instance);
+    if (rc != LMPC_OK) return rc;
+    for (int k = 0; k < nsets; ++k) {
+        const lmpc_vehicle_params& v = sets[k];
+        const double all[10] = {v.m, v.lf, v.lr, v.Iz, v.Df, v.Cf, v.Bf, v.Dr, v.Cr, v.Br};
+        bool ok = v.m > 0 && v.Iz > 0 && v.lf > 0 && v.lr > 0;
+        for (double x : all) ok = ok && isfinite(x);
+        if (!ok)
+            return fail(LMPC_E_INVALID, std::string(who) + ": vehicle " + std::to_string(k) +
+                                            ": m, Iz, lf, lr must be positive and all ten values finite");
+    }
+    if (nsets == 0) {
+        const lmpc_vehicle_params ref = reference_vehicle();
+        return swap_table(h, who, &ref, 1, nullptr, &h->d_veh, &h->d_veh_idx);
+    }
+    return swap_table(h, who, sets, nsets, set_of_instance, &h->d_veh, &h->d_veh_idx);
 }
 
 // Regression(x, u, lamb) of Utilities.py:5-28 on every instance's closed-loop record: per-instance LTI model in the device

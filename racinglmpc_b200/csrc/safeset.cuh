@@ -788,6 +788,9 @@ __global__ void shift_state_kernel(const ShiftArgs a) {
 // np.random.randn() in this order: vx, vy, wz); when z == nullptr they come from Philox4x32-10 keyed by
 // (seed, instance, step) — statistical, not bit-wise, parity with the reference's unseeded global RNG.
 // Also appends (x, u) to the closed-loop buffer and flags lap completion (SysModel.py:45-47).
+// The ten vehicle constants (SysModel.py:61-70) are read from a per-instance record: row veh_idx[b] of veh, or row 0 when veh_idx
+// is null (a handle without vehicle sets points at a one-row table holding the reference vehicle).  The arithmetic is the same
+// with the constants in memory as with them folded in at compile time (DESIGN.md, "Per-controller vehicles").
 struct SimArgs {
     int batch;
     int b0 = 0, b1 = -1;   // instance range [b0, b1) of this launch (b1 < 0: up to batch); arrays stay globally indexed
@@ -808,6 +811,8 @@ struct SimArgs {
     const int* flags;      // [B] step flags (K1/K2/addPoint) and QP status of the step that produced u, or nullptr;
     const int* status;     //     accumulated into health[b] (OR of flags) and health[B + b] (steps with status != 1)
     int* health;
+    const lmpc_vehicle_params* veh;   // vehicle table (lmpc_rollout_set_vehicles)
+    const int* veh_idx;               // [B] row of every instance, or nullptr: row 0
 };
 
 }  // namespace lmpc
@@ -823,9 +828,10 @@ __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimA
         if (a.status && a.status[b] != 1) a.health[a.batch + b] += 1;
     }
     // vehicle parameters, SysModel.py:61-70
-    const double mass = 1.98, lf = 0.125, lr = 0.125, Iz = 0.024;
-    const double Df = 0.8 * mass * 9.81 / 2.0, Cf = 1.25, Bf = 1.0;
-    const double Dr = 0.8 * mass * 9.81 / 2.0, Cr = 1.25, Br = 1.0;
+    const lmpc_vehicle_params& v = a.veh[a.veh_idx ? a.veh_idx[b] : 0];
+    const double mass = v.m, lf = v.lf, lr = v.lr, Iz = v.Iz;
+    const double Df = v.Df, Cf = v.Cf, Bf = v.Bf;
+    const double Dr = v.Dr, Cr = v.Cr, Br = v.Br;
     const double h = 0.001;
     const double* x = a.x + (size_t)b * 6;
     const double* g = a.xg + (size_t)b * 6;

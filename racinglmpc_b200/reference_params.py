@@ -1,5 +1,6 @@
 """The reference's tuning constants, values only (src/initControllerParameters.py:4-58, src/main.py:43-50).
 They define the benchmark configurations of BASELINE.json; nothing here is executed by the reference."""
+from dataclasses import dataclass
 from types import SimpleNamespace
 import numpy as np
 
@@ -32,3 +33,32 @@ def lmpc_params(N=12):
                         Fx=Fx, bx=np.array([HALF_WIDTH, HALF_WIDTH]), Fu=Fu, bu=bu, xRef=np.zeros(6),
                         slacks=True, timeVarying=True)
     return 4, 48, 44, 400, 500 * np.eye(6), p
+
+
+@dataclass(frozen=True)
+class VehicleParams:
+    """The vehicle of Simulator.dynModel (SysModel.py:61-70): mass, CoG to front / rear axle, yaw inertia and the Pacejka
+    coefficients of the front and rear tyre, Fy = D sin(C atan(B alpha)).  The device simulator takes one per controller
+    (BatchedController.set_vehicles)."""
+    m: float
+    lf: float
+    lr: float
+    Iz: float
+    Df: float
+    Cf: float
+    Bf: float
+    Dr: float
+    Cr: float
+    Br: float
+
+    @classmethod
+    def reference(cls):
+        """The reference's car: friction coefficient 0.8."""
+        return cls.from_friction(0.8)
+
+    @classmethod
+    def from_friction(cls, mu, m=1.98, lf=0.125, lr=0.125, Iz=0.024, Cf=1.25, Bf=1.0, Cr=1.25, Br=1.0):
+        """Peak tyre force D = mu * m * 9.81 / 2.0 on both axles, in the reference's operation order (mu = 0.8 gives its D bit
+        for bit)."""
+        D = mu * m * 9.81 / 2.0
+        return cls(m, lf, lr, Iz, D, Cf, Bf, D, Cr, Br)
