@@ -36,7 +36,7 @@ from racinglmpc_b200.controller import BatchedController                      # 
 
 
 def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, poll=8, max_steps=0, seed=1234, local=None, warm=False,
-        final=None, param_sets=None, vehicle_sets=None, books=None):
+        final=None, param_sets=None, vehicle_sets=None, books=None, track_sets=None):
     """One Monte-Carlo run on this rank's GPU (torch.distributed may or may not be initialised).  Returns a dict (all ranks).
     final: None, or a dict that receives the closed loop's end state (rollout_state) and the last step's solver report (step_results).
     books: None, or a dict that receives the lap books (books) and the health counters (flags_or, unsolved).
@@ -44,7 +44,12 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     parameter sweep over the batch; the result then holds per-set lap statistics under "per_set_rank0").
     vehicle_sets: None, or (vehicles, index) handed to BatchedController.set_vehicles (a sweep over the plant, PID lap included; the
     result then holds per-vehicle lap statistics under "per_vehicle_rank0").  The pooled mode still exchanges laps between
-    controllers whatever their car, so plant sweeps run in the independent mode."""
+    controllers whatever their car, so plant sweeps run in the independent mode.
+    track_sets: None, or (tracks, index) handed to BatchedController.set_tracks (several circuits in one batch; the result then
+    holds per-track lap statistics under "per_track_rank0").  A lap of another circuit is not a trajectory of this one, so more
+    than one track runs in the independent mode only (ValueError otherwise, raised before any collective)."""
+    if track_sets is not None and mode == "pooled" and len(track_sets[0]) > 1:
+        raise ValueError("the pooled mode exchanges laps between controllers: it needs one track, got %d" % len(track_sets[0]))
     rank = dist.get_rank() if dist.is_initialized() else 0
     world = dist.get_world_size() if dist.is_initialized() else 1
     local = int(os.environ.get("LOCAL_RANK", 0)) if local is None else local
@@ -58,6 +63,8 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         c.set_param_sets(*param_sets)
     if vehicle_sets is not None:
         c.set_vehicles(*vehicle_sets)
+    if track_sets is not None:
+        c.set_tracks(*track_sets)
     stream = torch.cuda.ExternalStream(c.stream, device=dev)
     x0 = np.tile(np.array([0.5, 0, 0, 0, 0, 0.0]), (B, 1))
     # ---- main.py:65-66 + 99-110 on the device: every controller drives its OWN PID lap (the full 100 s) and is seeded with it
@@ -142,6 +149,9 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     if vehicle_sets is not None:
         idx = np.asarray(vehicle_sets[1]).reshape(B)
         out["per_vehicle_rank0"] = [_set_stats(bk, flags_or, unsolved, idx == k, laps) for k in range(len(vehicle_sets[0]))]
+    if track_sets is not None:
+        idx = np.asarray(track_sets[1]).reshape(B)
+        out["per_track_rank0"] = [_set_stats(bk, flags_or, unsolved, idx == k, laps) for k in range(len(track_sets[0]))]
     if final is not None:
         final.update(c.rollout_state())
         final.update(c.step_results())

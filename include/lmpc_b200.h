@@ -189,6 +189,28 @@ int lmpc_solve_lmpc_dev(lmpc_handle* h, const double* x0, const double* uOld, co
  */
 int lmpc_store_create(lmpc_handle* h, const lmpc_model_params* mp, int ss_cap, int model_cap, int Tmax);
 
+/* A circuit: the table Map.curvature reads (Track.py:292-310) and the lap length. */
+typedef struct lmpc_track_params {
+    int nseg;                         /* rows of the table, 1 .. LMPC_MAX_SEG                        */
+    double seg[LMPC_MAX_SEG * 3];     /* [s_start, length, curvature] = Map.PointAndTangent[:,3:6]   */
+    double TrackLength;
+} lmpc_track_params;
+/* Per-controller tracks (several circuits in one batch; no reference counterpart: the reference drives one track).  Controller b
+ * uses sets[set_of_instance[b]] (host arrays) in every later regression (curvature), safe-set selection (lap-wrap fix, Q-function
+ * shift), addPoint, lap cost, lap hand-over and simulator launch, host-driven and device-resident alike.  nsets == 0 (sets,
+ * set_of_instance NULL) returns every controller to the track of lmpc_store_create, which every store starts with.
+ *   - Requires lmpc_store_create (else LMPC_E_STATE), and no lap stored yet in either pool by any entry point (put_lap, seeding,
+ *     commit, import; else LMPC_E_STATE): a stored lap is in the s-coordinate of the track it was driven on.
+ *   - 1 <= nsets <= batch, every index in [0, nsets); per set: 1 <= nseg <= LMPC_MAX_SEG, all values finite, lengths >= 0,
+ *     seg start 0 == 0, start i == start i-1 + length i-1 exactly, TrackLength == start + length of the last row exactly and > 0
+ *     (the way Track.py:54-133 builds the table).  Any failed check returns LMPC_E_INVALID and leaves the handle as it was.
+ *   - The call synchronises the handle's streams before it replaces the table.
+ *   - The track index is independent of the parameter-set and the vehicle index (crossed designs work).  The lane half-width
+ *     enters the QP through Fx/bx (lmpc_set_param_sets), not through this table.
+ *   - While more than one set is installed, the pooled exchange (lmpc_pool_export_dev, lmpc_pool_import_dev,
+ *     lmpc_ss_import_laps_dev) returns LMPC_E_STATE: a lap driven on another circuit is not a trajectory of this one. */
+int lmpc_set_tracks(lmpc_handle* h, const lmpc_track_params* sets, int nsets, const int* set_of_instance);
+
 /* PredictiveModel.addTrajectory (PredictiveModel.py:35-46): copy one lap into a regression slot. */
 int lmpc_model_put_lap(lmpc_handle* h, int inst, int slot, int T, const double* x, const double* u);
 /* usedIt order: slots[B,trToUse]. */
@@ -367,6 +389,7 @@ int lmpc_probe_fp64(int device, double* out8);
 int lmpc_sizeof_params(void);
 int lmpc_sizeof_model_params(void);
 int lmpc_sizeof_vehicle_params(void);
+int lmpc_sizeof_track_params(void);
 
 #ifdef __cplusplus
 }

@@ -34,6 +34,11 @@ class VehicleParams(C.Structure):
     _fields_ = [(f, C.c_double) for f in ("m", "lf", "lr", "Iz", "Df", "Cf", "Bf", "Dr", "Cr", "Br")]
 
 
+class TrackParams(C.Structure):
+    """lmpc_track_params: the [s_start, length, curvature] rows of Map.PointAndTangent and the lap length."""
+    _fields_ = [("nseg", C.c_int), ("seg", C.c_double * (MAX_SEG * 3)), ("TrackLength", C.c_double)]
+
+
 class NativeError(RuntimeError):
     pass
 
@@ -101,6 +106,7 @@ def lib():
     L.lmpc_rollout_get_health.argtypes = [_vp, _vp, _vp]
     L.lmpc_rollout_pid_step.argtypes = [_vp, C.c_double, _vp, _vp, C.c_ulonglong]
     L.lmpc_rollout_set_vehicles.argtypes = [_vp, C.POINTER(VehicleParams), C.c_int, _vp]
+    L.lmpc_set_tracks.argtypes = [_vp, C.POINTER(TrackParams), C.c_int, _vp]
     L.lmpc_rollout_sysid.argtypes = [_vp, C.c_double, _vp, _vp]
     L.lmpc_rollout_seed_from_record.argtypes = [_vp, C.c_int, C.c_int, C.c_int]
     L.lmpc_rollout_get_lap.argtypes = [_vp, C.c_int, ip, _vp, _vp]
@@ -127,9 +133,11 @@ def lib():
     L.lmpc_sizeof_params.restype = C.c_int
     L.lmpc_sizeof_model_params.restype = C.c_int
     L.lmpc_sizeof_vehicle_params.restype = C.c_int
+    L.lmpc_sizeof_track_params.restype = C.c_int
     assert L.lmpc_sizeof_params() == C.sizeof(Params), "lmpc_params ABI mismatch"
     assert L.lmpc_sizeof_model_params() == C.sizeof(ModelParams), "lmpc_model_params ABI mismatch"
     assert L.lmpc_sizeof_vehicle_params() == C.sizeof(VehicleParams), "lmpc_vehicle_params ABI mismatch"
+    assert L.lmpc_sizeof_track_params() == C.sizeof(TrackParams), "lmpc_track_params ABI mismatch"
     _LIB = L
     return L
 
@@ -259,7 +267,7 @@ def make_params(p, numSS_Points=0, numSS_it=0, QterminalSlack=None, eps_res=0.0,
 
 
 def _set_index(index, K, batch, what):
-    """The index rules of the per-controller tables (lmpc_set_param_sets, lmpc_rollout_set_vehicles): 1 <= K <= batch rows and
+    """The index rules of the per-controller tables (lmpc_set_param_sets, lmpc_rollout_set_vehicles, lmpc_set_tracks): 1 <= K <= batch rows and
     one integer row number in [0, K) per controller.  Returns the index as a contiguous int32 array; raises ValueError."""
     if index is None:
         raise ValueError("index is required: one set number per controller (%d)" % batch)
@@ -319,4 +327,39 @@ def make_vehicle_sets(vehicles, index, batch):
         if min(v.m, v.Iz, v.lf, v.lr) <= 0:
             raise ValueError("vehicle %d: m, Iz, lf and lr must be positive" % k)
         out[k] = VehicleParams(*vals)
+    return out, idx
+
+
+def make_track_sets(tracks, index, batch):
+    """Per-controller tracks for ``lmpc_set_tracks``: K objects ``tracks`` with ``seg_table`` ([nseg, 3] rows s_start, length,
+    curvature) and ``TrackLength`` (e.g. reference_params.TrackParams) and the track of every controller ``index[batch]``.
+    Raises ValueError where the library would refuse: the index rules of ``make_param_sets``, 1 .. 16 rows, a value that is not
+    finite, a negative length, a first start other than 0, a start other than the previous start + length, or a TrackLength that
+    is not positive or not the last start + length (all exact: Track.py:54-133 builds the table that way).
+    Returns (ctypes array TrackParams * K, int32 index array)."""
+    tracks = list(tracks)
+    K = len(tracks)
+    idx = _set_index(index, K, batch, "tracks")
+    out = (TrackParams * K)()
+    for k, t in enumerate(tracks):
+        seg = np.asarray(t.seg_table, dtype=float)
+        L = float(t.TrackLength)
+        if seg.ndim != 2 or seg.shape[1] != 3 or not 1 <= seg.shape[0] <= MAX_SEG:
+            raise ValueError("track %d: seg_table must have 1 .. %d rows of [s_start, length, curvature]" % (k, MAX_SEG))
+        if not (np.all(np.isfinite(seg)) and np.isfinite(L)):
+            raise ValueError("track %d: every value must be finite" % k)
+        if np.any(seg[:, 1] < 0):
+            raise ValueError("track %d: a segment has a negative length" % k)
+        if seg[0, 0] != 0.0:
+            raise ValueError("track %d: the first segment must start at s = 0" % k)
+        for i in range(1, seg.shape[0]):
+            if seg[i, 0] != seg[i - 1, 0] + seg[i - 1, 1]:
+                raise ValueError("track %d: segment %d does not start where segment %d ends" % (k, i, i - 1))
+        if not L > 0 or L != seg[-1, 0] + seg[-1, 1]:
+            raise ValueError("track %d: TrackLength must be positive and equal the end of the last segment" % k)
+        buf = np.zeros(MAX_SEG * 3)
+        buf[:seg.size] = seg.ravel()
+        out[k].nseg = seg.shape[0]
+        out[k].seg[:] = buf
+        out[k].TrackLength = L
     return out, idx

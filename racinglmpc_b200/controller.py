@@ -114,6 +114,21 @@ class BatchedController:
         sets, idx = nat.make_vehicle_sets(vehicles, index, self.B)
         nat.check(self._lib.lmpc_rollout_set_vehicles(self._h, sets, len(sets), nat.ptr(idx)))
 
+    def set_tracks(self, tracks, index=None):
+        """Per-controller tracks (several circuits in one batch): controller b drives ``tracks[index[b]]`` (objects with
+        ``seg_table`` and ``TrackLength``, e.g. reference_params.TrackParams) in every later regression, safe-set selection,
+        addPoint, lap cost, lap hand-over and simulator step.  ``index`` is required with ``tracks``.  ``tracks=None`` (no index)
+        returns to the track the controller was created with.  Independent of ``set_param_sets`` and ``set_vehicles``.
+        Only before the first lap is stored; while more than one track is installed the pooled exchange is refused.
+        Waits for work already enqueued."""
+        if tracks is None:
+            if index is not None:
+                raise ValueError("tracks=None reverts to the handle's own track and takes no index")
+            nat.check(self._lib.lmpc_set_tracks(self._h, None, 0, None))
+            return
+        sets, idx = nat.make_track_sets(tracks, index, self.B)
+        nat.check(self._lib.lmpc_set_tracks(self._h, sets, len(sets), nat.ptr(idx)))
+
     # ------------------------------------------------------------------ PredictiveModel.addTrajectory
     def model_add_trajectory(self, inst, x, u):
         """PredictiveModel.py:35-46: keep laps sorted by length; only the trToUse fastest are ever read."""

@@ -144,11 +144,12 @@ __device__ inline void copy_lap_block(const LapPool& pool, size_t lap, const dou
 // PC.py:445 (timeStep = 0).  One CTA per controller; no host involvement.
 __global__ void __launch_bounds__(256) commit_laps_books_kernel(int batch, LapPool ss, LapPool model, LapBooks k, const double* cl_x,
                                                                 const double* cl_u, int* cl_len, int Tcl, double* x_cur, int* timeStep,
-                                                                int* done, int* flags_or, double TrackLength, int lmpc) {
+                                                                int* done, int* flags_or, Tracks trk, int lmpc) {
     const int b = blockIdx.x;
     if (b >= batch || !done[b]) return;
     __shared__ int s_ss, s_md;
     const int Trec = cl_len[b];
+    const double TrackLength = trk.of(b).TrackLength;
     if (threadIdx.x == 0) {
         s_ss = lmpc ? book_ss_add(k, b, min(Trec, ss.Tmax), false) : -1;
         s_md = book_md_add(k, b, min(Trec, model.Tmax));
@@ -182,11 +183,12 @@ __global__ void __launch_bounds__(256) commit_laps_books_kernel(int batch, LapPo
 __global__ void __launch_bounds__(256) seed_books_kernel(int batch, LapPool ss, LapPool model, LapBooks k, int copies, const double* cl_x,
                                                          const double* cl_u, int* cl_len, int Tcl, int N, double* xLin, double* uLin,
                                                          double* zt, double* OldInput, int* timeStep, int* hasPred, int* done,
-                                                         double TrackLength, int lmpc) {
+                                                         Tracks trk, int lmpc) {
     const int b = blockIdx.x;
     if (b >= batch) return;
     __shared__ int s_ss, s_md;
     const int Trec = cl_len[b];
+    const double TrackLength = trk.of(b).TrackLength;
     const double* cx = cl_x + (size_t)b * Tcl * 6;
     const double* cu = cl_u + (size_t)b * Tcl * 2;
     if (threadIdx.x == 0) {                                      // fresh books

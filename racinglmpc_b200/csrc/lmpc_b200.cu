@@ -91,6 +91,14 @@ struct lmpc_handle {
     // lap stores + controller state (lmpc_store_create)
     bool has_store;
     ModelConst mc;
+    // tracks (lmpc_set_tracks): table TrackRec[ntrk] and track index [batch]; without sets a one-row table holding the track of
+    // lmpc_store_create (store_trk) and a null index.  trk_host / trk_idx_host mirror both for the host-side lap restart.
+    TrackRec store_trk;
+    TrackRec* d_trk;
+    int* d_trk_idx;
+    std::vector<TrackRec> trk_host;
+    std::vector<int> trk_idx_host;
+    bool laps_stored;          // a lap entered either pool: the track table is fixed from now on
     LapPool ss, mdl;
     int *d_used, *d_sel, *d_isprev, *d_prevslot, *d_timeStep, *d_hasPred, *d_flags, *d_minidx, *d_xchg, *d_health, *d_dropped;
     double *d_xLin, *d_uLin, *d_ztState, *d_ztFixed, *d_OldInput, *d_xPredPrev, *d_tmpx, *d_tmpu;
@@ -272,9 +280,14 @@ static void free_store(lmpc_handle* h) {
     free_null(h->d_tmpu); free_null(h->d_xchg); free_null(h->d_dropped);
     free_null(h->d_bkbuf); free_null(h->d_poolidx); free_null(h->d_stats);
     free_null(h->d_warm); free_null(h->d_warm_valid);
+    free_null(h->d_trk); free_null(h->d_trk_idx);
+    h->trk_host.clear(); h->trk_idx_host.clear();
+    h->laps_stored = false;
     h->has_books = false;
     h->has_store = false;
 }
+
+static Tracks tracks(const lmpc_handle* h) { return Tracks{h->d_trk, h->d_trk_idx}; }
 
 static void free_rollout(lmpc_handle* h) {
     for (int i = 0; i < 2; ++i) { free_null(h->d_rx[i]); free_null(h->d_rg[i]); }
@@ -755,6 +768,7 @@ int lmpc_solve_mpc_host(lmpc_handle* h, const double* x0, const double* uOld, co
 int lmpc_sizeof_params(void) { return (int)sizeof(lmpc_params); }
 int lmpc_sizeof_model_params(void) { return (int)sizeof(lmpc_model_params); }
 int lmpc_sizeof_vehicle_params(void) { return (int)sizeof(lmpc_vehicle_params); }
+int lmpc_sizeof_track_params(void) { return (int)sizeof(lmpc_track_params); }
 
 static int store_create_impl(lmpc_handle* h, const lmpc_model_params* mp, int ss_cap, int model_cap, int Tmax);
 int lmpc_store_create(lmpc_handle* h, const lmpc_model_params* mp, int ss_cap, int model_cap, int Tmax) {
@@ -782,9 +796,16 @@ static int store_create_impl(lmpc_handle* h, const lmpc_model_params* mp, int ss
     memset(&m, 0, sizeof(m));
     m.trToUse = mp->trToUse; m.MaxNumPoint = mp->MaxNumPoint; m.h = mp->h; m.lamb = mp->lamb; m.dt = mp->dt;
     for (int i = 0; i < 5; ++i) m.scaling[i] = mp->scaling[i];
-    m.nseg = mp->nseg;
-    for (int i = 0; i < mp->nseg * 3; ++i) m.seg[i] = mp->seg[i];
-    m.TrackLength = mp->TrackLength;
+    TrackRec& t = h->store_trk;
+    memset(&t, 0, sizeof(t));
+    t.nseg = mp->nseg;
+    for (int i = 0; i < mp->nseg * 3; ++i) t.seg[i] = mp->seg[i];
+    t.TrackLength = mp->TrackLength;
+    int rc = swap_table(h, "lmpc_store_create", &t, 1, nullptr, &h->d_trk, &h->d_trk_idx);
+    if (rc != LMPC_OK) return rc;
+    h->trk_host.assign(1, t);
+    h->trk_idx_host.clear();
+    h->laps_stored = false;
     const size_t B = h->batch, N = h->N;
     h->ss.cap = ss_cap > 0 ? ss_cap : 1; h->ss.Tmax = Tmax;
     h->mdl.cap = model_cap; h->mdl.Tmax = Tmax;
@@ -852,10 +873,54 @@ static int need_store(lmpc_handle* h) {
     return LMPC_OK;
 }
 
+// The pooled exchange hands laps between controllers: only when they all drive one circuit
+static int one_track(const lmpc_handle* h, const char* who) {
+    if (h->trk_host.size() > 1)
+        return fail(LMPC_E_STATE, std::string(who) + ": more than one track installed; a lap of another circuit is not a trajectory of this one");
+    return LMPC_OK;
+}
+
+// Per-controller tracks: every set is checked the way Track.py:54-133 builds the table (start i = start i-1 + length i-1 and
+// TrackLength = start + length of the last row, exactly), then the table replaces the previous one once the handle's streams are
+// idle.  Nothing about the handle changes unless every check passes.
+int lmpc_set_tracks(lmpc_handle* h, const lmpc_track_params* sets, int nsets, const int* set_of_instance) {
+    static const char* who = "lmpc_set_tracks";
+    int rc = need_store(h);
+    if (rc) return rc;
+    if (h->laps_stored) return fail(LMPC_E_STATE, std::string(who) + ": laps are stored already; install tracks before the first lap");
+    if ((rc = check_set_index(h, who, sets, nsets, set_of_instance)) != LMPC_OK) return rc;
+    for (int k = 0; k < nsets; ++k) {
+        const lmpc_track_params& t = sets[k];
+        const std::string w = std::string(who) + ": track " + std::to_string(k) + ": ";
+        if (t.nseg < 1 || t.nseg > LMPC_MAX_SEG) return fail(LMPC_E_INVALID, w + "nseg must be 1 .. 16");
+        bool finite = isfinite(t.TrackLength);
+        for (int i = 0; i < t.nseg * 3; ++i) finite = finite && isfinite(t.seg[i]);
+        if (!finite) return fail(LMPC_E_INVALID, w + "every value must be finite");
+        if (t.seg[0] != 0.0) return fail(LMPC_E_INVALID, w + "the first segment must start at s = 0");
+        for (int i = 0; i < t.nseg; ++i) {
+            if (t.seg[i * 3 + 1] < 0.0) return fail(LMPC_E_INVALID, w + "segment " + std::to_string(i) + " has a negative length");
+            if (i > 0 && t.seg[i * 3] != t.seg[(i - 1) * 3] + t.seg[(i - 1) * 3 + 1])
+                return fail(LMPC_E_INVALID, w + "segment " + std::to_string(i) + " does not start where the previous one ends");
+        }
+        const int l = (t.nseg - 1) * 3;
+        if (!(t.TrackLength > 0.0) || t.TrackLength != t.seg[l] + t.seg[l + 1])
+            return fail(LMPC_E_INVALID, w + "TrackLength must be positive and equal the end of the last segment");
+    }
+    std::vector<TrackRec> rows;
+    if (nsets == 0) rows.push_back(h->store_trk);
+    else rows.assign(sets, sets + nsets);
+    if ((rc = swap_table(h, who, rows.data(), (int)rows.size(), set_of_instance, &h->d_trk, &h->d_trk_idx)) != LMPC_OK) return rc;
+    h->trk_host = rows;
+    if (set_of_instance) h->trk_idx_host.assign(set_of_instance, set_of_instance + h->batch);
+    else h->trk_idx_host.clear();
+    return LMPC_OK;
+}
+
 static int put_lap(lmpc_handle* h, LapPool& pool, int inst, int slot, int T, const double* x, const double* u) {
     if (inst < 0 || inst >= h->batch || slot < 0 || slot >= pool.cap || T < 2 || T > pool.Tmax || !x || !u)
         return fail(LMPC_E_INVALID, "put_lap: bad instance/slot/length");
     CK(cudaSetDevice(h->device));
+    h->laps_stored = true;
     const size_t lap = pool.lap_index(inst, slot);
     CK(cudaMemcpyAsync(pool.x + lap * pool.Tmax * 6, x, sizeof(double) * T * 6, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(pool.u + lap * pool.Tmax * 2, u, sizeof(double) * T * 2, cudaMemcpyHostToDevice, h->stream));
@@ -891,7 +956,7 @@ int lmpc_ss_put_lap(lmpc_handle* h, int inst, int slot, int T, const double* x, 
     if (qfun) {
         CK(cudaMemcpyAsync(h->ss.q + lap * h->ss.Tmax, qfun, sizeof(double) * T, cudaMemcpyHostToDevice, h->stream));
     } else {
-        rollout_cost_kernel<<<1, 256, 0, h->stream>>>(h->ss, inst, slot, h->mc.TrackLength);
+        rollout_cost_kernel<<<1, 256, 0, h->stream>>>(h->ss, inst, slot, tracks(h));
         CK(cudaGetLastError());
         h->launches += 1;
     }
@@ -924,7 +989,7 @@ int lmpc_ss_add_point(lmpc_handle* h, const double* x, const double* u) {
     CK(cudaMemcpyAsync(h->d_tmpx, x, sizeof(double) * h->batch * 6, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(h->d_tmpu, u, sizeof(double) * h->batch * 2, cudaMemcpyHostToDevice, h->stream));
     ss_add_point_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->batch, h->ss, h->d_prevslot, h->d_tmpx, h->d_tmpu, 2,
-                                                                        h->mc.TrackLength, h->d_flags, h->d_dropped, 0);
+                                                                        tracks(h), h->d_flags, h->d_dropped, 0);
     CK(cudaGetLastError());
     h->launches += 1;
     int dropped = 0;
@@ -1008,6 +1073,7 @@ static int launch_k1(lmpc_handle* h, int b0 = 0, int nb = -1, cudaStream_t st = 
     a.wpb = h->N < 12 ? h->N : 12;
     a.pts_stride = k1_pts_stride(h->mc.trToUse);
     a.xLin = h->d_xLin; a.uLin = h->d_uLin; a.pool = h->mdl; a.used = h->d_used; a.abc = h->hb[0].abc; a.status = h->d_flags;
+    a.trk = tracks(h);
     dim3 grid(nb, (h->N + a.wpb - 1) / a.wpb);
     size_t smem = sizeof(float) * 5 * K1_TILE + sizeof(double) * (size_t)a.pts_stride * a.wpb;
     knn_ltv_regress_kernel<<<grid, 32 * a.wpb, smem, st>>>(h->mc, a);
@@ -1021,7 +1087,7 @@ static int launch_k2(lmpc_handle* h, const double* d_x0, int b0 = 0, int nb = -1
     if (!st) st = h->stream;
     K2Args a;
     a.batch = h->batch; a.N = h->N; a.b0 = b0; a.numSS_it = h->p.numSS_it; a.P = h->M / h->p.numSS_it;
-    a.TrackLength = h->mc.TrackLength;
+    a.trk = tracks(h);
     a.x0 = d_x0; a.zt = h->d_ztState; a.pool = h->ss; a.sel = h->d_sel; a.is_prev = h->d_isprev;
     a.timeStep = h->d_timeStep; a.has_pred = h->d_hasPred; a.xPred = h->d_xPredPrev;
     a.SS_sel = h->hb[0].SS; a.Qfun_sel = h->hb[0].Qfun; a.Succ_SS = h->hb[0].SuccSS; a.Succ_uSS = h->hb[0].SuccU;
@@ -1115,7 +1181,7 @@ static int step_range(lmpc_handle* h, int mode, const double* x0_dev, cudaEvent_
     if (tail) {
         if (lm) {                                                                    // SysModel.py:38 -> PC.py:466-476
             ss_add_point_kernel<<<(nb + 127) / 128, 128, 0, st>>>(b0 + nb, h->ss, h->d_prevslot, tail->xc, q.uPred, (long long)h->N * 2,
-                                                                  h->mc.TrackLength, h->d_flags, nullptr, b0);
+                                                                  tracks(h), h->d_flags, nullptr, b0);
             CK(cudaGetLastError());
             h->launches += 1;
         }
@@ -1323,7 +1389,7 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
     sa.xn = h->d_rx[h->cur ^ 1]; sa.xgn = h->d_rg[h->cur ^ 1];
     sa.cl_x = h->d_clx; sa.cl_u = h->d_clu; sa.cl_len = h->d_cllen; sa.Tcl = h->Tcl; sa.done = h->d_done; sa.active = nullptr;
     sa.flags = h->d_flags; sa.status = q.status; sa.health = h->d_health;
-    sa.veh = h->d_veh; sa.veh_idx = h->d_veh_idx;
+    sa.veh = h->d_veh; sa.veh_idx = h->d_veh_idx; sa.trk = tracks(h);
     // the trace of the chosen controllers reads the step's results and the state before dynModel: it has to sit between the
     // solve and the simulator, so a traced batch runs the simulator for the whole batch after it
     const bool fused_tail = !h->has_trace && mode != 2;
@@ -1339,7 +1405,7 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
     if (!fused_tail) {
         if (mode == 1) {
             ss_add_point_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->batch, h->ss, h->d_prevslot, xc, q.uPred,
-                                                                                (long long)h->N * 2, h->mc.TrackLength, h->d_flags, nullptr, 0);
+                                                                                (long long)h->N * 2, tracks(h), h->d_flags, nullptr, 0);
             CK(cudaGetLastError());
             h->launches += 1;
         }
@@ -1378,7 +1444,7 @@ int lmpc_rollout_pid_step(lmpc_handle* h, double vt, const double* z_pid_host, c
     sa.xn = h->d_rx[h->cur ^ 1]; sa.xgn = h->d_rg[h->cur ^ 1];
     sa.cl_x = h->d_clx; sa.cl_u = h->d_clu; sa.cl_len = h->d_cllen; sa.Tcl = h->Tcl; sa.done = h->d_done; sa.active = nullptr;
     sa.flags = nullptr; sa.status = nullptr; sa.health = nullptr;
-    sa.veh = h->d_veh; sa.veh_idx = h->d_veh_idx;
+    sa.veh = h->d_veh; sa.veh_idx = h->d_veh_idx; sa.trk = tracks(h);
     sim_step_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->mc, sa);
     CK(cudaGetLastError());
     h->launches += 2;
@@ -1435,10 +1501,11 @@ int lmpc_rollout_seed_from_record(lmpc_handle* h, int copies, int ss_slot0, int 
     if (copies < 1 || ss_slot0 < 0 || model_slot0 < 0 || ss_slot0 + copies > h->ss.cap || model_slot0 + copies > h->mdl.cap)
         return fail(LMPC_E_INVALID, "seed copies do not fit the lap pools");
     CK(cudaSetDevice(h->device));
+    h->laps_stored = true;
     if (h->d_warm_valid) CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * h->batch, h->stream));
     seed_from_record_kernel<<<h->batch, 256, 0, h->stream>>>(h->batch, h->ss, h->mdl, copies, ss_slot0, model_slot0, h->d_clx, h->d_clu,
                                                              h->d_cllen, h->Tcl, h->N, h->d_xLin, h->d_uLin, h->d_ztState, h->d_OldInput,
-                                                             h->d_timeStep, h->d_hasPred, h->d_done, h->mc.TrackLength);
+                                                             h->d_timeStep, h->d_hasPred, h->d_done, tracks(h));
     CK(cudaGetLastError());
     h->launches += 1;
     return LMPC_OK;
@@ -1465,9 +1532,10 @@ int lmpc_rollout_commit_lap(lmpc_handle* h, int inst, int ss_slot, int model_slo
     if (rc) return rc;
     if (inst < 0 || inst >= h->batch || ss_slot >= h->ss.cap || model_slot >= h->mdl.cap) return fail(LMPC_E_INVALID, "bad instance/slot");
     CK(cudaSetDevice(h->device));
+    if (ss_slot >= 0 || model_slot >= 0) h->laps_stored = true;
     if (ss_slot >= 0) {
         commit_lap_kernel<<<1, 256, 0, h->stream>>>(h->ss, inst, ss_slot, h->d_clx, h->d_clu, h->d_cllen, h->Tcl);
-        rollout_cost_kernel<<<1, 256, 0, h->stream>>>(h->ss, inst, ss_slot, h->mc.TrackLength);
+        rollout_cost_kernel<<<1, 256, 0, h->stream>>>(h->ss, inst, ss_slot, tracks(h));
         h->launches += 2;
     }
     if (model_slot >= 0) {
@@ -1479,7 +1547,7 @@ int lmpc_rollout_commit_lap(lmpc_handle* h, int inst, int ss_slot, int model_slo
     double s;
     CK(cudaMemcpyAsync(&s, h->d_rx[h->cur] + (size_t)inst * 6 + 4, sizeof(double), cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
-    s -= h->mc.TrackLength;
+    s -= h->trk_host[h->trk_idx_host.empty() ? 0 : h->trk_idx_host[inst]].TrackLength;
     const int zero = 0;
     CK(cudaMemcpyAsync(h->d_rx[h->cur] + (size_t)inst * 6 + 4, &s, sizeof(double), cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(h->d_cllen + inst, &zero, sizeof(int), cudaMemcpyHostToDevice, h->stream));
@@ -1499,12 +1567,14 @@ int lmpc_rollout_commit_laps(lmpc_handle* h, const int* fin, const int* ss_slots
         if (fin[b] && (ss_slots[b] >= h->ss.cap || model_slots[b] >= h->mdl.cap)) return fail(LMPC_E_INVALID, "slot out of range");
     const size_t B = h->batch;
     CK(cudaSetDevice(h->device));
+    for (int b = 0; b < h->batch; ++b)
+        if (fin[b] && (ss_slots[b] >= 0 || model_slots[b] >= 0)) h->laps_stored = true;
     CK(cudaMemcpyAsync(h->d_xchg, fin, sizeof(int) * B, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(h->d_xchg + B, ss_slots, sizeof(int) * B, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(h->d_xchg + 2 * B, model_slots, sizeof(int) * B, cudaMemcpyHostToDevice, h->stream));
     commit_laps_kernel<<<h->batch, 256, 0, h->stream>>>(h->batch, h->ss, h->mdl, h->d_xchg, h->d_xchg + B, h->d_xchg + 2 * B, h->d_clx,
                                                         h->d_clu, h->d_cllen, h->Tcl, h->d_rx[h->cur], h->d_timeStep, h->d_done,
-                                                        h->mc.TrackLength);
+                                                        tracks(h));
     CK(cudaGetLastError());
     h->launches += 1;
     CK(cudaStreamSynchronize(h->stream));   // the three host arrays are pageable memory of the caller
@@ -1542,12 +1612,15 @@ int lmpc_ss_import_laps_dev(lmpc_handle* h, const int* ss_slots, const int* mode
     int rc = need_store(h);
     if (rc) return rc;
     if (!ss_slots || !src || !rows_dev || !lens_dev || Tpad < 1 || n_src < 1) return fail(LMPC_E_INVALID, "bad import arguments");
+    if ((rc = one_track(h, "lmpc_ss_import_laps_dev")) != LMPC_OK) return rc;
     for (int b = 0; b < h->batch; ++b) {
         if (ss_slots[b] >= h->ss.cap || (model_slots && model_slots[b] >= h->mdl.cap)) return fail(LMPC_E_INVALID, "slot out of range");
         if (src[b] >= n_src) return fail(LMPC_E_INVALID, "source lap index out of range");
     }
     const size_t B = h->batch;
     CK(cudaSetDevice(h->device));
+    for (int b = 0; b < h->batch; ++b)
+        if (src[b] >= 0 && (ss_slots[b] >= 0 || (model_slots && model_slots[b] >= 0))) h->laps_stored = true;
     CK(cudaMemcpyAsync(h->d_xchg, ss_slots, sizeof(int) * B, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(h->d_xchg + B, src, sizeof(int) * B, cudaMemcpyHostToDevice, h->stream));
     if (model_slots) CK(cudaMemcpyAsync(h->d_xchg + 2 * B, model_slots, sizeof(int) * B, cudaMemcpyHostToDevice, h->stream));
@@ -1660,8 +1733,9 @@ int lmpc_rollout_commit_laps_dev(lmpc_handle* h) {
     if (rc) return rc;
     if ((rc = need_books(h)) != LMPC_OK) return rc;
     CK(cudaSetDevice(h->device));
+    h->laps_stored = true;     // enqueue only: which controllers finish a lap is not known here
     commit_laps_books_kernel<<<h->batch, 256, 0, h->stream>>>(h->batch, h->ss, h->mdl, h->bk, h->d_clx, h->d_clu, h->d_cllen, h->Tcl,
-                                                              h->d_rx[h->cur], h->d_timeStep, h->d_done, h->d_health, h->mc.TrackLength,
+                                                              h->d_rx[h->cur], h->d_timeStep, h->d_done, h->d_health, tracks(h),
                                                               h->M > 0 ? 1 : 0);
     CK(cudaGetLastError());
     h->launches += 1;
@@ -1674,10 +1748,11 @@ int lmpc_rollout_seed_from_record_dev(lmpc_handle* h, int copies) {
     if ((rc = need_books(h)) != LMPC_OK) return rc;
     if (copies < 1 || (h->M > 0 && copies > h->ss.cap) || copies > h->mdl.cap) return fail(LMPC_E_INVALID, "seed copies do not fit the lap pools");
     CK(cudaSetDevice(h->device));
+    h->laps_stored = true;
     if (h->d_warm_valid) CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * h->batch, h->stream));
     seed_books_kernel<<<h->batch, 256, 0, h->stream>>>(h->batch, h->ss, h->mdl, h->bk, copies, h->d_clx, h->d_clu, h->d_cllen, h->Tcl, h->N,
                                                        h->d_xLin, h->d_uLin, h->d_ztState, h->d_OldInput, h->d_timeStep, h->d_hasPred,
-                                                       h->d_done, h->mc.TrackLength, h->M > 0 ? 1 : 0);
+                                                       h->d_done, tracks(h), h->M > 0 ? 1 : 0);
     CK(cudaGetLastError());
     h->launches += 1;
     return LMPC_OK;
@@ -1703,6 +1778,7 @@ int lmpc_pool_export_dev(lmpc_handle* h, int kbest, int Tpad, long long gid_base
     if (rc) return rc;
     if (kbest < 1 || kbest > POOL_MAXK || Tpad < 1 || !rows_dev || !meta_dev) return fail(LMPC_E_INVALID, "bad export arguments");
     if (h->M <= 0) return fail(LMPC_E_STATE, "handle has no safe set");
+    if ((rc = one_track(h, "lmpc_pool_export_dev")) != LMPC_OK) return rc;
     CK(cudaSetDevice(h->device));
     pool_local_best_kernel<<<1, 1024, 0, h->stream>>>(h->batch, h->bk, kbest, h->d_poolidx);
     pool_export_kernel<<<kbest, 256, 0, h->stream>>>(h->ss, h->bk, h->d_poolidx, Tpad, gid_base, rows_dev, meta_dev);
@@ -1719,7 +1795,9 @@ int lmpc_pool_import_dev(lmpc_handle* h, int n_src, int share, int Tpad, long lo
     if (rc) return rc;
     if (n_src < 1 || n_src > 64 || share < 1 || Tpad < 1 || !rows_dev || !meta_dev) return fail(LMPC_E_INVALID, "bad import arguments");
     if (h->M <= 0) return fail(LMPC_E_STATE, "handle has no safe set");
+    if ((rc = one_track(h, "lmpc_pool_import_dev")) != LMPC_OK) return rc;
     CK(cudaSetDevice(h->device));
+    h->laps_stored = true;
     int* order = h->d_poolidx + 64;
     int* took = h->d_poolidx + 200;
     CK(cudaMemsetAsync(took, 0, sizeof(int), h->stream));

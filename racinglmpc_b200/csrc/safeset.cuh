@@ -20,9 +20,16 @@ struct ModelConst {
     int trToUse, MaxNumPoint;
     double h, lamb, dt;
     double scaling[5];
-    int nseg;
-    double seg[16 * 3];   // s_start, length, curvature
-    double TrackLength;
+};
+
+// A track is one row of the handle's track table (lmpc_set_tracks); the ABI record is the device record.
+using TrackRec = lmpc_track_params;
+// The track of every controller: row idx[b] of tab, or row 0 when idx is null (a handle without track sets holds a one-row table
+// with the track of lmpc_store_create).
+struct Tracks {
+    const TrackRec* tab;
+    const int* idx;
+    __device__ __forceinline__ const TrackRec& of(int b) const { return tab[idx ? idx[b] : 0]; }
 };
 
 struct LapPool {
@@ -37,7 +44,7 @@ struct LapPool {
 // Track.py:292-310 — wrap by repeated subtraction, first segment with s in [s0, s0+len)
 // (a non-finite or absurdly large s -- an unsolved QP feeding garbage to the simulator -- would spin forever in the
 // reference's loop; here it fails the lookup like a negative s does, so the instance is flagged instead of hanging the stream)
-__device__ __forceinline__ double curvature_lookup(const ModelConst& m, double s, int* ok) {
+__device__ __forceinline__ double curvature_lookup(const TrackRec& m, double s, int* ok) {
     if (!(s <= 64.0 * m.TrackLength)) { *ok = 0; return 0.0; }
     while (s > m.TrackLength) s = s - m.TrackLength;
     for (int i = 0; i < m.nseg; ++i) {
@@ -126,6 +133,7 @@ struct K1Args {
     const double* uLin;   // [B][N][2]
     LapPool pool;         // model pool
     const int* used;      // [B][trToUse] slot ids, in usedIt order
+    Tracks trk;           // the curvature of the linearisation point
     double* abc;          // [B][N][54]
     int* status;          // [B] : 0 ok, else bit flags (1 = singular regression, 2 = curvature lookup failed,
                           //        4 = a single neighbour in a lap — cases where the reference raises,
@@ -422,7 +430,7 @@ __global__ void __launch_bounds__(32 * 12, LMPC_K1_MINBLOCKS) knn_ltv_regress_ke
         const double vx = xl[0], vy = xl[1], wz = xl[2], epsi = xl[3], sc = xl[4], ey = xl[5];
         const double dt = m.dt;
         int okc = 1;
-        const double cur = curvature_lookup(m, sc, &okc);
+        const double cur = curvature_lookup(a.trk.of(b), sc, &okc);
         if (!okc) flags |= 2;
         const double den = 1.0 - cur * ey;
         const double rden = fast_rcp(den), rden2 = rden * rden;
@@ -462,7 +470,7 @@ __global__ void __launch_bounds__(32 * 12, LMPC_K1_MINBLOCKS) knn_ltv_regress_ke
 struct K2Args {
     int batch, N, numSS_it, P;   // P = numSS_Points / numSS_it
     int b0 = 0;              // first instance of this launch's range (see K1Args::b0); batch bounds the global index
-    double TrackLength;
+    Tracks trk;
     const double* x0;        // [B][6]
     const double* zt;        // [B][6]
     LapPool pool;            // safe-set pool
@@ -487,11 +495,12 @@ __global__ void __launch_bounds__(32 * 8) ss_select_kernel(const K2Args a) {
     const int lane = threadIdx.x & 31;
     if (b >= a.batch || c >= a.numSS_it) return;
     const int M = a.P * a.numSS_it;
+    const double TrackLength = a.trk.of(b).TrackLength;
     // lap-wrap fix of the terminal guess (PC.py:392-393)
     double z[6];
 #pragma unroll
     for (int j = 0; j < 6; ++j) z[j] = a.zt[(size_t)b * 6 + j];
-    if (z[4] - a.x0[(size_t)b * 6 + 4] > a.TrackLength / 2) z[4] = fmax(z[4] - a.TrackLength, 0.0);
+    if (z[4] - a.x0[(size_t)b * 6 + 4] > TrackLength / 2) z[4] = fmax(z[4] - TrackLength, 0.0);
     if (c == 0 && lane < 6) a.zt_fixed[(size_t)b * 6 + lane] = z[lane];
 
     const int slot = a.sel[(size_t)b * a.numSS_it + c];
@@ -535,7 +544,7 @@ __global__ void __launch_bounds__(32 * 8) ss_select_kernel(const K2Args a) {
     double adj = 0.0;
     if (a.has_pred[b]) {
         int over = 0;
-        for (int k = 0; k <= a.N; ++k) over += (a.xPred[((size_t)b * (a.N + 1) + k) * 6 + 4] > a.TrackLength) ? 1 : 0;
+        for (int k = 0; k <= a.N; ++k) over += (a.xPred[((size_t)b * (a.N + 1) + k) * 6 + 4] > TrackLength) ? 1 : 0;
         if (over > 0) {
             if (!a.is_prev[(size_t)b * a.numSS_it + c]) adj = Q[0];
             else adj = (double)a.timeStep[b] + (double)(a.N - over);
@@ -563,7 +572,7 @@ __global__ void __launch_bounds__(32 * 8) ss_select_kernel(const K2Args a) {
 // ------------------------------------------------------------------------------------------------
 // LMPC.addPoint (PC.py:466-476): append x + [0,0,0,0,L,0], u to lap it-1; Qfun extends by last - 1.
 __global__ void ss_add_point_kernel(int batch, LapPool pool, const int* prev_slot, const double* x, const double* u,
-                                    long long u_stride, double TrackLength, int* status, int* dropped, int b0) {
+                                    long long u_stride, Tracks trk, int* status, int* dropped, int b0) {
     const int b = b0 + blockIdx.x * blockDim.x + threadIdx.x;     // instances [b0, batch)
     if (b >= batch) return;
     const int slot = prev_slot[b];
@@ -578,6 +587,7 @@ __global__ void ss_add_point_kernel(int batch, LapPool pool, const int* prev_slo
     double* X = pool.x + (lap * pool.Tmax + T) * 6;
     double* U = pool.u + (lap * pool.Tmax + T) * 2;
     double* Q = pool.q + lap * pool.Tmax;
+    const double TrackLength = trk.of(b).TrackLength;
 #pragma unroll
     for (int j = 0; j < 6; ++j) X[j] = x[(size_t)b * 6 + j] + (j == 4 ? TrackLength : 0.0);
     U[0] = u[(size_t)b * u_stride];
@@ -703,8 +713,8 @@ __device__ void lap_cost_block(const LapPool& pool, size_t lap, double TrackLeng
     }
 }
 
-__global__ void __launch_bounds__(256) rollout_cost_kernel(LapPool pool, int b, int slot, double TrackLength) {
-    lap_cost_block(pool, pool.lap_index(b, slot), TrackLength);
+__global__ void __launch_bounds__(256) rollout_cost_kernel(LapPool pool, int b, int slot, Tracks trk) {
+    lap_cost_block(pool, pool.lap_index(b, slot), trk.of(b).TrackLength);
 }
 
 // Lap hand-over of every instance with fin[b] != 0, one CTA per instance (main.py:113-119 + SysModel.py:50 + PC.py:445):
@@ -712,10 +722,11 @@ __global__ void __launch_bounds__(256) rollout_cost_kernel(LapPool pool, int b, 
 // (>= 0); then the record restarts, s -= TrackLength, timeStep = 0, done = 0.
 __global__ void __launch_bounds__(256) commit_laps_kernel(int batch, LapPool ss, LapPool model, const int* fin, const int* ss_slot,
                                                           const int* model_slot, const double* cl_x, const double* cl_u, int* cl_len,
-                                                          int Tcl, double* x_cur, int* timeStep, int* done, double TrackLength) {
+                                                          int Tcl, double* x_cur, int* timeStep, int* done, Tracks trk) {
     const int b = blockIdx.x;
     if (b >= batch || !fin[b]) return;
     const int Trec = cl_len[b];
+    const double TrackLength = trk.of(b).TrackLength;
     if (ss_slot[b] >= 0) {
         const int T = min(Trec, ss.Tmax);
         const size_t lap = ss.lap_index(b, ss_slot[b]);
@@ -813,6 +824,7 @@ struct SimArgs {
     int* health;
     const lmpc_vehicle_params* veh;   // vehicle table (lmpc_rollout_set_vehicles)
     const int* veh_idx;               // [B] row of every instance, or nullptr: row 0
+    Tracks trk;                       // curvature and finish line of every instance (lmpc_set_tracks)
 };
 
 }  // namespace lmpc
@@ -832,6 +844,7 @@ __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimA
     const double mass = v.m, lf = v.lf, lr = v.lr, Iz = v.Iz;
     const double Df = v.Df, Cf = v.Cf, Bf = v.Bf;
     const double Dr = v.Dr, Cr = v.Cr, Br = v.Br;
+    const TrackRec& trk = a.trk.of(b);
     const double h = 0.001;
     const double* x = a.x + (size_t)b * 6;
     const double* g = a.xg + (size_t)b * 6;
@@ -862,7 +875,7 @@ __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimA
         const double npsi = psi + h * wz;
         const double nX = X + h * (vx * cos(psi) - vy * sin(psi));
         const double nY = Y + h * (vx * sin(psi) + vy * cos(psi));
-        const double cur = curvature_lookup(m, s, &okc);
+        const double cur = curvature_lookup(trk, s, &okc);
         const double ce = cos(epsi), se = sin(epsi);
         const double nepsi = epsi + h * (wz - (vx * ce - vy * se) / (1 - cur * ey) * cur);
         const double ns = s + h * ((vx * ce - vy * se) / (1 - cur * ey));
@@ -890,7 +903,7 @@ __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimA
     gn[0] = vx; gn[1] = vy; gn[2] = wz; gn[3] = psi; gn[4] = X; gn[5] = Y;
     xn[0] = vx + 0.01 * n_vx; xn[1] = vy + 0.01 * n_vy; xn[2] = wz + 0.01 * n_wz;
     xn[3] = epsi; xn[4] = s; xn[5] = ey;
-    if (a.done) a.done[b] = (s > m.TrackLength) ? 1 : 0;
+    if (a.done) a.done[b] = (s > trk.TrackLength) ? 1 : 0;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -995,10 +1008,11 @@ __global__ void __launch_bounds__(32) ridge_sysid_kernel(int batch, const double
 __global__ void __launch_bounds__(256) seed_from_record_kernel(int batch, LapPool ss, LapPool model, int copies, int ss_slot0, int model_slot0,
                                                               const double* cl_x, const double* cl_u, int* cl_len, int Tcl, int N,
                                                               double* xLin, double* uLin, double* zt, double* OldInput, int* timeStep,
-                                                              int* hasPred, int* done, double TrackLength) {
+                                                              int* hasPred, int* done, Tracks trk) {
     const int b = blockIdx.x;
     if (b >= batch) return;
     const int Trec = cl_len[b];
+    const double TrackLength = trk.of(b).TrackLength;
     for (int c = 0; c < copies; ++c) {
         {
             const int T = min(Trec, ss.Tmax);

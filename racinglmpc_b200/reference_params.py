@@ -62,3 +62,80 @@ class VehicleParams:
         for bit)."""
         D = mu * m * 9.81 / 2.0
         return cls(m, lf, lr, Iz, D, Cf, Bf, D, Cr, Br)
+
+
+def _wrap(a):
+    if a < -np.pi:
+        return 2 * np.pi + a
+    if a > np.pi:
+        return a - 2 * np.pi
+    return a
+
+
+class TrackParams:
+    """A circuit as Map builds it (Track.py:54-133) from a spec of [length, radius] rows (radius 0: straight; negative: a right
+    turn), closed by a straight back to the origin.  ``table6`` = Map.PointAndTangent (x_end, y_end, psi_end, s_start, length,
+    curvature per row), ``seg_table`` = its columns 3:6 (what the device reads), ``TrackLength``.  The device takes one per
+    controller (BatchedController.set_tracks)."""
+
+    def __init__(self, table6):
+        self.table6 = np.array(table6, dtype=float).reshape(-1, 6)
+        self.seg_table = np.ascontiguousarray(self.table6[:, 3:6])
+        self.TrackLength = self.table6[-1, 3] + self.table6[-1, 4]
+
+    @classmethod
+    def from_spec(cls, spec):
+        """Map.__init__'s construction, operation for operation, so that the table equals the reference's bit for bit."""
+        spec = np.asarray(spec, dtype=float).reshape(-1, 2)
+        P = np.zeros((spec.shape[0] + 1, 6))
+        for i in range(spec.shape[0]):
+            length, r = spec[i, 0], spec[i, 1]
+            # where the segment starts: the origin heading along x, or the end of the previous segment
+            ang, x0, y0 = (0, 0, 0) if i == 0 else (P[i - 1, 2], P[i - 1, 0], P[i - 1, 1])
+            s0 = P[i, 3] if i == 0 else P[i - 1, 3] + P[i - 1, 4]
+            if r == 0.0:
+                P[i] = [x0 + length * np.cos(ang), y0 + length * np.sin(ang), ang, s0, length, 0]
+            else:
+                d = 1 if r >= 0 else -1
+                cx = x0 + np.abs(r) * np.cos(ang + d * np.pi / 2)
+                cy = y0 + np.abs(r) * np.sin(ang + d * np.pi / 2)
+                span = length / np.abs(r)
+                psi = _wrap(ang + span * np.sign(r))
+                normal = _wrap(d * np.pi / 2 + ang)
+                a = -(np.pi - np.abs(normal)) * (1 if normal >= 0 else -1)
+                P[i] = [cx + np.abs(r) * np.cos(a + d * span), cy + np.abs(r) * np.sin(a + d * span), psi, s0, length, 1 / r]
+        xs, ys = P[-2, 0], P[-2, 1]
+        P[-1] = [0, 0, 0, P[-2, 3] + P[-2, 4], np.sqrt((0 - xs) ** 2 + (0 - ys) ** 2), 0]
+        return cls(P)
+
+    @staticmethod
+    def l_shaped_spec():
+        """The track the reference drives (Track.py:30-40)."""
+        lc = 4.5
+        return np.array([[1.0, 0], [lc, lc / np.pi], [lc / 2, -lc / np.pi], [lc, lc / np.pi], [lc / np.pi * 2, 0],
+                         [lc / 2, lc / np.pi]])
+
+    @staticmethod
+    def goggle_spec():
+        """The goggle-shaped track (Track.py:15-28, commented out in the reference)."""
+        return np.array([[60 * 0.03, 0], [80 * 0.03, -80 * 0.03 * 2 / np.pi], [20 * 0.03, 0], [80 * 0.03, -80 * 0.03 * 2 / np.pi],
+                         [40 * 0.03, +40 * 0.03 * 10 / np.pi], [60 * 0.03, -60 * 0.03 * 5 / np.pi],
+                         [40 * 0.03, +40 * 0.03 * 10 / np.pi], [80 * 0.03, -80 * 0.03 * 2 / np.pi], [20 * 0.03, 0],
+                         [80 * 0.03, -80 * 0.03 * 2 / np.pi]])
+
+    @staticmethod
+    def oval_spec():
+        """A right-turning oval (Track.py:43-48, commented out in the reference).  Its closing straight is 6.3e-16 long."""
+        return np.array([[1.0, 0], [4.5, -4.5 / np.pi], [2.0, 0], [4.5, -4.5 / np.pi], [1.0, 0]])
+
+    @classmethod
+    def l_shaped(cls):
+        return cls.from_spec(cls.l_shaped_spec())
+
+    @classmethod
+    def goggle(cls):
+        return cls.from_spec(cls.goggle_spec())
+
+    @classmethod
+    def oval(cls):
+        return cls.from_spec(cls.oval_spec())
