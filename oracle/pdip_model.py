@@ -70,9 +70,9 @@ def kernel_constants(N, lmpc):
 
 
 def solve(qp, eps=1e-9, max_iter=60, verbose=False, eps_step=1e-7, eps_gap=None, mu0="auto", s0=0.3, gamma=0.01, warm=None, snap_mu=None,
-          warm_theta=0.5, mu0_scale=1.0, step=0.995, backoff=0.8, endgame_aff=None):
+          warm_theta=0.5, mu0_scale=1.0, step=0.995, backoff=0.8):
     """Returns dict(x[N+1,n], u[N,d], s[N,ncx], lam[m], xi[n], iters, r_prim, r_dual, gap, status).
-    s0 / mu0_scale / step / backoff / gamma / endgame_aff: starting point and step rule (defaults = the round-1 kernel;
+    s0 / mu0_scale / step / backoff / gamma: starting point and step rule (defaults = the round-1 kernel;
     ``solve(qp, **kernel_constants(qp.N, qp.m > 0))`` follows the kernel for either problem type)."""
     N, n, d = qp.N, 6, 2
     Fx, bx, Fu, bu = qp.Fx, qp.bx, qp.Fu, qp.bu
@@ -345,12 +345,8 @@ def solve(qp, eps=1e-9, max_iter=60, verbose=False, eps_step=1e-7, eps_gap=None,
         cc = solve_rhs(w1 * nu1 + aff["dw1"] * aff["dnu1"] - sm, w2 * nu2 + aff["dw2"] * aff["dnu2"] - sm,
                        s * nu3 + aff["ds"] * aff["dnu3"] - sm,
                        (lam * nu4 + aff["dlam"] * aff["dnu4"] - sm) if lmpc else None)
-        # end game (LMPC_TUNE_ENDGAME in the kernel): once the affine step is almost full, go to within max(step, min(0.9999, 1 - mu)) of the
-        # boundary and drop the neighbourhood test
-        endgame = endgame_aff is not None and a_aff >= endgame_aff
-        step_c = max(step, min(0.9999, 1.0 - mu)) if endgame else step
-        al = min(1.0, step_c * max_step(cc, 1e300))       # as the kernel: full step when the boundary is > 1/step away
-        if gamma > 0.0 and not endgame:
+        al = min(1.0, step * max_step(cc, 1e300))         # as the kernel: full step when the boundary is > 1/step away
+        if gamma > 0.0:
             # stay in a wide neighbourhood of the central path: min_i w_i nu_i >= gamma * mu
             def prods(a):
                 pr = [((w1 + a * cc["dw1"]) * (nu1 + a * cc["dnu1"])).ravel(), ((w2 + a * cc["dw2"]) * (nu2 + a * cc["dnu2"])).ravel(),

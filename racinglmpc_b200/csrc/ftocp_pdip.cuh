@@ -64,6 +64,9 @@
 //   LMPC_TUNE_MU0SCALE  initial complementarity of the input bounds and the simplex relative to the mean lane-row product
 //   LMPC_TUNE_MUFLOOR   floor of those products
 //   LMPC_TUNE_STEP      fraction of the step to the boundary
+// An end-game rule was tried and dropped: once the affine step is almost full, step to within max(fraction, 1 - mu) of the boundary
+// with no neighbourhood test; it saved 3-9 % of the iterations on the host emulation and made configs[1] and [2] 1-2 % faster, but
+// the Monte-Carlo rollouts left 67 instead of 2 of 5 M closed-loop QPs unsolved (DESIGN.md section 8).
 #ifndef LMPC_TUNE_S0
 #define LMPC_TUNE_S0 (LMPC ? 0.3 : (N <= 16 ? 0.1 : (N <= 24 ? 0.2 : 0.5)))
 #endif
@@ -75,29 +78,6 @@
 #endif
 #ifndef LMPC_TUNE_STEP
 #define LMPC_TUNE_STEP (LMPC ? 0.995 : 0.999)
-#endif
-// End game: once the affine (pure Newton) direction can be followed almost to the end (a_aff >= LMPC_TUNE_ENDGAME_AFF) the iterate is
-// in the region of fast local convergence; holding the corrector step back by the fixed fraction then only caps the gap reduction
-// at (1 - fraction) per iteration (the last two or three iterations of every solve walked from 1e-5 to 1e-11 that way), and the
-// neighbourhood test has nothing left to protect.  There the step goes to within a fraction max(LMPC_TUNE_STEP, min(CAP, 1 - K mu)) of the
-// boundary and the neighbourhood is LMPC_TUNE_ENDGAME_GAMMA (0 = not tested).  Host-emulation sweep: mean iterations
-// 6.10 / 6.92 / 7.57 / 8.92 -> 5.54 / 6.61 / 7.28 / 8.66 (MPC-type, N = 6 / 12 / 24 / 48), 10.87 -> 10.30 (closed-loop LMPC QPs), the
-// maxima unchanged.  OFF by default: on the device it is worth 1.8 % on configs[1] and 1.2 % on a configs[2] step, and the
-// Monte-Carlo rollouts, 3.6 % faster, left 67 instead of 2 of 5 M closed-loop QPs unsolved (DESIGN.md section 8).
-#ifndef LMPC_TUNE_ENDGAME
-#define LMPC_TUNE_ENDGAME 0
-#endif
-#ifndef LMPC_TUNE_ENDGAME_AFF
-#define LMPC_TUNE_ENDGAME_AFF 0.99
-#endif
-#ifndef LMPC_TUNE_ENDGAME_K
-#define LMPC_TUNE_ENDGAME_K 1.0
-#endif
-#ifndef LMPC_TUNE_ENDGAME_CAP
-#define LMPC_TUNE_ENDGAME_CAP 0.9999      // the gap shrinks by at most 1e4 per iteration: 1e-5 -> 1e-9 -> 1e-13 without running the barrier
-#endif                                    // weights into the rounding floor of the factorisation
-#ifndef LMPC_TUNE_ENDGAME_GAMMA
-#define LMPC_TUNE_ENDGAME_GAMMA 0.0
 #endif
 #ifndef LMPC_TUNE_SIGMA
 #define LMPC_TUNE_SIGMA(s) ((s) * (s) * (s))      // Mehrotra's centring parameter from the affine complementarity ratio
@@ -1938,13 +1918,7 @@ LMPC_SWEEP_UNROLL
                     }
                 }
                 const double amax = wmin_nn(ratio_bound(rn, rd, 1e300));
-#if LMPC_TUNE_ENDGAME
-                const bool endgame = (pass == 0) && (a_aff >= LMPC_TUNE_ENDGAME_AFF);
-                al = fmin(1.0, (endgame ? fmax(LMPC_TUNE_STEP, fmin(LMPC_TUNE_ENDGAME_CAP, 1.0 - LMPC_TUNE_ENDGAME_K * mu)) : LMPC_TUNE_STEP) * amax);
-#else
-                const bool endgame = false;
                 al = fmin(1.0, LMPC_TUNE_STEP * amax);
-#endif
                 if (!(al > 0.0) || !(al <= 1.0)) { bad_step = true; break; }
                 // Stay in a wide neighbourhood of the central path, min_i w_i nu_i >= gamma * mean: without it
                 // Mehrotra steps can 2-cycle against a blocking bound (seen on 3 of 4096 workload QPs).
@@ -1971,7 +1945,7 @@ LMPC_SWEEP_UNROLL
                     }
                     pmin = wmin(pmin);
                     psum = wsum(psum);
-                    if (pmin >= ((endgame ? LMPC_TUNE_ENDGAME_GAMMA : LMPC_TUNE_GAMMA) / n_ineq) * psum) { inside = true; break; }
+                    if (pmin >= (LMPC_TUNE_GAMMA / n_ineq) * psum) { inside = true; break; }
                     if (pass == 0 && tries >= RECENTRE_AFTER) break;
 #if defined(LMPC_HOST_COUNT) && !defined(__CUDA_ARCH__)
                     g_host_count[2] += 1;                // step reductions

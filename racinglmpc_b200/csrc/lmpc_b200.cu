@@ -34,9 +34,6 @@
 using namespace lmpc;
 
 #define LMPC_HOST_SLOTS 4              // buffer sets (batches in flight) of the asynchronous host entry points
-#ifndef LMPC_STEP_SPLIT_DEFAULT
-#define LMPC_STEP_SPLIT_DEFAULT 1     // instance ranges of the pipelined device-resident step (1 = one launch sequence)
-#endif
 
 // ------------------------------------------------------------------------------------------------
 // host side
@@ -69,12 +66,6 @@ struct lmpc_handle {
     int hb_chunks[LMPC_HOST_SLOTS];
     bool hb_pending[LMPC_HOST_SLOTS];            // enqueued and not yet waited for
     bool hb_lone;                                // set by the synchronous entry points: the batch being enqueued runs alone
-    // pipelined device-resident step: the batch is cut into step_split instance ranges, each running its kernel sequence on its
-    // own stream (cstream[0..3]) between a fork and a join event on `stream`
-    int step_split;
-    cudaEvent_t ev_fork, ev_join[4];
-    bool trace_on;
-    cudaEvent_t tev[4][3], t0ev;
     long long launches;
     // QP buffer sets, one per slot of the *_host entry points.  hb[0] is allocated at creation and is also the device-resident
     // step's (K1 writes its abc, K2 its safe set, the QP kernel its outputs; lmpc_device_buffer); hb[1..] on first use.
@@ -355,10 +346,6 @@ static int create_device_side(lmpc_handle* h) {
     if (rc != LMPC_OK) return rc;
     CK(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
     for (int i = 0; i < 4 * LMPC_HOST_SLOTS; ++i) CK(cudaStreamCreateWithFlags(&h->cstream[i], cudaStreamNonBlocking));
-    CK(cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming));
-    for (int i = 0; i < 4; ++i) CK(cudaEventCreateWithFlags(&h->ev_join[i], cudaEventDisableTiming));
-    h->step_split = LMPC_STEP_SPLIT_DEFAULT;
-    if (const char* e = getenv("LMPC_B200_STEP_SPLIT")) { const int v = atoi(e); if (v >= 1 && v <= 4) h->step_split = v; }   // tuning knob
     if (!qp_bufs(h, 0)) return LMPC_E_CUDA;
     CK(cudaMalloc((void**)&h->d_late, sizeof(unsigned long long)));
     CK(cudaMemset(h->d_late, 0, sizeof(unsigned long long)));
@@ -514,8 +501,6 @@ int lmpc_destroy(lmpc_handle* h) {
     cudaFree(h->d_veh_idx);
     if (h->stream) cudaStreamDestroy(h->stream);
     for (int i = 0; i < 4 * LMPC_HOST_SLOTS; ++i) if (h->cstream[i]) cudaStreamDestroy(h->cstream[i]);
-    if (h->ev_fork) cudaEventDestroy(h->ev_fork);
-    for (int i = 0; i < 4; ++i) if (h->ev_join[i]) cudaEventDestroy(h->ev_join[i]);
     delete h;
     return LMPC_OK;
 }
@@ -582,7 +567,7 @@ int lmpc_solve_lmpc_dev(lmpc_handle* h, const double* x0, const double* uOld, co
     if (lm && ((rc = check_align(SS_sel, "SS_sel")) != LMPC_OK || (rc = check_align(Qfun_sel, "Qfun_sel")) != LMPC_OK)) return rc;
     CK(cudaSetDevice(h->device));
     FtocpArgs a = {};   // no warm-start records: caller-supplied QPs start cold; the controllers of the device-resident step
-                        // carry warm-start records (step_range)
+                        // carry warm-start records (step_dev_impl)
     a.batch = h->batch;
     a.x0 = x0; a.uOld = uOld; a.abc = abc;
     a.abc_inst_stride = abc_inst_stride; a.abc_stage_stride = abc_stage_stride;
@@ -633,20 +618,13 @@ static int enqueue_host_solve_impl(lmpc_handle* h, int slot, const double* x0, c
     // of range i+1, the solve of range i and the D2H copy of range i-1 overlap (PCIe is full duplex).
     // A batch enqueued through the asynchronous entry points shares the device with the batches of the other buffer sets: that
     // overlap is already there, every further piece is ten more driver calls on the enqueueing thread and one more under-filled
-    // last wave.  Measured on configs[1] (4096 QPs, three sets in flight, tools/e2e_probe.py, two hosts): 8.8-9.6 M solves/s uncut,
-    // 8.7-9.6 M in two pieces, 8.2-8.6 M in four; a lone synchronous batch: 3.1 M uncut, 3.7 M in two, 3.9 M in four.
+    // last wave.  Measured on configs[1] (4096 QPs, three sets in flight, two hosts) with tools/e2e_probe.py, which A/B'd the
+    // policies through an environment override that has since been removed: 8.8-9.6 M solves/s uncut, 8.7-9.6 M in two pieces,
+    // 8.2-8.6 M in four; a lone synchronous batch: 3.1 M uncut, 3.7 M in two, 3.9 M in four.
     bool others = false;
     for (int sl = 0; sl < LMPC_HOST_SLOTS; ++sl) others |= (sl != slot && h->hb_pending[sl]);
     const bool lone = h->hb_lone && !others;
-    int nchunk = B >= 2048 ? (lone ? 4 : (others ? 1 : 2)) : (B >= 512 ? (others ? 1 : 2) : 1);
-    if (const char* e = getenv("LMPC_B200_CHUNKS")) { int v = atoi(e); if (v >= 1 && v <= 4 && (size_t)v <= B) nchunk = v; }   // tuning knob
-    const bool trace = slot == 0 && getenv("LMPC_B200_TRACE") != nullptr;
-    if (trace) {
-        cudaEventCreate(&h->t0ev);
-        for (int i = 0; i < nchunk; ++i) for (int j = 0; j < 3; ++j) cudaEventCreate(&h->tev[i][j]);
-        cudaEventRecord(h->t0ev, cs[0]);
-    }
-    h->trace_on = trace;
+    const int nchunk = B >= 2048 ? (lone ? 4 : (others ? 1 : 2)) : (B >= 512 ? (others ? 1 : 2) : 1);
     FtocpArgs all = qp_args(h, hb, lm, (Succ_SS ? QP_SUCC_SS : 0) | (Succ_uSS ? QP_SUCC_U : 0) | (slack ? QP_SLACK : 0) |
                                        (lambd ? QP_LAMBD : 0) | (slackTerminal ? QP_SLACKT : 0) | (zt ? QP_ZT : 0) |
                                        (zt_u ? QP_ZTU : 0));
@@ -663,10 +641,8 @@ static int enqueue_host_solve_impl(lmpc_handle* h, int slot, const double* x0, c
             if (Succ_SS) CK(cudaMemcpyAsync(hb.SuccSS + lo * 6 * M, Succ_SS + lo * 6 * M, nb * 6 * M * D, cudaMemcpyHostToDevice, s));
             if (Succ_uSS) CK(cudaMemcpyAsync(hb.SuccU + lo * 2 * M, Succ_uSS + lo * 2 * M, nb * 2 * M * D, cudaMemcpyHostToDevice, s));
         }
-        if (trace) cudaEventRecord(h->tev[ci][0], s);
         int rc = launch(h, all.range((int)lo, (int)nb, (int)N, h->M), lm, s);
         if (rc != LMPC_OK) return rc;
-        if (trace) cudaEventRecord(h->tev[ci][1], s);
         CK(cudaMemcpyAsync(xPred + lo * (N + 1) * 6, hb.xPred + lo * (N + 1) * 6, nb * (N + 1) * 6 * D, cudaMemcpyDeviceToHost, s));
         CK(cudaMemcpyAsync(uPred + lo * N * 2, hb.uPred + lo * N * 2, nb * N * 2 * D, cudaMemcpyDeviceToHost, s));
         if (slack) CK(cudaMemcpyAsync(slack + lo * N * 2, hb.slack + lo * N * 2, nb * N * 2 * D, cudaMemcpyDeviceToHost, s));
@@ -677,7 +653,6 @@ static int enqueue_host_solve_impl(lmpc_handle* h, int slot, const double* x0, c
         CK(cudaMemcpyAsync(status + lo, hb.status + lo, nb * sizeof(int), cudaMemcpyDeviceToHost, s));
         CK(cudaMemcpyAsync(iters + lo, hb.iters + lo, nb * sizeof(int), cudaMemcpyDeviceToHost, s));
         CK(cudaMemcpyAsync(resid + lo * 3, hb.resid + lo * 3, nb * 3 * D, cudaMemcpyDeviceToHost, s));
-        if (trace) cudaEventRecord(h->tev[ci][2], s);
     }
     h->hb_chunks[slot] = nchunk;
     h->hb_pending[slot] = true;
@@ -715,16 +690,6 @@ int lmpc_host_wait(lmpc_handle* h, int slot) {
     const int nchunk = h->hb_chunks[slot] > 0 ? h->hb_chunks[slot] : 4;
     for (int ci = 0; ci < nchunk; ++ci) CK(cudaStreamSynchronize(h->cstream[4 * slot + ci]));
     h->hb_pending[slot] = false;
-    if (slot == 0 && h->trace_on) {
-        for (int i = 0; i < nchunk; ++i) {
-            float a_ = 0, b_ = 0, c_ = 0;
-            cudaEventElapsedTime(&a_, h->t0ev, h->tev[i][0]); cudaEventElapsedTime(&b_, h->t0ev, h->tev[i][1]); cudaEventElapsedTime(&c_, h->t0ev, h->tev[i][2]);
-            fprintf(stderr, "chunk %d: h2d done %.3f ms, kernel done %.3f, d2h done %.3f\n", i, a_, b_, c_);
-            for (int j = 0; j < 3; ++j) cudaEventDestroy(h->tev[i][j]);
-        }
-        cudaEventDestroy(h->t0ev);
-        h->trace_on = false;
-    }
     return LMPC_OK;
 }
 
@@ -989,7 +954,7 @@ int lmpc_ss_add_point(lmpc_handle* h, const double* x, const double* u) {
     CK(cudaMemcpyAsync(h->d_tmpx, x, sizeof(double) * h->batch * 6, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(h->d_tmpu, u, sizeof(double) * h->batch * 2, cudaMemcpyHostToDevice, h->stream));
     ss_add_point_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->batch, h->ss, h->d_prevslot, h->d_tmpx, h->d_tmpu, 2,
-                                                                        tracks(h), h->d_flags, h->d_dropped, 0);
+                                                                        tracks(h), h->d_flags, h->d_dropped);
     CK(cudaGetLastError());
     h->launches += 1;
     int dropped = 0;
@@ -1065,34 +1030,30 @@ int lmpc_state_get(lmpc_handle* h, double* xLin, double* uLin, double* zt, doubl
     return LMPC_OK;
 }
 
-static int launch_k1(lmpc_handle* h, int b0 = 0, int nb = -1, cudaStream_t st = nullptr) {
-    if (nb < 0) nb = h->batch;
-    if (!st) st = h->stream;
+static int launch_k1(lmpc_handle* h) {
     K1Args a;
-    a.batch = h->batch; a.N = h->N; a.b0 = b0;
+    a.batch = h->batch; a.N = h->N;
     a.wpb = h->N < 12 ? h->N : 12;
     a.pts_stride = k1_pts_stride(h->mc.trToUse);
     a.xLin = h->d_xLin; a.uLin = h->d_uLin; a.pool = h->mdl; a.used = h->d_used; a.abc = h->hb[0].abc; a.status = h->d_flags;
     a.trk = tracks(h);
-    dim3 grid(nb, (h->N + a.wpb - 1) / a.wpb);
+    dim3 grid(h->batch, (h->N + a.wpb - 1) / a.wpb);
     size_t smem = sizeof(float) * 5 * K1_TILE + sizeof(double) * (size_t)a.pts_stride * a.wpb;
-    knn_ltv_regress_kernel<<<grid, 32 * a.wpb, smem, st>>>(h->mc, a);
+    knn_ltv_regress_kernel<<<grid, 32 * a.wpb, smem, h->stream>>>(h->mc, a);
     CK(cudaGetLastError());
     h->launches += 1;
     return LMPC_OK;
 }
 
-static int launch_k2(lmpc_handle* h, const double* d_x0, int b0 = 0, int nb = -1, cudaStream_t st = nullptr) {
-    if (nb < 0) nb = h->batch;
-    if (!st) st = h->stream;
+static int launch_k2(lmpc_handle* h, const double* d_x0) {
     K2Args a;
-    a.batch = h->batch; a.N = h->N; a.b0 = b0; a.numSS_it = h->p.numSS_it; a.P = h->M / h->p.numSS_it;
+    a.batch = h->batch; a.N = h->N; a.numSS_it = h->p.numSS_it; a.P = h->M / h->p.numSS_it;
     a.trk = tracks(h);
     a.x0 = d_x0; a.zt = h->d_ztState; a.pool = h->ss; a.sel = h->d_sel; a.is_prev = h->d_isprev;
     a.timeStep = h->d_timeStep; a.has_pred = h->d_hasPred; a.xPred = h->d_xPredPrev;
     a.SS_sel = h->hb[0].SS; a.Qfun_sel = h->hb[0].Qfun; a.Succ_SS = h->hb[0].SuccSS; a.Succ_uSS = h->hb[0].SuccU;
     a.zt_fixed = h->d_ztFixed; a.status = h->d_flags; a.min_index = h->d_minidx;
-    ss_select_kernel<<<nb, 32 * a.numSS_it, 0, st>>>(a);
+    ss_select_kernel<<<h->batch, 32 * a.numSS_it, 0, h->stream>>>(a);
     CK(cudaGetLastError());
     h->launches += 1;
     return LMPC_OK;
@@ -1133,9 +1094,49 @@ int lmpc_select_host(lmpc_handle* h, const double* x0, double* SS_sel, double* Q
     return LMPC_OK;
 }
 
-struct StepTail;
-static int step_dev_impl(lmpc_handle* h, int mode, const double* x0_dev, cudaEvent_t* ev, const StepTail* tail);
-int lmpc_step_dev(lmpc_handle* h, int mode, const double* x0_dev) { return step_dev_impl(h, mode, x0_dev, nullptr, nullptr); }
+}  // extern "C"
+
+// One device-resident step for the whole batch on the handle's stream: K1 -> K2 -> QP -> shift (PC.py:110-137).  ev (five events
+// or null) brackets the four kernels for lmpc_step_profile.
+static int step_dev_impl(lmpc_handle* h, int mode, const double* x0_dev, cudaEvent_t* ev) {
+    int rc = need_store(h);
+    if (rc) return rc;
+    if (!x0_dev || (mode != 0 && mode != 1)) return fail(LMPC_E_INVALID, "bad mode or null x0");
+    if (mode == 1 && h->M <= 0) return fail(LMPC_E_INVALID, "LMPC step on a handle without a safe set");
+    CK(cudaSetDevice(h->device));
+    cudaStream_t st = h->stream;
+    CK(cudaMemsetAsync(h->d_flags, 0, sizeof(int) * h->batch, st));
+    if (h->d_warm && h->warm_mode != mode) {             // records of the other problem type are not comparable
+        CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * h->batch, st));
+        h->warm_mode = mode;
+    }
+    const bool lm = mode == 1;
+    const QpBufs& q = h->hb[0];
+    if (ev) CK(cudaEventRecord(ev[0], st));
+    if ((rc = launch_k1(h)) != LMPC_OK) return rc;                                   // PC.py:117
+    if (ev) CK(cudaEventRecord(ev[1], st));
+    if (lm && (rc = launch_k2(h, x0_dev)) != LMPC_OK) return rc;                     // PC.py:121
+    if (ev) CK(cudaEventRecord(ev[2], st));
+    FtocpArgs a = qp_args(h, q, lm, QP_ALL);                                         // PC.py:124-125
+    a.x0 = x0_dev; a.uOld = h->d_OldInput;
+    if (h->d_warm) { a.warm = h->d_warm; a.warm_valid = h->d_warm_valid; a.warm_stride = h->warm_stride; }
+    if ((rc = launch(h, a, lm, st)) != LMPC_OK) return rc;
+    if (ev) CK(cudaEventRecord(ev[3], st));
+    ShiftArgs sa;
+    sa.batch = h->batch; sa.N = h->N; sa.lmpc = mode;
+    sa.xPred = q.xPred; sa.uPred = q.uPred; sa.zt_in = q.zt; sa.ztu_in = q.ztu;
+    sa.xLin = h->d_xLin; sa.uLin = h->d_uLin; sa.zt = h->d_ztState; sa.OldInput = h->d_OldInput; sa.xPredPrev = h->d_xPredPrev;
+    sa.timeStep = h->d_timeStep; sa.has_pred = h->d_hasPred;
+    shift_state_kernel<<<h->batch, 64, 0, st>>>(sa);                                 // PC.py:129-137
+    CK(cudaGetLastError());
+    h->launches += 1;
+    if (ev) CK(cudaEventRecord(ev[4], st));
+    return LMPC_OK;
+}
+
+extern "C" {
+
+int lmpc_step_dev(lmpc_handle* h, int mode, const double* x0_dev) { return step_dev_impl(h, mode, x0_dev, nullptr); }
 
 // The same step with CUDA events between its kernels: ms4 = durations of K1 (regression), K2 (selection; 0 for mode 0), the QP
 // kernel and the state shift.  Measurement support (bench.py's per-kernel rooflines); synchronises.
@@ -1144,91 +1145,13 @@ int lmpc_step_profile(lmpc_handle* h, int mode, const double* x0_dev, float* ms4
     CK(cudaSetDevice(h->device));
     cudaEvent_t ev[5];
     for (int i = 0; i < 5; ++i) CK(cudaEventCreate(&ev[i]));
-    int rc = step_dev_impl(h, mode, x0_dev, ev, nullptr);
+    int rc = step_dev_impl(h, mode, x0_dev, ev);
     if (rc == LMPC_OK && cudaStreamSynchronize(h->stream) != cudaSuccess) rc = fail(LMPC_E_CUDA, "stream synchronisation failed");
     if (rc == LMPC_OK)
         for (int i = 0; i < 4; ++i) cudaEventElapsedTime(&ms4[i], ev[i], ev[i + 1]);
     for (int i = 0; i < 5; ++i) cudaEventDestroy(ev[i]);
     return rc;
 }
-}  // extern "C"
-
-// K1 -> K2 -> QP -> shift (PC.py:110-137) for the controllers [b0, b0 + nb) on stream st.  `tail` (rollouts) appends what
-// Simulator.sim does with the result for the same controllers: addPoint (mode 1) and dynModel.
-struct StepTail { const double* xc; SimArgs sim; };
-static int step_range(lmpc_handle* h, int mode, const double* x0_dev, cudaEvent_t* ev, int b0, int nb, cudaStream_t st, const StepTail* tail) {
-    int rc;
-    const bool lm = mode == 1;
-    const QpBufs& q = h->hb[0];
-    if ((rc = launch_k1(h, b0, nb, st)) != LMPC_OK) return rc;                       // PC.py:117
-    if (ev) CK(cudaEventRecord(ev[1], st));
-    if (lm && (rc = launch_k2(h, x0_dev, b0, nb, st)) != LMPC_OK) return rc;         // PC.py:121
-    if (ev) CK(cudaEventRecord(ev[2], st));
-    FtocpArgs a = qp_args(h, q, lm, QP_ALL);                                         // PC.py:124-125
-    a.x0 = x0_dev; a.uOld = h->d_OldInput;
-    if (h->d_warm) { a.warm = h->d_warm; a.warm_valid = h->d_warm_valid; a.warm_stride = h->warm_stride; }
-    if ((rc = launch(h, a.range(b0, nb, h->N, h->M), lm, st)) != LMPC_OK) return rc;
-    if (ev) CK(cudaEventRecord(ev[3], st));
-    ShiftArgs sa;
-    sa.batch = h->batch; sa.N = h->N; sa.lmpc = mode; sa.b0 = b0;
-    sa.xPred = q.xPred; sa.uPred = q.uPred; sa.zt_in = q.zt; sa.ztu_in = q.ztu;
-    sa.xLin = h->d_xLin; sa.uLin = h->d_uLin; sa.zt = h->d_ztState; sa.OldInput = h->d_OldInput; sa.xPredPrev = h->d_xPredPrev;
-    sa.timeStep = h->d_timeStep; sa.has_pred = h->d_hasPred;
-    shift_state_kernel<<<nb, 64, 0, st>>>(sa);                                       // PC.py:129-137
-    CK(cudaGetLastError());
-    h->launches += 1;
-    if (ev) CK(cudaEventRecord(ev[4], st));
-    if (tail) {
-        if (lm) {                                                                    // SysModel.py:38 -> PC.py:466-476
-            ss_add_point_kernel<<<(nb + 127) / 128, 128, 0, st>>>(b0 + nb, h->ss, h->d_prevslot, tail->xc, q.uPred, (long long)h->N * 2,
-                                                                  tracks(h), h->d_flags, nullptr, b0);
-            CK(cudaGetLastError());
-            h->launches += 1;
-        }
-        SimArgs sim = tail->sim;                                                     // SysModel.py:40 (dynModel)
-        sim.b0 = b0; sim.b1 = b0 + nb;
-        sim_step_kernel<<<(nb + 127) / 128, 128, 0, st>>>(h->mc, sim);
-        CK(cudaGetLastError());
-        h->launches += 1;
-    }
-    return LMPC_OK;
-}
-
-// The whole batch: one launch sequence on the handle's stream, or -- step_split > 1 -- one per instance range, each on its own
-// stream between a fork and a join on the handle's stream.  The controllers are independent (PC.py:317-333), so the ranges only
-// share the GPU: the regression scan of one range (issue-bound) runs under the interior-point solves of another (latency-bound)
-// and the last waves of one range's solves are filled by the next range's.  Results are bit-identical to the unsplit step.
-static int step_dev_impl(lmpc_handle* h, int mode, const double* x0_dev, cudaEvent_t* ev, const StepTail* tail) {
-    int rc = need_store(h);
-    if (rc) return rc;
-    if (!x0_dev || (mode != 0 && mode != 1)) return fail(LMPC_E_INVALID, "bad mode or null x0");
-    if (mode == 1 && h->M <= 0) return fail(LMPC_E_INVALID, "LMPC step on a handle without a safe set");
-    CK(cudaSetDevice(h->device));
-    CK(cudaMemsetAsync(h->d_flags, 0, sizeof(int) * h->batch, h->stream));
-    if (h->d_warm && h->warm_mode != mode) {             // records of the other problem type are not comparable
-        CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * h->batch, h->stream));
-        h->warm_mode = mode;
-    }
-    if (ev) CK(cudaEventRecord(ev[0], h->stream));
-    int split = ev ? 1 : h->step_split;                  // the per-kernel timing of lmpc_step_profile needs the kernels back to back
-    if (split > h->batch / 256) split = h->batch / 256;  // ranges below a few hundred controllers only add launches
-    if (split <= 1) return step_range(h, mode, x0_dev, ev, 0, h->batch, h->stream, tail);
-    CK(cudaEventRecord(h->ev_fork, h->stream));
-    for (int r = 0; r < split; ++r) {
-        const int b0 = (int)((long long)h->batch * r / split), b1 = (int)((long long)h->batch * (r + 1) / split);
-        cudaStream_t st = h->cstream[r];
-        CK(cudaStreamWaitEvent(st, h->ev_fork, 0));
-        if ((rc = step_range(h, mode, x0_dev, nullptr, b0, b1 - b0, st, tail)) != LMPC_OK) break;
-        CK(cudaEventRecord(h->ev_join[r], st));
-    }
-    if (rc != LMPC_OK) {                                  // ranges already enqueued finish before the error is reported
-        for (int r = 0; r < split; ++r) cudaStreamSynchronize(h->cstream[r]);
-        return rc;
-    }
-    for (int r = 0; r < split; ++r) CK(cudaStreamWaitEvent(h->stream, h->ev_join[r], 0));
-    return LMPC_OK;
-}
-extern "C" {
 
 int lmpc_step_host(lmpc_handle* h, int mode, const double* x0, double* xPred, double* uPred, double* lambd, double* zt,
                    double* zt_u, double* SS_sel, int* status, int* iters, double* resid, int* flags) {
@@ -1372,6 +1295,18 @@ int lmpc_rollout_get_health(lmpc_handle* h, int* flags_or, int* unsolved_steps) 
     return LMPC_OK;
 }
 
+// The simulator's arguments for one closed-loop step of the whole batch: state cur -> cur ^ 1 under the input uPred[b][0], noise z
+// ([B][3] standard-normal draws) or, when null, Philox.  The health inputs (flags, status, health) stay null.
+static SimArgs sim_args(const lmpc_handle* h, const double* z, unsigned long long seed) {
+    SimArgs sa = {};
+    sa.batch = h->batch; sa.x = h->d_rx[h->cur]; sa.xg = h->d_rg[h->cur]; sa.u = h->hb[0].uPred; sa.u_stride = (long long)h->N * 2;
+    sa.z = z; sa.seed = seed; sa.step = h->sim_step;
+    sa.xn = h->d_rx[h->cur ^ 1]; sa.xgn = h->d_rg[h->cur ^ 1];
+    sa.cl_x = h->d_clx; sa.cl_u = h->d_clu; sa.cl_len = h->d_cllen; sa.Tcl = h->Tcl; sa.done = h->d_done;
+    sa.veh = h->d_veh; sa.veh_idx = h->d_veh_idx; sa.trk = tracks(h);
+    return sa;
+}
+
 // One closed-loop step for every instance, all on the device (SysModel.py:34-48):
 //   Controller.solve(x) -> u = uPred[0] -> Controller.addPoint(x, u) (LMPC) -> x+ = dynModel(x, x_glob, u); done = s+ > TrackLength
 int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned long long seed) {
@@ -1381,44 +1316,33 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
     const QpBufs& q = h->hb[0];
     const double* xc = h->d_rx[h->cur];
     if (z_host) CK(cudaMemcpyAsync(h->d_z, z_host, sizeof(double) * h->batch * 3, cudaMemcpyHostToDevice, h->stream));
-    StepTail tail;
-    tail.xc = xc;
-    SimArgs& sa = tail.sim;
-    sa.batch = h->batch; sa.x = xc; sa.xg = h->d_rg[h->cur]; sa.u = q.uPred; sa.u_stride = (long long)h->N * 2;
-    sa.z = z_host ? h->d_z : nullptr; sa.seed = seed; sa.step = h->sim_step;
-    sa.xn = h->d_rx[h->cur ^ 1]; sa.xgn = h->d_rg[h->cur ^ 1];
-    sa.cl_x = h->d_clx; sa.cl_u = h->d_clu; sa.cl_len = h->d_cllen; sa.Tcl = h->Tcl; sa.done = h->d_done; sa.active = nullptr;
-    sa.flags = h->d_flags; sa.status = q.status; sa.health = h->d_health;
-    sa.veh = h->d_veh; sa.veh_idx = h->d_veh_idx; sa.trk = tracks(h);
-    // the trace of the chosen controllers reads the step's results and the state before dynModel: it has to sit between the
-    // solve and the simulator, so a traced batch runs the simulator for the whole batch after it
-    const bool fused_tail = !h->has_trace && mode != 2;
     if (mode == 2) {
         CK(cudaMemsetAsync(h->d_flags, 0, sizeof(int) * h->batch, h->stream));
         // LTI MPC with the per-instance model identified by lmpc_rollout_sysid (main.py:72-80); like the reference's LTI
         // controller it never refreshes the input-rate reference (OldInput keeps its initial value, PC.py:113-115)
         rc = lmpc_solve_mpc_dev(h, xc, h->d_OldInput, h->d_abc_lti, 54, 0, q.xPred, q.uPred, q.slack, q.status, q.iters, q.resid);
     } else {
-        rc = step_dev_impl(h, mode, xc, nullptr, fused_tail ? &tail : nullptr);
+        rc = step_dev_impl(h, mode, xc, nullptr);
     }
     if (rc) return rc;
-    if (!fused_tail) {
-        if (mode == 1) {
-            ss_add_point_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->batch, h->ss, h->d_prevslot, xc, q.uPred,
-                                                                                (long long)h->N * 2, tracks(h), h->d_flags, nullptr, 0);
-            CK(cudaGetLastError());
-            h->launches += 1;
-        }
-        if (h->has_trace) {
-            trace_step_kernel<<<h->tr.n, 128, 0, h->stream>>>(h->tr, xc, h->d_rg[h->cur], q.uPred, (long long)h->N * 2, q.xPred,
-                                                            mode == 1 ? q.SS : nullptr, h->has_books ? h->bk.lap_n : nullptr);
-            CK(cudaGetLastError());
-            h->launches += 1;
-        }
-        sim_step_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->mc, sa);
+    if (mode == 1) {                                                                 // SysModel.py:38 -> PC.py:466-476
+        ss_add_point_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->batch, h->ss, h->d_prevslot, xc, q.uPred,
+                                                                            (long long)h->N * 2, tracks(h), h->d_flags, nullptr);
         CK(cudaGetLastError());
         h->launches += 1;
     }
+    // the trace of the chosen controllers reads the step's results and the state before dynModel
+    if (h->has_trace) {
+        trace_step_kernel<<<h->tr.n, 128, 0, h->stream>>>(h->tr, xc, h->d_rg[h->cur], q.uPred, (long long)h->N * 2, q.xPred,
+                                                        mode == 1 ? q.SS : nullptr, h->has_books ? h->bk.lap_n : nullptr);
+        CK(cudaGetLastError());
+        h->launches += 1;
+    }
+    SimArgs sa = sim_args(h, z_host ? h->d_z : nullptr, seed);                       // SysModel.py:40 (dynModel)
+    sa.flags = h->d_flags; sa.status = q.status; sa.health = h->d_health;
+    sim_step_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->mc, sa);
+    CK(cudaGetLastError());
+    h->launches += 1;
     h->cur ^= 1;
     h->sim_step += 1;
     return LMPC_OK;
@@ -1438,14 +1362,7 @@ int lmpc_rollout_pid_step(lmpc_handle* h, double vt, const double* z_pid_host, c
     pa.batch = h->batch; pa.x = xc; pa.vt = vt; pa.z = z_pid_host ? h->d_zpid : nullptr; pa.seed = seed; pa.step = h->sim_step;
     pa.u = h->hb[0].uPred; pa.u_stride = (long long)h->N * 2;
     pid_input_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(pa);
-    SimArgs sa;
-    sa.batch = h->batch; sa.x = xc; sa.xg = h->d_rg[h->cur]; sa.u = h->hb[0].uPred; sa.u_stride = (long long)h->N * 2;
-    sa.z = z_sim_host ? h->d_z : nullptr; sa.seed = seed; sa.step = h->sim_step;
-    sa.xn = h->d_rx[h->cur ^ 1]; sa.xgn = h->d_rg[h->cur ^ 1];
-    sa.cl_x = h->d_clx; sa.cl_u = h->d_clu; sa.cl_len = h->d_cllen; sa.Tcl = h->Tcl; sa.done = h->d_done; sa.active = nullptr;
-    sa.flags = nullptr; sa.status = nullptr; sa.health = nullptr;
-    sa.veh = h->d_veh; sa.veh_idx = h->d_veh_idx; sa.trk = tracks(h);
-    sim_step_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->mc, sa);
+    sim_step_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->mc, sim_args(h, z_sim_host ? h->d_z : nullptr, seed));
     CK(cudaGetLastError());
     h->launches += 2;
     h->cur ^= 1;

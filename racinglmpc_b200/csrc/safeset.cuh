@@ -127,9 +127,11 @@ constexpr float K1_FAR = 1.0e18f; // feature value of the padding rows of a tile
 
 struct K1Args {
     int batch, N, wpb, pts_stride;   // warps per block; doubles of per-warp scratch (see k1_pts_stride)
-    int b0 = 0;           // first instance of the range this launch covers (grid.x = its size): the pipelined step launches one
-                          // instance range per stream, every array below stays indexed by the global instance
-    const double* xLin;   // [B][N+1][6]
+    // Always 0: every launch covers the whole batch.  Kept because with the instance index read as b0 + blockIdx.x ptxas
+    // rematerialises it instead of holding it in a register; with b = blockIdx.x the kernel spills 16 B at its 56-register cap and
+    // the closed loop of configs[3] ran about 1 % slower (H100 80GB HBM3, profiles/h100_one_step_sequence_ab.txt).
+    int b0 = 0;
+    const double* xLin;  // [B][N+1][6]
     const double* uLin;   // [B][N][2]
     LapPool pool;         // model pool
     const int* used;      // [B][trToUse] slot ids, in usedIt order
@@ -469,7 +471,6 @@ __global__ void __launch_bounds__(32 * 12, LMPC_K1_MINBLOCKS) knn_ltv_regress_ke
 // ------------------------------------------------------------------------------------------------
 struct K2Args {
     int batch, N, numSS_it, P;   // P = numSS_Points / numSS_it
-    int b0 = 0;              // first instance of this launch's range (see K1Args::b0); batch bounds the global index
     Tracks trk;
     const double* x0;        // [B][6]
     const double* zt;        // [B][6]
@@ -490,7 +491,7 @@ struct K2Args {
 
 // One CTA per instance, one warp per selected lap.
 __global__ void __launch_bounds__(32 * 8) ss_select_kernel(const K2Args a) {
-    const int b = a.b0 + blockIdx.x;
+    const int b = blockIdx.x;
     const int c = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     if (b >= a.batch || c >= a.numSS_it) return;
@@ -572,8 +573,8 @@ __global__ void __launch_bounds__(32 * 8) ss_select_kernel(const K2Args a) {
 // ------------------------------------------------------------------------------------------------
 // LMPC.addPoint (PC.py:466-476): append x + [0,0,0,0,L,0], u to lap it-1; Qfun extends by last - 1.
 __global__ void ss_add_point_kernel(int batch, LapPool pool, const int* prev_slot, const double* x, const double* u,
-                                    long long u_stride, Tracks trk, int* status, int* dropped, int b0) {
-    const int b = b0 + blockIdx.x * blockDim.x + threadIdx.x;     // instances [b0, batch)
+                                    long long u_stride, Tracks trk, int* status, int* dropped) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= batch) return;
     const int slot = prev_slot[b];
     if (slot < 0) return;
@@ -755,8 +756,7 @@ __global__ void __launch_bounds__(256) commit_laps_kernel(int batch, LapPool ss,
 // MPC.solve tail (PC.py:129-137): xLin = [xPred[1:]; zt], uLin = [uPred[1:]; zt_u], OldInput = uPred[0], timeStep += 1
 struct ShiftArgs {
     int batch, N, lmpc;
-    int b0 = 0;            // first instance of this launch's range (see K1Args::b0)
-    const double* xPred;   // [B][N+1][6]
+    const double* xPred;  // [B][N+1][6]
     const double* uPred;   // [B][N][2]
     const double* zt_in;   // [B][6]  (LMPC: Succ_SS lam; MPC: unused -> xPred[N])
     const double* ztu_in;  // [B][2]
@@ -769,7 +769,7 @@ struct ShiftArgs {
     int* has_pred;
 };
 __global__ void shift_state_kernel(const ShiftArgs a) {
-    const int b = a.b0 + blockIdx.x;
+    const int b = blockIdx.x;
     if (b >= a.batch) return;
     const int N = a.N;
     for (int e = threadIdx.x; e < (N + 1) * 6; e += blockDim.x) {
@@ -804,8 +804,7 @@ __global__ void shift_state_kernel(const ShiftArgs a) {
 // with the constants in memory as with them folded in at compile time (DESIGN.md, "Per-controller vehicles").
 struct SimArgs {
     int batch;
-    int b0 = 0, b1 = -1;   // instance range [b0, b1) of this launch (b1 < 0: up to batch); arrays stay globally indexed
-    const double* x;       // [B][6] curvilinear state
+    const double* x;      // [B][6] curvilinear state
     const double* xg;      // [B][6] global state (psi, X, Y at 3..5)
     const double* u;       // [B][2]  or uPred [B][N][2] with u_stride = N*2
     long long u_stride;
@@ -818,8 +817,7 @@ struct SimArgs {
     int* cl_len;           // [B]
     int Tcl;
     int* done;             // [B] 1 when s_next > TrackLength
-    const int* active;     // [B] or nullptr: instances with active == 0 are left untouched
-    const int* flags;      // [B] step flags (K1/K2/addPoint) and QP status of the step that produced u, or nullptr;
+    const int* flags;     // [B] step flags (K1/K2/addPoint) and QP status of the step that produced u, or nullptr;
     const int* status;     //     accumulated into health[b] (OR of flags) and health[B + b] (steps with status != 1)
     int* health;
     const lmpc_vehicle_params* veh;   // vehicle table (lmpc_rollout_set_vehicles)
@@ -832,9 +830,8 @@ struct SimArgs {
 namespace lmpc {
 
 __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimArgs a) {
-    const int b = a.b0 + blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= (a.b1 < 0 ? a.batch : a.b1)) return;
-    if (a.active && !a.active[b]) return;
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= a.batch) return;
     if (a.health) {
         if (a.flags && a.flags[b]) a.health[b] |= a.flags[b];
         if (a.status && a.status[b] != 1) a.health[a.batch + b] += 1;

@@ -534,45 +534,3 @@ def test_warm_started_closed_loop_matches_cold_start(gold, track):
     print("interior-point iterations per solve: cold %.2f, warm %.2f" % (mc, mw))
     assert mw < mc - 0.3, (mc, mw)
     cc.close(); cw.close()
-
-
-def test_pipelined_step_is_bit_identical_to_the_single_launch_sequence(track, monkeypatch):
-    """The device-resident step cut into instance ranges on separate streams (LMPC_B200_STEP_SPLIT; the controllers are
-    independent, PC.py:317-333) must return exactly what the single K1 -> K2 -> QP -> shift sequence returns: same kernels,
-    same per-controller arithmetic -- for the fused step and for closed-loop steps with addPoint and dynModel in the ranges."""
-    _need_gpu()
-    from racinglmpc_b200 import workloads
-    B, N = 1024, 12
-    data = workloads.lmpc_batch(B)
-    numSS_it, numSS_Points, _, _, Qts, par = rp.lmpc_params(N)
-    zs = np.random.default_rng(11).standard_normal((3, B, 3))
-
-    def run(split):
-        monkeypatch.setenv("LMPC_B200_STEP_SPLIT", str(split))
-        c = BatchedController(par, B, track.seg_table(), track.TrackLength, trToUse=5, numSS_Points=numSS_Points,
-                              numSS_it=numSS_it, QterminalSlack=Qts, Tmax=1280, ss_cap=6, model_cap=6)
-        workloads.restore_lmpc_batch(c, data)
-        l0 = c.kernel_launches
-        o = {k: v.copy() for k, v in c.step(data["x0"]).items()}
-        n_step = c.kernel_launches - l0
-        c.enable_rollout(Tcl=64)
-        c.rollout_set_state(data["x0"], data["x0"])
-        l0 = c.kernel_launches
-        for k in range(3):
-            c.rollout_step(z=zs[k])
-        c.sync()
-        n_roll = c.kernel_launches - l0
-        r = {k: np.array(v).copy() for k, v in c.step_results().items()}
-        st = {k: np.array(v).copy() for k, v in c.rollout_state().items()}
-        c.close()
-        return o, r, st, n_step, n_roll
-    o1, r1, s1, n1, m1 = run(1)
-    o4, r4, s4, n4, m4 = run(4)
-    assert (n1, m1) == (4, 3 * 6) and (n4, m4) == (4 * 4, 3 * 4 * 6), (n1, m1, n4, m4)
-    assert np.all(o1["status"] == 1) and np.all(r1["status"] == 1)
-    for k in o1:
-        assert np.array_equal(o1[k], o4[k]), k
-    for k in r1:
-        assert np.array_equal(r1[k], r4[k]), k
-    for k in s1:
-        assert np.array_equal(s1[k], s4[k]), k
