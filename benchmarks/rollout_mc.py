@@ -36,20 +36,35 @@ from racinglmpc_b200.controller import BatchedController                      # 
 
 
 def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, poll=8, max_steps=0, seed=1234, local=None, warm=False,
-        final=None, param_sets=None, vehicle_sets=None, books=None, track_sets=None):
+        final=None, param_sets=None, vehicle_sets=None, books=None, track_sets=None, pool_groups=None):
     """One Monte-Carlo run on this rank's GPU (torch.distributed may or may not be initialised).  Returns a dict (all ranks).
     final: None, or a dict that receives the closed loop's end state (rollout_state) and the last step's solver report (step_results).
     books: None, or a dict that receives the lap books (books) and the health counters (flags_or, unsolved).
     param_sets: None, or (params, index, QterminalSlack) handed to BatchedController.set_param_sets after construction (a
     parameter sweep over the batch; the result then holds per-set lap statistics under "per_set_rank0").
     vehicle_sets: None, or (vehicles, index) handed to BatchedController.set_vehicles (a sweep over the plant, PID lap included; the
-    result then holds per-vehicle lap statistics under "per_vehicle_rank0").  The pooled mode still exchanges laps between
-    controllers whatever their car, so plant sweeps run in the independent mode.
+    result then holds per-vehicle lap statistics under "per_vehicle_rank0").  The pooled mode exchanges laps between the
+    controllers of a pool group whatever their car, so a pooled plant sweep groups by car (pool_groups).
     track_sets: None, or (tracks, index) handed to BatchedController.set_tracks (several circuits in one batch; the result then
-    holds per-track lap statistics under "per_track_rank0").  A lap of another circuit is not a trajectory of this one, so more
-    than one track runs in the independent mode only (ValueError otherwise, raised before any collective)."""
+    holds per-track lap statistics under "per_track_rank0").  A lap of another circuit is not a trajectory of this one, so the
+    pooled mode with more than one track needs pool_groups in which every group drives one circuit (ValueError otherwise,
+    raised before any device work or collective).
+    pool_groups: None, or (index, G) handed to BatchedController.set_pool_groups (e.g. sharding.design_groups(track index,
+    parameter-set index)): the pooled mode then exchanges laps within each group; the exchange buffers hold G * (share + 1) laps
+    per rank and the result holds the laps filed per group under "laps_filed_per_group_rank0" (stored laps counted from the books;
+    too low for a controller with health flag 64).  The exchange waits for the slowest controller of the whole batch; a lap ships
+    only once it has `ship_after` rows past its finish line (lmpc_set_pool_min_overrun), so a group lapping faster ships the
+    fastest of its laps that qualify."""
     if track_sets is not None and mode == "pooled" and len(track_sets[0]) > 1:
-        raise ValueError("the pooled mode exchanges laps between controllers: it needs one track, got %d" % len(track_sets[0]))
+        if pool_groups is None:
+            raise ValueError("the pooled mode exchanges laps between controllers: with %d tracks it needs pool groups that each drive "
+                             "one track" % len(track_sets[0]))
+        tidx, gidx = np.asarray(track_sets[1]).reshape(-1), np.asarray(pool_groups[0]).reshape(-1)
+        if tidx.shape != gidx.shape:
+            raise ValueError("pool_groups and track_sets need one index entry per controller")
+        for g in np.unique(gidx):
+            if len(np.unique(tidx[gidx == g])) > 1:
+                raise ValueError("pool group %d spans two tracks: a lap of another circuit is not a trajectory of this one" % g)
     rank = dist.get_rank() if dist.is_initialized() else 0
     world = dist.get_world_size() if dist.is_initialized() else 1
     local = int(os.environ.get("LOCAL_RANK", 0)) if local is None else local
@@ -65,6 +80,12 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         c.set_vehicles(*vehicle_sets)
     if track_sets is not None:
         c.set_tracks(*track_sets)
+    if pool_groups is not None:
+        c.set_pool_groups(*pool_groups)
+    # every shipped lap has at least `ship_after` rows past its finish line: the readiness poll below guarantees it for the
+    # slowest controllers of the batch, the export for the others (a group lapping faster holds laps that just ended)
+    c.set_pool_min_overrun(ship_after)
+    G = c.pool_groups
     stream = torch.cuda.ExternalStream(c.stream, device=dev)
     x0 = np.tile(np.array([0.5, 0, 0, 0, 0, 0.0]), (B, 1))
     # ---- main.py:65-66 + 99-110 on the device: every controller drives its OWN PID lap (the full 100 s) and is seeded with it
@@ -78,10 +99,10 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     pid_s = time.perf_counter() - t0
     c.rollout_set_state(x0, x0)
     kbest = share + 1
-    rows = torch.zeros(kbest, tpad, 9, dtype=torch.float64, device=dev)
-    meta = torch.zeros(kbest, 4, dtype=torch.int32, device=dev)
-    rows_all = torch.zeros(world * kbest, tpad, 9, dtype=torch.float64, device=dev)
-    meta_all = torch.zeros(world * kbest, 4, dtype=torch.int32, device=dev)
+    rows = torch.zeros(G * kbest, tpad, 9, dtype=torch.float64, device=dev)
+    meta = torch.zeros(G * kbest, 4, dtype=torch.int32, device=dev)
+    rows_all = torch.zeros(world * G * kbest, tpad, 9, dtype=torch.float64, device=dev)
+    meta_all = torch.zeros(world * G * kbest, 4, dtype=torch.int32, device=dev)
     agree = torch.zeros(2, dtype=torch.int32, device=dev)
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     if world > 1:
@@ -115,9 +136,9 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
                 if world > 1:
                     dist.all_gather_into_tensor(rows_all, rows)
                     dist.all_gather_into_tensor(meta_all, meta)
-                    took_total += c.pool_import(world * kbest, share, tpad, rank * B, rows_all, meta_all, count=True)
+                    took_total += c.pool_import(world * G * kbest, share, tpad, rank * B, rows_all, meta_all, count=True)
                 else:
-                    took_total += c.pool_import(kbest, share, tpad, 0, rows, meta, count=True)
+                    took_total += c.pool_import(G * kbest, share, tpad, 0, rows, meta, count=True)
             xchg_s += time.perf_counter() - tx
             n_xchg += 1
             next_round += 1
@@ -152,6 +173,13 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     if track_sets is not None:
         idx = np.asarray(track_sets[1]).reshape(B)
         out["per_track_rank0"] = [_set_stats(bk, flags_or, unsolved, idx == k, laps) for k in range(len(track_sets[0]))]
+    if pool_groups is not None:
+        # a stored lap advances `it`: 4 seeded copies + every own lap handed over + every imported lap filed.  Exact unless an
+        # own lap found the safe-set pool full (health flag 64): then that controller's count is one too low per such lap.
+        filed = bk["it"].astype(np.int64) - 4 - bk["lap_n"]
+        gidx = np.asarray(pool_groups[0]).reshape(B)
+        out["pool_groups"] = G
+        out["laps_filed_per_group_rank0"] = [int(filed[gidx == g].sum()) for g in range(G)]
     if final is not None:
         final.update(c.rollout_state())
         final.update(c.step_results())

@@ -34,6 +34,7 @@ extern "C" {
 #define LMPC_MAX_NCX 4
 #define LMPC_MAX_NCU 8
 #define LMPC_MAX_SEG 16
+#define LMPC_MAX_POOL_GROUPS 64
 
 /* Controller parameters.  Field names/meaning follow MPCParams (PredictiveControllers.py:24-51) and the
  * extra LMPC constructor arguments (PredictiveControllers.py:293).  n = 6, d = 2 are fixed (the
@@ -95,8 +96,9 @@ int lmpc_create(const lmpc_params* p, int batch, int device, lmpc_handle** out);
  *   - The call synchronises the handle's streams before it replaces the table: batches enqueued earlier (e.g. through the _async
  *     entry points) complete with the parameters they were enqueued with.
  *   - It invalidates the warm-start records (lmpc_params.warm_start): the next solve of every controller starts cold.
- *   - The pooled safe-set exchange (lmpc_pool_*, lmpc_ss_import_laps_dev) still hands laps between all controllers whatever their
- *     set; a clean sweep (each tuning learning from its own laps only) runs in the independent mode.
+ *   - The pooled safe-set exchange (lmpc_pool_*) hands laps between the controllers of one pool group (lmpc_set_pool_groups)
+ *     whatever their set; a clean sweep (each tuning learning from its own tuning's laps only) puts each set in its own group.
+ *     lmpc_ss_import_laps_dev hands laps wherever the caller says.
  * A handle with sets installed launches a QP kernel variant that stages the instance's parameter record (1 776 B) in shared
  * memory next to its stage model (DESIGN.md, "Per-controller parameters"); handles without sets launch the uniform kernel. */
 int lmpc_set_param_sets(lmpc_handle* h, const lmpc_params* sets, int nsets, const int* set_of_instance);
@@ -207,8 +209,9 @@ typedef struct lmpc_track_params {
  *   - The call synchronises the handle's streams before it replaces the table.
  *   - The track index is independent of the parameter-set and the vehicle index (crossed designs work).  The lane half-width
  *     enters the QP through Fx/bx (lmpc_set_param_sets), not through this table.
- *   - While more than one set is installed, the pooled exchange (lmpc_pool_export_dev, lmpc_pool_import_dev,
- *     lmpc_ss_import_laps_dev) returns LMPC_E_STATE: a lap driven on another circuit is not a trajectory of this one. */
+ *   - While more than one set is installed, a lap driven on another circuit is not a trajectory of this one: the pooled exchange
+ *     (lmpc_pool_export_dev, lmpc_pool_import_dev) returns LMPC_E_STATE unless pool groups are installed and the controllers of
+ *     every group on this rank share one track index; lmpc_ss_import_laps_dev always returns LMPC_E_STATE. */
 int lmpc_set_tracks(lmpc_handle* h, const lmpc_track_params* sets, int nsets, const int* set_of_instance);
 
 /* PredictiveModel.addTrajectory (PredictiveModel.py:35-46): copy one lap into a regression slot. */
@@ -307,8 +310,9 @@ typedef struct lmpc_vehicle_params {
  *   - The call synchronises the handle's streams before it replaces the table.
  *   - The vehicle index is independent of the parameter-set index of lmpc_set_param_sets (crossed designs work).  The QP entry
  *     points, the noise model, dt and the 1 ms sub-step are unchanged.
- *   - The pooled safe-set exchange (lmpc_pool_*, lmpc_ss_import_laps_dev) still hands laps between all controllers whatever their
- *     car; a lap another car drove is not a feasible trajectory of this one, so clean plant sweeps run in the independent mode. */
+ *   - The pooled safe-set exchange (lmpc_pool_*) hands laps between the controllers of one pool group whatever their car; a lap
+ *     another car drove is not a feasible trajectory of this one, so a clean plant sweep puts each car in its own group
+ *     (lmpc_set_pool_groups). */
 int lmpc_rollout_set_vehicles(lmpc_handle* h, const lmpc_vehicle_params* sets, int nsets, const int* set_of_instance);
 int lmpc_rollout_sysid(lmpc_handle* h, double lamb, double* abc_host, int* flags_host);
 int lmpc_rollout_seed_from_record(lmpc_handle* h, int copies, int ss_slot0, int model_slot0);
@@ -356,15 +360,34 @@ int lmpc_rollout_seed_from_record_dev(lmpc_handle* h, int copies);
 /* Progress of the batch: out4 = { min laps driven, max laps driven, min steps into the current lap among the controllers at the
  * minimum, controllers with a health flag }.  Synchronises. */
 int lmpc_rollout_stats(lmpc_handle* h, int* out4);
-/* Pooled safe-set exchange with device books (SURVEY §8e).  Only the globally fastest laps are ever selected (PC.py:395), so a
- * rank ships its `kbest` fastest latest-own laps instead of all of them: rows_dev[kbest,Tpad,9] = (x | u | Qfun) incl. the rows
- * addPoint appended so far, meta_dev[kbest,4] = (rows, lap time, gid_base + controller, 0).  After the all-gather,
- * lmpc_pool_import_dev ranks the n_src <= 64 gathered laps by (lap time, global id) and every controller files the `share`
- * fastest laps it does not own before its own latest lap (addTrajectory of a lap another controller drove, into both stores).
- * took_host (may be NULL; non-NULL synchronises) receives the number of laps stored. */
+/* Pooled safe-set exchange with device books (SURVEY §8e), separately within each of G pool groups (G = 1 without groups: every
+ * controller in group 0).  Only the fastest laps of a group are ever selected (PC.py:395), so a rank ships, per group, its `kbest`
+ * fastest latest-own laps instead of all of them: rows_dev[G,kbest,Tpad,9] = (x | u | Qfun) incl. the rows addPoint appended so
+ * far, meta_dev[G,kbest,4] = (rows, lap time, gid_base + controller, group); a group without a lap on this rank ships rows with
+ * global id -1.  After the all-gather, lmpc_pool_import_dev ranks the n_src <= 64 * G gathered rows of each group g (meta[.,3] ==
+ * g; at most 64 per group; rows of a group outside [0, G) are never ranked) by (lap time, global id) and every controller files
+ * the `share` fastest laps of its own group it does not own before its own latest lap (addTrajectory of a lap another controller
+ * drove, into both stores).  took_host (may be NULL; non-NULL synchronises) receives the number of laps stored.
+ * Every rank must install the same group numbering.  With more than one track installed both calls return LMPC_E_STATE unless
+ * every group's controllers on this rank share one track (lmpc_set_tracks). */
 int lmpc_pool_export_dev(lmpc_handle* h, int kbest, int Tpad, long long gid_base, double* rows_dev, int* meta_dev);
 int lmpc_pool_import_dev(lmpc_handle* h, int n_src, int share, int Tpad, long long gid_base, const double* rows_dev, const int* meta_dev,
                          int* took_host);
+/* Pool groups of the exchange (fleet learning per design cell: per circuit, car or tuning of a sweep; no reference counterpart).
+ * Controller b exchanges laps only with the controllers of group group_of_instance[b] (host array [batch]); group numbers are
+ * global labels, the same on every rank, and a group may be empty.  ngroups == 0 (group_of_instance NULL) returns to one pool.
+ *   - Requires lmpc_store_create (else LMPC_E_STATE).  Allowed after laps are stored: it affects the exchanges that follow.
+ *   - 0 <= ngroups <= min(batch, LMPC_MAX_POOL_GROUPS), ngroups == 0 exactly when group_of_instance is NULL, every index in
+ *     [0, ngroups).  Any failed check returns LMPC_E_INVALID and leaves the handle as it was.
+ *   - The call synchronises the handle's streams before it replaces the index.
+ *   - Groups are not checked against parameter sets or vehicles: a group mixing tunings or cars shares laps between them. */
+int lmpc_set_pool_groups(lmpc_handle* h, int ngroups, const int* group_of_instance);
+/* Rows past the finish line a latest own lap must ship (min(stored rows, Tpad) - lap time; LMPC.addPoint appends them during the
+ * next lap) before lmpc_pool_export_dev ships it; 0 (every handle's default) ships any latest lap, whatever its length.  An importer's safe-set window
+ * (PC.py:492-495) near the finish line reaches into these rows: a lap shipped right after its controller crossed the line sends
+ * the importers' selection past the stored lap (K2 flag 8; the reference raises IndexError).  A group without such a lap on this
+ * rank ships rows with global id -1.  rows >= 0 (else LMPC_E_INVALID). */
+int lmpc_set_pool_min_overrun(lmpc_handle* h, int rows);
 
 /* ---- presentation support (SURVEY §8f rank 4: the inputs of the reference's plot.py for device-resident batches) --------------
  * lmpc_track_global_position: Map.getGlobalPosition (Track.py:135-189) for n points; table6[nseg,6] = Map.PointAndTangent

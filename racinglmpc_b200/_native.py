@@ -11,6 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _SO = os.environ.get("LMPC_B200_SO", os.path.join(_HERE, "liblmpc_b200.so"))   # override: kernel-variant experiments only
 
 MAX_NCX, MAX_NCU, MAX_SEG = 4, 8, 16
+MAX_POOL_GROUPS = 64
 
 
 class Params(C.Structure):
@@ -126,6 +127,8 @@ def lib():
     L.lmpc_rollout_stats.argtypes = [_vp, _vp]
     L.lmpc_pool_export_dev.argtypes = [_vp, C.c_int, C.c_int, C.c_longlong, _vp, _vp]
     L.lmpc_pool_import_dev.argtypes = [_vp, C.c_int, C.c_int, C.c_int, C.c_longlong, _vp, _vp, _vp]
+    L.lmpc_set_pool_groups.argtypes = [_vp, C.c_int, _vp]
+    L.lmpc_set_pool_min_overrun.argtypes = [_vp, C.c_int]
     L.lmpc_host_alloc.argtypes = [C.c_int, C.c_size_t, C.POINTER(_vp)]
     L.lmpc_host_free.argtypes = [_vp]
     L.lmpc_host_numa_node.argtypes = [C.c_int]
@@ -267,7 +270,8 @@ def make_params(p, numSS_Points=0, numSS_it=0, QterminalSlack=None, eps_res=0.0,
 
 
 def _set_index(index, K, batch, what):
-    """The index rules of the per-controller tables (lmpc_set_param_sets, lmpc_rollout_set_vehicles, lmpc_set_tracks): 1 <= K <= batch rows and
+    """The index rules of the per-controller tables (lmpc_set_param_sets, lmpc_rollout_set_vehicles, lmpc_set_tracks) and of the pool
+    groups (lmpc_set_pool_groups): 1 <= K <= batch rows and
     one integer row number in [0, K) per controller.  Returns the index as a contiguous int32 array; raises ValueError."""
     if index is None:
         raise ValueError("index is required: one set number per controller (%d)" % batch)
@@ -328,6 +332,21 @@ def make_vehicle_sets(vehicles, index, batch):
             raise ValueError("vehicle %d: m, Iz, lf and lr must be positive" % k)
         out[k] = VehicleParams(*vals)
     return out, idx
+
+
+def make_pool_groups(index, ngroups, batch):
+    """Pool groups for ``lmpc_set_pool_groups``: the group of every controller ``index[batch]`` among ``ngroups``.  ``ngroups == 0``
+    goes with ``index=None`` (one pool) and returns None.  Raises ValueError where the library would refuse: the index rules of
+    ``make_param_sets`` (with groups for sets; a group may be empty), more than MAX_POOL_GROUPS groups, or an index with
+    ``ngroups == 0``.  Returns the int32 index array."""
+    ngroups = int(ngroups)
+    if ngroups == 0:
+        if index is not None:
+            raise ValueError("ngroups == 0 returns to one pool and takes no index")
+        return None
+    if ngroups > MAX_POOL_GROUPS:
+        raise ValueError("at most %d pool groups, got %d" % (MAX_POOL_GROUPS, ngroups))
+    return _set_index(index, ngroups, batch, "pool groups")
 
 
 def make_track_sets(tracks, index, batch):

@@ -64,6 +64,7 @@ class BatchedController:
         self._sel_rows, self._used_rows = None, None
         nit = max(self.numSS_it, 1)
         self.device_books = False
+        self._pool_groups = 1
         self._sel = np.zeros((self.B, nit), np.int32); self._isp = np.zeros((self.B, nit), np.int32)
         self._prev = -np.ones(self.B, np.int32); self._used = np.zeros((self.B, self.trToUse), np.int32)
 
@@ -128,6 +129,32 @@ class BatchedController:
             return
         sets, idx = nat.make_track_sets(tracks, index, self.B)
         nat.check(self._lib.lmpc_set_tracks(self._h, sets, len(sets), nat.ptr(idx)))
+
+    def set_pool_groups(self, index=None, ngroups=None):
+        """Pool groups of the pooled exchange (fleet learning per design cell): controller b exchanges laps only with the
+        controllers of group ``index[b]`` in ``[0, ngroups)`` (None: ``max(index) + 1``; e.g. sharding.design_groups).  Group
+        numbers are global: every rank installs the same numbering.  ``index=None`` returns to one pool.  With several tracks
+        installed every group must drive one circuit, or the exchange is refused.  Allowed after laps are stored; waits for work
+        already enqueued."""
+        if index is None:
+            if ngroups not in (None, 0):
+                raise ValueError("index=None returns to one pool and takes no ngroups")
+            ngroups = 0
+        elif ngroups is None:
+            ngroups = int(np.max(index)) + 1
+        idx = nat.make_pool_groups(index, ngroups, self.B)
+        nat.check(self._lib.lmpc_set_pool_groups(self._h, int(ngroups), nat.ptr(idx)))
+        self._pool_groups = int(ngroups) or 1
+
+    def set_pool_min_overrun(self, rows):
+        """Ship a latest own lap in ``pool_export`` only once it has ``rows`` rows past its finish line (0, the default: any).
+        An importer's safe-set window near the finish reaches into those rows."""
+        nat.check(self._lib.lmpc_set_pool_min_overrun(self._h, int(rows)))
+
+    @property
+    def pool_groups(self):
+        """G, the number of pool groups of the exchange (1 without groups): pool_export writes G * kbest rows."""
+        return self._pool_groups
 
     # ------------------------------------------------------------------ PredictiveModel.addTrajectory
     def model_add_trajectory(self, inst, x, u):
@@ -541,11 +568,14 @@ class BatchedController:
         return tuple(int(v) for v in o)
 
     def pool_export(self, kbest, Tpad, gid_base, rows_dev, meta_dev):
-        """Send side of the pooled exchange: this rank's ``kbest`` fastest latest-own laps -> rows[kbest,Tpad,9], meta[kbest,4]."""
+        """Send side of the pooled exchange: per pool group, this rank's ``kbest`` fastest latest-own laps (with at least
+        ``set_pool_min_overrun`` rows past the finish line) -> rows[G*kbest,Tpad,9], meta[G*kbest,4] = (rows, lap time, global id
+        or -1, group), group-major; G = ``pool_groups``."""
         nat.check(self._lib.lmpc_pool_export_dev(self._h, int(kbest), int(Tpad), int(gid_base), nat.ptr(rows_dev), nat.ptr(meta_dev)))
 
     def pool_import(self, n_src, share, Tpad, gid_base, rows_dev, meta_dev, count=False):
-        """Receive side: every controller files the ``share`` globally fastest gathered laps it does not own."""
+        """Receive side: every controller files the ``share`` fastest gathered laps of its own pool group that it does not own.
+        ``n_src`` rows of rows/meta, world * G * kbest after an all-gather of ``pool_export``'s buffers (at most 64 * G)."""
         took = np.zeros(1, np.int32) if count else None
         nat.check(self._lib.lmpc_pool_import_dev(self._h, int(n_src), int(share), int(Tpad), int(gid_base), nat.ptr(rows_dev),
                                                  nat.ptr(meta_dev), nat.ptr(took)))

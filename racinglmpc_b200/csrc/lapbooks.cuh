@@ -221,23 +221,42 @@ __global__ void __launch_bounds__(256) seed_books_kernel(int batch, LapPool ss, 
 }
 
 // ---- pooled safe-set exchange (SURVEY §8e) -------------------------------------------------------------------------------
-// meta rows of an exchanged lap: (rows incl. the addPoint overrun, lap time, global controller id, -)
+// meta rows of an exchanged lap: (rows incl. the addPoint overrun, lap time, global controller id, pool group)
+// Pool groups (lmpc_set_pool_groups): controller b exchanges laps only within group grp[b] of G; grp == null puts every
+// controller in group 0 (G = 1).  Every pool array is group-major: G blocks of kbest rows on the send side, and on the receive
+// side G rankings of at most POOL_MAXSRC rows each.
 constexpr int POOL_MAXK = 8;
+constexpr int POOL_MAXSRC = 64;            // gathered candidates ranked per group
+constexpr int POOL_MAXG = 64;              // LMPC_MAX_POOL_GROUPS
+// int scratch of the exchange, sized once for POOL_MAXG groups: best instances [G][kbest], rankings [G][POOL_MAXSRC], ranked
+// rows per group [G], laps filed [1]
+constexpr int POOL_ORDER = POOL_MAXG * POOL_MAXK;
+constexpr int POOL_COUNT = POOL_ORDER + POOL_MAXG * POOL_MAXSRC;
+constexpr int POOL_TOOK = POOL_COUNT + POOL_MAXG;
+constexpr int POOL_SCRATCH = POOL_TOOK + 1;
 
-// The k fastest "latest own laps" of this rank, ascending (lap time, controller id): the only laps of this rank that can be
-// among the global k fastest.  One CTA; k rounds of block arg-min over the batch.
-__global__ void __launch_bounds__(1024) pool_local_best_kernel(int batch, LapBooks k, int kbest, int* best_inst) {
+__device__ __forceinline__ int pool_group(const int* grp, int b) { return grp ? grp[b] : 0; }
+
+// The k fastest "latest own laps" of this rank in group blockIdx.x, ascending (lap time, controller id): the only laps of this
+// rank that can be among the group's k fastest.  A latest lap takes part only once the rows it ships (at most Tpad) reach
+// `min_over` rows past its finish line (rows - lap time; addPoint appends them during the next lap): an importer's safe-set
+// window near the finish reaches into those rows.  One CTA per group; k rounds of block arg-min over the group's controllers.
+__global__ void __launch_bounds__(1024) pool_local_best_kernel(int batch, LapPool ss, LapBooks k, int kbest, int Tpad, int min_over,
+                                                               const int* grp, int* best_inst) {
     __shared__ unsigned long long red[32];
     __shared__ int taken[POOL_MAXK];
+    const int g = blockIdx.x;
     for (int r = 0; r < kbest; ++r) {
         unsigned long long mine = ~0ull;
         for (int b = threadIdx.x; b < batch; b += blockDim.x) {
             const int sl = k.prevslot[b];
-            if (sl < 0) continue;
+            if (sl < 0 || pool_group(grp, b) != g) continue;
+            const int t = k.ss_time[(size_t)b * k.ss_cap + sl];
+            if (min_over > 0 && min(ss.len[ss.lap_index(b, sl)], Tpad) - t < min_over) continue;
             bool skip = false;
             for (int j = 0; j < r; ++j) skip |= (taken[j] == b);
             if (skip) continue;
-            const unsigned long long key = ((unsigned long long)(unsigned)k.ss_time[(size_t)b * k.ss_cap + sl] << 32) | (unsigned)b;
+            const unsigned long long key = ((unsigned long long)(unsigned)t << 32) | (unsigned)b;
             mine = key < mine ? key : mine;
         }
         for (int o = 16; o > 0; o >>= 1) { const unsigned long long v = __shfl_xor_sync(0xffffffffu, mine, o); mine = v < mine ? v : mine; }
@@ -246,15 +265,16 @@ __global__ void __launch_bounds__(1024) pool_local_best_kernel(int batch, LapBoo
         if (threadIdx.x < 32) {
             mine = (threadIdx.x < (blockDim.x >> 5)) ? red[threadIdx.x] : ~0ull;
             for (int o = 16; o > 0; o >>= 1) { const unsigned long long v = __shfl_xor_sync(0xffffffffu, mine, o); mine = v < mine ? v : mine; }
-            if (threadIdx.x == 0) { taken[r] = (mine == ~0ull) ? -1 : (int)(mine & 0xffffffffu); best_inst[r] = taken[r]; }
+            if (threadIdx.x == 0) { taken[r] = (mine == ~0ull) ? -1 : (int)(mine & 0xffffffffu); best_inst[g * kbest + r] = taken[r]; }
         }
         __syncthreads();
     }
 }
 
-// Pack the latest own lap of the chosen controllers: rows[kbest][Tpad][9] = (x 6 | u 2 | Qfun 1), meta[kbest][4].
-__global__ void __launch_bounds__(256) pool_export_kernel(LapPool ss, LapBooks k, const int* best_inst, int Tpad, long long gid_base,
-                                                          double* rows, int* meta) {
+// Pack the latest own lap of the chosen controllers: rows[G][kbest][Tpad][9] = (x 6 | u 2 | Qfun 1), meta[G][kbest][4].
+// One CTA per row r = g * kbest + j.
+__global__ void __launch_bounds__(256) pool_export_kernel(LapPool ss, LapBooks k, const int* best_inst, int kbest, int Tpad,
+                                                          long long gid_base, double* rows, int* meta) {
     const int r = blockIdx.x;
     const int b = best_inst[r];
     const int sl = b < 0 ? -1 : k.prevslot[b];
@@ -273,35 +293,49 @@ __global__ void __launch_bounds__(256) pool_export_kernel(LapPool ss, LapBooks k
         meta[r * 4 + 0] = T;
         meta[r * 4 + 1] = sl < 0 ? 0x7fffffff : k.ss_time[(size_t)b * k.ss_cap + sl];
         meta[r * 4 + 2] = sl < 0 ? -1 : (int)(gid_base + b);
-        meta[r * 4 + 3] = 0;
+        meta[r * 4 + 3] = r / kbest;
     }
 }
 
-// Rank the gathered laps (n_src <= 64, a few per rank) by (lap time, global id): order[0..n_src).
-__global__ void __launch_bounds__(64) pool_rank_kernel(int n_src, const int* meta, int* order) {
-    const int i = threadIdx.x;
-    if (i >= n_src) return;
-    const int t = meta[i * 4 + 1], g = meta[i * 4 + 2], len = meta[i * 4 + 0];
-    int rank = 0;
-    for (int j = 0; j < n_src; ++j) {
-        const int tj = meta[j * 4 + 1], gj = meta[j * 4 + 2], lj = meta[j * 4 + 0];
-        const bool vj = gj >= 0 && lj >= 2, vi = g >= 0 && len >= 2;
-        if (j != i && ((vj && !vi) || (vj == vi && (key_less(tj, gj, t, g) || (tj == t && gj == g && j < i))))) ++rank;
+// Rank the gathered laps of group blockIdx.x (meta[.,3] == g; a few per rank) by (lap time, global id): order[g][0..cnt[g]).
+// Rows of another group are skipped; a row whose group lies outside [0, G) -- it came from another rank -- is ranked by no
+// block.  A group holds at most POOL_MAXSRC ranked rows: slower ones are dropped (only the `share` + 1 fastest are ever read).
+__global__ void __launch_bounds__(64) pool_rank_kernel(int n_src, const int* meta, int* order, int* cnt) {
+    const int grp = blockIdx.x;
+    __shared__ int s_n;
+    if (threadIdx.x == 0) s_n = 0;
+    __syncthreads();
+    for (int i = threadIdx.x; i < n_src; i += blockDim.x) {
+        if (meta[i * 4 + 3] != grp) continue;
+        const int t = meta[i * 4 + 1], g = meta[i * 4 + 2], len = meta[i * 4 + 0];
+        int rank = 0;
+        for (int j = 0; j < n_src; ++j) {
+            if (meta[j * 4 + 3] != grp) continue;
+            const int tj = meta[j * 4 + 1], gj = meta[j * 4 + 2], lj = meta[j * 4 + 0];
+            const bool vj = gj >= 0 && lj >= 2, vi = g >= 0 && len >= 2;
+            if (j != i && ((vj && !vi) || (vj == vi && (key_less(tj, gj, t, g) || (tj == t && gj == g && j < i))))) ++rank;
+        }
+        if (rank < POOL_MAXSRC) order[grp * POOL_MAXSRC + rank] = i;
+        atomicAdd(&s_n, 1);
     }
-    order[rank] = i;
+    __syncthreads();
+    if (threadIdx.x == 0) cnt[grp] = min(s_n, POOL_MAXSRC);
 }
 
-// Every controller takes the `share` globally fastest laps it does not own (LMPC.addTrajectory + PredictiveModel.addTrajectory
-// of a lap another controller drove, main.py:117-119), filed before its own latest lap.  One CTA per controller.
-__global__ void __launch_bounds__(256) pool_import_kernel(int batch, LapPool ss, LapPool model, LapBooks k, int n_src, int share, int Tpad,
-                                                          const double* rows, const int* meta, const int* order, long long gid_base,
-                                                          int* took, int* flags_or) {
+// Every controller takes the `share` fastest laps of its own pool group that it does not own (LMPC.addTrajectory +
+// PredictiveModel.addTrajectory of a lap another controller drove, main.py:117-119), filed before its own latest lap.  One CTA
+// per controller.
+__global__ void __launch_bounds__(256) pool_import_kernel(int batch, LapPool ss, LapPool model, LapBooks k, int share, int Tpad,
+                                                          const double* rows, const int* meta, const int* grp, const int* order,
+                                                          const int* cnt, long long gid_base, int* took, int* flags_or) {
     const int b = blockIdx.x;
     if (b >= batch) return;
     __shared__ int s_ss, s_md, s_src;
+    const int g = pool_group(grp, b);
+    const int n = cnt[g];
     int given = 0;
-    for (int o = 0; o < n_src && given < share; ++o) {
-        const int src = order[o];
+    for (int o = 0; o < n && given < share; ++o) {
+        const int src = order[g * POOL_MAXSRC + o];
         const int len = meta[src * 4 + 0], lt = meta[src * 4 + 1], gid = meta[src * 4 + 2];
         if (gid < 0 || len < 2) break;                            // nothing valid further down the ranking
         if ((long long)gid == gid_base + b) continue;             // its own lap

@@ -32,6 +32,7 @@
 #include "ftocp_launch.cuh"
 
 using namespace lmpc;
+static_assert(POOL_MAXG == LMPC_MAX_POOL_GROUPS, "the exchange scratch is sized for LMPC_MAX_POOL_GROUPS groups");
 
 #define LMPC_HOST_SLOTS 4              // buffer sets (batches in flight) of the asynchronous host entry points
 
@@ -107,6 +108,11 @@ struct lmpc_handle {
     LapBooks bk;
     int *d_bkbuf, *d_poolidx, *d_stats;
     bool has_books;
+    // pool groups of the exchange (lmpc_set_pool_groups): group index [batch] and its host mirror; null / 0 = one pool
+    int* d_pool_grp;
+    int ngroups;
+    std::vector<int> pool_grp_host;
+    int pool_min_over;         // rows a latest lap must have past its finish line to be exported (lmpc_set_pool_min_overrun)
     // rollout trace of chosen controllers (presentation support, lmpc_rollout_trace_*)
     TraceBufs tr;
     int* d_trinst;
@@ -273,6 +279,9 @@ static void free_store(lmpc_handle* h) {
     free_null(h->d_warm); free_null(h->d_warm_valid);
     free_null(h->d_trk); free_null(h->d_trk_idx);
     h->trk_host.clear(); h->trk_idx_host.clear();
+    free_null(h->d_pool_grp);
+    h->ngroups = 0;
+    h->pool_grp_host.clear();
     h->laps_stored = false;
     h->has_books = false;
     h->has_store = false;
@@ -810,7 +819,7 @@ static int store_create_impl(lmpc_handle* h, const lmpc_model_params* mp, int ss
         CK(cudaMemsetAsync(k.it, 0, sizeof(int) * B, h->stream));
         CK(cudaMemsetAsync(k.md_cnt, 0, sizeof(int) * B, h->stream));
         CK(cudaMemsetAsync(k.lap_n, 0, sizeof(int) * B, h->stream));
-        DA2(h->d_poolidx, int, 256);
+        DA2(h->d_poolidx, int, POOL_SCRATCH);
         DA2(h->d_stats, int, 8);
         h->has_books = true;
     }
@@ -838,10 +847,51 @@ static int need_store(lmpc_handle* h) {
     return LMPC_OK;
 }
 
-// The pooled exchange hands laps between controllers: only when they all drive one circuit
+// The host-chosen exchange (lmpc_ss_import_laps_dev) hands laps between any controllers: only when they all drive one circuit
 static int one_track(const lmpc_handle* h, const char* who) {
     if (h->trk_host.size() > 1)
         return fail(LMPC_E_STATE, std::string(who) + ": more than one track installed; a lap of another circuit is not a trajectory of this one");
+    return LMPC_OK;
+}
+
+// The pooled exchange hands laps only within a pool group: with several tracks installed, every group must drive one circuit
+static int one_track_per_group(const lmpc_handle* h, const char* who) {
+    if (h->trk_host.size() <= 1) return LMPC_OK;
+    if (h->ngroups == 0)
+        return fail(LMPC_E_STATE, std::string(who) + ": more than one track installed and no pool groups; a lap of another circuit is "
+                                                     "not a trajectory of this one");
+    std::vector<int> trk(h->ngroups, -1);
+    for (int b = 0; b < h->batch; ++b) {
+        int& t = trk[h->pool_grp_host[b]];
+        if (t >= 0 && t != h->trk_idx_host[b])
+            return fail(LMPC_E_STATE, std::string(who) + ": pool group " + std::to_string(h->pool_grp_host[b]) + " spans two tracks");
+        t = h->trk_idx_host[b];
+    }
+    return LMPC_OK;
+}
+
+// A latest own lap is exported only once it has `rows` rows past its finish line; 0 exports any.
+int lmpc_set_pool_min_overrun(lmpc_handle* h, int rows) {
+    if (!h) return fail(LMPC_E_INVALID, "null handle");
+    if (rows < 0) return fail(LMPC_E_INVALID, "lmpc_set_pool_min_overrun: rows must be >= 0");
+    h->pool_min_over = rows;
+    return LMPC_OK;
+}
+
+// Pool groups: controller b exchanges laps only with the controllers of group group_of_instance[b].  Nothing about the handle
+// changes unless every check passes; regrouping affects the exchanges that follow, not the laps already filed.
+int lmpc_set_pool_groups(lmpc_handle* h, int ngroups, const int* group_of_instance) {
+    static const char* who = "lmpc_set_pool_groups";
+    int rc = need_store(h);
+    if (rc) return rc;
+    if (ngroups > LMPC_MAX_POOL_GROUPS) return fail(LMPC_E_INVALID, std::string(who) + ": ngroups above LMPC_MAX_POOL_GROUPS");
+    // the index rules of the per-controller tables; there is no table, so the index stands in for its rows
+    if ((rc = check_set_index(h, who, ngroups ? group_of_instance : nullptr, ngroups, group_of_instance)) != LMPC_OK) return rc;
+    int* no_table = nullptr;
+    if ((rc = swap_table<int>(h, who, nullptr, 0, group_of_instance, &no_table, &h->d_pool_grp)) != LMPC_OK) return rc;
+    h->ngroups = ngroups;
+    if (group_of_instance) h->pool_grp_host.assign(group_of_instance, group_of_instance + h->batch);
+    else h->pool_grp_host.clear();
     return LMPC_OK;
 }
 
@@ -1689,38 +1739,43 @@ int lmpc_rollout_stats(lmpc_handle* h, int* out4) {
     return LMPC_OK;
 }
 
-// Send side of the pooled exchange: the kbest fastest latest-own laps of this rank, packed on the device.
+// Send side of the pooled exchange: per pool group, the kbest fastest latest-own laps of this rank, packed on the device.
 int lmpc_pool_export_dev(lmpc_handle* h, int kbest, int Tpad, long long gid_base, double* rows_dev, int* meta_dev) {
     int rc = need_books(h);
     if (rc) return rc;
     if (kbest < 1 || kbest > POOL_MAXK || Tpad < 1 || !rows_dev || !meta_dev) return fail(LMPC_E_INVALID, "bad export arguments");
     if (h->M <= 0) return fail(LMPC_E_STATE, "handle has no safe set");
-    if ((rc = one_track(h, "lmpc_pool_export_dev")) != LMPC_OK) return rc;
+    if ((rc = one_track_per_group(h, "lmpc_pool_export_dev")) != LMPC_OK) return rc;
     CK(cudaSetDevice(h->device));
-    pool_local_best_kernel<<<1, 1024, 0, h->stream>>>(h->batch, h->bk, kbest, h->d_poolidx);
-    pool_export_kernel<<<kbest, 256, 0, h->stream>>>(h->ss, h->bk, h->d_poolidx, Tpad, gid_base, rows_dev, meta_dev);
+    const int G = h->ngroups > 0 ? h->ngroups : 1;
+    pool_local_best_kernel<<<G, 1024, 0, h->stream>>>(h->batch, h->ss, h->bk, kbest, Tpad, h->pool_min_over, h->d_pool_grp,
+                                                       h->d_poolidx);
+    pool_export_kernel<<<G * kbest, 256, 0, h->stream>>>(h->ss, h->bk, h->d_poolidx, kbest, Tpad, gid_base, rows_dev, meta_dev);
     CK(cudaGetLastError());
     h->launches += 2;
     return LMPC_OK;
 }
 
-// Receive side: rank the gathered laps, every controller files the `share` fastest it does not own.  took_host (may be NULL)
-// receives the number of laps stored; the call then synchronises.
+// Receive side: rank the gathered laps per pool group, every controller files the `share` fastest of its group it does not own.
+// took_host (may be NULL) receives the number of laps stored; the call then synchronises.
 int lmpc_pool_import_dev(lmpc_handle* h, int n_src, int share, int Tpad, long long gid_base, const double* rows_dev, const int* meta_dev,
                          int* took_host) {
     int rc = need_books(h);
     if (rc) return rc;
-    if (n_src < 1 || n_src > 64 || share < 1 || Tpad < 1 || !rows_dev || !meta_dev) return fail(LMPC_E_INVALID, "bad import arguments");
+    const int G = h->ngroups > 0 ? h->ngroups : 1;
+    if (n_src < 1 || n_src > POOL_MAXSRC * G || share < 1 || Tpad < 1 || !rows_dev || !meta_dev)
+        return fail(LMPC_E_INVALID, "bad import arguments");
     if (h->M <= 0) return fail(LMPC_E_STATE, "handle has no safe set");
-    if ((rc = one_track(h, "lmpc_pool_import_dev")) != LMPC_OK) return rc;
+    if ((rc = one_track_per_group(h, "lmpc_pool_import_dev")) != LMPC_OK) return rc;
     CK(cudaSetDevice(h->device));
     h->laps_stored = true;
-    int* order = h->d_poolidx + 64;
-    int* took = h->d_poolidx + 200;
+    int* order = h->d_poolidx + POOL_ORDER;
+    int* cnt = h->d_poolidx + POOL_COUNT;
+    int* took = h->d_poolidx + POOL_TOOK;
     CK(cudaMemsetAsync(took, 0, sizeof(int), h->stream));
-    pool_rank_kernel<<<1, 64, 0, h->stream>>>(n_src, meta_dev, order);
-    pool_import_kernel<<<h->batch, 256, 0, h->stream>>>(h->batch, h->ss, h->mdl, h->bk, n_src, share, Tpad, rows_dev, meta_dev, order, gid_base,
-                                                        took, h->has_rollout ? h->d_health : nullptr);
+    pool_rank_kernel<<<G, 64, 0, h->stream>>>(n_src, meta_dev, order, cnt);
+    pool_import_kernel<<<h->batch, 256, 0, h->stream>>>(h->batch, h->ss, h->mdl, h->bk, share, Tpad, rows_dev, meta_dev, h->d_pool_grp, order,
+                                                        cnt, gid_base, took, h->has_rollout ? h->d_health : nullptr);
     CK(cudaGetLastError());
     h->launches += 2;
     if (took_host) {

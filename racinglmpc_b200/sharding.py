@@ -59,13 +59,28 @@ def allgather_vec(v, group=None):
     return out
 
 
-def pooled_fastest(lens_all, k, valid_min=2):
+def pooled_fastest(lens_all, k, valid_min=2, groups=None):
     """Indices (into the gathered order) of the k fastest finished laps, ties to the lower global index —
-    the stable counterpart of np.argsort(LapTime)[:k] (PC.py:395,402)."""
+    the stable counterpart of np.argsort(LapTime)[:k] (PC.py:395,402).
+    groups: None, or the pool group of every gathered lap; then a list whose entry g holds the k fastest laps of group g, for
+    g in 0 .. max(groups) (laps of a negative group are never ranked) — the host counterpart of the grouped exchange."""
     lens_np = lens_all.cpu().numpy() if torch.is_tensor(lens_all) else np.asarray(lens_all)
+    if groups is not None:
+        groups = np.asarray(groups).reshape(-1)
+        return [np.nonzero(groups == g)[0][pooled_fastest(lens_np[groups == g], k, valid_min)] for g in range(int(groups.max()) + 1)]
     idx = np.where(lens_np >= valid_min)[0]
     order = idx[np.argsort(lens_np[idx], kind="stable")]
     return order[:k]
+
+
+def design_groups(*indices):
+    """Pool groups of a crossed design: every distinct combination of the per-controller indices (e.g. track, vehicle and
+    parameter-set index) is one group, numbered 0 .. G-1 in order of first appearance.  Returns (group index int32 [batch], G)."""
+    cols = np.stack([np.asarray(i).reshape(-1) for i in indices], axis=1)
+    seen, out = {}, np.empty(cols.shape[0], np.int32)
+    for b, key in enumerate(map(tuple, cols.tolist())):
+        out[b] = seen.setdefault(key, len(seen))
+    return out, len(seen)
 
 
 def max_over_ranks(value, device, group=None):
