@@ -11,7 +11,8 @@ Leg 2, grid: the three circuits of Track.py (L-shaped, goggle, oval) x 3 frictio
 controllers (track = controller mod 3, friction = (controller // 3) mod 3), pooled per cell (sharding.design_groups: 9 groups)
 against the same batch in the independent mode: per cell, mean / minimum length of every LMPC lap, unsolved steps and
 controllers with health flags in both modes, laps filed per group, and the exchange time and bytes with 9 groups.  The exchange
-waits for the slowest controller of the whole batch, so the groups on shorter circuits ship a lap from further on.
+waits for the slowest controller of the whole batch, so the groups on shorter circuits ship a lap from further on
+(benchmarks/pool_readiness.py runs the same grid with each group exchanging on its own schedule).
 
   python benchmarks/pool_groups.py [--rounds 5 --batch 8192 --laps 3] [--out FILE]
 Prints one JSON line per leg (card name and power limit read in the same run); --out appends them to FILE as well."""
@@ -62,12 +63,18 @@ def leg_ab(rounds, batch, laps, dev):
             "exchange_ms_each": xms, "laps_filed_rank0": fl_a, "identical": list(SAME), "lap_stats_rank0": st_a}
 
 
-def leg_grid(batch, laps, dev):
+def grid_design(batch):
+    """The circuits x frictions grid of leg 2: (tracks, vehicles, track index, vehicle index, pool group per cell, G)."""
     ts = [make() for _, make in TRACKS]
     vs = [VehicleParams.from_friction(mu) for mu in FRICTION]
     b = np.arange(batch)
     t_idx, v_idx = b % len(ts), (b // len(ts)) % len(vs)
     groups, G = sharding.design_groups(t_idx, v_idx)
+    return ts, vs, t_idx, v_idx, groups, G
+
+
+def leg_grid(batch, laps, dev):
+    ts, vs, t_idx, v_idx, groups, G = grid_design(batch)
     runs = {}
     for mode in ("independent", "pooled"):
         fin = {}

@@ -14,6 +14,9 @@ a collective the others skip.
                        a rank's candidates are its own fastest few: ~60 KB per rank instead of every lap), all ranks all-gather
                        them over NCCL, rank them by (lap time, global id) and every controller files the `share` fastest laps
                        it does not own as additional stored laps (safe set + regression model).
+With pool groups (run(pool_groups=...)) the exchange runs within each group; run(readiness="group") gives every group its
+own round counter, so a group exchanges once its own slowest controller is `ship_after` steps into lap r+1 (the ranks then
+agree on one vector of ready groups per poll).
 
   python benchmarks/rollout_mc.py --batch 8192 --laps 3            (1 GPU)
   python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 benchmarks/rollout_mc.py --batch 8192
@@ -36,7 +39,7 @@ from racinglmpc_b200.controller import BatchedController                      # 
 
 
 def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, poll=8, max_steps=0, seed=1234, local=None, warm=False,
-        final=None, param_sets=None, vehicle_sets=None, books=None, track_sets=None, pool_groups=None):
+        final=None, param_sets=None, vehicle_sets=None, books=None, track_sets=None, pool_groups=None, readiness="batch"):
     """One Monte-Carlo run on this rank's GPU (torch.distributed may or may not be initialised).  Returns a dict (all ranks).
     final: None, or a dict that receives the closed loop's end state (rollout_state) and the last step's solver report (step_results).
     books: None, or a dict that receives the lap books (books) and the health counters (flags_or, unsolved).
@@ -52,9 +55,21 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     pool_groups: None, or (index, G) handed to BatchedController.set_pool_groups (e.g. sharding.design_groups(track index,
     parameter-set index)): the pooled mode then exchanges laps within each group; the exchange buffers hold G * (share + 1) laps
     per rank and the result holds the laps filed per group under "laps_filed_per_group_rank0" (stored laps counted from the books;
-    too low for a controller with health flag 64).  The exchange waits for the slowest controller of the whole batch; a lap ships
-    only once it has `ship_after` rows past its finish line (lmpc_set_pool_min_overrun), so a group lapping faster ships the
-    fastest of its laps that qualify."""
+    too low for a controller with health flag 64).  A lap ships only once it has `ship_after` rows past its finish line
+    (lmpc_set_pool_min_overrun), so a group lapping faster ships the fastest of its laps that qualify.
+    readiness: when the pooled mode exchanges round r (sharding.ready_groups at every poll, agreed over the ranks).
+      "batch"  every group together, once the slowest controller of the whole batch is `ship_after` steps into lap r + 1;
+      "group"  each pool group on its own round counter, once the slowest controller of that group is; one export / all-gather /
+               import per poll exchanges every group that is ready (lmpc_pool_export_groups_dev masks the others out), so a
+               group's controllers follow the schedule they would follow alone.  Groups with no controller on any rank never
+               exchange.  Needs the pooled mode (ValueError otherwise, before any device work).  Without groups it makes the
+               same decisions at the same steps as "batch".
+    With pool_groups or readiness="group" the result holds the readiness and the closed-loop steps at which each group
+    exchanged under "exchange_steps_per_group_rank0"."""
+    if readiness not in ("batch", "group"):
+        raise ValueError("readiness is 'batch' or 'group', got %r" % (readiness,))
+    if readiness == "group" and mode != "pooled":
+        raise ValueError("readiness='group' schedules the pooled exchange; the %s mode exchanges nothing" % mode)
     if track_sets is not None and mode == "pooled" and len(track_sets[0]) > 1:
         if pool_groups is None:
             raise ValueError("the pooled mode exchanges laps between controllers: with %d tracks it needs pool groups that each drive "
@@ -104,12 +119,19 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     rows_all = torch.zeros(world * G * kbest, tpad, 9, dtype=torch.float64, device=dev)
     meta_all = torch.zeros(world * G * kbest, 4, dtype=torch.int32, device=dev)
     agree = torch.zeros(2, dtype=torch.int32, device=dev)
+    gidx = np.zeros(B, np.int64) if pool_groups is None else np.asarray(pool_groups[0]).reshape(B)
+    if readiness == "group":
+        # a group with no controller on any rank reports the empty-group sentinel everywhere and would count as ready: never exchange it
+        live = sharding.sum_over_ranks(np.bincount(gidx, minlength=G), dev) > 0
+        next_rounds = np.ones(G, np.int64)
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     if world > 1:
         dist.barrier()
     torch.cuda.synchronize()
     max_steps = int(max_steps) or 300 * laps
     steps, next_round, n_xchg, xchg_s, took_total = 0, 1, 0, 0.0, 0
+    xsteps = [[] for _ in range(G)]                      # closed-loop steps at which each group exchanged
+    every_group = np.ones(G, bool)
     it_sum, it_n, it_max = 0.0, 0, 0                     # interior-point iterations, sampled at the polls
     l0 = c.kernel_launches
     e0.record(stream)
@@ -119,20 +141,27 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         steps += 1
         if steps % poll:
             continue
-        # ---- poll: four integers of progress; ranks agree on what happens next (same decision everywhere, no deadlock)
-        lap_min, lap_max, since, flagged = c.rollout_stats()
+        # ---- poll: four integers of progress (per group); ranks agree on what happens next (same decision everywhere, no deadlock)
+        prog = c.rollout_group_stats() if readiness == "group" else np.array([c.rollout_stats()])
         its = c.step_results()["iters"]
         it_sum += float(its.mean()); it_n += 1; it_max = max(it_max, int(its.max()))
-        ready = int(mode == "pooled" and next_round < laps and lap_min >= next_round and (lap_min > next_round or since >= ship_after))
-        done = int(lap_min >= laps)
-        if world > 1:
-            agree[0], agree[1] = ready, done
-            dist.all_reduce(agree, op=dist.ReduceOp.MIN)
-            ready, done = int(agree[0].item()), int(agree[1].item())
+        if readiness == "group":
+            ready_g, done = sharding.agree_groups(sharding.ready_groups(prog, next_rounds, laps, ship_after) & live,
+                                                  prog[:, 0].min() >= laps, dev)
+            ready = int(ready_g.any())
+            ship = None if ready_g.all() else ready_g
+        else:
+            ready = int(mode == "pooled" and sharding.ready_groups(prog, next_round, laps, ship_after)[0])
+            done = int(prog[0, 0] >= laps)
+            if world > 1:
+                agree[0], agree[1] = ready, done
+                dist.all_reduce(agree, op=dist.ReduceOp.MIN)
+                ready, done = int(agree[0].item()), int(agree[1].item())
+            ready_g, ship = every_group, None
         if ready:
             tx = time.perf_counter()
             with torch.cuda.stream(stream):
-                c.pool_export(kbest, tpad, rank * B, rows, meta)
+                c.pool_export(kbest, tpad, rank * B, rows, meta, groups=ship)
                 if world > 1:
                     dist.all_gather_into_tensor(rows_all, rows)
                     dist.all_gather_into_tensor(meta_all, meta)
@@ -142,6 +171,10 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
             xchg_s += time.perf_counter() - tx
             n_xchg += 1
             next_round += 1
+            for g in np.nonzero(ready_g)[0]:
+                xsteps[g].append(steps)
+            if readiness == "group":
+                next_rounds[ready_g] += 1
         if done:
             break
     e1.record(stream)
@@ -177,9 +210,11 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         # a stored lap advances `it`: 4 seeded copies + every own lap handed over + every imported lap filed.  Exact unless an
         # own lap found the safe-set pool full (health flag 64): then that controller's count is one too low per such lap.
         filed = bk["it"].astype(np.int64) - 4 - bk["lap_n"]
-        gidx = np.asarray(pool_groups[0]).reshape(B)
         out["pool_groups"] = G
         out["laps_filed_per_group_rank0"] = [int(filed[gidx == g].sum()) for g in range(G)]
+    if pool_groups is not None or readiness == "group":
+        out["readiness"] = readiness
+        out["exchange_steps_per_group_rank0"] = xsteps
     if final is not None:
         final.update(c.rollout_state())
         final.update(c.step_results())

@@ -360,6 +360,11 @@ int lmpc_rollout_seed_from_record_dev(lmpc_handle* h, int copies);
 /* Progress of the batch: out4 = { min laps driven, max laps driven, min steps into the current lap among the controllers at the
  * minimum, controllers with a health flag }.  Synchronises. */
 int lmpc_rollout_stats(lmpc_handle* h, int* out4);
+/* The same four numbers per pool group: out[G][4] (host), G = the handle's pool groups (1 without groups, where the row equals
+ * lmpc_rollout_stats).  Row g is taken over the controllers of group g only; a group without a controller on this handle reports
+ * { INT32_MAX, 0, INT32_MAX, 0 }, so that a MIN over ranks takes the other ranks' values.  Preconditions as for
+ * lmpc_rollout_stats.  Synchronises. */
+int lmpc_rollout_group_stats(lmpc_handle* h, int* out);
 /* Pooled safe-set exchange with device books (SURVEY §8e), separately within each of G pool groups (G = 1 without groups: every
  * controller in group 0).  Only the fastest laps of a group are ever selected (PC.py:395), so a rank ships, per group, its `kbest`
  * fastest latest-own laps instead of all of them: rows_dev[G,kbest,Tpad,9] = (x | u | Qfun) incl. the rows addPoint appended so
@@ -371,6 +376,14 @@ int lmpc_rollout_stats(lmpc_handle* h, int* out4);
  * Every rank must install the same group numbering.  With more than one track installed both calls return LMPC_E_STATE unless
  * every group's controllers on this rank share one track (lmpc_set_tracks). */
 int lmpc_pool_export_dev(lmpc_handle* h, int kbest, int Tpad, long long gid_base, double* rows_dev, int* meta_dev);
+/* lmpc_pool_export_dev for the pool groups with ship_host[g] == 1 only (host array [G], every entry 0 or 1; else, or NULL,
+ * LMPC_E_INVALID and the handle is left as it was).  A group with ship_host[g] == 0 ships its kbest rows with global id -1
+ * (meta = { 0, INT32_MAX, -1, g }), so lmpc_pool_import_dev files nothing of it and leaves the books of its controllers as they
+ * were: the groups exchange on schedules of their own.  The same checks as lmpc_pool_export_dev otherwise.  Every rank must pass
+ * the same mask: a group shipped by one rank and masked out by another exchanges laps of some ranks only.  The mask is copied
+ * before the call returns. */
+int lmpc_pool_export_groups_dev(lmpc_handle* h, int kbest, int Tpad, long long gid_base, const int* ship_host, double* rows_dev,
+                                int* meta_dev);
 int lmpc_pool_import_dev(lmpc_handle* h, int n_src, int share, int Tpad, long long gid_base, const double* rows_dev, const int* meta_dev,
                          int* took_host);
 /* Pool groups of the exchange (fleet learning per design cell: per circuit, car or tuning of a sweep; no reference counterpart).

@@ -125,7 +125,9 @@ def lib():
     L.lmpc_rollout_commit_laps_dev.argtypes = [_vp]
     L.lmpc_rollout_seed_from_record_dev.argtypes = [_vp, C.c_int]
     L.lmpc_rollout_stats.argtypes = [_vp, _vp]
+    L.lmpc_rollout_group_stats.argtypes = [_vp, _vp]
     L.lmpc_pool_export_dev.argtypes = [_vp, C.c_int, C.c_int, C.c_longlong, _vp, _vp]
+    L.lmpc_pool_export_groups_dev.argtypes = [_vp, C.c_int, C.c_int, C.c_longlong, _vp, _vp, _vp]
     L.lmpc_pool_import_dev.argtypes = [_vp, C.c_int, C.c_int, C.c_int, C.c_longlong, _vp, _vp, _vp]
     L.lmpc_set_pool_groups.argtypes = [_vp, C.c_int, _vp]
     L.lmpc_set_pool_min_overrun.argtypes = [_vp, C.c_int]

@@ -567,11 +567,29 @@ class BatchedController:
         nat.check(self._lib.lmpc_rollout_stats(self._h, nat.ptr(o)))
         return tuple(int(v) for v in o)
 
-    def pool_export(self, kbest, Tpad, gid_base, rows_dev, meta_dev):
+    def rollout_group_stats(self):
+        """``rollout_stats`` per pool group: int32 [G, 4], G = ``pool_groups``.  A group without a controller here reports
+        (INT32_MAX, 0, INT32_MAX, 0)."""
+        o = np.zeros((self._pool_groups, 4), np.int32)
+        nat.check(self._lib.lmpc_rollout_group_stats(self._h, nat.ptr(o)))
+        return o
+
+    def pool_export(self, kbest, Tpad, gid_base, rows_dev, meta_dev, groups=None):
         """Send side of the pooled exchange: per pool group, this rank's ``kbest`` fastest latest-own laps (with at least
         ``set_pool_min_overrun`` rows past the finish line) -> rows[G*kbest,Tpad,9], meta[G*kbest,4] = (rows, lap time, global id
-        or -1, group), group-major; G = ``pool_groups``."""
-        nat.check(self._lib.lmpc_pool_export_dev(self._h, int(kbest), int(Tpad), int(gid_base), nat.ptr(rows_dev), nat.ptr(meta_dev)))
+        or -1, group), group-major; G = ``pool_groups``.  ``groups``: None (every group ships), or a length-G bool / 0-1 array;
+        a group with False ships rows with global id -1, so ``pool_import`` files nothing of it.  Every rank passes the same mask."""
+        if groups is None:
+            nat.check(self._lib.lmpc_pool_export_dev(self._h, int(kbest), int(Tpad), int(gid_base), nat.ptr(rows_dev), nat.ptr(meta_dev)))
+            return
+        mask = np.asarray(groups).reshape(-1)
+        if mask.shape[0] != self._pool_groups:
+            raise ValueError("pool_export: groups needs one entry per pool group (%d), got %d" % (self._pool_groups, mask.shape[0]))
+        if not np.all((mask == 0) | (mask == 1)):
+            raise ValueError("pool_export: groups entries must be 0 or 1 (or bool)")
+        mask = np.ascontiguousarray(mask, np.int32)
+        nat.check(self._lib.lmpc_pool_export_groups_dev(self._h, int(kbest), int(Tpad), int(gid_base), nat.ptr(mask), nat.ptr(rows_dev),
+                                                        nat.ptr(meta_dev)))
 
     def pool_import(self, n_src, share, Tpad, gid_base, rows_dev, meta_dev, count=False):
         """Receive side: every controller files the ``share`` fastest gathered laps of its own pool group that it does not own.

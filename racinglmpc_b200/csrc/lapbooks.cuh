@@ -229,11 +229,12 @@ constexpr int POOL_MAXK = 8;
 constexpr int POOL_MAXSRC = 64;            // gathered candidates ranked per group
 constexpr int POOL_MAXG = 64;              // LMPC_MAX_POOL_GROUPS
 // int scratch of the exchange, sized once for POOL_MAXG groups: best instances [G][kbest], rankings [G][POOL_MAXSRC], ranked
-// rows per group [G], laps filed [1]
+// rows per group [G], laps filed [1], ship mask of a masked export [G]
 constexpr int POOL_ORDER = POOL_MAXG * POOL_MAXK;
 constexpr int POOL_COUNT = POOL_ORDER + POOL_MAXG * POOL_MAXSRC;
 constexpr int POOL_TOOK = POOL_COUNT + POOL_MAXG;
-constexpr int POOL_SCRATCH = POOL_TOOK + 1;
+constexpr int POOL_SHIP = POOL_TOOK + 1;
+constexpr int POOL_SCRATCH = POOL_SHIP + POOL_MAXG;
 
 __device__ __forceinline__ int pool_group(const int* grp, int b) { return grp ? grp[b] : 0; }
 
@@ -241,11 +242,17 @@ __device__ __forceinline__ int pool_group(const int* grp, int b) { return grp ? 
 // rank that can be among the group's k fastest.  A latest lap takes part only once the rows it ships (at most Tpad) reach
 // `min_over` rows past its finish line (rows - lap time; addPoint appends them during the next lap): an importer's safe-set
 // window near the finish reaches into those rows.  One CTA per group; k rounds of block arg-min over the group's controllers.
+// ship (null: every group) masks groups out of this export: a group with ship[g] == 0 chooses no controller, so
+// pool_export_kernel ships its kbest rows with global id -1 and importers file nothing of it.
 __global__ void __launch_bounds__(1024) pool_local_best_kernel(int batch, LapPool ss, LapBooks k, int kbest, int Tpad, int min_over,
-                                                               const int* grp, int* best_inst) {
+                                                               const int* grp, const int* ship, int* best_inst) {
     __shared__ unsigned long long red[32];
     __shared__ int taken[POOL_MAXK];
     const int g = blockIdx.x;
+    if (ship && !ship[g]) {                                       // uniform over the CTA: no barrier is skipped by part of it
+        if (threadIdx.x < kbest) best_inst[g * kbest + threadIdx.x] = -1;
+        return;
+    }
     for (int r = 0; r < kbest; ++r) {
         unsigned long long mine = ~0ull;
         for (int b = threadIdx.x; b < batch; b += blockDim.x) {
@@ -378,22 +385,44 @@ __global__ void __launch_bounds__(256) pool_import_kernel(int batch, LapPool ss,
     if (threadIdx.x == 0 && given > 0) book_refresh(k, b);
 }
 
-// Progress of a Monte-Carlo batch in four numbers, so that the host only polls a few bytes every few steps:
-// out[0] = min over controllers of laps driven, out[1] = max, out[2] = min closed-loop steps into the current lap over the
-// controllers that are at lap out[0], out[3] = controllers with a non-zero health flag.
-__global__ void __launch_bounds__(1024) rollout_stats_kernel(int batch, LapBooks k, const int* cl_len, const int* health, int* out) {
-    __shared__ int s_min, s_max, s_since, s_flag;
-    if (threadIdx.x == 0) { s_min = 0x7fffffff; s_max = 0; s_since = 0x7fffffff; s_flag = 0; }
+// Progress of a Monte-Carlo batch in four numbers per pool group, so that the host only polls a few bytes every few steps:
+// out[g][0] = min over the controllers of group g of laps driven, out[g][1] = max, out[g][2] = min closed-loop steps into the
+// current lap over the group's controllers that are at lap out[g][0], out[g][3] = the group's controllers with a non-zero health
+// flag.  grp == null puts every controller in group 0 (G = 1): the batch's four numbers.  A group without a controller reports
+// (INT32_MAX, 0, INT32_MAX, 0), which a MIN over ranks leaves to the ranks that have some.  Each thread accumulates in registers
+// while consecutive controllers of its stride stay in one group and folds into shared memory when the group changes (once per
+// thread without groups).
+__global__ void __launch_bounds__(1024) rollout_stats_kernel(int batch, LapBooks k, const int* cl_len, const int* health,
+                                                             const int* grp, int G, int* out) {
+    __shared__ int s_min[POOL_MAXG], s_max[POOL_MAXG], s_since[POOL_MAXG], s_flag[POOL_MAXG];
+    for (int g = threadIdx.x; g < G; g += blockDim.x) { s_min[g] = 0x7fffffff; s_max[g] = 0; s_since[g] = 0x7fffffff; s_flag[g] = 0; }
     __syncthreads();
-    int mn = 0x7fffffff, mx = 0, fl = 0;
-    for (int b = threadIdx.x; b < batch; b += blockDim.x) { const int n = k.lap_n[b]; mn = min(mn, n); mx = max(mx, n); fl += (health && health[b]) ? 1 : 0; }
-    atomicMin(&s_min, mn); atomicMax(&s_max, mx); atomicAdd(&s_flag, fl);
+    int cur = -1, mn = 0x7fffffff, mx = 0, fl = 0;
+    for (int b = threadIdx.x; b < batch; b += blockDim.x) {
+        const int g = pool_group(grp, b);
+        if (g != cur) {
+            if (cur >= 0) { atomicMin(&s_min[cur], mn); atomicMax(&s_max[cur], mx); atomicAdd(&s_flag[cur], fl); }
+            cur = g; mn = 0x7fffffff; mx = 0; fl = 0;
+        }
+        const int n = k.lap_n[b]; mn = min(mn, n); mx = max(mx, n); fl += (health && health[b]) ? 1 : 0;
+    }
+    if (cur >= 0) { atomicMin(&s_min[cur], mn); atomicMax(&s_max[cur], mx); atomicAdd(&s_flag[cur], fl); }
     __syncthreads();
     int since = 0x7fffffff;
-    for (int b = threadIdx.x; b < batch; b += blockDim.x) if (k.lap_n[b] == s_min) since = min(since, cl_len[b]);
-    atomicMin(&s_since, since);
+    cur = -1;
+    for (int b = threadIdx.x; b < batch; b += blockDim.x) {
+        const int g = pool_group(grp, b);
+        if (g != cur) {
+            if (cur >= 0) atomicMin(&s_since[cur], since);
+            cur = g; since = 0x7fffffff;
+        }
+        if (k.lap_n[b] == s_min[g]) since = min(since, cl_len[b]);
+    }
+    if (cur >= 0) atomicMin(&s_since[cur], since);
     __syncthreads();
-    if (threadIdx.x == 0) { out[0] = s_min; out[1] = s_max; out[2] = s_since; out[3] = s_flag; }
+    for (int g = threadIdx.x; g < G; g += blockDim.x) {
+        out[g * 4 + 0] = s_min[g]; out[g * 4 + 1] = s_max[g]; out[g * 4 + 2] = s_since[g]; out[g * 4 + 3] = s_flag[g];
+    }
 }
 
 // ---- presentation support (SURVEY §8f rank 4: what plot.py reads) ----------------------------------------------------------

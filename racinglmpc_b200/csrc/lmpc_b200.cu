@@ -820,7 +820,7 @@ static int store_create_impl(lmpc_handle* h, const lmpc_model_params* mp, int ss
         CK(cudaMemsetAsync(k.md_cnt, 0, sizeof(int) * B, h->stream));
         CK(cudaMemsetAsync(k.lap_n, 0, sizeof(int) * B, h->stream));
         DA2(h->d_poolidx, int, POOL_SCRATCH);
-        DA2(h->d_stats, int, 8);
+        DA2(h->d_stats, int, POOL_MAXG * 4);          // rollout_stats_kernel: [G][4]
         h->has_books = true;
     }
     CK(cudaMemsetAsync(h->ss.len, 0, sizeof(int) * B * h->ss.cap, h->stream));
@@ -1731,7 +1731,7 @@ int lmpc_rollout_stats(lmpc_handle* h, int* out4) {
     if ((rc = need_books(h)) != LMPC_OK) return rc;
     if (!out4) return fail(LMPC_E_INVALID, "null output");
     CK(cudaSetDevice(h->device));
-    rollout_stats_kernel<<<1, 1024, 0, h->stream>>>(h->batch, h->bk, h->d_cllen, h->d_health, h->d_stats);
+    rollout_stats_kernel<<<1, 1024, 0, h->stream>>>(h->batch, h->bk, h->d_cllen, h->d_health, nullptr, 1, h->d_stats);
     CK(cudaGetLastError());
     h->launches += 1;
     CK(cudaMemcpyAsync(out4, h->d_stats, sizeof(int) * 4, cudaMemcpyDeviceToHost, h->stream));
@@ -1739,21 +1739,62 @@ int lmpc_rollout_stats(lmpc_handle* h, int* out4) {
     return LMPC_OK;
 }
 
+int lmpc_rollout_group_stats(lmpc_handle* h, int* out) {
+    int rc = need_rollout(h);
+    if (rc) return rc;
+    if ((rc = need_books(h)) != LMPC_OK) return rc;
+    if (!out) return fail(LMPC_E_INVALID, "null output");
+    CK(cudaSetDevice(h->device));
+    const int G = h->ngroups > 0 ? h->ngroups : 1;
+    rollout_stats_kernel<<<1, 1024, 0, h->stream>>>(h->batch, h->bk, h->d_cllen, h->d_health, h->d_pool_grp, G, h->d_stats);
+    CK(cudaGetLastError());
+    h->launches += 1;
+    CK(cudaMemcpyAsync(out, h->d_stats, sizeof(int) * 4 * G, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return LMPC_OK;
+}
+
 // Send side of the pooled exchange: per pool group, the kbest fastest latest-own laps of this rank, packed on the device.
-int lmpc_pool_export_dev(lmpc_handle* h, int kbest, int Tpad, long long gid_base, double* rows_dev, int* meta_dev) {
+// ship_host (null: every group) is a checked 0/1 mask [G]; a masked-out group ships rows with global id -1.
+static int pool_export(lmpc_handle* h, const char* who, int kbest, int Tpad, long long gid_base, const int* ship_host, double* rows_dev,
+                       int* meta_dev) {
     int rc = need_books(h);
     if (rc) return rc;
     if (kbest < 1 || kbest > POOL_MAXK || Tpad < 1 || !rows_dev || !meta_dev) return fail(LMPC_E_INVALID, "bad export arguments");
     if (h->M <= 0) return fail(LMPC_E_STATE, "handle has no safe set");
-    if ((rc = one_track_per_group(h, "lmpc_pool_export_dev")) != LMPC_OK) return rc;
+    if ((rc = one_track_per_group(h, who)) != LMPC_OK) return rc;
     CK(cudaSetDevice(h->device));
     const int G = h->ngroups > 0 ? h->ngroups : 1;
-    pool_local_best_kernel<<<G, 1024, 0, h->stream>>>(h->batch, h->ss, h->bk, kbest, Tpad, h->pool_min_over, h->d_pool_grp,
+    int* ship = nullptr;
+    if (ship_host) {     // staged from pageable stack memory, so the caller's array may change once the call returns
+        int mask[POOL_MAXG];
+        for (int g = 0; g < G; ++g) mask[g] = ship_host[g];
+        ship = h->d_poolidx + POOL_SHIP;
+        CK(cudaMemcpyAsync(ship, mask, sizeof(int) * G, cudaMemcpyHostToDevice, h->stream));
+    }
+    pool_local_best_kernel<<<G, 1024, 0, h->stream>>>(h->batch, h->ss, h->bk, kbest, Tpad, h->pool_min_over, h->d_pool_grp, ship,
                                                        h->d_poolidx);
     pool_export_kernel<<<G * kbest, 256, 0, h->stream>>>(h->ss, h->bk, h->d_poolidx, kbest, Tpad, gid_base, rows_dev, meta_dev);
     CK(cudaGetLastError());
     h->launches += 2;
     return LMPC_OK;
+}
+
+int lmpc_pool_export_dev(lmpc_handle* h, int kbest, int Tpad, long long gid_base, double* rows_dev, int* meta_dev) {
+    return pool_export(h, "lmpc_pool_export_dev", kbest, Tpad, gid_base, nullptr, rows_dev, meta_dev);
+}
+
+int lmpc_pool_export_groups_dev(lmpc_handle* h, int kbest, int Tpad, long long gid_base, const int* ship_host, double* rows_dev,
+                                int* meta_dev) {
+    static const char* who = "lmpc_pool_export_groups_dev";
+    int rc = need_books(h);
+    if (rc) return rc;
+    if (!ship_host) return fail(LMPC_E_INVALID, std::string(who) + ": null ship mask");
+    const int G = h->ngroups > 0 ? h->ngroups : 1;
+    for (int g = 0; g < G; ++g)
+        if (ship_host[g] != 0 && ship_host[g] != 1)
+            return fail(LMPC_E_INVALID, std::string(who) + ": ship mask entry " + std::to_string(g) + " is neither 0 nor 1");
+    return pool_export(h, who, kbest, Tpad, gid_base, ship_host, rows_dev, meta_dev);
 }
 
 // Receive side: rank the gathered laps per pool group, every controller files the `share` fastest of its group it does not own.

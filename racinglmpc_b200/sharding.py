@@ -83,6 +83,41 @@ def design_groups(*indices):
     return out, len(seen)
 
 
+def ready_groups(stats, next_round, laps, ship_after):
+    """The readiness rule of the pooled exchange, per row of ``stats`` [G, 4] (rollout_group_stats, or the one row of
+    rollout_stats for the whole batch): row g is ready for round next_round[g] (a scalar applies to every row) once the round
+    exists (r < laps), every controller of the row has driven r laps, and either every one has driven more than r laps or the
+    slowest are ``ship_after`` steps into lap r + 1.  Returns bool [G].
+    Applied per rank and combined with AND (agree_groups), it equals the rule on the union of the ranks' controllers: the union's
+    minimum is the smallest rank minimum, and its steps-into-lap is the smallest among the ranks at that minimum.  A row without
+    controllers (INT32_MAX, 0, INT32_MAX, 0) is ready for every round below ``laps`` and so leaves the decision to the others."""
+    s = np.asarray(stats).reshape(-1, 4)
+    r = np.asarray(next_round)
+    lap_min, since = s[:, 0], s[:, 2]
+    return (r < laps) & (lap_min >= r) & ((lap_min > r) | (since >= ship_after))
+
+
+def agree_groups(ready, done, device, group=None):
+    """One MIN all-reduce of [ready_0 .. ready_{G-1}, done] (int32): a group exchanges only if it is ready on every rank, and the
+    batch stops only once every rank is done.  Returns (ready bool [G], done bool), the same on every rank."""
+    v = np.append(np.asarray(ready, bool).reshape(-1), bool(done)).astype(np.int32)
+    if dist.is_initialized() and dist.get_world_size(group) > 1:
+        t = torch.from_numpy(v).to(device)
+        dist.all_reduce(t, op=dist.ReduceOp.MIN, group=group)
+        v = t.cpu().numpy()
+    return v[:-1] != 0, bool(v[-1])
+
+
+def sum_over_ranks(values, device, group=None):
+    """Element-wise sum of an integer vector over the ranks (int64 numpy array)."""
+    v = np.asarray(values, np.int64).reshape(-1)
+    if dist.is_initialized() and dist.get_world_size(group) > 1:
+        t = torch.from_numpy(v.copy()).to(device)
+        dist.all_reduce(t, op=dist.ReduceOp.SUM, group=group)
+        v = t.cpu().numpy()
+    return v
+
+
 def max_over_ranks(value, device, group=None):
     t = torch.tensor([float(value)], dtype=torch.float64, device=device)
     if dist.is_initialized() and dist.get_world_size(group) > 1:
