@@ -37,9 +37,20 @@ if ROOT not in sys.path:
 from racinglmpc_b200 import workloads, sharding, reference_params as rp      # noqa: E402
 from racinglmpc_b200.controller import BatchedController                      # noqa: E402
 
+# the controllers of every run: horizon, regression laps and the sizes of the lap stores and the closed-loop record
+N_HORIZON, TR_TO_USE, TMAX, SS_CAP, MODEL_CAP, TCL = 12, 4, 1280, 7, 5, 1024
+
+
+def layout(warm=False):
+    """The snapshot layout (BatchedController.snapshot_layout without "bytes") of run()'s controllers."""
+    numSS_it, numSS_Points = rp.lmpc_params(N_HORIZON)[:2]
+    return dict(N=N_HORIZON, M=numSS_Points, ncx=2, ncu=4, numSS_it=numSS_it, trToUse=TR_TO_USE, ss_cap=SS_CAP, model_cap=MODEL_CAP,
+                Tmax=TMAX, Tcl=TCL, warm_start=int(bool(warm)))
+
 
 def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, poll=8, max_steps=0, seed=1234, local=None, warm=False,
-        final=None, param_sets=None, vehicle_sets=None, books=None, track_sets=None, pool_groups=None, readiness="batch"):
+        final=None, param_sets=None, vehicle_sets=None, books=None, track_sets=None, pool_groups=None, readiness="batch",
+        capture=None, start=None):
     """One Monte-Carlo run on this rank's GPU (torch.distributed may or may not be initialised).  Returns a dict (all ranks).
     final: None, or a dict that receives the closed loop's end state (rollout_state) and the last step's solver report (step_results).
     books: None, or a dict that receives the lap books (books) and the health counters (flags_or, unsolved).
@@ -65,7 +76,25 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
                exchange.  Needs the pooled mode (ValueError otherwise, before any device work).  Without groups it makes the
                same decisions at the same steps as "batch".
     With pool_groups or readiness="group" the result holds the readiness and the closed-loop steps at which each group
-    exchanged under "exchange_steps_per_group_rank0"."""
+    exchanged under "exchange_steps_per_group_rank0".
+    capture: None, or a dict that receives, at the end of the run, everything a later run needs to go on from here: "records"
+    (every controller's snapshot record, a uint8 CUDA tensor), "clock" (the simulator step that keys the Philox noise), the loop's
+    scheduler state ("steps", "next_round", "next_rounds", the groups that exchanged at the last poll, the exchange steps so far)
+    and what it has to match (batch, laps, mode, readiness, poll, warm, pool groups, record layout).  torch.save stores it.
+    "diverged_step" is None unless, under group readiness, some group was ready for a round >= laps before the last poll: a
+    longer run exchanged there and this one did not, so a resumed run cannot equal it (the result of that resumed run says so
+    under "resume_exact").
+    start: None, or a capture dict: instead of the PID lap and the seeding, every controller is restored from its record, the
+    clock and the scheduler state are set, and the run first repeats the poll the capture was taken at, under the new `laps`
+    (groups that exchanged at that poll are not exchanged again), then steps on.  A run to 3 laps captured and resumed to 5
+    therefore equals a run to 5 laps bit for bit (books, end states, health, exchange steps).  Tables (param_sets, vehicle_sets,
+    track_sets, pool_groups) are installed from the arguments, as for a fresh run.  ValueError before any device work when start
+    does not match the batch, the layout, the mode, the readiness, the poll interval or the pool groups, or when laps is not
+    above the captured laps."""
+    if start is not None:
+        _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups)
+    if capture is not None and not isinstance(capture, dict):
+        raise ValueError("capture is a dict that receives the run's end state")
     if readiness not in ("batch", "group"):
         raise ValueError("readiness is 'batch' or 'group', got %r" % (readiness,))
     if readiness == "group" and mode != "pooled":
@@ -85,10 +114,11 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     local = int(os.environ.get("LOCAL_RANK", 0)) if local is None else local
     dev = torch.device("cuda", local)
     torch.cuda.set_device(dev)
-    B, N = int(batch), 12
+    B, N = int(batch), N_HORIZON
     numSS_it, numSS_Points, _, _, Qts, par = rp.lmpc_params(N)
-    c = BatchedController(par, B, workloads.track_seg_table(), rp.TRACK_LENGTH, trToUse=4, numSS_Points=numSS_Points,
-                          numSS_it=numSS_it, QterminalSlack=Qts, device=local, Tmax=1280, ss_cap=7, model_cap=5, warm_start=warm)
+    c = BatchedController(par, B, workloads.track_seg_table(), rp.TRACK_LENGTH, trToUse=TR_TO_USE, numSS_Points=numSS_Points,
+                          numSS_it=numSS_it, QterminalSlack=Qts, device=local, Tmax=TMAX, ss_cap=SS_CAP, model_cap=MODEL_CAP,
+                          warm_start=warm)
     if param_sets is not None:
         c.set_param_sets(*param_sets)
     if vehicle_sets is not None:
@@ -105,14 +135,21 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     x0 = np.tile(np.array([0.5, 0, 0, 0, 0, 0.0]), (B, 1))
     # ---- main.py:65-66 + 99-110 on the device: every controller drives its OWN PID lap (the full 100 s) and is seeded with it
     t0 = time.perf_counter()
-    c.enable_rollout(Tcl=1024)
-    c.rollout_set_state(x0, x0)
-    for _ in range(1000):
-        c.rollout_pid_step(0.8, seed=4321 + rank)
-    c.rollout_seed_from_record_dev(copies=4)
-    c.sync()
-    pid_s = time.perf_counter() - t0
-    c.rollout_set_state(x0, x0)
+    c.enable_rollout(Tcl=TCL)
+    if start is None:
+        c.rollout_set_state(x0, x0)
+        for _ in range(1000):
+            c.rollout_pid_step(0.8, seed=4321 + rank)
+        c.rollout_seed_from_record_dev(copies=4)
+        c.sync()
+        pid_s = time.perf_counter() - t0
+        c.rollout_set_state(x0, x0)
+    else:                                                # the controllers and the clock of the captured run
+        c.restore(start["records"])
+        c.rollout_clock = int(start["clock"])
+        c.sync()
+        pid_s = 0.0
+        restore_s = time.perf_counter() - t0
     kbest = share + 1
     rows = torch.zeros(G * kbest, tpad, 9, dtype=torch.float64, device=dev)
     meta = torch.zeros(G * kbest, 4, dtype=torch.int32, device=dev)
@@ -131,33 +168,51 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     max_steps = int(max_steps) or 300 * laps
     steps, next_round, n_xchg, xchg_s, took_total = 0, 1, 0, 0.0, 0
     xsteps = [[] for _ in range(G)]                      # closed-loop steps at which each group exchanged
+    repeat, skip, diverged = False, np.zeros(G, bool), None
+    last_poll, last_ready = -1, None                    # the last poll, and the groups it exchanged (None: none)
+    if start is not None:
+        steps, next_round = int(start["steps"]), int(start["next_round"])
+        if readiness == "group":
+            next_rounds = np.asarray(start["next_rounds"], np.int64).copy()
+        xsteps = [list(v) for v in start["exchange_steps"]]
+        repeat = steps % poll == 0                      # the capture was taken at a poll: decide it again under the new laps
+        skip = np.asarray(start["exchanged"], bool).reshape(G)
+    steps0 = steps
     every_group = np.ones(G, bool)
     it_sum, it_n, it_max = 0.0, 0, 0                     # interior-point iterations, sampled at the polls
     l0 = c.kernel_launches
     e0.record(stream)
-    while steps < max_steps:
-        c.rollout_step(seed=seed + rank)
-        c.rollout_commit_laps_dev()                       # every controller whose lap just ended hands it over, on the device
-        steps += 1
-        if steps % poll:
-            continue
+    while steps < max_steps or repeat:
+        if not repeat:
+            c.rollout_step(seed=seed + rank)
+            c.rollout_commit_laps_dev()                   # every controller whose lap just ended hands it over, on the device
+            steps += 1
+            if steps % poll:
+                continue
         # ---- poll: four integers of progress (per group); ranks agree on what happens next (same decision everywhere, no deadlock)
         prog = c.rollout_group_stats() if readiness == "group" else np.array([c.rollout_stats()])
-        its = c.step_results()["iters"]
-        it_sum += float(its.mean()); it_n += 1; it_max = max(it_max, int(its.max()))
+        if not repeat:                                    # the repeated poll of a resumed run has no step of its own
+            its = c.step_results()["iters"]
+            it_sum += float(its.mean()); it_n += 1; it_max = max(it_max, int(its.max()))
         if readiness == "group":
-            ready_g, done = sharding.agree_groups(sharding.ready_groups(prog, next_rounds, laps, ship_after) & live,
+            ready_g, done = sharding.agree_groups(sharding.ready_groups(prog, next_rounds, laps, ship_after) & live & ~skip,
                                                   prog[:, 0].min() >= laps, dev)
+            if capture is not None and diverged is None and not done and \
+                    (sharding.ready_groups(prog, next_rounds, np.iinfo(np.int32).max, ship_after) & live & ~ready_g).any():
+                diverged = steps                          # a longer run exchanges a round >= laps here
             ready = int(ready_g.any())
             ship = None if ready_g.all() else ready_g
         else:
-            ready = int(mode == "pooled" and sharding.ready_groups(prog, next_round, laps, ship_after)[0])
+            ready = int(mode == "pooled" and sharding.ready_groups(prog, next_round, laps, ship_after)[0] and not skip[0])
             done = int(prog[0, 0] >= laps)
             if world > 1:
                 agree[0], agree[1] = ready, done
                 dist.all_reduce(agree, op=dist.ReduceOp.MIN)
                 ready, done = int(agree[0].item()), int(agree[1].item())
             ready_g, ship = every_group, None
+        if repeat:
+            repeat, skip = False, np.zeros(G, bool)
+        last_poll, last_ready = steps, (ready_g if ready else None)
         if ready:
             tx = time.perf_counter()
             with torch.cuda.stream(stream):
@@ -182,6 +237,15 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     torch.cuda.synchronize()
     ms = sharding.max_over_ranks(e0.elapsed_time(e1), dev)
     bk = c.books()
+    if capture is not None:
+        tc = time.perf_counter()
+        capture.update(records=c.snapshot(), clock=c.rollout_clock)
+        c.sync()
+        capture.update(capture_s=time.perf_counter() - tc, steps=steps, next_round=next_round,
+                       next_rounds=next_rounds.tolist() if readiness == "group" else None,
+                       exchanged=(last_ready if last_poll == steps and last_ready is not None else np.zeros(G, bool)).tolist(), exchange_steps=xsteps,
+                       diverged_step=diverged, batch=B, laps=laps, mode=mode, readiness=readiness, poll=poll, warm=bool(warm),
+                       pool_groups=G, layout=c.snapshot_layout())
     flags_or, unsolved = c.rollout_health()
     stats = []
     for r in range(laps):
@@ -189,7 +253,7 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         a = a if a.size else np.array([0])
         stats.append({"lap": r + 1, "n": int((bk["lap_n"] > r).sum()), "mean": float(a.mean()), "min": int(a.min()), "max": int(a.max())})
     out = {"benchmark": "configs[3] LMPC Monte-Carlo rollouts", "mode": mode, "n_gpus": world, "batch_per_gpu": B,
-           "closed_loop_steps": steps, "ms_total": ms, "controller_steps_per_s": B * world * steps / (ms * 1e-3),
+           "closed_loop_steps": steps, "ms_total": ms, "controller_steps_per_s": B * world * (steps - steps0) / (ms * 1e-3),
            "kernel_launches_rank0": int(c.kernel_launches - l0), "lap_stats_rank0": stats, "device_pid_laps_s": pid_s,
            "exchanges": n_xchg, "exchange_s_total": xchg_s, "exchange_ms_each": 1e3 * xchg_s / max(n_xchg, 1),
            "allgather_bytes_per_rank": int(rows.numel() * 8 + meta.numel() * 4), "laps_filed_rank0": took_total,
@@ -215,6 +279,12 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     if pool_groups is not None or readiness == "group":
         out["readiness"] = readiness
         out["exchange_steps_per_group_rank0"] = xsteps
+    if start is not None:
+        out["resumed_from_step"] = int(start["steps"])
+        out["restore_s"] = restore_s
+        out["resume_exact"] = start["diverged_step"] is None
+    if capture is not None:
+        out["capture_s"] = capture["capture_s"]
     if final is not None:
         final.update(c.rollout_state())
         final.update(c.step_results())
@@ -222,6 +292,32 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         books.update(bk, flags_or=flags_or, unsolved=unsolved)
     c.close()
     return out
+
+
+def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups):
+    """The refusals of run(start=...), before any device work: a start that does not match this run, or laps not above the
+    captured laps."""
+    if not isinstance(start, dict):
+        raise ValueError("start is a capture dict of an earlier run")
+    need = ("records", "clock", "steps", "next_round", "next_rounds", "exchanged", "exchange_steps", "diverged_step", "batch", "laps",
+            "mode", "readiness", "poll", "warm", "pool_groups", "layout")
+    missing = [k for k in need if k not in start]
+    if missing:
+        raise ValueError("start lacks %s: pass the dict run(capture=...) filled" % ", ".join(missing))
+    for key, mine in (("batch", int(batch)), ("mode", mode), ("readiness", readiness), ("poll", int(poll)), ("warm", bool(warm))):
+        if start[key] != mine:
+            raise ValueError("start was captured with %s = %r, this run has %r" % (key, start[key], mine))
+    G = 1 if pool_groups is None else int(pool_groups[1])
+    if int(start["pool_groups"]) != G:
+        raise ValueError("start was captured with %d pool groups, this run has %d" % (int(start["pool_groups"]), G))
+    if int(laps) <= int(start["laps"]):
+        raise ValueError("laps (%d) must be above the captured run's laps (%d)" % (int(laps), int(start["laps"])))
+    rec = start["records"]
+    if getattr(rec, "shape", (None,))[0] != int(batch):
+        raise ValueError("start holds %s records, this run has %d controllers" % (getattr(rec, "shape", ("no",))[0], int(batch)))
+    for k, v in layout(warm).items():
+        if int(start["layout"].get(k, -1)) != v:
+            raise ValueError("start records have %s = %s, this run's controllers %d" % (k, start["layout"].get(k), v))
 
 
 def _set_stats(bk, flags_or, unsolved, sel, laps):

@@ -402,6 +402,48 @@ int lmpc_set_pool_groups(lmpc_handle* h, int ngroups, const int* group_of_instan
  * rank ships rows with global id -1.  rows >= 0 (else LMPC_E_INVALID). */
 int lmpc_set_pool_min_overrun(lmpc_handle* h, int rows);
 
+/* ---- controller snapshots (no reference counterpart beyond pickling an LMPC object; racinglmpc_b200/csrc/snapshot.cuh) --------
+ * What a controller of the device-resident step has learned and where it is, as one fixed-size byte record per controller:
+ * both lap pools, the lap books, the controller state, the warm-start record, and with a rollout the simulator state, the
+ * closed-loop record, the health counters and the LTI model (DESIGN.md, "Controller snapshots", lists every per-controller buffer
+ * as carried or scratch).  Not in a record: what the handle is told to drive -- parameter sets, vehicles, tracks, pool groups --
+ * and handle-wide counters.  The lap books travel in the record, so a caller that keeps its own host copy of them (the
+ * host-driven bookkeeping of lmpc_ss_set_selection / lmpc_model_set_used) must not restore into its handle.
+ * Record = header (below) + sections at 16-byte aligned offsets; every section is one controller's slice of one [B][...] buffer. */
+#define LMPC_SNAPSHOT_MAGIC 0x50414e53      /* "SNAP" */
+#define LMPC_SNAPSHOT_VERSION 1
+#define LMPC_SNAPSHOT_SECTIONS 40           /* section slots of the header, fixed order (DESIGN.md); bytes 0 = absent */
+typedef struct lmpc_snapshot_header {
+    int magic, version;
+    int bytes;                              /* record size, header included, a multiple of 16 */
+    int N, M, ncx, ncu, numSS_it, trToUse, ss_cap, model_cap, Tmax;
+    int Tcl;                                /* closed-loop record rows, 0 = the handle has no rollout */
+    int warm_start;
+    int warm_mode;                          /* problem type the warm-start record belongs to: -1 none, 0 LTV-MPC, 1 LMPC */
+    int nsect;                              /* LMPC_SNAPSHOT_SECTIONS */
+    int sect_off[LMPC_SNAPSHOT_SECTIONS];   /* byte offset of every section in the record */
+    int sect_bytes[LMPC_SNAPSHOT_SECTIONS]; /* its bytes (0 = absent in this layout) */
+    lmpc_track_params track;                /* the controller's own track row: a stored lap is in its circuit's s-coordinate */
+} lmpc_snapshot_header;
+int lmpc_sizeof_snapshot_header(void);
+/* Bytes of one record of this handle (a multiple of 16).  Requires lmpc_store_create. */
+int lmpc_snapshot_bytes(lmpc_handle* h, size_t* bytes);
+/* Records of controllers inst_host[0..n) (host array; NULL = every controller, n == batch; repeats allowed) into the caller's
+ * device buffer rec_dev[n][bytes] (16-byte aligned).  Enqueued on the handle's stream, like lmpc_pool_export_dev. */
+int lmpc_snapshot_pack_dev(lmpc_handle* h, int n, const int* inst_host, void* rec_dev);
+/* Controller dst_host[i] takes record rec_of_dst_host[i] (NULL = i) of rec_dev[nrec][bytes], i < n (host arrays).  One record
+ * may be restored into many controllers.  A repeated destination or an index out of range returns LMPC_E_INVALID.  Records are
+ * outside input: one check kernel first validates every record used -- magic, version and layout equal to this handle's, the
+ * circuit (nseg, its nseg rows, TrackLength; bit for bit) the destination controller's, every index or bound field in range -- the
+ * call synchronises, and copies only if all passed; a refused call returns LMPC_E_INVALID naming the first failing record and
+ * field (lmpc_last_error) and leaves the handle as it was.  Warm start: the handle takes the records' warm_mode when it has none
+ * yet (no device-resident step since lmpc_store_create); otherwise every record's mode must be -1 or the handle's.  A successful
+ * unpack counts as a stored lap (lmpc_set_tracks then returns LMPC_E_STATE).  The copy is enqueued on the handle's stream. */
+int lmpc_snapshot_unpack_dev(lmpc_handle* h, const void* rec_dev, int nrec, int n, const int* dst_host, const int* rec_of_dst_host);
+/* The simulator's step counter, which keys the Philox noise with (seed, controller, step).  Requires lmpc_rollout_create. */
+int lmpc_rollout_get_clock(lmpc_handle* h, unsigned long long* step);
+int lmpc_rollout_set_clock(lmpc_handle* h, unsigned long long step);
+
 /* ---- presentation support (SURVEY §8f rank 4: the inputs of the reference's plot.py for device-resident batches) --------------
  * lmpc_track_global_position: Map.getGlobalPosition (Track.py:135-189) for n points; table6[nseg,6] = Map.PointAndTangent
  *   (x_end, y_end, psi_end, s_start, length, curvature), host arrays, xy[n,2] out, ok[n] (may be NULL) = 0 where the reference

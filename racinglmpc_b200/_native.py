@@ -40,6 +40,23 @@ class TrackParams(C.Structure):
     _fields_ = [("nseg", C.c_int), ("seg", C.c_double * (MAX_SEG * 3)), ("TrackLength", C.c_double)]
 
 
+SNAPSHOT_MAGIC, SNAPSHOT_VERSION, SNAPSHOT_SECTIONS = 0x50414E53, 1, 40
+# the layout ints of a record header, in header order (lmpc_snapshot_header)
+SNAPSHOT_LAYOUT = ("N", "M", "ncx", "ncu", "numSS_it", "trToUse", "ss_cap", "model_cap", "Tmax", "Tcl", "warm_start")
+# section slots of a record, in header order (csrc/snapshot.cuh, SnapSection); DESIGN.md "Controller snapshots"
+SNAPSHOT_SECTIONS_NAMES = ("ss_x", "ss_u", "ss_q", "ss_len", "model_x", "model_u", "model_len",
+                           "ss_time", "ss_lap", "it", "md_time", "md_seq", "md_cnt", "lap_hist", "lap_n", "sel", "is_prev", "prev_slot",
+                           "used", "xLin", "uLin", "zt", "OldInput", "xPredPrev", "timeStep", "has_pred", "warm", "warm_valid",
+                           "x", "xglob", "cl_x", "cl_u", "cl_len", "done", "health_flags", "health_unsolved", "abc_lti")
+
+
+class SnapshotHeader(C.Structure):
+    """lmpc_snapshot_header: the first bytes of every controller snapshot record."""
+    _fields_ = ([("magic", C.c_int), ("version", C.c_int), ("bytes", C.c_int)] + [(f, C.c_int) for f in SNAPSHOT_LAYOUT] +
+                [("warm_mode", C.c_int), ("nsect", C.c_int), ("sect_off", C.c_int * SNAPSHOT_SECTIONS),
+                 ("sect_bytes", C.c_int * SNAPSHOT_SECTIONS), ("track", TrackParams)])
+
+
 class NativeError(RuntimeError):
     pass
 
@@ -135,6 +152,12 @@ def lib():
     L.lmpc_host_free.argtypes = [_vp]
     L.lmpc_host_numa_node.argtypes = [C.c_int]
     L.lmpc_host_page_nodes.argtypes = [_vp, C.c_size_t, C.c_int, _vp]
+    L.lmpc_sizeof_snapshot_header.restype = C.c_int
+    L.lmpc_snapshot_bytes.argtypes = [_vp, C.POINTER(C.c_size_t)]
+    L.lmpc_snapshot_pack_dev.argtypes = [_vp, C.c_int, _vp, _vp]
+    L.lmpc_snapshot_unpack_dev.argtypes = [_vp, _vp, C.c_int, C.c_int, _vp, _vp]
+    L.lmpc_rollout_get_clock.argtypes = [_vp, C.POINTER(C.c_ulonglong)]
+    L.lmpc_rollout_set_clock.argtypes = [_vp, C.c_ulonglong]
     L.lmpc_sizeof_params.restype = C.c_int
     L.lmpc_sizeof_model_params.restype = C.c_int
     L.lmpc_sizeof_vehicle_params.restype = C.c_int
@@ -143,6 +166,7 @@ def lib():
     assert L.lmpc_sizeof_model_params() == C.sizeof(ModelParams), "lmpc_model_params ABI mismatch"
     assert L.lmpc_sizeof_vehicle_params() == C.sizeof(VehicleParams), "lmpc_vehicle_params ABI mismatch"
     assert L.lmpc_sizeof_track_params() == C.sizeof(TrackParams), "lmpc_track_params ABI mismatch"
+    assert L.lmpc_sizeof_snapshot_header() == C.sizeof(SnapshotHeader), "lmpc_snapshot_header ABI mismatch"
     _LIB = L
     return L
 
@@ -384,3 +408,84 @@ def make_track_sets(tracks, index, batch):
         out[k].seg[:] = buf
         out[k].TrackLength = L
     return out, idx
+
+
+# ---- controller snapshots: the checks the library makes, in Python, before any device work -----------------------------------
+def decode_snapshot_header(raw):
+    """Header of one snapshot record (bytes, or a uint8 array / CPU tensor holding at least the header) -> dict with magic, version,
+    bytes, the layout ints (SNAPSHOT_LAYOUT), warm_mode, the sections {name: (offset, bytes)} present, and the track row
+    (nseg, seg [nseg, 3], TrackLength).  Raises ValueError on a short buffer, a wrong magic or an unknown version."""
+    buf = bytes(np.asarray(raw, dtype=np.uint8).reshape(-1)[:C.sizeof(SnapshotHeader)]) if not isinstance(raw, (bytes, bytearray)) \
+        else bytes(raw[:C.sizeof(SnapshotHeader)])
+    if len(buf) < C.sizeof(SnapshotHeader):
+        raise ValueError("a snapshot record starts with a %d-byte header, got %d bytes" % (C.sizeof(SnapshotHeader), len(buf)))
+    h = SnapshotHeader.from_buffer_copy(buf)
+    if h.magic & 0xFFFFFFFF != SNAPSHOT_MAGIC:
+        raise ValueError("not a controller snapshot record (magic 0x%08x)" % (h.magic & 0xFFFFFFFF))
+    if h.version != SNAPSHOT_VERSION:
+        raise ValueError("snapshot record version %d; this build reads version %d" % (h.version, SNAPSHOT_VERSION))
+    out = {"magic": h.magic, "version": h.version, "bytes": h.bytes, "warm_mode": h.warm_mode}
+    out.update({f: getattr(h, f) for f in SNAPSHOT_LAYOUT})
+    out["sections"] = {n: (h.sect_off[k], h.sect_bytes[k]) for k, n in enumerate(SNAPSHOT_SECTIONS_NAMES) if h.sect_bytes[k] > 0}
+    nseg = int(h.track.nseg)
+    out["track"] = {"nseg": nseg, "seg": np.array(h.track.seg[:3 * max(0, min(nseg, MAX_SEG))]).reshape(-1, 3),
+                    "TrackLength": float(h.track.TrackLength)}
+    return out
+
+
+def snapshot_layout_mismatch(header, layout):
+    """The first layout field in which a decoded header differs from ``layout`` (a dict with SNAPSHOT_LAYOUT keys and "bytes"), as
+    a message, or None when the record fits."""
+    for f in SNAPSHOT_LAYOUT + ("bytes",):
+        if int(header[f]) != int(layout[f]):
+            return "snapshot layout mismatch: %s is %d in the record and %d in this controller" % (f, header[f], layout[f])
+    return None
+
+
+def snapshot_indices(index, batch, what, unique=False):
+    """Controller indices of a snapshot call: None stays None (every controller), else a non-empty 1-D list of integers in
+    [0, batch), unique when ``unique``.  Returns an int32 array; raises ValueError."""
+    if index is None:
+        return None
+    a = np.asarray(index).reshape(-1)
+    if a.size == 0:
+        raise ValueError("%s: at least one controller" % what)
+    idx = np.ascontiguousarray(a, dtype=np.int32)
+    if not np.issubdtype(a.dtype, np.integer) or not np.array_equal(idx, a):
+        raise ValueError("%s must hold integer controller indices" % what)
+    if idx.min() < 0 or idx.max() >= batch:
+        raise ValueError("%s: controller index out of range [0, %d)" % (what, batch))
+    if unique and np.unique(idx).size != idx.size:
+        raise ValueError("%s: a controller may be restored only once per call" % what)
+    return idx
+
+
+def snapshot_record_map(rec_of, n, nrec):
+    """Record of every destination for an unpack: None = record i for destination i (needs nrec >= n), else n integers in
+    [0, nrec).  Returns an int32 array; raises ValueError."""
+    if rec_of is None:
+        if nrec < n:
+            raise ValueError("%d destinations and %d records: pass rec_of to map records onto destinations" % (n, nrec))
+        return np.arange(n, dtype=np.int32)
+    a = np.asarray(rec_of).reshape(-1)
+    idx = np.ascontiguousarray(a, dtype=np.int32)
+    if a.size != n or not np.issubdtype(a.dtype, np.integer) or not np.array_equal(idx, a):
+        raise ValueError("rec_of needs one integer record index per destination (%d)" % n)
+    if n and (idx.min() < 0 or idx.max() >= nrec):
+        raise ValueError("rec_of: record index out of range [0, %d)" % nrec)
+    return idx
+
+
+def check_snapshot_tensor(t, device, nbytes, rows=None, what="records"):
+    """A record buffer: a contiguous uint8 CUDA tensor [rows, nbytes] on cuda:``device`` whose data is 16-byte aligned.  Raises
+    ValueError."""
+    if not hasattr(t, "is_cuda") or not hasattr(t, "dtype"):
+        raise ValueError("%s must be a torch tensor" % what)
+    if str(t.dtype) != "torch.uint8":
+        raise ValueError("%s must be uint8, got %s" % (what, t.dtype))
+    if not t.is_cuda or t.device.index != int(device):
+        raise ValueError("%s must live on cuda:%d, got %s" % (what, int(device), t.device))
+    if t.dim() != 2 or t.shape[1] != nbytes or (rows is not None and t.shape[0] != rows) or t.shape[0] < 1:
+        raise ValueError("%s must have shape [%s, %d], got %s" % (what, "n" if rows is None else rows, nbytes, tuple(t.shape)))
+    if not t.is_contiguous() or t.data_ptr() % 16:
+        raise ValueError("%s must be contiguous and 16-byte aligned" % what)

@@ -46,6 +46,7 @@ class BatchedController:
         h = C.c_void_p()
         nat.check(L.lmpc_create(C.byref(self._p), self.B, int(device), C.byref(h)))
         self._h = h
+        self._device = int(device)
         self.ss_cap = int(ss_cap) if ss_cap is not None else (self.numSS_it + 2 if self.lmpc else 0)
         self.model_cap = int(model_cap) if model_cap is not None else self.trToUse + 1
         self._mp = nat.make_model_params(seg_table, TrackLength, trToUse, **(model_kwargs or {}))
@@ -598,6 +599,131 @@ class BatchedController:
         nat.check(self._lib.lmpc_pool_import_dev(self._h, int(n_src), int(share), int(Tpad), int(gid_base), nat.ptr(rows_dev),
                                                  nat.ptr(meta_dev), nat.ptr(took)))
         return int(took[0]) if count else None
+
+    # ------------------------------------------------------------------ controller snapshots (csrc/snapshot.cuh)
+    def _snapshot_ready(self, restoring=False):
+        """Snapshots read and write the device lap books.  Host book mirrors would go stale, so a controller that keeps them
+        raises ValueError; one that has stored no lap yet may restore (and keeps device books from then on)."""
+        if self.device_books or (restoring and not any(self.it) and not any(self.model_count)):
+            return
+        raise ValueError("snapshots need device lap books (rollout_seed_from_record_dev or enable_device_books): this controller "
+                         "keeps host book mirrors, which a restore would leave stale")
+
+    @property
+    def snapshot_bytes(self):
+        """Bytes of one controller's snapshot record (a multiple of 16)."""
+        n = C.c_size_t(0)
+        nat.check(self._lib.lmpc_snapshot_bytes(self._h, C.byref(n)))
+        return int(n.value)
+
+    def snapshot_layout(self):
+        """The layout a record of this controller has (the keys of nat.SNAPSHOT_LAYOUT and "bytes")."""
+        return dict(N=self.N, M=self.M, ncx=int(self._p.ncx), ncu=int(self._p.ncu), numSS_it=max(self.numSS_it, 1),
+                    trToUse=self.trToUse, ss_cap=max(self.ss_cap, 1), model_cap=self.model_cap, Tmax=self.Tmax,
+                    Tcl=int(getattr(self, "Tcl", 0)), warm_start=int(self._p.warm_start), bytes=self.snapshot_bytes)
+
+    def _ext_stream(self, torch):
+        return torch.cuda.ExternalStream(self.stream, device=torch.device("cuda", self.device))
+
+    @property
+    def device(self):
+        return int(self._device)
+
+    def snapshot(self, inst=None, out=None):
+        """Records of controllers ``inst`` (None: every controller, in order; repeats allowed) as a uint8 CUDA tensor
+        [n, snapshot_bytes] on this controller's device (``out``: a tensor of that shape to write into).  What a controller learned
+        and where it is: lap pools, lap books, controller state, warm-start record, closed loop, health.  Not what it is told to
+        drive (parameter sets, vehicles, tracks, pool groups).  Ordered after the work enqueued so far and before later work on the
+        current torch stream."""
+        import torch
+        self._snapshot_ready()
+        idx = nat.snapshot_indices(inst, self.B, "inst")
+        n = self.B if idx is None else int(idx.size)
+        nbytes = self.snapshot_bytes
+        dev = torch.device("cuda", self.device)
+        if out is None:
+            out = torch.empty((n, nbytes), dtype=torch.uint8, device=dev)
+        nat.check_snapshot_tensor(out, self.device, nbytes, rows=n, what="out")
+        ext, cur = self._ext_stream(torch), torch.cuda.current_stream(dev)
+        ext.wait_stream(cur)                               # the buffer may still be in use by work of the current stream
+        nat.check(self._lib.lmpc_snapshot_pack_dev(self._h, n, nat.ptr(idx), nat.ptr(out)))
+        cur.wait_stream(ext)                               # later work on the current stream (reuse of the buffer included) follows
+        return out
+
+    def restore(self, records, inst=None, rec_of=None):
+        """Controller ``inst[i]`` (None: 0 .. n-1) takes record ``rec_of[i]`` (None: i) of ``records`` (uint8 CUDA tensor
+        [nrec, snapshot_bytes] on this device, e.g. from ``snapshot`` of a controller with the same layout, or torch.load).  One
+        record may go to many controllers.  The record's track must be the destination controller's; its car and tuning are
+        whatever this controller has installed.  Raises ValueError on a repeated or out-of-range destination, a bad tensor or a
+        layout mismatch (named) before any device work; the library then checks every record used and refuses (NativeError,
+        nothing restored) unless all pass."""
+        import torch
+        dst, rec = self._check_restore(records, inst, rec_of)
+        dev = torch.device("cuda", self.device)
+        ext, cur = self._ext_stream(torch), torch.cuda.current_stream(dev)
+        ext.wait_stream(cur)                               # records written on the current stream are complete
+        nat.check(self._lib.lmpc_snapshot_unpack_dev(self._h, nat.ptr(records), int(records.shape[0]), int(dst.size), nat.ptr(dst),
+                                                     nat.ptr(rec)))
+        cur.wait_stream(ext)
+        if not self.device_books:                          # a fresh controller: the restored books live on the device
+            self.device_books = True
+            self._sel_dirty = self._used_dirty = False
+
+    def _check_restore(self, records, inst, rec_of):
+        """The pure-Python checks of ``restore``: books, tensor, indices, and the header of every record used against this
+        layout.  Returns (destinations, record of each destination) as int32 arrays."""
+        import torch
+        self._snapshot_ready(restoring=True)
+        mine = self.snapshot_layout()
+        nat.check_snapshot_tensor(records, self.device, mine["bytes"])
+        nrec = int(records.shape[0])
+        dst = nat.snapshot_indices(inst, self.B, "inst", unique=True)
+        if dst is None:
+            dst = np.arange(min(self.B, nrec) if rec_of is None else self.B, dtype=np.int32)
+        rec = nat.snapshot_record_map(rec_of, int(dst.size), nrec)
+        used = np.unique(rec)
+        hsz = C.sizeof(nat.SnapshotHeader)
+        heads = records[:, :hsz].index_select(0, torch.from_numpy(used.astype(np.int64)).to(records.device)).cpu().numpy()
+        words = np.ascontiguousarray(heads[:, :64]).view(np.int32)     # magic, version, bytes, the layout ints, warm_mode, nsect
+        want = np.array([nat.SNAPSHOT_MAGIC, nat.SNAPSHOT_VERSION, mine["bytes"]] + [mine[f] for f in nat.SNAPSHOT_LAYOUT], np.int64)
+        bad = np.nonzero(np.any(words[:, :14].astype(np.int64) & 0xFFFFFFFF != want & 0xFFFFFFFF, axis=1))[0]
+        if bad.size:
+            r = int(used[bad[0]])
+            msg = nat.snapshot_layout_mismatch(nat.decode_snapshot_header(heads[bad[0]]), mine)
+            raise ValueError("record %d: %s" % (r, msg or "header does not match this controller"))
+        return dst, rec
+
+    def clone(self, src, dst):
+        """Controller ``dst[i]`` becomes a copy of controller ``src[i]`` (or of the single ``src`` for every ``dst``): packed into
+        a temporary buffer first, so overlapping ``src`` / ``dst`` are safe (a permutation works)."""
+        dst_i = nat.snapshot_indices(dst, self.B, "dst", unique=True)
+        if dst_i is None:
+            raise ValueError("dst: the controllers to overwrite are required")
+        src_i = nat.snapshot_indices(src, self.B, "src")
+        if src_i is None:
+            raise ValueError("src: the controllers to copy are required")
+        if src_i.size == 1 and dst_i.size > 1:
+            rec_of = np.zeros(dst_i.size, np.int32)
+        elif src_i.size == dst_i.size:
+            rec_of = None
+        else:
+            raise ValueError("clone: one src, or one src per dst (%d), got %d" % (dst_i.size, src_i.size))
+        self._snapshot_ready()
+        recs = self.snapshot(src_i)
+        self.restore(recs, dst_i, rec_of)
+
+    @property
+    def rollout_clock(self):
+        """The simulator's step counter: the Philox noise of a step is keyed by (seed, controller, this counter)."""
+        v = C.c_ulonglong(0)
+        nat.check(self._lib.lmpc_rollout_get_clock(self._h, C.byref(v)))
+        return int(v.value)
+
+    @rollout_clock.setter
+    def rollout_clock(self, step):
+        if int(step) < 0:
+            raise ValueError("the rollout clock counts steps: >= 0")
+        nat.check(self._lib.lmpc_rollout_set_clock(self._h, int(step)))
 
     def device_buffer(self, name):
         return int(self._lib.lmpc_device_buffer(self._h, name.encode()) or 0)

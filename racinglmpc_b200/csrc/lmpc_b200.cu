@@ -30,6 +30,7 @@
 #include "lapbooks.cuh"
 #include "probe.cuh"
 #include "ftocp_launch.cuh"
+#include "snapshot.cuh"
 
 using namespace lmpc;
 static_assert(POOL_MAXG == LMPC_MAX_POOL_GROUPS, "the exchange scratch is sized for LMPC_MAX_POOL_GROUPS groups");
@@ -117,6 +118,8 @@ struct lmpc_handle {
     TraceBufs tr;
     int* d_trinst;
     bool has_trace;
+    // controller snapshots (snapshot.cuh): header template [SNAP_HDR_WORDS] + check verdict [4], allocated on first use
+    int* d_snap;
 };
 
 static bool inv6(const double* A, double* Ai) {
@@ -275,7 +278,7 @@ static void free_store(lmpc_handle* h) {
     free_null(h->d_hasPred); free_null(h->d_flags); free_null(h->d_minidx); free_null(h->d_xLin); free_null(h->d_uLin);
     free_null(h->d_ztState); free_null(h->d_ztFixed); free_null(h->d_OldInput); free_null(h->d_xPredPrev); free_null(h->d_tmpx);
     free_null(h->d_tmpu); free_null(h->d_xchg); free_null(h->d_dropped);
-    free_null(h->d_bkbuf); free_null(h->d_poolidx); free_null(h->d_stats);
+    free_null(h->d_bkbuf); free_null(h->d_poolidx); free_null(h->d_stats); free_null(h->d_snap);
     free_null(h->d_warm); free_null(h->d_warm_valid);
     free_null(h->d_trk); free_null(h->d_trk_idx);
     h->trk_host.clear(); h->trk_idx_host.clear();
@@ -923,7 +926,15 @@ int lmpc_set_tracks(lmpc_handle* h, const lmpc_track_params* sets, int nsets, co
     }
     std::vector<TrackRec> rows;
     if (nsets == 0) rows.push_back(h->store_trk);
-    else rows.assign(sets, sets + nsets);
+    else {          // canonical rows: padding and the entries past nseg are zero, so a record's track row is the circuit alone
+        rows.resize(nsets);
+        for (int k = 0; k < nsets; ++k) {
+            memset(&rows[k], 0, sizeof(TrackRec));
+            rows[k].nseg = sets[k].nseg;
+            for (int i = 0; i < sets[k].nseg * 3; ++i) rows[k].seg[i] = sets[k].seg[i];
+            rows[k].TrackLength = sets[k].TrackLength;
+        }
+    }
     if ((rc = swap_table(h, who, rows.data(), (int)rows.size(), set_of_instance, &h->d_trk, &h->d_trk_idx)) != LMPC_OK) return rc;
     h->trk_host = rows;
     if (set_of_instance) h->trk_idx_host.assign(set_of_instance, set_of_instance + h->batch);
@@ -1823,6 +1834,235 @@ int lmpc_pool_import_dev(lmpc_handle* h, int n_src, int share, int Tpad, long lo
         CK(cudaMemcpyAsync(took_host, took, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
         CK(cudaStreamSynchronize(h->stream));
     }
+    return LMPC_OK;
+}
+
+// ================================================================================================
+// controller snapshots (snapshot.cuh): one byte record per controller
+// ================================================================================================
+}  // extern "C" (the helpers below have C++ linkage)
+
+static const char* snap_field_name(int f) {
+    static const char* names[SF_NFIELD] = {
+        "magic", "version", "record bytes", "N", "numSS_Points", "ncx", "ncu", "numSS_it", "trToUse", "ss_cap", "model_cap", "Tmax",
+        "Tcl", "warm_start", "warm_mode", "nsect", "section table", "track row", "safe-set lap length", "model lap length", "it",
+        "safe-set lap number", "md_cnt", "model arrival number", "lap_n", "sel", "is_prev", "prev_slot", "used", "timeStep",
+        "has_pred", "warm_valid", "cl_len", "done"};
+    return f >= 0 && f < SF_NFIELD ? names[f] : "?";
+}
+
+// The record layout of this handle: copy table t (handle buffers, record offsets, word sizes, chunks) and header hd (layout ints,
+// section offsets; the track row and warm_mode are per pack).  Every per-controller buffer of the store and the rollout is either
+// a section here or per-step scratch (DESIGN.md, "Controller snapshots").
+static void snap_layout(const lmpc_handle* h, SnapTable& t, lmpc_snapshot_header& hd) {
+    memset(&t, 0, sizeof(t));
+    memset(&hd, 0, sizeof(hd));
+    const long long B = h->batch, N = h->N, sc = h->ss.cap, mc = h->mdl.cap, T = h->ss.Tmax, D = sizeof(double), I = sizeof(int);
+    auto sect = [&](int k, const void* base, long long bytes) { t.s[k].base = (char*)base; t.s[k].stride = bytes; t.s[k].bytes = (int)bytes; };
+    sect(SN_SS_X, h->ss.x, sc * T * 6 * D); sect(SN_SS_U, h->ss.u, sc * T * 2 * D); sect(SN_SS_Q, h->ss.q, sc * T * D);
+    sect(SN_SS_LEN, h->ss.len, sc * I);
+    sect(SN_MD_X, h->mdl.x, mc * T * 6 * D); sect(SN_MD_U, h->mdl.u, mc * T * 2 * D); sect(SN_MD_LEN, h->mdl.len, mc * I);
+    const LapBooks& k = h->bk;
+    sect(SN_SS_TIME, k.ss_time, sc * I); sect(SN_SS_LAP, k.ss_lap, sc * I); sect(SN_IT, k.it, I);
+    sect(SN_MD_TIME, k.md_time, mc * I); sect(SN_MD_SEQ, k.md_seq, mc * I); sect(SN_MD_CNT, k.md_cnt, I);
+    sect(SN_LAP_HIST, k.lap_hist, LAP_HIST * I); sect(SN_LAP_N, k.lap_n, I);
+    sect(SN_SEL, k.sel, k.numSS_it * I); sect(SN_ISPREV, k.isprev, k.numSS_it * I); sect(SN_PREVSLOT, k.prevslot, I);
+    sect(SN_USED, k.used, k.trToUse * I);
+    sect(SN_XLIN, h->d_xLin, (N + 1) * 6 * D); sect(SN_ULIN, h->d_uLin, N * 2 * D); sect(SN_ZT, h->d_ztState, 6 * D);
+    sect(SN_OLDINPUT, h->d_OldInput, 2 * D); sect(SN_XPREDPREV, h->d_xPredPrev, (N + 1) * 6 * D);
+    sect(SN_TIMESTEP, h->d_timeStep, I); sect(SN_HASPRED, h->d_hasPred, I);
+    if (h->d_warm) { sect(SN_WARM, h->d_warm, h->warm_stride * D); sect(SN_WARM_VALID, h->d_warm_valid, I); }
+    if (h->has_rollout) {
+        sect(SN_RX, h->d_rx[h->cur], 6 * D); sect(SN_RG, h->d_rg[h->cur], 6 * D);
+        sect(SN_CLX, h->d_clx, (long long)h->Tcl * 6 * D); sect(SN_CLU, h->d_clu, (long long)h->Tcl * 2 * D);
+        sect(SN_CLLEN, h->d_cllen, I); sect(SN_DONE, h->d_done, I);
+        sect(SN_HEALTH_FLAGS, h->d_health, I); sect(SN_HEALTH_UNSOLVED, h->d_health + B, I);     // health is [2][B]
+        sect(SN_ABC_LTI, h->d_abc_lti, 54 * D);
+    }
+    auto up16 = [](long long v) { return (v + 15) / 16 * 16; };
+    long long off = up16(sizeof(lmpc_snapshot_header));
+    for (int s = 0; s < SN_COUNT; ++s) {
+        if (!t.s[s].bytes) continue;
+        t.s[s].rec_off = (int)off;
+        hd.sect_off[s] = (int)off;
+        hd.sect_bytes[s] = t.s[s].bytes;
+        off += up16(t.s[s].bytes);
+    }
+    t.s[SN_HEADER].base = (char*)h->d_snap;                       // the handle's header template (snap_scratch)
+    t.s[SN_HEADER].bytes = SNAP_HDR_WORDS * 4;
+    t.s[SN_HEADER].pack_only = 1;
+    t.s[SN_TRACK].base = (char*)h->d_trk;
+    t.s[SN_TRACK].idx = h->d_trk_idx;
+    t.s[SN_TRACK].stride = h->d_trk_idx ? sizeof(TrackRec) : 0;
+    t.s[SN_TRACK].bytes = sizeof(TrackRec);
+    t.s[SN_TRACK].rec_off = SNAP_HDR_WORDS * 4;
+    t.s[SN_TRACK].pack_only = 1;
+    for (int s = 0; s < SN_TABLE; ++s) {
+        SnapSect& e = t.s[s];
+        // every address a thread touches is base + k * stride + rec_off-relative offset: the word must divide all four (a buffer
+        // carved out of a larger allocation, like the lap history in the books buffer, need not be 16-byte aligned)
+        const long long all = e.bytes | e.stride | e.rec_off | (long long)(uintptr_t)e.base;
+        e.word = (all % 16 == 0) ? 16 : (all % 8 == 0) ? 8 : 4;
+    }
+    t.chunk_bytes = 16 << 10;
+    for (;;) {
+        int n = 0;
+        for (int s = 0; s < SN_TABLE; ++s) n += (t.s[s].bytes + t.chunk_bytes - 1) / t.chunk_bytes;
+        if (n <= SNAP_MAXCHUNK) break;
+        t.chunk_bytes *= 2;
+    }
+    for (int s = 0; s < SN_TABLE; ++s)
+        for (int c = 0; c * (long long)t.chunk_bytes < t.s[s].bytes; ++c) {
+            t.chunk_sect[t.nchunk] = (unsigned short)s;
+            t.chunk_no[t.nchunk] = (unsigned short)c;
+            ++t.nchunk;
+        }
+    hd.magic = LMPC_SNAPSHOT_MAGIC; hd.version = LMPC_SNAPSHOT_VERSION; hd.bytes = (int)off;
+    hd.N = h->N; hd.M = h->M; hd.ncx = h->p.ncx; hd.ncu = h->p.ncu; hd.numSS_it = k.numSS_it; hd.trToUse = k.trToUse;
+    hd.ss_cap = (int)sc; hd.model_cap = (int)mc; hd.Tmax = (int)T; hd.Tcl = h->has_rollout ? h->Tcl : 0;
+    hd.warm_start = h->d_warm ? 1 : 0;
+    hd.warm_mode = h->d_warm ? h->warm_mode : -1;
+    hd.nsect = LMPC_SNAPSHOT_SECTIONS;
+}
+
+// The header template and the check verdict of this handle, allocated on first use
+static int snap_scratch(lmpc_handle* h) {
+    if (!h->d_snap) CK(cudaMalloc((void**)&h->d_snap, sizeof(int) * (SNAP_HDR_WORDS + 4)));
+    return LMPC_OK;
+}
+
+// Upload the controller indices (and record indices) of one pack / unpack to stream-ordered scratch of their own
+static int snap_indices(lmpc_handle* h, const std::vector<int>& idx, int** d_idx) {
+    CK(cudaMallocAsync((void**)d_idx, sizeof(int) * idx.size(), h->stream));
+    CK(cudaMemcpyAsync(*d_idx, idx.data(), sizeof(int) * idx.size(), cudaMemcpyHostToDevice, h->stream));
+    return LMPC_OK;
+}
+
+extern "C" {
+
+int lmpc_sizeof_snapshot_header(void) { return (int)sizeof(lmpc_snapshot_header); }
+
+int lmpc_snapshot_bytes(lmpc_handle* h, size_t* bytes) {
+    int rc = need_books(h);
+    if (rc) return rc;
+    if (!bytes) return fail(LMPC_E_INVALID, "null output");
+    SnapTable t;
+    lmpc_snapshot_header hd;
+    snap_layout(h, t, hd);
+    *bytes = (size_t)hd.bytes;
+    return LMPC_OK;
+}
+
+int lmpc_snapshot_pack_dev(lmpc_handle* h, int n, const int* inst_host, void* rec_dev) {
+    static const char* who = "lmpc_snapshot_pack_dev";
+    int rc = need_books(h);
+    if (rc) return rc;
+    if (!rec_dev || n < 1) return fail(LMPC_E_INVALID, std::string(who) + ": null records or n < 1");
+    if (!inst_host && n != h->batch) return fail(LMPC_E_INVALID, std::string(who) + ": NULL controllers means every controller (n == batch)");
+    if ((rc = check_align(rec_dev, "the record buffer")) != LMPC_OK) return rc;
+    std::vector<int> idx(n);
+    for (int i = 0; i < n; ++i) {
+        idx[i] = inst_host ? inst_host[i] : i;
+        if (idx[i] < 0 || idx[i] >= h->batch)
+            return fail(LMPC_E_INVALID, std::string(who) + ": controller index " + std::to_string(i) + " out of range");
+    }
+    CK(cudaSetDevice(h->device));
+    if ((rc = snap_scratch(h)) != LMPC_OK) return rc;
+    SnapTable t;
+    lmpc_snapshot_header hd;
+    snap_layout(h, t, hd);
+    // the header template, staged from the stack (pageable memory: the copy has left it when the call returns)
+    CK(cudaMemcpyAsync(h->d_snap, &hd, SNAP_HDR_WORDS * 4, cudaMemcpyHostToDevice, h->stream));
+    int* d_idx = nullptr;
+    if ((rc = snap_indices(h, idx, &d_idx)) != LMPC_OK) return rc;
+    snapshot_copy_kernel<<<dim3(n, t.nchunk), 256, 0, h->stream>>>(t, 0, d_idx, nullptr, (char*)rec_dev, hd.bytes);
+    CK(cudaGetLastError());
+    CK(cudaFreeAsync(d_idx, h->stream));
+    h->launches += 1;
+    return LMPC_OK;
+}
+
+int lmpc_snapshot_unpack_dev(lmpc_handle* h, const void* rec_dev, int nrec, int n, const int* dst_host, const int* rec_of_dst_host) {
+    static const char* who = "lmpc_snapshot_unpack_dev";
+    int rc = need_books(h);
+    if (rc) return rc;
+    const std::string w = std::string(who) + ": ";
+    if (!rec_dev || !dst_host || nrec < 1 || n < 1 || n > h->batch)
+        return fail(LMPC_E_INVALID, w + "null records or destinations, nrec < 1, or n not in 1 .. batch");
+    if ((rc = check_align(rec_dev, "the record buffer")) != LMPC_OK) return rc;
+    std::vector<int> idx(2 * (size_t)n);               // destinations [n] | records [n]
+    std::vector<char> seen(h->batch, 0);
+    for (int i = 0; i < n; ++i) {
+        const int d = dst_host[i], r = rec_of_dst_host ? rec_of_dst_host[i] : i;
+        if (d < 0 || d >= h->batch) return fail(LMPC_E_INVALID, w + "destination " + std::to_string(i) + " out of range");
+        if (seen[d]) return fail(LMPC_E_INVALID, w + "controller " + std::to_string(d) + " is a destination twice");
+        if (r < 0 || r >= nrec) return fail(LMPC_E_INVALID, w + "record index of destination " + std::to_string(i) + " out of range");
+        seen[d] = 1;
+        idx[i] = d;
+        idx[n + i] = r;
+    }
+    CK(cudaSetDevice(h->device));
+    if ((rc = snap_scratch(h)) != LMPC_OK) return rc;
+    SnapTable t;
+    lmpc_snapshot_header hd;
+    snap_layout(h, t, hd);
+    int* verdict = h->d_snap + SNAP_HDR_WORDS;
+    const int init[3] = {INT32_MAX, INT32_MAX, INT32_MIN};
+    CK(cudaMemcpyAsync(h->d_snap, &hd, SNAP_HDR_WORDS * 4, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(verdict, init, sizeof(init), cudaMemcpyHostToDevice, h->stream));
+    int* d_idx = nullptr;
+    if ((rc = snap_indices(h, idx, &d_idx)) != LMPC_OK) return rc;
+    SnapCheckArgs a;
+    a.hdr = h->d_snap;
+    for (int s = 0; s < SN_COUNT; ++s) a.rec_off[s] = t.s[s].rec_off;
+    a.trk = tracks(h);
+    a.ss_cap = h->ss.cap; a.md_cap = h->mdl.cap; a.numSS_it = h->bk.numSS_it; a.trToUse = h->bk.trToUse; a.Tmax = h->ss.Tmax;
+    a.Tcl = hd.Tcl; a.warm_mode = hd.warm_mode;
+    snapshot_check_kernel<<<(n + 127) / 128, 128, 0, h->stream>>>(a, n, d_idx, d_idx + n, (const char*)rec_dev, hd.bytes, verdict);
+    h->launches += 1;
+    int got[3];
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(got, verdict, sizeof(got), cudaMemcpyDeviceToHost, h->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+    if (e != cudaSuccess) {
+        cudaFreeAsync(d_idx, h->stream);
+        return fail(LMPC_E_CUDA, w + "record check: " + cudaGetErrorString(e));
+    }
+    int mode = h->warm_mode;
+    std::string why;
+    if (got[0] != INT32_MAX) {
+        const int i = got[0] / 64, f = got[0] % 64;
+        why = "record " + std::to_string(idx[n + i]) + " (into controller " + std::to_string(idx[i]) + "): " + snap_field_name(f) +
+              (f <= SF_SECTIONS ? " differs from this handle's" : f == SF_TRACK ? " differs from the controller's track" : " out of range");
+    } else if (h->d_warm && got[1] <= got[2]) {
+        if (h->warm_mode < 0 && got[1] != got[2]) why = "the records hold warm-start records of two problem types";
+        else mode = got[1];
+    }
+    if (!why.empty()) {
+        cudaFreeAsync(d_idx, h->stream);
+        return fail(LMPC_E_INVALID, w + why + "; nothing was restored");
+    }
+    snapshot_copy_kernel<<<dim3(n, t.nchunk), 256, 0, h->stream>>>(t, 1, d_idx, d_idx + n, (char*)rec_dev, hd.bytes);
+    CK(cudaGetLastError());
+    CK(cudaFreeAsync(d_idx, h->stream));
+    h->launches += 1;
+    h->laps_stored = true;
+    if (h->d_warm) h->warm_mode = mode;
+    return LMPC_OK;
+}
+
+int lmpc_rollout_get_clock(lmpc_handle* h, unsigned long long* step) {
+    int rc = need_rollout(h);
+    if (rc) return rc;
+    if (!step) return fail(LMPC_E_INVALID, "null output");
+    *step = h->sim_step;
+    return LMPC_OK;
+}
+
+int lmpc_rollout_set_clock(lmpc_handle* h, unsigned long long step) {
+    int rc = need_rollout(h);
+    if (rc) return rc;
+    h->sim_step = step;
     return LMPC_OK;
 }
 
