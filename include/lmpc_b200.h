@@ -317,10 +317,9 @@ int lmpc_rollout_set_vehicles(lmpc_handle* h, const lmpc_vehicle_params* sets, i
 int lmpc_rollout_sysid(lmpc_handle* h, double lamb, double* abc_host, int* flags_host);
 int lmpc_rollout_seed_from_record(lmpc_handle* h, int copies, int ss_slot0, int model_slot0);
 int lmpc_rollout_get_lap(lmpc_handle* h, int inst, int* T, double* x, double* u);              /* closed-loop record   */
-/* Lap hand-over on the device = LMPC.addTrajectory + PredictiveModel.addTrajectory of the lap just driven (either slot may
- * be -1), then s -= TrackLength (SysModel.py:50), record restarted, timeStep = 0 (PC.py:445). */
-int lmpc_rollout_commit_lap(lmpc_handle* h, int inst, int ss_slot, int model_slot);
-/* The same for every instance with fin_host[b] != 0 in one launch; slots per instance as above ([B] host arrays). */
+/* Lap hand-over on the device = LMPC.addTrajectory + PredictiveModel.addTrajectory of the lap just driven, then
+ * s -= TrackLength (SysModel.py:50), record restarted, timeStep = 0 (PC.py:445), for every instance with fin_host[b] != 0 in
+ * one launch; per instance a safe-set and a regression slot, either of which may be -1 ([B] host arrays). */
 int lmpc_rollout_commit_laps(lmpc_handle* h, const int* fin_host, const int* ss_slots_host, const int* model_slots_host);
 /* Pack all closed-loop records into rows_dev[B,Tpad,8] = (x | u), lens_dev[B] (device buffers of the caller): the send
  * buffer of the once-per-lap all-gather of the pooled-safe-set mode (SURVEY §8e). */

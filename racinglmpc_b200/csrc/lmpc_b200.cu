@@ -10,6 +10,7 @@
 // wgmma has no f64 type — see DESIGN.md.
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <stddef.h>
 #include <string.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -51,13 +52,41 @@ static int fail(int code, const std::string& msg) {
         if (e_ != cudaSuccess) return fail(LMPC_E_CUDA, std::string(#call) + ": " + cudaGetErrorString(e_)); \
     } while (0)
 
-// The QP kernel's inputs and outputs for one whole batch: [B,6] x0, [B,2] uOld, [B,N,54] abc, [B,6,M] SS, [B,M] Qfun, [B,6,M]
-// SuccSS, [B,2,M] SuccU, [B,N+1,6] xPred, [B,N,2] uPred, [B,N*2] slack, [B,M] lambd, [B,6] slackT, [B,6] zt, [B,2] ztu,
-// [B,3] resid, [B] status, [B] iters (M = 1 for handles without a safe set)
-struct QpBufs {
-    double *x0, *uOld, *abc, *SS, *Qfun, *SuccSS, *SuccU, *xPred, *uPred, *slack, *lambd, *slackT, *zt, *ztu, *resid;
+// The QP kernel's inputs and outputs for one whole batch, either a buffer set of the handle or the caller's arrays (of which the
+// inputs are only read); null = not wanted.  QP_FIELDS describes every field.
+struct QpIo {
+    double *x0, *uOld, *abc, *SS, *Qfun, *SuccSS, *SuccU, *xPred, *uPred, *slack, *lambd, *slackT, *zt, *ztu;
     int *status, *iters;
+    double* resid;
 };
+
+// One field of QpIo: c1 + cN * N + cM * M elements per instance (M = 1 for handles without a safe set), input or output, and
+// whether only LMPC-type QPs (with a safe set) have it.  The table order is the order of the copies of a host solve.
+struct QpField {
+    size_t off, elem;
+    int c1, cN, cM;
+    bool in, lmpc_only;
+    const char* name;          // lmpc_device_buffer name of buffer set 0, or null
+    size_t count(size_t N, size_t M) const { return c1 + cN * N + cM * M; }
+    void*& at(QpIo& q) const { return *(void**)((char*)&q + off); }
+    void* at(const QpIo& q) const { return *(void* const*)((const char*)&q + off); }
+};
+#define QF(f, c1, cN, cM, in, lm, name) QpField{offsetof(QpIo, f), sizeof(*QpIo().f), c1, cN, cM, in, lm, name}
+static const QpField QP_FIELDS[] = {
+    QF(x0, 6, 0, 0, true, false, "x0"), QF(uOld, 2, 0, 0, true, false, nullptr), QF(abc, 0, 54, 0, true, false, "abc"),
+    QF(SS, 0, 0, 6, true, true, "SS_sel"), QF(Qfun, 0, 0, 1, true, true, "Qfun_sel"), QF(SuccSS, 0, 0, 6, true, true, "Succ_SS"),
+    QF(SuccU, 0, 0, 2, true, true, "Succ_uSS"),
+    QF(xPred, 6, 6, 0, false, false, "xPred"), QF(uPred, 0, 2, 0, false, false, "uPred"), QF(slack, 0, 2, 0, false, false, "slack"),
+    QF(lambd, 0, 0, 1, false, true, "lambd"), QF(slackT, 6, 0, 0, false, true, "slackT"), QF(zt, 6, 0, 0, false, true, "zt"),
+    QF(ztu, 2, 0, 0, false, true, "zt_u"), QF(status, 1, 0, 0, false, false, "status"), QF(iters, 1, 0, 0, false, false, "iters"),
+    QF(resid, 3, 0, 0, false, false, "resid")};
+#undef QF
+
+// The QP arrays of a public QP entry point's argument list
+#define CALLER_QP_IO                                                                                                        \
+    QpIo{const_cast<double*>(x0), const_cast<double*>(uOld), const_cast<double*>(abc), const_cast<double*>(SS_sel),        \
+         const_cast<double*>(Qfun_sel), const_cast<double*>(Succ_SS), const_cast<double*>(Succ_uSS), xPred, uPred, slack, \
+         lambd, slackTerminal, zt, zt_u, status, iters, resid}
 
 struct lmpc_handle {
     lmpc_params p;
@@ -71,7 +100,7 @@ struct lmpc_handle {
     long long launches;
     // QP buffer sets, one per slot of the *_host entry points.  hb[0] is allocated at creation and is also the device-resident
     // step's (K1 writes its abc, K2 its safe set, the QP kernel its outputs; lmpc_device_buffer); hb[1..] on first use.
-    QpBufs hb[LMPC_HOST_SLOTS];
+    QpIo hb[LMPC_HOST_SLOTS];
     unsigned long long* d_late;
     // warm-start records of the controllers of the device-resident step (lmpc_params.warm_start; allocated with the store)
     double* d_warm;
@@ -105,10 +134,9 @@ struct lmpc_handle {
     // sets a one-row table holding the reference vehicle and a null index (allocated at creation)
     lmpc_vehicle_params* d_veh;
     int* d_veh_idx;
-    // device lap books (lapbooks.cuh): slot tables of both pools, lap history, exchange scratch
+    // device lap books (lapbooks.cuh, allocated with the store): slot tables of both pools, lap history, exchange scratch
     LapBooks bk;
-    int *d_bkbuf, *d_poolidx, *d_stats;
-    bool has_books;
+    int *d_poolidx, *d_stats;
     // pool groups of the exchange (lmpc_set_pool_groups): group index [batch] and its host mirror; null / 0 = one pool
     int* d_pool_grp;
     int ngroups;
@@ -118,9 +146,116 @@ struct lmpc_handle {
     TraceBufs tr;
     int* d_trinst;
     bool has_trace;
-    // controller snapshots (snapshot.cuh): header template [SNAP_HDR_WORDS] + check verdict [4], allocated on first use
+    // controller snapshots (snapshot.cuh): header template [SNAP_HDR_WORDS] + check verdict [4], allocated with the store
     int* d_snap;
 };
+
+// The handle's device buffers outside the QP buffer sets.  A buffer is [rows][B][per] elements (rows == 0: `per` elements for
+// the whole handle), B being the batch, or the number of traced controllers for the trace.
+enum BufOwner : unsigned { OWN_HANDLE = 1, OWN_STORE = 2, OWN_WARM = 4, OWN_ROLLOUT = 8, OWN_TRACE = 16, OWN_QP = 32 };
+enum BufFill { FILL_NONE, FILL_ZERO, FILL_ONES };      // FILL_ONES: every int -1 (a free slot, no previous lap)
+constexpr int SN_SCRATCH = -1;
+struct DevBuf {
+    void** p;             // the typed handle member it fills
+    size_t elem, per;
+    int rows;
+    BufOwner own;         // what creates and frees it (OWN_WARM: the store, with lmpc_params.warm_start)
+    BufFill fill;
+    int sect;             // snapshot section of row 0 (row k: sect + k), or SN_SCRATCH
+    const char* name;     // lmpc_device_buffer name, or null
+    size_t bytes(size_t B) const { return elem * per * (rows ? rows * B : 1); }
+};
+template <typename T>
+static DevBuf dbuf(T*& p, size_t per, BufOwner own, BufFill fill = FILL_NONE, int sect = SN_SCRATCH, const char* name = nullptr,
+                   int rows = 1) {
+    return DevBuf{(void**)&p, sizeof(T), per, rows, own, fill, sect, name};
+}
+
+// Every such buffer, sized from the handle's current dimensions.  Allocation, initial fill, release, the snapshot sections and
+// the names of lmpc_device_buffer come from this table, so a new buffer gets a row here and nowhere else; every per-controller
+// buffer is a snapshot section or per-step scratch (DESIGN.md, "Controller snapshots").
+static std::vector<DevBuf> dev_bufs(lmpc_handle* h) {
+    const size_t N = h->N, np = (N + 1) * 6, sc = h->ss.cap, mc = h->mdl.cap, T = h->ss.Tmax, nit = h->bk.numSS_it;
+    const size_t Tcl = h->Tcl, cap = h->tr.cap, Mx = h->M > 0 ? h->M : 1;
+    const BufOwner S = OWN_STORE, R = OWN_ROLLOUT, X = OWN_TRACE;
+    LapBooks& k = h->bk;
+    const int cur = h->cur, oth = h->cur ^ 1;
+    return {
+        dbuf(h->d_late, 1, OWN_HANDLE, FILL_ZERO, SN_SCRATCH, nullptr, 0),
+        // lap pools, lap books, controller state
+        dbuf(h->ss.x, sc * T * 6, S, FILL_NONE, SN_SS_X), dbuf(h->ss.u, sc * T * 2, S, FILL_NONE, SN_SS_U),
+        dbuf(h->ss.q, sc * T, S, FILL_NONE, SN_SS_Q), dbuf(h->ss.len, sc, S, FILL_ZERO, SN_SS_LEN),
+        dbuf(h->mdl.x, mc * T * 6, S, FILL_NONE, SN_MD_X), dbuf(h->mdl.u, mc * T * 2, S, FILL_NONE, SN_MD_U),
+        dbuf(h->mdl.len, mc, S, FILL_ZERO, SN_MD_LEN),
+        dbuf(k.ss_time, sc, S, FILL_ONES, SN_SS_TIME), dbuf(k.ss_lap, sc, S, FILL_ONES, SN_SS_LAP), dbuf(k.it, 1, S, FILL_ZERO, SN_IT),
+        dbuf(k.md_time, mc, S, FILL_ONES, SN_MD_TIME), dbuf(k.md_seq, mc, S, FILL_ONES, SN_MD_SEQ),
+        dbuf(k.md_cnt, 1, S, FILL_ZERO, SN_MD_CNT), dbuf(k.lap_hist, LAP_HIST, S, FILL_ONES, SN_LAP_HIST),
+        dbuf(k.lap_n, 1, S, FILL_ZERO, SN_LAP_N),
+        dbuf(h->d_sel, nit, S, FILL_ZERO, SN_SEL), dbuf(h->d_isprev, nit, S, FILL_ZERO, SN_ISPREV),
+        dbuf(h->d_prevslot, 1, S, FILL_ONES, SN_PREVSLOT), dbuf(h->d_used, k.trToUse, S, FILL_ZERO, SN_USED),
+        dbuf(h->d_xLin, np, S, FILL_NONE, SN_XLIN, "xLin"), dbuf(h->d_uLin, N * 2, S, FILL_NONE, SN_ULIN, "uLin"),
+        dbuf(h->d_ztState, 6, S, FILL_ZERO, SN_ZT), dbuf(h->d_OldInput, 2, S, FILL_ZERO, SN_OLDINPUT, "OldInput"),
+        dbuf(h->d_xPredPrev, np, S, FILL_ZERO, SN_XPREDPREV), dbuf(h->d_timeStep, 1, S, FILL_ZERO, SN_TIMESTEP),
+        dbuf(h->d_hasPred, 1, S, FILL_ZERO, SN_HASPRED),
+        dbuf(h->d_warm, (size_t)h->warm_stride, OWN_WARM, FILL_NONE, SN_WARM),
+        dbuf(h->d_warm_valid, 1, OWN_WARM, FILL_ZERO, SN_WARM_VALID),
+        // store scratch: flags (cleared by every step), K2 outputs nothing reads later, staging of host arrays, exchange scratch
+        dbuf(h->d_flags, 1, S, FILL_ZERO, SN_SCRATCH, "flags"), dbuf(h->d_minidx, nit, S), dbuf(h->d_ztFixed, 6, S),
+        dbuf(h->d_tmpx, 6, S), dbuf(h->d_tmpu, 2, S), dbuf(h->d_xchg, 3, S),
+        dbuf(h->d_dropped, 1, S, FILL_ZERO, SN_SCRATCH, nullptr, 0), dbuf(h->d_poolidx, POOL_SCRATCH, S, FILL_NONE, SN_SCRATCH, nullptr, 0),
+        dbuf(h->d_stats, POOL_MAXG * 4, S, FILL_NONE, SN_SCRATCH, nullptr, 0),
+        dbuf(h->d_snap, SNAP_HDR_WORDS + 4, S, FILL_NONE, SN_SCRATCH, nullptr, 0),
+        // closed loop: the simulator's double buffer (the half at cur is the state, the other half is written before it is read)
+        dbuf(h->d_rx[cur], 6, R, FILL_NONE, SN_RX), dbuf(h->d_rg[cur], 6, R, FILL_NONE, SN_RG), dbuf(h->d_rx[oth], 6, R),
+        dbuf(h->d_rg[oth], 6, R), dbuf(h->d_clx, Tcl * 6, R, FILL_NONE, SN_CLX), dbuf(h->d_clu, Tcl * 2, R, FILL_NONE, SN_CLU),
+        dbuf(h->d_cllen, 1, R, FILL_ZERO, SN_CLLEN), dbuf(h->d_done, 1, R, FILL_ZERO, SN_DONE),
+        dbuf(h->d_health, 1, R, FILL_ZERO, SN_HEALTH_FLAGS, nullptr, 2),       // [2][B]: flags, then unsolved steps
+        dbuf(h->d_abc_lti, 54, R, FILL_ZERO, SN_ABC_LTI, "abc_lti"), dbuf(h->d_z, 3, R), dbuf(h->d_zpid, 2, R),
+        // trace of chosen controllers (per traced controller)
+        dbuf(h->d_trinst, 1, X), dbuf(h->tr.steps, 1, X, FILL_ZERO), dbuf(h->tr.x, cap * 6, X), dbuf(h->tr.g, cap * 6, X),
+        dbuf(h->tr.u, cap * 2, X), dbuf(h->tr.xPred, cap * np, X), dbuf(h->tr.ss, cap * 6 * Mx, X), dbuf(h->tr.lap, cap, X)};
+}
+
+template <typename T>
+static void free_null(T*& p) { if (p) cudaFree(p); p = nullptr; }
+
+static void free_bufs(const std::vector<DevBuf>& rows, unsigned owners) {
+    for (const DevBuf& r : rows) if (r.own & owners) free_null(*r.p);
+}
+
+// Allocate the buffers of `rows` that belong to `owners` (all null on entry) for nb controllers and give them their initial
+// fill.  On a failure every one of them is freed again, so nothing is left allocated and the call can be retried.
+static int alloc_bufs(lmpc_handle* h, const std::vector<DevBuf>& rows, unsigned owners, size_t nb, const char* who) {
+    cudaError_t e = cudaSuccess;
+    bool filled = false;
+    for (const DevBuf& r : rows) {
+        if (!(r.own & owners) || e != cudaSuccess) continue;
+        e = cudaMalloc(r.p, r.bytes(nb));
+        if (e == cudaSuccess && r.fill != FILL_NONE) {
+            e = cudaMemsetAsync(*r.p, r.fill == FILL_ONES ? 0xff : 0, r.bytes(nb), h->stream);
+            filled = true;
+        }
+    }
+    if (e == cudaSuccess && filled) e = cudaStreamSynchronize(h->stream);
+    if (e == cudaSuccess) return LMPC_OK;
+    free_bufs(rows, owners);
+    return fail(LMPC_E_CUDA, std::string(who) + ": device allocation: " + cudaGetErrorString(e));
+}
+
+// Whole-buffer copies between handle buffers (rows of dev_bufs, sized by the table) and the caller's arrays, on the handle's
+// stream: pairs (handle buffer, caller's array); a null array is skipped
+static int copy_bufs(lmpc_handle* h, cudaMemcpyKind kind, std::initializer_list<std::pair<void*, const void*>> pairs) {
+    const std::vector<DevBuf> rows = dev_bufs(h);
+    for (const auto& pr : pairs) {
+        if (!pr.second) continue;
+        size_t n = 0;
+        for (const DevBuf& r : rows) if (*r.p == pr.first) n = r.bytes(h->batch);
+        void* host = const_cast<void*>(pr.second);
+        if (kind == cudaMemcpyHostToDevice) CK(cudaMemcpyAsync(pr.first, host, n, kind, h->stream));
+        else CK(cudaMemcpyAsync(host, pr.first, n, kind, h->stream));
+    }
+    return LMPC_OK;
+}
 
 static bool inv6(const double* A, double* Ai) {
     double m[6][12];
@@ -268,88 +403,67 @@ static int configure(int N, int M) {
     return LMPC_OK;
 }
 
-template <typename T>
-static void free_null(T*& p) { if (p) cudaFree(p); p = nullptr; }
-
 static void free_store(lmpc_handle* h) {
-    free_null(h->ss.x); free_null(h->ss.u); free_null(h->ss.q); free_null(h->ss.len);
-    free_null(h->mdl.x); free_null(h->mdl.u); free_null(h->mdl.len);
-    free_null(h->d_used); free_null(h->d_sel); free_null(h->d_isprev); free_null(h->d_prevslot); free_null(h->d_timeStep);
-    free_null(h->d_hasPred); free_null(h->d_flags); free_null(h->d_minidx); free_null(h->d_xLin); free_null(h->d_uLin);
-    free_null(h->d_ztState); free_null(h->d_ztFixed); free_null(h->d_OldInput); free_null(h->d_xPredPrev); free_null(h->d_tmpx);
-    free_null(h->d_tmpu); free_null(h->d_xchg); free_null(h->d_dropped);
-    free_null(h->d_bkbuf); free_null(h->d_poolidx); free_null(h->d_stats); free_null(h->d_snap);
-    free_null(h->d_warm); free_null(h->d_warm_valid);
+    free_bufs(dev_bufs(h), OWN_STORE | OWN_WARM);
     free_null(h->d_trk); free_null(h->d_trk_idx);
     h->trk_host.clear(); h->trk_idx_host.clear();
     free_null(h->d_pool_grp);
     h->ngroups = 0;
     h->pool_grp_host.clear();
     h->laps_stored = false;
-    h->has_books = false;
     h->has_store = false;
 }
 
 static Tracks tracks(const lmpc_handle* h) { return Tracks{h->d_trk, h->d_trk_idx}; }
 
 static void free_rollout(lmpc_handle* h) {
-    for (int i = 0; i < 2; ++i) { free_null(h->d_rx[i]); free_null(h->d_rg[i]); }
-    free_null(h->d_clx); free_null(h->d_clu); free_null(h->d_z); free_null(h->d_zpid); free_null(h->d_abc_lti);
-    free_null(h->d_cllen); free_null(h->d_done); free_null(h->d_health);
-    free_null(h->d_trinst); free_null(h->tr.steps); free_null(h->tr.x); free_null(h->tr.g); free_null(h->tr.u); free_null(h->tr.xPred);
-    free_null(h->tr.ss); free_null(h->tr.lap);
+    free_bufs(dev_bufs(h), OWN_ROLLOUT | OWN_TRACE);
     h->has_trace = false;
     h->has_rollout = false;
 }
 
-static void free_qp_bufs(QpBufs& q) {
-    free_null(q.x0); free_null(q.uOld); free_null(q.abc); free_null(q.SS); free_null(q.Qfun); free_null(q.SuccSS); free_null(q.SuccU);
-    free_null(q.xPred); free_null(q.uPred); free_null(q.slack); free_null(q.lambd); free_null(q.slackT); free_null(q.zt); free_null(q.ztu);
-    free_null(q.resid); free_null(q.status); free_null(q.iters);
+// The rows of QP buffer set q: every field of QP_FIELDS for the whole batch
+static std::vector<DevBuf> qp_rows(const lmpc_handle* h, QpIo& q) {
+    std::vector<DevBuf> rows;
+    for (const QpField& f : QP_FIELDS)
+        rows.push_back(DevBuf{&f.at(q), f.elem, f.count(h->N, h->M > 0 ? h->M : 1), 1, OWN_QP, FILL_NONE, SN_SCRATCH, nullptr});
+    return rows;
 }
 
 // Buffer set `slot` of the handle, allocated on first use (x0 != null: allocated); null (and g_err set) if the allocation failed,
 // which leaves nothing behind
-static QpBufs* qp_bufs(lmpc_handle* h, int slot) {
-    QpBufs& q = h->hb[slot];
-    if (!q.x0) {
-        const size_t B = h->batch, N = h->N, M = h->M > 0 ? h->M : 1;
-        cudaError_t e = cudaSuccess;
-        auto alloc = [&](auto*& p, size_t count) { if (e == cudaSuccess) e = cudaMalloc((void**)&p, sizeof(*p) * count); };
-        alloc(q.x0, B * 6); alloc(q.uOld, B * 2); alloc(q.abc, B * N * 54);
-        alloc(q.SS, B * 6 * M); alloc(q.Qfun, B * M); alloc(q.SuccSS, B * 6 * M); alloc(q.SuccU, B * 2 * M);
-        alloc(q.xPred, B * (N + 1) * 6); alloc(q.uPred, B * N * 2); alloc(q.slack, B * N * 2);
-        alloc(q.lambd, B * M); alloc(q.slackT, B * 6); alloc(q.zt, B * 6); alloc(q.ztu, B * 2);
-        alloc(q.resid, B * 3); alloc(q.status, B); alloc(q.iters, B);
-        if (e != cudaSuccess) {
-            free_qp_bufs(q);
-            fail(LMPC_E_CUDA, std::string("cudaMalloc of QP buffer set ") + std::to_string(slot) + ": " + cudaGetErrorString(e));
-            return nullptr;
-        }
-    }
+static QpIo* qp_bufs(lmpc_handle* h, int slot) {
+    QpIo& q = h->hb[slot];
+    if (!q.x0 && alloc_bufs(h, qp_rows(h, q), OWN_QP, h->batch, ("QP buffer set " + std::to_string(slot)).c_str()) != LMPC_OK)
+        return nullptr;
     return &q;
 }
 
-// which of the QP kernel's optional inputs and outputs a caller wants (qp_args); the safe-set ones only count on LMPC-type QPs
-enum : unsigned { QP_SUCC_SS = 1, QP_SUCC_U = 2, QP_SLACK = 4, QP_LAMBD = 8, QP_SLACKT = 16, QP_ZT = 32, QP_ZTU = 64, QP_ALL = 127 };
-
-// Kernel arguments for the whole batch held in q (per-instance model, strides (N*54, 54)); what the caller does not want stays null,
-// which the kernel skips
-static FtocpArgs qp_args(const lmpc_handle* h, const QpBufs& q, bool lm, unsigned want) {
-    if (!lm) want &= QP_SLACK;
+// Kernel arguments for the whole batch held in q (per-instance model, strides (N*54, 54)); null fields, and the safe-set ones of
+// an MPC-type QP, stay null, which the kernel skips
+static FtocpArgs qp_args(const lmpc_handle* h, const QpIo& q, bool lm) {
     FtocpArgs a = {};
     a.batch = h->batch;
     a.x0 = q.x0; a.uOld = q.uOld; a.abc = q.abc;
     a.abc_inst_stride = (long long)h->N * 54; a.abc_stage_stride = 54;
-    a.SS = lm ? q.SS : nullptr; a.Qfun = lm ? q.Qfun : nullptr;
-    a.SuccSS = (want & QP_SUCC_SS) ? q.SuccSS : nullptr; a.SuccU = (want & QP_SUCC_U) ? q.SuccU : nullptr;
-    a.xPred = q.xPred; a.uPred = q.uPred; a.slack = (want & QP_SLACK) ? q.slack : nullptr;
-    a.lambd = (want & QP_LAMBD) ? q.lambd : nullptr; a.slackT = (want & QP_SLACKT) ? q.slackT : nullptr;
-    a.zt = (want & QP_ZT) ? q.zt : nullptr; a.ztu = (want & QP_ZTU) ? q.ztu : nullptr;
+    a.xPred = q.xPred; a.uPred = q.uPred; a.slack = q.slack;
+    if (lm) {
+        a.SS = q.SS; a.Qfun = q.Qfun; a.SuccSS = q.SuccSS; a.SuccU = q.SuccU;
+        a.lambd = q.lambd; a.slackT = q.slackT; a.zt = q.zt; a.ztu = q.ztu;
+    }
     a.status = q.status; a.iters = q.iters; a.resid = q.resid;
     a.late = h->d_late;
     a.set_idx = h->d_set_idx;
     return a;
+}
+
+// Copy the fields of buffer set 0 that dst names (the safe-set ones only when lm) into the caller's arrays, on the handle's stream
+static int copy_out(lmpc_handle* h, const QpIo& dst, bool lm) {
+    const size_t B = h->batch, N = h->N, M = h->M > 0 ? h->M : 1;
+    for (const QpField& f : QP_FIELDS)
+        if (f.at(dst) && (lm || !f.lmpc_only))
+            CK(cudaMemcpyAsync(f.at(dst), f.at(h->hb[0]), B * f.count(N, M) * f.elem, cudaMemcpyDeviceToHost, h->stream));
+    return LMPC_OK;
 }
 
 static int create_device_side(lmpc_handle* h) {
@@ -359,8 +473,7 @@ static int create_device_side(lmpc_handle* h) {
     CK(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
     for (int i = 0; i < 4 * LMPC_HOST_SLOTS; ++i) CK(cudaStreamCreateWithFlags(&h->cstream[i], cudaStreamNonBlocking));
     if (!qp_bufs(h, 0)) return LMPC_E_CUDA;
-    CK(cudaMalloc((void**)&h->d_late, sizeof(unsigned long long)));
-    CK(cudaMemset(h->d_late, 0, sizeof(unsigned long long)));
+    if ((rc = alloc_bufs(h, dev_bufs(h), OWN_HANDLE, 1, "lmpc_create")) != LMPC_OK) return rc;
     const lmpc_vehicle_params ref = reference_vehicle();
     return swap_table(h, "lmpc_create", &ref, 1, nullptr, &h->d_veh, &h->d_veh_idx);
 }
@@ -505,8 +618,8 @@ int lmpc_destroy(lmpc_handle* h) {
     // every pointer freed here is either a live allocation or still null (handle memory is zero-initialised)
     free_rollout(h);
     free_store(h);
-    for (QpBufs& q : h->hb) free_qp_bufs(q);
-    cudaFree(h->d_late);
+    free_bufs(dev_bufs(h), OWN_HANDLE);
+    for (QpIo& q : h->hb) free_bufs(qp_rows(h, q), OWN_QP);
     cudaFree(h->d_sets);
     cudaFree(h->d_set_idx);
     cudaFree(h->d_veh);
@@ -578,16 +691,10 @@ int lmpc_solve_lmpc_dev(lmpc_handle* h, const double* x0, const double* uOld, co
     if ((rc = check_align(abc, "abc")) != LMPC_OK) return rc;
     if (lm && ((rc = check_align(SS_sel, "SS_sel")) != LMPC_OK || (rc = check_align(Qfun_sel, "Qfun_sel")) != LMPC_OK)) return rc;
     CK(cudaSetDevice(h->device));
-    FtocpArgs a = {};   // no warm-start records: caller-supplied QPs start cold; the controllers of the device-resident step
-                        // carry warm-start records (step_dev_impl)
-    a.batch = h->batch;
-    a.x0 = x0; a.uOld = uOld; a.abc = abc;
+    // no warm-start records: caller-supplied QPs start cold; the controllers of the device-resident step carry warm-start
+    // records (step_dev_impl)
+    FtocpArgs a = qp_args(h, CALLER_QP_IO, lm);
     a.abc_inst_stride = abc_inst_stride; a.abc_stage_stride = abc_stage_stride;
-    a.SS = SS_sel; a.Qfun = Qfun_sel; a.SuccSS = Succ_SS; a.SuccU = Succ_uSS;
-    a.xPred = xPred; a.uPred = uPred; a.slack = slack; a.lambd = lambd; a.slackT = slackTerminal;
-    a.zt = zt; a.ztu = zt_u; a.status = status; a.iters = iters; a.resid = resid;
-    a.late = h->d_late;
-    a.set_idx = h->d_set_idx;
     return launch(h, a, lm, h->stream);
 }
 
@@ -598,22 +705,22 @@ int lmpc_solve_mpc_dev(lmpc_handle* h, const double* x0, const double* uOld, con
                                uPred, slack, nullptr, nullptr, nullptr, nullptr, status, iters, resid);
 }
 
-// Enqueue one host-buffer solve on buffer set / stream group `slot` (0 .. LMPC_HOST_SLOTS - 1) WITHOUT waiting for it.
-static int enqueue_host_solve_impl(lmpc_handle* h, int slot, const double* x0, const double* uOld, const double* abc,
-                              long long abc_inst_stride, long long abc_stage_stride, const double* SS_sel, const double* Qfun_sel,
-                              const double* Succ_SS, const double* Succ_uSS, double* xPred, double* uPred, double* slack,
-                              double* lambd, double* slackTerminal, double* zt, double* zt_u, int* status, int* iters,
-                              double* resid) {
-    if (!h || !x0 || !uOld || !abc || !xPred || !uPred || !status || !iters || !resid) return fail(LMPC_E_INVALID, "null argument");
-    const bool lm = (SS_sel != nullptr);
-    if (lm && (h->M <= 0 || !Qfun_sel)) return fail(LMPC_E_INVALID, "handle was created without a safe set (numSS_Points == 0)");
+}  // extern "C" (the helpers below have C++ linkage)
+
+// Enqueue one host-buffer solve of the caller's arrays io on buffer set / stream group `slot` (0 .. LMPC_HOST_SLOTS - 1)
+// WITHOUT waiting for it.
+static int enqueue_host_solve_impl(lmpc_handle* h, int slot, const QpIo& io, long long abc_inst_stride, long long abc_stage_stride) {
+    if (!h || !io.x0 || !io.uOld || !io.abc || !io.xPred || !io.uPred || !io.status || !io.iters || !io.resid)
+        return fail(LMPC_E_INVALID, "null argument");
+    const bool lm = (io.SS != nullptr);
+    if (lm && (h->M <= 0 || !io.Qfun)) return fail(LMPC_E_INVALID, "handle was created without a safe set (numSS_Points == 0)");
     if (slot < 0 || slot >= LMPC_HOST_SLOTS) return fail(LMPC_E_INVALID, "slot must be 0 .. 3");
     CK(cudaSetDevice(h->device));
     const size_t B = h->batch, N = h->N, M = h->M > 0 ? h->M : 1;
     const size_t D = sizeof(double);
-    const QpBufs* q = qp_bufs(h, slot);
+    const QpIo* q = qp_bufs(h, slot);
     if (!q) return LMPC_E_CUDA;
-    const QpBufs& hb = *q;
+    const QpIo& hb = *q;
     cudaStream_t* cs = h->cstream + 4 * slot;
     long long dis, dss;
     bool per_inst = false;
@@ -623,7 +730,7 @@ static int enqueue_host_solve_impl(lmpc_handle* h, int slot, const double* x0, c
     else return fail(LMPC_E_INVALID, "host entry supports abc strides (N*54,54), (0,54) or (0,0)");
     CK(cudaStreamSynchronize(h->stream));    // earlier work of this handle is done before the chunk streams start
     if (!per_inst) {
-        CK(cudaMemcpyAsync(hb.abc, abc, (dss ? N * 54 : 54) * D, cudaMemcpyHostToDevice, cs[0]));
+        CK(cudaMemcpyAsync(hb.abc, io.abc, (dss ? N * 54 : 54) * D, cudaMemcpyHostToDevice, cs[0]));
         CK(cudaStreamSynchronize(cs[0]));
     }
     // Chunk pipeline: the batch is cut into up to four instance ranges, each on its own stream, so that the H2D copy
@@ -637,50 +744,40 @@ static int enqueue_host_solve_impl(lmpc_handle* h, int slot, const double* x0, c
     for (int sl = 0; sl < LMPC_HOST_SLOTS; ++sl) others |= (sl != slot && h->hb_pending[sl]);
     const bool lone = h->hb_lone && !others;
     const int nchunk = B >= 2048 ? (lone ? 4 : (others ? 1 : 2)) : (B >= 512 ? (others ? 1 : 2) : 1);
-    FtocpArgs all = qp_args(h, hb, lm, (Succ_SS ? QP_SUCC_SS : 0) | (Succ_uSS ? QP_SUCC_U : 0) | (slack ? QP_SLACK : 0) |
-                                       (lambd ? QP_LAMBD : 0) | (slackTerminal ? QP_SLACKT : 0) | (zt ? QP_ZT : 0) |
-                                       (zt_u ? QP_ZTU : 0));
+    // what moves: the fields the caller passes (zt and zt_u are only computed with their successor points) and, per chunk, abc
+    // only when every instance has its own model
+    QpIo c = io, dev = hb;
+    if (!c.SuccSS) c.zt = nullptr;
+    if (!c.SuccU) c.ztu = nullptr;
+    for (const QpField& f : QP_FIELDS) if (!f.at(c)) f.at(dev) = nullptr;
+    FtocpArgs all = qp_args(h, dev, lm);
     all.abc_inst_stride = dis; all.abc_stage_stride = dss;
+    if (!per_inst) c.abc = nullptr;
     for (int ci = 0; ci < nchunk; ++ci) {
         const size_t lo = B * ci / nchunk, hi = B * (ci + 1) / nchunk, nb = hi - lo;
         cudaStream_t s = cs[ci];
-        CK(cudaMemcpyAsync(hb.x0 + lo * 6, x0 + lo * 6, nb * 6 * D, cudaMemcpyHostToDevice, s));
-        CK(cudaMemcpyAsync(hb.uOld + lo * 2, uOld + lo * 2, nb * 2 * D, cudaMemcpyHostToDevice, s));
-        if (per_inst) CK(cudaMemcpyAsync(hb.abc + lo * N * 54, abc + lo * N * 54, nb * N * 54 * D, cudaMemcpyHostToDevice, s));
-        if (lm) {
-            CK(cudaMemcpyAsync(hb.SS + lo * 6 * M, SS_sel + lo * 6 * M, nb * 6 * M * D, cudaMemcpyHostToDevice, s));
-            CK(cudaMemcpyAsync(hb.Qfun + lo * M, Qfun_sel + lo * M, nb * M * D, cudaMemcpyHostToDevice, s));
-            if (Succ_SS) CK(cudaMemcpyAsync(hb.SuccSS + lo * 6 * M, Succ_SS + lo * 6 * M, nb * 6 * M * D, cudaMemcpyHostToDevice, s));
-            if (Succ_uSS) CK(cudaMemcpyAsync(hb.SuccU + lo * 2 * M, Succ_uSS + lo * 2 * M, nb * 2 * M * D, cudaMemcpyHostToDevice, s));
-        }
+        for (const QpField& f : QP_FIELDS)
+            if (f.in && f.at(c) && (lm || !f.lmpc_only)) {
+                const size_t n = f.count(N, M) * f.elem;
+                CK(cudaMemcpyAsync((char*)f.at(hb) + lo * n, (const char*)f.at(c) + lo * n, nb * n, cudaMemcpyHostToDevice, s));
+            }
         int rc = launch(h, all.range((int)lo, (int)nb, (int)N, h->M), lm, s);
         if (rc != LMPC_OK) return rc;
-        CK(cudaMemcpyAsync(xPred + lo * (N + 1) * 6, hb.xPred + lo * (N + 1) * 6, nb * (N + 1) * 6 * D, cudaMemcpyDeviceToHost, s));
-        CK(cudaMemcpyAsync(uPred + lo * N * 2, hb.uPred + lo * N * 2, nb * N * 2 * D, cudaMemcpyDeviceToHost, s));
-        if (slack) CK(cudaMemcpyAsync(slack + lo * N * 2, hb.slack + lo * N * 2, nb * N * 2 * D, cudaMemcpyDeviceToHost, s));
-        if (lm && lambd) CK(cudaMemcpyAsync(lambd + lo * M, hb.lambd + lo * M, nb * M * D, cudaMemcpyDeviceToHost, s));
-        if (lm && slackTerminal) CK(cudaMemcpyAsync(slackTerminal + lo * 6, hb.slackT + lo * 6, nb * 6 * D, cudaMemcpyDeviceToHost, s));
-        if (lm && zt && Succ_SS) CK(cudaMemcpyAsync(zt + lo * 6, hb.zt + lo * 6, nb * 6 * D, cudaMemcpyDeviceToHost, s));
-        if (lm && zt_u && Succ_uSS) CK(cudaMemcpyAsync(zt_u + lo * 2, hb.ztu + lo * 2, nb * 2 * D, cudaMemcpyDeviceToHost, s));
-        CK(cudaMemcpyAsync(status + lo, hb.status + lo, nb * sizeof(int), cudaMemcpyDeviceToHost, s));
-        CK(cudaMemcpyAsync(iters + lo, hb.iters + lo, nb * sizeof(int), cudaMemcpyDeviceToHost, s));
-        CK(cudaMemcpyAsync(resid + lo * 3, hb.resid + lo * 3, nb * 3 * D, cudaMemcpyDeviceToHost, s));
+        for (const QpField& f : QP_FIELDS)
+            if (!f.in && f.at(c) && (lm || !f.lmpc_only)) {
+                const size_t n = f.count(N, M) * f.elem;
+                CK(cudaMemcpyAsync((char*)f.at(c) + lo * n, (const char*)f.at(hb) + lo * n, nb * n, cudaMemcpyDeviceToHost, s));
+            }
     }
     h->hb_chunks[slot] = nchunk;
     h->hb_pending[slot] = true;
     return LMPC_OK;
 }
 
-
 // Enqueue one host-buffer solve; on ANY failure part-way through, the chunks already enqueued are still copying into the
 // caller's arrays, so their streams are drained before the error is reported.
-static int enqueue_host_solve(lmpc_handle* h, int slot, const double* x0, const double* uOld, const double* abc,
-                              long long abc_inst_stride, long long abc_stage_stride, const double* SS_sel, const double* Qfun_sel,
-                              const double* Succ_SS, const double* Succ_uSS, double* xPred, double* uPred, double* slack,
-                              double* lambd, double* slackTerminal, double* zt, double* zt_u, int* status, int* iters,
-                              double* resid) {
-    const int rc = enqueue_host_solve_impl(h, slot, x0, uOld, abc, abc_inst_stride, abc_stage_stride, SS_sel, Qfun_sel, Succ_SS, Succ_uSS,
-                                           xPred, uPred, slack, lambd, slackTerminal, zt, zt_u, status, iters, resid);
+static int enqueue_host_solve(lmpc_handle* h, int slot, const QpIo& io, long long abc_inst_stride, long long abc_stage_stride) {
+    const int rc = enqueue_host_solve_impl(h, slot, io, abc_inst_stride, abc_stage_stride);
     if (rc != LMPC_OK && h && slot >= 0 && slot < LMPC_HOST_SLOTS) {
         const std::string msg = g_err;
         for (int i = 0; i < 4; ++i) cudaStreamSynchronize(h->cstream[4 * slot + i]);
@@ -689,6 +786,7 @@ static int enqueue_host_solve(lmpc_handle* h, int slot, const double* x0, const 
     return rc;
 }
 
+extern "C" {
 
 /* Instance ranges the most recent enqueue on `slot` was cut into (diagnostics of the chunk policy); -1 on a bad argument. */
 int lmpc_host_chunks(lmpc_handle* h, int slot) {
@@ -709,15 +807,14 @@ int lmpc_solve_lmpc_host_async(lmpc_handle* h, int slot, const double* x0, const
                                long long abc_stage_stride, const double* SS_sel, const double* Qfun_sel, const double* Succ_SS,
                                const double* Succ_uSS, double* xPred, double* uPred, double* slack, double* lambd,
                                double* slackTerminal, double* zt, double* zt_u, int* status, int* iters, double* resid) {
-    return enqueue_host_solve(h, slot, x0, uOld, abc, abc_inst_stride, abc_stage_stride, SS_sel, Qfun_sel, Succ_SS, Succ_uSS, xPred, uPred,
-                              slack, lambd, slackTerminal, zt, zt_u, status, iters, resid);
+    return enqueue_host_solve(h, slot, CALLER_QP_IO, abc_inst_stride, abc_stage_stride);
 }
 
 int lmpc_solve_mpc_host_async(lmpc_handle* h, int slot, const double* x0, const double* uOld, const double* abc, long long abc_inst_stride,
                               long long abc_stage_stride, double* xPred, double* uPred, double* slack, int* status, int* iters,
                               double* resid) {
-    return enqueue_host_solve(h, slot, x0, uOld, abc, abc_inst_stride, abc_stage_stride, nullptr, nullptr, nullptr, nullptr, xPred, uPred,
-                              slack, nullptr, nullptr, nullptr, nullptr, status, iters, resid);
+    return lmpc_solve_lmpc_host_async(h, slot, x0, uOld, abc, abc_inst_stride, abc_stage_stride, nullptr, nullptr, nullptr, nullptr,
+                                      xPred, uPred, slack, nullptr, nullptr, nullptr, nullptr, status, iters, resid);
 }
 
 int lmpc_solve_lmpc_host(lmpc_handle* h, const double* x0, const double* uOld, const double* abc, long long abc_inst_stride,
@@ -725,8 +822,7 @@ int lmpc_solve_lmpc_host(lmpc_handle* h, const double* x0, const double* uOld, c
                          const double* Succ_uSS, double* xPred, double* uPred, double* slack, double* lambd,
                          double* slackTerminal, double* zt, double* zt_u, int* status, int* iters, double* resid) {
     if (h) h->hb_lone = true;
-    int rc = enqueue_host_solve(h, 0, x0, uOld, abc, abc_inst_stride, abc_stage_stride, SS_sel, Qfun_sel, Succ_SS, Succ_uSS, xPred, uPred,
-                                slack, lambd, slackTerminal, zt, zt_u, status, iters, resid);
+    int rc = enqueue_host_solve(h, 0, CALLER_QP_IO, abc_inst_stride, abc_stage_stride);
     if (h) h->hb_lone = false;
     if (rc) return rc;
     return lmpc_host_wait(h, 0);
@@ -783,70 +879,29 @@ static int store_create_impl(lmpc_handle* h, const lmpc_model_params* mp, int ss
     h->trk_host.assign(1, t);
     h->trk_idx_host.clear();
     h->laps_stored = false;
-    const size_t B = h->batch, N = h->N;
     h->ss.cap = ss_cap > 0 ? ss_cap : 1; h->ss.Tmax = Tmax;
-    h->mdl.cap = model_cap; h->mdl.Tmax = Tmax;
-#define DA(ptr, T, count) CK(cudaMalloc((void**)&(ptr), sizeof(T) * (count)))
-#define DA2(ptr, T, count) CK(cudaMalloc((void**)&(ptr), sizeof(T) * (count)))
-    DA(h->ss.x, double, B * h->ss.cap * Tmax * 6); DA(h->ss.u, double, B * h->ss.cap * Tmax * 2); DA(h->ss.q, double, B * h->ss.cap * Tmax);
-    DA(h->ss.len, int, B * h->ss.cap);
-    DA(h->mdl.x, double, B * model_cap * Tmax * 6); DA(h->mdl.u, double, B * model_cap * Tmax * 2); h->mdl.q = nullptr;
-    DA(h->mdl.len, int, B * model_cap);
-    DA(h->d_used, int, B * K1_MAXLAPS); DA(h->d_sel, int, B * 8); DA(h->d_isprev, int, B * 8); DA(h->d_prevslot, int, B);
-    DA(h->d_timeStep, int, B); DA(h->d_hasPred, int, B); DA(h->d_flags, int, B); DA(h->d_minidx, int, B * 8);
-    DA(h->d_xLin, double, B * (N + 1) * 6); DA(h->d_uLin, double, B * N * 2); DA(h->d_ztState, double, B * 6);
-    DA(h->d_ztFixed, double, B * 6); DA(h->d_OldInput, double, B * 2); DA(h->d_xPredPrev, double, B * (N + 1) * 6);
-    DA(h->d_tmpx, double, B * 6); DA(h->d_tmpu, double, B * 2); DA(h->d_xchg, int, B * 3); DA(h->d_dropped, int, 1);
-#undef DA
-    CK(cudaMemsetAsync(h->d_dropped, 0, sizeof(int), h->stream));
+    h->mdl.cap = model_cap; h->mdl.Tmax = Tmax; h->mdl.q = nullptr;
+    LapBooks& k = h->bk;
+    k.ss_cap = h->ss.cap; k.md_cap = model_cap; k.numSS_it = h->p.numSS_it > 0 ? h->p.numSS_it : 1; k.trToUse = mp->trToUse;
     if (h->p.warm_start) {          // SURVEY §8f rank 2: per-controller interior-point snapshot for the next solve
-        const size_t Mx = h->M > 0 ? h->M : 0;
-        h->warm_stride = (long long)(N * 2 + 4 * N * h->p.ncx + N * h->p.ncu + 2 * Mx + 2);
-        DA2(h->d_warm, double, B * (size_t)h->warm_stride);
-        DA2(h->d_warm_valid, int, B);
-        CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * B, h->stream));
+        const long long N = h->N, Mx = h->M > 0 ? h->M : 0;
+        h->warm_stride = N * 2 + 4 * N * h->p.ncx + N * h->p.ncu + 2 * Mx + 2;
         h->warm_mode = -1;
     }
-    {   // device lap books: one int buffer carved into the slot tables
-        const size_t sc = h->ss.cap, mcp = model_cap;
-        const size_t n = B * (2 * sc + 1 + 2 * mcp + 1 + LAP_HIST + 1);
-        DA2(h->d_bkbuf, int, n);
-        int* p = h->d_bkbuf;
-        LapBooks& k = h->bk;
-        k.ss_time = p; p += B * sc; k.ss_lap = p; p += B * sc; k.it = p; p += B;
-        k.md_time = p; p += B * mcp; k.md_seq = p; p += B * mcp; k.md_cnt = p; p += B;
-        k.lap_hist = p; p += B * LAP_HIST; k.lap_n = p; p += B;
-        k.sel = h->d_sel; k.isprev = h->d_isprev; k.prevslot = h->d_prevslot; k.used = h->d_used;
-        k.ss_cap = (int)sc; k.md_cap = (int)mcp; k.numSS_it = h->p.numSS_it > 0 ? h->p.numSS_it : 1; k.trToUse = mp->trToUse;
-        CK(cudaMemsetAsync(h->d_bkbuf, 0xff, sizeof(int) * n, h->stream));          // every slot free (-1)
-        CK(cudaMemsetAsync(k.it, 0, sizeof(int) * B, h->stream));
-        CK(cudaMemsetAsync(k.md_cnt, 0, sizeof(int) * B, h->stream));
-        CK(cudaMemsetAsync(k.lap_n, 0, sizeof(int) * B, h->stream));
-        DA2(h->d_poolidx, int, POOL_SCRATCH);
-        DA2(h->d_stats, int, POOL_MAXG * 4);          // rollout_stats_kernel: [G][4]
-        h->has_books = true;
-    }
-    CK(cudaMemsetAsync(h->ss.len, 0, sizeof(int) * B * h->ss.cap, h->stream));
-    CK(cudaMemsetAsync(h->mdl.len, 0, sizeof(int) * B * model_cap, h->stream));
-    CK(cudaMemsetAsync(h->d_used, 0, sizeof(int) * B * K1_MAXLAPS, h->stream));
-    CK(cudaMemsetAsync(h->d_sel, 0, sizeof(int) * B * 8, h->stream));
-    CK(cudaMemsetAsync(h->d_isprev, 0, sizeof(int) * B * 8, h->stream));
-    CK(cudaMemsetAsync(h->d_prevslot, 0xff, sizeof(int) * B, h->stream));
-    CK(cudaMemsetAsync(h->d_timeStep, 0, sizeof(int) * B, h->stream));
-    CK(cudaMemsetAsync(h->d_hasPred, 0, sizeof(int) * B, h->stream));
-    CK(cudaMemsetAsync(h->d_flags, 0, sizeof(int) * B, h->stream));
-    CK(cudaMemsetAsync(h->d_OldInput, 0, sizeof(double) * B * 2, h->stream));
-    CK(cudaMemsetAsync(h->d_ztState, 0, sizeof(double) * B * 6, h->stream));
-    CK(cudaMemsetAsync(h->d_xPredPrev, 0, sizeof(double) * B * (N + 1) * 6, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
+    if ((rc = alloc_bufs(h, dev_bufs(h), OWN_STORE | (h->p.warm_start ? OWN_WARM : 0), h->batch, "lmpc_store_create")) != LMPC_OK)
+        return rc;
+    k.sel = h->d_sel; k.isprev = h->d_isprev; k.prevslot = h->d_prevslot; k.used = h->d_used;
     h->has_store = true;
     return LMPC_OK;
 }
 extern "C" {
 
+// The preconditions of an entry point, one line each: the handle has a store (need_store) or a store and a rollout
+// (need_rollout); both then select the handle's device.  The lap books are part of the store.
 static int need_store(lmpc_handle* h) {
     if (!h) return fail(LMPC_E_INVALID, "null handle");
     if (!h->has_store) return fail(LMPC_E_STATE, "call lmpc_store_create first");
+    CK(cudaSetDevice(h->device));
     return LMPC_OK;
 }
 
@@ -945,7 +1000,6 @@ int lmpc_set_tracks(lmpc_handle* h, const lmpc_track_params* sets, int nsets, co
 static int put_lap(lmpc_handle* h, LapPool& pool, int inst, int slot, int T, const double* x, const double* u) {
     if (inst < 0 || inst >= h->batch || slot < 0 || slot >= pool.cap || T < 2 || T > pool.Tmax || !x || !u)
         return fail(LMPC_E_INVALID, "put_lap: bad instance/slot/length");
-    CK(cudaSetDevice(h->device));
     h->laps_stored = true;
     const size_t lap = pool.lap_index(inst, slot);
     CK(cudaMemcpyAsync(pool.x + lap * pool.Tmax * 6, x, sizeof(double) * T * 6, cudaMemcpyHostToDevice, h->stream));
@@ -956,18 +1010,15 @@ static int put_lap(lmpc_handle* h, LapPool& pool, int inst, int slot, int T, con
 }
 
 int lmpc_model_put_lap(lmpc_handle* h, int inst, int slot, int T, const double* x, const double* u) {
-    int rc = need_store(h);
-    if (rc) return rc;
+    if (int rc = need_store(h)) return rc;
     return put_lap(h, h->mdl, inst, slot, T, x, u);
 }
 
 int lmpc_model_set_used(lmpc_handle* h, const int* slots) {
-    int rc = need_store(h);
-    if (rc) return rc;
+    if (int rc = need_store(h)) return rc;
     if (!slots) return fail(LMPC_E_INVALID, "null slots");
     for (size_t i = 0; i < (size_t)h->batch * h->mc.trToUse; ++i)
         if (slots[i] < 0 || slots[i] >= h->mdl.cap) return fail(LMPC_E_INVALID, "model slot out of range");
-    CK(cudaSetDevice(h->device));
     CK(cudaMemcpyAsync(h->d_used, slots, sizeof(int) * h->batch * h->mc.trToUse, cudaMemcpyHostToDevice, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     return LMPC_OK;
@@ -991,15 +1042,13 @@ int lmpc_ss_put_lap(lmpc_handle* h, int inst, int slot, int T, const double* x, 
 }
 
 int lmpc_ss_set_selection(lmpc_handle* h, const int* slots, const int* is_prev, const int* prev_slot) {
-    int rc = need_store(h);
-    if (rc) return rc;
+    if (int rc = need_store(h)) return rc;
     if (!slots || !is_prev || !prev_slot) return fail(LMPC_E_INVALID, "null argument");
     const int nit = h->p.numSS_it;
     for (size_t i = 0; i < (size_t)h->batch * nit; ++i)
         if (slots[i] < 0 || slots[i] >= h->ss.cap) return fail(LMPC_E_INVALID, "safe-set slot out of range");
     for (int b = 0; b < h->batch; ++b)
         if (prev_slot[b] >= h->ss.cap) return fail(LMPC_E_INVALID, "prev_slot out of range");
-    CK(cudaSetDevice(h->device));
     CK(cudaMemcpyAsync(h->d_sel, slots, sizeof(int) * h->batch * nit, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(h->d_isprev, is_prev, sizeof(int) * h->batch * nit, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(h->d_prevslot, prev_slot, sizeof(int) * h->batch, cudaMemcpyHostToDevice, h->stream));
@@ -1008,10 +1057,8 @@ int lmpc_ss_set_selection(lmpc_handle* h, const int* slots, const int* is_prev, 
 }
 
 int lmpc_ss_add_point(lmpc_handle* h, const double* x, const double* u) {
-    int rc = need_store(h);
-    if (rc) return rc;
+    if (int rc = need_store(h)) return rc;
     if (!x || !u) return fail(LMPC_E_INVALID, "null argument");
-    CK(cudaSetDevice(h->device));
     CK(cudaMemcpyAsync(h->d_tmpx, x, sizeof(double) * h->batch * 6, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(h->d_tmpu, u, sizeof(double) * h->batch * 2, cudaMemcpyHostToDevice, h->stream));
     ss_add_point_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->batch, h->ss, h->d_prevslot, h->d_tmpx, h->d_tmpu, 2,
@@ -1029,10 +1076,8 @@ int lmpc_ss_add_point(lmpc_handle* h, const double* x, const double* u) {
 }
 
 int lmpc_ss_get_lap(lmpc_handle* h, int inst, int slot, int* T, double* x, double* u, double* qfun) {
-    int rc = need_store(h);
-    if (rc) return rc;
+    if (int rc = need_store(h)) return rc;
     if (inst < 0 || inst >= h->batch || slot < 0 || slot >= h->ss.cap || !T) return fail(LMPC_E_INVALID, "bad instance/slot");
-    CK(cudaSetDevice(h->device));
     const size_t lap = h->ss.lap_index(inst, slot);
     CK(cudaMemcpyAsync(T, h->ss.len + lap, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
@@ -1044,11 +1089,9 @@ int lmpc_ss_get_lap(lmpc_handle* h, int inst, int slot, int* T, double* x, doubl
 }
 
 int lmpc_ss_patch_row(lmpc_handle* h, int inst, int slot, int row, const double* x6, int also_model_slot) {
-    int rc = need_store(h);
-    if (rc) return rc;
+    if (int rc = need_store(h)) return rc;
     if (inst < 0 || inst >= h->batch || slot < 0 || slot >= h->ss.cap || row < 0 || row >= h->ss.Tmax || !x6)
         return fail(LMPC_E_INVALID, "bad patch arguments");
-    CK(cudaSetDevice(h->device));
     CK(cudaMemcpyAsync(h->ss.x + (h->ss.lap_index(inst, slot) * h->ss.Tmax + row) * 6, x6, sizeof(double) * 6, cudaMemcpyHostToDevice, h->stream));
     if (also_model_slot >= 0 && also_model_slot < h->mdl.cap)
         CK(cudaMemcpyAsync(h->mdl.x + (h->mdl.lap_index(inst, also_model_slot) * h->mdl.Tmax + row) * 6, x6, sizeof(double) * 6,
@@ -1061,33 +1104,21 @@ int lmpc_state_set(lmpc_handle* h, const double* xLin, const double* uLin, const
                    const int* timeStep, const int* has_pred, const double* xPred) {
     int rc = need_store(h);
     if (rc) return rc;
-    CK(cudaSetDevice(h->device));
-    const size_t B = h->batch, N = h->N, D = sizeof(double);
-    cudaStream_t s = h->stream;
-    if (xLin) CK(cudaMemcpyAsync(h->d_xLin, xLin, B * (N + 1) * 6 * D, cudaMemcpyHostToDevice, s));
-    if (uLin) CK(cudaMemcpyAsync(h->d_uLin, uLin, B * N * 2 * D, cudaMemcpyHostToDevice, s));
-    if (zt) CK(cudaMemcpyAsync(h->d_ztState, zt, B * 6 * D, cudaMemcpyHostToDevice, s));
-    if (OldInput) CK(cudaMemcpyAsync(h->d_OldInput, OldInput, B * 2 * D, cudaMemcpyHostToDevice, s));
-    if (timeStep) CK(cudaMemcpyAsync(h->d_timeStep, timeStep, B * sizeof(int), cudaMemcpyHostToDevice, s));
-    if (has_pred) CK(cudaMemcpyAsync(h->d_hasPred, has_pred, B * sizeof(int), cudaMemcpyHostToDevice, s));
-    if (xPred) CK(cudaMemcpyAsync(h->d_xPredPrev, xPred, B * (N + 1) * 6 * D, cudaMemcpyHostToDevice, s));
-    if (h->d_warm_valid) CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * B, s));     // a new controller state starts cold
-    CK(cudaStreamSynchronize(s));
+    if ((rc = copy_bufs(h, cudaMemcpyHostToDevice, {{h->d_xLin, xLin}, {h->d_uLin, uLin}, {h->d_ztState, zt}, {h->d_OldInput, OldInput},
+                                                   {h->d_timeStep, timeStep}, {h->d_hasPred, has_pred}, {h->d_xPredPrev, xPred}})))
+        return rc;
+    if (h->d_warm_valid) CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * h->batch, h->stream));     // a new state starts cold
+    CK(cudaStreamSynchronize(h->stream));
     return LMPC_OK;
 }
 
 int lmpc_state_get(lmpc_handle* h, double* xLin, double* uLin, double* zt, double* OldInput, int* timeStep) {
     int rc = need_store(h);
     if (rc) return rc;
-    CK(cudaSetDevice(h->device));
-    const size_t B = h->batch, N = h->N, D = sizeof(double);
-    cudaStream_t s = h->stream;
-    if (xLin) CK(cudaMemcpyAsync(xLin, h->d_xLin, B * (N + 1) * 6 * D, cudaMemcpyDeviceToHost, s));
-    if (uLin) CK(cudaMemcpyAsync(uLin, h->d_uLin, B * N * 2 * D, cudaMemcpyDeviceToHost, s));
-    if (zt) CK(cudaMemcpyAsync(zt, h->d_ztState, B * 6 * D, cudaMemcpyDeviceToHost, s));
-    if (OldInput) CK(cudaMemcpyAsync(OldInput, h->d_OldInput, B * 2 * D, cudaMemcpyDeviceToHost, s));
-    if (timeStep) CK(cudaMemcpyAsync(timeStep, h->d_timeStep, B * sizeof(int), cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
+    if ((rc = copy_bufs(h, cudaMemcpyDeviceToHost, {{h->d_xLin, xLin}, {h->d_uLin, uLin}, {h->d_ztState, zt}, {h->d_OldInput, OldInput},
+                                                   {h->d_timeStep, timeStep}})))
+        return rc;
+    CK(cudaStreamSynchronize(h->stream));
     return LMPC_OK;
 }
 
@@ -1123,11 +1154,12 @@ static int launch_k2(lmpc_handle* h, const double* d_x0) {
 int lmpc_identify_host(lmpc_handle* h, double* abc_out, int* flags) {
     int rc = need_store(h);
     if (rc) return rc;
-    CK(cudaSetDevice(h->device));
     CK(cudaMemsetAsync(h->d_flags, 0, sizeof(int) * h->batch, h->stream));
     rc = launch_k1(h);
     if (rc) return rc;
-    if (abc_out) CK(cudaMemcpyAsync(abc_out, h->hb[0].abc, sizeof(double) * h->batch * h->N * 54, cudaMemcpyDeviceToHost, h->stream));
+    QpIo out = {};
+    out.abc = abc_out;
+    if ((rc = copy_out(h, out, false)) != LMPC_OK) return rc;
     if (flags) CK(cudaMemcpyAsync(flags, h->d_flags, sizeof(int) * h->batch, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     return LMPC_OK;
@@ -1138,17 +1170,15 @@ int lmpc_select_host(lmpc_handle* h, const double* x0, double* SS_sel, double* Q
     int rc = need_store(h);
     if (rc) return rc;
     if (h->M <= 0 || !x0) return fail(LMPC_E_INVALID, "handle has no safe set or x0 is null");
-    CK(cudaSetDevice(h->device));
-    const size_t B = h->batch, M = h->M, D = sizeof(double);
+    const size_t B = h->batch;
     cudaStream_t s = h->stream;
-    CK(cudaMemcpyAsync(h->hb[0].x0, x0, B * 6 * D, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(h->hb[0].x0, x0, B * 6 * sizeof(double), cudaMemcpyHostToDevice, s));
     CK(cudaMemsetAsync(h->d_flags, 0, sizeof(int) * B, s));
     rc = launch_k2(h, h->hb[0].x0);
     if (rc) return rc;
-    if (SS_sel) CK(cudaMemcpyAsync(SS_sel, h->hb[0].SS, B * 6 * M * D, cudaMemcpyDeviceToHost, s));
-    if (Qfun_sel) CK(cudaMemcpyAsync(Qfun_sel, h->hb[0].Qfun, B * M * D, cudaMemcpyDeviceToHost, s));
-    if (Succ_SS) CK(cudaMemcpyAsync(Succ_SS, h->hb[0].SuccSS, B * 6 * M * D, cudaMemcpyDeviceToHost, s));
-    if (Succ_uSS) CK(cudaMemcpyAsync(Succ_uSS, h->hb[0].SuccU, B * 2 * M * D, cudaMemcpyDeviceToHost, s));
+    QpIo out = {};
+    out.SS = SS_sel; out.Qfun = Qfun_sel; out.SuccSS = Succ_SS; out.SuccU = Succ_uSS;
+    if ((rc = copy_out(h, out, true)) != LMPC_OK) return rc;
     if (min_index) CK(cudaMemcpyAsync(min_index, h->d_minidx, B * h->p.numSS_it * sizeof(int), cudaMemcpyDeviceToHost, s));
     if (flags) CK(cudaMemcpyAsync(flags, h->d_flags, B * sizeof(int), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
@@ -1164,7 +1194,6 @@ static int step_dev_impl(lmpc_handle* h, int mode, const double* x0_dev, cudaEve
     if (rc) return rc;
     if (!x0_dev || (mode != 0 && mode != 1)) return fail(LMPC_E_INVALID, "bad mode or null x0");
     if (mode == 1 && h->M <= 0) return fail(LMPC_E_INVALID, "LMPC step on a handle without a safe set");
-    CK(cudaSetDevice(h->device));
     cudaStream_t st = h->stream;
     CK(cudaMemsetAsync(h->d_flags, 0, sizeof(int) * h->batch, st));
     if (h->d_warm && h->warm_mode != mode) {             // records of the other problem type are not comparable
@@ -1172,13 +1201,13 @@ static int step_dev_impl(lmpc_handle* h, int mode, const double* x0_dev, cudaEve
         h->warm_mode = mode;
     }
     const bool lm = mode == 1;
-    const QpBufs& q = h->hb[0];
+    const QpIo& q = h->hb[0];
     if (ev) CK(cudaEventRecord(ev[0], st));
     if ((rc = launch_k1(h)) != LMPC_OK) return rc;                                   // PC.py:117
     if (ev) CK(cudaEventRecord(ev[1], st));
     if (lm && (rc = launch_k2(h, x0_dev)) != LMPC_OK) return rc;                     // PC.py:121
     if (ev) CK(cudaEventRecord(ev[2], st));
-    FtocpArgs a = qp_args(h, q, lm, QP_ALL);                                         // PC.py:124-125
+    FtocpArgs a = qp_args(h, q, lm);                                         // PC.py:124-125
     a.x0 = x0_dev; a.uOld = h->d_OldInput;
     if (h->d_warm) { a.warm = h->d_warm; a.warm_valid = h->d_warm_valid; a.warm_stride = h->warm_stride; }
     if ((rc = launch(h, a, lm, st)) != LMPC_OK) return rc;
@@ -1219,23 +1248,15 @@ int lmpc_step_host(lmpc_handle* h, int mode, const double* x0, double* xPred, do
     int rc = need_store(h);
     if (rc) return rc;
     if (!x0) return fail(LMPC_E_INVALID, "null x0");
-    CK(cudaSetDevice(h->device));
-    const size_t B = h->batch, N = h->N, M = h->M > 0 ? h->M : 1, D = sizeof(double);
+    const size_t B = h->batch;
     cudaStream_t s = h->stream;
-    CK(cudaMemcpyAsync(h->hb[0].x0, x0, B * 6 * D, cudaMemcpyHostToDevice, s));
+    CK(cudaMemcpyAsync(h->hb[0].x0, x0, B * 6 * sizeof(double), cudaMemcpyHostToDevice, s));
     rc = lmpc_step_dev(h, mode, h->hb[0].x0);
     if (rc) return rc;
-    if (xPred) CK(cudaMemcpyAsync(xPred, h->hb[0].xPred, B * (N + 1) * 6 * D, cudaMemcpyDeviceToHost, s));
-    if (uPred) CK(cudaMemcpyAsync(uPred, h->hb[0].uPred, B * N * 2 * D, cudaMemcpyDeviceToHost, s));
-    if (mode == 1) {
-        if (lambd) CK(cudaMemcpyAsync(lambd, h->hb[0].lambd, B * M * D, cudaMemcpyDeviceToHost, s));
-        if (zt) CK(cudaMemcpyAsync(zt, h->hb[0].zt, B * 6 * D, cudaMemcpyDeviceToHost, s));
-        if (zt_u) CK(cudaMemcpyAsync(zt_u, h->hb[0].ztu, B * 2 * D, cudaMemcpyDeviceToHost, s));
-        if (SS_sel) CK(cudaMemcpyAsync(SS_sel, h->hb[0].SS, B * 6 * M * D, cudaMemcpyDeviceToHost, s));
-    }
-    if (status) CK(cudaMemcpyAsync(status, h->hb[0].status, B * sizeof(int), cudaMemcpyDeviceToHost, s));
-    if (iters) CK(cudaMemcpyAsync(iters, h->hb[0].iters, B * sizeof(int), cudaMemcpyDeviceToHost, s));
-    if (resid) CK(cudaMemcpyAsync(resid, h->hb[0].resid, B * 3 * D, cudaMemcpyDeviceToHost, s));
+    QpIo out = {};
+    out.xPred = xPred; out.uPred = uPred; out.lambd = lambd; out.zt = zt; out.ztu = zt_u; out.SS = SS_sel;
+    out.status = status; out.iters = iters; out.resid = resid;
+    if ((rc = copy_out(h, out, mode == 1)) != LMPC_OK) return rc;
     if (flags) CK(cudaMemcpyAsync(flags, h->d_flags, B * sizeof(int), cudaMemcpyDeviceToHost, s));
     CK(cudaStreamSynchronize(s));
     return LMPC_OK;
@@ -1254,25 +1275,18 @@ int lmpc_read_buffer(lmpc_handle* h, const char* name, size_t offset_bytes, void
 int lmpc_step_results(lmpc_handle* h, int* status, int* iters, double* resid, int* flags) {
     int rc = need_store(h);
     if (rc) return rc;
-    CK(cudaSetDevice(h->device));
-    const size_t B = h->batch;
-    if (status) CK(cudaMemcpyAsync(status, h->hb[0].status, sizeof(int) * B, cudaMemcpyDeviceToHost, h->stream));
-    if (iters) CK(cudaMemcpyAsync(iters, h->hb[0].iters, sizeof(int) * B, cudaMemcpyDeviceToHost, h->stream));
-    if (resid) CK(cudaMemcpyAsync(resid, h->hb[0].resid, sizeof(double) * B * 3, cudaMemcpyDeviceToHost, h->stream));
-    if (flags) CK(cudaMemcpyAsync(flags, h->d_flags, sizeof(int) * B, cudaMemcpyDeviceToHost, h->stream));
+    QpIo out = {};
+    out.status = status; out.iters = iters; out.resid = resid;
+    if ((rc = copy_out(h, out, false)) != LMPC_OK) return rc;
+    if (flags) CK(cudaMemcpyAsync(flags, h->d_flags, sizeof(int) * h->batch, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     return LMPC_OK;
 }
 
 void* lmpc_device_buffer(lmpc_handle* h, const char* name) {
     if (!h || !name) return nullptr;
-    const QpBufs& q = h->hb[0];
-    struct { const char* n; void* p; } tab[] = {
-        {"xPred", q.xPred}, {"uPred", q.uPred}, {"lambd", q.lambd}, {"zt", q.zt}, {"zt_u", q.ztu},
-        {"abc", q.abc}, {"SS_sel", q.SS}, {"Qfun_sel", q.Qfun}, {"Succ_SS", q.SuccSS}, {"Succ_uSS", q.SuccU},
-        {"status", q.status}, {"iters", q.iters}, {"resid", q.resid}, {"flags", h->d_flags}, {"xLin", h->d_xLin},
-        {"uLin", h->d_uLin}, {"x0", q.x0}, {"slack", q.slack}, {"slackT", q.slackT}, {"OldInput", h->d_OldInput}, {"abc_lti", h->has_rollout ? h->d_abc_lti : nullptr}};
-    for (auto& e : tab) if (strcmp(e.n, name) == 0) return e.p;
+    for (const QpField& f : QP_FIELDS) if (f.name && !strcmp(f.name, name)) return f.at(h->hb[0]);
+    for (const DevBuf& r : dev_bufs(h)) if (r.name && !strcmp(r.name, name)) return *r.p;
     return nullptr;
 }
 
@@ -1291,64 +1305,36 @@ static int rollout_create_impl(lmpc_handle* h, int Tcl) {
     if (rc) return rc;
     if (h->has_rollout) return fail(LMPC_E_STATE, "rollout buffers already created");
     if (Tcl < 16) return fail(LMPC_E_INVALID, "Tcl too small");
-    CK(cudaSetDevice(h->device));
-    const size_t B = h->batch;
-    for (int i = 0; i < 2; ++i) {
-        CK(cudaMalloc((void**)&h->d_rx[i], sizeof(double) * B * 6));
-        CK(cudaMalloc((void**)&h->d_rg[i], sizeof(double) * B * 6));
-    }
-    CK(cudaMalloc((void**)&h->d_clx, sizeof(double) * B * Tcl * 6));
-    CK(cudaMalloc((void**)&h->d_clu, sizeof(double) * B * Tcl * 2));
-    CK(cudaMalloc((void**)&h->d_z, sizeof(double) * B * 3));
-    CK(cudaMalloc((void**)&h->d_zpid, sizeof(double) * B * 2));
-    CK(cudaMalloc((void**)&h->d_abc_lti, sizeof(double) * B * 54));
-    CK(cudaMemsetAsync(h->d_abc_lti, 0, sizeof(double) * B * 54, h->stream));
-    CK(cudaMalloc((void**)&h->d_cllen, sizeof(int) * B));
-    CK(cudaMalloc((void**)&h->d_done, sizeof(int) * B));
-    CK(cudaMalloc((void**)&h->d_health, sizeof(int) * B * 2));
-    CK(cudaMemsetAsync(h->d_health, 0, sizeof(int) * B * 2, h->stream));
-    CK(cudaMemsetAsync(h->d_cllen, 0, sizeof(int) * B, h->stream));
-    CK(cudaMemsetAsync(h->d_done, 0, sizeof(int) * B, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    h->Tcl = Tcl; h->cur = 0; h->sim_step = 0; h->has_rollout = true;
+    h->Tcl = Tcl; h->cur = 0; h->sim_step = 0;
+    if ((rc = alloc_bufs(h, dev_bufs(h), OWN_ROLLOUT, h->batch, "lmpc_rollout_create")) != LMPC_OK) return rc;
+    h->has_rollout = true;
     return LMPC_OK;
 }
 extern "C" {
 
 static int need_rollout(lmpc_handle* h) {
-    int rc = need_store(h);
-    if (rc) return rc;
-    if (!h->has_rollout) return fail(LMPC_E_STATE, "call lmpc_rollout_create first");
-    return LMPC_OK;
+    if (h && h->has_store && !h->has_rollout) return fail(LMPC_E_STATE, "call lmpc_rollout_create first");
+    return need_store(h);
 }
 
 int lmpc_rollout_set_state(lmpc_handle* h, const double* x, const double* xglob) {
-    int rc = need_rollout(h);
-    if (rc) return rc;
-    CK(cudaSetDevice(h->device));
-    if (x) CK(cudaMemcpyAsync(h->d_rx[h->cur], x, sizeof(double) * h->batch * 6, cudaMemcpyHostToDevice, h->stream));
-    if (xglob) CK(cudaMemcpyAsync(h->d_rg[h->cur], xglob, sizeof(double) * h->batch * 6, cudaMemcpyHostToDevice, h->stream));
+    if (int rc = need_rollout(h)) return rc;
+    if (int rc = copy_bufs(h, cudaMemcpyHostToDevice, {{h->d_rx[h->cur], x}, {h->d_rg[h->cur], xglob}})) return rc;
     CK(cudaStreamSynchronize(h->stream));
     return LMPC_OK;
 }
 
 int lmpc_rollout_get_state(lmpc_handle* h, double* x, double* xglob, int* done, int* cl_len) {
-    int rc = need_rollout(h);
-    if (rc) return rc;
-    CK(cudaSetDevice(h->device));
-    const size_t B = h->batch;
-    if (x) CK(cudaMemcpyAsync(x, h->d_rx[h->cur], sizeof(double) * B * 6, cudaMemcpyDeviceToHost, h->stream));
-    if (xglob) CK(cudaMemcpyAsync(xglob, h->d_rg[h->cur], sizeof(double) * B * 6, cudaMemcpyDeviceToHost, h->stream));
-    if (done) CK(cudaMemcpyAsync(done, h->d_done, sizeof(int) * B, cudaMemcpyDeviceToHost, h->stream));
-    if (cl_len) CK(cudaMemcpyAsync(cl_len, h->d_cllen, sizeof(int) * B, cudaMemcpyDeviceToHost, h->stream));
+    if (int rc = need_rollout(h)) return rc;
+    if (int rc = copy_bufs(h, cudaMemcpyDeviceToHost, {{h->d_rx[h->cur], x}, {h->d_rg[h->cur], xglob}, {h->d_done, done},
+                                                     {h->d_cllen, cl_len}}))
+        return rc;
     CK(cudaStreamSynchronize(h->stream));
     return LMPC_OK;
 }
 
 int lmpc_rollout_get_health(lmpc_handle* h, int* flags_or, int* unsolved_steps) {
-    int rc = need_rollout(h);
-    if (rc) return rc;
-    CK(cudaSetDevice(h->device));
+    if (int rc = need_rollout(h)) return rc;
     const size_t B = h->batch;
     if (flags_or) CK(cudaMemcpyAsync(flags_or, h->d_health, sizeof(int) * B, cudaMemcpyDeviceToHost, h->stream));
     if (unsolved_steps) CK(cudaMemcpyAsync(unsolved_steps, h->d_health + B, sizeof(int) * B, cudaMemcpyDeviceToHost, h->stream));
@@ -1373,8 +1359,7 @@ static SimArgs sim_args(const lmpc_handle* h, const double* z, unsigned long lon
 int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned long long seed) {
     int rc = need_rollout(h);
     if (rc) return rc;
-    CK(cudaSetDevice(h->device));
-    const QpBufs& q = h->hb[0];
+    const QpIo& q = h->hb[0];
     const double* xc = h->d_rx[h->cur];
     if (z_host) CK(cudaMemcpyAsync(h->d_z, z_host, sizeof(double) * h->batch * 3, cudaMemcpyHostToDevice, h->stream));
     if (mode == 2) {
@@ -1395,7 +1380,7 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
     // the trace of the chosen controllers reads the step's results and the state before dynModel
     if (h->has_trace) {
         trace_step_kernel<<<h->tr.n, 128, 0, h->stream>>>(h->tr, xc, h->d_rg[h->cur], q.uPred, (long long)h->N * 2, q.xPred,
-                                                        mode == 1 ? q.SS : nullptr, h->has_books ? h->bk.lap_n : nullptr);
+                                                        mode == 1 ? q.SS : nullptr, h->bk.lap_n);
         CK(cudaGetLastError());
         h->launches += 1;
     }
@@ -1413,9 +1398,7 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
 // z_pid_host[B,2] / z_sim_host[B,3]: the reference's standard-normal draws in its order (PID steer, PID accel | vx, vy, wz);
 // NULL = Philox on the device.
 int lmpc_rollout_pid_step(lmpc_handle* h, double vt, const double* z_pid_host, const double* z_sim_host, unsigned long long seed) {
-    int rc = need_rollout(h);
-    if (rc) return rc;
-    CK(cudaSetDevice(h->device));
+    if (int rc = need_rollout(h)) return rc;
     const double* xc = h->d_rx[h->cur];
     if (z_pid_host) CK(cudaMemcpyAsync(h->d_zpid, z_pid_host, sizeof(double) * h->batch * 2, cudaMemcpyHostToDevice, h->stream));
     if (z_sim_host) CK(cudaMemcpyAsync(h->d_z, z_sim_host, sizeof(double) * h->batch * 3, cudaMemcpyHostToDevice, h->stream));
@@ -1458,9 +1441,7 @@ int lmpc_rollout_set_vehicles(lmpc_handle* h, const lmpc_vehicle_params* sets, i
 // Regression(x, u, lamb) of Utilities.py:5-28 on every instance's closed-loop record: per-instance LTI model in the device
 // buffer "abc_lti" ([B][54] = A | B | C = 0, the layout lmpc_solve_mpc_dev takes with strides (54, 0)); abc_host may be NULL.
 int lmpc_rollout_sysid(lmpc_handle* h, double lamb, double* abc_host, int* flags_host) {
-    int rc = need_rollout(h);
-    if (rc) return rc;
-    CK(cudaSetDevice(h->device));
+    if (int rc = need_rollout(h)) return rc;
     CK(cudaMemsetAsync(h->d_flags, 0, sizeof(int) * h->batch, h->stream));
     ridge_sysid_kernel<<<h->batch, 32, 0, h->stream>>>(h->batch, h->d_clx, h->d_clu, h->d_cllen, h->Tcl, lamb, h->d_abc_lti, h->d_flags);
     CK(cudaGetLastError());
@@ -1474,11 +1455,9 @@ int lmpc_rollout_sysid(lmpc_handle* h, double lamb, double* abc_host, int* flags
 // main.py:99-110 on the device: every instance's record becomes `copies` identical laps in safe-set slots ss_slot0.. and
 // regression slots model_slot0.., the controller state is initialised from it and the record restarts.
 int lmpc_rollout_seed_from_record(lmpc_handle* h, int copies, int ss_slot0, int model_slot0) {
-    int rc = need_rollout(h);
-    if (rc) return rc;
+    if (int rc = need_rollout(h)) return rc;
     if (copies < 1 || ss_slot0 < 0 || model_slot0 < 0 || ss_slot0 + copies > h->ss.cap || model_slot0 + copies > h->mdl.cap)
         return fail(LMPC_E_INVALID, "seed copies do not fit the lap pools");
-    CK(cudaSetDevice(h->device));
     h->laps_stored = true;
     if (h->d_warm_valid) CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * h->batch, h->stream));
     seed_from_record_kernel<<<h->batch, 256, 0, h->stream>>>(h->batch, h->ss, h->mdl, copies, ss_slot0, model_slot0, h->d_clx, h->d_clu,
@@ -1490,10 +1469,8 @@ int lmpc_rollout_seed_from_record(lmpc_handle* h, int copies, int ss_slot0, int 
 }
 
 int lmpc_rollout_get_lap(lmpc_handle* h, int inst, int* T, double* x, double* u) {
-    int rc = need_rollout(h);
-    if (rc) return rc;
+    if (int rc = need_rollout(h)) return rc;
     if (inst < 0 || inst >= h->batch || !T) return fail(LMPC_E_INVALID, "bad instance");
-    CK(cudaSetDevice(h->device));
     CK(cudaMemcpyAsync(T, h->d_cllen + inst, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     if (x) CK(cudaMemcpyAsync(x, h->d_clx + (size_t)inst * h->Tcl * 6, sizeof(double) * (*T) * 6, cudaMemcpyDeviceToHost, h->stream));
@@ -1502,49 +1479,16 @@ int lmpc_rollout_get_lap(lmpc_handle* h, int inst, int* T, double* x, double* u)
     return LMPC_OK;
 }
 
-// Hand the finished lap of `inst` over to the stores without leaving the device: safe-set slot (computeCost on the
-// device) and/or regression slot (either may be -1), then restart the record; the curvilinear state is moved back by one
-// track length (SysModel.py:50) and the controller's step counter is reset (PC.py:445).
-int lmpc_rollout_commit_lap(lmpc_handle* h, int inst, int ss_slot, int model_slot) {
-    int rc = need_rollout(h);
-    if (rc) return rc;
-    if (inst < 0 || inst >= h->batch || ss_slot >= h->ss.cap || model_slot >= h->mdl.cap) return fail(LMPC_E_INVALID, "bad instance/slot");
-    CK(cudaSetDevice(h->device));
-    if (ss_slot >= 0 || model_slot >= 0) h->laps_stored = true;
-    if (ss_slot >= 0) {
-        commit_lap_kernel<<<1, 256, 0, h->stream>>>(h->ss, inst, ss_slot, h->d_clx, h->d_clu, h->d_cllen, h->Tcl);
-        rollout_cost_kernel<<<1, 256, 0, h->stream>>>(h->ss, inst, ss_slot, tracks(h));
-        h->launches += 2;
-    }
-    if (model_slot >= 0) {
-        commit_lap_kernel<<<1, 256, 0, h->stream>>>(h->mdl, inst, model_slot, h->d_clx, h->d_clu, h->d_cllen, h->Tcl);
-        h->launches += 1;
-    }
-    CK(cudaGetLastError());
-    // restart: cl_len = 0, s -= TrackLength, timeStep = 0, done = 0
-    double s;
-    CK(cudaMemcpyAsync(&s, h->d_rx[h->cur] + (size_t)inst * 6 + 4, sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    s -= h->trk_host[h->trk_idx_host.empty() ? 0 : h->trk_idx_host[inst]].TrackLength;
-    const int zero = 0;
-    CK(cudaMemcpyAsync(h->d_rx[h->cur] + (size_t)inst * 6 + 4, &s, sizeof(double), cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(h->d_cllen + inst, &zero, sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(h->d_done + inst, &zero, sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(h->d_timeStep + inst, &zero, sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    return LMPC_OK;
-}
-
-// The same hand-over for every instance with fin[b] != 0 in ONE launch (a Monte-Carlo batch finishes hundreds of laps in
-// the same step).
+// Hand the finished laps over to the stores without leaving the device, for every instance with fin[b] != 0 in ONE launch (a
+// Monte-Carlo batch finishes hundreds of laps in the same step): safe-set slot (computeCost on the device) and/or regression slot
+// (either may be -1), then restart the record; the curvilinear state is moved back by one track length (SysModel.py:50) and the
+// controller's step counter is reset (PC.py:445).
 int lmpc_rollout_commit_laps(lmpc_handle* h, const int* fin, const int* ss_slots, const int* model_slots) {
-    int rc = need_rollout(h);
-    if (rc) return rc;
+    if (int rc = need_rollout(h)) return rc;
     if (!fin || !ss_slots || !model_slots) return fail(LMPC_E_INVALID, "null argument");
     for (int b = 0; b < h->batch; ++b)
         if (fin[b] && (ss_slots[b] >= h->ss.cap || model_slots[b] >= h->mdl.cap)) return fail(LMPC_E_INVALID, "slot out of range");
     const size_t B = h->batch;
-    CK(cudaSetDevice(h->device));
     for (int b = 0; b < h->batch; ++b)
         if (fin[b] && (ss_slots[b] >= 0 || model_slots[b] >= 0)) h->laps_stored = true;
     CK(cudaMemcpyAsync(h->d_xchg, fin, sizeof(int) * B, cudaMemcpyHostToDevice, h->stream));
@@ -1560,10 +1504,8 @@ int lmpc_rollout_commit_laps(lmpc_handle* h, const int* fin, const int* ss_slots
 }
 
 int lmpc_rollout_export_laps_dev(lmpc_handle* h, int Tpad, double* rows_dev, int* lens_dev) {
-    int rc = need_rollout(h);
-    if (rc) return rc;
+    if (int rc = need_rollout(h)) return rc;
     if (!rows_dev || !lens_dev || Tpad < 1) return fail(LMPC_E_INVALID, "bad export arguments");
-    CK(cudaSetDevice(h->device));
     export_laps_kernel<<<h->batch, 256, 0, h->stream>>>(h->batch, h->d_clx, h->d_clu, h->d_cllen, h->Tcl, Tpad, rows_dev, lens_dev);
     CK(cudaGetLastError());
     h->launches += 1;
@@ -1571,12 +1513,10 @@ int lmpc_rollout_export_laps_dev(lmpc_handle* h, int Tpad, double* rows_dev, int
 }
 
 int lmpc_ss_export_laps_dev(lmpc_handle* h, const int* slots, int Tpad, double* rows_dev, int* lens_dev) {
-    int rc = need_store(h);
-    if (rc) return rc;
+    if (int rc = need_store(h)) return rc;
     if (!slots || !rows_dev || !lens_dev || Tpad < 1) return fail(LMPC_E_INVALID, "bad export arguments");
     for (int b = 0; b < h->batch; ++b)
         if (slots[b] >= h->ss.cap) return fail(LMPC_E_INVALID, "safe-set slot out of range");
-    CK(cudaSetDevice(h->device));
     CK(cudaMemcpyAsync(h->d_xchg, slots, sizeof(int) * h->batch, cudaMemcpyHostToDevice, h->stream));
     ss_export_laps_kernel<<<h->batch, 256, 0, h->stream>>>(h->batch, h->ss, h->d_xchg, Tpad, rows_dev, lens_dev);
     CK(cudaGetLastError());
@@ -1596,7 +1536,6 @@ int lmpc_ss_import_laps_dev(lmpc_handle* h, const int* ss_slots, const int* mode
         if (src[b] >= n_src) return fail(LMPC_E_INVALID, "source lap index out of range");
     }
     const size_t B = h->batch;
-    CK(cudaSetDevice(h->device));
     for (int b = 0; b < h->batch; ++b)
         if (src[b] >= 0 && (ss_slots[b] >= 0 || (model_slots && model_slots[b] >= 0))) h->laps_stored = true;
     CK(cudaMemcpyAsync(h->d_xchg, ss_slots, sizeof(int) * B, cudaMemcpyHostToDevice, h->stream));
@@ -1662,55 +1601,36 @@ int lmpc_probe_fp64(int device, double* out8) {
 // ================================================================================================
 // device lap books (lapbooks.cuh): the reference's once-per-lap list bookkeeping without the host
 // ================================================================================================
-static int need_books(lmpc_handle* h) {
-    int rc = need_store(h);
-    if (rc) return rc;
-    if (!h->has_books) return fail(LMPC_E_STATE, "lap books not allocated");
-    return LMPC_OK;
-}
-
 int lmpc_books_set(lmpc_handle* h, const int* ss_time, const int* ss_lap, const int* it, const int* md_time, const int* md_seq,
                    const int* md_cnt) {
-    int rc = need_books(h);
+    int rc = need_store(h);
     if (rc) return rc;
     if (!ss_time || !ss_lap || !it || !md_time || !md_seq || !md_cnt) return fail(LMPC_E_INVALID, "null argument");
-    CK(cudaSetDevice(h->device));
-    const size_t B = h->batch, sc = h->bk.ss_cap, mc = h->bk.md_cap;
-    cudaStream_t s = h->stream;
-    CK(cudaMemcpyAsync(h->bk.ss_time, ss_time, sizeof(int) * B * sc, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(h->bk.ss_lap, ss_lap, sizeof(int) * B * sc, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(h->bk.it, it, sizeof(int) * B, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(h->bk.md_time, md_time, sizeof(int) * B * mc, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(h->bk.md_seq, md_seq, sizeof(int) * B * mc, cudaMemcpyHostToDevice, s));
-    CK(cudaMemcpyAsync(h->bk.md_cnt, md_cnt, sizeof(int) * B, cudaMemcpyHostToDevice, s));
-    CK(cudaMemsetAsync(h->bk.lap_n, 0, sizeof(int) * B, s));
-    CK(cudaStreamSynchronize(s));
+    const LapBooks& k = h->bk;
+    if ((rc = copy_bufs(h, cudaMemcpyHostToDevice, {{k.ss_time, ss_time}, {k.ss_lap, ss_lap}, {k.it, it}, {k.md_time, md_time},
+                                                   {k.md_seq, md_seq}, {k.md_cnt, md_cnt}})))
+        return rc;
+    CK(cudaMemsetAsync(k.lap_n, 0, sizeof(int) * h->batch, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
     return LMPC_OK;
 }
 
 int lmpc_books_get(lmpc_handle* h, int* ss_time, int* ss_lap, int* it, int* md_time, int* md_seq, int* md_cnt, int* sel, int* is_prev,
                    int* prev_slot, int* used, int* lap_hist, int* lap_n) {
-    int rc = need_books(h);
+    int rc = need_store(h);
     if (rc) return rc;
-    CK(cudaSetDevice(h->device));
-    const size_t B = h->batch, sc = h->bk.ss_cap, mc = h->bk.md_cap, nit = h->bk.numSS_it, tr = h->bk.trToUse;
-    cudaStream_t s = h->stream;
-#define GET(dst, src, n) if (dst) CK(cudaMemcpyAsync(dst, src, sizeof(int) * (n), cudaMemcpyDeviceToHost, s))
-    GET(ss_time, h->bk.ss_time, B * sc); GET(ss_lap, h->bk.ss_lap, B * sc); GET(it, h->bk.it, B);
-    GET(md_time, h->bk.md_time, B * mc); GET(md_seq, h->bk.md_seq, B * mc); GET(md_cnt, h->bk.md_cnt, B);
-    GET(sel, h->d_sel, B * nit); GET(is_prev, h->d_isprev, B * nit); GET(prev_slot, h->d_prevslot, B); GET(used, h->d_used, B * tr);
-    GET(lap_hist, h->bk.lap_hist, B * LAP_HIST); GET(lap_n, h->bk.lap_n, B);
-#undef GET
-    CK(cudaStreamSynchronize(s));
+    const LapBooks& k = h->bk;
+    if ((rc = copy_bufs(h, cudaMemcpyDeviceToHost, {{k.ss_time, ss_time}, {k.ss_lap, ss_lap}, {k.it, it}, {k.md_time, md_time},
+                                                   {k.md_seq, md_seq}, {k.md_cnt, md_cnt}, {k.sel, sel}, {k.isprev, is_prev},
+                                                   {k.prevslot, prev_slot}, {k.used, used}, {k.lap_hist, lap_hist}, {k.lap_n, lap_n}})))
+        return rc;
+    CK(cudaStreamSynchronize(h->stream));
     return LMPC_OK;
 }
 
 // Lap hand-over of every controller whose lap just ended, bookkeeping on the device; enqueue only.
 int lmpc_rollout_commit_laps_dev(lmpc_handle* h) {
-    int rc = need_rollout(h);
-    if (rc) return rc;
-    if ((rc = need_books(h)) != LMPC_OK) return rc;
-    CK(cudaSetDevice(h->device));
+    if (int rc = need_rollout(h)) return rc;
     h->laps_stored = true;     // enqueue only: which controllers finish a lap is not known here
     commit_laps_books_kernel<<<h->batch, 256, 0, h->stream>>>(h->batch, h->ss, h->mdl, h->bk, h->d_clx, h->d_clu, h->d_cllen, h->Tcl,
                                                               h->d_rx[h->cur], h->d_timeStep, h->d_done, h->d_health, tracks(h),
@@ -1721,11 +1641,8 @@ int lmpc_rollout_commit_laps_dev(lmpc_handle* h) {
 }
 
 int lmpc_rollout_seed_from_record_dev(lmpc_handle* h, int copies) {
-    int rc = need_rollout(h);
-    if (rc) return rc;
-    if ((rc = need_books(h)) != LMPC_OK) return rc;
+    if (int rc = need_rollout(h)) return rc;
     if (copies < 1 || (h->M > 0 && copies > h->ss.cap) || copies > h->mdl.cap) return fail(LMPC_E_INVALID, "seed copies do not fit the lap pools");
-    CK(cudaSetDevice(h->device));
     h->laps_stored = true;
     if (h->d_warm_valid) CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * h->batch, h->stream));
     seed_books_kernel<<<h->batch, 256, 0, h->stream>>>(h->batch, h->ss, h->mdl, h->bk, copies, h->d_clx, h->d_clu, h->d_cllen, h->Tcl, h->N,
@@ -1737,11 +1654,8 @@ int lmpc_rollout_seed_from_record_dev(lmpc_handle* h, int copies) {
 }
 
 int lmpc_rollout_stats(lmpc_handle* h, int* out4) {
-    int rc = need_rollout(h);
-    if (rc) return rc;
-    if ((rc = need_books(h)) != LMPC_OK) return rc;
+    if (int rc = need_rollout(h)) return rc;
     if (!out4) return fail(LMPC_E_INVALID, "null output");
-    CK(cudaSetDevice(h->device));
     rollout_stats_kernel<<<1, 1024, 0, h->stream>>>(h->batch, h->bk, h->d_cllen, h->d_health, nullptr, 1, h->d_stats);
     CK(cudaGetLastError());
     h->launches += 1;
@@ -1751,11 +1665,8 @@ int lmpc_rollout_stats(lmpc_handle* h, int* out4) {
 }
 
 int lmpc_rollout_group_stats(lmpc_handle* h, int* out) {
-    int rc = need_rollout(h);
-    if (rc) return rc;
-    if ((rc = need_books(h)) != LMPC_OK) return rc;
+    if (int rc = need_rollout(h)) return rc;
     if (!out) return fail(LMPC_E_INVALID, "null output");
-    CK(cudaSetDevice(h->device));
     const int G = h->ngroups > 0 ? h->ngroups : 1;
     rollout_stats_kernel<<<1, 1024, 0, h->stream>>>(h->batch, h->bk, h->d_cllen, h->d_health, h->d_pool_grp, G, h->d_stats);
     CK(cudaGetLastError());
@@ -1769,12 +1680,11 @@ int lmpc_rollout_group_stats(lmpc_handle* h, int* out) {
 // ship_host (null: every group) is a checked 0/1 mask [G]; a masked-out group ships rows with global id -1.
 static int pool_export(lmpc_handle* h, const char* who, int kbest, int Tpad, long long gid_base, const int* ship_host, double* rows_dev,
                        int* meta_dev) {
-    int rc = need_books(h);
+    int rc = need_store(h);
     if (rc) return rc;
     if (kbest < 1 || kbest > POOL_MAXK || Tpad < 1 || !rows_dev || !meta_dev) return fail(LMPC_E_INVALID, "bad export arguments");
     if (h->M <= 0) return fail(LMPC_E_STATE, "handle has no safe set");
     if ((rc = one_track_per_group(h, who)) != LMPC_OK) return rc;
-    CK(cudaSetDevice(h->device));
     const int G = h->ngroups > 0 ? h->ngroups : 1;
     int* ship = nullptr;
     if (ship_host) {     // staged from pageable stack memory, so the caller's array may change once the call returns
@@ -1798,8 +1708,7 @@ int lmpc_pool_export_dev(lmpc_handle* h, int kbest, int Tpad, long long gid_base
 int lmpc_pool_export_groups_dev(lmpc_handle* h, int kbest, int Tpad, long long gid_base, const int* ship_host, double* rows_dev,
                                 int* meta_dev) {
     static const char* who = "lmpc_pool_export_groups_dev";
-    int rc = need_books(h);
-    if (rc) return rc;
+    if (int rc = need_store(h)) return rc;
     if (!ship_host) return fail(LMPC_E_INVALID, std::string(who) + ": null ship mask");
     const int G = h->ngroups > 0 ? h->ngroups : 1;
     for (int g = 0; g < G; ++g)
@@ -1812,14 +1721,13 @@ int lmpc_pool_export_groups_dev(lmpc_handle* h, int kbest, int Tpad, long long g
 // took_host (may be NULL) receives the number of laps stored; the call then synchronises.
 int lmpc_pool_import_dev(lmpc_handle* h, int n_src, int share, int Tpad, long long gid_base, const double* rows_dev, const int* meta_dev,
                          int* took_host) {
-    int rc = need_books(h);
+    int rc = need_store(h);
     if (rc) return rc;
     const int G = h->ngroups > 0 ? h->ngroups : 1;
     if (n_src < 1 || n_src > POOL_MAXSRC * G || share < 1 || Tpad < 1 || !rows_dev || !meta_dev)
         return fail(LMPC_E_INVALID, "bad import arguments");
     if (h->M <= 0) return fail(LMPC_E_STATE, "handle has no safe set");
     if ((rc = one_track_per_group(h, "lmpc_pool_import_dev")) != LMPC_OK) return rc;
-    CK(cudaSetDevice(h->device));
     h->laps_stored = true;
     int* order = h->d_poolidx + POOL_ORDER;
     int* cnt = h->d_poolidx + POOL_COUNT;
@@ -1852,33 +1760,16 @@ static const char* snap_field_name(int f) {
 }
 
 // The record layout of this handle: copy table t (handle buffers, record offsets, word sizes, chunks) and header hd (layout ints,
-// section offsets; the track row and warm_mode are per pack).  Every per-controller buffer of the store and the rollout is either
-// a section here or per-step scratch (DESIGN.md, "Controller snapshots").
-static void snap_layout(const lmpc_handle* h, SnapTable& t, lmpc_snapshot_header& hd) {
+// section offsets; the track row and warm_mode are per pack).  The sections are the allocated rows of dev_bufs that name one.
+static void snap_layout(lmpc_handle* h, SnapTable& t, lmpc_snapshot_header& hd) {
     memset(&t, 0, sizeof(t));
     memset(&hd, 0, sizeof(hd));
-    const long long B = h->batch, N = h->N, sc = h->ss.cap, mc = h->mdl.cap, T = h->ss.Tmax, D = sizeof(double), I = sizeof(int);
-    auto sect = [&](int k, const void* base, long long bytes) { t.s[k].base = (char*)base; t.s[k].stride = bytes; t.s[k].bytes = (int)bytes; };
-    sect(SN_SS_X, h->ss.x, sc * T * 6 * D); sect(SN_SS_U, h->ss.u, sc * T * 2 * D); sect(SN_SS_Q, h->ss.q, sc * T * D);
-    sect(SN_SS_LEN, h->ss.len, sc * I);
-    sect(SN_MD_X, h->mdl.x, mc * T * 6 * D); sect(SN_MD_U, h->mdl.u, mc * T * 2 * D); sect(SN_MD_LEN, h->mdl.len, mc * I);
-    const LapBooks& k = h->bk;
-    sect(SN_SS_TIME, k.ss_time, sc * I); sect(SN_SS_LAP, k.ss_lap, sc * I); sect(SN_IT, k.it, I);
-    sect(SN_MD_TIME, k.md_time, mc * I); sect(SN_MD_SEQ, k.md_seq, mc * I); sect(SN_MD_CNT, k.md_cnt, I);
-    sect(SN_LAP_HIST, k.lap_hist, LAP_HIST * I); sect(SN_LAP_N, k.lap_n, I);
-    sect(SN_SEL, k.sel, k.numSS_it * I); sect(SN_ISPREV, k.isprev, k.numSS_it * I); sect(SN_PREVSLOT, k.prevslot, I);
-    sect(SN_USED, k.used, k.trToUse * I);
-    sect(SN_XLIN, h->d_xLin, (N + 1) * 6 * D); sect(SN_ULIN, h->d_uLin, N * 2 * D); sect(SN_ZT, h->d_ztState, 6 * D);
-    sect(SN_OLDINPUT, h->d_OldInput, 2 * D); sect(SN_XPREDPREV, h->d_xPredPrev, (N + 1) * 6 * D);
-    sect(SN_TIMESTEP, h->d_timeStep, I); sect(SN_HASPRED, h->d_hasPred, I);
-    if (h->d_warm) { sect(SN_WARM, h->d_warm, h->warm_stride * D); sect(SN_WARM_VALID, h->d_warm_valid, I); }
-    if (h->has_rollout) {
-        sect(SN_RX, h->d_rx[h->cur], 6 * D); sect(SN_RG, h->d_rg[h->cur], 6 * D);
-        sect(SN_CLX, h->d_clx, (long long)h->Tcl * 6 * D); sect(SN_CLU, h->d_clu, (long long)h->Tcl * 2 * D);
-        sect(SN_CLLEN, h->d_cllen, I); sect(SN_DONE, h->d_done, I);
-        sect(SN_HEALTH_FLAGS, h->d_health, I); sect(SN_HEALTH_UNSOLVED, h->d_health + B, I);     // health is [2][B]
-        sect(SN_ABC_LTI, h->d_abc_lti, 54 * D);
-    }
+    for (const DevBuf& r : dev_bufs(h))
+        for (int k = 0; r.sect != SN_SCRATCH && *r.p && k < r.rows; ++k) {     // row k of a [rows][B][per] buffer
+            SnapSect& e = t.s[r.sect + k];
+            e.stride = e.bytes = (int)(r.elem * r.per);
+            e.base = (char*)*r.p + k * r.bytes(h->batch) / r.rows;
+        }
     auto up16 = [](long long v) { return (v + 15) / 16 * 16; };
     long long off = up16(sizeof(lmpc_snapshot_header));
     for (int s = 0; s < SN_COUNT; ++s) {
@@ -1888,7 +1779,7 @@ static void snap_layout(const lmpc_handle* h, SnapTable& t, lmpc_snapshot_header
         hd.sect_bytes[s] = t.s[s].bytes;
         off += up16(t.s[s].bytes);
     }
-    t.s[SN_HEADER].base = (char*)h->d_snap;                       // the handle's header template (snap_scratch)
+    t.s[SN_HEADER].base = (char*)h->d_snap;                       // the handle's header template
     t.s[SN_HEADER].bytes = SNAP_HDR_WORDS * 4;
     t.s[SN_HEADER].pack_only = 1;
     t.s[SN_TRACK].base = (char*)h->d_trk;
@@ -1899,8 +1790,8 @@ static void snap_layout(const lmpc_handle* h, SnapTable& t, lmpc_snapshot_header
     t.s[SN_TRACK].pack_only = 1;
     for (int s = 0; s < SN_TABLE; ++s) {
         SnapSect& e = t.s[s];
-        // every address a thread touches is base + k * stride + rec_off-relative offset: the word must divide all four (a buffer
-        // carved out of a larger allocation, like the lap history in the books buffer, need not be 16-byte aligned)
+        // every address a thread touches is base + k * stride + rec_off-relative offset: the word must divide all four (the
+        // second row of a [2][B] buffer, for one, is only 4-byte aligned under an odd batch)
         const long long all = e.bytes | e.stride | e.rec_off | (long long)(uintptr_t)e.base;
         e.word = (all % 16 == 0) ? 16 : (all % 8 == 0) ? 8 : 4;
     }
@@ -1918,24 +1809,27 @@ static void snap_layout(const lmpc_handle* h, SnapTable& t, lmpc_snapshot_header
             ++t.nchunk;
         }
     hd.magic = LMPC_SNAPSHOT_MAGIC; hd.version = LMPC_SNAPSHOT_VERSION; hd.bytes = (int)off;
-    hd.N = h->N; hd.M = h->M; hd.ncx = h->p.ncx; hd.ncu = h->p.ncu; hd.numSS_it = k.numSS_it; hd.trToUse = k.trToUse;
-    hd.ss_cap = (int)sc; hd.model_cap = (int)mc; hd.Tmax = (int)T; hd.Tcl = h->has_rollout ? h->Tcl : 0;
+    hd.N = h->N; hd.M = h->M; hd.ncx = h->p.ncx; hd.ncu = h->p.ncu; hd.numSS_it = h->bk.numSS_it; hd.trToUse = h->bk.trToUse;
+    hd.ss_cap = h->ss.cap; hd.model_cap = h->mdl.cap; hd.Tmax = h->ss.Tmax; hd.Tcl = h->has_rollout ? h->Tcl : 0;
     hd.warm_start = h->d_warm ? 1 : 0;
     hd.warm_mode = h->d_warm ? h->warm_mode : -1;
     hd.nsect = LMPC_SNAPSHOT_SECTIONS;
 }
 
-// The header template and the check verdict of this handle, allocated on first use
-static int snap_scratch(lmpc_handle* h) {
-    if (!h->d_snap) CK(cudaMalloc((void**)&h->d_snap, sizeof(int) * (SNAP_HDR_WORDS + 4)));
+// Release the index scratch of a pack / unpack when e is an error, or always (`always`); report e, else the release's error
+static int snap_release(lmpc_handle* h, int* d_idx, cudaError_t e, bool always) {
+    if (e == cudaSuccess && !always) return LMPC_OK;
+    const cudaError_t f = cudaFreeAsync(d_idx, h->stream);
+    if (e == cudaSuccess) e = f;
+    if (e != cudaSuccess) return fail(LMPC_E_CUDA, std::string("snapshot index scratch: ") + cudaGetErrorString(e));
     return LMPC_OK;
 }
 
 // Upload the controller indices (and record indices) of one pack / unpack to stream-ordered scratch of their own
 static int snap_indices(lmpc_handle* h, const std::vector<int>& idx, int** d_idx) {
     CK(cudaMallocAsync((void**)d_idx, sizeof(int) * idx.size(), h->stream));
-    CK(cudaMemcpyAsync(*d_idx, idx.data(), sizeof(int) * idx.size(), cudaMemcpyHostToDevice, h->stream));
-    return LMPC_OK;
+    return snap_release(h, *d_idx, cudaMemcpyAsync(*d_idx, idx.data(), sizeof(int) * idx.size(), cudaMemcpyHostToDevice, h->stream),
+                        false);
 }
 
 extern "C" {
@@ -1943,8 +1837,7 @@ extern "C" {
 int lmpc_sizeof_snapshot_header(void) { return (int)sizeof(lmpc_snapshot_header); }
 
 int lmpc_snapshot_bytes(lmpc_handle* h, size_t* bytes) {
-    int rc = need_books(h);
-    if (rc) return rc;
+    if (int rc = need_store(h)) return rc;
     if (!bytes) return fail(LMPC_E_INVALID, "null output");
     SnapTable t;
     lmpc_snapshot_header hd;
@@ -1955,7 +1848,7 @@ int lmpc_snapshot_bytes(lmpc_handle* h, size_t* bytes) {
 
 int lmpc_snapshot_pack_dev(lmpc_handle* h, int n, const int* inst_host, void* rec_dev) {
     static const char* who = "lmpc_snapshot_pack_dev";
-    int rc = need_books(h);
+    int rc = need_store(h);
     if (rc) return rc;
     if (!rec_dev || n < 1) return fail(LMPC_E_INVALID, std::string(who) + ": null records or n < 1");
     if (!inst_host && n != h->batch) return fail(LMPC_E_INVALID, std::string(who) + ": NULL controllers means every controller (n == batch)");
@@ -1966,8 +1859,6 @@ int lmpc_snapshot_pack_dev(lmpc_handle* h, int n, const int* inst_host, void* re
         if (idx[i] < 0 || idx[i] >= h->batch)
             return fail(LMPC_E_INVALID, std::string(who) + ": controller index " + std::to_string(i) + " out of range");
     }
-    CK(cudaSetDevice(h->device));
-    if ((rc = snap_scratch(h)) != LMPC_OK) return rc;
     SnapTable t;
     lmpc_snapshot_header hd;
     snap_layout(h, t, hd);
@@ -1976,15 +1867,14 @@ int lmpc_snapshot_pack_dev(lmpc_handle* h, int n, const int* inst_host, void* re
     int* d_idx = nullptr;
     if ((rc = snap_indices(h, idx, &d_idx)) != LMPC_OK) return rc;
     snapshot_copy_kernel<<<dim3(n, t.nchunk), 256, 0, h->stream>>>(t, 0, d_idx, nullptr, (char*)rec_dev, hd.bytes);
-    CK(cudaGetLastError());
-    CK(cudaFreeAsync(d_idx, h->stream));
+    if ((rc = snap_release(h, d_idx, cudaGetLastError(), true)) != LMPC_OK) return rc;
     h->launches += 1;
     return LMPC_OK;
 }
 
 int lmpc_snapshot_unpack_dev(lmpc_handle* h, const void* rec_dev, int nrec, int n, const int* dst_host, const int* rec_of_dst_host) {
     static const char* who = "lmpc_snapshot_unpack_dev";
-    int rc = need_books(h);
+    int rc = need_store(h);
     if (rc) return rc;
     const std::string w = std::string(who) + ": ";
     if (!rec_dev || !dst_host || nrec < 1 || n < 1 || n > h->batch)
@@ -2001,8 +1891,6 @@ int lmpc_snapshot_unpack_dev(lmpc_handle* h, const void* rec_dev, int nrec, int 
         idx[i] = d;
         idx[n + i] = r;
     }
-    CK(cudaSetDevice(h->device));
-    if ((rc = snap_scratch(h)) != LMPC_OK) return rc;
     SnapTable t;
     lmpc_snapshot_header hd;
     snap_layout(h, t, hd);
@@ -2043,8 +1931,7 @@ int lmpc_snapshot_unpack_dev(lmpc_handle* h, const void* rec_dev, int nrec, int 
         return fail(LMPC_E_INVALID, w + why + "; nothing was restored");
     }
     snapshot_copy_kernel<<<dim3(n, t.nchunk), 256, 0, h->stream>>>(t, 1, d_idx, d_idx + n, (char*)rec_dev, hd.bytes);
-    CK(cudaGetLastError());
-    CK(cudaFreeAsync(d_idx, h->stream));
+    if ((rc = snap_release(h, d_idx, cudaGetLastError(), true)) != LMPC_OK) return rc;
     h->launches += 1;
     h->laps_stored = true;
     if (h->d_warm) h->warm_mode = mode;
@@ -2052,16 +1939,14 @@ int lmpc_snapshot_unpack_dev(lmpc_handle* h, const void* rec_dev, int nrec, int 
 }
 
 int lmpc_rollout_get_clock(lmpc_handle* h, unsigned long long* step) {
-    int rc = need_rollout(h);
-    if (rc) return rc;
+    if (int rc = need_rollout(h)) return rc;
     if (!step) return fail(LMPC_E_INVALID, "null output");
     *step = h->sim_step;
     return LMPC_OK;
 }
 
 int lmpc_rollout_set_clock(lmpc_handle* h, unsigned long long step) {
-    int rc = need_rollout(h);
-    if (rc) return rc;
+    if (int rc = need_rollout(h)) return rc;
     h->sim_step = step;
     return LMPC_OK;
 }
@@ -2098,34 +1983,29 @@ int lmpc_track_global_position(int device, const double* table6, int nseg, doubl
 }
 
 int lmpc_rollout_trace_create(lmpc_handle* h, int n, const int* inst, int cap_steps) {
-    int rc = need_rollout(h);
-    if (rc) return rc;
+    if (int rc = need_rollout(h)) return rc;
     if (h->has_trace) return fail(LMPC_E_STATE, "trace buffers already created");
     if (n < 1 || n > 1024 || !inst || cap_steps < 1) return fail(LMPC_E_INVALID, "bad trace arguments");
     for (int i = 0; i < n; ++i) if (inst[i] < 0 || inst[i] >= h->batch) return fail(LMPC_E_INVALID, "traced controller out of range");
-    CK(cudaSetDevice(h->device));
     TraceBufs& t = h->tr;
     t.n = n; t.cap = cap_steps; t.N = h->N; t.M = h->M > 0 ? h->M : 0;
-    const size_t rows = (size_t)n * cap_steps, np = (size_t)(h->N + 1) * 6;
-    CK(cudaMalloc((void**)&h->d_trinst, sizeof(int) * n));
-    CK(cudaMalloc((void**)&t.steps, sizeof(int) * n));
-    CK(cudaMalloc((void**)&t.x, sizeof(double) * rows * 6)); CK(cudaMalloc((void**)&t.g, sizeof(double) * rows * 6));
-    CK(cudaMalloc((void**)&t.u, sizeof(double) * rows * 2)); CK(cudaMalloc((void**)&t.xPred, sizeof(double) * rows * np));
-    CK(cudaMalloc((void**)&t.ss, sizeof(double) * rows * 6 * (t.M > 0 ? t.M : 1)));
-    CK(cudaMalloc((void**)&t.lap, sizeof(int) * rows));
-    CK(cudaMemcpyAsync(h->d_trinst, inst, sizeof(int) * n, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemsetAsync(t.steps, 0, sizeof(int) * n, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
+    const std::vector<DevBuf> rows = dev_bufs(h);
+    int rc = alloc_bufs(h, rows, OWN_TRACE, n, "lmpc_rollout_trace_create");
+    if (rc != LMPC_OK) return rc;
+    cudaError_t e = cudaMemcpyAsync(h->d_trinst, inst, sizeof(int) * n, cudaMemcpyHostToDevice, h->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+    if (e != cudaSuccess) {
+        free_bufs(rows, OWN_TRACE);
+        return fail(LMPC_E_CUDA, std::string("lmpc_rollout_trace_create: ") + cudaGetErrorString(e));
+    }
     t.inst = h->d_trinst;
     h->has_trace = true;
     return LMPC_OK;
 }
 
 int lmpc_rollout_trace_get(lmpc_handle* h, int tr, int* steps, double* x, double* xglob, double* u, double* xPred, double* SS_sel, int* lap) {
-    int rc = need_rollout(h);
-    if (rc) return rc;
+    if (int rc = need_rollout(h)) return rc;
     if (!h->has_trace || tr < 0 || tr >= h->tr.n || !steps) return fail(LMPC_E_INVALID, "no such trace");
-    CK(cudaSetDevice(h->device));
     const TraceBufs& t = h->tr;
     cudaStream_t s = h->stream;
     CK(cudaMemcpyAsync(steps, t.steps + tr, sizeof(int), cudaMemcpyDeviceToHost, s));

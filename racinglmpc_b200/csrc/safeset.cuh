@@ -597,16 +597,6 @@ __global__ void ss_add_point_kernel(int batch, LapPool pool, const int* prev_slo
     pool.len[lap] = T + 1;
 }
 
-// Copy the closed-loop record of instance b into a pool slot (device to device): the device-resident counterpart of
-// LMPC.addTrajectory / PredictiveModel.addTrajectory receiving the lap that Simulator.sim just returned.
-__global__ void commit_lap_kernel(LapPool pool, int b, int slot, const double* cl_x, const double* cl_u, const int* cl_len, int Tcl) {
-    const int T = min(cl_len[b], pool.Tmax);
-    const size_t lap = pool.lap_index(b, slot);
-    for (int e = threadIdx.x; e < T * 6; e += blockDim.x) pool.x[lap * pool.Tmax * 6 + e] = cl_x[(size_t)b * Tcl * 6 + e];
-    for (int e = threadIdx.x; e < T * 2; e += blockDim.x) pool.u[lap * pool.Tmax * 2 + e] = cl_u[(size_t)b * Tcl * 2 + e];
-    if (threadIdx.x == 0) pool.len[lap] = T;
-}
-
 // Pack every instance's closed-loop record into rows[B][Tpad][8] = (x | u) + lens[B]: the send buffer of the per-lap
 // all-gather of the pooled-safe-set mode (SURVEY §8e).
 __global__ void export_laps_kernel(int batch, const double* cl_x, const double* cl_u, const int* cl_len, int Tcl, int Tpad,
