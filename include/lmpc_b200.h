@@ -321,9 +321,6 @@ int lmpc_rollout_get_lap(lmpc_handle* h, int inst, int* T, double* x, double* u)
  * s -= TrackLength (SysModel.py:50), record restarted, timeStep = 0 (PC.py:445), for every instance with fin_host[b] != 0 in
  * one launch; per instance a safe-set and a regression slot, either of which may be -1 ([B] host arrays). */
 int lmpc_rollout_commit_laps(lmpc_handle* h, const int* fin_host, const int* ss_slots_host, const int* model_slots_host);
-/* Pack all closed-loop records into rows_dev[B,Tpad,8] = (x | u), lens_dev[B] (device buffers of the caller): the send
- * buffer of the once-per-lap all-gather of the pooled-safe-set mode (SURVEY §8e). */
-int lmpc_rollout_export_laps_dev(lmpc_handle* h, int Tpad, double* rows_dev, int* lens_dev);
 
 /* ---- pooled-safe-set exchange (SURVEY §8e; no reference counterpart: the reference runs one controller) ------------------
  * Send side: pack stored lap slots_host[b] (-1: none, lens = 0) of every instance, including the rows LMPC.addPoint

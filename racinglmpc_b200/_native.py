@@ -129,7 +129,6 @@ def lib():
     L.lmpc_rollout_seed_from_record.argtypes = [_vp, C.c_int, C.c_int, C.c_int]
     L.lmpc_rollout_get_lap.argtypes = [_vp, C.c_int, ip, _vp, _vp]
     L.lmpc_rollout_commit_laps.argtypes = [_vp, _vp, _vp, _vp]
-    L.lmpc_rollout_export_laps_dev.argtypes = [_vp, C.c_int, _vp, _vp]
     L.lmpc_ss_export_laps_dev.argtypes = [_vp, _vp, C.c_int, _vp, _vp]
     L.lmpc_ss_import_laps_dev.argtypes = [_vp, _vp, _vp, _vp, C.c_int, C.c_int, _vp, _vp]
     L.lmpc_probe_fp64.argtypes = [C.c_int, _vp]

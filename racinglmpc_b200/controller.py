@@ -461,10 +461,6 @@ class BatchedController:
             self._touch(b, sel=self.lmpc, used=to_model)
         return finished
 
-    def rollout_export_laps(self, Tpad, rows_dev, lens_dev):
-        """Pack the closed-loop records into caller-owned device tensors rows[B,Tpad,8], lens[B] (int32)."""
-        nat.check(self._lib.lmpc_rollout_export_laps_dev(self._h, int(Tpad), nat.ptr(rows_dev), nat.ptr(lens_dev)))
-
     # ------------------------------------------------------------------ pooled-safe-set exchange (SURVEY §8e)
     def own_lap_number(self, inst, j):
         """Current lap number of the j-th lap the instance drove itself (imported laps shift later numbers)."""

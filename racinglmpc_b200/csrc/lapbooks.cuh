@@ -132,13 +132,6 @@ __device__ inline int book_refresh(const LapBooks& k, int b) {
     return flag;
 }
 
-// Copy `T` rows of (x | u) from a closed-loop record into a pool slot; block-wide.
-__device__ inline void copy_lap_block(const LapPool& pool, size_t lap, const double* cx, const double* cu, int T) {
-    for (int e = threadIdx.x; e < T * 6; e += blockDim.x) pool.x[lap * pool.Tmax * 6 + e] = cx[e];
-    for (int e = threadIdx.x; e < T * 2; e += blockDim.x) pool.u[lap * pool.Tmax * 2 + e] = cu[e];
-    if (threadIdx.x == 0) pool.len[lap] = T;
-}
-
 // Lap hand-over of every controller whose lap just ended (done[b] != 0), bookkeeping included: main.py:113-119
 // (lmpc.addTrajectory + predictiveModel.addTrajectory of the lap Simulator.sim returned), SysModel.py:50 (s -= TrackLength),
 // PC.py:445 (timeStep = 0).  One CTA per controller; no host involvement.
@@ -160,22 +153,14 @@ __global__ void __launch_bounds__(256) commit_laps_books_kernel(int batch, LapPo
     __syncthreads();
     const double* cx = cl_x + (size_t)b * Tcl * 6;
     const double* cu = cl_u + (size_t)b * Tcl * 2;
-    if (s_ss >= 0) {
-        const size_t lap = ss.lap_index(b, s_ss);
-        copy_lap_block(ss, lap, cx, cu, min(Trec, ss.Tmax));
-        __syncthreads();
-        lap_cost_block(ss, lap, TrackLength);
-    }
-    if (s_md >= 0) copy_lap_block(model, model.lap_index(b, s_md), cx, cu, min(Trec, model.Tmax));
+    if (s_ss >= 0) copy_ss_lap_block(ss, ss.lap_index(b, s_ss), cx, cu, Trec, TrackLength);
+    if (s_md >= 0) copy_lap_block(model, model.lap_index(b, s_md), cx, cu, Trec);
     __syncthreads();
     if (threadIdx.x == 0) {
         int f = book_refresh(k, b);
         if (s_ss == -2) f |= 64;                                 // safe-set pool too small for numSS_it + 2 laps
         if (f && flags_or) flags_or[b] |= f;
-        cl_len[b] = 0;
-        x_cur[(size_t)b * 6 + 4] -= TrackLength;
-        timeStep[b] = 0;
-        done[b] = 0;
+        restart_record(b, cl_len, x_cur, timeStep, done, TrackLength);
     }
 }
 
@@ -203,20 +188,11 @@ __global__ void __launch_bounds__(256) seed_books_kernel(int batch, LapPool ss, 
             s_md = book_md_add(k, b, min(Trec, model.Tmax));
         }
         __syncthreads();
-        if (s_ss >= 0) {
-            const size_t lap = ss.lap_index(b, s_ss);
-            copy_lap_block(ss, lap, cx, cu, min(Trec, ss.Tmax));
-            __syncthreads();
-            lap_cost_block(ss, lap, TrackLength);
-        }
-        if (s_md >= 0) copy_lap_block(model, model.lap_index(b, s_md), cx, cu, min(Trec, model.Tmax));
+        if (s_ss >= 0) copy_ss_lap_block(ss, ss.lap_index(b, s_ss), cx, cu, Trec, TrackLength);
+        if (s_md >= 0) copy_lap_block(model, model.lap_index(b, s_md), cx, cu, Trec);
         __syncthreads();
     }
-    for (int e = threadIdx.x; e < (N + 1) * 6; e += blockDim.x) xLin[(size_t)b * (N + 1) * 6 + e] = cx[6 + e];     // PC.py:432
-    for (int e = threadIdx.x; e < N * 2; e += blockDim.x) uLin[(size_t)b * N * 2 + e] = cu[2 + e];                 // PC.py:433
-    __syncthreads();
-    if (threadIdx.x < 6) zt[(size_t)b * 6 + threadIdx.x] = (threadIdx.x == 4) ? 10.0 : 0.0;                         // PC.py:330
-    if (threadIdx.x < 2) OldInput[(size_t)b * 2 + threadIdx.x] = 0.0;
+    seed_state_block(b, N, cx, cu, xLin, uLin, zt, OldInput);
     if (threadIdx.x == 0) { book_refresh(k, b); timeStep[b] = 0; hasPred[b] = 0; cl_len[b] = 0; done[b] = 0; }
 }
 
@@ -278,7 +254,7 @@ __global__ void __launch_bounds__(1024) pool_local_best_kernel(int batch, LapPoo
     }
 }
 
-// Pack the latest own lap of the chosen controllers: rows[G][kbest][Tpad][9] = (x 6 | u 2 | Qfun 1), meta[G][kbest][4].
+// Pack the latest own lap of the chosen controllers into exchange rows rows[G][kbest][Tpad][XR_COLS], meta[G][kbest][4].
 // One CTA per row r = g * kbest + j.
 __global__ void __launch_bounds__(256) pool_export_kernel(LapPool ss, LapBooks k, const int* best_inst, int kbest, int Tpad,
                                                           long long gid_base, double* rows, int* meta) {
@@ -287,15 +263,7 @@ __global__ void __launch_bounds__(256) pool_export_kernel(LapPool ss, LapBooks k
     const int sl = b < 0 ? -1 : k.prevslot[b];
     const size_t lap = ss.lap_index(b < 0 ? 0 : b, sl < 0 ? 0 : sl);
     const int T = sl < 0 ? 0 : min(ss.len[lap], Tpad);
-    const double* X = ss.x + lap * ss.Tmax * 6;
-    const double* U = ss.u + lap * ss.Tmax * 2;
-    const double* Q = ss.q + lap * ss.Tmax;
-    for (int e = threadIdx.x; e < Tpad * 9; e += blockDim.x) {
-        const int t = e / 9, j = e - t * 9;
-        double v = 0.0;
-        if (t < T) v = (j < 6) ? X[t * 6 + j] : (j < 8 ? U[t * 2 + (j - 6)] : Q[t]);
-        rows[(size_t)r * Tpad * 9 + e] = v;
-    }
+    pack_lap_row_block(ss, lap, T, Tpad, rows + (size_t)r * Tpad * XR_COLS);
     if (threadIdx.x == 0) {
         meta[r * 4 + 0] = T;
         meta[r * 4 + 1] = sl < 0 ? 0x7fffffff : k.ss_time[(size_t)b * k.ss_cap + sl];
@@ -355,30 +323,10 @@ __global__ void __launch_bounds__(256) pool_import_kernel(int batch, LapPool ss,
         }
         __syncthreads();
         const int c_ss = s_ss, c_md = s_md;                       // private copies: thread 0 rewrites the shared ones next round
-        const double* R = rows + (size_t)s_src * Tpad * 9;
-        if (c_ss >= 0) {
-            const int T = min(len, min(Tpad, ss.Tmax));
-            const size_t lap = ss.lap_index(b, c_ss);
-            for (int e = threadIdx.x; e < T * 9; e += blockDim.x) {
-                const int t = e / 9, j = e - t * 9;
-                const double v = R[e];
-                if (j < 6) ss.x[(lap * ss.Tmax + t) * 6 + j] = v;
-                else if (j < 8) ss.u[(lap * ss.Tmax + t) * 2 + (j - 6)] = v;
-                else ss.q[lap * ss.Tmax + t] = v;
-            }
-            if (threadIdx.x == 0) { ss.len[lap] = T; if (took) atomicAdd(took, 1); }
-        }
-        if (c_md >= 0) {                                          // the model stores the lap as driven: rows up to the finish line
-            const int Tm = min(lt, min(len, model.Tmax));
-            const size_t lap = model.lap_index(b, c_md);
-            for (int e = threadIdx.x; e < Tm * 8; e += blockDim.x) {
-                const int t = e >> 3, j = e & 7;
-                const double v = R[t * 9 + j];
-                if (j < 6) model.x[(lap * model.Tmax + t) * 6 + j] = v;
-                else model.u[(lap * model.Tmax + t) * 2 + (j - 6)] = v;
-            }
-            if (threadIdx.x == 0) model.len[lap] = Tm;
-        }
+        const double* R = rows + (size_t)s_src * Tpad * XR_COLS;
+        if (c_ss >= 0) file_ss_row_block(ss, ss.lap_index(b, c_ss), R, min(len, min(Tpad, ss.Tmax)), took);
+        // the model stores the lap as driven: rows up to the finish line
+        if (c_md >= 0) file_model_row_block(model, model.lap_index(b, c_md), R, min(lt, min(len, model.Tmax)));
         __syncthreads();
         if (threadIdx.x == 0 && c_ss == -2 && flags_or) flags_or[b] |= 64;
     }

@@ -1503,15 +1503,6 @@ int lmpc_rollout_commit_laps(lmpc_handle* h, const int* fin, const int* ss_slots
     return LMPC_OK;
 }
 
-int lmpc_rollout_export_laps_dev(lmpc_handle* h, int Tpad, double* rows_dev, int* lens_dev) {
-    if (int rc = need_rollout(h)) return rc;
-    if (!rows_dev || !lens_dev || Tpad < 1) return fail(LMPC_E_INVALID, "bad export arguments");
-    export_laps_kernel<<<h->batch, 256, 0, h->stream>>>(h->batch, h->d_clx, h->d_clu, h->d_cllen, h->Tcl, Tpad, rows_dev, lens_dev);
-    CK(cudaGetLastError());
-    h->launches += 1;
-    return LMPC_OK;
-}
-
 int lmpc_ss_export_laps_dev(lmpc_handle* h, const int* slots, int Tpad, double* rows_dev, int* lens_dev) {
     if (int rc = need_store(h)) return rc;
     if (!slots || !rows_dev || !lens_dev || Tpad < 1) return fail(LMPC_E_INVALID, "bad export arguments");

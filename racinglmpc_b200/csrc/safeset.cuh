@@ -597,79 +597,6 @@ __global__ void ss_add_point_kernel(int batch, LapPool pool, const int* prev_slo
     pool.len[lap] = T + 1;
 }
 
-// Pack every instance's closed-loop record into rows[B][Tpad][8] = (x | u) + lens[B]: the send buffer of the per-lap
-// all-gather of the pooled-safe-set mode (SURVEY §8e).
-__global__ void export_laps_kernel(int batch, const double* cl_x, const double* cl_u, const int* cl_len, int Tcl, int Tpad,
-                                   double* rows, int* lens) {
-    const int b = blockIdx.x;
-    if (b >= batch) return;
-    const int T = min(cl_len[b], Tpad);
-    for (int e = threadIdx.x; e < Tpad * 8; e += blockDim.x) {
-        const int t = e >> 3, j = e & 7;
-        double v = 0.0;
-        if (t < T) v = (j < 6) ? cl_x[((size_t)b * Tcl + t) * 6 + j] : cl_u[((size_t)b * Tcl + t) * 2 + (j - 6)];
-        rows[(size_t)b * Tpad * 8 + e] = v;
-    }
-    if (threadIdx.x == 0) lens[b] = T;
-}
-
-// Pooled-safe-set exchange (SURVEY §8e): pack one stored lap per instance, slot[b] (< 0: none), into
-// rows[B][Tpad][9] = (x 6 | u 2 | Qfun 1) + lens[B] -- the send buffer of the once-per-lap all-gather ...
-__global__ void ss_export_laps_kernel(int batch, LapPool pool, const int* slot, int Tpad, double* rows, int* lens) {
-    const int b = blockIdx.x;
-    if (b >= batch) return;
-    const int sl = slot[b];
-    const size_t lap = pool.lap_index(b, sl < 0 ? 0 : sl);
-    const int T = sl < 0 ? 0 : min(pool.len[lap], Tpad);
-    const double* X = pool.x + lap * pool.Tmax * 6;
-    const double* U = pool.u + lap * pool.Tmax * 2;
-    const double* Q = pool.q + lap * pool.Tmax;
-    for (int e = threadIdx.x; e < Tpad * 9; e += blockDim.x) {
-        const int t = e / 9, j = e - t * 9;
-        double v = 0.0;
-        if (t < T) v = (j < 6) ? X[t * 6 + j] : (j < 8 ? U[t * 2 + (j - 6)] : Q[t]);
-        rows[(size_t)b * Tpad * 9 + e] = v;
-    }
-    if (threadIdx.x == 0) lens[b] = T;
-}
-
-// ... and its receive side: instance b stores gathered lap src[b] (index into rows[G][Tpad][9], < 0: skip) in safe-set slot
-// ss_slot[b] and, when model_slot[b] >= 0, in the regression-model pool too (main.py:117-119 adds a lap to both).
-__global__ void ss_import_laps_kernel(int batch, LapPool ss, LapPool model, const int* ss_slot, const int* model_slot, const int* src,
-                                      int Tpad, const double* rows, const int* lens) {
-    const int b = blockIdx.x;
-    if (b >= batch) return;
-    const int g = src[b];
-    if (g < 0) return;
-    const double* R = rows + (size_t)g * Tpad * 9;
-    const int T = min(lens[g], min(Tpad, ss.Tmax));
-    if (ss_slot[b] >= 0) {
-        const size_t lap = ss.lap_index(b, ss_slot[b]);
-        for (int e = threadIdx.x; e < T * 9; e += blockDim.x) {
-            const int t = e / 9, j = e - t * 9;
-            const double v = R[e];
-            if (j < 6) ss.x[(lap * ss.Tmax + t) * 6 + j] = v;
-            else if (j < 8) ss.u[(lap * ss.Tmax + t) * 2 + (j - 6)] = v;
-            else ss.q[lap * ss.Tmax + t] = v;
-        }
-        if (threadIdx.x == 0) ss.len[lap] = T;
-    }
-    if (model_slot && model_slot[b] >= 0) {
-        // the model stores the lap as driven (rows up to the finish line, Qfun > 0 ... = 0), not the addPoint overrun
-        int Tm = 0;
-        for (int t = 0; t < T; ++t) { if (R[t * 9 + 8] >= 0.0) Tm = t + 1; }
-        Tm = min(Tm, model.Tmax);
-        const size_t lap = model.lap_index(b, model_slot[b]);
-        for (int e = threadIdx.x; e < Tm * 8; e += blockDim.x) {
-            const int t = e >> 3, j = e & 7;
-            const double v = R[t * 9 + j];
-            if (j < 6) model.x[(lap * model.Tmax + t) * 6 + j] = v;
-            else model.u[(lap * model.Tmax + t) * 2 + (j - 6)] = v;
-        }
-        if (threadIdx.x == 0) model.len[lap] = Tm;
-    }
-}
-
 // LMPC.computeCost (PC.py:447-464) for one stored lap, block-parallel: the reference counts backwards
 //   Q[T-1] = 0;  Q[j] = Q[j+1] + 1 if s_j < TrackLength else 0
 // i.e. Q[j] = (first row r >= j that is the last row or has s_r >= TrackLength) - j.  Chunks of blockDim rows are walked from
@@ -704,13 +631,95 @@ __device__ void lap_cost_block(const LapPool& pool, size_t lap, double TrackLeng
     }
 }
 
+// ---- lap hand-over primitives ---------------------------------------------------------------------------------------------
+// The host-slot kernels below (slots chosen by the Python lap books) and the device-book kernels of lapbooks.cuh (slots chosen
+// on the device) copy laps only through these, so both keep stored laps bit-identical.  The *_block functions are called by
+// every thread of the CTA; those with a barrier only from a path that is uniform across the CTA.
+
+// Copy the first min(T, Tmax) rows of (x | u) of a closed-loop record into a pool slot.
+__device__ inline void copy_lap_block(const LapPool& pool, size_t lap, const double* cx, const double* cu, int T) {
+    T = min(T, pool.Tmax);
+    for (int e = threadIdx.x; e < T * 6; e += blockDim.x) pool.x[lap * pool.Tmax * 6 + e] = cx[e];
+    for (int e = threadIdx.x; e < T * 2; e += blockDim.x) pool.u[lap * pool.Tmax * 2 + e] = cu[e];
+    if (threadIdx.x == 0) pool.len[lap] = T;
+}
+
+// The same into a safe-set slot, followed by the lap's cost-to-go (LMPC.computeCost).
+__device__ inline void copy_ss_lap_block(const LapPool& ss, size_t lap, const double* cx, const double* cu, int T, double TrackLength) {
+    copy_lap_block(ss, lap, cx, cu, T);
+    __syncthreads();
+    lap_cost_block(ss, lap, TrackLength);
+}
+
+// Exchange row: one lap as both lap exchanges ship it, [Tpad][XR_COLS] doubles, each lap row (x 6 | u 2 | Qfun 1), zero past
+// the lap's length.  A model slot takes the first XR_Q columns.
+constexpr int XR_U = 6;       // first column of u
+constexpr int XR_Q = 8;       // column of Qfun
+constexpr int XR_COLS = 9;
+
+// Pack the first T rows of a stored safe-set lap into exchange row R.
+__device__ inline void pack_lap_row_block(const LapPool& ss, size_t lap, int T, int Tpad, double* R) {
+    const double* X = ss.x + lap * ss.Tmax * 6;
+    const double* U = ss.u + lap * ss.Tmax * 2;
+    const double* Q = ss.q + lap * ss.Tmax;
+    for (int e = threadIdx.x; e < Tpad * XR_COLS; e += blockDim.x) {
+        const int t = e / XR_COLS, j = e - t * XR_COLS;
+        double v = 0.0;
+        if (t < T) v = (j < XR_U) ? X[t * 6 + j] : (j < XR_Q ? U[t * 2 + (j - XR_U)] : Q[t]);
+        R[e] = v;
+    }
+}
+
+// File the first T rows of exchange row R into a safe-set slot, Qfun included, and count the lap in *filed when given (here,
+// in thread 0's one block of writes: counted by the caller after the call, pool_import_kernel takes 40 registers instead of 32).
+__device__ inline void file_ss_row_block(const LapPool& ss, size_t lap, const double* R, int T, int* filed = nullptr) {
+    for (int e = threadIdx.x; e < T * XR_COLS; e += blockDim.x) {
+        const int t = e / XR_COLS, j = e - t * XR_COLS;
+        const double v = R[e];
+        if (j < XR_U) ss.x[(lap * ss.Tmax + t) * 6 + j] = v;
+        else if (j < XR_Q) ss.u[(lap * ss.Tmax + t) * 2 + (j - XR_U)] = v;
+        else ss.q[lap * ss.Tmax + t] = v;
+    }
+    if (threadIdx.x == 0) { ss.len[lap] = T; if (filed) atomicAdd(filed, 1); }
+}
+
+// File the first Tm rows of exchange row R into a model slot.
+__device__ inline void file_model_row_block(const LapPool& model, size_t lap, const double* R, int Tm) {
+    for (int e = threadIdx.x; e < Tm * XR_Q; e += blockDim.x) {
+        const int t = e / XR_Q, j = e - t * XR_Q;
+        const double v = R[t * XR_COLS + j];
+        if (j < XR_U) model.x[(lap * model.Tmax + t) * 6 + j] = v;
+        else model.u[(lap * model.Tmax + t) * 2 + (j - XR_U)] = v;
+    }
+    if (threadIdx.x == 0) model.len[lap] = Tm;
+}
+
+// Restart the record of a finished lap (one thread): s -= TrackLength (SysModel.py:50), timeStep = 0 (PC.py:445), done = 0.
+__device__ __forceinline__ void restart_record(int b, int* cl_len, double* x_cur, int* timeStep, int* done, double TrackLength) {
+    cl_len[b] = 0;
+    x_cur[(size_t)b * 6 + 4] -= TrackLength;
+    timeStep[b] = 0;
+    done[b] = 0;
+}
+
+// The controller state a seeded controller starts from: xLin / uLin = rows 1..N+1 / 1..N of its record cx / cu (PC.py:432-433),
+// zt = [0,0,0,0,10,0] (PC.py:330), OldInput = 0.
+__device__ inline void seed_state_block(int b, int N, const double* cx, const double* cu, double* xLin, double* uLin, double* zt,
+                                        double* OldInput) {
+    for (int e = threadIdx.x; e < (N + 1) * 6; e += blockDim.x) xLin[(size_t)b * (N + 1) * 6 + e] = cx[6 + e];
+    for (int e = threadIdx.x; e < N * 2; e += blockDim.x) uLin[(size_t)b * N * 2 + e] = cu[2 + e];
+    __syncthreads();
+    if (threadIdx.x < 6) zt[(size_t)b * 6 + threadIdx.x] = (threadIdx.x == 4) ? 10.0 : 0.0;
+    if (threadIdx.x < 2) OldInput[(size_t)b * 2 + threadIdx.x] = 0.0;
+}
+
 __global__ void __launch_bounds__(256) rollout_cost_kernel(LapPool pool, int b, int slot, Tracks trk) {
     lap_cost_block(pool, pool.lap_index(b, slot), trk.of(b).TrackLength);
 }
 
 // Lap hand-over of every instance with fin[b] != 0, one CTA per instance (main.py:113-119 + SysModel.py:50 + PC.py:445):
 // the closed-loop record goes to safe-set slot ss_slot[b] (>= 0) with its cost-to-go and to regression slot model_slot[b]
-// (>= 0); then the record restarts, s -= TrackLength, timeStep = 0, done = 0.
+// (>= 0); then the record restarts.
 __global__ void __launch_bounds__(256) commit_laps_kernel(int batch, LapPool ss, LapPool model, const int* fin, const int* ss_slot,
                                                           const int* model_slot, const double* cl_x, const double* cl_u, int* cl_len,
                                                           int Tcl, double* x_cur, int* timeStep, int* done, Tracks trk) {
@@ -718,28 +727,41 @@ __global__ void __launch_bounds__(256) commit_laps_kernel(int batch, LapPool ss,
     if (b >= batch || !fin[b]) return;
     const int Trec = cl_len[b];
     const double TrackLength = trk.of(b).TrackLength;
-    if (ss_slot[b] >= 0) {
-        const int T = min(Trec, ss.Tmax);
-        const size_t lap = ss.lap_index(b, ss_slot[b]);
-        for (int e = threadIdx.x; e < T * 6; e += blockDim.x) ss.x[lap * ss.Tmax * 6 + e] = cl_x[(size_t)b * Tcl * 6 + e];
-        for (int e = threadIdx.x; e < T * 2; e += blockDim.x) ss.u[lap * ss.Tmax * 2 + e] = cl_u[(size_t)b * Tcl * 2 + e];
-        if (threadIdx.x == 0) ss.len[lap] = T;
-        __syncthreads();
-        lap_cost_block(ss, lap, TrackLength);
-    }
-    if (model_slot[b] >= 0) {
-        const int T = min(Trec, model.Tmax);
-        const size_t lap = model.lap_index(b, model_slot[b]);
-        for (int e = threadIdx.x; e < T * 6; e += blockDim.x) model.x[lap * model.Tmax * 6 + e] = cl_x[(size_t)b * Tcl * 6 + e];
-        for (int e = threadIdx.x; e < T * 2; e += blockDim.x) model.u[lap * model.Tmax * 2 + e] = cl_u[(size_t)b * Tcl * 2 + e];
-        if (threadIdx.x == 0) model.len[lap] = T;
-    }
+    const size_t rec = (size_t)b * Tcl;     // an offset, not two record pointers, lives across the safe-set store: 28 registers, not 31
+    if (ss_slot[b] >= 0) copy_ss_lap_block(ss, ss.lap_index(b, ss_slot[b]), cl_x + rec * 6, cl_u + rec * 2, Trec, TrackLength);
+    if (model_slot[b] >= 0) copy_lap_block(model, model.lap_index(b, model_slot[b]), cl_x + rec * 6, cl_u + rec * 2, Trec);
     __syncthreads();
-    if (threadIdx.x == 0) {
-        cl_len[b] = 0;
-        x_cur[(size_t)b * 6 + 4] -= TrackLength;
-        timeStep[b] = 0;
-        done[b] = 0;
+    if (threadIdx.x == 0) restart_record(b, cl_len, x_cur, timeStep, done, TrackLength);
+}
+
+// Pooled-safe-set exchange (SURVEY §8e): pack one stored lap per instance, slot[b] (< 0: none), into exchange rows
+// rows[B][Tpad][XR_COLS] + lens[B] -- the send buffer of the once-per-lap all-gather ...
+__global__ void ss_export_laps_kernel(int batch, LapPool pool, const int* slot, int Tpad, double* rows, int* lens) {
+    const int b = blockIdx.x;
+    if (b >= batch) return;
+    const int sl = slot[b];
+    const size_t lap = pool.lap_index(b, sl < 0 ? 0 : sl);
+    const int T = sl < 0 ? 0 : min(pool.len[lap], Tpad);
+    pack_lap_row_block(pool, lap, T, Tpad, rows + (size_t)b * Tpad * XR_COLS);
+    if (threadIdx.x == 0) lens[b] = T;
+}
+
+// ... and its receive side: instance b stores gathered lap src[b] (index into rows[G][Tpad][XR_COLS], < 0: skip) in safe-set
+// slot ss_slot[b] and, when model_slot[b] >= 0, in the regression-model pool too (main.py:117-119 adds a lap to both).
+__global__ void ss_import_laps_kernel(int batch, LapPool ss, LapPool model, const int* ss_slot, const int* model_slot, const int* src,
+                                      int Tpad, const double* rows, const int* lens) {
+    const int b = blockIdx.x;
+    if (b >= batch) return;
+    const int g = src[b];
+    if (g < 0) return;
+    const double* R = rows + (size_t)g * Tpad * XR_COLS;
+    const int T = min(lens[g], min(Tpad, ss.Tmax));
+    if (ss_slot[b] >= 0) file_ss_row_block(ss, ss.lap_index(b, ss_slot[b]), R, T);
+    if (model_slot && model_slot[b] >= 0) {
+        // the model stores the lap as driven (rows up to the finish line, Qfun > 0 ... = 0), not the addPoint overrun
+        int Tm = 0;
+        for (int t = 0; t < T; ++t) { if (R[t * XR_COLS + XR_Q] >= 0.0) Tm = t + 1; }
+        file_model_row_block(model, model.lap_index(b, model_slot[b]), R, min(Tm, model.Tmax));
     }
 }
 
@@ -990,8 +1012,8 @@ __global__ void __launch_bounds__(32) ridge_sysid_kernel(int batch, const double
 
 // Seed a controller from the closed-loop record the way main.py:99-110 does from the PID lap: the record is stored `copies`
 // times in the safe set (slots ss_slot0 ..) and in the regression model (slots model_slot0 ..), cost-to-go by computeCost,
-// xLin/uLin = rows 1..N+1 / 1..N of the lap (PC.py:432-433), zt = [0,0,0,0,10,0] (PC.py:330), OldInput = 0, timeStep = 0,
-// no previous prediction; the record restarts.  One CTA per instance.
+// the controller state from the record (seed_state_block), timeStep = 0, no previous prediction; the record restarts.  One CTA
+// per instance.
 __global__ void __launch_bounds__(256) seed_from_record_kernel(int batch, LapPool ss, LapPool model, int copies, int ss_slot0, int model_slot0,
                                                               const double* cl_x, const double* cl_u, int* cl_len, int Tcl, int N,
                                                               double* xLin, double* uLin, double* zt, double* OldInput, int* timeStep,
@@ -1000,29 +1022,13 @@ __global__ void __launch_bounds__(256) seed_from_record_kernel(int batch, LapPoo
     if (b >= batch) return;
     const int Trec = cl_len[b];
     const double TrackLength = trk.of(b).TrackLength;
+    const double* cx = cl_x + (size_t)b * Tcl * 6;
+    const double* cu = cl_u + (size_t)b * Tcl * 2;
     for (int c = 0; c < copies; ++c) {
-        {
-            const int T = min(Trec, ss.Tmax);
-            const size_t lap = ss.lap_index(b, ss_slot0 + c);
-            for (int e = threadIdx.x; e < T * 6; e += blockDim.x) ss.x[lap * ss.Tmax * 6 + e] = cl_x[(size_t)b * Tcl * 6 + e];
-            for (int e = threadIdx.x; e < T * 2; e += blockDim.x) ss.u[lap * ss.Tmax * 2 + e] = cl_u[(size_t)b * Tcl * 2 + e];
-            if (threadIdx.x == 0) ss.len[lap] = T;
-            __syncthreads();
-            lap_cost_block(ss, lap, TrackLength);
-        }
-        {
-            const int T = min(Trec, model.Tmax);
-            const size_t lap = model.lap_index(b, model_slot0 + c);
-            for (int e = threadIdx.x; e < T * 6; e += blockDim.x) model.x[lap * model.Tmax * 6 + e] = cl_x[(size_t)b * Tcl * 6 + e];
-            for (int e = threadIdx.x; e < T * 2; e += blockDim.x) model.u[lap * model.Tmax * 2 + e] = cl_u[(size_t)b * Tcl * 2 + e];
-            if (threadIdx.x == 0) model.len[lap] = T;
-        }
+        copy_ss_lap_block(ss, ss.lap_index(b, ss_slot0 + c), cx, cu, Trec, TrackLength);
+        copy_lap_block(model, model.lap_index(b, model_slot0 + c), cx, cu, Trec);
     }
-    for (int e = threadIdx.x; e < (N + 1) * 6; e += blockDim.x) xLin[(size_t)b * (N + 1) * 6 + e] = cl_x[(size_t)b * Tcl * 6 + 6 + e];
-    for (int e = threadIdx.x; e < N * 2; e += blockDim.x) uLin[(size_t)b * N * 2 + e] = cl_u[(size_t)b * Tcl * 2 + 2 + e];
-    __syncthreads();
-    if (threadIdx.x < 6) zt[(size_t)b * 6 + threadIdx.x] = (threadIdx.x == 4) ? 10.0 : 0.0;
-    if (threadIdx.x < 2) OldInput[(size_t)b * 2 + threadIdx.x] = 0.0;
+    seed_state_block(b, N, cx, cu, xLin, uLin, zt, OldInput);
     if (threadIdx.x == 0) { timeStep[b] = 0; hasPred[b] = 0; cl_len[b] = 0; done[b] = 0; }
 }
 

@@ -2,7 +2,7 @@
 """Small-batch run of every kernel for compute-sanitizer (memcheck / racecheck / synccheck / initcheck):
     compute-sanitizer --tool racecheck python tools/sanitize.py
 Exercises: ftocp_kernel<12,0> and <12,48> (host + device entry points), knn_ltv_regress, ss_select, shift_state,
-ss_add_point, rollout_cost, sim_step, commit_laps, export_laps, ss_export_laps, ss_import_laps; round 2: the long-horizon kernel
+ss_add_point, rollout_cost, sim_step, commit_laps, ss_export_laps, ss_import_laps; round 2: the long-horizon kernel
 that reads its model in place (N = 48), warm-started solves, pid_input, seed_books, commit_laps_books, rollout_stats, the pooled
 exchange (pool_local_best / export / rank / import), trace_step and track_global_position."""
 import os
@@ -35,11 +35,9 @@ for _ in range(3):
     c.rollout_step(seed=1)
 done, n = c.rollout_done()
 c.rollout_finish_laps(np.array([1] + [0] * (B - 1), np.int32), n)
-rows = torch.zeros(B, 16, 8, dtype=torch.float64, device="cuda")
-lens = torch.zeros(B, dtype=torch.int32, device="cuda")
-c.rollout_export_laps(16, rows, lens)
 c.sync()
 # pooled-safe-set exchange: export a stored lap of every instance, hand instance 0's lap to the others
+lens = torch.zeros(B, dtype=torch.int32, device="cuda")
 rows9 = torch.zeros(B, 512, 9, dtype=torch.float64, device="cuda")
 c.export_laps([1] * B, 512, rows9, lens)
 took = c.import_laps(np.array([-1] + [0] * (B - 1)), np.full(B, 100), 512, rows9, lens)
