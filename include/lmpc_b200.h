@@ -241,7 +241,8 @@ int lmpc_state_get(lmpc_handle* h, double* xLin, double* uLin, double* zt, doubl
 
 /* K1 alone — MPC.computeLTVdynamics (PC.py:140-145) from the stored xLin/uLin: abc_out[B,N,54] (may be NULL: result
  * stays on the device for the next solve), flags[B] (0 ok; 1 singular regression, 2 curvature lookup failed,
- * 4 single neighbour in a lap — cases where the reference raises). */
+ * 4 single neighbour in a lap — cases where the reference raises; 32 more than 32 rows fell within the rounding margin of
+ * the MaxNumPoint-th neighbour, so the selection is not certified to be the reference's). */
 int lmpc_identify_host(lmpc_handle* h, double* abc_out, int* flags);
 /* K2 alone — LMPC.addTerminalComponents (PC.py:386-416) for x0[B,6]: outputs as in lmpc_solve_lmpc_host plus
  * min_index[B,numSS_it] (argmin row per lap) and flags[B] (8 = window past the stored lap). */
@@ -252,7 +253,8 @@ int lmpc_select_host(lmpc_handle* h, const double* x0, double* SS_sel, double* Q
  *   mode 0: LTV-MPC   K1 -> QP -> shift          (timeVarying MPC, main.py:91-94)
  *   mode 1: LMPC      K1 -> K2 -> QP -> shift    (main.py:113-120)
  * x0[B,6] host.  Outputs (host, any may be NULL): xPred[B,N+1,6], uPred[B,N,2], lambd[B,M], zt[B,6], zt_u[B,2],
- * SS_sel[B,6,M] (for SSStoredPredTraj, PC.py:379), status[B], iters[B], resid[B,3], flags[B] (K1/K2 bits). */
+ * SS_sel[B,6,M] (for SSStoredPredTraj, PC.py:379), status[B], iters[B], resid[B,3], flags[B] (K1/K2 bits: 1, 2, 4, 32 as in
+ * lmpc_identify_host, 8 as in lmpc_select_host). */
 int lmpc_step_host(lmpc_handle* h, int mode, const double* x0, double* xPred, double* uPred, double* lambd, double* zt,
                    double* zt_u, double* SS_sel, int* status, int* iters, double* resid, int* flags);
 /* Same with x0 already on the device; results stay in the handle's device buffers (lmpc_device_buffer). */

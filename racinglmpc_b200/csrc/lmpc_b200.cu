@@ -863,12 +863,15 @@ static int store_create_impl(lmpc_handle* h, const lmpc_model_params* mp, int ss
         if (ss_cap < h->p.numSS_it) return fail(LMPC_E_INVALID, "ss_cap < numSS_it");
     }
     CK(cudaSetDevice(h->device));
-    CK(cudaFuncSetAttribute(knn_ltv_regress_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024));
+    // the largest launch: trToUse = K1_MAXLAPS at K1_MAXWPB warps (102592 B, above a flat 100 KiB)
+    CK(cudaFuncSetAttribute(knn_ltv_regress_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            (int)k1_smem_bytes(K1_MAXLAPS, K1_MAXWPB)));
     CK(cudaFuncSetAttribute(knn_ltv_regress_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     ModelConst& m = h->mc;
     memset(&m, 0, sizeof(m));
     m.trToUse = mp->trToUse; m.MaxNumPoint = mp->MaxNumPoint; m.h = mp->h; m.lamb = mp->lamb; m.dt = mp->dt;
-    for (int i = 0; i < 5; ++i) m.scaling[i] = mp->scaling[i];
+    // |(x - q) s| == |(x - q) |s|| bit for bit, and the fp32 scan of K1 needs non-negative partial distances to order its keys
+    for (int i = 0; i < 5; ++i) m.scaling[i] = fabs(mp->scaling[i]);
     TrackRec& t = h->store_trk;
     memset(&t, 0, sizeof(t));
     t.nseg = mp->nseg;
@@ -1125,12 +1128,12 @@ int lmpc_state_get(lmpc_handle* h, double* xLin, double* uLin, double* zt, doubl
 static int launch_k1(lmpc_handle* h) {
     K1Args a;
     a.batch = h->batch; a.N = h->N;
-    a.wpb = h->N < 12 ? h->N : 12;
+    a.wpb = h->N < K1_MAXWPB ? h->N : K1_MAXWPB;
     a.pts_stride = k1_pts_stride(h->mc.trToUse);
     a.xLin = h->d_xLin; a.uLin = h->d_uLin; a.pool = h->mdl; a.used = h->d_used; a.abc = h->hb[0].abc; a.status = h->d_flags;
     a.trk = tracks(h);
     dim3 grid(h->batch, (h->N + a.wpb - 1) / a.wpb);
-    size_t smem = sizeof(float) * 5 * K1_TILE + sizeof(double) * (size_t)a.pts_stride * a.wpb;
+    const size_t smem = k1_smem_bytes(h->mc.trToUse, a.wpb);
     knn_ltv_regress_kernel<<<grid, 32 * a.wpb, smem, h->stream>>>(h->mc, a);
     CK(cudaGetLastError());
     h->launches += 1;

@@ -146,6 +146,11 @@ struct K1Args {
 //                   | re-scoring buffer: K1_CAND exact distances + K1_CAND row indices | the query point (5 doubles, +1 pad)
 constexpr int K1_PW = 15;        // doubles per selected point
 __host__ __device__ inline int k1_pts_stride(int trToUse) { return K1_MAXPTS * trToUse * K1_PW + 48 + 20 + K1_CAND + K1_CAND / 2 + 6; }
+constexpr int K1_MAXWPB = 12;    // warps per block (__launch_bounds__ below)
+// dynamic shared memory of a launch: the fp32 tile + the per-warp scratch
+inline size_t k1_smem_bytes(int trToUse, int wpb) {
+    return sizeof(float) * 5 * K1_TILE + sizeof(double) * (size_t)k1_pts_stride(trToUse) * wpb;
+}
 
 // The reference's distance of one stored row to the query (PM.py:185-186): diff = (Data - x) * scaling, 1-norm summed left to
 // right (numpy semantics for 5 columns), in IEEE fp64 with no contraction: the value np.argsort ranks.
@@ -181,7 +186,7 @@ __constant__ signed char K1_ABC_SRC[54] = {
 #ifndef LMPC_K1_MINBLOCKS
 #define LMPC_K1_MINBLOCKS 3
 #endif
-__global__ void __launch_bounds__(32 * 12, LMPC_K1_MINBLOCKS) knn_ltv_regress_kernel(const __grid_constant__ ModelConst m, const K1Args a) {
+__global__ void __launch_bounds__(32 * K1_MAXWPB, LMPC_K1_MINBLOCKS) knn_ltv_regress_kernel(const __grid_constant__ ModelConst m, const K1Args a) {
     extern __shared__ __align__(16) unsigned char k1_smem[];
     const int b = a.b0 + blockIdx.x;
     const int wib = threadIdx.x >> 5;
@@ -261,11 +266,13 @@ __global__ void __launch_bounds__(32 * 12, LMPC_K1_MINBLOCKS) knn_ltv_regress_ke
         }
         if (!active) continue;
         // ---- G = an upper bound of the k-th smallest key: the k-th smallest of the 32 lane minima (k distinct rows are at or
-        //      below it); one REDUX.MIN per round
+        //      below it); one REDUX.MIN per round.  At least two rounds: the flag-4 count below needs every row inside h as a
+        //      candidate whenever fewer than two are, also at MaxNumPoint = 1
         unsigned G = 0xffffffffu;
         {
             unsigned cur = k0;
-            for (int rnd = 0; rnd < kk; ++rnd) {
+            const int kg = kk > 2 ? kk : 2;
+            for (int rnd = 0; rnd < kg; ++rnd) {
                 G = __reduce_min_sync(0xffffffffu, cur);
                 cur = (cur == G) ? 0xffffffffu : cur;
             }

@@ -3,7 +3,7 @@
 
 The reference has no tests of its own (SURVEY §4); these are the cases its code branches on:
 few / one neighbour (exact distance ties inside one lap are implementation-defined in the reference: np.argsort's default
-sort is not stable; the kernel takes the lowest rows), laps that straddle the kernel's 256-row tiles, the two selection-window rules, the window
+sort is not stable; the kernel takes the lowest rows), laps of assorted lengths, the two selection-window rules, the window
 running off a lap (the reference: IndexError), a full lap pool, unsupported sizes and null arguments."""
 import ctypes as C
 import numpy as np
@@ -58,7 +58,8 @@ def _oracle_abc(track, laps, xLin, uLin, N, trToUse):
 
 @pytest.mark.parametrize("T", [40, 256, 257, 258, 513, 1000])
 def test_k1_lap_lengths_across_tile_boundaries(track, T):
-    """Rows 0..T-2 are candidates (PM.py:183); the kernel stages 256-row tiles."""
+    """Rows 0..T-2 are candidates (PM.py:183) on random laps; the tile-edge lengths of the scan (LMPC_K1_TILE) are the
+    parametrisation of test_gpu_knn_regression.py."""
     _need_gpu()
     rng = np.random.default_rng(T)
     N = 12
