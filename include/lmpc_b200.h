@@ -277,7 +277,7 @@ void* lmpc_device_buffer(lmpc_handle* h, const char* name);
  *   Controller.solve(x) -> u = uPred[0] -> Controller.addPoint(x,u) -> x+ = Simulator.dynModel(x, x_glob, u)
  * (100 explicit-Euler sub-steps of the dynamic bicycle model with Pacejka tyres, SysModel.py:56-147).
  * z_host[B,3] = standard-normal draws for the (vx, vy, wz) noise in the reference's order; NULL = Philox4x32-10 on the
- * device keyed by (seed, instance, step).  The visited (x, u) pairs are recorded per instance (Tcl rows). */
+ * device keyed by (seed, stream, step), stream = instance unless lmpc_rollout_set_noise_streams says otherwise.  The visited (x, u) pairs are recorded per instance (Tcl rows). */
 int lmpc_rollout_create(lmpc_handle* h, int Tcl);
 int lmpc_rollout_set_state(lmpc_handle* h, const double* x, const double* xglob);              /* [B,6] host, may be NULL */
 int lmpc_rollout_get_state(lmpc_handle* h, double* x, double* xglob, int* done, int* cl_len);  /* any may be NULL      */
@@ -316,6 +316,34 @@ typedef struct lmpc_vehicle_params {
  *     another car drove is not a feasible trajectory of this one, so a clean plant sweep puts each car in its own group
  *     (lmpc_set_pool_groups). */
 int lmpc_rollout_set_vehicles(lmpc_handle* h, const lmpc_vehicle_params* sets, int nsets, const int* set_of_instance);
+/* Noise model of the device closed loop: the clipped Gaussian noise of Simulator.dynModel and of the PID path follower. */
+typedef struct lmpc_noise_params {
+    double sim_sigma[3];          /* vx, vy, wz: 0.01, 0.01, 0.005      SysModel.py:139-141 */
+    double sim_clip[3];           /* 0.05, 0.05, 0.05                                       */
+    double sim_gain;              /* 0.01                               SysModel.py:143-145 */
+    double pid_sigma[2];          /* steering, acceleration: 0.25, 0.10 Utilities.py:42-68  */
+    double pid_clip[2];           /* 0.9, 0.2                                               */
+} lmpc_noise_params;
+/* Per-controller noise models (robustness studies; no reference counterpart: the reference has one noise level).  Controller b
+ * draws its noise with sets[set_of_instance[b]] (host arrays) in every later lmpc_rollout_step (modes 0, 1, 2) and
+ * lmpc_rollout_pid_step, in the reference's form and operation order per channel j:
+ *   simulator  n_j = fmax(-sim_clip_j, fmin(z_j * sim_sigma_j, sim_clip_j)),  x_j += sim_gain * n_j  (curvilinear copy only)
+ *   PID        u_j += fmax(-pid_clip_j, fmin(z_j * pid_sigma_j, pid_clip_j))
+ * with z_j the standard-normal draws (Philox, or z_host / z_pid_host / z_sim_host when given).  nsets == 0 (sets,
+ * set_of_instance NULL) returns to the reference's constants, which every handle starts with.
+ *   - 1 <= nsets <= batch, every index in [0, nsets); every value finite and >= 0 (zero sigma or clip: a noise-free channel).
+ *   - Any failed check returns LMPC_E_INVALID and leaves the handle as it was.
+ *   - The call synchronises the handle's streams before it replaces the table.  It is allowed at any time: a noise change in
+ *     the middle of a run applies from the next step on.
+ *   - The noise index is independent of the parameter-set, vehicle, track and pool-group indices. */
+int lmpc_rollout_set_noise(lmpc_handle* h, const lmpc_noise_params* sets, int nsets, const int* set_of_instance);
+/* Noise streams (common random numbers): the Philox draws of controller b are keyed by (seed, stream_of_instance[b], clock) in
+ * the simulator and by (seed ^ constant, stream_of_instance[b], clock) in the PID, so controllers on one stream meet the same
+ * draws -- two tunings run on one stream share their PID lap, their seeded stores and every later draw, and compare in pairs.
+ * stream_of_instance is a host array [batch] of numbers >= 0; repeats are allowed.  NULL returns to stream b = b, which every
+ * handle starts with.  Host-given draws (z_host, z_pid_host, z_sim_host) do not use the streams.  Checks, refusal and
+ * synchronisation as lmpc_rollout_set_noise. */
+int lmpc_rollout_set_noise_streams(lmpc_handle* h, const int* stream_of_instance);
 int lmpc_rollout_sysid(lmpc_handle* h, double lamb, double* abc_host, int* flags_host);
 int lmpc_rollout_seed_from_record(lmpc_handle* h, int copies, int ss_slot0, int model_slot0);
 int lmpc_rollout_get_lap(lmpc_handle* h, int inst, int* T, double* x, double* u);              /* closed-loop record   */
@@ -404,8 +432,8 @@ int lmpc_set_pool_min_overrun(lmpc_handle* h, int rows);
  * What a controller of the device-resident step has learned and where it is, as one fixed-size byte record per controller:
  * both lap pools, the lap books, the controller state, the warm-start record, and with a rollout the simulator state, the
  * closed-loop record, the health counters and the LTI model (DESIGN.md, "Controller snapshots", lists every per-controller buffer
- * as carried or scratch).  Not in a record: what the handle is told to drive -- parameter sets, vehicles, tracks, pool groups --
- * and handle-wide counters.  The lap books travel in the record, so a caller that keeps its own host copy of them (the
+ * as carried or scratch).  Not in a record: what the handle is told to drive -- parameter sets, vehicles, tracks, noise sets,
+ * noise streams, pool groups -- and handle-wide counters.  The lap books travel in the record, so a caller that keeps its own host copy of them (the
  * host-driven bookkeeping of lmpc_ss_set_selection / lmpc_model_set_used) must not restore into its handle.
  * Record = header (below) + sections at 16-byte aligned offsets; every section is one controller's slice of one [B][...] buffer. */
 #define LMPC_SNAPSHOT_MAGIC 0x50414e53      /* "SNAP" */
@@ -438,7 +466,7 @@ int lmpc_snapshot_pack_dev(lmpc_handle* h, int n, const int* inst_host, void* re
  * yet (no device-resident step since lmpc_store_create); otherwise every record's mode must be -1 or the handle's.  A successful
  * unpack counts as a stored lap (lmpc_set_tracks then returns LMPC_E_STATE).  The copy is enqueued on the handle's stream. */
 int lmpc_snapshot_unpack_dev(lmpc_handle* h, const void* rec_dev, int nrec, int n, const int* dst_host, const int* rec_of_dst_host);
-/* The simulator's step counter, which keys the Philox noise with (seed, controller, step).  Requires lmpc_rollout_create. */
+/* The simulator's step counter, which keys the Philox noise with (seed, stream, step).  Requires lmpc_rollout_create. */
 int lmpc_rollout_get_clock(lmpc_handle* h, unsigned long long* step);
 int lmpc_rollout_set_clock(lmpc_handle* h, unsigned long long step);
 
@@ -466,6 +494,7 @@ int lmpc_sizeof_params(void);
 int lmpc_sizeof_model_params(void);
 int lmpc_sizeof_vehicle_params(void);
 int lmpc_sizeof_track_params(void);
+int lmpc_sizeof_noise_params(void);
 
 #ifdef __cplusplus
 }

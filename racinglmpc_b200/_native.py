@@ -35,6 +35,13 @@ class VehicleParams(C.Structure):
     _fields_ = [(f, C.c_double) for f in ("m", "lf", "lr", "Iz", "Df", "Cf", "Bf", "Dr", "Cr", "Br")]
 
 
+class NoiseParams(C.Structure):
+    """lmpc_noise_params: the clipped Gaussian noise of Simulator.dynModel (SysModel.py:139-145) and of the PID path follower
+    (Utilities.py:42-68)."""
+    _fields_ = [("sim_sigma", C.c_double * 3), ("sim_clip", C.c_double * 3), ("sim_gain", C.c_double),
+                ("pid_sigma", C.c_double * 2), ("pid_clip", C.c_double * 2)]
+
+
 class TrackParams(C.Structure):
     """lmpc_track_params: the [s_start, length, curvature] rows of Map.PointAndTangent and the lap length."""
     _fields_ = [("nseg", C.c_int), ("seg", C.c_double * (MAX_SEG * 3)), ("TrackLength", C.c_double)]
@@ -124,6 +131,8 @@ def lib():
     L.lmpc_rollout_get_health.argtypes = [_vp, _vp, _vp]
     L.lmpc_rollout_pid_step.argtypes = [_vp, C.c_double, _vp, _vp, C.c_ulonglong]
     L.lmpc_rollout_set_vehicles.argtypes = [_vp, C.POINTER(VehicleParams), C.c_int, _vp]
+    L.lmpc_rollout_set_noise.argtypes = [_vp, C.POINTER(NoiseParams), C.c_int, _vp]
+    L.lmpc_rollout_set_noise_streams.argtypes = [_vp, _vp]
     L.lmpc_set_tracks.argtypes = [_vp, C.POINTER(TrackParams), C.c_int, _vp]
     L.lmpc_rollout_sysid.argtypes = [_vp, C.c_double, _vp, _vp]
     L.lmpc_rollout_seed_from_record.argtypes = [_vp, C.c_int, C.c_int, C.c_int]
@@ -160,6 +169,8 @@ def lib():
     L.lmpc_sizeof_model_params.restype = C.c_int
     L.lmpc_sizeof_vehicle_params.restype = C.c_int
     L.lmpc_sizeof_track_params.restype = C.c_int
+    L.lmpc_sizeof_noise_params.restype = C.c_int
+    assert L.lmpc_sizeof_noise_params() == C.sizeof(NoiseParams), "lmpc_noise_params ABI mismatch"
     assert L.lmpc_sizeof_params() == C.sizeof(Params), "lmpc_params ABI mismatch"
     assert L.lmpc_sizeof_model_params() == C.sizeof(ModelParams), "lmpc_model_params ABI mismatch"
     assert L.lmpc_sizeof_vehicle_params() == C.sizeof(VehicleParams), "lmpc_vehicle_params ABI mismatch"
@@ -294,7 +305,8 @@ def make_params(p, numSS_Points=0, numSS_it=0, QterminalSlack=None, eps_res=0.0,
 
 
 def _set_index(index, K, batch, what):
-    """The index rules of the per-controller tables (lmpc_set_param_sets, lmpc_rollout_set_vehicles, lmpc_set_tracks) and of the pool
+    """The index rules of the per-controller tables (lmpc_set_param_sets, lmpc_rollout_set_vehicles, lmpc_rollout_set_noise,
+    lmpc_set_tracks) and of the pool
     groups (lmpc_set_pool_groups): 1 <= K <= batch rows and
     one integer row number in [0, K) per controller.  Returns the index as a contiguous int32 array; raises ValueError."""
     if index is None:
@@ -356,6 +368,50 @@ def make_vehicle_sets(vehicles, index, batch):
             raise ValueError("vehicle %d: m, Iz, lf and lr must be positive" % k)
         out[k] = VehicleParams(*vals)
     return out, idx
+
+
+NOISE_FIELDS = tuple(f for f, _ in NoiseParams._fields_)
+
+
+def make_noise_sets(noises, index, batch):
+    """Per-controller noise models for ``lmpc_rollout_set_noise``: K objects ``noises`` with the fields of NoiseParams
+    (sim_sigma[3], sim_clip[3], sim_gain, pid_sigma[2], pid_clip[2]; e.g. reference_params.NoiseParams) and the noise set of every
+    controller ``index[batch]``.  Raises ValueError where the library would refuse: the index rules of ``make_param_sets``, a
+    field of the wrong length, or a value that is not finite or is negative.  Returns (ctypes array NoiseParams * K, int32 index
+    array)."""
+    noises = list(noises)
+    K = len(noises)
+    idx = _set_index(index, K, batch, "noise sets")
+    out = (NoiseParams * K)()
+    for k, n in enumerate(noises):
+        for f, ct in NoiseParams._fields_:
+            v = np.asarray(getattr(n, f), dtype=float).reshape(-1)
+            want = getattr(ct, "_length_", 1)
+            if v.shape[0] != want:
+                raise ValueError("noise set %d: %s needs %d value%s, got %d" % (k, f, want, "s" if want > 1 else "", v.shape[0]))
+            if not np.all(np.isfinite(v)) or np.any(v < 0):
+                raise ValueError("noise set %d: %s must be finite and >= 0" % (k, f))
+            if want > 1:
+                getattr(out[k], f)[:] = v.tolist()
+            else:
+                setattr(out[k], f, float(v[0]))
+    return out, idx
+
+
+def make_noise_streams(streams, batch):
+    """Noise streams for ``lmpc_rollout_set_noise_streams``: one integer stream number >= 0 per controller ``streams[batch]``
+    (repeats allowed: controllers on one stream meet the same Philox draws).  ``None`` (stream b = b) returns None.  Raises
+    ValueError where the library would refuse.  Returns the int32 stream array."""
+    if streams is None:
+        return None
+    s = np.asarray(streams).reshape(-1)
+    with np.errstate(invalid="ignore"):              # NaN or an out-of-range value fails the comparison below
+        out = np.ascontiguousarray(s, dtype=np.int32)
+    if out.shape[0] != batch or not np.array_equal(out, s):
+        raise ValueError("streams must hold one integer stream number per controller (%d)" % batch)
+    if out.min() < 0:
+        raise ValueError("stream numbers must be >= 0")
+    return out
 
 
 def make_pool_groups(index, ngroups, batch):

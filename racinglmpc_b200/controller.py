@@ -116,6 +116,28 @@ class BatchedController:
         sets, idx = nat.make_vehicle_sets(vehicles, index, self.B)
         nat.check(self._lib.lmpc_rollout_set_vehicles(self._h, sets, len(sets), nat.ptr(idx)))
 
+    def set_noise(self, noises, index=None):
+        """Per-controller noise models of the device closed loop (a robustness study in one batch): controller b draws the
+        simulator's and the PID's noise with ``noises[index[b]]`` (objects with the fields of reference_params.NoiseParams) in
+        every later ``rollout_step`` and ``rollout_pid_step``, Philox or host-given draws alike.  ``index`` is required with
+        ``noises``.  ``noises=None`` (no index) returns to the reference's noise.  Independent of ``set_param_sets``,
+        ``set_vehicles``, ``set_tracks`` and the pool groups; allowed in the middle of a run.  Waits for work already enqueued."""
+        if noises is None:
+            if index is not None:
+                raise ValueError("noises=None reverts to the reference's noise and takes no index")
+            nat.check(self._lib.lmpc_rollout_set_noise(self._h, None, 0, None))
+            return
+        sets, idx = nat.make_noise_sets(noises, index, self.B)
+        nat.check(self._lib.lmpc_rollout_set_noise(self._h, sets, len(sets), nat.ptr(idx)))
+
+    def set_noise_streams(self, streams=None):
+        """Common random numbers: the Philox draws of controller b are keyed by ``streams[b]`` (integers >= 0, repeats allowed)
+        instead of b, so controllers on one stream meet the same noise -- e.g. two tunings interleaved with ``streams = b // 2``
+        share their PID lap, their seeded stores and every later draw.  ``streams=None`` returns to stream b = b.  Host-given
+        draws do not use the streams.  Waits for work already enqueued."""
+        s = nat.make_noise_streams(streams, self.B)
+        nat.check(self._lib.lmpc_rollout_set_noise_streams(self._h, nat.ptr(s)))
+
     def set_tracks(self, tracks, index=None):
         """Per-controller tracks (several circuits in one batch): controller b drives ``tracks[index[b]]`` (objects with
         ``seg_table`` and ``TrackLength``, e.g. reference_params.TrackParams) in every later regression, safe-set selection,
@@ -710,7 +732,8 @@ class BatchedController:
 
     @property
     def rollout_clock(self):
-        """The simulator's step counter: the Philox noise of a step is keyed by (seed, controller, this counter)."""
+        """The simulator's step counter: the Philox noise of a step is keyed by (seed, stream, this counter), the stream being
+        the controller's index unless ``set_noise_streams`` says otherwise."""
         v = C.c_ulonglong(0)
         nat.check(self._lib.lmpc_rollout_get_clock(self._h, C.byref(v)))
         return int(v.value)

@@ -134,6 +134,12 @@ struct lmpc_handle {
     // sets a one-row table holding the reference vehicle and a null index (allocated at creation)
     lmpc_vehicle_params* d_veh;
     int* d_veh_idx;
+    // noise of the simulator and the PID (lmpc_rollout_set_noise): table lmpc_noise_params[nsets] and noise index [batch]; without
+    // sets a one-row table holding the reference's constants and a null index (allocated at creation).  Philox stream of every
+    // controller (lmpc_rollout_set_noise_streams): [batch], or null for stream b = b.
+    lmpc_noise_params* d_noise;
+    int* d_noise_idx;
+    int* d_streams;
     // device lap books (lapbooks.cuh, allocated with the store): slot tables of both pools, lap history, exchange scratch
     LapBooks bk;
     int *d_poolidx, *d_stats;
@@ -309,8 +315,9 @@ static int build_const(const lmpc_params& p, FtocpConst& c) {
     return LMPC_OK;
 }
 
-// Per-controller tables (lmpc_set_param_sets, lmpc_rollout_set_vehicles): `nsets` rows and one row index per controller.
-// The argument rules both calls share: 0 <= nsets <= batch, nsets == 0 exactly when both arrays are NULL, every index in range.
+// Per-controller tables (lmpc_set_param_sets, lmpc_rollout_set_vehicles, lmpc_rollout_set_noise): `nsets` rows and one row index
+// per controller.
+// The argument rules these calls share: 0 <= nsets <= batch, nsets == 0 exactly when both arrays are NULL, every index in range.
 static int check_set_index(const lmpc_handle* h, const char* who, const void* sets, int nsets, const int* set_of_instance) {
     const std::string w(who);
     if (nsets < 0 || nsets > h->batch) return fail(LMPC_E_INVALID, w + ": nsets must be 0 .. batch");
@@ -359,6 +366,11 @@ static lmpc_vehicle_params reference_vehicle() {
     v.Df = 0.8 * v.m * 9.81 / 2.0; v.Cf = 1.25; v.Bf = 1.0;
     v.Dr = 0.8 * v.m * 9.81 / 2.0; v.Cr = 1.25; v.Br = 1.0;
     return v;
+}
+
+// The noise of Simulator.dynModel (SysModel.py:139-145) and of the PID path follower (Utilities.py:42-68)
+static lmpc_noise_params reference_noise() {
+    return lmpc_noise_params{{0.01, 0.01, 0.005}, {0.05, 0.05, 0.05}, 0.01, {0.25, 0.10}, {0.9, 0.2}};
 }
 
 template <int N, int M>
@@ -475,7 +487,9 @@ static int create_device_side(lmpc_handle* h) {
     if (!qp_bufs(h, 0)) return LMPC_E_CUDA;
     if ((rc = alloc_bufs(h, dev_bufs(h), OWN_HANDLE, 1, "lmpc_create")) != LMPC_OK) return rc;
     const lmpc_vehicle_params ref = reference_vehicle();
-    return swap_table(h, "lmpc_create", &ref, 1, nullptr, &h->d_veh, &h->d_veh_idx);
+    if ((rc = swap_table(h, "lmpc_create", &ref, 1, nullptr, &h->d_veh, &h->d_veh_idx)) != LMPC_OK) return rc;
+    const lmpc_noise_params noise = reference_noise();
+    return swap_table(h, "lmpc_create", &noise, 1, nullptr, &h->d_noise, &h->d_noise_idx);
 }
 
 extern "C" {
@@ -624,6 +638,9 @@ int lmpc_destroy(lmpc_handle* h) {
     cudaFree(h->d_set_idx);
     cudaFree(h->d_veh);
     cudaFree(h->d_veh_idx);
+    cudaFree(h->d_noise);
+    cudaFree(h->d_noise_idx);
+    cudaFree(h->d_streams);
     if (h->stream) cudaStreamDestroy(h->stream);
     for (int i = 0; i < 4 * LMPC_HOST_SLOTS; ++i) if (h->cstream[i]) cudaStreamDestroy(h->cstream[i]);
     delete h;
@@ -841,6 +858,7 @@ int lmpc_solve_mpc_host(lmpc_handle* h, const double* x0, const double* uOld, co
 int lmpc_sizeof_params(void) { return (int)sizeof(lmpc_params); }
 int lmpc_sizeof_model_params(void) { return (int)sizeof(lmpc_model_params); }
 int lmpc_sizeof_vehicle_params(void) { return (int)sizeof(lmpc_vehicle_params); }
+int lmpc_sizeof_noise_params(void) { return (int)sizeof(lmpc_noise_params); }
 int lmpc_sizeof_track_params(void) { return (int)sizeof(lmpc_track_params); }
 
 static int store_create_impl(lmpc_handle* h, const lmpc_model_params* mp, int ss_cap, int model_cap, int Tmax);
@@ -1354,6 +1372,7 @@ static SimArgs sim_args(const lmpc_handle* h, const double* z, unsigned long lon
     sa.xn = h->d_rx[h->cur ^ 1]; sa.xgn = h->d_rg[h->cur ^ 1];
     sa.cl_x = h->d_clx; sa.cl_u = h->d_clu; sa.cl_len = h->d_cllen; sa.Tcl = h->Tcl; sa.done = h->d_done;
     sa.veh = h->d_veh; sa.veh_idx = h->d_veh_idx; sa.trk = tracks(h);
+    sa.noise = h->d_noise; sa.noise_idx = h->d_noise_idx; sa.streams = h->d_streams;
     return sa;
 }
 
@@ -1408,6 +1427,7 @@ int lmpc_rollout_pid_step(lmpc_handle* h, double vt, const double* z_pid_host, c
     PidArgs pa;
     pa.batch = h->batch; pa.x = xc; pa.vt = vt; pa.z = z_pid_host ? h->d_zpid : nullptr; pa.seed = seed; pa.step = h->sim_step;
     pa.u = h->hb[0].uPred; pa.u_stride = (long long)h->N * 2;
+    pa.noise = h->d_noise; pa.noise_idx = h->d_noise_idx; pa.streams = h->d_streams;
     pid_input_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(pa);
     sim_step_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->mc, sim_args(h, z_sim_host ? h->d_z : nullptr, seed));
     CK(cudaGetLastError());
@@ -1439,6 +1459,39 @@ int lmpc_rollout_set_vehicles(lmpc_handle* h, const lmpc_vehicle_params* sets, i
         return swap_table(h, who, &ref, 1, nullptr, &h->d_veh, &h->d_veh_idx);
     }
     return swap_table(h, who, sets, nsets, set_of_instance, &h->d_veh, &h->d_veh_idx);
+}
+
+// Per-controller noise: the rules of lmpc_rollout_set_vehicles, with every value finite and >= 0.
+static_assert(sizeof(lmpc_noise_params) == 11 * sizeof(double), "lmpc_noise_params is checked as an array of its 11 doubles");
+int lmpc_rollout_set_noise(lmpc_handle* h, const lmpc_noise_params* sets, int nsets, const int* set_of_instance) {
+    static const char* who = "lmpc_rollout_set_noise";
+    if (!h) return fail(LMPC_E_INVALID, "null handle");
+    int rc = check_set_index(h, who, sets, nsets, set_of_instance);
+    if (rc != LMPC_OK) return rc;
+    for (int k = 0; k < nsets; ++k) {
+        const double* v = (const double*)&sets[k];
+        for (size_t j = 0; j < sizeof(lmpc_noise_params) / sizeof(double); ++j)
+            if (!(isfinite(v[j]) && v[j] >= 0.0))
+                return fail(LMPC_E_INVALID, std::string(who) + ": noise set " + std::to_string(k) +
+                                                ": every sigma, clip and the gain must be finite and >= 0");
+    }
+    if (nsets == 0) {
+        const lmpc_noise_params ref = reference_noise();
+        return swap_table(h, who, &ref, 1, nullptr, &h->d_noise, &h->d_noise_idx);
+    }
+    return swap_table(h, who, sets, nsets, set_of_instance, &h->d_noise, &h->d_noise_idx);
+}
+
+// Noise streams: every stream number >= 0 (repeats allowed), then the stream array replaces the previous one once the handle's
+// streams are idle; NULL returns to stream b = b.  It takes the place of the index of swap_table, with no table.
+int lmpc_rollout_set_noise_streams(lmpc_handle* h, const int* stream_of_instance) {
+    static const char* who = "lmpc_rollout_set_noise_streams";
+    if (!h) return fail(LMPC_E_INVALID, "null handle");
+    for (int b = 0; b < (stream_of_instance ? h->batch : 0); ++b)
+        if (stream_of_instance[b] < 0)
+            return fail(LMPC_E_INVALID, std::string(who) + ": stream of instance " + std::to_string(b) + " is negative");
+    int* no_table = nullptr;
+    return swap_table<int>(h, who, nullptr, 0, stream_of_instance, &no_table, &h->d_streams);
 }
 
 // Regression(x, u, lamb) of Utilities.py:5-28 on every instance's closed-loop record: per-instance LTI model in the device

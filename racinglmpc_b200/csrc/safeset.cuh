@@ -816,11 +816,14 @@ __global__ void shift_state_kernel(const ShiftArgs a) {
 // bicycle model with Pacejka tyres in the curvilinear and the global frame, then clipped Gaussian noise on
 // (vx, vy, wz).  One thread per instance.  `z` = three standard-normal draws per instance (the reference consumes
 // np.random.randn() in this order: vx, vy, wz); when z == nullptr they come from Philox4x32-10 keyed by
-// (seed, instance, step) — statistical, not bit-wise, parity with the reference's unseeded global RNG.
+// (seed, stream, step), stream = streams[b] or b when streams is null — statistical, not bit-wise, parity with the reference's
+// unseeded global RNG.
 // Also appends (x, u) to the closed-loop buffer and flags lap completion (SysModel.py:45-47).
 // The ten vehicle constants (SysModel.py:61-70) are read from a per-instance record: row veh_idx[b] of veh, or row 0 when veh_idx
 // is null (a handle without vehicle sets points at a one-row table holding the reference vehicle).  The arithmetic is the same
-// with the constants in memory as with them folded in at compile time (DESIGN.md, "Per-controller vehicles").
+// with the constants in memory as with them folded in at compile time (DESIGN.md, "Per-controller vehicles").  The noise
+// constants (SysModel.py:139-145) come the same way from row noise_idx[b] of noise (DESIGN.md, "Per-controller noise and
+// common random numbers").
 struct SimArgs {
     int batch;
     const double* x;      // [B][6] curvilinear state
@@ -842,6 +845,9 @@ struct SimArgs {
     const lmpc_vehicle_params* veh;   // vehicle table (lmpc_rollout_set_vehicles)
     const int* veh_idx;               // [B] row of every instance, or nullptr: row 0
     Tracks trk;                       // curvature and finish line of every instance (lmpc_set_tracks)
+    const lmpc_noise_params* noise;   // noise table (lmpc_rollout_set_noise)
+    const int* noise_idx;             // [B] row of every instance, or nullptr: row 0
+    const int* streams;               // [B] Philox stream of every instance (lmpc_rollout_set_noise_streams), or nullptr: b
 };
 
 }  // namespace lmpc
@@ -905,19 +911,23 @@ __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimA
         z0 = a.z[(size_t)b * 3]; z1 = a.z[(size_t)b * 3 + 1]; z2 = a.z[(size_t)b * 3 + 2];
     } else {
         curandStatePhilox4_32_10_t st;
-        curand_init(a.seed, (unsigned long long)b, a.step * 8ull, &st);   // 8 raw 32-bit draws per step: disjoint blocks
+        const int stream = a.streams ? a.streams[b] : b;
+        curand_init(a.seed, (unsigned long long)stream, a.step * 8ull, &st);   // 8 raw 32-bit draws per step: disjoint blocks
         const double2 n01 = curand_normal2_double(&st);
         const double2 n23 = curand_normal2_double(&st);
         z0 = n01.x; z1 = n01.y; z2 = n23.x;
     }
-    const double n_vx = fmax(-0.05, fmin(z0 * 0.01, 0.05));
-    const double n_vy = fmax(-0.05, fmin(z1 * 0.01, 0.05));
-    const double n_wz = fmax(-0.05, fmin(z2 * 0.005, 0.05));
+    // noise parameters, SysModel.py:139-145
+    const lmpc_noise_params& nz = a.noise[a.noise_idx ? a.noise_idx[b] : 0];
+    const double n_vx = fmax(-nz.sim_clip[0], fmin(z0 * nz.sim_sigma[0], nz.sim_clip[0]));
+    const double n_vy = fmax(-nz.sim_clip[1], fmin(z1 * nz.sim_sigma[1], nz.sim_clip[1]));
+    const double n_wz = fmax(-nz.sim_clip[2], fmin(z2 * nz.sim_sigma[2], nz.sim_clip[2]));
+    const double gain = nz.sim_gain;
     double* xn = a.xn + (size_t)b * 6;
     double* gn = a.xgn + (size_t)b * 6;
     // SysModel.py:143-147: the noise is added to the curvilinear copy only
     gn[0] = vx; gn[1] = vy; gn[2] = wz; gn[3] = psi; gn[4] = X; gn[5] = Y;
-    xn[0] = vx + 0.01 * n_vx; xn[1] = vy + 0.01 * n_vy; xn[2] = wz + 0.01 * n_wz;
+    xn[0] = vx + gain * n_vx; xn[1] = vy + gain * n_vy; xn[2] = wz + gain * n_wz;
     xn[3] = epsi; xn[4] = s; xn[5] = ey;
     if (a.done) a.done[b] = (s > trk.TrackLength) ? 1 : 0;
 }
@@ -925,7 +935,8 @@ __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimA
 // ------------------------------------------------------------------------------------------------
 // PID path-following controller, Utilities.py:42-68 (PID.solve): u = [-0.6 ey - 0.9 epsi + clip(0.25 z0, +-0.9),
 // 1.5 (vt - vx) + clip(0.10 z1, +-0.2)], z ~ N(0,1) drawn in that order.  Writes uPred[b][0] so that sim_step_kernel
-// consumes it like a controller's first predicted input.
+// consumes it like a controller's first predicted input.  The noise constants are row noise_idx[b] of noise (row 0 when
+// noise_idx is null), the Philox stream is streams[b] (b when streams is null), as in sim_step_kernel.
 struct PidArgs {
     int batch;
     const double* x;       // [B][6]
@@ -934,6 +945,9 @@ struct PidArgs {
     unsigned long long seed, step;
     double* u;             // [B][u_stride]
     long long u_stride;
+    const lmpc_noise_params* noise;   // noise table (lmpc_rollout_set_noise)
+    const int* noise_idx;             // [B] row of every instance, or nullptr: row 0
+    const int* streams;               // [B] Philox stream of every instance, or nullptr: b
 };
 __global__ void pid_input_kernel(const PidArgs a) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -943,13 +957,18 @@ __global__ void pid_input_kernel(const PidArgs a) {
         z0 = a.z[(size_t)b * 2]; z1 = a.z[(size_t)b * 2 + 1];
     } else {
         curandStatePhilox4_32_10_t st;
-        curand_init(a.seed ^ 0x9E3779B97F4A7C15ull, (unsigned long long)b, a.step * 8ull, &st);
+        const int stream = a.streams ? a.streams[b] : b;
+        curand_init(a.seed ^ 0x9E3779B97F4A7C15ull, (unsigned long long)stream, a.step * 8ull, &st);
         const double2 n01 = curand_normal2_double(&st);
         z0 = n01.x; z1 = n01.y;
     }
+    const lmpc_noise_params& nz = a.noise[a.noise_idx ? a.noise_idx[b] : 0];
     const double* x = a.x + (size_t)b * 6;
-    a.u[(size_t)b * a.u_stride] = -0.6 * x[5] - 0.9 * x[3] + fmax(-0.9, fmin(z0 * 0.25, 0.9));
-    a.u[(size_t)b * a.u_stride + 1] = 1.5 * (a.vt - x[0]) + fmax(-0.2, fmin(z1 * 0.10, 0.2));
+    // -0.6 ey - 0.9 epsi with the one contraction the device has always computed (ptxas fused it so when the noise constants were
+    // immediates); written out because the compiler otherwise picks its contraction from the surrounding code
+    a.u[(size_t)b * a.u_stride] = fma(-0.6, x[5], -(0.9 * x[3])) +
+                                  fmax(-nz.pid_clip[0], fmin(z0 * nz.pid_sigma[0], nz.pid_clip[0]));
+    a.u[(size_t)b * a.u_stride + 1] = 1.5 * (a.vt - x[0]) + fmax(-nz.pid_clip[1], fmin(z1 * nz.pid_sigma[1], nz.pid_clip[1]));
 }
 
 // LTI system identification by ridge regression, Utilities.py:5-28 (Regression): rows t = 1 .. T-2 of the closed-loop

@@ -64,6 +64,31 @@ class VehicleParams:
         return cls(m, lf, lr, Iz, D, Cf, Bf, D, Cr, Br)
 
 
+@dataclass(frozen=True)
+class NoiseParams:
+    """The noise of the closed loop: Simulator.dynModel adds sim_gain * clip(z_j * sim_sigma_j, +-sim_clip_j) to (vx, vy, wz)
+    (SysModel.py:139-145), the PID path follower adds clip(z_j * pid_sigma_j, +-pid_clip_j) to (steering, acceleration)
+    (Utilities.py:42-68), z_j standard normal.  The device closed loop takes one per controller (BatchedController.set_noise)."""
+    sim_sigma: tuple
+    sim_clip: tuple
+    sim_gain: float
+    pid_sigma: tuple
+    pid_clip: tuple
+
+    @classmethod
+    def reference(cls):
+        """The reference's constants."""
+        return cls((0.01, 0.01, 0.005), (0.05, 0.05, 0.05), 0.01, (0.25, 0.10), (0.9, 0.2))
+
+    @classmethod
+    def scaled(cls, sim=1.0, pid=1.0):
+        """The reference's noise with sigma and clip of the simulator multiplied by ``sim`` and those of the PID by ``pid`` (the
+        gain stays): 1 gives the reference's values bit for bit, 0 a noise-free plant or PID."""
+        r = cls.reference()
+        return cls(tuple(v * sim for v in r.sim_sigma), tuple(v * sim for v in r.sim_clip), r.sim_gain,
+                   tuple(v * pid for v in r.pid_sigma), tuple(v * pid for v in r.pid_clip))
+
+
 def _wrap(a):
     if a < -np.pi:
         return 2 * np.pi + a

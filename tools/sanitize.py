@@ -2,7 +2,7 @@
 """Small-batch run of every kernel for compute-sanitizer (memcheck / racecheck / synccheck / initcheck):
     compute-sanitizer --tool racecheck python tools/sanitize.py
 Exercises: ftocp_kernel<12,0> and <12,48> (host + device entry points), knn_ltv_regress, ss_select, shift_state,
-ss_add_point, rollout_cost, sim_step, commit_laps, ss_export_laps, ss_import_laps; round 2: the long-horizon kernel
+ss_add_point, rollout_cost, sim_step (with noise sets and noise streams), commit_laps, ss_export_laps, ss_import_laps; round 2: the long-horizon kernel
 that reads its model in place (N = 48), warm-started solves, pid_input, seed_books, commit_laps_books, rollout_stats, the pooled
 exchange (pool_local_best / export / rank / import), trace_step and track_global_position."""
 import os
@@ -31,6 +31,9 @@ assert np.all(o["status"] == 1) and np.all(o["flags"] == 0)
 c.add_point(data["x0"], o["uPred"][:, 0])
 c.enable_rollout(Tcl=64)
 c.rollout_set_state(data["x0"], data["x0"])
+# per-controller noise sets and shared noise streams: the simulator reads its row and its stream per controller
+c.set_noise([rp.NoiseParams.reference(), rp.NoiseParams.scaled(10, 0.5)], np.arange(B) % 2)
+c.set_noise_streams(np.arange(B) // 2)
 for _ in range(3):
     c.rollout_step(seed=1)
 done, n = c.rollout_done()
