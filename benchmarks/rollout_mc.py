@@ -50,7 +50,7 @@ def layout(warm=False):
 
 def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, poll=8, max_steps=0, seed=1234, local=None, warm=False,
         final=None, param_sets=None, vehicle_sets=None, books=None, track_sets=None, pool_groups=None, readiness="batch",
-        capture=None, start=None, noise_sets=None, noise_streams=None):
+        capture=None, start=None, noise_sets=None, noise_streams=None, regression_sets=None):
     """One Monte-Carlo run on this rank's GPU (torch.distributed may or may not be initialised).  Returns a dict (all ranks).
     final: None, or a dict that receives the closed loop's end state (rollout_state) and the last step's solver report (step_results).
     books: None, or a dict that receives the lap books (books) and the health counters (flags_or, unsolved).
@@ -68,6 +68,10 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     noise_streams: None, or the [batch] stream numbers handed to BatchedController.set_noise_streams (common random numbers:
     controllers on one stream meet the same draws).  Streams are local to a rank: every rank keys its Philox draws with its own
     seed (seed + rank), so controllers pair only with controllers of their own rank.
+    regression_sets: None, or (regs, index) handed to BatchedController.set_regression (a sweep over the learned model's
+    bandwidth, neighbour count, ridge, feature scaling and laps used, trToUse up to the store's 4; the result then holds
+    per-regression-set lap statistics under "per_regression_rank0").  The pooled mode exchanges laps whatever the model setting:
+    a lap driven under another setting is still a trajectory of this car on this circuit.
     pool_groups: None, or (index, G) handed to BatchedController.set_pool_groups (e.g. sharding.design_groups(track index,
     parameter-set index)): the pooled mode then exchanges laps within each group; the exchange buffers hold G * (share + 1) laps
     per rank and the result holds the laps filed per group under "laps_filed_per_group_rank0" (stored laps counted from the books;
@@ -93,7 +97,7 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     clock and the scheduler state are set, and the run first repeats the poll the capture was taken at, under the new `laps`
     (groups that exchanged at that poll are not exchanged again), then steps on.  A run to 3 laps captured and resumed to 5
     therefore equals a run to 5 laps bit for bit (books, end states, health, exchange steps).  Tables (param_sets, vehicle_sets,
-    noise_sets, noise_streams, track_sets, pool_groups) are installed from the arguments, as for a fresh run.  ValueError before any device work when start
+    noise_sets, noise_streams, regression_sets, track_sets, pool_groups) are installed from the arguments, as for a fresh run.  ValueError before any device work when start
     does not match the batch, the layout, the mode, the readiness, the poll interval or the pool groups, or when laps is not
     above the captured laps."""
     if start is not None:
@@ -132,6 +136,8 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         c.set_noise(*noise_sets)
     if noise_streams is not None:
         c.set_noise_streams(noise_streams)
+    if regression_sets is not None:
+        c.set_regression(*regression_sets)
     if track_sets is not None:
         c.set_tracks(*track_sets)
     if pool_groups is not None:
@@ -279,6 +285,10 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     if noise_sets is not None:
         idx = np.asarray(noise_sets[1]).reshape(B)
         out["per_noise_rank0"] = [_set_stats(bk, flags_or, unsolved, idx == k, laps) for k in range(len(noise_sets[0]))]
+    if regression_sets is not None:
+        idx = np.asarray(regression_sets[1]).reshape(B)
+        out["per_regression_rank0"] = [_set_stats(bk, flags_or, unsolved, idx == k, laps)
+                                       for k in range(len(regression_sets[0]))]
     if track_sets is not None:
         idx = np.asarray(track_sets[1]).reshape(B)
         out["per_track_rank0"] = [_set_stats(bk, flags_or, unsolved, idx == k, laps) for k in range(len(track_sets[0]))]

@@ -214,6 +214,34 @@ typedef struct lmpc_track_params {
  *     every group on this rank share one track index; lmpc_ss_import_laps_dev always returns LMPC_E_STATE. */
 int lmpc_set_tracks(lmpc_handle* h, const lmpc_track_params* sets, int nsets, const int* set_of_instance);
 
+/* The constants of the local regression model (PredictiveModel.py:18-31): the regression constants of lmpc_model_params. */
+typedef struct lmpc_regression_params {
+    int trToUse;                  /* stored laps used: 1 for the LTV-MPC, 4 for LMPC  main.py:88,102; PM.py:31 */
+    int MaxNumPoint;              /* 7                                               PM.py:18              */
+    double h, lamb;               /* 5, 0.0                                          PM.py:19-20           */
+    double scaling[5];            /* diag(0.1,1,1,1,1)                               PM.py:22-26           */
+} lmpc_regression_params;
+/* Per-controller regression models (studies of the learned model's settings in one batch; no reference counterpart: the reference
+ * builds one PredictiveModel per controller).  Controller b regresses with sets[set_of_instance[b]] (host arrays) in every later
+ * K1 launch -- lmpc_identify_host, lmpc_step_*, lmpc_rollout_step -- host-driven and device-resident alike.  nsets == 0 (sets,
+ * set_of_instance NULL) returns every controller to the constants of lmpc_store_create, which every store starts with.
+ *   - Requires lmpc_store_create (else LMPC_E_STATE).
+ *   - 1 <= nsets <= batch, every index in [0, nsets).  Per set: 1 <= trToUse <= the store's trToUse; 1 <= MaxNumPoint <= 7;
+ *     h finite, 2^-1022 <= h <= 2^1022 (a normal bandwidth with a normal reciprocal); lamb finite and >= 0; every scaling entry
+ *     finite with |s| == 0 or 2^-32 <= |s| <= 2^32, taken as |s| as lmpc_store_create does (the range in which the fp32
+ *     pre-filter of the neighbour scan is certified: DESIGN.md, "Per-controller regression models").  Any failed check returns
+ *     LMPC_E_INVALID and leaves the handle as it was.
+ *   - The store's trToUse still sizes the lap books, the regression scratch and the snapshot record.  A set with a smaller
+ *     trToUse regresses on the first trToUse entries of the controller's usedIt list: its trToUse shortest laps, which is what a
+ *     store created with that trToUse selects (PM.py:31,35-46).
+ *   - The call synchronises the handle's streams before it replaces the table.  It is allowed at any time: a change applies from
+ *     the next regression on; warm-start records stay (the QP's optimum does not depend on them).
+ *   - The regression index is independent of the parameter-set, vehicle, track, noise and pool-group indices.  The pooled
+ *     exchange does not look at it: a lap driven under another model setting is still a trajectory of this car on this circuit.
+ *   - dt stays per handle (it is the simulator's control period too).  Sets stay with the handle: the snapshot record does not
+ *     carry them. */
+int lmpc_set_regression_sets(lmpc_handle* h, const lmpc_regression_params* sets, int nsets, const int* set_of_instance);
+
 /* PredictiveModel.addTrajectory (PredictiveModel.py:35-46): copy one lap into a regression slot. */
 int lmpc_model_put_lap(lmpc_handle* h, int inst, int slot, int T, const double* x, const double* u);
 /* usedIt order: slots[B,trToUse]. */
@@ -433,7 +461,7 @@ int lmpc_set_pool_min_overrun(lmpc_handle* h, int rows);
  * both lap pools, the lap books, the controller state, the warm-start record, and with a rollout the simulator state, the
  * closed-loop record, the health counters and the LTI model (DESIGN.md, "Controller snapshots", lists every per-controller buffer
  * as carried or scratch).  Not in a record: what the handle is told to drive -- parameter sets, vehicles, tracks, noise sets,
- * noise streams, pool groups -- and handle-wide counters.  The lap books travel in the record, so a caller that keeps its own host copy of them (the
+ * noise streams, regression sets, pool groups -- and handle-wide counters.  The lap books travel in the record, so a caller that keeps its own host copy of them (the
  * host-driven bookkeeping of lmpc_ss_set_selection / lmpc_model_set_used) must not restore into its handle.
  * Record = header (below) + sections at 16-byte aligned offsets; every section is one controller's slice of one [B][...] buffer. */
 #define LMPC_SNAPSHOT_MAGIC 0x50414e53      /* "SNAP" */
@@ -495,6 +523,7 @@ int lmpc_sizeof_model_params(void);
 int lmpc_sizeof_vehicle_params(void);
 int lmpc_sizeof_track_params(void);
 int lmpc_sizeof_noise_params(void);
+int lmpc_sizeof_regression_params(void);
 
 #ifdef __cplusplus
 }

@@ -42,6 +42,12 @@ class NoiseParams(C.Structure):
                 ("pid_sigma", C.c_double * 2), ("pid_clip", C.c_double * 2)]
 
 
+class RegressionParams(C.Structure):
+    """lmpc_regression_params: the constants of the local regression model (PredictiveModel.py:18-31)."""
+    _fields_ = [("trToUse", C.c_int), ("MaxNumPoint", C.c_int), ("h", C.c_double), ("lamb", C.c_double),
+                ("scaling", C.c_double * 5)]
+
+
 class TrackParams(C.Structure):
     """lmpc_track_params: the [s_start, length, curvature] rows of Map.PointAndTangent and the lap length."""
     _fields_ = [("nseg", C.c_int), ("seg", C.c_double * (MAX_SEG * 3)), ("TrackLength", C.c_double)]
@@ -134,6 +140,7 @@ def lib():
     L.lmpc_rollout_set_noise.argtypes = [_vp, C.POINTER(NoiseParams), C.c_int, _vp]
     L.lmpc_rollout_set_noise_streams.argtypes = [_vp, _vp]
     L.lmpc_set_tracks.argtypes = [_vp, C.POINTER(TrackParams), C.c_int, _vp]
+    L.lmpc_set_regression_sets.argtypes = [_vp, C.POINTER(RegressionParams), C.c_int, _vp]
     L.lmpc_rollout_sysid.argtypes = [_vp, C.c_double, _vp, _vp]
     L.lmpc_rollout_seed_from_record.argtypes = [_vp, C.c_int, C.c_int, C.c_int]
     L.lmpc_rollout_get_lap.argtypes = [_vp, C.c_int, ip, _vp, _vp]
@@ -170,7 +177,9 @@ def lib():
     L.lmpc_sizeof_vehicle_params.restype = C.c_int
     L.lmpc_sizeof_track_params.restype = C.c_int
     L.lmpc_sizeof_noise_params.restype = C.c_int
+    L.lmpc_sizeof_regression_params.restype = C.c_int
     assert L.lmpc_sizeof_noise_params() == C.sizeof(NoiseParams), "lmpc_noise_params ABI mismatch"
+    assert L.lmpc_sizeof_regression_params() == C.sizeof(RegressionParams), "lmpc_regression_params ABI mismatch"
     assert L.lmpc_sizeof_params() == C.sizeof(Params), "lmpc_params ABI mismatch"
     assert L.lmpc_sizeof_model_params() == C.sizeof(ModelParams), "lmpc_model_params ABI mismatch"
     assert L.lmpc_sizeof_vehicle_params() == C.sizeof(VehicleParams), "lmpc_vehicle_params ABI mismatch"
@@ -306,7 +315,7 @@ def make_params(p, numSS_Points=0, numSS_it=0, QterminalSlack=None, eps_res=0.0,
 
 def _set_index(index, K, batch, what):
     """The index rules of the per-controller tables (lmpc_set_param_sets, lmpc_rollout_set_vehicles, lmpc_rollout_set_noise,
-    lmpc_set_tracks) and of the pool
+    lmpc_set_tracks, lmpc_set_regression_sets) and of the pool
     groups (lmpc_set_pool_groups): 1 <= K <= batch rows and
     one integer row number in [0, K) per controller.  Returns the index as a contiguous int32 array; raises ValueError."""
     if index is None:
@@ -412,6 +421,48 @@ def make_noise_streams(streams, batch):
     if out.min() < 0:
         raise ValueError("stream numbers must be >= 0")
     return out
+
+
+# the scaling entries the regression sets admit: 0 or this range (the fp32 pre-filter of K1 is certified there, csrc/safeset.cuh)
+SCALING_MIN, SCALING_MAX = 2.0 ** -32, 2.0 ** 32
+H_MIN, H_MAX = 2.0 ** -1022, 2.0 ** 1022
+
+
+def make_regression_sets(regs, index, batch, trToUse):
+    """Per-controller regression models for ``lmpc_set_regression_sets``: K objects ``regs`` with the fields of RegressionParams
+    (trToUse, MaxNumPoint, h, lamb, scaling[5]; e.g. reference_params.RegressionParams) and the regression set of every
+    controller ``index[batch]``; ``trToUse`` is the store's.  Raises ValueError where the library would refuse: the index rules
+    of ``make_param_sets``, 1 <= trToUse <= the store's, 1 <= MaxNumPoint <= 7, h finite in [2^-1022, 2^1022], lamb finite and
+    >= 0, five finite scaling entries with |s| == 0 or 2^-32 <= |s| <= 2^32.  Returns (ctypes array RegressionParams * K, int32
+    index array); the scaling is packed as given (the library takes |s|)."""
+    regs = list(regs)
+    K = len(regs)
+    idx = _set_index(index, K, batch, "regression sets")
+    out = (RegressionParams * K)()
+    for k, r in enumerate(regs):
+        w = "regression set %d: " % k
+        for f in ("trToUse", "MaxNumPoint"):
+            v = getattr(r, f)
+            if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)):
+                raise ValueError(w + "%s must be an integer" % f)
+        if not 1 <= int(r.trToUse) <= int(trToUse):
+            raise ValueError(w + "trToUse must be 1 .. the store's trToUse (%d), got %d" % (trToUse, r.trToUse))
+        if not 1 <= int(r.MaxNumPoint) <= 7:
+            raise ValueError(w + "MaxNumPoint must be 1 .. 7, got %d" % r.MaxNumPoint)
+        h, lamb = float(r.h), float(r.lamb)
+        if not H_MIN <= h <= H_MAX:
+            raise ValueError(w + "h must be finite and in [2^-1022, 2^1022], got %r" % h)
+        if not (np.isfinite(lamb) and lamb >= 0):
+            raise ValueError(w + "lamb must be finite and >= 0, got %r" % lamb)
+        s = np.asarray(r.scaling, dtype=float).reshape(-1)
+        if s.shape[0] != 5:
+            raise ValueError(w + "scaling needs 5 values, got %d" % s.shape[0])
+        a = np.abs(s)
+        if not np.all(np.isfinite(s)) or not np.all((a == 0) | ((a >= SCALING_MIN) & (a <= SCALING_MAX))):
+            raise ValueError(w + "every |scaling| must be 0 or in [2^-32, 2^32]")
+        out[k].trToUse, out[k].MaxNumPoint, out[k].h, out[k].lamb = int(r.trToUse), int(r.MaxNumPoint), h, lamb
+        out[k].scaling[:] = s.tolist()
+    return out, idx
 
 
 def make_pool_groups(index, ngroups, batch):

@@ -138,6 +138,22 @@ class BatchedController:
         s = nat.make_noise_streams(streams, self.B)
         nat.check(self._lib.lmpc_rollout_set_noise_streams(self._h, nat.ptr(s)))
 
+    def set_regression(self, regs, index=None):
+        """Per-controller regression models (a study of the learned model's settings in one batch): controller b identifies its
+        local LTV model with ``regs[index[b]]`` (objects with the fields of reference_params.RegressionParams: trToUse up to the
+        store's, MaxNumPoint, h, lamb, scaling) in every later ``identify``, ``step`` and ``rollout_step``.  ``index`` is required
+        with ``regs``.  ``regs=None`` (no index) returns to the constants the store was created with.  A set with a smaller trToUse
+        regresses on the controller's trToUse shortest laps.  Independent of the other tables and of the pool groups (a lap driven
+        under another model setting is still a trajectory of this car); allowed in the middle of a run.  Waits for work already
+        enqueued."""
+        if regs is None:
+            if index is not None:
+                raise ValueError("regs=None reverts to the store's own constants and takes no index")
+            nat.check(self._lib.lmpc_set_regression_sets(self._h, None, 0, None))
+            return
+        sets, idx = nat.make_regression_sets(regs, index, self.B, self.trToUse)
+        nat.check(self._lib.lmpc_set_regression_sets(self._h, sets, len(sets), nat.ptr(idx)))
+
     def set_tracks(self, tracks, index=None):
         """Per-controller tracks (several circuits in one batch): controller b drives ``tracks[index[b]]`` (objects with
         ``seg_table`` and ``TrackLength``, e.g. reference_params.TrackParams) in every later regression, safe-set selection,

@@ -121,6 +121,11 @@ struct lmpc_handle {
     std::vector<TrackRec> trk_host;
     std::vector<int> trk_idx_host;
     bool laps_stored;          // a lap entered either pool: the track table is fixed from now on
+    // regression constants (lmpc_set_regression_sets): table RegressionRec[nsets] and regression index [batch]; without sets a
+    // one-row table holding the constants of lmpc_store_create (store_reg) and a null index
+    RegressionRec store_reg;
+    RegressionRec* d_reg;
+    int* d_reg_idx;
     LapPool ss, mdl;
     int *d_used, *d_sel, *d_isprev, *d_prevslot, *d_timeStep, *d_hasPred, *d_flags, *d_minidx, *d_xchg, *d_health, *d_dropped;
     double *d_xLin, *d_uLin, *d_ztState, *d_ztFixed, *d_OldInput, *d_xPredPrev, *d_tmpx, *d_tmpu;
@@ -418,6 +423,7 @@ static int configure(int N, int M) {
 static void free_store(lmpc_handle* h) {
     free_bufs(dev_bufs(h), OWN_STORE | OWN_WARM);
     free_null(h->d_trk); free_null(h->d_trk_idx);
+    free_null(h->d_reg); free_null(h->d_reg_idx);
     h->trk_host.clear(); h->trk_idx_host.clear();
     free_null(h->d_pool_grp);
     h->ngroups = 0;
@@ -859,6 +865,7 @@ int lmpc_sizeof_params(void) { return (int)sizeof(lmpc_params); }
 int lmpc_sizeof_model_params(void) { return (int)sizeof(lmpc_model_params); }
 int lmpc_sizeof_vehicle_params(void) { return (int)sizeof(lmpc_vehicle_params); }
 int lmpc_sizeof_noise_params(void) { return (int)sizeof(lmpc_noise_params); }
+int lmpc_sizeof_regression_params(void) { return (int)sizeof(lmpc_regression_params); }
 int lmpc_sizeof_track_params(void) { return (int)sizeof(lmpc_track_params); }
 
 static int store_create_impl(lmpc_handle* h, const lmpc_model_params* mp, int ss_cap, int model_cap, int Tmax);
@@ -881,15 +888,18 @@ static int store_create_impl(lmpc_handle* h, const lmpc_model_params* mp, int ss
         if (ss_cap < h->p.numSS_it) return fail(LMPC_E_INVALID, "ss_cap < numSS_it");
     }
     CK(cudaSetDevice(h->device));
-    // the largest launch: trToUse = K1_MAXLAPS at K1_MAXWPB warps (102592 B, above a flat 100 KiB)
+    // the largest launch: trToUse = K1_MAXLAPS at K1_MAXWPB warps (103360 B, above a flat 100 KiB)
     CK(cudaFuncSetAttribute(knn_ltv_regress_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                             (int)k1_smem_bytes(K1_MAXLAPS, K1_MAXWPB)));
     CK(cudaFuncSetAttribute(knn_ltv_regress_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     ModelConst& m = h->mc;
     memset(&m, 0, sizeof(m));
-    m.trToUse = mp->trToUse; m.MaxNumPoint = mp->MaxNumPoint; m.h = mp->h; m.lamb = mp->lamb; m.dt = mp->dt;
+    m.trToUse = mp->trToUse; m.dt = mp->dt;
+    RegressionRec& r = h->store_reg;
+    memset(&r, 0, sizeof(r));
+    r.trToUse = mp->trToUse; r.MaxNumPoint = mp->MaxNumPoint; r.h = mp->h; r.lamb = mp->lamb;
     // |(x - q) s| == |(x - q) |s|| bit for bit, and the fp32 scan of K1 needs non-negative partial distances to order its keys
-    for (int i = 0; i < 5; ++i) m.scaling[i] = fabs(mp->scaling[i]);
+    for (int i = 0; i < 5; ++i) r.scaling[i] = fabs(mp->scaling[i]);
     TrackRec& t = h->store_trk;
     memset(&t, 0, sizeof(t));
     t.nseg = mp->nseg;
@@ -897,6 +907,7 @@ static int store_create_impl(lmpc_handle* h, const lmpc_model_params* mp, int ss
     t.TrackLength = mp->TrackLength;
     int rc = swap_table(h, "lmpc_store_create", &t, 1, nullptr, &h->d_trk, &h->d_trk_idx);
     if (rc != LMPC_OK) return rc;
+    if ((rc = swap_table(h, "lmpc_store_create", &r, 1, nullptr, &h->d_reg, &h->d_reg_idx)) != LMPC_OK) return rc;
     h->trk_host.assign(1, t);
     h->trk_idx_host.clear();
     h->laps_stored = false;
@@ -1016,6 +1027,37 @@ int lmpc_set_tracks(lmpc_handle* h, const lmpc_track_params* sets, int nsets, co
     if (set_of_instance) h->trk_idx_host.assign(set_of_instance, set_of_instance + h->batch);
     else h->trk_idx_host.clear();
     return LMPC_OK;
+}
+
+// Per-controller regression constants: every set checked (the scaling range is the one K1's fp32 pre-filter is certified for:
+// safeset.cuh, above its threshold), then the table replaces the previous one once the handle's streams are idle.  Nothing
+// about the handle changes unless every check passes.
+int lmpc_set_regression_sets(lmpc_handle* h, const lmpc_regression_params* sets, int nsets, const int* set_of_instance) {
+    static const char* who = "lmpc_set_regression_sets";
+    int rc = need_store(h);
+    if (rc) return rc;
+    if ((rc = check_set_index(h, who, sets, nsets, set_of_instance)) != LMPC_OK) return rc;
+    std::vector<RegressionRec> rows(nsets ? nsets : 1);
+    if (nsets == 0) rows[0] = h->store_reg;
+    for (int k = 0; k < nsets; ++k) {
+        const lmpc_regression_params& s = sets[k];
+        const std::string w = std::string(who) + ": set " + std::to_string(k) + ": ";
+        if (s.trToUse < 1 || s.trToUse > h->mc.trToUse)
+            return fail(LMPC_E_INVALID, w + "trToUse must be 1 .. the store's trToUse (" + std::to_string(h->mc.trToUse) + ")");
+        if (s.MaxNumPoint < 1 || s.MaxNumPoint > K1_MAXPTS) return fail(LMPC_E_INVALID, w + "MaxNumPoint must be 1 .. 7");
+        if (!(s.h >= 0x1p-1022 && s.h <= 0x1p1022)) return fail(LMPC_E_INVALID, w + "h must be finite and in [2^-1022, 2^1022]");
+        if (!(isfinite(s.lamb) && s.lamb >= 0.0)) return fail(LMPC_E_INVALID, w + "lamb must be finite and >= 0");
+        RegressionRec& r = rows[k];
+        memset(&r, 0, sizeof(r));
+        r.trToUse = s.trToUse; r.MaxNumPoint = s.MaxNumPoint; r.h = s.h; r.lamb = s.lamb;
+        for (int i = 0; i < 5; ++i) {
+            const double a = fabs(s.scaling[i]);
+            if (!(a == 0.0 || (a >= 0x1p-32 && a <= 0x1p32)))
+                return fail(LMPC_E_INVALID, w + "every |scaling| must be 0 or in [2^-32, 2^32]");
+            r.scaling[i] = a;
+        }
+    }
+    return swap_table(h, who, rows.data(), (int)rows.size(), set_of_instance, &h->d_reg, &h->d_reg_idx);
 }
 
 static int put_lap(lmpc_handle* h, LapPool& pool, int inst, int slot, int T, const double* x, const double* u) {
@@ -1150,6 +1192,7 @@ static int launch_k1(lmpc_handle* h) {
     a.pts_stride = k1_pts_stride(h->mc.trToUse);
     a.xLin = h->d_xLin; a.uLin = h->d_uLin; a.pool = h->mdl; a.used = h->d_used; a.abc = h->hb[0].abc; a.status = h->d_flags;
     a.trk = tracks(h);
+    a.reg = Regressions{h->d_reg, h->d_reg_idx};
     dim3 grid(h->batch, (h->N + a.wpb - 1) / a.wpb);
     const size_t smem = k1_smem_bytes(h->mc.trToUse, a.wpb);
     knn_ltv_regress_kernel<<<grid, 32 * a.wpb, smem, h->stream>>>(h->mc, a);

@@ -16,10 +16,20 @@
 
 namespace lmpc {
 
+// What stays per handle of the regression model: the store's trToUse (strides of the usedIt books, K1's scratch) and dt (the
+// simulator's control period too).  The regression constants are per controller (Regressions below).
 struct ModelConst {
-    int trToUse, MaxNumPoint;
-    double h, lamb, dt;
-    double scaling[5];
+    int trToUse;
+    double dt;
+};
+
+// The regression constants of every controller: row idx[b] of tab, or row 0 when idx is null (a store without regression sets
+// holds a one-row table with the constants of lmpc_store_create, |scaling| included).
+using RegressionRec = lmpc_regression_params;
+struct Regressions {
+    const RegressionRec* tab;
+    const int* idx;
+    __device__ __forceinline__ const RegressionRec& of(int b) const { return tab[idx ? idx[b] : 0]; }
 };
 
 // A track is one row of the handle's track table (lmpc_set_tracks); the ABI record is the device record.
@@ -134,8 +144,9 @@ struct K1Args {
     const double* xLin;  // [B][N+1][6]
     const double* uLin;   // [B][N][2]
     LapPool pool;         // model pool
-    const int* used;      // [B][trToUse] slot ids, in usedIt order
+    const int* used;      // [B][trToUse] slot ids, in usedIt order (the store's trToUse; a controller reads its first reg.trToUse)
     Tracks trk;           // the curvature of the linearisation point
+    Regressions reg;      // MaxNumPoint, h, lamb, scaling and laps used of every controller (lmpc_set_regression_sets)
     double* abc;          // [B][N][54]
     int* status;          // [B] : 0 ok, else bit flags (1 = singular regression, 2 = curvature lookup failed,
                           //        4 = a single neighbour in a lap — cases where the reference raises,
@@ -144,8 +155,13 @@ struct K1Args {
 // per-warp scratch: selected points [7*trToUse][15] (x0 x1 x2 delta a 1 | y0 y1 y2 | K*(x0 x1 x2 delta a 1)) | normal
 //                   equations 45 (+3 pad) | staging of the closed-form record entries (17, +3 pad)
 //                   | re-scoring buffer: K1_CAND exact distances + K1_CAND row indices | the query point (5 doubles, +1 pad)
+//                   | the controller's regression row (RegressionRec, 8 doubles)
 constexpr int K1_PW = 15;        // doubles per selected point
-__host__ __device__ inline int k1_pts_stride(int trToUse) { return K1_MAXPTS * trToUse * K1_PW + 48 + 20 + K1_CAND + K1_CAND / 2 + 6; }
+constexpr int K1_REGW = 8;       // doubles of a regression row
+static_assert(sizeof(RegressionRec) == K1_REGW * sizeof(double), "a regression row is staged as 8 doubles");
+__host__ __device__ inline int k1_pts_stride(int trToUse) {
+    return K1_MAXPTS * trToUse * K1_PW + 48 + 20 + K1_CAND + K1_CAND / 2 + 6 + K1_REGW;
+}
 constexpr int K1_MAXWPB = 12;    // warps per block (__launch_bounds__ below)
 // dynamic shared memory of a launch: the fp32 tile + the per-warp scratch
 inline size_t k1_smem_bytes(int trToUse, int wpb) {
@@ -154,14 +170,14 @@ inline size_t k1_smem_bytes(int trToUse, int wpb) {
 
 // The reference's distance of one stored row to the query (PM.py:185-186): diff = (Data - x) * scaling, 1-norm summed left to
 // right (numpy semantics for 5 columns), in IEEE fp64 with no contraction: the value np.argsort ranks.
-__device__ __noinline__ double k1_exact_dist(const ModelConst& m, const double* X, const double* U, int t, const double* q) {
+__device__ __noinline__ double k1_exact_dist(const double* sc, const double* X, const double* U, int t, const double* q) {
     const double* xr = X + (size_t)t * 6;
     const double* ur = U + (size_t)t * 2;
-    double d = fabs(__dmul_rn(__dsub_rn(xr[0], q[0]), m.scaling[0]));
-    d = __dadd_rn(d, fabs(__dmul_rn(__dsub_rn(xr[1], q[1]), m.scaling[1])));
-    d = __dadd_rn(d, fabs(__dmul_rn(__dsub_rn(xr[2], q[2]), m.scaling[2])));
-    d = __dadd_rn(d, fabs(__dmul_rn(__dsub_rn(ur[0], q[3]), m.scaling[3])));
-    d = __dadd_rn(d, fabs(__dmul_rn(__dsub_rn(ur[1], q[4]), m.scaling[4])));
+    double d = fabs(__dmul_rn(__dsub_rn(xr[0], q[0]), sc[0]));
+    d = __dadd_rn(d, fabs(__dmul_rn(__dsub_rn(xr[1], q[1]), sc[1])));
+    d = __dadd_rn(d, fabs(__dmul_rn(__dsub_rn(xr[2], q[2]), sc[2])));
+    d = __dadd_rn(d, fabs(__dmul_rn(__dsub_rn(ur[0], q[3]), sc[3])));
+    d = __dadd_rn(d, fabs(__dmul_rn(__dsub_rn(ur[1], q[4]), sc[4])));
     return d;
 }
 
@@ -210,15 +226,20 @@ __global__ void __launch_bounds__(32 * K1_MAXWPB, LMPC_K1_MINBLOCKS) knn_ltv_reg
     // the fp64 query lives in shared memory (read on the rare exact paths only); the scan keeps its fp32 copy in registers
     double* qv = reinterpret_cast<double*>(cbi + K1_CAND);
     if (lane < 5) qv[lane] = (lane < 3) ? xl[lane] : ul[lane - 3];
+    // this controller's regression constants: one 64 B row per warp, staged next to the query (b is uniform per CTA).  Read from
+    // shared memory where they are used, they hold no register across the scan (the row pointer and h would cost K1 a spill at
+    // its 56-register cap: DESIGN.md, "Per-controller regression models")
+    double* rw = qv + 6;
+    if (lane < K1_REGW) rw[lane] = reinterpret_cast<const double*>(&a.reg.of(b))[lane];
     __syncwarp();
+    const RegressionRec& rg = *reinterpret_cast<const RegressionRec*>(rw);
     const float f0 = (float)qv[0], f1 = (float)qv[1], f2 = (float)qv[2], f3 = (float)qv[3], f4 = (float)qv[4];
-    const float s0 = (float)m.scaling[0], s1 = (float)m.scaling[1], s2 = (float)m.scaling[2], s3 = (float)m.scaling[3], s4 = (float)m.scaling[4];
+    const float s0 = (float)rg.scaling[0], s1 = (float)rg.scaling[1], s2 = (float)rg.scaling[2], s3 = (float)rg.scaling[3], s4 = (float)rg.scaling[4];
     const float qsum = s0 * fabsf(f0) + s1 * fabsf(f1) + s2 * fabsf(f2) + s3 * fabsf(f3) + s4 * fabsf(f4);
-    const int kk = m.MaxNumPoint;
-    const double rh = fast_rcp(m.h);
+    const int kk = rg.MaxNumPoint;
     int flags = 0, npts = 0;
 
-    for (int c = 0; c < m.trToUse; ++c) {
+    for (int c = 0; c < rg.trToUse; ++c) {      // rg.trToUse <= m.trToUse, the stride of the usedIt books
         const int slot = a.used[(size_t)b * m.trToUse + c];
         const size_t lap = a.pool.lap_index(b, slot);
         const double* X = a.pool.x + lap * a.pool.Tmax * 6;
@@ -282,6 +303,16 @@ __global__ void __launch_bounds__(32 * K1_MAXWPB, LMPC_K1_MINBLOCKS) knn_ltv_reg
         // d64 < G (1 + 1.53e-5) + (G + 2 qsum) 4.3e-7, so every row of the exact top-k -- and, when fewer than k rows lie inside the
         // bandwidth h, every row inside it (then G >= h - margin) -- has a key below
         //     thr = G (1 + 3.2e-5) + (G + 2 qsum) 1.3e-6.
+        // Per-controller scaling and h (lmpc_set_regression_sets).  Every bound above is relative: the fp32 scaling is the fp64 one
+        // rounded once (2^-24, like a feature), and scaling every s_j by one factor scales the exact distances, the fp32 partial
+        // distances, G, qsum, thr and h by it too -- by a power of two exactly.  What is not relative is the fp32 range: (float)s
+        // must be normal, the padding rows' distance (K1_FAR s, five terms) must be finite and farther than every stored row, and
+        // the partial distances must stay normal and below K1_FAR 1e-3 (the `open` bound) for rows of physical size.  The sets
+        // admit |s| == 0 or 2^-32 <= |s| <= 2^32: then (float)s is normal; K1_FAR s <= 1e18 2^32 (x5 = 2.1e28) is finite and
+        // farther than any row with features below 1e17; a stored distance with features below 2^10 is at most 5 2^32 2^11 =
+        // 4.4e13 < 1e15, so a real G is never taken for `open`; and a partial distance stays normal down to feature differences
+        // of 2^-94.  (`open` only labels the padding: below that bound G of a lap shorter than k rows is a padding key, and thr
+        // then admits every stored row as `open` does.)  h enters only through the exact fp64 test d < h.
         const float Gf = __uint_as_float(G & ~K1_JMASK);
         const bool open = !(Gf < K1_FAR * 1e-3f);                   // fewer than k lanes hold a row: everything stored is a candidate
         const float thrf = open ? 3.0e38f : fmaf(Gf, 3.2e-5f, Gf) + (Gf + 2.0f * qsum) * 1.3e-6f;
@@ -328,10 +359,10 @@ __global__ void __launch_bounds__(32 * K1_MAXWPB, LMPC_K1_MINBLOCKS) knn_ltv_reg
         {
             double cd = 1e300;
             int ci = 0x7fffffff;
-            if (lane < nc) { ci = cbi[lane]; cd = k1_exact_dist(m, X, U, ci, qv); cbd[lane] = cd; }
+            if (lane < nc) { ci = cbi[lane]; cd = k1_exact_dist(rg.scaling, X, U, ci, qv); cbd[lane] = cd; }
             // PM.py:187-191: >= MaxNumPoint neighbours inside the bandwidth -> the MaxNumPoint closest, else all inside.  Every row
             // inside the bandwidth is a candidate whenever fewer than k are (see the threshold), so counting candidates decides it.
-            const int inside = __popc(__ballot_sync(0xffffffffu, cd < m.h));
+            const int inside = __popc(__ballot_sync(0xffffffffu, cd < rg.h));
             ksel = inside >= kk ? kk : inside;
             if (inside == 1) flags |= 4;    // np.squeeze() makes this case raise in the reference
             __syncwarp();
@@ -345,7 +376,7 @@ __global__ void __launch_bounds__(32 * K1_MAXWPB, LMPC_K1_MINBLOCKS) knn_ltv_reg
                 double* P = pts + (size_t)(npts + rank) * K1_PW;
                 const double* xr = X + (size_t)ci * 6;
                 const double* ur = U + (size_t)ci * 2;
-                const double rr = cd * rh;
+                const double rr = cd * fast_rcp(rg.h);
                 const double Kw = (1.0 - rr * rr) * 3.0 / 4.0;
                 const double z0 = xr[0], z1 = xr[1], z2 = xr[2], z3 = ur[0], z4 = ur[1];
                 P[0] = z0; P[1] = z1; P[2] = z2; P[3] = z3; P[4] = z4; P[5] = 1.0;
@@ -383,7 +414,7 @@ __global__ void __launch_bounds__(32 * K1_MAXWPB, LMPC_K1_MINBLOCKS) knn_ltv_reg
         double acc = 0.0;
         const double* P = pts;
         for (int p = 0; p < npts; ++p, P += K1_PW) acc = fma(P[9 + ir], P[ic], acc);
-        if (diag) acc += m.lamb;
+        if (diag) acc += rg.lamb;
         ne[e] = acc;
     }
     __syncwarp();

@@ -89,6 +89,24 @@ class NoiseParams:
                    tuple(v * pid for v in r.pid_sigma), tuple(v * pid for v in r.pid_clip))
 
 
+@dataclass(frozen=True)
+class RegressionParams:
+    """The constants of the local regression model (PredictiveModel.py:18-31): the laps used (the trToUse shortest stored laps),
+    the neighbour count, the Epanechnikov bandwidth h, the ridge term and the diagonal of the feature scaling of the 1-norm
+    distance over (vx, vy, wz, delta, a).  K1 takes one per controller (BatchedController.set_regression)."""
+    trToUse: int
+    MaxNumPoint: int
+    h: float
+    lamb: float
+    scaling: tuple
+
+    @classmethod
+    def reference(cls, trToUse=4):
+        """The reference's constants: PredictiveModel(n, d, map, trToUse) builds 1 for the LTV-MPC and 4 for LMPC
+        (main.py:88,102)."""
+        return cls(int(trToUse), 7, 5.0, 0.0, (0.1, 1.0, 1.0, 1.0, 1.0))
+
+
 def _wrap(a):
     if a < -np.pi:
         return 2 * np.pi + a

@@ -2,7 +2,7 @@
 """Small-batch run of every kernel for compute-sanitizer (memcheck / racecheck / synccheck / initcheck):
     compute-sanitizer --tool racecheck python tools/sanitize.py
 Exercises: ftocp_kernel<12,0> and <12,48> (host + device entry points), knn_ltv_regress, ss_select, shift_state,
-ss_add_point, rollout_cost, sim_step (with noise sets and noise streams), commit_laps, ss_export_laps, ss_import_laps; round 2: the long-horizon kernel
+ss_add_point, rollout_cost, sim_step (with noise sets and noise streams), knn_ltv_regress with regression sets, commit_laps, ss_export_laps, ss_import_laps; round 2: the long-horizon kernel
 that reads its model in place (N = 48), warm-started solves, pid_input, seed_books, commit_laps_books, rollout_stats, the pooled
 exchange (pool_local_best / export / rank / import), trace_step and track_global_position."""
 import os
@@ -34,6 +34,9 @@ c.rollout_set_state(data["x0"], data["x0"])
 # per-controller noise sets and shared noise streams: the simulator reads its row and its stream per controller
 c.set_noise([rp.NoiseParams.reference(), rp.NoiseParams.scaled(10, 0.5)], np.arange(B) % 2)
 c.set_noise_streams(np.arange(B) // 2)
+# per-controller regression sets: K1 stages its row per warp; fewer laps, other h / MaxNumPoint / lamb / scaling per controller
+r = rp.RegressionParams.reference(5)
+c.set_regression([r, rp.RegressionParams(2, 3, 0.5, 1e-6, (2.0 ** 32, 1.0, 0.0, 1.0, -(2.0 ** -32)))], np.arange(B) % 2)
 for _ in range(3):
     c.rollout_step(seed=1)
 done, n = c.rollout_done()
