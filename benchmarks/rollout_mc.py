@@ -34,7 +34,7 @@ import torch.distributed as dist
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
-from racinglmpc_b200 import workloads, sharding, reference_params as rp      # noqa: E402
+from racinglmpc_b200 import workloads, sharding, reference_params as rp, _native      # noqa: E402
 from racinglmpc_b200.controller import BatchedController                      # noqa: E402
 
 # the controllers of every run: horizon, regression laps and the sizes of the lap stores and the closed-loop record
@@ -50,7 +50,7 @@ def layout(warm=False):
 
 def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, poll=8, max_steps=0, seed=1234, local=None, warm=False,
         final=None, param_sets=None, vehicle_sets=None, books=None, track_sets=None, pool_groups=None, readiness="batch",
-        capture=None, start=None, noise_sets=None, noise_streams=None, regression_sets=None):
+        capture=None, start=None, noise_sets=None, noise_streams=None, regression_sets=None, lap_budget=None):
     """One Monte-Carlo run on this rank's GPU (torch.distributed may or may not be initialised).  Returns a dict (all ranks).
     final: None, or a dict that receives the closed loop's end state (rollout_state) and the last step's solver report (step_results).
     books: None, or a dict that receives the lap books (books) and the health counters (flags_or, unsolved).
@@ -99,9 +99,21 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     therefore equals a run to 5 laps bit for bit (books, end states, health, exchange steps).  Tables (param_sets, vehicle_sets,
     noise_sets, noise_streams, regression_sets, track_sets, pool_groups) are installed from the arguments, as for a fresh run.  ValueError before any device work when start
     does not match the batch, the layout, the mode, the readiness, the poll interval or the pool groups, or when laps is not
-    above the captured laps."""
+    above the captured laps.
+    lap_budget: None (every controller is stepped until the slowest has its laps), or the laps every controller drives before it
+    retires, one integer or [batch] (BatchedController.set_lap_budget, installed after the seeding or the restore).  A retired
+    controller costs no kernel time and keeps the state its last hand-over left it in, so with lap_budget = laps a controller ends
+    where it would end alone, whoever else is in the batch; the polls leave retired controllers out, so the run stops once every
+    controller has `laps` laps or has retired.  The result then holds the closed-loop steps the controllers really drove during
+    the run ("driven_controller_steps_rank0", from the lap books and the records) and "driven_steps_per_s" beside
+    controller_steps_per_s, which keeps meaning batch x steps / time; in the pooled mode also, per group, whether a controller had
+    retired when the group last exchanged ("retired_before_last_exchange_rank0"): a retired controller's last lap never ships
+    (nobody drives its rows past the finish line), so the exchange equals the run without a budget exactly when that is False
+    everywhere.  capture records the budget; start refuses a budget below the captured one for any controller (raising it revives
+    the controller where it stopped, with the noise draws of the later clock)."""
+    budget = _native.make_lap_budget(lap_budget, int(batch))       # ValueError where set_lap_budget would refuse, before any device work
     if start is not None:
-        _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups)
+        _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget)
     if capture is not None and not isinstance(capture, dict):
         raise ValueError("capture is a dict that receives the run's end state")
     if readiness not in ("batch", "group"):
@@ -165,6 +177,10 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         c.sync()
         pid_s = 0.0
         restore_s = time.perf_counter() - t0
+    if budget is not None:
+        c.set_lap_budget(budget)
+        driven0 = _driven_steps(c.books(), c.rollout_state())
+        retired_at_last = [False] * G
     kbest = share + 1
     rows = torch.zeros(G * kbest, tpad, 9, dtype=torch.float64, device=dev)
     meta = torch.zeros(G * kbest, 4, dtype=torch.int32, device=dev)
@@ -240,6 +256,10 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
                     took_total += c.pool_import(G * kbest, share, tpad, 0, rows, meta, count=True)
             xchg_s += time.perf_counter() - tx
             n_xchg += 1
+            if budget is not None:
+                retired = c.books()["lap_n"] >= budget
+                for g in np.nonzero(ready_g)[0]:
+                    retired_at_last[g] = bool(retired[gidx == g].any())
             next_round += 1
             for g in np.nonzero(ready_g)[0]:
                 xsteps[g].append(steps)
@@ -260,7 +280,7 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
                        next_rounds=next_rounds.tolist() if readiness == "group" else None,
                        exchanged=(last_ready if last_poll == steps and last_ready is not None else np.zeros(G, bool)).tolist(), exchange_steps=xsteps,
                        diverged_step=diverged, batch=B, laps=laps, mode=mode, readiness=readiness, poll=poll, warm=bool(warm),
-                       pool_groups=G, layout=c.snapshot_layout())
+                       pool_groups=G, layout=c.snapshot_layout(), lap_budget=None if budget is None else budget.tolist())
     flags_or, unsolved = c.rollout_health()
     stats = []
     for r in range(laps):
@@ -301,6 +321,13 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     if pool_groups is not None or readiness == "group":
         out["readiness"] = readiness
         out["exchange_steps_per_group_rank0"] = xsteps
+    if budget is not None:
+        driven = _driven_steps(bk, c.rollout_state()) - driven0
+        out["lap_budget"] = int(budget[0]) if (budget == budget[0]).all() else "per controller, %d .. %d" % (budget.min(), budget.max())
+        out["driven_controller_steps_rank0"] = driven
+        out["driven_steps_per_s"] = driven / (ms * 1e-3)
+        if mode == "pooled":
+            out["retired_before_last_exchange_rank0"] = retired_at_last
     if start is not None:
         out["resumed_from_step"] = int(start["steps"])
         out["restore_s"] = restore_s
@@ -316,9 +343,16 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     return out
 
 
-def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups):
-    """The refusals of run(start=...), before any device work: a start that does not match this run, or laps not above the
-    captured laps."""
+def _driven_steps(bk, state):
+    """Closed-loop steps the controllers have driven since the seeding: the laps handed over plus the lap under way."""
+    n = np.minimum(bk["lap_n"], bk["lap_hist"].shape[1])
+    filed = np.where(np.arange(bk["lap_hist"].shape[1])[None, :] < n[:, None], bk["lap_hist"], 0)
+    return int(filed.sum(dtype=np.int64) + state["cl_len"].sum(dtype=np.int64))
+
+
+def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget=None):
+    """The refusals of run(start=...), before any device work: a start that does not match this run, laps not above the
+    captured laps, or a lap budget below the captured one."""
     if not isinstance(start, dict):
         raise ValueError("start is a capture dict of an earlier run")
     need = ("records", "clock", "steps", "next_round", "next_rounds", "exchanged", "exchange_steps", "diverged_step", "batch", "laps",
@@ -334,6 +368,10 @@ def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups):
         raise ValueError("start was captured with %d pool groups, this run has %d" % (int(start["pool_groups"]), G))
     if int(laps) <= int(start["laps"]):
         raise ValueError("laps (%d) must be above the captured run's laps (%d)" % (int(laps), int(start["laps"])))
+    had = start.get("lap_budget")
+    if had is not None and budget is not None and (budget < np.asarray(had)).any():
+        raise ValueError("lap_budget is below the captured run's for %d controller(s): a budget can only be raised or removed"
+                         % int((budget < np.asarray(had)).sum()))
     rec = start["records"]
     if getattr(rec, "shape", (None,))[0] != int(batch):
         raise ValueError("start holds %s records, this run has %d controllers" % (getattr(rec, "shape", ("no",))[0], int(batch)))
@@ -364,11 +402,13 @@ def main():
     ap.add_argument("--ship-after", type=int, default=40, help="pooled mode: steps into the next lap before a lap is shipped")
     ap.add_argument("--poll", type=int, default=8, help="closed-loop steps between progress polls")
     ap.add_argument("--warm", action="store_true", help="warm-started interior-point solves (lmpc_params.warm_start)")
+    ap.add_argument("--lap-budget", type=int, default=0, help="laps after which a controller retires and costs no kernel time; 0 = none")
     args = ap.parse_args()
     world, local = int(os.environ.get("WORLD_SIZE", 1)), int(os.environ.get("LOCAL_RANK", 0))
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
-    out = run(args.batch, args.laps, args.mode, args.share, args.tpad, args.ship_after, args.poll, args.max_steps, local=local, warm=args.warm)
+    out = run(args.batch, args.laps, args.mode, args.share, args.tpad, args.ship_after, args.poll, args.max_steps, local=local, warm=args.warm,
+              lap_budget=args.lap_budget or None)
     if (dist.get_rank() if dist.is_initialized() else 0) == 0:
         print(json.dumps(out))
     if world > 1:

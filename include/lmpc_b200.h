@@ -372,6 +372,26 @@ int lmpc_rollout_set_noise(lmpc_handle* h, const lmpc_noise_params* sets, int ns
  * handle starts with.  Host-given draws (z_host, z_pid_host, z_sim_host) do not use the streams.  Checks, refusal and
  * synchronisation as lmpc_rollout_set_noise. */
 int lmpc_rollout_set_noise_streams(lmpc_handle* h, const int* stream_of_instance);
+/* Lap budgets: controller b is retired once it has handed over budget_of_instance[b] laps (lmpc_rollout_commit_laps_dev counts
+ * them: lap_n of lmpc_books_get).  A retired controller keeps the state that hand-over left it in (lap filed, books refreshed,
+ * record restarted: the start line of its next lap) and no kernel of lmpc_rollout_step (modes 0, 1, 2) or
+ * lmpc_rollout_commit_laps_dev works for it: no regression, selection, QP, shift, addPoint, simulator step, health count or trace
+ * row, so a batch of controllers with laps of different length stops paying for those that are finished, and every controller
+ * ends in the state it would end in alone.  Retired is derived (budget set and lap_n[b] >= budget[b]), not stored: raising the
+ * budget later revives a controller where it stopped, lmpc_rollout_seed_from_record_dev (lap_n = 0) revives everybody, and a
+ * restored snapshot needs nothing extra.  The budget stays with the handle and is not part of a snapshot record.
+ *   - budget_of_instance is a host array [batch] of numbers >= 1; NULL removes the budgets (every handle starts without).
+ *   - Needs lmpc_rollout_create (LMPC_E_STATE otherwise); an entry < 1 returns LMPC_E_INVALID and leaves the handle as it was.
+ *   - The call synchronises the handle's streams before it replaces the array.  It is allowed at any time.
+ *   - The simulator clock counts on for the whole handle, so the Philox draws of the live controllers do not depend on who retired.
+ *   - lmpc_rollout_stats / lmpc_rollout_group_stats leave retired controllers out of the minimum laps driven and of the steps into
+ *     the current lap (they still count in the maximum and in the flagged count); a batch or group whose controllers have all
+ *     retired reports { INT32_MAX, max laps driven, INT32_MAX, flagged }.
+ *   - The PID lap, the host-driven entry points (lmpc_step_*, lmpc_solve_*, lmpc_identify_host, lmpc_select_host), the host-slot
+ *     hand-over (lmpc_rollout_commit_laps) and the pooled exchange (lmpc_pool_*) ignore the budget: a retired controller still
+ *     files imported laps, and its last lap, which nobody extends past the finish line, never ships under
+ *     lmpc_set_pool_min_overrun. */
+int lmpc_rollout_set_lap_budget(lmpc_handle* h, const int* budget_of_instance);
 int lmpc_rollout_sysid(lmpc_handle* h, double lamb, double* abc_host, int* flags_host);
 int lmpc_rollout_seed_from_record(lmpc_handle* h, int copies, int ss_slot0, int model_slot0);
 int lmpc_rollout_get_lap(lmpc_handle* h, int inst, int* T, double* x, double* u);              /* closed-loop record   */

@@ -139,6 +139,7 @@ def lib():
     L.lmpc_rollout_set_vehicles.argtypes = [_vp, C.POINTER(VehicleParams), C.c_int, _vp]
     L.lmpc_rollout_set_noise.argtypes = [_vp, C.POINTER(NoiseParams), C.c_int, _vp]
     L.lmpc_rollout_set_noise_streams.argtypes = [_vp, _vp]
+    L.lmpc_rollout_set_lap_budget.argtypes = [_vp, _vp]
     L.lmpc_set_tracks.argtypes = [_vp, C.POINTER(TrackParams), C.c_int, _vp]
     L.lmpc_set_regression_sets.argtypes = [_vp, C.POINTER(RegressionParams), C.c_int, _vp]
     L.lmpc_rollout_sysid.argtypes = [_vp, C.c_double, _vp, _vp]
@@ -407,20 +408,35 @@ def make_noise_sets(noises, index, batch):
     return out, idx
 
 
+def _int_per_controller(values, batch, lo, what):
+    """One integer >= lo per controller ``values[batch]`` as a contiguous int32 array (the arrays without a table:
+    lmpc_rollout_set_noise_streams, lmpc_rollout_set_lap_budget); raises ValueError."""
+    s = np.asarray(values).reshape(-1)
+    with np.errstate(invalid="ignore"):              # NaN or an out-of-range value fails the comparison below
+        out = np.ascontiguousarray(s, dtype=np.int32)
+    if out.shape[0] != batch or not np.array_equal(out, s):
+        raise ValueError("need one integer %s per controller (%d)" % (what, batch))
+    if out.min() < lo:
+        raise ValueError("every %s must be >= %d" % (what, lo))
+    return out
+
+
 def make_noise_streams(streams, batch):
     """Noise streams for ``lmpc_rollout_set_noise_streams``: one integer stream number >= 0 per controller ``streams[batch]``
     (repeats allowed: controllers on one stream meet the same Philox draws).  ``None`` (stream b = b) returns None.  Raises
     ValueError where the library would refuse.  Returns the int32 stream array."""
-    if streams is None:
+    return None if streams is None else _int_per_controller(streams, batch, 0, "stream number")
+
+
+def make_lap_budget(budget, batch):
+    """Lap budgets for ``lmpc_rollout_set_lap_budget``: the laps every controller drives before it retires, one integer >= 1 for
+    the whole batch or one per controller ``budget[batch]``.  ``None`` (no budget) returns None.  Raises ValueError where the
+    library would refuse.  Returns the int32 budget array."""
+    if budget is None:
         return None
-    s = np.asarray(streams).reshape(-1)
-    with np.errstate(invalid="ignore"):              # NaN or an out-of-range value fails the comparison below
-        out = np.ascontiguousarray(s, dtype=np.int32)
-    if out.shape[0] != batch or not np.array_equal(out, s):
-        raise ValueError("streams must hold one integer stream number per controller (%d)" % batch)
-    if out.min() < 0:
-        raise ValueError("stream numbers must be >= 0")
-    return out
+    if np.ndim(budget) == 0:
+        budget = [budget] * batch
+    return _int_per_controller(budget, batch, 1, "lap budget")
 
 
 # the scaling entries the regression sets admit: 0 or this range (the fp32 pre-filter of K1 is certified there, csrc/safeset.cuh)

@@ -138,6 +138,16 @@ class BatchedController:
         s = nat.make_noise_streams(streams, self.B)
         nat.check(self._lib.lmpc_rollout_set_noise_streams(self._h, nat.ptr(s)))
 
+    def set_lap_budget(self, budget=None):
+        """Lap budgets of the device closed loop: controller b retires once it has handed over ``budget[b]`` laps (one integer
+        >= 1 for the whole batch, or one per controller).  A retired controller keeps the state its last hand-over left it in and
+        no kernel of ``rollout_step`` / ``rollout_commit_laps_dev`` works for it, so a batch whose controllers need different
+        numbers of steps stops paying for the finished ones and each ends in the state it would end in alone.  Raising the budget
+        later revives a controller where it stopped.  ``budget=None`` removes the budgets.  Needs ``enable_rollout``; allowed in
+        the middle of a run; not part of a snapshot.  Waits for work already enqueued."""
+        b = nat.make_lap_budget(budget, self.B)
+        nat.check(self._lib.lmpc_rollout_set_lap_budget(self._h, nat.ptr(b)))
+
     def set_regression(self, regs, index=None):
         """Per-controller regression models (a study of the learned model's settings in one batch): controller b identifies its
         local LTV model with ``regs[index[b]]`` (objects with the fields of reference_params.RegressionParams: trToUse up to the

@@ -9,6 +9,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include "ftocp_pdip.cuh"
+#include "lap_budget.cuh"
 
 using namespace lmpc;
 
@@ -74,6 +75,7 @@ struct FtocpArgs {
     long long warm_stride;
     const int* set_idx;   // [B] parameter set of each instance (lmpc_set_param_sets), or null = the handle's own parameters
     const FtocpConstRec* sets;   // the parameter table set_idx indexes (read by ftocp_kernel<..., true> only)
+    LapBudget retire;     // lap budgets of the closed loop: the warp of a retired instance solves nothing; every other caller leaves it null
 
     // The instances [lo, lo + nb) of these arguments as a batch of their own, for the <N, M, 2, 4> kernel: every per-instance
     // pointer moves by lo instances (null ones stay null; a shared model, abc_inst_stride == 0, stays in place); the late counter
@@ -89,6 +91,7 @@ struct FtocpArgs {
         r.status = at(status, 1); r.iters = at(iters, 1); r.resid = at(resid, 3);
         r.warm = at(warm, warm_stride); r.warm_valid = at(warm_valid, 1);
         r.set_idx = at(set_idx, 1);
+        r.retire.budget = at(retire.budget, 1); r.retire.lap_n = at(retire.lap_n, 1);
         return r;
     }
 };
@@ -139,6 +142,7 @@ __global__ void __launch_bounds__(32, ftocp_min_blocks(N, M, SETS ? (int)sizeof(
     auto& w = ks.w;
     const int b = blockIdx.x;
     if (b >= a.batch) return;
+    if (a.retire.retired(b)) return;       // before the mbarrier exists and before any bulk copy is in flight
     const int lane = threadIdx.x;
 
     // ---- stage the instance's model into shared memory (TMA 1-D bulk copies) ----

@@ -137,9 +137,9 @@ __device__ inline int book_refresh(const LapBooks& k, int b) {
 // PC.py:445 (timeStep = 0).  One CTA per controller; no host involvement.
 __global__ void __launch_bounds__(256) commit_laps_books_kernel(int batch, LapPool ss, LapPool model, LapBooks k, const double* cl_x,
                                                                 const double* cl_u, int* cl_len, int Tcl, double* x_cur, int* timeStep,
-                                                                int* done, int* flags_or, Tracks trk, int lmpc) {
+                                                                int* done, int* flags_or, Tracks trk, int lmpc, LapBudget retire) {
     const int b = blockIdx.x;
-    if (b >= batch || !done[b]) return;
+    if (b >= batch || retire.retired(b) || !done[b]) return;
     __shared__ int s_ss, s_md;
     const int Trec = cl_len[b];
     const double TrackLength = trk.of(b).TrackLength;
@@ -340,8 +340,11 @@ __global__ void __launch_bounds__(256) pool_import_kernel(int batch, LapPool ss,
 // (INT32_MAX, 0, INT32_MAX, 0), which a MIN over ranks leaves to the ranks that have some.  Each thread accumulates in registers
 // while consecutive controllers of its stride stay in one group and folds into shared memory when the group changes (once per
 // thread without groups).
+// Retired controllers (lap budgets) are left out of out[g][0] and out[g][2] and still count in out[g][1] and out[g][3]: a group is
+// not held back by a controller that will not drive again, and a group whose controllers have all retired reports the
+// empty-group row (INT32_MAX, lap_max, INT32_MAX, flagged), which reads as ready for every round and as done.
 __global__ void __launch_bounds__(1024) rollout_stats_kernel(int batch, LapBooks k, const int* cl_len, const int* health,
-                                                             const int* grp, int G, int* out) {
+                                                             const int* grp, int G, int* out, LapBudget retire) {
     __shared__ int s_min[POOL_MAXG], s_max[POOL_MAXG], s_since[POOL_MAXG], s_flag[POOL_MAXG];
     for (int g = threadIdx.x; g < G; g += blockDim.x) { s_min[g] = 0x7fffffff; s_max[g] = 0; s_since[g] = 0x7fffffff; s_flag[g] = 0; }
     __syncthreads();
@@ -352,7 +355,7 @@ __global__ void __launch_bounds__(1024) rollout_stats_kernel(int batch, LapBooks
             if (cur >= 0) { atomicMin(&s_min[cur], mn); atomicMax(&s_max[cur], mx); atomicAdd(&s_flag[cur], fl); }
             cur = g; mn = 0x7fffffff; mx = 0; fl = 0;
         }
-        const int n = k.lap_n[b]; mn = min(mn, n); mx = max(mx, n); fl += (health && health[b]) ? 1 : 0;
+        const int n = k.lap_n[b]; mn = retire.retired(b) ? mn : min(mn, n); mx = max(mx, n); fl += (health && health[b]) ? 1 : 0;
     }
     if (cur >= 0) { atomicMin(&s_min[cur], mn); atomicMax(&s_max[cur], mx); atomicAdd(&s_flag[cur], fl); }
     __syncthreads();
@@ -364,7 +367,7 @@ __global__ void __launch_bounds__(1024) rollout_stats_kernel(int batch, LapBooks
             if (cur >= 0) atomicMin(&s_since[cur], since);
             cur = g; since = 0x7fffffff;
         }
-        if (k.lap_n[b] == s_min[g]) since = min(since, cl_len[b]);
+        if (k.lap_n[b] == s_min[g] && !retire.retired(b)) since = min(since, cl_len[b]);
     }
     if (cur >= 0) atomicMin(&s_since[cur], since);
     __syncthreads();
@@ -431,10 +434,11 @@ struct TraceBufs {
     int* lap;             // [n][cap]      laps the controller had driven before this step
 };
 __global__ void trace_step_kernel(TraceBufs t, const double* x, const double* xg, const double* uPred, long long u_stride,
-                                  const double* xPred, const double* SS_sel, const int* lap_n) {
+                                  const double* xPred, const double* SS_sel, const int* lap_n, LapBudget retire) {
     const int tr = blockIdx.x;
     if (tr >= t.n) return;
     const int b = t.inst[tr];
+    if (retire.retired(b)) return;            // a retired controller writes no trace row
     const int row = t.steps[tr];
     if (row >= t.cap) return;
     const size_t o = (size_t)tr * t.cap + row;
@@ -442,7 +446,7 @@ __global__ void trace_step_kernel(TraceBufs t, const double* x, const double* xg
     for (int e = threadIdx.x; e < 2; e += blockDim.x) t.u[o * 2 + e] = uPred[(size_t)b * u_stride + e];
     const int np = (t.N + 1) * 6;
     for (int e = threadIdx.x; e < np; e += blockDim.x) t.xPred[o * np + e] = xPred[(size_t)b * np + e];
-    if (t.M > 0)
+    if (t.M > 0 && SS_sel)                    // a step without a safe set (modes 0 and 2) selected no points: the row's ss stays unwritten
         for (int e = threadIdx.x; e < 6 * t.M; e += blockDim.x) t.ss[o * 6 * t.M + e] = SS_sel[(size_t)b * 6 * t.M + e];
     __syncthreads();
     if (threadIdx.x == 0) { t.lap[o] = lap_n ? lap_n[b] : 0; t.steps[tr] = row + 1; }

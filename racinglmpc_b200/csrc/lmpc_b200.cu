@@ -145,6 +145,8 @@ struct lmpc_handle {
     lmpc_noise_params* d_noise;
     int* d_noise_idx;
     int* d_streams;
+    // lap budgets (lmpc_rollout_set_lap_budget): laps every controller drives before it retires [batch], or null for no budget
+    int* d_budget;
     // device lap books (lapbooks.cuh, allocated with the store): slot tables of both pools, lap history, exchange scratch
     LapBooks bk;
     int *d_poolidx, *d_stats;
@@ -434,6 +436,10 @@ static void free_store(lmpc_handle* h) {
 
 static Tracks tracks(const lmpc_handle* h) { return Tracks{h->d_trk, h->d_trk_idx}; }
 
+// The lap budgets as the kernels of the device-resident closed loop take them.  Everything else (the host-driven entry points,
+// the PID lap, the host-slot hand-over) passes LapBudget{}: nobody is retired there.
+static LapBudget lap_budget(const lmpc_handle* h) { return LapBudget{h->d_budget, h->bk.lap_n}; }
+
 static void free_rollout(lmpc_handle* h) {
     free_bufs(dev_bufs(h), OWN_ROLLOUT | OWN_TRACE);
     h->has_trace = false;
@@ -647,6 +653,7 @@ int lmpc_destroy(lmpc_handle* h) {
     cudaFree(h->d_noise);
     cudaFree(h->d_noise_idx);
     cudaFree(h->d_streams);
+    cudaFree(h->d_budget);
     if (h->stream) cudaStreamDestroy(h->stream);
     for (int i = 0; i < 4 * LMPC_HOST_SLOTS; ++i) if (h->cstream[i]) cudaStreamDestroy(h->cstream[i]);
     delete h;
@@ -702,23 +709,34 @@ static int check_align(const void* p, const char* what) {
     return LMPC_OK;
 }
 
+}  // extern "C" (the helper below has C++ linkage)
+
+// One solve of the device arrays io on the handle's stream; retire: the lap budgets (the closed loop's LTI-MPC step) or none
+static int solve_dev(lmpc_handle* h, const QpIo& io, long long abc_inst_stride, long long abc_stage_stride, LapBudget retire) {
+    if (!h || !io.x0 || !io.uOld || !io.abc || !io.xPred || !io.uPred || !io.status || !io.iters || !io.resid)
+        return fail(LMPC_E_INVALID, "null argument");
+    const bool lm = (io.SS != nullptr);
+    if (lm && (h->M <= 0 || !io.Qfun)) return fail(LMPC_E_INVALID, "handle was created without a safe set (numSS_Points == 0)");
+    if ((abc_inst_stride % 2) || (abc_stage_stride % 2)) return fail(LMPC_E_INVALID, "abc strides must be even (16-byte rows)");
+    int rc;
+    if ((rc = check_align(io.abc, "abc")) != LMPC_OK) return rc;
+    if (lm && ((rc = check_align(io.SS, "SS_sel")) != LMPC_OK || (rc = check_align(io.Qfun, "Qfun_sel")) != LMPC_OK)) return rc;
+    CK(cudaSetDevice(h->device));
+    // no warm-start records: caller-supplied QPs start cold; the controllers of the device-resident step carry warm-start
+    // records (step_dev_impl)
+    FtocpArgs a = qp_args(h, io, lm);
+    a.abc_inst_stride = abc_inst_stride; a.abc_stage_stride = abc_stage_stride;
+    a.retire = retire;
+    return launch(h, a, lm, h->stream);
+}
+
+extern "C" {
+
 int lmpc_solve_lmpc_dev(lmpc_handle* h, const double* x0, const double* uOld, const double* abc, long long abc_inst_stride,
                         long long abc_stage_stride, const double* SS_sel, const double* Qfun_sel, const double* Succ_SS,
                         const double* Succ_uSS, double* xPred, double* uPred, double* slack, double* lambd,
                         double* slackTerminal, double* zt, double* zt_u, int* status, int* iters, double* resid) {
-    if (!h || !x0 || !uOld || !abc || !xPred || !uPred || !status || !iters || !resid) return fail(LMPC_E_INVALID, "null argument");
-    const bool lm = (SS_sel != nullptr);
-    if (lm && (h->M <= 0 || !Qfun_sel)) return fail(LMPC_E_INVALID, "handle was created without a safe set (numSS_Points == 0)");
-    if ((abc_inst_stride % 2) || (abc_stage_stride % 2)) return fail(LMPC_E_INVALID, "abc strides must be even (16-byte rows)");
-    int rc;
-    if ((rc = check_align(abc, "abc")) != LMPC_OK) return rc;
-    if (lm && ((rc = check_align(SS_sel, "SS_sel")) != LMPC_OK || (rc = check_align(Qfun_sel, "Qfun_sel")) != LMPC_OK)) return rc;
-    CK(cudaSetDevice(h->device));
-    // no warm-start records: caller-supplied QPs start cold; the controllers of the device-resident step carry warm-start
-    // records (step_dev_impl)
-    FtocpArgs a = qp_args(h, CALLER_QP_IO, lm);
-    a.abc_inst_stride = abc_inst_stride; a.abc_stage_stride = abc_stage_stride;
-    return launch(h, a, lm, h->stream);
+    return solve_dev(h, CALLER_QP_IO, abc_inst_stride, abc_stage_stride, LapBudget{});
 }
 
 int lmpc_solve_mpc_dev(lmpc_handle* h, const double* x0, const double* uOld, const double* abc, long long abc_inst_stride,
@@ -1125,7 +1143,7 @@ int lmpc_ss_add_point(lmpc_handle* h, const double* x, const double* u) {
     CK(cudaMemcpyAsync(h->d_tmpx, x, sizeof(double) * h->batch * 6, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(h->d_tmpu, u, sizeof(double) * h->batch * 2, cudaMemcpyHostToDevice, h->stream));
     ss_add_point_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->batch, h->ss, h->d_prevslot, h->d_tmpx, h->d_tmpu, 2,
-                                                                        tracks(h), h->d_flags, h->d_dropped);
+                                                                        tracks(h), h->d_flags, h->d_dropped, LapBudget{});
     CK(cudaGetLastError());
     h->launches += 1;
     int dropped = 0;
@@ -1185,7 +1203,7 @@ int lmpc_state_get(lmpc_handle* h, double* xLin, double* uLin, double* zt, doubl
     return LMPC_OK;
 }
 
-static int launch_k1(lmpc_handle* h) {
+static int launch_k1(lmpc_handle* h, LapBudget retire = {}) {
     K1Args a;
     a.batch = h->batch; a.N = h->N;
     a.wpb = h->N < K1_MAXWPB ? h->N : K1_MAXWPB;
@@ -1193,6 +1211,7 @@ static int launch_k1(lmpc_handle* h) {
     a.xLin = h->d_xLin; a.uLin = h->d_uLin; a.pool = h->mdl; a.used = h->d_used; a.abc = h->hb[0].abc; a.status = h->d_flags;
     a.trk = tracks(h);
     a.reg = Regressions{h->d_reg, h->d_reg_idx};
+    a.retire = retire;
     dim3 grid(h->batch, (h->N + a.wpb - 1) / a.wpb);
     const size_t smem = k1_smem_bytes(h->mc.trToUse, a.wpb);
     knn_ltv_regress_kernel<<<grid, 32 * a.wpb, smem, h->stream>>>(h->mc, a);
@@ -1201,7 +1220,7 @@ static int launch_k1(lmpc_handle* h) {
     return LMPC_OK;
 }
 
-static int launch_k2(lmpc_handle* h, const double* d_x0) {
+static int launch_k2(lmpc_handle* h, const double* d_x0, LapBudget retire = {}) {
     K2Args a;
     a.batch = h->batch; a.N = h->N; a.numSS_it = h->p.numSS_it; a.P = h->M / h->p.numSS_it;
     a.trk = tracks(h);
@@ -1209,6 +1228,7 @@ static int launch_k2(lmpc_handle* h, const double* d_x0) {
     a.timeStep = h->d_timeStep; a.has_pred = h->d_hasPred; a.xPred = h->d_xPredPrev;
     a.SS_sel = h->hb[0].SS; a.Qfun_sel = h->hb[0].Qfun; a.Succ_SS = h->hb[0].SuccSS; a.Succ_uSS = h->hb[0].SuccU;
     a.zt_fixed = h->d_ztFixed; a.status = h->d_flags; a.min_index = h->d_minidx;
+    a.retire = retire;
     ss_select_kernel<<<h->batch, 32 * a.numSS_it, 0, h->stream>>>(a);
     CK(cudaGetLastError());
     h->launches += 1;
@@ -1252,8 +1272,8 @@ int lmpc_select_host(lmpc_handle* h, const double* x0, double* SS_sel, double* Q
 }  // extern "C"
 
 // One device-resident step for the whole batch on the handle's stream: K1 -> K2 -> QP -> shift (PC.py:110-137).  ev (five events
-// or null) brackets the four kernels for lmpc_step_profile.
-static int step_dev_impl(lmpc_handle* h, int mode, const double* x0_dev, cudaEvent_t* ev) {
+// or null) brackets the four kernels for lmpc_step_profile.  retire: the lap budgets (the closed loop) or none.
+static int step_dev_impl(lmpc_handle* h, int mode, const double* x0_dev, cudaEvent_t* ev, LapBudget retire = {}) {
     int rc = need_store(h);
     if (rc) return rc;
     if (!x0_dev || (mode != 0 && mode != 1)) return fail(LMPC_E_INVALID, "bad mode or null x0");
@@ -1267,13 +1287,14 @@ static int step_dev_impl(lmpc_handle* h, int mode, const double* x0_dev, cudaEve
     const bool lm = mode == 1;
     const QpIo& q = h->hb[0];
     if (ev) CK(cudaEventRecord(ev[0], st));
-    if ((rc = launch_k1(h)) != LMPC_OK) return rc;                                   // PC.py:117
+    if ((rc = launch_k1(h, retire)) != LMPC_OK) return rc;                           // PC.py:117
     if (ev) CK(cudaEventRecord(ev[1], st));
-    if (lm && (rc = launch_k2(h, x0_dev)) != LMPC_OK) return rc;                     // PC.py:121
+    if (lm && (rc = launch_k2(h, x0_dev, retire)) != LMPC_OK) return rc;             // PC.py:121
     if (ev) CK(cudaEventRecord(ev[2], st));
     FtocpArgs a = qp_args(h, q, lm);                                         // PC.py:124-125
     a.x0 = x0_dev; a.uOld = h->d_OldInput;
     if (h->d_warm) { a.warm = h->d_warm; a.warm_valid = h->d_warm_valid; a.warm_stride = h->warm_stride; }
+    a.retire = retire;
     if ((rc = launch(h, a, lm, st)) != LMPC_OK) return rc;
     if (ev) CK(cudaEventRecord(ev[3], st));
     ShiftArgs sa;
@@ -1281,6 +1302,7 @@ static int step_dev_impl(lmpc_handle* h, int mode, const double* x0_dev, cudaEve
     sa.xPred = q.xPred; sa.uPred = q.uPred; sa.zt_in = q.zt; sa.ztu_in = q.ztu;
     sa.xLin = h->d_xLin; sa.uLin = h->d_uLin; sa.zt = h->d_ztState; sa.OldInput = h->d_OldInput; sa.xPredPrev = h->d_xPredPrev;
     sa.timeStep = h->d_timeStep; sa.has_pred = h->d_hasPred;
+    sa.retire = retire;
     shift_state_kernel<<<h->batch, 64, 0, st>>>(sa);                                 // PC.py:129-137
     CK(cudaGetLastError());
     h->launches += 1;
@@ -1426,31 +1448,35 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
     if (rc) return rc;
     const QpIo& q = h->hb[0];
     const double* xc = h->d_rx[h->cur];
+    const LapBudget retire = lap_budget(h);
     if (z_host) CK(cudaMemcpyAsync(h->d_z, z_host, sizeof(double) * h->batch * 3, cudaMemcpyHostToDevice, h->stream));
     if (mode == 2) {
         CK(cudaMemsetAsync(h->d_flags, 0, sizeof(int) * h->batch, h->stream));
         // LTI MPC with the per-instance model identified by lmpc_rollout_sysid (main.py:72-80); like the reference's LTI
         // controller it never refreshes the input-rate reference (OldInput keeps its initial value, PC.py:113-115)
-        rc = lmpc_solve_mpc_dev(h, xc, h->d_OldInput, h->d_abc_lti, 54, 0, q.xPred, q.uPred, q.slack, q.status, q.iters, q.resid);
+        QpIo io = {};
+        io.x0 = const_cast<double*>(xc); io.uOld = h->d_OldInput; io.abc = h->d_abc_lti;
+        io.xPred = q.xPred; io.uPred = q.uPred; io.slack = q.slack; io.status = q.status; io.iters = q.iters; io.resid = q.resid;
+        rc = solve_dev(h, io, 54, 0, retire);
     } else {
-        rc = step_dev_impl(h, mode, xc, nullptr);
+        rc = step_dev_impl(h, mode, xc, nullptr, retire);
     }
     if (rc) return rc;
     if (mode == 1) {                                                                 // SysModel.py:38 -> PC.py:466-476
         ss_add_point_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->batch, h->ss, h->d_prevslot, xc, q.uPred,
-                                                                            (long long)h->N * 2, tracks(h), h->d_flags, nullptr);
+                                                                            (long long)h->N * 2, tracks(h), h->d_flags, nullptr, retire);
         CK(cudaGetLastError());
         h->launches += 1;
     }
     // the trace of the chosen controllers reads the step's results and the state before dynModel
     if (h->has_trace) {
         trace_step_kernel<<<h->tr.n, 128, 0, h->stream>>>(h->tr, xc, h->d_rg[h->cur], q.uPred, (long long)h->N * 2, q.xPred,
-                                                        mode == 1 ? q.SS : nullptr, h->bk.lap_n);
+                                                        mode == 1 ? q.SS : nullptr, h->bk.lap_n, retire);
         CK(cudaGetLastError());
         h->launches += 1;
     }
     SimArgs sa = sim_args(h, z_host ? h->d_z : nullptr, seed);                       // SysModel.py:40 (dynModel)
-    sa.flags = h->d_flags; sa.status = q.status; sa.health = h->d_health;
+    sa.flags = h->d_flags; sa.status = q.status; sa.health = h->d_health; sa.retire = retire;
     sim_step_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->mc, sa);
     CK(cudaGetLastError());
     h->launches += 1;
@@ -1535,6 +1561,18 @@ int lmpc_rollout_set_noise_streams(lmpc_handle* h, const int* stream_of_instance
             return fail(LMPC_E_INVALID, std::string(who) + ": stream of instance " + std::to_string(b) + " is negative");
     int* no_table = nullptr;
     return swap_table<int>(h, who, nullptr, 0, stream_of_instance, &no_table, &h->d_streams);
+}
+
+// Lap budgets: every budget >= 1, then the budget array replaces the previous one once the handle's streams are idle; NULL removes
+// the budgets.  Like the noise streams it takes the place of the index of swap_table, with no table.
+int lmpc_rollout_set_lap_budget(lmpc_handle* h, const int* budget_of_instance) {
+    static const char* who = "lmpc_rollout_set_lap_budget";
+    if (int rc = need_rollout(h)) return rc;
+    for (int b = 0; b < (budget_of_instance ? h->batch : 0); ++b)
+        if (budget_of_instance[b] < 1)
+            return fail(LMPC_E_INVALID, std::string(who) + ": budget of instance " + std::to_string(b) + " is below 1");
+    int* no_table = nullptr;
+    return swap_table<int>(h, who, nullptr, 0, budget_of_instance, &no_table, &h->d_budget);
 }
 
 // Regression(x, u, lamb) of Utilities.py:5-28 on every instance's closed-loop record: per-instance LTI model in the device
@@ -1724,7 +1762,7 @@ int lmpc_rollout_commit_laps_dev(lmpc_handle* h) {
     h->laps_stored = true;     // enqueue only: which controllers finish a lap is not known here
     commit_laps_books_kernel<<<h->batch, 256, 0, h->stream>>>(h->batch, h->ss, h->mdl, h->bk, h->d_clx, h->d_clu, h->d_cllen, h->Tcl,
                                                               h->d_rx[h->cur], h->d_timeStep, h->d_done, h->d_health, tracks(h),
-                                                              h->M > 0 ? 1 : 0);
+                                                              h->M > 0 ? 1 : 0, lap_budget(h));
     CK(cudaGetLastError());
     h->launches += 1;
     return LMPC_OK;
@@ -1746,7 +1784,7 @@ int lmpc_rollout_seed_from_record_dev(lmpc_handle* h, int copies) {
 int lmpc_rollout_stats(lmpc_handle* h, int* out4) {
     if (int rc = need_rollout(h)) return rc;
     if (!out4) return fail(LMPC_E_INVALID, "null output");
-    rollout_stats_kernel<<<1, 1024, 0, h->stream>>>(h->batch, h->bk, h->d_cllen, h->d_health, nullptr, 1, h->d_stats);
+    rollout_stats_kernel<<<1, 1024, 0, h->stream>>>(h->batch, h->bk, h->d_cllen, h->d_health, nullptr, 1, h->d_stats, lap_budget(h));
     CK(cudaGetLastError());
     h->launches += 1;
     CK(cudaMemcpyAsync(out4, h->d_stats, sizeof(int) * 4, cudaMemcpyDeviceToHost, h->stream));
@@ -1758,7 +1796,7 @@ int lmpc_rollout_group_stats(lmpc_handle* h, int* out) {
     if (int rc = need_rollout(h)) return rc;
     if (!out) return fail(LMPC_E_INVALID, "null output");
     const int G = h->ngroups > 0 ? h->ngroups : 1;
-    rollout_stats_kernel<<<1, 1024, 0, h->stream>>>(h->batch, h->bk, h->d_cllen, h->d_health, h->d_pool_grp, G, h->d_stats);
+    rollout_stats_kernel<<<1, 1024, 0, h->stream>>>(h->batch, h->bk, h->d_cllen, h->d_health, h->d_pool_grp, G, h->d_stats, lap_budget(h));
     CK(cudaGetLastError());
     h->launches += 1;
     CK(cudaMemcpyAsync(out, h->d_stats, sizeof(int) * 4 * G, cudaMemcpyDeviceToHost, h->stream));

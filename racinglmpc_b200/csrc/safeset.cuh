@@ -13,6 +13,7 @@
 #pragma once
 #include <math.h>
 #include <stdint.h>
+#include "lap_budget.cuh"
 
 namespace lmpc {
 
@@ -147,6 +148,7 @@ struct K1Args {
     const int* used;      // [B][trToUse] slot ids, in usedIt order (the store's trToUse; a controller reads its first reg.trToUse)
     Tracks trk;           // the curvature of the linearisation point
     Regressions reg;      // MaxNumPoint, h, lamb, scaling and laps used of every controller (lmpc_set_regression_sets)
+    LapBudget retire;     // the CTAs of a retired controller identify nothing
     double* abc;          // [B][N][54]
     int* status;          // [B] : 0 ok, else bit flags (1 = singular regression, 2 = curvature lookup failed,
                           //        4 = a single neighbour in a lap — cases where the reference raises,
@@ -205,6 +207,7 @@ __constant__ signed char K1_ABC_SRC[54] = {
 __global__ void __launch_bounds__(32 * K1_MAXWPB, LMPC_K1_MINBLOCKS) knn_ltv_regress_kernel(const __grid_constant__ ModelConst m, const K1Args a) {
     extern __shared__ __align__(16) unsigned char k1_smem[];
     const int b = a.b0 + blockIdx.x;
+    if (a.retire.retired(b)) return;          // uniform over the CTA: no barrier is skipped by part of it
     const int wib = threadIdx.x >> 5;
     const int i = blockIdx.y * a.wpb + wib;   // horizon step
     const int lane = threadIdx.x & 31;
@@ -525,6 +528,7 @@ struct K2Args {
     double* zt_fixed;        // [B][6] zt after the lap-wrap fix (PC.py:392-393)
     int* status;             // [B] bit 8 = selection window ran past the stored lap (reference: IndexError)
     int* min_index;          // [B][numSS_it] argmin row (for tests)
+    LapBudget retire;        // the CTA of a retired controller selects nothing
 };
 
 // One CTA per instance, one warp per selected lap.
@@ -532,7 +536,7 @@ __global__ void __launch_bounds__(32 * 8) ss_select_kernel(const K2Args a) {
     const int b = blockIdx.x;
     const int c = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
-    if (b >= a.batch || c >= a.numSS_it) return;
+    if (b >= a.batch || c >= a.numSS_it || a.retire.retired(b)) return;
     const int M = a.P * a.numSS_it;
     const double TrackLength = a.trk.of(b).TrackLength;
     // lap-wrap fix of the terminal guess (PC.py:392-393)
@@ -611,9 +615,9 @@ __global__ void __launch_bounds__(32 * 8) ss_select_kernel(const K2Args a) {
 // ------------------------------------------------------------------------------------------------
 // LMPC.addPoint (PC.py:466-476): append x + [0,0,0,0,L,0], u to lap it-1; Qfun extends by last - 1.
 __global__ void ss_add_point_kernel(int batch, LapPool pool, const int* prev_slot, const double* x, const double* u,
-                                    long long u_stride, Tracks trk, int* status, int* dropped) {
+                                    long long u_stride, Tracks trk, int* status, int* dropped, LapBudget retire) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= batch) return;
+    if (b >= batch || retire.retired(b)) return;
     const int slot = prev_slot[b];
     if (slot < 0) return;
     const size_t lap = pool.lap_index(b, slot);
@@ -817,10 +821,11 @@ struct ShiftArgs {
     double* xPredPrev;     // [B][N+1][6]
     int* timeStep;
     int* has_pred;
+    LapBudget retire;      // the state of a retired controller is not shifted
 };
 __global__ void shift_state_kernel(const ShiftArgs a) {
     const int b = blockIdx.x;
-    if (b >= a.batch) return;
+    if (b >= a.batch || a.retire.retired(b)) return;
     const int N = a.N;
     for (int e = threadIdx.x; e < (N + 1) * 6; e += blockDim.x) {
         const int k = e / 6, j = e % 6;
@@ -879,6 +884,7 @@ struct SimArgs {
     const lmpc_noise_params* noise;   // noise table (lmpc_rollout_set_noise)
     const int* noise_idx;             // [B] row of every instance, or nullptr: row 0
     const int* streams;               // [B] Philox stream of every instance (lmpc_rollout_set_noise_streams), or nullptr: b
+    LapBudget retire;                 // a retired instance is not driven (the PID lap passes a null budget)
 };
 
 }  // namespace lmpc
@@ -888,6 +894,12 @@ namespace lmpc {
 __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimArgs a) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= a.batch) return;
+    if (a.retire.retired(b)) {
+        // no record row, no health count, no draw.  The state (x, xg) is a double buffer whose halves swap every step: carrying
+        // the state over to the other half unchanged is what keeps it where the hand-over left it
+        for (int j = 0; j < 6; ++j) { a.xn[(size_t)b * 6 + j] = a.x[(size_t)b * 6 + j]; a.xgn[(size_t)b * 6 + j] = a.xg[(size_t)b * 6 + j]; }
+        return;
+    }
     if (a.health) {
         if (a.flags && a.flags[b]) a.health[b] |= a.flags[b];
         if (a.status && a.status[b] != 1) a.health[a.batch + b] += 1;
