@@ -140,20 +140,16 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     c = BatchedController(par, B, workloads.track_seg_table(), rp.TRACK_LENGTH, trToUse=TR_TO_USE, numSS_Points=numSS_Points,
                           numSS_it=numSS_it, QterminalSlack=Qts, device=local, Tmax=TMAX, ss_cap=SS_CAP, model_cap=MODEL_CAP,
                           warm_start=warm)
-    if param_sets is not None:
-        c.set_param_sets(*param_sets)
-    if vehicle_sets is not None:
-        c.set_vehicles(*vehicle_sets)
-    if noise_sets is not None:
-        c.set_noise(*noise_sets)
-    if noise_streams is not None:
-        c.set_noise_streams(noise_streams)
-    if regression_sets is not None:
-        c.set_regression(*regression_sets)
-    if track_sets is not None:
-        c.set_tracks(*track_sets)
-    if pool_groups is not None:
-        c.set_pool_groups(*pool_groups)
+    # the per-controller tables in the order they are installed: (arguments of the install call or None, install call, result key
+    # of the per-row lap statistics or None)
+    tables = ((param_sets, c.set_param_sets, "per_set_rank0"), (vehicle_sets, c.set_vehicles, "per_vehicle_rank0"),
+              (noise_sets, c.set_noise, "per_noise_rank0"),
+              (None if noise_streams is None else (noise_streams,), c.set_noise_streams, None),
+              (regression_sets, c.set_regression, "per_regression_rank0"), (track_sets, c.set_tracks, "per_track_rank0"),
+              (pool_groups, c.set_pool_groups, None))
+    for args, install, _ in tables:
+        if args is not None:
+            install(*args)
     # every shipped lap has at least `ship_after` rows past its finish line: the readiness poll below guarantees it for the
     # slowest controllers of the batch, the export for the others (a group lapping faster holds laps that just ended)
     c.set_pool_min_overrun(ship_after)
@@ -296,22 +292,10 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
            "ipm_iters_mean_sampled": it_sum / max(it_n, 1), "ipm_iters_max_sampled": it_max,
            "instances_with_flags_rank0": int((flags_or != 0).sum()), "flag_bits_rank0": int(np.bitwise_or.reduce(flags_or)),
            "unsolved_steps_rank0": int(unsolved.sum()), "late_accepts_rank0": c.late_accepts}
-    if param_sets is not None:
-        idx = np.asarray(param_sets[1]).reshape(B)
-        out["per_set_rank0"] = [_set_stats(bk, flags_or, unsolved, idx == k, laps) for k in range(len(param_sets[0]))]
-    if vehicle_sets is not None:
-        idx = np.asarray(vehicle_sets[1]).reshape(B)
-        out["per_vehicle_rank0"] = [_set_stats(bk, flags_or, unsolved, idx == k, laps) for k in range(len(vehicle_sets[0]))]
-    if noise_sets is not None:
-        idx = np.asarray(noise_sets[1]).reshape(B)
-        out["per_noise_rank0"] = [_set_stats(bk, flags_or, unsolved, idx == k, laps) for k in range(len(noise_sets[0]))]
-    if regression_sets is not None:
-        idx = np.asarray(regression_sets[1]).reshape(B)
-        out["per_regression_rank0"] = [_set_stats(bk, flags_or, unsolved, idx == k, laps)
-                                       for k in range(len(regression_sets[0]))]
-    if track_sets is not None:
-        idx = np.asarray(track_sets[1]).reshape(B)
-        out["per_track_rank0"] = [_set_stats(bk, flags_or, unsolved, idx == k, laps) for k in range(len(track_sets[0]))]
+    for args, _, key in tables:
+        if args is not None and key is not None:
+            idx = np.asarray(args[1]).reshape(B)
+            out[key] = [_set_stats(bk, flags_or, unsolved, idx == k, laps) for k in range(len(args[0]))]
     if pool_groups is not None:
         # a stored lap advances `it`: 4 seeded copies + every own lap handed over + every imported lap filed.  Exact unless an
         # own lap found the safe-set pool full (health flag 64): then that controller's count is one too low per such lap.

@@ -197,15 +197,21 @@ def make_model_params(seg_table, TrackLength, trToUse, MaxNumPoint=7, h=5.0, lam
     m.trToUse, m.MaxNumPoint = int(trToUse), int(MaxNumPoint)
     m.h, m.lamb, m.dt = float(h), float(lamb), float(dt)
     m.scaling[:] = list(scaling)
+    _pack_track(m, seg_table, TrackLength)
+    return m
+
+
+def _pack_track(row, seg_table, TrackLength):
+    """Writes a track into ``row`` (ModelParams or TrackParams): nseg, the [nseg, 3] segment rows zero-padded to MAX_SEG rows, and
+    TrackLength.  Raises ValueError for more than MAX_SEG rows."""
     seg = np.asarray(seg_table, float).reshape(-1, 3)
     if seg.shape[0] > MAX_SEG:
         raise ValueError("track table has more than %d segments" % MAX_SEG)
-    m.nseg = seg.shape[0]
+    row.nseg = seg.shape[0]
     buf = np.zeros(MAX_SEG * 3)
     buf[:seg.size] = seg.ravel()
-    m.seg[:] = buf
-    m.TrackLength = float(TrackLength)
-    return m
+    row.seg[:] = buf
+    row.TrackLength = float(TrackLength)
 
 
 def check(rc):
@@ -331,6 +337,18 @@ def _set_index(index, K, batch, what):
     return idx
 
 
+def _pack_sets(ctype, items, index, batch, what, make_row):
+    """The rows and the index of a per-controller table: the index rules of ``_set_index`` for K = len(items) ``what``, then
+    ``make_row(k, item)`` checks item k (raising ValueError) and returns its ``ctype`` row.  Returns (ctypes array ctype * K,
+    int32 index array)."""
+    items = list(items)
+    idx = _set_index(index, len(items), batch, what)
+    out = (ctype * len(items))()
+    for k, item in enumerate(items):
+        out[k] = make_row(k, item)
+    return out, idx
+
+
 def make_param_sets(base, params, index, batch, numSS_Points=0, numSS_it=0, QterminalSlack=None):
     """Per-controller parameters for ``lmpc_set_param_sets``: K MPCParams-like objects ``params``, the set of every controller
     ``index[batch]`` and ``QterminalSlack`` (None: the base's, or one 6x6 matrix per set).  ``base`` is the handle's own ``Params``;
@@ -338,24 +356,23 @@ def make_param_sets(base, params, index, batch, numSS_Points=0, numSS_it=0, Qter
     Raises ValueError where the library would refuse: an index of the wrong length or out of range, or a set that differs from
     the base in N, the rows of Fx or Fu, slacks or n/d.  Returns (ctypes array Params * K, int32 index array)."""
     params = list(params)
-    K = len(params)
-    idx = _set_index(index, K, batch, "parameter sets")
     if QterminalSlack is None:
-        qts = [np.ctypeslib.as_array(base.QterminalSlack).reshape(6, 6).copy()] * K
+        qts = [np.ctypeslib.as_array(base.QterminalSlack).reshape(6, 6).copy()] * len(params)
     else:
         qts = list(QterminalSlack)
-        if len(qts) != K:
-            raise ValueError("QterminalSlack needs one matrix per set (%d)" % K)
-    out = (Params * K)()
-    for k, (p, q) in enumerate(zip(params, qts)):
-        s = make_params(p, numSS_Points, numSS_it, q, base.eps_res, base.eps_gap, base.max_iter, base.eps_step, bool(base.warm_start))
+        if len(qts) != len(params):
+            raise ValueError("QterminalSlack needs one matrix per set (%d)" % len(params))
+
+    def row(k, p):
+        s = make_params(p, numSS_Points, numSS_it, qts[k], base.eps_res, base.eps_gap, base.max_iter, base.eps_step,
+                        bool(base.warm_start))
         if (s.N, s.ncx, s.ncu) != (base.N, base.ncx, base.ncu):
             raise ValueError("set %d: N / rows of Fx / rows of Fu (%d, %d, %d) differ from the handle's (%d, %d, %d)"
                              % (k, s.N, s.ncx, s.ncu, base.N, base.ncx, base.ncu))
         if (s.numSS_Points, s.numSS_it) != (base.numSS_Points, base.numSS_it):
             raise ValueError("set %d: numSS_Points / numSS_it differ from the handle's" % k)
-        out[k] = s
-    return out, idx
+        return s
+    return _pack_sets(Params, params, index, batch, "parameter sets", row)
 
 
 VEHICLE_FIELDS = tuple(f for f, _ in VehicleParams._fields_)
@@ -366,18 +383,14 @@ def make_vehicle_sets(vehicles, index, batch):
     lr, Iz, Df, Cf, Bf, Dr, Cr, Br; e.g. reference_params.VehicleParams) and the vehicle of every controller ``index[batch]``.
     Raises ValueError where the library would refuse: the index rules of ``make_param_sets``, a non-positive m, Iz, lf or lr,
     or a value that is not finite.  Returns (ctypes array VehicleParams * K, int32 index array)."""
-    vehicles = list(vehicles)
-    K = len(vehicles)
-    idx = _set_index(index, K, batch, "vehicles")
-    out = (VehicleParams * K)()
-    for k, v in enumerate(vehicles):
+    def row(k, v):
         vals = [float(getattr(v, f)) for f in VEHICLE_FIELDS]
         if not all(np.isfinite(vals)):
             raise ValueError("vehicle %d: every value must be finite" % k)
         if min(v.m, v.Iz, v.lf, v.lr) <= 0:
             raise ValueError("vehicle %d: m, Iz, lf and lr must be positive" % k)
-        out[k] = VehicleParams(*vals)
-    return out, idx
+        return VehicleParams(*vals)
+    return _pack_sets(VehicleParams, vehicles, index, batch, "vehicles", row)
 
 
 NOISE_FIELDS = tuple(f for f, _ in NoiseParams._fields_)
@@ -389,11 +402,8 @@ def make_noise_sets(noises, index, batch):
     controller ``index[batch]``.  Raises ValueError where the library would refuse: the index rules of ``make_param_sets``, a
     field of the wrong length, or a value that is not finite or is negative.  Returns (ctypes array NoiseParams * K, int32 index
     array)."""
-    noises = list(noises)
-    K = len(noises)
-    idx = _set_index(index, K, batch, "noise sets")
-    out = (NoiseParams * K)()
-    for k, n in enumerate(noises):
+    def row(k, n):
+        r = NoiseParams()
         for f, ct in NoiseParams._fields_:
             v = np.asarray(getattr(n, f), dtype=float).reshape(-1)
             want = getattr(ct, "_length_", 1)
@@ -402,10 +412,11 @@ def make_noise_sets(noises, index, batch):
             if not np.all(np.isfinite(v)) or np.any(v < 0):
                 raise ValueError("noise set %d: %s must be finite and >= 0" % (k, f))
             if want > 1:
-                getattr(out[k], f)[:] = v.tolist()
+                getattr(r, f)[:] = v.tolist()
             else:
-                setattr(out[k], f, float(v[0]))
-    return out, idx
+                setattr(r, f, float(v[0]))
+        return r
+    return _pack_sets(NoiseParams, noises, index, batch, "noise sets", row)
 
 
 def _int_per_controller(values, batch, lo, what):
@@ -451,11 +462,7 @@ def make_regression_sets(regs, index, batch, trToUse):
     of ``make_param_sets``, 1 <= trToUse <= the store's, 1 <= MaxNumPoint <= 7, h finite in [2^-1022, 2^1022], lamb finite and
     >= 0, five finite scaling entries with |s| == 0 or 2^-32 <= |s| <= 2^32.  Returns (ctypes array RegressionParams * K, int32
     index array); the scaling is packed as given (the library takes |s|)."""
-    regs = list(regs)
-    K = len(regs)
-    idx = _set_index(index, K, batch, "regression sets")
-    out = (RegressionParams * K)()
-    for k, r in enumerate(regs):
+    def row(k, r):
         w = "regression set %d: " % k
         for f in ("trToUse", "MaxNumPoint"):
             v = getattr(r, f)
@@ -476,9 +483,8 @@ def make_regression_sets(regs, index, batch, trToUse):
         a = np.abs(s)
         if not np.all(np.isfinite(s)) or not np.all((a == 0) | ((a >= SCALING_MIN) & (a <= SCALING_MAX))):
             raise ValueError(w + "every |scaling| must be 0 or in [2^-32, 2^32]")
-        out[k].trToUse, out[k].MaxNumPoint, out[k].h, out[k].lamb = int(r.trToUse), int(r.MaxNumPoint), h, lamb
-        out[k].scaling[:] = s.tolist()
-    return out, idx
+        return RegressionParams(int(r.trToUse), int(r.MaxNumPoint), h, lamb, tuple(s.tolist()))
+    return _pack_sets(RegressionParams, regs, index, batch, "regression sets", row)
 
 
 def make_pool_groups(index, ngroups, batch):
@@ -503,11 +509,7 @@ def make_track_sets(tracks, index, batch):
     finite, a negative length, a first start other than 0, a start other than the previous start + length, or a TrackLength that
     is not positive or not the last start + length (all exact: Track.py:54-133 builds the table that way).
     Returns (ctypes array TrackParams * K, int32 index array)."""
-    tracks = list(tracks)
-    K = len(tracks)
-    idx = _set_index(index, K, batch, "tracks")
-    out = (TrackParams * K)()
-    for k, t in enumerate(tracks):
+    def row(k, t):
         seg = np.asarray(t.seg_table, dtype=float)
         L = float(t.TrackLength)
         if seg.ndim != 2 or seg.shape[1] != 3 or not 1 <= seg.shape[0] <= MAX_SEG:
@@ -523,12 +525,10 @@ def make_track_sets(tracks, index, batch):
                 raise ValueError("track %d: segment %d does not start where segment %d ends" % (k, i, i - 1))
         if not L > 0 or L != seg[-1, 0] + seg[-1, 1]:
             raise ValueError("track %d: TrackLength must be positive and equal the end of the last segment" % k)
-        buf = np.zeros(MAX_SEG * 3)
-        buf[:seg.size] = seg.ravel()
-        out[k].nseg = seg.shape[0]
-        out[k].seg[:] = buf
-        out[k].TrackLength = L
-    return out, idx
+        r = TrackParams()
+        _pack_track(r, seg, L)
+        return r
+    return _pack_sets(TrackParams, tracks, index, batch, "tracks", row)
 
 
 # ---- controller snapshots: the checks the library makes, in Python, before any device work -----------------------------------

@@ -89,32 +89,33 @@ class BatchedController:
         """QPs accepted at the 1e-6 safety-net tolerance instead of eps_res / eps_gap since creation (expected 0)."""
         return int(self._lib.lmpc_late_accepts(self._h))
 
+    def _install(self, call, what, sets, index, pack):
+        """One set call of a per-controller table: ``sets=None`` (no index) reverts to the table's default, else ``pack()`` returns
+        the rows and the index (raising ValueError where the library would refuse)."""
+        if sets is None:
+            if index is not None:
+                raise ValueError("%s=None reverts to the default and takes no index" % what)
+            nat.check(call(self._h, None, 0, None))
+            return
+        rows, idx = pack()
+        nat.check(call(self._h, rows, len(rows), nat.ptr(idx)))
+
     def set_param_sets(self, params, index=None, QterminalSlack=None):
         """Per-controller QP parameters (a parameter sweep in one batch): controller b solves with ``params[index[b]]`` (objects
         with the reference's MPCParams field names; every field but N and the constraint row counts may differ) and, for LMPC,
         ``QterminalSlack[index[b]]`` (None: the handle's).  ``index`` is required with ``params``.  ``params=None`` (no index)
         returns to the parameters the handle was created with.
         Waits for work already enqueued; warm-start records start over."""
-        if params is None:
-            if index is not None:
-                raise ValueError("params=None reverts to the handle's own parameters and takes no index")
-            nat.check(self._lib.lmpc_set_param_sets(self._h, None, 0, None))
-            return
-        sets, idx = nat.make_param_sets(self._p, params, index, self.B, self._p.numSS_Points, self.numSS_it, QterminalSlack)
-        nat.check(self._lib.lmpc_set_param_sets(self._h, sets, len(sets), nat.ptr(idx)))
+        self._install(self._lib.lmpc_set_param_sets, "params", params, index,
+                      lambda: nat.make_param_sets(self._p, params, index, self.B, self._p.numSS_Points, self.numSS_it, QterminalSlack))
 
     def set_vehicles(self, vehicles, index=None):
         """Per-controller vehicles of the device simulator (a Monte-Carlo over the plant in one batch): controller b is driven
         with ``vehicles[index[b]]`` (objects with the reference's ten field names, e.g. reference_params.VehicleParams) by every
         later ``rollout_step`` and ``rollout_pid_step``.  ``index`` is required with ``vehicles``.  ``vehicles=None`` (no index)
         returns to the reference vehicle.  Independent of ``set_param_sets``.  Waits for work already enqueued."""
-        if vehicles is None:
-            if index is not None:
-                raise ValueError("vehicles=None reverts to the reference vehicle and takes no index")
-            nat.check(self._lib.lmpc_rollout_set_vehicles(self._h, None, 0, None))
-            return
-        sets, idx = nat.make_vehicle_sets(vehicles, index, self.B)
-        nat.check(self._lib.lmpc_rollout_set_vehicles(self._h, sets, len(sets), nat.ptr(idx)))
+        self._install(self._lib.lmpc_rollout_set_vehicles, "vehicles", vehicles, index,
+                      lambda: nat.make_vehicle_sets(vehicles, index, self.B))
 
     def set_noise(self, noises, index=None):
         """Per-controller noise models of the device closed loop (a robustness study in one batch): controller b draws the
@@ -122,13 +123,7 @@ class BatchedController:
         every later ``rollout_step`` and ``rollout_pid_step``, Philox or host-given draws alike.  ``index`` is required with
         ``noises``.  ``noises=None`` (no index) returns to the reference's noise.  Independent of ``set_param_sets``,
         ``set_vehicles``, ``set_tracks`` and the pool groups; allowed in the middle of a run.  Waits for work already enqueued."""
-        if noises is None:
-            if index is not None:
-                raise ValueError("noises=None reverts to the reference's noise and takes no index")
-            nat.check(self._lib.lmpc_rollout_set_noise(self._h, None, 0, None))
-            return
-        sets, idx = nat.make_noise_sets(noises, index, self.B)
-        nat.check(self._lib.lmpc_rollout_set_noise(self._h, sets, len(sets), nat.ptr(idx)))
+        self._install(self._lib.lmpc_rollout_set_noise, "noises", noises, index, lambda: nat.make_noise_sets(noises, index, self.B))
 
     def set_noise_streams(self, streams=None):
         """Common random numbers: the Philox draws of controller b are keyed by ``streams[b]`` (integers >= 0, repeats allowed)
@@ -156,13 +151,8 @@ class BatchedController:
         regresses on the controller's trToUse shortest laps.  Independent of the other tables and of the pool groups (a lap driven
         under another model setting is still a trajectory of this car); allowed in the middle of a run.  Waits for work already
         enqueued."""
-        if regs is None:
-            if index is not None:
-                raise ValueError("regs=None reverts to the store's own constants and takes no index")
-            nat.check(self._lib.lmpc_set_regression_sets(self._h, None, 0, None))
-            return
-        sets, idx = nat.make_regression_sets(regs, index, self.B, self.trToUse)
-        nat.check(self._lib.lmpc_set_regression_sets(self._h, sets, len(sets), nat.ptr(idx)))
+        self._install(self._lib.lmpc_set_regression_sets, "regs", regs, index,
+                      lambda: nat.make_regression_sets(regs, index, self.B, self.trToUse))
 
     def set_tracks(self, tracks, index=None):
         """Per-controller tracks (several circuits in one batch): controller b drives ``tracks[index[b]]`` (objects with
@@ -171,13 +161,7 @@ class BatchedController:
         returns to the track the controller was created with.  Independent of ``set_param_sets`` and ``set_vehicles``.
         Only before the first lap is stored; while more than one track is installed the pooled exchange is refused.
         Waits for work already enqueued."""
-        if tracks is None:
-            if index is not None:
-                raise ValueError("tracks=None reverts to the handle's own track and takes no index")
-            nat.check(self._lib.lmpc_set_tracks(self._h, None, 0, None))
-            return
-        sets, idx = nat.make_track_sets(tracks, index, self.B)
-        nat.check(self._lib.lmpc_set_tracks(self._h, sets, len(sets), nat.ptr(idx)))
+        self._install(self._lib.lmpc_set_tracks, "tracks", tracks, index, lambda: nat.make_track_sets(tracks, index, self.B))
 
     def set_pool_groups(self, index=None, ngroups=None):
         """Pool groups of the pooled exchange (fleet learning per design cell): controller b exchanges laps only with the

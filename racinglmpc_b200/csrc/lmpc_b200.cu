@@ -88,6 +88,18 @@ static const QpField QP_FIELDS[] = {
          const_cast<double*>(Qfun_sel), const_cast<double*>(Succ_SS), const_cast<double*>(Succ_uSS), xPred, uPred, slack, \
          lambd, slackTerminal, zt, zt_u, status, iters, resid}
 
+// A per-controller table of the handle (DESIGN.md, "Per-controller tables"): device rows tab[rows.size()], or none, and the row
+// of every controller idx[batch], or none (row 0 for all), with host copies of both (index empty when idx is null).  The arrays
+// without rows (noise streams, lap budgets, pool groups) are the index alone.  swap_table replaces one, free_tables frees it.
+template <typename T>
+struct HandleTable {
+    T* tab = nullptr;
+    int* idx = nullptr;
+    std::vector<T> rows;
+    std::vector<int> index;
+    Table<T> view() const { return Table<T>{tab, idx}; }
+};
+
 struct lmpc_handle {
     lmpc_params p;
     FtocpConst c;
@@ -107,25 +119,18 @@ struct lmpc_handle {
     int* d_warm_valid;
     long long warm_stride;
     int warm_mode;
-    // per-controller parameters (lmpc_set_param_sets): table FtocpConstRec[nsets] and set index [batch]; null = uniform handle
-    FtocpConstRec* d_sets;
-    int* d_set_idx;
+    // per-controller parameters (lmpc_set_param_sets); no table = uniform handle
+    HandleTable<FtocpConstRec> sets;
     // lap stores + controller state (lmpc_store_create)
     bool has_store;
     ModelConst mc;
-    // tracks (lmpc_set_tracks): table TrackRec[ntrk] and track index [batch]; without sets a one-row table holding the track of
-    // lmpc_store_create (store_trk) and a null index.  trk_host / trk_idx_host mirror both for the host-side lap restart.
+    // tracks (lmpc_set_tracks); without sets the track of lmpc_store_create (store_trk)
     TrackRec store_trk;
-    TrackRec* d_trk;
-    int* d_trk_idx;
-    std::vector<TrackRec> trk_host;
-    std::vector<int> trk_idx_host;
+    HandleTable<TrackRec> trk;
     bool laps_stored;          // a lap entered either pool: the track table is fixed from now on
-    // regression constants (lmpc_set_regression_sets): table RegressionRec[nsets] and regression index [batch]; without sets a
-    // one-row table holding the constants of lmpc_store_create (store_reg) and a null index
+    // regression constants (lmpc_set_regression_sets); without sets the constants of lmpc_store_create (store_reg)
     RegressionRec store_reg;
-    RegressionRec* d_reg;
-    int* d_reg_idx;
+    HandleTable<RegressionRec> reg;
     LapPool ss, mdl;
     int *d_used, *d_sel, *d_isprev, *d_prevslot, *d_timeStep, *d_hasPred, *d_flags, *d_minidx, *d_xchg, *d_health, *d_dropped;
     double *d_xLin, *d_uLin, *d_ztState, *d_ztFixed, *d_OldInput, *d_xPredPrev, *d_tmpx, *d_tmpu;
@@ -135,25 +140,20 @@ struct lmpc_handle {
     unsigned long long sim_step;
     double *d_rx[2], *d_rg[2], *d_clx, *d_clu, *d_z, *d_zpid, *d_abc_lti;
     int *d_cllen, *d_done, cur;
-    // vehicles of the simulator (lmpc_rollout_set_vehicles): table lmpc_vehicle_params[nsets] and vehicle index [batch]; without
-    // sets a one-row table holding the reference vehicle and a null index (allocated at creation)
-    lmpc_vehicle_params* d_veh;
-    int* d_veh_idx;
-    // noise of the simulator and the PID (lmpc_rollout_set_noise): table lmpc_noise_params[nsets] and noise index [batch]; without
-    // sets a one-row table holding the reference's constants and a null index (allocated at creation).  Philox stream of every
-    // controller (lmpc_rollout_set_noise_streams): [batch], or null for stream b = b.
-    lmpc_noise_params* d_noise;
-    int* d_noise_idx;
-    int* d_streams;
-    // lap budgets (lmpc_rollout_set_lap_budget): laps every controller drives before it retires [batch], or null for no budget
-    int* d_budget;
+    // vehicles of the simulator (lmpc_rollout_set_vehicles); without sets the reference vehicle (installed at creation)
+    HandleTable<lmpc_vehicle_params> veh;
+    // noise of the simulator and the PID (lmpc_rollout_set_noise); without sets the reference's constants (installed at
+    // creation).  Philox stream of every controller (lmpc_rollout_set_noise_streams), or none for stream b = b.
+    HandleTable<lmpc_noise_params> noise;
+    HandleTable<int> streams;
+    // lap budgets (lmpc_rollout_set_lap_budget): laps every controller drives before it retires, or none for no budget
+    HandleTable<int> budget;
     // device lap books (lapbooks.cuh, allocated with the store): slot tables of both pools, lap history, exchange scratch
     LapBooks bk;
     int *d_poolidx, *d_stats;
-    // pool groups of the exchange (lmpc_set_pool_groups): group index [batch] and its host mirror; null / 0 = one pool
-    int* d_pool_grp;
+    // pool groups of the exchange (lmpc_set_pool_groups): group of every controller; none / 0 = one pool
+    HandleTable<int> pool_grp;
     int ngroups;
-    std::vector<int> pool_grp_host;
     int pool_min_over;         // rows a latest lap must have past its finish line to be exported (lmpc_set_pool_min_overrun)
     // rollout trace of chosen controllers (presentation support, lmpc_rollout_trace_*)
     TraceBufs tr;
@@ -234,6 +234,18 @@ static void free_null(T*& p) { if (p) cudaFree(p); p = nullptr; }
 
 static void free_bufs(const std::vector<DevBuf>& rows, unsigned owners) {
     for (const DevBuf& r : rows) if (r.own & owners) free_null(*r.p);
+}
+
+// Free the per-controller tables that belong to `owners`: tracks, regression sets and pool groups go with the store, the others
+// with the handle
+static void free_tables(lmpc_handle* h, unsigned owners) {
+    auto release = [owners](auto& t, BufOwner own) {
+        if (!(own & owners)) return;
+        free_null(t.tab); free_null(t.idx);
+        t.rows.clear(); t.index.clear();
+    };
+    release(h->sets, OWN_HANDLE); release(h->veh, OWN_HANDLE); release(h->noise, OWN_HANDLE); release(h->streams, OWN_HANDLE);
+    release(h->budget, OWN_HANDLE); release(h->trk, OWN_STORE); release(h->reg, OWN_STORE); release(h->pool_grp, OWN_STORE);
 }
 
 // Allocate the buffers of `rows` that belong to `owners` (all null on entry) for nb controllers and give them their initial
@@ -322,9 +334,8 @@ static int build_const(const lmpc_params& p, FtocpConst& c) {
     return LMPC_OK;
 }
 
-// Per-controller tables (lmpc_set_param_sets, lmpc_rollout_set_vehicles, lmpc_rollout_set_noise): `nsets` rows and one row index
-// per controller.
-// The argument rules these calls share: 0 <= nsets <= batch, nsets == 0 exactly when both arrays are NULL, every index in range.
+// The argument rules of the calls that install a per-controller table: 0 <= nsets <= batch, nsets == 0 exactly when both arrays
+// are NULL, every index in range.
 static int check_set_index(const lmpc_handle* h, const char* who, const void* sets, int nsets, const int* set_of_instance) {
     const std::string w(who);
     if (nsets < 0 || nsets > h->batch) return fail(LMPC_E_INVALID, w + ": nsets must be 0 .. batch");
@@ -336,34 +347,52 @@ static int check_set_index(const lmpc_handle* h, const char* who, const void* se
     return LMPC_OK;
 }
 
-// Once the handle's streams are idle, replace the table *tab by rows[nrows] (none when nrows == 0) and the index *idx by
-// set_of_instance[batch] (none when it is NULL).  The handle keeps its old table unless every allocation and copy succeeds.
+// Once the handle's streams are idle, replace the rows of table t by rows[nrows] (none when nrows == 0) and its index by
+// set_of_instance[batch] (none when it is NULL), host copies included.  The handle keeps its old table unless every allocation
+// and copy succeeds.
 template <typename T>
-static int swap_table(lmpc_handle* h, const char* who, const T* rows, int nrows, const int* set_of_instance, T** tab, int** idx) {
+static int swap_table(lmpc_handle* h, const char* who, HandleTable<T>& t, const T* rows, int nrows, const int* set_of_instance) {
     CK(cudaSetDevice(h->device));
     // batches already enqueued (the _async entry points, the device-resident step) finish with the table they were enqueued with
     CK(cudaStreamSynchronize(h->stream));
     for (int i = 0; i < 4 * LMPC_HOST_SLOTS; ++i) CK(cudaStreamSynchronize(h->cstream[i]));
-    T* t = nullptr;
+    T* tab = nullptr;
     int* ix = nullptr;
     cudaError_t e = cudaSuccess;
     if (nrows > 0) {
-        e = cudaMalloc((void**)&t, sizeof(T) * nrows);
-        if (e == cudaSuccess) e = cudaMemcpy(t, rows, sizeof(T) * nrows, cudaMemcpyHostToDevice);
+        e = cudaMalloc((void**)&tab, sizeof(T) * nrows);
+        if (e == cudaSuccess) e = cudaMemcpy(tab, rows, sizeof(T) * nrows, cudaMemcpyHostToDevice);
     }
     if (e == cudaSuccess && set_of_instance) {
         e = cudaMalloc((void**)&ix, sizeof(int) * h->batch);
         if (e == cudaSuccess) e = cudaMemcpy(ix, set_of_instance, sizeof(int) * h->batch, cudaMemcpyHostToDevice);
     }
     if (e != cudaSuccess) {
-        cudaFree(t); cudaFree(ix);
+        cudaFree(tab); cudaFree(ix);
         return fail(LMPC_E_CUDA, std::string(who) + ": " + cudaGetErrorString(e));
     }
-    cudaFree(*tab);
-    cudaFree(*idx);
-    *tab = t;
-    *idx = ix;
+    cudaFree(t.tab);
+    cudaFree(t.idx);
+    t.tab = tab;
+    t.idx = ix;
+    t.rows.assign(rows, rows + nrows);
+    if (set_of_instance) t.index.assign(set_of_instance, set_of_instance + h->batch);
+    else t.index.clear();
     return LMPC_OK;
+}
+
+// The calls that install a table with rows: the index rules, then row(k, rows[k]) checks set k and converts it into its row (an
+// error refuses the call), then the swap.  nsets == 0 installs the default row *dflt, or no table when dflt is null.
+template <typename T, typename Row>
+static int install_table(lmpc_handle* h, const char* who, HandleTable<T>& t, const void* sets, int nsets, const int* set_of_instance,
+                         const T* dflt, Row row) {
+    int rc = check_set_index(h, who, sets, nsets, set_of_instance);
+    if (rc != LMPC_OK) return rc;
+    std::vector<T> rows(nsets);
+    for (int k = 0; k < nsets; ++k)
+        if ((rc = row(k, rows[k])) != LMPC_OK) return rc;
+    if (nsets == 0 && dflt) rows.assign(1, *dflt);
+    return swap_table(h, who, t, rows.data(), (int)rows.size(), set_of_instance);
 }
 
 // Simulator.dynModel's vehicle (SysModel.py:61-70), D in the reference's operation order
@@ -389,8 +418,8 @@ static int configure_t(cudaStream_t) {
 
 template <int N, int M>
 static int launch_t(lmpc_handle* h, const FtocpArgs& a, cudaStream_t st) {
-    if (h->d_sets)     // the handle has per-controller parameters: every instance reads its own row (ftocp_sets.cu)
-        CK(ftocp_sets_launch(N, M, h->d_sets, a, st));
+    if (h->sets.tab)     // the handle has per-controller parameters: every instance reads its own row (ftocp_sets.cu)
+        CK(ftocp_sets_launch(N, M, h->sets.tab, a, st));
     else {
         ftocp_kernel<N, M, 2, 4, false><<<a.batch, 32, sizeof(KernelSmem<N, M, 2, 4, false>), st>>>(h->c, a);
         CK(cudaGetLastError());
@@ -424,21 +453,17 @@ static int configure(int N, int M) {
 
 static void free_store(lmpc_handle* h) {
     free_bufs(dev_bufs(h), OWN_STORE | OWN_WARM);
-    free_null(h->d_trk); free_null(h->d_trk_idx);
-    free_null(h->d_reg); free_null(h->d_reg_idx);
-    h->trk_host.clear(); h->trk_idx_host.clear();
-    free_null(h->d_pool_grp);
+    free_tables(h, OWN_STORE);
     h->ngroups = 0;
-    h->pool_grp_host.clear();
     h->laps_stored = false;
     h->has_store = false;
 }
 
-static Tracks tracks(const lmpc_handle* h) { return Tracks{h->d_trk, h->d_trk_idx}; }
+static Tracks tracks(const lmpc_handle* h) { return h->trk.view(); }
 
 // The lap budgets as the kernels of the device-resident closed loop take them.  Everything else (the host-driven entry points,
 // the PID lap, the host-slot hand-over) passes LapBudget{}: nobody is retired there.
-static LapBudget lap_budget(const lmpc_handle* h) { return LapBudget{h->d_budget, h->bk.lap_n}; }
+static LapBudget lap_budget(const lmpc_handle* h) { return LapBudget{h->budget.idx, h->bk.lap_n}; }
 
 static void free_rollout(lmpc_handle* h) {
     free_bufs(dev_bufs(h), OWN_ROLLOUT | OWN_TRACE);
@@ -477,7 +502,7 @@ static FtocpArgs qp_args(const lmpc_handle* h, const QpIo& q, bool lm) {
     }
     a.status = q.status; a.iters = q.iters; a.resid = q.resid;
     a.late = h->d_late;
-    a.set_idx = h->d_set_idx;
+    a.set_idx = h->sets.idx;
     return a;
 }
 
@@ -499,9 +524,9 @@ static int create_device_side(lmpc_handle* h) {
     if (!qp_bufs(h, 0)) return LMPC_E_CUDA;
     if ((rc = alloc_bufs(h, dev_bufs(h), OWN_HANDLE, 1, "lmpc_create")) != LMPC_OK) return rc;
     const lmpc_vehicle_params ref = reference_vehicle();
-    if ((rc = swap_table(h, "lmpc_create", &ref, 1, nullptr, &h->d_veh, &h->d_veh_idx)) != LMPC_OK) return rc;
+    if ((rc = swap_table(h, "lmpc_create", h->veh, &ref, 1, nullptr)) != LMPC_OK) return rc;
     const lmpc_noise_params noise = reference_noise();
-    return swap_table(h, "lmpc_create", &noise, 1, nullptr, &h->d_noise, &h->d_noise_idx);
+    return swap_table(h, "lmpc_create", h->noise, &noise, 1, nullptr);
 }
 
 extern "C" {
@@ -618,7 +643,6 @@ int lmpc_create(const lmpc_params* p, int batch, int device, lmpc_handle** out) 
     if (prop.major != 9 || prop.minor != 0) return fail(LMPC_E_NODEVICE, "liblmpc_b200 is built for sm_90a (H100) only");
     lmpc_handle* h = new (std::nothrow) lmpc_handle();
     if (!h) return fail(LMPC_E_INVALID, "out of host memory");
-    memset(h, 0, sizeof(*h));
     h->p = *p;
     h->batch = batch;
     h->device = device;
@@ -645,15 +669,8 @@ int lmpc_destroy(lmpc_handle* h) {
     free_rollout(h);
     free_store(h);
     free_bufs(dev_bufs(h), OWN_HANDLE);
+    free_tables(h, OWN_HANDLE);
     for (QpIo& q : h->hb) free_bufs(qp_rows(h, q), OWN_QP);
-    cudaFree(h->d_sets);
-    cudaFree(h->d_set_idx);
-    cudaFree(h->d_veh);
-    cudaFree(h->d_veh_idx);
-    cudaFree(h->d_noise);
-    cudaFree(h->d_noise_idx);
-    cudaFree(h->d_streams);
-    cudaFree(h->d_budget);
     if (h->stream) cudaStreamDestroy(h->stream);
     for (int i = 0; i < 4 * LMPC_HOST_SLOTS; ++i) if (h->cstream[i]) cudaStreamDestroy(h->cstream[i]);
     delete h;
@@ -679,23 +696,21 @@ long long lmpc_late_accepts(lmpc_handle* h) {
 }
 long long lmpc_kernel_launches(lmpc_handle* h) { return h ? h->launches : 0; }
 
-// Per-controller parameters: every set goes through build_const (the conversion lmpc_create uses), then the table replaces the
-// previous one once the handle's streams are idle.  Nothing about the handle changes unless every check passes.
+// Per-controller parameters: every set goes through build_const (the conversion lmpc_create uses); nsets == 0 returns to the
+// uniform kernel (DESIGN.md, "Per-controller tables").
 int lmpc_set_param_sets(lmpc_handle* h, const lmpc_params* sets, int nsets, const int* set_of_instance) {
     if (!h) return fail(LMPC_E_INVALID, "null handle");
-    int rc = check_set_index(h, "lmpc_set_param_sets", sets, nsets, set_of_instance);
-    if (rc != LMPC_OK) return rc;
-    std::vector<FtocpConstRec> rows(nsets);
-    for (int k = 0; k < nsets; ++k) {
+    int rc = install_table(h, "lmpc_set_param_sets", h->sets, sets, nsets, set_of_instance, (const FtocpConstRec*)nullptr,
+                           [&](int k, FtocpConstRec& row) {
         const lmpc_params& s = sets[k];
         if (s.N != h->p.N || s.ncx != h->p.ncx || s.ncu != h->p.ncu || s.numSS_Points != h->p.numSS_Points ||
             s.numSS_it != h->p.numSS_it || s.warm_start != h->p.warm_start)
             return fail(LMPC_E_INVALID, "lmpc_set_param_sets: set " + std::to_string(k) +
                                             " differs from the handle in N, ncx, ncu, numSS_Points, numSS_it or warm_start");
-        rc = build_const(s, rows[k].c);
-        if (rc != LMPC_OK) return fail(rc, "lmpc_set_param_sets: set " + std::to_string(k) + ": " + g_err);
-    }
-    if ((rc = swap_table(h, "lmpc_set_param_sets", rows.data(), nsets, set_of_instance, &h->d_sets, &h->d_set_idx)) != LMPC_OK) return rc;
+        const int e = build_const(s, row.c);
+        return e == LMPC_OK ? e : fail(e, "lmpc_set_param_sets: set " + std::to_string(k) + ": " + g_err);
+    });
+    if (rc != LMPC_OK) return rc;
     // a warm-start record belongs to the QP it was taken from
     if (h->d_warm_valid) {
         CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * h->batch, h->stream));
@@ -923,11 +938,9 @@ static int store_create_impl(lmpc_handle* h, const lmpc_model_params* mp, int ss
     t.nseg = mp->nseg;
     for (int i = 0; i < mp->nseg * 3; ++i) t.seg[i] = mp->seg[i];
     t.TrackLength = mp->TrackLength;
-    int rc = swap_table(h, "lmpc_store_create", &t, 1, nullptr, &h->d_trk, &h->d_trk_idx);
+    int rc = swap_table(h, "lmpc_store_create", h->trk, &t, 1, nullptr);
     if (rc != LMPC_OK) return rc;
-    if ((rc = swap_table(h, "lmpc_store_create", &r, 1, nullptr, &h->d_reg, &h->d_reg_idx)) != LMPC_OK) return rc;
-    h->trk_host.assign(1, t);
-    h->trk_idx_host.clear();
+    if ((rc = swap_table(h, "lmpc_store_create", h->reg, &r, 1, nullptr)) != LMPC_OK) return rc;
     h->laps_stored = false;
     h->ss.cap = ss_cap > 0 ? ss_cap : 1; h->ss.Tmax = Tmax;
     h->mdl.cap = model_cap; h->mdl.Tmax = Tmax; h->mdl.q = nullptr;
@@ -957,23 +970,23 @@ static int need_store(lmpc_handle* h) {
 
 // The host-chosen exchange (lmpc_ss_import_laps_dev) hands laps between any controllers: only when they all drive one circuit
 static int one_track(const lmpc_handle* h, const char* who) {
-    if (h->trk_host.size() > 1)
+    if (h->trk.rows.size() > 1)
         return fail(LMPC_E_STATE, std::string(who) + ": more than one track installed; a lap of another circuit is not a trajectory of this one");
     return LMPC_OK;
 }
 
 // The pooled exchange hands laps only within a pool group: with several tracks installed, every group must drive one circuit
 static int one_track_per_group(const lmpc_handle* h, const char* who) {
-    if (h->trk_host.size() <= 1) return LMPC_OK;
+    if (h->trk.rows.size() <= 1) return LMPC_OK;
     if (h->ngroups == 0)
         return fail(LMPC_E_STATE, std::string(who) + ": more than one track installed and no pool groups; a lap of another circuit is "
                                                      "not a trajectory of this one");
     std::vector<int> trk(h->ngroups, -1);
     for (int b = 0; b < h->batch; ++b) {
-        int& t = trk[h->pool_grp_host[b]];
-        if (t >= 0 && t != h->trk_idx_host[b])
-            return fail(LMPC_E_STATE, std::string(who) + ": pool group " + std::to_string(h->pool_grp_host[b]) + " spans two tracks");
-        t = h->trk_idx_host[b];
+        int& t = trk[h->pool_grp.index[b]];
+        if (t >= 0 && t != h->trk.index[b])
+            return fail(LMPC_E_STATE, std::string(who) + ": pool group " + std::to_string(h->pool_grp.index[b]) + " spans two tracks");
+        t = h->trk.index[b];
     }
     return LMPC_OK;
 }
@@ -993,26 +1006,21 @@ int lmpc_set_pool_groups(lmpc_handle* h, int ngroups, const int* group_of_instan
     int rc = need_store(h);
     if (rc) return rc;
     if (ngroups > LMPC_MAX_POOL_GROUPS) return fail(LMPC_E_INVALID, std::string(who) + ": ngroups above LMPC_MAX_POOL_GROUPS");
-    // the index rules of the per-controller tables; there is no table, so the index stands in for its rows
+    // the index rules of the per-controller tables; there are no rows, so the index stands in for them
     if ((rc = check_set_index(h, who, ngroups ? group_of_instance : nullptr, ngroups, group_of_instance)) != LMPC_OK) return rc;
-    int* no_table = nullptr;
-    if ((rc = swap_table<int>(h, who, nullptr, 0, group_of_instance, &no_table, &h->d_pool_grp)) != LMPC_OK) return rc;
+    if ((rc = swap_table<int>(h, who, h->pool_grp, nullptr, 0, group_of_instance)) != LMPC_OK) return rc;
     h->ngroups = ngroups;
-    if (group_of_instance) h->pool_grp_host.assign(group_of_instance, group_of_instance + h->batch);
-    else h->pool_grp_host.clear();
     return LMPC_OK;
 }
 
 // Per-controller tracks: every set is checked the way Track.py:54-133 builds the table (start i = start i-1 + length i-1 and
-// TrackLength = start + length of the last row, exactly), then the table replaces the previous one once the handle's streams are
-// idle.  Nothing about the handle changes unless every check passes.
+// TrackLength = start + length of the last row, exactly); nsets == 0 returns to the track of lmpc_store_create.
 int lmpc_set_tracks(lmpc_handle* h, const lmpc_track_params* sets, int nsets, const int* set_of_instance) {
     static const char* who = "lmpc_set_tracks";
     int rc = need_store(h);
     if (rc) return rc;
     if (h->laps_stored) return fail(LMPC_E_STATE, std::string(who) + ": laps are stored already; install tracks before the first lap");
-    if ((rc = check_set_index(h, who, sets, nsets, set_of_instance)) != LMPC_OK) return rc;
-    for (int k = 0; k < nsets; ++k) {
+    return install_table(h, who, h->trk, sets, nsets, set_of_instance, &h->store_trk, [&](int k, TrackRec& row) {
         const lmpc_track_params& t = sets[k];
         const std::string w = std::string(who) + ": track " + std::to_string(k) + ": ";
         if (t.nseg < 1 || t.nseg > LMPC_MAX_SEG) return fail(LMPC_E_INVALID, w + "nseg must be 1 .. 16");
@@ -1028,36 +1036,22 @@ int lmpc_set_tracks(lmpc_handle* h, const lmpc_track_params* sets, int nsets, co
         const int l = (t.nseg - 1) * 3;
         if (!(t.TrackLength > 0.0) || t.TrackLength != t.seg[l] + t.seg[l + 1])
             return fail(LMPC_E_INVALID, w + "TrackLength must be positive and equal the end of the last segment");
-    }
-    std::vector<TrackRec> rows;
-    if (nsets == 0) rows.push_back(h->store_trk);
-    else {          // canonical rows: padding and the entries past nseg are zero, so a record's track row is the circuit alone
-        rows.resize(nsets);
-        for (int k = 0; k < nsets; ++k) {
-            memset(&rows[k], 0, sizeof(TrackRec));
-            rows[k].nseg = sets[k].nseg;
-            for (int i = 0; i < sets[k].nseg * 3; ++i) rows[k].seg[i] = sets[k].seg[i];
-            rows[k].TrackLength = sets[k].TrackLength;
-        }
-    }
-    if ((rc = swap_table(h, who, rows.data(), (int)rows.size(), set_of_instance, &h->d_trk, &h->d_trk_idx)) != LMPC_OK) return rc;
-    h->trk_host = rows;
-    if (set_of_instance) h->trk_idx_host.assign(set_of_instance, set_of_instance + h->batch);
-    else h->trk_idx_host.clear();
-    return LMPC_OK;
+        // canonical row: padding and the entries past nseg are zero, so a record's track row is the circuit alone
+        memset(&row, 0, sizeof(TrackRec));
+        row.nseg = t.nseg;
+        for (int i = 0; i < t.nseg * 3; ++i) row.seg[i] = t.seg[i];
+        row.TrackLength = t.TrackLength;
+        return LMPC_OK;
+    });
 }
 
 // Per-controller regression constants: every set checked (the scaling range is the one K1's fp32 pre-filter is certified for:
-// safeset.cuh, above its threshold), then the table replaces the previous one once the handle's streams are idle.  Nothing
-// about the handle changes unless every check passes.
+// safeset.cuh, above its threshold); nsets == 0 returns to the constants of lmpc_store_create.
 int lmpc_set_regression_sets(lmpc_handle* h, const lmpc_regression_params* sets, int nsets, const int* set_of_instance) {
     static const char* who = "lmpc_set_regression_sets";
     int rc = need_store(h);
     if (rc) return rc;
-    if ((rc = check_set_index(h, who, sets, nsets, set_of_instance)) != LMPC_OK) return rc;
-    std::vector<RegressionRec> rows(nsets ? nsets : 1);
-    if (nsets == 0) rows[0] = h->store_reg;
-    for (int k = 0; k < nsets; ++k) {
+    return install_table(h, who, h->reg, sets, nsets, set_of_instance, &h->store_reg, [&](int k, RegressionRec& r) {
         const lmpc_regression_params& s = sets[k];
         const std::string w = std::string(who) + ": set " + std::to_string(k) + ": ";
         if (s.trToUse < 1 || s.trToUse > h->mc.trToUse)
@@ -1065,7 +1059,6 @@ int lmpc_set_regression_sets(lmpc_handle* h, const lmpc_regression_params* sets,
         if (s.MaxNumPoint < 1 || s.MaxNumPoint > K1_MAXPTS) return fail(LMPC_E_INVALID, w + "MaxNumPoint must be 1 .. 7");
         if (!(s.h >= 0x1p-1022 && s.h <= 0x1p1022)) return fail(LMPC_E_INVALID, w + "h must be finite and in [2^-1022, 2^1022]");
         if (!(isfinite(s.lamb) && s.lamb >= 0.0)) return fail(LMPC_E_INVALID, w + "lamb must be finite and >= 0");
-        RegressionRec& r = rows[k];
         memset(&r, 0, sizeof(r));
         r.trToUse = s.trToUse; r.MaxNumPoint = s.MaxNumPoint; r.h = s.h; r.lamb = s.lamb;
         for (int i = 0; i < 5; ++i) {
@@ -1074,8 +1067,8 @@ int lmpc_set_regression_sets(lmpc_handle* h, const lmpc_regression_params* sets,
                 return fail(LMPC_E_INVALID, w + "every |scaling| must be 0 or in [2^-32, 2^32]");
             r.scaling[i] = a;
         }
-    }
-    return swap_table(h, who, rows.data(), (int)rows.size(), set_of_instance, &h->d_reg, &h->d_reg_idx);
+        return LMPC_OK;
+    });
 }
 
 static int put_lap(lmpc_handle* h, LapPool& pool, int inst, int slot, int T, const double* x, const double* u) {
@@ -1210,7 +1203,7 @@ static int launch_k1(lmpc_handle* h, LapBudget retire = {}) {
     a.pts_stride = k1_pts_stride(h->mc.trToUse);
     a.xLin = h->d_xLin; a.uLin = h->d_uLin; a.pool = h->mdl; a.used = h->d_used; a.abc = h->hb[0].abc; a.status = h->d_flags;
     a.trk = tracks(h);
-    a.reg = Regressions{h->d_reg, h->d_reg_idx};
+    a.reg = h->reg.view();
     a.retire = retire;
     dim3 grid(h->batch, (h->N + a.wpb - 1) / a.wpb);
     const size_t smem = k1_smem_bytes(h->mc.trToUse, a.wpb);
@@ -1436,8 +1429,7 @@ static SimArgs sim_args(const lmpc_handle* h, const double* z, unsigned long lon
     sa.z = z; sa.seed = seed; sa.step = h->sim_step;
     sa.xn = h->d_rx[h->cur ^ 1]; sa.xgn = h->d_rg[h->cur ^ 1];
     sa.cl_x = h->d_clx; sa.cl_u = h->d_clu; sa.cl_len = h->d_cllen; sa.Tcl = h->Tcl; sa.done = h->d_done;
-    sa.veh = h->d_veh; sa.veh_idx = h->d_veh_idx; sa.trk = tracks(h);
-    sa.noise = h->d_noise; sa.noise_idx = h->d_noise_idx; sa.streams = h->d_streams;
+    sa.veh = h->veh.view(); sa.trk = tracks(h); sa.noise = h->noise.view(); sa.streams = h->streams.idx;
     return sa;
 }
 
@@ -1496,7 +1488,7 @@ int lmpc_rollout_pid_step(lmpc_handle* h, double vt, const double* z_pid_host, c
     PidArgs pa;
     pa.batch = h->batch; pa.x = xc; pa.vt = vt; pa.z = z_pid_host ? h->d_zpid : nullptr; pa.seed = seed; pa.step = h->sim_step;
     pa.u = h->hb[0].uPred; pa.u_stride = (long long)h->N * 2;
-    pa.noise = h->d_noise; pa.noise_idx = h->d_noise_idx; pa.streams = h->d_streams;
+    pa.noise = h->noise.view(); pa.streams = h->streams.idx;
     pid_input_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(pa);
     sim_step_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->mc, sim_args(h, z_sim_host ? h->d_z : nullptr, seed));
     CK(cudaGetLastError());
@@ -1507,14 +1499,12 @@ int lmpc_rollout_pid_step(lmpc_handle* h, double vt, const double* z_pid_host, c
     return LMPC_OK;
 }
 
-// Per-controller vehicles: every set is checked, then the table replaces the previous one once the handle's streams are idle.
-// Nothing about the handle changes unless every check passes.
+// Per-controller vehicles: m, Iz, lf, lr positive and all ten values finite; nsets == 0 returns to the reference vehicle.
 int lmpc_rollout_set_vehicles(lmpc_handle* h, const lmpc_vehicle_params* sets, int nsets, const int* set_of_instance) {
     static const char* who = "lmpc_rollout_set_vehicles";
     if (!h) return fail(LMPC_E_INVALID, "null handle");
-    int rc = check_set_index(h, who, sets, nsets, set_of_instance);
-    if (rc != LMPC_OK) return rc;
-    for (int k = 0; k < nsets; ++k) {
+    const lmpc_vehicle_params ref = reference_vehicle();
+    return install_table(h, who, h->veh, sets, nsets, set_of_instance, &ref, [&](int k, lmpc_vehicle_params& row) {
         const lmpc_vehicle_params& v = sets[k];
         const double all[10] = {v.m, v.lf, v.lr, v.Iz, v.Df, v.Cf, v.Bf, v.Dr, v.Cr, v.Br};
         bool ok = v.m > 0 && v.Iz > 0 && v.lf > 0 && v.lr > 0;
@@ -1522,57 +1512,46 @@ int lmpc_rollout_set_vehicles(lmpc_handle* h, const lmpc_vehicle_params* sets, i
         if (!ok)
             return fail(LMPC_E_INVALID, std::string(who) + ": vehicle " + std::to_string(k) +
                                             ": m, Iz, lf, lr must be positive and all ten values finite");
-    }
-    if (nsets == 0) {
-        const lmpc_vehicle_params ref = reference_vehicle();
-        return swap_table(h, who, &ref, 1, nullptr, &h->d_veh, &h->d_veh_idx);
-    }
-    return swap_table(h, who, sets, nsets, set_of_instance, &h->d_veh, &h->d_veh_idx);
+        row = v;
+        return LMPC_OK;
+    });
 }
 
-// Per-controller noise: the rules of lmpc_rollout_set_vehicles, with every value finite and >= 0.
+// Per-controller noise: every value finite and >= 0; nsets == 0 returns to the reference's constants.
 static_assert(sizeof(lmpc_noise_params) == 11 * sizeof(double), "lmpc_noise_params is checked as an array of its 11 doubles");
 int lmpc_rollout_set_noise(lmpc_handle* h, const lmpc_noise_params* sets, int nsets, const int* set_of_instance) {
     static const char* who = "lmpc_rollout_set_noise";
     if (!h) return fail(LMPC_E_INVALID, "null handle");
-    int rc = check_set_index(h, who, sets, nsets, set_of_instance);
-    if (rc != LMPC_OK) return rc;
-    for (int k = 0; k < nsets; ++k) {
+    const lmpc_noise_params ref = reference_noise();
+    return install_table(h, who, h->noise, sets, nsets, set_of_instance, &ref, [&](int k, lmpc_noise_params& row) {
         const double* v = (const double*)&sets[k];
         for (size_t j = 0; j < sizeof(lmpc_noise_params) / sizeof(double); ++j)
             if (!(isfinite(v[j]) && v[j] >= 0.0))
                 return fail(LMPC_E_INVALID, std::string(who) + ": noise set " + std::to_string(k) +
                                                 ": every sigma, clip and the gain must be finite and >= 0");
-    }
-    if (nsets == 0) {
-        const lmpc_noise_params ref = reference_noise();
-        return swap_table(h, who, &ref, 1, nullptr, &h->d_noise, &h->d_noise_idx);
-    }
-    return swap_table(h, who, sets, nsets, set_of_instance, &h->d_noise, &h->d_noise_idx);
+        row = sets[k];
+        return LMPC_OK;
+    });
 }
 
-// Noise streams: every stream number >= 0 (repeats allowed), then the stream array replaces the previous one once the handle's
-// streams are idle; NULL returns to stream b = b.  It takes the place of the index of swap_table, with no table.
+// Noise streams: every stream number >= 0 (repeats allowed); NULL returns to stream b = b.  An array without rows.
 int lmpc_rollout_set_noise_streams(lmpc_handle* h, const int* stream_of_instance) {
     static const char* who = "lmpc_rollout_set_noise_streams";
     if (!h) return fail(LMPC_E_INVALID, "null handle");
     for (int b = 0; b < (stream_of_instance ? h->batch : 0); ++b)
         if (stream_of_instance[b] < 0)
             return fail(LMPC_E_INVALID, std::string(who) + ": stream of instance " + std::to_string(b) + " is negative");
-    int* no_table = nullptr;
-    return swap_table<int>(h, who, nullptr, 0, stream_of_instance, &no_table, &h->d_streams);
+    return swap_table<int>(h, who, h->streams, nullptr, 0, stream_of_instance);
 }
 
-// Lap budgets: every budget >= 1, then the budget array replaces the previous one once the handle's streams are idle; NULL removes
-// the budgets.  Like the noise streams it takes the place of the index of swap_table, with no table.
+// Lap budgets: every budget >= 1; NULL removes the budgets.  An array without rows, like the noise streams.
 int lmpc_rollout_set_lap_budget(lmpc_handle* h, const int* budget_of_instance) {
     static const char* who = "lmpc_rollout_set_lap_budget";
     if (int rc = need_rollout(h)) return rc;
     for (int b = 0; b < (budget_of_instance ? h->batch : 0); ++b)
         if (budget_of_instance[b] < 1)
             return fail(LMPC_E_INVALID, std::string(who) + ": budget of instance " + std::to_string(b) + " is below 1");
-    int* no_table = nullptr;
-    return swap_table<int>(h, who, nullptr, 0, budget_of_instance, &no_table, &h->d_budget);
+    return swap_table<int>(h, who, h->budget, nullptr, 0, budget_of_instance);
 }
 
 // Regression(x, u, lamb) of Utilities.py:5-28 on every instance's closed-loop record: per-instance LTI model in the device
@@ -1796,7 +1775,7 @@ int lmpc_rollout_group_stats(lmpc_handle* h, int* out) {
     if (int rc = need_rollout(h)) return rc;
     if (!out) return fail(LMPC_E_INVALID, "null output");
     const int G = h->ngroups > 0 ? h->ngroups : 1;
-    rollout_stats_kernel<<<1, 1024, 0, h->stream>>>(h->batch, h->bk, h->d_cllen, h->d_health, h->d_pool_grp, G, h->d_stats, lap_budget(h));
+    rollout_stats_kernel<<<1, 1024, 0, h->stream>>>(h->batch, h->bk, h->d_cllen, h->d_health, h->pool_grp.idx, G, h->d_stats, lap_budget(h));
     CK(cudaGetLastError());
     h->launches += 1;
     CK(cudaMemcpyAsync(out, h->d_stats, sizeof(int) * 4 * G, cudaMemcpyDeviceToHost, h->stream));
@@ -1821,7 +1800,7 @@ static int pool_export(lmpc_handle* h, const char* who, int kbest, int Tpad, lon
         ship = h->d_poolidx + POOL_SHIP;
         CK(cudaMemcpyAsync(ship, mask, sizeof(int) * G, cudaMemcpyHostToDevice, h->stream));
     }
-    pool_local_best_kernel<<<G, 1024, 0, h->stream>>>(h->batch, h->ss, h->bk, kbest, Tpad, h->pool_min_over, h->d_pool_grp, ship,
+    pool_local_best_kernel<<<G, 1024, 0, h->stream>>>(h->batch, h->ss, h->bk, kbest, Tpad, h->pool_min_over, h->pool_grp.idx, ship,
                                                        h->d_poolidx);
     pool_export_kernel<<<G * kbest, 256, 0, h->stream>>>(h->ss, h->bk, h->d_poolidx, kbest, Tpad, gid_base, rows_dev, meta_dev);
     CK(cudaGetLastError());
@@ -1862,7 +1841,7 @@ int lmpc_pool_import_dev(lmpc_handle* h, int n_src, int share, int Tpad, long lo
     int* took = h->d_poolidx + POOL_TOOK;
     CK(cudaMemsetAsync(took, 0, sizeof(int), h->stream));
     pool_rank_kernel<<<G, 64, 0, h->stream>>>(n_src, meta_dev, order, cnt);
-    pool_import_kernel<<<h->batch, 256, 0, h->stream>>>(h->batch, h->ss, h->mdl, h->bk, share, Tpad, rows_dev, meta_dev, h->d_pool_grp, order,
+    pool_import_kernel<<<h->batch, 256, 0, h->stream>>>(h->batch, h->ss, h->mdl, h->bk, share, Tpad, rows_dev, meta_dev, h->pool_grp.idx, order,
                                                         cnt, gid_base, took, h->has_rollout ? h->d_health : nullptr);
     CK(cudaGetLastError());
     h->launches += 2;
@@ -1910,9 +1889,9 @@ static void snap_layout(lmpc_handle* h, SnapTable& t, lmpc_snapshot_header& hd) 
     t.s[SN_HEADER].base = (char*)h->d_snap;                       // the handle's header template
     t.s[SN_HEADER].bytes = SNAP_HDR_WORDS * 4;
     t.s[SN_HEADER].pack_only = 1;
-    t.s[SN_TRACK].base = (char*)h->d_trk;
-    t.s[SN_TRACK].idx = h->d_trk_idx;
-    t.s[SN_TRACK].stride = h->d_trk_idx ? sizeof(TrackRec) : 0;
+    t.s[SN_TRACK].base = (char*)h->trk.tab;
+    t.s[SN_TRACK].idx = h->trk.idx;
+    t.s[SN_TRACK].stride = h->trk.idx ? sizeof(TrackRec) : 0;
     t.s[SN_TRACK].bytes = sizeof(TrackRec);
     t.s[SN_TRACK].rec_off = SNAP_HDR_WORDS * 4;
     t.s[SN_TRACK].pack_only = 1;

@@ -24,24 +24,23 @@ struct ModelConst {
     double dt;
 };
 
-// The regression constants of every controller: row idx[b] of tab, or row 0 when idx is null (a store without regression sets
-// holds a one-row table with the constants of lmpc_store_create, |scaling| included).
-using RegressionRec = lmpc_regression_params;
-struct Regressions {
-    const RegressionRec* tab;
+// A per-controller table as the kernels read it (DESIGN.md, "Per-controller tables"): controller b reads row idx[b] of tab, or
+// row 0 when idx is null (the one-row default table of a handle without sets).
+template <typename T>
+struct Table {
+    const T* tab;
     const int* idx;
-    __device__ __forceinline__ const RegressionRec& of(int b) const { return tab[idx ? idx[b] : 0]; }
+    __device__ __forceinline__ const T& of(int b) const { return tab[idx ? idx[b] : 0]; }
 };
 
-// A track is one row of the handle's track table (lmpc_set_tracks); the ABI record is the device record.
+// The regression constants of every controller (lmpc_set_regression_sets; default: those of lmpc_store_create, |scaling|
+// included)
+using RegressionRec = lmpc_regression_params;
+using Regressions = Table<RegressionRec>;
+
+// The track of every controller (lmpc_set_tracks; default: the track of lmpc_store_create); the ABI record is the device record.
 using TrackRec = lmpc_track_params;
-// The track of every controller: row idx[b] of tab, or row 0 when idx is null (a handle without track sets holds a one-row table
-// with the track of lmpc_store_create).
-struct Tracks {
-    const TrackRec* tab;
-    const int* idx;
-    __device__ __forceinline__ const TrackRec& of(int b) const { return tab[idx ? idx[b] : 0]; }
-};
+using Tracks = Table<TrackRec>;
 
 struct LapPool {
     double* x;      // [B][cap][Tmax][6]
@@ -855,11 +854,10 @@ __global__ void shift_state_kernel(const ShiftArgs a) {
 // (seed, stream, step), stream = streams[b] or b when streams is null — statistical, not bit-wise, parity with the reference's
 // unseeded global RNG.
 // Also appends (x, u) to the closed-loop buffer and flags lap completion (SysModel.py:45-47).
-// The ten vehicle constants (SysModel.py:61-70) are read from a per-instance record: row veh_idx[b] of veh, or row 0 when veh_idx
-// is null (a handle without vehicle sets points at a one-row table holding the reference vehicle).  The arithmetic is the same
-// with the constants in memory as with them folded in at compile time (DESIGN.md, "Per-controller vehicles").  The noise
-// constants (SysModel.py:139-145) come the same way from row noise_idx[b] of noise (DESIGN.md, "Per-controller noise and
-// common random numbers").
+// The ten vehicle constants (SysModel.py:61-70) are read from the instance's row of the vehicle table (a handle without vehicle
+// sets holds a one-row table with the reference vehicle).  The arithmetic is the same with the constants in memory as with them
+// folded in at compile time (DESIGN.md, "Per-controller vehicles").  The noise constants (SysModel.py:139-145) come the same way
+// from the noise table (DESIGN.md, "Per-controller noise and common random numbers").
 struct SimArgs {
     int batch;
     const double* x;      // [B][6] curvilinear state
@@ -878,11 +876,9 @@ struct SimArgs {
     const int* flags;     // [B] step flags (K1/K2/addPoint) and QP status of the step that produced u, or nullptr;
     const int* status;     //     accumulated into health[b] (OR of flags) and health[B + b] (steps with status != 1)
     int* health;
-    const lmpc_vehicle_params* veh;   // vehicle table (lmpc_rollout_set_vehicles)
-    const int* veh_idx;               // [B] row of every instance, or nullptr: row 0
+    Table<lmpc_vehicle_params> veh;   // vehicle of every instance (lmpc_rollout_set_vehicles)
     Tracks trk;                       // curvature and finish line of every instance (lmpc_set_tracks)
-    const lmpc_noise_params* noise;   // noise table (lmpc_rollout_set_noise)
-    const int* noise_idx;             // [B] row of every instance, or nullptr: row 0
+    Table<lmpc_noise_params> noise;   // noise of every instance (lmpc_rollout_set_noise)
     const int* streams;               // [B] Philox stream of every instance (lmpc_rollout_set_noise_streams), or nullptr: b
     LapBudget retire;                 // a retired instance is not driven (the PID lap passes a null budget)
 };
@@ -905,7 +901,7 @@ __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimA
         if (a.status && a.status[b] != 1) a.health[a.batch + b] += 1;
     }
     // vehicle parameters, SysModel.py:61-70
-    const lmpc_vehicle_params& v = a.veh[a.veh_idx ? a.veh_idx[b] : 0];
+    const lmpc_vehicle_params& v = a.veh.of(b);
     const double mass = v.m, lf = v.lf, lr = v.lr, Iz = v.Iz;
     const double Df = v.Df, Cf = v.Cf, Bf = v.Bf;
     const double Dr = v.Dr, Cr = v.Cr, Br = v.Br;
@@ -961,7 +957,7 @@ __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimA
         z0 = n01.x; z1 = n01.y; z2 = n23.x;
     }
     // noise parameters, SysModel.py:139-145
-    const lmpc_noise_params& nz = a.noise[a.noise_idx ? a.noise_idx[b] : 0];
+    const lmpc_noise_params& nz = a.noise.of(b);
     const double n_vx = fmax(-nz.sim_clip[0], fmin(z0 * nz.sim_sigma[0], nz.sim_clip[0]));
     const double n_vy = fmax(-nz.sim_clip[1], fmin(z1 * nz.sim_sigma[1], nz.sim_clip[1]));
     const double n_wz = fmax(-nz.sim_clip[2], fmin(z2 * nz.sim_sigma[2], nz.sim_clip[2]));
@@ -978,8 +974,8 @@ __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimA
 // ------------------------------------------------------------------------------------------------
 // PID path-following controller, Utilities.py:42-68 (PID.solve): u = [-0.6 ey - 0.9 epsi + clip(0.25 z0, +-0.9),
 // 1.5 (vt - vx) + clip(0.10 z1, +-0.2)], z ~ N(0,1) drawn in that order.  Writes uPred[b][0] so that sim_step_kernel
-// consumes it like a controller's first predicted input.  The noise constants are row noise_idx[b] of noise (row 0 when
-// noise_idx is null), the Philox stream is streams[b] (b when streams is null), as in sim_step_kernel.
+// consumes it like a controller's first predicted input.  The noise constants are the instance's row of the noise table, the
+// Philox stream is streams[b] (b when streams is null), as in sim_step_kernel.
 struct PidArgs {
     int batch;
     const double* x;       // [B][6]
@@ -988,8 +984,7 @@ struct PidArgs {
     unsigned long long seed, step;
     double* u;             // [B][u_stride]
     long long u_stride;
-    const lmpc_noise_params* noise;   // noise table (lmpc_rollout_set_noise)
-    const int* noise_idx;             // [B] row of every instance, or nullptr: row 0
+    Table<lmpc_noise_params> noise;   // noise of every instance (lmpc_rollout_set_noise)
     const int* streams;               // [B] Philox stream of every instance, or nullptr: b
 };
 __global__ void pid_input_kernel(const PidArgs a) {
@@ -1005,7 +1000,7 @@ __global__ void pid_input_kernel(const PidArgs a) {
         const double2 n01 = curand_normal2_double(&st);
         z0 = n01.x; z1 = n01.y;
     }
-    const lmpc_noise_params& nz = a.noise[a.noise_idx ? a.noise_idx[b] : 0];
+    const lmpc_noise_params& nz = a.noise.of(b);
     const double* x = a.x + (size_t)b * 6;
     // -0.6 ey - 0.9 epsi with the one contraction the device has always computed (ptxas fused it so when the noise constants were
     // immediates); written out because the compiler otherwise picks its contraction from the surrounding code
