@@ -311,7 +311,11 @@ int lmpc_rollout_set_state(lmpc_handle* h, const double* x, const double* xglob)
 int lmpc_rollout_get_state(lmpc_handle* h, double* x, double* xglob, int* done, int* cl_len);  /* any may be NULL      */
 int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned long long seed);   /* mode 0 LTV-MPC, 1 LMPC, 2 LTI-MPC */
 /* Since lmpc_rollout_create: OR of the per-step flags (bits as in lmpc_step_host) and number of steps whose QP was not
- * reported solved (the reference would have driven on with feasible = 0, PC.py:279-283), per instance; either may be NULL. */
+ * reported solved (the reference would have driven on with feasible = 0, PC.py:279-283), per instance; either may be NULL.
+ * The simulator adds two bits of its own, in lmpc_rollout_step and lmpc_rollout_pid_step alike: 128 = a curvature lookup of
+ * the plant failed (s < 0, s exactly at the finish line, s not finite or beyond 64 laps: the reference raises, Track.py:292-310;
+ * the step went on with curvature 0), 256 = a step found the closed-loop record full (Tcl rows) and was not recorded, so the
+ * lap is longer than the record and its hand-over files it truncated. */
 int lmpc_rollout_get_health(lmpc_handle* h, int* flags_or, int* unsolved_steps);                 /* [B] host             */
 /* The rest of main.py's pipeline on the device (SURVEY §8f rank 3).
  * lmpc_rollout_pid_step: one closed-loop step under the PID path follower (Utilities.py:42-68, target speed vt); z_pid_host[B,2]

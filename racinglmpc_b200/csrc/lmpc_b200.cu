@@ -1422,7 +1422,7 @@ int lmpc_rollout_get_health(lmpc_handle* h, int* flags_or, int* unsolved_steps) 
 }
 
 // The simulator's arguments for one closed-loop step of the whole batch: state cur -> cur ^ 1 under the input uPred[b][0], noise z
-// ([B][3] standard-normal draws) or, when null, Philox.  The health inputs (flags, status, health) stay null.
+// ([B][3] standard-normal draws) or, when null, Philox.  The health inputs (flags, status, health) stay null; the caller sets them.
 static SimArgs sim_args(const lmpc_handle* h, const double* z, unsigned long long seed) {
     SimArgs sa = {};
     sa.batch = h->batch; sa.x = h->d_rx[h->cur]; sa.xg = h->d_rg[h->cur]; sa.u = h->hb[0].uPred; sa.u_stride = (long long)h->N * 2;
@@ -1490,7 +1490,9 @@ int lmpc_rollout_pid_step(lmpc_handle* h, double vt, const double* z_pid_host, c
     pa.u = h->hb[0].uPred; pa.u_stride = (long long)h->N * 2;
     pa.noise = h->noise.view(); pa.streams = h->streams.idx;
     pid_input_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(pa);
-    sim_step_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->mc, sim_args(h, z_sim_host ? h->d_z : nullptr, seed));
+    SimArgs sa = sim_args(h, z_sim_host ? h->d_z : nullptr, seed);
+    sa.health = h->d_health;          // no step flags or QP status here: only the simulator's own bits
+    sim_step_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->mc, sa);
     CK(cudaGetLastError());
     h->launches += 2;
     h->cur ^= 1;

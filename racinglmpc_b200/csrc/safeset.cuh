@@ -875,13 +875,20 @@ struct SimArgs {
     int* done;             // [B] 1 when s_next > TrackLength
     const int* flags;     // [B] step flags (K1/K2/addPoint) and QP status of the step that produced u, or nullptr;
     const int* status;     //     accumulated into health[b] (OR of flags) and health[B + b] (steps with status != 1)
-    int* health;
+    int* health;           //     the simulator's own bits (SIM_LOOKUP_FAILED, SIM_RECORD_FULL) go to health[b] too
     Table<lmpc_vehicle_params> veh;   // vehicle of every instance (lmpc_rollout_set_vehicles)
     Tracks trk;                       // curvature and finish line of every instance (lmpc_set_tracks)
     Table<lmpc_noise_params> noise;   // noise of every instance (lmpc_rollout_set_noise)
     const int* streams;               // [B] Philox stream of every instance (lmpc_rollout_set_noise_streams), or nullptr: b
     LapBudget retire;                 // a retired instance is not driven (the PID lap passes a null budget)
 };
+// Health bits of the simulator itself (the step flags use 1 .. 64):
+//   SIM_LOOKUP_FAILED  a sub-step's curvature lookup failed (s < 0, s at the finish line after the wrap, s not finite or beyond
+//                      64 laps): the reference raises there (Track.py:292-310); the step went on with curvature 0
+//   SIM_RECORD_FULL    the closed-loop record already held Tcl rows, so this step's (x, u) was not recorded: the lap is longer
+//                      than the record and a hand-over of it files a truncated lap
+constexpr int SIM_LOOKUP_FAILED = 128;
+constexpr int SIM_RECORD_FULL = 256;
 
 }  // namespace lmpc
 #include <curand_kernel.h>
@@ -912,6 +919,7 @@ __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimA
     const double delta = a.u[(size_t)b * a.u_stride], acc = a.u[(size_t)b * a.u_stride + 1];
     double vx = x[0], vy = x[1], wz = x[2], epsi = x[3], s = x[4], ey = x[5];
     double psi = g[3], X = g[4], Y = g[5];
+    int sim_bits = 0;
     if (a.cl_x) {
         const int T = a.cl_len[b];
         if (T < a.Tcl) {
@@ -920,6 +928,8 @@ __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimA
             a.cl_u[((size_t)b * a.Tcl + T) * 2] = delta;
             a.cl_u[((size_t)b * a.Tcl + T) * 2 + 1] = acc;
             a.cl_len[b] = T + 1;
+        } else {
+            sim_bits = SIM_RECORD_FULL;
         }
     }
     const double sd = sin(delta), cd = cos(delta);
@@ -945,6 +955,8 @@ __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimA
         vx = nvx; vy = nvy; wz = nwz; epsi = nepsi; s = ns; ey = ney;
         ++i;
     }
+    if (!okc) sim_bits |= SIM_LOOKUP_FAILED;
+    if (a.health && sim_bits) a.health[b] |= sim_bits;
     double z0, z1, z2;
     if (a.z) {
         z0 = a.z[(size_t)b * 3]; z1 = a.z[(size_t)b * 3 + 1]; z2 = a.z[(size_t)b * 3 + 2];
