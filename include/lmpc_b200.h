@@ -424,7 +424,8 @@ int lmpc_ss_import_laps_dev(lmpc_handle* h, const int* ss_slots_host, const int*
  * entry points below keep the books on the device instead, so that a Monte-Carlo batch hands laps over without the host.
  * Slot tables per controller: safe set ss_time[B,ss_cap], ss_lap[B,ss_cap] (lap number, -1 = free), it[B]; regression model
  * md_time[B,model_cap], md_seq[B,model_cap] (arrival number, -1 = free), md_cnt[B].  lmpc_books_set uploads them (e.g. after
- * seeding through the host-driven path); lmpc_books_get reads them back with the derived selection (any pointer may be NULL):
+ * seeding through the host-driven path) and derives the selection of the uploaded tables, so that K2, addPoint, K1 and the
+ * pooled export read them from then on; lmpc_books_get reads them back with the derived selection (any pointer may be NULL):
  * sel/is_prev[B,numSS_it], prev_slot[B], used[B,trToUse], lap_hist[B,16] = lengths of the laps driven since, lap_n[B]. */
 int lmpc_books_set(lmpc_handle* h, const int* ss_time, const int* ss_lap, const int* it, const int* md_time, const int* md_seq,
                    const int* md_cnt);

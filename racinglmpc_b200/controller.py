@@ -510,8 +510,9 @@ class BatchedController:
         """Give instance b the gathered lap ``src[b]`` (index into rows[n_src,Tpad,9]; -1: nothing) as a lap driven BEFORE its
         own most recent one: LMPC.addTrajectory + PredictiveModel.addTrajectory (main.py:117-119) of a lap another controller
         drove.  The lap keeps its own Qfun and lap time ``lap_times[b]``; the instance's latest lap stays lap it-1 (the one
-        LMPC.addPoint extends, PC.py:466-476).  An instance for which the lap would not be among its numSS_it fastest is
-        skipped.  Returns the instances that took a lap."""
+        LMPC.addPoint extends, PC.py:466-476).  An instance for which the lap would not be among its numSS_it fastest leaves it out
+        of the safe set, but its regression model still takes it (main.py:117-119 adds every lap to both; with trToUse > numSS_it
+        it can be among the trToUse shortest).  Returns the instances whose safe set took a lap."""
         src = np.asarray(src, np.int32).reshape(self.B)
         n_src = int(lens_dev.shape[0])
         ss_slots = np.full(self.B, -1, np.int32); m_slots = np.full(self.B, -1, np.int32); use = np.full(self.B, -1, np.int32)
@@ -521,8 +522,11 @@ class BatchedController:
             lt, last = int(lap_times[b]), self.it[b] - 1
             times = self.LapTime[b][:last] + [lt] + self.LapTime[b][last:]
             order = list(np.argsort(np.array(times), kind="stable"))[:self.numSS_it]
-            if last not in order:
-                continue                                  # never selected (PC.py:395) -> not stored
+            if last not in order:                         # never selected (PC.py:395) -> not in the safe set
+                if to_model:
+                    m_slots[b] = self._model_slot_for(b, lt)
+                    use[b] = src[b]
+                continue
             book = self.ss_book[b]
             self.LapTime[b] = times
             if last in book.slot_of:                      # own latest lap moves up one lap number
@@ -540,13 +544,13 @@ class BatchedController:
             use[b] = src[b]
             if to_model:
                 m_slots[b] = self._model_slot_for(b, lt)
-        took = np.nonzero(use >= 0)[0]
-        if len(took):
+        given = np.nonzero(use >= 0)[0]
+        if len(given):
             nat.check(self._lib.lmpc_ss_import_laps_dev(self._h, nat.ptr(ss_slots), nat.ptr(m_slots) if to_model else None,
                                                         nat.ptr(use), n_src, int(Tpad), nat.ptr(rows_dev), nat.ptr(lens_dev)))
-            for b in took:
-                self._touch(b, sel=True, used=to_model)
-        return took
+            for b in given:
+                self._touch(b, sel=bool(ss_slots[b] >= 0), used=to_model)
+        return np.nonzero(ss_slots >= 0)[0]
 
     # ------------------------------------------------------------------ lap books on the device (csrc/lapbooks.cuh)
     def enable_device_books(self):

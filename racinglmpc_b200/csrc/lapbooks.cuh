@@ -7,7 +7,9 @@
 // (PredictiveModel.py:31,35-46).  For a Monte-Carlo batch these decisions are made for thousands of controllers in the same
 // step, so they live here: one thread per controller walks its (at most 8-entry) slot tables.  Only laps that can still be
 // selected are stored (a lap that is not among the fastest when it arrives never becomes one: faster laps only push it
-// further down), which makes the fixed-capacity pools equivalent to the reference's unbounded lists.
+// further down), which makes the fixed-capacity pools equivalent to the reference's unbounded lists as long as the laps that
+// must stay resident fit (health bit 64 otherwise).  tests/support/lapbook_exact.py restates the lists and the tests compare
+// the tables with them after every hand-over and import.
 //
 // Slot tables per controller b:  safe set  ss_time[b][cap], ss_lap[b][cap] (lap number, -1 = free), it[b];
 //                                model     md_time[b][mcap], md_seq[b][mcap] (arrival order, -1 = free), md_cnt[b].
@@ -31,7 +33,8 @@ __device__ __forceinline__ bool key_less(int t1, int n1, int t2, int n2) { retur
 // LMPC.addTrajectory bookkeeping for a lap of `T` rows.  import == false: the controller's own new lap (lap number it).
 // import == true: a lap another controller drove, filed BEFORE the controller's own latest lap (which stays lap it-1, the one
 // addPoint extends): it takes lap number it-1, the own latest moves to it; it is skipped (-1) when it would not be among the
-// numSS_it fastest.  Returns the slot to copy the lap into, -1 = not stored, -2 = pool too small.
+// numSS_it fastest.  Returns the slot to copy the lap into, -1 = not stored, -2 = pool too small (the tables are left as they
+// were).
 __device__ inline int book_ss_add(const LapBooks& k, int b, int T, bool import) {
     int* tm = k.ss_time + (size_t)b * k.ss_cap;
     int* ln = k.ss_lap + (size_t)b * k.ss_cap;
@@ -57,7 +60,10 @@ __device__ inline int book_ss_add(const LapBooks& k, int b, int T, bool import) 
             if (rank < k.numSS_it) continue;                     // one of the fastest: keep
             if (slot < 0 || tm[s] > vt || (tm[s] == vt && ln[s] < vn)) { slot = s; vt = tm[s]; vn = ln[s]; }
         }
-        if (slot < 0) return -2;
+        if (slot < 0) {                                          // nothing filed: the own latest lap keeps its number
+            if (import) for (int s = 0; s < k.ss_cap; ++s) if (ln[s] == it) ln[s] = it - 1;
+            return -2;
+        }
     }
     tm[slot] = T;
     ln[slot] = lapno;
@@ -101,7 +107,7 @@ __device__ inline int book_refresh(const LapBooks& k, int b) {
     const int* ln = k.ss_lap + (size_t)b * k.ss_cap;
     const int it = k.it[b];
     int flag = 0, prev = -1, last = 0;
-    for (int s = 0; s < k.ss_cap; ++s) if (ln[s] == it - 1) prev = s;
+    for (int s = 0; s < k.ss_cap; ++s) if (it > 0 && ln[s] == it - 1) prev = s;   // it = 0: no lap (a free slot has ln = -1)
     for (int c = 0; c < k.numSS_it; ++c) {
         int best = -1;
         for (int s = 0; s < k.ss_cap; ++s) {
@@ -112,7 +118,7 @@ __device__ inline int book_refresh(const LapBooks& k, int b) {
         }
         if (best < 0) { flag = 8; best = last; } else last = best;
         k.sel[(size_t)b * k.numSS_it + c] = best;
-        k.isprev[(size_t)b * k.numSS_it + c] = (ln[best] == it - 1) ? 1 : 0;
+        k.isprev[(size_t)b * k.numSS_it + c] = (it > 0 && ln[best] == it - 1) ? 1 : 0;
     }
     k.prevslot[b] = prev;
     const int* mt = k.md_time + (size_t)b * k.md_cap;
@@ -132,6 +138,12 @@ __device__ inline int book_refresh(const LapBooks& k, int b) {
     return flag;
 }
 
+// The selection of tables written from outside (lmpc_books_set): book_refresh of every controller.  One thread per controller.
+__global__ void books_refresh_kernel(int batch, LapBooks k) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b < batch) book_refresh(k, b);
+}
+
 // Lap hand-over of every controller whose lap just ended (done[b] != 0), bookkeeping included: main.py:113-119
 // (lmpc.addTrajectory + predictiveModel.addTrajectory of the lap Simulator.sim returned), SysModel.py:50 (s -= TrackLength),
 // PC.py:445 (timeStep = 0).  One CTA per controller; no host involvement.
@@ -144,8 +156,8 @@ __global__ void __launch_bounds__(256) commit_laps_books_kernel(int batch, LapPo
     const int Trec = cl_len[b];
     const double TrackLength = trk.of(b).TrackLength;
     if (threadIdx.x == 0) {
-        s_ss = lmpc ? book_ss_add(k, b, min(Trec, ss.Tmax), false) : -1;
-        s_md = book_md_add(k, b, min(Trec, model.Tmax));
+        s_ss = lmpc ? book_ss_add(k, b, Trec, false) : -1;       // ordered by the lap time; rows beyond Tmax are not stored
+        s_md = book_md_add(k, b, Trec);
         const int n = k.lap_n[b];
         if (n < LAP_HIST) k.lap_hist[(size_t)b * LAP_HIST + n] = Trec;
         k.lap_n[b] = n + 1;
@@ -184,8 +196,8 @@ __global__ void __launch_bounds__(256) seed_books_kernel(int batch, LapPool ss, 
     __syncthreads();
     for (int c = 0; c < copies; ++c) {
         if (threadIdx.x == 0) {
-            s_ss = lmpc ? book_ss_add(k, b, min(Trec, ss.Tmax), false) : -1;
-            s_md = book_md_add(k, b, min(Trec, model.Tmax));
+            s_ss = lmpc ? book_ss_add(k, b, Trec, false) : -1;
+            s_md = book_md_add(k, b, Trec);
         }
         __syncthreads();
         if (s_ss >= 0) copy_ss_lap_block(ss, ss.lap_index(b, s_ss), cx, cu, Trec, TrackLength);
@@ -298,7 +310,10 @@ __global__ void __launch_bounds__(64) pool_rank_kernel(int n_src, const int* met
 }
 
 // Every controller takes the `share` fastest laps of its own pool group that it does not own (LMPC.addTrajectory +
-// PredictiveModel.addTrajectory of a lap another controller drove, main.py:117-119), filed before its own latest lap.  One CTA
+// PredictiveModel.addTrajectory of a lap another controller drove, main.py:117-119), filed before its own latest lap.  A lap
+// is ordered by its lap time lt in both tables, as an own lap by Trec; only the rows that fit are stored.  The regression model
+// takes the lap also when the safe set drops it: main.py adds every lap to both lists, and with trToUse > numSS_it a lap outside
+// the numSS_it fastest can be among the trToUse shortest.  A controller with no lap of its own (it = 0) takes nothing.  One CTA
 // per controller.
 __global__ void __launch_bounds__(256) pool_import_kernel(int batch, LapPool ss, LapPool model, LapBooks k, int share, int Tpad,
                                                           const double* rows, const int* meta, const int* grp, const int* order,
@@ -319,14 +334,14 @@ __global__ void __launch_bounds__(256) pool_import_kernel(int batch, LapPool ss,
             s_src = src;
             s_ss = book_ss_add(k, b, lt, true);
             s_md = -1;
-            if (s_ss >= 0) s_md = book_md_add(k, b, lt);
+            if (s_ss != -2 && k.it[b] > 0) s_md = book_md_add(k, b, lt);
         }
         __syncthreads();
         const int c_ss = s_ss, c_md = s_md;                       // private copies: thread 0 rewrites the shared ones next round
         const double* R = rows + (size_t)s_src * Tpad * XR_COLS;
         if (c_ss >= 0) file_ss_row_block(ss, ss.lap_index(b, c_ss), R, min(len, min(Tpad, ss.Tmax)), took);
-        // the model stores the lap as driven: rows up to the finish line
-        if (c_md >= 0) file_model_row_block(model, model.lap_index(b, c_md), R, min(lt, min(len, model.Tmax)));
+        // the model stores the lap as driven: rows up to the finish line, of the Tpad rows shipped
+        if (c_md >= 0) file_model_row_block(model, model.lap_index(b, c_md), R, min(min(lt, len), min(Tpad, model.Tmax)));
         __syncthreads();
         if (threadIdx.x == 0 && c_ss == -2 && flags_or) flags_or[b] |= 64;
     }

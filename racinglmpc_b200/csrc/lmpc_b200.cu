@@ -1720,6 +1720,9 @@ int lmpc_books_set(lmpc_handle* h, const int* ss_time, const int* ss_lap, const 
                                                    {k.md_seq, md_seq}, {k.md_cnt, md_cnt}})))
         return rc;
     CK(cudaMemsetAsync(k.lap_n, 0, sizeof(int) * h->batch, h->stream));
+    books_refresh_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->batch, k);   // sel, is_prev, prev_slot, used of these tables
+    CK(cudaGetLastError());
+    h->launches += 1;
     CK(cudaStreamSynchronize(h->stream));
     return LMPC_OK;
 }
