@@ -14,9 +14,9 @@ a collective the others skip.
                        a rank's candidates are its own fastest few: ~60 KB per rank instead of every lap), all ranks all-gather
                        them over NCCL, rank them by (lap time, global id) and every controller files the `share` fastest laps
                        it does not own as additional stored laps (safe set + regression model).
-With pool groups (run(pool_groups=...)) the exchange runs within each group; run(readiness="group") gives every group its
-own round counter, so a group exchanges once its own slowest controller is `ship_after` steps into lap r+1 (the ranks then
-agree on one vector of ready groups per poll).
+With pool groups (run(pool_groups=...)) the exchange runs within each group.  One schedule (sharding.ExchangeSchedule) decides
+every poll, on one row for the whole batch or, with run(readiness="group"), one row and round counter per group, so a group
+exchanges once its own slowest controller is `ship_after` steps into lap r+1 (the ranks agree on the ready rows per poll).
 
   python benchmarks/rollout_mc.py --batch 8192 --laps 3            (1 GPU)
   python -m torch.distributed.run --nnodes=1 --nproc-per-node 8 --master-addr 127.0.0.1 benchmarks/rollout_mc.py --batch 8192
@@ -180,37 +180,23 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     kbest = share + 1
     rows = torch.zeros(G * kbest, tpad, 9, dtype=torch.float64, device=dev)
     meta = torch.zeros(G * kbest, 4, dtype=torch.int32, device=dev)
-    rows_all = torch.zeros(world * G * kbest, tpad, 9, dtype=torch.float64, device=dev)
-    meta_all = torch.zeros(world * G * kbest, 4, dtype=torch.int32, device=dev)
-    agree = torch.zeros(2, dtype=torch.int32, device=dev)
+    rows_all, meta_all = (rows, meta) if world == 1 else (torch.zeros(world * G * kbest, tpad, 9, dtype=torch.float64, device=dev),
+                                                          torch.zeros(world * G * kbest, 4, dtype=torch.int32, device=dev))
     gidx = np.zeros(B, np.int64) if pool_groups is None else np.asarray(pool_groups[0]).reshape(B)
-    if readiness == "group":
-        # a group with no controller on any rank reports the empty-group sentinel everywhere and would count as ready: never exchange it
-        live = sharding.sum_over_ranks(np.bincount(gidx, minlength=G), dev) > 0
-        next_rounds = np.ones(G, np.int64)
+    # a group with no controller on any rank reports the empty-group sentinel everywhere and would count as ready: never exchange it
+    live = sharding.sum_over_ranks(np.bincount(gidx, minlength=G), dev) > 0 if readiness == "group" else None
+    sched = sharding.ExchangeSchedule(G, laps, ship_after, poll, readiness, mode == "pooled", live, capture is not None, start)
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     if world > 1:
         dist.barrier()
     torch.cuda.synchronize()
     max_steps = int(max_steps) or 300 * laps
-    steps, next_round, n_xchg, xchg_s, took_total = 0, 1, 0, 0.0, 0
-    xsteps = [[] for _ in range(G)]                      # closed-loop steps at which each group exchanged
-    repeat, skip, diverged = False, np.zeros(G, bool), None
-    last_poll, last_ready = -1, None                    # the last poll, and the groups it exchanged (None: none)
-    if start is not None:
-        steps, next_round = int(start["steps"]), int(start["next_round"])
-        if readiness == "group":
-            next_rounds = np.asarray(start["next_rounds"], np.int64).copy()
-        xsteps = [list(v) for v in start["exchange_steps"]]
-        repeat = steps % poll == 0                      # the capture was taken at a poll: decide it again under the new laps
-        skip = np.asarray(start["exchanged"], bool).reshape(G)
-    steps0 = steps
-    every_group = np.ones(G, bool)
+    steps, n_xchg, xchg_s, took_total = sched.start_step, 0, 0.0, 0
     it_sum, it_n, it_max = 0.0, 0, 0                     # interior-point iterations, sampled at the polls
     l0 = c.kernel_launches
     e0.record(stream)
-    while steps < max_steps or repeat:
-        if not repeat:
+    while steps < max_steps or sched.repeat:
+        if not sched.repeat:
             c.rollout_step(seed=seed + rank)
             c.rollout_commit_laps_dev()                   # every controller whose lap just ended hands it over, on the device
             steps += 1
@@ -218,49 +204,24 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
                 continue
         # ---- poll: four integers of progress (per group); ranks agree on what happens next (same decision everywhere, no deadlock)
         prog = c.rollout_group_stats() if readiness == "group" else np.array([c.rollout_stats()])
-        if not repeat:                                    # the repeated poll of a resumed run has no step of its own
+        if not sched.repeat:                              # the repeated poll of a resumed run has no step of its own
             its = c.step_results()["iters"]
             it_sum += float(its.mean()); it_n += 1; it_max = max(it_max, int(its.max()))
-        if readiness == "group":
-            ready_g, done = sharding.agree_groups(sharding.ready_groups(prog, next_rounds, laps, ship_after) & live & ~skip,
-                                                  prog[:, 0].min() >= laps, dev)
-            if capture is not None and diverged is None and not done and \
-                    (sharding.ready_groups(prog, next_rounds, np.iinfo(np.int32).max, ship_after) & live & ~ready_g).any():
-                diverged = steps                          # a longer run exchanges a round >= laps here
-            ready = int(ready_g.any())
-            ship = None if ready_g.all() else ready_g
-        else:
-            ready = int(mode == "pooled" and sharding.ready_groups(prog, next_round, laps, ship_after)[0] and not skip[0])
-            done = int(prog[0, 0] >= laps)
-            if world > 1:
-                agree[0], agree[1] = ready, done
-                dist.all_reduce(agree, op=dist.ReduceOp.MIN)
-                ready, done = int(agree[0].item()), int(agree[1].item())
-            ready_g, ship = every_group, None
-        if repeat:
-            repeat, skip = False, np.zeros(G, bool)
-        last_poll, last_ready = steps, (ready_g if ready else None)
-        if ready:
+        ready_g, done = sched.poll(steps, prog, dev)
+        if ready_g.any():
             tx = time.perf_counter()
             with torch.cuda.stream(stream):
-                c.pool_export(kbest, tpad, rank * B, rows, meta, groups=ship)
+                c.pool_export(kbest, tpad, rank * B, rows, meta, groups=None if ready_g.all() else ready_g)
                 if world > 1:
                     dist.all_gather_into_tensor(rows_all, rows)
                     dist.all_gather_into_tensor(meta_all, meta)
-                    took_total += c.pool_import(world * G * kbest, share, tpad, rank * B, rows_all, meta_all, count=True)
-                else:
-                    took_total += c.pool_import(G * kbest, share, tpad, 0, rows, meta, count=True)
+                took_total += c.pool_import(world * G * kbest, share, tpad, rank * B, rows_all, meta_all, count=True)
             xchg_s += time.perf_counter() - tx
             n_xchg += 1
             if budget is not None:
                 retired = c.books()["lap_n"] >= budget
                 for g in np.nonzero(ready_g)[0]:
                     retired_at_last[g] = bool(retired[gidx == g].any())
-            next_round += 1
-            for g in np.nonzero(ready_g)[0]:
-                xsteps[g].append(steps)
-            if readiness == "group":
-                next_rounds[ready_g] += 1
         if done:
             break
     e1.record(stream)
@@ -272,11 +233,9 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         tc = time.perf_counter()
         capture.update(records=c.snapshot(), clock=c.rollout_clock)
         c.sync()
-        capture.update(capture_s=time.perf_counter() - tc, steps=steps, next_round=next_round,
-                       next_rounds=next_rounds.tolist() if readiness == "group" else None,
-                       exchanged=(last_ready if last_poll == steps and last_ready is not None else np.zeros(G, bool)).tolist(), exchange_steps=xsteps,
-                       diverged_step=diverged, batch=B, laps=laps, mode=mode, readiness=readiness, poll=poll, warm=bool(warm),
-                       pool_groups=G, layout=c.snapshot_layout(), lap_budget=None if budget is None else budget.tolist())
+        capture.update(capture_s=time.perf_counter() - tc, **sched.state(steps), batch=B, laps=laps, mode=mode, readiness=readiness,
+                       poll=poll, warm=bool(warm), pool_groups=G, layout=c.snapshot_layout(),
+                       lap_budget=None if budget is None else budget.tolist())
     flags_or, unsolved = c.rollout_health()
     stats = []
     for r in range(laps):
@@ -284,7 +243,7 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         a = a if a.size else np.array([0])
         stats.append({"lap": r + 1, "n": int((bk["lap_n"] > r).sum()), "mean": float(a.mean()), "min": int(a.min()), "max": int(a.max())})
     out = {"benchmark": "configs[3] LMPC Monte-Carlo rollouts", "mode": mode, "n_gpus": world, "batch_per_gpu": B,
-           "closed_loop_steps": steps, "ms_total": ms, "controller_steps_per_s": B * world * (steps - steps0) / (ms * 1e-3),
+           "closed_loop_steps": steps, "ms_total": ms, "controller_steps_per_s": B * world * (steps - sched.start_step) / (ms * 1e-3),
            "kernel_launches_rank0": int(c.kernel_launches - l0), "lap_stats_rank0": stats, "device_pid_laps_s": pid_s,
            "exchanges": n_xchg, "exchange_s_total": xchg_s, "exchange_ms_each": 1e3 * xchg_s / max(n_xchg, 1),
            "allgather_bytes_per_rank": int(rows.numel() * 8 + meta.numel() * 4), "laps_filed_rank0": took_total,
@@ -304,7 +263,7 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         out["laps_filed_per_group_rank0"] = [int(filed[gidx == g].sum()) for g in range(G)]
     if pool_groups is not None or readiness == "group":
         out["readiness"] = readiness
-        out["exchange_steps_per_group_rank0"] = xsteps
+        out["exchange_steps_per_group_rank0"] = sched.exchange_steps
     if budget is not None:
         driven = _driven_steps(bk, c.rollout_state()) - driven0
         out["lap_budget"] = int(budget[0]) if (budget == budget[0]).all() else "per controller, %d .. %d" % (budget.min(), budget.max())
@@ -339,8 +298,8 @@ def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, b
     captured laps, or a lap budget below the captured one."""
     if not isinstance(start, dict):
         raise ValueError("start is a capture dict of an earlier run")
-    need = ("records", "clock", "steps", "next_round", "next_rounds", "exchanged", "exchange_steps", "diverged_step", "batch", "laps",
-            "mode", "readiness", "poll", "warm", "pool_groups", "layout")
+    need = ("records", "clock") + sharding.ExchangeSchedule.FIELDS + ("batch", "laps", "mode", "readiness", "poll", "warm",
+                                                                      "pool_groups", "layout")
     missing = [k for k in need if k not in start]
     if missing:
         raise ValueError("start lacks %s: pass the dict run(capture=...) filled" % ", ".join(missing))

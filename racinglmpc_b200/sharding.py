@@ -100,12 +100,53 @@ def ready_groups(stats, next_round, laps, ship_after):
 def agree_groups(ready, done, device, group=None):
     """One MIN all-reduce of [ready_0 .. ready_{G-1}, done] (int32): a group exchanges only if it is ready on every rank, and the
     batch stops only once every rank is done.  Returns (ready bool [G], done bool), the same on every rank."""
-    v = np.append(np.asarray(ready, bool).reshape(-1), bool(done)).astype(np.int32)
+    ready, done = np.asarray(ready, bool).reshape(-1), bool(done)
     if dist.is_initialized() and dist.get_world_size(group) > 1:
-        t = torch.from_numpy(v).to(device)
+        t = torch.from_numpy(np.append(ready, done).astype(np.int32)).to(device)
         dist.all_reduce(t, op=dist.ReduceOp.MIN, group=group)
         v = t.cpu().numpy()
-    return v[:-1] != 0, bool(v[-1])
+        return v[:-1] != 0, bool(v[-1])
+    return ready, done
+
+
+class ExchangeSchedule:
+    """When the pooled exchange runs, and what a resumed run needs: one row for the whole batch (readiness="batch"; it decides for
+    every pool group) or one per group ("group"), each with a round counter.  A poll agrees over the ranks `done` and the rows that
+    ready_groups finds ready, less the independent mode, rows not `live` and what a repeated poll already exchanged.  With
+    `capture`, group readiness records the first poll, not done, at which a live group was ready for a round >= laps."""
+    FIELDS = ("steps", "next_round", "next_rounds", "exchanged", "exchange_steps", "diverged_step")
+
+    def __init__(self, groups, laps, ship_after, poll, readiness="batch", pooled=True, live=None, capture=False, start=None):
+        self.G, self.grouped, self.laps, self.ship_after = int(groups), readiness == "group", laps, ship_after
+        n = self.G if self.grouped else 1
+        self.live = (np.ones(n, bool) if live is None else np.asarray(live, bool).reshape(n)) & bool(pooled)
+        self.watch, self.diverged_step, self.last_poll = bool(capture) and self.grouped, None, -1
+        self.start_step, self.next_round = (0, 1) if start is None else (int(start["steps"]), int(start["next_round"]))
+        self.rounds = np.array(start["next_rounds"] if start is not None and self.grouped else [self.next_round] * n, np.int64)
+        self.exchange_steps = [[] for _ in range(self.G)] if start is None else [list(v) for v in start["exchange_steps"]]
+        self.exchanged = np.zeros(self.G, bool) if start is None else np.asarray(start["exchanged"], bool).reshape(self.G)
+        self.repeat = start is not None and self.start_step % poll == 0     # captured at a poll: decide it again, under new laps
+
+    def poll(self, steps, prog, device):
+        """The poll at closed-loop step `steps` on the progress rows prog [rows, 4] -> (bool [G]: groups to exchange now, done)."""
+        ok = self.live & ~self.exchanged[:len(self.rounds)] if self.repeat else self.live     # row r's first group is group r
+        ready, done = agree_groups(ready_groups(prog, self.rounds, self.laps, self.ship_after) & ok, prog[:, 0].min() >= self.laps, device)
+        if self.watch and self.diverged_step is None and not done and \
+                (ready_groups(prog, self.rounds, np.iinfo(np.int32).max, self.ship_after) & self.live & ~ready).any():
+            self.diverged_step = steps
+        self.exchanged, self.last_poll, self.repeat = ready if self.grouped else ready.repeat(self.G), steps, False
+        if ready.any():
+            self.next_round += 1
+            self.rounds += ready
+            for g in np.nonzero(self.exchanged)[0]:
+                self.exchange_steps[g].append(steps)
+        return self.exchanged, done
+
+    def state(self, steps):
+        """The FIELDS of a capture taken at closed-loop step `steps` (next_rounds is None under batch readiness)."""
+        return dict(steps=steps, next_round=self.next_round, next_rounds=self.rounds.tolist() if self.grouped else None,
+                    exchanged=(self.exchanged if self.last_poll == steps else np.zeros(self.G, bool)).tolist(),
+                    exchange_steps=self.exchange_steps, diverged_step=self.diverged_step)
 
 
 def sum_over_ranks(values, device, group=None):
