@@ -50,7 +50,7 @@ def layout(warm=False):
 
 def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, poll=8, max_steps=0, seed=1234, local=None, warm=False,
         final=None, param_sets=None, vehicle_sets=None, books=None, track_sets=None, pool_groups=None, readiness="batch",
-        capture=None, start=None, noise_sets=None, noise_streams=None, regression_sets=None, lap_budget=None):
+        capture=None, start=None, noise_sets=None, noise_streams=None, regression_sets=None, lap_budget=None, measurement_sets=None):
     """One Monte-Carlo run on this rank's GPU (torch.distributed may or may not be initialised).  Returns a dict (all ranks).
     final: None, or a dict that receives the closed loop's end state (rollout_state) and the last step's solver report (step_results).
     books: None, or a dict that receives the lap books (books) and the health counters (flags_or, unsolved).
@@ -68,6 +68,9 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     noise_streams: None, or the [batch] stream numbers handed to BatchedController.set_noise_streams (common random numbers:
     controllers on one stream meet the same draws).  Streams are local to a rank: every rank keys its Philox draws with its own
     seed (seed + rank), so controllers pair only with controllers of their own rank.
+    measurement_sets: None, or (meas, index) handed to BatchedController.set_measurement_noise (a sweep over the sensor noise the
+    controllers see, PID lap included: its record, and so the seeded stores, are measured data; the result then holds
+    per-measurement-set lap statistics under "per_measurement_rank0").  The measurement draws pair on noise_streams like the others.
     regression_sets: None, or (regs, index) handed to BatchedController.set_regression (a sweep over the learned model's
     bandwidth, neighbour count, ridge, feature scaling and laps used, trToUse up to the store's 4; the result then holds
     per-regression-set lap statistics under "per_regression_rank0").  The pooled mode exchanges laps whatever the model setting:
@@ -97,7 +100,7 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     clock and the scheduler state are set, and the run first repeats the poll the capture was taken at, under the new `laps`
     (groups that exchanged at that poll are not exchanged again), then steps on.  A run to 3 laps captured and resumed to 5
     therefore equals a run to 5 laps bit for bit (books, end states, health, exchange steps).  Tables (param_sets, vehicle_sets,
-    noise_sets, noise_streams, regression_sets, track_sets, pool_groups) are installed from the arguments, as for a fresh run.  ValueError before any device work when start
+    noise_sets, noise_streams, measurement_sets, regression_sets, track_sets, pool_groups) are installed from the arguments, as for a fresh run.  ValueError before any device work when start
     does not match the batch, the layout, the mode, the readiness, the poll interval or the pool groups, or when laps is not
     above the captured laps.
     lap_budget: None (every controller is stepped until the slowest has its laps), or the laps every controller drives before it
@@ -140,11 +143,13 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     c = BatchedController(par, B, workloads.track_seg_table(), rp.TRACK_LENGTH, trToUse=TR_TO_USE, numSS_Points=numSS_Points,
                           numSS_it=numSS_it, QterminalSlack=Qts, device=local, Tmax=TMAX, ss_cap=SS_CAP, model_cap=MODEL_CAP,
                           warm_start=warm)
+    c.enable_rollout(Tcl=TCL)                            # before the tables: the measurement noise belongs to the closed loop
     # the per-controller tables in the order they are installed: (arguments of the install call or None, install call, result key
     # of the per-row lap statistics or None)
     tables = ((param_sets, c.set_param_sets, "per_set_rank0"), (vehicle_sets, c.set_vehicles, "per_vehicle_rank0"),
               (noise_sets, c.set_noise, "per_noise_rank0"),
               (None if noise_streams is None else (noise_streams,), c.set_noise_streams, None),
+              (measurement_sets, c.set_measurement_noise, "per_measurement_rank0"),
               (regression_sets, c.set_regression, "per_regression_rank0"), (track_sets, c.set_tracks, "per_track_rank0"),
               (pool_groups, c.set_pool_groups, None))
     for args, install, _ in tables:
@@ -158,7 +163,6 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     x0 = np.tile(np.array([0.5, 0, 0, 0, 0, 0.0]), (B, 1))
     # ---- main.py:65-66 + 99-110 on the device: every controller drives its OWN PID lap (the full 100 s) and is seeded with it
     t0 = time.perf_counter()
-    c.enable_rollout(Tcl=TCL)
     if start is None:
         c.rollout_set_state(x0, x0)
         for _ in range(1000):

@@ -297,7 +297,8 @@ int lmpc_step_results(lmpc_handle* h, int* status, int* iters, double* resid, in
 int lmpc_read_buffer(lmpc_handle* h, const char* name, size_t offset_bytes, void* dst, size_t bytes);
 /* Device address of an internal buffer by name: "xPred","uPred","lambd","zt","zt_u","abc","SS_sel","Qfun_sel",
  * "Succ_SS","Succ_uSS","status","iters","resid","flags","xLin","uLin","x0","OldInput","slack","slackT" (lane slacks [B,N*ncx] and
- * terminal slack [B,6] of the most recent step), "abc_lti". */
+ * terminal slack [B,6] of the most recent step), "abc_lti", "x_meas" (the measured state [B,6] of the closed loop's current
+ * step under lmpc_rollout_set_measurement_noise). */
 void* lmpc_device_buffer(lmpc_handle* h, const char* name);
 
 /* ===== device-resident closed loop (the caller of the hot path, SURVEY §8f rank 1) =======================================
@@ -376,6 +377,29 @@ int lmpc_rollout_set_noise(lmpc_handle* h, const lmpc_noise_params* sets, int ns
  * handle starts with.  Host-given draws (z_host, z_pid_host, z_sim_host) do not use the streams.  Checks, refusal and
  * synchronisation as lmpc_rollout_set_noise. */
 int lmpc_rollout_set_noise_streams(lmpc_handle* h, const int* stream_of_instance);
+/* Measurement noise of the device closed loop: the clipped Gaussian sensor noise on the six curvilinear channels every
+ * controller sees (no reference counterpart: the reference's controllers read the simulator's exact state). */
+typedef struct lmpc_measurement_params {
+    double sigma[6];              /* vx, vy, wz, epsi, s, ey */
+    double clip[6];
+} lmpc_measurement_params;
+/* Per-controller measurement noise.  With a table installed, every lmpc_rollout_step (modes 0, 1, 2) and lmpc_rollout_pid_step
+ * first forms, for every controller that is not retired, the measurement
+ *   y_j = x_j + n_j,   n_j = fmax(-clip_j, fmin(z_j * sigma_j, clip_j))   (y_j = x_j exactly where n_j == 0)
+ * of the plant state x, z_j standard normal from Philox4x32-10 keyed by (seed ^ constant, stream, clock) with the stream of
+ * lmpc_rollout_set_noise_streams and a constant of its own (the process and PID draws are unchanged).  Everything the controller
+ * knows comes through y: the QP's x0 (modes 0, 1, 2), the safe-set selection, addPoint's row, the PID's input and the state rows
+ * of the closed-loop record, and through the record the lap hand-over, lmpc_rollout_sysid, the seeding and the pooled exchange.
+ * The plant (the simulator, done, the lap wrap, lmpc_rollout_get_state) and the trace keep the true state; the inputs of the
+ * record are the inputs applied.  y of the current step is the device buffer "x_meas" [B,6] (lmpc_read_buffer).
+ * controller b measures with sets[set_of_instance[b]] (host arrays); nsets == 0 (sets, set_of_instance NULL) removes the table,
+ * which every handle starts without: then no kernel is launched and every consumer reads the plant state, as before.
+ *   - 1 <= nsets <= batch, every index in [0, nsets); every value finite and >= 0 (zero sigma or clip: a noise-free channel).
+ *   - Needs lmpc_rollout_create (LMPC_E_STATE otherwise); any failed check returns LMPC_E_INVALID and leaves the handle as it was.
+ *   - The call synchronises the handle's streams before it replaces the table.  It is allowed at any time: a change in the
+ *     middle of a run applies from the next step on.  The table stays with the handle and is not part of a snapshot record.
+ *   - The host-driven entry points (lmpc_step_*, lmpc_solve_*) take the caller's x0 and are not affected. */
+int lmpc_rollout_set_measurement_noise(lmpc_handle* h, const lmpc_measurement_params* sets, int nsets, const int* set_of_instance);
 /* Lap budgets: controller b is retired once it has handed over budget_of_instance[b] laps (lmpc_rollout_commit_laps_dev counts
  * them: lap_n of lmpc_books_get).  A retired controller keeps the state that hand-over left it in (lap filed, books refreshed,
  * record restarted: the start line of its next lap) and no kernel of lmpc_rollout_step (modes 0, 1, 2) or
@@ -486,7 +510,7 @@ int lmpc_set_pool_min_overrun(lmpc_handle* h, int rows);
  * both lap pools, the lap books, the controller state, the warm-start record, and with a rollout the simulator state, the
  * closed-loop record, the health counters and the LTI model (DESIGN.md, "Controller snapshots", lists every per-controller buffer
  * as carried or scratch).  Not in a record: what the handle is told to drive -- parameter sets, vehicles, tracks, noise sets,
- * noise streams, regression sets, pool groups -- and handle-wide counters.  The lap books travel in the record, so a caller that keeps its own host copy of them (the
+ * noise streams, measurement sets, regression sets, pool groups -- and handle-wide counters.  The lap books travel in the record, so a caller that keeps its own host copy of them (the
  * host-driven bookkeeping of lmpc_ss_set_selection / lmpc_model_set_used) must not restore into its handle.
  * Record = header (below) + sections at 16-byte aligned offsets; every section is one controller's slice of one [B][...] buffer. */
 #define LMPC_SNAPSHOT_MAGIC 0x50414e53      /* "SNAP" */
@@ -548,6 +572,7 @@ int lmpc_sizeof_model_params(void);
 int lmpc_sizeof_vehicle_params(void);
 int lmpc_sizeof_track_params(void);
 int lmpc_sizeof_noise_params(void);
+int lmpc_sizeof_measurement_params(void);
 int lmpc_sizeof_regression_params(void);
 
 #ifdef __cplusplus

@@ -42,6 +42,12 @@ class NoiseParams(C.Structure):
                 ("pid_sigma", C.c_double * 2), ("pid_clip", C.c_double * 2)]
 
 
+class MeasurementParams(C.Structure):
+    """lmpc_measurement_params: the clipped Gaussian sensor noise on (vx, vy, wz, epsi, s, ey) that the controllers of the device
+    closed loop see."""
+    _fields_ = [("sigma", C.c_double * 6), ("clip", C.c_double * 6)]
+
+
 class RegressionParams(C.Structure):
     """lmpc_regression_params: the constants of the local regression model (PredictiveModel.py:18-31)."""
     _fields_ = [("trToUse", C.c_int), ("MaxNumPoint", C.c_int), ("h", C.c_double), ("lamb", C.c_double),
@@ -139,6 +145,7 @@ def lib():
     L.lmpc_rollout_set_vehicles.argtypes = [_vp, C.POINTER(VehicleParams), C.c_int, _vp]
     L.lmpc_rollout_set_noise.argtypes = [_vp, C.POINTER(NoiseParams), C.c_int, _vp]
     L.lmpc_rollout_set_noise_streams.argtypes = [_vp, _vp]
+    L.lmpc_rollout_set_measurement_noise.argtypes = [_vp, C.POINTER(MeasurementParams), C.c_int, _vp]
     L.lmpc_rollout_set_lap_budget.argtypes = [_vp, _vp]
     L.lmpc_set_tracks.argtypes = [_vp, C.POINTER(TrackParams), C.c_int, _vp]
     L.lmpc_set_regression_sets.argtypes = [_vp, C.POINTER(RegressionParams), C.c_int, _vp]
@@ -178,8 +185,10 @@ def lib():
     L.lmpc_sizeof_vehicle_params.restype = C.c_int
     L.lmpc_sizeof_track_params.restype = C.c_int
     L.lmpc_sizeof_noise_params.restype = C.c_int
+    L.lmpc_sizeof_measurement_params.restype = C.c_int
     L.lmpc_sizeof_regression_params.restype = C.c_int
     assert L.lmpc_sizeof_noise_params() == C.sizeof(NoiseParams), "lmpc_noise_params ABI mismatch"
+    assert L.lmpc_sizeof_measurement_params() == C.sizeof(MeasurementParams), "lmpc_measurement_params ABI mismatch"
     assert L.lmpc_sizeof_regression_params() == C.sizeof(RegressionParams), "lmpc_regression_params ABI mismatch"
     assert L.lmpc_sizeof_params() == C.sizeof(Params), "lmpc_params ABI mismatch"
     assert L.lmpc_sizeof_model_params() == C.sizeof(ModelParams), "lmpc_model_params ABI mismatch"
@@ -322,7 +331,7 @@ def make_params(p, numSS_Points=0, numSS_it=0, QterminalSlack=None, eps_res=0.0,
 
 def _set_index(index, K, batch, what):
     """The index rules of the per-controller tables (lmpc_set_param_sets, lmpc_rollout_set_vehicles, lmpc_rollout_set_noise,
-    lmpc_set_tracks, lmpc_set_regression_sets) and of the pool
+    lmpc_rollout_set_measurement_noise, lmpc_set_tracks, lmpc_set_regression_sets) and of the pool
     groups (lmpc_set_pool_groups): 1 <= K <= batch rows and
     one integer row number in [0, K) per controller.  Returns the index as a contiguous int32 array; raises ValueError."""
     if index is None:
@@ -417,6 +426,25 @@ def make_noise_sets(noises, index, batch):
                 setattr(r, f, float(v[0]))
         return r
     return _pack_sets(NoiseParams, noises, index, batch, "noise sets", row)
+
+
+def make_measurement_sets(meas, index, batch):
+    """Per-controller measurement noise for ``lmpc_rollout_set_measurement_noise``: K objects ``meas`` with the fields of
+    MeasurementParams (sigma[6], clip[6] over vx, vy, wz, epsi, s, ey; e.g. reference_params.MeasurementParams) and the
+    measurement set of every controller ``index[batch]``.  Raises ValueError where the library would refuse: the index rules of
+    ``make_param_sets``, a field of the wrong length, or a value that is not finite or is negative.  Returns (ctypes array
+    MeasurementParams * K, int32 index array)."""
+    def row(k, m):
+        r = MeasurementParams()
+        for f, _ in MeasurementParams._fields_:
+            v = np.asarray(getattr(m, f), dtype=float).reshape(-1)
+            if v.shape[0] != 6:
+                raise ValueError("measurement set %d: %s needs 6 values, got %d" % (k, f, v.shape[0]))
+            if not np.all(np.isfinite(v)) or np.any(v < 0):
+                raise ValueError("measurement set %d: %s must be finite and >= 0" % (k, f))
+            getattr(r, f)[:] = v.tolist()
+        return r
+    return _pack_sets(MeasurementParams, meas, index, batch, "measurement sets", row)
 
 
 def _int_per_controller(values, batch, lo, what):

@@ -133,6 +133,18 @@ class BatchedController:
         s = nat.make_noise_streams(streams, self.B)
         nat.check(self._lib.lmpc_rollout_set_noise_streams(self._h, nat.ptr(s)))
 
+    def set_measurement_noise(self, meas=None, index=None):
+        """Per-controller measurement noise of the device closed loop (how much sensor noise learning from one's own laps
+        absorbs): in every later ``rollout_step`` and ``rollout_pid_step`` controller b sees y = x + clip(z * sigma, +-clip) on
+        (vx, vy, wz, epsi, s, ey) with ``meas[index[b]]`` (objects with the fields of reference_params.MeasurementParams) instead
+        of the plant state x: its QP, safe-set selection, addPoint, PID input and closed-loop record all take y, so its stored
+        laps and learned models are measured data.  The plant, ``rollout_state`` and the trace keep x.  The draws are Philox,
+        keyed apart from the process and PID noise and paired by ``set_noise_streams``.  ``index`` is required with ``meas``.
+        ``meas=None`` (no index) removes the table: the controllers read x again and no kernel is added to a step.  Needs
+        ``enable_rollout``; allowed in the middle of a run; not part of a snapshot.  Waits for work already enqueued."""
+        self._install(self._lib.lmpc_rollout_set_measurement_noise, "meas", meas, index,
+                      lambda: nat.make_measurement_sets(meas, index, self.B))
+
     def set_lap_budget(self, budget=None):
         """Lap budgets of the device closed loop: controller b retires once it has handed over ``budget[b]`` laps (one integer
         >= 1 for the whole batch, or one per controller).  A retired controller keeps the state its last hand-over left it in and

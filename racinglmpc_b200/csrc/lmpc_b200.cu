@@ -146,6 +146,10 @@ struct lmpc_handle {
     // creation).  Philox stream of every controller (lmpc_rollout_set_noise_streams), or none for stream b = b.
     HandleTable<lmpc_noise_params> noise;
     HandleTable<int> streams;
+    // measurement noise of the controllers (lmpc_rollout_set_measurement_noise), or none: they read the plant state.  d_xmeas is
+    // the measured state of the current step (measure_kernel).
+    HandleTable<lmpc_measurement_params> meas;
+    double* d_xmeas;
     // lap budgets (lmpc_rollout_set_lap_budget): laps every controller drives before it retires, or none for no budget
     HandleTable<int> budget;
     // device lap books (lapbooks.cuh, allocated with the store): slot tables of both pools, lap history, exchange scratch
@@ -224,6 +228,7 @@ static std::vector<DevBuf> dev_bufs(lmpc_handle* h) {
         dbuf(h->d_cllen, 1, R, FILL_ZERO, SN_CLLEN), dbuf(h->d_done, 1, R, FILL_ZERO, SN_DONE),
         dbuf(h->d_health, 1, R, FILL_ZERO, SN_HEALTH_FLAGS, nullptr, 2),       // [2][B]: flags, then unsolved steps
         dbuf(h->d_abc_lti, 54, R, FILL_ZERO, SN_ABC_LTI, "abc_lti"), dbuf(h->d_z, 3, R), dbuf(h->d_zpid, 2, R),
+        dbuf(h->d_xmeas, 6, R, FILL_ZERO, SN_SCRATCH, "x_meas"),     // formed from the plant state and the clock every step
         // trace of chosen controllers (per traced controller)
         dbuf(h->d_trinst, 1, X), dbuf(h->tr.steps, 1, X, FILL_ZERO), dbuf(h->tr.x, cap * 6, X), dbuf(h->tr.g, cap * 6, X),
         dbuf(h->tr.u, cap * 2, X), dbuf(h->tr.xPred, cap * np, X), dbuf(h->tr.ss, cap * 6 * Mx, X), dbuf(h->tr.lap, cap, X)};
@@ -245,7 +250,7 @@ static void free_tables(lmpc_handle* h, unsigned owners) {
         t.rows.clear(); t.index.clear();
     };
     release(h->sets, OWN_HANDLE); release(h->veh, OWN_HANDLE); release(h->noise, OWN_HANDLE); release(h->streams, OWN_HANDLE);
-    release(h->budget, OWN_HANDLE); release(h->trk, OWN_STORE); release(h->reg, OWN_STORE); release(h->pool_grp, OWN_STORE);
+    release(h->meas, OWN_HANDLE); release(h->budget, OWN_HANDLE); release(h->trk, OWN_STORE); release(h->reg, OWN_STORE); release(h->pool_grp, OWN_STORE);
 }
 
 // Allocate the buffers of `rows` that belong to `owners` (all null on entry) for nb controllers and give them their initial
@@ -898,6 +903,7 @@ int lmpc_sizeof_params(void) { return (int)sizeof(lmpc_params); }
 int lmpc_sizeof_model_params(void) { return (int)sizeof(lmpc_model_params); }
 int lmpc_sizeof_vehicle_params(void) { return (int)sizeof(lmpc_vehicle_params); }
 int lmpc_sizeof_noise_params(void) { return (int)sizeof(lmpc_noise_params); }
+int lmpc_sizeof_measurement_params(void) { return (int)sizeof(lmpc_measurement_params); }
 int lmpc_sizeof_regression_params(void) { return (int)sizeof(lmpc_regression_params); }
 int lmpc_sizeof_track_params(void) { return (int)sizeof(lmpc_track_params); }
 
@@ -1433,34 +1439,52 @@ static SimArgs sim_args(const lmpc_handle* h, const double* z, unsigned long lon
     return sa;
 }
 
+// The state the controllers see this step (DESIGN.md, "Per-controller measurement noise"): with a measurement table, *y is the
+// measured state measure_kernel forms from the plant state and the clock; without one, *y is the plant state and nothing runs.
+static int measure(lmpc_handle* h, unsigned long long seed, LapBudget retire, const double** y) {
+    *y = h->d_rx[h->cur];
+    if (!h->meas.tab) return LMPC_OK;
+    MeasArgs ma;
+    ma.batch = h->batch; ma.x = h->d_rx[h->cur]; ma.y = h->d_xmeas; ma.seed = seed; ma.step = h->sim_step;
+    ma.meas = h->meas.view(); ma.streams = h->streams.idx; ma.retire = retire;
+    measure_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(ma);
+    CK(cudaGetLastError());
+    h->launches += 1;
+    *y = h->d_xmeas;
+    return LMPC_OK;
+}
+
 // One closed-loop step for every instance, all on the device (SysModel.py:34-48):
 //   Controller.solve(x) -> u = uPred[0] -> Controller.addPoint(x, u) (LMPC) -> x+ = dynModel(x, x_glob, u); done = s+ > TrackLength
+// The controller's x (solve, addPoint, the record) is the measured state y when a measurement table is installed.
 int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned long long seed) {
     int rc = need_rollout(h);
     if (rc) return rc;
     const QpIo& q = h->hb[0];
     const double* xc = h->d_rx[h->cur];
     const LapBudget retire = lap_budget(h);
+    const double* y = nullptr;
+    if ((rc = measure(h, seed, retire, &y)) != LMPC_OK) return rc;
     if (z_host) CK(cudaMemcpyAsync(h->d_z, z_host, sizeof(double) * h->batch * 3, cudaMemcpyHostToDevice, h->stream));
     if (mode == 2) {
         CK(cudaMemsetAsync(h->d_flags, 0, sizeof(int) * h->batch, h->stream));
         // LTI MPC with the per-instance model identified by lmpc_rollout_sysid (main.py:72-80); like the reference's LTI
         // controller it never refreshes the input-rate reference (OldInput keeps its initial value, PC.py:113-115)
         QpIo io = {};
-        io.x0 = const_cast<double*>(xc); io.uOld = h->d_OldInput; io.abc = h->d_abc_lti;
+        io.x0 = const_cast<double*>(y); io.uOld = h->d_OldInput; io.abc = h->d_abc_lti;
         io.xPred = q.xPred; io.uPred = q.uPred; io.slack = q.slack; io.status = q.status; io.iters = q.iters; io.resid = q.resid;
         rc = solve_dev(h, io, 54, 0, retire);
     } else {
-        rc = step_dev_impl(h, mode, xc, nullptr, retire);
+        rc = step_dev_impl(h, mode, y, nullptr, retire);
     }
     if (rc) return rc;
     if (mode == 1) {                                                                 // SysModel.py:38 -> PC.py:466-476
-        ss_add_point_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->batch, h->ss, h->d_prevslot, xc, q.uPred,
+        ss_add_point_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->batch, h->ss, h->d_prevslot, y, q.uPred,
                                                                             (long long)h->N * 2, tracks(h), h->d_flags, nullptr, retire);
         CK(cudaGetLastError());
         h->launches += 1;
     }
-    // the trace of the chosen controllers reads the step's results and the state before dynModel
+    // the trace of the chosen controllers reads the step's results and the plant state before dynModel
     if (h->has_trace) {
         trace_step_kernel<<<h->tr.n, 128, 0, h->stream>>>(h->tr, xc, h->d_rg[h->cur], q.uPred, (long long)h->N * 2, q.xPred,
                                                         mode == 1 ? q.SS : nullptr, h->bk.lap_n, retire);
@@ -1469,6 +1493,7 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
     }
     SimArgs sa = sim_args(h, z_host ? h->d_z : nullptr, seed);                       // SysModel.py:40 (dynModel)
     sa.flags = h->d_flags; sa.status = q.status; sa.health = h->d_health; sa.retire = retire;
+    if (h->meas.tab) sa.rec_x = y;
     sim_step_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->mc, sa);
     CK(cudaGetLastError());
     h->launches += 1;
@@ -1482,16 +1507,18 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
 // NULL = Philox on the device.
 int lmpc_rollout_pid_step(lmpc_handle* h, double vt, const double* z_pid_host, const double* z_sim_host, unsigned long long seed) {
     if (int rc = need_rollout(h)) return rc;
-    const double* xc = h->d_rx[h->cur];
+    const double* y = nullptr;                   // the PID's input and the record's state rows (measure)
+    if (int rc = measure(h, seed, LapBudget{}, &y)) return rc;
     if (z_pid_host) CK(cudaMemcpyAsync(h->d_zpid, z_pid_host, sizeof(double) * h->batch * 2, cudaMemcpyHostToDevice, h->stream));
     if (z_sim_host) CK(cudaMemcpyAsync(h->d_z, z_sim_host, sizeof(double) * h->batch * 3, cudaMemcpyHostToDevice, h->stream));
     PidArgs pa;
-    pa.batch = h->batch; pa.x = xc; pa.vt = vt; pa.z = z_pid_host ? h->d_zpid : nullptr; pa.seed = seed; pa.step = h->sim_step;
+    pa.batch = h->batch; pa.x = y; pa.vt = vt; pa.z = z_pid_host ? h->d_zpid : nullptr; pa.seed = seed; pa.step = h->sim_step;
     pa.u = h->hb[0].uPred; pa.u_stride = (long long)h->N * 2;
     pa.noise = h->noise.view(); pa.streams = h->streams.idx;
     pid_input_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(pa);
     SimArgs sa = sim_args(h, z_sim_host ? h->d_z : nullptr, seed);
     sa.health = h->d_health;          // no step flags or QP status here: only the simulator's own bits
+    if (h->meas.tab) sa.rec_x = y;
     sim_step_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->mc, sa);
     CK(cudaGetLastError());
     h->launches += 2;
@@ -1544,6 +1571,24 @@ int lmpc_rollout_set_noise_streams(lmpc_handle* h, const int* stream_of_instance
         if (stream_of_instance[b] < 0)
             return fail(LMPC_E_INVALID, std::string(who) + ": stream of instance " + std::to_string(b) + " is negative");
     return swap_table<int>(h, who, h->streams, nullptr, 0, stream_of_instance);
+}
+
+// Per-controller measurement noise: every value finite and >= 0; nsets == 0 removes the table (the controllers read the plant
+// state, no kernel runs), the precedent of the parameter sets.
+static_assert(sizeof(lmpc_measurement_params) == 12 * sizeof(double), "lmpc_measurement_params is checked as an array of its 12 doubles");
+int lmpc_rollout_set_measurement_noise(lmpc_handle* h, const lmpc_measurement_params* sets, int nsets, const int* set_of_instance) {
+    static const char* who = "lmpc_rollout_set_measurement_noise";
+    if (int rc = need_rollout(h)) return rc;
+    return install_table(h, who, h->meas, sets, nsets, set_of_instance, (const lmpc_measurement_params*)nullptr,
+                         [&](int k, lmpc_measurement_params& row) {
+        const double* v = (const double*)&sets[k];
+        for (size_t j = 0; j < sizeof(lmpc_measurement_params) / sizeof(double); ++j)
+            if (!(isfinite(v[j]) && v[j] >= 0.0))
+                return fail(LMPC_E_INVALID, std::string(who) + ": measurement set " + std::to_string(k) +
+                                                ": every sigma and clip must be finite and >= 0");
+        row = sets[k];
+        return LMPC_OK;
+    });
 }
 
 // Lap budgets: every budget >= 1; NULL removes the budgets.  An array without rows, like the noise streams.

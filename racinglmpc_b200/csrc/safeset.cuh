@@ -853,7 +853,8 @@ __global__ void shift_state_kernel(const ShiftArgs a) {
 // np.random.randn() in this order: vx, vy, wz); when z == nullptr they come from Philox4x32-10 keyed by
 // (seed, stream, step), stream = streams[b] or b when streams is null — statistical, not bit-wise, parity with the reference's
 // unseeded global RNG.
-// Also appends (x, u) to the closed-loop buffer and flags lap completion (SysModel.py:45-47).
+// Also appends (x, u) to the closed-loop buffer -- the measured state in place of x when rec_x is set -- and flags lap
+// completion (SysModel.py:45-47).
 // The ten vehicle constants (SysModel.py:61-70) are read from the instance's row of the vehicle table (a handle without vehicle
 // sets holds a one-row table with the reference vehicle).  The arithmetic is the same with the constants in memory as with them
 // folded in at compile time (DESIGN.md, "Per-controller vehicles").  The noise constants (SysModel.py:139-145) come the same way
@@ -869,6 +870,7 @@ struct SimArgs {
     double* xn;            // [B][6]
     double* xgn;           // [B][6]
     double* cl_x;          // [B][Tcl][6] closed-loop record (may be nullptr)
+    const double* rec_x;   // [B][6] the state rows the record takes: the measured state (measure_kernel), or nullptr: x
     double* cl_u;          // [B][Tcl][2]
     int* cl_len;           // [B]
     int Tcl;
@@ -923,8 +925,9 @@ __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimA
     if (a.cl_x) {
         const int T = a.cl_len[b];
         if (T < a.Tcl) {
+            const double* r = a.rec_x ? a.rec_x + (size_t)b * 6 : x;
 #pragma unroll
-            for (int j = 0; j < 6; ++j) a.cl_x[((size_t)b * a.Tcl + T) * 6 + j] = x[j];
+            for (int j = 0; j < 6; ++j) a.cl_x[((size_t)b * a.Tcl + T) * 6 + j] = r[j];
             a.cl_u[((size_t)b * a.Tcl + T) * 2] = delta;
             a.cl_u[((size_t)b * a.Tcl + T) * 2 + 1] = acc;
             a.cl_len[b] = T + 1;
@@ -1019,6 +1022,42 @@ __global__ void pid_input_kernel(const PidArgs a) {
     a.u[(size_t)b * a.u_stride] = fma(-0.6, x[5], -(0.9 * x[3])) +
                                   fmax(-nz.pid_clip[0], fmin(z0 * nz.pid_sigma[0], nz.pid_clip[0]));
     a.u[(size_t)b * a.u_stride + 1] = 1.5 * (a.vt - x[0]) + fmax(-nz.pid_clip[1], fmin(z1 * nz.pid_sigma[1], nz.pid_clip[1]));
+}
+
+// ------------------------------------------------------------------------------------------------
+// Measurement noise (DESIGN.md, "Per-controller measurement noise"): the state a controller sees, y = x + n on the six
+// curvilinear channels, n_j = clip(z_j * sigma_j, +-clip_j) in the form of the process noise, z_j standard normal from Philox keyed
+// by (seed ^ K_MEAS, stream, clock) -- three curand_normal2_double calls, 12 raw 32-bit draws, in blocks of 16 per step.  Where
+// n_j == 0 the state is copied, so a zero set gives y == x bit for bit (-0.0 + 0.0 would be +0.0).  One thread per controller; a
+// retired controller draws nothing and writes nothing.
+constexpr unsigned long long K_MEAS = 0xD1B54A32D192ED03ull;     // distinct from the PID's key constant
+struct MeasArgs {
+    int batch;
+    const double* x;       // [B][6] plant state
+    double* y;             // [B][6] measured state
+    unsigned long long seed, step;
+    Table<lmpc_measurement_params> meas;   // measurement noise of every instance (lmpc_rollout_set_measurement_noise)
+    const int* streams;                    // [B] Philox stream of every instance, or nullptr: b
+    LapBudget retire;
+};
+__global__ void measure_kernel(const MeasArgs a) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= a.batch || a.retire.retired(b)) return;
+    curandStatePhilox4_32_10_t st;
+    const int stream = a.streams ? a.streams[b] : b;
+    curand_init(a.seed ^ K_MEAS, (unsigned long long)stream, a.step * 16ull, &st);
+    const double2 n01 = curand_normal2_double(&st);
+    const double2 n23 = curand_normal2_double(&st);
+    const double2 n45 = curand_normal2_double(&st);
+    const double z[6] = {n01.x, n01.y, n23.x, n23.y, n45.x, n45.y};
+    const lmpc_measurement_params& m = a.meas.of(b);
+    const double* x = a.x + (size_t)b * 6;
+    double* y = a.y + (size_t)b * 6;
+#pragma unroll
+    for (int j = 0; j < 6; ++j) {
+        const double n = fmax(-m.clip[j], fmin(z[j] * m.sigma[j], m.clip[j]));
+        y[j] = n == 0.0 ? x[j] : x[j] + n;
+    }
 }
 
 // LTI system identification by ridge regression, Utilities.py:5-28 (Regression): rows t = 1 .. T-2 of the closed-loop

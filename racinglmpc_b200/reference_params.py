@@ -90,6 +90,26 @@ class NoiseParams:
 
 
 @dataclass(frozen=True)
+class MeasurementParams:
+    """The sensor noise of the closed loop (no reference counterpart: the reference's controllers read the simulator's exact
+    state): a controller sees y_j = x_j + clip(z_j * sigma_j, +-clip_j) on the six curvilinear channels (vx, vy, wz, epsi, s, ey),
+    z_j standard normal, in the form of the process noise.  The device closed loop takes one per controller
+    (BatchedController.set_measurement_noise)."""
+    sigma: tuple
+    clip: tuple
+
+    @classmethod
+    def zero(cls):
+        """No measurement noise: installed, it gives every controller the plant state bit for bit."""
+        return cls((0.0,) * 6, (0.0,) * 6)
+
+    @classmethod
+    def scaled(cls, k, base):
+        """``base`` with every sigma and clip multiplied by ``k``: 1 gives ``base`` bit for bit, 0 no noise."""
+        return cls(tuple(v * k for v in base.sigma), tuple(v * k for v in base.clip))
+
+
+@dataclass(frozen=True)
 class RegressionParams:
     """The constants of the local regression model (PredictiveModel.py:18-31): the laps used (the trToUse shortest stored laps),
     the neighbour count, the Epanechnikov bandwidth h, the ridge term and the diagonal of the feature scaling of the 1-norm

@@ -2,7 +2,7 @@
 """Small-batch run of every kernel for compute-sanitizer (memcheck / racecheck / synccheck / initcheck):
     compute-sanitizer --tool racecheck python tools/sanitize.py
 Exercises: ftocp_kernel<12,0> and <12,48> (host + device entry points), knn_ltv_regress, ss_select, shift_state,
-ss_add_point, rollout_cost, sim_step (with noise sets and noise streams), knn_ltv_regress with regression sets, commit_laps, ss_export_laps, ss_import_laps; round 2: the long-horizon kernel
+ss_add_point, rollout_cost, sim_step (with noise sets and noise streams), measure (with measurement sets), knn_ltv_regress with regression sets, commit_laps, ss_export_laps, ss_import_laps; round 2: the long-horizon kernel
 that reads its model in place (N = 48), warm-started solves, pid_input, seed_books, commit_laps_books, rollout_stats, the pooled
 exchange (pool_local_best / export / rank / import), trace_step and track_global_position."""
 import os
@@ -34,6 +34,8 @@ c.rollout_set_state(data["x0"], data["x0"])
 # per-controller noise sets and shared noise streams: the simulator reads its row and its stream per controller
 c.set_noise([rp.NoiseParams.reference(), rp.NoiseParams.scaled(10, 0.5)], np.arange(B) % 2)
 c.set_noise_streams(np.arange(B) // 2)
+# per-controller measurement noise: measure_kernel reads its row and its stream, the QP, addPoint and the record read its output
+c.set_measurement_noise([rp.MeasurementParams.zero(), rp.MeasurementParams((0.01,) * 6, (0.05,) * 6)], np.arange(B) % 2)
 # per-controller regression sets: K1 stages its row per warp; fewer laps, other h / MaxNumPoint / lamb / scaling per controller
 r = rp.RegressionParams.reference(5)
 c.set_regression([r, rp.RegressionParams(2, 3, 0.5, 1e-6, (2.0 ** 32, 1.0, 0.0, 1.0, -(2.0 ** -32)))], np.arange(B) % 2)
@@ -67,6 +69,7 @@ c = BatchedController(par, B, workloads.track_seg_table(), rp.TRACK_LENGTH, trTo
 xs = np.tile(np.array([0.5, 0, 0, 0, 0, 0.0]), (B, 1))
 c.enable_rollout(Tcl=1024)
 c.rollout_set_state(xs, xs)
+c.set_measurement_noise([rp.MeasurementParams((0.01,) * 6, (0.05,) * 6)], np.zeros(B, np.int32))   # the PID lap measures too
 for _ in range(int(os.environ.get("SANITIZE_PID_STEPS", "1000"))):
     c.rollout_pid_step(0.8, seed=7)
 c.rollout_seed_from_record_dev(copies=4)
