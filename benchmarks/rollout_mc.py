@@ -41,16 +41,38 @@ from racinglmpc_b200.controller import BatchedController                      # 
 N_HORIZON, TR_TO_USE, TMAX, SS_CAP, MODEL_CAP, TCL = 12, 4, 1280, 7, 5, 1024
 
 
-def layout(warm=False):
+def handle_shape(shape_sets=None):
+    """(N, numSS_Points) of run()'s handle: the reference's (12, 48) without shape_sets, else the smallest pair of the instantiated
+    grid that dominates every shape of shape_sets = (shapes, index), e.g. (14, 96) for any shapes at N <= 14 and (48, 48) for any
+    horizon at 48 points.  Raises ValueError when no pair of the grid dominates them all."""
+    numSS_Points = rp.lmpc_params(N_HORIZON)[1]
+    if shape_sets is None:
+        return N_HORIZON, numSS_Points
+    try:
+        shapes = [(int(n), int(m)) for n, m in shape_sets[0]]
+    except (TypeError, ValueError):
+        raise ValueError("shape_sets is (shapes, index) with (N, numSS_Points) pairs")
+    if not shapes:
+        raise ValueError("shape_sets needs at least one shape")
+    cover = sorted((n, m) for n, m in _native.SHAPE_GRID
+                   if m > 0 and all(n >= sn and m >= sm for sn, sm in shapes))
+    if not cover:
+        raise ValueError("no (N, numSS_Points) pair of the instantiated grid dominates the shapes %s" % sorted(set(shapes)))
+    return cover[0]
+
+
+def layout(warm=False, shape_sets=None):
     """The snapshot layout (BatchedController.snapshot_layout without "bytes") of run()'s controllers."""
-    numSS_it, numSS_Points = rp.lmpc_params(N_HORIZON)[:2]
-    return dict(N=N_HORIZON, M=numSS_Points, ncx=2, ncu=4, numSS_it=numSS_it, trToUse=TR_TO_USE, ss_cap=SS_CAP, model_cap=MODEL_CAP,
+    numSS_it = rp.lmpc_params(N_HORIZON)[0]
+    N, numSS_Points = handle_shape(shape_sets)
+    return dict(N=N, M=numSS_Points, ncx=2, ncu=4, numSS_it=numSS_it, trToUse=TR_TO_USE, ss_cap=SS_CAP, model_cap=MODEL_CAP,
                 Tmax=TMAX, Tcl=TCL, warm_start=int(bool(warm)))
 
 
 def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, poll=8, max_steps=0, seed=1234, local=None, warm=False,
         final=None, param_sets=None, vehicle_sets=None, books=None, track_sets=None, pool_groups=None, readiness="batch",
-        capture=None, start=None, noise_sets=None, noise_streams=None, regression_sets=None, lap_budget=None, measurement_sets=None):
+        capture=None, start=None, noise_sets=None, noise_streams=None, regression_sets=None, lap_budget=None, measurement_sets=None,
+        shape_sets=None):
     """One Monte-Carlo run on this rank's GPU (torch.distributed may or may not be initialised).  Returns a dict (all ranks).
     final: None, or a dict that receives the closed loop's end state (rollout_state) and the last step's solver report (step_results).
     books: None, or a dict that receives the lap books (books) and the health counters (flags_or, unsolved).
@@ -75,6 +97,11 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     bandwidth, neighbour count, ridge, feature scaling and laps used, trToUse up to the store's 4; the result then holds
     per-regression-set lap statistics under "per_regression_rank0").  The pooled mode exchanges laps whatever the model setting:
     a lap driven under another setting is still a trajectory of this car on this circuit.
+    shape_sets: None, or (shapes, index) handed to BatchedController.set_shapes: (N, numSS_Points) pairs of the instantiated grid
+    (a horizon / safe-set size sweep in one batch; the result then holds per-shape lap statistics under "per_shape_rank0").  The
+    handle is created at handle_shape(shape_sets), the smallest grid pair that dominates every shape (ValueError before any device
+    work when there is none, or where set_shapes would refuse a shape).  A shape equal to the handle's (12, 48) runs the shaped
+    QP kernel with the reference's parameters.
     pool_groups: None, or (index, G) handed to BatchedController.set_pool_groups (e.g. sharding.design_groups(track index,
     parameter-set index)): the pooled mode then exchanges laps within each group; the exchange buffers hold G * (share + 1) laps
     per rank and the result holds the laps filed per group under "laps_filed_per_group_rank0" (stored laps counted from the books;
@@ -115,8 +142,13 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     everywhere.  capture records the budget; start refuses a budget below the captured one for any controller (raising it revives
     the controller where it stopped, with the noise draws of the later clock)."""
     budget = _native.make_lap_budget(lap_budget, int(batch))       # ValueError where set_lap_budget would refuse, before any device work
+    N, M = handle_shape(shape_sets)
+    if shape_sets is not None:
+        if warm:
+            raise ValueError("shape_sets and warm start: the warm-start record is laid out per (N, numSS_Points)")
+        _native.make_shape_sets(shape_sets[0], shape_sets[1], int(batch), N, M, rp.lmpc_params(N)[0])
     if start is not None:
-        _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget)
+        _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget, shape_sets)
     if capture is not None and not isinstance(capture, dict):
         raise ValueError("capture is a dict that receives the run's end state")
     if readiness not in ("batch", "group"):
@@ -138,9 +170,9 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     local = int(os.environ.get("LOCAL_RANK", 0)) if local is None else local
     dev = torch.device("cuda", local)
     torch.cuda.set_device(dev)
-    B, N = int(batch), N_HORIZON
-    numSS_it, numSS_Points, _, _, Qts, par = rp.lmpc_params(N)
-    c = BatchedController(par, B, workloads.track_seg_table(), rp.TRACK_LENGTH, trToUse=TR_TO_USE, numSS_Points=numSS_Points,
+    B = int(batch)
+    numSS_it, _, _, _, Qts, par = rp.lmpc_params(N)
+    c = BatchedController(par, B, workloads.track_seg_table(), rp.TRACK_LENGTH, trToUse=TR_TO_USE, numSS_Points=M,
                           numSS_it=numSS_it, QterminalSlack=Qts, device=local, Tmax=TMAX, ss_cap=SS_CAP, model_cap=MODEL_CAP,
                           warm_start=warm)
     c.enable_rollout(Tcl=TCL)                            # before the tables: the measurement noise belongs to the closed loop
@@ -151,7 +183,7 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
               (None if noise_streams is None else (noise_streams,), c.set_noise_streams, None),
               (measurement_sets, c.set_measurement_noise, "per_measurement_rank0"),
               (regression_sets, c.set_regression, "per_regression_rank0"), (track_sets, c.set_tracks, "per_track_rank0"),
-              (pool_groups, c.set_pool_groups, None))
+              (pool_groups, c.set_pool_groups, None), (shape_sets, c.set_shapes, "per_shape_rank0"))
     for args, install, _ in tables:
         if args is not None:
             install(*args)
@@ -197,6 +229,7 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     max_steps = int(max_steps) or 300 * laps
     steps, n_xchg, xchg_s, took_total = sched.start_step, 0, 0.0, 0
     it_sum, it_n, it_max = 0.0, 0, 0                     # interior-point iterations, sampled at the polls
+    it_ctrl = np.zeros(B)                                # ... per controller (the per-shape means)
     l0 = c.kernel_launches
     e0.record(stream)
     while steps < max_steps or sched.repeat:
@@ -211,6 +244,7 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         if not sched.repeat:                              # the repeated poll of a resumed run has no step of its own
             its = c.step_results()["iters"]
             it_sum += float(its.mean()); it_n += 1; it_max = max(it_max, int(its.max()))
+            it_ctrl += its
         ready_g, done = sched.poll(steps, prog, dev)
         if ready_g.any():
             tx = time.perf_counter()
@@ -259,6 +293,12 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         if args is not None and key is not None:
             idx = np.asarray(args[1]).reshape(B)
             out[key] = [_set_stats(bk, flags_or, unsolved, idx == k, laps) for k in range(len(args[0]))]
+    if shape_sets is not None:
+        idx = np.asarray(shape_sets[1]).reshape(B)
+        for k, s in enumerate(out["per_shape_rank0"]):
+            s.update(N=int(shape_sets[0][k][0]), numSS_Points=int(shape_sets[0][k][1]),
+                     ipm_iters_mean_sampled=float(it_ctrl[idx == k].mean() / max(it_n, 1)) if (idx == k).any() else 0.0)
+        out["handle_shape"] = [N, M]
     if pool_groups is not None:
         # a stored lap advances `it`: 4 seeded copies + every own lap handed over + every imported lap filed.  Exact unless an
         # own lap found the safe-set pool full (health flag 64): then that controller's count is one too low per such lap.
@@ -297,7 +337,7 @@ def _driven_steps(bk, state):
     return int(filed.sum(dtype=np.int64) + state["cl_len"].sum(dtype=np.int64))
 
 
-def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget=None):
+def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget=None, shape_sets=None):
     """The refusals of run(start=...), before any device work: a start that does not match this run, laps not above the
     captured laps, or a lap budget below the captured one."""
     if not isinstance(start, dict):
@@ -322,7 +362,7 @@ def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, b
     rec = start["records"]
     if getattr(rec, "shape", (None,))[0] != int(batch):
         raise ValueError("start holds %s records, this run has %d controllers" % (getattr(rec, "shape", ("no",))[0], int(batch)))
-    for k, v in layout(warm).items():
+    for k, v in layout(warm, shape_sets).items():
         if int(start["layout"].get(k, -1)) != v:
             raise ValueError("start records have %s = %s, this run's controllers %d" % (k, start["layout"].get(k), v))
 

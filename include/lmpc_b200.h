@@ -242,6 +242,33 @@ typedef struct lmpc_regression_params {
  *     carry them. */
 int lmpc_set_regression_sets(lmpc_handle* h, const lmpc_regression_params* sets, int nsets, const int* set_of_instance);
 
+/* Per-controller shape: the horizon N and the safe-set size numSS_Points (numSS_Points / numSS_it points per lap). */
+typedef struct lmpc_shape_params {
+    int N, numSS_Points;
+} lmpc_shape_params;
+/* Per-controller horizons and safe-set sizes (the horizon / safe-set trade-off of Rosolia & Borrelli, TCST 2019, in one batch).
+ * Controller b is controlled with the shape sets[set_of_instance[b]] (host arrays): its regression (K1), safe-set selection (K2),
+ * QP and state shift work on N_b stages and M_b safe-set points.  nsets == 0 (sets, set_of_instance NULL) returns every controller
+ * to the handle's own (N, numSS_Points).
+ *   - Requires lmpc_store_create, and no lap stored yet in either pool (as lmpc_set_tracks; else LMPC_E_STATE): xLin, uLin and
+ *     the previous prediction have the length of the horizon they were made for.  Refused on a handle created with warm_start
+ *     (LMPC_E_STATE): the warm-start record is laid out per (N, M).
+ *   - 1 <= nsets <= batch, every index in [0, nsets).  Per set: (N, numSS_Points) is a pair of the instantiated grid; N <= the
+ *     handle's N and numSS_Points <= the handle's; numSS_Points > 0 exactly when the handle's is, a multiple of numSS_it with an
+ *     even number of points per lap.  Any failed check returns LMPC_E_INVALID and leaves the handle as it was.
+ *   - The call synchronises the handle's streams before it replaces the table.  It is independent of every other table; parameter
+ *     sets keep the handle's N and numSS_Points (the weights do not depend on the horizon).
+ *   - Honoured by lmpc_step_host / _dev / _profile, lmpc_identify_host, lmpc_select_host, lmpc_rollout_step (modes 0, 1, 2), the
+ *     seeding calls and the trace.  While shapes are installed the caller-problem entry points (lmpc_solve_*) return LMPC_E_STATE:
+ *     their arrays have no per-controller shape.  Shapes are not part of a snapshot record; records keep the handle's layout.
+ * Layout: every buffer keeps the handle's N and numSS_Points as its per-controller stride, and a controller of shape (N_b, M_b) uses
+ * the leading part of its region: a [N+1,6] / [N,2] block (xPred, uPred, xLin, uLin, the trace's xPred) holds N_b + 1 / N_b rows,
+ * abc holds N_b stages, SS_sel / Succ_SS / Succ_uSS hold a row-major [6,M_b] / [2,M_b] block at the start of the controller's
+ * region, Qfun_sel and lambd hold M_b entries.  A shaped controller never writes the tails.
+ * A shaped handle runs one QP launch per distinct shape present (per distinct N for the MPC-type QPs of modes 0 and 2), each over
+ * the controllers of that shape (DESIGN.md, "Per-controller horizons and safe-set sizes"). */
+int lmpc_set_shapes(lmpc_handle* h, const lmpc_shape_params* sets, int nsets, const int* set_of_instance);
+
 /* PredictiveModel.addTrajectory (PredictiveModel.py:35-46): copy one lap into a regression slot. */
 int lmpc_model_put_lap(lmpc_handle* h, int inst, int slot, int T, const double* x, const double* u);
 /* usedIt order: slots[B,trToUse]. */
@@ -574,6 +601,7 @@ int lmpc_sizeof_track_params(void);
 int lmpc_sizeof_noise_params(void);
 int lmpc_sizeof_measurement_params(void);
 int lmpc_sizeof_regression_params(void);
+int lmpc_sizeof_shape_params(void);
 
 #ifdef __cplusplus
 }

@@ -54,6 +54,17 @@ class RegressionParams(C.Structure):
                 ("scaling", C.c_double * 5)]
 
 
+class ShapeParams(C.Structure):
+    """lmpc_shape_params: the horizon N and the safe-set size numSS_Points of a controller."""
+    _fields_ = [("N", C.c_int), ("numSS_Points", C.c_int)]
+
+
+# The (N, numSS_Points) pairs the library instantiates the QP kernel for: LMPC_FOR_EACH_CASE in csrc/ftocp_launch.cuh (a CPU test
+# keeps the two equal)
+SHAPE_GRID = tuple([(n, 0) for n in (4, 6, 8, 10, 12, 14, 16, 20, 24, 32, 48)] + [(n, 48) for n in (4, 6, 8, 10, 12, 14, 16, 20, 24, 32, 48)] +
+                   [(n, m) for n in (12, 14) for m in (24, 32, 64, 96)])
+
+
 class TrackParams(C.Structure):
     """lmpc_track_params: the [s_start, length, curvature] rows of Map.PointAndTangent and the lap length."""
     _fields_ = [("nseg", C.c_int), ("seg", C.c_double * (MAX_SEG * 3)), ("TrackLength", C.c_double)]
@@ -149,6 +160,7 @@ def lib():
     L.lmpc_rollout_set_lap_budget.argtypes = [_vp, _vp]
     L.lmpc_set_tracks.argtypes = [_vp, C.POINTER(TrackParams), C.c_int, _vp]
     L.lmpc_set_regression_sets.argtypes = [_vp, C.POINTER(RegressionParams), C.c_int, _vp]
+    L.lmpc_set_shapes.argtypes = [_vp, C.POINTER(ShapeParams), C.c_int, _vp]
     L.lmpc_rollout_sysid.argtypes = [_vp, C.c_double, _vp, _vp]
     L.lmpc_rollout_seed_from_record.argtypes = [_vp, C.c_int, C.c_int, C.c_int]
     L.lmpc_rollout_get_lap.argtypes = [_vp, C.c_int, ip, _vp, _vp]
@@ -187,6 +199,8 @@ def lib():
     L.lmpc_sizeof_noise_params.restype = C.c_int
     L.lmpc_sizeof_measurement_params.restype = C.c_int
     L.lmpc_sizeof_regression_params.restype = C.c_int
+    L.lmpc_sizeof_shape_params.restype = C.c_int
+    assert L.lmpc_sizeof_shape_params() == C.sizeof(ShapeParams), "lmpc_shape_params ABI mismatch"
     assert L.lmpc_sizeof_noise_params() == C.sizeof(NoiseParams), "lmpc_noise_params ABI mismatch"
     assert L.lmpc_sizeof_measurement_params() == C.sizeof(MeasurementParams), "lmpc_measurement_params ABI mismatch"
     assert L.lmpc_sizeof_regression_params() == C.sizeof(RegressionParams), "lmpc_regression_params ABI mismatch"
@@ -513,6 +527,34 @@ def make_regression_sets(regs, index, batch, trToUse):
             raise ValueError(w + "every |scaling| must be 0 or in [2^-32, 2^32]")
         return RegressionParams(int(r.trToUse), int(r.MaxNumPoint), h, lamb, tuple(s.tolist()))
     return _pack_sets(RegressionParams, regs, index, batch, "regression sets", row)
+
+
+def make_shape_sets(shapes, index, batch, N, M, numSS_it):
+    """Per-controller shapes for ``lmpc_set_shapes``: K ``(N, numSS_Points)`` pairs ``shapes`` and the shape of every controller
+    ``index[batch]`` on a handle of horizon ``N``, safe-set size ``M`` and ``numSS_it`` laps.  Raises ValueError where the library
+    would refuse: the index rules of ``make_param_sets``, a pair outside SHAPE_GRID, N or numSS_Points above the handle's, a
+    numSS_Points that is 0 on an LMPC handle or > 0 on an MPC handle, or one that is not numSS_it times an even number of points
+    per lap.  Returns (ctypes array ShapeParams * K, int32 index array)."""
+    def row(k, sh):
+        w = "shape %d: " % k
+        try:
+            n, m = sh
+        except (TypeError, ValueError):
+            raise ValueError(w + "need an (N, numSS_Points) pair, got %r" % (sh,))
+        for v in (n, m):
+            if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)):
+                raise ValueError(w + "N and numSS_Points must be integers, got %r" % (sh,))
+        n, m = int(n), int(m)
+        if (n, m) not in SHAPE_GRID:
+            raise ValueError(w + "(%d, %d) is not an instantiated (N, numSS_Points) pair" % (n, m))
+        if n > int(N) or m > int(M):
+            raise ValueError(w + "(%d, %d) exceeds the handle's (%d, %d)" % (n, m, N, M))
+        if (m > 0) != (int(M) > 0):
+            raise ValueError(w + "numSS_Points must be > 0 exactly when the handle's is (%d)" % M)
+        if m > 0 and (m % int(numSS_it) or (m // int(numSS_it)) % 2):
+            raise ValueError(w + "numSS_Points must be numSS_it (%d) times an even number of points per lap" % numSS_it)
+        return ShapeParams(n, m)
+    return _pack_sets(ShapeParams, shapes, index, batch, "shapes", row)
 
 
 def make_pool_groups(index, ngroups, batch):

@@ -66,6 +66,7 @@ class BatchedController:
         nit = max(self.numSS_it, 1)
         self.device_books = False
         self._pool_groups = 1
+        self._shapes = None                                 # (shapes, index) of set_shapes, or None: the handle's own shape
         self._sel = np.zeros((self.B, nit), np.int32); self._isp = np.zeros((self.B, nit), np.int32)
         self._prev = -np.ones(self.B, np.int32); self._used = np.zeros((self.B, self.trToUse), np.int32)
 
@@ -165,6 +166,24 @@ class BatchedController:
         enqueued."""
         self._install(self._lib.lmpc_set_regression_sets, "regs", regs, index,
                       lambda: nat.make_regression_sets(regs, index, self.B, self.trToUse))
+
+    def set_shapes(self, shapes, index=None):
+        """Per-controller horizons and safe-set sizes (the horizon / safe-set trade-off in one batch): controller b plans over
+        ``shapes[index[b]] = (N_b, numSS_Points_b)`` in every later ``identify``, ``select``, ``step`` and ``rollout_step``, with
+        numSS_Points_b / numSS_it points per lap.  Every pair is one of nat.SHAPE_GRID, at most the controller's own (N,
+        numSS_Points) and on the same side of 0.  ``index`` is required with ``shapes``.  ``shapes=None`` (no index) returns every
+        controller to the handle's shape.  Only before the first lap is stored and not with warm start; independent of the other
+        tables.  While shapes are installed the ``solve*`` entry points on caller arrays are refused.  Device buffers keep the
+        handle's (N, numSS_Points) as their stride: ``read_buffer`` and the trace cut a controller's rows to its shape.  Waits for
+        work already enqueued."""
+        self._install(self._lib.lmpc_set_shapes, "shapes", shapes, index,
+                      lambda: nat.make_shape_sets(shapes, index, self.B, self.N, self.M, self.numSS_it))
+        self._shapes = None if shapes is None else ([tuple(int(v) for v in s) for s in shapes], np.asarray(index).reshape(-1).copy())
+
+    def shape_of(self, inst):
+        """(N, numSS_Points) controller ``inst`` plans with: its row of ``set_shapes``, or the handle's."""
+        sh = self._shapes
+        return (self.N, self.M) if sh is None else sh[0][int(sh[1][int(inst)])]
 
     def set_tracks(self, tracks, index=None):
         """Per-controller tracks (several circuits in one batch): controller b drives ``tracks[index[b]]`` (objects with
@@ -397,10 +416,25 @@ class BatchedController:
         return [float(v) for v in ms]
 
     def read_buffer(self, name, inst, shape, dtype=np.float64):
-        """Inspection: the slice of instance `inst` of a per-instance device buffer ("abc", "SS_sel", "Qfun_sel", ...)."""
+        """Inspection: the slice of instance `inst` of a per-instance device buffer ("abc", "SS_sel", "Qfun_sel", ...), ``shape``
+        being the handle's per-controller shape of it.  A shaped controller (``set_shapes``) gets its valid part: xPred cut to
+        N_b + 1 rows and SS_sel / Succ_SS / Succ_uSS / Qfun_sel / lambd to M_b columns."""
         out = np.zeros(shape, dtype)
         nat.check(self._lib.lmpc_read_buffer(self._h, name.encode(), int(inst) * out.nbytes, nat.ptr(out), out.nbytes))
-        return out
+        return self._cut_to_shape(name, inst, out)
+
+    def _cut_to_shape(self, name, inst, a):
+        """The valid part of one controller's slice ``a`` of buffer ``name`` (the handle's shape) under its own shape."""
+        Nb, Mb = self.shape_of(inst)
+        if (Nb, Mb) == (self.N, self.M):
+            return a
+        if name == "xPred" and a.shape[0] == self.N + 1:
+            return a[:Nb + 1].copy()
+        if name in ("SS_sel", "Succ_SS", "Succ_uSS") and a.ndim == 2 and a.shape[1] == self.M:
+            return a.reshape(-1)[:a.shape[0] * Mb].reshape(a.shape[0], Mb).copy()
+        if name in ("Qfun_sel", "lambd") and a.shape[0] == self.M:
+            return a[:Mb].copy()
+        return a
 
     def step_results(self):
         """status, iters, resid[B,3], flags of the most recent step_dev / rollout_step."""

@@ -2,6 +2,7 @@
 // resident-warp bounds and the instantiated (horizon, safe-set size) grid.  One kernel template, two variants:
 //   ftocp_kernel<..., false> (lmpc_b200.cu) : parameters of the whole launch in the constant bank (handles without parameter sets)
 //   ftocp_kernel<..., true>  (ftocp_sets.cu) : each instance's parameters from a table (lmpc_set_param_sets)
+// and, for handles with per-controller shapes, ftocp_shaped_kernel (ftocp_shapes.cu), a kernel of its own for the same reason.
 // Each translation unit instantiates only its own variant, and the body is the kernel itself, not a function inlined into two
 // wrappers.  Both matter for the uniform kernels' code: with both variants instantiated in one unit, or with the body inlined into
 // two __global__ wrappers, the compiler scheduled all 30 uniform instantiations differently (profiles/h100_param_sets.txt).
@@ -233,3 +234,15 @@ __global__ void __launch_bounds__(32, ftocp_min_blocks(N, M, SETS ? (int)sizeof(
 // with a.sets = table; both return a CUDA error code (cudaErrorInvalidValue for a pair outside the grid)
 cudaError_t ftocp_sets_configure(int N, int M);
 cudaError_t ftocp_sets_launch(int N, int M, const FtocpConstRec* table, FtocpArgs a, cudaStream_t st);
+
+// ftocp_shapes.cu: the QP kernel of handles with per-controller shapes (lmpc_set_shapes), ftocp_shaped_kernel<N_b, M_b, 2, 4>.  One
+// launch covers the controllers inst[0 .. n) of one shape; each reads its parameters from the table a.sets (row a.set_idx[b], or
+// row 0 when a.set_idx is null) and addresses every buffer with the handle's strides N, M (M = 0: no safe set).
+struct ShapedLaunch {
+    const int* inst;
+    int N, M;
+};
+// opt the shaped instantiations (N, M) and (N, 0) into their shared-memory size on the current device; launch n controllers of
+// shape (N, M) with a.sets = table.  Both return a CUDA error code (cudaErrorInvalidValue for a pair outside the grid).
+cudaError_t ftocp_shaped_configure(int N, int M);
+cudaError_t ftocp_shaped_launch(int N, int M, const FtocpConstRec* table, ShapedLaunch s, int n, FtocpArgs a, cudaStream_t st);

@@ -180,7 +180,7 @@ __global__ void __launch_bounds__(256) commit_laps_books_kernel(int batch, LapPo
 __global__ void __launch_bounds__(256) seed_books_kernel(int batch, LapPool ss, LapPool model, LapBooks k, int copies, const double* cl_x,
                                                          const double* cl_u, int* cl_len, int Tcl, int N, double* xLin, double* uLin,
                                                          double* zt, double* OldInput, int* timeStep, int* hasPred, int* done,
-                                                         Tracks trk, int lmpc) {
+                                                         Tracks trk, int lmpc, Shapes shp) {
     const int b = blockIdx.x;
     if (b >= batch) return;
     __shared__ int s_ss, s_md;
@@ -204,7 +204,7 @@ __global__ void __launch_bounds__(256) seed_books_kernel(int batch, LapPool ss, 
         if (s_md >= 0) copy_lap_block(model, model.lap_index(b, s_md), cx, cu, Trec);
         __syncthreads();
     }
-    seed_state_block(b, N, cx, cu, xLin, uLin, zt, OldInput);
+    seed_state_block(b, N, shp, cx, cu, xLin, uLin, zt, OldInput);
     if (threadIdx.x == 0) { book_refresh(k, b); timeStep[b] = 0; hasPred[b] = 0; cl_len[b] = 0; done[b] = 0; }
 }
 

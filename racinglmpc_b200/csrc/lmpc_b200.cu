@@ -24,6 +24,8 @@
 #include <map>
 #include <vector>
 #include <mutex>
+#include <algorithm>
+#include <utility>
 
 #include "../../include/lmpc_b200.h"
 #include "ftocp_pdip.cuh"
@@ -131,6 +133,13 @@ struct lmpc_handle {
     // regression constants (lmpc_set_regression_sets); without sets the constants of lmpc_store_create (store_reg)
     RegressionRec store_reg;
     HandleTable<RegressionRec> reg;
+    // per-controller shapes (lmpc_set_shapes), or none; shp_order's index is the batch sorted by (N, M), shp_cells the runs of
+    // one shape in it (only shapes with controllers), own_c the one-row parameter table of a shaped handle without parameter sets
+    HandleTable<ShapeRec> shp;
+    HandleTable<int> shp_order;
+    struct ShapeCell { int N, M, off, n; };
+    std::vector<ShapeCell> shp_cells;
+    HandleTable<FtocpConstRec> own_c;
     LapPool ss, mdl;
     int *d_used, *d_sel, *d_isprev, *d_prevslot, *d_timeStep, *d_hasPred, *d_flags, *d_minidx, *d_xchg, *d_health, *d_dropped;
     double *d_xLin, *d_uLin, *d_ztState, *d_ztFixed, *d_OldInput, *d_xPredPrev, *d_tmpx, *d_tmpu;
@@ -251,6 +260,8 @@ static void free_tables(lmpc_handle* h, unsigned owners) {
     };
     release(h->sets, OWN_HANDLE); release(h->veh, OWN_HANDLE); release(h->noise, OWN_HANDLE); release(h->streams, OWN_HANDLE);
     release(h->meas, OWN_HANDLE); release(h->budget, OWN_HANDLE); release(h->trk, OWN_STORE); release(h->reg, OWN_STORE); release(h->pool_grp, OWN_STORE);
+    release(h->shp, OWN_STORE); release(h->shp_order, OWN_STORE); release(h->own_c, OWN_HANDLE);
+    if (owners & OWN_STORE) h->shp_cells.clear();
 }
 
 // Allocate the buffers of `rows` that belong to `owners` (all null on entry) for nb controllers and give them their initial
@@ -433,7 +444,23 @@ static int launch_t(lmpc_handle* h, const FtocpArgs& a, cudaStream_t st) {
     return LMPC_OK;
 }
 
+// A shaped handle (lmpc_set_shapes): one launch of ftocp_shaped_kernel per run of one shape in the sorted batch, or per run of one
+// horizon for the MPC-type QP; parameters from the parameter-set table, or the handle's own row
+static int launch_shaped(lmpc_handle* h, const FtocpArgs& a, bool lmpc_mode, cudaStream_t st) {
+    const FtocpConstRec* table = h->sets.tab ? h->sets.tab : h->own_c.tab;
+    const auto& cells = h->shp_cells;
+    for (size_t k = 0, j; k < cells.size(); k = j) {
+        int n = 0;
+        for (j = k; j < cells.size() && cells[j].N == cells[k].N && (!lmpc_mode || cells[j].M == cells[k].M); ++j) n += cells[j].n;
+        const ShapedLaunch s{h->shp_order.idx + cells[k].off, h->N, h->M};
+        CK(ftocp_shaped_launch(cells[k].N, lmpc_mode ? cells[k].M : 0, table, s, n, a, st));
+        h->launches += 1;
+    }
+    return LMPC_OK;
+}
+
 static int launch(lmpc_handle* h, const FtocpArgs& a, bool lmpc_mode, cudaStream_t st) {
+    if (h->shp.tab) return launch_shaped(h, a, lmpc_mode, st);
     const int N = h->N, M = lmpc_mode ? h->M : 0;
 #define LCASE(n, m) if (N == n && M == m) return launch_t<n, m>(h, a, st);
     LMPC_FOR_EACH_CASE(LCASE)
@@ -528,6 +555,9 @@ static int create_device_side(lmpc_handle* h) {
     for (int i = 0; i < 4 * LMPC_HOST_SLOTS; ++i) CK(cudaStreamCreateWithFlags(&h->cstream[i], cudaStreamNonBlocking));
     if (!qp_bufs(h, 0)) return LMPC_E_CUDA;
     if ((rc = alloc_bufs(h, dev_bufs(h), OWN_HANDLE, 1, "lmpc_create")) != LMPC_OK) return rc;
+    FtocpConstRec own;
+    own.c = h->c;
+    if ((rc = swap_table(h, "lmpc_create", h->own_c, &own, 1, nullptr)) != LMPC_OK) return rc;
     const lmpc_vehicle_params ref = reference_vehicle();
     if ((rc = swap_table(h, "lmpc_create", h->veh, &ref, 1, nullptr)) != LMPC_OK) return rc;
     const lmpc_noise_params noise = reference_noise();
@@ -756,6 +786,7 @@ int lmpc_solve_lmpc_dev(lmpc_handle* h, const double* x0, const double* uOld, co
                         long long abc_stage_stride, const double* SS_sel, const double* Qfun_sel, const double* Succ_SS,
                         const double* Succ_uSS, double* xPred, double* uPred, double* slack, double* lambd,
                         double* slackTerminal, double* zt, double* zt_u, int* status, int* iters, double* resid) {
+    if (h && h->shp.tab) return fail(LMPC_E_STATE, "lmpc_solve_*: per-controller shapes are installed; the caller's arrays have no per-controller shape");
     return solve_dev(h, CALLER_QP_IO, abc_inst_stride, abc_stage_stride, LapBudget{});
 }
 
@@ -776,6 +807,7 @@ static int enqueue_host_solve_impl(lmpc_handle* h, int slot, const QpIo& io, lon
     const bool lm = (io.SS != nullptr);
     if (lm && (h->M <= 0 || !io.Qfun)) return fail(LMPC_E_INVALID, "handle was created without a safe set (numSS_Points == 0)");
     if (slot < 0 || slot >= LMPC_HOST_SLOTS) return fail(LMPC_E_INVALID, "slot must be 0 .. 3");
+    if (h->shp.tab) return fail(LMPC_E_STATE, "lmpc_solve_*: per-controller shapes are installed; the caller's arrays have no per-controller shape");
     CK(cudaSetDevice(h->device));
     const size_t B = h->batch, N = h->N, M = h->M > 0 ? h->M : 1;
     const size_t D = sizeof(double);
@@ -905,6 +937,7 @@ int lmpc_sizeof_vehicle_params(void) { return (int)sizeof(lmpc_vehicle_params); 
 int lmpc_sizeof_noise_params(void) { return (int)sizeof(lmpc_noise_params); }
 int lmpc_sizeof_measurement_params(void) { return (int)sizeof(lmpc_measurement_params); }
 int lmpc_sizeof_regression_params(void) { return (int)sizeof(lmpc_regression_params); }
+int lmpc_sizeof_shape_params(void) { return (int)sizeof(lmpc_shape_params); }
 int lmpc_sizeof_track_params(void) { return (int)sizeof(lmpc_track_params); }
 
 static int store_create_impl(lmpc_handle* h, const lmpc_model_params* mp, int ss_cap, int model_cap, int Tmax);
@@ -928,9 +961,10 @@ static int store_create_impl(lmpc_handle* h, const lmpc_model_params* mp, int ss
     }
     CK(cudaSetDevice(h->device));
     // the largest launch: trToUse = K1_MAXLAPS at K1_MAXWPB warps (103360 B, above a flat 100 KiB)
-    CK(cudaFuncSetAttribute(knn_ltv_regress_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                            (int)k1_smem_bytes(K1_MAXLAPS, K1_MAXWPB)));
-    CK(cudaFuncSetAttribute(knn_ltv_regress_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    for (auto k1 : {knn_ltv_regress_kernel<false>, knn_ltv_regress_kernel<true>}) {
+        CK(cudaFuncSetAttribute(k1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem_bytes(K1_MAXLAPS, K1_MAXWPB)));
+        CK(cudaFuncSetAttribute(k1, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    }
     ModelConst& m = h->mc;
     memset(&m, 0, sizeof(m));
     m.trToUse = mp->trToUse; m.dt = mp->dt;
@@ -1077,6 +1111,59 @@ int lmpc_set_regression_sets(lmpc_handle* h, const lmpc_regression_params* sets,
     });
 }
 
+static bool on_grid(int N, int M) {
+#define GCASE(n, m) if (N == n && M == m) return true;
+    LMPC_FOR_EACH_CASE(GCASE)
+#undef GCASE
+    return false;
+}
+
+// Per-controller shapes: every set checked against the grid and the handle, the shaped kernels of every set opted into their
+// shared-memory size, then the table and the sorted instance list (DESIGN.md, "Per-controller horizons and safe-set sizes");
+// nsets == 0 returns to the handle's own shape.
+int lmpc_set_shapes(lmpc_handle* h, const lmpc_shape_params* sets, int nsets, const int* set_of_instance) {
+    static const char* who = "lmpc_set_shapes";
+    int rc = need_store(h);
+    if (rc) return rc;
+    if (h->laps_stored) return fail(LMPC_E_STATE, std::string(who) + ": laps are stored already; install shapes before the first lap");
+    if (h->p.warm_start) return fail(LMPC_E_STATE, std::string(who) + ": the handle was created with warm_start; its records are laid out per (N, M)");
+    const int nit = h->p.numSS_it;
+    rc = install_table(h, who, h->shp, sets, nsets, set_of_instance, (const ShapeRec*)nullptr, [&](int k, ShapeRec& row) {
+        const lmpc_shape_params& s = sets[k];
+        const std::string w = std::string(who) + ": set " + std::to_string(k) + ": ";
+        if (!on_grid(s.N, s.numSS_Points)) return fail(LMPC_E_INVALID, w + "(N, numSS_Points) is not instantiated: built for " LMPC_GRID_TEXT);
+        if (s.N > h->N || s.numSS_Points > h->M)
+            return fail(LMPC_E_INVALID, w + "N and numSS_Points must not exceed the handle's (" + std::to_string(h->N) + ", " +
+                                            std::to_string(h->M) + ")");
+        if ((s.numSS_Points > 0) != (h->M > 0)) return fail(LMPC_E_INVALID, w + "numSS_Points must be > 0 exactly when the handle's is");
+        if (s.numSS_Points > 0 && (s.numSS_Points % nit || (s.numSS_Points / nit) % 2))
+            return fail(LMPC_E_INVALID, w + "numSS_Points must be a multiple of numSS_it with an even number of points per lap");
+        const cudaError_t e = ftocp_shaped_configure(s.N, s.numSS_Points);
+        if (e != cudaSuccess) return fail(LMPC_E_CUDA, w + cudaGetErrorString(e));
+        row = s;
+        return LMPC_OK;
+    });
+    if (rc != LMPC_OK) return rc;
+    // the batch sorted by (N, M) and the runs of one shape in it
+    std::vector<int> order(nsets ? h->batch : 0);
+    for (size_t b = 0; b < order.size(); ++b) order[b] = (int)b;
+    auto key = [&](int b) { const ShapeRec& r = h->shp.rows[h->shp.index[b]]; return std::make_pair(r.N, r.numSS_Points); };
+    std::stable_sort(order.begin(), order.end(), [&](int x, int y) { return key(x) < key(y); });
+    h->shp_cells.clear();
+    for (size_t i = 0; i < order.size(); ++i) {
+        const auto k = key(order[i]);
+        if (i == 0 || k != key(order[i - 1])) h->shp_cells.push_back({k.first, k.second, (int)i, 0});
+        h->shp_cells.back().n += 1;
+    }
+    if ((rc = swap_table<int>(h, who, h->shp_order, nullptr, 0, nsets ? order.data() : nullptr)) != LMPC_OK) {
+        const std::string msg = g_err;      // no shapes rather than shapes without their instance list
+        swap_table<ShapeRec>(h, who, h->shp, nullptr, 0, nullptr);
+        h->shp_cells.clear();
+        g_err = msg;
+    }
+    return rc;
+}
+
 static int put_lap(lmpc_handle* h, LapPool& pool, int inst, int slot, int T, const double* x, const double* u) {
     if (inst < 0 || inst >= h->batch || slot < 0 || slot >= pool.cap || T < 2 || T > pool.Tmax || !x || !u)
         return fail(LMPC_E_INVALID, "put_lap: bad instance/slot/length");
@@ -1211,9 +1298,10 @@ static int launch_k1(lmpc_handle* h, LapBudget retire = {}) {
     a.trk = tracks(h);
     a.reg = h->reg.view();
     a.retire = retire;
+    a.shp = h->shp.view();
     dim3 grid(h->batch, (h->N + a.wpb - 1) / a.wpb);
     const size_t smem = k1_smem_bytes(h->mc.trToUse, a.wpb);
-    knn_ltv_regress_kernel<<<grid, 32 * a.wpb, smem, h->stream>>>(h->mc, a);
+    (h->shp.tab ? knn_ltv_regress_kernel<true> : knn_ltv_regress_kernel<false>)<<<grid, 32 * a.wpb, smem, h->stream>>>(h->mc, a);
     CK(cudaGetLastError());
     h->launches += 1;
     return LMPC_OK;
@@ -1228,7 +1316,8 @@ static int launch_k2(lmpc_handle* h, const double* d_x0, LapBudget retire = {}) 
     a.SS_sel = h->hb[0].SS; a.Qfun_sel = h->hb[0].Qfun; a.Succ_SS = h->hb[0].SuccSS; a.Succ_uSS = h->hb[0].SuccU;
     a.zt_fixed = h->d_ztFixed; a.status = h->d_flags; a.min_index = h->d_minidx;
     a.retire = retire;
-    ss_select_kernel<<<h->batch, 32 * a.numSS_it, 0, h->stream>>>(a);
+    a.shp = h->shp.view();
+    (h->shp.tab ? ss_select_kernel<true> : ss_select_kernel<false>)<<<h->batch, 32 * a.numSS_it, 0, h->stream>>>(a);
     CK(cudaGetLastError());
     h->launches += 1;
     return LMPC_OK;
@@ -1302,7 +1391,8 @@ static int step_dev_impl(lmpc_handle* h, int mode, const double* x0_dev, cudaEve
     sa.xLin = h->d_xLin; sa.uLin = h->d_uLin; sa.zt = h->d_ztState; sa.OldInput = h->d_OldInput; sa.xPredPrev = h->d_xPredPrev;
     sa.timeStep = h->d_timeStep; sa.has_pred = h->d_hasPred;
     sa.retire = retire;
-    shift_state_kernel<<<h->batch, 64, 0, st>>>(sa);                                 // PC.py:129-137
+    sa.shp = h->shp.view();
+    (h->shp.tab ? shift_state_kernel<true> : shift_state_kernel<false>)<<<h->batch, 64, 0, st>>>(sa);   // PC.py:129-137
     CK(cudaGetLastError());
     h->launches += 1;
     if (ev) CK(cudaEventRecord(ev[4], st));
@@ -1625,7 +1715,7 @@ int lmpc_rollout_seed_from_record(lmpc_handle* h, int copies, int ss_slot0, int 
     if (h->d_warm_valid) CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * h->batch, h->stream));
     seed_from_record_kernel<<<h->batch, 256, 0, h->stream>>>(h->batch, h->ss, h->mdl, copies, ss_slot0, model_slot0, h->d_clx, h->d_clu,
                                                              h->d_cllen, h->Tcl, h->N, h->d_xLin, h->d_uLin, h->d_ztState, h->d_OldInput,
-                                                             h->d_timeStep, h->d_hasPred, h->d_done, tracks(h));
+                                                             h->d_timeStep, h->d_hasPred, h->d_done, tracks(h), h->shp.view());
     CK(cudaGetLastError());
     h->launches += 1;
     return LMPC_OK;
@@ -1804,7 +1894,7 @@ int lmpc_rollout_seed_from_record_dev(lmpc_handle* h, int copies) {
     if (h->d_warm_valid) CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * h->batch, h->stream));
     seed_books_kernel<<<h->batch, 256, 0, h->stream>>>(h->batch, h->ss, h->mdl, h->bk, copies, h->d_clx, h->d_clu, h->d_cllen, h->Tcl, h->N,
                                                        h->d_xLin, h->d_uLin, h->d_ztState, h->d_OldInput, h->d_timeStep, h->d_hasPred,
-                                                       h->d_done, tracks(h), h->M > 0 ? 1 : 0);
+                                                       h->d_done, tracks(h), h->M > 0 ? 1 : 0, h->shp.view());
     CK(cudaGetLastError());
     h->launches += 1;
     return LMPC_OK;

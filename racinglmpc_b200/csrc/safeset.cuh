@@ -42,6 +42,14 @@ using Regressions = Table<RegressionRec>;
 using TrackRec = lmpc_track_params;
 using Tracks = Table<TrackRec>;
 
+// The shape of every controller (lmpc_set_shapes): horizon N_b and safe-set size M_b, or no table (tab == null) for the handle's
+// own (N, numSS_Points).  Buffers keep the handle's N and M as their per-controller strides; a controller uses the leading part.
+using ShapeRec = lmpc_shape_params;
+using Shapes = Table<ShapeRec>;
+// K1, K2 and the state shift come in two instantiations, SHAPED = a table is installed: without one the kernels are the code they
+// were before shapes existed (a branch on a null table cost the closed loop of configs[3] about 1 %)
+__device__ __forceinline__ int horizon_of(const Shapes& s, int b, int N) { return s.tab ? s.of(b).N : N; }
+
 struct LapPool {
     double* x;      // [B][cap][Tmax][6]
     double* u;      // [B][cap][Tmax][2]
@@ -152,6 +160,7 @@ struct K1Args {
     int* status;          // [B] : 0 ok, else bit flags (1 = singular regression, 2 = curvature lookup failed,
                           //        4 = a single neighbour in a lap — cases where the reference raises,
                           //        32 = more than K1_CAND rows within rounding distance of the k-th neighbour)
+    Shapes shp;           // the horizon of every controller: stages i >= N_b are not identified
 };
 // per-warp scratch: selected points [7*trToUse][15] (x0 x1 x2 delta a 1 | y0 y1 y2 | K*(x0 x1 x2 delta a 1)) | normal
 //                   equations 45 (+3 pad) | staging of the closed-form record entries (17, +3 pad)
@@ -203,15 +212,19 @@ __constant__ signed char K1_ABC_SRC[54] = {
 #ifndef LMPC_K1_MINBLOCKS
 #define LMPC_K1_MINBLOCKS 3
 #endif
+template <bool SHAPED>
 __global__ void __launch_bounds__(32 * K1_MAXWPB, LMPC_K1_MINBLOCKS) knn_ltv_regress_kernel(const __grid_constant__ ModelConst m, const K1Args a) {
     extern __shared__ __align__(16) unsigned char k1_smem[];
     const int b = a.b0 + blockIdx.x;
     if (a.retire.retired(b)) return;          // uniform over the CTA: no barrier is skipped by part of it
+    // every stage of this CTA lies past the controller's horizon (uniform over the CTA).  The shape is read where it is tested, not
+    // held as a horizon: as one int across the scan it cost K1 a 12-byte spill at its 56-register cap
+    if (SHAPED && (int)blockIdx.y * a.wpb >= a.shp.of(b).N) return;
     const int wib = threadIdx.x >> 5;
     const int i = blockIdx.y * a.wpb + wib;   // horizon step
     const int lane = threadIdx.x & 31;
     const int nthr = blockDim.x;
-    const bool active = (i < a.N);            // all warps take part in the tile loads
+    const bool active = SHAPED ? i < a.shp.of(b).N : i < a.N;             // all warps take part in the tile loads
     float4* tile4 = reinterpret_cast<float4*>(k1_smem);                // [K1_TILE] : (vx, vy, wz, delta) of a row, one 16-byte load
     float* tile1 = reinterpret_cast<float*>(k1_smem) + 4 * K1_TILE;    // [K1_TILE] : a
     double* wbase = reinterpret_cast<double*>(k1_smem + sizeof(float) * 5 * K1_TILE) + (size_t)wib * a.pts_stride;
@@ -510,7 +523,7 @@ __global__ void __launch_bounds__(32 * K1_MAXWPB, LMPC_K1_MINBLOCKS) knn_ltv_reg
 
 // ------------------------------------------------------------------------------------------------
 struct K2Args {
-    int batch, N, numSS_it, P;   // P = numSS_Points / numSS_it
+    int batch, N, numSS_it, P;   // P = numSS_Points / numSS_it (the handle's; a shaped controller has P_b = M_b / numSS_it)
     Tracks trk;
     const double* x0;        // [B][6]
     const double* zt;        // [B][6]
@@ -528,15 +541,18 @@ struct K2Args {
     int* status;             // [B] bit 8 = selection window ran past the stored lap (reference: IndexError)
     int* min_index;          // [B][numSS_it] argmin row (for tests)
     LapBudget retire;        // the CTA of a retired controller selects nothing
+    Shapes shp;              // N_b and M_b of every controller: the [6,M_b] block at the start of the controller's [6,M] region
 };
 
 // One CTA per instance, one warp per selected lap.
+template <bool SHAPED>
 __global__ void __launch_bounds__(32 * 8) ss_select_kernel(const K2Args a) {
     const int b = blockIdx.x;
     const int c = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     if (b >= a.batch || c >= a.numSS_it || a.retire.retired(b)) return;
-    const int M = a.P * a.numSS_it;
+    const int Mh = a.P * a.numSS_it;                         // the handle's M: the per-controller stride of the outputs
+    const int M = SHAPED ? a.shp.of(b).numSS_Points : Mh, P = SHAPED ? M / a.numSS_it : a.P, Nb = SHAPED ? a.shp.of(b).N : a.N;
     const double TrackLength = a.trk.of(b).TrackLength;
     // lap-wrap fix of the terminal guess (PC.py:392-393)
     double z[6];
@@ -572,7 +588,7 @@ __global__ void __launch_bounds__(32 * 8) ss_select_kernel(const K2Args a) {
     }
     const int mn = bi;
     // window (PC.py:492-495), numPoints = P + 1
-    const int npt = a.P + 1;
+    const int npt = P + 1;
     const int half = npt / 2;
     int start, count;
     if ((double)mn - (double)npt / 2.0 >= 0.0) { start = mn - half; count = 2 * half + 1; }
@@ -586,27 +602,27 @@ __global__ void __launch_bounds__(32 * 8) ss_select_kernel(const K2Args a) {
     double adj = 0.0;
     if (a.has_pred[b]) {
         int over = 0;
-        for (int k = 0; k <= a.N; ++k) over += (a.xPred[((size_t)b * (a.N + 1) + k) * 6 + 4] > TrackLength) ? 1 : 0;
+        for (int k = 0; k <= Nb; ++k) over += (a.xPred[((size_t)b * (a.N + 1) + k) * 6 + 4] > TrackLength) ? 1 : 0;
         if (over > 0) {
             if (!a.is_prev[(size_t)b * a.numSS_it + c]) adj = Q[0];
-            else adj = (double)a.timeStep[b] + (double)(a.N - over);
+            else adj = (double)a.timeStep[b] + (double)(Nb - over);
         }
     }
     for (int l = lane; l < count; l += 32) {
         const int row = start + l;
         const double* xr = X + (size_t)row * 6;
-        if (l < a.P) {
-            const int col = c * a.P + l;
+        if (l < P) {
+            const int col = c * P + l;
 #pragma unroll
-            for (int j = 0; j < 6; ++j) a.SS_sel[((size_t)b * 6 + j) * M + col] = xr[j];
-            a.Qfun_sel[(size_t)b * M + col] = Q[row] + adj;
+            for (int j = 0; j < 6; ++j) a.SS_sel[SHAPED ? (size_t)b * 6 * Mh + j * M + col : ((size_t)b * 6 + j) * M + col] = xr[j];
+            a.Qfun_sel[(size_t)b * (SHAPED ? Mh : M) + col] = Q[row] + adj;
         }
         if (l >= 1) {
-            const int col = c * a.P + (l - 1);
+            const int col = c * P + (l - 1);
 #pragma unroll
-            for (int j = 0; j < 6; ++j) a.Succ_SS[((size_t)b * 6 + j) * M + col] = xr[j];
-            a.Succ_uSS[((size_t)b * 2 + 0) * M + col] = U[(size_t)row * 2];
-            a.Succ_uSS[((size_t)b * 2 + 1) * M + col] = U[(size_t)row * 2 + 1];
+            for (int j = 0; j < 6; ++j) a.Succ_SS[SHAPED ? (size_t)b * 6 * Mh + j * M + col : ((size_t)b * 6 + j) * M + col] = xr[j];
+            a.Succ_uSS[SHAPED ? (size_t)b * 2 * Mh + 0 * M + col : ((size_t)b * 2 + 0) * M + col] = U[(size_t)row * 2];
+            a.Succ_uSS[SHAPED ? (size_t)b * 2 * Mh + 1 * M + col : ((size_t)b * 2 + 1) * M + col] = U[(size_t)row * 2 + 1];
         }
     }
 }
@@ -743,12 +759,13 @@ __device__ __forceinline__ void restart_record(int b, int* cl_len, double* x_cur
     done[b] = 0;
 }
 
-// The controller state a seeded controller starts from: xLin / uLin = rows 1..N+1 / 1..N of its record cx / cu (PC.py:432-433),
-// zt = [0,0,0,0,10,0] (PC.py:330), OldInput = 0.
-__device__ inline void seed_state_block(int b, int N, const double* cx, const double* cu, double* xLin, double* uLin, double* zt,
-                                        double* OldInput) {
-    for (int e = threadIdx.x; e < (N + 1) * 6; e += blockDim.x) xLin[(size_t)b * (N + 1) * 6 + e] = cx[6 + e];
-    for (int e = threadIdx.x; e < N * 2; e += blockDim.x) uLin[(size_t)b * N * 2 + e] = cu[2 + e];
+// The controller state a seeded controller starts from: xLin / uLin = rows 1..N_b+1 / 1..N_b of its record cx / cu
+// (PC.py:432-433) at the handle's stride N, zt = [0,0,0,0,10,0] (PC.py:330), OldInput = 0.
+__device__ inline void seed_state_block(int b, int N, const Shapes& shp, const double* cx, const double* cu, double* xLin, double* uLin,
+                                        double* zt, double* OldInput) {
+    const int Nb = horizon_of(shp, b, N);
+    for (int e = threadIdx.x; e < (Nb + 1) * 6; e += blockDim.x) xLin[(size_t)b * (N + 1) * 6 + e] = cx[6 + e];
+    for (int e = threadIdx.x; e < Nb * 2; e += blockDim.x) uLin[(size_t)b * N * 2 + e] = cu[2 + e];
     __syncthreads();
     if (threadIdx.x < 6) zt[(size_t)b * 6 + threadIdx.x] = (threadIdx.x == 4) ? 10.0 : 0.0;
     if (threadIdx.x < 2) OldInput[(size_t)b * 2 + threadIdx.x] = 0.0;
@@ -821,25 +838,27 @@ struct ShiftArgs {
     int* timeStep;
     int* has_pred;
     LapBudget retire;      // the state of a retired controller is not shifted
+    Shapes shp;            // the horizon N_b of every controller (the blocks keep the handle's stride N)
 };
+template <bool SHAPED>
 __global__ void shift_state_kernel(const ShiftArgs a) {
     const int b = blockIdx.x;
     if (b >= a.batch || a.retire.retired(b)) return;
-    const int N = a.N;
-    for (int e = threadIdx.x; e < (N + 1) * 6; e += blockDim.x) {
+    const int N = a.N, Nb = SHAPED ? a.shp.of(b).N : N;
+    for (int e = threadIdx.x; e < (Nb + 1) * 6; e += blockDim.x) {
         const int k = e / 6, j = e % 6;
         double v;
-        if (k < N) v = a.xPred[((size_t)b * (N + 1) + k + 1) * 6 + j];
-        else v = a.lmpc ? a.zt_in[(size_t)b * 6 + j] : a.xPred[((size_t)b * (N + 1) + N) * 6 + j];
+        if (k < Nb) v = a.xPred[((size_t)b * (N + 1) + k + 1) * 6 + j];
+        else v = a.lmpc ? a.zt_in[(size_t)b * 6 + j] : a.xPred[((size_t)b * (N + 1) + Nb) * 6 + j];
         a.xLin[(size_t)b * (N + 1) * 6 + e] = v;
         a.xPredPrev[(size_t)b * (N + 1) * 6 + e] = a.xPred[(size_t)b * (N + 1) * 6 + e];
-        if (k == N) a.zt[(size_t)b * 6 + j] = v;
+        if (k == Nb) a.zt[(size_t)b * 6 + j] = v;
     }
-    for (int e = threadIdx.x; e < N * 2; e += blockDim.x) {
+    for (int e = threadIdx.x; e < Nb * 2; e += blockDim.x) {
         const int k = e / 2, j = e % 2;
         double v;
-        if (k < N - 1) v = a.uPred[((size_t)b * N + k + 1) * 2 + j];
-        else v = a.lmpc ? a.ztu_in[(size_t)b * 2 + j] : a.uPred[((size_t)b * N + N - 1) * 2 + j];
+        if (k < Nb - 1) v = a.uPred[((size_t)b * N + k + 1) * 2 + j];
+        else v = a.lmpc ? a.ztu_in[(size_t)b * 2 + j] : a.uPred[((size_t)b * N + Nb - 1) * 2 + j];
         a.uLin[(size_t)b * N * 2 + e] = v;
     }
     if (threadIdx.x < 2) a.OldInput[(size_t)b * 2 + threadIdx.x] = a.uPred[(size_t)b * N * 2 + threadIdx.x];
@@ -1132,7 +1151,7 @@ __global__ void __launch_bounds__(32) ridge_sysid_kernel(int batch, const double
 __global__ void __launch_bounds__(256) seed_from_record_kernel(int batch, LapPool ss, LapPool model, int copies, int ss_slot0, int model_slot0,
                                                               const double* cl_x, const double* cl_u, int* cl_len, int Tcl, int N,
                                                               double* xLin, double* uLin, double* zt, double* OldInput, int* timeStep,
-                                                              int* hasPred, int* done, Tracks trk) {
+                                                              int* hasPred, int* done, Tracks trk, Shapes shp) {
     const int b = blockIdx.x;
     if (b >= batch) return;
     const int Trec = cl_len[b];
@@ -1143,7 +1162,7 @@ __global__ void __launch_bounds__(256) seed_from_record_kernel(int batch, LapPoo
         copy_ss_lap_block(ss, ss.lap_index(b, ss_slot0 + c), cx, cu, Trec, TrackLength);
         copy_lap_block(model, model.lap_index(b, model_slot0 + c), cx, cu, Trec);
     }
-    seed_state_block(b, N, cx, cu, xLin, uLin, zt, OldInput);
+    seed_state_block(b, N, shp, cx, cu, xLin, uLin, zt, OldInput);
     if (threadIdx.x == 0) { timeStep[b] = 0; hasPred[b] = 0; cl_len[b] = 0; done[b] = 0; }
 }
 

@@ -35,21 +35,28 @@ class RolloutTrace:
         nat.check(ctrl._lib.lmpc_rollout_trace_create(ctrl._h, len(self.instances), nat.ptr(inst), self.cap))
 
     def get(self, tr):
-        """Arrays of trace `tr` (index into `instances`): x[T,6], x_glob[T,6], u[T,2], xPred[T,N+1,6], SS_sel[T,6,M], lap[T]."""
+        """Arrays of trace `tr` (index into `instances`): x[T,6], x_glob[T,6], u[T,2], xPred[T,N+1,6], SS_sel[T,6,M], lap[T]; for a
+        controller with its own shape (BatchedController.set_shapes) N and M are its N_b and M_b."""
         c, N, M = self.c, self.c.N, max(self.c.M, 1)
         steps = C.c_int(0)
         o = dict(x=np.zeros((self.cap, 6)), x_glob=np.zeros((self.cap, 6)), u=np.zeros((self.cap, 2)), xPred=np.zeros((self.cap, N + 1, 6)),
                  SS_sel=np.zeros((self.cap, 6, M)), lap=np.zeros(self.cap, np.int32))
         nat.check(c._lib.lmpc_rollout_trace_get(c._h, int(tr), C.byref(steps), nat.ptr(o["x"]), nat.ptr(o["x_glob"]), nat.ptr(o["u"]),
                                                 nat.ptr(o["xPred"]), nat.ptr(o["SS_sel"]), nat.ptr(o["lap"])))
-        return {k: v[:steps.value].copy() for k, v in o.items()}
+        out = {k: v[:steps.value].copy() for k, v in o.items()}
+        Nb, Mb = c.shape_of(self.instances[tr])
+        if (Nb, Mb) != (c.N, c.M):      # the leading N_b + 1 rows and the row-major [6, M_b] block of the handle-sized regions
+            out["xPred"] = out["xPred"][:, :Nb + 1].copy()
+            out["SS_sel"] = out["SS_sel"].reshape(out["SS_sel"].shape[0], -1)[:, :6 * max(Mb, 1)].reshape(-1, 6, max(Mb, 1)).copy()
+        return out
 
     def plot_view(self, tr, first_lap_number=0):
         """One traced controller as an object with the attributes plot.py reads (laps = the laps completed within the trace;
         lap numbers start at `first_lap_number`, e.g. 4 after main.py's four seed laps)."""
         t = self.get(tr)
         laps = sorted(set(int(l) for l in t["lap"]))
-        v = SimpleNamespace(N=self.c.N, numSS_Points=self.c.M, SS=[], uSS=[], SS_glob=[], LapTime=[], xStoredPredTraj=[],
+        Nb, Mb = self.c.shape_of(self.instances[tr])
+        v = SimpleNamespace(N=Nb, numSS_Points=Mb, SS=[], uSS=[], SS_glob=[], LapTime=[], xStoredPredTraj=[],
                             SSStoredPredTraj=[], it=0)
         for l in laps[:-1] if len(laps) > 1 else laps:          # the last lap of the trace is usually still being driven
             m = t["lap"] == l
