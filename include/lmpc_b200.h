@@ -280,7 +280,8 @@ int lmpc_ss_put_lap(lmpc_handle* h, int inst, int slot, int T, const double* x, 
 /* Selection for the coming lap: slots[B,numSS_it] in argsort(LapTime) order (PC.py:395,402); is_prev[B,numSS_it] = 1
  * where that lap is iteration it-1 (PC.py:506-512); prev_slot[B] = slot receiving addPoint rows (-1: none). */
 int lmpc_ss_set_selection(lmpc_handle* h, const int* slots, const int* is_prev, const int* prev_slot);
-/* LMPC.addPoint (PC.py:466-476) for every instance: x[B,6], u[B,2] (host). */
+/* LMPC.addPoint (PC.py:466-476) for every instance: x[B,6], u[B,2] (host).  A non-finite value anywhere is refused with
+ * LMPC_E_INVALID and nothing is appended (the reference would store it; the device closed loop skips such a point, flag 512). */
 int lmpc_ss_add_point(lmpc_handle* h, const double* x, const double* u);
 /* Read a safe-set lap back (tests, plotting): x[Tmax,6], u[Tmax,2], qfun[Tmax] caller-allocated, *T rows valid. */
 int lmpc_ss_get_lap(lmpc_handle* h, int inst, int slot, int* T, double* x, double* u, double* qfun);
@@ -300,7 +301,9 @@ int lmpc_state_get(lmpc_handle* h, double* xLin, double* uLin, double* zt, doubl
  * the MaxNumPoint-th neighbour, so the selection is not certified to be the reference's). */
 int lmpc_identify_host(lmpc_handle* h, double* abc_out, int* flags);
 /* K2 alone — LMPC.addTerminalComponents (PC.py:386-416) for x0[B,6]: outputs as in lmpc_solve_lmpc_host plus
- * min_index[B,numSS_it] (argmin row per lap) and flags[B] (8 = window past the stored lap). */
+ * min_index[B,numSS_it] (argmin row per lap) and flags[B] (8 = window past the stored lap, or a lap without rows).  The argmin
+ * row is np.argmin's for any zt and lap: the first row at a NaN distance if there is one, else the first minimum, +inf included
+ * (a lap at distance +inf everywhere selects row 0).  A lap without rows writes neither selection nor min_index. */
 int lmpc_select_host(lmpc_handle* h, const double* x0, double* SS_sel, double* Qfun_sel, double* Succ_SS,
                      double* Succ_uSS, int* min_index, int* flags);
 
@@ -343,7 +346,8 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
  * The simulator adds two bits of its own, in lmpc_rollout_step and lmpc_rollout_pid_step alike: 128 = a curvature lookup of
  * the plant failed (s < 0, s exactly at the finish line, s not finite or beyond 64 laps: the reference raises, Track.py:292-310;
  * the step went on with curvature 0), 256 = a step found the closed-loop record full (Tcl rows) and was not recorded, so the
- * lap is longer than the record and its hand-over files it truncated. */
+ * lap is longer than the record and its hand-over files it truncated.  Mode 1 adds 512 = the controller's state or input was not
+ * finite, so addPoint did not append it to lap it-1 (the lap the pooled exchange exports). */
 int lmpc_rollout_get_health(lmpc_handle* h, int* flags_or, int* unsolved_steps);                 /* [B] host             */
 /* The rest of main.py's pipeline on the device (SURVEY §8f rank 3).
  * lmpc_rollout_pid_step: one closed-loop step under the PID path follower (Utilities.py:42-68, target speed vt); z_pid_host[B,2]

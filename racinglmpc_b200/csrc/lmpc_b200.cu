@@ -1226,6 +1226,10 @@ int lmpc_ss_set_selection(lmpc_handle* h, const int* slots, const int* is_prev, 
 int lmpc_ss_add_point(lmpc_handle* h, const double* x, const double* u) {
     if (int rc = need_store(h)) return rc;
     if (!x || !u) return fail(LMPC_E_INVALID, "null argument");
+    for (int b = 0; b < h->batch; ++b)       // the kernel would skip such a point and flag 512; the host caller hears of it here
+        for (int j = 0; j < 6; ++j)
+            if (!isfinite(x[(size_t)b * 6 + j]) || (j < 2 && !isfinite(u[(size_t)b * 2 + j])))
+                return fail(LMPC_E_INVALID, "addPoint: non-finite x or u of instance " + std::to_string(b));
     CK(cudaMemcpyAsync(h->d_tmpx, x, sizeof(double) * h->batch * 6, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(h->d_tmpu, u, sizeof(double) * h->batch * 2, cudaMemcpyHostToDevice, h->stream));
     ss_add_point_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->batch, h->ss, h->d_prevslot, h->d_tmpx, h->d_tmpu, 2,

@@ -12,6 +12,7 @@
 // Rows are contiguous, so a warp scanning a lap issues fully coalesced 48 B/row (x) + 16 B/row (u) loads.
 #pragma once
 #include <math.h>
+#include <math_constants.h>
 #include <stdint.h>
 #include "lap_budget.cuh"
 
@@ -567,8 +568,10 @@ __global__ void __launch_bounds__(32 * 8) ss_select_kernel(const K2Args a) {
     const double* U = a.pool.u + lap * a.pool.Tmax * 2;
     const double* Q = a.pool.q + lap * a.pool.Tmax;
     const int T = a.pool.len[lap];
-    // 1-nearest neighbour in the 1-norm over all six states (PC.py:486-490); first minimum wins
-    double bd = 1e300;
+    // 1-nearest neighbour in the 1-norm over all six states (PC.py:486-490) in np.argmin's order: the first NaN distance if there
+    // is one (a NaN counts as -1, below every distance), else the first minimum.  A minimum of +inf is no candidate below: then
+    // every distance is +inf, and np.argmin returns row 0
+    double bd = CUDART_INF;
     int bi = 0x7fffffff;
     for (int t = lane; t < T; t += 32) {
         const double* xr = X + (size_t)t * 6;
@@ -578,6 +581,7 @@ __global__ void __launch_bounds__(32 * 8) ss_select_kernel(const K2Args a) {
         d = __dadd_rn(d, fabs(__dsub_rn(xr[3], z[3])));
         d = __dadd_rn(d, fabs(__dsub_rn(xr[4], z[4])));
         d = __dadd_rn(d, fabs(__dsub_rn(xr[5], z[5])));
+        if (isnan(d)) d = -1.0;
         if (d < bd) { bd = d; bi = t; }
     }
 #pragma unroll
@@ -586,7 +590,11 @@ __global__ void __launch_bounds__(32 * 8) ss_select_kernel(const K2Args a) {
         int oi = __shfl_xor_sync(0xffffffffu, bi, o);
         if (cand_less(od, oi, bd, bi)) { bd = od; bi = oi; }
     }
-    const int mn = bi;
+    const int mn = bi == 0x7fffffff ? 0 : bi;
+    if (mn >= T) {                                            // a lap without rows (np.argmin of an empty array raises)
+        if (lane == 0) atomicOr(&a.status[b], 8);
+        return;
+    }
     // window (PC.py:492-495), numPoints = P + 1
     const int npt = P + 1;
     const int half = npt / 2;
@@ -629,12 +637,21 @@ __global__ void __launch_bounds__(32 * 8) ss_select_kernel(const K2Args a) {
 
 // ------------------------------------------------------------------------------------------------
 // LMPC.addPoint (PC.py:466-476): append x + [0,0,0,0,L,0], u to lap it-1; Qfun extends by last - 1.
+// A point with a non-finite value is not appended (the reference would store it): flag 512.  Lap it-1 is the lap the pooled
+// exchange exports, so a diverged controller would otherwise hand NaN rows to every importer of its group.
 __global__ void ss_add_point_kernel(int batch, LapPool pool, const int* prev_slot, const double* x, const double* u,
                                     long long u_stride, Tracks trk, int* status, int* dropped, LapBudget retire) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= batch || retire.retired(b)) return;
     const int slot = prev_slot[b];
     if (slot < 0) return;
+    bool finite = isfinite(u[(size_t)b * u_stride]) && isfinite(u[(size_t)b * u_stride + 1]);
+#pragma unroll
+    for (int j = 0; j < 6; ++j) finite = finite && isfinite(x[(size_t)b * 6 + j]);
+    if (!finite) {
+        atomicOr(&status[b], 512);
+        return;
+    }
     const size_t lap = pool.lap_index(b, slot);
     const int T = pool.len[lap];
     if (T >= pool.Tmax || T < 1) {       // the lap cannot grow (the reference would keep appending): flag it, count it
@@ -903,7 +920,7 @@ struct SimArgs {
     const int* streams;               // [B] Philox stream of every instance (lmpc_rollout_set_noise_streams), or nullptr: b
     LapBudget retire;                 // a retired instance is not driven (the PID lap passes a null budget)
 };
-// Health bits of the simulator itself (the step flags use 1 .. 64):
+// Health bits of the simulator itself (the step flags use 1 .. 64 and 512):
 //   SIM_LOOKUP_FAILED  a sub-step's curvature lookup failed (s < 0, s at the finish line after the wrap, s not finite or beyond
 //                      64 laps): the reference raises there (Track.py:292-310); the step went on with curvature 0
 //   SIM_RECORD_FULL    the closed-loop record already held Tcl rows, so this step's (x, u) was not recorded: the lap is longer

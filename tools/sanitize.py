@@ -4,7 +4,8 @@
 Exercises: ftocp_kernel<12,0> and <12,48> (host + device entry points), knn_ltv_regress, ss_select, shift_state,
 ss_add_point, rollout_cost, sim_step (with noise sets and noise streams), measure (with measurement sets), knn_ltv_regress with regression sets, commit_laps, ss_export_laps, ss_import_laps; round 2: the long-horizon kernel
 that reads its model in place (N = 48), warm-started solves, pid_input, seed_books, commit_laps_books, rollout_stats, the pooled
-exchange (pool_local_best / export / rank / import), trace_step and track_global_position."""
+exchange (pool_local_best / export / rank / import), trace_step and track_global_position, and a controller made
+non-finite in the closed loop (ss_select on a NaN terminal guess, ss_add_point refusing the point)."""
 import os
 import sys
 import numpy as np
@@ -78,6 +79,15 @@ tr = export.RolloutTrace(c, [0, 3], cap_steps=64)
 for _ in range(6):
     c.rollout_step(seed=3)                               # warm-started from the second step on
     c.rollout_commit_laps_dev()
+# a controller whose state stops being finite: K2 on its non-finite terminal guess, addPoint refusing its point (flag 512)
+st = c.rollout_state()
+xb = st["x"].copy()
+xb[1, 0] = np.nan
+c.rollout_set_state(xb, st["xglob"])
+for _ in range(3):
+    c.rollout_step(seed=3)
+    c.rollout_commit_laps_dev()
+assert c.rollout_health()[0][1] & 512
 print("stats", c.rollout_stats())
 rows = torch.zeros(3, 288, 9, dtype=torch.float64, device="cuda")
 meta = torch.zeros(3, 4, dtype=torch.int32, device="cuda")
