@@ -72,7 +72,7 @@ def layout(warm=False, shape_sets=None):
 def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, poll=8, max_steps=0, seed=1234, local=None, warm=False,
         final=None, param_sets=None, vehicle_sets=None, books=None, track_sets=None, pool_groups=None, readiness="batch",
         capture=None, start=None, noise_sets=None, noise_streams=None, regression_sets=None, lap_budget=None, measurement_sets=None,
-        shape_sets=None):
+        shape_sets=None, ss_laps_sets=None):
     """One Monte-Carlo run on this rank's GPU (torch.distributed may or may not be initialised).  Returns a dict (all ranks).
     final: None, or a dict that receives the closed loop's end state (rollout_state) and the last step's solver report (step_results).
     books: None, or a dict that receives the lap books (books) and the health counters (flags_or, unsolved).
@@ -102,6 +102,13 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     handle is created at handle_shape(shape_sets), the smallest grid pair that dominates every shape (ValueError before any device
     work when there is none, or where set_shapes would refuse a shape).  A shape equal to the handle's (12, 48) runs the shaped
     QP kernel with the reference's parameters.
+    ss_laps_sets: None, or (values, index) handed to BatchedController.set_ss_laps: numSS_it per controller, 1 .. the handle's 4
+    (how to split the safe set between laps and points per lap in one batch; the result then holds per-value lap statistics and
+    mean interior-point iterations under "per_ss_laps_rank0").  Every controller's numSS_Points (its shape, or the handle's) must be
+    its value times an even number of points per lap.  ValueError before any device work where set_ss_laps would refuse.  The
+    seeding stores 4 copies of the PID lap whatever the value (main.py:103-110).  The pooled mode ranks an import against the
+    importer's own value, so pool groups may mix values.  With shape_sets as well, the result also holds the statistics of every
+    (shape, value) cell under "per_shape_ss_laps_rank0".
     pool_groups: None, or (index, G) handed to BatchedController.set_pool_groups (e.g. sharding.design_groups(track index,
     parameter-set index)): the pooled mode then exchanges laps within each group; the exchange buffers hold G * (share + 1) laps
     per rank and the result holds the laps filed per group under "laps_filed_per_group_rank0" (stored laps counted from the books;
@@ -127,7 +134,8 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     clock and the scheduler state are set, and the run first repeats the poll the capture was taken at, under the new `laps`
     (groups that exchanged at that poll are not exchanged again), then steps on.  A run to 3 laps captured and resumed to 5
     therefore equals a run to 5 laps bit for bit (books, end states, health, exchange steps).  Tables (param_sets, vehicle_sets,
-    noise_sets, noise_streams, measurement_sets, regression_sets, track_sets, pool_groups) are installed from the arguments, as for a fresh run.  ValueError before any device work when start
+    noise_sets, noise_streams, measurement_sets, regression_sets, track_sets, pool_groups, shape_sets, ss_laps_sets) are installed
+    from the arguments, as for a fresh run; restore a record into a controller of the value it was captured with.  ValueError before any device work when start
     does not match the batch, the layout, the mode, the readiness, the poll interval or the pool groups, or when laps is not
     above the captured laps.
     lap_budget: None (every controller is stepped until the slowest has its laps), or the laps every controller drives before it
@@ -143,10 +151,15 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     the controller where it stopped, with the noise draws of the later clock)."""
     budget = _native.make_lap_budget(lap_budget, int(batch))       # ValueError where set_lap_budget would refuse, before any device work
     N, M = handle_shape(shape_sets)
+    numSS_it = rp.lmpc_params(N)[0]
+    points = [M] * int(batch)                                      # every controller's numSS_Points
     if shape_sets is not None:
         if warm:
             raise ValueError("shape_sets and warm start: the warm-start record is laid out per (N, numSS_Points)")
-        _native.make_shape_sets(shape_sets[0], shape_sets[1], int(batch), N, M, rp.lmpc_params(N)[0])
+        rows, sidx = _native.make_shape_sets(shape_sets[0], shape_sets[1], int(batch), N, M, numSS_it)
+        points = [rows[k].numSS_Points for k in sidx]
+    if ss_laps_sets is not None:
+        _native.make_ss_laps_sets(ss_laps_sets[0], ss_laps_sets[1], int(batch), numSS_it, points)
     if start is not None:
         _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget, shape_sets)
     if capture is not None and not isinstance(capture, dict):
@@ -171,7 +184,7 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     dev = torch.device("cuda", local)
     torch.cuda.set_device(dev)
     B = int(batch)
-    numSS_it, _, _, _, Qts, par = rp.lmpc_params(N)
+    _, _, _, _, Qts, par = rp.lmpc_params(N)
     c = BatchedController(par, B, workloads.track_seg_table(), rp.TRACK_LENGTH, trToUse=TR_TO_USE, numSS_Points=M,
                           numSS_it=numSS_it, QterminalSlack=Qts, device=local, Tmax=TMAX, ss_cap=SS_CAP, model_cap=MODEL_CAP,
                           warm_start=warm)
@@ -183,7 +196,8 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
               (None if noise_streams is None else (noise_streams,), c.set_noise_streams, None),
               (measurement_sets, c.set_measurement_noise, "per_measurement_rank0"),
               (regression_sets, c.set_regression, "per_regression_rank0"), (track_sets, c.set_tracks, "per_track_rank0"),
-              (pool_groups, c.set_pool_groups, None), (shape_sets, c.set_shapes, "per_shape_rank0"))
+              (pool_groups, c.set_pool_groups, None), (shape_sets, c.set_shapes, "per_shape_rank0"),
+              (ss_laps_sets, c.set_ss_laps, "per_ss_laps_rank0"))
     for args, install, _ in tables:
         if args is not None:
             install(*args)
@@ -229,7 +243,7 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     max_steps = int(max_steps) or 300 * laps
     steps, n_xchg, xchg_s, took_total = sched.start_step, 0, 0.0, 0
     it_sum, it_n, it_max = 0.0, 0, 0                     # interior-point iterations, sampled at the polls
-    it_ctrl = np.zeros(B)                                # ... per controller (the per-shape means)
+    it_ctrl = np.zeros(B)                                # ... per controller (the per-shape and per-lap-count means)
     l0 = c.kernel_launches
     e0.record(stream)
     while steps < max_steps or sched.repeat:
@@ -299,6 +313,22 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
             s.update(N=int(shape_sets[0][k][0]), numSS_Points=int(shape_sets[0][k][1]),
                      ipm_iters_mean_sampled=float(it_ctrl[idx == k].mean() / max(it_n, 1)) if (idx == k).any() else 0.0)
         out["handle_shape"] = [N, M]
+    if ss_laps_sets is not None:
+        idx = np.asarray(ss_laps_sets[1]).reshape(B)
+        for k, s in enumerate(out["per_ss_laps_rank0"]):
+            s.update(numSS_it=int(ss_laps_sets[0][k]),
+                     ipm_iters_mean_sampled=float(it_ctrl[idx == k].mean() / max(it_n, 1)) if (idx == k).any() else 0.0)
+        if shape_sets is not None:
+            sidx = np.asarray(shape_sets[1]).reshape(B)
+            out["per_shape_ss_laps_rank0"] = []
+            for j, sh in enumerate(shape_sets[0]):
+                for k, v in enumerate(ss_laps_sets[0]):
+                    cell = (sidx == j) & (idx == k)
+                    if cell.any():
+                        s = _set_stats(bk, flags_or, unsolved, cell, laps)
+                        s.update(N=int(sh[0]), numSS_Points=int(sh[1]), numSS_it=int(v),
+                                 ipm_iters_mean_sampled=float(it_ctrl[cell].mean() / max(it_n, 1)))
+                        out["per_shape_ss_laps_rank0"].append(s)
     if pool_groups is not None:
         # a stored lap advances `it`: 4 seeded copies + every own lap handed over + every imported lap filed.  Exact unless an
         # own lap found the safe-set pool full (health flag 64): then that controller's count is one too low per such lap.

@@ -266,8 +266,40 @@ typedef struct lmpc_shape_params {
  * abc holds N_b stages, SS_sel / Succ_SS / Succ_uSS hold a row-major [6,M_b] / [2,M_b] block at the start of the controller's
  * region, Qfun_sel and lambd hold M_b entries.  A shaped controller never writes the tails.
  * A shaped handle runs one QP launch per distinct shape present (per distinct N for the MPC-type QPs of modes 0 and 2), each over
- * the controllers of that shape (DESIGN.md, "Per-controller horizons and safe-set sizes"). */
+ * the controllers of that shape (DESIGN.md, "Per-controller horizons and safe-set sizes").
+ * With a lap-count table installed (lmpc_set_ss_laps) every controller's numSS_Points must instead be its own numSS_it times an
+ * even number of points per lap; a pair that breaks this is refused with LMPC_E_INVALID, whichever table is installed first. */
 int lmpc_set_shapes(lmpc_handle* h, const lmpc_shape_params* sets, int nsets, const int* set_of_instance);
+
+/* Per-controller safe-set lap count: numSS_it, the number of fastest past laps the sampled safe set draws from (PC.py:395-407). */
+typedef struct lmpc_ss_laps_params {
+    int numSS_it;
+} lmpc_ss_laps_params;
+/* Per-controller safe-set lap counts (how to split the safe set between laps and points per lap, in one batch).  Controller b
+ * selects its safe set from its numSS_it_b = sets[set_of_instance[b]].numSS_it fastest laps, M_b / numSS_it_b points per lap, M_b
+ * being its numSS_Points (lmpc_set_shapes, else the handle's).  nsets == 0 (sets, set_of_instance NULL) returns every controller
+ * to the handle's numSS_it.
+ *   - Requires lmpc_store_create and an LMPC handle (numSS_Points > 0), and no lap stored yet in either pool (as lmpc_set_tracks
+ *     and lmpc_set_shapes; else LMPC_E_STATE): the lap books evict laps against the controller's value, so raising it later would
+ *     select laps already gone, where the reference's unbounded lists still hold them.
+ *   - 1 <= nsets <= batch, every index in [0, nsets).  Per set: 1 <= numSS_it <= the handle's numSS_it, which keeps sizing sel,
+ *     is_prev, min_index, K2's block and the snapshot record.  Per controller: M_b is numSS_it_b times an even number of points per
+ *     lap (checked against the installed shapes here, and by lmpc_set_shapes against this table).  Any failed check returns
+ *     LMPC_E_INVALID and leaves the handle as it was.
+ *   - The call synchronises the handle's streams before it replaces the table.
+ *   - Honoured by lmpc_select_host, lmpc_step_host / _dev / _profile, lmpc_rollout_step mode 1, the device lap hand-over
+ *     (lmpc_rollout_commit_laps_dev) and seeding (lmpc_rollout_seed_from_record_dev), lmpc_pool_import_dev (an importer ranks a
+ *     lap against its own numSS_it_b; the exporter is unchanged, so pool groups may mix values) and lmpc_books_set.  The device
+ *     books then rank, evict and flag (8: fewer than numSS_it_b laps; 64: pool too small) exactly as a handle created with
+ *     numSS_it_b and the same ss_cap.  Seeding still stores the copies the caller asks for: a controller whose numSS_it_b exceeds
+ *     them gets flag 8, as the handle does.
+ *   - Layout: sel / is_prev / min_index keep the handle's numSS_it entries per controller.  Entries c < numSS_it_b are the
+ *     controller's selection; entries c >= numSS_it_b of sel repeat its last selected slot and those of is_prev are 0 (valid and
+ *     deterministic, so records pack and restore bit for bit); min_index keeps what it held there.  K2 writes columns
+ *     c * P_b + l, P_b = M_b / numSS_it_b, of the controller's [6, M_b] block.
+ *   - Unchanged: lmpc_set_param_sets still requires the handle's numSS_it, the snapshot header keeps the handle's value, and the
+ *     table is not part of a snapshot record (restore a record into a controller of the same numSS_it_b to resume it). */
+int lmpc_set_ss_laps(lmpc_handle* h, const lmpc_ss_laps_params* sets, int nsets, const int* set_of_instance);
 
 /* PredictiveModel.addTrajectory (PredictiveModel.py:35-46): copy one lap into a regression slot. */
 int lmpc_model_put_lap(lmpc_handle* h, int inst, int slot, int T, const double* x, const double* u);
@@ -606,6 +638,7 @@ int lmpc_sizeof_noise_params(void);
 int lmpc_sizeof_measurement_params(void);
 int lmpc_sizeof_regression_params(void);
 int lmpc_sizeof_shape_params(void);
+int lmpc_sizeof_ss_laps_params(void);
 
 #ifdef __cplusplus
 }

@@ -59,6 +59,11 @@ class ShapeParams(C.Structure):
     _fields_ = [("N", C.c_int), ("numSS_Points", C.c_int)]
 
 
+class SsLapsParams(C.Structure):
+    """lmpc_ss_laps_params: numSS_it, the number of fastest past laps a controller's safe set draws from."""
+    _fields_ = [("numSS_it", C.c_int)]
+
+
 # The (N, numSS_Points) pairs the library instantiates the QP kernel for: LMPC_FOR_EACH_CASE in csrc/ftocp_launch.cuh (a CPU test
 # keeps the two equal)
 SHAPE_GRID = tuple([(n, 0) for n in (4, 6, 8, 10, 12, 14, 16, 20, 24, 32, 48)] + [(n, 48) for n in (4, 6, 8, 10, 12, 14, 16, 20, 24, 32, 48)] +
@@ -161,6 +166,7 @@ def lib():
     L.lmpc_set_tracks.argtypes = [_vp, C.POINTER(TrackParams), C.c_int, _vp]
     L.lmpc_set_regression_sets.argtypes = [_vp, C.POINTER(RegressionParams), C.c_int, _vp]
     L.lmpc_set_shapes.argtypes = [_vp, C.POINTER(ShapeParams), C.c_int, _vp]
+    L.lmpc_set_ss_laps.argtypes = [_vp, C.POINTER(SsLapsParams), C.c_int, _vp]
     L.lmpc_rollout_sysid.argtypes = [_vp, C.c_double, _vp, _vp]
     L.lmpc_rollout_seed_from_record.argtypes = [_vp, C.c_int, C.c_int, C.c_int]
     L.lmpc_rollout_get_lap.argtypes = [_vp, C.c_int, ip, _vp, _vp]
@@ -201,6 +207,8 @@ def lib():
     L.lmpc_sizeof_regression_params.restype = C.c_int
     L.lmpc_sizeof_shape_params.restype = C.c_int
     assert L.lmpc_sizeof_shape_params() == C.sizeof(ShapeParams), "lmpc_shape_params ABI mismatch"
+    L.lmpc_sizeof_ss_laps_params.restype = C.c_int
+    assert L.lmpc_sizeof_ss_laps_params() == C.sizeof(SsLapsParams), "lmpc_ss_laps_params ABI mismatch"
     assert L.lmpc_sizeof_noise_params() == C.sizeof(NoiseParams), "lmpc_noise_params ABI mismatch"
     assert L.lmpc_sizeof_measurement_params() == C.sizeof(MeasurementParams), "lmpc_measurement_params ABI mismatch"
     assert L.lmpc_sizeof_regression_params() == C.sizeof(RegressionParams), "lmpc_regression_params ABI mismatch"
@@ -529,12 +537,18 @@ def make_regression_sets(regs, index, batch, trToUse):
     return _pack_sets(RegressionParams, regs, index, batch, "regression sets", row)
 
 
-def make_shape_sets(shapes, index, batch, N, M, numSS_it):
+def _even_split(M, nit):
+    """M safe-set points split into nit laps of an even number of points each (PC.py:403,492-495)"""
+    return M % nit == 0 and (M // nit) % 2 == 0
+
+
+def make_shape_sets(shapes, index, batch, N, M, numSS_it, ss_laps=None):
     """Per-controller shapes for ``lmpc_set_shapes``: K ``(N, numSS_Points)`` pairs ``shapes`` and the shape of every controller
     ``index[batch]`` on a handle of horizon ``N``, safe-set size ``M`` and ``numSS_it`` laps.  Raises ValueError where the library
     would refuse: the index rules of ``make_param_sets``, a pair outside SHAPE_GRID, N or numSS_Points above the handle's, a
     numSS_Points that is 0 on an LMPC handle or > 0 on an MPC handle, or one that is not numSS_it times an even number of points
-    per lap.  Returns (ctypes array ShapeParams * K, int32 index array)."""
+    per lap.  ``ss_laps`` (the numSS_it of every controller under ``lmpc_set_ss_laps``, or None) replaces numSS_it in that last
+    check, controller by controller.  Returns (ctypes array ShapeParams * K, int32 index array)."""
     def row(k, sh):
         w = "shape %d: " % k
         try:
@@ -551,10 +565,39 @@ def make_shape_sets(shapes, index, batch, N, M, numSS_it):
             raise ValueError(w + "(%d, %d) exceeds the handle's (%d, %d)" % (n, m, N, M))
         if (m > 0) != (int(M) > 0):
             raise ValueError(w + "numSS_Points must be > 0 exactly when the handle's is (%d)" % M)
-        if m > 0 and (m % int(numSS_it) or (m // int(numSS_it)) % 2):
+        if ss_laps is None and m > 0 and not _even_split(m, int(numSS_it)):
             raise ValueError(w + "numSS_Points must be numSS_it (%d) times an even number of points per lap" % numSS_it)
         return ShapeParams(n, m)
-    return _pack_sets(ShapeParams, shapes, index, batch, "shapes", row)
+    rows, idx = _pack_sets(ShapeParams, shapes, index, batch, "shapes", row)
+    if ss_laps is not None:
+        for b in range(batch):
+            m, v = rows[idx[b]].numSS_Points, int(ss_laps[b])
+            if not _even_split(m, v):
+                raise ValueError("controller %d: numSS_Points %d is not its numSS_it (%d) times an even number of points per lap" % (b, m, v))
+    return rows, idx
+
+
+def make_ss_laps_sets(values, index, batch, numSS_it, points):
+    """Per-controller safe-set lap counts for ``lmpc_set_ss_laps``: K values of numSS_it ``values`` and the value of every
+    controller ``index[batch]`` on an LMPC handle of ``numSS_it`` laps whose controllers have ``points[batch]`` safe-set points
+    (their shapes, or the handle's numSS_Points).  Raises ValueError where the library would refuse: the index rules of
+    ``make_param_sets``, a value that is not an integer in 1 .. numSS_it, or a controller whose points are not its value times an
+    even number of points per lap.  Returns (ctypes array SsLapsParams * K, int32 index array)."""
+    if int(numSS_it) < 1 or min(int(m) for m in points) <= 0:
+        raise ValueError("per-controller lap counts need an LMPC handle (numSS_Points > 0)")
+
+    def row(k, v):
+        if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)):
+            raise ValueError("lap count %d: numSS_it must be an integer, got %r" % (k, v))
+        if not 1 <= int(v) <= int(numSS_it):
+            raise ValueError("lap count %d: numSS_it must be 1 .. the handle's %d, got %d" % (k, numSS_it, v))
+        return SsLapsParams(int(v))
+    rows, idx = _pack_sets(SsLapsParams, values, index, batch, "lap counts", row)
+    for b in range(batch):
+        m, v = int(points[b]), rows[idx[b]].numSS_it
+        if not _even_split(m, v):
+            raise ValueError("controller %d: numSS_Points %d is not numSS_it (%d) times an even number of points per lap" % (b, m, v))
+    return rows, idx
 
 
 def make_pool_groups(index, ngroups, batch):

@@ -67,6 +67,7 @@ class BatchedController:
         self.device_books = False
         self._pool_groups = 1
         self._shapes = None                                 # (shapes, index) of set_shapes, or None: the handle's own shape
+        self._ss_laps = None                                # numSS_it of every controller (set_ss_laps), or None: the handle's
         self._sel = np.zeros((self.B, nit), np.int32); self._isp = np.zeros((self.B, nit), np.int32)
         self._prev = -np.ones(self.B, np.int32); self._used = np.zeros((self.B, self.trToUse), np.int32)
 
@@ -177,13 +178,38 @@ class BatchedController:
         handle's (N, numSS_Points) as their stride: ``read_buffer`` and the trace cut a controller's rows to its shape.  Waits for
         work already enqueued."""
         self._install(self._lib.lmpc_set_shapes, "shapes", shapes, index,
-                      lambda: nat.make_shape_sets(shapes, index, self.B, self.N, self.M, self.numSS_it))
+                      lambda: nat.make_shape_sets(shapes, index, self.B, self.N, self.M, self.numSS_it, self._ss_laps))
         self._shapes = None if shapes is None else ([tuple(int(v) for v in s) for s in shapes], np.asarray(index).reshape(-1).copy())
 
     def shape_of(self, inst):
         """(N, numSS_Points) controller ``inst`` plans with: its row of ``set_shapes``, or the handle's."""
         sh = self._shapes
         return (self.N, self.M) if sh is None else sh[0][int(sh[1][int(inst)])]
+
+    def set_ss_laps(self, values, index=None):
+        """Per-controller safe-set lap counts (how to split the safe set between laps and points per lap, in one batch):
+        controller b draws its safe set from its ``values[index[b]]`` fastest laps, numSS_Points_b / values[index[b]] points per
+        lap, in every later ``select``, ``step`` and ``rollout_step`` and in the lap books (host or device), which rank, evict and
+        flag as a controller created with that numSS_it and the same ss_cap.  Every value is an integer in 1 .. the handle's
+        numSS_it, and every controller's numSS_Points (``shape_of``) must be its value times an even number of points per lap.
+        ``index`` is required with ``values``.  ``values=None`` (no index) returns every controller to the handle's numSS_it.
+        Only on an LMPC handle and before the first lap is stored; seeding still stores the copies asked for, so a controller
+        whose value exceeds them is flagged as the handle would be.  Not part of a snapshot.  Waits for work already enqueued."""
+        if values is None:
+            points = [self.shape_of(b)[1] for b in range(self.B)]
+            if any(not nat._even_split(m, max(self.numSS_it, 1)) for m in points):
+                raise ValueError("the installed shapes need their lap counts: the handle's numSS_it does not split them evenly")
+        self._install(self._lib.lmpc_set_ss_laps, "values", values, index,
+                      lambda: nat.make_ss_laps_sets(values, index, self.B, self.numSS_it, [self.shape_of(b)[1] for b in range(self.B)]))
+        if values is None:
+            self._ss_laps = None
+        else:
+            rows = [int(v) for v in values]
+            self._ss_laps = np.array([rows[int(i)] for i in np.asarray(index).reshape(-1)], np.int32)
+
+    def ss_laps_of(self, inst):
+        """numSS_it of controller ``inst``: its value of ``set_ss_laps``, or the handle's."""
+        return self.numSS_it if self._ss_laps is None else int(self._ss_laps[int(inst)])
 
     def set_tracks(self, tracks, index=None):
         """Per-controller tracks (several circuits in one batch): controller b drives ``tracks[index[b]]`` (objects with
@@ -290,14 +316,14 @@ class BatchedController:
         return first, slot
 
     def _ss_slot_for(self, inst, lap_time):
-        """LMPC.addTrajectory bookkeeping (PC.py:425-428): new lap number = it; keep the numSS_it fastest + lap it-1."""
+        """LMPC.addTrajectory bookkeeping (PC.py:425-428): new lap number = it; keep the controller's numSS_it fastest + lap it-1."""
         lapno = self.it[inst]
         self.LapTime[inst].append(int(lap_time))
         self.own_laps[inst].append(lapno)
         book = self.ss_book[inst]
         if not book.free:
             order = list(np.argsort(np.array(self.LapTime[inst]), kind="stable"))
-            keep = set(order[:self.numSS_it]) | {lapno}
+            keep = set(order[:self.ss_laps_of(inst)]) | {lapno}
             victims = [ln for ln in book.slot_of if ln not in keep]
             if not victims:
                 raise RuntimeError("safe-set pool too small")
@@ -314,12 +340,12 @@ class BatchedController:
             self._push_selection()
 
     def _push_selection(self):
-        nit = max(self.numSS_it, 1)
         sel, isp, prev = self._sel, self._isp, self._prev
         rows = range(self.B) if self._sel_rows is None else self._sel_rows
         for b in rows:
             if not self.LapTime[b]:
                 continue
+            nit = max(self.ss_laps_of(b), 1)
             if len(self.LapTime[b]) < nit:
                 # the reference indexes sortedLapTime[0:numSS_it] lap by lap and raises IndexError here (PC.py:402-403)
                 raise IndexError("instance %d has %d stored laps, fewer than numSS_it = %d" % (b, len(self.LapTime[b]), nit))
@@ -327,6 +353,8 @@ class BatchedController:
             for c, jj in enumerate(order):
                 sel[b, c] = self.ss_book[b].slot_of[int(jj)]
                 isp[b, c] = 0 if int(jj) < self.it[b] - 1 else 1                    # PC.py:506
+            sel[b, nit:] = sel[b, nit - 1]                                          # entries K2 does not read, as the device books
+            isp[b, nit:] = 0
             prev[b] = self.ss_book[b].slot_of.get(self.it[b] - 1, -1)
         self._sel_rows = set()
         nat.check(self._lib.lmpc_ss_set_selection(self._h, nat.ptr(sel), nat.ptr(isp), nat.ptr(prev)))
@@ -567,7 +595,7 @@ class BatchedController:
                 continue
             lt, last = int(lap_times[b]), self.it[b] - 1
             times = self.LapTime[b][:last] + [lt] + self.LapTime[b][last:]
-            order = list(np.argsort(np.array(times), kind="stable"))[:self.numSS_it]
+            order = list(np.argsort(np.array(times), kind="stable"))[:self.ss_laps_of(b)]
             if last not in order:                         # never selected (PC.py:395) -> not in the safe set
                 if to_model:
                     m_slots[b] = self._model_slot_for(b, lt)

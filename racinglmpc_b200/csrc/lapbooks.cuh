@@ -30,12 +30,17 @@ constexpr int LAP_HIST = 16;
 
 __device__ __forceinline__ bool key_less(int t1, int n1, int t2, int n2) { return t1 < t2 || (t1 == t2 && n1 < n2); }
 
+// numSS_it of controller b in a book kernel.  The kernels that rank safe-set laps come in two instantiations, LAPS = a lap-count
+// table is installed (lmpc_set_ss_laps): without one they read the handle's value, the code they were before the table existed.
+template <bool LAPS>
+__device__ __forceinline__ int book_laps(const LapBooks& k, const SsLaps& laps, int b) { return LAPS ? laps.of(b).numSS_it : k.numSS_it; }
+
 // LMPC.addTrajectory bookkeeping for a lap of `T` rows.  import == false: the controller's own new lap (lap number it).
 // import == true: a lap another controller drove, filed BEFORE the controller's own latest lap (which stays lap it-1, the one
 // addPoint extends): it takes lap number it-1, the own latest moves to it; it is skipped (-1) when it would not be among the
-// numSS_it fastest.  Returns the slot to copy the lap into, -1 = not stored, -2 = pool too small (the tables are left as they
-// were).
-__device__ inline int book_ss_add(const LapBooks& k, int b, int T, bool import) {
+// nit fastest (nit: the controller's numSS_it).  Returns the slot to copy the lap into, -1 = not stored, -2 = pool too small (the
+// tables are left as they were).
+__device__ inline int book_ss_add(const LapBooks& k, int b, int T, bool import, int nit) {
     int* tm = k.ss_time + (size_t)b * k.ss_cap;
     int* ln = k.ss_lap + (size_t)b * k.ss_cap;
     const int it = k.it[b];
@@ -46,7 +51,7 @@ __device__ inline int book_ss_add(const LapBooks& k, int b, int T, bool import) 
         int rank = 0;
         for (int s = 0; s < k.ss_cap; ++s)
             if (ln[s] >= 0) { const int n2 = (ln[s] == it - 1) ? it : ln[s]; if (key_less(tm[s], n2, T, lapno)) ++rank; }
-        if (rank >= k.numSS_it) return -1;                       // never selected (PC.py:395) -> not stored
+        if (rank >= nit) return -1;                              // never selected (PC.py:395) -> not stored
         for (int s = 0; s < k.ss_cap; ++s) if (ln[s] == it - 1) ln[s] = it;
     }
     int slot = -1;
@@ -57,7 +62,7 @@ __device__ inline int book_ss_add(const LapBooks& k, int b, int T, bool import) 
             if (import && ln[s] == it) continue;                 // the own latest lap stays
             int rank = key_less(T, lapno, tm[s], ln[s]) ? 1 : 0;
             for (int j = 0; j < k.ss_cap; ++j) if (j != s && key_less(tm[j], ln[j], tm[s], ln[s])) ++rank;
-            if (rank < k.numSS_it) continue;                     // one of the fastest: keep
+            if (rank < nit) continue;                            // one of the fastest: keep
             if (slot < 0 || tm[s] > vt || (tm[s] == vt && ln[s] < vn)) { slot = s; vt = tm[s]; vn = ln[s]; }
         }
         if (slot < 0) {                                          // nothing filed: the own latest lap keeps its number
@@ -99,16 +104,17 @@ __device__ inline int book_md_add(const LapBooks& k, int b, int T) {
     return slot;
 }
 
-// What the next lap reads: the numSS_it fastest safe-set laps in argsort order, which of them is lap it-1, the slot addPoint
-// extends, and usedIt of the regression model.  Returns 0, or 8 when fewer than numSS_it laps are stored (the reference
-// raises IndexError at PC.py:402-403).
-__device__ inline int book_refresh(const LapBooks& k, int b) {
+// What the next lap reads: the nit fastest safe-set laps in argsort order (nit: the controller's numSS_it), which of them is lap
+// it-1, the slot addPoint extends, and usedIt of the regression model.  Returns 0, or 8 when fewer than nit laps are stored (the
+// reference raises IndexError at PC.py:402-403).  Entries nit .. k.numSS_it-1 of sel repeat the last selected slot and those of
+// isprev are 0: K2 reads none of them, and a snapshot packs them as they are.
+__device__ inline int book_refresh(const LapBooks& k, int b, int nit) {
     const int* tm = k.ss_time + (size_t)b * k.ss_cap;
     const int* ln = k.ss_lap + (size_t)b * k.ss_cap;
     const int it = k.it[b];
     int flag = 0, prev = -1, last = 0;
     for (int s = 0; s < k.ss_cap; ++s) if (it > 0 && ln[s] == it - 1) prev = s;   // it = 0: no lap (a free slot has ln = -1)
-    for (int c = 0; c < k.numSS_it; ++c) {
+    for (int c = 0; c < nit; ++c) {
         int best = -1;
         for (int s = 0; s < k.ss_cap; ++s) {
             if (ln[s] < 0) continue;
@@ -120,6 +126,7 @@ __device__ inline int book_refresh(const LapBooks& k, int b) {
         k.sel[(size_t)b * k.numSS_it + c] = best;
         k.isprev[(size_t)b * k.numSS_it + c] = (it > 0 && ln[best] == it - 1) ? 1 : 0;
     }
+    for (int c = nit; c < k.numSS_it; ++c) { k.sel[(size_t)b * k.numSS_it + c] = last; k.isprev[(size_t)b * k.numSS_it + c] = 0; }
     k.prevslot[b] = prev;
     const int* mt = k.md_time + (size_t)b * k.md_cap;
     const int* ms = k.md_seq + (size_t)b * k.md_cap;
@@ -139,24 +146,27 @@ __device__ inline int book_refresh(const LapBooks& k, int b) {
 }
 
 // The selection of tables written from outside (lmpc_books_set): book_refresh of every controller.  One thread per controller.
-__global__ void books_refresh_kernel(int batch, LapBooks k) {
+template <bool LAPS>
+__global__ void books_refresh_kernel(int batch, LapBooks k, SsLaps laps) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b < batch) book_refresh(k, b);
+    if (b < batch) book_refresh(k, b, book_laps<LAPS>(k, laps, b));
 }
 
 // Lap hand-over of every controller whose lap just ended (done[b] != 0), bookkeeping included: main.py:113-119
 // (lmpc.addTrajectory + predictiveModel.addTrajectory of the lap Simulator.sim returned), SysModel.py:50 (s -= TrackLength),
 // PC.py:445 (timeStep = 0).  One CTA per controller; no host involvement.
+template <bool LAPS>
 __global__ void __launch_bounds__(256) commit_laps_books_kernel(int batch, LapPool ss, LapPool model, LapBooks k, const double* cl_x,
                                                                 const double* cl_u, int* cl_len, int Tcl, double* x_cur, int* timeStep,
-                                                                int* done, int* flags_or, Tracks trk, int lmpc, LapBudget retire) {
+                                                                int* done, int* flags_or, Tracks trk, int lmpc, LapBudget retire,
+                                                                SsLaps laps) {
     const int b = blockIdx.x;
     if (b >= batch || retire.retired(b) || !done[b]) return;
     __shared__ int s_ss, s_md;
     const int Trec = cl_len[b];
     const double TrackLength = trk.of(b).TrackLength;
     if (threadIdx.x == 0) {
-        s_ss = lmpc ? book_ss_add(k, b, Trec, false) : -1;       // ordered by the lap time; rows beyond Tmax are not stored
+        s_ss = lmpc ? book_ss_add(k, b, Trec, false, book_laps<LAPS>(k, laps, b)) : -1;   // ordered by the lap time; rows beyond Tmax are not stored
         s_md = book_md_add(k, b, Trec);
         const int n = k.lap_n[b];
         if (n < LAP_HIST) k.lap_hist[(size_t)b * LAP_HIST + n] = Trec;
@@ -169,7 +179,7 @@ __global__ void __launch_bounds__(256) commit_laps_books_kernel(int batch, LapPo
     if (s_md >= 0) copy_lap_block(model, model.lap_index(b, s_md), cx, cu, Trec);
     __syncthreads();
     if (threadIdx.x == 0) {
-        int f = book_refresh(k, b);
+        int f = book_refresh(k, b, book_laps<LAPS>(k, laps, b));
         if (s_ss == -2) f |= 64;                                 // safe-set pool too small for numSS_it + 2 laps
         if (f && flags_or) flags_or[b] |= f;
         restart_record(b, cl_len, x_cur, timeStep, done, TrackLength);
@@ -177,10 +187,11 @@ __global__ void __launch_bounds__(256) commit_laps_books_kernel(int batch, LapPo
 }
 
 // main.py:99-110 with device bookkeeping: the record every controller just drove becomes `copies` laps of both stores.
+template <bool LAPS>
 __global__ void __launch_bounds__(256) seed_books_kernel(int batch, LapPool ss, LapPool model, LapBooks k, int copies, const double* cl_x,
                                                          const double* cl_u, int* cl_len, int Tcl, int N, double* xLin, double* uLin,
                                                          double* zt, double* OldInput, int* timeStep, int* hasPred, int* done,
-                                                         Tracks trk, int lmpc, Shapes shp) {
+                                                         Tracks trk, int lmpc, Shapes shp, SsLaps laps) {
     const int b = blockIdx.x;
     if (b >= batch) return;
     __shared__ int s_ss, s_md;
@@ -196,7 +207,7 @@ __global__ void __launch_bounds__(256) seed_books_kernel(int batch, LapPool ss, 
     __syncthreads();
     for (int c = 0; c < copies; ++c) {
         if (threadIdx.x == 0) {
-            s_ss = lmpc ? book_ss_add(k, b, Trec, false) : -1;
+            s_ss = lmpc ? book_ss_add(k, b, Trec, false, book_laps<LAPS>(k, laps, b)) : -1;
             s_md = book_md_add(k, b, Trec);
         }
         __syncthreads();
@@ -205,7 +216,7 @@ __global__ void __launch_bounds__(256) seed_books_kernel(int batch, LapPool ss, 
         __syncthreads();
     }
     seed_state_block(b, N, shp, cx, cu, xLin, uLin, zt, OldInput);
-    if (threadIdx.x == 0) { book_refresh(k, b); timeStep[b] = 0; hasPred[b] = 0; cl_len[b] = 0; done[b] = 0; }
+    if (threadIdx.x == 0) { book_refresh(k, b, book_laps<LAPS>(k, laps, b)); timeStep[b] = 0; hasPred[b] = 0; cl_len[b] = 0; done[b] = 0; }
 }
 
 // ---- pooled safe-set exchange (SURVEY §8e) -------------------------------------------------------------------------------
@@ -313,11 +324,12 @@ __global__ void __launch_bounds__(64) pool_rank_kernel(int n_src, const int* met
 // PredictiveModel.addTrajectory of a lap another controller drove, main.py:117-119), filed before its own latest lap.  A lap
 // is ordered by its lap time lt in both tables, as an own lap by Trec; only the rows that fit are stored.  The regression model
 // takes the lap also when the safe set drops it: main.py adds every lap to both lists, and with trToUse > numSS_it a lap outside
-// the numSS_it fastest can be among the trToUse shortest.  A controller with no lap of its own (it = 0) takes nothing.  One CTA
-// per controller.
+// the numSS_it fastest can be among the trToUse shortest.  A controller with no lap of its own (it = 0) takes nothing.  The
+// importer ranks a lap against its own numSS_it (LAPS), so a group may mix lap counts.  One CTA per controller.
+template <bool LAPS>
 __global__ void __launch_bounds__(256) pool_import_kernel(int batch, LapPool ss, LapPool model, LapBooks k, int share, int Tpad,
                                                           const double* rows, const int* meta, const int* grp, const int* order,
-                                                          const int* cnt, long long gid_base, int* took, int* flags_or) {
+                                                          const int* cnt, long long gid_base, int* took, int* flags_or, SsLaps laps) {
     const int b = blockIdx.x;
     if (b >= batch) return;
     __shared__ int s_ss, s_md, s_src;
@@ -332,7 +344,7 @@ __global__ void __launch_bounds__(256) pool_import_kernel(int batch, LapPool ss,
         ++given;
         if (threadIdx.x == 0) {
             s_src = src;
-            s_ss = book_ss_add(k, b, lt, true);
+            s_ss = book_ss_add(k, b, lt, true, book_laps<LAPS>(k, laps, b));
             s_md = -1;
             if (s_ss != -2 && k.it[b] > 0) s_md = book_md_add(k, b, lt);
         }
@@ -345,7 +357,7 @@ __global__ void __launch_bounds__(256) pool_import_kernel(int batch, LapPool ss,
         __syncthreads();
         if (threadIdx.x == 0 && c_ss == -2 && flags_or) flags_or[b] |= 64;
     }
-    if (threadIdx.x == 0 && given > 0) book_refresh(k, b);
+    if (threadIdx.x == 0 && given > 0) book_refresh(k, b, book_laps<LAPS>(k, laps, b));
 }
 
 // Progress of a Monte-Carlo batch in four numbers per pool group, so that the host only polls a few bytes every few steps:

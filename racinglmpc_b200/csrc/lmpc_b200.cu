@@ -140,6 +140,8 @@ struct lmpc_handle {
     struct ShapeCell { int N, M, off, n; };
     std::vector<ShapeCell> shp_cells;
     HandleTable<FtocpConstRec> own_c;
+    // per-controller safe-set lap counts (lmpc_set_ss_laps), or none: the handle's numSS_it
+    HandleTable<SsLapsRec> ssl;
     LapPool ss, mdl;
     int *d_used, *d_sel, *d_isprev, *d_prevslot, *d_timeStep, *d_hasPred, *d_flags, *d_minidx, *d_xchg, *d_health, *d_dropped;
     double *d_xLin, *d_uLin, *d_ztState, *d_ztFixed, *d_OldInput, *d_xPredPrev, *d_tmpx, *d_tmpu;
@@ -260,7 +262,7 @@ static void free_tables(lmpc_handle* h, unsigned owners) {
     };
     release(h->sets, OWN_HANDLE); release(h->veh, OWN_HANDLE); release(h->noise, OWN_HANDLE); release(h->streams, OWN_HANDLE);
     release(h->meas, OWN_HANDLE); release(h->budget, OWN_HANDLE); release(h->trk, OWN_STORE); release(h->reg, OWN_STORE); release(h->pool_grp, OWN_STORE);
-    release(h->shp, OWN_STORE); release(h->shp_order, OWN_STORE); release(h->own_c, OWN_HANDLE);
+    release(h->shp, OWN_STORE); release(h->shp_order, OWN_STORE); release(h->own_c, OWN_HANDLE); release(h->ssl, OWN_STORE);
     if (owners & OWN_STORE) h->shp_cells.clear();
 }
 
@@ -938,6 +940,7 @@ int lmpc_sizeof_noise_params(void) { return (int)sizeof(lmpc_noise_params); }
 int lmpc_sizeof_measurement_params(void) { return (int)sizeof(lmpc_measurement_params); }
 int lmpc_sizeof_regression_params(void) { return (int)sizeof(lmpc_regression_params); }
 int lmpc_sizeof_shape_params(void) { return (int)sizeof(lmpc_shape_params); }
+int lmpc_sizeof_ss_laps_params(void) { return (int)sizeof(lmpc_ss_laps_params); }
 int lmpc_sizeof_track_params(void) { return (int)sizeof(lmpc_track_params); }
 
 static int store_create_impl(lmpc_handle* h, const lmpc_model_params* mp, int ss_cap, int model_cap, int Tmax);
@@ -1118,6 +1121,12 @@ static bool on_grid(int N, int M) {
     return false;
 }
 
+// numSS_it / numSS_Points of controller b: its row of the lap-count / shape table, or the handle's
+static int laps_of(const lmpc_handle* h, int b) { return h->ssl.tab ? h->ssl.rows[h->ssl.index[b]].numSS_it : h->p.numSS_it; }
+static int points_of(const lmpc_handle* h, int b) { return h->shp.tab ? h->shp.rows[h->shp.index[b]].numSS_Points : h->M; }
+// M points split into nit laps of an even number of points each (PC.py:403,492-495)
+static bool even_split(int M, int nit) { return M % nit == 0 && (M / nit) % 2 == 0; }
+
 // Per-controller shapes: every set checked against the grid and the handle, the shaped kernels of every set opted into their
 // shared-memory size, then the table and the sorted instance list (DESIGN.md, "Per-controller horizons and safe-set sizes");
 // nsets == 0 returns to the handle's own shape.
@@ -1128,6 +1137,15 @@ int lmpc_set_shapes(lmpc_handle* h, const lmpc_shape_params* sets, int nsets, co
     if (h->laps_stored) return fail(LMPC_E_STATE, std::string(who) + ": laps are stored already; install shapes before the first lap");
     if (h->p.warm_start) return fail(LMPC_E_STATE, std::string(who) + ": the handle was created with warm_start; its records are laid out per (N, M)");
     const int nit = h->p.numSS_it;
+    if (h->ssl.tab) {                   // every controller's numSS_Points against its own numSS_it (lmpc_set_ss_laps)
+        if ((rc = check_set_index(h, who, sets, nsets, set_of_instance)) != LMPC_OK) return rc;
+        for (int b = 0; b < h->batch; ++b) {
+            const int m = nsets ? sets[set_of_instance[b]].numSS_Points : h->M;
+            if (!even_split(m, laps_of(h, b)))
+                return fail(LMPC_E_INVALID, std::string(who) + ": controller " + std::to_string(b) + ": numSS_Points " + std::to_string(m) +
+                                                " is not its numSS_it (" + std::to_string(laps_of(h, b)) + ") times an even number of points per lap");
+        }
+    }
     rc = install_table(h, who, h->shp, sets, nsets, set_of_instance, (const ShapeRec*)nullptr, [&](int k, ShapeRec& row) {
         const lmpc_shape_params& s = sets[k];
         const std::string w = std::string(who) + ": set " + std::to_string(k) + ": ";
@@ -1136,7 +1154,7 @@ int lmpc_set_shapes(lmpc_handle* h, const lmpc_shape_params* sets, int nsets, co
             return fail(LMPC_E_INVALID, w + "N and numSS_Points must not exceed the handle's (" + std::to_string(h->N) + ", " +
                                             std::to_string(h->M) + ")");
         if ((s.numSS_Points > 0) != (h->M > 0)) return fail(LMPC_E_INVALID, w + "numSS_Points must be > 0 exactly when the handle's is");
-        if (s.numSS_Points > 0 && (s.numSS_Points % nit || (s.numSS_Points / nit) % 2))
+        if (!h->ssl.tab && s.numSS_Points > 0 && !even_split(s.numSS_Points, nit))
             return fail(LMPC_E_INVALID, w + "numSS_Points must be a multiple of numSS_it with an even number of points per lap");
         const cudaError_t e = ftocp_shaped_configure(s.N, s.numSS_Points);
         if (e != cudaSuccess) return fail(LMPC_E_CUDA, w + cudaGetErrorString(e));
@@ -1162,6 +1180,33 @@ int lmpc_set_shapes(lmpc_handle* h, const lmpc_shape_params* sets, int nsets, co
         g_err = msg;
     }
     return rc;
+}
+
+// Per-controller safe-set lap counts: every set checked against the handle, every controller's numSS_Points against its value,
+// then the table (DESIGN.md, "Per-controller safe-set lap counts"); nsets == 0 returns to the handle's numSS_it.
+int lmpc_set_ss_laps(lmpc_handle* h, const lmpc_ss_laps_params* sets, int nsets, const int* set_of_instance) {
+    static const char* who = "lmpc_set_ss_laps";
+    int rc = need_store(h);
+    if (rc) return rc;
+    if (h->laps_stored) return fail(LMPC_E_STATE, std::string(who) + ": laps are stored already; install lap counts before the first lap");
+    if (h->M <= 0) return fail(LMPC_E_INVALID, std::string(who) + ": the handle has no safe set (numSS_Points == 0)");
+    if ((rc = check_set_index(h, who, sets, nsets, set_of_instance)) != LMPC_OK) return rc;
+    const int nit = h->p.numSS_it;
+    for (int k = 0; k < nsets; ++k)
+        if (sets[k].numSS_it < 1 || sets[k].numSS_it > nit)
+            return fail(LMPC_E_INVALID, std::string(who) + ": set " + std::to_string(k) + ": numSS_it must be 1 .. the handle's " +
+                                            std::to_string(nit));
+    for (int b = 0; b < h->batch; ++b) {       // nsets == 0: the handle's numSS_it against the installed shapes
+        const int v = nsets ? sets[set_of_instance[b]].numSS_it : nit;
+        if (!even_split(points_of(h, b), v))
+            return fail(LMPC_E_INVALID, std::string(who) + ": controller " + std::to_string(b) + ": its numSS_Points " +
+                                            std::to_string(points_of(h, b)) + " is not numSS_it (" + std::to_string(v) +
+                                            ") times an even number of points per lap");
+    }
+    return install_table(h, who, h->ssl, sets, nsets, set_of_instance, (const SsLapsRec*)nullptr, [&](int k, SsLapsRec& row) {
+        row = sets[k];
+        return LMPC_OK;
+    });
 }
 
 static int put_lap(lmpc_handle* h, LapPool& pool, int inst, int slot, int T, const double* x, const double* u) {
@@ -1321,7 +1366,8 @@ static int launch_k2(lmpc_handle* h, const double* d_x0, LapBudget retire = {}) 
     a.zt_fixed = h->d_ztFixed; a.status = h->d_flags; a.min_index = h->d_minidx;
     a.retire = retire;
     a.shp = h->shp.view();
-    (h->shp.tab ? ss_select_kernel<true> : ss_select_kernel<false>)<<<h->batch, 32 * a.numSS_it, 0, h->stream>>>(a);
+    a.laps = h->ssl.view();
+    (h->shp.tab || h->ssl.tab ? ss_select_kernel<true> : ss_select_kernel<false>)<<<h->batch, 32 * a.numSS_it, 0, h->stream>>>(a);
     CK(cudaGetLastError());
     h->launches += 1;
     return LMPC_OK;
@@ -1859,7 +1905,8 @@ int lmpc_books_set(lmpc_handle* h, const int* ss_time, const int* ss_lap, const 
                                                    {k.md_seq, md_seq}, {k.md_cnt, md_cnt}})))
         return rc;
     CK(cudaMemsetAsync(k.lap_n, 0, sizeof(int) * h->batch, h->stream));
-    books_refresh_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->batch, k);   // sel, is_prev, prev_slot, used of these tables
+    // sel, is_prev, prev_slot, used of these tables
+    (h->ssl.tab ? books_refresh_kernel<true> : books_refresh_kernel<false>)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->batch, k, h->ssl.view());
     CK(cudaGetLastError());
     h->launches += 1;
     CK(cudaStreamSynchronize(h->stream));
@@ -1883,9 +1930,9 @@ int lmpc_books_get(lmpc_handle* h, int* ss_time, int* ss_lap, int* it, int* md_t
 int lmpc_rollout_commit_laps_dev(lmpc_handle* h) {
     if (int rc = need_rollout(h)) return rc;
     h->laps_stored = true;     // enqueue only: which controllers finish a lap is not known here
-    commit_laps_books_kernel<<<h->batch, 256, 0, h->stream>>>(h->batch, h->ss, h->mdl, h->bk, h->d_clx, h->d_clu, h->d_cllen, h->Tcl,
-                                                              h->d_rx[h->cur], h->d_timeStep, h->d_done, h->d_health, tracks(h),
-                                                              h->M > 0 ? 1 : 0, lap_budget(h));
+    (h->ssl.tab ? commit_laps_books_kernel<true> : commit_laps_books_kernel<false>)<<<h->batch, 256, 0, h->stream>>>(
+        h->batch, h->ss, h->mdl, h->bk, h->d_clx, h->d_clu, h->d_cllen, h->Tcl, h->d_rx[h->cur], h->d_timeStep, h->d_done, h->d_health,
+        tracks(h), h->M > 0 ? 1 : 0, lap_budget(h), h->ssl.view());
     CK(cudaGetLastError());
     h->launches += 1;
     return LMPC_OK;
@@ -1896,9 +1943,9 @@ int lmpc_rollout_seed_from_record_dev(lmpc_handle* h, int copies) {
     if (copies < 1 || (h->M > 0 && copies > h->ss.cap) || copies > h->mdl.cap) return fail(LMPC_E_INVALID, "seed copies do not fit the lap pools");
     h->laps_stored = true;
     if (h->d_warm_valid) CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * h->batch, h->stream));
-    seed_books_kernel<<<h->batch, 256, 0, h->stream>>>(h->batch, h->ss, h->mdl, h->bk, copies, h->d_clx, h->d_clu, h->d_cllen, h->Tcl, h->N,
-                                                       h->d_xLin, h->d_uLin, h->d_ztState, h->d_OldInput, h->d_timeStep, h->d_hasPred,
-                                                       h->d_done, tracks(h), h->M > 0 ? 1 : 0, h->shp.view());
+    (h->ssl.tab ? seed_books_kernel<true> : seed_books_kernel<false>)<<<h->batch, 256, 0, h->stream>>>(
+        h->batch, h->ss, h->mdl, h->bk, copies, h->d_clx, h->d_clu, h->d_cllen, h->Tcl, h->N, h->d_xLin, h->d_uLin, h->d_ztState,
+        h->d_OldInput, h->d_timeStep, h->d_hasPred, h->d_done, tracks(h), h->M > 0 ? 1 : 0, h->shp.view(), h->ssl.view());
     CK(cudaGetLastError());
     h->launches += 1;
     return LMPC_OK;
@@ -1985,8 +2032,9 @@ int lmpc_pool_import_dev(lmpc_handle* h, int n_src, int share, int Tpad, long lo
     int* took = h->d_poolidx + POOL_TOOK;
     CK(cudaMemsetAsync(took, 0, sizeof(int), h->stream));
     pool_rank_kernel<<<G, 64, 0, h->stream>>>(n_src, meta_dev, order, cnt);
-    pool_import_kernel<<<h->batch, 256, 0, h->stream>>>(h->batch, h->ss, h->mdl, h->bk, share, Tpad, rows_dev, meta_dev, h->pool_grp.idx, order,
-                                                        cnt, gid_base, took, h->has_rollout ? h->d_health : nullptr);
+    (h->ssl.tab ? pool_import_kernel<true> : pool_import_kernel<false>)<<<h->batch, 256, 0, h->stream>>>(
+        h->batch, h->ss, h->mdl, h->bk, share, Tpad, rows_dev, meta_dev, h->pool_grp.idx, order, cnt, gid_base, took,
+        h->has_rollout ? h->d_health : nullptr, h->ssl.view());
     CK(cudaGetLastError());
     h->launches += 2;
     if (took_host) {

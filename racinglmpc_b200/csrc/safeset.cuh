@@ -50,6 +50,14 @@ using Shapes = Table<ShapeRec>;
 // K1, K2 and the state shift come in two instantiations, SHAPED = a table is installed: without one the kernels are the code they
 // were before shapes existed (a branch on a null table cost the closed loop of configs[3] about 1 %)
 __device__ __forceinline__ int horizon_of(const Shapes& s, int b, int N) { return s.tab ? s.of(b).N : N; }
+__device__ __forceinline__ int ss_points_of(const Shapes& s, int b, int M) { return s.tab ? s.of(b).numSS_Points : M; }
+
+// The safe-set lap count numSS_it_b of every controller (lmpc_set_ss_laps), or no table (tab == null) for the handle's numSS_it,
+// which stays the stride of sel / is_prev / min_index and K2's block size.  K2 takes SHAPED when either table is installed; the
+// lap-book kernels (lapbooks.cuh) have their own LAPS instantiation, so without a table both are the code they were before.
+using SsLapsRec = lmpc_ss_laps_params;
+using SsLaps = Table<SsLapsRec>;
+__device__ __forceinline__ int ss_laps_of(const SsLaps& l, int b, int nit) { return l.tab ? l.of(b).numSS_it : nit; }
 
 struct LapPool {
     double* x;      // [B][cap][Tmax][6]
@@ -524,7 +532,7 @@ __global__ void __launch_bounds__(32 * K1_MAXWPB, LMPC_K1_MINBLOCKS) knn_ltv_reg
 
 // ------------------------------------------------------------------------------------------------
 struct K2Args {
-    int batch, N, numSS_it, P;   // P = numSS_Points / numSS_it (the handle's; a shaped controller has P_b = M_b / numSS_it)
+    int batch, N, numSS_it, P;   // P = numSS_Points / numSS_it (the handle's; under SHAPED controller b has P_b = M_b / numSS_it_b)
     Tracks trk;
     const double* x0;        // [B][6]
     const double* zt;        // [B][6]
@@ -543,9 +551,10 @@ struct K2Args {
     int* min_index;          // [B][numSS_it] argmin row (for tests)
     LapBudget retire;        // the CTA of a retired controller selects nothing
     Shapes shp;              // N_b and M_b of every controller: the [6,M_b] block at the start of the controller's [6,M] region
+    SsLaps laps;             // numSS_it_b of every controller: warps c >= numSS_it_b select nothing
 };
 
-// One CTA per instance, one warp per selected lap.
+// One CTA per instance, one warp per selected lap.  SHAPED: a shape table or a lap-count table (or both) is installed.
 template <bool SHAPED>
 __global__ void __launch_bounds__(32 * 8) ss_select_kernel(const K2Args a) {
     const int b = blockIdx.x;
@@ -553,7 +562,9 @@ __global__ void __launch_bounds__(32 * 8) ss_select_kernel(const K2Args a) {
     const int lane = threadIdx.x & 31;
     if (b >= a.batch || c >= a.numSS_it || a.retire.retired(b)) return;
     const int Mh = a.P * a.numSS_it;                         // the handle's M: the per-controller stride of the outputs
-    const int M = SHAPED ? a.shp.of(b).numSS_Points : Mh, P = SHAPED ? M / a.numSS_it : a.P, Nb = SHAPED ? a.shp.of(b).N : a.N;
+    const int nit = SHAPED ? ss_laps_of(a.laps, b, a.numSS_it) : a.numSS_it;
+    if (SHAPED && c >= nit) return;                          // uniform over the warp; K2 has no block barrier
+    const int M = SHAPED ? ss_points_of(a.shp, b, Mh) : Mh, P = SHAPED ? M / nit : a.P, Nb = SHAPED ? horizon_of(a.shp, b, a.N) : a.N;
     const double TrackLength = a.trk.of(b).TrackLength;
     // lap-wrap fix of the terminal guess (PC.py:392-393)
     double z[6];

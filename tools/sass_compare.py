@@ -4,6 +4,10 @@
 Kernels are matched by variant and (N, M) across their old and new names:
   uniform  ftocp_kernel<N, M, 2, 4>  or  ftocp_kernel<N, M, 2, 4, false>
   sets     ftocp_sets_kernel<N, M, 2, 4>  or  ftocp_kernel<N, M, 2, 4, true>
+and the instantiations that run without a per-controller table of the other kernels of a step and of the lap books, matched
+across their untemplated names:
+  default  knn_ltv_regress_kernel, ss_select_kernel, shift_state_kernel (<false>: no shape or lap-count table) and
+           books_refresh_kernel, commit_laps_books_kernel, seed_books_kernel, pool_import_kernel (<false>: no lap-count table)
 and compared by instruction text (cuobjdump -sass without addresses and encodings).  Each differing line pair is classified:
   dfma-swap   one DFMA with its two factors exchanged (a*b+c = b*a+c)
   lds-swap    LDS.128 loads of unchanged addresses whose destination registers are permuted among themselves
@@ -19,6 +23,8 @@ import subprocess
 import sys
 
 NAME = re.compile(r"^(?:void )?(ftocp_kernel|ftocp_sets_kernel)<(\d+), (\d+), 2, 4(?:, (true|false))?>")
+DEFAULT = re.compile(r"^(?:void )?lmpc::(knn_ltv_regress_kernel|ss_select_kernel|shift_state_kernel|books_refresh_kernel|"
+                     r"commit_laps_books_kernel|seed_books_kernel|pool_import_kernel)(<false>)?\(")
 
 
 def kernels(path):
@@ -30,10 +36,13 @@ def kernels(path):
         if m:
             name = subprocess.run(["c++filt", m.group(1)], capture_output=True, text=True).stdout.strip()
             k = NAME.match(name)
+            d = DEFAULT.match(name)
             cur = None
             if k:
                 sets = k.group(1) == "ftocp_sets_kernel" or k.group(4) == "true"
                 cur = out.setdefault(("sets" if sets else "uniform", int(k.group(2)), int(k.group(3))), [])
+            elif d:
+                cur = out.setdefault(("default", d.group(1), 0), [])
             continue
         m = re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(.*?)\s*;", line)
         if m and cur is not None:
@@ -79,15 +88,16 @@ def main(old, new):
     totals = collections.defaultdict(collections.Counter)
     for key in sorted(set(ko) | set(kn)):
         variant, n, m = key
+        label = ("%-24s" % n) if variant == "default" else "<%2d,%2d>" % (n, m)
         if key not in ko or key not in kn:
-            print("%-7s <%2d,%2d>  only in %s" % (variant, n, m, "new" if key in kn else "old"))
+            print("%-7s %s  only in %s" % (variant, label, "new" if key in kn else "old"))
             totals[variant]["unmatched"] += 1
             continue
         c = compare(ko[key], kn[key])
         verdict = "identical" if not c else ("other" if c["other"] else "+".join(sorted(c)))
         totals[variant][verdict] += 1
-        print("%-7s <%2d,%2d>  %5d instructions  %s%s" % (variant, n, m, len(kn[key]), verdict,
-                                                         "" if not c else "  (" + ", ".join("%s %d" % kv for kv in sorted(c.items())) + " lines)"))
+        print("%-7s %s  %5d instructions  %s%s" % (variant, label, len(kn[key]), verdict,
+                                                  "" if not c else "  (" + ", ".join("%s %d" % kv for kv in sorted(c.items())) + " lines)"))
     for variant, t in sorted(totals.items()):
         print("%s: %d kernels: %s" % (variant, sum(t.values()), ", ".join("%d %s" % (v, k) for k, v in sorted(t.items()))))
 
