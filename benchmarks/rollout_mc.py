@@ -61,21 +61,40 @@ def handle_shape(shape_sets=None):
     return cover[0]
 
 
-def layout(warm=False, shape_sets=None):
-    """The snapshot layout (BatchedController.snapshot_layout without "bytes") of run()'s controllers."""
+def layout(warm=False, shape_sets=None, lap_reports=None):
+    """The snapshot layout (BatchedController.snapshot_layout without "bytes") of run()'s controllers; "lap_reports" only when
+    reports are on."""
     numSS_it = rp.lmpc_params(N_HORIZON)[0]
     N, numSS_Points = handle_shape(shape_sets)
-    return dict(N=N, M=numSS_Points, ncx=2, ncu=4, numSS_it=numSS_it, trToUse=TR_TO_USE, ss_cap=SS_CAP, model_cap=MODEL_CAP,
-                Tmax=TMAX, Tcl=TCL, warm_start=int(bool(warm)))
+    out = dict(N=N, M=numSS_Points, ncx=2, ncu=4, numSS_it=numSS_it, trToUse=TR_TO_USE, ss_cap=SS_CAP, model_cap=MODEL_CAP,
+               Tmax=TMAX, Tcl=TCL, warm_start=int(bool(warm)))
+    if lap_reports:
+        out["lap_reports"] = int(lap_reports)
+    return out
+
+
+def check_lap_reports(lap_reports, laps):
+    """The refusals of run(lap_reports=...), before any device work: None needs laps <= 16 (lap_hist's length), else an integer
+    capacity L with laps <= L <= 1024.  Returns L, or 0 for no reports."""
+    if lap_reports is None:
+        if int(laps) > 16:
+            raise ValueError("laps = %d: the lap books keep the lengths of 16 laps; pass lap_reports >= laps to report longer runs"
+                             % int(laps))
+        return 0
+    L = _native.check_lap_reports(lap_reports)
+    if L < max(int(laps), 1):
+        raise ValueError("lap_reports = %d keeps fewer rows than the %d laps of the run" % (L, int(laps)))
+    return L
 
 
 def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, poll=8, max_steps=0, seed=1234, local=None, warm=False,
         final=None, param_sets=None, vehicle_sets=None, books=None, track_sets=None, pool_groups=None, readiness="batch",
         capture=None, start=None, noise_sets=None, noise_streams=None, regression_sets=None, lap_budget=None, measurement_sets=None,
-        shape_sets=None, ss_laps_sets=None):
+        shape_sets=None, ss_laps_sets=None, lap_reports=None):
     """One Monte-Carlo run on this rank's GPU (torch.distributed may or may not be initialised).  Returns a dict (all ranks).
     final: None, or a dict that receives the closed loop's end state (rollout_state) and the last step's solver report (step_results).
-    books: None, or a dict that receives the lap books (books) and the health counters (flags_or, unsolved).
+    books: None, or a dict that receives the lap books (books) and the health counters (flags_or, unsolved), and with lap_reports
+    the reports (BatchedController.lap_reports) under "lap_reports".
     param_sets: None, or (params, index, QterminalSlack) handed to BatchedController.set_param_sets after construction (a
     parameter sweep over the batch; the result then holds per-set lap statistics under "per_set_rank0").
     vehicle_sets: None, or (vehicles, index) handed to BatchedController.set_vehicles (a sweep over the plant, PID lap included; the
@@ -148,7 +167,14 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     retired when the group last exchanged ("retired_before_last_exchange_rank0"): a retired controller's last lap never ships
     (nobody drives its rows past the finish line), so the exchange equals the run without a budget exactly when that is False
     everywhere.  capture records the budget; start refuses a budget below the captured one for any controller (raising it revives
-    the controller where it stopped, with the noise draws of the later clock)."""
+    the controller where it stopped, with the noise draws of the later clock).
+    lap_reports: None, or the report capacity L >= laps (BatchedController.enable_lap_reports, enabled before the PID lap): every
+    controller then files one report per lap (steps, flags, unsolved QPs, lane violations of its plant state, interior-point
+    iterations).  The result gains "lap_reports_rank0", a summary per lap (lap_report_summary), every per-table entry gains the same
+    list under "reports", and "lap_stats_rank0" covers every lap, taken from the reports' steps (equal to the lap books' lengths
+    wherever no step found the record full, flag 256).  Without reports laps is at most 16, the laps the lap books keep.  capture
+    records L and start refuses another.  ValueError before any device work."""
+    L = check_lap_reports(lap_reports, laps)
     budget = _native.make_lap_budget(lap_budget, int(batch))       # ValueError where set_lap_budget would refuse, before any device work
     N, M = handle_shape(shape_sets)
     numSS_it = rp.lmpc_params(N)[0]
@@ -161,7 +187,7 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     if ss_laps_sets is not None:
         _native.make_ss_laps_sets(ss_laps_sets[0], ss_laps_sets[1], int(batch), numSS_it, points)
     if start is not None:
-        _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget, shape_sets)
+        _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget, shape_sets, L)
     if capture is not None and not isinstance(capture, dict):
         raise ValueError("capture is a dict that receives the run's end state")
     if readiness not in ("batch", "group"):
@@ -189,6 +215,8 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
                           numSS_it=numSS_it, QterminalSlack=Qts, device=local, Tmax=TMAX, ss_cap=SS_CAP, model_cap=MODEL_CAP,
                           warm_start=warm)
     c.enable_rollout(Tcl=TCL)                            # before the tables: the measurement noise belongs to the closed loop
+    if L:
+        c.enable_lap_reports(L)                          # before the PID lap (its record is consumed by the seeding, unreported)
     # the per-controller tables in the order they are installed: (arguments of the install call or None, install call, result key
     # of the per-row lap statistics or None)
     tables = ((param_sets, c.set_param_sets, "per_set_rank0"), (vehicle_sets, c.set_vehicles, "per_vehicle_rank0"),
@@ -289,11 +317,13 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
                        poll=poll, warm=bool(warm), pool_groups=G, layout=c.snapshot_layout(),
                        lap_budget=None if budget is None else budget.tolist())
     flags_or, unsolved = c.rollout_health()
+    reps = c.lap_reports() if L else None
+    lens, n_laps = (reps["steps"], reps["n"]) if L else (bk["lap_hist"], bk["lap_n"])
     stats = []
     for r in range(laps):
-        a = bk["lap_hist"][bk["lap_n"] > r, r]
+        a = lens[n_laps > r, r]
         a = a if a.size else np.array([0])
-        stats.append({"lap": r + 1, "n": int((bk["lap_n"] > r).sum()), "mean": float(a.mean()), "min": int(a.min()), "max": int(a.max())})
+        stats.append({"lap": r + 1, "n": int((n_laps > r).sum()), "mean": float(a.mean()), "min": int(a.min()), "max": int(a.max())})
     out = {"benchmark": "configs[3] LMPC Monte-Carlo rollouts", "mode": mode, "n_gpus": world, "batch_per_gpu": B,
            "closed_loop_steps": steps, "ms_total": ms, "controller_steps_per_s": B * world * (steps - sched.start_step) / (ms * 1e-3),
            "kernel_launches_rank0": int(c.kernel_launches - l0), "lap_stats_rank0": stats, "device_pid_laps_s": pid_s,
@@ -303,10 +333,13 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
            "ipm_iters_mean_sampled": it_sum / max(it_n, 1), "ipm_iters_max_sampled": it_max,
            "instances_with_flags_rank0": int((flags_or != 0).sum()), "flag_bits_rank0": int(np.bitwise_or.reduce(flags_or)),
            "unsolved_steps_rank0": int(unsolved.sum()), "late_accepts_rank0": c.late_accepts}
+    if L:
+        out["lap_reports"] = L
+        out["lap_reports_rank0"] = lap_report_summary(reps, np.ones(B, bool), laps)
     for args, _, key in tables:
         if args is not None and key is not None:
             idx = np.asarray(args[1]).reshape(B)
-            out[key] = [_set_stats(bk, flags_or, unsolved, idx == k, laps) for k in range(len(args[0]))]
+            out[key] = [_set_stats(bk, flags_or, unsolved, idx == k, laps, reps) for k in range(len(args[0]))]
     if shape_sets is not None:
         idx = np.asarray(shape_sets[1]).reshape(B)
         for k, s in enumerate(out["per_shape_rank0"]):
@@ -325,7 +358,7 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
                 for k, v in enumerate(ss_laps_sets[0]):
                     cell = (sidx == j) & (idx == k)
                     if cell.any():
-                        s = _set_stats(bk, flags_or, unsolved, cell, laps)
+                        s = _set_stats(bk, flags_or, unsolved, cell, laps, reps)
                         s.update(N=int(sh[0]), numSS_Points=int(sh[1]), numSS_it=int(v),
                                  ipm_iters_mean_sampled=float(it_ctrl[cell].mean() / max(it_n, 1)))
                         out["per_shape_ss_laps_rank0"].append(s)
@@ -355,7 +388,7 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         final.update(c.rollout_state())
         final.update(c.step_results())
     if books is not None:
-        books.update(bk, flags_or=flags_or, unsolved=unsolved)
+        books.update(bk, flags_or=flags_or, unsolved=unsolved, **({"lap_reports": reps} if L else {}))
     c.close()
     return out
 
@@ -367,9 +400,9 @@ def _driven_steps(bk, state):
     return int(filed.sum(dtype=np.int64) + state["cl_len"].sum(dtype=np.int64))
 
 
-def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget=None, shape_sets=None):
-    """The refusals of run(start=...), before any device work: a start that does not match this run, laps not above the
-    captured laps, or a lap budget below the captured one."""
+def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget=None, shape_sets=None, lap_reports=0):
+    """The refusals of run(start=...), before any device work: a start that does not match this run (report capacity included),
+    laps not above the captured laps, or a lap budget below the captured one."""
     if not isinstance(start, dict):
         raise ValueError("start is a capture dict of an earlier run")
     need = ("records", "clock") + sharding.ExchangeSchedule.FIELDS + ("batch", "laps", "mode", "readiness", "poll", "warm",
@@ -392,20 +425,47 @@ def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, b
     rec = start["records"]
     if getattr(rec, "shape", (None,))[0] != int(batch):
         raise ValueError("start holds %s records, this run has %d controllers" % (getattr(rec, "shape", ("no",))[0], int(batch)))
+    had = int(start["layout"].get("lap_reports", 0))
+    if had != int(lap_reports):
+        raise ValueError("start records have lap_reports = %d, this run %d" % (had, int(lap_reports)))
     for k, v in layout(warm, shape_sets).items():
         if int(start["layout"].get(k, -1)) != v:
             raise ValueError("start records have %s = %s, this run's controllers %d" % (k, start["layout"].get(k), v))
 
 
-def _set_stats(bk, flags_or, unsolved, sel, laps):
-    """Lap lengths (mean / min per LMPC lap), unsolved steps and flagged controllers of the controllers `sel` of one parameter set or vehicle."""
+def _set_stats(bk, flags_or, unsolved, sel, laps, reps=None):
+    """Lap lengths (mean / min per LMPC lap), unsolved steps and flagged controllers of the controllers `sel` of one parameter set or
+    vehicle; with reports (BatchedController.lap_reports) the lengths are the reports' steps and "reports" holds lap_report_summary."""
+    lens, n_laps = (reps["steps"], reps["n"]) if reps is not None else (bk["lap_hist"], bk["lap_n"])
     laps_out = []
     for r in range(laps):
-        m = sel & (bk["lap_n"] > r)
-        a = bk["lap_hist"][m, r]
+        m = sel & (n_laps > r)
+        a = lens[m, r]
         laps_out.append({"lap": r + 1, "n": int(m.sum()), "mean": float(a.mean()) if a.size else 0.0, "min": int(a.min()) if a.size else 0})
-    return {"controllers": int(sel.sum()), "laps": laps_out, "unsolved_steps": int(unsolved[sel].sum()),
-            "instances_with_flags": int((flags_or[sel] != 0).sum())}
+    out = {"controllers": int(sel.sum()), "laps": laps_out, "unsolved_steps": int(unsolved[sel].sum()),
+           "instances_with_flags": int((flags_or[sel] != 0).sum())}
+    if reps is not None:
+        out["reports"] = lap_report_summary(reps, sel, laps)
+    return out
+
+
+def lap_report_summary(reps, sel, laps):
+    """Per lap r < laps, over the controllers `sel` that filed a report of lap r (BatchedController.lap_reports): how many, their
+    steps (mean / min / max), how many violated a lane constraint at some step and the mean violating steps, the max and mean of
+    viol_max, the unsolved QPs in total and the interior-point iterations per step (total iterations over total steps)."""
+    out = []
+    for r in range(laps):
+        m = sel & (reps["n"] > r)
+        k = int(m.sum())
+        st, vs, vm = reps["steps"][m, r], reps["viol_steps"][m, r], reps["viol_max"][m, r]
+        tot = int(st.sum(dtype=np.int64))
+        out.append({"lap": r + 1, "controllers": k,
+                    "steps_mean": float(st.mean()) if k else 0.0, "steps_min": int(st.min()) if k else 0, "steps_max": int(st.max()) if k else 0,
+                    "violating": int((vs > 0).sum()), "viol_steps_mean": float(vs.mean()) if k else 0.0,
+                    "viol_max_max": float(vm.max()) if k else 0.0, "viol_max_mean": float(vm.mean()) if k else 0.0,
+                    "unsolved": int(reps["unsolved"][m, r].sum(dtype=np.int64)),
+                    "ipm_iters_per_step": float(reps["ipm_iters"][m, r].sum(dtype=np.int64)) / tot if tot else 0.0})
+    return out
 
 
 def main():

@@ -483,6 +483,39 @@ int lmpc_rollout_set_measurement_noise(lmpc_handle* h, const lmpc_measurement_pa
  *     files imported laps, and its last lap, which nobody extends past the finish line, never ships under
  *     lmpc_set_pool_min_overrun. */
 int lmpc_rollout_set_lap_budget(lmpc_handle* h, const int* budget_of_instance);
+/* Per-lap reports of the device closed loop (no reference counterpart; DESIGN.md, "Per-lap reports"): one row per lap a controller
+ * drives and hands over, accumulated on the device by the kernels every step already runs.  Over the steps of the lap: */
+typedef struct lmpc_lap_report {
+    int steps;                    /* closed-loop steps driven, including any that found the record full (flag 256) */
+    int flags;                    /* OR of the step flags and the simulator's bits: the rule of lmpc_rollout_get_health's flags_or */
+    int unsolved;                 /* steps whose QP status != 1: the rule of its unsolved_steps */
+    int viol_steps;               /* steps whose plant state x violates a row i of the controller's own Fx x <= bx (see below) */
+    int ipm_iters;                /* sum of the interior-point iterations of the steps' QPs */
+    int ipm_iters_max;            /* their maximum */
+    double viol_max;              /* max over the steps and rows of Fx[i] . x - bx[i]; -inf for a lap without steps */
+} lmpc_lap_report;
+/* lmpc_rollout_enable_lap_reports: keep up to max_laps (1 .. 1024) report rows per controller; 0 turns reports off and frees them.
+ *   - x is the plant state the step was driven from (the row the rollout trace records), never the measured state of
+ *     lmpc_rollout_set_measurement_noise.  Fx, bx are the controller's QP constants: its parameter-set row, else the handle's.
+ *     Row i is violated when d_i = (sum over j = 0..5, in order, of Fx[i][j] * x[j], fp64 without fused multiply-adds) - bx[i]
+ *     is > 0; viol_max = fmax over the d_i.  A step whose x has a non-finite entry counts as violated and sets viol_max = +inf.
+ *   - lmpc_rollout_step (modes 0, 1, 2) adds every field; lmpc_rollout_pid_step adds steps, flags and the violation fields only.
+ *     A retired controller (lap budget) adds nothing.
+ *   - The running row describes the record under way: a lap hand-over (lmpc_rollout_commit_laps_dev, lmpc_rollout_commit_laps)
+ *     files it as report n (stored when n < max_laps), counts n on and resets the row; the seeding (lmpc_rollout_seed_from_record,
+ *     lmpc_rollout_seed_from_record_dev) consumes the PID record without a report and starts the table afresh (n = 0).  Imported
+ *     laps (lmpc_pool_*) are not driven and file nothing.  lmpc_rollout_set_state does not restart the record or the row.
+ *   - Needs lmpc_rollout_create (LMPC_E_STATE otherwise).  Enabling (max_laps >= 1) is refused with LMPC_E_STATE while any
+ *     controller's closed-loop record holds rows, so every report covers a whole record; enable before the PID lap or right after a
+ *     hand-over or seeding.  Enabling again with another max_laps starts an empty table.  Any refusal leaves the handle as it was.
+ *   - Memory: batch * max_laps * 32 bytes + batch * 48 (64 MB at batch 8192, 256 laps).  Both buffers are snapshot sections
+ *     (absent, 0 bytes, without reports: such records are unchanged); a restore refuses records whose report sections differ.
+ *   - Without reports the kernels run the code they run without this feature (template instantiations). */
+int lmpc_rollout_enable_lap_reports(lmpc_handle* h, int max_laps);
+/* Report rows rows[B][max_laps] and the count n[B] of laps filed (which may exceed max_laps; rows >= min(n, max_laps) are
+ * unused) into host arrays, either may be NULL.  LMPC_E_STATE without reports.  Synchronises. */
+int lmpc_rollout_get_lap_reports(lmpc_handle* h, lmpc_lap_report* rows, int* n);
+int lmpc_sizeof_lap_report(void);
 int lmpc_rollout_sysid(lmpc_handle* h, double lamb, double* abc_host, int* flags_host);
 int lmpc_rollout_seed_from_record(lmpc_handle* h, int copies, int ss_slot0, int model_slot0);
 int lmpc_rollout_get_lap(lmpc_handle* h, int inst, int* T, double* x, double* u);              /* closed-loop record   */

@@ -75,6 +75,27 @@ class TrackParams(C.Structure):
     _fields_ = [("nseg", C.c_int), ("seg", C.c_double * (MAX_SEG * 3)), ("TrackLength", C.c_double)]
 
 
+class LapReport(C.Structure):
+    """lmpc_lap_report: one lap of one controller of the device closed loop (lmpc_rollout_enable_lap_reports)."""
+    _fields_ = [("steps", C.c_int), ("flags", C.c_int), ("unsolved", C.c_int), ("viol_steps", C.c_int), ("ipm_iters", C.c_int),
+                ("ipm_iters_max", C.c_int), ("viol_max", C.c_double)]
+
+
+LAP_REPORT_FIELDS = tuple(f for f, _ in LapReport._fields_)
+LAP_REPORT_DTYPE = np.dtype([(f, np.float64 if f == "viol_max" else np.int32) for f in LAP_REPORT_FIELDS])
+MAX_LAP_REPORTS = 1024
+
+
+def check_lap_reports(max_laps):
+    """The capacity of BatchedController.enable_lap_reports: an integer 0 .. MAX_LAP_REPORTS (0 turns reports off).  Returns it as
+    an int; raises ValueError."""
+    if isinstance(max_laps, (bool, np.bool_)) or not isinstance(max_laps, (int, np.integer)):
+        raise ValueError("max_laps must be an integer, got %r" % (max_laps,))
+    if not 0 <= int(max_laps) <= MAX_LAP_REPORTS:
+        raise ValueError("max_laps must be 0 .. %d, got %d" % (MAX_LAP_REPORTS, int(max_laps)))
+    return int(max_laps)
+
+
 SNAPSHOT_MAGIC, SNAPSHOT_VERSION, SNAPSHOT_SECTIONS = 0x50414E53, 1, 40
 # the layout ints of a record header, in header order (lmpc_snapshot_header)
 SNAPSHOT_LAYOUT = ("N", "M", "ncx", "ncu", "numSS_it", "trToUse", "ss_cap", "model_cap", "Tmax", "Tcl", "warm_start")
@@ -82,7 +103,8 @@ SNAPSHOT_LAYOUT = ("N", "M", "ncx", "ncu", "numSS_it", "trToUse", "ss_cap", "mod
 SNAPSHOT_SECTIONS_NAMES = ("ss_x", "ss_u", "ss_q", "ss_len", "model_x", "model_u", "model_len",
                            "ss_time", "ss_lap", "it", "md_time", "md_seq", "md_cnt", "lap_hist", "lap_n", "sel", "is_prev", "prev_slot",
                            "used", "xLin", "uLin", "zt", "OldInput", "xPredPrev", "timeStep", "has_pred", "warm", "warm_valid",
-                           "x", "xglob", "cl_x", "cl_u", "cl_len", "done", "health_flags", "health_unsolved", "abc_lti")
+                           "x", "xglob", "cl_x", "cl_u", "cl_len", "done", "health_flags", "health_unsolved", "abc_lti",
+                           "lap_reports", "lap_report_run")
 
 
 class SnapshotHeader(C.Structure):
@@ -163,6 +185,8 @@ def lib():
     L.lmpc_rollout_set_noise_streams.argtypes = [_vp, _vp]
     L.lmpc_rollout_set_measurement_noise.argtypes = [_vp, C.POINTER(MeasurementParams), C.c_int, _vp]
     L.lmpc_rollout_set_lap_budget.argtypes = [_vp, _vp]
+    L.lmpc_rollout_enable_lap_reports.argtypes = [_vp, C.c_int]
+    L.lmpc_rollout_get_lap_reports.argtypes = [_vp, _vp, _vp]
     L.lmpc_set_tracks.argtypes = [_vp, C.POINTER(TrackParams), C.c_int, _vp]
     L.lmpc_set_regression_sets.argtypes = [_vp, C.POINTER(RegressionParams), C.c_int, _vp]
     L.lmpc_set_shapes.argtypes = [_vp, C.POINTER(ShapeParams), C.c_int, _vp]
@@ -209,6 +233,8 @@ def lib():
     assert L.lmpc_sizeof_shape_params() == C.sizeof(ShapeParams), "lmpc_shape_params ABI mismatch"
     L.lmpc_sizeof_ss_laps_params.restype = C.c_int
     assert L.lmpc_sizeof_ss_laps_params() == C.sizeof(SsLapsParams), "lmpc_ss_laps_params ABI mismatch"
+    L.lmpc_sizeof_lap_report.restype = C.c_int
+    assert L.lmpc_sizeof_lap_report() == C.sizeof(LapReport), "lmpc_lap_report ABI mismatch"
     assert L.lmpc_sizeof_noise_params() == C.sizeof(NoiseParams), "lmpc_noise_params ABI mismatch"
     assert L.lmpc_sizeof_measurement_params() == C.sizeof(MeasurementParams), "lmpc_measurement_params ABI mismatch"
     assert L.lmpc_sizeof_regression_params() == C.sizeof(RegressionParams), "lmpc_regression_params ABI mismatch"
@@ -667,9 +693,19 @@ def decode_snapshot_header(raw):
     return out
 
 
+def snapshot_lap_reports(header):
+    """Report capacity L of a decoded header's record: 0 without report sections."""
+    return header["sections"].get("lap_reports", (0, 0))[1] // C.sizeof(LapReport)
+
+
 def snapshot_layout_mismatch(header, layout):
-    """The first layout field in which a decoded header differs from ``layout`` (a dict with SNAPSHOT_LAYOUT keys and "bytes"), as
-    a message, or None when the record fits."""
+    """The first layout field in which a decoded header differs from ``layout`` (a dict with SNAPSHOT_LAYOUT keys and "bytes", and
+    "lap_reports" = the report capacity when reports are on), as a message, or None when the record fits.  The report capacity is
+    compared before the size, which it changes."""
+    had, mine = snapshot_lap_reports(header), int(layout.get("lap_reports", 0))
+    if had != mine:
+        what = lambda L: "%d report rows" % L if L else "no lap reports"
+        return "snapshot layout mismatch: lap_reports: the record has %s and this controller %s" % (what(had), what(mine))
     for f in SNAPSHOT_LAYOUT + ("bytes",):
         if int(header[f]) != int(layout[f]):
             return "snapshot layout mismatch: %s is %d in the record and %d in this controller" % (f, header[f], layout[f])

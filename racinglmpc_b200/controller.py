@@ -542,6 +542,31 @@ class BatchedController:
         nat.check(self._lib.lmpc_rollout_get_health(self._h, nat.ptr(f), nat.ptr(n)))
         return f, n
 
+    def enable_lap_reports(self, max_laps):
+        """Per-lap reports (lmpc_rollout_enable_lap_reports): from now on every controller files one report per lap it drives and
+        hands over, up to ``max_laps`` rows (1 .. 1024; 0 turns reports off).  Needs ``enable_rollout`` and an empty closed-loop
+        record (before the PID lap, or right after a hand-over or seeding).  ValueError before any native call on a bad capacity."""
+        L = nat.check_lap_reports(max_laps)
+        if not hasattr(self, "Tcl"):
+            raise ValueError("enable_lap_reports needs enable_rollout first")
+        nat.check(self._lib.lmpc_rollout_enable_lap_reports(self._h, L))
+        self.lap_report_cap = L
+
+    def lap_reports(self):
+        """{"n": int32 [B] laps filed (may exceed the capacity L), field: [B, L] for every lmpc_lap_report field} with the rows
+        at or beyond min(n, L) zeroed.  ValueError without reports."""
+        L = getattr(self, "lap_report_cap", 0)
+        if not L:
+            raise ValueError("lap reports are not enabled (enable_lap_reports)")
+        rows = np.zeros((self.B, L), nat.LAP_REPORT_DTYPE)
+        n = np.zeros(self.B, np.int32)
+        nat.check(self._lib.lmpc_rollout_get_lap_reports(self._h, nat.ptr(rows), nat.ptr(n)))
+        used = np.arange(L)[None, :] < np.minimum(n, L)[:, None]
+        out = {"n": n}
+        for f in nat.LAP_REPORT_FIELDS:
+            out[f] = np.where(used, rows[f], 0).astype(rows[f].dtype)
+        return out
+
     def rollout_get_lap(self, inst):
         T = C.c_int(0)
         x, u = np.zeros((self.Tcl, 6)), np.zeros((self.Tcl, 2))
@@ -723,10 +748,12 @@ class BatchedController:
         return int(n.value)
 
     def snapshot_layout(self):
-        """The layout a record of this controller has (the keys of nat.SNAPSHOT_LAYOUT and "bytes")."""
+        """The layout a record of this controller has (the keys of nat.SNAPSHOT_LAYOUT and "bytes", and "lap_reports" = the report
+        capacity when reports are on)."""
         return dict(N=self.N, M=self.M, ncx=int(self._p.ncx), ncu=int(self._p.ncu), numSS_it=max(self.numSS_it, 1),
                     trToUse=self.trToUse, ss_cap=max(self.ss_cap, 1), model_cap=self.model_cap, Tmax=self.Tmax,
-                    Tcl=int(getattr(self, "Tcl", 0)), warm_start=int(self._p.warm_start), bytes=self.snapshot_bytes)
+                    Tcl=int(getattr(self, "Tcl", 0)), warm_start=int(self._p.warm_start), bytes=self.snapshot_bytes,
+                    **({"lap_reports": self.lap_report_cap} if getattr(self, "lap_report_cap", 0) else {}))
 
     def _ext_stream(self, torch):
         return torch.cuda.ExternalStream(self.stream, device=torch.device("cuda", self.device))
@@ -792,7 +819,11 @@ class BatchedController:
         heads = records[:, :hsz].index_select(0, torch.from_numpy(used.astype(np.int64)).to(records.device)).cpu().numpy()
         words = np.ascontiguousarray(heads[:, :64]).view(np.int32)     # magic, version, bytes, the layout ints, warm_mode, nsect
         want = np.array([nat.SNAPSHOT_MAGIC, nat.SNAPSHOT_VERSION, mine["bytes"]] + [mine[f] for f in nat.SNAPSHOT_LAYOUT], np.int64)
-        bad = np.nonzero(np.any(words[:, :14].astype(np.int64) & 0xFFFFFFFF != want & 0xFFFFFFFF, axis=1))[0]
+        bad = np.any(words[:, :14].astype(np.int64) & 0xFFFFFFFF != want & 0xFFFFFFFF, axis=1)
+        rep = C.sizeof(nat.LapReport) * mine.get("lap_reports", 0)     # bytes of the report rows section (slot of "lap_reports")
+        k = nat.SNAPSHOT_SECTIONS_NAMES.index("lap_reports")
+        sect_bytes = np.ascontiguousarray(heads[:, 64 + 4 * nat.SNAPSHOT_SECTIONS:64 + 8 * nat.SNAPSHOT_SECTIONS]).view(np.int32)
+        bad = np.nonzero(bad | (sect_bytes[:, k] != rep))[0]
         if bad.size:
             r = int(used[bad[0]])
             msg = nat.snapshot_layout_mismatch(nat.decode_snapshot_header(heads[bad[0]]), mine)

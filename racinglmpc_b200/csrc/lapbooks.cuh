@@ -154,12 +154,12 @@ __global__ void books_refresh_kernel(int batch, LapBooks k, SsLaps laps) {
 
 // Lap hand-over of every controller whose lap just ended (done[b] != 0), bookkeeping included: main.py:113-119
 // (lmpc.addTrajectory + predictiveModel.addTrajectory of the lap Simulator.sim returned), SysModel.py:50 (s -= TrackLength),
-// PC.py:445 (timeStep = 0).  One CTA per controller; no host involvement.
-template <bool LAPS>
+// PC.py:445 (timeStep = 0).  One CTA per controller; no host involvement.  REPORTS: the running report row is filed as the lap's.
+template <bool LAPS, bool REPORTS>
 __global__ void __launch_bounds__(256) commit_laps_books_kernel(int batch, LapPool ss, LapPool model, LapBooks k, const double* cl_x,
                                                                 const double* cl_u, int* cl_len, int Tcl, double* x_cur, int* timeStep,
                                                                 int* done, int* flags_or, Tracks trk, int lmpc, LapBudget retire,
-                                                                SsLaps laps) {
+                                                                SsLaps laps, LapReports rep) {
     const int b = blockIdx.x;
     if (b >= batch || retire.retired(b) || !done[b]) return;
     __shared__ int s_ss, s_md;
@@ -182,16 +182,18 @@ __global__ void __launch_bounds__(256) commit_laps_books_kernel(int batch, LapPo
         int f = book_refresh(k, b, book_laps<LAPS>(k, laps, b));
         if (s_ss == -2) f |= 64;                                 // safe-set pool too small for numSS_it + 2 laps
         if (f && flags_or) flags_or[b] |= f;
+        if constexpr (REPORTS) report_file(rep, b);
         restart_record(b, cl_len, x_cur, timeStep, done, TrackLength);
     }
 }
 
 // main.py:99-110 with device bookkeeping: the record every controller just drove becomes `copies` laps of both stores.
-template <bool LAPS>
+// REPORTS: the report table starts afresh, like lap_n.
+template <bool LAPS, bool REPORTS>
 __global__ void __launch_bounds__(256) seed_books_kernel(int batch, LapPool ss, LapPool model, LapBooks k, int copies, const double* cl_x,
                                                          const double* cl_u, int* cl_len, int Tcl, int N, double* xLin, double* uLin,
                                                          double* zt, double* OldInput, int* timeStep, int* hasPred, int* done,
-                                                         Tracks trk, int lmpc, Shapes shp, SsLaps laps) {
+                                                         Tracks trk, int lmpc, Shapes shp, SsLaps laps, LapReports rep) {
     const int b = blockIdx.x;
     if (b >= batch) return;
     __shared__ int s_ss, s_md;
@@ -216,7 +218,16 @@ __global__ void __launch_bounds__(256) seed_books_kernel(int batch, LapPool ss, 
         __syncthreads();
     }
     seed_state_block(b, N, shp, cx, cu, xLin, uLin, zt, OldInput);
-    if (threadIdx.x == 0) { book_refresh(k, b, book_laps<LAPS>(k, laps, b)); timeStep[b] = 0; hasPred[b] = 0; cl_len[b] = 0; done[b] = 0; }
+    if (threadIdx.x == 0) {
+        book_refresh(k, b, book_laps<LAPS>(k, laps, b)); timeStep[b] = 0; hasPred[b] = 0; cl_len[b] = 0; done[b] = 0;
+        if constexpr (REPORTS) report_restart(rep, b);
+    }
+}
+
+// The state of a freshly enabled report table: n = 0 and an empty running row for every controller.
+__global__ void lap_reports_reset_kernel(int batch, LapReports rep) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b < batch) report_restart(rep, b);
 }
 
 // ---- pooled safe-set exchange (SURVEY §8e) -------------------------------------------------------------------------------

@@ -176,11 +176,15 @@ struct lmpc_handle {
     bool has_trace;
     // controller snapshots (snapshot.cuh): header template [SNAP_HDR_WORDS] + check verdict [4], allocated with the store
     int* d_snap;
+    // per-lap reports (lmpc_rollout_enable_lap_reports): rows [B][rep_L] and running rows [B], or none (rep_L == 0)
+    lmpc_lap_report* d_rep_rows;
+    LapRun* d_rep_run;
+    int rep_L;
 };
 
 // The handle's device buffers outside the QP buffer sets.  A buffer is [rows][B][per] elements (rows == 0: `per` elements for
 // the whole handle), B being the batch, or the number of traced controllers for the trace.
-enum BufOwner : unsigned { OWN_HANDLE = 1, OWN_STORE = 2, OWN_WARM = 4, OWN_ROLLOUT = 8, OWN_TRACE = 16, OWN_QP = 32 };
+enum BufOwner : unsigned { OWN_HANDLE = 1, OWN_STORE = 2, OWN_WARM = 4, OWN_ROLLOUT = 8, OWN_TRACE = 16, OWN_QP = 32, OWN_REPORTS = 64 };
 enum BufFill { FILL_NONE, FILL_ZERO, FILL_ONES };      // FILL_ONES: every int -1 (a free slot, no previous lap)
 constexpr int SN_SCRATCH = -1;
 struct DevBuf {
@@ -240,6 +244,8 @@ static std::vector<DevBuf> dev_bufs(lmpc_handle* h) {
         dbuf(h->d_health, 1, R, FILL_ZERO, SN_HEALTH_FLAGS, nullptr, 2),       // [2][B]: flags, then unsolved steps
         dbuf(h->d_abc_lti, 54, R, FILL_ZERO, SN_ABC_LTI, "abc_lti"), dbuf(h->d_z, 3, R), dbuf(h->d_zpid, 2, R),
         dbuf(h->d_xmeas, 6, R, FILL_ZERO, SN_SCRATCH, "x_meas"),     // formed from the plant state and the clock every step
+        // per-lap reports (lap_reports_reset_kernel gives the running rows their start)
+        dbuf(h->d_rep_rows, (size_t)h->rep_L, OWN_REPORTS, FILL_ZERO, SN_LAP_REPORTS), dbuf(h->d_rep_run, 1, OWN_REPORTS, FILL_ZERO, SN_LAP_RUN),
         // trace of chosen controllers (per traced controller)
         dbuf(h->d_trinst, 1, X), dbuf(h->tr.steps, 1, X, FILL_ZERO), dbuf(h->tr.x, cap * 6, X), dbuf(h->tr.g, cap * 6, X),
         dbuf(h->tr.u, cap * 2, X), dbuf(h->tr.xPred, cap * np, X), dbuf(h->tr.ss, cap * 6 * Mx, X), dbuf(h->tr.lap, cap, X)};
@@ -499,8 +505,16 @@ static Tracks tracks(const lmpc_handle* h) { return h->trk.view(); }
 // the PID lap, the host-slot hand-over) passes LapBudget{}: nobody is retired there.
 static LapBudget lap_budget(const lmpc_handle* h) { return LapBudget{h->budget.idx, h->bk.lap_n}; }
 
+// The report buffers and the QP constants the kernels of the closed loop read (all null without reports: only the REPORTS
+// instantiations read them)
+static LapReports reports(const lmpc_handle* h) {
+    if (!h->rep_L) return LapReports{};
+    return LapReports{h->d_rep_rows, h->d_rep_run, h->rep_L, h->sets.tab ? h->sets.view() : h->own_c.view()};
+}
+
 static void free_rollout(lmpc_handle* h) {
-    free_bufs(dev_bufs(h), OWN_ROLLOUT | OWN_TRACE);
+    free_bufs(dev_bufs(h), OWN_ROLLOUT | OWN_TRACE | OWN_REPORTS);
+    h->rep_L = 0;
     h->has_trace = false;
     h->has_rollout = false;
 }
@@ -1634,7 +1648,7 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
     SimArgs sa = sim_args(h, z_host ? h->d_z : nullptr, seed);                       // SysModel.py:40 (dynModel)
     sa.flags = h->d_flags; sa.status = q.status; sa.health = h->d_health; sa.retire = retire;
     if (h->meas.tab) sa.rec_x = y;
-    sim_step_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->mc, sa);
+    (h->rep_L ? sim_step_kernel<true> : sim_step_kernel<false>)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->mc, sa, reports(h), q.iters);
     CK(cudaGetLastError());
     h->launches += 1;
     h->cur ^= 1;
@@ -1659,7 +1673,7 @@ int lmpc_rollout_pid_step(lmpc_handle* h, double vt, const double* z_pid_host, c
     SimArgs sa = sim_args(h, z_sim_host ? h->d_z : nullptr, seed);
     sa.health = h->d_health;          // no step flags or QP status here: only the simulator's own bits
     if (h->meas.tab) sa.rec_x = y;
-    sim_step_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->mc, sa);
+    (h->rep_L ? sim_step_kernel<true> : sim_step_kernel<false>)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->mc, sa, reports(h), nullptr);
     CK(cudaGetLastError());
     h->launches += 2;
     h->cur ^= 1;
@@ -1741,6 +1755,59 @@ int lmpc_rollout_set_lap_budget(lmpc_handle* h, const int* budget_of_instance) {
     return swap_table<int>(h, who, h->budget, nullptr, 0, budget_of_instance);
 }
 
+// Per-lap reports: 1 <= max_laps <= 1024 allocates an empty table (refused while a record holds rows), 0 frees it.  New buffers are
+// allocated before the old ones go, so a failed allocation leaves the handle as it was.
+int lmpc_rollout_enable_lap_reports(lmpc_handle* h, int max_laps) {
+    static const char* who = "lmpc_rollout_enable_lap_reports";
+    if (int rc = need_rollout(h)) return rc;
+    if (max_laps < 0 || max_laps > 1024) return fail(LMPC_E_INVALID, std::string(who) + ": max_laps must be 0 .. 1024");
+    CK(cudaSetDevice(h->device));
+    CK(cudaStreamSynchronize(h->stream));
+    if (max_laps > 0) {
+        std::vector<int> cl(h->batch);
+        CK(cudaMemcpy(cl.data(), h->d_cllen, sizeof(int) * h->batch, cudaMemcpyDeviceToHost));
+        for (int b = 0; b < h->batch; ++b)
+            if (cl[b] > 0)
+                return fail(LMPC_E_STATE, std::string(who) + ": the closed-loop record of controller " + std::to_string(b) +
+                                              " holds rows; enable reports before the PID lap or right after a hand-over or seeding");
+    }
+    lmpc_lap_report* old_rows = h->d_rep_rows;
+    LapRun* old_run = h->d_rep_run;
+    const int old_L = h->rep_L;
+    h->d_rep_rows = nullptr; h->d_rep_run = nullptr; h->rep_L = max_laps;
+    if (max_laps > 0) {
+        int rc = alloc_bufs(h, dev_bufs(h), OWN_REPORTS, h->batch, who);
+        if (rc == LMPC_OK) {
+            lap_reports_reset_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->batch, reports(h));
+            cudaError_t e = cudaGetLastError();
+            if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+            if (e != cudaSuccess) {
+                free_bufs(dev_bufs(h), OWN_REPORTS);
+                rc = fail(LMPC_E_CUDA, std::string(who) + ": " + cudaGetErrorString(e));
+            }
+        }
+        if (rc != LMPC_OK) {
+            h->d_rep_rows = old_rows; h->d_rep_run = old_run; h->rep_L = old_L;
+            return rc;
+        }
+        h->launches += 1;
+    }
+    if (old_rows) cudaFree(old_rows);
+    if (old_run) cudaFree(old_run);
+    return LMPC_OK;
+}
+
+int lmpc_rollout_get_lap_reports(lmpc_handle* h, lmpc_lap_report* rows, int* n) {
+    if (int rc = need_rollout(h)) return rc;
+    if (!h->rep_L) return fail(LMPC_E_STATE, "lmpc_rollout_get_lap_reports: lap reports are not enabled");
+    if (rows) CK(cudaMemcpyAsync(rows, h->d_rep_rows, sizeof(lmpc_lap_report) * h->batch * h->rep_L, cudaMemcpyDeviceToHost, h->stream));
+    if (n) CK(cudaMemcpy2DAsync(n, sizeof(int), &h->d_rep_run->n, sizeof(LapRun), sizeof(int), h->batch, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return LMPC_OK;
+}
+
+int lmpc_sizeof_lap_report(void) { return (int)sizeof(lmpc_lap_report); }
+
 // Regression(x, u, lamb) of Utilities.py:5-28 on every instance's closed-loop record: per-instance LTI model in the device
 // buffer "abc_lti" ([B][54] = A | B | C = 0, the layout lmpc_solve_mpc_dev takes with strides (54, 0)); abc_host may be NULL.
 int lmpc_rollout_sysid(lmpc_handle* h, double lamb, double* abc_host, int* flags_host) {
@@ -1763,9 +1830,9 @@ int lmpc_rollout_seed_from_record(lmpc_handle* h, int copies, int ss_slot0, int 
         return fail(LMPC_E_INVALID, "seed copies do not fit the lap pools");
     h->laps_stored = true;
     if (h->d_warm_valid) CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * h->batch, h->stream));
-    seed_from_record_kernel<<<h->batch, 256, 0, h->stream>>>(h->batch, h->ss, h->mdl, copies, ss_slot0, model_slot0, h->d_clx, h->d_clu,
-                                                             h->d_cllen, h->Tcl, h->N, h->d_xLin, h->d_uLin, h->d_ztState, h->d_OldInput,
-                                                             h->d_timeStep, h->d_hasPred, h->d_done, tracks(h), h->shp.view());
+    (h->rep_L ? seed_from_record_kernel<true> : seed_from_record_kernel<false>)<<<h->batch, 256, 0, h->stream>>>(
+        h->batch, h->ss, h->mdl, copies, ss_slot0, model_slot0, h->d_clx, h->d_clu, h->d_cllen, h->Tcl, h->N, h->d_xLin, h->d_uLin,
+        h->d_ztState, h->d_OldInput, h->d_timeStep, h->d_hasPred, h->d_done, tracks(h), h->shp.view(), reports(h));
     CK(cudaGetLastError());
     h->launches += 1;
     return LMPC_OK;
@@ -1797,9 +1864,9 @@ int lmpc_rollout_commit_laps(lmpc_handle* h, const int* fin, const int* ss_slots
     CK(cudaMemcpyAsync(h->d_xchg, fin, sizeof(int) * B, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(h->d_xchg + B, ss_slots, sizeof(int) * B, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(h->d_xchg + 2 * B, model_slots, sizeof(int) * B, cudaMemcpyHostToDevice, h->stream));
-    commit_laps_kernel<<<h->batch, 256, 0, h->stream>>>(h->batch, h->ss, h->mdl, h->d_xchg, h->d_xchg + B, h->d_xchg + 2 * B, h->d_clx,
-                                                        h->d_clu, h->d_cllen, h->Tcl, h->d_rx[h->cur], h->d_timeStep, h->d_done,
-                                                        tracks(h));
+    (h->rep_L ? commit_laps_kernel<true> : commit_laps_kernel<false>)<<<h->batch, 256, 0, h->stream>>>(
+        h->batch, h->ss, h->mdl, h->d_xchg, h->d_xchg + B, h->d_xchg + 2 * B, h->d_clx, h->d_clu, h->d_cllen, h->Tcl, h->d_rx[h->cur],
+        h->d_timeStep, h->d_done, tracks(h), reports(h));
     CK(cudaGetLastError());
     h->launches += 1;
     CK(cudaStreamSynchronize(h->stream));   // the three host arrays are pageable memory of the caller
@@ -1930,9 +1997,10 @@ int lmpc_books_get(lmpc_handle* h, int* ss_time, int* ss_lap, int* it, int* md_t
 int lmpc_rollout_commit_laps_dev(lmpc_handle* h) {
     if (int rc = need_rollout(h)) return rc;
     h->laps_stored = true;     // enqueue only: which controllers finish a lap is not known here
-    (h->ssl.tab ? commit_laps_books_kernel<true> : commit_laps_books_kernel<false>)<<<h->batch, 256, 0, h->stream>>>(
+    (h->ssl.tab ? (h->rep_L ? commit_laps_books_kernel<true, true> : commit_laps_books_kernel<true, false>)
+                : (h->rep_L ? commit_laps_books_kernel<false, true> : commit_laps_books_kernel<false, false>))<<<h->batch, 256, 0, h->stream>>>(
         h->batch, h->ss, h->mdl, h->bk, h->d_clx, h->d_clu, h->d_cllen, h->Tcl, h->d_rx[h->cur], h->d_timeStep, h->d_done, h->d_health,
-        tracks(h), h->M > 0 ? 1 : 0, lap_budget(h), h->ssl.view());
+        tracks(h), h->M > 0 ? 1 : 0, lap_budget(h), h->ssl.view(), reports(h));
     CK(cudaGetLastError());
     h->launches += 1;
     return LMPC_OK;
@@ -1943,9 +2011,10 @@ int lmpc_rollout_seed_from_record_dev(lmpc_handle* h, int copies) {
     if (copies < 1 || (h->M > 0 && copies > h->ss.cap) || copies > h->mdl.cap) return fail(LMPC_E_INVALID, "seed copies do not fit the lap pools");
     h->laps_stored = true;
     if (h->d_warm_valid) CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * h->batch, h->stream));
-    (h->ssl.tab ? seed_books_kernel<true> : seed_books_kernel<false>)<<<h->batch, 256, 0, h->stream>>>(
+    (h->ssl.tab ? (h->rep_L ? seed_books_kernel<true, true> : seed_books_kernel<true, false>)
+                : (h->rep_L ? seed_books_kernel<false, true> : seed_books_kernel<false, false>))<<<h->batch, 256, 0, h->stream>>>(
         h->batch, h->ss, h->mdl, h->bk, copies, h->d_clx, h->d_clu, h->d_cllen, h->Tcl, h->N, h->d_xLin, h->d_uLin, h->d_ztState,
-        h->d_OldInput, h->d_timeStep, h->d_hasPred, h->d_done, tracks(h), h->M > 0 ? 1 : 0, h->shp.view(), h->ssl.view());
+        h->d_OldInput, h->d_timeStep, h->d_hasPred, h->d_done, tracks(h), h->M > 0 ? 1 : 0, h->shp.view(), h->ssl.view(), reports(h));
     CK(cudaGetLastError());
     h->launches += 1;
     return LMPC_OK;
@@ -2054,7 +2123,7 @@ static const char* snap_field_name(int f) {
         "magic", "version", "record bytes", "N", "numSS_Points", "ncx", "ncu", "numSS_it", "trToUse", "ss_cap", "model_cap", "Tmax",
         "Tcl", "warm_start", "warm_mode", "nsect", "section table", "track row", "safe-set lap length", "model lap length", "it",
         "safe-set lap number", "md_cnt", "model arrival number", "lap_n", "sel", "is_prev", "prev_slot", "used", "timeStep",
-        "has_pred", "warm_valid", "cl_len", "done"};
+        "has_pred", "warm_valid", "cl_len", "done", "lap report layout", "lap report count"};
     return f >= 0 && f < SF_NFIELD ? names[f] : "?";
 }
 
@@ -2220,7 +2289,7 @@ int lmpc_snapshot_unpack_dev(lmpc_handle* h, const void* rec_dev, int nrec, int 
     if (got[0] != INT32_MAX) {
         const int i = got[0] / 64, f = got[0] % 64;
         why = "record " + std::to_string(idx[n + i]) + " (into controller " + std::to_string(idx[i]) + "): " + snap_field_name(f) +
-              (f <= SF_SECTIONS ? " differs from this handle's" : f == SF_TRACK ? " differs from the controller's track" : " out of range");
+              (f <= SF_SECTIONS || f == SF_LAP_REPORTS ? " differs from this handle's" : f == SF_TRACK ? " differs from the controller's track" : " out of range");
     } else if (h->d_warm && got[1] <= got[2]) {
         if (h->warm_mode < 0 && got[1] != got[2]) why = "the records hold warm-start records of two problem types";
         else mode = got[1];

@@ -15,6 +15,7 @@
 #include <math_constants.h>
 #include <stdint.h>
 #include "lap_budget.cuh"
+#include "ftocp_launch.cuh"
 
 namespace lmpc {
 
@@ -58,6 +59,73 @@ __device__ __forceinline__ int ss_points_of(const Shapes& s, int b, int M) { ret
 using SsLapsRec = lmpc_ss_laps_params;
 using SsLaps = Table<SsLapsRec>;
 __device__ __forceinline__ int ss_laps_of(const SsLaps& l, int b, int nit) { return l.tab ? l.of(b).numSS_it : nit; }
+
+// Per-lap reports (lmpc_rollout_enable_lap_reports, DESIGN.md "Per-lap reports"): rows[B][L] filed at the lap hand-overs, and the
+// running row of the record under way with the count n of rows filed.  The kernels that touch them come in two instantiations,
+// REPORTS = reports are enabled: without them they are the code they were before reports existed.
+struct LapRun {
+    lmpc_lap_report row;
+    int n, pad[3];
+};
+static_assert(sizeof(lmpc_lap_report) == 32 && sizeof(LapRun) == 48, "report rows are 32 bytes, running rows 48");
+struct LapReports {
+    lmpc_lap_report* rows;       // [B][L]
+    LapRun* run;                 // [B]
+    int L;
+    Table<FtocpConstRec> qp;     // the QP constants (Fx, bx) of every controller: its parameter-set row, else the handle's
+};
+__device__ __forceinline__ void report_reset(lmpc_lap_report& r) {
+    r.steps = 0; r.flags = 0; r.unsolved = 0; r.viol_steps = 0; r.ipm_iters = 0; r.ipm_iters_max = 0;
+    r.viol_max = -CUDART_INF;
+}
+// A hand-over: the running row becomes report n (stored while n < L), n counts on, the row restarts with the record.  One thread.
+__device__ __forceinline__ void report_file(const LapReports& rep, int b) {
+    LapRun& r = rep.run[b];
+    const int n = r.n;
+    if ((unsigned)n < (unsigned)rep.L) rep.rows[(size_t)b * rep.L + n] = r.row;
+    r.n = n + 1;
+    report_reset(r.row);
+}
+// The seeding: the PID record is consumed without a report and the table starts afresh.  One thread.
+__device__ __forceinline__ void report_restart(const LapReports& rep, int b) {
+    rep.run[b].n = 0;
+    report_reset(rep.run[b].row);
+}
+// One closed-loop step of controller b driven from plant state x: flags = the step flags | the simulator's bits, status / iters of
+// the step's QP (null for a PID step).  The lane rows are evaluated without contraction so that a host restatement gives the same
+// bits (tests/support/lap_reports.py).
+__device__ __forceinline__ void report_step(const LapReports& rep, int b, const double* x, int flags, const int* status,
+                                            const int* iters) {
+    const FtocpConst& c = rep.qp.of(b).c;
+    lmpc_lap_report r = rep.run[b].row;
+    bool finite = true, viol = false;
+#pragma unroll
+    for (int j = 0; j < 6; ++j) finite = finite && isfinite(x[j]);
+    if (!finite) {
+        viol = true;
+        r.viol_max = CUDART_INF;
+    } else {
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {                            // ncx == 2 lane rows (lmpc_create)
+            double s = __dmul_rn(c.Fx[i * 6], x[0]);
+#pragma unroll
+            for (int j = 1; j < 6; ++j) s = __dadd_rn(s, __dmul_rn(c.Fx[i * 6 + j], x[j]));
+            const double d = __dsub_rn(s, c.bx[i]);
+            viol = viol || d > 0.0;
+            r.viol_max = fmax(r.viol_max, d);
+        }
+    }
+    r.steps += 1;
+    r.flags |= flags;
+    r.viol_steps += viol ? 1 : 0;
+    if (status) {
+        r.unsolved += status[b] != 1 ? 1 : 0;
+        const int it = iters[b];
+        r.ipm_iters += it;
+        r.ipm_iters_max = max(r.ipm_iters_max, it);
+    }
+    rep.run[b].row = r;
+}
 
 struct LapPool {
     double* x;      // [B][cap][Tmax][6]
@@ -805,10 +873,11 @@ __global__ void __launch_bounds__(256) rollout_cost_kernel(LapPool pool, int b, 
 
 // Lap hand-over of every instance with fin[b] != 0, one CTA per instance (main.py:113-119 + SysModel.py:50 + PC.py:445):
 // the closed-loop record goes to safe-set slot ss_slot[b] (>= 0) with its cost-to-go and to regression slot model_slot[b]
-// (>= 0); then the record restarts.
+// (>= 0); then the record restarts (REPORTS: its running report row is filed first).
+template <bool REPORTS>
 __global__ void __launch_bounds__(256) commit_laps_kernel(int batch, LapPool ss, LapPool model, const int* fin, const int* ss_slot,
                                                           const int* model_slot, const double* cl_x, const double* cl_u, int* cl_len,
-                                                          int Tcl, double* x_cur, int* timeStep, int* done, Tracks trk) {
+                                                          int Tcl, double* x_cur, int* timeStep, int* done, Tracks trk, LapReports rep) {
     const int b = blockIdx.x;
     if (b >= batch || !fin[b]) return;
     const int Trec = cl_len[b];
@@ -817,7 +886,10 @@ __global__ void __launch_bounds__(256) commit_laps_kernel(int batch, LapPool ss,
     if (ss_slot[b] >= 0) copy_ss_lap_block(ss, ss.lap_index(b, ss_slot[b]), cl_x + rec * 6, cl_u + rec * 2, Trec, TrackLength);
     if (model_slot[b] >= 0) copy_lap_block(model, model.lap_index(b, model_slot[b]), cl_x + rec * 6, cl_u + rec * 2, Trec);
     __syncthreads();
-    if (threadIdx.x == 0) restart_record(b, cl_len, x_cur, timeStep, done, TrackLength);
+    if (threadIdx.x == 0) {
+        if constexpr (REPORTS) report_file(rep, b);
+        restart_record(b, cl_len, x_cur, timeStep, done, TrackLength);
+    }
 }
 
 // Pooled-safe-set exchange (SURVEY §8e): pack one stored lap per instance, slot[b] (< 0: none), into exchange rows
@@ -943,7 +1015,10 @@ constexpr int SIM_RECORD_FULL = 256;
 #include <curand_kernel.h>
 namespace lmpc {
 
-__global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimArgs a) {
+// REPORTS: the step is also added to the controller's running report row (report_step) with its QP's status a.status and
+// iterations rep_iters, both null for a PID step.  The parameters after a are read only by that instantiation.
+template <bool REPORTS>
+__global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimArgs a, const LapReports rep, const int* rep_iters) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= a.batch) return;
     if (a.retire.retired(b)) {
@@ -1007,6 +1082,7 @@ __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimA
     }
     if (!okc) sim_bits |= SIM_LOOKUP_FAILED;
     if (a.health && sim_bits) a.health[b] |= sim_bits;
+    if constexpr (REPORTS) report_step(rep, b, x, (a.flags ? a.flags[b] : 0) | sim_bits, a.status, rep_iters);
     double z0, z1, z2;
     if (a.z) {
         z0 = a.z[(size_t)b * 3]; z1 = a.z[(size_t)b * 3 + 1]; z2 = a.z[(size_t)b * 3 + 2];
@@ -1175,11 +1251,12 @@ __global__ void __launch_bounds__(32) ridge_sysid_kernel(int batch, const double
 // Seed a controller from the closed-loop record the way main.py:99-110 does from the PID lap: the record is stored `copies`
 // times in the safe set (slots ss_slot0 ..) and in the regression model (slots model_slot0 ..), cost-to-go by computeCost,
 // the controller state from the record (seed_state_block), timeStep = 0, no previous prediction; the record restarts.  One CTA
-// per instance.
+// per instance.  REPORTS: the report table starts afresh.
+template <bool REPORTS>
 __global__ void __launch_bounds__(256) seed_from_record_kernel(int batch, LapPool ss, LapPool model, int copies, int ss_slot0, int model_slot0,
                                                               const double* cl_x, const double* cl_u, int* cl_len, int Tcl, int N,
                                                               double* xLin, double* uLin, double* zt, double* OldInput, int* timeStep,
-                                                              int* hasPred, int* done, Tracks trk, Shapes shp) {
+                                                              int* hasPred, int* done, Tracks trk, Shapes shp, LapReports rep) {
     const int b = blockIdx.x;
     if (b >= batch) return;
     const int Trec = cl_len[b];
@@ -1191,7 +1268,10 @@ __global__ void __launch_bounds__(256) seed_from_record_kernel(int batch, LapPoo
         copy_lap_block(model, model.lap_index(b, model_slot0 + c), cx, cu, Trec);
     }
     seed_state_block(b, N, shp, cx, cu, xLin, uLin, zt, OldInput);
-    if (threadIdx.x == 0) { timeStep[b] = 0; hasPred[b] = 0; cl_len[b] = 0; done[b] = 0; }
+    if (threadIdx.x == 0) {
+        timeStep[b] = 0; hasPred[b] = 0; cl_len[b] = 0; done[b] = 0;
+        if constexpr (REPORTS) report_restart(rep, b);
+    }
 }
 
 }  // namespace lmpc

@@ -19,6 +19,7 @@ enum SnapSection {
     SN_XLIN, SN_ULIN, SN_ZT, SN_OLDINPUT, SN_XPREDPREV, SN_TIMESTEP, SN_HASPRED,
     SN_WARM, SN_WARM_VALID,
     SN_RX, SN_RG, SN_CLX, SN_CLU, SN_CLLEN, SN_DONE, SN_HEALTH_FLAGS, SN_HEALTH_UNSOLVED, SN_ABC_LTI,
+    SN_LAP_REPORTS, SN_LAP_RUN,          // lmpc_rollout_enable_lap_reports: absent (0 bytes) without reports
     SN_COUNT,
     // pack-only entries of the copy table: the header (up to the track row) and the controller's track row
     SN_HEADER = SN_COUNT, SN_TRACK, SN_TABLE
@@ -76,7 +77,8 @@ __global__ void __launch_bounds__(256) snapshot_copy_kernel(const __grid_constan
 // lmpc_b200.cu, snap_field_name)
 enum SnapField {
     SF_WARM_MODE = 14, SF_SECTIONS = 16, SF_TRACK, SF_SS_LEN, SF_MD_LEN, SF_IT, SF_SS_LAP, SF_MD_CNT, SF_MD_SEQ, SF_LAP_N, SF_SEL,
-    SF_ISPREV, SF_PREVSLOT, SF_USED, SF_TIMESTEP, SF_HASPRED, SF_WARM_VALID, SF_CLLEN, SF_DONE, SF_NFIELD
+    SF_ISPREV, SF_PREVSLOT, SF_USED, SF_TIMESTEP, SF_HASPRED, SF_WARM_VALID, SF_CLLEN, SF_DONE, SF_LAP_REPORTS, SF_LAP_REPORT_N,
+    SF_NFIELD
 };
 constexpr int SNAP_HDR_WORDS = 16 + 2 * LMPC_SNAPSHOT_SECTIONS;   // int words of the header before the track row
 
@@ -104,6 +106,9 @@ __global__ void __launch_bounds__(128) snapshot_check_kernel(const SnapCheckArgs
         const int w = j < 2 ? j : j < 15 ? j + 1 : j == 15 ? 2 : j;     // magic, version, the layout ints, then the sizes
         if (w != SF_WARM_MODE && H[w] != a.hdr[w]) f = w < SF_SECTIONS ? w : SF_SECTIONS;
     }
+    // a record with or without reports, or with another report capacity, differs in its size too: name the reports instead
+    for (int s = SN_LAP_REPORTS; f >= 2 && f != SF_NFIELD && s <= SN_LAP_RUN; ++s)
+        if (H[16 + LMPC_SNAPSHOT_SECTIONS + s] != a.hdr[16 + LMPC_SNAPSHOT_SECTIONS + s]) f = SF_LAP_REPORTS;
     if (f == SF_NFIELD) {      // the layout is this handle's: the sections lie where this handle puts them
         // the circuit, bit for bit: nseg, its nseg rows and TrackLength (padding and unused rows are not part of it)
         const TrackRec& tr = *reinterpret_cast<const TrackRec*>(R + SNAP_HDR_WORDS * 4);
@@ -153,6 +158,7 @@ __global__ void __launch_bounds__(128) snapshot_check_kernel(const SnapCheckArgs
             BAD(cl < 0 || cl > a.Tcl, SF_CLLEN);
             BAD(dn != 0 && dn != 1, SF_DONE);
         }
+        if (a.rec_off[SN_LAP_RUN] > 0) BAD(reinterpret_cast<const LapRun*>(R + a.rec_off[SN_LAP_RUN])->n < 0, SF_LAP_REPORT_N);
     }
 #undef BAD
     if (f != SF_NFIELD) atomicMin(&out[0], i * 64 + f);

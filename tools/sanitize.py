@@ -5,7 +5,8 @@ Exercises: ftocp_kernel<12,0> and <12,48> (host + device entry points), knn_ltv_
 ss_add_point, rollout_cost, sim_step (with noise sets and noise streams), measure (with measurement sets), knn_ltv_regress with regression sets, commit_laps, ss_export_laps, ss_import_laps; round 2: the long-horizon kernel
 that reads its model in place (N = 48), warm-started solves, pid_input, seed_books, commit_laps_books, rollout_stats, the pooled
 exchange (pool_local_best / export / rank / import), trace_step and track_global_position, and a controller made
-non-finite in the closed loop (ss_select on a NaN terminal guess, ss_add_point refusing the point)."""
+non-finite in the closed loop (ss_select on a NaN terminal guess, ss_add_point refusing the point), all with per-lap reports on
+(the report instantiations of sim_step, seed_books and commit_laps_books, lap_reports_reset)."""
 import os
 import sys
 import numpy as np
@@ -69,6 +70,7 @@ c = BatchedController(par, B, workloads.track_seg_table(), rp.TRACK_LENGTH, trTo
                       numSS_it=numSS_it, QterminalSlack=Qts, Tmax=1280, ss_cap=7, model_cap=5, warm_start=True)
 xs = np.tile(np.array([0.5, 0, 0, 0, 0, 0.0]), (B, 1))
 c.enable_rollout(Tcl=1024)
+c.enable_lap_reports(2)                              # per-lap reports: the report instantiations of the step, hand-over and seeding
 c.rollout_set_state(xs, xs)
 c.set_measurement_noise([rp.MeasurementParams((0.01,) * 6, (0.05,) * 6)], np.zeros(B, np.int32))   # the PID lap measures too
 for _ in range(int(os.environ.get("SANITIZE_PID_STEPS", "1000"))):
@@ -88,6 +90,7 @@ for _ in range(3):
     c.rollout_step(seed=3)
     c.rollout_commit_laps_dev()
 assert c.rollout_health()[0][1] & 512
+rep = c.lap_reports()                                # the non-finite controller's running row holds viol_max = +inf
 print("stats", c.rollout_stats())
 rows = torch.zeros(3, 288, 9, dtype=torch.float64, device="cuda")
 meta = torch.zeros(3, 4, dtype=torch.int32, device="cuda")

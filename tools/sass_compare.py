@@ -6,8 +6,10 @@ Kernels are matched by variant and (N, M) across their old and new names:
   sets     ftocp_sets_kernel<N, M, 2, 4>  or  ftocp_kernel<N, M, 2, 4, true>
 and the instantiations that run without a per-controller table of the other kernels of a step and of the lap books, matched
 across their untemplated names:
-  default  knn_ltv_regress_kernel, ss_select_kernel, shift_state_kernel (<false>: no shape or lap-count table) and
-           books_refresh_kernel, commit_laps_books_kernel, seed_books_kernel, pool_import_kernel (<false>: no lap-count table)
+  default  knn_ltv_regress_kernel, ss_select_kernel, shift_state_kernel (<false>: no shape or lap-count table),
+           books_refresh_kernel, commit_laps_books_kernel, seed_books_kernel, pool_import_kernel (<false>: no lap-count table;
+           <false, false>: no lap-count table and no lap reports) and sim_step_kernel, commit_laps_kernel, seed_from_record_kernel
+           (<false>: no lap reports)
 and compared by instruction text (cuobjdump -sass without addresses and encodings).  Each differing line pair is classified:
   dfma-swap   one DFMA with its two factors exchanged (a*b+c = b*a+c)
   lds-swap    LDS.128 loads of unchanged addresses whose destination registers are permuted among themselves
@@ -24,7 +26,8 @@ import sys
 
 NAME = re.compile(r"^(?:void )?(ftocp_kernel|ftocp_sets_kernel)<(\d+), (\d+), 2, 4(?:, (true|false))?>")
 DEFAULT = re.compile(r"^(?:void )?lmpc::(knn_ltv_regress_kernel|ss_select_kernel|shift_state_kernel|books_refresh_kernel|"
-                     r"commit_laps_books_kernel|seed_books_kernel|pool_import_kernel)(<false>)?\(")
+                     r"commit_laps_books_kernel|seed_books_kernel|pool_import_kernel|sim_step_kernel|commit_laps_kernel|"
+                     r"seed_from_record_kernel)(<false>|<false, false>)?\(")
 
 
 def kernels(path):
