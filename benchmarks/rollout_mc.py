@@ -87,10 +87,52 @@ def check_lap_reports(lap_reports, laps):
     return L
 
 
+def check_lap_schedules(lap_schedules, batch, lap_reports, tables):
+    """The refusals of run(lap_schedules=...), before any device work: every kind is one of BatchedController.set_lap_schedule's,
+    has its table in `tables` ({kind: (rows, index) or None}) and a schedule the table's rows cover, and the run keeps lap reports
+    (the per-lap statistics come from them).  Returns {kind: [batch, L] int32 schedule}, empty without schedules."""
+    if lap_schedules is None:
+        return {}
+    if not isinstance(lap_schedules, dict):
+        raise ValueError("lap_schedules is a dict {kind: rows} with kind in %s" % sorted(_native.LAP_SCHEDULE_TABLES))
+    out = {}
+    for kind, rows in lap_schedules.items():
+        if kind not in _native.LAP_SCHEDULE_TABLES:
+            raise ValueError("lap_schedules: kind is one of %s, got %r" % (sorted(_native.LAP_SCHEDULE_TABLES), kind))
+        if tables.get(kind) is None:
+            raise ValueError("a %s lap schedule needs %s_sets: the schedule names rows of that table" % (kind, kind))
+        out[kind] = _native.make_lap_schedule(rows, int(batch), len(tables[kind][0]))
+    if out and not lap_reports:
+        raise ValueError("lap_schedules need lap_reports >= laps: the per-lap statistics of a schedule come from the reports")
+    return out
+
+
+def lap_row_summary(reps, schedules, laps):
+    """Per schedule kind, LMPC lap k < laps and table row r, over the controllers that filed a report of lap k while on row r
+    (schedule[b][min(k, L - 1)] == r): how many, their mean steps, the share with a lane violation (viol_steps > 0) and the unsolved
+    QPs in total.  From the reports (BatchedController.lap_reports) and the host schedules alone."""
+    out = {}
+    for kind, sched in schedules.items():
+        L = sched.shape[1]
+        rows = []
+        for k in range(laps):
+            on = sched[:, min(k, L - 1)]
+            filed = reps["n"] > k
+            for r in np.unique(on):
+                m = filed & (on == r)
+                n = int(m.sum())
+                rows.append({"lap": k + 1, "row": int(r), "controllers": n,
+                             "steps_mean": float(reps["steps"][m, k].mean()) if n else 0.0,
+                             "violating_share": float((reps["viol_steps"][m, k] > 0).mean()) if n else 0.0,
+                             "unsolved": int(reps["unsolved"][m, k].sum(dtype=np.int64))})
+        out[kind] = rows
+    return out
+
+
 def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, poll=8, max_steps=0, seed=1234, local=None, warm=False,
         final=None, param_sets=None, vehicle_sets=None, books=None, track_sets=None, pool_groups=None, readiness="batch",
         capture=None, start=None, noise_sets=None, noise_streams=None, regression_sets=None, lap_budget=None, measurement_sets=None,
-        shape_sets=None, ss_laps_sets=None, lap_reports=None):
+        shape_sets=None, ss_laps_sets=None, lap_reports=None, lap_schedules=None):
     """One Monte-Carlo run on this rank's GPU (torch.distributed may or may not be initialised).  Returns a dict (all ranks).
     final: None, or a dict that receives the closed loop's end state (rollout_state) and the last step's solver report (step_results).
     books: None, or a dict that receives the lap books (books) and the health counters (flags_or, unsolved), and with lap_reports
@@ -173,8 +215,16 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     iterations).  The result gains "lap_reports_rank0", a summary per lap (lap_report_summary), every per-table entry gains the same
     list under "reports", and "lap_stats_rank0" covers every lap, taken from the reports' steps (equal to the lap books' lengths
     wherever no step found the record full, flag 256).  Without reports laps is at most 16, the laps the lap books keep.  capture
-    records L and start refuses another.  ValueError before any device work."""
+    records L and start refuses another.  ValueError before any device work.
+    lap_schedules: None, or {kind: rows} handed to BatchedController.set_lap_schedule after the seeding (or the restore), kind in
+    "vehicle", "noise", "measurement" and rows [L] or [batch, L] naming rows of vehicle_sets, noise_sets or measurement_sets
+    (conditions that change at the laps each controller reaches; entry 0 is the first LMPC lap).  Each kind needs its table and the
+    run needs lap_reports >= laps.  The result gains "per_lap_row_rank0": per kind, lap and row, the controllers on that row, their
+    mean steps, the share with a lane violation and the unsolved QPs (lap_row_summary).  capture records the schedules and start
+    refuses others.  ValueError before any device work."""
     L = check_lap_reports(lap_reports, laps)
+    scheds = check_lap_schedules(lap_schedules, batch, L, {"vehicle": vehicle_sets, "noise": noise_sets,
+                                                           "measurement": measurement_sets})
     budget = _native.make_lap_budget(lap_budget, int(batch))       # ValueError where set_lap_budget would refuse, before any device work
     N, M = handle_shape(shape_sets)
     numSS_it = rp.lmpc_params(N)[0]
@@ -187,7 +237,7 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     if ss_laps_sets is not None:
         _native.make_ss_laps_sets(ss_laps_sets[0], ss_laps_sets[1], int(batch), numSS_it, points)
     if start is not None:
-        _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget, shape_sets, L)
+        _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget, shape_sets, L, scheds)
     if capture is not None and not isinstance(capture, dict):
         raise ValueError("capture is a dict that receives the run's end state")
     if readiness not in ("batch", "group"):
@@ -251,6 +301,8 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         c.sync()
         pid_s = 0.0
         restore_s = time.perf_counter() - t0
+    for kind, row_of_lap in scheds.items():                # after the seeding: entry 0 is the first LMPC lap
+        c.set_lap_schedule(kind, row_of_lap)
     if budget is not None:
         c.set_lap_budget(budget)
         driven0 = _driven_steps(c.books(), c.rollout_state())
@@ -315,7 +367,8 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         c.sync()
         capture.update(capture_s=time.perf_counter() - tc, **sched.state(steps), batch=B, laps=laps, mode=mode, readiness=readiness,
                        poll=poll, warm=bool(warm), pool_groups=G, layout=c.snapshot_layout(),
-                       lap_budget=None if budget is None else budget.tolist())
+                       lap_budget=None if budget is None else budget.tolist(),
+                       lap_schedules={kind: row_of_lap.tolist() for kind, row_of_lap in scheds.items()})
     flags_or, unsolved = c.rollout_health()
     reps = c.lap_reports() if L else None
     lens, n_laps = (reps["steps"], reps["n"]) if L else (bk["lap_hist"], bk["lap_n"])
@@ -336,6 +389,8 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     if L:
         out["lap_reports"] = L
         out["lap_reports_rank0"] = lap_report_summary(reps, np.ones(B, bool), laps)
+    if scheds:
+        out["per_lap_row_rank0"] = lap_row_summary(reps, scheds, laps)
     for args, _, key in tables:
         if args is not None and key is not None:
             idx = np.asarray(args[1]).reshape(B)
@@ -400,9 +455,10 @@ def _driven_steps(bk, state):
     return int(filed.sum(dtype=np.int64) + state["cl_len"].sum(dtype=np.int64))
 
 
-def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget=None, shape_sets=None, lap_reports=0):
-    """The refusals of run(start=...), before any device work: a start that does not match this run (report capacity included),
-    laps not above the captured laps, or a lap budget below the captured one."""
+def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget=None, shape_sets=None, lap_reports=0,
+                 lap_schedules=None):
+    """The refusals of run(start=...), before any device work: a start that does not match this run (report capacity and lap
+    schedules included), laps not above the captured laps, or a lap budget below the captured one."""
     if not isinstance(start, dict):
         raise ValueError("start is a capture dict of an earlier run")
     need = ("records", "clock") + sharding.ExchangeSchedule.FIELDS + ("batch", "laps", "mode", "readiness", "poll", "warm",
@@ -428,6 +484,11 @@ def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, b
     had = int(start["layout"].get("lap_reports", 0))
     if had != int(lap_reports):
         raise ValueError("start records have lap_reports = %d, this run %d" % (had, int(lap_reports)))
+    had = {k: np.asarray(v) for k, v in (start.get("lap_schedules") or {}).items()}
+    mine = lap_schedules or {}
+    if sorted(had) != sorted(mine) or any(not np.array_equal(had[k], mine[k]) for k in had):
+        raise ValueError("start was captured with lap_schedules for %s, this run has %s (or other rows): a run resumes under the "
+                         "schedules it was captured with" % (sorted(had) or "none", sorted(mine) or "none"))
     for k, v in layout(warm, shape_sets).items():
         if int(start["layout"].get(k, -1)) != v:
             raise ValueError("start records have %s = %s, this run's controllers %d" % (k, start["layout"].get(k), v))

@@ -516,6 +516,35 @@ int lmpc_rollout_enable_lap_reports(lmpc_handle* h, int max_laps);
  * unused) into host arrays, either may be NULL.  LMPC_E_STATE without reports.  Synchronises. */
 int lmpc_rollout_get_lap_reports(lmpc_handle* h, lmpc_lap_report* rows, int* n);
 int lmpc_sizeof_lap_report(void);
+/* Lap schedules (no reference counterpart; DESIGN.md, "Per-lap schedules"): a plant-side table whose row changes at the laps a
+ * controller reaches -- a track that gets wet at lap 10, a car whose mass changes, a sensor that degrades.  For the table `table`
+ * (vehicles of lmpc_rollout_set_vehicles, process and PID noise of lmpc_rollout_set_noise, measurement noise of
+ * lmpc_rollout_set_measurement_noise), row_of_lap is a host array [batch][nlaps], 1 <= nlaps <= 1024:
+ *   - In every lmpc_rollout_step (modes 0, 1, 2) controller b reads row row_of_lap[b][min(lap_n[b], nlaps - 1)] of the table in
+ *     place of its set_of_instance[b], in the measurement kernel and in the simulator.  lap_n is the count of laps handed over since
+ *     the seeding (lmpc_books_get), read as the step starts: a lap is driven entirely under its entry and a change takes effect on
+ *     the first step after the hand-over that advanced lap_n.  Entry 0 is the first LMPC (or LTV / LTI-MPC) lap after the seeding;
+ *     the last entry holds for every later lap.
+ *   - The PID lap (lmpc_rollout_pid_step, its pid_input_kernel noise included) and the host-driven entry points ignore schedules,
+ *     as they ignore lap budgets: the seeding lap is driven under set_of_instance.  The host-slot hand-over
+ *     (lmpc_rollout_commit_laps) does not advance lap_n, so a run that hands over through it stays at the entry lap_n names.
+ *   - A retired controller (lmpc_rollout_set_lap_budget) reads nothing.  The schedule stays with the handle and is not part of a
+ *     snapshot record; lap_n is, so a restored controller resumes at its entry.
+ *   - Tracks, QP parameters, regression models, shapes and safe-set lap counts are not schedulable: a track change invalidates every
+ *     stored lap, and schedules of the controller's own tables are a separate question.
+ *   - nlaps == 0 with row_of_lap == NULL removes the schedule.  Refusals, each leaving the handle as it was: LMPC_E_STATE without
+ *     lmpc_store_create (the lap books hold lap_n) or lmpc_rollout_create, or for LMPC_SCHEDULE_MEASUREMENT without a measurement
+ *     table; LMPC_E_INVALID for an unknown table, nlaps outside 1 .. 1024 with an array, nlaps != 0 without one or the reverse, or
+ *     an entry outside [0, nsets) of the table as installed (a table reverted with nsets == 0 has one row).
+ *   - Both install orders: while a schedule is installed, lmpc_rollout_set_vehicles / _noise / _measurement_noise refuse
+ *     (LMPC_E_INVALID) a table whose rows do not cover the schedule's largest entry, an nsets == 0 revert to one row and the removal
+ *     of the measurement table included.
+ *   - The call synchronises the handle's streams before it replaces the schedule.  It is allowed at any time.  Without a schedule
+ *     the kernels run the code they run without this feature (template instantiations). */
+#define LMPC_SCHEDULE_VEHICLE      0
+#define LMPC_SCHEDULE_NOISE        1
+#define LMPC_SCHEDULE_MEASUREMENT  2
+int lmpc_rollout_set_lap_schedule(lmpc_handle* h, int table, int nlaps, const int* row_of_lap);
 int lmpc_rollout_sysid(lmpc_handle* h, double lamb, double* abc_host, int* flags_host);
 int lmpc_rollout_seed_from_record(lmpc_handle* h, int copies, int ss_slot0, int model_slot0);
 int lmpc_rollout_get_lap(lmpc_handle* h, int inst, int* T, double* x, double* u);              /* closed-loop record   */

@@ -187,6 +187,7 @@ def lib():
     L.lmpc_rollout_set_lap_budget.argtypes = [_vp, _vp]
     L.lmpc_rollout_enable_lap_reports.argtypes = [_vp, C.c_int]
     L.lmpc_rollout_get_lap_reports.argtypes = [_vp, _vp, _vp]
+    L.lmpc_rollout_set_lap_schedule.argtypes = [_vp, C.c_int, C.c_int, _vp]
     L.lmpc_set_tracks.argtypes = [_vp, C.POINTER(TrackParams), C.c_int, _vp]
     L.lmpc_set_regression_sets.argtypes = [_vp, C.POINTER(RegressionParams), C.c_int, _vp]
     L.lmpc_set_shapes.argtypes = [_vp, C.POINTER(ShapeParams), C.c_int, _vp]
@@ -524,6 +525,31 @@ def make_lap_budget(budget, batch):
     if np.ndim(budget) == 0:
         budget = [budget] * batch
     return _int_per_controller(budget, batch, 1, "lap budget")
+
+
+# lmpc_rollout_set_lap_schedule: the tables a lap schedule can index (LMPC_SCHEDULE_*) and the longest schedule
+LAP_SCHEDULE_TABLES = {"vehicle": 0, "noise": 1, "measurement": 2}
+MAX_LAP_SCHEDULE = 1024
+
+
+def make_lap_schedule(rows, batch, nsets):
+    """A lap schedule for ``lmpc_rollout_set_lap_schedule``: the row of a table of ``nsets`` rows that every controller drives each
+    LMPC lap under, ``rows[L]`` (the same for every controller) or ``rows[batch, L]``, 1 <= L <= 1024; the last entry holds for
+    every later lap.  Raises ValueError where the library would refuse: another shape, entries that are not integers, L outside
+    1 .. 1024, or an entry outside [0, nsets).  Returns the [batch, L] schedule as a contiguous int32 array."""
+    a = np.asarray(rows)
+    if a.ndim not in (1, 2) or a.size == 0:
+        raise ValueError("a lap schedule is [L] or [batch, L] with L >= 1, got shape %s" % (a.shape,))
+    if a.dtype.kind not in "iu" and not (a.dtype.kind == "f" and np.all(np.isfinite(a)) and np.array_equal(a, np.round(a))):
+        raise ValueError("lap schedule entries must be integer row numbers")
+    if a.ndim == 2 and a.shape[0] != int(batch):
+        raise ValueError("a [batch, L] lap schedule needs %d rows, got %d" % (int(batch), a.shape[0]))
+    L = a.shape[-1]
+    if not 1 <= L <= MAX_LAP_SCHEDULE:
+        raise ValueError("a lap schedule holds 1 .. %d laps, got %d" % (MAX_LAP_SCHEDULE, L))
+    if a.min() < 0 or a.max() >= int(nsets):
+        raise ValueError("lap schedule entry out of range [0, %d): the table has %d row(s)" % (int(nsets), int(nsets)))
+    return np.ascontiguousarray(np.broadcast_to(a, (int(batch), L)), dtype=np.int32)
 
 
 # the scaling entries the regression sets admit: 0 or this range (the fp32 pre-filter of K1 is certified there, csrc/safeset.cuh)

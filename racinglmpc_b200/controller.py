@@ -68,6 +68,10 @@ class BatchedController:
         self._pool_groups = 1
         self._shapes = None                                 # (shapes, index) of set_shapes, or None: the handle's own shape
         self._ss_laps = None                                # numSS_it of every controller (set_ss_laps), or None: the handle's
+        # rows of the plant-side tables a lap schedule indexes (the defaults: one reference vehicle and noise, no measurement
+        # table) and the installed schedules [B, L] of set_lap_schedule
+        self._table_rows = {"vehicle": 1, "noise": 1, "measurement": 0}
+        self._lap_schedules = {}
         self._sel = np.zeros((self.B, nit), np.int32); self._isp = np.zeros((self.B, nit), np.int32)
         self._prev = -np.ones(self.B, np.int32); self._used = np.zeros((self.B, self.trToUse), np.int32)
 
@@ -115,17 +119,25 @@ class BatchedController:
         """Per-controller vehicles of the device simulator (a Monte-Carlo over the plant in one batch): controller b is driven
         with ``vehicles[index[b]]`` (objects with the reference's ten field names, e.g. reference_params.VehicleParams) by every
         later ``rollout_step`` and ``rollout_pid_step``.  ``index`` is required with ``vehicles``.  ``vehicles=None`` (no index)
-        returns to the reference vehicle.  Independent of ``set_param_sets``.  Waits for work already enqueued."""
+        returns to the reference vehicle.  Independent of ``set_param_sets``.  While a vehicle lap schedule is installed the new
+        table must cover its largest entry (ValueError).  Waits for work already enqueued."""
+        rows = 1 if vehicles is None else len(vehicles)
+        self._check_schedule_cover("vehicle", rows)
         self._install(self._lib.lmpc_rollout_set_vehicles, "vehicles", vehicles, index,
                       lambda: nat.make_vehicle_sets(vehicles, index, self.B))
+        self._table_rows["vehicle"] = rows
 
     def set_noise(self, noises, index=None):
         """Per-controller noise models of the device closed loop (a robustness study in one batch): controller b draws the
         simulator's and the PID's noise with ``noises[index[b]]`` (objects with the fields of reference_params.NoiseParams) in
         every later ``rollout_step`` and ``rollout_pid_step``, Philox or host-given draws alike.  ``index`` is required with
         ``noises``.  ``noises=None`` (no index) returns to the reference's noise.  Independent of ``set_param_sets``,
-        ``set_vehicles``, ``set_tracks`` and the pool groups; allowed in the middle of a run.  Waits for work already enqueued."""
+        ``set_vehicles``, ``set_tracks`` and the pool groups; allowed in the middle of a run.  While a noise lap schedule is
+        installed the new table must cover its largest entry (ValueError).  Waits for work already enqueued."""
+        rows = 1 if noises is None else len(noises)
+        self._check_schedule_cover("noise", rows)
         self._install(self._lib.lmpc_rollout_set_noise, "noises", noises, index, lambda: nat.make_noise_sets(noises, index, self.B))
+        self._table_rows["noise"] = rows
 
     def set_noise_streams(self, streams=None):
         """Common random numbers: the Philox draws of controller b are keyed by ``streams[b]`` (integers >= 0, repeats allowed)
@@ -143,9 +155,13 @@ class BatchedController:
         laps and learned models are measured data.  The plant, ``rollout_state`` and the trace keep x.  The draws are Philox,
         keyed apart from the process and PID noise and paired by ``set_noise_streams``.  ``index`` is required with ``meas``.
         ``meas=None`` (no index) removes the table: the controllers read x again and no kernel is added to a step.  Needs
-        ``enable_rollout``; allowed in the middle of a run; not part of a snapshot.  Waits for work already enqueued."""
+        ``enable_rollout``; allowed in the middle of a run; not part of a snapshot.  While a measurement lap schedule is installed
+        the new table must cover its largest entry, and it cannot be removed (ValueError).  Waits for work already enqueued."""
+        rows = 0 if meas is None else len(meas)
+        self._check_schedule_cover("measurement", rows)
         self._install(self._lib.lmpc_rollout_set_measurement_noise, "meas", meas, index,
                       lambda: nat.make_measurement_sets(meas, index, self.B))
+        self._table_rows["measurement"] = rows
 
     def set_lap_budget(self, budget=None):
         """Lap budgets of the device closed loop: controller b retires once it has handed over ``budget[b]`` laps (one integer
@@ -156,6 +172,45 @@ class BatchedController:
         the middle of a run; not part of a snapshot.  Waits for work already enqueued."""
         b = nat.make_lap_budget(budget, self.B)
         nat.check(self._lib.lmpc_rollout_set_lap_budget(self._h, nat.ptr(b)))
+
+    def _check_schedule_cover(self, kind, rows):
+        """Both install orders of a lap schedule: a table of `rows` rows must cover the largest entry of an installed schedule."""
+        s = self._lap_schedules.get(kind)
+        if s is not None and int(s.max()) >= rows:
+            raise ValueError("the %s lap schedule names row %d and the new table has %d row(s): install a covering schedule first "
+                             "or remove it" % (kind, int(s.max()), rows))
+
+    def set_lap_schedule(self, kind, rows=None):
+        """Lap schedules of the device closed loop (conditions that change while the controllers learn: a track that gets wet at
+        lap 10, a car whose mass changes, a sensor that degrades): ``kind`` is "vehicle", "noise" or "measurement", and in every
+        later ``rollout_step`` controller b drives LMPC lap k (k = 0 is the first lap after the seeding, lap_n of ``books``)
+        under row ``rows[b][min(k, L - 1)]`` of that table (``set_vehicles``, ``set_noise``, ``set_measurement_noise``) in place
+        of its index.  ``rows`` is [L] (the same for every controller) or [batch, L], 1 <= L <= 1024, entries in the table's rows;
+        ``rows=None`` removes the schedule.  The change takes effect on the first step after the hand-over that advanced lap_n
+        (``rollout_commit_laps_dev``; the host-slot hand-over does not count laps).  The PID lap ignores schedules.  Needs
+        ``enable_rollout``; allowed at any time; not part of a snapshot (lap_n is, so a restored controller resumes at its entry).
+        ValueError before any native call where the library would refuse.  Waits for work already enqueued."""
+        if kind not in nat.LAP_SCHEDULE_TABLES:
+            raise ValueError("kind is one of %s, got %r" % (sorted(nat.LAP_SCHEDULE_TABLES), kind))
+        if not hasattr(self, "Tcl"):
+            raise ValueError("set_lap_schedule needs enable_rollout first")
+        k = nat.LAP_SCHEDULE_TABLES[kind]
+        if rows is None:
+            nat.check(self._lib.lmpc_rollout_set_lap_schedule(self._h, k, 0, None))
+            self._lap_schedules.pop(kind, None)
+            return
+        if kind == "measurement" and not self._table_rows[kind]:
+            raise ValueError("a measurement lap schedule needs a measurement table (set_measurement_noise)")
+        s = nat.make_lap_schedule(rows, self.B, self._table_rows[kind])
+        nat.check(self._lib.lmpc_rollout_set_lap_schedule(self._h, k, s.shape[1], nat.ptr(s)))
+        self._lap_schedules[kind] = s
+
+    def lap_schedule_of(self, kind):
+        """The installed lap schedule of ``kind`` as [batch, L] int32 (a copy), or None."""
+        if kind not in nat.LAP_SCHEDULE_TABLES:
+            raise ValueError("kind is one of %s, got %r" % (sorted(nat.LAP_SCHEDULE_TABLES), kind))
+        s = self._lap_schedules.get(kind)
+        return None if s is None else s.copy()
 
     def set_regression(self, regs, index=None):
         """Per-controller regression models (a study of the learned model's settings in one batch): controller b identifies its

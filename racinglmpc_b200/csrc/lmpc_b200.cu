@@ -15,6 +15,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string>
+#include <algorithm>
 #include <new>
 #include <ctype.h>
 #include <errno.h>
@@ -163,6 +164,10 @@ struct lmpc_handle {
     double* d_xmeas;
     // lap budgets (lmpc_rollout_set_lap_budget): laps every controller drives before it retires, or none for no budget
     HandleTable<int> budget;
+    // lap schedules (lmpc_rollout_set_lap_schedule) of the vehicle, noise and measurement tables (LMPC_SCHEDULE_*): rows [B][L] of
+    // the table per lap and no index, or none; sched_L[k] = L
+    HandleTable<int> sched[3];
+    int sched_L[3];
     // device lap books (lapbooks.cuh, allocated with the store): slot tables of both pools, lap history, exchange scratch
     LapBooks bk;
     int *d_poolidx, *d_stats;
@@ -268,6 +273,7 @@ static void free_tables(lmpc_handle* h, unsigned owners) {
     };
     release(h->sets, OWN_HANDLE); release(h->veh, OWN_HANDLE); release(h->noise, OWN_HANDLE); release(h->streams, OWN_HANDLE);
     release(h->meas, OWN_HANDLE); release(h->budget, OWN_HANDLE); release(h->trk, OWN_STORE); release(h->reg, OWN_STORE); release(h->pool_grp, OWN_STORE);
+    for (auto& t : h->sched) release(t, OWN_HANDLE);
     release(h->shp, OWN_STORE); release(h->shp_order, OWN_STORE); release(h->own_c, OWN_HANDLE); release(h->ssl, OWN_STORE);
     if (owners & OWN_STORE) h->shp_cells.clear();
 }
@@ -504,6 +510,10 @@ static Tracks tracks(const lmpc_handle* h) { return h->trk.view(); }
 // The lap budgets as the kernels of the device-resident closed loop take them.  Everything else (the host-driven entry points,
 // the PID lap, the host-slot hand-over) passes LapBudget{}: nobody is retired there.
 static LapBudget lap_budget(const lmpc_handle* h) { return LapBudget{h->budget.idx, h->bk.lap_n}; }
+
+// The lap schedule of table k (LMPC_SCHEDULE_*) as lmpc_rollout_step's kernels take it; the same places that pass LapBudget{} pass
+// LapSchedule{} (the table's own index)
+static LapSchedule lap_schedule(const lmpc_handle* h, int k) { return LapSchedule{h->sched[k].tab, h->sched_L[k], h->bk.lap_n}; }
 
 // The report buffers and the QP constants the kernels of the closed loop read (all null without reports: only the REPORTS
 // instantiations read them)
@@ -1595,13 +1605,13 @@ static SimArgs sim_args(const lmpc_handle* h, const double* z, unsigned long lon
 
 // The state the controllers see this step (DESIGN.md, "Per-controller measurement noise"): with a measurement table, *y is the
 // measured state measure_kernel forms from the plant state and the clock; without one, *y is the plant state and nothing runs.
-static int measure(lmpc_handle* h, unsigned long long seed, LapBudget retire, const double** y) {
+static int measure(lmpc_handle* h, unsigned long long seed, LapBudget retire, LapSchedule sched, const double** y) {
     *y = h->d_rx[h->cur];
     if (!h->meas.tab) return LMPC_OK;
     MeasArgs ma;
     ma.batch = h->batch; ma.x = h->d_rx[h->cur]; ma.y = h->d_xmeas; ma.seed = seed; ma.step = h->sim_step;
     ma.meas = h->meas.view(); ma.streams = h->streams.idx; ma.retire = retire;
-    measure_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(ma);
+    (sched.rows ? measure_kernel<true> : measure_kernel<false>)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(ma, sched);
     CK(cudaGetLastError());
     h->launches += 1;
     *y = h->d_xmeas;
@@ -1618,7 +1628,7 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
     const double* xc = h->d_rx[h->cur];
     const LapBudget retire = lap_budget(h);
     const double* y = nullptr;
-    if ((rc = measure(h, seed, retire, &y)) != LMPC_OK) return rc;
+    if ((rc = measure(h, seed, retire, lap_schedule(h, LMPC_SCHEDULE_MEASUREMENT), &y)) != LMPC_OK) return rc;
     if (z_host) CK(cudaMemcpyAsync(h->d_z, z_host, sizeof(double) * h->batch * 3, cudaMemcpyHostToDevice, h->stream));
     if (mode == 2) {
         CK(cudaMemsetAsync(h->d_flags, 0, sizeof(int) * h->batch, h->stream));
@@ -1648,7 +1658,10 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
     SimArgs sa = sim_args(h, z_host ? h->d_z : nullptr, seed);                       // SysModel.py:40 (dynModel)
     sa.flags = h->d_flags; sa.status = q.status; sa.health = h->d_health; sa.retire = retire;
     if (h->meas.tab) sa.rec_x = y;
-    (h->rep_L ? sim_step_kernel<true> : sim_step_kernel<false>)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->mc, sa, reports(h), q.iters);
+    const LapSchedule vs = lap_schedule(h, LMPC_SCHEDULE_VEHICLE), ns = lap_schedule(h, LMPC_SCHEDULE_NOISE);
+    (vs.rows || ns.rows ? (h->rep_L ? sim_step_kernel<true, true> : sim_step_kernel<false, true>)
+                        : (h->rep_L ? sim_step_kernel<true, false> : sim_step_kernel<false, false>))<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(
+        h->mc, sa, reports(h), q.iters, vs, ns);
     CK(cudaGetLastError());
     h->launches += 1;
     h->cur ^= 1;
@@ -1662,7 +1675,7 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
 int lmpc_rollout_pid_step(lmpc_handle* h, double vt, const double* z_pid_host, const double* z_sim_host, unsigned long long seed) {
     if (int rc = need_rollout(h)) return rc;
     const double* y = nullptr;                   // the PID's input and the record's state rows (measure)
-    if (int rc = measure(h, seed, LapBudget{}, &y)) return rc;
+    if (int rc = measure(h, seed, LapBudget{}, LapSchedule{}, &y)) return rc;
     if (z_pid_host) CK(cudaMemcpyAsync(h->d_zpid, z_pid_host, sizeof(double) * h->batch * 2, cudaMemcpyHostToDevice, h->stream));
     if (z_sim_host) CK(cudaMemcpyAsync(h->d_z, z_sim_host, sizeof(double) * h->batch * 3, cudaMemcpyHostToDevice, h->stream));
     PidArgs pa;
@@ -1673,7 +1686,8 @@ int lmpc_rollout_pid_step(lmpc_handle* h, double vt, const double* z_pid_host, c
     SimArgs sa = sim_args(h, z_sim_host ? h->d_z : nullptr, seed);
     sa.health = h->d_health;          // no step flags or QP status here: only the simulator's own bits
     if (h->meas.tab) sa.rec_x = y;
-    (h->rep_L ? sim_step_kernel<true> : sim_step_kernel<false>)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->mc, sa, reports(h), nullptr);
+    (h->rep_L ? sim_step_kernel<true, false> : sim_step_kernel<false, false>)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(
+        h->mc, sa, reports(h), nullptr, LapSchedule{}, LapSchedule{});
     CK(cudaGetLastError());
     h->launches += 2;
     h->cur ^= 1;
@@ -1682,10 +1696,21 @@ int lmpc_rollout_pid_step(lmpc_handle* h, double vt, const double* z_pid_host, c
     return LMPC_OK;
 }
 
+// Both install orders of a lap schedule: while schedule k indexes a table, a new table of nrows rows must cover its largest entry
+static int check_schedule_cover(const lmpc_handle* h, const char* who, int k, int nrows) {
+    const std::vector<int>& r = h->sched[k].rows;
+    if (r.empty()) return LMPC_OK;
+    const int top = *std::max_element(r.begin(), r.end());
+    if (top < nrows) return LMPC_OK;
+    return fail(LMPC_E_INVALID, std::string(who) + ": the installed lap schedule names row " + std::to_string(top) + ", the new table has " +
+                                    std::to_string(nrows) + " row(s); install a covering schedule first or remove it");
+}
+
 // Per-controller vehicles: m, Iz, lf, lr positive and all ten values finite; nsets == 0 returns to the reference vehicle.
 int lmpc_rollout_set_vehicles(lmpc_handle* h, const lmpc_vehicle_params* sets, int nsets, const int* set_of_instance) {
     static const char* who = "lmpc_rollout_set_vehicles";
     if (!h) return fail(LMPC_E_INVALID, "null handle");
+    if (int rc = check_schedule_cover(h, who, LMPC_SCHEDULE_VEHICLE, nsets > 0 ? nsets : 1)) return rc;
     const lmpc_vehicle_params ref = reference_vehicle();
     return install_table(h, who, h->veh, sets, nsets, set_of_instance, &ref, [&](int k, lmpc_vehicle_params& row) {
         const lmpc_vehicle_params& v = sets[k];
@@ -1705,6 +1730,7 @@ static_assert(sizeof(lmpc_noise_params) == 11 * sizeof(double), "lmpc_noise_para
 int lmpc_rollout_set_noise(lmpc_handle* h, const lmpc_noise_params* sets, int nsets, const int* set_of_instance) {
     static const char* who = "lmpc_rollout_set_noise";
     if (!h) return fail(LMPC_E_INVALID, "null handle");
+    if (int rc = check_schedule_cover(h, who, LMPC_SCHEDULE_NOISE, nsets > 0 ? nsets : 1)) return rc;
     const lmpc_noise_params ref = reference_noise();
     return install_table(h, who, h->noise, sets, nsets, set_of_instance, &ref, [&](int k, lmpc_noise_params& row) {
         const double* v = (const double*)&sets[k];
@@ -1733,6 +1759,7 @@ static_assert(sizeof(lmpc_measurement_params) == 12 * sizeof(double), "lmpc_meas
 int lmpc_rollout_set_measurement_noise(lmpc_handle* h, const lmpc_measurement_params* sets, int nsets, const int* set_of_instance) {
     static const char* who = "lmpc_rollout_set_measurement_noise";
     if (int rc = need_rollout(h)) return rc;
+    if (int rc = check_schedule_cover(h, who, LMPC_SCHEDULE_MEASUREMENT, nsets)) return rc;
     return install_table(h, who, h->meas, sets, nsets, set_of_instance, (const lmpc_measurement_params*)nullptr,
                          [&](int k, lmpc_measurement_params& row) {
         const double* v = (const double*)&sets[k];
@@ -1753,6 +1780,31 @@ int lmpc_rollout_set_lap_budget(lmpc_handle* h, const int* budget_of_instance) {
         if (budget_of_instance[b] < 1)
             return fail(LMPC_E_INVALID, std::string(who) + ": budget of instance " + std::to_string(b) + " is below 1");
     return swap_table<int>(h, who, h->budget, nullptr, 0, budget_of_instance);
+}
+
+// Lap schedules: row_of_lap[B][nlaps] of table `table`, every entry a row of the table as installed; nlaps 0 + NULL removes it.
+// Stored as a table whose rows are the schedule and which has no index (swap_table), so a failed allocation changes nothing.
+int lmpc_rollout_set_lap_schedule(lmpc_handle* h, int table, int nlaps, const int* row_of_lap) {
+    static const char* who = "lmpc_rollout_set_lap_schedule";
+    if (int rc = need_rollout(h)) return rc;
+    const std::string w(who);
+    if (table < LMPC_SCHEDULE_VEHICLE || table > LMPC_SCHEDULE_MEASUREMENT)
+        return fail(LMPC_E_INVALID, w + ": table must be LMPC_SCHEDULE_VEHICLE, _NOISE or _MEASUREMENT");
+    const size_t nrows = table == LMPC_SCHEDULE_VEHICLE ? h->veh.rows.size()
+                       : table == LMPC_SCHEDULE_NOISE   ? h->noise.rows.size() : h->meas.rows.size();
+    if (table == LMPC_SCHEDULE_MEASUREMENT && !h->meas.tab && row_of_lap)
+        return fail(LMPC_E_STATE, w + ": a measurement schedule needs a measurement table (lmpc_rollout_set_measurement_noise)");
+    if ((nlaps == 0) != (row_of_lap == nullptr))
+        return fail(LMPC_E_INVALID, w + ": nlaps == 0 goes with a NULL row_of_lap, nlaps >= 1 with an array");
+    if (nlaps < 0 || nlaps > 1024) return fail(LMPC_E_INVALID, w + ": nlaps must be 0 .. 1024");
+    const size_t n = (size_t)h->batch * nlaps;
+    for (size_t i = 0; i < n; ++i)
+        if (row_of_lap[i] < 0 || (size_t)row_of_lap[i] >= nrows)
+            return fail(LMPC_E_INVALID, w + ": entry " + std::to_string(i % nlaps) + " of controller " + std::to_string(i / nlaps) +
+                                            " is outside the table's " + std::to_string(nrows) + " row(s)");
+    if (int rc = swap_table<int>(h, who, h->sched[table], row_of_lap, (int)n, nullptr)) return rc;
+    h->sched_L[table] = nlaps;
+    return LMPC_OK;
 }
 
 // Per-lap reports: 1 <= max_laps <= 1024 allocates an empty table (refused while a record holds rows), 0 frees it.  New buffers are

@@ -1013,12 +1013,15 @@ constexpr int SIM_RECORD_FULL = 256;
 
 }  // namespace lmpc
 #include <curand_kernel.h>
+#include "lap_schedule.cuh"
 namespace lmpc {
 
 // REPORTS: the step is also added to the controller's running report row (report_step) with its QP's status a.status and
-// iterations rep_iters, both null for a PID step.  The parameters after a are read only by that instantiation.
-template <bool REPORTS>
-__global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimArgs a, const LapReports rep, const int* rep_iters) {
+// iterations rep_iters, both null for a PID step.  SCHED: the vehicle and noise rows come from the lap schedules veh_s and
+// noise_s (lap_schedule.cuh; either may be null).  The parameters after a are read only by those instantiations.
+template <bool REPORTS, bool SCHED>
+__global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimArgs a, const LapReports rep, const int* rep_iters,
+                                const LapSchedule veh_s, const LapSchedule noise_s) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= a.batch) return;
     if (a.retire.retired(b)) {
@@ -1032,7 +1035,7 @@ __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimA
         if (a.status && a.status[b] != 1) a.health[a.batch + b] += 1;
     }
     // vehicle parameters, SysModel.py:61-70
-    const lmpc_vehicle_params& v = a.veh.of(b);
+    const lmpc_vehicle_params& v = SCHED ? veh_s.of(a.veh, b) : a.veh.of(b);
     const double mass = v.m, lf = v.lf, lr = v.lr, Iz = v.Iz;
     const double Df = v.Df, Cf = v.Cf, Bf = v.Bf;
     const double Dr = v.Dr, Cr = v.Cr, Br = v.Br;
@@ -1095,7 +1098,7 @@ __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimA
         z0 = n01.x; z1 = n01.y; z2 = n23.x;
     }
     // noise parameters, SysModel.py:139-145
-    const lmpc_noise_params& nz = a.noise.of(b);
+    const lmpc_noise_params& nz = SCHED ? noise_s.of(a.noise, b) : a.noise.of(b);
     const double n_vx = fmax(-nz.sim_clip[0], fmin(z0 * nz.sim_sigma[0], nz.sim_clip[0]));
     const double n_vy = fmax(-nz.sim_clip[1], fmin(z1 * nz.sim_sigma[1], nz.sim_clip[1]));
     const double n_wz = fmax(-nz.sim_clip[2], fmin(z2 * nz.sim_sigma[2], nz.sim_clip[2]));
@@ -1152,7 +1155,7 @@ __global__ void pid_input_kernel(const PidArgs a) {
 // curvilinear channels, n_j = clip(z_j * sigma_j, +-clip_j) in the form of the process noise, z_j standard normal from Philox keyed
 // by (seed ^ K_MEAS, stream, clock) -- three curand_normal2_double calls, 12 raw 32-bit draws, in blocks of 16 per step.  Where
 // n_j == 0 the state is copied, so a zero set gives y == x bit for bit (-0.0 + 0.0 would be +0.0).  One thread per controller; a
-// retired controller draws nothing and writes nothing.
+// retired controller draws nothing and writes nothing.  SCHED: the row comes from the lap schedule meas_s (lap_schedule.cuh).
 constexpr unsigned long long K_MEAS = 0xD1B54A32D192ED03ull;     // distinct from the PID's key constant
 struct MeasArgs {
     int batch;
@@ -1163,7 +1166,8 @@ struct MeasArgs {
     const int* streams;                    // [B] Philox stream of every instance, or nullptr: b
     LapBudget retire;
 };
-__global__ void measure_kernel(const MeasArgs a) {
+template <bool SCHED>
+__global__ void measure_kernel(const MeasArgs a, const LapSchedule meas_s) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= a.batch || a.retire.retired(b)) return;
     curandStatePhilox4_32_10_t st;
@@ -1173,7 +1177,7 @@ __global__ void measure_kernel(const MeasArgs a) {
     const double2 n23 = curand_normal2_double(&st);
     const double2 n45 = curand_normal2_double(&st);
     const double z[6] = {n01.x, n01.y, n23.x, n23.y, n45.x, n45.y};
-    const lmpc_measurement_params& m = a.meas.of(b);
+    const lmpc_measurement_params& m = SCHED ? meas_s.of(a.meas, b) : a.meas.of(b);
     const double* x = a.x + (size_t)b * 6;
     double* y = a.y + (size_t)b * 6;
 #pragma unroll

@@ -8,8 +8,10 @@ and the instantiations that run without a per-controller table of the other kern
 across their untemplated names:
   default  knn_ltv_regress_kernel, ss_select_kernel, shift_state_kernel (<false>: no shape or lap-count table),
            books_refresh_kernel, commit_laps_books_kernel, seed_books_kernel, pool_import_kernel (<false>: no lap-count table;
-           <false, false>: no lap-count table and no lap reports) and sim_step_kernel, commit_laps_kernel, seed_from_record_kernel
-           (<false>: no lap reports)
+           <false, false>: no lap-count table and no lap reports), commit_laps_kernel, seed_from_record_kernel (<false>: no lap
+           reports), sim_step_kernel (<false> or <false, false>: no lap reports and no lap schedule) and measure_kernel (<false>:
+           no lap schedule)
+  reports  sim_step_kernel<true> or <true, false>: lap reports and no lap schedule
 and compared by instruction text (cuobjdump -sass without addresses and encodings).  Each differing line pair is classified:
   dfma-swap   one DFMA with its two factors exchanged (a*b+c = b*a+c)
   lds-swap    LDS.128 loads of unchanged addresses whose destination registers are permuted among themselves
@@ -27,7 +29,8 @@ import sys
 NAME = re.compile(r"^(?:void )?(ftocp_kernel|ftocp_sets_kernel)<(\d+), (\d+), 2, 4(?:, (true|false))?>")
 DEFAULT = re.compile(r"^(?:void )?lmpc::(knn_ltv_regress_kernel|ss_select_kernel|shift_state_kernel|books_refresh_kernel|"
                      r"commit_laps_books_kernel|seed_books_kernel|pool_import_kernel|sim_step_kernel|commit_laps_kernel|"
-                     r"seed_from_record_kernel)(<false>|<false, false>)?\(")
+                     r"seed_from_record_kernel|measure_kernel)(<false>|<false, false>)?\(")
+REPORTS = re.compile(r"^(?:void )?lmpc::(sim_step_kernel)<true(?:, false)?>\(")
 
 
 def kernels(path):
@@ -40,12 +43,15 @@ def kernels(path):
             name = subprocess.run(["c++filt", m.group(1)], capture_output=True, text=True).stdout.strip()
             k = NAME.match(name)
             d = DEFAULT.match(name)
+            r = REPORTS.match(name)
             cur = None
             if k:
                 sets = k.group(1) == "ftocp_sets_kernel" or k.group(4) == "true"
                 cur = out.setdefault(("sets" if sets else "uniform", int(k.group(2)), int(k.group(3))), [])
             elif d:
                 cur = out.setdefault(("default", d.group(1), 0), [])
+            elif r:
+                cur = out.setdefault(("reports", r.group(1), 0), [])
             continue
         m = re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(.*?)\s*;", line)
         if m and cur is not None:
@@ -91,7 +97,7 @@ def main(old, new):
     totals = collections.defaultdict(collections.Counter)
     for key in sorted(set(ko) | set(kn)):
         variant, n, m = key
-        label = ("%-24s" % n) if variant == "default" else "<%2d,%2d>" % (n, m)
+        label = ("%-24s" % n) if variant in ("default", "reports") else "<%2d,%2d>" % (n, m)
         if key not in ko or key not in kn:
             print("%-7s %s  only in %s" % (variant, label, "new" if key in kn else "old"))
             totals[variant]["unmatched"] += 1
