@@ -58,7 +58,10 @@ typedef struct lmpc_params {
     int warm_start;               /* != 0: the controllers of the device-resident step (lmpc_step_* / lmpc_rollout_step) start each
                                      solve from a mid-path interior-point iterate of their previous solve, shifted by one stage
                                      (SURVEY §8f rank 2).  The reference always starts cold (PC.py:124,276: `initvals` unused);
-                                     the optimum returned is the same, only the iteration count changes.  0 = cold start. */
+                                     the optimum returned is the same, only the iteration count changes.  A warm start that is
+                                     not through after min(16, max_iter) iterations restarts cold inside the same solve, with
+                                     the full max_iter of its own (at most min(16, max_iter) + max_iter iterations in all), and
+                                     the record is dropped.  0 = cold start. */
     double eps_step;              /* <= 0 selects the default 1e-7: besides the residuals, the last primal step
                                      |alpha (dx, du)|_inf must be below it -- on QPs without strict complementarity the
                                      iterate is O(sqrt(gap)) from the optimum while the residuals are already tiny */

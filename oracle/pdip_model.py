@@ -70,10 +70,11 @@ def kernel_constants(N, lmpc):
 
 
 def solve(qp, eps=1e-9, max_iter=60, verbose=False, eps_step=1e-7, eps_gap=None, mu0="auto", s0=0.3, gamma=0.01, warm=None, snap_mu=None,
-          warm_theta=0.5, mu0_scale=1.0, step=0.995, backoff=0.8):
+          warm_theta=0.25, mu0_scale=1.0, step=0.995, backoff=0.8):
     """Returns dict(x[N+1,n], u[N,d], s[N,ncx], lam[m], xi[n], iters, r_prim, r_dual, gap, status).
     s0 / mu0_scale / step / backoff / gamma: starting point and step rule (defaults = the round-1 kernel;
-    ``solve(qp, **kernel_constants(qp.N, qp.m > 0))`` follows the kernel for either problem type)."""
+    ``solve(qp, **kernel_constants(qp.N, qp.m > 0))`` follows the kernel for either problem type).  warm_theta: the floor of a
+    warm start's derived slacks as a fraction of their old value (the kernel's Pdip::WARM_THETA)."""
     N, n, d = qp.N, 6, 2
     Fx, bx, Fu, bu = qp.Fx, qp.bx, qp.Fu, qp.bu
     ncx, ncu, m = Fx.shape[0], Fu.shape[0], qp.m

@@ -370,7 +370,8 @@ struct Pdip {
     // The snapshot is the first iterate (the starting point included) whose gap lies in [WARM_MIN_MU, WARM_SNAP_MU]: an iterate
     // closer to the boundary makes a poor start (measured: snapshots at mu <= 1e-2 cost iterations and can stall).  A record is
     // re-used for at most WARM_MAX_AGE consecutive solves before a cold start re-anchors it, and it is dropped whenever a solve
-    // started from it does not finish cleanly within WARM_MAX_ITERS iterations -- the next solve of that controller is cold.
+    // started from it does not finish cleanly within WARM_MAX_ITERS iterations (max_iter if that is smaller) -- the solve then
+    // restarts cold inside the same call with the full max_iter budget, and the next solve of that controller is cold.
     static constexpr double WARM_SNAP_MU = 0.1, WARM_MIN_MU = 0.01, WARM_THETA = 0.25;
     static constexpr int WARM_MAX_AGE = 8, WARM_MAX_ITERS = 16;
 
@@ -1647,7 +1648,10 @@ LMPC_SWEEP_UNROLL
         if (LMPC_LANE == 0) w.flag = 0;
         wsync();
         bool snapped = (warm == nullptr), warm_started = false, warm_restarted = false;
-        int late_it = LATE_ACCEPT_IT;
+        // late_it / max_it: iteration limits of the start the solve runs from; a restart moves both by restart_it, so the cold
+        // start that replaces a warm one has the budget it would have had without the record
+        int late_it = LATE_ACCEPT_IT, max_it = c.max_iter;
+        const int restart_it = (c.max_iter < WARM_MAX_ITERS) ? c.max_iter : WARM_MAX_ITERS;
         int age = 0;
         if (warm != nullptr) {
             age = *warm_valid;                            // 0 = no record, else 1 + number of solves it has been carried through
@@ -1666,14 +1670,15 @@ LMPC_SWEEP_UNROLL
         const double d4_floor = c.d4_min;
 
         for (;; ++it) {
-            if (warm_started && it == WARM_MAX_ITERS) {
+            if (warm_started && it == restart_it) {
                 // a start from the previous solve's iterate that is still not through: give the QP the cold start it would have
-                // had without the record (the same answer at the same tolerances, a few iterations later), drop the record
+                // had without the record (the same answer at the same tolerances, restart_it iterations later), drop the record
                 init_point(w, g, c, x0, false);
                 wsync();
                 warm_started = false;
                 warm_restarted = true;
-                late_it = LATE_ACCEPT_IT + WARM_MAX_ITERS;
+                late_it = LATE_ACCEPT_IT + restart_it;
+                max_it = c.max_iter + restart_it;
                 al_prev = 0.0; ru_prev = 0.0; step_prev = 1e300; res_ok = false;
             }
             // ---- lane-local residuals, barrier diagonals, predictor right-hand sides -------
@@ -1750,12 +1755,12 @@ LMPC_SWEEP_UNROLL
                 // Stragglers: on a few LMPC instances (LP-degenerate simplex block) the covariance-form recovery of
                 // d(lambda) puts a noise floor of ~1e-7..1e-6 under the dual residual and the tail converges linearly.
                 // Once the iterate meets the 1e-6 parity contract, stop after LATE_ACCEPT_IT iterations (and at max_iter).
-                if ((it >= late_it || it >= c.max_iter) && r_prim <= 1e-6 && r_dual <= 1e-6 && mu <= 1e-6) {
+                if ((it >= late_it || it >= max_it) && r_prim <= 1e-6 && r_dual <= 1e-6 && mu <= 1e-6) {
                     status = ST_SOLVED;
                     late = res_ok ? 0 : 1;
                     break;
                 }
-                if (it >= c.max_iter) { status = ST_MAX_ITER; break; }
+                if (it >= max_it) { status = ST_MAX_ITER; break; }
             }
             // ---- factorising backward sweep (also yields the input residual) ------------------
             if (LMPC) {
@@ -1775,7 +1780,7 @@ LMPC_SWEEP_UNROLL
             r_dual = fmax(rd_loc, ru_max);
             if (w.flag != 0) { status = res_ok ? ST_SOLVED : w.flag; break; }
             if (r_prim <= c.eps_res && r_dual <= c.eps_res && mu <= c.eps_gap && step_prev <= c.eps_step) { status = ST_SOLVED; break; }
-            if (it >= c.max_iter) {
+            if (it >= max_it) {
                 if (res_ok) { status = ST_SOLVED; }
                 else if (r_prim <= 1e-6 && r_dual <= 1e-6 && mu <= 1e-6) { status = ST_SOLVED; late = 1; }
                 else { status = ST_MAX_ITER; }

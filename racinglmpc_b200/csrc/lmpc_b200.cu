@@ -234,8 +234,8 @@ static std::vector<DevBuf> dev_bufs(lmpc_handle* h) {
         dbuf(h->d_ztState, 6, S, FILL_ZERO, SN_ZT), dbuf(h->d_OldInput, 2, S, FILL_ZERO, SN_OLDINPUT, "OldInput"),
         dbuf(h->d_xPredPrev, np, S, FILL_ZERO, SN_XPREDPREV), dbuf(h->d_timeStep, 1, S, FILL_ZERO, SN_TIMESTEP),
         dbuf(h->d_hasPred, 1, S, FILL_ZERO, SN_HASPRED),
-        dbuf(h->d_warm, (size_t)h->warm_stride, OWN_WARM, FILL_NONE, SN_WARM),
-        dbuf(h->d_warm_valid, 1, OWN_WARM, FILL_ZERO, SN_WARM_VALID),
+        dbuf(h->d_warm, (size_t)h->warm_stride, OWN_WARM, FILL_NONE, SN_WARM, "warm"),
+        dbuf(h->d_warm_valid, 1, OWN_WARM, FILL_ZERO, SN_WARM_VALID, "warm_valid"),
         // store scratch: flags (cleared by every step), K2 outputs nothing reads later, staging of host arrays, exchange scratch
         dbuf(h->d_flags, 1, S, FILL_ZERO, SN_SCRATCH, "flags"), dbuf(h->d_minidx, nit, S), dbuf(h->d_ztFixed, 6, S),
         dbuf(h->d_tmpx, 6, S), dbuf(h->d_tmpu, 2, S), dbuf(h->d_xchg, 3, S),

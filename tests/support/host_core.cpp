@@ -38,6 +38,33 @@ extern "C" int host_core_solve(int N, int M, const FtocpConst* c, const double* 
 #undef CASE
     return -1;
 }
+// The starting point Pdip::warm_point builds from a warm-start record wb (WS_SIZE doubles), before any iteration:
+// out = x [(N+1)*6] | u [N*2] | s, nu1, nu3 [N*2 each] | nu2 [N*4] | lam, nu4 [M each] | y1.
+template <int N, int M>
+static int warm_point_run(const FtocpConst* c, const double* abc, const double* x0, const double* wb, double* out) {
+    using P = Pdip<N, M, 2, 4>;
+    typename P::W* w = new typename P::W();
+    typename P::RG* g = new typename P::RG();
+    std::memcpy(w->ABC, abc, sizeof(double) * N * 54);
+    P::warm_point(*w, *g, *c, x0, wb);
+    double* o = out;
+    auto put = [&](const double* src, int n) { std::memcpy(o, src, sizeof(double) * n); o += n; };
+    put(w->x, (N + 1) * 6); put(w->u, N * 2);
+    put(g->s, P::R1); put(g->nu1, P::R1); put(g->nu3, P::R1); put(g->nu2, P::R2);
+    if (M > 0) { put(g->lam, M); put(g->nu4, M); put(&g->y1, 1); }
+    delete g;
+    delete w;
+    return P::WS_SIZE;
+}
+
+extern "C" int host_core_warm_point(int N, int M, const FtocpConst* c, const double* abc, const double* x0, const double* wb,
+                                    double* out) {
+#define CASE(n, m) if (N == n && M == m) return warm_point_run<n, m>(c, abc, x0, wb, out);
+    CASE(6, 0) CASE(12, 0) CASE(14, 0) CASE(24, 0) CASE(48, 0)
+    CASE(6, 48) CASE(12, 48) CASE(14, 48) CASE(24, 48) CASE(48, 48)
+#undef CASE
+    return -1;
+}
 #ifdef LMPC_HOST_COUNT
 extern "C" void host_core_counts(long* out3, int reset) {
     for (int i = 0; i < 3; ++i) { out3[i] = lmpc::g_host_count[i]; if (reset) lmpc::g_host_count[i] = 0; }

@@ -91,3 +91,21 @@ def solve(const, N, abc, x0, uOld, SS=None, Qfun=None, warm=None):
     assert rc != -1, "unsupported (N, M)"
     return dict(x=xp, u=up, lam=lam[:M], s=slack.reshape(N, 2), status=int(info[0]), iters=int(info[1]),
                 r_prim=info[2], r_dual=info[3], gap=info[4])
+
+
+def warm_point(const, N, M, abc, x0, record):
+    """The starting point Pdip::warm_point builds from a warm-start record (float64[>= WS_SIZE]) for the QP (abc, x0):
+    dict of x[N+1,6], u[N,2], s, nu1, nu3 [N*2], nu2 [N*4] and, with a safe set, lam, nu4 [M], y1; plus ws_size."""
+    dp = lambda a: a.ctypes.data_as(C.POINTER(C.c_double))
+    abc = np.ascontiguousarray(abc, float); x0 = np.ascontiguousarray(x0, float); rec = np.ascontiguousarray(record, float)
+    R1, R2 = 2 * N, 4 * N                         # the emulation is built for ncx = 2, ncu = 4
+    out = np.zeros((N + 1) * 6 + N * 2 + 3 * R1 + R2 + 2 * M + 1)
+    n = lib().host_core_warm_point(N, M, C.byref(const), dp(abc), dp(x0), dp(rec), dp(out))
+    assert n != -1, "unsupported (N, M)"
+    parts, o = {}, 0
+    for name, size in (("x", (N + 1) * 6), ("u", N * 2), ("s", R1), ("nu1", R1), ("nu3", R1), ("nu2", R2)) + \
+            ((("lam", M), ("nu4", M), ("y1", 1)) if M > 0 else ()):
+        parts[name] = out[o:o + size].copy(); o += size
+    parts["x"], parts["u"] = parts["x"].reshape(N + 1, 6), parts["u"].reshape(N, 2)
+    parts["ws_size"] = n
+    return parts
