@@ -27,6 +27,8 @@ D4_MIN = 1e-6   # floor on the lambda barrier diagonal nu4/lambda (static primal
                 # Without W_REFINE the 6x6 covariance-form elimination of lambda loses the Newton direction below
                 # ~1e-5 (measured: tests/golden snapshots); with one refinement step 1e-4..1e-7 all converge in
                 # 9-16 iterations and 1e-6 removes the stall of LP-degenerate instances the 1e-4 floor caused.
+LATE_ACCEPT_IT = 20   # kernel: LATE_ACCEPT_IT.  From this iteration on, and at max_iter, an iterate within 1e-6 (residuals and gap)
+                      # is accepted (status 1, "late" unless it also meets eps / eps_gap)
 
 
 class StageQP:
@@ -71,7 +73,9 @@ def kernel_constants(N, lmpc):
 
 def solve(qp, eps=1e-9, max_iter=60, verbose=False, eps_step=1e-7, eps_gap=None, mu0="auto", s0=0.3, gamma=0.01, warm=None, snap_mu=None,
           warm_theta=0.25, mu0_scale=1.0, step=0.995, backoff=0.8):
-    """Returns dict(x[N+1,n], u[N,d], s[N,ncx], lam[m], xi[n], iters, r_prim, r_dual, gap, status).
+    """Returns dict(x[N+1,n], u[N,d], s[N,ncx], lam[m], xi[n], iters, r_prim, r_dual, gap, status, late).
+    As in the kernel, max_iter = k returns the iterate after k steps (status 2, iters k), or status 1 when that iterate is within
+    1e-6 (late: not within eps / eps_gap).
     s0 / mu0_scale / step / backoff / gamma: starting point and step rule (defaults = the round-1 kernel;
     ``solve(qp, **kernel_constants(qp.N, qp.m > 0))`` follows the kernel for either problem type).  warm_theta: the floor of a
     warm start's derived slacks as a fraction of their old value (the kernel's Pdip::WARM_THETA)."""
@@ -159,7 +163,7 @@ def solve(qp, eps=1e-9, max_iter=60, verbose=False, eps_step=1e-7, eps_gap=None,
                 gr[k] += dR2 * (u[k] - u[k + 1])
         return gr
 
-    status, it = 2, 0
+    status, it, late = 2, 0, False
     d4_floor, rdual_prev, al_prev = D4_MIN, 1e300, 0.0
     step_prev = np.inf       # |alpha (dx, du)|_inf of the step just taken: residuals alone do not bound the distance to the optimum
     for it in range(max_iter + 1):
@@ -193,8 +197,12 @@ def solve(qp, eps=1e-9, max_iter=60, verbose=False, eps_step=1e-7, eps_gap=None,
             snap = dict(u=u.copy(), s=s.copy(), w1=w1.copy(), nu1=nu1.copy(), nu2=nu2.copy(), nu3=nu3.copy(), mu=mu, it=it)
             if lmpc:
                 snap.update(lam=lam.copy(), nu4=nu4.copy(), y1=y1)
-        if r_prim <= eps and r_dual <= eps and mu <= (eps if eps_gap is None else eps_gap) and step_prev <= eps_step:
+        res_ok = r_prim <= eps and r_dual <= eps and mu <= (eps if eps_gap is None else eps_gap)
+        if res_ok and step_prev <= eps_step:
             status = 1
+            break
+        if it > 0 and (it >= LATE_ACCEPT_IT or it == max_iter) and max(r_prim, r_dual, mu) <= 1e-6:
+            status, late = 1, not res_ok
             break
         if ADAPTIVE_FLOOR and lmpc and it > 0 and al_prev >= 0.9 and r_dual > 0.25 * rdual_prev:
             d4_floor = min(d4_floor, 0.1 * D4_MIN)
@@ -416,7 +424,7 @@ def solve(qp, eps=1e-9, max_iter=60, verbose=False, eps_step=1e-7, eps_gap=None,
             lam, xi = lam + al * cc["dlam"], xi + al * cc["dxi"]
             yT, y1, nu4 = yT + al * cc["dyT"], y1 + al * cc["dy1"], nu4 + al * cc["dnu4"]
 
-    out = dict(x=x, u=u, s=s, iters=it, r_prim=r_prim, r_dual=r_dual, gap=mu, status=status, snap=snap)
+    out = dict(x=x, u=u, s=s, iters=it, r_prim=r_prim, r_dual=r_dual, gap=mu, status=status, late=late, snap=snap)
     if lmpc:
         out.update(lam=lam, xi=xi)
     return out

@@ -5,6 +5,7 @@ oracle.  The product package never loads this library.
 """
 import ctypes as C
 import os
+import re
 import subprocess
 import numpy as np
 
@@ -59,24 +60,46 @@ def pack_abc(A, B, Cc, N):
     return out
 
 
-_LIB = None
+_LAUNCH = os.path.join(_HERE, "..", "..", "racinglmpc_b200", "csrc", "ftocp_launch.cuh")
 
 
-def lib():
-    global _LIB
-    if _LIB is None:
-        so = os.path.join(_HERE, "libhost_core.so")
+def kernel_grid():
+    """The (N, M) pairs the QP kernel is instantiated for: LMPC_FOR_EACH_CASE of ftocp_launch.cuh, in its order."""
+    src = open(_LAUNCH).read()
+    body = re.search(r"#define LMPC_FOR_EACH_CASE\(X\)((?:[^\n]*\\\n)*[^\n]*)", src).group(1)
+    return [(int(n), int(m)) for n, m in re.findall(r"X\((\d+),\s*(\d+)\)", body)]
+
+
+_LIBS = {}
+
+
+def lib(count=False):
+    """The host emulation, built on first use.  count=True: a separately named build with -DLMPC_HOST_COUNT that also exports
+    host_core_counts (see counts()); its arithmetic is the same."""
+    if count not in _LIBS:
+        so = os.path.join(_HERE, "libhost_core_count.so" if count else "libhost_core.so")
         src = os.path.join(_HERE, "host_core.cpp")
         hdr = os.path.join(_HERE, "..", "..", "racinglmpc_b200", "csrc", "ftocp_pdip.cuh")
         if (not os.path.exists(so)) or os.path.getmtime(so) < max(os.path.getmtime(src), os.path.getmtime(hdr)):
-            subprocess.run(["/usr/bin/g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wno-unknown-pragmas", "-o", so, src], check=True)
-        _LIB = C.CDLL(so)
-        assert _LIB.host_core_const_size() == C.sizeof(FtocpConst)
-    return _LIB
+            flags = ["-DLMPC_HOST_COUNT"] if count else []
+            subprocess.run(["/usr/bin/g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wno-unknown-pragmas"] + flags + ["-o", so, src],
+                           check=True)
+        L = C.CDLL(so)
+        assert L.host_core_const_size() == C.sizeof(FtocpConst)
+        _LIBS[count] = L
+    return _LIBS[count]
 
 
-def solve(const, N, abc, x0, uOld, SS=None, Qfun=None, warm=None):
-    """warm: None, or a dict {"buf": float64[>= 512], "valid": int32[1]} carried from solve to solve (the controller's warm-start record)."""
+def counts(reset=True):
+    """Branch counts of the counting build since the last reset: dict of corrector passes, recentring passes, step reductions."""
+    out = np.zeros(3, np.int64)
+    lib(count=True).host_core_counts(out.ctypes.data_as(C.POINTER(C.c_long)), int(reset))
+    return dict(corrector=int(out[0]), recentre=int(out[1]), reduce=int(out[2]))
+
+
+def solve(const, N, abc, x0, uOld, SS=None, Qfun=None, warm=None, count=False):
+    """warm: None, or a dict {"buf": float64[>= 512], "valid": int32[1]} carried from solve to solve (the controller's warm-start record).
+    count: solve with the counting build (lib(count=True)).  late: 1 when the solve was accepted by the 1e-6 safety net."""
     M = 0 if SS is None else SS.shape[1]
     dp = lambda a: a.ctypes.data_as(C.POINTER(C.c_double))
     abc = np.ascontiguousarray(abc, float)
@@ -84,13 +107,13 @@ def solve(const, N, abc, x0, uOld, SS=None, Qfun=None, warm=None):
     qf = np.ascontiguousarray(Qfun if Qfun is not None else np.zeros(1), float)
     x0 = np.ascontiguousarray(x0, float); uOld = np.ascontiguousarray(np.asarray(uOld, float).ravel())
     xp, up = np.zeros((N + 1, 6)), np.zeros((N, 2))
-    lam, slack, info = np.zeros(max(M, 1)), np.zeros(N * 2), np.zeros(5)
+    lam, slack, info = np.zeros(max(M, 1)), np.zeros(N * 2), np.zeros(6)
     wb = None if warm is None else dp(warm["buf"])
     wv = None if warm is None else warm["valid"].ctypes.data_as(C.POINTER(C.c_int))
-    rc = lib().host_core_solve(N, M, C.byref(const), dp(abc), dp(ss), dp(qf), dp(x0), dp(uOld), dp(xp), dp(up), dp(lam), dp(slack), dp(info), wb, wv)
+    rc = lib(count).host_core_solve(N, M, C.byref(const), dp(abc), dp(ss), dp(qf), dp(x0), dp(uOld), dp(xp), dp(up), dp(lam), dp(slack), dp(info), wb, wv)
     assert rc != -1, "unsupported (N, M)"
     return dict(x=xp, u=up, lam=lam[:M], s=slack.reshape(N, 2), status=int(info[0]), iters=int(info[1]),
-                r_prim=info[2], r_dual=info[3], gap=info[4])
+                r_prim=info[2], r_dual=info[3], gap=info[4], late=int(info[5]))
 
 
 def warm_point(const, N, M, abc, x0, record):

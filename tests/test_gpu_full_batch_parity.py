@@ -21,6 +21,7 @@ from racinglmpc_b200 import BatchedFTOCP, pack_abc, workloads, reference_params 
 from racinglmpc_b200.controller import BatchedController                                 # noqa: E402
 from oracle import ftocp, kkt                                                            # noqa: E402
 import oracle_batch as ob                                                                # noqa: E402
+from qp_inputs import ltv_inputs, lmpc_qp_inputs                                         # noqa: E402
 
 
 def _need_gpu():
@@ -132,40 +133,6 @@ def test_config2_all_4096_instances_vs_oracle(track):
           (ok.sum(), B, err[ok].max(), r[:, 0].max(), r[:, 1].max()))
 
 
-def _ltv_inputs(B, N):
-    """LTV-MPC inputs at any horizon <= 48: the first N stage models of the N = 48 fixture when N has no fixture of its own."""
-    try:
-        x0, uold, abc = workloads.ltv_mpc_batch(B, N=N)
-        start = np.load(workloads._GOLD + "/workload_ltv.npz")["N%d_start" % N]
-    except KeyError:
-        x0, uold, abc = workloads.ltv_mpc_batch(B, N=48)
-        abc = np.ascontiguousarray(abc[:, :N])
-        start = np.load(workloads._GOLD + "/workload_ltv.npz")["N48_start"]
-    return x0, uold, abc, start[np.arange(B) % start.shape[0]]
-
-
-def _lmpc_qp_inputs(gold, N, B, duplicate_laps, M=48):
-    """LMPC-type QPs at horizon N: stage models from the LTV workload fixture, safe set = 4 x 12 consecutive rows of the PID
-    lap around the end of the prediction (4 identical laps when `duplicate_laps`: the reference's own first LMPC laps,
-    main.py:109-110, the LP-degenerate case), cost-to-go counting down."""
-    x0, uold, abc, start = _ltv_inputs(B, N)
-    xP, uP = gold["pid_x"], gold["pid_u"]
-    P = M // 4
-    SS = np.zeros((B, 6, M)); Qf = np.zeros((B, M)); SuS = np.zeros((B, 6, M)); SuU = np.zeros((B, 2, M))
-    for b in range(B):
-        i0 = int(min(start[b] + N - P // 2, xP.shape[0] - P - 12))
-        for j in range(4):
-            rows = np.arange(i0, i0 + P + 1) + (0 if duplicate_laps else 2 * j)
-            blk = xP[rows].copy()
-            if not duplicate_laps:
-                blk[:, 0:3] += 1e-3 * (j + 1)
-            SS[b, :, P * j:P * j + P] = blk[:P].T
-            SuS[b, :, P * j:P * j + P] = blk[1:].T
-            SuU[b, :, P * j:P * j + P] = uP[rows[1:]].T
-            Qf[b, P * j:P * j + P] = 300.0 - rows[:P] * 0.3 + 5.0 * j
-    return x0, uold, abc, SS, Qf, SuS, SuU
-
-
 @pytest.mark.parametrize("N,dup,M", [(14, False, 48), (14, True, 48), (24, False, 48), (48, False, 48), (6, True, 48), (4, False, 48),
                                      (16, False, 48), (32, False, 48), (12, False, 24), (12, True, 96), (14, False, 64), (14, False, 32)])
 def test_lmpc_qp_instantiations_vs_oracle(gold, track, N, dup, M):
@@ -175,7 +142,7 @@ def test_lmpc_qp_instantiations_vs_oracle(gold, track, N, dup, M):
     B = 16
     numSS_it, _, _, _, Qts, par = rp.lmpc_params(N)
     numSS_Points = M
-    x0, uold, abc, SS, Qf, SuS, SuU = _lmpc_qp_inputs(gold, N, B, dup, M)
+    x0, uold, abc, SS, Qf, SuS, SuU = lmpc_qp_inputs(gold, N, B, dup, M)
     s = BatchedFTOCP(par, batch=B, numSS_Points=numSS_Points, numSS_it=numSS_it, QterminalSlack=Qts)
     o = s.solve(x0, uold, abc, SS, Qf, SuS, SuU)
     counts = dict(zip(*np.unique(o["status"], return_counts=True)))
@@ -214,7 +181,7 @@ def test_mpc_qp_horizon_grid_vs_oracle(N):
     against the oracle."""
     _need_gpu()
     B = 64
-    x0, uold, abc, _ = _ltv_inputs(B, N)
+    x0, uold, abc, _ = ltv_inputs(B, N)
     prob = ob.ltv_problem_set(x0, uold, abc, N)
     zo, infos = ob.tight_batch(prob)
     assert _certified(infos).all()
