@@ -132,7 +132,7 @@ def lap_row_summary(reps, schedules, laps):
 def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, poll=8, max_steps=0, seed=1234, local=None, warm=False,
         final=None, param_sets=None, vehicle_sets=None, books=None, track_sets=None, pool_groups=None, readiness="batch",
         capture=None, start=None, noise_sets=None, noise_streams=None, regression_sets=None, lap_budget=None, measurement_sets=None,
-        shape_sets=None, ss_laps_sets=None, lap_reports=None, lap_schedules=None):
+        shape_sets=None, ss_laps_sets=None, lap_reports=None, lap_schedules=None, lap_window_sets=None):
     """One Monte-Carlo run on this rank's GPU (torch.distributed may or may not be initialised).  Returns a dict (all ranks).
     final: None, or a dict that receives the closed loop's end state (rollout_state) and the last step's solver report (step_results).
     books: None, or a dict that receives the lap books (books) and the health counters (flags_or, unsolved), and with lap_reports
@@ -221,7 +221,12 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     (conditions that change at the laps each controller reaches; entry 0 is the first LMPC lap).  Each kind needs its table and the
     run needs lap_reports >= laps.  The result gains "per_lap_row_rank0": per kind, lap and row, the controllers on that row, their
     mean steps, the share with a lane violation and the unsolved QPs (lap_row_summary).  capture records the schedules and start
-    refuses others.  ValueError before any device work."""
+    refuses others.  ValueError before any device work.
+    lap_window_sets: None, or (windows, index) handed to BatchedController.set_lap_windows with the other tables, before the PID
+    lap: objects with ss_window (0 or the controller's numSS_it .. ss_cap 7) and model_window (0 or trToUse 4 .. model_cap 5), 0
+    = unbounded (controllers that trust only their most recent laps).  The result then holds per-window lap statistics and mean
+    interior-point iterations under "per_lap_window_rank0".  capture records every controller's windows and start refuses others.
+    ValueError before any device work where set_lap_windows would refuse."""
     L = check_lap_reports(lap_reports, laps)
     scheds = check_lap_schedules(lap_schedules, batch, L, {"vehicle": vehicle_sets, "noise": noise_sets,
                                                            "measurement": measurement_sets})
@@ -234,10 +239,17 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
             raise ValueError("shape_sets and warm start: the warm-start record is laid out per (N, numSS_Points)")
         rows, sidx = _native.make_shape_sets(shape_sets[0], shape_sets[1], int(batch), N, M, numSS_it)
         points = [rows[k].numSS_Points for k in sidx]
+    laps_of = [numSS_it] * int(batch)                              # every controller's numSS_it
     if ss_laps_sets is not None:
-        _native.make_ss_laps_sets(ss_laps_sets[0], ss_laps_sets[1], int(batch), numSS_it, points)
+        rows, lidx = _native.make_ss_laps_sets(ss_laps_sets[0], ss_laps_sets[1], int(batch), numSS_it, points)
+        laps_of = [rows[k].numSS_it for k in lidx]
+    windows = None                                                 # [batch, 2] (ss_window, model_window), or None
+    if lap_window_sets is not None:
+        rows, widx = _native.make_lap_window_sets(lap_window_sets[0], lap_window_sets[1], int(batch), laps_of, SS_CAP, TR_TO_USE,
+                                                  MODEL_CAP)
+        windows = np.array([[rows[k].ss_window, rows[k].model_window] for k in widx], np.int32)
     if start is not None:
-        _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget, shape_sets, L, scheds)
+        _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget, shape_sets, L, scheds, windows)
     if capture is not None and not isinstance(capture, dict):
         raise ValueError("capture is a dict that receives the run's end state")
     if readiness not in ("batch", "group"):
@@ -275,7 +287,7 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
               (measurement_sets, c.set_measurement_noise, "per_measurement_rank0"),
               (regression_sets, c.set_regression, "per_regression_rank0"), (track_sets, c.set_tracks, "per_track_rank0"),
               (pool_groups, c.set_pool_groups, None), (shape_sets, c.set_shapes, "per_shape_rank0"),
-              (ss_laps_sets, c.set_ss_laps, "per_ss_laps_rank0"))
+              (ss_laps_sets, c.set_ss_laps, "per_ss_laps_rank0"), (lap_window_sets, c.set_lap_windows, "per_lap_window_rank0"))
     for args, install, _ in tables:
         if args is not None:
             install(*args)
@@ -368,7 +380,8 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         capture.update(capture_s=time.perf_counter() - tc, **sched.state(steps), batch=B, laps=laps, mode=mode, readiness=readiness,
                        poll=poll, warm=bool(warm), pool_groups=G, layout=c.snapshot_layout(),
                        lap_budget=None if budget is None else budget.tolist(),
-                       lap_schedules={kind: row_of_lap.tolist() for kind, row_of_lap in scheds.items()})
+                       lap_schedules={kind: row_of_lap.tolist() for kind, row_of_lap in scheds.items()},
+                       lap_windows=None if windows is None else windows.tolist())
     flags_or, unsolved = c.rollout_health()
     reps = c.lap_reports() if L else None
     lens, n_laps = (reps["steps"], reps["n"]) if L else (bk["lap_hist"], bk["lap_n"])
@@ -417,6 +430,12 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
                         s.update(N=int(sh[0]), numSS_Points=int(sh[1]), numSS_it=int(v),
                                  ipm_iters_mean_sampled=float(it_ctrl[cell].mean() / max(it_n, 1)))
                         out["per_shape_ss_laps_rank0"].append(s)
+    if lap_window_sets is not None:
+        idx = np.asarray(lap_window_sets[1]).reshape(B)
+        for k, s in enumerate(out["per_lap_window_rank0"]):
+            w = lap_window_sets[0][k]
+            s.update(ss_window=int(w.ss_window), model_window=int(w.model_window),
+                     ipm_iters_mean_sampled=float(it_ctrl[idx == k].mean() / max(it_n, 1)) if (idx == k).any() else 0.0)
     if pool_groups is not None:
         # a stored lap advances `it`: 4 seeded copies + every own lap handed over + every imported lap filed.  Exact unless an
         # own lap found the safe-set pool full (health flag 64): then that controller's count is one too low per such lap.
@@ -456,9 +475,9 @@ def _driven_steps(bk, state):
 
 
 def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget=None, shape_sets=None, lap_reports=0,
-                 lap_schedules=None):
-    """The refusals of run(start=...), before any device work: a start that does not match this run (report capacity and lap
-    schedules included), laps not above the captured laps, or a lap budget below the captured one."""
+                 lap_schedules=None, lap_windows=None):
+    """The refusals of run(start=...), before any device work: a start that does not match this run (report capacity, lap
+    schedules and lap windows included), laps not above the captured laps, or a lap budget below the captured one."""
     if not isinstance(start, dict):
         raise ValueError("start is a capture dict of an earlier run")
     need = ("records", "clock") + sharding.ExchangeSchedule.FIELDS + ("batch", "laps", "mode", "readiness", "poll", "warm",
@@ -489,9 +508,18 @@ def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, b
     if sorted(had) != sorted(mine) or any(not np.array_equal(had[k], mine[k]) for k in had):
         raise ValueError("start was captured with lap_schedules for %s, this run has %s (or other rows): a run resumes under the "
                          "schedules it was captured with" % (sorted(had) or "none", sorted(mine) or "none"))
+    check_start_windows(start.get("lap_windows"), lap_windows)
     for k, v in layout(warm, shape_sets).items():
         if int(start["layout"].get(k, -1)) != v:
             raise ValueError("start records have %s = %s, this run's controllers %d" % (k, start["layout"].get(k), v))
+
+
+def check_start_windows(had, mine):
+    """start's refusal of other lap windows: `had` the captured [batch, 2] windows (a list, or None without a table), `mine` this
+    run's (an array, or None).  The windows are not part of a record, and the books evicted against them."""
+    if (had is None) != (mine is None) or (had is not None and not np.array_equal(np.asarray(had), mine)):
+        raise ValueError("start was captured with other lap windows: a record resumes exactly only under the windows it was captured "
+                         "with")
 
 
 def _set_stats(bk, flags_or, unsolved, sel, laps, reps=None):

@@ -304,6 +304,37 @@ typedef struct lmpc_ss_laps_params {
  *     table is not part of a snapshot record (restore a record into a controller of the same numSS_it_b to resume it). */
 int lmpc_set_ss_laps(lmpc_handle* h, const lmpc_ss_laps_params* sets, int nsets, const int* set_of_instance);
 
+/* Per-controller lap windows: how many of its most recent laps a controller's safe set and learned model draw from (0 =
+ * unbounded, the reference's rule). */
+typedef struct lmpc_lap_window_params {
+    int ss_window;       /* safe set: lap numbers [it - ss_window, it) */
+    int model_window;    /* regression model: arrival numbers [md_cnt - model_window, md_cnt) */
+} lmpc_lap_window_params;
+/* Per-controller lap windows (a controller that trusts only its recent laps, e.g. after the car or the track changed).
+ * Controller b reads row sets[set_of_instance[b]].  nsets == 0 (sets, set_of_instance NULL) removes the table: every window is
+ * unbounded again.
+ *   - Safe set: with ss_window = W > 0 the selection is the stable argsort by (lap time, lap number) of the laps numbered
+ *     [it - W, it), first numSS_it_b of them (the reference's order restricted to the window).  Lap it-1 is always in the window,
+ *     so is_prev and prev_slot are unchanged; an import is still filed as lap it-1.
+ *   - Model: with model_window = Wm > 0 usedIt is the first trToUse laps of the (length, arrival) order among arrival numbers
+ *     [md_cnt - Wm, md_cnt); with fewer the slowest repeats, as without a window.
+ *   - Storage: under a window a lap stays stored while it is in the window and fewer than numSS_it_b (trToUse) newer laps rank
+ *     ahead of it; a new own lap is always stored, an import is left out of the safe set when it is outside the window on arrival
+ *     (ss_window 1) or its newer laps already rank ahead of it numSS_it_b times.  Evicted among the laps that can no longer be
+ *     selected: the slowest, then the oldest.  With ss_window <= ss_cap and model_window <= model_cap a window never sets health
+ *     bit 64.  Without a window the books are exactly as before.
+ *   - Requires lmpc_store_create and no lap stored yet in either pool (else LMPC_E_STATE): the books evict against the window,
+ *     so a later change would need laps that are already gone.
+ *   - 1 <= nsets <= batch, every index in [0, nsets).  Per set: ss_window is 0 or numSS_it_b .. ss_cap for every controller of
+ *     the set (numSS_it_b: its value under lmpc_set_ss_laps, else the handle's), and 0 on a handle without a safe set;
+ *     model_window is 0 or trToUse .. model_cap (the store's trToUse).  lmpc_set_ss_laps refuses a value above a controller's
+ *     installed nonzero ss_window.  Any failed check returns LMPC_E_INVALID and leaves the handle as it was.
+ *   - The call synchronises the handle's streams before it replaces the table.
+ *   - Honoured by the device books (lmpc_rollout_commit_laps_dev, lmpc_rollout_seed_from_record_dev, lmpc_books_set and
+ *     lmpc_pool_import_dev).  The pooled export is unchanged: it ships each controller's latest own lap.
+ *   - Not part of a snapshot record (LMPC_SNAPSHOT_VERSION is unchanged): a record resumes exactly only under the same windows. */
+int lmpc_set_lap_windows(lmpc_handle* h, const lmpc_lap_window_params* sets, int nsets, const int* set_of_instance);
+
 /* PredictiveModel.addTrajectory (PredictiveModel.py:35-46): copy one lap into a regression slot. */
 int lmpc_model_put_lap(lmpc_handle* h, int inst, int slot, int T, const double* x, const double* u);
 /* usedIt order: slots[B,trToUse]. */
@@ -704,6 +735,7 @@ int lmpc_sizeof_measurement_params(void);
 int lmpc_sizeof_regression_params(void);
 int lmpc_sizeof_shape_params(void);
 int lmpc_sizeof_ss_laps_params(void);
+int lmpc_sizeof_lap_window_params(void);
 
 #ifdef __cplusplus
 }

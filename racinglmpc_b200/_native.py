@@ -64,6 +64,12 @@ class SsLapsParams(C.Structure):
     _fields_ = [("numSS_it", C.c_int)]
 
 
+class LapWindowParams(C.Structure):
+    """lmpc_lap_window_params: the most recent laps a controller's safe set (ss_window) and learned model (model_window) draw
+    from; 0 = unbounded."""
+    _fields_ = [("ss_window", C.c_int), ("model_window", C.c_int)]
+
+
 # The (N, numSS_Points) pairs the library instantiates the QP kernel for: LMPC_FOR_EACH_CASE in csrc/ftocp_launch.cuh (a CPU test
 # keeps the two equal)
 SHAPE_GRID = tuple([(n, 0) for n in (4, 6, 8, 10, 12, 14, 16, 20, 24, 32, 48)] + [(n, 48) for n in (4, 6, 8, 10, 12, 14, 16, 20, 24, 32, 48)] +
@@ -192,6 +198,7 @@ def lib():
     L.lmpc_set_regression_sets.argtypes = [_vp, C.POINTER(RegressionParams), C.c_int, _vp]
     L.lmpc_set_shapes.argtypes = [_vp, C.POINTER(ShapeParams), C.c_int, _vp]
     L.lmpc_set_ss_laps.argtypes = [_vp, C.POINTER(SsLapsParams), C.c_int, _vp]
+    L.lmpc_set_lap_windows.argtypes = [_vp, C.POINTER(LapWindowParams), C.c_int, _vp]
     L.lmpc_rollout_sysid.argtypes = [_vp, C.c_double, _vp, _vp]
     L.lmpc_rollout_seed_from_record.argtypes = [_vp, C.c_int, C.c_int, C.c_int]
     L.lmpc_rollout_get_lap.argtypes = [_vp, C.c_int, ip, _vp, _vp]
@@ -234,6 +241,8 @@ def lib():
     assert L.lmpc_sizeof_shape_params() == C.sizeof(ShapeParams), "lmpc_shape_params ABI mismatch"
     L.lmpc_sizeof_ss_laps_params.restype = C.c_int
     assert L.lmpc_sizeof_ss_laps_params() == C.sizeof(SsLapsParams), "lmpc_ss_laps_params ABI mismatch"
+    L.lmpc_sizeof_lap_window_params.restype = C.c_int
+    assert L.lmpc_sizeof_lap_window_params() == C.sizeof(LapWindowParams), "lmpc_lap_window_params ABI mismatch"
     L.lmpc_sizeof_lap_report.restype = C.c_int
     assert L.lmpc_sizeof_lap_report() == C.sizeof(LapReport), "lmpc_lap_report ABI mismatch"
     assert L.lmpc_sizeof_noise_params() == C.sizeof(NoiseParams), "lmpc_noise_params ABI mismatch"
@@ -649,6 +658,37 @@ def make_ss_laps_sets(values, index, batch, numSS_it, points):
         m, v = int(points[b]), rows[idx[b]].numSS_it
         if not _even_split(m, v):
             raise ValueError("controller %d: numSS_Points %d is not numSS_it (%d) times an even number of points per lap" % (b, m, v))
+    return rows, idx
+
+
+def make_lap_window_sets(windows, index, batch, ss_laps, ss_cap, trToUse, model_cap, lmpc=True):
+    """Per-controller lap windows for ``lmpc_set_lap_windows``: K objects ``windows`` with ``ss_window`` and ``model_window``
+    (e.g. reference_params.LapWindowParams; 0 = unbounded) and the row of every controller ``index[batch]``, on a store of
+    ``ss_cap`` / ``model_cap`` slots and ``trToUse`` laps whose controllers have the lap counts ``ss_laps[batch]`` (their values
+    under ``lmpc_set_ss_laps``, or the handle's numSS_it).  Raises ValueError where the library would refuse: the index rules of
+    ``make_param_sets``, a window that is not an integer, an ss_window > 0 without a safe set (``lmpc`` False) or outside
+    numSS_it_b .. ss_cap of a controller b of its row, a model_window outside trToUse .. model_cap.  Returns (ctypes array
+    LapWindowParams * K, int32 index array)."""
+    def row(k, w):
+        vals = []
+        for f in ("ss_window", "model_window"):
+            v = getattr(w, f)
+            if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, np.integer)):
+                raise ValueError("lap window %d: %s must be an integer, got %r" % (k, f, v))
+            vals.append(int(v))
+        sw, mw = vals
+        if sw != 0 and not lmpc:
+            raise ValueError("lap window %d: ss_window must be 0: the handle has no safe set (numSS_Points == 0)" % k)
+        if not (sw == 0 or 1 <= sw <= int(ss_cap)):
+            raise ValueError("lap window %d: ss_window must be 0 or numSS_it .. ss_cap (%d), got %d" % (k, ss_cap, sw))
+        if not (mw == 0 or int(trToUse) <= mw <= int(model_cap)):
+            raise ValueError("lap window %d: model_window must be 0 or trToUse (%d) .. model_cap (%d), got %d" % (k, trToUse, model_cap, mw))
+        return LapWindowParams(sw, mw)
+    rows, idx = _pack_sets(LapWindowParams, windows, index, batch, "lap windows", row)
+    for b in range(batch):
+        w, v = rows[idx[b]].ss_window, int(ss_laps[b])
+        if 0 < w < v:
+            raise ValueError("controller %d: ss_window %d is below its numSS_it (%d)" % (b, w, v))
     return rows, idx
 
 

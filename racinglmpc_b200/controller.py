@@ -68,6 +68,7 @@ class BatchedController:
         self._pool_groups = 1
         self._shapes = None                                 # (shapes, index) of set_shapes, or None: the handle's own shape
         self._ss_laps = None                                # numSS_it of every controller (set_ss_laps), or None: the handle's
+        self._windows = None                                # [B, 2] (ss_window, model_window) of set_lap_windows, or None: unbounded
         # rows of the plant-side tables a lap schedule indexes (the defaults: one reference vehicle and noise, no measurement
         # table) and the installed schedules [B, L] of set_lap_schedule
         self._table_rows = {"vehicle": 1, "noise": 1, "measurement": 0}
@@ -254,6 +255,12 @@ class BatchedController:
             points = [self.shape_of(b)[1] for b in range(self.B)]
             if any(not nat._even_split(m, max(self.numSS_it, 1)) for m in points):
                 raise ValueError("the installed shapes need their lap counts: the handle's numSS_it does not split them evenly")
+        if self._windows is not None:                     # the other install order of set_lap_windows
+            for b in range(self.B):
+                v = self.numSS_it if values is None else values[int(np.asarray(index).reshape(-1)[b])]
+                w = int(self._windows[b, 0])
+                if 0 < w < int(v):
+                    raise ValueError("controller %d: numSS_it %d exceeds its ss_window (%d)" % (b, int(v), w))
         self._install(self._lib.lmpc_set_ss_laps, "values", values, index,
                       lambda: nat.make_ss_laps_sets(values, index, self.B, self.numSS_it, [self.shape_of(b)[1] for b in range(self.B)]))
         if values is None:
@@ -265,6 +272,29 @@ class BatchedController:
     def ss_laps_of(self, inst):
         """numSS_it of controller ``inst``: its value of ``set_ss_laps``, or the handle's."""
         return self.numSS_it if self._ss_laps is None else int(self._ss_laps[int(inst)])
+
+    def set_lap_windows(self, windows, index=None):
+        """Per-controller lap windows (a controller that trusts only its recent laps, e.g. after its car or the track changed):
+        controller b's safe set selects its ``ss_laps_of(b)`` fastest laps among its ``windows[index[b]].ss_window`` most recent
+        ones, and its learned model regresses on the trToUse shortest of the last ``model_window`` laps it filed (objects with
+        those two fields, e.g. reference_params.LapWindowParams; 0 = unbounded, the reference's rule).  The lap books (host or
+        device) then store only the laps that can still be selected under the window, so ss_window <= ss_cap and model_window <=
+        model_cap never overflow them.  ss_window is 0 or ``ss_laps_of(b)`` .. ss_cap (0 on an MPC handle), model_window 0 or
+        trToUse .. model_cap.  ``index`` is required with ``windows``.  ``windows=None`` (no index) removes the table.  Only before
+        the first lap is stored; not part of a snapshot (a record resumes exactly under the same windows).  ValueError before any
+        native call where the library would refuse a value.  Waits for work already enqueued."""
+        self._install(self._lib.lmpc_set_lap_windows, "windows", windows, index,
+                      lambda: nat.make_lap_window_sets(windows, index, self.B, [self.ss_laps_of(b) for b in range(self.B)],
+                                                       max(self.ss_cap, 1), self.trToUse, self.model_cap, self.lmpc))
+        if windows is None:
+            self._windows = None
+        else:
+            rows = [(int(w.ss_window), int(w.model_window)) for w in windows]
+            self._windows = np.array([rows[int(i)] for i in np.asarray(index).reshape(-1)], np.int32).reshape(self.B, 2)
+
+    def lap_windows_of(self, inst):
+        """(ss_window, model_window) of controller ``inst`` under ``set_lap_windows``, (0, 0) (unbounded) without a table."""
+        return (0, 0) if self._windows is None else (int(self._windows[int(inst), 0]), int(self._windows[int(inst), 1]))
 
     def set_tracks(self, tracks, index=None):
         """Per-controller tracks (several circuits in one batch): controller b drives ``tracks[index[b]]`` (objects with
@@ -321,6 +351,15 @@ class BatchedController:
         else:
             pos = next(i for i, (t, _) in enumerate(laps) if T < t)
         laps.insert(pos, (T, lapno))
+        W = self.lap_windows_of(inst)[1]
+        if W > 0:                                                               # the new lap is always stored
+            book = self.model_book[inst]
+            if len(book.slot_of) >= self.model_cap:
+                keep = self._window_keep([t for (t, _) in sorted(laps, key=lambda e: e[1])], self.trToUse, W)
+                victims = [ln for (_, ln) in laps if ln in book.slot_of and ln not in keep]
+                stored = [ln for (_, ln) in laps if ln in book.slot_of]
+                book.drop(victims[-1] if victims else stored[-1])             # the slowest that can no longer be used
+            return book.take(lapno)
         if pos < self.trToUse or len(laps) <= self.trToUse:
             if len(self.model_book[inst].slot_of) >= self.model_cap:          # evict the slowest stored lap not in usedIt
                 stored = [ln for (_, ln) in laps if ln in self.model_book[inst].slot_of and ln != lapno]
@@ -329,6 +368,14 @@ class BatchedController:
                 self.model_book[inst].drop(victims[-1] if victims else stored[-1])
             return self.model_book[inst].take(lapno)
         return -1
+
+    @staticmethod
+    def _window_keep(times, n, W, start=0):
+        """Numbers of the laps ``times`` (indexed by lap or arrival number) that can still be among the ``n`` first under a window
+        of the W most recent: those in the window with fewer than n newer laps strictly faster (a newer lap of equal time sorts
+        after).  ``start``: laps before it are no longer stored and are not counted."""
+        m = len(times)
+        return {j for j in range(max(m - W, start), m) if sum(1 for i in range(j + 1, m) if times[i] < times[j]) < n}
 
     def _touch(self, inst, sel=False, used=False):
         """Mark one instance's selection / usedIt rows as stale (rebuilt at the next _flush)."""
@@ -347,6 +394,9 @@ class BatchedController:
         used = self._used
         for b in rows:
             laps = self.model_laps[b]
+            W = self.lap_windows_of(b)[1]
+            if W > 0:                                     # usedIt among the last W arrivals
+                laps = [e for e in laps if e[1] >= self.model_count[b] - W]
             for c in range(self.trToUse):
                 if c < len(laps) and laps[c][1] in self.model_book[b].slot_of:
                     used[b, c] = self.model_book[b].slot_of[laps[c][1]]
@@ -376,7 +426,15 @@ class BatchedController:
         self.LapTime[inst].append(int(lap_time))
         self.own_laps[inst].append(lapno)
         book = self.ss_book[inst]
-        if not book.free:
+        W = self.lap_windows_of(inst)[0]
+        if W > 0 and not book.free:                       # evict the slowest, then oldest, lap that can no longer be selected
+            times = self.LapTime[inst]
+            keep = self._window_keep(times, self.ss_laps_of(inst), W)
+            victims = [ln for ln in book.slot_of if ln not in keep]
+            if not victims:
+                raise RuntimeError("safe-set pool too small")
+            book.drop(max(victims, key=lambda ln: (times[ln], -ln)))
+        elif not book.free:
             order = list(np.argsort(np.array(self.LapTime[inst]), kind="stable"))
             keep = set(order[:self.ss_laps_of(inst)]) | {lapno}
             victims = [ln for ln in book.slot_of if ln not in keep]
@@ -404,7 +462,9 @@ class BatchedController:
             if len(self.LapTime[b]) < nit:
                 # the reference indexes sortedLapTime[0:numSS_it] lap by lap and raises IndexError here (PC.py:402-403)
                 raise IndexError("instance %d has %d stored laps, fewer than numSS_it = %d" % (b, len(self.LapTime[b]), nit))
-            order = np.argsort(np.array(self.LapTime[b]), kind="stable")[:nit]     # PC.py:395,402
+            W = self.lap_windows_of(b)[0]
+            lo = max(len(self.LapTime[b]) - W, 0) if W > 0 else 0                 # the window: lap numbers [it - W, it)
+            order = lo + np.argsort(np.array(self.LapTime[b][lo:]), kind="stable")[:nit]     # PC.py:395,402
             for c, jj in enumerate(order):
                 sel[b, c] = self.ss_book[b].slot_of[int(jj)]
                 isp[b, c] = 0 if int(jj) < self.it[b] - 1 else 1                    # PC.py:506
@@ -675,7 +735,11 @@ class BatchedController:
                 continue
             lt, last = int(lap_times[b]), self.it[b] - 1
             times = self.LapTime[b][:last] + [lt] + self.LapTime[b][last:]
-            order = list(np.argsort(np.array(times), kind="stable"))[:self.ss_laps_of(b)]
+            W = self.lap_windows_of(b)[0]
+            if W > 0:                                     # the laps that can still be selected under the window
+                order = self._window_keep(times, self.ss_laps_of(b), W)
+            else:
+                order = list(np.argsort(np.array(times), kind="stable"))[:self.ss_laps_of(b)]
             if last not in order:                         # never selected (PC.py:395) -> not in the safe set
                 if to_model:
                     m_slots[b] = self._model_slot_for(b, lt)
@@ -692,7 +756,7 @@ class BatchedController:
                 victims = [ln for ln in book.slot_of if ln not in keep]
                 if not victims:
                     raise RuntimeError("safe-set pool too small")
-                book.drop(max(victims, key=lambda ln: times[ln]))
+                book.drop(max(victims, key=(lambda ln: (times[ln], -ln)) if W > 0 else (lambda ln: times[ln])))
             ss_slots[b] = book.take(last)
             self.it[b] += 1
             use[b] = src[b]

@@ -35,6 +35,86 @@ __device__ __forceinline__ bool key_less(int t1, int n1, int t2, int n2) { retur
 template <bool LAPS>
 __device__ __forceinline__ int book_laps(const LapBooks& k, const SsLaps& laps, int b) { return LAPS ? laps.of(b).numSS_it : k.numSS_it; }
 
+// The lap windows of every controller (lmpc_set_lap_windows): ss_window / model_window most recent laps, 0 = unbounded.  The four
+// kernels that rank laps come in two more instantiations, WIN = a window table is installed; without one they never read it and
+// the book functions below are the code they were before windows existed.
+using LapWindowRec = lmpc_lap_window_params;
+using LapWindows = Table<LapWindowRec>;
+template <bool WIN>
+__device__ __forceinline__ LapWindowRec book_windows(const LapWindows& w, int b) { return WIN ? w.of(b) : LapWindowRec{0, 0}; }
+
+// book_ss_add under a safe-set window of W >= 1 laps: after the event the window is lap numbers [it' - W, it'), it' = it + 1.  A
+// lap stays stored while it is in the window and fewer than nit NEWER laps rank ahead of it: older laps leave the window before it
+// does, newer ones stay as long as it does, so only they can keep it out of the selection for good.  An import's only newer lap
+// is the own latest: it is not stored when it lies outside the window on arrival (W = 1) or nit == 1 and the own latest is faster.
+// Among the stored laps that can no longer be selected the slowest, then the oldest, is evicted, as without a window.  With
+// W <= ss_cap a lap outside the window is always there to evict, so -2 needs W > ss_cap.
+__device__ inline int book_ss_add_window(const LapBooks& k, int b, int T, bool import, int nit, int W) {
+    int* tm = k.ss_time + (size_t)b * k.ss_cap;
+    int* ln = k.ss_lap + (size_t)b * k.ss_cap;
+    const int it = k.it[b];
+    const int lapno = import ? it - 1 : it;
+    const int lo = it + 1 - W;                                   // oldest lap number of the window after the event
+    if (import) {
+        if (it < 1) return -1;
+        int ahead = 0;                                           // the own latest (it-1 -> it) ahead of the new lap
+        for (int s = 0; s < k.ss_cap; ++s) if (ln[s] == it - 1 && key_less(tm[s], it, T, lapno)) ahead = 1;
+        if (lapno < lo || ahead >= nit) return -1;               // never selected -> not stored
+        for (int s = 0; s < k.ss_cap; ++s) if (ln[s] == it - 1) ln[s] = it;
+    }
+    int slot = -1;
+    for (int s = 0; s < k.ss_cap; ++s) if (ln[s] < 0) { slot = s; break; }
+    if (slot < 0) {
+        int vt = -1, vn = 0;
+        for (int s = 0; s < k.ss_cap; ++s) {
+            if (import && ln[s] == it) continue;                 // the own latest lap stays
+            if (ln[s] >= lo) {                                   // in the window: evictable once nit newer laps rank ahead
+                int newer = key_less(T, lapno, tm[s], ln[s]) ? 1 : 0;    // every candidate is older than the new lap
+                for (int j = 0; j < k.ss_cap; ++j) if (ln[j] > ln[s] && key_less(tm[j], ln[j], tm[s], ln[s])) ++newer;
+                if (newer < nit) continue;
+            }
+            if (slot < 0 || tm[s] > vt || (tm[s] == vt && ln[s] < vn)) { slot = s; vt = tm[s]; vn = ln[s]; }
+        }
+        if (slot < 0) {
+            if (import) for (int s = 0; s < k.ss_cap; ++s) if (ln[s] == it) ln[s] = it - 1;
+            return -2;
+        }
+    }
+    tm[slot] = T;
+    ln[slot] = lapno;
+    k.it[b] = it + 1;
+    return slot;
+}
+
+// book_md_add under a model window of W >= 1 laps: arrival numbers [md_cnt' - W, md_cnt').  The new lap has no newer lap, so it is
+// always stored; a stored lap stays while it is in the window and fewer than trToUse newer laps are shorter.  Among the others
+// the slowest (length, arrival) is evicted; with W <= md_cap there always is one.
+__device__ inline int book_md_add_window(const LapBooks& k, int b, int T, int W) {
+    int* tm = k.md_time + (size_t)b * k.md_cap;
+    int* sq = k.md_seq + (size_t)b * k.md_cap;
+    const int seq = k.md_cnt[b];
+    k.md_cnt[b] = seq + 1;
+    const int lo = seq + 1 - W;
+    int slot = -1;
+    for (int s = 0; s < k.md_cap; ++s) if (sq[s] < 0) { slot = s; break; }
+    if (slot < 0) {
+        int vt = -1, vs = -1, any = -1, at = -1, as = -1;
+        for (int s = 0; s < k.md_cap; ++s) {
+            if (any < 0 || key_less(at, as, tm[s], sq[s])) { any = s; at = tm[s]; as = sq[s]; }
+            if (sq[s] >= lo) {
+                int newer = (T < tm[s]) ? 1 : 0;                 // the new lap is newer than every stored one
+                for (int j = 0; j < k.md_cap; ++j) if (sq[j] > sq[s] && key_less(tm[j], sq[j], tm[s], sq[s])) ++newer;
+                if (newer < k.trToUse) continue;
+            }
+            if (slot < 0 || key_less(vt, vs, tm[s], sq[s])) { slot = s; vt = tm[s]; vs = sq[s]; }
+        }
+        if (slot < 0) slot = any;
+    }
+    tm[slot] = T;
+    sq[slot] = seq;
+    return slot;
+}
+
 // LMPC.addTrajectory bookkeeping for a lap of `T` rows.  import == false: the controller's own new lap (lap number it).
 // import == true: a lap another controller drove, filed BEFORE the controller's own latest lap (which stays lap it-1, the one
 // addPoint extends): it takes lap number it-1, the own latest moves to it; it is skipped (-1) when it would not be among the
@@ -104,22 +184,37 @@ __device__ inline int book_md_add(const LapBooks& k, int b, int T) {
     return slot;
 }
 
+// The book functions of a kernel with a lap-window table (WIN) take the controller's window W (0 = unbounded, the function
+// above); without one they are the function above and W is not read.
+template <bool WIN>
+__device__ __forceinline__ int book_ss_add(const LapBooks& k, int b, int T, bool import, int nit, int W) {
+    return WIN && W > 0 ? book_ss_add_window(k, b, T, import, nit, W) : book_ss_add(k, b, T, import, nit);
+}
+template <bool WIN>
+__device__ __forceinline__ int book_md_add(const LapBooks& k, int b, int T, int W) {
+    return WIN && W > 0 ? book_md_add_window(k, b, T, W) : book_md_add(k, b, T);
+}
+
 // What the next lap reads: the nit fastest safe-set laps in argsort order (nit: the controller's numSS_it), which of them is lap
 // it-1, the slot addPoint extends, and usedIt of the regression model.  Returns 0, or 8 when fewer than nit laps are stored (the
 // reference raises IndexError at PC.py:402-403).  Entries nit .. k.numSS_it-1 of sel repeat the last selected slot and those of
-// isprev are 0: K2 reads none of them, and a snapshot packs them as they are.
-__device__ inline int book_refresh(const LapBooks& k, int b, int nit) {
+// isprev are 0: K2 reads none of them, and a snapshot packs them as they are.  WIN: only laps in the controller's windows w count
+// (lap numbers >= it - ss_window, arrival numbers >= md_cnt - model_window; a window of 0 starts at 0, and a free slot, -1, is
+// below every start).
+template <bool WIN>
+__device__ inline int book_refresh(const LapBooks& k, int b, int nit, LapWindowRec w) {
     const int* tm = k.ss_time + (size_t)b * k.ss_cap;
     const int* ln = k.ss_lap + (size_t)b * k.ss_cap;
     const int it = k.it[b];
+    const int lo = WIN && w.ss_window > 0 ? max(it - w.ss_window, 0) : 0;
     int flag = 0, prev = -1, last = 0;
     for (int s = 0; s < k.ss_cap; ++s) if (it > 0 && ln[s] == it - 1) prev = s;   // it = 0: no lap (a free slot has ln = -1)
     for (int c = 0; c < nit; ++c) {
         int best = -1;
         for (int s = 0; s < k.ss_cap; ++s) {
-            if (ln[s] < 0) continue;
+            if (ln[s] < lo) continue;
             int rank = 0;
-            for (int j = 0; j < k.ss_cap; ++j) if (j != s && ln[j] >= 0 && key_less(tm[j], ln[j], tm[s], ln[s])) ++rank;
+            for (int j = 0; j < k.ss_cap; ++j) if (j != s && ln[j] >= lo && key_less(tm[j], ln[j], tm[s], ln[s])) ++rank;
             if (rank == c) best = s;
         }
         if (best < 0) { flag = 8; best = last; } else last = best;
@@ -130,13 +225,14 @@ __device__ inline int book_refresh(const LapBooks& k, int b, int nit) {
     k.prevslot[b] = prev;
     const int* mt = k.md_time + (size_t)b * k.md_cap;
     const int* ms = k.md_seq + (size_t)b * k.md_cap;
+    const int lom = WIN && w.model_window > 0 ? max(k.md_cnt[b] - w.model_window, 0) : 0;
     last = 0;
     for (int c = 0; c < k.trToUse; ++c) {
         int best = -1;
         for (int s = 0; s < k.md_cap; ++s) {
-            if (ms[s] < 0) continue;
+            if (ms[s] < lom) continue;
             int rank = 0;
-            for (int j = 0; j < k.md_cap; ++j) if (j != s && ms[j] >= 0 && key_less(mt[j], ms[j], mt[s], ms[s])) ++rank;
+            for (int j = 0; j < k.md_cap; ++j) if (j != s && ms[j] >= lom && key_less(mt[j], ms[j], mt[s], ms[s])) ++rank;
             if (rank == c) best = s;
         }
         if (best < 0) best = last; else last = best;             // fewer laps than trToUse: the slowest one repeats
@@ -146,28 +242,30 @@ __device__ inline int book_refresh(const LapBooks& k, int b, int nit) {
 }
 
 // The selection of tables written from outside (lmpc_books_set): book_refresh of every controller.  One thread per controller.
-template <bool LAPS>
-__global__ void books_refresh_kernel(int batch, LapBooks k, SsLaps laps) {
+template <bool LAPS, bool WIN>
+__global__ void books_refresh_kernel(int batch, LapBooks k, SsLaps laps, LapWindows win) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b < batch) book_refresh(k, b, book_laps<LAPS>(k, laps, b));
+    if (b < batch) book_refresh<WIN>(k, b, book_laps<LAPS>(k, laps, b), book_windows<WIN>(win, b));
 }
 
 // Lap hand-over of every controller whose lap just ended (done[b] != 0), bookkeeping included: main.py:113-119
 // (lmpc.addTrajectory + predictiveModel.addTrajectory of the lap Simulator.sim returned), SysModel.py:50 (s -= TrackLength),
 // PC.py:445 (timeStep = 0).  One CTA per controller; no host involvement.  REPORTS: the running report row is filed as the lap's.
-template <bool LAPS, bool REPORTS>
+// WIN: a lap-window table is installed.
+template <bool LAPS, bool REPORTS, bool WIN>
 __global__ void __launch_bounds__(256) commit_laps_books_kernel(int batch, LapPool ss, LapPool model, LapBooks k, const double* cl_x,
                                                                 const double* cl_u, int* cl_len, int Tcl, double* x_cur, int* timeStep,
                                                                 int* done, int* flags_or, Tracks trk, int lmpc, LapBudget retire,
-                                                                SsLaps laps, LapReports rep) {
+                                                                SsLaps laps, LapReports rep, LapWindows win) {
     const int b = blockIdx.x;
     if (b >= batch || retire.retired(b) || !done[b]) return;
     __shared__ int s_ss, s_md;
     const int Trec = cl_len[b];
     const double TrackLength = trk.of(b).TrackLength;
     if (threadIdx.x == 0) {
-        s_ss = lmpc ? book_ss_add(k, b, Trec, false, book_laps<LAPS>(k, laps, b)) : -1;   // ordered by the lap time; rows beyond Tmax are not stored
-        s_md = book_md_add(k, b, Trec);
+        const LapWindowRec w = book_windows<WIN>(win, b);
+        s_ss = lmpc ? book_ss_add<WIN>(k, b, Trec, false, book_laps<LAPS>(k, laps, b), w.ss_window) : -1;   // ordered by the lap time; rows beyond Tmax are not stored
+        s_md = book_md_add<WIN>(k, b, Trec, w.model_window);
         const int n = k.lap_n[b];
         if (n < LAP_HIST) k.lap_hist[(size_t)b * LAP_HIST + n] = Trec;
         k.lap_n[b] = n + 1;
@@ -179,7 +277,7 @@ __global__ void __launch_bounds__(256) commit_laps_books_kernel(int batch, LapPo
     if (s_md >= 0) copy_lap_block(model, model.lap_index(b, s_md), cx, cu, Trec);
     __syncthreads();
     if (threadIdx.x == 0) {
-        int f = book_refresh(k, b, book_laps<LAPS>(k, laps, b));
+        int f = book_refresh<WIN>(k, b, book_laps<LAPS>(k, laps, b), book_windows<WIN>(win, b));
         if (s_ss == -2) f |= 64;                                 // safe-set pool too small for numSS_it + 2 laps
         if (f && flags_or) flags_or[b] |= f;
         if constexpr (REPORTS) report_file(rep, b);
@@ -188,12 +286,12 @@ __global__ void __launch_bounds__(256) commit_laps_books_kernel(int batch, LapPo
 }
 
 // main.py:99-110 with device bookkeeping: the record every controller just drove becomes `copies` laps of both stores.
-// REPORTS: the report table starts afresh, like lap_n.
-template <bool LAPS, bool REPORTS>
+// REPORTS: the report table starts afresh, like lap_n.  WIN: a lap-window table is installed.
+template <bool LAPS, bool REPORTS, bool WIN>
 __global__ void __launch_bounds__(256) seed_books_kernel(int batch, LapPool ss, LapPool model, LapBooks k, int copies, const double* cl_x,
                                                          const double* cl_u, int* cl_len, int Tcl, int N, double* xLin, double* uLin,
                                                          double* zt, double* OldInput, int* timeStep, int* hasPred, int* done,
-                                                         Tracks trk, int lmpc, Shapes shp, SsLaps laps, LapReports rep) {
+                                                         Tracks trk, int lmpc, Shapes shp, SsLaps laps, LapReports rep, LapWindows win) {
     const int b = blockIdx.x;
     if (b >= batch) return;
     __shared__ int s_ss, s_md;
@@ -209,8 +307,9 @@ __global__ void __launch_bounds__(256) seed_books_kernel(int batch, LapPool ss, 
     __syncthreads();
     for (int c = 0; c < copies; ++c) {
         if (threadIdx.x == 0) {
-            s_ss = lmpc ? book_ss_add(k, b, Trec, false, book_laps<LAPS>(k, laps, b)) : -1;
-            s_md = book_md_add(k, b, Trec);
+            const LapWindowRec w = book_windows<WIN>(win, b);
+            s_ss = lmpc ? book_ss_add<WIN>(k, b, Trec, false, book_laps<LAPS>(k, laps, b), w.ss_window) : -1;
+            s_md = book_md_add<WIN>(k, b, Trec, w.model_window);
         }
         __syncthreads();
         if (s_ss >= 0) copy_ss_lap_block(ss, ss.lap_index(b, s_ss), cx, cu, Trec, TrackLength);
@@ -219,7 +318,7 @@ __global__ void __launch_bounds__(256) seed_books_kernel(int batch, LapPool ss, 
     }
     seed_state_block(b, N, shp, cx, cu, xLin, uLin, zt, OldInput);
     if (threadIdx.x == 0) {
-        book_refresh(k, b, book_laps<LAPS>(k, laps, b)); timeStep[b] = 0; hasPred[b] = 0; cl_len[b] = 0; done[b] = 0;
+        book_refresh<WIN>(k, b, book_laps<LAPS>(k, laps, b), book_windows<WIN>(win, b)); timeStep[b] = 0; hasPred[b] = 0; cl_len[b] = 0; done[b] = 0;
         if constexpr (REPORTS) report_restart(rep, b);
     }
 }
@@ -336,11 +435,13 @@ __global__ void __launch_bounds__(64) pool_rank_kernel(int n_src, const int* met
 // is ordered by its lap time lt in both tables, as an own lap by Trec; only the rows that fit are stored.  The regression model
 // takes the lap also when the safe set drops it: main.py adds every lap to both lists, and with trToUse > numSS_it a lap outside
 // the numSS_it fastest can be among the trToUse shortest.  A controller with no lap of its own (it = 0) takes nothing.  The
-// importer ranks a lap against its own numSS_it (LAPS), so a group may mix lap counts.  One CTA per controller.
-template <bool LAPS>
+// importer ranks a lap against its own numSS_it (LAPS) and its own windows (WIN), so a group may mix lap counts and windows.
+// One CTA per controller.
+template <bool LAPS, bool WIN>
 __global__ void __launch_bounds__(256) pool_import_kernel(int batch, LapPool ss, LapPool model, LapBooks k, int share, int Tpad,
                                                           const double* rows, const int* meta, const int* grp, const int* order,
-                                                          const int* cnt, long long gid_base, int* took, int* flags_or, SsLaps laps) {
+                                                          const int* cnt, long long gid_base, int* took, int* flags_or, SsLaps laps,
+                                                          LapWindows win) {
     const int b = blockIdx.x;
     if (b >= batch) return;
     __shared__ int s_ss, s_md, s_src;
@@ -355,9 +456,10 @@ __global__ void __launch_bounds__(256) pool_import_kernel(int batch, LapPool ss,
         ++given;
         if (threadIdx.x == 0) {
             s_src = src;
-            s_ss = book_ss_add(k, b, lt, true, book_laps<LAPS>(k, laps, b));
+            const LapWindowRec w = book_windows<WIN>(win, b);
+            s_ss = book_ss_add<WIN>(k, b, lt, true, book_laps<LAPS>(k, laps, b), w.ss_window);
             s_md = -1;
-            if (s_ss != -2 && k.it[b] > 0) s_md = book_md_add(k, b, lt);
+            if (s_ss != -2 && k.it[b] > 0) s_md = book_md_add<WIN>(k, b, lt, w.model_window);
         }
         __syncthreads();
         const int c_ss = s_ss, c_md = s_md;                       // private copies: thread 0 rewrites the shared ones next round
@@ -368,7 +470,7 @@ __global__ void __launch_bounds__(256) pool_import_kernel(int batch, LapPool ss,
         __syncthreads();
         if (threadIdx.x == 0 && c_ss == -2 && flags_or) flags_or[b] |= 64;
     }
-    if (threadIdx.x == 0 && given > 0) book_refresh(k, b, book_laps<LAPS>(k, laps, b));
+    if (threadIdx.x == 0 && given > 0) book_refresh<WIN>(k, b, book_laps<LAPS>(k, laps, b), book_windows<WIN>(win, b));
 }
 
 // Progress of a Monte-Carlo batch in four numbers per pool group, so that the host only polls a few bytes every few steps:

@@ -143,6 +143,8 @@ struct lmpc_handle {
     HandleTable<FtocpConstRec> own_c;
     // per-controller safe-set lap counts (lmpc_set_ss_laps), or none: the handle's numSS_it
     HandleTable<SsLapsRec> ssl;
+    // per-controller lap windows (lmpc_set_lap_windows), or none: every window unbounded
+    HandleTable<LapWindowRec> lwin;
     LapPool ss, mdl;
     int *d_used, *d_sel, *d_isprev, *d_prevslot, *d_timeStep, *d_hasPred, *d_flags, *d_minidx, *d_xchg, *d_health, *d_dropped;
     double *d_xLin, *d_uLin, *d_ztState, *d_ztFixed, *d_OldInput, *d_xPredPrev, *d_tmpx, *d_tmpu;
@@ -275,6 +277,7 @@ static void free_tables(lmpc_handle* h, unsigned owners) {
     release(h->meas, OWN_HANDLE); release(h->budget, OWN_HANDLE); release(h->trk, OWN_STORE); release(h->reg, OWN_STORE); release(h->pool_grp, OWN_STORE);
     for (auto& t : h->sched) release(t, OWN_HANDLE);
     release(h->shp, OWN_STORE); release(h->shp_order, OWN_STORE); release(h->own_c, OWN_HANDLE); release(h->ssl, OWN_STORE);
+    release(h->lwin, OWN_STORE);
     if (owners & OWN_STORE) h->shp_cells.clear();
 }
 
@@ -965,6 +968,7 @@ int lmpc_sizeof_measurement_params(void) { return (int)sizeof(lmpc_measurement_p
 int lmpc_sizeof_regression_params(void) { return (int)sizeof(lmpc_regression_params); }
 int lmpc_sizeof_shape_params(void) { return (int)sizeof(lmpc_shape_params); }
 int lmpc_sizeof_ss_laps_params(void) { return (int)sizeof(lmpc_ss_laps_params); }
+int lmpc_sizeof_lap_window_params(void) { return (int)sizeof(lmpc_lap_window_params); }
 int lmpc_sizeof_track_params(void) { return (int)sizeof(lmpc_track_params); }
 
 static int store_create_impl(lmpc_handle* h, const lmpc_model_params* mp, int ss_cap, int model_cap, int Tmax);
@@ -1147,6 +1151,8 @@ static bool on_grid(int N, int M) {
 
 // numSS_it / numSS_Points of controller b: its row of the lap-count / shape table, or the handle's
 static int laps_of(const lmpc_handle* h, int b) { return h->ssl.tab ? h->ssl.rows[h->ssl.index[b]].numSS_it : h->p.numSS_it; }
+// ss_window of controller b: its row of the lap-window table, or 0 (unbounded)
+static int ss_window_of(const lmpc_handle* h, int b) { return h->lwin.tab ? h->lwin.rows[h->lwin.index[b]].ss_window : 0; }
 static int points_of(const lmpc_handle* h, int b) { return h->shp.tab ? h->shp.rows[h->shp.index[b]].numSS_Points : h->M; }
 // M points split into nit laps of an even number of points each (PC.py:403,492-495)
 static bool even_split(int M, int nit) { return M % nit == 0 && (M / nit) % 2 == 0; }
@@ -1220,15 +1226,46 @@ int lmpc_set_ss_laps(lmpc_handle* h, const lmpc_ss_laps_params* sets, int nsets,
         if (sets[k].numSS_it < 1 || sets[k].numSS_it > nit)
             return fail(LMPC_E_INVALID, std::string(who) + ": set " + std::to_string(k) + ": numSS_it must be 1 .. the handle's " +
                                             std::to_string(nit));
-    for (int b = 0; b < h->batch; ++b) {       // nsets == 0: the handle's numSS_it against the installed shapes
+    for (int b = 0; b < h->batch; ++b) {       // nsets == 0: the handle's numSS_it against the installed shapes and windows
         const int v = nsets ? sets[set_of_instance[b]].numSS_it : nit;
         if (!even_split(points_of(h, b), v))
             return fail(LMPC_E_INVALID, std::string(who) + ": controller " + std::to_string(b) + ": its numSS_Points " +
                                             std::to_string(points_of(h, b)) + " is not numSS_it (" + std::to_string(v) +
                                             ") times an even number of points per lap");
+        if (ss_window_of(h, b) > 0 && v > ss_window_of(h, b))
+            return fail(LMPC_E_INVALID, std::string(who) + ": controller " + std::to_string(b) + ": numSS_it " + std::to_string(v) +
+                                            " exceeds its ss_window (" + std::to_string(ss_window_of(h, b)) + ")");
     }
     return install_table(h, who, h->ssl, sets, nsets, set_of_instance, (const SsLapsRec*)nullptr, [&](int k, SsLapsRec& row) {
         row = sets[k];
+        return LMPC_OK;
+    });
+}
+
+// Per-controller lap windows: every set checked against the store and every controller's numSS_it, then the table (DESIGN.md,
+// "Per-controller lap windows"); nsets == 0 removes it.
+int lmpc_set_lap_windows(lmpc_handle* h, const lmpc_lap_window_params* sets, int nsets, const int* set_of_instance) {
+    static const char* who = "lmpc_set_lap_windows";
+    int rc = need_store(h);
+    if (rc) return rc;
+    if (h->laps_stored) return fail(LMPC_E_STATE, std::string(who) + ": laps are stored already; install lap windows before the first lap");
+    if ((rc = check_set_index(h, who, sets, nsets, set_of_instance)) != LMPC_OK) return rc;
+    for (int b = 0; b < (nsets ? h->batch : 0); ++b) {    // the safe-set window against the controller's own numSS_it
+        const int w = sets[set_of_instance[b]].ss_window;
+        if (w > 0 && w < laps_of(h, b))
+            return fail(LMPC_E_INVALID, std::string(who) + ": controller " + std::to_string(b) + ": ss_window " + std::to_string(w) +
+                                            " is below its numSS_it (" + std::to_string(laps_of(h, b)) + ")");
+    }
+    return install_table(h, who, h->lwin, sets, nsets, set_of_instance, (const LapWindowRec*)nullptr, [&](int k, LapWindowRec& row) {
+        const lmpc_lap_window_params& s = sets[k];
+        const std::string w = std::string(who) + ": set " + std::to_string(k) + ": ";
+        if (s.ss_window != 0 && h->M <= 0) return fail(LMPC_E_INVALID, w + "ss_window must be 0: the handle has no safe set (numSS_Points == 0)");
+        if (s.ss_window < 0 || s.ss_window > h->ss.cap)
+            return fail(LMPC_E_INVALID, w + "ss_window must be 0 or numSS_it .. ss_cap (" + std::to_string(h->ss.cap) + ")");
+        if (s.model_window != 0 && (s.model_window < h->mc.trToUse || s.model_window > h->mdl.cap))
+            return fail(LMPC_E_INVALID, w + "model_window must be 0 or trToUse (" + std::to_string(h->mc.trToUse) + ") .. model_cap (" +
+                                            std::to_string(h->mdl.cap) + ")");
+        row = s;
         return LMPC_OK;
     });
 }
@@ -2014,6 +2051,12 @@ int lmpc_probe_fp64(int device, double* out8) {
 // ================================================================================================
 // device lap books (lapbooks.cuh): the reference's once-per-lap list bookkeeping without the host
 // ================================================================================================
+// The instantiation of a lap-book kernel for what the handle has installed: a lap-count table (LAPS), lap reports (REPORTS, the
+// three-flag kernels only) and a lap-window table (WIN, always the last flag)
+#define BOOK_KERNEL2(K, a, w) ((a) ? ((w) ? K<true, true> : K<true, false>) : ((w) ? K<false, true> : K<false, false>))
+#define BOOK_KERNEL3(K, a, r, w)                                                                                     \
+    ((a) ? ((r) ? ((w) ? K<true, true, true> : K<true, true, false>) : ((w) ? K<true, false, true> : K<true, false, false>))   \
+         : ((r) ? ((w) ? K<false, true, true> : K<false, true, false>) : ((w) ? K<false, false, true> : K<false, false, false>)))
 int lmpc_books_set(lmpc_handle* h, const int* ss_time, const int* ss_lap, const int* it, const int* md_time, const int* md_seq,
                    const int* md_cnt) {
     int rc = need_store(h);
@@ -2025,7 +2068,8 @@ int lmpc_books_set(lmpc_handle* h, const int* ss_time, const int* ss_lap, const 
         return rc;
     CK(cudaMemsetAsync(k.lap_n, 0, sizeof(int) * h->batch, h->stream));
     // sel, is_prev, prev_slot, used of these tables
-    (h->ssl.tab ? books_refresh_kernel<true> : books_refresh_kernel<false>)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->batch, k, h->ssl.view());
+    BOOK_KERNEL2(books_refresh_kernel, h->ssl.tab, h->lwin.tab)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->batch, k, h->ssl.view(),
+                                                                                                              h->lwin.view());
     CK(cudaGetLastError());
     h->launches += 1;
     CK(cudaStreamSynchronize(h->stream));
@@ -2049,10 +2093,9 @@ int lmpc_books_get(lmpc_handle* h, int* ss_time, int* ss_lap, int* it, int* md_t
 int lmpc_rollout_commit_laps_dev(lmpc_handle* h) {
     if (int rc = need_rollout(h)) return rc;
     h->laps_stored = true;     // enqueue only: which controllers finish a lap is not known here
-    (h->ssl.tab ? (h->rep_L ? commit_laps_books_kernel<true, true> : commit_laps_books_kernel<true, false>)
-                : (h->rep_L ? commit_laps_books_kernel<false, true> : commit_laps_books_kernel<false, false>))<<<h->batch, 256, 0, h->stream>>>(
+    BOOK_KERNEL3(commit_laps_books_kernel, h->ssl.tab, h->rep_L, h->lwin.tab)<<<h->batch, 256, 0, h->stream>>>(
         h->batch, h->ss, h->mdl, h->bk, h->d_clx, h->d_clu, h->d_cllen, h->Tcl, h->d_rx[h->cur], h->d_timeStep, h->d_done, h->d_health,
-        tracks(h), h->M > 0 ? 1 : 0, lap_budget(h), h->ssl.view(), reports(h));
+        tracks(h), h->M > 0 ? 1 : 0, lap_budget(h), h->ssl.view(), reports(h), h->lwin.view());
     CK(cudaGetLastError());
     h->launches += 1;
     return LMPC_OK;
@@ -2063,10 +2106,10 @@ int lmpc_rollout_seed_from_record_dev(lmpc_handle* h, int copies) {
     if (copies < 1 || (h->M > 0 && copies > h->ss.cap) || copies > h->mdl.cap) return fail(LMPC_E_INVALID, "seed copies do not fit the lap pools");
     h->laps_stored = true;
     if (h->d_warm_valid) CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * h->batch, h->stream));
-    (h->ssl.tab ? (h->rep_L ? seed_books_kernel<true, true> : seed_books_kernel<true, false>)
-                : (h->rep_L ? seed_books_kernel<false, true> : seed_books_kernel<false, false>))<<<h->batch, 256, 0, h->stream>>>(
+    BOOK_KERNEL3(seed_books_kernel, h->ssl.tab, h->rep_L, h->lwin.tab)<<<h->batch, 256, 0, h->stream>>>(
         h->batch, h->ss, h->mdl, h->bk, copies, h->d_clx, h->d_clu, h->d_cllen, h->Tcl, h->N, h->d_xLin, h->d_uLin, h->d_ztState,
-        h->d_OldInput, h->d_timeStep, h->d_hasPred, h->d_done, tracks(h), h->M > 0 ? 1 : 0, h->shp.view(), h->ssl.view(), reports(h));
+        h->d_OldInput, h->d_timeStep, h->d_hasPred, h->d_done, tracks(h), h->M > 0 ? 1 : 0, h->shp.view(), h->ssl.view(), reports(h),
+        h->lwin.view());
     CK(cudaGetLastError());
     h->launches += 1;
     return LMPC_OK;
@@ -2153,9 +2196,9 @@ int lmpc_pool_import_dev(lmpc_handle* h, int n_src, int share, int Tpad, long lo
     int* took = h->d_poolidx + POOL_TOOK;
     CK(cudaMemsetAsync(took, 0, sizeof(int), h->stream));
     pool_rank_kernel<<<G, 64, 0, h->stream>>>(n_src, meta_dev, order, cnt);
-    (h->ssl.tab ? pool_import_kernel<true> : pool_import_kernel<false>)<<<h->batch, 256, 0, h->stream>>>(
+    BOOK_KERNEL2(pool_import_kernel, h->ssl.tab, h->lwin.tab)<<<h->batch, 256, 0, h->stream>>>(
         h->batch, h->ss, h->mdl, h->bk, share, Tpad, rows_dev, meta_dev, h->pool_grp.idx, order, cnt, gid_base, took,
-        h->has_rollout ? h->d_health : nullptr, h->ssl.view());
+        h->has_rollout ? h->d_health : nullptr, h->ssl.view(), h->lwin.view());
     CK(cudaGetLastError());
     h->launches += 2;
     if (took_host) {

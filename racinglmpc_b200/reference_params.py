@@ -127,6 +127,21 @@ class RegressionParams:
         return cls(int(trToUse), 7, 5.0, 0.0, (0.1, 1.0, 1.0, 1.0, 1.0))
 
 
+@dataclass(frozen=True)
+class LapWindowParams:
+    """How many of its most recent laps a controller's safe set and learned model draw from (0 = unbounded, the reference's
+    rule): the safe set selects its numSS_it fastest laps among lap numbers [it - ss_window, it), the model regresses on the
+    trToUse shortest laps among the last model_window it filed.  The device takes one per controller
+    (BatchedController.set_lap_windows)."""
+    ss_window: int = 0
+    model_window: int = 0
+
+    @classmethod
+    def unbounded(cls):
+        """Both windows unbounded: installed, the controllers select and store exactly what they do without a table."""
+        return cls(0, 0)
+
+
 def _wrap(a):
     if a < -np.pi:
         return 2 * np.pi + a
