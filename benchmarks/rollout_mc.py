@@ -132,7 +132,8 @@ def lap_row_summary(reps, schedules, laps):
 def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, poll=8, max_steps=0, seed=1234, local=None, warm=False,
         final=None, param_sets=None, vehicle_sets=None, books=None, track_sets=None, pool_groups=None, readiness="batch",
         capture=None, start=None, noise_sets=None, noise_streams=None, regression_sets=None, lap_budget=None, measurement_sets=None,
-        shape_sets=None, ss_laps_sets=None, lap_reports=None, lap_schedules=None, lap_window_sets=None):
+        shape_sets=None, ss_laps_sets=None, lap_reports=None, lap_schedules=None, lap_window_sets=None,
+        lane_rule_sets=None):
     """One Monte-Carlo run on this rank's GPU (torch.distributed may or may not be initialised).  Returns a dict (all ranks).
     final: None, or a dict that receives the closed loop's end state (rollout_state) and the last step's solver report (step_results).
     books: None, or a dict that receives the lap books (books) and the health counters (flags_or, unsolved), and with lap_reports
@@ -226,7 +227,14 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     lap: objects with ss_window (0 or the controller's numSS_it .. ss_cap 7) and model_window (0 or trToUse 4 .. model_cap 5), 0
     = unbounded (controllers that trust only their most recent laps).  The result then holds per-window lap statistics and mean
     interior-point iterations under "per_lap_window_rank0".  capture records every controller's windows and start refuses others.
-    ValueError before any device work where set_lap_windows would refuse."""
+    ValueError before any device work where set_lap_windows would refuse.
+    lane_rule_sets: None, or (rules, index) handed to BatchedController.set_lane_rules with the other tables, before the PID lap:
+    objects with mode (0: the reference's ranking, 1: a lap that left the lane by more than lane_tol ranks behind every lap that kept
+    to it) and lane_tol.  The result then holds per-rule lap statistics and mean interior-point iterations under
+    "per_lane_rule_rank0", with lap reports the share of laps judged lane-unsafe per lap ("lane_unsafe_share" of every
+    lap_reports_rank0 row and of every per-rule report row), and "lane_unsafe_selected_share_rank0": the share of controllers whose
+    final selection holds a lane-unsafe lap.  capture records every controller's rule and start refuses others.  ValueError before
+    any device work where set_lane_rules would refuse."""
     L = check_lap_reports(lap_reports, laps)
     scheds = check_lap_schedules(lap_schedules, batch, L, {"vehicle": vehicle_sets, "noise": noise_sets,
                                                            "measurement": measurement_sets})
@@ -248,8 +256,12 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         rows, widx = _native.make_lap_window_sets(lap_window_sets[0], lap_window_sets[1], int(batch), laps_of, SS_CAP, TR_TO_USE,
                                                   MODEL_CAP)
         windows = np.array([[rows[k].ss_window, rows[k].model_window] for k in widx], np.int32)
+    lanes = None                                                   # [batch, 2] (mode, lane_tol), or None
+    if lane_rule_sets is not None:
+        rows, ridx = _native.make_lane_rule_sets(lane_rule_sets[0], lane_rule_sets[1], int(batch), True, TCL)
+        lanes = np.array([[rows[k].mode, rows[k].lane_tol] for k in ridx], np.float64)
     if start is not None:
-        _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget, shape_sets, L, scheds, windows)
+        _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget, shape_sets, L, scheds, windows, lanes)
     if capture is not None and not isinstance(capture, dict):
         raise ValueError("capture is a dict that receives the run's end state")
     if readiness not in ("batch", "group"):
@@ -287,7 +299,8 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
               (measurement_sets, c.set_measurement_noise, "per_measurement_rank0"),
               (regression_sets, c.set_regression, "per_regression_rank0"), (track_sets, c.set_tracks, "per_track_rank0"),
               (pool_groups, c.set_pool_groups, None), (shape_sets, c.set_shapes, "per_shape_rank0"),
-              (ss_laps_sets, c.set_ss_laps, "per_ss_laps_rank0"), (lap_window_sets, c.set_lap_windows, "per_lap_window_rank0"))
+              (ss_laps_sets, c.set_ss_laps, "per_ss_laps_rank0"), (lap_window_sets, c.set_lap_windows, "per_lap_window_rank0"),
+              (lane_rule_sets, c.set_lane_rules, "per_lane_rule_rank0"))
     for args, install, _ in tables:
         if args is not None:
             install(*args)
@@ -381,7 +394,8 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
                        poll=poll, warm=bool(warm), pool_groups=G, layout=c.snapshot_layout(),
                        lap_budget=None if budget is None else budget.tolist(),
                        lap_schedules={kind: row_of_lap.tolist() for kind, row_of_lap in scheds.items()},
-                       lap_windows=None if windows is None else windows.tolist())
+                       lap_windows=None if windows is None else windows.tolist(),
+                       lane_rules=None if lanes is None else lanes.tolist())
     flags_or, unsolved = c.rollout_health()
     reps = c.lap_reports() if L else None
     lens, n_laps = (reps["steps"], reps["n"]) if L else (bk["lap_hist"], bk["lap_n"])
@@ -436,6 +450,20 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
             w = lap_window_sets[0][k]
             s.update(ss_window=int(w.ss_window), model_window=int(w.model_window),
                      ipm_iters_mean_sampled=float(it_ctrl[idx == k].mean() / max(it_n, 1)) if (idx == k).any() else 0.0)
+    if lane_rule_sets is not None:
+        idx = np.asarray(lane_rule_sets[1]).reshape(B)
+        for k, s in enumerate(out["per_lane_rule_rank0"]):
+            r = lane_rule_sets[0][k]
+            s.update(mode=int(r.mode), lane_tol=float(r.lane_tol),
+                     ipm_iters_mean_sampled=float(it_ctrl[idx == k].mean() / max(it_n, 1)) if (idx == k).any() else 0.0)
+            if L:
+                _add_unsafe_share(s["reports"], reps, idx == k, laps)
+        if L:
+            _add_unsafe_share(out["lap_reports_rank0"], reps, np.ones(B, bool), laps)
+        _, unsafe = _native.split_lane_key(bk["ss_time"])
+        nit = np.array([c.ss_laps_of(b) for b in range(B)])
+        held = np.array([unsafe[b, bk["sel"][b, :nit[b]]].any() for b in range(B)])
+        out["lane_unsafe_selected_share_rank0"] = float(held.mean())
     if pool_groups is not None:
         # a stored lap advances `it`: 4 seeded copies + every own lap handed over + every imported lap filed.  Exact unless an
         # own lap found the safe-set pool full (health flag 64): then that controller's count is one too low per such lap.
@@ -475,7 +503,7 @@ def _driven_steps(bk, state):
 
 
 def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget=None, shape_sets=None, lap_reports=0,
-                 lap_schedules=None, lap_windows=None):
+                 lap_schedules=None, lap_windows=None, lane_rules=None):
     """The refusals of run(start=...), before any device work: a start that does not match this run (report capacity, lap
     schedules and lap windows included), laps not above the captured laps, or a lap budget below the captured one."""
     if not isinstance(start, dict):
@@ -509,6 +537,7 @@ def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, b
         raise ValueError("start was captured with lap_schedules for %s, this run has %s (or other rows): a run resumes under the "
                          "schedules it was captured with" % (sorted(had) or "none", sorted(mine) or "none"))
     check_start_windows(start.get("lap_windows"), lap_windows)
+    check_start_lane_rules(start.get("lane_rules"), lane_rules)
     for k, v in layout(warm, shape_sets).items():
         if int(start["layout"].get(k, -1)) != v:
             raise ValueError("start records have %s = %s, this run's controllers %d" % (k, start["layout"].get(k), v))
@@ -520,6 +549,22 @@ def check_start_windows(had, mine):
     if (had is None) != (mine is None) or (had is not None and not np.array_equal(np.asarray(had), mine)):
         raise ValueError("start was captured with other lap windows: a record resumes exactly only under the windows it was captured "
                          "with")
+
+
+def check_start_lane_rules(had, mine):
+    """start's refusal of other lane rules: `had` the captured [batch, 2] (mode, lane_tol) rows (a list, or None without a table),
+    `mine` this run's (an array, or None).  The rules are not part of a record, and the books ranked the stored laps under them."""
+    if (had is None) != (mine is None) or (had is not None and not np.array_equal(np.asarray(had, np.float64), mine)):
+        raise ValueError("start was captured with other lane rules: a record resumes exactly only under the rules it was captured "
+                         "with")
+
+
+def _add_unsafe_share(rows, reps, sel, laps):
+    """Adds "lane_unsafe_share" to every per-lap row of lap_report_summary: the share of the controllers `sel` that filed lap r whose
+    report carries the lane-unsafe bit (their own lap was judged lane-unsafe at its hand-over)."""
+    for r, row in enumerate(rows[:laps]):
+        m = sel & (reps["n"] > r)
+        row["lane_unsafe_share"] = float(((reps["flags"][m, r] & _native.REPORT_LANE_UNSAFE) != 0).mean()) if m.any() else 0.0
 
 
 def _set_stats(bk, flags_or, unsolved, sel, laps, reps=None):

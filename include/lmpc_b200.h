@@ -335,6 +335,43 @@ typedef struct lmpc_lap_window_params {
  *   - Not part of a snapshot record (LMPC_SNAPSHOT_VERSION is unchanged): a record resumes exactly only under the same windows. */
 int lmpc_set_lap_windows(lmpc_handle* h, const lmpc_lap_window_params* sets, int nsets, const int* set_of_instance);
 
+/* Per-controller lane rules: whether a lap that left the lane may rank among the laps a controller's safe set draws from. */
+#define LMPC_LANE_UNSAFE_KEY (1 << 24)       /* added to the safe-set key (ss_time) of a lap judged lane-unsafe */
+#define LMPC_REPORT_LANE_UNSAFE (1 << 16)    /* report-only flag bit: the filed own lap was judged lane-unsafe */
+typedef struct lmpc_lane_rule_params {
+    int mode;            /* 0: the reference's rule (laps ranked by lap time alone); 1: every lap filed is judged */
+    int pad;
+    double lane_tol;     /* mode 1: a lap is lane-unsafe when a judged row leaves a lane row by more than lane_tol */
+} lmpc_lane_rule_params;
+/* Per-controller lane rules (LMPC's sampled safe set assumes laps that satisfy the constraints; the QP's lane is soft, so a lap
+ * that crossed it is stored like any other and, being faster, is the first one selected).  Controller b reads row
+ * sets[set_of_instance[b]].  nsets == 0 (sets, set_of_instance NULL) removes the table: every controller ranks by lap time.
+ *   - Judgement (mode 1): a lap is lane-unsafe when one of its judged rows x has a non-finite entry, or when for a lane row i
+ *     d_i = (sum over j = 0..5, in order, of Fx[i][j] * x[j], fp64 without fused multiply-adds) - bx[i] > lane_tol: the
+ *     arithmetic of the lap reports (lmpc_rollout_enable_lap_reports) with the threshold lane_tol.  Fx, bx are the controller's
+ *     own QP constants: its parameter-set row, else the handle's.  Judged rows: an own lap's rows 0 .. Trec-1 of the closed-loop
+ *     record at the hand-over (the rows the controller files: under measurement noise the measured states); the seeded record
+ *     once for all its copies; an import's shipped rows 0 .. min(lap time, rows, Tpad)-1, against the importer's own Fx, bx and
+ *     lane_tol (the export still chooses and ships by raw lap time).
+ *   - Ranking: an unsafe lap is filed with the key ss_time = lap time + LMPC_LANE_UNSAFE_KEY, a safe one with its lap time.  The
+ *     books compare (ss_time, lap number) as before, so the selection is the stable argsort by (unsafe, lap time, lap number),
+ *     first numSS_it_b; unsafe laps still fill it when fewer safe laps exist (flag 8 and the storage rule are unchanged), and an
+ *     unsafe own latest lap stays lap it-1 for addPoint.  The regression model (md_time, usedIt), lap_hist and the reports keep
+ *     raw lengths.  The pooled export strips the offset for its ranking, its min_overrun test and meta[.,1].
+ *   - Reports: the filed report of an own lap judged unsafe carries LMPC_REPORT_LANE_UNSAFE in its flags (the health word does
+ *     not).
+ *   - Requires lmpc_store_create and a safe set (numSS_Points > 0), and no lap stored yet in either pool, whether the call
+ *     installs or removes (else LMPC_E_STATE).  1 <= nsets <= batch, every index in [0, nsets); mode 0 or 1, lane_tol finite and
+ *     >= 0; with a mode 1 row, a rollout of Tcl >= LMPC_LANE_UNSAFE_KEY is refused.  Any failed check returns LMPC_E_INVALID
+ *     and leaves the handle as it was.  The call synchronises the handle's streams before it replaces the table.
+ *   - While a mode 1 row is installed, the host-slot paths (lmpc_rollout_commit_laps, lmpc_rollout_seed_from_record) return
+ *     LMPC_E_STATE (they take the caller's books, which do not judge laps) and lmpc_rollout_create refuses Tcl >=
+ *     LMPC_LANE_UNSAFE_KEY.  Keys >= LMPC_LANE_UNSAFE_KEY are only valid where a controller's rule is on: lmpc_books_set and
+ *     lmpc_snapshot_unpack_dev (field "lane key") refuse an occupied slot with such a key for a controller whose rule is off.
+ *   - Not part of a snapshot record (LMPC_SNAPSHOT_VERSION is unchanged): the keys travel in ss_time, so a record resumes exactly
+ *     under the same rules. */
+int lmpc_set_lane_rules(lmpc_handle* h, const lmpc_lane_rule_params* sets, int nsets, const int* set_of_instance);
+
 /* PredictiveModel.addTrajectory (PredictiveModel.py:35-46): copy one lap into a regression slot. */
 int lmpc_model_put_lap(lmpc_handle* h, int inst, int slot, int T, const double* x, const double* u);
 /* usedIt order: slots[B,trToUse]. */
@@ -736,6 +773,7 @@ int lmpc_sizeof_regression_params(void);
 int lmpc_sizeof_shape_params(void);
 int lmpc_sizeof_ss_laps_params(void);
 int lmpc_sizeof_lap_window_params(void);
+int lmpc_sizeof_lane_rule_params(void);
 
 #ifdef __cplusplus
 }

@@ -70,6 +70,28 @@ class LapWindowParams(C.Structure):
     _fields_ = [("ss_window", C.c_int), ("model_window", C.c_int)]
 
 
+class LaneRuleParams(C.Structure):
+    """lmpc_lane_rule_params: mode 0 ranks laps by lap time (the reference's rule), mode 1 ranks a lap that left the lane by more
+    than lane_tol behind every lap that kept to it."""
+    _fields_ = [("mode", C.c_int), ("pad", C.c_int), ("lane_tol", C.c_double)]
+
+
+LANE_UNSAFE_KEY = 1 << 24           # LMPC_LANE_UNSAFE_KEY: added to the safe-set key of a lane-unsafe lap
+REPORT_LANE_UNSAFE = 1 << 16        # LMPC_REPORT_LANE_UNSAFE: report flag of an own lap judged lane-unsafe
+
+
+def split_lane_key(ss_time):
+    """(lap time, unsafe) of safe-set keys (``books()["ss_time"]``, a scalar or an array): a key >= LANE_UNSAFE_KEY is a lap judged
+    lane-unsafe under a lane rule, filed as lap time + LANE_UNSAFE_KEY.  A free slot's key (INT32_MAX) is returned as it is, unsafe
+    False."""
+    k = np.asarray(ss_time, np.int64)
+    unsafe = (k >= LANE_UNSAFE_KEY) & (k != 0x7FFFFFFF)
+    t = np.where(unsafe, k - LANE_UNSAFE_KEY, k)
+    if t.ndim == 0:
+        return int(t), bool(unsafe)
+    return t.astype(np.int32), unsafe
+
+
 # The (N, numSS_Points) pairs the library instantiates the QP kernel for: LMPC_FOR_EACH_CASE in csrc/ftocp_launch.cuh (a CPU test
 # keeps the two equal)
 SHAPE_GRID = tuple([(n, 0) for n in (4, 6, 8, 10, 12, 14, 16, 20, 24, 32, 48)] + [(n, 48) for n in (4, 6, 8, 10, 12, 14, 16, 20, 24, 32, 48)] +
@@ -199,6 +221,7 @@ def lib():
     L.lmpc_set_shapes.argtypes = [_vp, C.POINTER(ShapeParams), C.c_int, _vp]
     L.lmpc_set_ss_laps.argtypes = [_vp, C.POINTER(SsLapsParams), C.c_int, _vp]
     L.lmpc_set_lap_windows.argtypes = [_vp, C.POINTER(LapWindowParams), C.c_int, _vp]
+    L.lmpc_set_lane_rules.argtypes = [_vp, C.POINTER(LaneRuleParams), C.c_int, _vp]
     L.lmpc_rollout_sysid.argtypes = [_vp, C.c_double, _vp, _vp]
     L.lmpc_rollout_seed_from_record.argtypes = [_vp, C.c_int, C.c_int, C.c_int]
     L.lmpc_rollout_get_lap.argtypes = [_vp, C.c_int, ip, _vp, _vp]
@@ -243,6 +266,8 @@ def lib():
     assert L.lmpc_sizeof_ss_laps_params() == C.sizeof(SsLapsParams), "lmpc_ss_laps_params ABI mismatch"
     L.lmpc_sizeof_lap_window_params.restype = C.c_int
     assert L.lmpc_sizeof_lap_window_params() == C.sizeof(LapWindowParams), "lmpc_lap_window_params ABI mismatch"
+    L.lmpc_sizeof_lane_rule_params.restype = C.c_int
+    assert L.lmpc_sizeof_lane_rule_params() == C.sizeof(LaneRuleParams), "lmpc_lane_rule_params ABI mismatch"
     L.lmpc_sizeof_lap_report.restype = C.c_int
     assert L.lmpc_sizeof_lap_report() == C.sizeof(LapReport), "lmpc_lap_report ABI mismatch"
     assert L.lmpc_sizeof_noise_params() == C.sizeof(NoiseParams), "lmpc_noise_params ABI mismatch"
@@ -690,6 +715,29 @@ def make_lap_window_sets(windows, index, batch, ss_laps, ss_cap, trToUse, model_
         if 0 < w < v:
             raise ValueError("controller %d: ss_window %d is below its numSS_it (%d)" % (b, w, v))
     return rows, idx
+
+
+def make_lane_rule_sets(rules, index, batch, lmpc=True, Tcl=0):
+    """Per-controller lane rules for ``lmpc_set_lane_rules``: K objects ``rules`` with ``mode`` (0 or 1) and ``lane_tol`` (e.g.
+    reference_params.LaneRuleParams) and the row of every controller ``index[batch]``.  Raises ValueError where the library would
+    refuse a value: the index rules of ``make_param_sets``, a handle without a safe set (``lmpc`` False), a mode that is not the
+    integer 0 or 1, a lane_tol that is not a finite number >= 0, or a mode 1 row with a rollout of ``Tcl`` >= LANE_UNSAFE_KEY.
+    Returns (ctypes array LaneRuleParams * K, int32 index array)."""
+    if not lmpc:
+        raise ValueError("lane rules need a safe set: the handle has numSS_Points == 0")
+
+    def row(k, r):
+        m, tol = r.mode, r.lane_tol
+        if isinstance(m, (bool, np.bool_)) or not isinstance(m, (int, np.integer)) or int(m) not in (0, 1):
+            raise ValueError("lane rule %d: mode must be 0 or 1, got %r" % (k, m))
+        if isinstance(tol, (bool, np.bool_)) or not isinstance(tol, (int, float, np.integer, np.floating)):
+            raise ValueError("lane rule %d: lane_tol must be a number, got %r" % (k, tol))
+        if not (np.isfinite(float(tol)) and float(tol) >= 0.0):
+            raise ValueError("lane rule %d: lane_tol must be finite and >= 0, got %r" % (k, tol))
+        if int(m) == 1 and int(Tcl) >= LANE_UNSAFE_KEY:
+            raise ValueError("lane rule %d: the rollout's Tcl (%d) must stay below LANE_UNSAFE_KEY" % (k, int(Tcl)))
+        return LaneRuleParams(int(m), 0, float(tol))
+    return _pack_sets(LaneRuleParams, rules, index, batch, "lane rules", row)
 
 
 def make_pool_groups(index, ngroups, batch):

@@ -69,6 +69,7 @@ class BatchedController:
         self._shapes = None                                 # (shapes, index) of set_shapes, or None: the handle's own shape
         self._ss_laps = None                                # numSS_it of every controller (set_ss_laps), or None: the handle's
         self._windows = None                                # [B, 2] (ss_window, model_window) of set_lap_windows, or None: unbounded
+        self._lane = None                                   # [(mode, lane_tol)] * B of set_lane_rules, or None: the reference's rule
         # rows of the plant-side tables a lap schedule indexes (the defaults: one reference vehicle and noise, no measurement
         # table) and the installed schedules [B, L] of set_lap_schedule
         self._table_rows = {"vehicle": 1, "noise": 1, "measurement": 0}
@@ -295,6 +296,33 @@ class BatchedController:
     def lap_windows_of(self, inst):
         """(ss_window, model_window) of controller ``inst`` under ``set_lap_windows``, (0, 0) (unbounded) without a table."""
         return (0, 0) if self._windows is None else (int(self._windows[int(inst), 0]), int(self._windows[int(inst), 1]))
+
+    def set_lane_rules(self, rules, index=None):
+        """Per-controller lane rules (lane-safe safe sets): controller b with ``rules[index[b]].mode == 1`` judges every lap it
+        files -- its own laps, the seeded record and every import, against its own QP's lane rows Fx x <= bx -- and ranks a lap
+        whose rows leave a lane row by more than ``lane_tol`` (or hold a non-finite entry) behind every lap that kept to it; mode 0
+        is the reference's rule (objects with ``mode`` and ``lane_tol``, e.g. reference_params.LaneRuleParams).  Such a lap is
+        filed with the safe-set key lap time + LANE_UNSAFE_KEY (``_native.split_lane_key`` splits ``books()["ss_time"]``); the
+        learned model and the lap history keep raw lengths.  ``index`` is required with ``rules``.  ``rules=None`` (no index)
+        removes the table.  Only on an LMPC handle and before the first lap is stored; under a mode 1 row the host-slot hand-over
+        and seeding are refused (use the device books).  Not part of a snapshot (a record resumes exactly under the same rules).
+        ValueError before any native call where the library would refuse a value.  Waits for work already enqueued."""
+        self._install(self._lib.lmpc_set_lane_rules, "rules", rules, index,
+                      lambda: nat.make_lane_rule_sets(rules, index, self.B, self.lmpc, getattr(self, "Tcl", 0)))
+        if rules is None:
+            self._lane = None
+        else:
+            rows = [(int(r.mode), float(r.lane_tol)) for r in rules]
+            self._lane = [rows[int(i)] for i in np.asarray(index).reshape(-1)]
+
+    def lane_rules_of(self, inst):
+        """(mode, lane_tol) of controller ``inst`` under ``set_lane_rules``, (0, 0.0) (the reference's rule) without a table."""
+        return (0, 0.0) if self._lane is None else self._lane[int(inst)]
+
+    def _no_lane_rule(self, what):
+        """The host-slot paths keep the caller's books, which do not judge laps: refused while a mode 1 lane rule is installed."""
+        if self._lane is not None and any(m == 1 for m, _ in self._lane):
+            raise ValueError("%s: a lane rule is installed; lane rules need the device books (the *_dev methods)" % what)
 
     def set_tracks(self, tracks, index=None):
         """Per-controller tracks (several circuits in one batch): controller b drives ``tracks[index[b]]`` (objects with
@@ -588,6 +616,8 @@ class BatchedController:
 
     # ------------------------------------------------------------------ device-resident closed loop
     def enable_rollout(self, Tcl=512):
+        if int(Tcl) >= nat.LANE_UNSAFE_KEY and self._lane is not None and any(m == 1 for m, _ in self._lane):
+            raise ValueError("enable_rollout: a lane rule is installed: Tcl must stay below LANE_UNSAFE_KEY")
         nat.check(self._lib.lmpc_rollout_create(self._h, int(Tcl)))
         self.Tcl = int(Tcl)
 
@@ -627,6 +657,7 @@ class BatchedController:
     def rollout_seed_from_record(self, cl_len, copies=4):
         """main.py:99-110 on the device: the record every instance just drove (cl_len[b] rows, e.g. its PID lap) becomes
         ``copies`` identical laps of the safe set and of the regression model, and the controller state is initialised from it."""
+        self._no_lane_rule("rollout_seed_from_record")
         ss0 = m0 = None
         for b in range(self.B):
             T = int(cl_len[b])
@@ -691,6 +722,7 @@ class BatchedController:
     def rollout_finish_laps(self, done, cl_len, to_model=True):
         """main.py:113-119 for every instance whose lap just ended: lmpc.addTrajectory + predictiveModel.addTrajectory of the
         lap recorded on the device (no host copy of the lap), then the next lap starts from xF (SysModel.py:50)."""
+        self._no_lane_rule("rollout_finish_laps")
         finished = np.nonzero(done)[0]
         if not len(finished):
             return finished

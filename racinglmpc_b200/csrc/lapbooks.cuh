@@ -43,6 +43,52 @@ using LapWindows = Table<LapWindowRec>;
 template <bool WIN>
 __device__ __forceinline__ LapWindowRec book_windows(const LapWindows& w, int b) { return WIN ? w.of(b) : LapWindowRec{0, 0}; }
 
+// The lane rules of every controller (lmpc_set_lane_rules) and the QP constants (Fx, bx) they judge against: the controller's
+// parameter-set row, else the handle's.  The five kernels that file or ship safe-set laps come in two more instantiations, LANE =
+// a rule table is installed; without one they never read it and the key of a lap is its lap time, the code they were before.
+using LaneRuleRec = lmpc_lane_rule_params;
+struct LaneRules {
+    Table<LaneRuleRec> rule;
+    Table<FtocpConstRec> qp;
+};
+
+// Is the lap x[0 .. T) (row r at x + r * stride, its state in the first 6 entries) lane-unsafe for controller b?  False without a
+// table (LANE) or under mode 0.  A row is unsafe when an entry is not finite or d_i = Fx[i] . x - bx[i] > lane_tol for one of the
+// ncx == 2 lane rows, evaluated in order without contraction: the arithmetic of report_step (safeset.cuh), kept as a copy of its
+// own so that the closed loop's step kernel stays the code it was.  One block-wide pass; every thread of the block must call it.
+template <bool LANE>
+__device__ __forceinline__ bool lane_unsafe_block(const LaneRules& lr, int b, const double* x, int T, int stride) {
+    if constexpr (!LANE) {
+        return false;
+    } else {
+        const LaneRuleRec r = lr.rule.of(b);
+        if (r.mode != 1) return false;                           // uniform over the block: no barrier is skipped by part of it
+        const FtocpConst& c = lr.qp.of(b).c;
+        bool bad = false;
+        for (int t = threadIdx.x; t < T && !bad; t += blockDim.x) {
+            const double* xr = x + (size_t)t * stride;
+            double v[6];
+            bool finite = true;
+#pragma unroll
+            for (int j = 0; j < 6; ++j) { v[j] = xr[j]; finite = finite && isfinite(v[j]); }
+            if (!finite) { bad = true; break; }
+#pragma unroll
+            for (int i = 0; i < 2; ++i) {
+                double s = __dmul_rn(c.Fx[i * 6], v[0]);
+#pragma unroll
+                for (int j = 1; j < 6; ++j) s = __dadd_rn(s, __dmul_rn(c.Fx[i * 6 + j], v[j]));
+                bad = bad || __dsub_rn(s, c.bx[i]) > r.lane_tol;
+            }
+        }
+        return __syncthreads_or(bad) != 0;
+    }
+}
+// The safe-set key a lap of lap time T is filed with: T, plus LMPC_LANE_UNSAFE_KEY when it was judged lane-unsafe
+__device__ __forceinline__ int lane_key(int T, bool unsafe) { return unsafe ? T + LMPC_LANE_UNSAFE_KEY : T; }
+// The lap time of a safe-set key (the pooled export ranks and ships raw lap times)
+template <bool LANE>
+__device__ __forceinline__ int lane_lap_time(int key) { return LANE && key >= LMPC_LANE_UNSAFE_KEY ? key - LMPC_LANE_UNSAFE_KEY : key; }
+
 // book_ss_add under a safe-set window of W >= 1 laps: after the event the window is lap numbers [it' - W, it'), it' = it + 1.  A
 // lap stays stored while it is in the window and fewer than nit NEWER laps rank ahead of it: older laps leave the window before it
 // does, newer ones stay as long as it does, so only they can keep it out of the selection for good.  An import's only newer lap
@@ -251,20 +297,22 @@ __global__ void books_refresh_kernel(int batch, LapBooks k, SsLaps laps, LapWind
 // Lap hand-over of every controller whose lap just ended (done[b] != 0), bookkeeping included: main.py:113-119
 // (lmpc.addTrajectory + predictiveModel.addTrajectory of the lap Simulator.sim returned), SysModel.py:50 (s -= TrackLength),
 // PC.py:445 (timeStep = 0).  One CTA per controller; no host involvement.  REPORTS: the running report row is filed as the lap's.
-// WIN: a lap-window table is installed.
-template <bool LAPS, bool REPORTS, bool WIN>
+// WIN: a lap-window table is installed.  LANE: a lane-rule table is installed; the lap's rows 0 .. Trec-1 are judged and an unsafe
+// lap is filed with its lap time + LMPC_LANE_UNSAFE_KEY as its safe-set key (its report carries LMPC_REPORT_LANE_UNSAFE).
+template <bool LAPS, bool REPORTS, bool WIN, bool LANE>
 __global__ void __launch_bounds__(256) commit_laps_books_kernel(int batch, LapPool ss, LapPool model, LapBooks k, const double* cl_x,
                                                                 const double* cl_u, int* cl_len, int Tcl, double* x_cur, int* timeStep,
                                                                 int* done, int* flags_or, Tracks trk, int lmpc, LapBudget retire,
-                                                                SsLaps laps, LapReports rep, LapWindows win) {
+                                                                SsLaps laps, LapReports rep, LapWindows win, LaneRules lane) {
     const int b = blockIdx.x;
     if (b >= batch || retire.retired(b) || !done[b]) return;
     __shared__ int s_ss, s_md;
     const int Trec = cl_len[b];
     const double TrackLength = trk.of(b).TrackLength;
+    const bool unsafe = lane_unsafe_block<LANE>(lane, b, cl_x + (size_t)b * Tcl * 6, Trec, 6);
     if (threadIdx.x == 0) {
         const LapWindowRec w = book_windows<WIN>(win, b);
-        s_ss = lmpc ? book_ss_add<WIN>(k, b, Trec, false, book_laps<LAPS>(k, laps, b), w.ss_window) : -1;   // ordered by the lap time; rows beyond Tmax are not stored
+        s_ss = lmpc ? book_ss_add<WIN>(k, b, lane_key(Trec, unsafe), false, book_laps<LAPS>(k, laps, b), w.ss_window) : -1;   // ordered by the lap time; rows beyond Tmax are not stored
         s_md = book_md_add<WIN>(k, b, Trec, w.model_window);
         const int n = k.lap_n[b];
         if (n < LAP_HIST) k.lap_hist[(size_t)b * LAP_HIST + n] = Trec;
@@ -280,18 +328,23 @@ __global__ void __launch_bounds__(256) commit_laps_books_kernel(int batch, LapPo
         int f = book_refresh<WIN>(k, b, book_laps<LAPS>(k, laps, b), book_windows<WIN>(win, b));
         if (s_ss == -2) f |= 64;                                 // safe-set pool too small for numSS_it + 2 laps
         if (f && flags_or) flags_or[b] |= f;
-        if constexpr (REPORTS) report_file(rep, b);
+        if constexpr (REPORTS) {
+            if (unsafe) rep.run[b].row.flags |= LMPC_REPORT_LANE_UNSAFE;
+            report_file(rep, b);
+        }
         restart_record(b, cl_len, x_cur, timeStep, done, TrackLength);
     }
 }
 
 // main.py:99-110 with device bookkeeping: the record every controller just drove becomes `copies` laps of both stores.
-// REPORTS: the report table starts afresh, like lap_n.  WIN: a lap-window table is installed.
-template <bool LAPS, bool REPORTS, bool WIN>
+// REPORTS: the report table starts afresh, like lap_n.  WIN: a lap-window table is installed.  LANE: a lane-rule table is
+// installed; the record is judged once and every copy is filed with the same key.
+template <bool LAPS, bool REPORTS, bool WIN, bool LANE>
 __global__ void __launch_bounds__(256) seed_books_kernel(int batch, LapPool ss, LapPool model, LapBooks k, int copies, const double* cl_x,
                                                          const double* cl_u, int* cl_len, int Tcl, int N, double* xLin, double* uLin,
                                                          double* zt, double* OldInput, int* timeStep, int* hasPred, int* done,
-                                                         Tracks trk, int lmpc, Shapes shp, SsLaps laps, LapReports rep, LapWindows win) {
+                                                         Tracks trk, int lmpc, Shapes shp, SsLaps laps, LapReports rep, LapWindows win,
+                                                         LaneRules lane) {
     const int b = blockIdx.x;
     if (b >= batch) return;
     __shared__ int s_ss, s_md;
@@ -304,11 +357,12 @@ __global__ void __launch_bounds__(256) seed_books_kernel(int batch, LapPool ss, 
         for (int s = 0; s < k.md_cap; ++s) { k.md_seq[(size_t)b * k.md_cap + s] = -1; k.md_time[(size_t)b * k.md_cap + s] = 0x7fffffff; }
         k.it[b] = 0; k.md_cnt[b] = 0; k.lap_n[b] = 0;
     }
+    const bool unsafe = lane_unsafe_block<LANE>(lane, b, cx, Trec, 6);
     __syncthreads();
     for (int c = 0; c < copies; ++c) {
         if (threadIdx.x == 0) {
             const LapWindowRec w = book_windows<WIN>(win, b);
-            s_ss = lmpc ? book_ss_add<WIN>(k, b, Trec, false, book_laps<LAPS>(k, laps, b), w.ss_window) : -1;
+            s_ss = lmpc ? book_ss_add<WIN>(k, b, lane_key(Trec, unsafe), false, book_laps<LAPS>(k, laps, b), w.ss_window) : -1;
             s_md = book_md_add<WIN>(k, b, Trec, w.model_window);
         }
         __syncthreads();
@@ -352,7 +406,9 @@ __device__ __forceinline__ int pool_group(const int* grp, int b) { return grp ? 
 // `min_over` rows past its finish line (rows - lap time; addPoint appends them during the next lap): an importer's safe-set
 // window near the finish reaches into those rows.  One CTA per group; k rounds of block arg-min over the group's controllers.
 // ship (null: every group) masks groups out of this export: a group with ship[g] == 0 chooses no controller, so
-// pool_export_kernel ships its kbest rows with global id -1 and importers file nothing of it.
+// pool_export_kernel ships its kbest rows with global id -1 and importers file nothing of it.  LANE: a lane-rule table is
+// installed; a latest lap is ranked and tested by its lap time, its safe-set key without LMPC_LANE_UNSAFE_KEY.
+template <bool LANE>
 __global__ void __launch_bounds__(1024) pool_local_best_kernel(int batch, LapPool ss, LapBooks k, int kbest, int Tpad, int min_over,
                                                                const int* grp, const int* ship, int* best_inst) {
     __shared__ unsigned long long red[32];
@@ -367,7 +423,7 @@ __global__ void __launch_bounds__(1024) pool_local_best_kernel(int batch, LapPoo
         for (int b = threadIdx.x; b < batch; b += blockDim.x) {
             const int sl = k.prevslot[b];
             if (sl < 0 || pool_group(grp, b) != g) continue;
-            const int t = k.ss_time[(size_t)b * k.ss_cap + sl];
+            const int t = lane_lap_time<LANE>(k.ss_time[(size_t)b * k.ss_cap + sl]);
             if (min_over > 0 && min(ss.len[ss.lap_index(b, sl)], Tpad) - t < min_over) continue;
             bool skip = false;
             for (int j = 0; j < r; ++j) skip |= (taken[j] == b);
@@ -388,7 +444,8 @@ __global__ void __launch_bounds__(1024) pool_local_best_kernel(int batch, LapPoo
 }
 
 // Pack the latest own lap of the chosen controllers into exchange rows rows[G][kbest][Tpad][XR_COLS], meta[G][kbest][4].
-// One CTA per row r = g * kbest + j.
+// One CTA per row r = g * kbest + j.  LANE: meta[.,1] is the lap time, the safe-set key without LMPC_LANE_UNSAFE_KEY.
+template <bool LANE>
 __global__ void __launch_bounds__(256) pool_export_kernel(LapPool ss, LapBooks k, const int* best_inst, int kbest, int Tpad,
                                                           long long gid_base, double* rows, int* meta) {
     const int r = blockIdx.x;
@@ -399,7 +456,7 @@ __global__ void __launch_bounds__(256) pool_export_kernel(LapPool ss, LapBooks k
     pack_lap_row_block(ss, lap, T, Tpad, rows + (size_t)r * Tpad * XR_COLS);
     if (threadIdx.x == 0) {
         meta[r * 4 + 0] = T;
-        meta[r * 4 + 1] = sl < 0 ? 0x7fffffff : k.ss_time[(size_t)b * k.ss_cap + sl];
+        meta[r * 4 + 1] = sl < 0 ? 0x7fffffff : lane_lap_time<LANE>(k.ss_time[(size_t)b * k.ss_cap + sl]);
         meta[r * 4 + 2] = sl < 0 ? -1 : (int)(gid_base + b);
         meta[r * 4 + 3] = r / kbest;
     }
@@ -436,12 +493,14 @@ __global__ void __launch_bounds__(64) pool_rank_kernel(int n_src, const int* met
 // takes the lap also when the safe set drops it: main.py adds every lap to both lists, and with trToUse > numSS_it a lap outside
 // the numSS_it fastest can be among the trToUse shortest.  A controller with no lap of its own (it = 0) takes nothing.  The
 // importer ranks a lap against its own numSS_it (LAPS) and its own windows (WIN), so a group may mix lap counts and windows.
-// One CTA per controller.
-template <bool LAPS, bool WIN>
+// LANE: a lane-rule table is installed; the importer judges the shipped rows 0 .. min(lt, rows, Tpad)-1 against its own rule and
+// QP constants and files an unsafe lap with the safe-set key lt + LMPC_LANE_UNSAFE_KEY (the model takes lt).  One CTA per
+// controller.
+template <bool LAPS, bool WIN, bool LANE>
 __global__ void __launch_bounds__(256) pool_import_kernel(int batch, LapPool ss, LapPool model, LapBooks k, int share, int Tpad,
                                                           const double* rows, const int* meta, const int* grp, const int* order,
                                                           const int* cnt, long long gid_base, int* took, int* flags_or, SsLaps laps,
-                                                          LapWindows win) {
+                                                          LapWindows win, LaneRules lane) {
     const int b = blockIdx.x;
     if (b >= batch) return;
     __shared__ int s_ss, s_md, s_src;
@@ -454,10 +513,11 @@ __global__ void __launch_bounds__(256) pool_import_kernel(int batch, LapPool ss,
         if (gid < 0 || len < 2) break;                            // nothing valid further down the ranking
         if ((long long)gid == gid_base + b) continue;             // its own lap
         ++given;
+        const bool unsafe = lane_unsafe_block<LANE>(lane, b, rows + (size_t)src * Tpad * XR_COLS, min(min(lt, len), Tpad), XR_COLS);
         if (threadIdx.x == 0) {
             s_src = src;
             const LapWindowRec w = book_windows<WIN>(win, b);
-            s_ss = book_ss_add<WIN>(k, b, lt, true, book_laps<LAPS>(k, laps, b), w.ss_window);
+            s_ss = book_ss_add<WIN>(k, b, lane_key(lt, unsafe), true, book_laps<LAPS>(k, laps, b), w.ss_window);
             s_md = -1;
             if (s_ss != -2 && k.it[b] > 0) s_md = book_md_add<WIN>(k, b, lt, w.model_window);
         }

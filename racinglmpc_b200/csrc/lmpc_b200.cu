@@ -145,6 +145,8 @@ struct lmpc_handle {
     HandleTable<SsLapsRec> ssl;
     // per-controller lap windows (lmpc_set_lap_windows), or none: every window unbounded
     HandleTable<LapWindowRec> lwin;
+    // per-controller lane rules (lmpc_set_lane_rules), or none: every lap ranked by its lap time
+    HandleTable<LaneRuleRec> lrule;
     LapPool ss, mdl;
     int *d_used, *d_sel, *d_isprev, *d_prevslot, *d_timeStep, *d_hasPred, *d_flags, *d_minidx, *d_xchg, *d_health, *d_dropped;
     double *d_xLin, *d_uLin, *d_ztState, *d_ztFixed, *d_OldInput, *d_xPredPrev, *d_tmpx, *d_tmpu;
@@ -277,7 +279,7 @@ static void free_tables(lmpc_handle* h, unsigned owners) {
     release(h->meas, OWN_HANDLE); release(h->budget, OWN_HANDLE); release(h->trk, OWN_STORE); release(h->reg, OWN_STORE); release(h->pool_grp, OWN_STORE);
     for (auto& t : h->sched) release(t, OWN_HANDLE);
     release(h->shp, OWN_STORE); release(h->shp_order, OWN_STORE); release(h->own_c, OWN_HANDLE); release(h->ssl, OWN_STORE);
-    release(h->lwin, OWN_STORE);
+    release(h->lwin, OWN_STORE); release(h->lrule, OWN_STORE);
     if (owners & OWN_STORE) h->shp_cells.clear();
 }
 
@@ -524,6 +526,18 @@ static LapReports reports(const lmpc_handle* h) {
     if (!h->rep_L) return LapReports{};
     return LapReports{h->d_rep_rows, h->d_rep_run, h->rep_L, h->sets.tab ? h->sets.view() : h->own_c.view()};
 }
+
+// The lane rules and the QP constants they judge against, as the lap-book kernels take them (only the LANE instantiations read them)
+static LaneRules lane_rules(const lmpc_handle* h) {
+    return LaneRules{h->lrule.view(), h->sets.tab ? h->sets.view() : h->own_c.view()};
+}
+// A lane rule of mode 1 is installed (a row of the table; rows nobody reads count too)
+static bool lane_rules_on(const lmpc_handle* h) {
+    for (const LaneRuleRec& r : h->lrule.rows) if (r.mode == 1) return true;
+    return false;
+}
+// Controller b's rule is on: its safe-set keys may carry LMPC_LANE_UNSAFE_KEY
+static bool lane_rule_of(const lmpc_handle* h, int b) { return h->lrule.tab && h->lrule.rows[h->lrule.index[b]].mode == 1; }
 
 static void free_rollout(lmpc_handle* h) {
     free_bufs(dev_bufs(h), OWN_ROLLOUT | OWN_TRACE | OWN_REPORTS);
@@ -969,6 +983,7 @@ int lmpc_sizeof_regression_params(void) { return (int)sizeof(lmpc_regression_par
 int lmpc_sizeof_shape_params(void) { return (int)sizeof(lmpc_shape_params); }
 int lmpc_sizeof_ss_laps_params(void) { return (int)sizeof(lmpc_ss_laps_params); }
 int lmpc_sizeof_lap_window_params(void) { return (int)sizeof(lmpc_lap_window_params); }
+int lmpc_sizeof_lane_rule_params(void) { return (int)sizeof(lmpc_lane_rule_params); }
 int lmpc_sizeof_track_params(void) { return (int)sizeof(lmpc_track_params); }
 
 static int store_create_impl(lmpc_handle* h, const lmpc_model_params* mp, int ss_cap, int model_cap, int Tmax);
@@ -1266,6 +1281,26 @@ int lmpc_set_lap_windows(lmpc_handle* h, const lmpc_lap_window_params* sets, int
             return fail(LMPC_E_INVALID, w + "model_window must be 0 or trToUse (" + std::to_string(h->mc.trToUse) + ") .. model_cap (" +
                                             std::to_string(h->mdl.cap) + ")");
         row = s;
+        return LMPC_OK;
+    });
+}
+
+// Per-controller lane rules: every set checked, then the table (DESIGN.md, "Lane-safe safe sets"); nsets == 0 removes it.
+int lmpc_set_lane_rules(lmpc_handle* h, const lmpc_lane_rule_params* sets, int nsets, const int* set_of_instance) {
+    static const char* who = "lmpc_set_lane_rules";
+    int rc = need_store(h);
+    if (rc) return rc;
+    if (h->M <= 0) return fail(LMPC_E_STATE, std::string(who) + ": the handle has no safe set (numSS_Points == 0)");
+    if (h->laps_stored) return fail(LMPC_E_STATE, std::string(who) + ": laps are stored already; install lane rules before the first lap");
+    return install_table(h, who, h->lrule, sets, nsets, set_of_instance, (const LaneRuleRec*)nullptr, [&](int k, LaneRuleRec& row) {
+        const lmpc_lane_rule_params& s = sets[k];
+        const std::string w = std::string(who) + ": set " + std::to_string(k) + ": ";
+        if (s.mode != 0 && s.mode != 1) return fail(LMPC_E_INVALID, w + "mode must be 0 or 1");
+        if (!isfinite(s.lane_tol) || s.lane_tol < 0.0) return fail(LMPC_E_INVALID, w + "lane_tol must be finite and >= 0");
+        if (s.mode == 1 && h->has_rollout && h->Tcl >= LMPC_LANE_UNSAFE_KEY)
+            return fail(LMPC_E_INVALID, w + "the rollout's Tcl is not below LMPC_LANE_UNSAFE_KEY");
+        row = s;
+        row.pad = 0;
         return LMPC_OK;
     });
 }
@@ -1591,6 +1626,8 @@ static int rollout_create_impl(lmpc_handle* h, int Tcl) {
     if (rc) return rc;
     if (h->has_rollout) return fail(LMPC_E_STATE, "rollout buffers already created");
     if (Tcl < 16) return fail(LMPC_E_INVALID, "Tcl too small");
+    if (Tcl >= LMPC_LANE_UNSAFE_KEY && lane_rules_on(h))
+        return fail(LMPC_E_INVALID, "lmpc_rollout_create: a lane rule is installed: a lap time must stay below LMPC_LANE_UNSAFE_KEY");
     h->Tcl = Tcl; h->cur = 0; h->sim_step = 0;
     if ((rc = alloc_bufs(h, dev_bufs(h), OWN_ROLLOUT, h->batch, "lmpc_rollout_create")) != LMPC_OK) return rc;
     h->has_rollout = true;
@@ -1915,6 +1952,7 @@ int lmpc_rollout_sysid(lmpc_handle* h, double lamb, double* abc_host, int* flags
 // regression slots model_slot0.., the controller state is initialised from it and the record restarts.
 int lmpc_rollout_seed_from_record(lmpc_handle* h, int copies, int ss_slot0, int model_slot0) {
     if (int rc = need_rollout(h)) return rc;
+    if (lane_rules_on(h)) return fail(LMPC_E_STATE, "lmpc_rollout_seed_from_record: lane rules need the device books (_dev)");
     if (copies < 1 || ss_slot0 < 0 || model_slot0 < 0 || ss_slot0 + copies > h->ss.cap || model_slot0 + copies > h->mdl.cap)
         return fail(LMPC_E_INVALID, "seed copies do not fit the lap pools");
     h->laps_stored = true;
@@ -1944,6 +1982,7 @@ int lmpc_rollout_get_lap(lmpc_handle* h, int inst, int* T, double* x, double* u)
 // controller's step counter is reset (PC.py:445).
 int lmpc_rollout_commit_laps(lmpc_handle* h, const int* fin, const int* ss_slots, const int* model_slots) {
     if (int rc = need_rollout(h)) return rc;
+    if (lane_rules_on(h)) return fail(LMPC_E_STATE, "lmpc_rollout_commit_laps: lane rules need the device books (_dev)");
     if (!fin || !ss_slots || !model_slots) return fail(LMPC_E_INVALID, "null argument");
     for (int b = 0; b < h->batch; ++b)
         if (fin[b] && (ss_slots[b] >= h->ss.cap || model_slots[b] >= h->mdl.cap)) return fail(LMPC_E_INVALID, "slot out of range");
@@ -2052,24 +2091,32 @@ int lmpc_probe_fp64(int device, double* out8) {
 // device lap books (lapbooks.cuh): the reference's once-per-lap list bookkeeping without the host
 // ================================================================================================
 // The instantiation of a lap-book kernel for what the handle has installed: a lap-count table (LAPS), lap reports (REPORTS, the
-// three-flag kernels only) and a lap-window table (WIN, always the last flag)
-#define BOOK_KERNEL2(K, a, w) ((a) ? ((w) ? K<true, true> : K<true, false>) : ((w) ? K<false, true> : K<false, false>))
-#define BOOK_KERNEL3(K, a, r, w)                                                                                     \
-    ((a) ? ((r) ? ((w) ? K<true, true, true> : K<true, true, false>) : ((w) ? K<true, false, true> : K<true, false, false>))   \
-         : ((r) ? ((w) ? K<false, true, true> : K<false, true, false>) : ((w) ? K<false, false, true> : K<false, false, false>)))
+// kernels of BOOK_KERNEL3 only), a lap-window table (WIN) and a lane-rule table (LANE, always the last flag; books_refresh_kernel
+// has none).  BOOK_FLAG appends the flags w (and l) to the leading ones in __VA_ARGS__.
+#define BOOK_FLAG(K, w, ...) ((w) ? K<__VA_ARGS__, true> : K<__VA_ARGS__, false>)
+#define BOOK_FLAGS(K, w, l, ...) ((w) ? BOOK_FLAG(K, l, __VA_ARGS__, true) : BOOK_FLAG(K, l, __VA_ARGS__, false))
+#define BOOK_REFRESH(a, w) ((a) ? BOOK_FLAG(books_refresh_kernel, w, true) : BOOK_FLAG(books_refresh_kernel, w, false))
+#define BOOK_KERNEL2(K, a, w, l) ((a) ? BOOK_FLAGS(K, w, l, true) : BOOK_FLAGS(K, w, l, false))
+#define BOOK_KERNEL3(K, a, r, w, l)                                                                              \
+    ((a) ? ((r) ? BOOK_FLAGS(K, w, l, true, true) : BOOK_FLAGS(K, w, l, true, false))                            \
+         : ((r) ? BOOK_FLAGS(K, w, l, false, true) : BOOK_FLAGS(K, w, l, false, false)))
 int lmpc_books_set(lmpc_handle* h, const int* ss_time, const int* ss_lap, const int* it, const int* md_time, const int* md_seq,
                    const int* md_cnt) {
     int rc = need_store(h);
     if (rc) return rc;
     if (!ss_time || !ss_lap || !it || !md_time || !md_seq || !md_cnt) return fail(LMPC_E_INVALID, "null argument");
     const LapBooks& k = h->bk;
+    for (int b = 0; b < h->batch; ++b)     // a lane-unsafe key belongs to a controller whose lane rule is on
+        for (int s = 0; s < k.ss_cap && !lane_rule_of(h, b); ++s)
+            if (ss_lap[(size_t)b * k.ss_cap + s] >= 0 && ss_time[(size_t)b * k.ss_cap + s] >= LMPC_LANE_UNSAFE_KEY)
+                return fail(LMPC_E_INVALID, "lmpc_books_set: controller " + std::to_string(b) + ", slot " + std::to_string(s) +
+                                                ": a lane-unsafe key (>= LMPC_LANE_UNSAFE_KEY) without a lane rule");
     if ((rc = copy_bufs(h, cudaMemcpyHostToDevice, {{k.ss_time, ss_time}, {k.ss_lap, ss_lap}, {k.it, it}, {k.md_time, md_time},
                                                    {k.md_seq, md_seq}, {k.md_cnt, md_cnt}})))
         return rc;
     CK(cudaMemsetAsync(k.lap_n, 0, sizeof(int) * h->batch, h->stream));
     // sel, is_prev, prev_slot, used of these tables
-    BOOK_KERNEL2(books_refresh_kernel, h->ssl.tab, h->lwin.tab)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->batch, k, h->ssl.view(),
-                                                                                                              h->lwin.view());
+    BOOK_REFRESH(h->ssl.tab, h->lwin.tab)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->batch, k, h->ssl.view(), h->lwin.view());
     CK(cudaGetLastError());
     h->launches += 1;
     CK(cudaStreamSynchronize(h->stream));
@@ -2093,9 +2140,9 @@ int lmpc_books_get(lmpc_handle* h, int* ss_time, int* ss_lap, int* it, int* md_t
 int lmpc_rollout_commit_laps_dev(lmpc_handle* h) {
     if (int rc = need_rollout(h)) return rc;
     h->laps_stored = true;     // enqueue only: which controllers finish a lap is not known here
-    BOOK_KERNEL3(commit_laps_books_kernel, h->ssl.tab, h->rep_L, h->lwin.tab)<<<h->batch, 256, 0, h->stream>>>(
+    BOOK_KERNEL3(commit_laps_books_kernel, h->ssl.tab, h->rep_L, h->lwin.tab, h->lrule.tab)<<<h->batch, 256, 0, h->stream>>>(
         h->batch, h->ss, h->mdl, h->bk, h->d_clx, h->d_clu, h->d_cllen, h->Tcl, h->d_rx[h->cur], h->d_timeStep, h->d_done, h->d_health,
-        tracks(h), h->M > 0 ? 1 : 0, lap_budget(h), h->ssl.view(), reports(h), h->lwin.view());
+        tracks(h), h->M > 0 ? 1 : 0, lap_budget(h), h->ssl.view(), reports(h), h->lwin.view(), lane_rules(h));
     CK(cudaGetLastError());
     h->launches += 1;
     return LMPC_OK;
@@ -2106,10 +2153,10 @@ int lmpc_rollout_seed_from_record_dev(lmpc_handle* h, int copies) {
     if (copies < 1 || (h->M > 0 && copies > h->ss.cap) || copies > h->mdl.cap) return fail(LMPC_E_INVALID, "seed copies do not fit the lap pools");
     h->laps_stored = true;
     if (h->d_warm_valid) CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * h->batch, h->stream));
-    BOOK_KERNEL3(seed_books_kernel, h->ssl.tab, h->rep_L, h->lwin.tab)<<<h->batch, 256, 0, h->stream>>>(
+    BOOK_KERNEL3(seed_books_kernel, h->ssl.tab, h->rep_L, h->lwin.tab, h->lrule.tab)<<<h->batch, 256, 0, h->stream>>>(
         h->batch, h->ss, h->mdl, h->bk, copies, h->d_clx, h->d_clu, h->d_cllen, h->Tcl, h->N, h->d_xLin, h->d_uLin, h->d_ztState,
         h->d_OldInput, h->d_timeStep, h->d_hasPred, h->d_done, tracks(h), h->M > 0 ? 1 : 0, h->shp.view(), h->ssl.view(), reports(h),
-        h->lwin.view());
+        h->lwin.view(), lane_rules(h));
     CK(cudaGetLastError());
     h->launches += 1;
     return LMPC_OK;
@@ -2155,9 +2202,10 @@ static int pool_export(lmpc_handle* h, const char* who, int kbest, int Tpad, lon
         ship = h->d_poolidx + POOL_SHIP;
         CK(cudaMemcpyAsync(ship, mask, sizeof(int) * G, cudaMemcpyHostToDevice, h->stream));
     }
-    pool_local_best_kernel<<<G, 1024, 0, h->stream>>>(h->batch, h->ss, h->bk, kbest, Tpad, h->pool_min_over, h->pool_grp.idx, ship,
-                                                       h->d_poolidx);
-    pool_export_kernel<<<G * kbest, 256, 0, h->stream>>>(h->ss, h->bk, h->d_poolidx, kbest, Tpad, gid_base, rows_dev, meta_dev);
+    (h->lrule.tab ? pool_local_best_kernel<true> : pool_local_best_kernel<false>)<<<G, 1024, 0, h->stream>>>(
+        h->batch, h->ss, h->bk, kbest, Tpad, h->pool_min_over, h->pool_grp.idx, ship, h->d_poolidx);
+    (h->lrule.tab ? pool_export_kernel<true> : pool_export_kernel<false>)<<<G * kbest, 256, 0, h->stream>>>(
+        h->ss, h->bk, h->d_poolidx, kbest, Tpad, gid_base, rows_dev, meta_dev);
     CK(cudaGetLastError());
     h->launches += 2;
     return LMPC_OK;
@@ -2196,9 +2244,9 @@ int lmpc_pool_import_dev(lmpc_handle* h, int n_src, int share, int Tpad, long lo
     int* took = h->d_poolidx + POOL_TOOK;
     CK(cudaMemsetAsync(took, 0, sizeof(int), h->stream));
     pool_rank_kernel<<<G, 64, 0, h->stream>>>(n_src, meta_dev, order, cnt);
-    BOOK_KERNEL2(pool_import_kernel, h->ssl.tab, h->lwin.tab)<<<h->batch, 256, 0, h->stream>>>(
+    BOOK_KERNEL2(pool_import_kernel, h->ssl.tab, h->lwin.tab, h->lrule.tab)<<<h->batch, 256, 0, h->stream>>>(
         h->batch, h->ss, h->mdl, h->bk, share, Tpad, rows_dev, meta_dev, h->pool_grp.idx, order, cnt, gid_base, took,
-        h->has_rollout ? h->d_health : nullptr, h->ssl.view(), h->lwin.view());
+        h->has_rollout ? h->d_health : nullptr, h->ssl.view(), h->lwin.view(), lane_rules(h));
     CK(cudaGetLastError());
     h->launches += 2;
     if (took_host) {
@@ -2218,7 +2266,7 @@ static const char* snap_field_name(int f) {
         "magic", "version", "record bytes", "N", "numSS_Points", "ncx", "ncu", "numSS_it", "trToUse", "ss_cap", "model_cap", "Tmax",
         "Tcl", "warm_start", "warm_mode", "nsect", "section table", "track row", "safe-set lap length", "model lap length", "it",
         "safe-set lap number", "md_cnt", "model arrival number", "lap_n", "sel", "is_prev", "prev_slot", "used", "timeStep",
-        "has_pred", "warm_valid", "cl_len", "done", "lap report layout", "lap report count"};
+        "has_pred", "warm_valid", "cl_len", "done", "lap report layout", "lap report count", "lane key"};
     return f >= 0 && f < SF_NFIELD ? names[f] : "?";
 }
 
@@ -2369,6 +2417,7 @@ int lmpc_snapshot_unpack_dev(lmpc_handle* h, const void* rec_dev, int nrec, int 
     a.trk = tracks(h);
     a.ss_cap = h->ss.cap; a.md_cap = h->mdl.cap; a.numSS_it = h->bk.numSS_it; a.trToUse = h->bk.trToUse; a.Tmax = h->ss.Tmax;
     a.Tcl = hd.Tcl; a.warm_mode = hd.warm_mode;
+    a.lane = h->lrule.view();
     snapshot_check_kernel<<<(n + 127) / 128, 128, 0, h->stream>>>(a, n, d_idx, d_idx + n, (const char*)rec_dev, hd.bytes, verdict);
     h->launches += 1;
     int got[3];
@@ -2384,7 +2433,8 @@ int lmpc_snapshot_unpack_dev(lmpc_handle* h, const void* rec_dev, int nrec, int 
     if (got[0] != INT32_MAX) {
         const int i = got[0] / 64, f = got[0] % 64;
         why = "record " + std::to_string(idx[n + i]) + " (into controller " + std::to_string(idx[i]) + "): " + snap_field_name(f) +
-              (f <= SF_SECTIONS || f == SF_LAP_REPORTS ? " differs from this handle's" : f == SF_TRACK ? " differs from the controller's track" : " out of range");
+              (f <= SF_SECTIONS || f == SF_LAP_REPORTS ? " differs from this handle's" : f == SF_TRACK ? " differs from the controller's track"
+               : f == SF_LANE_KEY ? " marks a lane-unsafe lap of a controller whose lane rule is off" : " out of range");
     } else if (h->d_warm && got[1] <= got[2]) {
         if (h->warm_mode < 0 && got[1] != got[2]) why = "the records hold warm-start records of two problem types";
         else mode = got[1];

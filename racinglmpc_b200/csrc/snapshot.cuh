@@ -78,7 +78,7 @@ __global__ void __launch_bounds__(256) snapshot_copy_kernel(const __grid_constan
 enum SnapField {
     SF_WARM_MODE = 14, SF_SECTIONS = 16, SF_TRACK, SF_SS_LEN, SF_MD_LEN, SF_IT, SF_SS_LAP, SF_MD_CNT, SF_MD_SEQ, SF_LAP_N, SF_SEL,
     SF_ISPREV, SF_PREVSLOT, SF_USED, SF_TIMESTEP, SF_HASPRED, SF_WARM_VALID, SF_CLLEN, SF_DONE, SF_LAP_REPORTS, SF_LAP_REPORT_N,
-    SF_NFIELD
+    SF_LANE_KEY, SF_NFIELD
 };
 constexpr int SNAP_HDR_WORDS = 16 + 2 * LMPC_SNAPSHOT_SECTIONS;   // int words of the header before the track row
 
@@ -87,6 +87,7 @@ struct SnapCheckArgs {
     int rec_off[SN_COUNT];
     Tracks trk;
     int ss_cap, md_cap, numSS_it, trToUse, Tmax, Tcl, warm_mode;
+    Table<LaneRuleRec> lane;   // lane rules (lmpc_set_lane_rules): only a controller whose rule is on may hold a lane-unsafe key
 };
 
 __device__ __forceinline__ const int* snap_ints(const char* R, const SnapCheckArgs& a, int sect) {
@@ -128,6 +129,8 @@ __global__ void __launch_bounds__(128) snapshot_check_kernel(const SnapCheckArgs
             const int len = snap_ints(R, a, SN_SS_LEN)[s], ln = snap_ints(R, a, SN_SS_LAP)[s];
             BAD(len < 0 || len > a.Tmax, SF_SS_LEN);
             BAD(ln < -1 || ln >= it, SF_SS_LAP);
+            BAD(ln >= 0 && snap_ints(R, a, SN_SS_TIME)[s] >= LMPC_LANE_UNSAFE_KEY && !(a.lane.tab && a.lane.of(inst[i]).mode == 1),
+                SF_LANE_KEY);
         }
         for (int s = 0; s < a.md_cap; ++s) {
             const int len = snap_ints(R, a, SN_MD_LEN)[s], sq = snap_ints(R, a, SN_MD_SEQ)[s];

@@ -142,6 +142,21 @@ class LapWindowParams:
         return cls(0, 0)
 
 
+@dataclass(frozen=True)
+class LaneRuleParams:
+    """Whether a controller's safe set ranks a lap that left the lane behind every lap that kept to it: mode 0 is the
+    reference's rule (laps ranked by lap time alone), mode 1 judges every lap the controller files and ranks one whose rows leave
+    a lane row by more than lane_tol behind the others.  The device takes one per controller
+    (BatchedController.set_lane_rules)."""
+    mode: int = 0
+    lane_tol: float = 0.0
+
+    @classmethod
+    def reference(cls):
+        """The reference's rule: installed, the controllers rank and store exactly what they do without a table."""
+        return cls(0, 0.0)
+
+
 def _wrap(a):
     if a < -np.pi:
         return 2 * np.pi + a

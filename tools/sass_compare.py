@@ -8,8 +8,10 @@ and the instantiations that run without a per-controller table of the other kern
 across their untemplated names:
   default  knn_ltv_regress_kernel, ss_select_kernel, shift_state_kernel (<false>: no shape or lap-count table),
            books_refresh_kernel, commit_laps_books_kernel, seed_books_kernel, pool_import_kernel (<false>: no lap-count table;
-           <false, false>: no lap-count table and no lap reports, or no lap-count table and no lap-window table; <false, false,
-           false>: no lap-count table, no lap reports and no lap-window table), commit_laps_kernel, seed_from_record_kernel
+           <false, false>: no lap-count table and no lap-window table; <false, false, false>: no lap-count table, no lap-window
+           table and no lane-rule table; <false, false, false, false>: no lap-count table, no lap reports, no lap-window table and
+           no lane-rule table), pool_local_best_kernel, pool_export_kernel (<false>: no lane-rule table), commit_laps_kernel,
+           seed_from_record_kernel
            (<false>: no lap reports), sim_step_kernel (<false> or <false, false>: no lap reports and no lap schedule) and measure_kernel (<false>:
            no lap schedule)
   reports  sim_step_kernel<true> or <true, false>: lap reports and no lap schedule
@@ -30,7 +32,8 @@ import sys
 NAME = re.compile(r"^(?:void )?(ftocp_kernel|ftocp_sets_kernel)<(\d+), (\d+), 2, 4(?:, (true|false))?>")
 DEFAULT = re.compile(r"^(?:void )?lmpc::(knn_ltv_regress_kernel|ss_select_kernel|shift_state_kernel|books_refresh_kernel|"
                      r"commit_laps_books_kernel|seed_books_kernel|pool_import_kernel|sim_step_kernel|commit_laps_kernel|"
-                     r"seed_from_record_kernel|measure_kernel)(<false>|<false, false>|<false, false, false>)?\(")
+                     r"seed_from_record_kernel|measure_kernel|pool_local_best_kernel|pool_export_kernel)"
+                     r"(<false>|<false, false>|<false, false, false>|<false, false, false, false>)?\(")
 REPORTS = re.compile(r"^(?:void )?lmpc::(sim_step_kernel)<true(?:, false)?>\(")
 
 
