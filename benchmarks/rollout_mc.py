@@ -133,11 +133,12 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         final=None, param_sets=None, vehicle_sets=None, books=None, track_sets=None, pool_groups=None, readiness="batch",
         capture=None, start=None, noise_sets=None, noise_streams=None, regression_sets=None, lap_budget=None, measurement_sets=None,
         shape_sets=None, ss_laps_sets=None, lap_reports=None, lap_schedules=None, lap_window_sets=None,
-        lane_rule_sets=None):
+        lane_rule_sets=None, lane_margin_sets=None):
     """One Monte-Carlo run on this rank's GPU (torch.distributed may or may not be initialised).  Returns a dict (all ranks).
     final: None, or a dict that receives the closed loop's end state (rollout_state) and the last step's solver report (step_results).
     books: None, or a dict that receives the lap books (books) and the health counters (flags_or, unsolved), and with lap_reports
-    the reports (BatchedController.lap_reports) under "lap_reports".
+    the reports (BatchedController.lap_reports) under "lap_reports", and with lane_margin_sets every controller's final margin under
+    "lane_margins".
     param_sets: None, or (params, index, QterminalSlack) handed to BatchedController.set_param_sets after construction (a
     parameter sweep over the batch; the result then holds per-set lap statistics under "per_set_rank0").
     vehicle_sets: None, or (vehicles, index) handed to BatchedController.set_vehicles (a sweep over the plant, PID lap included; the
@@ -234,7 +235,14 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     "per_lane_rule_rank0", with lap reports the share of laps judged lane-unsafe per lap ("lane_unsafe_share" of every
     lap_reports_rank0 row and of every per-rule report row), and "lane_unsafe_selected_share_rank0": the share of controllers whose
     final selection holds a lane-unsafe lap.  capture records every controller's rule and start refuses others.  ValueError before
-    any device work where set_lane_rules would refuse."""
+    any device work where set_lane_rules would refuse.
+    lane_margin_sets: None, or (margins, index) handed to BatchedController.set_lane_margins after the other tables, before the PID
+    lap: objects with mode (0: none, 1: the fixed margin0, 2: adapted lap by lap within [margin0, margin_max] by step_up /
+    step_down) that narrow the lane every QP plans in while reports and lane rules judge the given lane.  The result then holds
+    per-row lap statistics (with lap reports, the per-lap lane-violation share) and mean interior-point iterations under
+    "per_lane_margin_rank0", and per row the min / mean / max of the final margins under "lane_margin_final_rank0".  capture
+    records every controller's row and start refuses others.  ValueError before any device work where set_lane_margins would
+    refuse."""
     L = check_lap_reports(lap_reports, laps)
     scheds = check_lap_schedules(lap_schedules, batch, L, {"vehicle": vehicle_sets, "noise": noise_sets,
                                                            "measurement": measurement_sets})
@@ -260,8 +268,20 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     if lane_rule_sets is not None:
         rows, ridx = _native.make_lane_rule_sets(lane_rule_sets[0], lane_rule_sets[1], int(batch), True, TCL)
         lanes = np.array([[rows[k].mode, rows[k].lane_tol] for k in ridx], np.float64)
+    margins = None                                                 # [batch, 5] (mode, margin0, margin_max, step_up, step_down), or None
+    if lane_margin_sets is not None:
+        base = rp.lmpc_params(N)[5]
+        bx_min = np.full(int(batch), float(np.min(np.asarray(base.bx, float).ravel()[:2])))
+        if param_sets is not None:
+            pidx = np.asarray(param_sets[1]).reshape(-1)
+            if pidx.size == int(batch) and np.issubdtype(pidx.dtype, np.integer) and pidx.min() >= 0 and pidx.max() < len(param_sets[0]):
+                bx_min = np.array([float(np.min(np.asarray(p.bx, float).ravel()[:2])) for p in param_sets[0]])[pidx]
+        rows, midx = _native.make_lane_margin_sets(lane_margin_sets[0], lane_margin_sets[1], int(batch), bx_min)
+        margins = np.array([[rows[k].mode, rows[k].margin0, rows[k].margin_max, rows[k].step_up, rows[k].step_down]
+                            for k in midx], np.float64)
     if start is not None:
-        _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget, shape_sets, L, scheds, windows, lanes)
+        _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget, shape_sets, L, scheds, windows, lanes,
+                     margins)
     if capture is not None and not isinstance(capture, dict):
         raise ValueError("capture is a dict that receives the run's end state")
     if readiness not in ("batch", "group"):
@@ -300,7 +320,7 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
               (regression_sets, c.set_regression, "per_regression_rank0"), (track_sets, c.set_tracks, "per_track_rank0"),
               (pool_groups, c.set_pool_groups, None), (shape_sets, c.set_shapes, "per_shape_rank0"),
               (ss_laps_sets, c.set_ss_laps, "per_ss_laps_rank0"), (lap_window_sets, c.set_lap_windows, "per_lap_window_rank0"),
-              (lane_rule_sets, c.set_lane_rules, "per_lane_rule_rank0"))
+              (lane_rule_sets, c.set_lane_rules, "per_lane_rule_rank0"), (lane_margin_sets, c.set_lane_margins, "per_lane_margin_rank0"))
     for args, install, _ in tables:
         if args is not None:
             install(*args)
@@ -395,7 +415,8 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
                        lap_budget=None if budget is None else budget.tolist(),
                        lap_schedules={kind: row_of_lap.tolist() for kind, row_of_lap in scheds.items()},
                        lap_windows=None if windows is None else windows.tolist(),
-                       lane_rules=None if lanes is None else lanes.tolist())
+                       lane_rules=None if lanes is None else lanes.tolist(),
+                       lane_margins=None if margins is None else margins.tolist())
     flags_or, unsolved = c.rollout_health()
     reps = c.lap_reports() if L else None
     lens, n_laps = (reps["steps"], reps["n"]) if L else (bk["lap_hist"], bk["lap_n"])
@@ -464,6 +485,19 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         nit = np.array([c.ss_laps_of(b) for b in range(B)])
         held = np.array([unsafe[b, bk["sel"][b, :nit[b]]].any() for b in range(B)])
         out["lane_unsafe_selected_share_rank0"] = float(held.mean())
+    if lane_margin_sets is not None:
+        idx = np.asarray(lane_margin_sets[1]).reshape(B)
+        m_end = c.lane_margin_values()
+        out["lane_margin_final_rank0"] = []
+        for k, s in enumerate(out["per_lane_margin_rank0"]):
+            r = lane_margin_sets[0][k]
+            s.update(mode=int(r.mode), margin0=float(r.margin0), margin_max=float(r.margin_max), step_up=float(r.step_up),
+                     step_down=float(r.step_down),
+                     ipm_iters_mean_sampled=float(it_ctrl[idx == k].mean() / max(it_n, 1)) if (idx == k).any() else 0.0)
+            m = m_end[idx == k]
+            out["lane_margin_final_rank0"].append({"row": k, "n": int(m.size), "min": float(m.min()) if m.size else 0.0,
+                                                   "mean": float(m.mean()) if m.size else 0.0,
+                                                   "max": float(m.max()) if m.size else 0.0})
     if pool_groups is not None:
         # a stored lap advances `it`: 4 seeded copies + every own lap handed over + every imported lap filed.  Exact unless an
         # own lap found the safe-set pool full (health flag 64): then that controller's count is one too low per such lap.
@@ -490,7 +524,8 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         final.update(c.rollout_state())
         final.update(c.step_results())
     if books is not None:
-        books.update(bk, flags_or=flags_or, unsolved=unsolved, **({"lap_reports": reps} if L else {}))
+        books.update(bk, flags_or=flags_or, unsolved=unsolved, **({"lap_reports": reps} if L else {}),
+                     **({"lane_margins": m_end} if lane_margin_sets is not None else {}))
     c.close()
     return out
 
@@ -503,7 +538,7 @@ def _driven_steps(bk, state):
 
 
 def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget=None, shape_sets=None, lap_reports=0,
-                 lap_schedules=None, lap_windows=None, lane_rules=None):
+                 lap_schedules=None, lap_windows=None, lane_rules=None, lane_margins=None):
     """The refusals of run(start=...), before any device work: a start that does not match this run (report capacity, lap
     schedules and lap windows included), laps not above the captured laps, or a lap budget below the captured one."""
     if not isinstance(start, dict):
@@ -538,6 +573,7 @@ def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, b
                          "schedules it was captured with" % (sorted(had) or "none", sorted(mine) or "none"))
     check_start_windows(start.get("lap_windows"), lap_windows)
     check_start_lane_rules(start.get("lane_rules"), lane_rules)
+    check_start_lane_margins(start.get("lane_margins"), lane_margins)
     for k, v in layout(warm, shape_sets).items():
         if int(start["layout"].get(k, -1)) != v:
             raise ValueError("start records have %s = %s, this run's controllers %d" % (k, start["layout"].get(k), v))
@@ -557,6 +593,14 @@ def check_start_lane_rules(had, mine):
     if (had is None) != (mine is None) or (had is not None and not np.array_equal(np.asarray(had, np.float64), mine)):
         raise ValueError("start was captured with other lane rules: a record resumes exactly only under the rules it was captured "
                          "with")
+
+
+def check_start_lane_margins(had, mine):
+    """start's refusal of other lane margins: `had` the captured [batch, 5] rows (a list, or None without a table), `mine` this
+    run's (an array, or None).  A record carries the margins, not the rows that adapt them."""
+    if (had is None) != (mine is None) or (had is not None and not np.array_equal(np.asarray(had, np.float64), mine)):
+        raise ValueError("start was captured with other lane margins: a record resumes exactly only under the margin rows it was "
+                         "captured with")
 
 
 def _add_unsafe_share(rows, reps, sel, laps):

@@ -349,7 +349,7 @@ typedef struct lmpc_lane_rule_params {
  *   - Judgement (mode 1): a lap is lane-unsafe when one of its judged rows x has a non-finite entry, or when for a lane row i
  *     d_i = (sum over j = 0..5, in order, of Fx[i][j] * x[j], fp64 without fused multiply-adds) - bx[i] > lane_tol: the
  *     arithmetic of the lap reports (lmpc_rollout_enable_lap_reports) with the threshold lane_tol.  Fx, bx are the controller's
- *     own QP constants: its parameter-set row, else the handle's.  Judged rows: an own lap's rows 0 .. Trec-1 of the closed-loop
+ *     untightened lane: its parameter-set row, else the handle's (not the lmpc_set_lane_margins planning lane).  Judged rows: an own lap's rows 0 .. Trec-1 of the closed-loop
  *     record at the hand-over (the rows the controller files: under measurement noise the measured states); the seeded record
  *     once for all its copies; an import's shipped rows 0 .. min(lap time, rows, Tpad)-1, against the importer's own Fx, bx and
  *     lane_tol (the export still chooses and ships by raw lap time).
@@ -371,6 +371,43 @@ typedef struct lmpc_lane_rule_params {
  *   - Not part of a snapshot record (LMPC_SNAPSHOT_VERSION is unchanged): the keys travel in ss_time, so a record resumes exactly
  *     under the same rules. */
 int lmpc_set_lane_rules(lmpc_handle* h, const lmpc_lane_rule_params* sets, int nsets, const int* set_of_instance);
+
+/* Per-controller lane margins: the lane a controller plans in, narrowed by a margin m_b, apart from the lane it is judged against. */
+typedef struct lmpc_lane_margin_params {
+    int mode;            /* 0: no margin (the reference); 1: fixed margin0; 2: adaptive */
+    int pad;
+    double margin0;      /* mode 1: the margin; mode 2: the starting value and the floor */
+    double margin_max;   /* mode 2: the ceiling */
+    double step_up;      /* mode 2: added after a lap that left the lane */
+    double step_down;    /* mode 2: removed after a lap that kept to it (0: the margin only ratchets up) */
+} lmpc_lane_margin_params;
+/* Per-controller lane margins (constraint tightening: the learned model is off by a few centimetres, so a plan that ends at the
+ * lane's edge puts the plant over it).  Controller b reads row sets[set_of_instance[b]].  nsets == 0 (sets, set_of_instance NULL)
+ * removes the table.
+ *   - Margin m_b of every controller: 0 under mode 0, margin0 under mode 1; under mode 2 margin0 at the install and at every
+ *     seeding (lmpc_rollout_seed_from_record(_dev)), then adapted at every own-lap hand-over of lmpc_rollout_commit_laps_dev: when
+ *     the lap's recorded rows 0 .. Trec-1 (under measurement noise the measured states) leave the lane -- a row with a non-finite
+ *     entry, or d_i > 0 with d_i the arithmetic of the lap reports -- m_b = fmin(m_b + step_up, margin_max), else m_b =
+ *     fmax(m_b - step_down, margin0), each rounded once.  Imports, the PID lap and retired controllers leave m_b as it is.
+ *   - Planning lane: every QP the handle solves (lmpc_solve_*, lmpc_step_*, lmpc_rollout_step, shaped handles included) plans
+ *     controller b with bx_i - m_b for every lane row i < ncx at every stage; Fx, Fu, bu, the weights, K1 and K2 are unchanged.
+ *   - Judged lane: the lap reports (viol_steps, viol_max), the lane rules and the mode 2 verdict judge against the untightened
+ *     row: the controller's parameter-set row, else the handle's.
+ *   - Requires lmpc_store_create (else LMPC_E_STATE).  1 <= nsets <= batch, every index in [0, nsets); mode 0, 1 or 2; every
+ *     value finite and >= 0, margin0 <= margin_max; a margin must leave a lane: margin0 (mode 1) or margin_max (mode 2) below
+ *     min_i bx_i of the QP row the controller reads (lmpc_set_param_sets refuses sets that break this for an installed table).  Any
+ *     failed check returns LMPC_E_INVALID and leaves the handle as it was.  Allowed at any time; it synchronises the handle's
+ *     streams.  Installing or removing the table invalidates every warm-start record; a hand-over that changes m_b invalidates
+ *     that controller's.
+ *   - While a mode 2 row is installed, lmpc_rollout_commit_laps returns LMPC_E_STATE (the host-slot hand-over does not adapt).
+ *   - Memory: m_b (8 B) and a derived parameter row (the source row with the tightened bx, 1 776 B) per controller, with an
+ *     identity index (4 B): 14.6 MB at batch 8192.
+ *   - m_b is a snapshot section ("lane_margin", slot 39), absent without a table; lmpc_snapshot_unpack_dev refuses a record of
+ *     the other layout ("lane margin layout") and a non-finite or negative value, or under mode 2 one outside [margin0,
+ *     margin_max] ("lane margin"): the adaptation never leaves that range, so such a record was captured under another row.  The table itself is not part of a record, and the snapshot version is unchanged. */
+int lmpc_set_lane_margins(lmpc_handle* h, const lmpc_lane_margin_params* sets, int nsets, const int* set_of_instance);
+/* m[batch] = m_b of every controller (synchronises); LMPC_E_STATE without a table. */
+int lmpc_get_lane_margins(lmpc_handle* h, double* m);
 
 /* PredictiveModel.addTrajectory (PredictiveModel.py:35-46): copy one lap into a regression slot. */
 int lmpc_model_put_lap(lmpc_handle* h, int inst, int slot, int T, const double* x, const double* u);
@@ -567,7 +604,8 @@ typedef struct lmpc_lap_report {
 } lmpc_lap_report;
 /* lmpc_rollout_enable_lap_reports: keep up to max_laps (1 .. 1024) report rows per controller; 0 turns reports off and frees them.
  *   - x is the plant state the step was driven from (the row the rollout trace records), never the measured state of
- *     lmpc_rollout_set_measurement_noise.  Fx, bx are the controller's QP constants: its parameter-set row, else the handle's.
+ *     lmpc_rollout_set_measurement_noise.  Fx, bx are the controller's untightened lane: its parameter-set row, else the handle's
+ *     (never the bx - m_b its QPs plan with under lmpc_set_lane_margins).
  *     Row i is violated when d_i = (sum over j = 0..5, in order, of Fx[i][j] * x[j], fp64 without fused multiply-adds) - bx[i]
  *     is > 0; viol_max = fmax over the d_i.  A step whose x has a non-finite entry counts as violated and sets viol_max = +inf.
  *   - lmpc_rollout_step (modes 0, 1, 2) adds every field; lmpc_rollout_pid_step adds steps, flags and the violation fields only.
@@ -774,6 +812,7 @@ int lmpc_sizeof_shape_params(void);
 int lmpc_sizeof_ss_laps_params(void);
 int lmpc_sizeof_lap_window_params(void);
 int lmpc_sizeof_lane_rule_params(void);
+int lmpc_sizeof_lane_margin_params(void);
 
 #ifdef __cplusplus
 }

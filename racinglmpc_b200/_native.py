@@ -76,6 +76,13 @@ class LaneRuleParams(C.Structure):
     _fields_ = [("mode", C.c_int), ("pad", C.c_int), ("lane_tol", C.c_double)]
 
 
+class LaneMarginParams(C.Structure):
+    """lmpc_lane_margin_params: the margin a controller's QPs narrow its lane by -- mode 0 none, mode 1 margin0, mode 2 adapted
+    lap by lap within [margin0, margin_max] (step_up after a lap that left the lane, step_down after one that kept to it)."""
+    _fields_ = [("mode", C.c_int), ("pad", C.c_int), ("margin0", C.c_double), ("margin_max", C.c_double), ("step_up", C.c_double),
+                ("step_down", C.c_double)]
+
+
 LANE_UNSAFE_KEY = 1 << 24           # LMPC_LANE_UNSAFE_KEY: added to the safe-set key of a lane-unsafe lap
 REPORT_LANE_UNSAFE = 1 << 16        # LMPC_REPORT_LANE_UNSAFE: report flag of an own lap judged lane-unsafe
 
@@ -133,6 +140,8 @@ SNAPSHOT_SECTIONS_NAMES = ("ss_x", "ss_u", "ss_q", "ss_len", "model_x", "model_u
                            "used", "xLin", "uLin", "zt", "OldInput", "xPredPrev", "timeStep", "has_pred", "warm", "warm_valid",
                            "x", "xglob", "cl_x", "cl_u", "cl_len", "done", "health_flags", "health_unsolved", "abc_lti",
                            "lap_reports", "lap_report_run")
+# every section slot 0 .. 39: the slots above and the lane margins of lmpc_set_lane_margins in the last one
+SNAPSHOT_SLOT_NAMES = SNAPSHOT_SECTIONS_NAMES + ("lane_margin",)
 
 
 class SnapshotHeader(C.Structure):
@@ -222,6 +231,8 @@ def lib():
     L.lmpc_set_ss_laps.argtypes = [_vp, C.POINTER(SsLapsParams), C.c_int, _vp]
     L.lmpc_set_lap_windows.argtypes = [_vp, C.POINTER(LapWindowParams), C.c_int, _vp]
     L.lmpc_set_lane_rules.argtypes = [_vp, C.POINTER(LaneRuleParams), C.c_int, _vp]
+    L.lmpc_set_lane_margins.argtypes = [_vp, C.POINTER(LaneMarginParams), C.c_int, _vp]
+    L.lmpc_get_lane_margins.argtypes = [_vp, _vp]
     L.lmpc_rollout_sysid.argtypes = [_vp, C.c_double, _vp, _vp]
     L.lmpc_rollout_seed_from_record.argtypes = [_vp, C.c_int, C.c_int, C.c_int]
     L.lmpc_rollout_get_lap.argtypes = [_vp, C.c_int, ip, _vp, _vp]
@@ -268,6 +279,8 @@ def lib():
     assert L.lmpc_sizeof_lap_window_params() == C.sizeof(LapWindowParams), "lmpc_lap_window_params ABI mismatch"
     L.lmpc_sizeof_lane_rule_params.restype = C.c_int
     assert L.lmpc_sizeof_lane_rule_params() == C.sizeof(LaneRuleParams), "lmpc_lane_rule_params ABI mismatch"
+    L.lmpc_sizeof_lane_margin_params.restype = C.c_int
+    assert L.lmpc_sizeof_lane_margin_params() == C.sizeof(LaneMarginParams), "lmpc_lane_margin_params ABI mismatch"
     L.lmpc_sizeof_lap_report.restype = C.c_int
     assert L.lmpc_sizeof_lap_report() == C.sizeof(LapReport), "lmpc_lap_report ABI mismatch"
     assert L.lmpc_sizeof_noise_params() == C.sizeof(NoiseParams), "lmpc_noise_params ABI mismatch"
@@ -740,6 +753,51 @@ def make_lane_rule_sets(rules, index, batch, lmpc=True, Tcl=0):
     return _pack_sets(LaneRuleParams, rules, index, batch, "lane rules", row)
 
 
+def make_lane_margin_sets(margins, index, batch, bx_min):
+    """Per-controller lane margins for ``lmpc_set_lane_margins``: K objects ``margins`` with ``mode`` (0, 1 or 2), ``margin0``,
+    ``margin_max``, ``step_up`` and ``step_down`` (e.g. reference_params.LaneMarginParams) and the row of every controller
+    ``index[batch]``; ``bx_min[batch]`` is min_i bx_i of the QP row each controller reads.  Raises ValueError where the library
+    would refuse: the index rules of ``make_param_sets``, a mode that is not the integer 0, 1 or 2, a value that is not a finite
+    number >= 0, margin0 > margin_max, or a margin that does not leave a lane (``check_margins_leave_lane``).  Returns (ctypes
+    array LaneMarginParams * K, int32 index array)."""
+    def row(k, r):
+        m = r.mode
+        if isinstance(m, (bool, np.bool_)) or not isinstance(m, (int, np.integer)) or int(m) not in (0, 1, 2):
+            raise ValueError("lane margin %d: mode must be 0, 1 or 2, got %r" % (k, m))
+        vals = []
+        for f in ("margin0", "margin_max", "step_up", "step_down"):
+            v = getattr(r, f)
+            if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, float, np.integer, np.floating)):
+                raise ValueError("lane margin %d: %s must be a number, got %r" % (k, f, v))
+            if not (np.isfinite(float(v)) and float(v) >= 0.0):
+                raise ValueError("lane margin %d: %s must be finite and >= 0, got %r" % (k, f, v))
+            vals.append(float(v))
+        if vals[0] > vals[1]:
+            raise ValueError("lane margin %d: margin0 (%r) must not exceed margin_max (%r)" % (k, vals[0], vals[1]))
+        return LaneMarginParams(int(m), 0, *vals)
+    rows, idx = _pack_sets(LaneMarginParams, margins, index, batch, "lane margins", row)
+    check_margins_leave_lane(rows, idx, bx_min)
+    return rows, idx
+
+
+def margin_width(r):
+    """The widest margin a lane-margin row plans with: margin0 under mode 1, margin_max under mode 2, None under mode 0."""
+    return None if int(r.mode) == 0 else float(r.margin0 if int(r.mode) == 1 else r.margin_max)
+
+
+def check_margins_leave_lane(rows, idx, bx_min):
+    """ValueError unless every controller's margin leaves a lane: margin_width(rows[idx[b]]) < bx_min[b] (min_i bx_i of the QP row
+    controller b reads) wherever the row has a margin."""
+    bx_min = np.asarray(bx_min, np.float64).reshape(-1)
+    for k, r in enumerate(rows):
+        w = margin_width(r)
+        sel = np.nonzero(np.asarray(idx) == k)[0]
+        if w is not None and sel.size and not (w < bx_min[sel]).all():
+            b = int(sel[np.argmin(bx_min[sel])])
+            raise ValueError("lane margin %d: the margin %r of controller %d does not leave a lane (its bx reaches %r)"
+                             % (k, w, b, float(bx_min[b])))
+
+
 def make_pool_groups(index, ngroups, batch):
     """Pool groups for ``lmpc_set_pool_groups``: the group of every controller ``index[batch]`` among ``ngroups``.  ``ngroups == 0``
     goes with ``index=None`` (one pool) and returns None.  Raises ValueError where the library would refuse: the index rules of
@@ -800,7 +858,7 @@ def decode_snapshot_header(raw):
         raise ValueError("snapshot record version %d; this build reads version %d" % (h.version, SNAPSHOT_VERSION))
     out = {"magic": h.magic, "version": h.version, "bytes": h.bytes, "warm_mode": h.warm_mode}
     out.update({f: getattr(h, f) for f in SNAPSHOT_LAYOUT})
-    out["sections"] = {n: (h.sect_off[k], h.sect_bytes[k]) for k, n in enumerate(SNAPSHOT_SECTIONS_NAMES) if h.sect_bytes[k] > 0}
+    out["sections"] = {n: (h.sect_off[k], h.sect_bytes[k]) for k, n in enumerate(SNAPSHOT_SLOT_NAMES) if h.sect_bytes[k] > 0}
     nseg = int(h.track.nseg)
     out["track"] = {"nseg": nseg, "seg": np.array(h.track.seg[:3 * max(0, min(nseg, MAX_SEG))]).reshape(-1, 3),
                     "TrackLength": float(h.track.TrackLength)}
@@ -813,13 +871,17 @@ def snapshot_lap_reports(header):
 
 
 def snapshot_layout_mismatch(header, layout):
-    """The first layout field in which a decoded header differs from ``layout`` (a dict with SNAPSHOT_LAYOUT keys and "bytes", and
-    "lap_reports" = the report capacity when reports are on), as a message, or None when the record fits.  The report capacity is
-    compared before the size, which it changes."""
+    """The first layout field in which a decoded header differs from ``layout`` (a dict with SNAPSHOT_LAYOUT keys and "bytes",
+    "lap_reports" = the report capacity when reports are on and "lane_margin" = 1 under a lane-margin table), as a message, or None
+    when the record fits.  The report capacity and the lane margin are compared before the size, which they change."""
     had, mine = snapshot_lap_reports(header), int(layout.get("lap_reports", 0))
     if had != mine:
         what = lambda L: "%d report rows" % L if L else "no lap reports"
         return "snapshot layout mismatch: lap_reports: the record has %s and this controller %s" % (what(had), what(mine))
+    had, mine = int("lane_margin" in header["sections"]), int(layout.get("lane_margin", 0))
+    if had != mine:
+        what = lambda m: "a lane margin" if m else "no lane margin"
+        return "snapshot layout mismatch: lane margin layout: the record has %s and this controller %s" % (what(had), what(mine))
     for f in SNAPSHOT_LAYOUT + ("bytes",):
         if int(header[f]) != int(layout[f]):
             return "snapshot layout mismatch: %s is %d in the record and %d in this controller" % (f, header[f], layout[f])

@@ -70,6 +70,8 @@ class BatchedController:
         self._ss_laps = None                                # numSS_it of every controller (set_ss_laps), or None: the handle's
         self._windows = None                                # [B, 2] (ss_window, model_window) of set_lap_windows, or None: unbounded
         self._lane = None                                   # [(mode, lane_tol)] * B of set_lane_rules, or None: the reference's rule
+        self._margins = None                                # (rows, index) of set_lane_margins, or None: no margin
+        self._bx_min = np.full(self.B, self._row_bx_min(self._p))   # min_i bx_i of the QP row every controller reads
         # rows of the plant-side tables a lap schedule indexes (the defaults: one reference vehicle and noise, no measurement
         # table) and the installed schedules [B, L] of set_lap_schedule
         self._table_rows = {"vehicle": 1, "noise": 1, "measurement": 0}
@@ -114,8 +116,58 @@ class BatchedController:
         ``QterminalSlack[index[b]]`` (None: the handle's).  ``index`` is required with ``params``.  ``params=None`` (no index)
         returns to the parameters the handle was created with.
         Waits for work already enqueued; warm-start records start over."""
-        self._install(self._lib.lmpc_set_param_sets, "params", params, index,
-                      lambda: nat.make_param_sets(self._p, params, index, self.B, self._p.numSS_Points, self.numSS_it, QterminalSlack))
+        packed = {}
+
+        def pack():
+            rows, idx = nat.make_param_sets(self._p, params, index, self.B, self._p.numSS_Points, self.numSS_it, QterminalSlack)
+            packed["bx_min"] = np.array([self._row_bx_min(rows[k]) for k in range(len(rows))])[idx]
+            if self._margins is not None:                    # an installed margin must still leave a lane of the new rows
+                nat.check_margins_leave_lane(self._margins[0], self._margins[1], packed["bx_min"])
+            return rows, idx
+        if params is None and self._margins is not None:
+            nat.check_margins_leave_lane(self._margins[0], self._margins[1], np.full(self.B, self._row_bx_min(self._p)))
+        self._install(self._lib.lmpc_set_param_sets, "params", params, index, pack)
+        self._bx_min = packed.get("bx_min", np.full(self.B, self._row_bx_min(self._p)))
+
+    @staticmethod
+    def _row_bx_min(p):
+        """min_i bx_i of the lane rows of a Params row"""
+        return float(min(p.bx[i] for i in range(int(p.ncx))))
+
+    def set_lane_margins(self, margins, index=None):
+        """Per-controller lane margins (constraint tightening): every QP controller b solves plans inside its lane narrowed by a
+        margin m_b -- bx_i - m_b for every lane row -- while its lap reports, lane rules and adaptation judge the lane it was
+        given.  ``margins[index[b]]`` (objects with ``mode``, ``margin0``, ``margin_max``, ``step_up``, ``step_down``, e.g.
+        reference_params.LaneMarginParams): mode 0 no margin, mode 1 the fixed margin0, mode 2 a margin that starts at margin0 (at
+        this call and at every seeding) and after every own lap handed over on the device rises by step_up (a lap that left the
+        lane, capped at margin_max) or falls by step_down (one that kept to it, floored at margin0).  ``index`` is required with
+        ``margins``; ``margins=None`` (no index) removes the table.  A margin must leave a lane: margin0 (mode 1) or margin_max
+        (mode 2) below min_i bx_i of the controller's QP row.  Allowed at any time; warm-start records start over; under a mode 2
+        row the host-slot hand-over is refused.  m_b is part of a snapshot, the table is not.  ValueError before any native call
+        where the library would refuse a value.  Waits for work already enqueued."""
+        packed = {}
+
+        def pack():
+            packed["v"] = nat.make_lane_margin_sets(margins, index, self.B, self._bx_min)
+            return packed["v"]
+        self._install(self._lib.lmpc_set_lane_margins, "margins", margins, index, pack)
+        self._margins = packed.get("v")
+
+    def lane_margins_of(self, inst):
+        """(mode, margin0, margin_max, step_up, step_down) of controller ``inst`` under ``set_lane_margins``, None without a
+        table."""
+        if self._margins is None:
+            return None
+        r = self._margins[0][int(self._margins[1][int(inst)])]
+        return (int(r.mode), float(r.margin0), float(r.margin_max), float(r.step_up), float(r.step_down))
+
+    def lane_margin_values(self):
+        """m_b of every controller, float64 [B] (synchronises); ValueError without a lane-margin table."""
+        if self._margins is None:
+            raise ValueError("lane_margin_values: no lane-margin table is installed")
+        m = np.zeros(self.B, np.float64)
+        nat.check(self._lib.lmpc_get_lane_margins(self._h, nat.ptr(m)))
+        return m
 
     def set_vehicles(self, vehicles, index=None):
         """Per-controller vehicles of the device simulator (a Monte-Carlo over the plant in one batch): controller b is driven
@@ -723,6 +775,8 @@ class BatchedController:
         """main.py:113-119 for every instance whose lap just ended: lmpc.addTrajectory + predictiveModel.addTrajectory of the
         lap recorded on the device (no host copy of the lap), then the next lap starts from xF (SysModel.py:50)."""
         self._no_lane_rule("rollout_finish_laps")
+        if self._margins is not None and any(int(r.mode) == 2 for r in self._margins[0]):
+            raise ValueError("rollout_finish_laps: adaptive lane margins need the device hand-over (rollout_commit_laps_dev)")
         finished = np.nonzero(done)[0]
         if not len(finished):
             return finished
@@ -899,12 +953,13 @@ class BatchedController:
         return int(n.value)
 
     def snapshot_layout(self):
-        """The layout a record of this controller has (the keys of nat.SNAPSHOT_LAYOUT and "bytes", and "lap_reports" = the report
-        capacity when reports are on)."""
+        """The layout a record of this controller has (the keys of nat.SNAPSHOT_LAYOUT and "bytes", "lap_reports" = the report
+        capacity when reports are on, and "lane_margin" = 1 under a lane-margin table)."""
         return dict(N=self.N, M=self.M, ncx=int(self._p.ncx), ncu=int(self._p.ncu), numSS_it=max(self.numSS_it, 1),
                     trToUse=self.trToUse, ss_cap=max(self.ss_cap, 1), model_cap=self.model_cap, Tmax=self.Tmax,
                     Tcl=int(getattr(self, "Tcl", 0)), warm_start=int(self._p.warm_start), bytes=self.snapshot_bytes,
-                    **({"lap_reports": self.lap_report_cap} if getattr(self, "lap_report_cap", 0) else {}))
+                    **({"lap_reports": self.lap_report_cap} if getattr(self, "lap_report_cap", 0) else {}),
+                    **({"lane_margin": 1} if self._margins is not None else {}))
 
     def _ext_stream(self, torch):
         return torch.cuda.ExternalStream(self.stream, device=torch.device("cuda", self.device))

@@ -52,10 +52,32 @@ struct LaneRules {
     Table<FtocpConstRec> qp;
 };
 
-// Is the lap x[0 .. T) (row r at x + r * stride, its state in the first 6 entries) lane-unsafe for controller b?  False without a
-// table (LANE) or under mode 0.  A row is unsafe when an entry is not finite or d_i = Fx[i] . x - bx[i] > lane_tol for one of the
-// ncx == 2 lane rows, evaluated in order without contraction: the arithmetic of report_step (safeset.cuh), kept as a copy of its
-// own so that the closed loop's step kernel stays the code it was.  One block-wide pass; every thread of the block must call it.
+// Does the lap x[0 .. T) (row r at x + r * stride, its state in the first 6 entries) leave the lane Fx x <= bx of c by more than
+// tol?  A row does when an entry is not finite or d_i = Fx[i] . x - bx[i] > tol for one of the ncx == 2 lane rows, evaluated in
+// order without contraction: the arithmetic of report_step (safeset.cuh), kept as a copy of its own so that the closed loop's
+// step kernel stays the code it was.  One block-wide pass; every thread of the block must call it.
+__device__ __forceinline__ bool lane_leaves_block(const FtocpConst& c, const double* x, int T, int stride, double tol) {
+    bool bad = false;
+    for (int t = threadIdx.x; t < T && !bad; t += blockDim.x) {
+        const double* xr = x + (size_t)t * stride;
+        double v[6];
+        bool finite = true;
+#pragma unroll
+        for (int j = 0; j < 6; ++j) { v[j] = xr[j]; finite = finite && isfinite(v[j]); }
+        if (!finite) { bad = true; break; }
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            double s = __dmul_rn(c.Fx[i * 6], v[0]);
+#pragma unroll
+            for (int j = 1; j < 6; ++j) s = __dadd_rn(s, __dmul_rn(c.Fx[i * 6 + j], v[j]));
+            bad = bad || __dsub_rn(s, c.bx[i]) > tol;
+        }
+    }
+    return __syncthreads_or(bad) != 0;
+}
+
+// Is the lap x[0 .. T) lane-unsafe for controller b: does it leave its lane by more than its lane_tol?  False without a table
+// (LANE) or under mode 0.
 template <bool LANE>
 __device__ __forceinline__ bool lane_unsafe_block(const LaneRules& lr, int b, const double* x, int T, int stride) {
     if constexpr (!LANE) {
@@ -63,24 +85,7 @@ __device__ __forceinline__ bool lane_unsafe_block(const LaneRules& lr, int b, co
     } else {
         const LaneRuleRec r = lr.rule.of(b);
         if (r.mode != 1) return false;                           // uniform over the block: no barrier is skipped by part of it
-        const FtocpConst& c = lr.qp.of(b).c;
-        bool bad = false;
-        for (int t = threadIdx.x; t < T && !bad; t += blockDim.x) {
-            const double* xr = x + (size_t)t * stride;
-            double v[6];
-            bool finite = true;
-#pragma unroll
-            for (int j = 0; j < 6; ++j) { v[j] = xr[j]; finite = finite && isfinite(v[j]); }
-            if (!finite) { bad = true; break; }
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-                double s = __dmul_rn(c.Fx[i * 6], v[0]);
-#pragma unroll
-                for (int j = 1; j < 6; ++j) s = __dadd_rn(s, __dmul_rn(c.Fx[i * 6 + j], v[j]));
-                bad = bad || __dsub_rn(s, c.bx[i]) > r.lane_tol;
-            }
-        }
-        return __syncthreads_or(bad) != 0;
+        return lane_leaves_block(lr.qp.of(b).c, x, T, stride, r.lane_tol);
     }
 }
 // The safe-set key a lap of lap time T is filed with: T, plus LMPC_LANE_UNSAFE_KEY when it was judged lane-unsafe
@@ -88,6 +93,49 @@ __device__ __forceinline__ int lane_key(int T, bool unsafe) { return unsafe ? T 
 // The lap time of a safe-set key (the pooled export ranks and ships raw lap times)
 template <bool LANE>
 __device__ __forceinline__ int lane_lap_time(int key) { return LANE && key >= LMPC_LANE_UNSAFE_KEY ? key - LMPC_LANE_UNSAFE_KEY : key; }
+
+// The lane margins of every controller (lmpc_set_lane_margins): the table, the untightened QP rows (the controller's parameter-set
+// row, else the handle's), the derived planning rows plan[B] (the source row with bx_i - m_b) that every QP of the handle reads,
+// the margins m[B] and the warm-start validity (null without warm start).  commit_laps_books_kernel comes in two more
+// instantiations, MARGIN = a margin table is installed; without one it never reads this.
+using LaneMarginRec = lmpc_lane_margin_params;
+struct LaneMargins {
+    Table<LaneMarginRec> rule;
+    Table<FtocpConstRec> qp;
+    FtocpConstRec* plan;
+    double* m;
+    int* warm_valid;
+};
+// Row b of the planning table plans with margin m: the lane rows of its source row, moved in by m (rounded once)
+__device__ __forceinline__ void margin_plan_bx(const LaneMargins& lm, int b, double m) {
+    const FtocpConst& src = lm.qp.of(b).c;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) lm.plan[b].c.bx[i] = __dsub_rn(src.bx[i], m);
+}
+// The margin after a lap under a mode 2 row r: up by step_up after a lap that left the lane, down by step_down after one that kept
+// to it, within [margin0, margin_max]
+__device__ __forceinline__ double margin_adapt(const LaneMarginRec& r, double m, bool left) {
+    return left ? fmin(__dadd_rn(m, r.step_up), r.margin_max) : fmax(__dsub_rn(m, r.step_down), r.margin0);
+}
+
+// Every controller's planning row from its source row and its margin: m_b = 0 (mode 0), margin0 (mode 1), margin0 under mode 2
+// when reset2 (the install and the seedings), else the m_b it has (lmpc_set_param_sets, a snapshot restore).  idx[b] = b: the
+// identity index the QP kernels read the table through.  One CTA of 128 threads per controller copies the 1 776-byte row.
+__global__ void __launch_bounds__(128) lane_margin_rows_kernel(int batch, LaneMargins lm, int* idx, int reset2) {
+    const int b = blockIdx.x;
+    if (b >= batch) return;
+    const uint4* src = reinterpret_cast<const uint4*>(&lm.qp.of(b));
+    uint4* dst = reinterpret_cast<uint4*>(lm.plan + b);
+    for (int e = threadIdx.x; e < (int)(sizeof(FtocpConstRec) / 16); e += blockDim.x) dst[e] = src[e];
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        const LaneMarginRec r = lm.rule.of(b);
+        const double m = r.mode == 0 ? 0.0 : r.mode == 1 || reset2 ? r.margin0 : lm.m[b];
+        lm.m[b] = m;
+        margin_plan_bx(lm, b, m);
+        idx[b] = b;
+    }
+}
 
 // book_ss_add under a safe-set window of W >= 1 laps: after the event the window is lap numbers [it' - W, it'), it' = it + 1.  A
 // lap stays stored while it is in the window and fewer than nit NEWER laps rank ahead of it: older laps leave the window before it
@@ -299,17 +347,34 @@ __global__ void books_refresh_kernel(int batch, LapBooks k, SsLaps laps, LapWind
 // PC.py:445 (timeStep = 0).  One CTA per controller; no host involvement.  REPORTS: the running report row is filed as the lap's.
 // WIN: a lap-window table is installed.  LANE: a lane-rule table is installed; the lap's rows 0 .. Trec-1 are judged and an unsafe
 // lap is filed with its lap time + LMPC_LANE_UNSAFE_KEY as its safe-set key (its report carries LMPC_REPORT_LANE_UNSAFE).
-template <bool LAPS, bool REPORTS, bool WIN, bool LANE>
+// MARGIN: a lane-margin table is installed; under a mode 2 row the same rows adapt the margin m_b (margin_adapt, threshold 0), and
+// a margin that changed rewrites the controller's planning bx and invalidates its warm-start record.
+template <bool LAPS, bool REPORTS, bool WIN, bool LANE, bool MARGIN>
 __global__ void __launch_bounds__(256) commit_laps_books_kernel(int batch, LapPool ss, LapPool model, LapBooks k, const double* cl_x,
                                                                 const double* cl_u, int* cl_len, int Tcl, double* x_cur, int* timeStep,
                                                                 int* done, int* flags_or, Tracks trk, int lmpc, LapBudget retire,
-                                                                SsLaps laps, LapReports rep, LapWindows win, LaneRules lane) {
+                                                                SsLaps laps, LapReports rep, LapWindows win, LaneRules lane,
+                                                                LaneMargins margin) {
     const int b = blockIdx.x;
     if (b >= batch || retire.retired(b) || !done[b]) return;
     __shared__ int s_ss, s_md;
     const int Trec = cl_len[b];
     const double TrackLength = trk.of(b).TrackLength;
     const bool unsafe = lane_unsafe_block<LANE>(lane, b, cl_x + (size_t)b * Tcl * 6, Trec, 6);
+    if constexpr (MARGIN) {
+        const LaneMarginRec r = margin.rule.of(b);
+        if (r.mode == 2) {                                       // uniform over the block: no barrier is skipped by part of it
+            const bool left = lane_leaves_block(margin.qp.of(b).c, cl_x + (size_t)b * Tcl * 6, Trec, 6, 0.0);
+            if (threadIdx.x == 0) {
+                const double m0 = margin.m[b], m1 = margin_adapt(r, m0, left);
+                if (m1 != m0) {
+                    margin.m[b] = m1;
+                    margin_plan_bx(margin, b, m1);
+                    if (margin.warm_valid) margin.warm_valid[b] = 0;
+                }
+            }
+        }
+    }
     if (threadIdx.x == 0) {
         const LapWindowRec w = book_windows<WIN>(win, b);
         s_ss = lmpc ? book_ss_add<WIN>(k, b, lane_key(Trec, unsafe), false, book_laps<LAPS>(k, laps, b), w.ss_window) : -1;   // ordered by the lap time; rows beyond Tmax are not stored

@@ -147,6 +147,12 @@ struct lmpc_handle {
     HandleTable<LapWindowRec> lwin;
     // per-controller lane rules (lmpc_set_lane_rules), or none: every lap ranked by its lap time
     HandleTable<LaneRuleRec> lrule;
+    // per-controller lane margins (lmpc_set_lane_margins), or none: every controller plans in the lane it is judged against.
+    // d_margin [B] the margins m_b, d_plan [B] the planning rows every QP reads through the identity index d_plan_idx [B].
+    HandleTable<LaneMarginRec> lmar;
+    double* d_margin;
+    FtocpConstRec* d_plan;
+    int* d_plan_idx;
     LapPool ss, mdl;
     int *d_used, *d_sel, *d_isprev, *d_prevslot, *d_timeStep, *d_hasPred, *d_flags, *d_minidx, *d_xchg, *d_health, *d_dropped;
     double *d_xLin, *d_uLin, *d_ztState, *d_ztFixed, *d_OldInput, *d_xPredPrev, *d_tmpx, *d_tmpu;
@@ -193,7 +199,9 @@ struct lmpc_handle {
 
 // The handle's device buffers outside the QP buffer sets.  A buffer is [rows][B][per] elements (rows == 0: `per` elements for
 // the whole handle), B being the batch, or the number of traced controllers for the trace.
-enum BufOwner : unsigned { OWN_HANDLE = 1, OWN_STORE = 2, OWN_WARM = 4, OWN_ROLLOUT = 8, OWN_TRACE = 16, OWN_QP = 32, OWN_REPORTS = 64 };
+enum BufOwner : unsigned {
+    OWN_HANDLE = 1, OWN_STORE = 2, OWN_WARM = 4, OWN_ROLLOUT = 8, OWN_TRACE = 16, OWN_QP = 32, OWN_REPORTS = 64, OWN_MARGIN = 128
+};
 enum BufFill { FILL_NONE, FILL_ZERO, FILL_ONES };      // FILL_ONES: every int -1 (a free slot, no previous lap)
 constexpr int SN_SCRATCH = -1;
 struct DevBuf {
@@ -255,6 +263,8 @@ static std::vector<DevBuf> dev_bufs(lmpc_handle* h) {
         dbuf(h->d_xmeas, 6, R, FILL_ZERO, SN_SCRATCH, "x_meas"),     // formed from the plant state and the clock every step
         // per-lap reports (lap_reports_reset_kernel gives the running rows their start)
         dbuf(h->d_rep_rows, (size_t)h->rep_L, OWN_REPORTS, FILL_ZERO, SN_LAP_REPORTS), dbuf(h->d_rep_run, 1, OWN_REPORTS, FILL_ZERO, SN_LAP_RUN),
+        // lane margins (lmpc_set_lane_margins; lane_margin_rows_kernel fills them)
+        dbuf(h->d_margin, 1, OWN_MARGIN, FILL_ZERO, SN_LANE_MARGIN), dbuf(h->d_plan, 1, OWN_MARGIN), dbuf(h->d_plan_idx, 1, OWN_MARGIN),
         // trace of chosen controllers (per traced controller)
         dbuf(h->d_trinst, 1, X), dbuf(h->tr.steps, 1, X, FILL_ZERO), dbuf(h->tr.x, cap * 6, X), dbuf(h->tr.g, cap * 6, X),
         dbuf(h->tr.u, cap * 2, X), dbuf(h->tr.xPred, cap * np, X), dbuf(h->tr.ss, cap * 6 * Mx, X), dbuf(h->tr.lap, cap, X)};
@@ -279,7 +289,7 @@ static void free_tables(lmpc_handle* h, unsigned owners) {
     release(h->meas, OWN_HANDLE); release(h->budget, OWN_HANDLE); release(h->trk, OWN_STORE); release(h->reg, OWN_STORE); release(h->pool_grp, OWN_STORE);
     for (auto& t : h->sched) release(t, OWN_HANDLE);
     release(h->shp, OWN_STORE); release(h->shp_order, OWN_STORE); release(h->own_c, OWN_HANDLE); release(h->ssl, OWN_STORE);
-    release(h->lwin, OWN_STORE); release(h->lrule, OWN_STORE);
+    release(h->lwin, OWN_STORE); release(h->lrule, OWN_STORE); release(h->lmar, OWN_STORE);
     if (owners & OWN_STORE) h->shp_cells.clear();
 }
 
@@ -451,10 +461,13 @@ static int configure_t(cudaStream_t) {
     return LMPC_OK;
 }
 
+// The parameter table the QP kernels read: the planning rows of a lane-margin table, else the parameter sets, else none
+static const FtocpConstRec* qp_table(const lmpc_handle* h) { return h->lmar.tab ? h->d_plan : h->sets.tab; }
+
 template <int N, int M>
 static int launch_t(lmpc_handle* h, const FtocpArgs& a, cudaStream_t st) {
-    if (h->sets.tab)     // the handle has per-controller parameters: every instance reads its own row (ftocp_sets.cu)
-        CK(ftocp_sets_launch(N, M, h->sets.tab, a, st));
+    if (qp_table(h))     // per-controller parameters or margins: every instance reads its own row (ftocp_sets.cu)
+        CK(ftocp_sets_launch(N, M, qp_table(h), a, st));
     else {
         ftocp_kernel<N, M, 2, 4, false><<<a.batch, 32, sizeof(KernelSmem<N, M, 2, 4, false>), st>>>(h->c, a);
         CK(cudaGetLastError());
@@ -464,9 +477,10 @@ static int launch_t(lmpc_handle* h, const FtocpArgs& a, cudaStream_t st) {
 }
 
 // A shaped handle (lmpc_set_shapes): one launch of ftocp_shaped_kernel per run of one shape in the sorted batch, or per run of one
-// horizon for the MPC-type QP; parameters from the parameter-set table, or the handle's own row
+// horizon for the MPC-type QP; parameters from the planning rows of a lane-margin table, the parameter-set table, or the handle's
+// own row
 static int launch_shaped(lmpc_handle* h, const FtocpArgs& a, bool lmpc_mode, cudaStream_t st) {
-    const FtocpConstRec* table = h->sets.tab ? h->sets.tab : h->own_c.tab;
+    const FtocpConstRec* table = qp_table(h) ? qp_table(h) : h->own_c.tab;
     const auto& cells = h->shp_cells;
     for (size_t k = 0, j; k < cells.size(); k = j) {
         int n = 0;
@@ -503,7 +517,7 @@ static int configure(int N, int M) {
 }
 
 static void free_store(lmpc_handle* h) {
-    free_bufs(dev_bufs(h), OWN_STORE | OWN_WARM);
+    free_bufs(dev_bufs(h), OWN_STORE | OWN_WARM | OWN_MARGIN);
     free_tables(h, OWN_STORE);
     h->ngroups = 0;
     h->laps_stored = false;
@@ -538,6 +552,31 @@ static bool lane_rules_on(const lmpc_handle* h) {
 }
 // Controller b's rule is on: its safe-set keys may carry LMPC_LANE_UNSAFE_KEY
 static bool lane_rule_of(const lmpc_handle* h, int b) { return h->lrule.tab && h->lrule.rows[h->lrule.index[b]].mode == 1; }
+
+// The lane margins, their untightened source rows and the planning rows, as the kernels take them (only the MARGIN instantiations
+// and lane_margin_rows_kernel read them)
+static LaneMargins lane_margins(const lmpc_handle* h) {
+    return LaneMargins{h->lmar.view(), h->sets.tab ? h->sets.view() : h->own_c.view(), h->d_plan, h->d_margin, h->d_warm_valid};
+}
+// A lane-margin row of mode 2 is installed (rows nobody reads count too)
+static bool lane_margins_adapt(const lmpc_handle* h) {
+    for (const LaneMarginRec& r : h->lmar.rows) if (r.mode == 2) return true;
+    return false;
+}
+// The planning rows of every controller from its source row and margin (lane_margin_rows_kernel); reset2: mode 2 margins start
+// over at margin0.  Enqueued on the handle's stream; nothing without a table.
+static int lane_margin_rows(lmpc_handle* h, bool reset2) {
+    if (!h->lmar.tab) return LMPC_OK;
+    lane_margin_rows_kernel<<<h->batch, 128, 0, h->stream>>>(h->batch, lane_margins(h), h->d_plan_idx, reset2 ? 1 : 0);
+    CK(cudaGetLastError());
+    h->launches += 1;
+    return LMPC_OK;
+}
+// Does the margin of row r leave a lane of QP constants c: margin0 (mode 1) or margin_max (mode 2) below min_i bx_i
+static bool margin_leaves_lane(const LaneMarginRec& r, const FtocpConst& c) {
+    const double m = r.mode == 1 ? r.margin0 : r.mode == 2 ? r.margin_max : -1.0;
+    return r.mode == 0 || (m < c.bx[0] && m < c.bx[1]);
+}
 
 static void free_rollout(lmpc_handle* h) {
     free_bufs(dev_bufs(h), OWN_ROLLOUT | OWN_TRACE | OWN_REPORTS);
@@ -577,7 +616,7 @@ static FtocpArgs qp_args(const lmpc_handle* h, const QpIo& q, bool lm) {
     }
     a.status = q.status; a.iters = q.iters; a.resid = q.resid;
     a.late = h->d_late;
-    a.set_idx = h->sets.idx;
+    a.set_idx = h->lmar.tab ? h->d_plan_idx : h->sets.idx;
     return a;
 }
 
@@ -778,6 +817,27 @@ long long lmpc_kernel_launches(lmpc_handle* h) { return h ? h->launches : 0; }
 // uniform kernel (DESIGN.md, "Per-controller tables").
 int lmpc_set_param_sets(lmpc_handle* h, const lmpc_params* sets, int nsets, const int* set_of_instance) {
     if (!h) return fail(LMPC_E_INVALID, "null handle");
+    // under a lane-margin table every controller's margin must leave a lane of its new row: need[k] is the widest margin a
+    // controller of set k plans with (margin0 of mode 1, margin_max of mode 2), held by controller who[k]
+    std::vector<double> need;
+    std::vector<int> who;
+    if (h->lmar.tab) {
+        int rc = check_set_index(h, "lmpc_set_param_sets", sets, nsets, set_of_instance);
+        if (rc != LMPC_OK) return rc;
+        need.assign(nsets, -1.0);
+        who.assign(nsets, -1);
+        for (int b = 0; b < h->batch; ++b) {
+            const LaneMarginRec& r = h->lmar.rows[h->lmar.index[b]];
+            if (nsets == 0 && !margin_leaves_lane(r, h->c))
+                return fail(LMPC_E_INVALID, "lmpc_set_param_sets: the lane margin of controller " + std::to_string(b) +
+                                                " does not leave a lane of the handle's own bx");
+            const double m = r.mode == 1 ? r.margin0 : r.mode == 2 ? r.margin_max : -1.0;
+            if (nsets > 0 && r.mode != 0 && (who[set_of_instance[b]] < 0 || m > need[set_of_instance[b]])) {
+                need[set_of_instance[b]] = m;
+                who[set_of_instance[b]] = b;
+            }
+        }
+    }
     int rc = install_table(h, "lmpc_set_param_sets", h->sets, sets, nsets, set_of_instance, (const FtocpConstRec*)nullptr,
                            [&](int k, FtocpConstRec& row) {
         const lmpc_params& s = sets[k];
@@ -786,9 +846,14 @@ int lmpc_set_param_sets(lmpc_handle* h, const lmpc_params* sets, int nsets, cons
             return fail(LMPC_E_INVALID, "lmpc_set_param_sets: set " + std::to_string(k) +
                                             " differs from the handle in N, ncx, ncu, numSS_Points, numSS_it or warm_start");
         const int e = build_const(s, row.c);
-        return e == LMPC_OK ? e : fail(e, "lmpc_set_param_sets: set " + std::to_string(k) + ": " + g_err);
+        if (e != LMPC_OK) return fail(e, "lmpc_set_param_sets: set " + std::to_string(k) + ": " + g_err);
+        if (h->lmar.tab && who[k] >= 0 && !margin_leaves_lane(h->lmar.rows[h->lmar.index[who[k]]], row.c))
+            return fail(LMPC_E_INVALID, "lmpc_set_param_sets: set " + std::to_string(k) + ": the lane margin of controller " +
+                                            std::to_string(who[k]) + " does not leave a lane of its bx");
+        return LMPC_OK;
     });
     if (rc != LMPC_OK) return rc;
+    if ((rc = lane_margin_rows(h, false)) != LMPC_OK) return rc;     // the planning rows follow the new source rows
     // a warm-start record belongs to the QP it was taken from
     if (h->d_warm_valid) {
         CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * h->batch, h->stream));
@@ -984,6 +1049,7 @@ int lmpc_sizeof_shape_params(void) { return (int)sizeof(lmpc_shape_params); }
 int lmpc_sizeof_ss_laps_params(void) { return (int)sizeof(lmpc_ss_laps_params); }
 int lmpc_sizeof_lap_window_params(void) { return (int)sizeof(lmpc_lap_window_params); }
 int lmpc_sizeof_lane_rule_params(void) { return (int)sizeof(lmpc_lane_rule_params); }
+int lmpc_sizeof_lane_margin_params(void) { return (int)sizeof(lmpc_lane_margin_params); }
 int lmpc_sizeof_track_params(void) { return (int)sizeof(lmpc_track_params); }
 
 static int store_create_impl(lmpc_handle* h, const lmpc_model_params* mp, int ss_cap, int model_cap, int Tmax);
@@ -1303,6 +1369,56 @@ int lmpc_set_lane_rules(lmpc_handle* h, const lmpc_lane_rule_params* sets, int n
         row.pad = 0;
         return LMPC_OK;
     });
+}
+
+// Per-controller lane margins: every set checked, every controller's margin against the QP row it reads, then the margin buffers
+// (allocated with the first table), the table and the planning rows (DESIGN.md, "Lane margins"); nsets == 0 removes them.
+int lmpc_set_lane_margins(lmpc_handle* h, const lmpc_lane_margin_params* sets, int nsets, const int* set_of_instance) {
+    static const char* who = "lmpc_set_lane_margins";
+    int rc = need_store(h);
+    if (rc) return rc;
+    if ((rc = check_set_index(h, who, sets, nsets, set_of_instance)) != LMPC_OK) return rc;
+    for (int b = 0; b < (nsets ? h->batch : 0); ++b) {
+        const int k = set_of_instance[b];
+        const FtocpConst& c = h->sets.tab ? h->sets.rows[h->sets.index[b]].c : h->c;
+        const lmpc_lane_margin_params& r = sets[k];
+        if ((r.mode == 1 || r.mode == 2) && isfinite(r.margin0) && isfinite(r.margin_max) && !margin_leaves_lane(r, c))
+            return fail(LMPC_E_INVALID, std::string(who) + ": set " + std::to_string(k) + ": the margin of controller " +
+                                            std::to_string(b) + " does not leave a lane (" + (r.mode == 1 ? "margin0" : "margin_max") +
+                                            " must be below min_i bx_i of its QP row)");
+    }
+    const bool fresh = nsets > 0 && !h->d_margin;
+    if (fresh && (rc = alloc_bufs(h, dev_bufs(h), OWN_MARGIN, h->batch, who)) != LMPC_OK) return rc;
+    rc = install_table(h, who, h->lmar, sets, nsets, set_of_instance, (const LaneMarginRec*)nullptr, [&](int k, LaneMarginRec& row) {
+        const lmpc_lane_margin_params& s = sets[k];
+        const std::string w = std::string(who) + ": set " + std::to_string(k) + ": ";
+        if (s.mode < 0 || s.mode > 2) return fail(LMPC_E_INVALID, w + "mode must be 0, 1 or 2");
+        for (double v : {s.margin0, s.margin_max, s.step_up, s.step_down})
+            if (!isfinite(v) || v < 0.0) return fail(LMPC_E_INVALID, w + "margin0, margin_max, step_up and step_down must be finite and >= 0");
+        if (s.margin0 > s.margin_max) return fail(LMPC_E_INVALID, w + "margin0 must not exceed margin_max");
+        row = s;
+        row.pad = 0;
+        return LMPC_OK;
+    });
+    if (rc != LMPC_OK) {
+        if (fresh) free_bufs(dev_bufs(h), OWN_MARGIN);
+        return rc;
+    }
+    if (nsets == 0) free_bufs(dev_bufs(h), OWN_MARGIN);     // swap_table left the streams idle
+    if ((rc = lane_margin_rows(h, true)) != LMPC_OK) return rc;
+    // a warm-start record belongs to the QP it was taken from
+    if (h->d_warm_valid) CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * h->batch, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return LMPC_OK;
+}
+
+int lmpc_get_lane_margins(lmpc_handle* h, double* m) {
+    if (int rc = need_store(h)) return rc;
+    if (!h->lmar.tab) return fail(LMPC_E_STATE, "lmpc_get_lane_margins: no lane-margin table is installed");
+    if (!m) return fail(LMPC_E_INVALID, "null output");
+    CK(cudaMemcpyAsync(m, h->d_margin, sizeof(double) * h->batch, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    return LMPC_OK;
 }
 
 static int put_lap(lmpc_handle* h, LapPool& pool, int inst, int slot, int T, const double* x, const double* u) {
@@ -1962,7 +2078,7 @@ int lmpc_rollout_seed_from_record(lmpc_handle* h, int copies, int ss_slot0, int 
         h->d_ztState, h->d_OldInput, h->d_timeStep, h->d_hasPred, h->d_done, tracks(h), h->shp.view(), reports(h));
     CK(cudaGetLastError());
     h->launches += 1;
-    return LMPC_OK;
+    return lane_margin_rows(h, true);       // adaptive margins start over with the seeded stores
 }
 
 int lmpc_rollout_get_lap(lmpc_handle* h, int inst, int* T, double* x, double* u) {
@@ -1983,6 +2099,7 @@ int lmpc_rollout_get_lap(lmpc_handle* h, int inst, int* T, double* x, double* u)
 int lmpc_rollout_commit_laps(lmpc_handle* h, const int* fin, const int* ss_slots, const int* model_slots) {
     if (int rc = need_rollout(h)) return rc;
     if (lane_rules_on(h)) return fail(LMPC_E_STATE, "lmpc_rollout_commit_laps: lane rules need the device books (_dev)");
+    if (lane_margins_adapt(h)) return fail(LMPC_E_STATE, "lmpc_rollout_commit_laps: adaptive lane margins need the device hand-over (_dev)");
     if (!fin || !ss_slots || !model_slots) return fail(LMPC_E_INVALID, "null argument");
     for (int b = 0; b < h->batch; ++b)
         if (fin[b] && (ss_slots[b] >= h->ss.cap || model_slots[b] >= h->mdl.cap)) return fail(LMPC_E_INVALID, "slot out of range");
@@ -2100,6 +2217,11 @@ int lmpc_probe_fp64(int device, double* out8) {
 #define BOOK_KERNEL3(K, a, r, w, l)                                                                              \
     ((a) ? ((r) ? BOOK_FLAGS(K, w, l, true, true) : BOOK_FLAGS(K, w, l, true, false))                            \
          : ((r) ? BOOK_FLAGS(K, w, l, false, true) : BOOK_FLAGS(K, w, l, false, false)))
+// commit_laps_books_kernel: the flags of BOOK_KERNEL3 and a lane-margin table (MARGIN, its last flag)
+#define BOOK_FLAGS3(K, w, l, m, ...) ((w) ? BOOK_FLAGS(K, l, m, __VA_ARGS__, true) : BOOK_FLAGS(K, l, m, __VA_ARGS__, false))
+#define BOOK_COMMIT(a, r, w, l, m)                                                                                            \
+    ((a) ? ((r) ? BOOK_FLAGS3(commit_laps_books_kernel, w, l, m, true, true) : BOOK_FLAGS3(commit_laps_books_kernel, w, l, m, true, false)) \
+         : ((r) ? BOOK_FLAGS3(commit_laps_books_kernel, w, l, m, false, true) : BOOK_FLAGS3(commit_laps_books_kernel, w, l, m, false, false)))
 int lmpc_books_set(lmpc_handle* h, const int* ss_time, const int* ss_lap, const int* it, const int* md_time, const int* md_seq,
                    const int* md_cnt) {
     int rc = need_store(h);
@@ -2140,9 +2262,9 @@ int lmpc_books_get(lmpc_handle* h, int* ss_time, int* ss_lap, int* it, int* md_t
 int lmpc_rollout_commit_laps_dev(lmpc_handle* h) {
     if (int rc = need_rollout(h)) return rc;
     h->laps_stored = true;     // enqueue only: which controllers finish a lap is not known here
-    BOOK_KERNEL3(commit_laps_books_kernel, h->ssl.tab, h->rep_L, h->lwin.tab, h->lrule.tab)<<<h->batch, 256, 0, h->stream>>>(
+    BOOK_COMMIT(h->ssl.tab, h->rep_L, h->lwin.tab, h->lrule.tab, h->lmar.tab)<<<h->batch, 256, 0, h->stream>>>(
         h->batch, h->ss, h->mdl, h->bk, h->d_clx, h->d_clu, h->d_cllen, h->Tcl, h->d_rx[h->cur], h->d_timeStep, h->d_done, h->d_health,
-        tracks(h), h->M > 0 ? 1 : 0, lap_budget(h), h->ssl.view(), reports(h), h->lwin.view(), lane_rules(h));
+        tracks(h), h->M > 0 ? 1 : 0, lap_budget(h), h->ssl.view(), reports(h), h->lwin.view(), lane_rules(h), lane_margins(h));
     CK(cudaGetLastError());
     h->launches += 1;
     return LMPC_OK;
@@ -2159,7 +2281,7 @@ int lmpc_rollout_seed_from_record_dev(lmpc_handle* h, int copies) {
         h->lwin.view(), lane_rules(h));
     CK(cudaGetLastError());
     h->launches += 1;
-    return LMPC_OK;
+    return lane_margin_rows(h, true);       // adaptive margins start over with the seeded books
 }
 
 int lmpc_rollout_stats(lmpc_handle* h, int* out4) {
@@ -2266,7 +2388,7 @@ static const char* snap_field_name(int f) {
         "magic", "version", "record bytes", "N", "numSS_Points", "ncx", "ncu", "numSS_it", "trToUse", "ss_cap", "model_cap", "Tmax",
         "Tcl", "warm_start", "warm_mode", "nsect", "section table", "track row", "safe-set lap length", "model lap length", "it",
         "safe-set lap number", "md_cnt", "model arrival number", "lap_n", "sel", "is_prev", "prev_slot", "used", "timeStep",
-        "has_pred", "warm_valid", "cl_len", "done", "lap report layout", "lap report count", "lane key"};
+        "has_pred", "warm_valid", "cl_len", "done", "lap report layout", "lap report count", "lane key", "lane margin layout", "lane margin"};
     return f >= 0 && f < SF_NFIELD ? names[f] : "?";
 }
 
@@ -2418,6 +2540,7 @@ int lmpc_snapshot_unpack_dev(lmpc_handle* h, const void* rec_dev, int nrec, int 
     a.ss_cap = h->ss.cap; a.md_cap = h->mdl.cap; a.numSS_it = h->bk.numSS_it; a.trToUse = h->bk.trToUse; a.Tmax = h->ss.Tmax;
     a.Tcl = hd.Tcl; a.warm_mode = hd.warm_mode;
     a.lane = h->lrule.view();
+    a.margin = h->lmar.view();
     snapshot_check_kernel<<<(n + 127) / 128, 128, 0, h->stream>>>(a, n, d_idx, d_idx + n, (const char*)rec_dev, hd.bytes, verdict);
     h->launches += 1;
     int got[3];
@@ -2433,7 +2556,7 @@ int lmpc_snapshot_unpack_dev(lmpc_handle* h, const void* rec_dev, int nrec, int 
     if (got[0] != INT32_MAX) {
         const int i = got[0] / 64, f = got[0] % 64;
         why = "record " + std::to_string(idx[n + i]) + " (into controller " + std::to_string(idx[i]) + "): " + snap_field_name(f) +
-              (f <= SF_SECTIONS || f == SF_LAP_REPORTS ? " differs from this handle's" : f == SF_TRACK ? " differs from the controller's track"
+              (f <= SF_SECTIONS || f == SF_LAP_REPORTS || f == SF_LANE_MARGIN_LAYOUT ? " differs from this handle's" : f == SF_TRACK ? " differs from the controller's track"
                : f == SF_LANE_KEY ? " marks a lane-unsafe lap of a controller whose lane rule is off" : " out of range");
     } else if (h->d_warm && got[1] <= got[2]) {
         if (h->warm_mode < 0 && got[1] != got[2]) why = "the records hold warm-start records of two problem types";
@@ -2448,7 +2571,7 @@ int lmpc_snapshot_unpack_dev(lmpc_handle* h, const void* rec_dev, int nrec, int 
     h->launches += 1;
     h->laps_stored = true;
     if (h->d_warm) h->warm_mode = mode;
-    return LMPC_OK;
+    return lane_margin_rows(h, false);      // the restored margins plan from here on
 }
 
 int lmpc_rollout_get_clock(lmpc_handle* h, unsigned long long* step) {

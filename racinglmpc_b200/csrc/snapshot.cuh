@@ -20,6 +20,7 @@ enum SnapSection {
     SN_WARM, SN_WARM_VALID,
     SN_RX, SN_RG, SN_CLX, SN_CLU, SN_CLLEN, SN_DONE, SN_HEALTH_FLAGS, SN_HEALTH_UNSOLVED, SN_ABC_LTI,
     SN_LAP_REPORTS, SN_LAP_RUN,          // lmpc_rollout_enable_lap_reports: absent (0 bytes) without reports
+    SN_LANE_MARGIN,                      // lmpc_set_lane_margins: absent (0 bytes) without a table
     SN_COUNT,
     // pack-only entries of the copy table: the header (up to the track row) and the controller's track row
     SN_HEADER = SN_COUNT, SN_TRACK, SN_TABLE
@@ -78,7 +79,7 @@ __global__ void __launch_bounds__(256) snapshot_copy_kernel(const __grid_constan
 enum SnapField {
     SF_WARM_MODE = 14, SF_SECTIONS = 16, SF_TRACK, SF_SS_LEN, SF_MD_LEN, SF_IT, SF_SS_LAP, SF_MD_CNT, SF_MD_SEQ, SF_LAP_N, SF_SEL,
     SF_ISPREV, SF_PREVSLOT, SF_USED, SF_TIMESTEP, SF_HASPRED, SF_WARM_VALID, SF_CLLEN, SF_DONE, SF_LAP_REPORTS, SF_LAP_REPORT_N,
-    SF_LANE_KEY, SF_NFIELD
+    SF_LANE_KEY, SF_LANE_MARGIN_LAYOUT, SF_LANE_MARGIN, SF_NFIELD
 };
 constexpr int SNAP_HDR_WORDS = 16 + 2 * LMPC_SNAPSHOT_SECTIONS;   // int words of the header before the track row
 
@@ -88,6 +89,7 @@ struct SnapCheckArgs {
     Tracks trk;
     int ss_cap, md_cap, numSS_it, trToUse, Tmax, Tcl, warm_mode;
     Table<LaneRuleRec> lane;   // lane rules (lmpc_set_lane_rules): only a controller whose rule is on may hold a lane-unsafe key
+    Table<LaneMarginRec> margin;   // lane margins (lmpc_set_lane_margins): a margin is finite, >= 0 and, under mode 2, in [margin0, margin_max]
 };
 
 __device__ __forceinline__ const int* snap_ints(const char* R, const SnapCheckArgs& a, int sect) {
@@ -110,6 +112,10 @@ __global__ void __launch_bounds__(128) snapshot_check_kernel(const SnapCheckArgs
     // a record with or without reports, or with another report capacity, differs in its size too: name the reports instead
     for (int s = SN_LAP_REPORTS; f >= 2 && f != SF_NFIELD && s <= SN_LAP_RUN; ++s)
         if (H[16 + LMPC_SNAPSHOT_SECTIONS + s] != a.hdr[16 + LMPC_SNAPSHOT_SECTIONS + s]) f = SF_LAP_REPORTS;
+    // so does a record with or without a lane margin
+    if (f >= 2 && f != SF_NFIELD && f != SF_LAP_REPORTS &&
+        H[16 + LMPC_SNAPSHOT_SECTIONS + SN_LANE_MARGIN] != a.hdr[16 + LMPC_SNAPSHOT_SECTIONS + SN_LANE_MARGIN])
+        f = SF_LANE_MARGIN_LAYOUT;
     if (f == SF_NFIELD) {      // the layout is this handle's: the sections lie where this handle puts them
         // the circuit, bit for bit: nseg, its nseg rows and TrackLength (padding and unused rows are not part of it)
         const TrackRec& tr = *reinterpret_cast<const TrackRec*>(R + SNAP_HDR_WORDS * 4);
@@ -162,6 +168,11 @@ __global__ void __launch_bounds__(128) snapshot_check_kernel(const SnapCheckArgs
             BAD(dn != 0 && dn != 1, SF_DONE);
         }
         if (a.rec_off[SN_LAP_RUN] > 0) BAD(reinterpret_cast<const LapRun*>(R + a.rec_off[SN_LAP_RUN])->n < 0, SF_LAP_REPORT_N);
+        if (a.rec_off[SN_LANE_MARGIN] > 0) {
+            const double m = *reinterpret_cast<const double*>(R + a.rec_off[SN_LANE_MARGIN]);
+            const LaneMarginRec& r = a.margin.of(inst[i]);
+            BAD(!(isfinite(m) && m >= 0.0) || (r.mode == 2 && (m < r.margin0 || m > r.margin_max)), SF_LANE_MARGIN);
+        }
     }
 #undef BAD
     if (f != SF_NFIELD) atomicMin(&out[0], i * 64 + f);

@@ -157,6 +157,24 @@ class LaneRuleParams:
         return cls(0, 0.0)
 
 
+@dataclass(frozen=True)
+class LaneMarginParams:
+    """The margin a controller's QPs narrow its lane by, while its reports and lane rules judge the lane it was given: mode 0
+    none (the reference), mode 1 the fixed margin0, mode 2 a margin adapted after every own lap within [margin0, margin_max] --
+    up by step_up after a lap that left the lane, down by step_down after one that kept to it.  The device takes one per
+    controller (BatchedController.set_lane_margins)."""
+    mode: int = 0
+    margin0: float = 0.0
+    margin_max: float = 0.0
+    step_up: float = 0.0
+    step_down: float = 0.0
+
+    @classmethod
+    def reference(cls):
+        """No margin: installed, the controllers plan in the lane they are judged against."""
+        return cls(0, 0.0, 0.0, 0.0, 0.0)
+
+
 def _wrap(a):
     if a < -np.pi:
         return 2 * np.pi + a

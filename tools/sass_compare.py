@@ -10,7 +10,7 @@ across their untemplated names:
            books_refresh_kernel, commit_laps_books_kernel, seed_books_kernel, pool_import_kernel (<false>: no lap-count table;
            <false, false>: no lap-count table and no lap-window table; <false, false, false>: no lap-count table, no lap-window
            table and no lane-rule table; <false, false, false, false>: no lap-count table, no lap reports, no lap-window table and
-           no lane-rule table), pool_local_best_kernel, pool_export_kernel (<false>: no lane-rule table), commit_laps_kernel,
+           no lane-rule table; <false, false, false, false, false>: the same and no lane-margin table), pool_local_best_kernel, pool_export_kernel (<false>: no lane-rule table), commit_laps_kernel,
            seed_from_record_kernel
            (<false>: no lap reports), sim_step_kernel (<false> or <false, false>: no lap reports and no lap schedule) and measure_kernel (<false>:
            no lap schedule)
@@ -33,7 +33,7 @@ NAME = re.compile(r"^(?:void )?(ftocp_kernel|ftocp_sets_kernel)<(\d+), (\d+), 2,
 DEFAULT = re.compile(r"^(?:void )?lmpc::(knn_ltv_regress_kernel|ss_select_kernel|shift_state_kernel|books_refresh_kernel|"
                      r"commit_laps_books_kernel|seed_books_kernel|pool_import_kernel|sim_step_kernel|commit_laps_kernel|"
                      r"seed_from_record_kernel|measure_kernel|pool_local_best_kernel|pool_export_kernel)"
-                     r"(<false>|<false, false>|<false, false, false>|<false, false, false, false>)?\(")
+                     r"(<false>|<false, false>|<false, false, false>|<false, false, false, false>|<false, false, false, false, false>)?\(")
 REPORTS = re.compile(r"^(?:void )?lmpc::(sim_step_kernel)<true(?:, false)?>\(")
 
 
