@@ -23,6 +23,7 @@ exchanges once its own slowest controller is `ship_after` steps into lap r+1 (th
 Prints one JSON line (rank 0): closed-loop steps/s over all GPUs (device events, max over ranks), lap-length statistics per
 LMPC lap, exchange time and bytes."""
 import argparse
+import ctypes as C
 import json
 import os
 import sys
@@ -133,7 +134,7 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         final=None, param_sets=None, vehicle_sets=None, books=None, track_sets=None, pool_groups=None, readiness="batch",
         capture=None, start=None, noise_sets=None, noise_streams=None, regression_sets=None, lap_budget=None, measurement_sets=None,
         shape_sets=None, ss_laps_sets=None, lap_reports=None, lap_schedules=None, lap_window_sets=None,
-        lane_rule_sets=None, lane_margin_sets=None):
+        lane_rule_sets=None, lane_margin_sets=None, prediction_model_sets=None, trace=None):
     """One Monte-Carlo run on this rank's GPU (torch.distributed may or may not be initialised).  Returns a dict (all ranks).
     final: None, or a dict that receives the closed loop's end state (rollout_state) and the last step's solver report (step_results).
     books: None, or a dict that receives the lap books (books) and the health counters (flags_or, unsolved), and with lap_reports
@@ -242,7 +243,16 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     per-row lap statistics (with lap reports, the per-lap lane-violation share) and mean interior-point iterations under
     "per_lane_margin_rank0", and per row the min / mean / max of the final margins under "lane_margin_final_rank0".  capture
     records every controller's row and start refuses others.  ValueError before any device work where set_lane_margins would
-    refuse."""
+    refuse.
+    prediction_model_sets: None, or (models, index) handed to BatchedController.set_prediction_models with the other tables, before
+    the PID lap: objects with mode (0: the learned k-NN model, 1: the exact linearisation of their vehicle, 2: that of the plant's
+    own vehicle row, through its lap schedule) and vehicle.  Needs lap_reports >= laps.  The result then holds, per row, its lap
+    statistics with the per-lap reports (controllers, mean steps, the share with a lane violation, unsolved QPs) under
+    "per_prediction_model_rank0".  capture records every controller's row and start refuses others.  ValueError before any device
+    work where set_prediction_models would refuse.
+    trace: None, or a dict with "inst" (controller numbers) and "cap" (rows per controller): those controllers' LMPC steps are
+    traced (lmpc_rollout_trace_create, after the seeding) and the dict receives per traced controller "steps" and the arrays "x"
+    [cap, 6] (the plant state the step started from), "xPred" [cap, N+1, 6] and "lap" [cap]."""
     L = check_lap_reports(lap_reports, laps)
     scheds = check_lap_schedules(lap_schedules, batch, L, {"vehicle": vehicle_sets, "noise": noise_sets,
                                                            "measurement": measurement_sets})
@@ -279,9 +289,10 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         rows, midx = _native.make_lane_margin_sets(lane_margin_sets[0], lane_margin_sets[1], int(batch), bx_min)
         margins = np.array([[rows[k].mode, rows[k].margin0, rows[k].margin_max, rows[k].step_up, rows[k].step_down]
                             for k in midx], np.float64)
+    models = check_prediction_models(prediction_model_sets, batch, L)
     if start is not None:
         _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget, shape_sets, L, scheds, windows, lanes,
-                     margins)
+                     margins, models)
     if capture is not None and not isinstance(capture, dict):
         raise ValueError("capture is a dict that receives the run's end state")
     if readiness not in ("batch", "group"):
@@ -320,7 +331,8 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
               (regression_sets, c.set_regression, "per_regression_rank0"), (track_sets, c.set_tracks, "per_track_rank0"),
               (pool_groups, c.set_pool_groups, None), (shape_sets, c.set_shapes, "per_shape_rank0"),
               (ss_laps_sets, c.set_ss_laps, "per_ss_laps_rank0"), (lap_window_sets, c.set_lap_windows, "per_lap_window_rank0"),
-              (lane_rule_sets, c.set_lane_rules, "per_lane_rule_rank0"), (lane_margin_sets, c.set_lane_margins, "per_lane_margin_rank0"))
+              (lane_rule_sets, c.set_lane_rules, "per_lane_rule_rank0"), (lane_margin_sets, c.set_lane_margins, "per_lane_margin_rank0"),
+              (prediction_model_sets, c.set_prediction_models, "per_prediction_model_rank0"))
     for args, install, _ in tables:
         if args is not None:
             install(*args)
@@ -352,6 +364,9 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         c.set_lap_budget(budget)
         driven0 = _driven_steps(c.books(), c.rollout_state())
         retired_at_last = [False] * G
+    if trace is not None:
+        tr_inst = np.ascontiguousarray(np.asarray(trace["inst"]).reshape(-1), np.int32)
+        _native.check(_native.lib().lmpc_rollout_trace_create(c._h, len(tr_inst), _native.ptr(tr_inst), int(trace["cap"])))
     kbest = share + 1
     rows = torch.zeros(G * kbest, tpad, 9, dtype=torch.float64, device=dev)
     meta = torch.zeros(G * kbest, 4, dtype=torch.int32, device=dev)
@@ -416,7 +431,17 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
                        lap_schedules={kind: row_of_lap.tolist() for kind, row_of_lap in scheds.items()},
                        lap_windows=None if windows is None else windows.tolist(),
                        lane_rules=None if lanes is None else lanes.tolist(),
-                       lane_margins=None if margins is None else margins.tolist())
+                       lane_margins=None if margins is None else margins.tolist(),
+                       prediction_models=None if models is None else models.tolist())
+    if trace is not None:
+        cap = int(trace["cap"])
+        trace.update(steps=[], x=[], xPred=[], lap=[])
+        for t in range(len(tr_inst)):
+            n, x, xp, lp = C.c_int(0), np.zeros((cap, 6)), np.zeros((cap, N + 1, 6)), np.zeros(cap, np.int32)
+            _native.check(_native.lib().lmpc_rollout_trace_get(c._h, t, C.byref(n), _native.ptr(x), None, None, _native.ptr(xp), None,
+                                                               _native.ptr(lp)))
+            for k, v in (("steps", n.value), ("x", x), ("xPred", xp), ("lap", lp)):
+                trace[k].append(v)
     flags_or, unsolved = c.rollout_health()
     reps = c.lap_reports() if L else None
     lens, n_laps = (reps["steps"], reps["n"]) if L else (bk["lap_hist"], bk["lap_n"])
@@ -498,6 +523,9 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
             out["lane_margin_final_rank0"].append({"row": k, "n": int(m.size), "min": float(m.min()) if m.size else 0.0,
                                                    "mean": float(m.mean()) if m.size else 0.0,
                                                    "max": float(m.max()) if m.size else 0.0})
+    if prediction_model_sets is not None:
+        for k, s in enumerate(out["per_prediction_model_rank0"]):
+            s.update(mode=int(prediction_model_sets[0][k].mode))
     if pool_groups is not None:
         # a stored lap advances `it`: 4 seeded copies + every own lap handed over + every imported lap filed.  Exact unless an
         # own lap found the safe-set pool full (health flag 64): then that controller's count is one too low per such lap.
@@ -538,7 +566,7 @@ def _driven_steps(bk, state):
 
 
 def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget=None, shape_sets=None, lap_reports=0,
-                 lap_schedules=None, lap_windows=None, lane_rules=None, lane_margins=None):
+                 lap_schedules=None, lap_windows=None, lane_rules=None, lane_margins=None, prediction_models=None):
     """The refusals of run(start=...), before any device work: a start that does not match this run (report capacity, lap
     schedules and lap windows included), laps not above the captured laps, or a lap budget below the captured one."""
     if not isinstance(start, dict):
@@ -574,6 +602,7 @@ def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, b
     check_start_windows(start.get("lap_windows"), lap_windows)
     check_start_lane_rules(start.get("lane_rules"), lane_rules)
     check_start_lane_margins(start.get("lane_margins"), lane_margins)
+    check_start_prediction_models(start.get("prediction_models"), prediction_models)
     for k, v in layout(warm, shape_sets).items():
         if int(start["layout"].get(k, -1)) != v:
             raise ValueError("start records have %s = %s, this run's controllers %d" % (k, start["layout"].get(k), v))
@@ -600,6 +629,26 @@ def check_start_lane_margins(had, mine):
     run's (an array, or None).  A record carries the margins, not the rows that adapt them."""
     if (had is None) != (mine is None) or (had is not None and not np.array_equal(np.asarray(had, np.float64), mine)):
         raise ValueError("start was captured with other lane margins: a record resumes exactly only under the margin rows it was "
+                         "captured with")
+
+
+def check_prediction_models(prediction_model_sets, batch, lap_reports):
+    """The refusals of run(prediction_model_sets=...), before any device work: the checks of set_prediction_models, and lap
+    reports (the per-row summary is taken from them).  Returns every controller's row as [batch, 11] (mode, the ten vehicle
+    values), or None without a table."""
+    if prediction_model_sets is None:
+        return None
+    if not lap_reports:
+        raise ValueError("prediction_model_sets needs lap_reports >= laps: the per-row summary is taken from the lap reports")
+    rows, idx = _native.make_prediction_model_sets(prediction_model_sets[0], prediction_model_sets[1], int(batch))
+    return np.array([[rows[k].mode] + [getattr(rows[k].vehicle, f) for f in _native.VEHICLE_FIELDS] for k in idx], np.float64)
+
+
+def check_start_prediction_models(had, mine):
+    """start's refusal of other prediction models: `had` the captured [batch, 11] rows (a list, or None without a table), `mine`
+    this run's (an array, or None).  The table is not part of a record."""
+    if (had is None) != (mine is None) or (had is not None and not np.array_equal(np.asarray(had, np.float64), mine)):
+        raise ValueError("start was captured with other prediction models: a record resumes exactly only under the model rows it was "
                          "captured with")
 
 

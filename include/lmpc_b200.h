@@ -458,7 +458,8 @@ int lmpc_step_host(lmpc_handle* h, int mode, const double* x0, double* xPred, do
 /* Same with x0 already on the device; results stay in the handle's device buffers (lmpc_device_buffer). */
 int lmpc_step_dev(lmpc_handle* h, int mode, const double* x0_dev);
 /* lmpc_step_dev with CUDA events between its kernels: ms4 = milliseconds of K1 (k-NN regression), K2 (safe-set selection, 0 for
- * mode 0), the QP kernel and the state shift.  Measurement support for per-kernel rooflines; synchronises. */
+ * mode 0), the QP kernel and the state shift.  Measurement support for per-kernel rooflines; synchronises.  With a prediction-model
+ * table installed (lmpc_set_prediction_models), ms4[0] covers K1 and the nominal-model kernel together. */
 int lmpc_step_profile(lmpc_handle* h, int mode, const double* x0_dev, float* ms4);
 /* QP status / iterations / residuals [B,3] / step flags of the most recent lmpc_step_dev or lmpc_rollout_step (any NULL). */
 int lmpc_step_results(lmpc_handle* h, int* status, int* iters, double* resid, int* flags);
@@ -520,6 +521,41 @@ typedef struct lmpc_vehicle_params {
  *     another car drove is not a feasible trajectory of this one, so a clean plant sweep puts each car in its own group
  *     (lmpc_set_pool_groups). */
 int lmpc_rollout_set_vehicles(lmpc_handle* h, const lmpc_vehicle_params* sets, int nsets, const int* set_of_instance);
+
+/* Per-controller prediction model: where rows 0..2 (vx, vy, wz) of a controller's LTV model come from. */
+#define LMPC_FLAG_NOMINAL_NONFINITE 1024     /* step flag: an entry of a nominal controller's rows 0..2 is not finite */
+typedef struct lmpc_prediction_model_params {
+    int mode;                     /* 0 learned (the reference's k-NN regression), 1 nominal: `vehicle`, 2 nominal: the plant's own vehicle row */
+    int pad;
+    lmpc_vehicle_params vehicle;  /* the car a mode 1 controller believes it drives; not read under modes 0 and 2 */
+} lmpc_prediction_model_params;
+/* Per-controller prediction models (what the learned model costs or buys, against a controller that plans with the exact
+ * linearisation of a car).  Controller b reads row sets[set_of_instance[b]].  nsets == 0 (sets, set_of_instance NULL) removes
+ * the table.  Honoured wherever the k-NN regression runs: lmpc_identify_host, lmpc_step_host / _dev / _profile (modes 0, 1) and
+ * lmpc_rollout_step (modes 0, 1).
+ *   - Mode 0 is the k-NN regression, unchanged.
+ *   - Modes 1 and 2: stage i < N_b is identified at (xbar, ubar) = (xLin[i], uLin[i]).  Phi is the noise-free map of the velocity
+ *     subsystem (vx, vy, wz, delta, a) -> (vx, vy, wz) over one control period, the simulator's loop exactly (h = 0.001 s while
+ *     (i + 1) h <= dt, the reference's lf in alpha_r).  Rows 0..2 of A are dPhi/d(vx, vy, wz) with columns 3..5 zero; rows 0..2
+ *     of B are dPhi/d(delta, a), both columns filled; C_r = Phi_r(xbar, ubar) - (sum_j A_rj xbar_j + sum_k B_rk ubar_k), summed
+ *     left to right.  Rows 3..5 are the reference's closed-form kinematic rows, bit for bit what the regression writes for the
+ *     same xLin.  The sensitivities are propagated through the sub-steps (forward mode, fp64).
+ *   - Vehicle: mode 1 uses the row's own; mode 2 the row the simulator uses for b: in lmpc_rollout_step its vehicle-table row
+ *     through the vehicle lap schedule when one is installed (lap_n as the step starts), in the host-driven entry points its
+ *     vehicle-table row (set_of_instance of lmpc_rollout_set_vehicles).
+ *   - Flags: a nominal controller never sets 1, 4 or 32; it sets 2 as the regression does, and LMPC_FLAG_NOMINAL_NONFINITE when
+ *     an entry of its rows 0..2 is not finite (the rollout health word ORs it in like the other step flags).
+ *   - Rollout mode 2 (LTI), the model pool, the lap books and the pooled exchange do not look at the table: a nominal controller
+ *     keeps filing laps, and a return to mode 0 regresses on them.  Retired controllers identify nothing; shaped handles
+ *     identify stages < N_b.
+ *   - Requires lmpc_store_create (else LMPC_E_STATE).  1 <= nsets <= batch, every index in [0, nsets); mode 0, 1 or 2; all ten
+ *     vehicle values finite in every row, and m, lf, lr, Iz > 0 in a mode 1 row.  Any failed check returns LMPC_E_INVALID and
+ *     leaves the handle as it was.  Allowed at any time; it synchronises the handle's streams and applies from the next
+ *     identification; warm-start records stay.
+ *   - Not part of a snapshot record (LMPC_SNAPSHOT_VERSION is unchanged).
+ *   - While a table is installed, lmpc_step_profile's ms4[0] covers the regression and the nominal-model kernel together. */
+int lmpc_set_prediction_models(lmpc_handle* h, const lmpc_prediction_model_params* sets, int nsets, const int* set_of_instance);
+
 /* Noise model of the device closed loop: the clipped Gaussian noise of Simulator.dynModel and of the PID path follower. */
 typedef struct lmpc_noise_params {
     double sim_sigma[3];          /* vx, vy, wz: 0.01, 0.01, 0.005      SysModel.py:139-141 */
@@ -813,6 +849,7 @@ int lmpc_sizeof_ss_laps_params(void);
 int lmpc_sizeof_lap_window_params(void);
 int lmpc_sizeof_lane_rule_params(void);
 int lmpc_sizeof_lane_margin_params(void);
+int lmpc_sizeof_prediction_model_params(void);
 
 #ifdef __cplusplus
 }

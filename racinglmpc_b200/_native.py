@@ -83,6 +83,13 @@ class LaneMarginParams(C.Structure):
                 ("step_down", C.c_double)]
 
 
+class PredictionModelParams(C.Structure):
+    """lmpc_prediction_model_params: where rows 0..2 of a controller's LTV model come from -- mode 0 the k-NN regression (the
+    reference), mode 1 the exact linearisation of ``vehicle``, mode 2 that of the plant's own vehicle row."""
+    _fields_ = [("mode", C.c_int), ("pad", C.c_int), ("vehicle", VehicleParams)]
+
+
+FLAG_NOMINAL_NONFINITE = 1024       # LMPC_FLAG_NOMINAL_NONFINITE: step flag of a nominal controller whose rows 0..2 are not finite
 LANE_UNSAFE_KEY = 1 << 24           # LMPC_LANE_UNSAFE_KEY: added to the safe-set key of a lane-unsafe lap
 REPORT_LANE_UNSAFE = 1 << 16        # LMPC_REPORT_LANE_UNSAFE: report flag of an own lap judged lane-unsafe
 
@@ -233,6 +240,7 @@ def lib():
     L.lmpc_set_lane_rules.argtypes = [_vp, C.POINTER(LaneRuleParams), C.c_int, _vp]
     L.lmpc_set_lane_margins.argtypes = [_vp, C.POINTER(LaneMarginParams), C.c_int, _vp]
     L.lmpc_get_lane_margins.argtypes = [_vp, _vp]
+    L.lmpc_set_prediction_models.argtypes = [_vp, C.POINTER(PredictionModelParams), C.c_int, _vp]
     L.lmpc_rollout_sysid.argtypes = [_vp, C.c_double, _vp, _vp]
     L.lmpc_rollout_seed_from_record.argtypes = [_vp, C.c_int, C.c_int, C.c_int]
     L.lmpc_rollout_get_lap.argtypes = [_vp, C.c_int, ip, _vp, _vp]
@@ -281,6 +289,8 @@ def lib():
     assert L.lmpc_sizeof_lane_rule_params() == C.sizeof(LaneRuleParams), "lmpc_lane_rule_params ABI mismatch"
     L.lmpc_sizeof_lane_margin_params.restype = C.c_int
     assert L.lmpc_sizeof_lane_margin_params() == C.sizeof(LaneMarginParams), "lmpc_lane_margin_params ABI mismatch"
+    L.lmpc_sizeof_prediction_model_params.restype = C.c_int
+    assert L.lmpc_sizeof_prediction_model_params() == C.sizeof(PredictionModelParams), "lmpc_prediction_model_params ABI mismatch"
     L.lmpc_sizeof_lap_report.restype = C.c_int
     assert L.lmpc_sizeof_lap_report() == C.sizeof(LapReport), "lmpc_lap_report ABI mismatch"
     assert L.lmpc_sizeof_noise_params() == C.sizeof(NoiseParams), "lmpc_noise_params ABI mismatch"
@@ -778,6 +788,28 @@ def make_lane_margin_sets(margins, index, batch, bx_min):
     rows, idx = _pack_sets(LaneMarginParams, margins, index, batch, "lane margins", row)
     check_margins_leave_lane(rows, idx, bx_min)
     return rows, idx
+
+
+def make_prediction_model_sets(models, index, batch):
+    """Per-controller prediction models for ``lmpc_set_prediction_models``: K objects ``models`` with ``mode`` (0, 1 or 2) and
+    ``vehicle`` (an object with the reference's ten vehicle field names; e.g. reference_params.PredictionModelParams) and the row
+    of every controller ``index[batch]``.  Raises ValueError where the library would refuse: the index rules of
+    ``make_param_sets``, a mode that is not the integer 0, 1 or 2, a vehicle value that is not finite, or a mode 1 vehicle with
+    m, lf, lr or Iz not positive.  Returns (ctypes array PredictionModelParams * K, int32 index array)."""
+    def row(k, r):
+        m = r.mode
+        if isinstance(m, (bool, np.bool_)) or not isinstance(m, (int, np.integer)) or int(m) not in (0, 1, 2):
+            raise ValueError("prediction model %d: mode must be 0, 1 or 2, got %r" % (k, m))
+        vals = []
+        for f in VEHICLE_FIELDS:
+            v = getattr(r.vehicle, f)
+            if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, float, np.integer, np.floating)) or not np.isfinite(float(v)):
+                raise ValueError("prediction model %d: vehicle %s must be a finite number, got %r" % (k, f, v))
+            vals.append(float(v))
+        if int(m) == 1 and min(vals[0], vals[1], vals[2], vals[3]) <= 0:
+            raise ValueError("prediction model %d: a mode 1 vehicle needs m, lf, lr and Iz > 0" % k)
+        return PredictionModelParams(int(m), 0, VehicleParams(*vals))
+    return _pack_sets(PredictionModelParams, models, index, batch, "prediction models", row)
 
 
 def margin_width(r):

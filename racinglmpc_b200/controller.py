@@ -9,6 +9,7 @@ and "usedIt", exactly as the reference's Python lists do.
 import ctypes as C
 import numpy as np
 from . import _native as nat
+from . import reference_params
 
 
 class _LapBook:
@@ -71,6 +72,7 @@ class BatchedController:
         self._windows = None                                # [B, 2] (ss_window, model_window) of set_lap_windows, or None: unbounded
         self._lane = None                                   # [(mode, lane_tol)] * B of set_lane_rules, or None: the reference's rule
         self._margins = None                                # (rows, index) of set_lane_margins, or None: no margin
+        self._models = None                                 # (rows, index) of set_prediction_models, or None: all learned
         self._bx_min = np.full(self.B, self._row_bx_min(self._p))   # min_i bx_i of the QP row every controller reads
         # rows of the plant-side tables a lap schedule indexes (the defaults: one reference vehicle and noise, no measurement
         # table) and the installed schedules [B, L] of set_lap_schedule
@@ -168,6 +170,31 @@ class BatchedController:
         m = np.zeros(self.B, np.float64)
         nat.check(self._lib.lmpc_get_lane_margins(self._h, nat.ptr(m)))
         return m
+
+    def set_prediction_models(self, models, index=None):
+        """Per-controller prediction models: where rows 0..2 (vx, vy, wz) of controller b's LTV model come from in every later
+        ``identify``, ``step`` (modes 0, 1) and ``rollout_step`` (modes 0, 1).  ``models[index[b]]`` (objects with ``mode`` and
+        ``vehicle``, e.g. reference_params.PredictionModelParams): mode 0 the k-NN regression (the reference), mode 1 the exact
+        linearisation of the simulator's one-period map for ``vehicle``, mode 2 that of the plant's own vehicle row (through
+        the vehicle lap schedule in ``rollout_step``).  Rows 3..5 stay the closed-form kinematic rows.  A nominal controller keeps
+        filing laps, and never sets step flags 1, 4 or 32; it sets FLAG_NOMINAL_NONFINITE when its rows 0..2 are not finite.
+        ``index`` is required with ``models``; ``models=None`` (no index) removes the table.  Allowed at any time; not part of a
+        snapshot.  ValueError before any native call where the library would refuse a value.  Waits for work already enqueued."""
+        packed = {}
+
+        def pack():
+            packed["v"] = nat.make_prediction_model_sets(models, index, self.B)
+            return packed["v"]
+        self._install(self._lib.lmpc_set_prediction_models, "models", models, index, pack)
+        self._models = packed.get("v")
+
+    def prediction_models_of(self, inst):
+        """(mode, vehicle as a reference_params.VehicleParams) of controller ``inst`` under ``set_prediction_models``, None
+        without a table."""
+        if self._models is None:
+            return None
+        r = self._models[0][int(self._models[1][int(inst)])]
+        return (int(r.mode), reference_params.VehicleParams(*[float(getattr(r.vehicle, f)) for f in nat.VEHICLE_FIELDS]))
 
     def set_vehicles(self, vehicles, index=None):
         """Per-controller vehicles of the device simulator (a Monte-Carlo over the plant in one batch): controller b is driven

@@ -32,6 +32,7 @@
 #include "ftocp_pdip.cuh"
 #include "safeset.cuh"
 #include "lapbooks.cuh"
+#include "nominal_model.cuh"
 #include "probe.cuh"
 #include "ftocp_launch.cuh"
 #include "snapshot.cuh"
@@ -134,6 +135,8 @@ struct lmpc_handle {
     // regression constants (lmpc_set_regression_sets); without sets the constants of lmpc_store_create (store_reg)
     RegressionRec store_reg;
     HandleTable<RegressionRec> reg;
+    // per-controller prediction models (lmpc_set_prediction_models), or none: every controller regresses (K1)
+    HandleTable<PredictionModelRec> pmod;
     // per-controller shapes (lmpc_set_shapes), or none; shp_order's index is the batch sorted by (N, M), shp_cells the runs of
     // one shape in it (only shapes with controllers), own_c the one-row parameter table of a shaped handle without parameter sets
     HandleTable<ShapeRec> shp;
@@ -289,7 +292,7 @@ static void free_tables(lmpc_handle* h, unsigned owners) {
     release(h->meas, OWN_HANDLE); release(h->budget, OWN_HANDLE); release(h->trk, OWN_STORE); release(h->reg, OWN_STORE); release(h->pool_grp, OWN_STORE);
     for (auto& t : h->sched) release(t, OWN_HANDLE);
     release(h->shp, OWN_STORE); release(h->shp_order, OWN_STORE); release(h->own_c, OWN_HANDLE); release(h->ssl, OWN_STORE);
-    release(h->lwin, OWN_STORE); release(h->lrule, OWN_STORE); release(h->lmar, OWN_STORE);
+    release(h->lwin, OWN_STORE); release(h->lrule, OWN_STORE); release(h->lmar, OWN_STORE); release(h->pmod, OWN_STORE);
     if (owners & OWN_STORE) h->shp_cells.clear();
 }
 
@@ -1050,6 +1053,7 @@ int lmpc_sizeof_ss_laps_params(void) { return (int)sizeof(lmpc_ss_laps_params); 
 int lmpc_sizeof_lap_window_params(void) { return (int)sizeof(lmpc_lap_window_params); }
 int lmpc_sizeof_lane_rule_params(void) { return (int)sizeof(lmpc_lane_rule_params); }
 int lmpc_sizeof_lane_margin_params(void) { return (int)sizeof(lmpc_lane_margin_params); }
+int lmpc_sizeof_prediction_model_params(void) { return (int)sizeof(lmpc_prediction_model_params); }
 int lmpc_sizeof_track_params(void) { return (int)sizeof(lmpc_track_params); }
 
 static int store_create_impl(lmpc_handle* h, const lmpc_model_params* mp, int ss_cap, int model_cap, int Tmax);
@@ -1073,7 +1077,8 @@ static int store_create_impl(lmpc_handle* h, const lmpc_model_params* mp, int ss
     }
     CK(cudaSetDevice(h->device));
     // the largest launch: trToUse = K1_MAXLAPS at K1_MAXWPB warps (103360 B, above a flat 100 KiB)
-    for (auto k1 : {knn_ltv_regress_kernel<false>, knn_ltv_regress_kernel<true>}) {
+    for (auto k1 : {knn_ltv_regress_kernel<false, false>, knn_ltv_regress_kernel<true, false>, knn_ltv_regress_kernel<false, true>,
+                    knn_ltv_regress_kernel<true, true>}) {
         CK(cudaFuncSetAttribute(k1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)k1_smem_bytes(K1_MAXLAPS, K1_MAXWPB)));
         CK(cudaFuncSetAttribute(k1, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     }
@@ -1219,6 +1224,29 @@ int lmpc_set_regression_sets(lmpc_handle* h, const lmpc_regression_params* sets,
                 return fail(LMPC_E_INVALID, w + "every |scaling| must be 0 or in [2^-32, 2^32]");
             r.scaling[i] = a;
         }
+        return LMPC_OK;
+    });
+}
+
+// Per-controller prediction models: mode 0, 1 or 2, all ten vehicle values finite, and m, lf, lr, Iz positive in a mode 1 row;
+// nsets == 0 removes the table.
+int lmpc_set_prediction_models(lmpc_handle* h, const lmpc_prediction_model_params* sets, int nsets, const int* set_of_instance) {
+    static const char* who = "lmpc_set_prediction_models";
+    int rc = need_store(h);
+    if (rc) return rc;
+    return install_table(h, who, h->pmod, sets, nsets, set_of_instance, (const PredictionModelRec*)nullptr, [&](int k, PredictionModelRec& r) {
+        const lmpc_prediction_model_params& s = sets[k];
+        const lmpc_vehicle_params& v = s.vehicle;
+        const std::string w = std::string(who) + ": row " + std::to_string(k) + ": ";
+        if (s.mode < 0 || s.mode > 2) return fail(LMPC_E_INVALID, w + "mode must be 0, 1 or 2");
+        const double all[10] = {v.m, v.lf, v.lr, v.Iz, v.Df, v.Cf, v.Bf, v.Dr, v.Cr, v.Br};
+        for (double x : all)
+            if (!isfinite(x)) return fail(LMPC_E_INVALID, w + "all ten vehicle values must be finite");
+        if (s.mode == 1 && !(v.m > 0 && v.lf > 0 && v.lr > 0 && v.Iz > 0))
+            return fail(LMPC_E_INVALID, w + "a mode 1 vehicle needs m, lf, lr, Iz > 0");
+        memset(&r, 0, sizeof(r));
+        r.mode = s.mode;
+        r.vehicle = v;
         return LMPC_OK;
     });
 }
@@ -1550,7 +1578,9 @@ int lmpc_state_get(lmpc_handle* h, double* xLin, double* uLin, double* zt, doubl
     return LMPC_OK;
 }
 
-static int launch_k1(lmpc_handle* h, LapBudget retire = {}) {
+// K1 for the whole batch, and with a prediction-model table the nominal model after it (nominal_model.cuh).  vsched: the vehicle lap
+// schedule a mode 2 controller follows (lmpc_rollout_step), or none: its vehicle-table row.
+static int launch_k1(lmpc_handle* h, LapBudget retire = {}, LapSchedule vsched = {}) {
     K1Args a;
     a.batch = h->batch; a.N = h->N;
     a.wpb = h->N < K1_MAXWPB ? h->N : K1_MAXWPB;
@@ -1560,9 +1590,23 @@ static int launch_k1(lmpc_handle* h, LapBudget retire = {}) {
     a.reg = h->reg.view();
     a.retire = retire;
     a.shp = h->shp.view();
+    a.pm = h->pmod.view();
     dim3 grid(h->batch, (h->N + a.wpb - 1) / a.wpb);
     const size_t smem = k1_smem_bytes(h->mc.trToUse, a.wpb);
-    (h->shp.tab ? knn_ltv_regress_kernel<true> : knn_ltv_regress_kernel<false>)<<<grid, 32 * a.wpb, smem, h->stream>>>(h->mc, a);
+    if (!h->pmod.tab) {
+        (h->shp.tab ? knn_ltv_regress_kernel<true, false> : knn_ltv_regress_kernel<false, false>)<<<grid, 32 * a.wpb, smem, h->stream>>>(h->mc, a);
+    } else {
+        (h->shp.tab ? knn_ltv_regress_kernel<true, true> : knn_ltv_regress_kernel<false, true>)<<<grid, 32 * a.wpb, smem, h->stream>>>(h->mc, a);
+    }
+    CK(cudaGetLastError());
+    h->launches += 1;
+    if (!h->pmod.tab) return LMPC_OK;
+    NominalArgs na;
+    na.batch = h->batch; na.N = h->N; na.dt = h->mc.dt; na.xLin = h->d_xLin; na.uLin = h->d_uLin;
+    na.pm = h->pmod.view(); na.veh = h->veh.view(); na.veh_s = vsched; na.trk = tracks(h); na.retire = retire; na.shp = h->shp.view();
+    na.abc = h->hb[0].abc; na.status = h->d_flags;
+    const long long nthr = (long long)h->batch * h->N;
+    nominal_model_kernel<<<(unsigned)((nthr + 127) / 128), 128, 0, h->stream>>>(na);
     CK(cudaGetLastError());
     h->launches += 1;
     return LMPC_OK;
@@ -1622,8 +1666,10 @@ int lmpc_select_host(lmpc_handle* h, const double* x0, double* SS_sel, double* Q
 }  // extern "C"
 
 // One device-resident step for the whole batch on the handle's stream: K1 -> K2 -> QP -> shift (PC.py:110-137).  ev (five events
-// or null) brackets the four kernels for lmpc_step_profile.  retire: the lap budgets (the closed loop) or none.
-static int step_dev_impl(lmpc_handle* h, int mode, const double* x0_dev, cudaEvent_t* ev, LapBudget retire = {}) {
+// or null) brackets the four kernels for lmpc_step_profile.  retire: the lap budgets (the closed loop) or none; vsched: the vehicle
+// lap schedule a mode 2 prediction model follows (the closed loop) or none.
+static int step_dev_impl(lmpc_handle* h, int mode, const double* x0_dev, cudaEvent_t* ev, LapBudget retire = {},
+                         LapSchedule vsched = {}) {
     int rc = need_store(h);
     if (rc) return rc;
     if (!x0_dev || (mode != 0 && mode != 1)) return fail(LMPC_E_INVALID, "bad mode or null x0");
@@ -1637,7 +1683,7 @@ static int step_dev_impl(lmpc_handle* h, int mode, const double* x0_dev, cudaEve
     const bool lm = mode == 1;
     const QpIo& q = h->hb[0];
     if (ev) CK(cudaEventRecord(ev[0], st));
-    if ((rc = launch_k1(h, retire)) != LMPC_OK) return rc;                           // PC.py:117
+    if ((rc = launch_k1(h, retire, vsched)) != LMPC_OK) return rc;                   // PC.py:117
     if (ev) CK(cudaEventRecord(ev[1], st));
     if (lm && (rc = launch_k2(h, x0_dev, retire)) != LMPC_OK) return rc;             // PC.py:121
     if (ev) CK(cudaEventRecord(ev[2], st));
@@ -1829,7 +1875,7 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
         io.xPred = q.xPred; io.uPred = q.uPred; io.slack = q.slack; io.status = q.status; io.iters = q.iters; io.resid = q.resid;
         rc = solve_dev(h, io, 54, 0, retire);
     } else {
-        rc = step_dev_impl(h, mode, y, nullptr, retire);
+        rc = step_dev_impl(h, mode, y, nullptr, retire, lap_schedule(h, LMPC_SCHEDULE_VEHICLE));
     }
     if (rc) return rc;
     if (mode == 1) {                                                                 // SysModel.py:38 -> PC.py:466-476

@@ -1,0 +1,154 @@
+// racinglmpc_b200/csrc/nominal_model.cuh — the nominal prediction model of lmpc_set_prediction_models (DESIGN.md,
+// "Per-controller prediction models").
+//
+// A controller of mode 1 or 2 plans with the exact linearisation of a car instead of the k-NN regression of K1: rows 0..2 of
+// its stage model are the derivatives of the simulator's own one-period map Phi of (vx, vy, wz) (SysModel.py:94-106,
+// sim_step_kernel), rows 3..5 the closed-form kinematic rows K1 writes.  K1 skips such a controller (its NOMINAL instantiation),
+// and nominal_model_kernel, launched after it, writes all 54 entries of the controller's stages.
+#pragma once
+
+namespace lmpc {
+
+struct NominalArgs {
+    int batch, N;
+    double dt;                        // the control period (ModelConst::dt): the simulator's loop runs while (i + 1) h <= dt
+    const double* xLin;               // [B][N+1][6]
+    const double* uLin;               // [B][N][2]
+    PredictionModels pm;              // the mode (and mode 1 vehicle) of every controller
+    Table<lmpc_vehicle_params> veh;   // the simulator's vehicle table (mode 2)
+    LapSchedule veh_s;                // its lap schedule in the closed loop, else rows == nullptr: the table's own index
+    Tracks trk;                       // the curvature of the linearisation point (rows 3..5)
+    LapBudget retire;                 // a retired controller identifies nothing
+    Shapes shp;                       // stages i >= N_b are not identified
+    double* abc;                      // [B][N][54]
+    int* status;                      // [B] step flags: 2 (curvature lookup failed), LMPC_FLAG_NOMINAL_NONFINITE
+};
+
+// One thread per (controller, stage).  The state z = (vx, vy, wz) and its forward sensitivity S = dz/d(vx0, vy0, wz0, delta, a)
+// (3 x 5) stay in registers through the sub-steps: z <- z + h f(z, u), S <- S + h (f_z S + f_u E), E = [0 | I2], f_z and f_u
+// taken at the sub-step's starting state, which is the derivative of the explicit-Euler map itself.
+__global__ void __launch_bounds__(128) nominal_model_kernel(const NominalArgs a) {
+    const int t = blockIdx.x * blockDim.x + threadIdx.x;
+    const int b = t / a.N, i = t - b * a.N;
+    if (b >= a.batch || a.retire.retired(b)) return;
+    const PredictionModelRec& row = a.pm.of(b);
+    if (row.mode == 0) return;
+    if (i >= (a.shp.tab ? a.shp.of(b).N : a.N)) return;
+    const lmpc_vehicle_params& v = row.mode == 1 ? row.vehicle : a.veh_s.of(a.veh, b);
+    const double mass = v.m, lf = v.lf, lr = v.lr, Iz = v.Iz;
+    const double Df = v.Df, Cf = v.Cf, Bf = v.Bf;
+    const double Dr = v.Dr, Cr = v.Cr, Br = v.Br;
+    const double* xl = a.xLin + ((size_t)b * (a.N + 1) + i) * 6;
+    const double* ul = a.uLin + ((size_t)b * a.N + i) * 2;
+    const double delta = ul[0], acc = ul[1];
+    const double h = 0.001;
+    double vx = xl[0], vy = xl[1], wz = xl[2];
+    double S[3][5] = {{1, 0, 0, 0, 0}, {0, 1, 0, 0, 0}, {0, 0, 1, 0, 0}};
+    const double sd = sin(delta), cd = cos(delta);
+    int k = 0;
+    while ((k + 1) * h <= a.dt) {
+        // the simulator's sub-step (sim_step_kernel), with the reference's lf in alpha_r
+        const double pf = vy + lf * wz, pq = vy - lf * wz;
+        const double af = delta - atan2(pf, vx);
+        const double ar = -atan2(pq, vx);
+        const double tf = atan(Bf * af), tr = atan(Br * ar);
+        const double Fyf = Df * sin(Cf * tf);
+        const double Fyr = Dr * sin(Cr * tr);
+        // dFy/dalpha and dalpha/d(vx, vy, wz); d alpha_f / d delta = 1
+        const double gf = Df * cos(Cf * tf) * Cf * Bf / (1.0 + (Bf * af) * (Bf * af));
+        const double gr = Dr * cos(Cr * tr) * Cr * Br / (1.0 + (Br * ar) * (Br * ar));
+        const double rf = 1.0 / (vx * vx + pf * pf), rr = 1.0 / (vx * vx + pq * pq);
+        const double daf[3] = {pf * rf, -vx * rf, -lf * vx * rf};
+        const double dar[3] = {pq * rr, -vx * rr, lf * vx * rr};
+        // f_z (3 x 3) and f_u (3 x 2)
+        double Fz[3][3], Fu[3][2];
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+            Fz[0][j] = -sd / mass * gf * daf[j];
+            Fz[1][j] = (cd * gf * daf[j] + gr * dar[j]) / mass;
+            Fz[2][j] = (lf * cd * gf * daf[j] - lr * gr * dar[j]) / Iz;
+        }
+        Fz[0][1] += wz; Fz[0][2] += vy;
+        Fz[1][0] -= wz; Fz[1][2] -= vx;
+        Fu[0][0] = -(gf * sd + Fyf * cd) / mass; Fu[0][1] = 1.0;
+        Fu[1][0] = (gf * cd - Fyf * sd) / mass; Fu[1][1] = 0.0;
+        Fu[2][0] = lf * (gf * cd - Fyf * sd) / Iz; Fu[2][1] = 0.0;
+        double Sn[3][5];
+#pragma unroll
+        for (int r = 0; r < 3; ++r) {
+#pragma unroll
+            for (int c = 0; c < 5; ++c) {
+                double d = Fz[r][0] * S[0][c] + Fz[r][1] * S[1][c] + Fz[r][2] * S[2][c];
+                if (c >= 3) d += Fu[r][c - 3];
+                Sn[r][c] = S[r][c] + h * d;
+            }
+        }
+#pragma unroll
+        for (int r = 0; r < 3; ++r)
+#pragma unroll
+            for (int c = 0; c < 5; ++c) S[r][c] = Sn[r][c];
+        const double nvx = vx + h * (acc - 1 / mass * Fyf * sd + wz * vy);
+        const double nvy = vy + h * (1 / mass * (Fyf * cd + Fyr) - wz * vx);
+        const double nwz = wz + h * (1 / Iz * (lf * Fyf * cd - lr * Fyr));
+        vx = nvx; vy = nvy; wz = nwz;
+        ++k;
+    }
+    double* out = a.abc + ((size_t)b * a.N + i) * 54;
+    const double phi[3] = {vx, vy, wz};
+    int flags = 0;
+    bool finite = true;
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+        // C_r = Phi_r - (sum_j A_rj xbar_j + sum_k B_rk ubar_k), left to right, columns 3..5 of A included (they are 0)
+        double s = __dmul_rn(S[r][0], xl[0]);
+        s = __dadd_rn(s, __dmul_rn(S[r][1], xl[1]));
+        s = __dadd_rn(s, __dmul_rn(S[r][2], xl[2]));
+        s = __dadd_rn(s, __dmul_rn(0.0, xl[3]));
+        s = __dadd_rn(s, __dmul_rn(0.0, xl[4]));
+        s = __dadd_rn(s, __dmul_rn(0.0, xl[5]));
+        s = __dadd_rn(s, __dmul_rn(S[r][3], delta));
+        s = __dadd_rn(s, __dmul_rn(S[r][4], acc));
+        const double c = __dsub_rn(phi[r], s);
+        out[r * 6 + 0] = S[r][0]; out[r * 6 + 1] = S[r][1]; out[r * 6 + 2] = S[r][2];
+        out[r * 6 + 3] = 0.0; out[r * 6 + 4] = 0.0; out[r * 6 + 5] = 0.0;
+        out[36 + 2 * r] = S[r][3]; out[36 + 2 * r + 1] = S[r][4];
+        out[48 + r] = c;
+#pragma unroll
+        for (int j = 0; j < 5; ++j) finite = finite && isfinite(S[r][j]);
+        finite = finite && isfinite(c);
+    }
+    if (!finite) flags |= LMPC_FLAG_NOMINAL_NONFINITE;
+    // rows 3..5: K1's closed-form block (knn_ltv_regress_kernel, "rows 3..5"), the same expressions in the same order
+    {
+        const double vx = xl[0], vy = xl[1], wz = xl[2], epsi = xl[3], sc = xl[4], ey = xl[5];
+        const double dt = a.dt;
+        int okc = 1;
+        const double cur = curvature_lookup(a.trk.of(b), sc, &okc);
+        if (!okc) flags |= 2;
+        const double den = 1.0 - cur * ey;
+        const double rden = fast_rcp(den), rden2 = rden * rden;
+        double se, ce;
+        sincos(epsi, &se, &ce);
+        const double vl = vx * ce - vy * se;          // longitudinal speed along the centre line
+        const double vt = -vx * se - vy * ce;
+        const double a30 = -dt * ce * rden * cur, a31 = dt * se * rden * cur, a33 = 1.0 - dt * vt * rden * cur;
+        const double a35 = dt * vl * rden2 * cur * (-cur);
+        const double a40 = dt * (ce * rden), a41 = -dt * (se * rden), a43 = dt * vt * rden, a45 = -dt * vl * rden2 * (-cur);
+        const double a50 = dt * se, a51 = dt * ce, a53 = dt * vl;
+        const double f3 = epsi + dt * (wz - vl * rden * cur);
+        const double f4 = sc + dt * (vl * rden);
+        const double f5 = ey + dt * (vx * se + vy * ce);
+        const double c3 = f3 - (a30 * vx + a31 * vy + dt * wz + a33 * epsi + 0.0 * sc + a35 * ey);
+        const double c4 = f4 - (a40 * vx + a41 * vy + 0.0 * wz + a43 * epsi + sc + a45 * ey);
+        const double c5 = f5 - (a50 * vx + a51 * vy + 0.0 * wz + a53 * epsi + 0.0 * sc + ey);
+        // the entries K1_ABC_SRC gives rows 3..5 of A, B and C
+        const double row3[6] = {a30, a31, dt, a33, 0.0, a35}, row4[6] = {a40, a41, 0.0, a43, 1.0, a45};
+        const double row5[6] = {a50, a51, 0.0, a53, 0.0, 1.0};
+#pragma unroll
+        for (int j = 0; j < 6; ++j) { out[18 + j] = row3[j]; out[24 + j] = row4[j]; out[30 + j] = row5[j]; out[42 + j] = 0.0; }
+        out[51] = c3; out[52] = c4; out[53] = c5;
+    }
+    if (flags) atomicOr(&a.status[b], flags);
+}
+
+}  // namespace lmpc

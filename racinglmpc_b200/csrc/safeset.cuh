@@ -56,6 +56,11 @@ __device__ __forceinline__ int ss_points_of(const Shapes& s, int b, int M) { ret
 // The safe-set lap count numSS_it_b of every controller (lmpc_set_ss_laps), or no table (tab == null) for the handle's numSS_it,
 // which stays the stride of sel / is_prev / min_index and K2's block size.  K2 takes SHAPED when either table is installed; the
 // lap-book kernels (lapbooks.cuh) have their own LAPS instantiation, so without a table both are the code they were before.
+// The prediction model of every controller (lmpc_set_prediction_models), or no table (tab == null): the k-NN regression for all.
+// K1 takes NOMINAL when a table is installed and then skips the controllers of a nominal mode (nominal_model.cuh).
+using PredictionModelRec = lmpc_prediction_model_params;
+using PredictionModels = Table<PredictionModelRec>;
+
 using SsLapsRec = lmpc_ss_laps_params;
 using SsLaps = Table<SsLapsRec>;
 __device__ __forceinline__ int ss_laps_of(const SsLaps& l, int b, int nit) { return l.tab ? l.of(b).numSS_it : nit; }
@@ -238,6 +243,7 @@ struct K1Args {
                           //        4 = a single neighbour in a lap — cases where the reference raises,
                           //        32 = more than K1_CAND rows within rounding distance of the k-th neighbour)
     Shapes shp;           // the horizon of every controller: stages i >= N_b are not identified
+    PredictionModels pm;  // NOMINAL: the prediction model of every controller; a controller of mode 1 or 2 is not regressed
 };
 // per-warp scratch: selected points [7*trToUse][15] (x0 x1 x2 delta a 1 | y0 y1 y2 | K*(x0 x1 x2 delta a 1)) | normal
 //                   equations 45 (+3 pad) | staging of the closed-form record entries (17, +3 pad)
@@ -289,11 +295,12 @@ __constant__ signed char K1_ABC_SRC[54] = {
 #ifndef LMPC_K1_MINBLOCKS
 #define LMPC_K1_MINBLOCKS 3
 #endif
-template <bool SHAPED>
+template <bool SHAPED, bool NOMINAL>
 __global__ void __launch_bounds__(32 * K1_MAXWPB, LMPC_K1_MINBLOCKS) knn_ltv_regress_kernel(const __grid_constant__ ModelConst m, const K1Args a) {
     extern __shared__ __align__(16) unsigned char k1_smem[];
     const int b = a.b0 + blockIdx.x;
     if (a.retire.retired(b)) return;          // uniform over the CTA: no barrier is skipped by part of it
+    if (NOMINAL && a.pm.of(b).mode != 0) return;   // nominal_model_kernel identifies this controller (uniform over the CTA)
     // every stage of this CTA lies past the controller's horizon (uniform over the CTA).  The shape is read where it is tested, not
     // held as a horizon: as one int across the scan it cost K1 a 12-byte spill at its 56-register cap
     if (SHAPED && (int)blockIdx.y * a.wpb >= a.shp.of(b).N) return;

@@ -175,6 +175,31 @@ class LaneMarginParams:
         return cls(0, 0.0, 0.0, 0.0, 0.0)
 
 
+@dataclass(frozen=True)
+class PredictionModelParams:
+    """Where rows 0..2 (vx, vy, wz) of a controller's LTV model come from: mode 0 the k-NN regression of its stored laps (the
+    reference), mode 1 the exact linearisation of the simulator's one-period map for ``vehicle`` (a car the controller believes
+    it drives), mode 2 the same for the plant's own vehicle row (``vehicle`` is not read).  The device takes one per controller
+    (BatchedController.set_prediction_models)."""
+    mode: int = 0
+    vehicle: VehicleParams = VehicleParams.reference()
+
+    @classmethod
+    def learned(cls):
+        """The k-NN regression: installed, the controllers identify exactly what they do without a table."""
+        return cls(0)
+
+    @classmethod
+    def plant(cls):
+        """The exact linearisation of the car the simulator drives for the controller."""
+        return cls(2)
+
+    @classmethod
+    def believes(cls, vehicle):
+        """The exact linearisation of ``vehicle``, whatever the plant drives."""
+        return cls(1, vehicle)
+
+
 def _wrap(a):
     if a < -np.pi:
         return 2 * np.pi + a
