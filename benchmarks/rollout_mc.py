@@ -134,7 +134,7 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         final=None, param_sets=None, vehicle_sets=None, books=None, track_sets=None, pool_groups=None, readiness="batch",
         capture=None, start=None, noise_sets=None, noise_streams=None, regression_sets=None, lap_budget=None, measurement_sets=None,
         shape_sets=None, ss_laps_sets=None, lap_reports=None, lap_schedules=None, lap_window_sets=None,
-        lane_rule_sets=None, lane_margin_sets=None, prediction_model_sets=None, trace=None):
+        lane_rule_sets=None, lane_margin_sets=None, prediction_model_sets=None, trace=None, surface_sets=None):
     """One Monte-Carlo run on this rank's GPU (torch.distributed may or may not be initialised).  Returns a dict (all ranks).
     final: None, or a dict that receives the closed loop's end state (rollout_state) and the last step's solver report (step_results).
     books: None, or a dict that receives the lap books (books) and the health counters (flags_or, unsolved), and with lap_reports
@@ -220,7 +220,8 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     wherever no step found the record full, flag 256).  Without reports laps is at most 16, the laps the lap books keep.  capture
     records L and start refuses another.  ValueError before any device work.
     lap_schedules: None, or {kind: rows} handed to BatchedController.set_lap_schedule after the seeding (or the restore), kind in
-    "vehicle", "noise", "measurement" and rows [L] or [batch, L] naming rows of vehicle_sets, noise_sets or measurement_sets
+    "vehicle", "noise", "measurement", "surface" and rows [L] or [batch, L] naming rows of vehicle_sets, noise_sets,
+    measurement_sets or surface_sets
     (conditions that change at the laps each controller reaches; entry 0 is the first LMPC lap).  Each kind needs its table and the
     run needs lap_reports >= laps.  The result gains "per_lap_row_rank0": per kind, lap and row, the controllers on that row, their
     mean steps, the share with a lane violation and the unsolved QPs (lap_row_summary).  capture records the schedules and start
@@ -250,12 +251,19 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     statistics with the per-lap reports (controllers, mean steps, the share with a lane violation, unsolved QPs) under
     "per_prediction_model_rank0".  capture records every controller's row and start refuses others.  ValueError before any device
     work where set_prediction_models would refuse.
+    surface_sets: None, or (surfaces, index) handed to BatchedController.set_surfaces with the other tables, before the PID lap
+    (friction zones along the circuit, PID lap included; the result then holds per-surface lap statistics under
+    "per_surface_rank0").  lap_schedules={"surface": rows} switches rows at the laps.  The pooled mode exchanges laps whatever the
+    surface, so a clean pooled surface study puts each surface in its own pool group.  ValueError before any device work where
+    set_surfaces would refuse.
     trace: None, or a dict with "inst" (controller numbers) and "cap" (rows per controller): those controllers' LMPC steps are
     traced (lmpc_rollout_trace_create, after the seeding) and the dict receives per traced controller "steps" and the arrays "x"
     [cap, 6] (the plant state the step started from), "xPred" [cap, N+1, 6] and "lap" [cap]."""
     L = check_lap_reports(lap_reports, laps)
+    if surface_sets is not None:                                   # ValueError where set_surfaces would refuse
+        _native.make_surface_sets(surface_sets[0], surface_sets[1], int(batch))
     scheds = check_lap_schedules(lap_schedules, batch, L, {"vehicle": vehicle_sets, "noise": noise_sets,
-                                                           "measurement": measurement_sets})
+                                                           "measurement": measurement_sets, "surface": surface_sets})
     budget = _native.make_lap_budget(lap_budget, int(batch))       # ValueError where set_lap_budget would refuse, before any device work
     N, M = handle_shape(shape_sets)
     numSS_it = rp.lmpc_params(N)[0]
@@ -332,7 +340,8 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
               (pool_groups, c.set_pool_groups, None), (shape_sets, c.set_shapes, "per_shape_rank0"),
               (ss_laps_sets, c.set_ss_laps, "per_ss_laps_rank0"), (lap_window_sets, c.set_lap_windows, "per_lap_window_rank0"),
               (lane_rule_sets, c.set_lane_rules, "per_lane_rule_rank0"), (lane_margin_sets, c.set_lane_margins, "per_lane_margin_rank0"),
-              (prediction_model_sets, c.set_prediction_models, "per_prediction_model_rank0"))
+              (prediction_model_sets, c.set_prediction_models, "per_prediction_model_rank0"),
+              (surface_sets, c.set_surfaces, "per_surface_rank0"))
     for args, install, _ in tables:
         if args is not None:
             install(*args)

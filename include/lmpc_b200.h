@@ -522,6 +522,40 @@ typedef struct lmpc_vehicle_params {
  *     (lmpc_set_pool_groups). */
 int lmpc_rollout_set_vehicles(lmpc_handle* h, const lmpc_vehicle_params* sets, int nsets, const int* set_of_instance);
 
+/* Track surface of the device simulator: friction zones along the circuit (a wet corner, a dusty straight). */
+#define LMPC_MAX_ZONES 16
+typedef struct lmpc_surface_params {
+    int nzone;                           /* 0 .. LMPC_MAX_ZONES; 0 = a dry row (no zone) */
+    int pad;
+    double zone[LMPC_MAX_ZONES * 4];     /* per zone: s_start, s_end, mu_f, mu_r; entries past nzone are not read */
+} lmpc_surface_params;
+/* Per-controller track surfaces (DESIGN.md, "Track surfaces"; no reference counterpart: the reference's grip is the same all
+ * round the lap).  Controller b is simulated on row sets[set_of_instance[b]] (host arrays).  nsets == 0 (sets, set_of_instance
+ * NULL) removes the table; every handle starts without one.
+ *   - Rule, per sub-step i of the simulator's loop: s_w is the sub-step's starting s -- the value its curvature lookup takes --
+ *     wrapped as that lookup wraps it (repeated subtraction of TrackLength while s > TrackLength, only when s <= 64 TrackLength).
+ *     Zone k matches when s_start_k <= s_w < s_end_k; it gives the sub-step the peak tyre forces fl(mu_f Df) and fl(mu_r Dr), the
+ *     rest of the sub-step unchanged.  Otherwise -- no zone matches, s is not finite or s is beyond 64 laps -- the sub-step uses
+ *     Df and Dr exactly, so a sub-step off every zone computes what it computes without a table.  Df and Dr are the controller's
+ *     vehicle row (under a vehicle lap schedule, the scheduled row).  Scaling D is how a friction coefficient enters the
+ *     reference's car (D = mu m g / 2): a zone is a stretch with mu_f / mu_r times the car's grip.
+ *   - Zones are not checked against TrackLength: a zone past the lap never matches, and [0, 2 TrackLength) covers the whole lap,
+ *     a wrapped s == TrackLength included.
+ *   - Read by every lmpc_rollout_step (modes 0, 1, 2; through the surface lap schedule when one is installed, LMPC_SCHEDULE_SURFACE),
+ *     by lmpc_rollout_pid_step (set_of_instance; the PID lap ignores schedules) and by the mode 2 nominal model
+ *     (lmpc_set_prediction_models).  A retired controller reads nothing.  The caller-problem solves, the host-driven steps (except
+ *     through a mode 2 nominal model), K1, K2, the lap books, lmpc_rollout_sysid, the measurement kernel, the reports and the trace
+ *     ignore it.  A mode 1 controller plans on the car it believes in without a surface; a surface it believes in is not covered.
+ *   - The pooled exchange hands laps between the controllers of a pool group whatever their surface: a clean surface study puts
+ *     each surface in its own group (lmpc_set_pool_groups).
+ *   - 1 <= nsets <= batch, every index in [0, nsets); per row 0 <= nzone <= LMPC_MAX_ZONES and, for every zone k < nzone, all
+ *     four values finite, 0 <= s_start < s_end, mu_f >= 0, mu_r >= 0, and the zones ascending without overlap
+ *     (s_end_k <= s_start_{k+1}).  While a surface lap schedule is installed, a table that does not cover its largest entry and
+ *     the removal are refused.  Any failed check returns LMPC_E_INVALID and leaves the handle as it was.
+ *   - Allowed at any time; it synchronises the handle's streams and applies from the next step.  Not part of a snapshot record
+ *     (LMPC_SNAPSHOT_VERSION is unchanged).  Without a table the kernels run the code they run without this feature. */
+int lmpc_rollout_set_surfaces(lmpc_handle* h, const lmpc_surface_params* sets, int nsets, const int* set_of_instance);
+
 /* Per-controller prediction model: where rows 0..2 (vx, vy, wz) of a controller's LTV model come from. */
 #define LMPC_FLAG_NOMINAL_NONFINITE 1024     /* step flag: an entry of a nominal controller's rows 0..2 is not finite */
 typedef struct lmpc_prediction_model_params {
@@ -664,7 +698,8 @@ int lmpc_sizeof_lap_report(void);
 /* Lap schedules (no reference counterpart; DESIGN.md, "Per-lap schedules"): a plant-side table whose row changes at the laps a
  * controller reaches -- a track that gets wet at lap 10, a car whose mass changes, a sensor that degrades.  For the table `table`
  * (vehicles of lmpc_rollout_set_vehicles, process and PID noise of lmpc_rollout_set_noise, measurement noise of
- * lmpc_rollout_set_measurement_noise), row_of_lap is a host array [batch][nlaps], 1 <= nlaps <= 1024:
+ * lmpc_rollout_set_measurement_noise, track surfaces of lmpc_rollout_set_surfaces), row_of_lap is a host array [batch][nlaps],
+ * 1 <= nlaps <= 1024:
  *   - In every lmpc_rollout_step (modes 0, 1, 2) controller b reads row row_of_lap[b][min(lap_n[b], nlaps - 1)] of the table in
  *     place of its set_of_instance[b], in the measurement kernel and in the simulator.  lap_n is the count of laps handed over since
  *     the seeding (lmpc_books_get), read as the step starts: a lap is driven entirely under its entry and a change takes effect on
@@ -679,16 +714,17 @@ int lmpc_sizeof_lap_report(void);
  *     stored lap, and schedules of the controller's own tables are a separate question.
  *   - nlaps == 0 with row_of_lap == NULL removes the schedule.  Refusals, each leaving the handle as it was: LMPC_E_STATE without
  *     lmpc_store_create (the lap books hold lap_n) or lmpc_rollout_create, or for LMPC_SCHEDULE_MEASUREMENT without a measurement
- *     table; LMPC_E_INVALID for an unknown table, nlaps outside 1 .. 1024 with an array, nlaps != 0 without one or the reverse, or
+ *     table; LMPC_E_INVALID for LMPC_SCHEDULE_SURFACE without a surface table (its entries name rows of no table), an unknown table, nlaps outside 1 .. 1024 with an array, nlaps != 0 without one or the reverse, or
  *     an entry outside [0, nsets) of the table as installed (a table reverted with nsets == 0 has one row).
- *   - Both install orders: while a schedule is installed, lmpc_rollout_set_vehicles / _noise / _measurement_noise refuse
- *     (LMPC_E_INVALID) a table whose rows do not cover the schedule's largest entry, an nsets == 0 revert to one row and the removal
- *     of the measurement table included.
+ *   - Both install orders: while a schedule is installed, lmpc_rollout_set_vehicles / _noise / _measurement_noise / _surfaces
+ *     refuse (LMPC_E_INVALID) a table whose rows do not cover the schedule's largest entry, an nsets == 0 revert to one row and the
+ *     removal of the measurement or surface table included.
  *   - The call synchronises the handle's streams before it replaces the schedule.  It is allowed at any time.  Without a schedule
  *     the kernels run the code they run without this feature (template instantiations). */
 #define LMPC_SCHEDULE_VEHICLE      0
 #define LMPC_SCHEDULE_NOISE        1
 #define LMPC_SCHEDULE_MEASUREMENT  2
+#define LMPC_SCHEDULE_SURFACE      3     /* the track surfaces of lmpc_rollout_set_surfaces, under the measurement kind's rules */
 int lmpc_rollout_set_lap_schedule(lmpc_handle* h, int table, int nlaps, const int* row_of_lap);
 int lmpc_rollout_sysid(lmpc_handle* h, double lamb, double* abc_host, int* flags_host);
 int lmpc_rollout_seed_from_record(lmpc_handle* h, int copies, int ss_slot0, int model_slot0);
@@ -850,6 +886,7 @@ int lmpc_sizeof_lap_window_params(void);
 int lmpc_sizeof_lane_rule_params(void);
 int lmpc_sizeof_lane_margin_params(void);
 int lmpc_sizeof_prediction_model_params(void);
+int lmpc_sizeof_surface_params(void);
 
 #ifdef __cplusplus
 }

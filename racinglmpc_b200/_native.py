@@ -89,6 +89,15 @@ class PredictionModelParams(C.Structure):
     _fields_ = [("mode", C.c_int), ("pad", C.c_int), ("vehicle", VehicleParams)]
 
 
+MAX_ZONES = 16                      # LMPC_MAX_ZONES: zones of one track-surface row
+
+
+class SurfaceParams(C.Structure):
+    """lmpc_surface_params: nzone friction zones (s_start, s_end, mu_f, mu_r) along the lap; a sub-step whose wrapped s lies in
+    [s_start, s_end) of a zone drives with peak tyre forces mu_f Df and mu_r Dr."""
+    _fields_ = [("nzone", C.c_int), ("pad", C.c_int), ("zone", C.c_double * (MAX_ZONES * 4))]
+
+
 FLAG_NOMINAL_NONFINITE = 1024       # LMPC_FLAG_NOMINAL_NONFINITE: step flag of a nominal controller whose rows 0..2 are not finite
 LANE_UNSAFE_KEY = 1 << 24           # LMPC_LANE_UNSAFE_KEY: added to the safe-set key of a lane-unsafe lap
 REPORT_LANE_UNSAFE = 1 << 16        # LMPC_REPORT_LANE_UNSAFE: report flag of an own lap judged lane-unsafe
@@ -241,6 +250,7 @@ def lib():
     L.lmpc_set_lane_margins.argtypes = [_vp, C.POINTER(LaneMarginParams), C.c_int, _vp]
     L.lmpc_get_lane_margins.argtypes = [_vp, _vp]
     L.lmpc_set_prediction_models.argtypes = [_vp, C.POINTER(PredictionModelParams), C.c_int, _vp]
+    L.lmpc_rollout_set_surfaces.argtypes = [_vp, C.POINTER(SurfaceParams), C.c_int, _vp]
     L.lmpc_rollout_sysid.argtypes = [_vp, C.c_double, _vp, _vp]
     L.lmpc_rollout_seed_from_record.argtypes = [_vp, C.c_int, C.c_int, C.c_int]
     L.lmpc_rollout_get_lap.argtypes = [_vp, C.c_int, ip, _vp, _vp]
@@ -291,6 +301,8 @@ def lib():
     assert L.lmpc_sizeof_lane_margin_params() == C.sizeof(LaneMarginParams), "lmpc_lane_margin_params ABI mismatch"
     L.lmpc_sizeof_prediction_model_params.restype = C.c_int
     assert L.lmpc_sizeof_prediction_model_params() == C.sizeof(PredictionModelParams), "lmpc_prediction_model_params ABI mismatch"
+    L.lmpc_sizeof_surface_params.restype = C.c_int
+    assert L.lmpc_sizeof_surface_params() == C.sizeof(SurfaceParams), "lmpc_surface_params ABI mismatch"
     L.lmpc_sizeof_lap_report.restype = C.c_int
     assert L.lmpc_sizeof_lap_report() == C.sizeof(LapReport), "lmpc_lap_report ABI mismatch"
     assert L.lmpc_sizeof_noise_params() == C.sizeof(NoiseParams), "lmpc_noise_params ABI mismatch"
@@ -508,6 +520,36 @@ def make_vehicle_sets(vehicles, index, batch):
     return _pack_sets(VehicleParams, vehicles, index, batch, "vehicles", row)
 
 
+def make_surface_sets(surfaces, index, batch):
+    """Per-controller track surfaces for ``lmpc_rollout_set_surfaces``: K objects ``surfaces`` with ``zones``, a sequence of
+    (s_start, s_end, mu_f, mu_r) (e.g. reference_params.SurfaceParams), and the surface of every controller ``index[batch]``.
+    Raises ValueError where the library would refuse: the index rules of ``make_param_sets``, more than MAX_ZONES zones, a value
+    that is not finite, s_start < 0, s_start >= s_end, a negative mu, or zones that do not ascend without overlap.  Returns
+    (ctypes array SurfaceParams * K, int32 index array)."""
+    def row(k, srf):
+        zones = [tuple(float(v) for v in z) for z in srf.zones]
+        if len(zones) > MAX_ZONES:
+            raise ValueError("surface %d: at most %d zones, got %d" % (k, MAX_ZONES, len(zones)))
+        r = SurfaceParams()
+        r.nzone = len(zones)
+        for j, z in enumerate(zones):
+            if len(z) != 4:
+                raise ValueError("surface %d, zone %d: a zone is (s_start, s_end, mu_f, mu_r)" % (k, j))
+            s0, s1, muf, mur = z
+            if not all(np.isfinite(z)):
+                raise ValueError("surface %d, zone %d: s_start, s_end, mu_f and mu_r must be finite" % (k, j))
+            if not 0.0 <= s0 < s1:
+                raise ValueError("surface %d, zone %d: needs 0 <= s_start < s_end, got [%r, %r)" % (k, j, s0, s1))
+            if muf < 0.0 or mur < 0.0:
+                raise ValueError("surface %d, zone %d: mu_f and mu_r must be >= 0" % (k, j))
+            if j and not zones[j - 1][1] <= s0:
+                raise ValueError("surface %d, zone %d: zones must ascend without overlap (previous s_end %r > s_start %r)"
+                                 % (k, j, zones[j - 1][1], s0))
+            r.zone[4 * j:4 * j + 4] = list(z)
+        return r
+    return _pack_sets(SurfaceParams, surfaces, index, batch, "surfaces", row)
+
+
 NOISE_FIELDS = tuple(f for f, _ in NoiseParams._fields_)
 
 
@@ -585,7 +627,7 @@ def make_lap_budget(budget, batch):
 
 
 # lmpc_rollout_set_lap_schedule: the tables a lap schedule can index (LMPC_SCHEDULE_*) and the longest schedule
-LAP_SCHEDULE_TABLES = {"vehicle": 0, "noise": 1, "measurement": 2}
+LAP_SCHEDULE_TABLES = {"vehicle": 0, "noise": 1, "measurement": 2, "surface": 3}
 MAX_LAP_SCHEDULE = 1024
 
 

@@ -74,9 +74,10 @@ class BatchedController:
         self._margins = None                                # (rows, index) of set_lane_margins, or None: no margin
         self._models = None                                 # (rows, index) of set_prediction_models, or None: all learned
         self._bx_min = np.full(self.B, self._row_bx_min(self._p))   # min_i bx_i of the QP row every controller reads
-        # rows of the plant-side tables a lap schedule indexes (the defaults: one reference vehicle and noise, no measurement
-        # table) and the installed schedules [B, L] of set_lap_schedule
-        self._table_rows = {"vehicle": 1, "noise": 1, "measurement": 0}
+        # rows of the plant-side tables a lap schedule indexes (the defaults: one reference vehicle and noise, no measurement or
+        # surface table) and the installed schedules [B, L] of set_lap_schedule
+        self._table_rows = {"vehicle": 1, "noise": 1, "measurement": 0, "surface": 0}
+        self._surfaces = None                               # (rows, index) of set_surfaces, or None: no surface table
         self._lap_schedules = {}
         self._sel = np.zeros((self.B, nit), np.int32); self._isp = np.zeros((self.B, nit), np.int32)
         self._prev = -np.ones(self.B, np.int32); self._used = np.zeros((self.B, self.trToUse), np.int32)
@@ -208,6 +209,35 @@ class BatchedController:
                       lambda: nat.make_vehicle_sets(vehicles, index, self.B))
         self._table_rows["vehicle"] = rows
 
+    def set_surfaces(self, surfaces, index=None):
+        """Per-controller track surfaces of the device simulator (friction zones along the circuit): in every later
+        ``rollout_step`` (through the surface lap schedule when one is installed) and ``rollout_pid_step``, each simulator sub-step
+        of controller b whose s -- wrapped as the curvature lookup wraps it -- lies in [s_start, s_end) of a zone of
+        ``surfaces[index[b]]`` (objects with ``zones``, e.g. reference_params.SurfaceParams) drives with peak tyre forces
+        fl(mu_f Df) and fl(mu_r Dr); every other sub-step drives the car's own Df and Dr exactly.  A mode 2 prediction model
+        (``set_prediction_models``) plans with the same surface.  ``index`` is required with ``surfaces``; ``surfaces=None`` (no
+        index) removes the table.  While a surface lap schedule is installed the new table must cover its largest entry, and it
+        cannot be removed (ValueError).  Allowed at any time; not part of a snapshot.  ValueError before any native call where the
+        library would refuse a value.  Waits for work already enqueued."""
+        rows = 0 if surfaces is None else len(surfaces)
+        self._check_schedule_cover("surface", rows)
+        packed = {}
+
+        def pack():
+            packed["v"] = nat.make_surface_sets(surfaces, index, self.B)
+            return packed["v"]
+        self._install(self._lib.lmpc_rollout_set_surfaces, "surfaces", surfaces, index, pack)
+        self._surfaces = packed.get("v")
+        self._table_rows["surface"] = rows
+
+    def surface_of(self, inst):
+        """The zones of controller ``inst``'s surface under ``set_surfaces`` as a reference_params.SurfaceParams, None without a
+        table."""
+        if self._surfaces is None:
+            return None
+        r = self._surfaces[0][int(self._surfaces[1][int(inst)])]
+        return reference_params.SurfaceParams(tuple(tuple(r.zone[4 * j:4 * j + 4]) for j in range(r.nzone)))
+
     def set_noise(self, noises, index=None):
         """Per-controller noise models of the device closed loop (a robustness study in one batch): controller b draws the
         simulator's and the PID's noise with ``noises[index[b]]`` (objects with the fields of reference_params.NoiseParams) in
@@ -263,9 +293,10 @@ class BatchedController:
 
     def set_lap_schedule(self, kind, rows=None):
         """Lap schedules of the device closed loop (conditions that change while the controllers learn: a track that gets wet at
-        lap 10, a car whose mass changes, a sensor that degrades): ``kind`` is "vehicle", "noise" or "measurement", and in every
-        later ``rollout_step`` controller b drives LMPC lap k (k = 0 is the first lap after the seeding, lap_n of ``books``)
-        under row ``rows[b][min(k, L - 1)]`` of that table (``set_vehicles``, ``set_noise``, ``set_measurement_noise``) in place
+        lap 10, a car whose mass changes, a sensor that degrades, a corner that gets wet): ``kind`` is "vehicle", "noise",
+        "measurement" or "surface", and in every later ``rollout_step`` controller b drives LMPC lap k (k = 0 is the first lap after
+        the seeding, lap_n of ``books``) under row ``rows[b][min(k, L - 1)]`` of that table (``set_vehicles``, ``set_noise``,
+        ``set_measurement_noise``, ``set_surfaces``) in place
         of its index.  ``rows`` is [L] (the same for every controller) or [batch, L], 1 <= L <= 1024, entries in the table's rows;
         ``rows=None`` removes the schedule.  The change takes effect on the first step after the hand-over that advanced lap_n
         (``rollout_commit_laps_dev``; the host-slot hand-over does not count laps).  The PID lap ignores schedules.  Needs
@@ -282,6 +313,8 @@ class BatchedController:
             return
         if kind == "measurement" and not self._table_rows[kind]:
             raise ValueError("a measurement lap schedule needs a measurement table (set_measurement_noise)")
+        if kind == "surface" and not self._table_rows[kind]:
+            raise ValueError("a surface lap schedule needs a surface table (set_surfaces)")
         s = nat.make_lap_schedule(rows, self.B, self._table_rows[kind])
         nat.check(self._lib.lmpc_rollout_set_lap_schedule(self._h, k, s.shape[1], nat.ptr(s)))
         self._lap_schedules[kind] = s

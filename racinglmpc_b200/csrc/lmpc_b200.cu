@@ -177,10 +177,12 @@ struct lmpc_handle {
     double* d_xmeas;
     // lap budgets (lmpc_rollout_set_lap_budget): laps every controller drives before it retires, or none for no budget
     HandleTable<int> budget;
-    // lap schedules (lmpc_rollout_set_lap_schedule) of the vehicle, noise and measurement tables (LMPC_SCHEDULE_*): rows [B][L] of
-    // the table per lap and no index, or none; sched_L[k] = L
-    HandleTable<int> sched[3];
-    int sched_L[3];
+    // track surfaces of the simulator (lmpc_rollout_set_surfaces), or none: the vehicle's grip all round the lap
+    HandleTable<lmpc_surface_params> surf;
+    // lap schedules (lmpc_rollout_set_lap_schedule) of the vehicle, noise, measurement and surface tables (LMPC_SCHEDULE_*): rows
+    // [B][L] of the table per lap and no index, or none; sched_L[k] = L
+    HandleTable<int> sched[4];
+    int sched_L[4];
     // device lap books (lapbooks.cuh, allocated with the store): slot tables of both pools, lap history, exchange scratch
     LapBooks bk;
     int *d_poolidx, *d_stats;
@@ -289,7 +291,7 @@ static void free_tables(lmpc_handle* h, unsigned owners) {
         t.rows.clear(); t.index.clear();
     };
     release(h->sets, OWN_HANDLE); release(h->veh, OWN_HANDLE); release(h->noise, OWN_HANDLE); release(h->streams, OWN_HANDLE);
-    release(h->meas, OWN_HANDLE); release(h->budget, OWN_HANDLE); release(h->trk, OWN_STORE); release(h->reg, OWN_STORE); release(h->pool_grp, OWN_STORE);
+    release(h->meas, OWN_HANDLE); release(h->surf, OWN_HANDLE); release(h->budget, OWN_HANDLE); release(h->trk, OWN_STORE); release(h->reg, OWN_STORE); release(h->pool_grp, OWN_STORE);
     for (auto& t : h->sched) release(t, OWN_HANDLE);
     release(h->shp, OWN_STORE); release(h->shp_order, OWN_STORE); release(h->own_c, OWN_HANDLE); release(h->ssl, OWN_STORE);
     release(h->lwin, OWN_STORE); release(h->lrule, OWN_STORE); release(h->lmar, OWN_STORE); release(h->pmod, OWN_STORE);
@@ -1054,6 +1056,7 @@ int lmpc_sizeof_lap_window_params(void) { return (int)sizeof(lmpc_lap_window_par
 int lmpc_sizeof_lane_rule_params(void) { return (int)sizeof(lmpc_lane_rule_params); }
 int lmpc_sizeof_lane_margin_params(void) { return (int)sizeof(lmpc_lane_margin_params); }
 int lmpc_sizeof_prediction_model_params(void) { return (int)sizeof(lmpc_prediction_model_params); }
+int lmpc_sizeof_surface_params(void) { return (int)sizeof(lmpc_surface_params); }
 int lmpc_sizeof_track_params(void) { return (int)sizeof(lmpc_track_params); }
 
 static int store_create_impl(lmpc_handle* h, const lmpc_model_params* mp, int ss_cap, int model_cap, int Tmax);
@@ -1578,9 +1581,9 @@ int lmpc_state_get(lmpc_handle* h, double* xLin, double* uLin, double* zt, doubl
     return LMPC_OK;
 }
 
-// K1 for the whole batch, and with a prediction-model table the nominal model after it (nominal_model.cuh).  vsched: the vehicle lap
-// schedule a mode 2 controller follows (lmpc_rollout_step), or none: its vehicle-table row.
-static int launch_k1(lmpc_handle* h, LapBudget retire = {}, LapSchedule vsched = {}) {
+// K1 for the whole batch, and with a prediction-model table the nominal model after it (nominal_model.cuh).  vsched, ssched: the
+// vehicle and surface lap schedules a mode 2 controller follows (lmpc_rollout_step), or none: its vehicle- and surface-table rows.
+static int launch_k1(lmpc_handle* h, LapBudget retire = {}, LapSchedule vsched = {}, LapSchedule ssched = {}) {
     K1Args a;
     a.batch = h->batch; a.N = h->N;
     a.wpb = h->N < K1_MAXWPB ? h->N : K1_MAXWPB;
@@ -1605,8 +1608,9 @@ static int launch_k1(lmpc_handle* h, LapBudget retire = {}, LapSchedule vsched =
     na.batch = h->batch; na.N = h->N; na.dt = h->mc.dt; na.xLin = h->d_xLin; na.uLin = h->d_uLin;
     na.pm = h->pmod.view(); na.veh = h->veh.view(); na.veh_s = vsched; na.trk = tracks(h); na.retire = retire; na.shp = h->shp.view();
     na.abc = h->hb[0].abc; na.status = h->d_flags;
+    na.surf = h->surf.view(); na.surf_s = ssched;
     const long long nthr = (long long)h->batch * h->N;
-    nominal_model_kernel<<<(unsigned)((nthr + 127) / 128), 128, 0, h->stream>>>(na);
+    (h->surf.tab ? nominal_model_kernel<true> : nominal_model_kernel<false>)<<<(unsigned)((nthr + 127) / 128), 128, 0, h->stream>>>(na);
     CK(cudaGetLastError());
     h->launches += 1;
     return LMPC_OK;
@@ -1666,10 +1670,10 @@ int lmpc_select_host(lmpc_handle* h, const double* x0, double* SS_sel, double* Q
 }  // extern "C"
 
 // One device-resident step for the whole batch on the handle's stream: K1 -> K2 -> QP -> shift (PC.py:110-137).  ev (five events
-// or null) brackets the four kernels for lmpc_step_profile.  retire: the lap budgets (the closed loop) or none; vsched: the vehicle
-// lap schedule a mode 2 prediction model follows (the closed loop) or none.
+// or null) brackets the four kernels for lmpc_step_profile.  retire: the lap budgets (the closed loop) or none; vsched, ssched: the
+// vehicle and surface lap schedules a mode 2 prediction model follows (the closed loop) or none.
 static int step_dev_impl(lmpc_handle* h, int mode, const double* x0_dev, cudaEvent_t* ev, LapBudget retire = {},
-                         LapSchedule vsched = {}) {
+                         LapSchedule vsched = {}, LapSchedule ssched = {}) {
     int rc = need_store(h);
     if (rc) return rc;
     if (!x0_dev || (mode != 0 && mode != 1)) return fail(LMPC_E_INVALID, "bad mode or null x0");
@@ -1683,7 +1687,7 @@ static int step_dev_impl(lmpc_handle* h, int mode, const double* x0_dev, cudaEve
     const bool lm = mode == 1;
     const QpIo& q = h->hb[0];
     if (ev) CK(cudaEventRecord(ev[0], st));
-    if ((rc = launch_k1(h, retire, vsched)) != LMPC_OK) return rc;                   // PC.py:117
+    if ((rc = launch_k1(h, retire, vsched, ssched)) != LMPC_OK) return rc;                   // PC.py:117
     if (ev) CK(cudaEventRecord(ev[1], st));
     if (lm && (rc = launch_k2(h, x0_dev, retire)) != LMPC_OK) return rc;             // PC.py:121
     if (ev) CK(cudaEventRecord(ev[2], st));
@@ -1854,6 +1858,17 @@ static int measure(lmpc_handle* h, unsigned long long seed, LapBudget retire, La
     return LMPC_OK;
 }
 
+// The instantiation of sim_step_kernel a step launches: lap reports, lap schedules (sched) and a surface table as installed
+using SimStepKernel = void (*)(const ModelConst, const SimArgs, const LapReports, const int*, const LapSchedule, const LapSchedule,
+                               const Table<lmpc_surface_params>, const LapSchedule);
+static SimStepKernel sim_step_launch(const lmpc_handle* h, bool sched) {
+    const bool rp = h->rep_L != 0, sf = h->surf.tab != nullptr;
+    if (sf) return rp ? (sched ? sim_step_kernel<true, true, true> : sim_step_kernel<true, false, true>)
+                      : (sched ? sim_step_kernel<false, true, true> : sim_step_kernel<false, false, true>);
+    return rp ? (sched ? sim_step_kernel<true, true, false> : sim_step_kernel<true, false, false>)
+              : (sched ? sim_step_kernel<false, true, false> : sim_step_kernel<false, false, false>);
+}
+
 // One closed-loop step for every instance, all on the device (SysModel.py:34-48):
 //   Controller.solve(x) -> u = uPred[0] -> Controller.addPoint(x, u) (LMPC) -> x+ = dynModel(x, x_glob, u); done = s+ > TrackLength
 // The controller's x (solve, addPoint, the record) is the measured state y when a measurement table is installed.
@@ -1875,7 +1890,7 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
         io.xPred = q.xPred; io.uPred = q.uPred; io.slack = q.slack; io.status = q.status; io.iters = q.iters; io.resid = q.resid;
         rc = solve_dev(h, io, 54, 0, retire);
     } else {
-        rc = step_dev_impl(h, mode, y, nullptr, retire, lap_schedule(h, LMPC_SCHEDULE_VEHICLE));
+        rc = step_dev_impl(h, mode, y, nullptr, retire, lap_schedule(h, LMPC_SCHEDULE_VEHICLE), lap_schedule(h, LMPC_SCHEDULE_SURFACE));
     }
     if (rc) return rc;
     if (mode == 1) {                                                                 // SysModel.py:38 -> PC.py:466-476
@@ -1895,9 +1910,8 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
     sa.flags = h->d_flags; sa.status = q.status; sa.health = h->d_health; sa.retire = retire;
     if (h->meas.tab) sa.rec_x = y;
     const LapSchedule vs = lap_schedule(h, LMPC_SCHEDULE_VEHICLE), ns = lap_schedule(h, LMPC_SCHEDULE_NOISE);
-    (vs.rows || ns.rows ? (h->rep_L ? sim_step_kernel<true, true> : sim_step_kernel<false, true>)
-                        : (h->rep_L ? sim_step_kernel<true, false> : sim_step_kernel<false, false>))<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(
-        h->mc, sa, reports(h), q.iters, vs, ns);
+    sim_step_launch(h, vs.rows || ns.rows)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(
+        h->mc, sa, reports(h), q.iters, vs, ns, h->surf.view(), lap_schedule(h, LMPC_SCHEDULE_SURFACE));
     CK(cudaGetLastError());
     h->launches += 1;
     h->cur ^= 1;
@@ -1922,8 +1936,8 @@ int lmpc_rollout_pid_step(lmpc_handle* h, double vt, const double* z_pid_host, c
     SimArgs sa = sim_args(h, z_sim_host ? h->d_z : nullptr, seed);
     sa.health = h->d_health;          // no step flags or QP status here: only the simulator's own bits
     if (h->meas.tab) sa.rec_x = y;
-    (h->rep_L ? sim_step_kernel<true, false> : sim_step_kernel<false, false>)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(
-        h->mc, sa, reports(h), nullptr, LapSchedule{}, LapSchedule{});
+    sim_step_launch(h, false)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(
+        h->mc, sa, reports(h), nullptr, LapSchedule{}, LapSchedule{}, h->surf.view(), LapSchedule{});
     CK(cudaGetLastError());
     h->launches += 2;
     h->cur ^= 1;
@@ -1957,6 +1971,34 @@ int lmpc_rollout_set_vehicles(lmpc_handle* h, const lmpc_vehicle_params* sets, i
             return fail(LMPC_E_INVALID, std::string(who) + ": vehicle " + std::to_string(k) +
                                             ": m, Iz, lf, lr must be positive and all ten values finite");
         row = v;
+        return LMPC_OK;
+    });
+}
+
+// Per-controller track surfaces: per row 0 <= nzone <= LMPC_MAX_ZONES, every zone's values finite, 0 <= s_start < s_end, mu_f and
+// mu_r >= 0, zones ascending without overlap; nsets == 0 removes the table (refused while a surface schedule names a row).
+int lmpc_rollout_set_surfaces(lmpc_handle* h, const lmpc_surface_params* sets, int nsets, const int* set_of_instance) {
+    static const char* who = "lmpc_rollout_set_surfaces";
+    if (!h) return fail(LMPC_E_INVALID, "null handle");
+    if (int rc = check_schedule_cover(h, who, LMPC_SCHEDULE_SURFACE, nsets)) return rc;
+    return install_table(h, who, h->surf, sets, nsets, set_of_instance, (const lmpc_surface_params*)nullptr,
+                         [&](int k, lmpc_surface_params& row) {
+        const lmpc_surface_params& r = sets[k];
+        const std::string w = std::string(who) + ": surface " + std::to_string(k);
+        if (r.nzone < 0 || r.nzone > LMPC_MAX_ZONES)
+            return fail(LMPC_E_INVALID, w + ": nzone must be 0 .. " + std::to_string(LMPC_MAX_ZONES));
+        for (int z = 0; z < r.nzone; ++z) {
+            const double* v = r.zone + 4 * z;
+            const std::string wz = w + ", zone " + std::to_string(z);
+            if (!(isfinite(v[0]) && isfinite(v[1]) && isfinite(v[2]) && isfinite(v[3])))
+                return fail(LMPC_E_INVALID, wz + ": s_start, s_end, mu_f and mu_r must be finite");
+            if (!(v[0] >= 0.0 && v[0] < v[1]))
+                return fail(LMPC_E_INVALID, wz + ": needs 0 <= s_start < s_end");
+            if (!(v[2] >= 0.0 && v[3] >= 0.0)) return fail(LMPC_E_INVALID, wz + ": mu_f and mu_r must be >= 0");
+            if (z > 0 && !(r.zone[4 * (z - 1) + 1] <= v[0]))
+                return fail(LMPC_E_INVALID, wz + ": zones must ascend without overlap (s_end of the previous zone <= s_start)");
+        }
+        row = r;
         return LMPC_OK;
     });
 }
@@ -2024,12 +2066,15 @@ int lmpc_rollout_set_lap_schedule(lmpc_handle* h, int table, int nlaps, const in
     static const char* who = "lmpc_rollout_set_lap_schedule";
     if (int rc = need_rollout(h)) return rc;
     const std::string w(who);
-    if (table < LMPC_SCHEDULE_VEHICLE || table > LMPC_SCHEDULE_MEASUREMENT)
-        return fail(LMPC_E_INVALID, w + ": table must be LMPC_SCHEDULE_VEHICLE, _NOISE or _MEASUREMENT");
+    if (table < LMPC_SCHEDULE_VEHICLE || table > LMPC_SCHEDULE_SURFACE)
+        return fail(LMPC_E_INVALID, w + ": table must be LMPC_SCHEDULE_VEHICLE, _NOISE, _MEASUREMENT or _SURFACE");
     const size_t nrows = table == LMPC_SCHEDULE_VEHICLE ? h->veh.rows.size()
-                       : table == LMPC_SCHEDULE_NOISE   ? h->noise.rows.size() : h->meas.rows.size();
+                       : table == LMPC_SCHEDULE_NOISE   ? h->noise.rows.size()
+                       : table == LMPC_SCHEDULE_MEASUREMENT ? h->meas.rows.size() : h->surf.rows.size();
     if (table == LMPC_SCHEDULE_MEASUREMENT && !h->meas.tab && row_of_lap)
         return fail(LMPC_E_STATE, w + ": a measurement schedule needs a measurement table (lmpc_rollout_set_measurement_noise)");
+    if (table == LMPC_SCHEDULE_SURFACE && !h->surf.tab && row_of_lap)     // every entry names a row of an absent table
+        return fail(LMPC_E_INVALID, w + ": a surface schedule needs a surface table (lmpc_rollout_set_surfaces)");
     if ((nlaps == 0) != (row_of_lap == nullptr))
         return fail(LMPC_E_INVALID, w + ": nlaps == 0 goes with a NULL row_of_lap, nlaps >= 1 with an array");
     if (nlaps < 0 || nlaps > 1024) return fail(LMPC_E_INVALID, w + ": nlaps must be 0 .. 1024");

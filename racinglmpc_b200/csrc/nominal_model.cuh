@@ -22,11 +22,17 @@ struct NominalArgs {
     Shapes shp;                       // stages i >= N_b are not identified
     double* abc;                      // [B][N][54]
     int* status;                      // [B] step flags: 2 (curvature lookup failed), LMPC_FLAG_NOMINAL_NONFINITE
+    Table<lmpc_surface_params> surf;  // the simulator's surface table (mode 2; read by the SURF instantiation only)
+    LapSchedule surf_s;               // its lap schedule in the closed loop, else rows == nullptr: the table's own index
 };
 
 // One thread per (controller, stage).  The state z = (vx, vy, wz) and its forward sensitivity S = dz/d(vx0, vy0, wz0, delta, a)
 // (3 x 5) stay in registers through the sub-steps: z <- z + h f(z, u), S <- S + h (f_z S + f_u E), E = [0 | I2], f_z and f_u
 // taken at the sub-step's starting state, which is the derivative of the explicit-Euler map itself.
+// SURF (a surface table is installed): a mode 2 controller also carries (epsi, s, ey) through the sub-steps with the simulator's
+// own curvature lookup, so that each sub-step's peak forces follow the zone the plant's s is in (sim_step_kernel).  The zone is
+// piecewise constant in s, so it adds nothing to the derivatives: rows 0..2 of A keep columns 3..5 zero.
+template <bool SURF>
 __global__ void __launch_bounds__(128) nominal_model_kernel(const NominalArgs a) {
     const int t = blockIdx.x * blockDim.x + threadIdx.x;
     const int b = t / a.N, i = t - b * a.N;
@@ -45,18 +51,27 @@ __global__ void __launch_bounds__(128) nominal_model_kernel(const NominalArgs a)
     double vx = xl[0], vy = xl[1], wz = xl[2];
     double S[3][5] = {{1, 0, 0, 0, 0}, {0, 1, 0, 0, 0}, {0, 0, 1, 0, 0}};
     const double sd = sin(delta), cd = cos(delta);
+    // SURF: the kinematic states of the plant's sub-steps and the zone cursor (zoned: a mode 2 controller)
+    const bool zoned = SURF && row.mode == 2;
+    double epsi = xl[3], sk = xl[4], ey = xl[5];
+    SurfaceCursor zc{zoned ? &a.surf_s.of(a.surf, b) : nullptr, 0};
+    const TrackRec* trk = zoned ? &a.trk.of(b) : nullptr;
     int k = 0;
     while ((k + 1) * h <= a.dt) {
+        double Dfi = Df, Dri = Dr;
+        if constexpr (SURF) {
+            if (zoned) surface_forces(zc, sk, trk->TrackLength, Df, Dr, &Dfi, &Dri);
+        }
         // the simulator's sub-step (sim_step_kernel), with the reference's lf in alpha_r
         const double pf = vy + lf * wz, pq = vy - lf * wz;
         const double af = delta - atan2(pf, vx);
         const double ar = -atan2(pq, vx);
         const double tf = atan(Bf * af), tr = atan(Br * ar);
-        const double Fyf = Df * sin(Cf * tf);
-        const double Fyr = Dr * sin(Cr * tr);
+        const double Fyf = Dfi * sin(Cf * tf);
+        const double Fyr = Dri * sin(Cr * tr);
         // dFy/dalpha and dalpha/d(vx, vy, wz); d alpha_f / d delta = 1
-        const double gf = Df * cos(Cf * tf) * Cf * Bf / (1.0 + (Bf * af) * (Bf * af));
-        const double gr = Dr * cos(Cr * tr) * Cr * Br / (1.0 + (Br * ar) * (Br * ar));
+        const double gf = Dfi * cos(Cf * tf) * Cf * Bf / (1.0 + (Bf * af) * (Bf * af));
+        const double gr = Dri * cos(Cr * tr) * Cr * Br / (1.0 + (Br * ar) * (Br * ar));
         const double rf = 1.0 / (vx * vx + pf * pf), rr = 1.0 / (vx * vx + pq * pq);
         const double daf[3] = {pf * rf, -vx * rf, -lf * vx * rf};
         const double dar[3] = {pq * rr, -vx * rr, lf * vx * rr};
@@ -87,6 +102,17 @@ __global__ void __launch_bounds__(128) nominal_model_kernel(const NominalArgs a)
         for (int r = 0; r < 3; ++r)
 #pragma unroll
             for (int c = 0; c < 5; ++c) S[r][c] = Sn[r][c];
+        if constexpr (SURF) {
+            if (zoned) {      // the simulator's (epsi, s, ey) update, from the sub-step's starting state
+                int okz = 1;
+                const double cur = curvature_lookup(*trk, sk, &okz);
+                const double ce = cos(epsi), se = sin(epsi);
+                const double nepsi = epsi + h * (wz - (vx * ce - vy * se) / (1 - cur * ey) * cur);
+                const double ns = sk + h * ((vx * ce - vy * se) / (1 - cur * ey));
+                const double ney = ey + h * (vx * se + vy * ce);
+                epsi = nepsi; sk = ns; ey = ney;
+            }
+        }
         const double nvx = vx + h * (acc - 1 / mass * Fyf * sd + wz * vy);
         const double nvy = vy + h * (1 / mass * (Fyf * cd + Fyr) - wz * vx);
         const double nwz = wz + h * (1 / Iz * (lf * Fyf * cd - lr * Fyr));

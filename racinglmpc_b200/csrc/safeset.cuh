@@ -1023,12 +1023,50 @@ constexpr int SIM_RECORD_FULL = 256;
 #include "lap_schedule.cuh"
 namespace lmpc {
 
+// Track surfaces (lmpc_rollout_set_surfaces): the zone of one controller's sub-steps, found by a cursor that follows s.  The
+// zones of a row ascend without overlap, so their s_end ascend strictly, and the first zone whose s_end lies above the wrapped s
+// is the only one that can hold it.  The cursor walks to that zone from where the last sub-step left it (s moves by at most
+// vx h per sub-step), in either direction, so it returns what a scan of every zone returns at any s.
+struct SurfaceCursor {
+    const lmpc_surface_params* row;
+    int c;
+    // true and the zone's (mu_f, mu_r) when a zone holds s, wrapped as curvature_lookup wraps it; false when none does, s is not
+    // finite or s is beyond 64 laps
+    __device__ __forceinline__ bool at(double s, double L, double* muf, double* mur) {
+        if (!(s <= 64.0 * L)) return false;
+        while (s > L) s = s - L;
+        const double* z = row->zone;
+        const int n = row->nzone;
+        while (c > 0 && z[(c - 1) * 4 + 1] > s) --c;
+        while (c < n && z[c * 4 + 1] <= s) ++c;
+        if (c >= n || !(z[c * 4] <= s)) return false;
+        *muf = z[c * 4 + 2];
+        *mur = z[c * 4 + 3];
+        return true;
+    }
+};
+
+// The peak tyre forces of a sub-step at s: fl(mu_f Df), fl(mu_r Dr) in a zone, else Df and Dr exactly
+__device__ __forceinline__ void surface_forces(SurfaceCursor& zc, double s, double L, double Df, double Dr, double* Dfi, double* Dri) {
+    double muf, mur;
+    if (zc.at(s, L, &muf, &mur)) {
+        *Dfi = __dmul_rn(muf, Df);
+        *Dri = __dmul_rn(mur, Dr);
+    } else {
+        *Dfi = Df;
+        *Dri = Dr;
+    }
+}
+
 // REPORTS: the step is also added to the controller's running report row (report_step) with its QP's status a.status and
 // iterations rep_iters, both null for a PID step.  SCHED: the vehicle and noise rows come from the lap schedules veh_s and
-// noise_s (lap_schedule.cuh; either may be null).  The parameters after a are read only by those instantiations.
-template <bool REPORTS, bool SCHED>
+// noise_s (lap_schedule.cuh; either may be null).  SURF: each sub-step's peak tyre forces follow the controller's surface row of
+// surf, through the lap schedule surf_s (null: the table's own index).  The parameters after a are read only by those
+// instantiations.
+template <bool REPORTS, bool SCHED, bool SURF>
 __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimArgs a, const LapReports rep, const int* rep_iters,
-                                const LapSchedule veh_s, const LapSchedule noise_s) {
+                                const LapSchedule veh_s, const LapSchedule noise_s, const Table<lmpc_surface_params> surf,
+                                const LapSchedule surf_s) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= a.batch) return;
     if (a.retire.retired(b)) {
@@ -1070,11 +1108,14 @@ __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimA
     const double sd = sin(delta), cd = cos(delta);
     int i = 0;
     int okc = 1;
+    SurfaceCursor zc{SURF ? &surf_s.of(surf, b) : nullptr, 0};
     while ((i + 1) * h <= m.dt) {
+        double Dfi = Df, Dri = Dr;
+        if constexpr (SURF) surface_forces(zc, s, trk.TrackLength, Df, Dr, &Dfi, &Dri);
         const double af = delta - atan2(vy + lf * wz, vx);
         const double ar = -atan2(vy - lf * wz, vx);
-        const double Fyf = Df * sin(Cf * atan(Bf * af));
-        const double Fyr = Dr * sin(Cr * atan(Br * ar));
+        const double Fyf = Dfi * sin(Cf * atan(Bf * af));
+        const double Fyr = Dri * sin(Cr * atan(Br * ar));
         const double nvx = vx + h * (acc - 1 / mass * Fyf * sd + wz * vy);
         const double nvy = vy + h * (1 / mass * (Fyf * cd + Fyr) - wz * vx);
         const double nwz = wz + h * (1 / Iz * (lf * Fyf * cd - lr * Fyr));

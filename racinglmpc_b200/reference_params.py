@@ -200,6 +200,35 @@ class PredictionModelParams:
         return cls(1, vehicle)
 
 
+@dataclass(frozen=True)
+class SurfaceParams:
+    """A track surface (no reference counterpart: the reference's grip is the same all round the lap): up to 16 zones
+    (s_start, s_end, mu_f, mu_r), ascending without overlap, in the s-coordinate of the controller's track.  A simulator sub-step
+    whose s (wrapped as the curvature lookup wraps it) lies in [s_start, s_end) of a zone drives with peak tyre forces mu_f Df and
+    mu_r Dr of its car; elsewhere the car's own.  The device takes one per controller (BatchedController.set_surfaces)."""
+    zones: tuple = ()
+
+    def __post_init__(self):
+        object.__setattr__(self, "zones", tuple(tuple(float(v) for v in z) for z in self.zones))
+
+    @classmethod
+    def dry(cls):
+        """No zone: installed, the controllers drive exactly what they drive without a table."""
+        return cls(())
+
+    @classmethod
+    def from_zones(cls, zones):
+        """Zones given as (s_start, s_end, mu_f, mu_r) rows."""
+        return cls(tuple(zones))
+
+    @classmethod
+    def on_segment(cls, track, row, mu_f, mu_r=None):
+        """One zone covering segment ``row`` of ``track`` (a TrackParams): [s_start, s_start + length) of its seg_table row, the
+        end rounded as the curvature lookup forms it; ``mu_r`` None takes ``mu_f``."""
+        s0, ln = float(track.seg_table[row, 0]), float(track.seg_table[row, 1])
+        return cls(((s0, float(np.float64(s0) + np.float64(ln)), float(mu_f), float(mu_f if mu_r is None else mu_r)),))
+
+
 def _wrap(a):
     if a < -np.pi:
         return 2 * np.pi + a

@@ -12,9 +12,10 @@ across their untemplated names:
            table and no lane-rule table; <false, false, false, false>: no lap-count table, no lap reports, no lap-window table and
            no lane-rule table; <false, false, false, false, false>: the same and no lane-margin table), pool_local_best_kernel, pool_export_kernel (<false>: no lane-rule table), commit_laps_kernel,
            seed_from_record_kernel
-           (<false>: no lap reports), sim_step_kernel (<false> or <false, false>: no lap reports and no lap schedule) and measure_kernel (<false>:
-           no lap schedule)
-  reports  sim_step_kernel<true> or <true, false>: lap reports and no lap schedule
+           (<false>: no lap reports), sim_step_kernel (<false>, <false, false> or <false, false, false>: no lap reports, no lap
+           schedule and no surface table), measure_kernel (<false>: no lap schedule) and nominal_model_kernel (<false>: no
+           surface table)
+  reports  sim_step_kernel<true>, <true, false> or <true, false, false>: lap reports, no lap schedule and no surface table
 and compared by instruction text (cuobjdump -sass without addresses and encodings).  Each differing line pair is classified:
   dfma-swap   one DFMA with its two factors exchanged (a*b+c = b*a+c)
   lds-swap    LDS.128 loads of unchanged addresses whose destination registers are permuted among themselves
@@ -32,9 +33,9 @@ import sys
 NAME = re.compile(r"^(?:void )?(ftocp_kernel|ftocp_sets_kernel)<(\d+), (\d+), 2, 4(?:, (true|false))?>")
 DEFAULT = re.compile(r"^(?:void )?lmpc::(knn_ltv_regress_kernel|ss_select_kernel|shift_state_kernel|books_refresh_kernel|"
                      r"commit_laps_books_kernel|seed_books_kernel|pool_import_kernel|sim_step_kernel|commit_laps_kernel|"
-                     r"seed_from_record_kernel|measure_kernel|pool_local_best_kernel|pool_export_kernel)"
+                     r"seed_from_record_kernel|measure_kernel|pool_local_best_kernel|pool_export_kernel|nominal_model_kernel)"
                      r"(<false>|<false, false>|<false, false, false>|<false, false, false, false>|<false, false, false, false, false>)?\(")
-REPORTS = re.compile(r"^(?:void )?lmpc::(sim_step_kernel)<true(?:, false)?>\(")
+REPORTS = re.compile(r"^(?:void )?lmpc::(sim_step_kernel)<true(?:, false){0,2}>\(")
 
 
 def kernels(path):
