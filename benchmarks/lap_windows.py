@@ -5,7 +5,7 @@ LMPC learns.
 Leg 1, cost: benchmarks/rollout_mc.run (PID lap, seeding, `laps` LMPC laps, independent mode, lap reports on) in alternating
 rounds in the same process, with
   none       no window table;
-  unbounded  a table of all-(0, 0) rows: every book kernel runs its window instantiation, every window unbounded.
+  unbounded  a table of all-(0, 0) rows: every book kernel reads the window table, every window unbounded.
 Per round: ms of the LMPC laps and controller steps/s (device events).  Both arms must drive the same closed loop: books, end
 states, health, solver reports and lap reports are asserted identical.
 Leg 2, against the parent build (--parent-root: a checkout of the previous commit with its library built): bench.py --config 1, 2

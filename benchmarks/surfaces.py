@@ -5,7 +5,7 @@ and a physics prediction model cope with grip that changes within a lap.
 Leg 1, identity and cost: benchmarks/rollout_mc.run at configs[3] (8 192 controllers, 3 LMPC laps, lap reports on), independent
 and pooled, in alternating rounds in one process, under
   none     no table;
-  dry      an all-dry table (nzone = 0): sim_step_kernel<..., true> with an empty row;
+  dry      an all-dry table (nzone = 0): sim_step_kernel with an empty row;
   ones16   a 16-zone table with every mu = 1 spread over the lap (the worst-case lookup: the cursor walks every zone).
 All arms must drive the same closed loop: books, end states, health, solver reports and lap reports are asserted identical in the
 run.  Per round: ms of the LMPC laps; each table's difference against the round-to-round spread.
@@ -113,7 +113,7 @@ def leg_kernel(batches, rounds, reps, dev):
                 for a, sets in _tables(B).items():
                     c.set_surfaces(*(sets if sets is not None else (None,)))
                     c.rollout_set_state(x0, x0)
-                    c.rollout_pid_step(1.0, seed=5)                    # warm-up launch of this instantiation
+                    c.rollout_pid_step(1.0, seed=5)                    # warm-up launch under this table
                     c.sync()
                     with torch.profiler.profile(activities=act) as prof:
                         for _ in range(reps):

@@ -689,7 +689,7 @@ typedef struct lmpc_lap_report {
  *     hand-over or seeding.  Enabling again with another max_laps starts an empty table.  Any refusal leaves the handle as it was.
  *   - Memory: batch * max_laps * 32 bytes + batch * 48 (64 MB at batch 8192, 256 laps).  Both buffers are snapshot sections
  *     (absent, 0 bytes, without reports: such records are unchanged); a restore refuses records whose report sections differ.
- *   - Without reports the kernels run the code they run without this feature (template instantiations). */
+ *   - Without reports the kernels read no report buffer: they test for them at run time. */
 int lmpc_rollout_enable_lap_reports(lmpc_handle* h, int max_laps);
 /* Report rows rows[B][max_laps] and the count n[B] of laps filed (which may exceed max_laps; rows >= min(n, max_laps) are
  * unused) into host arrays, either may be NULL.  LMPC_E_STATE without reports.  Synchronises. */
@@ -720,7 +720,7 @@ int lmpc_sizeof_lap_report(void);
  *     refuse (LMPC_E_INVALID) a table whose rows do not cover the schedule's largest entry, an nsets == 0 revert to one row and the
  *     removal of the measurement or surface table included.
  *   - The call synchronises the handle's streams before it replaces the schedule.  It is allowed at any time.  Without a schedule
- *     the kernels run the code they run without this feature (template instantiations). */
+ *     the kernels read set_of_instance[b]. */
 #define LMPC_SCHEDULE_VEHICLE      0
 #define LMPC_SCHEDULE_NOISE        1
 #define LMPC_SCHEDULE_MEASUREMENT  2

@@ -3,7 +3,7 @@
 // A schedule replaces controller b's row of a plant-side table (vehicles, process noise, measurement noise) by the row of the lap
 // it drives: rows[b][min(lap_n[b], L - 1)], lap_n being the laps handed over since the seeding (the lap books).  Like the lap
 // budget it is derived from the lap count and never stored per step, so a restored snapshot resumes at its entry.  A null schedule
-// (the PID lap, a handle without one for this table) reads the table's own index.  Only the kernels' SCHED instantiations take it.
+// (the PID lap, a handle without one for this table) reads the table's own index.
 #pragma once
 
 namespace lmpc {

@@ -30,22 +30,15 @@ constexpr int LAP_HIST = 16;
 
 __device__ __forceinline__ bool key_less(int t1, int n1, int t2, int n2) { return t1 < t2 || (t1 == t2 && n1 < n2); }
 
-// numSS_it of controller b in a book kernel.  The kernels that rank safe-set laps come in two instantiations, LAPS = a lap-count
-// table is installed (lmpc_set_ss_laps): without one they read the handle's value, the code they were before the table existed.
-template <bool LAPS>
-__device__ __forceinline__ int book_laps(const LapBooks& k, const SsLaps& laps, int b) { return LAPS ? laps.of(b).numSS_it : k.numSS_it; }
-
-// The lap windows of every controller (lmpc_set_lap_windows): ss_window / model_window most recent laps, 0 = unbounded.  The four
-// kernels that rank laps come in two more instantiations, WIN = a window table is installed; without one they never read it and
-// the book functions below are the code they were before windows existed.
+// The lap windows of every controller (lmpc_set_lap_windows): ss_window / model_window most recent laps, 0 = unbounded.  Without a
+// window table (tab == null) every window is unbounded.
 using LapWindowRec = lmpc_lap_window_params;
 using LapWindows = Table<LapWindowRec>;
-template <bool WIN>
-__device__ __forceinline__ LapWindowRec book_windows(const LapWindows& w, int b) { return WIN ? w.of(b) : LapWindowRec{0, 0}; }
+__device__ __forceinline__ LapWindowRec book_windows(const LapWindows& w, int b) { return w.tab ? w.of(b) : LapWindowRec{0, 0}; }
 
 // The lane rules of every controller (lmpc_set_lane_rules) and the QP constants (Fx, bx) they judge against: the controller's
-// parameter-set row, else the handle's.  The five kernels that file or ship safe-set laps come in two more instantiations, LANE =
-// a rule table is installed; without one they never read it and the key of a lap is its lap time, the code they were before.
+// parameter-set row, else the handle's.  Without a rule table (rule.tab == null) no lap is judged and the key of a lap is its lap
+// time.
 using LaneRuleRec = lmpc_lane_rule_params;
 struct LaneRules {
     Table<LaneRuleRec> rule;
@@ -54,8 +47,8 @@ struct LaneRules {
 
 // Does the lap x[0 .. T) (row r at x + r * stride, its state in the first 6 entries) leave the lane Fx x <= bx of c by more than
 // tol?  A row does when an entry is not finite or d_i = Fx[i] . x - bx[i] > tol for one of the ncx == 2 lane rows, evaluated in
-// order without contraction: the arithmetic of report_step (safeset.cuh), kept as a copy of its own so that the closed loop's
-// step kernel stays the code it was.  One block-wide pass; every thread of the block must call it.
+// order without contraction: the arithmetic of report_step (safeset.cuh), kept as a copy rather than a helper shared with the
+// closed loop's step kernel.  One block-wide pass; every thread of the block must call it.
 __device__ __forceinline__ bool lane_leaves_block(const FtocpConst& c, const double* x, int T, int stride, double tol) {
     bool bad = false;
     for (int t = threadIdx.x; t < T && !bad; t += blockDim.x) {
@@ -76,28 +69,25 @@ __device__ __forceinline__ bool lane_leaves_block(const FtocpConst& c, const dou
     return __syncthreads_or(bad) != 0;
 }
 
-// Is the lap x[0 .. T) lane-unsafe for controller b: does it leave its lane by more than its lane_tol?  False without a table
-// (LANE) or under mode 0.
-template <bool LANE>
+// Is the lap x[0 .. T) lane-unsafe for controller b: does it leave its lane by more than its lane_tol?  False without a table or
+// under mode 0.  Both tests are uniform over the block (a kernel argument, the controller's own row): no barrier is skipped by part
+// of it.
 __device__ __forceinline__ bool lane_unsafe_block(const LaneRules& lr, int b, const double* x, int T, int stride) {
-    if constexpr (!LANE) {
-        return false;
-    } else {
-        const LaneRuleRec r = lr.rule.of(b);
-        if (r.mode != 1) return false;                           // uniform over the block: no barrier is skipped by part of it
-        return lane_leaves_block(lr.qp.of(b).c, x, T, stride, r.lane_tol);
-    }
+    if (!lr.rule.tab) return false;
+    const LaneRuleRec r = lr.rule.of(b);
+    if (r.mode != 1) return false;
+    return lane_leaves_block(lr.qp.of(b).c, x, T, stride, r.lane_tol);
 }
 // The safe-set key a lap of lap time T is filed with: T, plus LMPC_LANE_UNSAFE_KEY when it was judged lane-unsafe
 __device__ __forceinline__ int lane_key(int T, bool unsafe) { return unsafe ? T + LMPC_LANE_UNSAFE_KEY : T; }
-// The lap time of a safe-set key (the pooled export ranks and ships raw lap times)
-template <bool LANE>
-__device__ __forceinline__ int lane_lap_time(int key) { return LANE && key >= LMPC_LANE_UNSAFE_KEY ? key - LMPC_LANE_UNSAFE_KEY : key; }
+// The lap time of a safe-set key (the pooled export ranks and ships raw lap times); rules: a lane-rule table is installed.  Without
+// one a key is its lap time, whatever its value.
+__device__ __forceinline__ int lane_lap_time(int key, bool rules) { return rules && key >= LMPC_LANE_UNSAFE_KEY ? key - LMPC_LANE_UNSAFE_KEY : key; }
 
 // The lane margins of every controller (lmpc_set_lane_margins): the table, the untightened QP rows (the controller's parameter-set
 // row, else the handle's), the derived planning rows plan[B] (the source row with bx_i - m_b) that every QP of the handle reads,
-// the margins m[B] and the warm-start validity (null without warm start).  commit_laps_books_kernel comes in two more
-// instantiations, MARGIN = a margin table is installed; without one it never reads this.
+// the margins m[B] and the warm-start validity (null without warm start).  Without a margin table (rule.tab == null)
+// commit_laps_books_kernel reads none of it.
 using LaneMarginRec = lmpc_lane_margin_params;
 struct LaneMargins {
     Table<LaneMarginRec> rule;
@@ -213,8 +203,9 @@ __device__ inline int book_md_add_window(const LapBooks& k, int b, int T, int W)
 // import == true: a lap another controller drove, filed BEFORE the controller's own latest lap (which stays lap it-1, the one
 // addPoint extends): it takes lap number it-1, the own latest moves to it; it is skipped (-1) when it would not be among the
 // nit fastest (nit: the controller's numSS_it).  Returns the slot to copy the lap into, -1 = not stored, -2 = pool too small (the
-// tables are left as they were).
-__device__ inline int book_ss_add(const LapBooks& k, int b, int T, bool import, int nit) {
+// tables are left as they were).  W: the controller's safe-set window, 0 = unbounded; W > 0 files under book_ss_add_window.
+__device__ inline int book_ss_add(const LapBooks& k, int b, int T, bool import, int nit, int W) {
+    if (W > 0) return book_ss_add_window(k, b, T, import, nit, W);
     int* tm = k.ss_time + (size_t)b * k.ss_cap;
     int* ln = k.ss_lap + (size_t)b * k.ss_cap;
     const int it = k.it[b];
@@ -251,8 +242,9 @@ __device__ inline int book_ss_add(const LapBooks& k, int b, int T, bool import, 
 }
 
 // PredictiveModel.addTrajectory bookkeeping for a lap of `T` rows.  Returns the slot, or -1 when the lap can never be among
-// the trToUse shortest.
-__device__ inline int book_md_add(const LapBooks& k, int b, int T) {
+// the trToUse shortest.  W: the controller's model window, 0 = unbounded; W > 0 files under book_md_add_window.
+__device__ inline int book_md_add(const LapBooks& k, int b, int T, int W) {
+    if (W > 0) return book_md_add_window(k, b, T, W);
     int* tm = k.md_time + (size_t)b * k.md_cap;
     int* sq = k.md_seq + (size_t)b * k.md_cap;
     const int seq = k.md_cnt[b];
@@ -278,29 +270,17 @@ __device__ inline int book_md_add(const LapBooks& k, int b, int T) {
     return slot;
 }
 
-// The book functions of a kernel with a lap-window table (WIN) take the controller's window W (0 = unbounded, the function
-// above); without one they are the function above and W is not read.
-template <bool WIN>
-__device__ __forceinline__ int book_ss_add(const LapBooks& k, int b, int T, bool import, int nit, int W) {
-    return WIN && W > 0 ? book_ss_add_window(k, b, T, import, nit, W) : book_ss_add(k, b, T, import, nit);
-}
-template <bool WIN>
-__device__ __forceinline__ int book_md_add(const LapBooks& k, int b, int T, int W) {
-    return WIN && W > 0 ? book_md_add_window(k, b, T, W) : book_md_add(k, b, T);
-}
-
 // What the next lap reads: the nit fastest safe-set laps in argsort order (nit: the controller's numSS_it), which of them is lap
 // it-1, the slot addPoint extends, and usedIt of the regression model.  Returns 0, or 8 when fewer than nit laps are stored (the
 // reference raises IndexError at PC.py:402-403).  Entries nit .. k.numSS_it-1 of sel repeat the last selected slot and those of
-// isprev are 0: K2 reads none of them, and a snapshot packs them as they are.  WIN: only laps in the controller's windows w count
+// isprev are 0: K2 reads none of them, and a snapshot packs them as they are.  Only laps in the controller's windows w count
 // (lap numbers >= it - ss_window, arrival numbers >= md_cnt - model_window; a window of 0 starts at 0, and a free slot, -1, is
 // below every start).
-template <bool WIN>
 __device__ inline int book_refresh(const LapBooks& k, int b, int nit, LapWindowRec w) {
     const int* tm = k.ss_time + (size_t)b * k.ss_cap;
     const int* ln = k.ss_lap + (size_t)b * k.ss_cap;
     const int it = k.it[b];
-    const int lo = WIN && w.ss_window > 0 ? max(it - w.ss_window, 0) : 0;
+    const int lo = w.ss_window > 0 ? max(it - w.ss_window, 0) : 0;
     int flag = 0, prev = -1, last = 0;
     for (int s = 0; s < k.ss_cap; ++s) if (it > 0 && ln[s] == it - 1) prev = s;   // it = 0: no lap (a free slot has ln = -1)
     for (int c = 0; c < nit; ++c) {
@@ -319,7 +299,7 @@ __device__ inline int book_refresh(const LapBooks& k, int b, int nit, LapWindowR
     k.prevslot[b] = prev;
     const int* mt = k.md_time + (size_t)b * k.md_cap;
     const int* ms = k.md_seq + (size_t)b * k.md_cap;
-    const int lom = WIN && w.model_window > 0 ? max(k.md_cnt[b] - w.model_window, 0) : 0;
+    const int lom = w.model_window > 0 ? max(k.md_cnt[b] - w.model_window, 0) : 0;
     last = 0;
     for (int c = 0; c < k.trToUse; ++c) {
         int best = -1;
@@ -336,20 +316,18 @@ __device__ inline int book_refresh(const LapBooks& k, int b, int nit, LapWindowR
 }
 
 // The selection of tables written from outside (lmpc_books_set): book_refresh of every controller.  One thread per controller.
-template <bool LAPS, bool WIN>
 __global__ void books_refresh_kernel(int batch, LapBooks k, SsLaps laps, LapWindows win) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b < batch) book_refresh<WIN>(k, b, book_laps<LAPS>(k, laps, b), book_windows<WIN>(win, b));
+    if (b < batch) book_refresh(k, b, ss_laps_of(laps, b, k.numSS_it), book_windows(win, b));
 }
 
 // Lap hand-over of every controller whose lap just ended (done[b] != 0), bookkeeping included: main.py:113-119
 // (lmpc.addTrajectory + predictiveModel.addTrajectory of the lap Simulator.sim returned), SysModel.py:50 (s -= TrackLength),
-// PC.py:445 (timeStep = 0).  One CTA per controller; no host involvement.  REPORTS: the running report row is filed as the lap's.
-// WIN: a lap-window table is installed.  LANE: a lane-rule table is installed; the lap's rows 0 .. Trec-1 are judged and an unsafe
+// PC.py:445 (timeStep = 0).  One CTA per controller; no host involvement.  Each table below is read only while it is installed.
+// Lap reports: the running report row is filed as the lap's.  Lane rules: the lap's rows 0 .. Trec-1 are judged and an unsafe
 // lap is filed with its lap time + LMPC_LANE_UNSAFE_KEY as its safe-set key (its report carries LMPC_REPORT_LANE_UNSAFE).
-// MARGIN: a lane-margin table is installed; under a mode 2 row the same rows adapt the margin m_b (margin_adapt, threshold 0), and
-// a margin that changed rewrites the controller's planning bx and invalidates its warm-start record.
-template <bool LAPS, bool REPORTS, bool WIN, bool LANE, bool MARGIN>
+// Lane margins: under a mode 2 row the same rows adapt the margin m_b (margin_adapt, threshold 0), and a margin that changed
+// rewrites the controller's planning bx and invalidates its warm-start record.
 __global__ void __launch_bounds__(256) commit_laps_books_kernel(int batch, LapPool ss, LapPool model, LapBooks k, const double* cl_x,
                                                                 const double* cl_u, int* cl_len, int Tcl, double* x_cur, int* timeStep,
                                                                 int* done, int* flags_or, Tracks trk, int lmpc, LapBudget retire,
@@ -360,8 +338,8 @@ __global__ void __launch_bounds__(256) commit_laps_books_kernel(int batch, LapPo
     __shared__ int s_ss, s_md;
     const int Trec = cl_len[b];
     const double TrackLength = trk.of(b).TrackLength;
-    const bool unsafe = lane_unsafe_block<LANE>(lane, b, cl_x + (size_t)b * Tcl * 6, Trec, 6);
-    if constexpr (MARGIN) {
+    const bool unsafe = lane_unsafe_block(lane, b, cl_x + (size_t)b * Tcl * 6, Trec, 6);
+    if (margin.rule.tab) {
         const LaneMarginRec r = margin.rule.of(b);
         if (r.mode == 2) {                                       // uniform over the block: no barrier is skipped by part of it
             const bool left = lane_leaves_block(margin.qp.of(b).c, cl_x + (size_t)b * Tcl * 6, Trec, 6, 0.0);
@@ -376,9 +354,9 @@ __global__ void __launch_bounds__(256) commit_laps_books_kernel(int batch, LapPo
         }
     }
     if (threadIdx.x == 0) {
-        const LapWindowRec w = book_windows<WIN>(win, b);
-        s_ss = lmpc ? book_ss_add<WIN>(k, b, lane_key(Trec, unsafe), false, book_laps<LAPS>(k, laps, b), w.ss_window) : -1;   // ordered by the lap time; rows beyond Tmax are not stored
-        s_md = book_md_add<WIN>(k, b, Trec, w.model_window);
+        const LapWindowRec w = book_windows(win, b);
+        s_ss = lmpc ? book_ss_add(k, b, lane_key(Trec, unsafe), false, ss_laps_of(laps, b, k.numSS_it), w.ss_window) : -1;   // ordered by the lap time; rows beyond Tmax are not stored
+        s_md = book_md_add(k, b, Trec, w.model_window);
         const int n = k.lap_n[b];
         if (n < LAP_HIST) k.lap_hist[(size_t)b * LAP_HIST + n] = Trec;
         k.lap_n[b] = n + 1;
@@ -390,10 +368,10 @@ __global__ void __launch_bounds__(256) commit_laps_books_kernel(int batch, LapPo
     if (s_md >= 0) copy_lap_block(model, model.lap_index(b, s_md), cx, cu, Trec);
     __syncthreads();
     if (threadIdx.x == 0) {
-        int f = book_refresh<WIN>(k, b, book_laps<LAPS>(k, laps, b), book_windows<WIN>(win, b));
+        int f = book_refresh(k, b, ss_laps_of(laps, b, k.numSS_it), book_windows(win, b));
         if (s_ss == -2) f |= 64;                                 // safe-set pool too small for numSS_it + 2 laps
         if (f && flags_or) flags_or[b] |= f;
-        if constexpr (REPORTS) {
+        if (rep.rows) {
             if (unsafe) rep.run[b].row.flags |= LMPC_REPORT_LANE_UNSAFE;
             report_file(rep, b);
         }
@@ -402,9 +380,8 @@ __global__ void __launch_bounds__(256) commit_laps_books_kernel(int batch, LapPo
 }
 
 // main.py:99-110 with device bookkeeping: the record every controller just drove becomes `copies` laps of both stores.
-// REPORTS: the report table starts afresh, like lap_n.  WIN: a lap-window table is installed.  LANE: a lane-rule table is
-// installed; the record is judged once and every copy is filed with the same key.
-template <bool LAPS, bool REPORTS, bool WIN, bool LANE>
+// With lap reports the report table starts afresh, like lap_n.  With lane rules the record is judged once and every copy is filed
+// with the same key.
 __global__ void __launch_bounds__(256) seed_books_kernel(int batch, LapPool ss, LapPool model, LapBooks k, int copies, const double* cl_x,
                                                          const double* cl_u, int* cl_len, int Tcl, int N, double* xLin, double* uLin,
                                                          double* zt, double* OldInput, int* timeStep, int* hasPred, int* done,
@@ -422,13 +399,13 @@ __global__ void __launch_bounds__(256) seed_books_kernel(int batch, LapPool ss, 
         for (int s = 0; s < k.md_cap; ++s) { k.md_seq[(size_t)b * k.md_cap + s] = -1; k.md_time[(size_t)b * k.md_cap + s] = 0x7fffffff; }
         k.it[b] = 0; k.md_cnt[b] = 0; k.lap_n[b] = 0;
     }
-    const bool unsafe = lane_unsafe_block<LANE>(lane, b, cx, Trec, 6);
+    const bool unsafe = lane_unsafe_block(lane, b, cx, Trec, 6);
     __syncthreads();
     for (int c = 0; c < copies; ++c) {
         if (threadIdx.x == 0) {
-            const LapWindowRec w = book_windows<WIN>(win, b);
-            s_ss = lmpc ? book_ss_add<WIN>(k, b, lane_key(Trec, unsafe), false, book_laps<LAPS>(k, laps, b), w.ss_window) : -1;
-            s_md = book_md_add<WIN>(k, b, Trec, w.model_window);
+            const LapWindowRec w = book_windows(win, b);
+            s_ss = lmpc ? book_ss_add(k, b, lane_key(Trec, unsafe), false, ss_laps_of(laps, b, k.numSS_it), w.ss_window) : -1;
+            s_md = book_md_add(k, b, Trec, w.model_window);
         }
         __syncthreads();
         if (s_ss >= 0) copy_ss_lap_block(ss, ss.lap_index(b, s_ss), cx, cu, Trec, TrackLength);
@@ -437,8 +414,8 @@ __global__ void __launch_bounds__(256) seed_books_kernel(int batch, LapPool ss, 
     }
     seed_state_block(b, N, shp, cx, cu, xLin, uLin, zt, OldInput);
     if (threadIdx.x == 0) {
-        book_refresh<WIN>(k, b, book_laps<LAPS>(k, laps, b), book_windows<WIN>(win, b)); timeStep[b] = 0; hasPred[b] = 0; cl_len[b] = 0; done[b] = 0;
-        if constexpr (REPORTS) report_restart(rep, b);
+        book_refresh(k, b, ss_laps_of(laps, b, k.numSS_it), book_windows(win, b)); timeStep[b] = 0; hasPred[b] = 0; cl_len[b] = 0; done[b] = 0;
+        if (rep.rows) report_restart(rep, b);
     }
 }
 
@@ -471,11 +448,11 @@ __device__ __forceinline__ int pool_group(const int* grp, int b) { return grp ? 
 // `min_over` rows past its finish line (rows - lap time; addPoint appends them during the next lap): an importer's safe-set
 // window near the finish reaches into those rows.  One CTA per group; k rounds of block arg-min over the group's controllers.
 // ship (null: every group) masks groups out of this export: a group with ship[g] == 0 chooses no controller, so
-// pool_export_kernel ships its kbest rows with global id -1 and importers file nothing of it.  LANE: a lane-rule table is
-// installed; a latest lap is ranked and tested by its lap time, its safe-set key without LMPC_LANE_UNSAFE_KEY.
-template <bool LANE>
+// pool_export_kernel ships its kbest rows with global id -1 and importers file nothing of it.  rules (null: none) is the lane-rule
+// table: with one, a latest lap is ranked and tested by its lap time, its safe-set key without LMPC_LANE_UNSAFE_KEY.
 __global__ void __launch_bounds__(1024) pool_local_best_kernel(int batch, LapPool ss, LapBooks k, int kbest, int Tpad, int min_over,
-                                                               const int* grp, const int* ship, int* best_inst) {
+                                                               const int* grp, const int* ship, int* best_inst,
+                                                               const LaneRuleRec* rules) {
     __shared__ unsigned long long red[32];
     __shared__ int taken[POOL_MAXK];
     const int g = blockIdx.x;
@@ -488,7 +465,7 @@ __global__ void __launch_bounds__(1024) pool_local_best_kernel(int batch, LapPoo
         for (int b = threadIdx.x; b < batch; b += blockDim.x) {
             const int sl = k.prevslot[b];
             if (sl < 0 || pool_group(grp, b) != g) continue;
-            const int t = lane_lap_time<LANE>(k.ss_time[(size_t)b * k.ss_cap + sl]);
+            const int t = lane_lap_time(k.ss_time[(size_t)b * k.ss_cap + sl], rules != nullptr);
             if (min_over > 0 && min(ss.len[ss.lap_index(b, sl)], Tpad) - t < min_over) continue;
             bool skip = false;
             for (int j = 0; j < r; ++j) skip |= (taken[j] == b);
@@ -509,10 +486,10 @@ __global__ void __launch_bounds__(1024) pool_local_best_kernel(int batch, LapPoo
 }
 
 // Pack the latest own lap of the chosen controllers into exchange rows rows[G][kbest][Tpad][XR_COLS], meta[G][kbest][4].
-// One CTA per row r = g * kbest + j.  LANE: meta[.,1] is the lap time, the safe-set key without LMPC_LANE_UNSAFE_KEY.
-template <bool LANE>
+// One CTA per row r = g * kbest + j.  With a lane-rule table (rules, null: none) meta[.,1] is the lap time, the safe-set key
+// without LMPC_LANE_UNSAFE_KEY.
 __global__ void __launch_bounds__(256) pool_export_kernel(LapPool ss, LapBooks k, const int* best_inst, int kbest, int Tpad,
-                                                          long long gid_base, double* rows, int* meta) {
+                                                          long long gid_base, double* rows, int* meta, const LaneRuleRec* rules) {
     const int r = blockIdx.x;
     const int b = best_inst[r];
     const int sl = b < 0 ? -1 : k.prevslot[b];
@@ -521,7 +498,7 @@ __global__ void __launch_bounds__(256) pool_export_kernel(LapPool ss, LapBooks k
     pack_lap_row_block(ss, lap, T, Tpad, rows + (size_t)r * Tpad * XR_COLS);
     if (threadIdx.x == 0) {
         meta[r * 4 + 0] = T;
-        meta[r * 4 + 1] = sl < 0 ? 0x7fffffff : lane_lap_time<LANE>(k.ss_time[(size_t)b * k.ss_cap + sl]);
+        meta[r * 4 + 1] = sl < 0 ? 0x7fffffff : lane_lap_time(k.ss_time[(size_t)b * k.ss_cap + sl], rules != nullptr);
         meta[r * 4 + 2] = sl < 0 ? -1 : (int)(gid_base + b);
         meta[r * 4 + 3] = r / kbest;
     }
@@ -557,11 +534,9 @@ __global__ void __launch_bounds__(64) pool_rank_kernel(int n_src, const int* met
 // is ordered by its lap time lt in both tables, as an own lap by Trec; only the rows that fit are stored.  The regression model
 // takes the lap also when the safe set drops it: main.py adds every lap to both lists, and with trToUse > numSS_it a lap outside
 // the numSS_it fastest can be among the trToUse shortest.  A controller with no lap of its own (it = 0) takes nothing.  The
-// importer ranks a lap against its own numSS_it (LAPS) and its own windows (WIN), so a group may mix lap counts and windows.
-// LANE: a lane-rule table is installed; the importer judges the shipped rows 0 .. min(lt, rows, Tpad)-1 against its own rule and
-// QP constants and files an unsafe lap with the safe-set key lt + LMPC_LANE_UNSAFE_KEY (the model takes lt).  One CTA per
-// controller.
-template <bool LAPS, bool WIN, bool LANE>
+// importer ranks a lap against its own numSS_it and its own windows, so a group may mix lap counts and windows.  With lane rules
+// the importer judges the shipped rows 0 .. min(lt, rows, Tpad)-1 against its own rule and QP constants and files an unsafe lap
+// with the safe-set key lt + LMPC_LANE_UNSAFE_KEY (the model takes lt).  One CTA per controller.
 __global__ void __launch_bounds__(256) pool_import_kernel(int batch, LapPool ss, LapPool model, LapBooks k, int share, int Tpad,
                                                           const double* rows, const int* meta, const int* grp, const int* order,
                                                           const int* cnt, long long gid_base, int* took, int* flags_or, SsLaps laps,
@@ -578,13 +553,13 @@ __global__ void __launch_bounds__(256) pool_import_kernel(int batch, LapPool ss,
         if (gid < 0 || len < 2) break;                            // nothing valid further down the ranking
         if ((long long)gid == gid_base + b) continue;             // its own lap
         ++given;
-        const bool unsafe = lane_unsafe_block<LANE>(lane, b, rows + (size_t)src * Tpad * XR_COLS, min(min(lt, len), Tpad), XR_COLS);
+        const bool unsafe = lane_unsafe_block(lane, b, rows + (size_t)src * Tpad * XR_COLS, min(min(lt, len), Tpad), XR_COLS);
         if (threadIdx.x == 0) {
             s_src = src;
-            const LapWindowRec w = book_windows<WIN>(win, b);
-            s_ss = book_ss_add<WIN>(k, b, lane_key(lt, unsafe), true, book_laps<LAPS>(k, laps, b), w.ss_window);
+            const LapWindowRec w = book_windows(win, b);
+            s_ss = book_ss_add(k, b, lane_key(lt, unsafe), true, ss_laps_of(laps, b, k.numSS_it), w.ss_window);
             s_md = -1;
-            if (s_ss != -2 && k.it[b] > 0) s_md = book_md_add<WIN>(k, b, lt, w.model_window);
+            if (s_ss != -2 && k.it[b] > 0) s_md = book_md_add(k, b, lt, w.model_window);
         }
         __syncthreads();
         const int c_ss = s_ss, c_md = s_md;                       // private copies: thread 0 rewrites the shared ones next round
@@ -595,7 +570,7 @@ __global__ void __launch_bounds__(256) pool_import_kernel(int batch, LapPool ss,
         __syncthreads();
         if (threadIdx.x == 0 && c_ss == -2 && flags_or) flags_or[b] |= 64;
     }
-    if (threadIdx.x == 0 && given > 0) book_refresh<WIN>(k, b, book_laps<LAPS>(k, laps, b), book_windows<WIN>(win, b));
+    if (threadIdx.x == 0 && given > 0) book_refresh(k, b, ss_laps_of(laps, b, k.numSS_it), book_windows(win, b));
 }
 
 // Progress of a Monte-Carlo batch in four numbers per pool group, so that the host only polls a few bytes every few steps:

@@ -539,14 +539,14 @@ static LapBudget lap_budget(const lmpc_handle* h) { return LapBudget{h->budget.i
 // LapSchedule{} (the table's own index)
 static LapSchedule lap_schedule(const lmpc_handle* h, int k) { return LapSchedule{h->sched[k].tab, h->sched_L[k], h->bk.lap_n}; }
 
-// The report buffers and the QP constants the kernels of the closed loop read (all null without reports: only the REPORTS
-// instantiations read them)
+// The report buffers and the QP constants the kernels of the closed loop read (all null without reports: the kernels then read
+// none of them)
 static LapReports reports(const lmpc_handle* h) {
     if (!h->rep_L) return LapReports{};
     return LapReports{h->d_rep_rows, h->d_rep_run, h->rep_L, h->sets.tab ? h->sets.view() : h->own_c.view()};
 }
 
-// The lane rules and the QP constants they judge against, as the lap-book kernels take them (only the LANE instantiations read them)
+// The lane rules and the QP constants they judge against, as the lap-book kernels take them (read only while a rule table is installed)
 static LaneRules lane_rules(const lmpc_handle* h) {
     return LaneRules{h->lrule.view(), h->sets.tab ? h->sets.view() : h->own_c.view()};
 }
@@ -558,8 +558,8 @@ static bool lane_rules_on(const lmpc_handle* h) {
 // Controller b's rule is on: its safe-set keys may carry LMPC_LANE_UNSAFE_KEY
 static bool lane_rule_of(const lmpc_handle* h, int b) { return h->lrule.tab && h->lrule.rows[h->lrule.index[b]].mode == 1; }
 
-// The lane margins, their untightened source rows and the planning rows, as the kernels take them (only the MARGIN instantiations
-// and lane_margin_rows_kernel read them)
+// The lane margins, their untightened source rows and the planning rows, as the kernels take them (read only while a margin table
+// is installed)
 static LaneMargins lane_margins(const lmpc_handle* h) {
     return LaneMargins{h->lmar.view(), h->sets.tab ? h->sets.view() : h->own_c.view(), h->d_plan, h->d_margin, h->d_warm_valid};
 }
@@ -1851,22 +1851,11 @@ static int measure(lmpc_handle* h, unsigned long long seed, LapBudget retire, La
     MeasArgs ma;
     ma.batch = h->batch; ma.x = h->d_rx[h->cur]; ma.y = h->d_xmeas; ma.seed = seed; ma.step = h->sim_step;
     ma.meas = h->meas.view(); ma.streams = h->streams.idx; ma.retire = retire;
-    (sched.rows ? measure_kernel<true> : measure_kernel<false>)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(ma, sched);
+    measure_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(ma, sched);
     CK(cudaGetLastError());
     h->launches += 1;
     *y = h->d_xmeas;
     return LMPC_OK;
-}
-
-// The instantiation of sim_step_kernel a step launches: lap reports, lap schedules (sched) and a surface table as installed
-using SimStepKernel = void (*)(const ModelConst, const SimArgs, const LapReports, const int*, const LapSchedule, const LapSchedule,
-                               const Table<lmpc_surface_params>, const LapSchedule);
-static SimStepKernel sim_step_launch(const lmpc_handle* h, bool sched) {
-    const bool rp = h->rep_L != 0, sf = h->surf.tab != nullptr;
-    if (sf) return rp ? (sched ? sim_step_kernel<true, true, true> : sim_step_kernel<true, false, true>)
-                      : (sched ? sim_step_kernel<false, true, true> : sim_step_kernel<false, false, true>);
-    return rp ? (sched ? sim_step_kernel<true, true, false> : sim_step_kernel<true, false, false>)
-              : (sched ? sim_step_kernel<false, true, false> : sim_step_kernel<false, false, false>);
 }
 
 // One closed-loop step for every instance, all on the device (SysModel.py:34-48):
@@ -1909,9 +1898,9 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
     SimArgs sa = sim_args(h, z_host ? h->d_z : nullptr, seed);                       // SysModel.py:40 (dynModel)
     sa.flags = h->d_flags; sa.status = q.status; sa.health = h->d_health; sa.retire = retire;
     if (h->meas.tab) sa.rec_x = y;
-    const LapSchedule vs = lap_schedule(h, LMPC_SCHEDULE_VEHICLE), ns = lap_schedule(h, LMPC_SCHEDULE_NOISE);
-    sim_step_launch(h, vs.rows || ns.rows)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(
-        h->mc, sa, reports(h), q.iters, vs, ns, h->surf.view(), lap_schedule(h, LMPC_SCHEDULE_SURFACE));
+    (h->surf.tab ? sim_step_kernel<true> : sim_step_kernel<false>)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(
+        h->mc, sa, reports(h), q.iters, lap_schedule(h, LMPC_SCHEDULE_VEHICLE), lap_schedule(h, LMPC_SCHEDULE_NOISE), h->surf.view(),
+        lap_schedule(h, LMPC_SCHEDULE_SURFACE));
     CK(cudaGetLastError());
     h->launches += 1;
     h->cur ^= 1;
@@ -1936,7 +1925,7 @@ int lmpc_rollout_pid_step(lmpc_handle* h, double vt, const double* z_pid_host, c
     SimArgs sa = sim_args(h, z_sim_host ? h->d_z : nullptr, seed);
     sa.health = h->d_health;          // no step flags or QP status here: only the simulator's own bits
     if (h->meas.tab) sa.rec_x = y;
-    sim_step_launch(h, false)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(
+    (h->surf.tab ? sim_step_kernel<true> : sim_step_kernel<false>)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(
         h->mc, sa, reports(h), nullptr, LapSchedule{}, LapSchedule{}, h->surf.view(), LapSchedule{});
     CK(cudaGetLastError());
     h->launches += 2;
@@ -2164,7 +2153,7 @@ int lmpc_rollout_seed_from_record(lmpc_handle* h, int copies, int ss_slot0, int 
         return fail(LMPC_E_INVALID, "seed copies do not fit the lap pools");
     h->laps_stored = true;
     if (h->d_warm_valid) CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * h->batch, h->stream));
-    (h->rep_L ? seed_from_record_kernel<true> : seed_from_record_kernel<false>)<<<h->batch, 256, 0, h->stream>>>(
+    seed_from_record_kernel<<<h->batch, 256, 0, h->stream>>>(
         h->batch, h->ss, h->mdl, copies, ss_slot0, model_slot0, h->d_clx, h->d_clu, h->d_cllen, h->Tcl, h->N, h->d_xLin, h->d_uLin,
         h->d_ztState, h->d_OldInput, h->d_timeStep, h->d_hasPred, h->d_done, tracks(h), h->shp.view(), reports(h));
     CK(cudaGetLastError());
@@ -2200,7 +2189,7 @@ int lmpc_rollout_commit_laps(lmpc_handle* h, const int* fin, const int* ss_slots
     CK(cudaMemcpyAsync(h->d_xchg, fin, sizeof(int) * B, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(h->d_xchg + B, ss_slots, sizeof(int) * B, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(h->d_xchg + 2 * B, model_slots, sizeof(int) * B, cudaMemcpyHostToDevice, h->stream));
-    (h->rep_L ? commit_laps_kernel<true> : commit_laps_kernel<false>)<<<h->batch, 256, 0, h->stream>>>(
+    commit_laps_kernel<<<h->batch, 256, 0, h->stream>>>(
         h->batch, h->ss, h->mdl, h->d_xchg, h->d_xchg + B, h->d_xchg + 2 * B, h->d_clx, h->d_clu, h->d_cllen, h->Tcl, h->d_rx[h->cur],
         h->d_timeStep, h->d_done, tracks(h), reports(h));
     CK(cudaGetLastError());
@@ -2298,21 +2287,6 @@ int lmpc_probe_fp64(int device, double* out8) {
 // ================================================================================================
 // device lap books (lapbooks.cuh): the reference's once-per-lap list bookkeeping without the host
 // ================================================================================================
-// The instantiation of a lap-book kernel for what the handle has installed: a lap-count table (LAPS), lap reports (REPORTS, the
-// kernels of BOOK_KERNEL3 only), a lap-window table (WIN) and a lane-rule table (LANE, always the last flag; books_refresh_kernel
-// has none).  BOOK_FLAG appends the flags w (and l) to the leading ones in __VA_ARGS__.
-#define BOOK_FLAG(K, w, ...) ((w) ? K<__VA_ARGS__, true> : K<__VA_ARGS__, false>)
-#define BOOK_FLAGS(K, w, l, ...) ((w) ? BOOK_FLAG(K, l, __VA_ARGS__, true) : BOOK_FLAG(K, l, __VA_ARGS__, false))
-#define BOOK_REFRESH(a, w) ((a) ? BOOK_FLAG(books_refresh_kernel, w, true) : BOOK_FLAG(books_refresh_kernel, w, false))
-#define BOOK_KERNEL2(K, a, w, l) ((a) ? BOOK_FLAGS(K, w, l, true) : BOOK_FLAGS(K, w, l, false))
-#define BOOK_KERNEL3(K, a, r, w, l)                                                                              \
-    ((a) ? ((r) ? BOOK_FLAGS(K, w, l, true, true) : BOOK_FLAGS(K, w, l, true, false))                            \
-         : ((r) ? BOOK_FLAGS(K, w, l, false, true) : BOOK_FLAGS(K, w, l, false, false)))
-// commit_laps_books_kernel: the flags of BOOK_KERNEL3 and a lane-margin table (MARGIN, its last flag)
-#define BOOK_FLAGS3(K, w, l, m, ...) ((w) ? BOOK_FLAGS(K, l, m, __VA_ARGS__, true) : BOOK_FLAGS(K, l, m, __VA_ARGS__, false))
-#define BOOK_COMMIT(a, r, w, l, m)                                                                                            \
-    ((a) ? ((r) ? BOOK_FLAGS3(commit_laps_books_kernel, w, l, m, true, true) : BOOK_FLAGS3(commit_laps_books_kernel, w, l, m, true, false)) \
-         : ((r) ? BOOK_FLAGS3(commit_laps_books_kernel, w, l, m, false, true) : BOOK_FLAGS3(commit_laps_books_kernel, w, l, m, false, false)))
 int lmpc_books_set(lmpc_handle* h, const int* ss_time, const int* ss_lap, const int* it, const int* md_time, const int* md_seq,
                    const int* md_cnt) {
     int rc = need_store(h);
@@ -2329,7 +2303,7 @@ int lmpc_books_set(lmpc_handle* h, const int* ss_time, const int* ss_lap, const 
         return rc;
     CK(cudaMemsetAsync(k.lap_n, 0, sizeof(int) * h->batch, h->stream));
     // sel, is_prev, prev_slot, used of these tables
-    BOOK_REFRESH(h->ssl.tab, h->lwin.tab)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->batch, k, h->ssl.view(), h->lwin.view());
+    books_refresh_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(h->batch, k, h->ssl.view(), h->lwin.view());
     CK(cudaGetLastError());
     h->launches += 1;
     CK(cudaStreamSynchronize(h->stream));
@@ -2353,7 +2327,7 @@ int lmpc_books_get(lmpc_handle* h, int* ss_time, int* ss_lap, int* it, int* md_t
 int lmpc_rollout_commit_laps_dev(lmpc_handle* h) {
     if (int rc = need_rollout(h)) return rc;
     h->laps_stored = true;     // enqueue only: which controllers finish a lap is not known here
-    BOOK_COMMIT(h->ssl.tab, h->rep_L, h->lwin.tab, h->lrule.tab, h->lmar.tab)<<<h->batch, 256, 0, h->stream>>>(
+    commit_laps_books_kernel<<<h->batch, 256, 0, h->stream>>>(
         h->batch, h->ss, h->mdl, h->bk, h->d_clx, h->d_clu, h->d_cllen, h->Tcl, h->d_rx[h->cur], h->d_timeStep, h->d_done, h->d_health,
         tracks(h), h->M > 0 ? 1 : 0, lap_budget(h), h->ssl.view(), reports(h), h->lwin.view(), lane_rules(h), lane_margins(h));
     CK(cudaGetLastError());
@@ -2366,7 +2340,7 @@ int lmpc_rollout_seed_from_record_dev(lmpc_handle* h, int copies) {
     if (copies < 1 || (h->M > 0 && copies > h->ss.cap) || copies > h->mdl.cap) return fail(LMPC_E_INVALID, "seed copies do not fit the lap pools");
     h->laps_stored = true;
     if (h->d_warm_valid) CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * h->batch, h->stream));
-    BOOK_KERNEL3(seed_books_kernel, h->ssl.tab, h->rep_L, h->lwin.tab, h->lrule.tab)<<<h->batch, 256, 0, h->stream>>>(
+    seed_books_kernel<<<h->batch, 256, 0, h->stream>>>(
         h->batch, h->ss, h->mdl, h->bk, copies, h->d_clx, h->d_clu, h->d_cllen, h->Tcl, h->N, h->d_xLin, h->d_uLin, h->d_ztState,
         h->d_OldInput, h->d_timeStep, h->d_hasPred, h->d_done, tracks(h), h->M > 0 ? 1 : 0, h->shp.view(), h->ssl.view(), reports(h),
         h->lwin.view(), lane_rules(h));
@@ -2415,10 +2389,9 @@ static int pool_export(lmpc_handle* h, const char* who, int kbest, int Tpad, lon
         ship = h->d_poolidx + POOL_SHIP;
         CK(cudaMemcpyAsync(ship, mask, sizeof(int) * G, cudaMemcpyHostToDevice, h->stream));
     }
-    (h->lrule.tab ? pool_local_best_kernel<true> : pool_local_best_kernel<false>)<<<G, 1024, 0, h->stream>>>(
-        h->batch, h->ss, h->bk, kbest, Tpad, h->pool_min_over, h->pool_grp.idx, ship, h->d_poolidx);
-    (h->lrule.tab ? pool_export_kernel<true> : pool_export_kernel<false>)<<<G * kbest, 256, 0, h->stream>>>(
-        h->ss, h->bk, h->d_poolidx, kbest, Tpad, gid_base, rows_dev, meta_dev);
+    pool_local_best_kernel<<<G, 1024, 0, h->stream>>>(h->batch, h->ss, h->bk, kbest, Tpad, h->pool_min_over, h->pool_grp.idx, ship,
+                                                      h->d_poolidx, h->lrule.tab);
+    pool_export_kernel<<<G * kbest, 256, 0, h->stream>>>(h->ss, h->bk, h->d_poolidx, kbest, Tpad, gid_base, rows_dev, meta_dev, h->lrule.tab);
     CK(cudaGetLastError());
     h->launches += 2;
     return LMPC_OK;
@@ -2457,7 +2430,7 @@ int lmpc_pool_import_dev(lmpc_handle* h, int n_src, int share, int Tpad, long lo
     int* took = h->d_poolidx + POOL_TOOK;
     CK(cudaMemsetAsync(took, 0, sizeof(int), h->stream));
     pool_rank_kernel<<<G, 64, 0, h->stream>>>(n_src, meta_dev, order, cnt);
-    BOOK_KERNEL2(pool_import_kernel, h->ssl.tab, h->lwin.tab, h->lrule.tab)<<<h->batch, 256, 0, h->stream>>>(
+    pool_import_kernel<<<h->batch, 256, 0, h->stream>>>(
         h->batch, h->ss, h->mdl, h->bk, share, Tpad, rows_dev, meta_dev, h->pool_grp.idx, order, cnt, gid_base, took,
         h->has_rollout ? h->d_health : nullptr, h->ssl.view(), h->lwin.view(), lane_rules(h));
     CK(cudaGetLastError());

@@ -55,7 +55,7 @@ __device__ __forceinline__ int ss_points_of(const Shapes& s, int b, int M) { ret
 
 // The safe-set lap count numSS_it_b of every controller (lmpc_set_ss_laps), or no table (tab == null) for the handle's numSS_it,
 // which stays the stride of sel / is_prev / min_index and K2's block size.  K2 takes SHAPED when either table is installed; the
-// lap-book kernels (lapbooks.cuh) have their own LAPS instantiation, so without a table both are the code they were before.
+// lap-book kernels (lapbooks.cuh) read the table through ss_laps_of.
 // The prediction model of every controller (lmpc_set_prediction_models), or no table (tab == null): the k-NN regression for all.
 // K1 takes NOMINAL when a table is installed and then skips the controllers of a nominal mode (nominal_model.cuh).
 using PredictionModelRec = lmpc_prediction_model_params;
@@ -66,8 +66,8 @@ using SsLaps = Table<SsLapsRec>;
 __device__ __forceinline__ int ss_laps_of(const SsLaps& l, int b, int nit) { return l.tab ? l.of(b).numSS_it : nit; }
 
 // Per-lap reports (lmpc_rollout_enable_lap_reports, DESIGN.md "Per-lap reports"): rows[B][L] filed at the lap hand-overs, and the
-// running row of the record under way with the count n of rows filed.  The kernels that touch them come in two instantiations,
-// REPORTS = reports are enabled: without them they are the code they were before reports existed.
+// running row of the record under way with the count n of rows filed.  Without reports every pointer is null and the kernels
+// that file reports test rows.
 struct LapRun {
     lmpc_lap_report row;
     int n, pad[3];
@@ -880,8 +880,7 @@ __global__ void __launch_bounds__(256) rollout_cost_kernel(LapPool pool, int b, 
 
 // Lap hand-over of every instance with fin[b] != 0, one CTA per instance (main.py:113-119 + SysModel.py:50 + PC.py:445):
 // the closed-loop record goes to safe-set slot ss_slot[b] (>= 0) with its cost-to-go and to regression slot model_slot[b]
-// (>= 0); then the record restarts (REPORTS: its running report row is filed first).
-template <bool REPORTS>
+// (>= 0); then the record restarts (with reports, its running report row is filed first).
 __global__ void __launch_bounds__(256) commit_laps_kernel(int batch, LapPool ss, LapPool model, const int* fin, const int* ss_slot,
                                                           const int* model_slot, const double* cl_x, const double* cl_u, int* cl_len,
                                                           int Tcl, double* x_cur, int* timeStep, int* done, Tracks trk, LapReports rep) {
@@ -894,7 +893,7 @@ __global__ void __launch_bounds__(256) commit_laps_kernel(int batch, LapPool ss,
     if (model_slot[b] >= 0) copy_lap_block(model, model.lap_index(b, model_slot[b]), cl_x + rec * 6, cl_u + rec * 2, Trec);
     __syncthreads();
     if (threadIdx.x == 0) {
-        if constexpr (REPORTS) report_file(rep, b);
+        if (rep.rows) report_file(rep, b);
         restart_record(b, cl_len, x_cur, timeStep, done, TrackLength);
     }
 }
@@ -1058,12 +1057,13 @@ __device__ __forceinline__ void surface_forces(SurfaceCursor& zc, double s, doub
     }
 }
 
-// REPORTS: the step is also added to the controller's running report row (report_step) with its QP's status a.status and
-// iterations rep_iters, both null for a PID step.  SCHED: the vehicle and noise rows come from the lap schedules veh_s and
-// noise_s (lap_schedule.cuh; either may be null).  SURF: each sub-step's peak tyre forces follow the controller's surface row of
-// surf, through the lap schedule surf_s (null: the table's own index).  The parameters after a are read only by those
-// instantiations.
-template <bool REPORTS, bool SCHED, bool SURF>
+// With reports (rep.rows) the step is also added to the controller's running report row (report_step) with its QP's status
+// a.status and iterations rep_iters, both null for a PID step.  The vehicle and noise rows come from the lap schedules veh_s and
+// noise_s (lap_schedule.cuh; a null schedule reads the table's own index).  SURF (a surface table is installed): each sub-step's
+// peak tyre forces follow the controller's surface row of surf, through the lap schedule surf_s; without one surf is not read.
+// Surfaces stay a template flag: a run-time test in the sub-step loop cost the table-free step 1.5 % per launch on an H100
+// (DESIGN.md, "Track surfaces").
+template <bool SURF>
 __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimArgs a, const LapReports rep, const int* rep_iters,
                                 const LapSchedule veh_s, const LapSchedule noise_s, const Table<lmpc_surface_params> surf,
                                 const LapSchedule surf_s) {
@@ -1080,7 +1080,7 @@ __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimA
         if (a.status && a.status[b] != 1) a.health[a.batch + b] += 1;
     }
     // vehicle parameters, SysModel.py:61-70
-    const lmpc_vehicle_params& v = SCHED ? veh_s.of(a.veh, b) : a.veh.of(b);
+    const lmpc_vehicle_params& v = veh_s.of(a.veh, b);
     const double mass = v.m, lf = v.lf, lr = v.lr, Iz = v.Iz;
     const double Df = v.Df, Cf = v.Cf, Bf = v.Bf;
     const double Dr = v.Dr, Cr = v.Cr, Br = v.Br;
@@ -1133,7 +1133,7 @@ __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimA
     }
     if (!okc) sim_bits |= SIM_LOOKUP_FAILED;
     if (a.health && sim_bits) a.health[b] |= sim_bits;
-    if constexpr (REPORTS) report_step(rep, b, x, (a.flags ? a.flags[b] : 0) | sim_bits, a.status, rep_iters);
+    if (rep.rows) report_step(rep, b, x, (a.flags ? a.flags[b] : 0) | sim_bits, a.status, rep_iters);
     double z0, z1, z2;
     if (a.z) {
         z0 = a.z[(size_t)b * 3]; z1 = a.z[(size_t)b * 3 + 1]; z2 = a.z[(size_t)b * 3 + 2];
@@ -1146,7 +1146,7 @@ __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimA
         z0 = n01.x; z1 = n01.y; z2 = n23.x;
     }
     // noise parameters, SysModel.py:139-145
-    const lmpc_noise_params& nz = SCHED ? noise_s.of(a.noise, b) : a.noise.of(b);
+    const lmpc_noise_params& nz = noise_s.of(a.noise, b);
     const double n_vx = fmax(-nz.sim_clip[0], fmin(z0 * nz.sim_sigma[0], nz.sim_clip[0]));
     const double n_vy = fmax(-nz.sim_clip[1], fmin(z1 * nz.sim_sigma[1], nz.sim_clip[1]));
     const double n_wz = fmax(-nz.sim_clip[2], fmin(z2 * nz.sim_sigma[2], nz.sim_clip[2]));
@@ -1203,7 +1203,8 @@ __global__ void pid_input_kernel(const PidArgs a) {
 // curvilinear channels, n_j = clip(z_j * sigma_j, +-clip_j) in the form of the process noise, z_j standard normal from Philox keyed
 // by (seed ^ K_MEAS, stream, clock) -- three curand_normal2_double calls, 12 raw 32-bit draws, in blocks of 16 per step.  Where
 // n_j == 0 the state is copied, so a zero set gives y == x bit for bit (-0.0 + 0.0 would be +0.0).  One thread per controller; a
-// retired controller draws nothing and writes nothing.  SCHED: the row comes from the lap schedule meas_s (lap_schedule.cuh).
+// retired controller draws nothing and writes nothing.  The row comes from the lap schedule meas_s (lap_schedule.cuh; a null
+// schedule reads the table's own index).
 constexpr unsigned long long K_MEAS = 0xD1B54A32D192ED03ull;     // distinct from the PID's key constant
 struct MeasArgs {
     int batch;
@@ -1214,7 +1215,6 @@ struct MeasArgs {
     const int* streams;                    // [B] Philox stream of every instance, or nullptr: b
     LapBudget retire;
 };
-template <bool SCHED>
 __global__ void measure_kernel(const MeasArgs a, const LapSchedule meas_s) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= a.batch || a.retire.retired(b)) return;
@@ -1225,7 +1225,7 @@ __global__ void measure_kernel(const MeasArgs a, const LapSchedule meas_s) {
     const double2 n23 = curand_normal2_double(&st);
     const double2 n45 = curand_normal2_double(&st);
     const double z[6] = {n01.x, n01.y, n23.x, n23.y, n45.x, n45.y};
-    const lmpc_measurement_params& m = SCHED ? meas_s.of(a.meas, b) : a.meas.of(b);
+    const lmpc_measurement_params& m = meas_s.of(a.meas, b);
     const double* x = a.x + (size_t)b * 6;
     double* y = a.y + (size_t)b * 6;
 #pragma unroll
@@ -1303,8 +1303,7 @@ __global__ void __launch_bounds__(32) ridge_sysid_kernel(int batch, const double
 // Seed a controller from the closed-loop record the way main.py:99-110 does from the PID lap: the record is stored `copies`
 // times in the safe set (slots ss_slot0 ..) and in the regression model (slots model_slot0 ..), cost-to-go by computeCost,
 // the controller state from the record (seed_state_block), timeStep = 0, no previous prediction; the record restarts.  One CTA
-// per instance.  REPORTS: the report table starts afresh.
-template <bool REPORTS>
+// per instance.  With reports the report table starts afresh.
 __global__ void __launch_bounds__(256) seed_from_record_kernel(int batch, LapPool ss, LapPool model, int copies, int ss_slot0, int model_slot0,
                                                               const double* cl_x, const double* cl_u, int* cl_len, int Tcl, int N,
                                                               double* xLin, double* uLin, double* zt, double* OldInput, int* timeStep,
@@ -1322,7 +1321,7 @@ __global__ void __launch_bounds__(256) seed_from_record_kernel(int batch, LapPoo
     seed_state_block(b, N, shp, cx, cu, xLin, uLin, zt, OldInput);
     if (threadIdx.x == 0) {
         timeStep[b] = 0; hasPred[b] = 0; cl_len[b] = 0; done[b] = 0;
-        if constexpr (REPORTS) report_restart(rep, b);
+        if (rep.rows) report_restart(rep, b);
     }
 }
 

@@ -1,4 +1,4 @@
-"""GPU tier: track surfaces (lmpc_rollout_set_surfaces, sim_step_kernel<..., SURF>, nominal_model_kernel<SURF>).
+"""GPU tier: track surfaces (lmpc_rollout_set_surfaces, sim_step_kernel, nominal_model_kernel).
 
 No table, an all-dry table, a 16-zone table with every mu = 1 and a removed table drive the same closed loop bit for bit (PID
 lap, seeding, three LMPC laps, lap reports, records), also with an all-learned prediction table; under mode 2 a dry row and
@@ -93,7 +93,7 @@ def test_neutral_tables_equal_no_table(models):
 
 
 def test_mode_2_under_a_dry_and_a_16_zone_mu_1_row_is_one_closed_loop():
-    """Both rows run the surface instantiation of the simulator and the nominal model, and neither changes a peak force."""
+    """Both rows run the surface path of the simulator and the nominal model, and neither changes a peak force."""
     _need_gpu()
     B = 64
     pm = ([P.plant(), P.learned()], np.arange(B) % 2)

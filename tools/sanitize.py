@@ -6,7 +6,7 @@ ss_add_point, rollout_cost, sim_step (with noise sets and noise streams), measur
 that reads its model in place (N = 48), warm-started solves, pid_input, seed_books, commit_laps_books, rollout_stats, the pooled
 exchange (pool_local_best / export / rank / import), trace_step and track_global_position, and a controller made
 non-finite in the closed loop (ss_select on a NaN terminal guess, ss_add_point refusing the point), all with per-lap reports on
-(the report instantiations of sim_step, seed_books and commit_laps_books, lap_reports_reset)."""
+(the report paths of sim_step, seed_books and commit_laps_books, lap_reports_reset)."""
 import os
 import sys
 import numpy as np
@@ -70,7 +70,7 @@ c = BatchedController(par, B, workloads.track_seg_table(), rp.TRACK_LENGTH, trTo
                       numSS_it=numSS_it, QterminalSlack=Qts, Tmax=1280, ss_cap=7, model_cap=5, warm_start=True)
 xs = np.tile(np.array([0.5, 0, 0, 0, 0, 0.0]), (B, 1))
 c.enable_rollout(Tcl=1024)
-c.enable_lap_reports(2)                              # per-lap reports: the report instantiations of the step, hand-over and seeding
+c.enable_lap_reports(2)                              # per-lap reports: the report paths of the step, hand-over and seeding
 c.rollout_set_state(xs, xs)
 c.set_measurement_noise([rp.MeasurementParams((0.01,) * 6, (0.05,) * 6)], np.zeros(B, np.int32))   # the PID lap measures too
 for _ in range(int(os.environ.get("SANITIZE_PID_STEPS", "1000"))):

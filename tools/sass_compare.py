@@ -4,18 +4,16 @@
 Kernels are matched by variant and (N, M) across their old and new names:
   uniform  ftocp_kernel<N, M, 2, 4>  or  ftocp_kernel<N, M, 2, 4, false>
   sets     ftocp_sets_kernel<N, M, 2, 4>  or  ftocp_kernel<N, M, 2, 4, true>
-and the instantiations that run without a per-controller table of the other kernels of a step and of the lap books, matched
-across their untemplated names:
+and the other kernels of a step and of the lap books, each matched by its name with or without a template argument list of up
+to five `false` flags, so that the instantiation without a per-controller table of an older build meets the untemplated kernel:
   default  knn_ltv_regress_kernel, ss_select_kernel, shift_state_kernel (<false>: no shape or lap-count table),
-           books_refresh_kernel, commit_laps_books_kernel, seed_books_kernel, pool_import_kernel (<false>: no lap-count table;
-           <false, false>: no lap-count table and no lap-window table; <false, false, false>: no lap-count table, no lap-window
-           table and no lane-rule table; <false, false, false, false>: no lap-count table, no lap reports, no lap-window table and
-           no lane-rule table; <false, false, false, false, false>: the same and no lane-margin table), pool_local_best_kernel, pool_export_kernel (<false>: no lane-rule table), commit_laps_kernel,
-           seed_from_record_kernel
-           (<false>: no lap reports), sim_step_kernel (<false>, <false, false> or <false, false, false>: no lap reports, no lap
-           schedule and no surface table), measure_kernel (<false>: no lap schedule) and nominal_model_kernel (<false>: no
-           surface table)
-  reports  sim_step_kernel<true>, <true, false> or <true, false, false>: lap reports, no lap schedule and no surface table
+           books_refresh_kernel, commit_laps_books_kernel, seed_books_kernel, pool_import_kernel, pool_local_best_kernel,
+           pool_export_kernel, commit_laps_kernel, seed_from_record_kernel and measure_kernel (untemplated; older builds had one
+           flag per table they read: lap counts, lap reports, lap windows, lane rules, lane margins, lap schedules),
+           sim_step_kernel and nominal_model_kernel (<false>: no surface table; older builds: <false, false> or
+           <false, false, false>, no lap reports, no lap schedule and no surface table)
+  reports  sim_step_kernel<true, false> or <true, false, false> of an older build: lap reports, no lap schedule and no surface
+           table (later builds have no such kernel: their sim_step_kernel<true> is the surface instantiation)
 and compared by instruction text (cuobjdump -sass without addresses and encodings).  Each differing line pair is classified:
   dfma-swap   one DFMA with its two factors exchanged (a*b+c = b*a+c)
   lds-swap    LDS.128 loads of unchanged addresses whose destination registers are permuted among themselves
@@ -35,7 +33,7 @@ DEFAULT = re.compile(r"^(?:void )?lmpc::(knn_ltv_regress_kernel|ss_select_kernel
                      r"commit_laps_books_kernel|seed_books_kernel|pool_import_kernel|sim_step_kernel|commit_laps_kernel|"
                      r"seed_from_record_kernel|measure_kernel|pool_local_best_kernel|pool_export_kernel|nominal_model_kernel)"
                      r"(<false>|<false, false>|<false, false, false>|<false, false, false, false>|<false, false, false, false, false>)?\(")
-REPORTS = re.compile(r"^(?:void )?lmpc::(sim_step_kernel)<true(?:, false){0,2}>\(")
+REPORTS = re.compile(r"^(?:void )?lmpc::(sim_step_kernel)<true(?:, false){1,2}>\(")
 
 
 def kernels(path):
