@@ -23,6 +23,7 @@ exchanges once its own slowest controller is `ship_after` steps into lap r+1 (th
 Prints one JSON line (rank 0): closed-loop steps/s over all GPUs (device events, max over ranks), lap-length statistics per
 LMPC lap, exchange time and bytes."""
 import argparse
+import collections
 import ctypes as C
 import json
 import os
@@ -130,6 +131,102 @@ def lap_row_summary(reps, schedules, laps):
     return out
 
 
+def _by_index(make, *extra):
+    """The pack step of a table installed from (rows, index): make(rows, index, batch, *extra)."""
+    return lambda ctx, rows, index=None: make(rows, index, ctx["B"], *extra)
+
+
+def _pack_params(ctx, params, index=None, QterminalSlack=None):
+    rows, idx = _native.make_param_sets(ctx["params"], params, index, ctx["B"], ctx["M"], ctx["numSS_it"], QterminalSlack)
+    ctx["bx_min"] = np.array([min(r.bx[:r.ncx]) for r in rows])[idx]
+    return rows, idx
+
+
+def _pack_shapes(ctx, shapes, index=None):
+    if ctx["warm"]:
+        raise ValueError("shape_sets and warm start: the warm-start record is laid out per (N, numSS_Points)")
+    rows, idx = _native.make_shape_sets(shapes, index, ctx["B"], ctx["N"], ctx["M"], ctx["numSS_it"])
+    ctx["points"] = [rows[k].numSS_Points for k in idx]
+    return rows, idx
+
+
+def _pack_ss_laps(ctx, values, index=None):
+    rows, idx = _native.make_ss_laps_sets(values, index, ctx["B"], ctx["numSS_it"], ctx["points"])
+    ctx["laps_of"] = [rows[k].numSS_it for k in idx]
+    return rows, idx
+
+
+# One table argument of run(): its keyword, its name in messages, the BatchedController method that installs it, the result key of
+# its per-row statistics (or None), the row fields copied into each per-row entry and whether that entry gets the row's sampled
+# interior-point iterations, pack(ctx, *install arguments) -> (rows, index) (rows None for the integer tables: streams, groups),
+# and args(value) -> the install arguments.
+Table = collections.namedtuple("Table", "keyword name install key fields ipm pack args", defaults=(tuple,))
+
+# every table in install order: the margins need the parameter rows' lanes, the windows the lap counts
+TABLES = (
+    Table("param_sets", "parameter sets", "set_param_sets", "per_set_rank0", (), False, _pack_params),
+    Table("vehicle_sets", "vehicles", "set_vehicles", "per_vehicle_rank0", (), False, _by_index(_native.make_vehicle_sets)),
+    Table("noise_sets", "noise sets", "set_noise", "per_noise_rank0", (), False, _by_index(_native.make_noise_sets)),
+    Table("noise_streams", "noise streams", "set_noise_streams", None, (), False,
+          lambda ctx, streams: (None, _native.make_noise_streams(streams, ctx["B"])), lambda streams: (streams,)),
+    Table("measurement_sets", "measurement sets", "set_measurement_noise", "per_measurement_rank0", (), False,
+          _by_index(_native.make_measurement_sets)),
+    Table("regression_sets", "regression sets", "set_regression", "per_regression_rank0", (), False,
+          _by_index(_native.make_regression_sets, TR_TO_USE)),
+    Table("track_sets", "tracks", "set_tracks", "per_track_rank0", (), False, _by_index(_native.make_track_sets)),
+    Table("pool_groups", "pool groups", "set_pool_groups", None, (), False,
+          lambda ctx, index, ngroups: (None, _native.make_pool_groups(index, ngroups, ctx["B"]))),
+    Table("shape_sets", "shapes", "set_shapes", "per_shape_rank0", ("N", "numSS_Points"), True, _pack_shapes),
+    Table("ss_laps_sets", "lap counts", "set_ss_laps", "per_ss_laps_rank0", ("numSS_it",), True, _pack_ss_laps),
+    Table("lap_window_sets", "lap windows", "set_lap_windows", "per_lap_window_rank0", ("ss_window", "model_window"), True,
+          lambda ctx, windows, index=None: _native.make_lap_window_sets(windows, index, ctx["B"], ctx["laps_of"], SS_CAP, TR_TO_USE,
+                                                                        MODEL_CAP)),
+    Table("lane_rule_sets", "lane rules", "set_lane_rules", "per_lane_rule_rank0", ("mode", "lane_tol"), True,
+          _by_index(_native.make_lane_rule_sets, True, TCL)),
+    Table("lane_margin_sets", "lane margins", "set_lane_margins", "per_lane_margin_rank0",
+          ("mode", "margin0", "margin_max", "step_up", "step_down"), True,
+          lambda ctx, margins, index=None: _native.make_lane_margin_sets(margins, index, ctx["B"], ctx["bx_min"])),
+    Table("prediction_model_sets", "prediction models", "set_prediction_models", "per_prediction_model_rank0", ("mode",), False,
+          _by_index(_native.make_prediction_model_sets)),
+    Table("surface_sets", "surfaces", "set_surfaces", "per_surface_rank0", (), False, _by_index(_native.make_surface_sets)),
+)
+
+
+def pack_tables(batch, warm=False, **given):
+    """Packs every table of `given` ({keyword: run() argument}, None for none) on the host, in install order, with the
+    _native.make_* call and the arguments its install in run() will use, so it raises that call's ValueError before any device
+    work.  Returns ({keyword: (rows, index)} of the given tables, ctx): ctx holds the handle's (N, M) and numSS_it (handle_shape)
+    and what later tables take from earlier ones, every controller's numSS_Points ("points"), numSS_it ("laps_of") and min_i
+    bx_i of its QP row ("bx_min")."""
+    B = int(batch)
+    N, M = handle_shape(given.get("shape_sets"))
+    numSS_it, _, _, _, Qts, par = rp.lmpc_params(N)
+    base = _native.make_params(par, M, numSS_it, Qts, warm_start=warm)            # the Params row run()'s handle is created with
+    ctx = dict(B=B, N=N, M=M, numSS_it=numSS_it, warm=bool(warm), params=base, points=[M] * B, laps_of=[numSS_it] * B,
+               bx_min=np.full(B, min(base.bx[:base.ncx])))
+    packed = {}
+    for t in TABLES:
+        if given.get(t.keyword) is not None:
+            packed[t.keyword] = t.pack(ctx, *t.args(given[t.keyword]))
+    return packed, ctx
+
+
+def table_rows(packed):
+    """What capture records of the tables (pack_tables' first result): {keyword: every controller's row, controller by controller,
+    as the bytes the library is given}, the int32 values for streams and groups."""
+    return {k: idx.tobytes() if rows is None else np.frombuffer(rows, np.uint8).reshape(len(rows), -1)[idx].tobytes()
+            for k, (rows, idx) in packed.items()}
+
+
+def check_start_tables(had, mine):
+    """start's refusal of other tables: `had` the captured table_rows, `mine` this run's.  No table is part of a record, and the
+    records were learned under the rows installed when they were captured."""
+    for t in TABLES:
+        if had.get(t.keyword) != mine.get(t.keyword):
+            raise ValueError("start was captured with other %s: a record resumes exactly only under the tables it was captured with"
+                             % t.name)
+
+
 def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, poll=8, max_steps=0, seed=1234, local=None, warm=False,
         final=None, param_sets=None, vehicle_sets=None, books=None, track_sets=None, pool_groups=None, readiness="batch",
         capture=None, start=None, noise_sets=None, noise_streams=None, regression_sets=None, lap_budget=None, measurement_sets=None,
@@ -140,44 +237,55 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     books: None, or a dict that receives the lap books (books) and the health counters (flags_or, unsolved), and with lap_reports
     the reports (BatchedController.lap_reports) under "lap_reports", and with lane_margin_sets every controller's final margin under
     "lane_margins".
-    param_sets: None, or (params, index, QterminalSlack) handed to BatchedController.set_param_sets after construction (a
-    parameter sweep over the batch; the result then holds per-set lap statistics under "per_set_rank0").
-    vehicle_sets: None, or (vehicles, index) handed to BatchedController.set_vehicles (a sweep over the plant, PID lap included; the
-    result then holds per-vehicle lap statistics under "per_vehicle_rank0").  The pooled mode exchanges laps between the
-    controllers of a pool group whatever their car, so a pooled plant sweep groups by car (pool_groups).
-    track_sets: None, or (tracks, index) handed to BatchedController.set_tracks (several circuits in one batch; the result then
-    holds per-track lap statistics under "per_track_rank0").  A lap of another circuit is not a trajectory of this one, so the
-    pooled mode with more than one track needs pool_groups in which every group drives one circuit (ValueError otherwise,
-    raised before any device work or collective).
-    noise_sets: None, or (noises, index) handed to BatchedController.set_noise (a sweep over the simulator's and the PID's noise,
-    PID lap included; the result then holds per-noise-set lap statistics under "per_noise_rank0").
-    noise_streams: None, or the [batch] stream numbers handed to BatchedController.set_noise_streams (common random numbers:
-    controllers on one stream meet the same draws).  Streams are local to a rank: every rank keys its Philox draws with its own
-    seed (seed + rank), so controllers pair only with controllers of their own rank.
-    measurement_sets: None, or (meas, index) handed to BatchedController.set_measurement_noise (a sweep over the sensor noise the
-    controllers see, PID lap included: its record, and so the seeded stores, are measured data; the result then holds
-    per-measurement-set lap statistics under "per_measurement_rank0").  The measurement draws pair on noise_streams like the others.
-    regression_sets: None, or (regs, index) handed to BatchedController.set_regression (a sweep over the learned model's
-    bandwidth, neighbour count, ridge, feature scaling and laps used, trToUse up to the store's 4; the result then holds
-    per-regression-set lap statistics under "per_regression_rank0").  The pooled mode exchanges laps whatever the model setting:
-    a lap driven under another setting is still a trajectory of this car on this circuit.
-    shape_sets: None, or (shapes, index) handed to BatchedController.set_shapes: (N, numSS_Points) pairs of the instantiated grid
-    (a horizon / safe-set size sweep in one batch; the result then holds per-shape lap statistics under "per_shape_rank0").  The
-    handle is created at handle_shape(shape_sets), the smallest grid pair that dominates every shape (ValueError before any device
-    work when there is none, or where set_shapes would refuse a shape).  A shape equal to the handle's (12, 48) runs the shaped
-    QP kernel with the reference's parameters.
-    ss_laps_sets: None, or (values, index) handed to BatchedController.set_ss_laps: numSS_it per controller, 1 .. the handle's 4
-    (how to split the safe set between laps and points per lap in one batch; the result then holds per-value lap statistics and
-    mean interior-point iterations under "per_ss_laps_rank0").  Every controller's numSS_Points (its shape, or the handle's) must be
-    its value times an even number of points per lap.  ValueError before any device work where set_ss_laps would refuse.  The
-    seeding stores 4 copies of the PID lap whatever the value (main.py:103-110).  The pooled mode ranks an import against the
-    importer's own value, so pool groups may mix values.  With shape_sets as well, the result also holds the statistics of every
-    (shape, value) cell under "per_shape_ss_laps_rank0".
-    pool_groups: None, or (index, G) handed to BatchedController.set_pool_groups (e.g. sharding.design_groups(track index,
-    parameter-set index)): the pooled mode then exchanges laps within each group; the exchange buffers hold G * (share + 1) laps
-    per rank and the result holds the laps filed per group under "laps_filed_per_group_rank0" (stored laps counted from the books;
-    too low for a controller with health flag 64).  A lap ships only once it has `ship_after` rows past its finish line
-    (lmpc_set_pool_min_overrun), so a group lapping faster ships the fastest of its laps that qualify.
+    The table arguments below (TABLES, in install order) are each None or the arguments of their BatchedController install,
+    called after enable_rollout, before the PID lap.  Before any device work every given table is packed with the call its install
+    uses (pack_tables), so a row or an index the install would refuse raises its ValueError first.  capture records every
+    installed table under "tables" ({keyword: every controller's packed row}, table_rows), and start refuses a start whose tables
+    or rows differ: no table is part of a record, and a record resumes exactly only under the tables it was captured with.  A table
+    with a result key adds one entry per row: the lap statistics of its controllers (_set_stats), its row fields and, for some,
+    their mean interior-point iterations sampled at the polls (table_stats).
+    param_sets: (params, index, QterminalSlack) for set_param_sets (a parameter sweep over the batch); "per_set_rank0".
+    vehicle_sets: (vehicles, index) for set_vehicles (a sweep over the plant, PID lap included); "per_vehicle_rank0".  The pooled
+    mode exchanges laps between the controllers of a pool group whatever their car, so a pooled plant sweep groups by car.
+    noise_sets: (noises, index) for set_noise (the simulator's and the PID's noise, PID lap included); "per_noise_rank0".
+    noise_streams: the [batch] stream numbers for set_noise_streams (common random numbers: controllers on one stream meet the same
+    draws).  Streams are local to a rank: every rank keys its Philox draws with its own seed (seed + rank).
+    measurement_sets: (meas, index) for set_measurement_noise (the sensor noise the controllers see, PID lap included: its record,
+    and so the seeded stores, are measured data); "per_measurement_rank0".  The draws pair on noise_streams like the others.
+    regression_sets: (regs, index) for set_regression (the learned model's bandwidth, neighbour count, ridge, feature scaling and
+    laps used, trToUse up to the store's 4); "per_regression_rank0".  The pooled mode exchanges laps whatever the model setting.
+    track_sets: (tracks, index) for set_tracks (several circuits in one batch); "per_track_rank0".  A lap of another circuit is not
+    a trajectory of this one, so the pooled mode with more than one track needs pool_groups in which every group drives one
+    circuit.
+    pool_groups: (index, G) for set_pool_groups (e.g. sharding.design_groups(track index, parameter-set index)): the pooled mode
+    then exchanges laps within each group; the exchange buffers hold G * (share + 1) laps per rank and the result holds the laps
+    filed per group under "laps_filed_per_group_rank0" (stored laps counted from the books; too low for a controller with health
+    flag 64).  A lap ships only once it has `ship_after` rows past its finish line (lmpc_set_pool_min_overrun), so a group lapping
+    faster ships the fastest of its laps that qualify.
+    shape_sets: (shapes, index) for set_shapes: (N, numSS_Points) pairs of the instantiated grid (a horizon / safe-set size sweep);
+    "per_shape_rank0" with N, numSS_Points and the sampled iterations.  The handle is created at handle_shape(shape_sets), the
+    smallest grid pair that dominates every shape (ValueError when there is none, or with warm start); the result then holds it
+    under "handle_shape".
+    ss_laps_sets: (values, index) for set_ss_laps: numSS_it per controller, 1 .. the handle's 4, and every controller's
+    numSS_Points its value times an even number of points per lap; "per_ss_laps_rank0" with numSS_it and the sampled iterations.
+    With shape_sets as well, "per_shape_ss_laps_rank0" holds the statistics of every (shape, value) cell.
+    lap_window_sets: (windows, index) for set_lap_windows: ss_window (0 or the controller's numSS_it .. ss_cap 7) and model_window
+    (0 or trToUse 4 .. model_cap 5), 0 = unbounded (controllers that trust only their most recent laps); "per_lap_window_rank0"
+    with both windows and the sampled iterations.
+    lane_rule_sets: (rules, index) for set_lane_rules: mode (0: the reference's ranking, 1: a lap that left the lane by more than
+    lane_tol ranks behind every lap that kept to it) and lane_tol; "per_lane_rule_rank0" with both and the sampled iterations.
+    With lap reports the share of laps judged lane-unsafe per lap is added to every lap_reports_rank0 row and every per-rule report
+    row ("lane_unsafe_share"), and "lane_unsafe_selected_share_rank0" is the share of controllers whose final selection holds a
+    lane-unsafe lap.
+    lane_margin_sets: (margins, index) for set_lane_margins: mode (0: none, 1: the fixed margin0, 2: adapted lap by lap within
+    [margin0, margin_max] by step_up / step_down) that narrow the lane every QP plans in while reports and lane rules judge the
+    given lane; "per_lane_margin_rank0" with the row's five values and the sampled iterations, and per row the min / mean / max
+    of the final margins under "lane_margin_final_rank0".
+    prediction_model_sets: (models, index) for set_prediction_models: mode (0: the learned k-NN model, 1: the exact linearisation
+    of their vehicle, 2: that of the plant's own vehicle row, through its lap schedule) and vehicle.  Needs lap_reports >= laps;
+    "per_prediction_model_rank0" with the mode and the per-lap reports.
+    surface_sets: (surfaces, index) for set_surfaces (friction zones along the circuit, PID lap included); "per_surface_rank0".
+    The pooled mode exchanges laps whatever the surface, so a clean pooled surface study puts each surface in its own pool group.
     readiness: when the pooled mode exchanges round r (sharding.ready_groups at every poll, agreed over the ranks).
       "batch"  every group together, once the slowest controller of the whole batch is `ship_after` steps into lap r + 1;
       "group"  each pool group on its own round counter, once the slowest controller of that group is; one export / all-gather /
@@ -190,18 +298,16 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     capture: None, or a dict that receives, at the end of the run, everything a later run needs to go on from here: "records"
     (every controller's snapshot record, a uint8 CUDA tensor), "clock" (the simulator step that keys the Philox noise), the loop's
     scheduler state ("steps", "next_round", "next_rounds", the groups that exchanged at the last poll, the exchange steps so far)
-    and what it has to match (batch, laps, mode, readiness, poll, warm, pool groups, record layout).  torch.save stores it.
+    and what it has to match (batch, laps, mode, readiness, poll, warm, pool groups, record layout, tables).  torch.save stores it.
     "diverged_step" is None unless, under group readiness, some group was ready for a round >= laps before the last poll: a
     longer run exchanged there and this one did not, so a resumed run cannot equal it (the result of that resumed run says so
     under "resume_exact").
     start: None, or a capture dict: instead of the PID lap and the seeding, every controller is restored from its record, the
     clock and the scheduler state are set, and the run first repeats the poll the capture was taken at, under the new `laps`
     (groups that exchanged at that poll are not exchanged again), then steps on.  A run to 3 laps captured and resumed to 5
-    therefore equals a run to 5 laps bit for bit (books, end states, health, exchange steps).  Tables (param_sets, vehicle_sets,
-    noise_sets, noise_streams, measurement_sets, regression_sets, track_sets, pool_groups, shape_sets, ss_laps_sets) are installed
-    from the arguments, as for a fresh run; restore a record into a controller of the value it was captured with.  ValueError before any device work when start
-    does not match the batch, the layout, the mode, the readiness, the poll interval or the pool groups, or when laps is not
-    above the captured laps.
+    therefore equals a run to 5 laps bit for bit (books, end states, health, exchange steps).  ValueError before any device work
+    when start does not match the batch, the layout, the mode, the readiness, the poll interval, the pool groups or the tables,
+    or when laps is not above the captured laps.
     lap_budget: None (every controller is stepped until the slowest has its laps), or the laps every controller drives before it
     retires, one integer or [batch] (BatchedController.set_lap_budget, installed after the seeding or the restore).  A retired
     controller costs no kernel time and keeps the state its last hand-over left it in, so with lap_budget = laps a controller ends
@@ -226,103 +332,42 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     run needs lap_reports >= laps.  The result gains "per_lap_row_rank0": per kind, lap and row, the controllers on that row, their
     mean steps, the share with a lane violation and the unsolved QPs (lap_row_summary).  capture records the schedules and start
     refuses others.  ValueError before any device work.
-    lap_window_sets: None, or (windows, index) handed to BatchedController.set_lap_windows with the other tables, before the PID
-    lap: objects with ss_window (0 or the controller's numSS_it .. ss_cap 7) and model_window (0 or trToUse 4 .. model_cap 5), 0
-    = unbounded (controllers that trust only their most recent laps).  The result then holds per-window lap statistics and mean
-    interior-point iterations under "per_lap_window_rank0".  capture records every controller's windows and start refuses others.
-    ValueError before any device work where set_lap_windows would refuse.
-    lane_rule_sets: None, or (rules, index) handed to BatchedController.set_lane_rules with the other tables, before the PID lap:
-    objects with mode (0: the reference's ranking, 1: a lap that left the lane by more than lane_tol ranks behind every lap that kept
-    to it) and lane_tol.  The result then holds per-rule lap statistics and mean interior-point iterations under
-    "per_lane_rule_rank0", with lap reports the share of laps judged lane-unsafe per lap ("lane_unsafe_share" of every
-    lap_reports_rank0 row and of every per-rule report row), and "lane_unsafe_selected_share_rank0": the share of controllers whose
-    final selection holds a lane-unsafe lap.  capture records every controller's rule and start refuses others.  ValueError before
-    any device work where set_lane_rules would refuse.
-    lane_margin_sets: None, or (margins, index) handed to BatchedController.set_lane_margins after the other tables, before the PID
-    lap: objects with mode (0: none, 1: the fixed margin0, 2: adapted lap by lap within [margin0, margin_max] by step_up /
-    step_down) that narrow the lane every QP plans in while reports and lane rules judge the given lane.  The result then holds
-    per-row lap statistics (with lap reports, the per-lap lane-violation share) and mean interior-point iterations under
-    "per_lane_margin_rank0", and per row the min / mean / max of the final margins under "lane_margin_final_rank0".  capture
-    records every controller's row and start refuses others.  ValueError before any device work where set_lane_margins would
-    refuse.
-    prediction_model_sets: None, or (models, index) handed to BatchedController.set_prediction_models with the other tables, before
-    the PID lap: objects with mode (0: the learned k-NN model, 1: the exact linearisation of their vehicle, 2: that of the plant's
-    own vehicle row, through its lap schedule) and vehicle.  Needs lap_reports >= laps.  The result then holds, per row, its lap
-    statistics with the per-lap reports (controllers, mean steps, the share with a lane violation, unsolved QPs) under
-    "per_prediction_model_rank0".  capture records every controller's row and start refuses others.  ValueError before any device
-    work where set_prediction_models would refuse.
-    surface_sets: None, or (surfaces, index) handed to BatchedController.set_surfaces with the other tables, before the PID lap
-    (friction zones along the circuit, PID lap included; the result then holds per-surface lap statistics under
-    "per_surface_rank0").  lap_schedules={"surface": rows} switches rows at the laps.  The pooled mode exchanges laps whatever the
-    surface, so a clean pooled surface study puts each surface in its own pool group.  ValueError before any device work where
-    set_surfaces would refuse.
     trace: None, or a dict with "inst" (controller numbers) and "cap" (rows per controller): those controllers' LMPC steps are
     traced (lmpc_rollout_trace_create, after the seeding) and the dict receives per traced controller "steps" and the arrays "x"
     [cap, 6] (the plant state the step started from), "xPred" [cap, N+1, 6] and "lap" [cap]."""
+    arguments = dict(locals())                                     # run()'s arguments, before any other name is bound
+    given = {t.keyword: arguments[t.keyword] for t in TABLES}
     L = check_lap_reports(lap_reports, laps)
-    if surface_sets is not None:                                   # ValueError where set_surfaces would refuse
-        _native.make_surface_sets(surface_sets[0], surface_sets[1], int(batch))
-    scheds = check_lap_schedules(lap_schedules, batch, L, {"vehicle": vehicle_sets, "noise": noise_sets,
-                                                           "measurement": measurement_sets, "surface": surface_sets})
+    packed, ctx = pack_tables(batch, warm, **given)
+    # the rules between tables
+    if "prediction_model_sets" in packed and not L:
+        raise ValueError("prediction_model_sets needs lap_reports >= laps: the per-row summary is taken from the lap reports")
+    if "track_sets" in packed and mode == "pooled" and len(packed["track_sets"][0]) > 1:
+        if "pool_groups" not in packed:
+            raise ValueError("the pooled mode exchanges laps between controllers: with %d tracks it needs pool groups that each drive "
+                             "one track" % len(packed["track_sets"][0]))
+        tidx, gidx = packed["track_sets"][1], packed["pool_groups"][1]
+        for g in np.unique(gidx):
+            if len(np.unique(tidx[gidx == g])) > 1:
+                raise ValueError("pool group %d spans two tracks: a lap of another circuit is not a trajectory of this one" % g)
+    scheds = check_lap_schedules(lap_schedules, batch, L, {kind: given[kind + "_sets"] for kind in _native.LAP_SCHEDULE_TABLES})
     budget = _native.make_lap_budget(lap_budget, int(batch))       # ValueError where set_lap_budget would refuse, before any device work
-    N, M = handle_shape(shape_sets)
-    numSS_it = rp.lmpc_params(N)[0]
-    points = [M] * int(batch)                                      # every controller's numSS_Points
-    if shape_sets is not None:
-        if warm:
-            raise ValueError("shape_sets and warm start: the warm-start record is laid out per (N, numSS_Points)")
-        rows, sidx = _native.make_shape_sets(shape_sets[0], shape_sets[1], int(batch), N, M, numSS_it)
-        points = [rows[k].numSS_Points for k in sidx]
-    laps_of = [numSS_it] * int(batch)                              # every controller's numSS_it
-    if ss_laps_sets is not None:
-        rows, lidx = _native.make_ss_laps_sets(ss_laps_sets[0], ss_laps_sets[1], int(batch), numSS_it, points)
-        laps_of = [rows[k].numSS_it for k in lidx]
-    windows = None                                                 # [batch, 2] (ss_window, model_window), or None
-    if lap_window_sets is not None:
-        rows, widx = _native.make_lap_window_sets(lap_window_sets[0], lap_window_sets[1], int(batch), laps_of, SS_CAP, TR_TO_USE,
-                                                  MODEL_CAP)
-        windows = np.array([[rows[k].ss_window, rows[k].model_window] for k in widx], np.int32)
-    lanes = None                                                   # [batch, 2] (mode, lane_tol), or None
-    if lane_rule_sets is not None:
-        rows, ridx = _native.make_lane_rule_sets(lane_rule_sets[0], lane_rule_sets[1], int(batch), True, TCL)
-        lanes = np.array([[rows[k].mode, rows[k].lane_tol] for k in ridx], np.float64)
-    margins = None                                                 # [batch, 5] (mode, margin0, margin_max, step_up, step_down), or None
-    if lane_margin_sets is not None:
-        base = rp.lmpc_params(N)[5]
-        bx_min = np.full(int(batch), float(np.min(np.asarray(base.bx, float).ravel()[:2])))
-        if param_sets is not None:
-            pidx = np.asarray(param_sets[1]).reshape(-1)
-            if pidx.size == int(batch) and np.issubdtype(pidx.dtype, np.integer) and pidx.min() >= 0 and pidx.max() < len(param_sets[0]):
-                bx_min = np.array([float(np.min(np.asarray(p.bx, float).ravel()[:2])) for p in param_sets[0]])[pidx]
-        rows, midx = _native.make_lane_margin_sets(lane_margin_sets[0], lane_margin_sets[1], int(batch), bx_min)
-        margins = np.array([[rows[k].mode, rows[k].margin0, rows[k].margin_max, rows[k].step_up, rows[k].step_down]
-                            for k in midx], np.float64)
-    models = check_prediction_models(prediction_model_sets, batch, L)
+    rows_of = table_rows(packed)
     if start is not None:
-        _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget, shape_sets, L, scheds, windows, lanes,
-                     margins, models)
+        _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget, shape_sets, L, scheds, rows_of)
     if capture is not None and not isinstance(capture, dict):
         raise ValueError("capture is a dict that receives the run's end state")
     if readiness not in ("batch", "group"):
         raise ValueError("readiness is 'batch' or 'group', got %r" % (readiness,))
     if readiness == "group" and mode != "pooled":
         raise ValueError("readiness='group' schedules the pooled exchange; the %s mode exchanges nothing" % mode)
-    if track_sets is not None and mode == "pooled" and len(track_sets[0]) > 1:
-        if pool_groups is None:
-            raise ValueError("the pooled mode exchanges laps between controllers: with %d tracks it needs pool groups that each drive "
-                             "one track" % len(track_sets[0]))
-        tidx, gidx = np.asarray(track_sets[1]).reshape(-1), np.asarray(pool_groups[0]).reshape(-1)
-        if tidx.shape != gidx.shape:
-            raise ValueError("pool_groups and track_sets need one index entry per controller")
-        for g in np.unique(gidx):
-            if len(np.unique(tidx[gidx == g])) > 1:
-                raise ValueError("pool group %d spans two tracks: a lap of another circuit is not a trajectory of this one" % g)
     rank = dist.get_rank() if dist.is_initialized() else 0
     world = dist.get_world_size() if dist.is_initialized() else 1
     local = int(os.environ.get("LOCAL_RANK", 0)) if local is None else local
     dev = torch.device("cuda", local)
     torch.cuda.set_device(dev)
     B = int(batch)
+    N, M, numSS_it = ctx["N"], ctx["M"], ctx["numSS_it"]
     _, _, _, _, Qts, par = rp.lmpc_params(N)
     c = BatchedController(par, B, workloads.track_seg_table(), rp.TRACK_LENGTH, trToUse=TR_TO_USE, numSS_Points=M,
                           numSS_it=numSS_it, QterminalSlack=Qts, device=local, Tmax=TMAX, ss_cap=SS_CAP, model_cap=MODEL_CAP,
@@ -330,21 +375,9 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
     c.enable_rollout(Tcl=TCL)                            # before the tables: the measurement noise belongs to the closed loop
     if L:
         c.enable_lap_reports(L)                          # before the PID lap (its record is consumed by the seeding, unreported)
-    # the per-controller tables in the order they are installed: (arguments of the install call or None, install call, result key
-    # of the per-row lap statistics or None)
-    tables = ((param_sets, c.set_param_sets, "per_set_rank0"), (vehicle_sets, c.set_vehicles, "per_vehicle_rank0"),
-              (noise_sets, c.set_noise, "per_noise_rank0"),
-              (None if noise_streams is None else (noise_streams,), c.set_noise_streams, None),
-              (measurement_sets, c.set_measurement_noise, "per_measurement_rank0"),
-              (regression_sets, c.set_regression, "per_regression_rank0"), (track_sets, c.set_tracks, "per_track_rank0"),
-              (pool_groups, c.set_pool_groups, None), (shape_sets, c.set_shapes, "per_shape_rank0"),
-              (ss_laps_sets, c.set_ss_laps, "per_ss_laps_rank0"), (lap_window_sets, c.set_lap_windows, "per_lap_window_rank0"),
-              (lane_rule_sets, c.set_lane_rules, "per_lane_rule_rank0"), (lane_margin_sets, c.set_lane_margins, "per_lane_margin_rank0"),
-              (prediction_model_sets, c.set_prediction_models, "per_prediction_model_rank0"),
-              (surface_sets, c.set_surfaces, "per_surface_rank0"))
-    for args, install, _ in tables:
-        if args is not None:
-            install(*args)
+    for t in TABLES:
+        if t.keyword in packed:
+            getattr(c, t.install)(*t.args(given[t.keyword]))
     # every shipped lap has at least `ship_after` rows past its finish line: the readiness poll below guarantees it for the
     # slowest controllers of the batch, the export for the others (a group lapping faster holds laps that just ended)
     c.set_pool_min_overrun(ship_after)
@@ -437,11 +470,7 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         capture.update(capture_s=time.perf_counter() - tc, **sched.state(steps), batch=B, laps=laps, mode=mode, readiness=readiness,
                        poll=poll, warm=bool(warm), pool_groups=G, layout=c.snapshot_layout(),
                        lap_budget=None if budget is None else budget.tolist(),
-                       lap_schedules={kind: row_of_lap.tolist() for kind, row_of_lap in scheds.items()},
-                       lap_windows=None if windows is None else windows.tolist(),
-                       lane_rules=None if lanes is None else lanes.tolist(),
-                       lane_margins=None if margins is None else margins.tolist(),
-                       prediction_models=None if models is None else models.tolist())
+                       lap_schedules={kind: row_of_lap.tolist() for kind, row_of_lap in scheds.items()}, tables=rows_of)
     if trace is not None:
         cap = int(trace["cap"])
         trace.update(steps=[], x=[], xPred=[], lap=[])
@@ -453,6 +482,8 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
                 trace[k].append(v)
     flags_or, unsolved = c.rollout_health()
     reps = c.lap_reports() if L else None
+    bk.update(flags_or=flags_or, unsolved=unsolved, **({"lap_reports": reps} if L else {}),
+              **({"lane_margins": c.lane_margin_values()} if "lane_margin_sets" in packed else {}))
     lens, n_laps = (reps["steps"], reps["n"]) if L else (bk["lap_hist"], bk["lap_n"])
     stats = []
     for r in range(laps):
@@ -473,68 +504,7 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         out["lap_reports_rank0"] = lap_report_summary(reps, np.ones(B, bool), laps)
     if scheds:
         out["per_lap_row_rank0"] = lap_row_summary(reps, scheds, laps)
-    for args, _, key in tables:
-        if args is not None and key is not None:
-            idx = np.asarray(args[1]).reshape(B)
-            out[key] = [_set_stats(bk, flags_or, unsolved, idx == k, laps, reps) for k in range(len(args[0]))]
-    if shape_sets is not None:
-        idx = np.asarray(shape_sets[1]).reshape(B)
-        for k, s in enumerate(out["per_shape_rank0"]):
-            s.update(N=int(shape_sets[0][k][0]), numSS_Points=int(shape_sets[0][k][1]),
-                     ipm_iters_mean_sampled=float(it_ctrl[idx == k].mean() / max(it_n, 1)) if (idx == k).any() else 0.0)
-        out["handle_shape"] = [N, M]
-    if ss_laps_sets is not None:
-        idx = np.asarray(ss_laps_sets[1]).reshape(B)
-        for k, s in enumerate(out["per_ss_laps_rank0"]):
-            s.update(numSS_it=int(ss_laps_sets[0][k]),
-                     ipm_iters_mean_sampled=float(it_ctrl[idx == k].mean() / max(it_n, 1)) if (idx == k).any() else 0.0)
-        if shape_sets is not None:
-            sidx = np.asarray(shape_sets[1]).reshape(B)
-            out["per_shape_ss_laps_rank0"] = []
-            for j, sh in enumerate(shape_sets[0]):
-                for k, v in enumerate(ss_laps_sets[0]):
-                    cell = (sidx == j) & (idx == k)
-                    if cell.any():
-                        s = _set_stats(bk, flags_or, unsolved, cell, laps, reps)
-                        s.update(N=int(sh[0]), numSS_Points=int(sh[1]), numSS_it=int(v),
-                                 ipm_iters_mean_sampled=float(it_ctrl[cell].mean() / max(it_n, 1)))
-                        out["per_shape_ss_laps_rank0"].append(s)
-    if lap_window_sets is not None:
-        idx = np.asarray(lap_window_sets[1]).reshape(B)
-        for k, s in enumerate(out["per_lap_window_rank0"]):
-            w = lap_window_sets[0][k]
-            s.update(ss_window=int(w.ss_window), model_window=int(w.model_window),
-                     ipm_iters_mean_sampled=float(it_ctrl[idx == k].mean() / max(it_n, 1)) if (idx == k).any() else 0.0)
-    if lane_rule_sets is not None:
-        idx = np.asarray(lane_rule_sets[1]).reshape(B)
-        for k, s in enumerate(out["per_lane_rule_rank0"]):
-            r = lane_rule_sets[0][k]
-            s.update(mode=int(r.mode), lane_tol=float(r.lane_tol),
-                     ipm_iters_mean_sampled=float(it_ctrl[idx == k].mean() / max(it_n, 1)) if (idx == k).any() else 0.0)
-            if L:
-                _add_unsafe_share(s["reports"], reps, idx == k, laps)
-        if L:
-            _add_unsafe_share(out["lap_reports_rank0"], reps, np.ones(B, bool), laps)
-        _, unsafe = _native.split_lane_key(bk["ss_time"])
-        nit = np.array([c.ss_laps_of(b) for b in range(B)])
-        held = np.array([unsafe[b, bk["sel"][b, :nit[b]]].any() for b in range(B)])
-        out["lane_unsafe_selected_share_rank0"] = float(held.mean())
-    if lane_margin_sets is not None:
-        idx = np.asarray(lane_margin_sets[1]).reshape(B)
-        m_end = c.lane_margin_values()
-        out["lane_margin_final_rank0"] = []
-        for k, s in enumerate(out["per_lane_margin_rank0"]):
-            r = lane_margin_sets[0][k]
-            s.update(mode=int(r.mode), margin0=float(r.margin0), margin_max=float(r.margin_max), step_up=float(r.step_up),
-                     step_down=float(r.step_down),
-                     ipm_iters_mean_sampled=float(it_ctrl[idx == k].mean() / max(it_n, 1)) if (idx == k).any() else 0.0)
-            m = m_end[idx == k]
-            out["lane_margin_final_rank0"].append({"row": k, "n": int(m.size), "min": float(m.min()) if m.size else 0.0,
-                                                   "mean": float(m.mean()) if m.size else 0.0,
-                                                   "max": float(m.max()) if m.size else 0.0})
-    if prediction_model_sets is not None:
-        for k, s in enumerate(out["per_prediction_model_rank0"]):
-            s.update(mode=int(prediction_model_sets[0][k].mode))
+    out.update(table_stats(packed, ctx, bk, it_ctrl, it_n, laps))
     if pool_groups is not None:
         # a stored lap advances `it`: 4 seeded copies + every own lap handed over + every imported lap filed.  Exact unless an
         # own lap found the safe-set pool full (health flag 64): then that controller's count is one too low per such lap.
@@ -561,8 +531,7 @@ def run(batch=8192, laps=3, mode="pooled", share=2, tpad=288, ship_after=40, pol
         final.update(c.rollout_state())
         final.update(c.step_results())
     if books is not None:
-        books.update(bk, flags_or=flags_or, unsolved=unsolved, **({"lap_reports": reps} if L else {}),
-                     **({"lane_margins": m_end} if lane_margin_sets is not None else {}))
+        books.update(bk)
     c.close()
     return out
 
@@ -575,9 +544,10 @@ def _driven_steps(bk, state):
 
 
 def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, budget=None, shape_sets=None, lap_reports=0,
-                 lap_schedules=None, lap_windows=None, lane_rules=None, lane_margins=None, prediction_models=None):
+                 lap_schedules=None, tables=None):
     """The refusals of run(start=...), before any device work: a start that does not match this run (report capacity, lap
-    schedules and lap windows included), laps not above the captured laps, or a lap budget below the captured one."""
+    schedules and tables, {keyword: rows} of table_rows, included; a start without "tables" was captured without any), laps not
+    above the captured laps, or a lap budget below the captured one."""
     if not isinstance(start, dict):
         raise ValueError("start is a capture dict of an earlier run")
     need = ("records", "clock") + sharding.ExchangeSchedule.FIELDS + ("batch", "laps", "mode", "readiness", "poll", "warm",
@@ -608,57 +578,69 @@ def _check_start(start, batch, laps, mode, readiness, poll, warm, pool_groups, b
     if sorted(had) != sorted(mine) or any(not np.array_equal(had[k], mine[k]) for k in had):
         raise ValueError("start was captured with lap_schedules for %s, this run has %s (or other rows): a run resumes under the "
                          "schedules it was captured with" % (sorted(had) or "none", sorted(mine) or "none"))
-    check_start_windows(start.get("lap_windows"), lap_windows)
-    check_start_lane_rules(start.get("lane_rules"), lane_rules)
-    check_start_lane_margins(start.get("lane_margins"), lane_margins)
-    check_start_prediction_models(start.get("prediction_models"), prediction_models)
     for k, v in layout(warm, shape_sets).items():
         if int(start["layout"].get(k, -1)) != v:
             raise ValueError("start records have %s = %s, this run's controllers %d" % (k, start["layout"].get(k), v))
+    check_start_tables(start.get("tables", {}), tables or {})                 # a start without "tables" was taken without any
 
 
-def check_start_windows(had, mine):
-    """start's refusal of other lap windows: `had` the captured [batch, 2] windows (a list, or None without a table), `mine` this
-    run's (an array, or None).  The windows are not part of a record, and the books evicted against them."""
-    if (had is None) != (mine is None) or (had is not None and not np.array_equal(np.asarray(had), mine)):
-        raise ValueError("start was captured with other lap windows: a record resumes exactly only under the windows it was captured "
-                         "with")
+def table_stats(packed, ctx, bk, it_ctrl, it_n, laps):
+    """The result's entries of the tables (pack_tables' packed and ctx): per row of every table with a result key, _set_stats of
+    its controllers, its declared fields and, where declared, their interior-point iterations per poll (it_ctrl: every
+    controller's sum over it_n sampled polls); then the entries that join tables: "handle_shape", the (shape, lap count) cells
+    "per_shape_ss_laps_rank0", under lane rules the lane-unsafe shares (lap_reports_rank0 again, with them) and
+    "lane_unsafe_selected_share_rank0", and under lane margins "lane_margin_final_rank0".  bk holds the lap books, "flags_or",
+    "unsolved" and, where run() has them, "lap_reports" and "lane_margins"."""
+    flags_or, unsolved, reps = bk["flags_or"], bk["unsolved"], bk.get("lap_reports")
+    everyone = np.ones(len(flags_or), bool)
 
+    def entry(sel):
+        return _set_stats(bk, flags_or, unsolved, sel, laps, reps)
 
-def check_start_lane_rules(had, mine):
-    """start's refusal of other lane rules: `had` the captured [batch, 2] (mode, lane_tol) rows (a list, or None without a table),
-    `mine` this run's (an array, or None).  The rules are not part of a record, and the books ranked the stored laps under them."""
-    if (had is None) != (mine is None) or (had is not None and not np.array_equal(np.asarray(had, np.float64), mine)):
-        raise ValueError("start was captured with other lane rules: a record resumes exactly only under the rules it was captured "
-                         "with")
-
-
-def check_start_lane_margins(had, mine):
-    """start's refusal of other lane margins: `had` the captured [batch, 5] rows (a list, or None without a table), `mine` this
-    run's (an array, or None).  A record carries the margins, not the rows that adapt them."""
-    if (had is None) != (mine is None) or (had is not None and not np.array_equal(np.asarray(had, np.float64), mine)):
-        raise ValueError("start was captured with other lane margins: a record resumes exactly only under the margin rows it was "
-                         "captured with")
-
-
-def check_prediction_models(prediction_model_sets, batch, lap_reports):
-    """The refusals of run(prediction_model_sets=...), before any device work: the checks of set_prediction_models, and lap
-    reports (the per-row summary is taken from them).  Returns every controller's row as [batch, 11] (mode, the ten vehicle
-    values), or None without a table."""
-    if prediction_model_sets is None:
-        return None
-    if not lap_reports:
-        raise ValueError("prediction_model_sets needs lap_reports >= laps: the per-row summary is taken from the lap reports")
-    rows, idx = _native.make_prediction_model_sets(prediction_model_sets[0], prediction_model_sets[1], int(batch))
-    return np.array([[rows[k].mode] + [getattr(rows[k].vehicle, f) for f in _native.VEHICLE_FIELDS] for k in idx], np.float64)
-
-
-def check_start_prediction_models(had, mine):
-    """start's refusal of other prediction models: `had` the captured [batch, 11] rows (a list, or None without a table), `mine`
-    this run's (an array, or None).  The table is not part of a record."""
-    if (had is None) != (mine is None) or (had is not None and not np.array_equal(np.asarray(had, np.float64), mine)):
-        raise ValueError("start was captured with other prediction models: a record resumes exactly only under the model rows it was "
-                         "captured with")
+    def ipm(sel):
+        return float(it_ctrl[sel].mean() / max(it_n, 1)) if sel.any() else 0.0
+    out = {}
+    for t in TABLES:
+        if t.key is not None and t.keyword in packed:
+            rows, idx = packed[t.keyword]
+            out[t.key] = []
+            for k, row in enumerate(rows):
+                s = entry(idx == k)
+                s.update({f: getattr(row, f) for f in t.fields})
+                if t.ipm:
+                    s["ipm_iters_mean_sampled"] = ipm(idx == k)
+                out[t.key].append(s)
+    if "shape_sets" in packed:
+        out["handle_shape"] = [ctx["N"], ctx["M"]]
+    if "shape_sets" in packed and "ss_laps_sets" in packed:
+        (shapes, sidx), (values, lidx) = packed["shape_sets"], packed["ss_laps_sets"]
+        out["per_shape_ss_laps_rank0"] = []
+        for j, sh in enumerate(shapes):
+            for k, v in enumerate(values):
+                cell = (sidx == j) & (lidx == k)
+                if cell.any():
+                    s = entry(cell)
+                    s.update(N=sh.N, numSS_Points=sh.numSS_Points, numSS_it=v.numSS_it, ipm_iters_mean_sampled=ipm(cell))
+                    out["per_shape_ss_laps_rank0"].append(s)
+    if "lane_rule_sets" in packed:
+        idx = packed["lane_rule_sets"][1]
+        if reps is not None:
+            for k, s in enumerate(out["per_lane_rule_rank0"]):
+                _add_unsafe_share(s["reports"], reps, idx == k, laps)
+            out["lap_reports_rank0"] = lap_report_summary(reps, everyone, laps)
+            _add_unsafe_share(out["lap_reports_rank0"], reps, everyone, laps)
+        _, unsafe = _native.split_lane_key(bk["ss_time"])
+        held = np.array([unsafe[b, bk["sel"][b, :nit]].any() for b, nit in enumerate(ctx["laps_of"])])
+        out["lane_unsafe_selected_share_rank0"] = float(held.mean())
+    if "lane_margin_sets" in packed:
+        idx, m_end = packed["lane_margin_sets"][1], bk["lane_margins"]
+        out["lane_margin_final_rank0"] = []
+        for k in range(len(packed["lane_margin_sets"][0])):
+            m = m_end[idx == k]
+            out["lane_margin_final_rank0"].append({"row": k, "n": int(m.size), "min": float(m.min()) if m.size else 0.0,
+                                                   "mean": float(m.mean()) if m.size else 0.0,
+                                                   "max": float(m.max()) if m.size else 0.0})
+    return out
 
 
 def _add_unsafe_share(rows, reps, sel, laps):

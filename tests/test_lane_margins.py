@@ -122,7 +122,7 @@ def test_both_install_orders_against_parameter_sets():
         s.set_lane_margins(None, [0, 0, 0, 0])                             # removal takes no index
 
 
-def test_driver_refusals_before_any_device_work():
+def test_driver_refusals_and_start_margin_rows():
     rmc = rollout_mc
     for bad in (([G(3)], np.zeros(8, int)), ([G(1, -1.0)], np.zeros(8, int)), ([G(1, 0.0)], np.ones(8, int)),
                 ([G(1, 0.0)], np.zeros(7, int)), ([G(1, 0.4, 0.4)], np.zeros(8, int)), ([G(2, 0.0, 0.5, 0.01)], np.zeros(8, int))):
@@ -131,15 +131,13 @@ def test_driver_refusals_before_any_device_work():
     with pytest.raises(ValueError, match="does not leave a lane"):
         rmc.run(batch=8, laps=1, param_sets=([_par(0.4), _par(0.1)], np.arange(8) % 2),
                 lane_margin_sets=([G(1, 0.1, 0.1)], np.zeros(8, int)))
-    row = [2, 0.0, 0.1, 0.01, 0.0025]
-    with pytest.raises(ValueError):
-        rmc.check_start_lane_margins([row] * 8, None)
-    with pytest.raises(ValueError):
-        rmc.check_start_lane_margins(None, np.array([row] * 8))
-    with pytest.raises(ValueError):
-        rmc.check_start_lane_margins([row] * 8, np.array([[2, 0.0, 0.1, 0.01, 0.0]] * 8))
-    rmc.check_start_lane_margins([row] * 8, np.array([row] * 8))
-    rmc.check_start_lane_margins(None, None)
+    row, none = rmc.table_rows(rmc.pack_tables(8, lane_margin_sets=([G(2, 0.0, 0.1, 0.01, 0.0025)], np.zeros(8, int)))[0]), {}
+    other = rmc.table_rows(rmc.pack_tables(8, lane_margin_sets=([G(2, 0.0, 0.1, 0.01, 0.0)], np.zeros(8, int)))[0])
+    for had, mine in ((row, none), (none, row), (row, other)):
+        with pytest.raises(ValueError, match="other lane margins"):
+            rmc.check_start_tables(had, mine)
+    rmc.check_start_tables(row, row)
+    rmc.check_start_tables(none, none)
 
 
 def _x(ey):

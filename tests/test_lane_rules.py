@@ -103,20 +103,19 @@ def test_both_install_orders():
         _Stub(lmpc=False).set_lane_rules([R(0, 0.0)], np.zeros(4, int))
 
 
-def test_driver_refusals_before_any_device_work():
+def test_driver_refusals_and_start_rule_rows():
     rmc = rollout_mc
     for bad in (([R(2, 0.0)], np.zeros(8, int)), ([R(1, -1.0)], np.zeros(8, int)), ([R(1, 0.0)], np.ones(8, int)),
                 ([R(1, 0.0)], np.zeros(7, int))):
         with pytest.raises(ValueError):
             rmc.run(batch=8, laps=1, lane_rule_sets=bad)
-    with pytest.raises(ValueError):
-        rmc.check_start_lane_rules([[1, 0.0]] * 8, None)
-    with pytest.raises(ValueError):
-        rmc.check_start_lane_rules(None, np.array([[1, 0.0]] * 8))
-    with pytest.raises(ValueError):
-        rmc.check_start_lane_rules([[1, 0.0]] * 8, np.array([[1, 0.01]] * 8))
-    rmc.check_start_lane_rules([[1, 0.0]] * 8, np.array([[1, 0.0]] * 8))
-    rmc.check_start_lane_rules(None, None)
+    rule, none = rmc.table_rows(rmc.pack_tables(8, lane_rule_sets=([R(1, 0.0)], np.zeros(8, int)))[0]), {}
+    other = rmc.table_rows(rmc.pack_tables(8, lane_rule_sets=([R(1, 0.01)], np.zeros(8, int)))[0])
+    for had, mine in ((rule, none), (none, rule), (rule, other)):
+        with pytest.raises(ValueError, match="other lane rules"):
+            rmc.check_start_tables(had, mine)
+    rmc.check_start_tables(rule, rule)
+    rmc.check_start_tables(none, none)
 
 
 def _row(ey):

@@ -60,7 +60,7 @@ def test_driver_refuses_bad_budgets_before_any_device_work():
             rollout_mc.run(batch=B, lap_budget=bad)
     start = dict(records=np.zeros((B, 1)), clock=0, steps=8, next_round=1, next_rounds=None, exchanged=[False], exchange_steps=[[]],
                  diverged_step=None, batch=B, laps=3, mode="independent", readiness="batch", poll=8, warm=False, pool_groups=1,
-                 layout=rollout_mc.layout(), lap_budget=[3] * B)
+                 layout=rollout_mc.layout(), lap_budget=[3] * B, tables={})
     with pytest.raises(ValueError, match="lap_budget is below"):
         rollout_mc.run(batch=B, laps=5, mode="independent", start=start, lap_budget=np.where(np.arange(B) == 4, 2, 5))
 

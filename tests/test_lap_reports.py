@@ -76,7 +76,7 @@ def test_run_refusals_before_device_work(kw, monkeypatch):
 def _start(L):
     s = {k: 0 for k in sharding.ExchangeSchedule.FIELDS}
     s.update(records=np.zeros((8, 16), np.uint8), clock=0, batch=8, laps=3, mode="pooled", readiness="batch", poll=8, warm=False,
-             pool_groups=1, layout=dict(rollout_mc.layout(lap_reports=L), bytes=16))
+             pool_groups=1, layout=dict(rollout_mc.layout(lap_reports=L), bytes=16), tables={})
     return s
 
 

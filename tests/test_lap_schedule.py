@@ -169,7 +169,8 @@ def test_run_refusals_before_device_work(kw, what, monkeypatch):
 def _start(scheds):
     s = {k: 0 for k in sharding.ExchangeSchedule.FIELDS}
     s.update(records=np.zeros((8, 16), np.uint8), clock=0, batch=8, laps=3, mode="pooled", readiness="batch", poll=8, warm=False,
-             pool_groups=1, layout=dict(rollout_mc.layout(lap_reports=8), bytes=16), lap_schedules=scheds)
+             pool_groups=1, layout=dict(rollout_mc.layout(lap_reports=8), bytes=16), lap_schedules=scheds,
+             tables=rollout_mc.table_rows(rollout_mc.pack_tables(8, vehicle_sets=VS)[0]))
     return s
 
 

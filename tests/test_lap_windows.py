@@ -275,7 +275,7 @@ def test_windows_of_the_recent_laps_select_the_last_laps():
         assert not m.dead
 
 
-def test_driver_refuses_bad_windows_before_any_device_work():
+def test_driver_refuses_bad_windows_and_other_window_rows():
     with pytest.raises(ValueError, match=r"ss_window must be 0 or numSS_it \.\. ss_cap \(7\)"):
         rollout_mc.run(batch=8, lap_window_sets=([W(0, 0), W(8, 0)], np.arange(8) % 2))
     with pytest.raises(ValueError, match=r"controller 1: ss_window 3 is below its numSS_it \(4\)"):
@@ -287,12 +287,14 @@ def test_driver_refuses_bad_windows_before_any_device_work():
     # with lap counts the window is checked against each controller's own value: 3 is fine for numSS_it 2
     with pytest.raises(ValueError, match=r"controller 0: ss_window 3 is below its numSS_it \(4\)"):
         rollout_mc.run(batch=8, ss_laps_sets=([4, 2], np.arange(8) % 2), lap_window_sets=([W(3, 0)], np.zeros(8, int)))
-    w = np.array([[4, 4]] * 8, np.int32)
-    rollout_mc.check_start_windows(None, None)
-    rollout_mc.check_start_windows(w.tolist(), w)
-    for had, mine in ((None, w), (w.tolist(), None), (w.tolist(), np.zeros((8, 2), np.int32))):
+    def rows(*windows):
+        return rollout_mc.table_rows(rollout_mc.pack_tables(8, lap_window_sets=(list(windows), np.zeros(8, int)))[0])
+    w = rows(W(4, 4))
+    rollout_mc.check_start_tables({}, {})
+    rollout_mc.check_start_tables(w, rows(W(4, 4)))
+    for had, mine in (({}, w), (w, {}), (w, rows(W(0, 0)))):
         with pytest.raises(ValueError, match="other lap windows"):
-            rollout_mc.check_start_windows(had, mine)
+            rollout_mc.check_start_tables(had, mine)
 
 
 def test_window_lists_with_unbounded_windows_are_the_unbounded_lists():

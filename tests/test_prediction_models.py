@@ -85,7 +85,7 @@ def test_rounded_exact_rows_meet_the_bound_and_every_variant_is_rejected():
                 assert nm.deviation(_f64(nm.rows(car, x, u, variant=v)), exact) > 1e3 * nm.NOMINAL_BOUND, (car, x, v)
 
 
-def test_driver_refusals_before_any_device_work():
+def test_driver_refusals_and_start_model_rows():
     import os
     import sys
     sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "benchmarks"))
@@ -97,19 +97,20 @@ def test_driver_refusals_before_any_device_work():
                 ([P.plant()], np.zeros(7, int)), ([_with("Df", math.nan, 2)], np.zeros(8, int))):
         with pytest.raises(ValueError):
             rmc.run(batch=8, laps=1, lap_reports=1, prediction_model_sets=bad)
-    rows = rmc.check_prediction_models(([P.learned(), P.believes(CARS[1])], np.arange(8) % 2), 8, 1)
-    assert rows.shape == (8, 11) and list(rows[1]) == [1.0] + [getattr(CARS[1], f) for f in nat.VEHICLE_FIELDS]
-    assert rmc.check_prediction_models(None, 8, 0) is None
-    with pytest.raises(ValueError):
-        rmc.check_start_prediction_models(rows.tolist(), None)
-    with pytest.raises(ValueError):
-        rmc.check_start_prediction_models(None, rows)
-    other = rows.copy()
-    other[3, 0] = 2.0
-    with pytest.raises(ValueError, match="other prediction models"):
-        rmc.check_start_prediction_models(rows.tolist(), other)
-    rmc.check_start_prediction_models(rows.tolist(), rows)
-    rmc.check_start_prediction_models(None, None)
+    models = [P.learned(), P.believes(CARS[1])]
+    packed = rmc.pack_tables(8, prediction_model_sets=(models, np.arange(8) % 2))[0]
+    rows, idx = packed["prediction_model_sets"]
+    assert len(idx) == 8 and rows[idx[1]].mode == 1
+    assert [getattr(rows[idx[1]].vehicle, f) for f in nat.VEHICLE_FIELDS] == [getattr(CARS[1], f) for f in nat.VEHICLE_FIELDS]
+    assert rmc.pack_tables(8, prediction_model_sets=None)[0] == {}
+    had, none = rmc.table_rows(packed), {}
+    other = rmc.table_rows(rmc.pack_tables(8, prediction_model_sets=([P.learned(), P.believes(CARS[1]), P.plant()],
+                                                                      np.where(np.arange(8) == 3, 2, np.arange(8) % 2)))[0])
+    for a, b in ((had, none), (none, had), (had, other)):
+        with pytest.raises(ValueError, match="other prediction models"):
+            rmc.check_start_tables(a, b)
+    rmc.check_start_tables(had, rmc.table_rows(packed))
+    rmc.check_start_tables(none, none)
 
 
 def test_benchmark_prediction_error_and_table():

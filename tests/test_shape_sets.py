@@ -132,6 +132,7 @@ def test_driver_layout_and_start_follow_the_shapes():
     assert rollout_mc.layout() == rollout_mc.layout(shape_sets=([(12, 48)], np.zeros(B, int)))
     start = dict(records=np.zeros((B, 1)), clock=0, steps=8, next_round=1, next_rounds=None, exchanged=[False], exchange_steps=[[]],
                  diverged_step=None, batch=B, laps=3, mode="independent", readiness="batch", poll=8, warm=False, pool_groups=1,
-                 layout=rollout_mc.layout(), lap_budget=None)
+                 layout=rollout_mc.layout(), lap_budget=None,
+                 tables=rollout_mc.table_rows(rollout_mc.pack_tables(B, shape_sets=shapes)[0]))
     with pytest.raises(ValueError, match="start records have N"):
         rollout_mc.run(batch=B, laps=5, mode="independent", start=start, shape_sets=shapes)

@@ -110,7 +110,7 @@ def _capture(**over):
     numSS_it, numSS_Points = rp.lmpc_params(12)[:2]
     cap = dict(records=torch.zeros((16, 32), dtype=torch.uint8), clock=1400, steps=400, next_round=3, next_rounds=None,
                exchanged=[False], exchange_steps=[[200, 320]], diverged_step=None, batch=16, laps=3, mode="pooled",
-               readiness="batch", poll=8, warm=False, pool_groups=1,
+               readiness="batch", poll=8, warm=False, pool_groups=1, tables={},
                layout=dict(N=12, M=numSS_Points, ncx=2, ncu=4, numSS_it=numSS_it, trToUse=4, ss_cap=7, model_cap=5, Tmax=1280, Tcl=1024,
                            warm_start=0))
     cap.update(over)
