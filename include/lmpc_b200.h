@@ -469,7 +469,9 @@ int lmpc_read_buffer(lmpc_handle* h, const char* name, size_t offset_bytes, void
 /* Device address of an internal buffer by name: "xPred","uPred","lambd","zt","zt_u","abc","SS_sel","Qfun_sel",
  * "Succ_SS","Succ_uSS","status","iters","resid","flags","xLin","uLin","x0","OldInput","slack","slackT" (lane slacks [B,N*ncx] and
  * terminal slack [B,6] of the most recent step), "abc_lti", "x_meas" (the measured state [B,6] of the closed loop's current
- * step under lmpc_rollout_set_measurement_noise). */
+ * step under lmpc_rollout_set_measurement_noise), "x_est" (the state [B,6] the controllers read in that step under
+ * lmpc_rollout_set_observers), "xPredPrev" (the previous step's prediction [B,N+1,6]) and "has_pred" (int [B]: 1 when it is
+ * one), the observer's prior. */
 void* lmpc_device_buffer(lmpc_handle* h, const char* name);
 
 /* ===== device-resident closed loop (the caller of the hot path, SURVEY §8f rank 1) =======================================
@@ -641,6 +643,45 @@ typedef struct lmpc_measurement_params {
  *     middle of a run applies from the next step on.  The table stays with the handle and is not part of a snapshot record.
  *   - The host-driven entry points (lmpc_step_*, lmpc_solve_*) take the caller's x0 and are not affected. */
 int lmpc_rollout_set_measurement_noise(lmpc_handle* h, const lmpc_measurement_params* sets, int nsets, const int* set_of_instance);
+/* State observer of the device closed loop: a fixed-gain predictor-corrector on the state a controller reads (no reference
+ * counterpart; DESIGN.md, "Per-controller state observers"). */
+#define LMPC_FLAG_OBSERVER_RESET 2048        /* step flag: the observer's prior was not finite, the controller read y */
+typedef struct lmpc_observer_params {
+    int mode;                     /* 0 no observer (the controller reads y), 1 observer */
+    int pad;
+    double gain[6];               /* l_j in [0, 1] per channel vx, vy, wz, epsi, s, ey; not read under mode 0 */
+} lmpc_observer_params;
+/* Per-controller state observers.  Controller b reads row sets[set_of_instance[b]] (host arrays); nsets == 0 (sets,
+ * set_of_instance NULL) removes the table, which every handle starts without: then no kernel is launched and every kernel runs
+ * the code it runs without this feature.  With a table installed, every lmpc_rollout_step (modes 0, 1, 2) and
+ * lmpc_rollout_pid_step launches one more kernel, right after the measurement kernel, which forms the state x_hat [B,6] the
+ * controller reads from y, the measured state under lmpc_rollout_set_measurement_noise and the plant state otherwise:
+ *   - Mode 0 rows: x_hat = y exactly.
+ *   - Mode 1 rows in a step of mode 0 or 1: the prior is p = xPred[1] of the QP the controller solved in its previous step (row 1
+ *     of the state section xPredPrev), read only when has_pred == 1.  Lap wrap: when p_s - y_s > TrackLength / 2 (the plant
+ *     wrapped s at a hand-over, p did not), p_s = fmax(p_s - TrackLength, 0), the rule of the safe-set selection's terminal
+ *     guess.  Then per channel j
+ *       x_hat_j = p_j + l_j (y_j - p_j)   in fp64 without fused multiply-adds, rounded per operation,
+ *     except that l_j == 1 copies y_j and l_j == 0 takes p_j exactly.  Without a prior (has_pred == 0: the first step after the
+ *     seeding, after a PID or LTI step, after lmpc_state_set) x_hat = y exactly.  A prior with a non-finite entry on a channel
+ *     with l_j < 1 is not used: x_hat = y and the step sets LMPC_FLAG_OBSERVER_RESET, which reaches the health word and the lap
+ *     reports like every step flag.  A row whose gains are all 1 never reads the prior and never sets the flag.
+ *   - Mode 1 rows in a PID step or a rollout step of mode 2: xPredPrev is only written by the state shift of modes 0 and 1, so
+ *     such a step clears has_pred and the controller reads x_hat = y.
+ *   - x_hat replaces y as the QP's x0 (and so the safe-set selection), addPoint's row and the state rows of the closed-loop
+ *     record (and so the lap hand-over, the safe set, the learned model, the lane rules and the adapted lane margins).  The PID's
+ *     input and the LTI QP's x0 read x_hat = y.  The plant, done, the lap wrap, lmpc_rollout_get_state, the trace and the lap
+ *     reports keep the true state.  x_hat of the current step is the device buffer "x_est" [B,6] (lmpc_read_buffer).
+ *   - A retired controller (lmpc_rollout_set_lap_budget) reads, writes and flags nothing.
+ *   - 1 <= nsets <= batch, every index in [0, nsets); mode 0 or 1; every gain finite and in [0, 1].
+ *   - Needs lmpc_rollout_create (LMPC_E_STATE otherwise); any failed check returns LMPC_E_INVALID.  Every refusal leaves the
+ *     handle as it was.
+ *   - The call synchronises the handle's streams before it replaces the table.  It is allowed at any time: a change in the middle
+ *     of a run applies from the next step on.  The table stays with the handle, is not part of a snapshot record and is not
+ *     schedulable; the observer's memory (xPredPrev, has_pred) is part of every record, so a restored controller under the same
+ *     table continues exactly.
+ *   - The host-driven entry points (lmpc_step_*, lmpc_solve_*) take the caller's x0 and are not affected. */
+int lmpc_rollout_set_observers(lmpc_handle* h, const lmpc_observer_params* sets, int nsets, const int* set_of_instance);
 /* Lap budgets: controller b is retired once it has handed over budget_of_instance[b] laps (lmpc_rollout_commit_laps_dev counts
  * them: lap_n of lmpc_books_get).  A retired controller keeps the state that hand-over left it in (lap filed, books refreshed,
  * record restarted: the start line of its next lap) and no kernel of lmpc_rollout_step (modes 0, 1, 2) or
@@ -879,6 +920,7 @@ int lmpc_sizeof_vehicle_params(void);
 int lmpc_sizeof_track_params(void);
 int lmpc_sizeof_noise_params(void);
 int lmpc_sizeof_measurement_params(void);
+int lmpc_sizeof_observer_params(void);
 int lmpc_sizeof_regression_params(void);
 int lmpc_sizeof_shape_params(void);
 int lmpc_sizeof_ss_laps_params(void);

@@ -48,6 +48,12 @@ class MeasurementParams(C.Structure):
     _fields_ = [("sigma", C.c_double * 6), ("clip", C.c_double * 6)]
 
 
+class ObserverParams(C.Structure):
+    """lmpc_observer_params: the fixed-gain state observer of a controller of the device closed loop -- mode 0 none, mode 1
+    x_hat_j = p_j + gain_j (y_j - p_j) over (vx, vy, wz, epsi, s, ey), p the controller's own one-step prediction."""
+    _fields_ = [("mode", C.c_int), ("pad", C.c_int), ("gain", C.c_double * 6)]
+
+
 class RegressionParams(C.Structure):
     """lmpc_regression_params: the constants of the local regression model (PredictiveModel.py:18-31)."""
     _fields_ = [("trToUse", C.c_int), ("MaxNumPoint", C.c_int), ("h", C.c_double), ("lamb", C.c_double),
@@ -99,6 +105,7 @@ class SurfaceParams(C.Structure):
 
 
 FLAG_NOMINAL_NONFINITE = 1024       # LMPC_FLAG_NOMINAL_NONFINITE: step flag of a nominal controller whose rows 0..2 are not finite
+FLAG_OBSERVER_RESET = 2048          # LMPC_FLAG_OBSERVER_RESET: step flag of an observer whose prior was not finite (it read y)
 LANE_UNSAFE_KEY = 1 << 24           # LMPC_LANE_UNSAFE_KEY: added to the safe-set key of a lane-unsafe lap
 REPORT_LANE_UNSAFE = 1 << 16        # LMPC_REPORT_LANE_UNSAFE: report flag of an own lap judged lane-unsafe
 
@@ -237,6 +244,7 @@ def lib():
     L.lmpc_rollout_set_noise.argtypes = [_vp, C.POINTER(NoiseParams), C.c_int, _vp]
     L.lmpc_rollout_set_noise_streams.argtypes = [_vp, _vp]
     L.lmpc_rollout_set_measurement_noise.argtypes = [_vp, C.POINTER(MeasurementParams), C.c_int, _vp]
+    L.lmpc_rollout_set_observers.argtypes = [_vp, C.POINTER(ObserverParams), C.c_int, _vp]
     L.lmpc_rollout_set_lap_budget.argtypes = [_vp, _vp]
     L.lmpc_rollout_enable_lap_reports.argtypes = [_vp, C.c_int]
     L.lmpc_rollout_get_lap_reports.argtypes = [_vp, _vp, _vp]
@@ -307,6 +315,8 @@ def lib():
     assert L.lmpc_sizeof_lap_report() == C.sizeof(LapReport), "lmpc_lap_report ABI mismatch"
     assert L.lmpc_sizeof_noise_params() == C.sizeof(NoiseParams), "lmpc_noise_params ABI mismatch"
     assert L.lmpc_sizeof_measurement_params() == C.sizeof(MeasurementParams), "lmpc_measurement_params ABI mismatch"
+    L.lmpc_sizeof_observer_params.restype = C.c_int
+    assert L.lmpc_sizeof_observer_params() == C.sizeof(ObserverParams), "lmpc_observer_params ABI mismatch"
     assert L.lmpc_sizeof_regression_params() == C.sizeof(RegressionParams), "lmpc_regression_params ABI mismatch"
     assert L.lmpc_sizeof_params() == C.sizeof(Params), "lmpc_params ABI mismatch"
     assert L.lmpc_sizeof_model_params() == C.sizeof(ModelParams), "lmpc_model_params ABI mismatch"
@@ -593,6 +603,28 @@ def make_measurement_sets(meas, index, batch):
             getattr(r, f)[:] = v.tolist()
         return r
     return _pack_sets(MeasurementParams, meas, index, batch, "measurement sets", row)
+
+
+def make_observer_sets(observers, index, batch):
+    """Per-controller state observers for ``lmpc_rollout_set_observers``: K objects ``observers`` with ``mode`` (0 none, 1
+    observer) and ``gain`` (six gains over vx, vy, wz, epsi, s, ey; e.g. reference_params.ObserverParams) and the observer of
+    every controller ``index[batch]``.  Raises ValueError where the library would refuse: the index rules of
+    ``make_param_sets``, a mode other than 0 or 1, a gain field of the wrong length, or a gain that is not finite or lies outside
+    [0, 1].  Returns (ctypes array ObserverParams * K, int32 index array)."""
+    def row(k, o):
+        mode = o.mode
+        if isinstance(mode, (bool, np.bool_)) or not isinstance(mode, (int, np.integer)) or int(mode) not in (0, 1):
+            raise ValueError("observer %d: mode must be 0 or 1, got %r" % (k, mode))
+        g = np.asarray(o.gain, dtype=float).reshape(-1)
+        if g.shape[0] != 6:
+            raise ValueError("observer %d: gain needs 6 values, got %d" % (k, g.shape[0]))
+        if not np.all(np.isfinite(g)) or np.any(g < 0) or np.any(g > 1):
+            raise ValueError("observer %d: every gain must be finite and in [0, 1]" % k)
+        r = ObserverParams()
+        r.mode = int(mode)
+        r.gain[:] = g.tolist()
+        return r
+    return _pack_sets(ObserverParams, observers, index, batch, "observers", row)
 
 
 def _int_per_controller(values, batch, lo, what):

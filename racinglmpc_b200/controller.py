@@ -274,6 +274,22 @@ class BatchedController:
                       lambda: nat.make_measurement_sets(meas, index, self.B))
         self._table_rows["measurement"] = rows
 
+    def set_observers(self, observers=None, index=None):
+        """Per-controller state observers of the device closed loop (a fixed-gain predictor-corrector on a noisy sensor): in every
+        later ``rollout_step`` of mode 0 or 1 a controller whose row ``observers[index[b]]`` (objects with ``mode`` and ``gain``,
+        e.g. reference_params.ObserverParams) has mode 1 reads x_hat_j = p_j + gain_j (y_j - p_j) on (vx, vy, wz, epsi, s, ey) in
+        place of y, the measured state (``set_measurement_noise``) or the plant state: p is its own prediction xPred[1] of the
+        previous step, its s wrapped back by TrackLength after a hand-over.  Its QP, safe-set selection, addPoint and closed-loop
+        record all take x_hat, so its stored laps and learned models are filtered data.  Gain 1 copies y, gain 0 takes p.  Without
+        a prior (the first step after the seeding, after a PID or mode 2 step, which clear it) x_hat = y; a non-finite prior
+        gives x_hat = y and the step flag FLAG_OBSERVER_RESET.  Mode 0 rows read y.  The plant, ``rollout_state``, the trace and
+        the lap reports keep x; x_hat of the step is ``read_buffer("x_est", ...)``.  ``index`` is required with ``observers``.
+        ``observers=None`` (no index) removes the table: no kernel is added to a step.  Needs ``enable_rollout``; allowed in the
+        middle of a run; not part of a snapshot.  ValueError before any native call where the library would refuse a value.
+        Waits for work already enqueued."""
+        self._install(self._lib.lmpc_rollout_set_observers, "observers", observers, index,
+                      lambda: nat.make_observer_sets(observers, index, self.B))
+
     def set_lap_budget(self, budget=None):
         """Lap budgets of the device closed loop: controller b retires once it has handed over ``budget[b]`` laps (one integer
         >= 1 for the whole batch, or one per controller).  A retired controller keeps the state its last hand-over left it in and

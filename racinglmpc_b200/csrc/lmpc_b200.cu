@@ -175,6 +175,10 @@ struct lmpc_handle {
     // the measured state of the current step (measure_kernel).
     HandleTable<lmpc_measurement_params> meas;
     double* d_xmeas;
+    // state observers of the controllers (lmpc_rollout_set_observers), or none: they read the measured or plant state.  d_xest is
+    // the state the controllers read in the current step (observe_kernel).
+    HandleTable<lmpc_observer_params> obs;
+    double* d_xest;
     // lap budgets (lmpc_rollout_set_lap_budget): laps every controller drives before it retires, or none for no budget
     HandleTable<int> budget;
     // track surfaces of the simulator (lmpc_rollout_set_surfaces), or none: the vehicle's grip all round the lap
@@ -249,8 +253,8 @@ static std::vector<DevBuf> dev_bufs(lmpc_handle* h) {
         dbuf(h->d_prevslot, 1, S, FILL_ONES, SN_PREVSLOT), dbuf(h->d_used, k.trToUse, S, FILL_ZERO, SN_USED),
         dbuf(h->d_xLin, np, S, FILL_NONE, SN_XLIN, "xLin"), dbuf(h->d_uLin, N * 2, S, FILL_NONE, SN_ULIN, "uLin"),
         dbuf(h->d_ztState, 6, S, FILL_ZERO, SN_ZT), dbuf(h->d_OldInput, 2, S, FILL_ZERO, SN_OLDINPUT, "OldInput"),
-        dbuf(h->d_xPredPrev, np, S, FILL_ZERO, SN_XPREDPREV), dbuf(h->d_timeStep, 1, S, FILL_ZERO, SN_TIMESTEP),
-        dbuf(h->d_hasPred, 1, S, FILL_ZERO, SN_HASPRED),
+        dbuf(h->d_xPredPrev, np, S, FILL_ZERO, SN_XPREDPREV, "xPredPrev"), dbuf(h->d_timeStep, 1, S, FILL_ZERO, SN_TIMESTEP),
+        dbuf(h->d_hasPred, 1, S, FILL_ZERO, SN_HASPRED, "has_pred"),
         dbuf(h->d_warm, (size_t)h->warm_stride, OWN_WARM, FILL_NONE, SN_WARM, "warm"),
         dbuf(h->d_warm_valid, 1, OWN_WARM, FILL_ZERO, SN_WARM_VALID, "warm_valid"),
         // store scratch: flags (cleared by every step), K2 outputs nothing reads later, staging of host arrays, exchange scratch
@@ -266,6 +270,7 @@ static std::vector<DevBuf> dev_bufs(lmpc_handle* h) {
         dbuf(h->d_health, 1, R, FILL_ZERO, SN_HEALTH_FLAGS, nullptr, 2),       // [2][B]: flags, then unsolved steps
         dbuf(h->d_abc_lti, 54, R, FILL_ZERO, SN_ABC_LTI, "abc_lti"), dbuf(h->d_z, 3, R), dbuf(h->d_zpid, 2, R),
         dbuf(h->d_xmeas, 6, R, FILL_ZERO, SN_SCRATCH, "x_meas"),     // formed from the plant state and the clock every step
+        dbuf(h->d_xest, 6, R, FILL_ZERO, SN_SCRATCH, "x_est"),       // formed from x_meas and xPredPrev every step
         // per-lap reports (lap_reports_reset_kernel gives the running rows their start)
         dbuf(h->d_rep_rows, (size_t)h->rep_L, OWN_REPORTS, FILL_ZERO, SN_LAP_REPORTS), dbuf(h->d_rep_run, 1, OWN_REPORTS, FILL_ZERO, SN_LAP_RUN),
         // lane margins (lmpc_set_lane_margins; lane_margin_rows_kernel fills them)
@@ -291,7 +296,7 @@ static void free_tables(lmpc_handle* h, unsigned owners) {
         t.rows.clear(); t.index.clear();
     };
     release(h->sets, OWN_HANDLE); release(h->veh, OWN_HANDLE); release(h->noise, OWN_HANDLE); release(h->streams, OWN_HANDLE);
-    release(h->meas, OWN_HANDLE); release(h->surf, OWN_HANDLE); release(h->budget, OWN_HANDLE); release(h->trk, OWN_STORE); release(h->reg, OWN_STORE); release(h->pool_grp, OWN_STORE);
+    release(h->meas, OWN_HANDLE); release(h->obs, OWN_HANDLE); release(h->surf, OWN_HANDLE); release(h->budget, OWN_HANDLE); release(h->trk, OWN_STORE); release(h->reg, OWN_STORE); release(h->pool_grp, OWN_STORE);
     for (auto& t : h->sched) release(t, OWN_HANDLE);
     release(h->shp, OWN_STORE); release(h->shp_order, OWN_STORE); release(h->own_c, OWN_HANDLE); release(h->ssl, OWN_STORE);
     release(h->lwin, OWN_STORE); release(h->lrule, OWN_STORE); release(h->lmar, OWN_STORE); release(h->pmod, OWN_STORE);
@@ -1049,6 +1054,7 @@ int lmpc_sizeof_model_params(void) { return (int)sizeof(lmpc_model_params); }
 int lmpc_sizeof_vehicle_params(void) { return (int)sizeof(lmpc_vehicle_params); }
 int lmpc_sizeof_noise_params(void) { return (int)sizeof(lmpc_noise_params); }
 int lmpc_sizeof_measurement_params(void) { return (int)sizeof(lmpc_measurement_params); }
+int lmpc_sizeof_observer_params(void) { return (int)sizeof(lmpc_observer_params); }
 int lmpc_sizeof_regression_params(void) { return (int)sizeof(lmpc_regression_params); }
 int lmpc_sizeof_shape_params(void) { return (int)sizeof(lmpc_shape_params); }
 int lmpc_sizeof_ss_laps_params(void) { return (int)sizeof(lmpc_ss_laps_params); }
@@ -1672,14 +1678,15 @@ int lmpc_select_host(lmpc_handle* h, const double* x0, double* SS_sel, double* Q
 // One device-resident step for the whole batch on the handle's stream: K1 -> K2 -> QP -> shift (PC.py:110-137).  ev (five events
 // or null) brackets the four kernels for lmpc_step_profile.  retire: the lap budgets (the closed loop) or none; vsched, ssched: the
 // vehicle and surface lap schedules a mode 2 prediction model follows (the closed loop) or none.
+// flags_cleared: the caller cleared the step flags before a kernel of its own set some (the state observer), so they stay.
 static int step_dev_impl(lmpc_handle* h, int mode, const double* x0_dev, cudaEvent_t* ev, LapBudget retire = {},
-                         LapSchedule vsched = {}, LapSchedule ssched = {}) {
+                         LapSchedule vsched = {}, LapSchedule ssched = {}, bool flags_cleared = false) {
     int rc = need_store(h);
     if (rc) return rc;
     if (!x0_dev || (mode != 0 && mode != 1)) return fail(LMPC_E_INVALID, "bad mode or null x0");
     if (mode == 1 && h->M <= 0) return fail(LMPC_E_INVALID, "LMPC step on a handle without a safe set");
     cudaStream_t st = h->stream;
-    CK(cudaMemsetAsync(h->d_flags, 0, sizeof(int) * h->batch, st));
+    if (!flags_cleared) CK(cudaMemsetAsync(h->d_flags, 0, sizeof(int) * h->batch, st));
     if (h->d_warm && h->warm_mode != mode) {             // records of the other problem type are not comparable
         CK(cudaMemsetAsync(h->d_warm_valid, 0, sizeof(int) * h->batch, st));
         h->warm_mode = mode;
@@ -1858,9 +1865,26 @@ static int measure(lmpc_handle* h, unsigned long long seed, LapBudget retire, La
     return LMPC_OK;
 }
 
+// The state the controllers read this step (DESIGN.md, "Per-controller state observers"): with an observer table, *y becomes
+// x_hat, which observe_kernel forms from *y and the controllers' previous predictions; without one, *y stays and nothing runs.
+// blend: a step of mode 0 or 1 (the step flags are cleared before the launch, so a reset flag survives); else a PID or LTI step.
+static int observe(lmpc_handle* h, bool blend, LapBudget retire, const double** y) {
+    if (!h->obs.tab) return LMPC_OK;
+    if (blend) CK(cudaMemsetAsync(h->d_flags, 0, sizeof(int) * h->batch, h->stream));
+    ObserveArgs oa;
+    oa.batch = h->batch; oa.N = h->N; oa.blend = blend ? 1 : 0; oa.y = *y; oa.xPredPrev = h->d_xPredPrev; oa.has_pred = h->d_hasPred;
+    oa.x_est = h->d_xest; oa.flags = h->d_flags; oa.obs = h->obs.view(); oa.trk = tracks(h); oa.retire = retire;
+    observe_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(oa);
+    CK(cudaGetLastError());
+    h->launches += 1;
+    *y = h->d_xest;
+    return LMPC_OK;
+}
+
 // One closed-loop step for every instance, all on the device (SysModel.py:34-48):
 //   Controller.solve(x) -> u = uPred[0] -> Controller.addPoint(x, u) (LMPC) -> x+ = dynModel(x, x_glob, u); done = s+ > TrackLength
-// The controller's x (solve, addPoint, the record) is the measured state y when a measurement table is installed.
+// The controller's x (solve, addPoint, the record) is the measured state y when a measurement table is installed, and the
+// observer's x_hat formed from it when an observer table is installed.
 int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned long long seed) {
     int rc = need_rollout(h);
     if (rc) return rc;
@@ -1869,6 +1893,7 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
     const LapBudget retire = lap_budget(h);
     const double* y = nullptr;
     if ((rc = measure(h, seed, retire, lap_schedule(h, LMPC_SCHEDULE_MEASUREMENT), &y)) != LMPC_OK) return rc;
+    if ((rc = observe(h, mode != 2, retire, &y)) != LMPC_OK) return rc;
     if (z_host) CK(cudaMemcpyAsync(h->d_z, z_host, sizeof(double) * h->batch * 3, cudaMemcpyHostToDevice, h->stream));
     if (mode == 2) {
         CK(cudaMemsetAsync(h->d_flags, 0, sizeof(int) * h->batch, h->stream));
@@ -1879,7 +1904,8 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
         io.xPred = q.xPred; io.uPred = q.uPred; io.slack = q.slack; io.status = q.status; io.iters = q.iters; io.resid = q.resid;
         rc = solve_dev(h, io, 54, 0, retire);
     } else {
-        rc = step_dev_impl(h, mode, y, nullptr, retire, lap_schedule(h, LMPC_SCHEDULE_VEHICLE), lap_schedule(h, LMPC_SCHEDULE_SURFACE));
+        rc = step_dev_impl(h, mode, y, nullptr, retire, lap_schedule(h, LMPC_SCHEDULE_VEHICLE), lap_schedule(h, LMPC_SCHEDULE_SURFACE),
+                           h->obs.tab != nullptr);
     }
     if (rc) return rc;
     if (mode == 1) {                                                                 // SysModel.py:38 -> PC.py:466-476
@@ -1897,7 +1923,7 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
     }
     SimArgs sa = sim_args(h, z_host ? h->d_z : nullptr, seed);                       // SysModel.py:40 (dynModel)
     sa.flags = h->d_flags; sa.status = q.status; sa.health = h->d_health; sa.retire = retire;
-    if (h->meas.tab) sa.rec_x = y;
+    if (h->meas.tab || h->obs.tab) sa.rec_x = y;
     (h->surf.tab ? sim_step_kernel<true> : sim_step_kernel<false>)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(
         h->mc, sa, reports(h), q.iters, lap_schedule(h, LMPC_SCHEDULE_VEHICLE), lap_schedule(h, LMPC_SCHEDULE_NOISE), h->surf.view(),
         lap_schedule(h, LMPC_SCHEDULE_SURFACE));
@@ -1913,8 +1939,9 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
 // NULL = Philox on the device.
 int lmpc_rollout_pid_step(lmpc_handle* h, double vt, const double* z_pid_host, const double* z_sim_host, unsigned long long seed) {
     if (int rc = need_rollout(h)) return rc;
-    const double* y = nullptr;                   // the PID's input and the record's state rows (measure)
+    const double* y = nullptr;                   // the PID's input and the record's state rows (measure, observe)
     if (int rc = measure(h, seed, LapBudget{}, LapSchedule{}, &y)) return rc;
+    if (int rc = observe(h, false, LapBudget{}, &y)) return rc;
     if (z_pid_host) CK(cudaMemcpyAsync(h->d_zpid, z_pid_host, sizeof(double) * h->batch * 2, cudaMemcpyHostToDevice, h->stream));
     if (z_sim_host) CK(cudaMemcpyAsync(h->d_z, z_sim_host, sizeof(double) * h->batch * 3, cudaMemcpyHostToDevice, h->stream));
     PidArgs pa;
@@ -1924,7 +1951,7 @@ int lmpc_rollout_pid_step(lmpc_handle* h, double vt, const double* z_pid_host, c
     pid_input_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(pa);
     SimArgs sa = sim_args(h, z_sim_host ? h->d_z : nullptr, seed);
     sa.health = h->d_health;          // no step flags or QP status here: only the simulator's own bits
-    if (h->meas.tab) sa.rec_x = y;
+    if (h->meas.tab || h->obs.tab) sa.rec_x = y;
     (h->surf.tab ? sim_step_kernel<true> : sim_step_kernel<false>)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(
         h->mc, sa, reports(h), nullptr, LapSchedule{}, LapSchedule{}, h->surf.view(), LapSchedule{});
     CK(cudaGetLastError());
@@ -2035,6 +2062,24 @@ int lmpc_rollout_set_measurement_noise(lmpc_handle* h, const lmpc_measurement_pa
                 return fail(LMPC_E_INVALID, std::string(who) + ": measurement set " + std::to_string(k) +
                                                 ": every sigma and clip must be finite and >= 0");
         row = sets[k];
+        return LMPC_OK;
+    });
+}
+
+// Per-controller state observers: mode 0 or 1, every gain finite and in [0, 1]; nsets == 0 removes the table (the controllers
+// read the measured or plant state, no kernel runs).
+int lmpc_rollout_set_observers(lmpc_handle* h, const lmpc_observer_params* sets, int nsets, const int* set_of_instance) {
+    static const char* who = "lmpc_rollout_set_observers";
+    if (int rc = need_rollout(h)) return rc;
+    return install_table(h, who, h->obs, sets, nsets, set_of_instance, (const lmpc_observer_params*)nullptr,
+                         [&](int k, lmpc_observer_params& row) {
+        const lmpc_observer_params& o = sets[k];
+        const std::string w = std::string(who) + ": observer " + std::to_string(k);
+        if (o.mode != 0 && o.mode != 1) return fail(LMPC_E_INVALID, w + ": mode must be 0 or 1");
+        for (double l : o.gain)
+            if (!(isfinite(l) && l >= 0.0 && l <= 1.0)) return fail(LMPC_E_INVALID, w + ": every gain must be finite and in [0, 1]");
+        row = o;
+        row.pad = 0;
         return LMPC_OK;
     });
 }

@@ -629,6 +629,12 @@ struct K2Args {
     SsLaps laps;             // numSS_it_b of every controller: warps c >= numSS_it_b select nothing
 };
 
+// Lap-wrap fix of a guess of s made before the finish line (PC.py:392-393): after a hand-over the state's s has moved back by
+// TrackLength and the guess has not.  K2's terminal guess and the state observer's prior (observe_kernel) both take it.
+__device__ __forceinline__ void wrap_guess_s(double& guess_s, double x_s, double TrackLength) {
+    if (guess_s - x_s > TrackLength / 2) guess_s = fmax(guess_s - TrackLength, 0.0);
+}
+
 // One CTA per instance, one warp per selected lap.  SHAPED: a shape table or a lap-count table (or both) is installed.
 template <bool SHAPED>
 __global__ void __launch_bounds__(32 * 8) ss_select_kernel(const K2Args a) {
@@ -645,7 +651,7 @@ __global__ void __launch_bounds__(32 * 8) ss_select_kernel(const K2Args a) {
     double z[6];
 #pragma unroll
     for (int j = 0; j < 6; ++j) z[j] = a.zt[(size_t)b * 6 + j];
-    if (z[4] - a.x0[(size_t)b * 6 + 4] > TrackLength / 2) z[4] = fmax(z[4] - TrackLength, 0.0);
+    wrap_guess_s(z[4], a.x0[(size_t)b * 6 + 4], TrackLength);
     if (c == 0 && lane < 6) a.zt_fixed[(size_t)b * 6 + lane] = z[lane];
 
     const int slot = a.sel[(size_t)b * a.numSS_it + c];
@@ -1232,6 +1238,60 @@ __global__ void measure_kernel(const MeasArgs a, const LapSchedule meas_s) {
     for (int j = 0; j < 6; ++j) {
         const double n = fmax(-m.clip[j], fmin(z[j] * m.sigma[j], m.clip[j]));
         y[j] = n == 0.0 ? x[j] : x[j] + n;
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// State observers (DESIGN.md, "Per-controller state observers"): the state x_hat a controller reads, blended from the state it
+// is given, y, and its own one-step prediction p = xPred[1] of its previous QP (row 1 of xPredPrev), with the fixed gains of its
+// row: x_hat_j = p_j + l_j (y_j - p_j), each operation rounded on its own (no contraction), l_j == 1 copying y_j and l_j == 0
+// taking p_j.  p_s gets K2's lap-wrap fix first.  No prior (has_pred == 0), a mode 0 row or a step that is not an LMPC / LTV step
+// gives x_hat = y exactly; a non-finite prior on a channel with l_j < 1 gives x_hat = y and LMPC_FLAG_OBSERVER_RESET.  In a PID
+// or LTI step (blend == 0) a mode 1 row also clears has_pred: xPredPrev is not shifted there and would be stale next step.  One
+// thread per controller; a retired controller reads, writes and flags nothing.  The observer has no state of its own.
+struct ObserveArgs {
+    int batch, N;
+    int blend;                     // 1: a step of mode 0 or 1; 0: a PID step or a step of mode 2
+    const double* y;               // [B][6] the state the controllers are given (x_meas, or the plant state)
+    const double* xPredPrev;       // [B][N+1][6] the previous QP's prediction
+    int* has_pred;                 // [B]
+    double* x_est;                 // [B][6] x_hat
+    int* flags;                    // [B] step flags, cleared before this launch (blend == 1)
+    Table<lmpc_observer_params> obs;
+    Tracks trk;
+    LapBudget retire;
+};
+__global__ void observe_kernel(const ObserveArgs a) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= a.batch || a.retire.retired(b)) return;
+    const lmpc_observer_params& o = a.obs.of(b);
+    const double* y = a.y + (size_t)b * 6;
+    double* xe = a.x_est + (size_t)b * 6;
+    const bool on = o.mode == 1;
+    if (on && !a.blend) a.has_pred[b] = 0;
+    double yv[6], p[6];
+#pragma unroll
+    for (int j = 0; j < 6; ++j) yv[j] = y[j];
+    bool prior = on && a.blend && a.has_pred[b];
+    if (prior) {
+        const double* pp = a.xPredPrev + ((size_t)b * (a.N + 1) + 1) * 6;
+#pragma unroll
+        for (int j = 0; j < 6; ++j) p[j] = pp[j];
+        wrap_guess_s(p[4], yv[4], a.trk.of(b).TrackLength);
+        bool finite = true;
+#pragma unroll
+        for (int j = 0; j < 6; ++j) finite = finite && (o.gain[j] == 1.0 || isfinite(p[j]));
+        if (!finite) {
+            a.flags[b] |= LMPC_FLAG_OBSERVER_RESET;
+            prior = false;
+        }
+    }
+#pragma unroll
+    for (int j = 0; j < 6; ++j) {
+        const double l = o.gain[j];
+        double v = yv[j];
+        if (prior && l != 1.0) v = l == 0.0 ? p[j] : __dadd_rn(p[j], __dmul_rn(l, __dsub_rn(yv[j], p[j])));
+        xe[j] = v;
     }
 }
 

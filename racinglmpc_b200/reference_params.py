@@ -1,5 +1,6 @@
 """The reference's tuning constants, values only (src/initControllerParameters.py:4-58, src/main.py:43-50).
 They define the benchmark configurations of BASELINE.json; nothing here is executed by the reference."""
+import math
 from dataclasses import dataclass
 from types import SimpleNamespace
 import numpy as np
@@ -107,6 +108,52 @@ class MeasurementParams:
     def scaled(cls, k, base):
         """``base`` with every sigma and clip multiplied by ``k``: 1 gives ``base`` bit for bit, 0 no noise."""
         return cls(tuple(v * k for v in base.sigma), tuple(v * k for v in base.clip))
+
+
+@dataclass(frozen=True)
+class ObserverParams:
+    """A fixed-gain state observer (no reference counterpart): a mode 1 controller reads x_hat_j = p_j + gain_j (y_j - p_j) on
+    the six curvilinear channels (vx, vy, wz, epsi, s, ey) in place of the state y it is given (measured or true), p being its own
+    one-step prediction xPred[1] of the previous step.  Gain 1 trusts the measurement, gain 0 the prediction.  Mode 0 reads y.
+    The device closed loop takes one per controller (BatchedController.set_observers)."""
+    mode: int = 0
+    gain: tuple = (1.0,) * 6
+
+    @classmethod
+    def off(cls):
+        """No observer: installed, the controllers read the state they are given, bit for bit."""
+        return cls(0, (1.0,) * 6)
+
+    @classmethod
+    def uniform(cls, l):
+        """An observer with gain ``l`` on every channel (1 reads y bit for bit)."""
+        return cls(1, (float(l),) * 6)
+
+    @classmethod
+    def gains(cls, vx, vy, wz, epsi, s, ey):
+        """An observer with one gain per channel."""
+        return cls(1, tuple(float(v) for v in (vx, vy, wz, epsi, s, ey)))
+
+    @classmethod
+    def from_noise(cls, model_sigma, meas_sigma):
+        """Per channel, the steady-state Kalman gain of a scalar random walk x_{k+1} = x_k + w (w of standard deviation
+        model_sigma) measured as y = x + v (v of standard deviation meas_sigma): with q = model_sigma^2 and r = meas_sigma^2 the
+        prior variance solves P = P r / (P + r) + q, so P = (q + sqrt(q^2 + 4 q r)) / 2, and l = P / (P + r).  meas_sigma == 0
+        gives l = 1 (a perfect sensor), and model_sigma == 0 with meas_sigma > 0 gives l = 0.  Each argument is one value for
+        every channel or six."""
+        ms = np.broadcast_to(np.asarray(model_sigma, float), (6,))
+        rs = np.broadcast_to(np.asarray(meas_sigma, float), (6,))
+        if not (np.all(np.isfinite(ms)) and np.all(np.isfinite(rs)) and np.all(ms >= 0) and np.all(rs >= 0)):
+            raise ValueError("model_sigma and meas_sigma must be finite and >= 0")
+        out = []
+        for m, s in zip(ms, rs):
+            q, r = float(m) * float(m), float(s) * float(s)
+            if r == 0.0:
+                out.append(1.0)
+                continue
+            P = (q + math.sqrt(q * q + 4.0 * q * r)) / 2.0
+            out.append(P / (P + r))
+        return cls(1, tuple(out))
 
 
 @dataclass(frozen=True)
