@@ -471,7 +471,8 @@ int lmpc_read_buffer(lmpc_handle* h, const char* name, size_t offset_bytes, void
  * terminal slack [B,6] of the most recent step), "abc_lti", "x_meas" (the measured state [B,6] of the closed loop's current
  * step under lmpc_rollout_set_measurement_noise), "x_est" (the state [B,6] the controllers read in that step under
  * lmpc_rollout_set_observers), "xPredPrev" (the previous step's prediction [B,N+1,6]) and "has_pred" (int [B]: 1 when it is
- * one), the observer's prior. */
+ * one), the observer's prior, and "x_prior" (the prior [B,6] the observer formed in that step under
+ * lmpc_rollout_set_observer_priors). */
 void* lmpc_device_buffer(lmpc_handle* h, const char* name);
 
 /* ===== device-resident closed loop (the caller of the hot path, SURVEY §8f rank 1) =======================================
@@ -682,6 +683,41 @@ typedef struct lmpc_observer_params {
  *     table continues exactly.
  *   - The host-driven entry points (lmpc_step_*, lmpc_solve_*) take the caller's x0 and are not affected. */
 int lmpc_rollout_set_observers(lmpc_handle* h, const lmpc_observer_params* sets, int nsets, const int* set_of_instance);
+/* Where a mode 1 observer takes its prior from (DESIGN.md, "Observer priors").  The row mirrors lmpc_prediction_model_params:
+ * "a believed car" and "the plant's own car" mean the same in both tables. */
+typedef struct lmpc_observer_prior_params {
+    int source;                   /* 0 own plan (xPred[1] of the previous QP), 1 a believed car: `vehicle`, 2 the plant's own car */
+    int pad;
+    lmpc_vehicle_params vehicle;  /* read under source 1 only */
+} lmpc_observer_prior_params;
+/* Per-controller observer priors.  Controller b reads row sets[set_of_instance[b]] (host arrays); nsets == 0 (sets,
+ * set_of_instance NULL) removes the table, which every handle starts without.  The table changes what the observer kernel of
+ * lmpc_rollout_set_observers computes and adds no launch; without an observer table it is stored and does nothing.
+ *   - Source 0: the prior is the controller's own plan, exactly as without a prior table (bit for bit).
+ *   - Sources 1 and 2, in a rollout step of mode 0 or 1, for a controller whose observer row is mode 1 with has_pred == 1 and a
+ *     gain below 1: the prior is p = Phi_car(xPredPrev[b][0], OldInput[b]), the estimate the controller read in its previous
+ *     step (row 0 of its previous QP's prediction is its x0) carried over one control period under the input applied in that
+ *     step.  Phi_car is the simulator's noise-free control period on the six curvilinear states: its sub-step loop (h = 0.001 s
+ *     while (i + 1) h <= dt, the reference's lf in alpha_r, the same curvature lookup) with the same expressions, without the
+ *     global frame and the process noise.
+ *       source 1  the row's `vehicle`, no surface (prediction model mode 1);
+ *       source 2  the vehicle row and, with a surface table, the surface row the plant drove the previous step with, both through
+ *                 their lap schedules.  That step's lap is lap_n - 1 when xPredPrev[b][0].s - y.s > TrackLength / 2 (a hand-over
+ *                 came in between and moved lap_n on), else lap_n.
+ *     Then, as for source 0: the lap-wrap fix of p_s against y_s and the blend x_hat_j = p_j + l_j (y_j - p_j).
+ *   - The prior is not used (x_hat = y and the step sets LMPC_FLAG_OBSERVER_RESET) when an input of Phi (xPredPrev[b][0],
+ *     OldInput[b]) is not finite, a sub-step's curvature lookup failed, or p_j is not finite on a channel with l_j < 1.  A row
+ *     whose gains are all 1 forms no prior and never sets the flag.
+ *   - "x_prior" [B,6] (lmpc_read_buffer) holds the prior the observer formed in the current step, after the lap-wrap fix, for
+ *     every controller that is not retired, and NaN where it formed none.  It is written only while a prior table is installed.
+ *   - 1 <= nsets <= batch, every index in [0, nsets); source 0, 1 or 2; under source 1 all ten vehicle values finite and
+ *     m, lf, lr, Iz > 0.
+ *   - Needs lmpc_rollout_create (LMPC_E_STATE otherwise); any failed check returns LMPC_E_INVALID.  Every refusal leaves the
+ *     handle as it was.
+ *   - The call synchronises the handle's streams before it replaces the table.  It is allowed at any time and applies from the
+ *     next step on.  Not schedulable and not part of a snapshot record (LMPC_SNAPSHOT_VERSION is unchanged): the prior's inputs
+ *     (xPredPrev, OldInput, has_pred) are already part of every record. */
+int lmpc_rollout_set_observer_priors(lmpc_handle* h, const lmpc_observer_prior_params* sets, int nsets, const int* set_of_instance);
 /* Lap budgets: controller b is retired once it has handed over budget_of_instance[b] laps (lmpc_rollout_commit_laps_dev counts
  * them: lap_n of lmpc_books_get).  A retired controller keeps the state that hand-over left it in (lap filed, books refreshed,
  * record restarted: the start line of its next lap) and no kernel of lmpc_rollout_step (modes 0, 1, 2) or
@@ -921,6 +957,7 @@ int lmpc_sizeof_track_params(void);
 int lmpc_sizeof_noise_params(void);
 int lmpc_sizeof_measurement_params(void);
 int lmpc_sizeof_observer_params(void);
+int lmpc_sizeof_observer_prior_params(void);
 int lmpc_sizeof_regression_params(void);
 int lmpc_sizeof_shape_params(void);
 int lmpc_sizeof_ss_laps_params(void);

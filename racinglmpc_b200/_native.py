@@ -95,6 +95,12 @@ class PredictionModelParams(C.Structure):
     _fields_ = [("mode", C.c_int), ("pad", C.c_int), ("vehicle", VehicleParams)]
 
 
+class ObserverPriorParams(C.Structure):
+    """lmpc_observer_prior_params: where a mode 1 observer takes its prior from -- source 0 its own plan, source 1 the
+    simulator's noise-free control period for ``vehicle``, source 2 that of the plant's own vehicle and surface rows."""
+    _fields_ = [("source", C.c_int), ("pad", C.c_int), ("vehicle", VehicleParams)]
+
+
 MAX_ZONES = 16                      # LMPC_MAX_ZONES: zones of one track-surface row
 
 
@@ -245,6 +251,7 @@ def lib():
     L.lmpc_rollout_set_noise_streams.argtypes = [_vp, _vp]
     L.lmpc_rollout_set_measurement_noise.argtypes = [_vp, C.POINTER(MeasurementParams), C.c_int, _vp]
     L.lmpc_rollout_set_observers.argtypes = [_vp, C.POINTER(ObserverParams), C.c_int, _vp]
+    L.lmpc_rollout_set_observer_priors.argtypes = [_vp, C.POINTER(ObserverPriorParams), C.c_int, _vp]
     L.lmpc_rollout_set_lap_budget.argtypes = [_vp, _vp]
     L.lmpc_rollout_enable_lap_reports.argtypes = [_vp, C.c_int]
     L.lmpc_rollout_get_lap_reports.argtypes = [_vp, _vp, _vp]
@@ -317,6 +324,8 @@ def lib():
     assert L.lmpc_sizeof_measurement_params() == C.sizeof(MeasurementParams), "lmpc_measurement_params ABI mismatch"
     L.lmpc_sizeof_observer_params.restype = C.c_int
     assert L.lmpc_sizeof_observer_params() == C.sizeof(ObserverParams), "lmpc_observer_params ABI mismatch"
+    L.lmpc_sizeof_observer_prior_params.restype = C.c_int
+    assert L.lmpc_sizeof_observer_prior_params() == C.sizeof(ObserverPriorParams), "lmpc_observer_prior_params ABI mismatch"
     assert L.lmpc_sizeof_regression_params() == C.sizeof(RegressionParams), "lmpc_regression_params ABI mismatch"
     assert L.lmpc_sizeof_params() == C.sizeof(Params), "lmpc_params ABI mismatch"
     assert L.lmpc_sizeof_model_params() == C.sizeof(ModelParams), "lmpc_model_params ABI mismatch"
@@ -625,6 +634,31 @@ def make_observer_sets(observers, index, batch):
         r.gain[:] = g.tolist()
         return r
     return _pack_sets(ObserverParams, observers, index, batch, "observers", row)
+
+
+def make_observer_prior_sets(priors, index, batch):
+    """Per-controller observer priors for ``lmpc_rollout_set_observer_priors``: K objects ``priors`` with ``source`` (0 own plan,
+    1 a believed car, 2 the plant's car) and ``vehicle`` (an object with the reference's ten vehicle field names, read under
+    source 1; e.g. reference_params.ObserverPrior) and the row of every controller ``index[batch]``.  Raises ValueError where the
+    library would refuse: the index rules of ``make_param_sets``, a source that is not the integer 0, 1 or 2, or a source 1
+    vehicle with a value that is not finite or with m, lf, lr or Iz not positive.  Returns (ctypes array ObserverPriorParams * K,
+    int32 index array)."""
+    def row(k, r):
+        src = r.source
+        if isinstance(src, (bool, np.bool_)) or not isinstance(src, (int, np.integer)) or int(src) not in (0, 1, 2):
+            raise ValueError("observer prior %d: source must be 0, 1 or 2, got %r" % (k, src))
+        if int(src) != 1:
+            return ObserverPriorParams(int(src), 0, VehicleParams())
+        vals = []
+        for f in VEHICLE_FIELDS:
+            v = getattr(r.vehicle, f)
+            if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, float, np.integer, np.floating)) or not np.isfinite(float(v)):
+                raise ValueError("observer prior %d: vehicle %s must be a finite number, got %r" % (k, f, v))
+            vals.append(float(v))
+        if min(vals[0], vals[1], vals[2], vals[3]) <= 0:
+            raise ValueError("observer prior %d: a source 1 vehicle needs m, lf, lr and Iz > 0" % k)
+        return ObserverPriorParams(1, 0, VehicleParams(*vals))
+    return _pack_sets(ObserverPriorParams, priors, index, batch, "observer priors", row)
 
 
 def _int_per_controller(values, batch, lo, what):

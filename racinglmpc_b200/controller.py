@@ -290,6 +290,20 @@ class BatchedController:
         self._install(self._lib.lmpc_rollout_set_observers, "observers", observers, index,
                       lambda: nat.make_observer_sets(observers, index, self.B))
 
+    def set_observer_priors(self, priors=None, index=None):
+        """Where the state observers (``set_observers``) take their prior from, per controller: ``priors[index[b]]`` (objects with
+        ``source`` and ``vehicle``, e.g. reference_params.ObserverPrior).  Source 0 is the controller's own plan xPred[1], exactly
+        as without a table.  Sources 1 and 2 carry the estimate the controller read in its previous step, xPredPrev[0], over one
+        control period under the input it applied, OldInput, with the simulator's noise-free map: source 1 for ``vehicle``
+        without a surface, source 2 for the plant's own vehicle and surface rows of that step (through their lap schedules).
+        The prior then gets the lap-wrap fix and the observer's blend.  A non-finite input or prior, or a failed curvature
+        lookup, gives x_hat = y and FLAG_OBSERVER_RESET.  The prior of the step is ``read_buffer("x_prior", ...)`` (NaN where
+        none was formed).  ``index`` is required with ``priors``; ``priors=None`` (no index) removes the table.  Adds no launch;
+        without an observer table it does nothing.  Needs ``enable_rollout``; allowed in the middle of a run; not part of a
+        snapshot.  ValueError before any native call where the library would refuse a value.  Waits for work already enqueued."""
+        self._install(self._lib.lmpc_rollout_set_observer_priors, "priors", priors, index,
+                      lambda: nat.make_observer_prior_sets(priors, index, self.B))
+
     def set_lap_budget(self, budget=None):
         """Lap budgets of the device closed loop: controller b retires once it has handed over ``budget[b]`` laps (one integer
         >= 1 for the whole batch, or one per controller).  A retired controller keeps the state its last hand-over left it in and

@@ -17,6 +17,12 @@ struct LapSchedule {
         if (!rows) return t.of(b);
         return t.tab[rows[(size_t)b * L + min(lap_n[b], L - 1)]];
     }
+    // the row of lap lap_n[b] - back (back 0 or 1: the observer's model prior looks at the step before a hand-over)
+    template <typename T>
+    __device__ __forceinline__ const T& of_before(const Table<T>& t, int b, int back) const {
+        if (!rows) return t.of(b);
+        return t.tab[rows[(size_t)b * L + min(max(lap_n[b] - back, 0), L - 1)]];
+    }
 };
 
 }  // namespace lmpc

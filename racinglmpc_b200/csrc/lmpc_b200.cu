@@ -179,6 +179,10 @@ struct lmpc_handle {
     // the state the controllers read in the current step (observe_kernel).
     HandleTable<lmpc_observer_params> obs;
     double* d_xest;
+    // where the observers take their prior from (lmpc_rollout_set_observer_priors), or none: their own plan.  d_xprior is the prior
+    // formed in the current step (observe_kernel<true>).
+    HandleTable<lmpc_observer_prior_params> opri;
+    double* d_xprior;
     // lap budgets (lmpc_rollout_set_lap_budget): laps every controller drives before it retires, or none for no budget
     HandleTable<int> budget;
     // track surfaces of the simulator (lmpc_rollout_set_surfaces), or none: the vehicle's grip all round the lap
@@ -271,6 +275,7 @@ static std::vector<DevBuf> dev_bufs(lmpc_handle* h) {
         dbuf(h->d_abc_lti, 54, R, FILL_ZERO, SN_ABC_LTI, "abc_lti"), dbuf(h->d_z, 3, R), dbuf(h->d_zpid, 2, R),
         dbuf(h->d_xmeas, 6, R, FILL_ZERO, SN_SCRATCH, "x_meas"),     // formed from the plant state and the clock every step
         dbuf(h->d_xest, 6, R, FILL_ZERO, SN_SCRATCH, "x_est"),       // formed from x_meas and xPredPrev every step
+        dbuf(h->d_xprior, 6, R, FILL_ZERO, SN_SCRATCH, "x_prior"),   // formed from xPredPrev and OldInput every step (prior table)
         // per-lap reports (lap_reports_reset_kernel gives the running rows their start)
         dbuf(h->d_rep_rows, (size_t)h->rep_L, OWN_REPORTS, FILL_ZERO, SN_LAP_REPORTS), dbuf(h->d_rep_run, 1, OWN_REPORTS, FILL_ZERO, SN_LAP_RUN),
         // lane margins (lmpc_set_lane_margins; lane_margin_rows_kernel fills them)
@@ -296,7 +301,7 @@ static void free_tables(lmpc_handle* h, unsigned owners) {
         t.rows.clear(); t.index.clear();
     };
     release(h->sets, OWN_HANDLE); release(h->veh, OWN_HANDLE); release(h->noise, OWN_HANDLE); release(h->streams, OWN_HANDLE);
-    release(h->meas, OWN_HANDLE); release(h->obs, OWN_HANDLE); release(h->surf, OWN_HANDLE); release(h->budget, OWN_HANDLE); release(h->trk, OWN_STORE); release(h->reg, OWN_STORE); release(h->pool_grp, OWN_STORE);
+    release(h->meas, OWN_HANDLE); release(h->obs, OWN_HANDLE); release(h->opri, OWN_HANDLE); release(h->surf, OWN_HANDLE); release(h->budget, OWN_HANDLE); release(h->trk, OWN_STORE); release(h->reg, OWN_STORE); release(h->pool_grp, OWN_STORE);
     for (auto& t : h->sched) release(t, OWN_HANDLE);
     release(h->shp, OWN_STORE); release(h->shp_order, OWN_STORE); release(h->own_c, OWN_HANDLE); release(h->ssl, OWN_STORE);
     release(h->lwin, OWN_STORE); release(h->lrule, OWN_STORE); release(h->lmar, OWN_STORE); release(h->pmod, OWN_STORE);
@@ -1055,6 +1060,7 @@ int lmpc_sizeof_vehicle_params(void) { return (int)sizeof(lmpc_vehicle_params); 
 int lmpc_sizeof_noise_params(void) { return (int)sizeof(lmpc_noise_params); }
 int lmpc_sizeof_measurement_params(void) { return (int)sizeof(lmpc_measurement_params); }
 int lmpc_sizeof_observer_params(void) { return (int)sizeof(lmpc_observer_params); }
+int lmpc_sizeof_observer_prior_params(void) { return (int)sizeof(lmpc_observer_prior_params); }
 int lmpc_sizeof_regression_params(void) { return (int)sizeof(lmpc_regression_params); }
 int lmpc_sizeof_shape_params(void) { return (int)sizeof(lmpc_shape_params); }
 int lmpc_sizeof_ss_laps_params(void) { return (int)sizeof(lmpc_ss_laps_params); }
@@ -1868,13 +1874,18 @@ static int measure(lmpc_handle* h, unsigned long long seed, LapBudget retire, La
 // The state the controllers read this step (DESIGN.md, "Per-controller state observers"): with an observer table, *y becomes
 // x_hat, which observe_kernel forms from *y and the controllers' previous predictions; without one, *y stays and nothing runs.
 // blend: a step of mode 0 or 1 (the step flags are cleared before the launch, so a reset flag survives); else a PID or LTI step.
-static int observe(lmpc_handle* h, bool blend, LapBudget retire, const double** y) {
+// With a prior table (DESIGN.md, "Observer priors") the MODEL instantiation runs: vsched, ssched are the plant's vehicle and
+// surface lap schedules.
+static int observe(lmpc_handle* h, bool blend, LapBudget retire, const double** y, LapSchedule vsched = {}, LapSchedule ssched = {}) {
     if (!h->obs.tab) return LMPC_OK;
     if (blend) CK(cudaMemsetAsync(h->d_flags, 0, sizeof(int) * h->batch, h->stream));
     ObserveArgs oa;
     oa.batch = h->batch; oa.N = h->N; oa.blend = blend ? 1 : 0; oa.y = *y; oa.xPredPrev = h->d_xPredPrev; oa.has_pred = h->d_hasPred;
     oa.x_est = h->d_xest; oa.flags = h->d_flags; oa.obs = h->obs.view(); oa.trk = tracks(h); oa.retire = retire;
-    observe_kernel<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(oa);
+    ObservePrior op;
+    op.pri = h->opri.view(); op.dt = h->mc.dt; op.OldInput = h->d_OldInput; op.x_prior = h->d_xprior;
+    op.veh = h->veh.view(); op.veh_s = vsched; op.surf = h->surf.view(); op.surf_s = ssched;
+    (h->opri.tab ? observe_kernel<true> : observe_kernel<false>)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(oa, op);
     CK(cudaGetLastError());
     h->launches += 1;
     *y = h->d_xest;
@@ -1893,7 +1904,8 @@ int lmpc_rollout_step(lmpc_handle* h, int mode, const double* z_host, unsigned l
     const LapBudget retire = lap_budget(h);
     const double* y = nullptr;
     if ((rc = measure(h, seed, retire, lap_schedule(h, LMPC_SCHEDULE_MEASUREMENT), &y)) != LMPC_OK) return rc;
-    if ((rc = observe(h, mode != 2, retire, &y)) != LMPC_OK) return rc;
+    if ((rc = observe(h, mode != 2, retire, &y, lap_schedule(h, LMPC_SCHEDULE_VEHICLE), lap_schedule(h, LMPC_SCHEDULE_SURFACE))) != LMPC_OK)
+        return rc;
     if (z_host) CK(cudaMemcpyAsync(h->d_z, z_host, sizeof(double) * h->batch * 3, cudaMemcpyHostToDevice, h->stream));
     if (mode == 2) {
         CK(cudaMemsetAsync(h->d_flags, 0, sizeof(int) * h->batch, h->stream));
@@ -2080,6 +2092,30 @@ int lmpc_rollout_set_observers(lmpc_handle* h, const lmpc_observer_params* sets,
             if (!(isfinite(l) && l >= 0.0 && l <= 1.0)) return fail(LMPC_E_INVALID, w + ": every gain must be finite and in [0, 1]");
         row = o;
         row.pad = 0;
+        return LMPC_OK;
+    });
+}
+
+// Per-controller observer priors: source 0, 1 or 2; under source 1 all ten vehicle values finite and m, lf, lr, Iz > 0 (the
+// rule of a mode 1 prediction model); nsets == 0 removes the table (every observer takes its own plan, observe_kernel<false>).
+int lmpc_rollout_set_observer_priors(lmpc_handle* h, const lmpc_observer_prior_params* sets, int nsets, const int* set_of_instance) {
+    static const char* who = "lmpc_rollout_set_observer_priors";
+    if (int rc = need_rollout(h)) return rc;
+    return install_table(h, who, h->opri, sets, nsets, set_of_instance, (const lmpc_observer_prior_params*)nullptr,
+                         [&](int k, lmpc_observer_prior_params& r) {
+        const lmpc_observer_prior_params& s = sets[k];
+        const lmpc_vehicle_params& v = s.vehicle;
+        const std::string w = std::string(who) + ": row " + std::to_string(k) + ": ";
+        if (s.source < 0 || s.source > 2) return fail(LMPC_E_INVALID, w + "source must be 0, 1 or 2");
+        memset(&r, 0, sizeof(r));
+        r.source = s.source;
+        if (s.source == 1) {
+            const double all[10] = {v.m, v.lf, v.lr, v.Iz, v.Df, v.Cf, v.Bf, v.Dr, v.Cr, v.Br};
+            for (double x : all)
+                if (!isfinite(x)) return fail(LMPC_E_INVALID, w + "all ten vehicle values must be finite");
+            if (!(v.m > 0 && v.lf > 0 && v.lr > 0 && v.Iz > 0)) return fail(LMPC_E_INVALID, w + "a source 1 vehicle needs m, lf, lr, Iz > 0");
+            r.vehicle = v;
+        }
         return LMPC_OK;
     });
 }

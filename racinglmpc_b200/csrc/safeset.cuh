@@ -1063,6 +1063,36 @@ __device__ __forceinline__ void surface_forces(SurfaceCursor& zc, double s, doub
     }
 }
 
+// One explicit-Euler sub-step of Simulator.dynModel (SysModel.py:94-137), with the reference's lf in alpha_r: the curvilinear
+// state (vx, vy, wz, epsi, s, ey) and, GLOBAL, the global pose (psi, X, Y), all updated from the sub-step's starting state.  Dfi,
+// Dri are the sub-step's peak tyre forces (surface_forces), sd, cd = sin, cos(delta).  A failed curvature lookup clears *okc.
+// sim_step_kernel and the observer's model prior (sim_period) both take it, so the prior is the plant's arithmetic exactly.
+template <bool GLOBAL>
+__device__ __forceinline__ void sim_substep(double mass, double lf, double lr, double Iz, double Dfi, double Cf, double Bf,
+                                            double Dri, double Cr, double Br, double delta, double acc, double sd, double cd,
+                                            double h, const TrackRec& trk, int* okc, double& vx, double& vy, double& wz,
+                                            double& epsi, double& s, double& ey, double& psi, double& X, double& Y) {
+    const double af = delta - atan2(vy + lf * wz, vx);
+    const double ar = -atan2(vy - lf * wz, vx);
+    const double Fyf = Dfi * sin(Cf * atan(Bf * af));
+    const double Fyr = Dri * sin(Cr * atan(Br * ar));
+    const double nvx = vx + h * (acc - 1 / mass * Fyf * sd + wz * vy);
+    const double nvy = vy + h * (1 / mass * (Fyf * cd + Fyr) - wz * vx);
+    const double nwz = wz + h * (1 / Iz * (lf * Fyf * cd - lr * Fyr));
+    if constexpr (GLOBAL) {
+        const double npsi = psi + h * wz;
+        const double nX = X + h * (vx * cos(psi) - vy * sin(psi));
+        const double nY = Y + h * (vx * sin(psi) + vy * cos(psi));
+        psi = npsi; X = nX; Y = nY;
+    }
+    const double cur = curvature_lookup(trk, s, okc);
+    const double ce = cos(epsi), se = sin(epsi);
+    const double nepsi = epsi + h * (wz - (vx * ce - vy * se) / (1 - cur * ey) * cur);
+    const double ns = s + h * ((vx * ce - vy * se) / (1 - cur * ey));
+    const double ney = ey + h * (vx * se + vy * ce);
+    vx = nvx; vy = nvy; wz = nwz; epsi = nepsi; s = ns; ey = ney;
+}
+
 // With reports (rep.rows) the step is also added to the controller's running report row (report_step) with its QP's status
 // a.status and iterations rep_iters, both null for a PID step.  The vehicle and noise rows come from the lap schedules veh_s and
 // noise_s (lap_schedule.cuh; a null schedule reads the table's own index).  SURF (a surface table is installed): each sub-step's
@@ -1118,23 +1148,8 @@ __global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimA
     while ((i + 1) * h <= m.dt) {
         double Dfi = Df, Dri = Dr;
         if constexpr (SURF) surface_forces(zc, s, trk.TrackLength, Df, Dr, &Dfi, &Dri);
-        const double af = delta - atan2(vy + lf * wz, vx);
-        const double ar = -atan2(vy - lf * wz, vx);
-        const double Fyf = Dfi * sin(Cf * atan(Bf * af));
-        const double Fyr = Dri * sin(Cr * atan(Br * ar));
-        const double nvx = vx + h * (acc - 1 / mass * Fyf * sd + wz * vy);
-        const double nvy = vy + h * (1 / mass * (Fyf * cd + Fyr) - wz * vx);
-        const double nwz = wz + h * (1 / Iz * (lf * Fyf * cd - lr * Fyr));
-        const double npsi = psi + h * wz;
-        const double nX = X + h * (vx * cos(psi) - vy * sin(psi));
-        const double nY = Y + h * (vx * sin(psi) + vy * cos(psi));
-        const double cur = curvature_lookup(trk, s, &okc);
-        const double ce = cos(epsi), se = sin(epsi);
-        const double nepsi = epsi + h * (wz - (vx * ce - vy * se) / (1 - cur * ey) * cur);
-        const double ns = s + h * ((vx * ce - vy * se) / (1 - cur * ey));
-        const double ney = ey + h * (vx * se + vy * ce);
-        psi = npsi; X = nX; Y = nY;
-        vx = nvx; vy = nvy; wz = nwz; epsi = nepsi; s = ns; ey = ney;
+        sim_substep<true>(mass, lf, lr, Iz, Dfi, Cf, Bf, Dri, Cr, Br, delta, acc, sd, cd, h, trk, &okc, vx, vy, wz, epsi, s, ey,
+                          psi, X, Y);
         ++i;
     }
     if (!okc) sim_bits |= SIM_LOOKUP_FAILED;
@@ -1249,6 +1264,8 @@ __global__ void measure_kernel(const MeasArgs a, const LapSchedule meas_s) {
 // gives x_hat = y exactly; a non-finite prior on a channel with l_j < 1 gives x_hat = y and LMPC_FLAG_OBSERVER_RESET.  In a PID
 // or LTI step (blend == 0) a mode 1 row also clears has_pred: xPredPrev is not shifted there and would be stale next step.  One
 // thread per controller; a retired controller reads, writes and flags nothing.  The observer has no state of its own.
+// MODEL (a prior table is installed, DESIGN.md, "Observer priors"): a row of source 1 or 2 takes the model prior
+// p = Phi_car(xPredPrev[0], OldInput) (sim_period) in place of the plan, and the kernel writes the prior it formed to x_prior.
 struct ObserveArgs {
     int batch, N;
     int blend;                     // 1: a step of mode 0 or 1; 0: a PID step or a step of mode 2
@@ -1261,7 +1278,68 @@ struct ObserveArgs {
     Tracks trk;
     LapBudget retire;
 };
-__global__ void observe_kernel(const ObserveArgs a) {
+// What the MODEL instantiation reads besides (a second kernel parameter: the instantiation without a prior table keeps the code
+// it had before this feature)
+struct ObservePrior {
+    Table<lmpc_observer_prior_params> pri;   // the prior source of every controller
+    double dt;                               // the control period (ModelConst::dt)
+    const double* OldInput;                  // [B][2] the input applied in the previous step
+    double* x_prior;                         // [B][6] the prior formed (NaN: none)
+    Table<lmpc_vehicle_params> veh;          // the simulator's vehicle table and lap schedule (source 2)
+    LapSchedule veh_s;
+    Table<lmpc_surface_params> surf;         // the simulator's surface table (tab null: none) and lap schedule (source 2)
+    LapSchedule surf_s;
+};
+
+// Phi_car: the simulator's noise-free control period on the curvilinear state x under the input (delta, acc) -- sim_step_kernel's
+// sub-step loop with car v and, when zones is not null, its surface row, without the global frame.  false when a sub-step's
+// curvature lookup failed.
+__device__ __forceinline__ bool sim_period(const lmpc_vehicle_params& v, const TrackRec& trk, const lmpc_surface_params* zones,
+                                           double dt, double delta, double acc, double (&x)[6]) {
+    const double mass = v.m, lf = v.lf, lr = v.lr, Iz = v.Iz;
+    const double Df = v.Df, Cf = v.Cf, Bf = v.Bf;
+    const double Dr = v.Dr, Cr = v.Cr, Br = v.Br;
+    const double h = 0.001;
+    const double sd = sin(delta), cd = cos(delta);
+    double vx = x[0], vy = x[1], wz = x[2], epsi = x[3], s = x[4], ey = x[5];
+    double psi = 0.0, X = 0.0, Y = 0.0;
+    int i = 0;
+    int okc = 1;
+    SurfaceCursor zc{zones, 0};
+    while ((i + 1) * h <= dt) {
+        double Dfi = Df, Dri = Dr;
+        if (zones) surface_forces(zc, s, trk.TrackLength, Df, Dr, &Dfi, &Dri);
+        sim_substep<false>(mass, lf, lr, Iz, Dfi, Cf, Bf, Dri, Cr, Br, delta, acc, sd, cd, h, trk, &okc, vx, vy, wz, epsi, s, ey,
+                           psi, X, Y);
+        ++i;
+    }
+    x[0] = vx; x[1] = vy; x[2] = wz; x[3] = epsi; x[4] = s; x[5] = ey;
+    return okc != 0;
+}
+
+// The model prior of controller b (source 1: the row's car, no surface; source 2: the car and surface the plant drove the
+// previous step with -- the lap before lap_n when a hand-over came in between, seen as x_hat_{k-1}.s - y.s > TrackLength / 2).
+// false when an input is not finite or a curvature lookup failed.
+__device__ __forceinline__ bool model_prior(const ObserveArgs& a, const ObservePrior& m, int b, const lmpc_observer_prior_params& r,
+                                            const double (&yv)[6], double (&p)[6]) {
+    const double* xp = a.xPredPrev + (size_t)b * (a.N + 1) * 6;
+    const double delta = m.OldInput[(size_t)b * 2], acc = m.OldInput[(size_t)b * 2 + 1];
+    bool finite = isfinite(delta) && isfinite(acc);
+#pragma unroll
+    for (int j = 0; j < 6; ++j) {
+        p[j] = xp[j];
+        finite = finite && isfinite(p[j]);
+    }
+    const TrackRec& trk = a.trk.of(b);
+    const int back = p[4] - yv[4] > trk.TrackLength / 2 ? 1 : 0;
+    const bool plant = r.source == 2;
+    const lmpc_vehicle_params& v = plant ? m.veh_s.of_before(m.veh, b, back) : r.vehicle;
+    const lmpc_surface_params* zones = plant && m.surf.tab ? &m.surf_s.of_before(m.surf, b, back) : nullptr;
+    return sim_period(v, trk, zones, m.dt, delta, acc, p) && finite;
+}
+
+template <bool MODEL>
+__global__ void observe_kernel(const ObserveArgs a, const ObservePrior m) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= a.batch || a.retire.retired(b)) return;
     const lmpc_observer_params& o = a.obs.of(b);
@@ -1273,18 +1351,38 @@ __global__ void observe_kernel(const ObserveArgs a) {
 #pragma unroll
     for (int j = 0; j < 6; ++j) yv[j] = y[j];
     bool prior = on && a.blend && a.has_pred[b];
-    if (prior) {
-        const double* pp = a.xPredPrev + ((size_t)b * (a.N + 1) + 1) * 6;
+    if constexpr (MODEL) {       // a row whose gains are all 1 forms no prior
+        bool reads = false;
 #pragma unroll
-        for (int j = 0; j < 6; ++j) p[j] = pp[j];
+        for (int j = 0; j < 6; ++j) reads = reads || o.gain[j] != 1.0;
+        prior = prior && reads;
+    }
+    const bool formed = prior;
+    if (prior) {
+        bool model = false, ok = true;
+        if constexpr (MODEL) {
+            const lmpc_observer_prior_params& r = m.pri.of(b);
+            model = r.source != 0;
+            if (model) ok = model_prior(a, m, b, r, yv, p);
+        }
+        if (!model) {
+            const double* pp = a.xPredPrev + ((size_t)b * (a.N + 1) + 1) * 6;
+#pragma unroll
+            for (int j = 0; j < 6; ++j) p[j] = pp[j];
+        }
         wrap_guess_s(p[4], yv[4], a.trk.of(b).TrackLength);
-        bool finite = true;
+        bool finite = ok;
 #pragma unroll
         for (int j = 0; j < 6; ++j) finite = finite && (o.gain[j] == 1.0 || isfinite(p[j]));
         if (!finite) {
             a.flags[b] |= LMPC_FLAG_OBSERVER_RESET;
             prior = false;
         }
+    }
+    if constexpr (MODEL) {
+        double* xq = m.x_prior + (size_t)b * 6;
+#pragma unroll
+        for (int j = 0; j < 6; ++j) xq[j] = formed ? p[j] : __longlong_as_double(0x7ff8000000000000ll);
     }
 #pragma unroll
     for (int j = 0; j < 6; ++j) {

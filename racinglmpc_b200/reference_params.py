@@ -248,6 +248,32 @@ class PredictionModelParams:
 
 
 @dataclass(frozen=True)
+class ObserverPrior:
+    """Where a state observer (ObserverParams mode 1) takes its prior from (no reference counterpart): source 0 the controller's
+    own plan (its previous QP's xPred[1]), source 1 the estimate of the previous step carried over one control period under the
+    input applied, by the simulator's noise-free map for ``vehicle`` (a car the controller believes it drives, no surface),
+    source 2 the same map for the plant's own vehicle and surface rows.  The device takes one per controller
+    (BatchedController.set_observer_priors)."""
+    source: int = 0
+    vehicle: VehicleParams = VehicleParams.reference()
+
+    @classmethod
+    def plan(cls):
+        """The controller's own plan: installed, the observers compute exactly what they compute without a table."""
+        return cls(0)
+
+    @classmethod
+    def car(cls, vehicle):
+        """The one-period map of ``vehicle``, whatever the plant drives."""
+        return cls(1, vehicle)
+
+    @classmethod
+    def plant(cls):
+        """The one-period map of the car and surface the plant drove the previous step with."""
+        return cls(2)
+
+
+@dataclass(frozen=True)
 class SurfaceParams:
     """A track surface (no reference counterpart: the reference's grip is the same all round the lap): up to 16 zones
     (s_start, s_end, mu_f, mu_r), ascending without overlap, in the s-coordinate of the controller's track.  A simulator sub-step
