@@ -471,8 +471,9 @@ int lmpc_read_buffer(lmpc_handle* h, const char* name, size_t offset_bytes, void
  * terminal slack [B,6] of the most recent step), "abc_lti", "x_meas" (the measured state [B,6] of the closed loop's current
  * step under lmpc_rollout_set_measurement_noise), "x_est" (the state [B,6] the controllers read in that step under
  * lmpc_rollout_set_observers), "xPredPrev" (the previous step's prediction [B,N+1,6]) and "has_pred" (int [B]: 1 when it is
- * one), the observer's prior, and "x_prior" (the prior [B,6] the observer formed in that step under
- * lmpc_rollout_set_observer_priors). */
+ * one), the observer's prior, "x_prior" (the prior [B,6] the observer formed in that step under
+ * lmpc_rollout_set_observer_priors), and "obs_jac", "obs_cov", "obs_gain" (A, P and K [B,6,6] of the step's model gains under
+ * lmpc_rollout_set_observer_gains). */
 void* lmpc_device_buffer(lmpc_handle* h, const char* name);
 
 /* ===== device-resident closed loop (the caller of the hot path, SURVEY §8f rank 1) =======================================
@@ -712,12 +713,51 @@ typedef struct lmpc_observer_prior_params {
  *     every controller that is not retired, and NaN where it formed none.  It is written only while a prior table is installed.
  *   - 1 <= nsets <= batch, every index in [0, nsets); source 0, 1 or 2; under source 1 all ten vehicle values finite and
  *     m, lf, lr, Iz > 0.
+ *   - While an observer gain table (lmpc_rollout_set_observer_gains) gives a controller a mode 1 row, a table or a removal that
+ *     would give that controller source 0 is refused.
  *   - Needs lmpc_rollout_create (LMPC_E_STATE otherwise); any failed check returns LMPC_E_INVALID.  Every refusal leaves the
  *     handle as it was.
  *   - The call synchronises the handle's streams before it replaces the table.  It is allowed at any time and applies from the
  *     next step on.  Not schedulable and not part of a snapshot record (LMPC_SNAPSHOT_VERSION is unchanged): the prior's inputs
  *     (xPredPrev, OldInput, has_pred) are already part of every record. */
 int lmpc_rollout_set_observer_priors(lmpc_handle* h, const lmpc_observer_prior_params* sets, int nsets, const int* set_of_instance);
+/* Model-based observer gains (DESIGN.md, "Observer gains"): the frozen-time Kalman gain of the linearised car in place of the
+ * observer row's fixed gains. */
+#define LMPC_FLAG_OBSERVER_GAIN 4096         /* step flag: the model gain could not be formed, the controller read y */
+typedef struct lmpc_observer_gain_params {
+    int mode;                     /* 0 the observer row's fixed gains, 1 model gains */
+    int pad;
+    double q[6];                  /* process covariance diagonal per control period, (vx, vy, wz, epsi, s, ey); read under mode 1 */
+    double r[6];                  /* measurement covariance diagonal; read under mode 1 */
+} lmpc_observer_gain_params;
+/* Per-controller observer gains.  Controller b reads row sets[set_of_instance[b]] (host arrays); nsets == 0 (sets,
+ * set_of_instance NULL) removes the table, which every handle starts without.
+ *   - Mode 0: the observer computes exactly what it computes without a gain table (bit for bit).
+ *   - Mode 1, in a rollout step of mode 0 or 1, for a controller whose observer row is mode 1 with has_pred == 1 (its prior row is
+ *     source 1 or 2, see below): the prior p = Phi_car(xPredPrev[b][0], OldInput[b]) of lmpc_rollout_set_observer_priors,
+ *     unchanged, and the Jacobian A = dPhi_car/dx [6,6] at the same point, by forward mode through the same sub-steps and
+ *     expressions (the curvature and the surface zones' forces, piecewise constant in s, count as constants; the input is not
+ *     differentiated).  P solves the filter DARE P = A P A' - A P (P + R)^-1 P A' + Q, Q = diag(q), R = diag(r) (structured
+ *     doubling in fp64, at most 64 doublings, stopped once max|H' - H| <= 1e-13 max|H'|), and K = P (P + R)^-1.  After the
+ *     lap-wrap fix of p_s: e_j = y_j - p_j and x_hat_i = p_i + (K_i0 e_0 + K_i1 e_1 + ... + K_i5 e_5), summed left to right,
+ *     every product and sum rounded on its own.  The observer row's gains are not read.  There is no covariance carried from
+ *     step to step (this is not an extended Kalman filter): the gain is a function of the step's own inputs.
+ *   - A non-finite input, a failed curvature lookup or a non-finite p gives x_hat = y and LMPC_FLAG_OBSERVER_RESET, as without a
+ *     gain table.  A non-finite A, P or K, or a DARE that did not converge, gives x_hat = y and LMPC_FLAG_OBSERVER_GAIN, which
+ *     reaches the health word and the lap reports like every step flag.  PID and mode 2 steps clear has_pred and read y.
+ *   - "obs_jac", "obs_cov", "obs_gain" [B,6,6] (lmpc_read_buffer) hold A, P and K of the current step for every controller that
+ *     is not retired, NaN where no model gain was formed (K also where A, P or K is not finite or the DARE did not converge).
+ *   - With a gain table installed, every lmpc_rollout_step of mode 0 or 1 with an observer table launches one more kernel,
+ *     between the measurement and the observer kernels; PID and mode 2 steps launch none.
+ *   - 1 <= nsets <= batch, every index in [0, nsets); mode 0 or 1; under mode 1 every q_j and r_j finite and > 0 (the DARE then
+ *     has a unique stabilising solution).  A mode 1 row for a controller without an observer prior table, or whose prior row is
+ *     source 0, is refused; while such rows are installed, lmpc_rollout_set_observer_priors refuses a table or a removal that
+ *     would give one of those controllers source 0.
+ *   - Needs lmpc_rollout_create (LMPC_E_STATE otherwise); any failed check returns LMPC_E_INVALID.  Every refusal leaves the
+ *     handle as it was.
+ *   - The call synchronises the handle's streams before it replaces the table.  It is allowed at any time and applies from the
+ *     next step on.  Not schedulable and not part of a snapshot record (LMPC_SNAPSHOT_VERSION is unchanged). */
+int lmpc_rollout_set_observer_gains(lmpc_handle* h, const lmpc_observer_gain_params* sets, int nsets, const int* set_of_instance);
 /* Lap budgets: controller b is retired once it has handed over budget_of_instance[b] laps (lmpc_rollout_commit_laps_dev counts
  * them: lap_n of lmpc_books_get).  A retired controller keeps the state that hand-over left it in (lap filed, books refreshed,
  * record restarted: the start line of its next lap) and no kernel of lmpc_rollout_step (modes 0, 1, 2) or
@@ -958,6 +998,7 @@ int lmpc_sizeof_noise_params(void);
 int lmpc_sizeof_measurement_params(void);
 int lmpc_sizeof_observer_params(void);
 int lmpc_sizeof_observer_prior_params(void);
+int lmpc_sizeof_observer_gain_params(void);
 int lmpc_sizeof_regression_params(void);
 int lmpc_sizeof_shape_params(void);
 int lmpc_sizeof_ss_laps_params(void);

@@ -95,6 +95,13 @@ class PredictionModelParams(C.Structure):
     _fields_ = [("mode", C.c_int), ("pad", C.c_int), ("vehicle", VehicleParams)]
 
 
+class ObserverGainParams(C.Structure):
+    """lmpc_observer_gain_params: the gains a mode 1 observer blends with -- mode 0 its row's fixed gains, mode 1 the frozen-time
+    Kalman gain of the linearised car for the diagonal process covariance ``q`` (per control period) and measurement covariance
+    ``r`` over (vx, vy, wz, epsi, s, ey)."""
+    _fields_ = [("mode", C.c_int), ("pad", C.c_int), ("q", C.c_double * 6), ("r", C.c_double * 6)]
+
+
 class ObserverPriorParams(C.Structure):
     """lmpc_observer_prior_params: where a mode 1 observer takes its prior from -- source 0 its own plan, source 1 the
     simulator's noise-free control period for ``vehicle``, source 2 that of the plant's own vehicle and surface rows."""
@@ -112,6 +119,7 @@ class SurfaceParams(C.Structure):
 
 FLAG_NOMINAL_NONFINITE = 1024       # LMPC_FLAG_NOMINAL_NONFINITE: step flag of a nominal controller whose rows 0..2 are not finite
 FLAG_OBSERVER_RESET = 2048          # LMPC_FLAG_OBSERVER_RESET: step flag of an observer whose prior was not finite (it read y)
+FLAG_OBSERVER_GAIN = 4096           # LMPC_FLAG_OBSERVER_GAIN: step flag of an observer whose model gain could not be formed (it read y)
 LANE_UNSAFE_KEY = 1 << 24           # LMPC_LANE_UNSAFE_KEY: added to the safe-set key of a lane-unsafe lap
 REPORT_LANE_UNSAFE = 1 << 16        # LMPC_REPORT_LANE_UNSAFE: report flag of an own lap judged lane-unsafe
 
@@ -252,6 +260,7 @@ def lib():
     L.lmpc_rollout_set_measurement_noise.argtypes = [_vp, C.POINTER(MeasurementParams), C.c_int, _vp]
     L.lmpc_rollout_set_observers.argtypes = [_vp, C.POINTER(ObserverParams), C.c_int, _vp]
     L.lmpc_rollout_set_observer_priors.argtypes = [_vp, C.POINTER(ObserverPriorParams), C.c_int, _vp]
+    L.lmpc_rollout_set_observer_gains.argtypes = [_vp, C.POINTER(ObserverGainParams), C.c_int, _vp]
     L.lmpc_rollout_set_lap_budget.argtypes = [_vp, _vp]
     L.lmpc_rollout_enable_lap_reports.argtypes = [_vp, C.c_int]
     L.lmpc_rollout_get_lap_reports.argtypes = [_vp, _vp, _vp]
@@ -326,6 +335,8 @@ def lib():
     assert L.lmpc_sizeof_observer_params() == C.sizeof(ObserverParams), "lmpc_observer_params ABI mismatch"
     L.lmpc_sizeof_observer_prior_params.restype = C.c_int
     assert L.lmpc_sizeof_observer_prior_params() == C.sizeof(ObserverPriorParams), "lmpc_observer_prior_params ABI mismatch"
+    L.lmpc_sizeof_observer_gain_params.restype = C.c_int
+    assert L.lmpc_sizeof_observer_gain_params() == C.sizeof(ObserverGainParams), "lmpc_observer_gain_params ABI mismatch"
     assert L.lmpc_sizeof_regression_params() == C.sizeof(RegressionParams), "lmpc_regression_params ABI mismatch"
     assert L.lmpc_sizeof_params() == C.sizeof(Params), "lmpc_params ABI mismatch"
     assert L.lmpc_sizeof_model_params() == C.sizeof(ModelParams), "lmpc_model_params ABI mismatch"
@@ -634,6 +645,33 @@ def make_observer_sets(observers, index, batch):
         r.gain[:] = g.tolist()
         return r
     return _pack_sets(ObserverParams, observers, index, batch, "observers", row)
+
+
+def make_observer_gain_sets(gains, index, batch):
+    """Per-controller observer gains for ``lmpc_rollout_set_observer_gains``: K objects ``gains`` with ``mode`` (0 the observer
+    row's fixed gains, 1 model gains) and, read under mode 1, ``q`` and ``r`` (six values each over vx, vy, wz, epsi, s, ey; e.g.
+    reference_params.ObserverGains), and the row of every controller ``index[batch]``.  Raises ValueError where the library would
+    refuse a row: the index rules of ``make_param_sets``, a mode that is not the integer 0 or 1, or under mode 1 a q or r of the
+    wrong length or with a value that is not finite and > 0.  (The library also refuses a mode 1 row for a controller without a
+    source 1 or 2 observer prior; that needs the handle and is raised by its call.)  Returns (ctypes array ObserverGainParams *
+    K, int32 index array)."""
+    def row(k, o):
+        mode = o.mode
+        if isinstance(mode, (bool, np.bool_)) or not isinstance(mode, (int, np.integer)) or int(mode) not in (0, 1):
+            raise ValueError("observer gains %d: mode must be 0 or 1, got %r" % (k, mode))
+        r = ObserverGainParams()
+        r.mode = int(mode)
+        if r.mode == 0:
+            return r
+        for f in ("q", "r"):
+            v = np.asarray(getattr(o, f), dtype=float).reshape(-1)
+            if v.shape[0] != 6:
+                raise ValueError("observer gains %d: %s needs 6 values, got %d" % (k, f, v.shape[0]))
+            if not np.all(np.isfinite(v)) or np.any(v <= 0):
+                raise ValueError("observer gains %d: every %s must be finite and > 0" % (k, f))
+            getattr(r, f)[:] = v.tolist()
+        return r
+    return _pack_sets(ObserverGainParams, gains, index, batch, "observer gains", row)
 
 
 def make_observer_prior_sets(priors, index, batch):

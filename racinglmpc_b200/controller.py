@@ -304,6 +304,20 @@ class BatchedController:
         self._install(self._lib.lmpc_rollout_set_observer_priors, "priors", priors, index,
                       lambda: nat.make_observer_prior_sets(priors, index, self.B))
 
+    def set_observer_gains(self, gains=None, index=None):
+        """Which gains the state observers (``set_observers``) blend with, per controller: ``gains[index[b]]`` (objects with
+        ``mode``, ``q`` and ``r``, e.g. reference_params.ObserverGains).  Mode 0 keeps the observer row's fixed gains, exactly as
+        without a table.  Mode 1, for a controller whose observer prior (``set_observer_priors``) is a car (source 1 or 2): every
+        step of mode 0 or 1 linearises the prior's one-period map at its point, A = dPhi/dx, solves the filter DARE for that A
+        with Q = diag(q), R = diag(r), and blends x_hat = p + K (y - p) with K = P (P + R)^-1.  No covariance is carried from step
+        to step.  A, P and K of the step are ``read_buffer("obs_jac" / "obs_cov" / "obs_gain", ...)`` [B, 6, 6], NaN where no gain
+        was formed; a gain that could not be formed gives x_hat = y and FLAG_OBSERVER_GAIN.  One more launch per step of mode 0 or
+        1.  ``index`` is required with ``gains``; ``gains=None`` (no index) removes the table.  Needs ``enable_rollout``; allowed
+        in the middle of a run; not part of a snapshot.  ValueError before any native call where the library would refuse a
+        row; NativeError for a mode 1 row of a controller without a car prior.  Waits for work already enqueued."""
+        self._install(self._lib.lmpc_rollout_set_observer_gains, "gains", gains, index,
+                      lambda: nat.make_observer_gain_sets(gains, index, self.B))
+
     def set_lap_budget(self, budget=None):
         """Lap budgets of the device closed loop: controller b retires once it has handed over ``budget[b]`` laps (one integer
         >= 1 for the whole batch, or one per controller).  A retired controller keeps the state its last hand-over left it in and

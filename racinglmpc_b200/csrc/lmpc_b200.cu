@@ -103,6 +103,9 @@ struct HandleTable {
     std::vector<int> index;
     Table<T> view() const { return Table<T>{tab, idx}; }
 };
+// the row controller b reads from t (which has rows)
+template <typename T>
+static int table_row(const HandleTable<T>& t, int b) { return t.index.empty() ? 0 : t.index[b]; }
 
 struct lmpc_handle {
     lmpc_params p;
@@ -183,6 +186,10 @@ struct lmpc_handle {
     // formed in the current step (observe_kernel<true>).
     HandleTable<lmpc_observer_prior_params> opri;
     double* d_xprior;
+    // the observers' gains (lmpc_rollout_set_observer_gains), or none: every observer row's fixed gains.  d_ojac, d_ocov, d_ogain
+    // are A, P and K of the current step's model gains (observer_gain_kernel).
+    HandleTable<lmpc_observer_gain_params> ogain;
+    double *d_ojac, *d_ocov, *d_ogain;
     // lap budgets (lmpc_rollout_set_lap_budget): laps every controller drives before it retires, or none for no budget
     HandleTable<int> budget;
     // track surfaces of the simulator (lmpc_rollout_set_surfaces), or none: the vehicle's grip all round the lap
@@ -276,6 +283,9 @@ static std::vector<DevBuf> dev_bufs(lmpc_handle* h) {
         dbuf(h->d_xmeas, 6, R, FILL_ZERO, SN_SCRATCH, "x_meas"),     // formed from the plant state and the clock every step
         dbuf(h->d_xest, 6, R, FILL_ZERO, SN_SCRATCH, "x_est"),       // formed from x_meas and xPredPrev every step
         dbuf(h->d_xprior, 6, R, FILL_ZERO, SN_SCRATCH, "x_prior"),   // formed from xPredPrev and OldInput every step (prior table)
+        dbuf(h->d_ojac, 36, R, FILL_ZERO, SN_SCRATCH, "obs_jac"),    // formed from xPredPrev, OldInput and the rows every step (gain table)
+        dbuf(h->d_ocov, 36, R, FILL_ZERO, SN_SCRATCH, "obs_cov"),
+        dbuf(h->d_ogain, 36, R, FILL_ZERO, SN_SCRATCH, "obs_gain"),
         // per-lap reports (lap_reports_reset_kernel gives the running rows their start)
         dbuf(h->d_rep_rows, (size_t)h->rep_L, OWN_REPORTS, FILL_ZERO, SN_LAP_REPORTS), dbuf(h->d_rep_run, 1, OWN_REPORTS, FILL_ZERO, SN_LAP_RUN),
         // lane margins (lmpc_set_lane_margins; lane_margin_rows_kernel fills them)
@@ -301,7 +311,7 @@ static void free_tables(lmpc_handle* h, unsigned owners) {
         t.rows.clear(); t.index.clear();
     };
     release(h->sets, OWN_HANDLE); release(h->veh, OWN_HANDLE); release(h->noise, OWN_HANDLE); release(h->streams, OWN_HANDLE);
-    release(h->meas, OWN_HANDLE); release(h->obs, OWN_HANDLE); release(h->opri, OWN_HANDLE); release(h->surf, OWN_HANDLE); release(h->budget, OWN_HANDLE); release(h->trk, OWN_STORE); release(h->reg, OWN_STORE); release(h->pool_grp, OWN_STORE);
+    release(h->meas, OWN_HANDLE); release(h->obs, OWN_HANDLE); release(h->opri, OWN_HANDLE); release(h->ogain, OWN_HANDLE); release(h->surf, OWN_HANDLE); release(h->budget, OWN_HANDLE); release(h->trk, OWN_STORE); release(h->reg, OWN_STORE); release(h->pool_grp, OWN_STORE);
     for (auto& t : h->sched) release(t, OWN_HANDLE);
     release(h->shp, OWN_STORE); release(h->shp_order, OWN_STORE); release(h->own_c, OWN_HANDLE); release(h->ssl, OWN_STORE);
     release(h->lwin, OWN_STORE); release(h->lrule, OWN_STORE); release(h->lmar, OWN_STORE); release(h->pmod, OWN_STORE);
@@ -1061,6 +1071,7 @@ int lmpc_sizeof_noise_params(void) { return (int)sizeof(lmpc_noise_params); }
 int lmpc_sizeof_measurement_params(void) { return (int)sizeof(lmpc_measurement_params); }
 int lmpc_sizeof_observer_params(void) { return (int)sizeof(lmpc_observer_params); }
 int lmpc_sizeof_observer_prior_params(void) { return (int)sizeof(lmpc_observer_prior_params); }
+int lmpc_sizeof_observer_gain_params(void) { return (int)sizeof(lmpc_observer_gain_params); }
 int lmpc_sizeof_regression_params(void) { return (int)sizeof(lmpc_regression_params); }
 int lmpc_sizeof_shape_params(void) { return (int)sizeof(lmpc_shape_params); }
 int lmpc_sizeof_ss_laps_params(void) { return (int)sizeof(lmpc_ss_laps_params); }
@@ -1875,7 +1886,8 @@ static int measure(lmpc_handle* h, unsigned long long seed, LapBudget retire, La
 // x_hat, which observe_kernel forms from *y and the controllers' previous predictions; without one, *y stays and nothing runs.
 // blend: a step of mode 0 or 1 (the step flags are cleared before the launch, so a reset flag survives); else a PID or LTI step.
 // With a prior table (DESIGN.md, "Observer priors") the MODEL instantiation runs: vsched, ssched are the plant's vehicle and
-// surface lap schedules.
+// surface lap schedules.  With a gain table as well (DESIGN.md, "Observer gains") observer_gain_kernel forms the model gains first
+// in a step of mode 0 or 1, and the GAIN instantiation blends with them.
 static int observe(lmpc_handle* h, bool blend, LapBudget retire, const double** y, LapSchedule vsched = {}, LapSchedule ssched = {}) {
     if (!h->obs.tab) return LMPC_OK;
     if (blend) CK(cudaMemsetAsync(h->d_flags, 0, sizeof(int) * h->batch, h->stream));
@@ -1885,7 +1897,16 @@ static int observe(lmpc_handle* h, bool blend, LapBudget retire, const double** 
     ObservePrior op;
     op.pri = h->opri.view(); op.dt = h->mc.dt; op.OldInput = h->d_OldInput; op.x_prior = h->d_xprior;
     op.veh = h->veh.view(); op.veh_s = vsched; op.surf = h->surf.view(); op.surf_s = ssched;
-    (h->opri.tab ? observe_kernel<true> : observe_kernel<false>)<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(oa, op);
+    ObserveGain og;
+    og.gains = h->ogain.view(); og.jac = h->d_ojac; og.cov = h->d_ocov; og.gain = h->d_ogain;
+    if (h->ogain.tab && blend) {
+        constexpr int per_block = OBS_GAIN_WARPS * OBS_GAIN_PER_WARP;
+        observer_gain_kernel<<<(h->batch + per_block - 1) / per_block, 32 * OBS_GAIN_WARPS, 0, h->stream>>>(oa, op, og);
+        CK(cudaGetLastError());
+        h->launches += 1;
+    }
+    auto kern = !h->opri.tab ? observe_kernel<false, false> : h->ogain.tab ? observe_kernel<true, true> : observe_kernel<true, false>;
+    kern<<<(h->batch + 127) / 128, 128, 0, h->stream>>>(oa, op, og);
     CK(cudaGetLastError());
     h->launches += 1;
     *y = h->d_xest;
@@ -2101,6 +2122,15 @@ int lmpc_rollout_set_observers(lmpc_handle* h, const lmpc_observer_params* sets,
 int lmpc_rollout_set_observer_priors(lmpc_handle* h, const lmpc_observer_prior_params* sets, int nsets, const int* set_of_instance) {
     static const char* who = "lmpc_rollout_set_observer_priors";
     if (int rc = need_rollout(h)) return rc;
+    if (h->ogain.tab) {        // a mode 1 gain row needs a model prior: the table, or its removal, must not take it away
+        if (int rc = check_set_index(h, who, sets, nsets, set_of_instance)) return rc;
+        for (int b = 0; b < h->batch; ++b) {
+            if (h->ogain.rows[table_row(h->ogain, b)].mode != 1) continue;
+            if (nsets == 0 || sets[set_of_instance[b]].source == 0)
+                return fail(LMPC_E_INVALID, std::string(who) + ": controller " + std::to_string(b) +
+                                                " has a mode 1 observer gain row (lmpc_rollout_set_observer_gains), which needs source 1 or 2");
+        }
+    }
     return install_table(h, who, h->opri, sets, nsets, set_of_instance, (const lmpc_observer_prior_params*)nullptr,
                          [&](int k, lmpc_observer_prior_params& r) {
         const lmpc_observer_prior_params& s = sets[k];
@@ -2115,6 +2145,35 @@ int lmpc_rollout_set_observer_priors(lmpc_handle* h, const lmpc_observer_prior_p
                 if (!isfinite(x)) return fail(LMPC_E_INVALID, w + "all ten vehicle values must be finite");
             if (!(v.m > 0 && v.lf > 0 && v.lr > 0 && v.Iz > 0)) return fail(LMPC_E_INVALID, w + "a source 1 vehicle needs m, lf, lr, Iz > 0");
             r.vehicle = v;
+        }
+        return LMPC_OK;
+    });
+}
+
+// Per-controller observer gains: mode 0 or 1; under mode 1 every q_j and r_j finite and > 0, and the controller's observer prior
+// row source 1 or 2 (check_gain_priors); nsets == 0 removes the table (every observer blends with its row's fixed gains).
+int lmpc_rollout_set_observer_gains(lmpc_handle* h, const lmpc_observer_gain_params* sets, int nsets, const int* set_of_instance) {
+    static const char* who = "lmpc_rollout_set_observer_gains";
+    if (int rc = need_rollout(h)) return rc;
+    if (int rc = check_set_index(h, who, sets, nsets, set_of_instance)) return rc;
+    for (int b = 0; b < (nsets > 0 ? h->batch : 0); ++b) {
+        if (sets[set_of_instance[b]].mode != 1) continue;
+        if (!h->opri.tab || h->opri.rows[table_row(h->opri, b)].source == 0)
+            return fail(LMPC_E_INVALID, std::string(who) + ": controller " + std::to_string(b) +
+                                            ": a mode 1 row needs an observer prior of source 1 or 2 (lmpc_rollout_set_observer_priors)");
+    }
+    return install_table(h, who, h->ogain, sets, nsets, set_of_instance, (const lmpc_observer_gain_params*)nullptr,
+                         [&](int k, lmpc_observer_gain_params& r) {
+        const lmpc_observer_gain_params& s = sets[k];
+        const std::string w = std::string(who) + ": row " + std::to_string(k) + ": ";
+        if (s.mode != 0 && s.mode != 1) return fail(LMPC_E_INVALID, w + "mode must be 0 or 1");
+        memset(&r, 0, sizeof(r));
+        r.mode = s.mode;
+        if (s.mode == 1) {
+            for (int j = 0; j < 6; ++j)
+                if (!(isfinite(s.q[j]) && s.q[j] > 0.0 && isfinite(s.r[j]) && s.r[j] > 0.0))
+                    return fail(LMPC_E_INVALID, w + "every q and r must be finite and > 0");
+            for (int j = 0; j < 6; ++j) { r.q[j] = s.q[j]; r.r[j] = s.r[j]; }
         }
         return LMPC_OK;
     });

@@ -273,6 +273,65 @@ class ObserverPrior:
         return cls(2)
 
 
+def clipped_normal_variance(sigma, clip):
+    """Var(clip(sigma Z, +-clip)) for a standard normal Z: with a = clip / sigma, sigma^2 [(1 - 2 Phi(-a)) - 2 a phi(a)] +
+    2 clip^2 Phi(-a) (the variance of the noise the simulator and the sensor add).  0 when sigma or clip is 0."""
+    sigma, clip = float(sigma), float(clip)
+    if sigma == 0.0 or clip == 0.0:
+        return 0.0
+    if math.isinf(clip):
+        return sigma * sigma
+    a = clip / sigma
+    tail = 0.5 * math.erfc(a / math.sqrt(2.0))                       # Phi(-a)
+    dens = math.exp(-0.5 * a * a) / math.sqrt(2.0 * math.pi)          # phi(a)
+    return sigma * sigma * ((1.0 - 2.0 * tail) - 2.0 * a * dens) + 2.0 * clip * clip * tail
+
+
+@dataclass(frozen=True)
+class ObserverGains:
+    """The gains a state observer (ObserverParams mode 1) blends with (no reference counterpart): mode 0 its row's fixed gains,
+    mode 1 the frozen-time Kalman gain K = P (P + R)^-1 of the linearised one-period map of its prior's car, P solving the filter
+    DARE for diagonal Q = diag(q) (process covariance per control period) and R = diag(r) (measurement covariance) over (vx, vy,
+    wz, epsi, s, ey).  Mode 1 needs a car prior (ObserverPrior.car or .plant).  The device takes one per controller
+    (BatchedController.set_observer_gains)."""
+    mode: int = 0
+    q: tuple = (1.0,) * 6
+    r: tuple = (1.0,) * 6
+
+    @classmethod
+    def fixed(cls):
+        """The observer row's fixed gains: installed, the observers compute exactly what they compute without a table."""
+        return cls(0)
+
+    @classmethod
+    def kalman(cls, q, r):
+        """Model gains for the covariance diagonals ``q`` and ``r`` (one value for every channel or six, each finite and > 0)."""
+        qs = np.broadcast_to(np.asarray(q, float), (6,))
+        rs = np.broadcast_to(np.asarray(r, float), (6,))
+        return cls(1, tuple(float(v) for v in qs), tuple(float(v) for v in rs))
+
+    @classmethod
+    def from_noise(cls, noise, measurement, model_sigma):
+        """Model gains matched to the closed loop's noise: r_j the exact variance of the clipped sensor noise of ``measurement``
+        (MeasurementParams), q on vx, vy, wz the variance of the simulator's process noise of ``noise`` (NoiseParams:
+        sim_gain^2 Var(clip(sim_sigma Z, +-sim_clip))) plus model_sigma_j^2, q on epsi, s, ey model_sigma_j^2 alone.
+        ``model_sigma`` (one value or six, finite and >= 0) is the standard deviation per control period of the model's own
+        error, e.g. of the prior against the true state in a noise-free run.  Raises ValueError where a q_j or r_j would be 0 (a
+        noise-free sensor channel, or a channel without process noise and model error) or is not finite."""
+        ms = np.broadcast_to(np.asarray(model_sigma, float), (6,))
+        if not (np.all(np.isfinite(ms)) and np.all(ms >= 0)):
+            raise ValueError("model_sigma must be finite and >= 0")
+        g = float(noise.sim_gain)
+        q = [g * g * clipped_normal_variance(noise.sim_sigma[j], noise.sim_clip[j]) + float(ms[j]) ** 2 for j in range(3)]
+        q += [float(ms[j]) ** 2 for j in range(3, 6)]
+        r = [clipped_normal_variance(measurement.sigma[j], measurement.clip[j]) for j in range(6)]
+        for name, v in (("q", q), ("r", r)):
+            bad = [j for j in range(6) if not (math.isfinite(v[j]) and v[j] > 0.0)]
+            if bad:
+                raise ValueError("ObserverGains.from_noise: %s is not > 0 on channel(s) %s" % (name, bad))
+        return cls(1, tuple(q), tuple(r))
+
+
 @dataclass(frozen=True)
 class SurfaceParams:
     """A track surface (no reference counterpart: the reference's grip is the same all round the lap): up to 16 zones

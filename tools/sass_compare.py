@@ -11,11 +11,12 @@ to five `false` flags, so that the instantiation without a per-controller table 
            pool_export_kernel, commit_laps_kernel, seed_from_record_kernel and measure_kernel (untemplated; older builds had one
            flag per table they read: lap counts, lap reports, lap windows, lane rules, lane margins, lap schedules),
            sim_step_kernel and nominal_model_kernel (<false>: no surface table; older builds: <false, false> or
-           <false, false, false>, no lap reports, no lap schedule and no surface table), observe_kernel (<false>: no observer
-           prior table; older builds: untemplated)
+           <false, false, false>, no lap reports, no lap schedule and no surface table), observe_kernel (<false, false>: no
+           observer prior table; older builds: <false> or untemplated)
   reports  sim_step_kernel<true, false> or <true, false, false> of an older build: lap reports, no lap schedule and no surface
            table (later builds have no such kernel: their sim_step_kernel<true> is the surface instantiation)
   surface  sim_step_kernel<true> and nominal_model_kernel<true>: the surface instantiations (builds with track surfaces)
+  prior    observe_kernel<true, false> or <true>: an observer prior table without a gain table (builds with observer priors)
 and compared by instruction text (cuobjdump -sass without addresses and encodings).  Each differing line pair is classified:
   dfma-swap   one DFMA with its two factors exchanged (a*b+c = b*a+c)
   lds-swap    LDS.128 loads of unchanged addresses whose destination registers are permuted among themselves
@@ -37,6 +38,7 @@ DEFAULT = re.compile(r"^(?:void )?lmpc::(knn_ltv_regress_kernel|ss_select_kernel
                      r"(<false>|<false, false>|<false, false, false>|<false, false, false, false>|<false, false, false, false, false>)?\(")
 REPORTS = re.compile(r"^(?:void )?lmpc::(sim_step_kernel)<true(?:, false){1,2}>\(")
 SURFACE = re.compile(r"^(?:void )?lmpc::(sim_step_kernel|nominal_model_kernel)<true>\(")
+PRIOR = re.compile(r"^(?:void )?lmpc::(observe_kernel)<true(?:, false)?>\(")
 
 
 def kernels(path):
@@ -51,6 +53,7 @@ def kernels(path):
             d = DEFAULT.match(name)
             r = REPORTS.match(name)
             sf = SURFACE.match(name)
+            pr = PRIOR.match(name)
             cur = None
             if k:
                 sets = k.group(1) == "ftocp_sets_kernel" or k.group(4) == "true"
@@ -61,6 +64,8 @@ def kernels(path):
                 cur = out.setdefault(("reports", r.group(1), 0), [])
             elif sf:
                 cur = out.setdefault(("surface", sf.group(1), 0), [])
+            elif pr:
+                cur = out.setdefault(("prior", pr.group(1), 0), [])
             continue
         m = re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(.*?)\s*;", line)
         if m and cur is not None:
@@ -106,7 +111,7 @@ def main(old, new):
     totals = collections.defaultdict(collections.Counter)
     for key in sorted(set(ko) | set(kn)):
         variant, n, m = key
-        label = ("%-24s" % n) if variant in ("default", "reports", "surface") else "<%2d,%2d>" % (n, m)
+        label = ("%-24s" % n) if variant in ("default", "reports", "surface", "prior") else "<%2d,%2d>" % (n, m)
         if key not in ko or key not in kn:
             print("%-7s %s  only in %s" % (variant, label, "new" if key in kn else "old"))
             totals[variant]["unmatched"] += 1
