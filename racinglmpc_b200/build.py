@@ -8,7 +8,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 SRC = os.path.join(HERE, "csrc", "lmpc_b200.cu")
 SRCS = [SRC, os.path.join(HERE, "csrc", "ftocp_sets.cu"),      # the QP kernel for per-controller parameters (ftocp_launch.cuh)
         os.path.join(HERE, "csrc", "ftocp_shapes.cu")]             # ... and for per-controller shapes
-DEPS = SRCS + [os.path.join(HERE, "csrc", f) for f in ("ftocp_pdip.cuh", "ftocp_launch.cuh", "lap_budget.cuh", "lap_schedule.cuh", "nominal_model.cuh", "safeset.cuh", "lapbooks.cuh", "probe.cuh", "snapshot.cuh")] + \
+DEPS = SRCS + [os.path.join(HERE, "csrc", f) for f in ("ftocp_pdip.cuh", "ftocp_launch.cuh", "lap_budget.cuh", "lap_schedule.cuh", "nominal_model.cuh", "car.cuh", "safeset.cuh", "plant.cuh", "observer.cuh", "lapbooks.cuh", "probe.cuh", "snapshot.cuh")] + \
        [os.path.join(HERE, "..", "include", "lmpc_b200.h"), os.path.abspath(__file__)]   # this file holds the architecture flags
 OUT = os.path.join(HERE, "liblmpc_b200.so")
 CUDA_HOME = os.environ.get("CUDA_HOME", "/usr/local/cuda")

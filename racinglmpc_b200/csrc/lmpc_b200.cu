@@ -31,6 +31,8 @@
 #include "../../include/lmpc_b200.h"
 #include "ftocp_pdip.cuh"
 #include "safeset.cuh"
+#include "plant.cuh"
+#include "observer.cuh"
 #include "lapbooks.cuh"
 #include "nominal_model.cuh"
 #include "probe.cuh"

@@ -6,12 +6,14 @@
 // sim_step_kernel), rows 3..5 the closed-form kinematic rows K1 writes.  K1 skips such a controller (its NOMINAL instantiation),
 // and nominal_model_kernel, launched after it, writes all 54 entries of the controller's stages.
 #pragma once
+#include "lap_schedule.cuh"
+#include "car.cuh"
 
 namespace lmpc {
 
 struct NominalArgs {
     int batch, N;
-    double dt;                        // the control period (ModelConst::dt): the simulator's loop runs while (i + 1) h <= dt
+    double dt;                        // the control period (ModelConst::dt): the sub-steps of period_substeps
     const double* xLin;               // [B][N+1][6]
     const double* uLin;               // [B][N][2]
     PredictionModels pm;              // the mode (and mode 1 vehicle) of every controller
@@ -47,34 +49,30 @@ __global__ void __launch_bounds__(128) nominal_model_kernel(const NominalArgs a)
     const double* xl = a.xLin + ((size_t)b * (a.N + 1) + i) * 6;
     const double* ul = a.uLin + ((size_t)b * a.N + i) * 2;
     const double delta = ul[0], acc = ul[1];
-    const double h = 0.001;
+    const double h = CAR_H;
     double vx = xl[0], vy = xl[1], wz = xl[2];
     double S[3][5] = {{1, 0, 0, 0, 0}, {0, 1, 0, 0, 0}, {0, 0, 1, 0, 0}};
     const double sd = sin(delta), cd = cos(delta);
-    // SURF: the kinematic states of the plant's sub-steps and the zone cursor (zoned: a mode 2 controller)
+    // SURF: the kinematic states of the plant's sub-steps and the zone row (zoned: a mode 2 controller)
     const bool zoned = SURF && row.mode == 2;
     double epsi = xl[3], sk = xl[4], ey = xl[5];
     SurfaceCursor zc{zoned ? &a.surf_s.of(a.surf, b) : nullptr, 0};
     const TrackRec* trk = zoned ? &a.trk.of(b) : nullptr;
+    // the loop of period_substeps<SURF> written out: through the helper, the abc of a mode 2 controller under a surface moved
     int k = 0;
     while ((k + 1) * h <= a.dt) {
         double Dfi = Df, Dri = Dr;
         if constexpr (SURF) {
             if (zoned) surface_forces(zc, sk, trk->TrackLength, Df, Dr, &Dfi, &Dri);
         }
-        // the simulator's sub-step (sim_step_kernel), with the reference's lf in alpha_r
-        const double pf = vy + lf * wz, pq = vy - lf * wz;
-        const double af = delta - atan2(pf, vx);
-        const double ar = -atan2(pq, vx);
-        const double tf = atan(Bf * af), tr = atan(Br * ar);
-        const double Fyf = Dfi * sin(Cf * tf);
-        const double Fyr = Dri * sin(Cr * tr);
+        // the simulator's sub-step (sim_substep)
+        const Tyres t = tyre_forces(lf, Dfi, Cf, Bf, Dri, Cr, Br, delta, vx, vy, wz);
         // dFy/dalpha and dalpha/d(vx, vy, wz); d alpha_f / d delta = 1
-        const double gf = Dfi * cos(Cf * tf) * Cf * Bf / (1.0 + (Bf * af) * (Bf * af));
-        const double gr = Dri * cos(Cr * tr) * Cr * Br / (1.0 + (Br * ar) * (Br * ar));
-        const double rf = 1.0 / (vx * vx + pf * pf), rr = 1.0 / (vx * vx + pq * pq);
-        const double daf[3] = {pf * rf, -vx * rf, -lf * vx * rf};
-        const double dar[3] = {pq * rr, -vx * rr, lf * vx * rr};
+        const double gf = Dfi * cos(Cf * t.tf) * Cf * Bf / (1.0 + (Bf * t.af) * (Bf * t.af));
+        const double gr = Dri * cos(Cr * t.tr) * Cr * Br / (1.0 + (Br * t.ar) * (Br * t.ar));
+        const double rf = 1.0 / (vx * vx + t.yf * t.yf), rr = 1.0 / (vx * vx + t.yr * t.yr);
+        const double daf[3] = {t.yf * rf, -vx * rf, -lf * vx * rf};
+        const double dar[3] = {t.yr * rr, -vx * rr, lf * vx * rr};
         // f_z (3 x 3) and f_u (3 x 2)
         double Fz[3][3], Fu[3][2];
 #pragma unroll
@@ -85,9 +83,9 @@ __global__ void __launch_bounds__(128) nominal_model_kernel(const NominalArgs a)
         }
         Fz[0][1] += wz; Fz[0][2] += vy;
         Fz[1][0] -= wz; Fz[1][2] -= vx;
-        Fu[0][0] = -(gf * sd + Fyf * cd) / mass; Fu[0][1] = 1.0;
-        Fu[1][0] = (gf * cd - Fyf * sd) / mass; Fu[1][1] = 0.0;
-        Fu[2][0] = lf * (gf * cd - Fyf * sd) / Iz; Fu[2][1] = 0.0;
+        Fu[0][0] = -(gf * sd + t.Fyf * cd) / mass; Fu[0][1] = 1.0;
+        Fu[1][0] = (gf * cd - t.Fyf * sd) / mass; Fu[1][1] = 0.0;
+        Fu[2][0] = lf * (gf * cd - t.Fyf * sd) / Iz; Fu[2][1] = 0.0;
         double Sn[3][5];
 #pragma unroll
         for (int r = 0; r < 3; ++r) {
@@ -105,18 +103,12 @@ __global__ void __launch_bounds__(128) nominal_model_kernel(const NominalArgs a)
         if constexpr (SURF) {
             if (zoned) {      // the simulator's (epsi, s, ey) update, from the sub-step's starting state
                 int okz = 1;
-                const double cur = curvature_lookup(*trk, sk, &okz);
-                const double ce = cos(epsi), se = sin(epsi);
-                const double nepsi = epsi + h * (wz - (vx * ce - vy * se) / (1 - cur * ey) * cur);
-                const double ns = sk + h * ((vx * ce - vy * se) / (1 - cur * ey));
-                const double ney = ey + h * (vx * se + vy * ce);
-                epsi = nepsi; sk = ns; ey = ney;
+                const Kinematics q = kinematic_update(*trk, &okz, h, vx, vy, wz, epsi, sk, ey);
+                epsi = q.epsi; sk = q.s; ey = q.ey;
             }
         }
-        const double nvx = vx + h * (acc - 1 / mass * Fyf * sd + wz * vy);
-        const double nvy = vy + h * (1 / mass * (Fyf * cd + Fyr) - wz * vx);
-        const double nwz = wz + h * (1 / Iz * (lf * Fyf * cd - lr * Fyr));
-        vx = nvx; vy = nvy; wz = nwz;
+        const Velocities n = velocity_update(mass, lf, lr, Iz, acc, sd, cd, h, t, vx, vy, wz);
+        vx = n.vx; vy = n.vy; wz = n.wz;
         ++k;
     }
     double* out = a.abc + ((size_t)b * a.N + i) * 54;
@@ -144,35 +136,19 @@ __global__ void __launch_bounds__(128) nominal_model_kernel(const NominalArgs a)
         finite = finite && isfinite(c);
     }
     if (!finite) flags |= LMPC_FLAG_NOMINAL_NONFINITE;
-    // rows 3..5: K1's closed-form block (knn_ltv_regress_kernel, "rows 3..5"), the same expressions in the same order
+    // rows 3..5: K1's closed-form block (kinematic_rows), at the entries K1_ABC_SRC gives them
     {
-        const double vx = xl[0], vy = xl[1], wz = xl[2], epsi = xl[3], sc = xl[4], ey = xl[5];
-        const double dt = a.dt;
+        const double x[6] = {xl[0], xl[1], xl[2], xl[3], xl[4], xl[5]};
         int okc = 1;
-        const double cur = curvature_lookup(a.trk.of(b), sc, &okc);
+        const double cur = curvature_lookup(a.trk.of(b), x[4], &okc);
         if (!okc) flags |= 2;
-        const double den = 1.0 - cur * ey;
-        const double rden = fast_rcp(den), rden2 = rden * rden;
-        double se, ce;
-        sincos(epsi, &se, &ce);
-        const double vl = vx * ce - vy * se;          // longitudinal speed along the centre line
-        const double vt = -vx * se - vy * ce;
-        const double a30 = -dt * ce * rden * cur, a31 = dt * se * rden * cur, a33 = 1.0 - dt * vt * rden * cur;
-        const double a35 = dt * vl * rden2 * cur * (-cur);
-        const double a40 = dt * (ce * rden), a41 = -dt * (se * rden), a43 = dt * vt * rden, a45 = -dt * vl * rden2 * (-cur);
-        const double a50 = dt * se, a51 = dt * ce, a53 = dt * vl;
-        const double f3 = epsi + dt * (wz - vl * rden * cur);
-        const double f4 = sc + dt * (vl * rden);
-        const double f5 = ey + dt * (vx * se + vy * ce);
-        const double c3 = f3 - (a30 * vx + a31 * vy + dt * wz + a33 * epsi + 0.0 * sc + a35 * ey);
-        const double c4 = f4 - (a40 * vx + a41 * vy + 0.0 * wz + a43 * epsi + sc + a45 * ey);
-        const double c5 = f5 - (a50 * vx + a51 * vy + 0.0 * wz + a53 * epsi + 0.0 * sc + ey);
-        // the entries K1_ABC_SRC gives rows 3..5 of A, B and C
-        const double row3[6] = {a30, a31, dt, a33, 0.0, a35}, row4[6] = {a40, a41, 0.0, a43, 1.0, a45};
-        const double row5[6] = {a50, a51, 0.0, a53, 0.0, 1.0};
+        double kv[17];
+        kinematic_rows(x, cur, a.dt, kv);
+        const double row3[6] = {kv[3], kv[4], kv[2], kv[5], kv[0], kv[6]}, row4[6] = {kv[7], kv[8], kv[0], kv[9], kv[1], kv[10]};
+        const double row5[6] = {kv[11], kv[12], kv[0], kv[13], kv[0], kv[1]};
 #pragma unroll
-        for (int j = 0; j < 6; ++j) { out[18 + j] = row3[j]; out[24 + j] = row4[j]; out[30 + j] = row5[j]; out[42 + j] = 0.0; }
-        out[51] = c3; out[52] = c4; out[53] = c5;
+        for (int j = 0; j < 6; ++j) { out[18 + j] = row3[j]; out[24 + j] = row4[j]; out[30 + j] = row5[j]; out[42 + j] = kv[0]; }
+        out[51] = kv[14]; out[52] = kv[15]; out[53] = kv[16];
     }
     if (flags) atomicOr(&a.status[b], flags);
 }

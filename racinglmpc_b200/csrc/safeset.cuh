@@ -16,6 +16,7 @@
 #include <stdint.h>
 #include "lap_budget.cuh"
 #include "ftocp_launch.cuh"
+#include "car.cuh"
 
 namespace lmpc {
 
@@ -40,8 +41,7 @@ struct Table {
 using RegressionRec = lmpc_regression_params;
 using Regressions = Table<RegressionRec>;
 
-// The track of every controller (lmpc_set_tracks; default: the track of lmpc_store_create); the ABI record is the device record.
-using TrackRec = lmpc_track_params;
+// The track of every controller (TrackRec, car.cuh)
 using Tracks = Table<TrackRec>;
 
 // The shape of every controller (lmpc_set_shapes): horizon N_b and safe-set size M_b, or no table (tab == null) for the handle's
@@ -140,29 +140,6 @@ struct LapPool {
     int cap, Tmax;
     __host__ __device__ size_t lap_index(int b, int slot) const { return (size_t)b * cap + slot; }
 };
-
-// Track.py:292-310 — wrap by repeated subtraction, first segment with s in [s0, s0+len)
-// (a non-finite or absurdly large s -- an unsolved QP feeding garbage to the simulator -- would spin forever in the
-// reference's loop; here it fails the lookup like a negative s does, so the instance is flagged instead of hanging the stream)
-__device__ __forceinline__ double curvature_lookup(const TrackRec& m, double s, int* ok) {
-    if (!(s <= 64.0 * m.TrackLength)) { *ok = 0; return 0.0; }
-    while (s > m.TrackLength) s = s - m.TrackLength;
-    for (int i = 0; i < m.nseg; ++i) {
-        double s0 = m.seg[i * 3], ln = m.seg[i * 3 + 1];
-        if (s >= s0 && s < s0 + ln) return m.seg[i * 3 + 2];
-    }
-    *ok = 0;   // the reference raises here (negative s / exact end point)
-    return 0.0;
-}
-
-// 1 / x for a normal, finite x to ~1 ulp: hardware seed (20 bits) + two Newton steps; no slow-path call, so no registers are
-// parked in local memory around it
-__device__ __forceinline__ double fast_rcp(double x) {
-    double r;
-    asm("rcp.approx.ftz.f64 %0, %1;" : "=d"(r) : "d"(x));
-    r = fma(fma(-x, r, 1.0), r, r);
-    return fma(fma(-x, r, 1.0), r, r);
-}
 
 // (dist, idx) lexicographic "less": ties go to the lower row index
 __device__ __forceinline__ bool cand_less(double d1, int i1, double d2, int i2) { return d1 < d2 || (d1 == d2 && i1 < i2); }
@@ -563,38 +540,22 @@ __global__ void __launch_bounds__(32 * K1_MAXWPB, LMPC_K1_MINBLOCKS) knn_ltv_reg
         out[36 + 2 * lane + (lane == 0 ? 1 : 0)] = th[3];   // vx uses the acceleration input, the lateral rows the steering (PM.py:29-30)
         out[48 + lane] = th[4];
     }
-    // rows 3..5: Jacobian of the curvilinear kinematics; every lane evaluates the few distinct values, lane 3 stages them and the
-    // warp writes the record through an index table
+    // rows 3..5: Jacobian of the curvilinear kinematics (kinematic_rows); every lane evaluates the few distinct values, lane 3
+    // stages them and the warp writes the record through an index table
     {
-        const double vx = xl[0], vy = xl[1], wz = xl[2], epsi = xl[3], sc = xl[4], ey = xl[5];
-        const double dt = m.dt;
+        const double x[6] = {xl[0], xl[1], xl[2], xl[3], xl[4], xl[5]};
         int okc = 1;
-        const double cur = curvature_lookup(a.trk.of(b), sc, &okc);
+        const double cur = curvature_lookup(a.trk.of(b), x[4], &okc);
         if (!okc) flags |= 2;
-        const double den = 1.0 - cur * ey;
-        const double rden = fast_rcp(den), rden2 = rden * rden;
-        double se, ce;
-        sincos(epsi, &se, &ce);
-        const double vl = vx * ce - vy * se;          // longitudinal speed along the centre line
-        const double vt = -vx * se - vy * ce;
-        const double a30 = -dt * ce * rden * cur, a31 = dt * se * rden * cur, a33 = 1.0 - dt * vt * rden * cur;
-        const double a35 = dt * vl * rden2 * cur * (-cur);
-        const double a40 = dt * (ce * rden), a41 = -dt * (se * rden), a43 = dt * vt * rden, a45 = -dt * vl * rden2 * (-cur);
-        const double a50 = dt * se, a51 = dt * ce, a53 = dt * vl;
-        // C_r = f_r(x) - A_r x, products summed left to right like np.dot on 6 terms
-        const double f3 = epsi + dt * (wz - vl * rden * cur);
-        const double f4 = sc + dt * (vl * rden);
-        const double f5 = ey + dt * (vx * se + vy * ce);
-        const double c3 = f3 - (a30 * vx + a31 * vy + dt * wz + a33 * epsi + 0.0 * sc + a35 * ey);
-        const double c4 = f4 - (a40 * vx + a41 * vy + 0.0 * wz + a43 * epsi + sc + a45 * ey);
-        const double c5 = f5 - (a50 * vx + a51 * vy + 0.0 * wz + a53 * epsi + 0.0 * sc + ey);
+        double kv[17];
+        kinematic_rows(x, cur, m.dt, kv);
         double* vals = sys;
         if (lane == 3) {
-            vals[0] = 0.0; vals[1] = 1.0; vals[2] = dt;
-            vals[3] = a30; vals[4] = a31; vals[5] = a33; vals[6] = a35;
-            vals[7] = a40; vals[8] = a41; vals[9] = a43; vals[10] = a45;
-            vals[11] = a50; vals[12] = a51; vals[13] = a53;
-            vals[14] = c3; vals[15] = c4; vals[16] = c5;
+            vals[0] = kv[0]; vals[1] = kv[1]; vals[2] = kv[2];
+            vals[3] = kv[3]; vals[4] = kv[4]; vals[5] = kv[5]; vals[6] = kv[6];
+            vals[7] = kv[7]; vals[8] = kv[8]; vals[9] = kv[9]; vals[10] = kv[10];
+            vals[11] = kv[11]; vals[12] = kv[12]; vals[13] = kv[13];
+            vals[14] = kv[14]; vals[15] = kv[15]; vals[16] = kv[16];
         }
         __syncwarp();
         for (int e = lane; e < 54; e += 32) {
@@ -975,812 +936,6 @@ __global__ void shift_state_kernel(const ShiftArgs a) {
     }
     if (threadIdx.x < 2) a.OldInput[(size_t)b * 2 + threadIdx.x] = a.uPred[(size_t)b * N * 2 + threadIdx.x];
     if (threadIdx.x == 0) { a.timeStep[b] += 1; a.has_pred[b] = 1; }
-}
-
-// ------------------------------------------------------------------------------------------------
-// Simulator.dynModel (src/fnc/simulator/SysModel.py:56-147): 100 explicit-Euler sub-steps (1 ms) of the dynamic
-// bicycle model with Pacejka tyres in the curvilinear and the global frame, then clipped Gaussian noise on
-// (vx, vy, wz).  One thread per instance.  `z` = three standard-normal draws per instance (the reference consumes
-// np.random.randn() in this order: vx, vy, wz); when z == nullptr they come from Philox4x32-10 keyed by
-// (seed, stream, step), stream = streams[b] or b when streams is null — statistical, not bit-wise, parity with the reference's
-// unseeded global RNG.
-// Also appends (x, u) to the closed-loop buffer -- the measured state in place of x when rec_x is set -- and flags lap
-// completion (SysModel.py:45-47).
-// The ten vehicle constants (SysModel.py:61-70) are read from the instance's row of the vehicle table (a handle without vehicle
-// sets holds a one-row table with the reference vehicle).  The arithmetic is the same with the constants in memory as with them
-// folded in at compile time (DESIGN.md, "Per-controller vehicles").  The noise constants (SysModel.py:139-145) come the same way
-// from the noise table (DESIGN.md, "Per-controller noise and common random numbers").
-struct SimArgs {
-    int batch;
-    const double* x;      // [B][6] curvilinear state
-    const double* xg;      // [B][6] global state (psi, X, Y at 3..5)
-    const double* u;       // [B][2]  or uPred [B][N][2] with u_stride = N*2
-    long long u_stride;
-    const double* z;       // [B][3] or nullptr
-    unsigned long long seed, step;
-    double* xn;            // [B][6]
-    double* xgn;           // [B][6]
-    double* cl_x;          // [B][Tcl][6] closed-loop record (may be nullptr)
-    const double* rec_x;   // [B][6] the state rows the record takes: the measured state (measure_kernel), or nullptr: x
-    double* cl_u;          // [B][Tcl][2]
-    int* cl_len;           // [B]
-    int Tcl;
-    int* done;             // [B] 1 when s_next > TrackLength
-    const int* flags;     // [B] step flags (K1/K2/addPoint) and QP status of the step that produced u, or nullptr;
-    const int* status;     //     accumulated into health[b] (OR of flags) and health[B + b] (steps with status != 1)
-    int* health;           //     the simulator's own bits (SIM_LOOKUP_FAILED, SIM_RECORD_FULL) go to health[b] too
-    Table<lmpc_vehicle_params> veh;   // vehicle of every instance (lmpc_rollout_set_vehicles)
-    Tracks trk;                       // curvature and finish line of every instance (lmpc_set_tracks)
-    Table<lmpc_noise_params> noise;   // noise of every instance (lmpc_rollout_set_noise)
-    const int* streams;               // [B] Philox stream of every instance (lmpc_rollout_set_noise_streams), or nullptr: b
-    LapBudget retire;                 // a retired instance is not driven (the PID lap passes a null budget)
-};
-// Health bits of the simulator itself (the step flags use 1 .. 64 and 512):
-//   SIM_LOOKUP_FAILED  a sub-step's curvature lookup failed (s < 0, s at the finish line after the wrap, s not finite or beyond
-//                      64 laps): the reference raises there (Track.py:292-310); the step went on with curvature 0
-//   SIM_RECORD_FULL    the closed-loop record already held Tcl rows, so this step's (x, u) was not recorded: the lap is longer
-//                      than the record and a hand-over of it files a truncated lap
-constexpr int SIM_LOOKUP_FAILED = 128;
-constexpr int SIM_RECORD_FULL = 256;
-
-}  // namespace lmpc
-#include <curand_kernel.h>
-#include "lap_schedule.cuh"
-namespace lmpc {
-
-// Track surfaces (lmpc_rollout_set_surfaces): the zone of one controller's sub-steps, found by a cursor that follows s.  The
-// zones of a row ascend without overlap, so their s_end ascend strictly, and the first zone whose s_end lies above the wrapped s
-// is the only one that can hold it.  The cursor walks to that zone from where the last sub-step left it (s moves by at most
-// vx h per sub-step), in either direction, so it returns what a scan of every zone returns at any s.
-struct SurfaceCursor {
-    const lmpc_surface_params* row;
-    int c;
-    // true and the zone's (mu_f, mu_r) when a zone holds s, wrapped as curvature_lookup wraps it; false when none does, s is not
-    // finite or s is beyond 64 laps
-    __device__ __forceinline__ bool at(double s, double L, double* muf, double* mur) {
-        if (!(s <= 64.0 * L)) return false;
-        while (s > L) s = s - L;
-        const double* z = row->zone;
-        const int n = row->nzone;
-        while (c > 0 && z[(c - 1) * 4 + 1] > s) --c;
-        while (c < n && z[c * 4 + 1] <= s) ++c;
-        if (c >= n || !(z[c * 4] <= s)) return false;
-        *muf = z[c * 4 + 2];
-        *mur = z[c * 4 + 3];
-        return true;
-    }
-};
-
-// The peak tyre forces of a sub-step at s: fl(mu_f Df), fl(mu_r Dr) in a zone, else Df and Dr exactly
-__device__ __forceinline__ void surface_forces(SurfaceCursor& zc, double s, double L, double Df, double Dr, double* Dfi, double* Dri) {
-    double muf, mur;
-    if (zc.at(s, L, &muf, &mur)) {
-        *Dfi = __dmul_rn(muf, Df);
-        *Dri = __dmul_rn(mur, Dr);
-    } else {
-        *Dfi = Df;
-        *Dri = Dr;
-    }
-}
-
-// One explicit-Euler sub-step of Simulator.dynModel (SysModel.py:94-137), with the reference's lf in alpha_r: the curvilinear
-// state (vx, vy, wz, epsi, s, ey) and, GLOBAL, the global pose (psi, X, Y), all updated from the sub-step's starting state.  Dfi,
-// Dri are the sub-step's peak tyre forces (surface_forces), sd, cd = sin, cos(delta).  A failed curvature lookup clears *okc.
-// sim_step_kernel and the observer's model prior (sim_period) both take it, so the prior is the plant's arithmetic exactly.
-template <bool GLOBAL>
-__device__ __forceinline__ void sim_substep(double mass, double lf, double lr, double Iz, double Dfi, double Cf, double Bf,
-                                            double Dri, double Cr, double Br, double delta, double acc, double sd, double cd,
-                                            double h, const TrackRec& trk, int* okc, double& vx, double& vy, double& wz,
-                                            double& epsi, double& s, double& ey, double& psi, double& X, double& Y) {
-    const double af = delta - atan2(vy + lf * wz, vx);
-    const double ar = -atan2(vy - lf * wz, vx);
-    const double Fyf = Dfi * sin(Cf * atan(Bf * af));
-    const double Fyr = Dri * sin(Cr * atan(Br * ar));
-    const double nvx = vx + h * (acc - 1 / mass * Fyf * sd + wz * vy);
-    const double nvy = vy + h * (1 / mass * (Fyf * cd + Fyr) - wz * vx);
-    const double nwz = wz + h * (1 / Iz * (lf * Fyf * cd - lr * Fyr));
-    if constexpr (GLOBAL) {
-        const double npsi = psi + h * wz;
-        const double nX = X + h * (vx * cos(psi) - vy * sin(psi));
-        const double nY = Y + h * (vx * sin(psi) + vy * cos(psi));
-        psi = npsi; X = nX; Y = nY;
-    }
-    const double cur = curvature_lookup(trk, s, okc);
-    const double ce = cos(epsi), se = sin(epsi);
-    const double nepsi = epsi + h * (wz - (vx * ce - vy * se) / (1 - cur * ey) * cur);
-    const double ns = s + h * ((vx * ce - vy * se) / (1 - cur * ey));
-    const double ney = ey + h * (vx * se + vy * ce);
-    vx = nvx; vy = nvy; wz = nwz; epsi = nepsi; s = ns; ey = ney;
-}
-
-// With reports (rep.rows) the step is also added to the controller's running report row (report_step) with its QP's status
-// a.status and iterations rep_iters, both null for a PID step.  The vehicle and noise rows come from the lap schedules veh_s and
-// noise_s (lap_schedule.cuh; a null schedule reads the table's own index).  SURF (a surface table is installed): each sub-step's
-// peak tyre forces follow the controller's surface row of surf, through the lap schedule surf_s; without one surf is not read.
-// Surfaces stay a template flag: a run-time test in the sub-step loop cost the table-free step 1.5 % per launch on an H100
-// (DESIGN.md, "Track surfaces").
-template <bool SURF>
-__global__ void sim_step_kernel(const __grid_constant__ ModelConst m, const SimArgs a, const LapReports rep, const int* rep_iters,
-                                const LapSchedule veh_s, const LapSchedule noise_s, const Table<lmpc_surface_params> surf,
-                                const LapSchedule surf_s) {
-    const int b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= a.batch) return;
-    if (a.retire.retired(b)) {
-        // no record row, no health count, no draw.  The state (x, xg) is a double buffer whose halves swap every step: carrying
-        // the state over to the other half unchanged is what keeps it where the hand-over left it
-        for (int j = 0; j < 6; ++j) { a.xn[(size_t)b * 6 + j] = a.x[(size_t)b * 6 + j]; a.xgn[(size_t)b * 6 + j] = a.xg[(size_t)b * 6 + j]; }
-        return;
-    }
-    if (a.health) {
-        if (a.flags && a.flags[b]) a.health[b] |= a.flags[b];
-        if (a.status && a.status[b] != 1) a.health[a.batch + b] += 1;
-    }
-    // vehicle parameters, SysModel.py:61-70
-    const lmpc_vehicle_params& v = veh_s.of(a.veh, b);
-    const double mass = v.m, lf = v.lf, lr = v.lr, Iz = v.Iz;
-    const double Df = v.Df, Cf = v.Cf, Bf = v.Bf;
-    const double Dr = v.Dr, Cr = v.Cr, Br = v.Br;
-    const TrackRec& trk = a.trk.of(b);
-    const double h = 0.001;
-    const double* x = a.x + (size_t)b * 6;
-    const double* g = a.xg + (size_t)b * 6;
-    const double delta = a.u[(size_t)b * a.u_stride], acc = a.u[(size_t)b * a.u_stride + 1];
-    double vx = x[0], vy = x[1], wz = x[2], epsi = x[3], s = x[4], ey = x[5];
-    double psi = g[3], X = g[4], Y = g[5];
-    int sim_bits = 0;
-    if (a.cl_x) {
-        const int T = a.cl_len[b];
-        if (T < a.Tcl) {
-            const double* r = a.rec_x ? a.rec_x + (size_t)b * 6 : x;
-#pragma unroll
-            for (int j = 0; j < 6; ++j) a.cl_x[((size_t)b * a.Tcl + T) * 6 + j] = r[j];
-            a.cl_u[((size_t)b * a.Tcl + T) * 2] = delta;
-            a.cl_u[((size_t)b * a.Tcl + T) * 2 + 1] = acc;
-            a.cl_len[b] = T + 1;
-        } else {
-            sim_bits = SIM_RECORD_FULL;
-        }
-    }
-    const double sd = sin(delta), cd = cos(delta);
-    int i = 0;
-    int okc = 1;
-    SurfaceCursor zc{SURF ? &surf_s.of(surf, b) : nullptr, 0};
-    while ((i + 1) * h <= m.dt) {
-        double Dfi = Df, Dri = Dr;
-        if constexpr (SURF) surface_forces(zc, s, trk.TrackLength, Df, Dr, &Dfi, &Dri);
-        sim_substep<true>(mass, lf, lr, Iz, Dfi, Cf, Bf, Dri, Cr, Br, delta, acc, sd, cd, h, trk, &okc, vx, vy, wz, epsi, s, ey,
-                          psi, X, Y);
-        ++i;
-    }
-    if (!okc) sim_bits |= SIM_LOOKUP_FAILED;
-    if (a.health && sim_bits) a.health[b] |= sim_bits;
-    if (rep.rows) report_step(rep, b, x, (a.flags ? a.flags[b] : 0) | sim_bits, a.status, rep_iters);
-    double z0, z1, z2;
-    if (a.z) {
-        z0 = a.z[(size_t)b * 3]; z1 = a.z[(size_t)b * 3 + 1]; z2 = a.z[(size_t)b * 3 + 2];
-    } else {
-        curandStatePhilox4_32_10_t st;
-        const int stream = a.streams ? a.streams[b] : b;
-        curand_init(a.seed, (unsigned long long)stream, a.step * 8ull, &st);   // 8 raw 32-bit draws per step: disjoint blocks
-        const double2 n01 = curand_normal2_double(&st);
-        const double2 n23 = curand_normal2_double(&st);
-        z0 = n01.x; z1 = n01.y; z2 = n23.x;
-    }
-    // noise parameters, SysModel.py:139-145
-    const lmpc_noise_params& nz = noise_s.of(a.noise, b);
-    const double n_vx = fmax(-nz.sim_clip[0], fmin(z0 * nz.sim_sigma[0], nz.sim_clip[0]));
-    const double n_vy = fmax(-nz.sim_clip[1], fmin(z1 * nz.sim_sigma[1], nz.sim_clip[1]));
-    const double n_wz = fmax(-nz.sim_clip[2], fmin(z2 * nz.sim_sigma[2], nz.sim_clip[2]));
-    const double gain = nz.sim_gain;
-    double* xn = a.xn + (size_t)b * 6;
-    double* gn = a.xgn + (size_t)b * 6;
-    // SysModel.py:143-147: the noise is added to the curvilinear copy only
-    gn[0] = vx; gn[1] = vy; gn[2] = wz; gn[3] = psi; gn[4] = X; gn[5] = Y;
-    xn[0] = vx + gain * n_vx; xn[1] = vy + gain * n_vy; xn[2] = wz + gain * n_wz;
-    xn[3] = epsi; xn[4] = s; xn[5] = ey;
-    if (a.done) a.done[b] = (s > trk.TrackLength) ? 1 : 0;
-}
-
-// ------------------------------------------------------------------------------------------------
-// PID path-following controller, Utilities.py:42-68 (PID.solve): u = [-0.6 ey - 0.9 epsi + clip(0.25 z0, +-0.9),
-// 1.5 (vt - vx) + clip(0.10 z1, +-0.2)], z ~ N(0,1) drawn in that order.  Writes uPred[b][0] so that sim_step_kernel
-// consumes it like a controller's first predicted input.  The noise constants are the instance's row of the noise table, the
-// Philox stream is streams[b] (b when streams is null), as in sim_step_kernel.
-struct PidArgs {
-    int batch;
-    const double* x;       // [B][6]
-    double vt;
-    const double* z;       // [B][2] or nullptr (Philox)
-    unsigned long long seed, step;
-    double* u;             // [B][u_stride]
-    long long u_stride;
-    Table<lmpc_noise_params> noise;   // noise of every instance (lmpc_rollout_set_noise)
-    const int* streams;               // [B] Philox stream of every instance, or nullptr: b
-};
-__global__ void pid_input_kernel(const PidArgs a) {
-    const int b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= a.batch) return;
-    double z0, z1;
-    if (a.z) {
-        z0 = a.z[(size_t)b * 2]; z1 = a.z[(size_t)b * 2 + 1];
-    } else {
-        curandStatePhilox4_32_10_t st;
-        const int stream = a.streams ? a.streams[b] : b;
-        curand_init(a.seed ^ 0x9E3779B97F4A7C15ull, (unsigned long long)stream, a.step * 8ull, &st);
-        const double2 n01 = curand_normal2_double(&st);
-        z0 = n01.x; z1 = n01.y;
-    }
-    const lmpc_noise_params& nz = a.noise.of(b);
-    const double* x = a.x + (size_t)b * 6;
-    // -0.6 ey - 0.9 epsi with the one contraction the device has always computed (ptxas fused it so when the noise constants were
-    // immediates); written out because the compiler otherwise picks its contraction from the surrounding code
-    a.u[(size_t)b * a.u_stride] = fma(-0.6, x[5], -(0.9 * x[3])) +
-                                  fmax(-nz.pid_clip[0], fmin(z0 * nz.pid_sigma[0], nz.pid_clip[0]));
-    a.u[(size_t)b * a.u_stride + 1] = 1.5 * (a.vt - x[0]) + fmax(-nz.pid_clip[1], fmin(z1 * nz.pid_sigma[1], nz.pid_clip[1]));
-}
-
-// ------------------------------------------------------------------------------------------------
-// Measurement noise (DESIGN.md, "Per-controller measurement noise"): the state a controller sees, y = x + n on the six
-// curvilinear channels, n_j = clip(z_j * sigma_j, +-clip_j) in the form of the process noise, z_j standard normal from Philox keyed
-// by (seed ^ K_MEAS, stream, clock) -- three curand_normal2_double calls, 12 raw 32-bit draws, in blocks of 16 per step.  Where
-// n_j == 0 the state is copied, so a zero set gives y == x bit for bit (-0.0 + 0.0 would be +0.0).  One thread per controller; a
-// retired controller draws nothing and writes nothing.  The row comes from the lap schedule meas_s (lap_schedule.cuh; a null
-// schedule reads the table's own index).
-constexpr unsigned long long K_MEAS = 0xD1B54A32D192ED03ull;     // distinct from the PID's key constant
-struct MeasArgs {
-    int batch;
-    const double* x;       // [B][6] plant state
-    double* y;             // [B][6] measured state
-    unsigned long long seed, step;
-    Table<lmpc_measurement_params> meas;   // measurement noise of every instance (lmpc_rollout_set_measurement_noise)
-    const int* streams;                    // [B] Philox stream of every instance, or nullptr: b
-    LapBudget retire;
-};
-__global__ void measure_kernel(const MeasArgs a, const LapSchedule meas_s) {
-    const int b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= a.batch || a.retire.retired(b)) return;
-    curandStatePhilox4_32_10_t st;
-    const int stream = a.streams ? a.streams[b] : b;
-    curand_init(a.seed ^ K_MEAS, (unsigned long long)stream, a.step * 16ull, &st);
-    const double2 n01 = curand_normal2_double(&st);
-    const double2 n23 = curand_normal2_double(&st);
-    const double2 n45 = curand_normal2_double(&st);
-    const double z[6] = {n01.x, n01.y, n23.x, n23.y, n45.x, n45.y};
-    const lmpc_measurement_params& m = meas_s.of(a.meas, b);
-    const double* x = a.x + (size_t)b * 6;
-    double* y = a.y + (size_t)b * 6;
-#pragma unroll
-    for (int j = 0; j < 6; ++j) {
-        const double n = fmax(-m.clip[j], fmin(z[j] * m.sigma[j], m.clip[j]));
-        y[j] = n == 0.0 ? x[j] : x[j] + n;
-    }
-}
-
-// ------------------------------------------------------------------------------------------------
-// State observers (DESIGN.md, "Per-controller state observers"): the state x_hat a controller reads, blended from the state it
-// is given, y, and its own one-step prediction p = xPred[1] of its previous QP (row 1 of xPredPrev), with the fixed gains of its
-// row: x_hat_j = p_j + l_j (y_j - p_j), each operation rounded on its own (no contraction), l_j == 1 copying y_j and l_j == 0
-// taking p_j.  p_s gets K2's lap-wrap fix first.  No prior (has_pred == 0), a mode 0 row or a step that is not an LMPC / LTV step
-// gives x_hat = y exactly; a non-finite prior on a channel with l_j < 1 gives x_hat = y and LMPC_FLAG_OBSERVER_RESET.  In a PID
-// or LTI step (blend == 0) a mode 1 row also clears has_pred: xPredPrev is not shifted there and would be stale next step.  One
-// thread per controller; a retired controller reads, writes and flags nothing.  The observer has no state of its own.
-// MODEL (a prior table is installed, DESIGN.md, "Observer priors"): a row of source 1 or 2 takes the model prior
-// p = Phi_car(xPredPrev[0], OldInput) (sim_period) in place of the plan, and the kernel writes the prior it formed to x_prior.
-struct ObserveArgs {
-    int batch, N;
-    int blend;                     // 1: a step of mode 0 or 1; 0: a PID step or a step of mode 2
-    const double* y;               // [B][6] the state the controllers are given (x_meas, or the plant state)
-    const double* xPredPrev;       // [B][N+1][6] the previous QP's prediction
-    int* has_pred;                 // [B]
-    double* x_est;                 // [B][6] x_hat
-    int* flags;                    // [B] step flags, cleared before this launch (blend == 1)
-    Table<lmpc_observer_params> obs;
-    Tracks trk;
-    LapBudget retire;
-};
-// What the MODEL instantiation reads besides (a second kernel parameter: the instantiation without a prior table keeps the code
-// it had before this feature)
-struct ObservePrior {
-    Table<lmpc_observer_prior_params> pri;   // the prior source of every controller
-    double dt;                               // the control period (ModelConst::dt)
-    const double* OldInput;                  // [B][2] the input applied in the previous step
-    double* x_prior;                         // [B][6] the prior formed (NaN: none)
-    Table<lmpc_vehicle_params> veh;          // the simulator's vehicle table and lap schedule (source 2)
-    LapSchedule veh_s;
-    Table<lmpc_surface_params> surf;         // the simulator's surface table (tab null: none) and lap schedule (source 2)
-    LapSchedule surf_s;
-};
-
-// Phi_car: the simulator's noise-free control period on the curvilinear state x under the input (delta, acc) -- sim_step_kernel's
-// sub-step loop with car v and, when zones is not null, its surface row, without the global frame.  false when a sub-step's
-// curvature lookup failed.
-__device__ __forceinline__ bool sim_period(const lmpc_vehicle_params& v, const TrackRec& trk, const lmpc_surface_params* zones,
-                                           double dt, double delta, double acc, double (&x)[6]) {
-    const double mass = v.m, lf = v.lf, lr = v.lr, Iz = v.Iz;
-    const double Df = v.Df, Cf = v.Cf, Bf = v.Bf;
-    const double Dr = v.Dr, Cr = v.Cr, Br = v.Br;
-    const double h = 0.001;
-    const double sd = sin(delta), cd = cos(delta);
-    double vx = x[0], vy = x[1], wz = x[2], epsi = x[3], s = x[4], ey = x[5];
-    double psi = 0.0, X = 0.0, Y = 0.0;
-    int i = 0;
-    int okc = 1;
-    SurfaceCursor zc{zones, 0};
-    while ((i + 1) * h <= dt) {
-        double Dfi = Df, Dri = Dr;
-        if (zones) surface_forces(zc, s, trk.TrackLength, Df, Dr, &Dfi, &Dri);
-        sim_substep<false>(mass, lf, lr, Iz, Dfi, Cf, Bf, Dri, Cr, Br, delta, acc, sd, cd, h, trk, &okc, vx, vy, wz, epsi, s, ey,
-                           psi, X, Y);
-        ++i;
-    }
-    x[0] = vx; x[1] = vy; x[2] = wz; x[3] = epsi; x[4] = s; x[5] = ey;
-    return okc != 0;
-}
-
-// The model prior of controller b (source 1: the row's car, no surface; source 2: the car and surface the plant drove the
-// previous step with -- the lap before lap_n when a hand-over came in between, seen as x_hat_{k-1}.s - y.s > TrackLength / 2).
-// false when an input is not finite or a curvature lookup failed.
-__device__ __forceinline__ bool model_prior(const ObserveArgs& a, const ObservePrior& m, int b, const lmpc_observer_prior_params& r,
-                                            const double (&yv)[6], double (&p)[6]) {
-    const double* xp = a.xPredPrev + (size_t)b * (a.N + 1) * 6;
-    const double delta = m.OldInput[(size_t)b * 2], acc = m.OldInput[(size_t)b * 2 + 1];
-    bool finite = isfinite(delta) && isfinite(acc);
-#pragma unroll
-    for (int j = 0; j < 6; ++j) {
-        p[j] = xp[j];
-        finite = finite && isfinite(p[j]);
-    }
-    const TrackRec& trk = a.trk.of(b);
-    const int back = p[4] - yv[4] > trk.TrackLength / 2 ? 1 : 0;
-    const bool plant = r.source == 2;
-    const lmpc_vehicle_params& v = plant ? m.veh_s.of_before(m.veh, b, back) : r.vehicle;
-    const lmpc_surface_params* zones = plant && m.surf.tab ? &m.surf_s.of_before(m.surf, b, back) : nullptr;
-    return sim_period(v, trk, zones, m.dt, delta, acc, p) && finite;
-}
-
-// ------------------------------------------------------------------------------------------------
-// Model-based observer gains (DESIGN.md, "Observer gains"): the frozen-time Kalman gain of every mode 1 row of the gain table.
-// observer_gain_kernel linearises the controller's one-period map at the prior's point, A = dPhi_car/dx (sim_period_tangent),
-// solves the filter DARE P = A P A' - A P (P + R)^-1 P A' + Q for that A (observer_dare), and writes A, P and K = P (P + R)^-1;
-// observe_kernel<true, true> then blends with K.  Nothing is carried from step to step: the gain is a function of the step's own
-// inputs (xPredPrev[0], OldInput, y and the rows), so it adds no state and no snapshot section.
-struct ObserveGain {
-    Table<lmpc_observer_gain_params> gains;   // the gain row of every controller
-    double* jac;                              // [B][6][6] A (NaN: no model gain formed)
-    double* cov;                              // [B][6][6] P
-    double* gain;                             // [B][6][6] K (NaN: none formed, or A, P or K not finite, or no convergence)
-};
-constexpr int OBS_DARE_ITERS = 64;            // the doubling's iteration cap
-constexpr double OBS_DARE_TOL = 1e-13;        // stop once max|H' - H| <= tol max|H'|
-
-// One sub-step of sim_substep<false> with the tangent (dvx .. dey) of one direction carried alongside: the primal is computed by
-// the same expressions, and the tangent differentiates them.  The curvature (piecewise constant in s) and the sub-step's peak
-// tyre forces Dfi, Dri (piecewise constant in s through the surface zones) are taken as constants.  The inputs are not
-// differentiated.  A separate function, so that sim_substep's code, and the simulator's, stay as they are.
-__device__ __forceinline__ void sim_substep_tangent(double mass, double lf, double lr, double Iz, double Dfi, double Cf, double Bf,
-                                                    double Dri, double Cr, double Br, double delta, double acc, double sd,
-                                                    double cd, double h, const TrackRec& trk, int* okc, double (&x)[6],
-                                                    double (&d)[6]) {
-    const double vx = x[0], vy = x[1], wz = x[2], epsi = x[3], s = x[4], ey = x[5];
-    const double dvx = d[0], dvy = d[1], dwz = d[2], depsi = d[3], ds = d[4], dey = d[5];
-    const double yf = vy + lf * wz, yr = vy - lf * wz;
-    const double af = delta - atan2(yf, vx);
-    const double ar = -atan2(yr, vx);
-    const double daf = -(vx * (dvy + lf * dwz) - yf * dvx) / (vx * vx + yf * yf);
-    const double dar = -(vx * (dvy - lf * dwz) - yr * dvx) / (vx * vx + yr * yr);
-    const double tf = Cf * atan(Bf * af), tr = Cr * atan(Br * ar);
-    const double Fyf = Dfi * sin(tf);
-    const double Fyr = Dri * sin(tr);
-    const double dFyf = Dfi * cos(tf) * Cf * Bf / (1 + Bf * af * Bf * af) * daf;
-    const double dFyr = Dri * cos(tr) * Cr * Br / (1 + Br * ar * Br * ar) * dar;
-    const double nvx = vx + h * (acc - 1 / mass * Fyf * sd + wz * vy);
-    const double nvy = vy + h * (1 / mass * (Fyf * cd + Fyr) - wz * vx);
-    const double nwz = wz + h * (1 / Iz * (lf * Fyf * cd - lr * Fyr));
-    d[0] = dvx + h * (-(1 / mass) * dFyf * sd + dwz * vy + wz * dvy);
-    d[1] = dvy + h * (1 / mass * (dFyf * cd + dFyr) - dwz * vx - wz * dvx);
-    d[2] = dwz + h * (1 / Iz * (lf * dFyf * cd - lr * dFyr));
-    const double cur = curvature_lookup(trk, s, okc);
-    const double ce = cos(epsi), se = sin(epsi);
-    const double den = 1 - cur * ey;
-    const double q = (vx * ce - vy * se) / den;
-    const double dnum = dvx * ce - vx * se * depsi - dvy * se - vy * ce * depsi;
-    const double dq = (dnum + q * cur * dey) / den;
-    const double nepsi = epsi + h * (wz - (vx * ce - vy * se) / (1 - cur * ey) * cur);
-    const double ns = s + h * ((vx * ce - vy * se) / (1 - cur * ey));
-    const double ney = ey + h * (vx * se + vy * ce);
-    d[3] = depsi + h * (dwz - dq * cur);
-    d[4] = ds + h * dq;
-    d[5] = dey + h * (dvx * se + vx * ce * depsi + dvy * ce - vy * se * depsi);
-    x[0] = nvx; x[1] = nvy; x[2] = nwz; x[3] = nepsi; x[4] = ns; x[5] = ney;
-}
-
-// sim_period with the tangent d of one direction: x and d in, Phi_car(x) and A d out.  false when a curvature lookup failed.
-__device__ __forceinline__ bool sim_period_tangent(const lmpc_vehicle_params& v, const TrackRec& trk, const lmpc_surface_params* zones,
-                                                   double dt, double delta, double acc, double (&x)[6], double (&d)[6]) {
-    const double h = 0.001;
-    const double sd = sin(delta), cd = cos(delta);
-    int i = 0;
-    int okc = 1;
-    SurfaceCursor zc{zones, 0};
-    while ((i + 1) * h <= dt) {
-        double Dfi = v.Df, Dri = v.Dr;
-        if (zones) surface_forces(zc, x[4], trk.TrackLength, v.Df, v.Dr, &Dfi, &Dri);
-        sim_substep_tangent(v.m, v.lf, v.lr, v.Iz, Dfi, v.Cf, v.Bf, Dri, v.Cr, v.Br, delta, acc, sd, cd, h, trk, &okc, x, d);
-        ++i;
-    }
-    return okc != 0;
-}
-
-// Gauss-Jordan elimination with partial pivoting of one controller's 6 x NC system in shared memory, M[6][NC] = [S | RHS]: lane r
-// of the controller's six owns row r and every lane picks the same pivots.  On return the solution row k, S^-1 RHS, is row
-// piv[k] of M (columns 6 .. NC - 1).  Every lane of the warp calls it (active or not): it synchronises the warp.
-template <int NC>
-__device__ __forceinline__ void gj_solve(double* M, int r, bool active, int (&piv)[6]) {
-    unsigned used = 0;
-#pragma unroll 1
-    for (int k = 0; k < 6; ++k) {
-        int pk = 0;
-        double best = -1.0;
-        for (int i = 0; i < 6; ++i) {
-            const double v = fabs(M[i * NC + k]);
-            if (!(used & (1u << i)) && v > best) { best = v; pk = i; }
-        }
-        piv[k] = pk;
-        used |= 1u << pk;
-        __syncwarp();
-        if (active && r == pk) {
-            const double inv = 1.0 / M[pk * NC + k];
-            for (int c = 0; c < NC; ++c) M[pk * NC + c] *= inv;
-        }
-        __syncwarp();
-        double f = 0.0;
-        if (active && r != pk) f = M[r * NC + k];
-        __syncwarp();
-        if (active && r != pk)
-            for (int c = 0; c < NC; ++c) M[r * NC + c] -= f * M[pk * NC + c];
-        __syncwarp();
-    }
-}
-
-// The filter DARE of one controller by the structured doubling algorithm on the dual (control) problem: A0 = A', G0 = R^-1,
-// H0 = Q; W = I + G H; A <- A W^-1 A, G <- G + A W^-1 G A', H <- H + A' H W^-1 A; H converges to P.  Lane r owns row r of the
-// controller's matrices in shared memory: At (A0, then the iterates), G, H, the 6 x 18 system [W | A | G] and U = H W^-1 A.  The
-// iteration stops once max|H' - H| <= OBS_DARE_TOL max|H'| (true), or after OBS_DARE_ITERS (false).  Every lane of the warp takes
-// the same number of iterations (a controller that has converged, or is not active, idles through them): the warp synchronises.
-struct DareSmem {
-    double At[36], G[36], H[36], M[6 * 18], U[36], red[6];
-};
-__device__ __forceinline__ bool observer_dare(DareSmem& S, int r, bool active) {
-    bool done = !active, conv = false;
-#pragma unroll 1
-    for (int it = 0; it < OBS_DARE_ITERS; ++it) {
-        if (!__any_sync(0xffffffffu, !done)) break;
-        const bool go = !done;
-        if (go) {   // [W | A | G], row r
-            for (int c = 0; c < 6; ++c) {
-                double w = r == c ? 1.0 : 0.0;
-                for (int k = 0; k < 6; ++k) w += S.G[r * 6 + k] * S.H[k * 6 + c];
-                S.M[r * 18 + c] = w;
-                S.M[r * 18 + 6 + c] = S.At[r * 6 + c];
-                S.M[r * 18 + 12 + c] = S.G[r * 6 + c];
-            }
-        }
-        __syncwarp();
-        int piv[6];
-        gj_solve<18>(S.M, r, go, piv);
-        // X1 = W^-1 A (row k: M[piv[k]][6..11]), X2 = W^-1 G (M[piv[k]][12..17])
-        double An[6], T[6], Gn[6];
-        if (go) {
-            for (int c = 0; c < 6; ++c) {
-                double a = 0.0, t = 0.0, u = 0.0;
-                for (int k = 0; k < 6; ++k) {
-                    a += S.At[r * 6 + k] * S.M[piv[k] * 18 + 6 + c];
-                    t += S.At[r * 6 + k] * S.M[piv[k] * 18 + 12 + c];
-                    u += S.H[r * 6 + k] * S.M[piv[k] * 18 + 6 + c];
-                }
-                An[c] = a; T[c] = t;
-                S.U[r * 6 + c] = u;
-            }
-            for (int c = 0; c < 6; ++c) {
-                double g = S.G[r * 6 + c];
-                for (int k = 0; k < 6; ++k) g += T[k] * S.At[c * 6 + k];
-                Gn[c] = g;
-            }
-        }
-        __syncwarp();
-        double Hn[6], dmax = 0.0, hmax = 0.0;
-        if (go) {
-            for (int c = 0; c < 6; ++c) {
-                double v = S.H[r * 6 + c];
-                for (int k = 0; k < 6; ++k) v += S.At[k * 6 + r] * S.U[k * 6 + c];
-                Hn[c] = v;
-                dmax = fmax(dmax, fabs(v - S.H[r * 6 + c]));
-                hmax = fmax(hmax, fabs(v));
-            }
-        }
-        __syncwarp();
-        if (go) {
-            for (int c = 0; c < 6; ++c) { S.At[r * 6 + c] = An[c]; S.G[r * 6 + c] = Gn[c]; S.H[r * 6 + c] = Hn[c]; }
-            S.red[r] = dmax <= OBS_DARE_TOL * hmax ? 1.0 : 0.0;   // NaN or inf anywhere: not converged
-        }
-        __syncwarp();
-        if (go) {
-            bool all = true;
-            for (int k = 0; k < 6; ++k) all = all && S.red[k] == 1.0;
-            if (all) { done = true; conv = true; }
-        }
-        __syncwarp();
-    }
-    return conv;
-}
-
-// Five controllers per warp, six lanes each (lanes 30, 31 idle); lane r of a controller carries the prior's primal and the tangent
-// of direction e_r through the period (column r of A), then owns row r in the DARE and the gain.  A controller forms a model gain
-// when it is not retired, its observer row is mode 1 with has_pred == 1, its gain row is mode 1 and its prior row is source 1 or
-// 2, and the prior's inputs are finite and its curvature lookups succeed (else observe_kernel sets LMPC_FLAG_OBSERVER_RESET).
-// Every controller that is not retired gets all three [6][6] outputs: NaN where no gain was formed.  Launched only in rollout
-// steps of mode 0 and 1, between the measurement and the observer kernels.
-constexpr int OBS_GAIN_WARPS = 2;                 // warps per block
-constexpr int OBS_GAIN_PER_WARP = 5;
-__global__ void __launch_bounds__(32 * OBS_GAIN_WARPS) observer_gain_kernel(const ObserveArgs a, const ObservePrior m,
-                                                                           const ObserveGain g) {
-    __shared__ DareSmem sm[OBS_GAIN_WARPS * OBS_GAIN_PER_WARP];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int grp = lane / 6, r = lane - grp * 6;
-    const int slot = warp * OBS_GAIN_PER_WARP + min(grp, OBS_GAIN_PER_WARP - 1);
-    const int b = (blockIdx.x * OBS_GAIN_WARPS + warp) * OBS_GAIN_PER_WARP + grp;
-    const bool mine = grp < OBS_GAIN_PER_WARP && b < a.batch && !a.retire.retired(b);
-    DareSmem& S = sm[slot];
-    bool form = mine && a.obs.of(b).mode == 1 && a.has_pred[b] && m.pri.tab && g.gains.of(b).mode == 1 && m.pri.of(b).source != 0;
-    double x[6], d[6];
-    if (form) {                                  // the prior's point and car, as model_prior picks them
-        const lmpc_observer_prior_params& pr = m.pri.of(b);
-        const double* xp = a.xPredPrev + (size_t)b * (a.N + 1) * 6;
-        const double delta = m.OldInput[(size_t)b * 2], acc = m.OldInput[(size_t)b * 2 + 1];
-        bool finite = isfinite(delta) && isfinite(acc);
-        for (int j = 0; j < 6; ++j) {
-            x[j] = xp[j];
-            d[j] = j == r ? 1.0 : 0.0;
-            finite = finite && isfinite(x[j]);
-        }
-        const TrackRec& trk = a.trk.of(b);
-        const int back = x[4] - a.y[(size_t)b * 6 + 4] > trk.TrackLength / 2 ? 1 : 0;
-        const bool plant = pr.source == 2;
-        const lmpc_vehicle_params& v = plant ? m.veh_s.of_before(m.veh, b, back) : pr.vehicle;
-        const lmpc_surface_params* zones = plant && m.surf.tab ? &m.surf_s.of_before(m.surf, b, back) : nullptr;
-        form = finite && sim_period_tangent(v, trk, zones, m.dt, delta, acc, x, d);
-        for (int j = 0; j < 6; ++j) form = form && isfinite(x[j]);
-    }
-    // every lane of a controller takes the same decision
-    const unsigned ok = __ballot_sync(0xffffffffu, form);
-    form = mine && ((ok >> (grp * 6)) & 0x3fu) == 0x3fu;
-    bool fin = true;
-    if (form) {
-        const lmpc_observer_gain_params& gp = g.gains.of(b);
-        for (int c = 0; c < 6; ++c) {
-            S.At[r * 6 + c] = d[c];              // A0 = A': row r is the tangent of direction r
-            S.G[r * 6 + c] = r == c ? 1.0 / gp.r[r] : 0.0;
-            S.H[r * 6 + c] = r == c ? gp.q[r] : 0.0;
-            fin = fin && isfinite(d[c]);
-        }
-    }
-    const unsigned fa = __ballot_sync(0xffffffffu, fin);
-    const bool jac_ok = ((fa >> (grp * 6)) & 0x3fu) == 0x3fu;
-    __syncwarp();
-    const bool conv = observer_dare(S, r, form && jac_ok);
-    // P = (H + H') / 2, then K = P (P + R)^-1 = (S^-1 P)' with S = P + R: the system [S | P]
-    double P[6];
-    if (form && jac_ok) {
-        const lmpc_observer_gain_params& gp = g.gains.of(b);
-        for (int c = 0; c < 6; ++c) P[c] = 0.5 * (S.H[r * 6 + c] + S.H[c * 6 + r]);
-        for (int c = 0; c < 6; ++c) {
-            S.M[r * 12 + c] = r == c ? P[c] + gp.r[r] : P[c];
-            S.M[r * 12 + 6 + c] = P[c];
-        }
-    }
-    __syncwarp();
-    int piv[6];
-    gj_solve<12>(S.M, r, form && jac_ok && conv, piv);
-    if (!mine) return;
-    const double nan = __longlong_as_double(0x7ff8000000000000ll);
-    double* J = g.jac + (size_t)b * 36;
-    double* C = g.cov + (size_t)b * 36;
-    double* K = g.gain + (size_t)b * 36;
-    double Kr[6];
-    bool good = form && jac_ok && conv;
-    for (int c = 0; c < 6; ++c) {
-        Kr[c] = good ? S.M[piv[c] * 12 + 6 + r] : nan;
-        good = good && isfinite(Kr[c]) && isfinite(P[c]);
-    }
-    const unsigned gb = __ballot_sync(__activemask(), good);
-    good = ((gb >> (grp * 6)) & 0x3fu) == 0x3fu;
-    for (int c = 0; c < 6; ++c) {
-        J[c * 6 + r] = form ? d[c] : nan;        // column r of A
-        C[r * 6 + c] = form && jac_ok ? P[c] : nan;
-        K[r * 6 + c] = good ? Kr[c] : nan;
-    }
-}
-
-template <bool MODEL, bool GAIN>
-__global__ void observe_kernel(const ObserveArgs a, const ObservePrior m, const ObserveGain g) {
-    const int b = blockIdx.x * blockDim.x + threadIdx.x;
-    if (b >= a.batch || a.retire.retired(b)) return;
-    const lmpc_observer_params& o = a.obs.of(b);
-    const double* y = a.y + (size_t)b * 6;
-    double* xe = a.x_est + (size_t)b * 6;
-    const bool on = o.mode == 1;
-    if (on && !a.blend) a.has_pred[b] = 0;
-    double yv[6], p[6];
-#pragma unroll
-    for (int j = 0; j < 6; ++j) yv[j] = y[j];
-    bool prior = on && a.blend && a.has_pred[b];
-    bool kal = false;            // GAIN: a mode 1 gain row blends with the model gain K; its fixed gains are not read
-    if constexpr (GAIN) kal = on && g.gains.of(b).mode == 1;
-    if constexpr (MODEL) {       // a row whose gains are all 1 forms no prior
-        bool reads = kal;
-#pragma unroll
-        for (int j = 0; j < 6; ++j) reads = reads || o.gain[j] != 1.0;
-        prior = prior && reads;
-    }
-    const bool formed = prior;
-    if (prior) {
-        bool model = false, ok = true;
-        if constexpr (MODEL) {
-            const lmpc_observer_prior_params& r = m.pri.of(b);
-            model = r.source != 0;
-            if (model) ok = model_prior(a, m, b, r, yv, p);
-        }
-        if (!model) {
-            const double* pp = a.xPredPrev + ((size_t)b * (a.N + 1) + 1) * 6;
-#pragma unroll
-            for (int j = 0; j < 6; ++j) p[j] = pp[j];
-        }
-        wrap_guess_s(p[4], yv[4], a.trk.of(b).TrackLength);
-        bool finite = ok;
-#pragma unroll
-        for (int j = 0; j < 6; ++j) finite = finite && ((!kal && o.gain[j] == 1.0) || isfinite(p[j]));
-        if (!finite) {
-            a.flags[b] |= LMPC_FLAG_OBSERVER_RESET;
-            prior = false;
-        }
-    }
-    if constexpr (MODEL) {
-        double* xq = m.x_prior + (size_t)b * 6;
-#pragma unroll
-        for (int j = 0; j < 6; ++j) xq[j] = formed ? p[j] : __longlong_as_double(0x7ff8000000000000ll);
-    }
-    if constexpr (GAIN) {
-        if (!a.blend) {          // observer_gain_kernel does not run in PID and mode 2 steps: no gain was formed
-            const double nan = __longlong_as_double(0x7ff8000000000000ll);
-            for (int e = 0; e < 36; ++e) {
-                g.jac[(size_t)b * 36 + e] = nan; g.cov[(size_t)b * 36 + e] = nan; g.gain[(size_t)b * 36 + e] = nan;
-            }
-        }
-        if (kal) {               // x_hat_i = p_i + sum_j K_ij (y_j - p_j), left to right, each operation rounded on its own
-            if (prior) {
-                const double* K = g.gain + (size_t)b * 36;
-                bool fin = true;
-                for (int e = 0; e < 36; ++e) fin = fin && isfinite(K[e]);
-                if (!fin) {
-                    a.flags[b] |= LMPC_FLAG_OBSERVER_GAIN;
-                    prior = false;
-                }
-            }
-            double e[6];
-#pragma unroll
-            for (int j = 0; j < 6; ++j) e[j] = prior ? __dsub_rn(yv[j], p[j]) : 0.0;
-#pragma unroll
-            for (int i = 0; i < 6; ++i) {
-                double v = yv[i];
-                if (prior) {
-                    const double* K = g.gain + (size_t)b * 36 + i * 6;
-                    double c = __dmul_rn(K[0], e[0]);
-#pragma unroll
-                    for (int j = 1; j < 6; ++j) c = __dadd_rn(c, __dmul_rn(K[j], e[j]));
-                    v = __dadd_rn(p[i], c);
-                }
-                xe[i] = v;
-            }
-            return;
-        }
-    }
-#pragma unroll
-    for (int j = 0; j < 6; ++j) {
-        const double l = o.gain[j];
-        double v = yv[j];
-        if (prior && l != 1.0) v = l == 0.0 ? p[j] : __dadd_rn(p[j], __dmul_rn(l, __dsub_rn(yv[j], p[j])));
-        xe[j] = v;
-    }
-}
-
-// LTI system identification by ridge regression, Utilities.py:5-28 (Regression): rows t = 1 .. T-2 of the closed-loop
-// record, z_t = [x_t u_t] (8), y_t = x_{t+1} (6); W = (Z'Z + lamb I)^-1 Z'Y; A = W'[:, 0:6], B = W'[:, 6:8].
-// One warp per instance: lane e < 36 owns one entry of the upper triangle of Z'Z, lanes own the 48 entries of Z'Y in two
-// rounds; the 8 x 8 system with 6 right-hand sides is solved by Gaussian elimination with partial pivoting in shared memory.
-// Output abc[b][54] = A (36, row-major) | B (12) | C = 0 (6): the per-instance LTI model in the layout ftocp_kernel reads.
-__global__ void __launch_bounds__(32) ridge_sysid_kernel(int batch, const double* cl_x, const double* cl_u, const int* cl_len, int Tcl,
-                                                         double lamb, double* abc, int* status) {
-    const int b = blockIdx.x;
-    if (b >= batch) return;
-    const int lane = threadIdx.x;
-    __shared__ double S[8][14];      // [Z'Z + lamb I | Z'Y]
-    const int T = cl_len[b];
-    const double* X = cl_x + (size_t)b * Tcl * 6;
-    const double* U = cl_u + (size_t)b * Tcl * 2;
-    auto zval = [&](int t, int j) { return j < 6 ? X[(size_t)t * 6 + j] : U[(size_t)t * 2 + (j - 6)]; };
-    for (int e = lane; e < 36 + 48; e += 32) {
-        int r, c;
-        if (e < 36) { r = 0; int k = e; while (k >= 8 - r) { k -= 8 - r; ++r; } c = k + r; }
-        else { r = (e - 36) / 6; c = 8 + (e - 36) % 6; }
-        double acc = 0.0;
-        for (int t = 1; t <= T - 2; ++t) {
-            const double zr = zval(t, r);
-            const double other = (c < 8) ? zval(t, c) : X[(size_t)(t + 1) * 6 + (c - 8)];
-            acc += zr * other;
-        }
-        if (c < 8) {
-            if (r == c) acc += lamb;
-            S[r][c] = acc; S[c][r] = acc;
-        } else {
-            S[r][c] = acc;
-        }
-    }
-    __syncwarp();
-    bool ok = T >= 12;
-    for (int p = 0; p < 8; ++p) {
-        int piv = p;
-        double best = fabs(S[p][p]);
-        for (int r = p + 1; r < 8; ++r) { const double v = fabs(S[r][p]); if (v > best) { best = v; piv = r; } }
-        if (!(best > 0.0)) ok = false;
-        __syncwarp();
-        if (lane < 14 && piv != p) { const double t = S[p][lane]; S[p][lane] = S[piv][lane]; S[piv][lane] = t; }
-        __syncwarp();
-        const double inv = (S[p][p] != 0.0) ? 1.0 / S[p][p] : 0.0;
-        double f[8];
-#pragma unroll
-        for (int r = 0; r < 8; ++r) f[r] = S[r][p] * inv;
-        const double prow = lane < 14 ? S[p][lane] : 0.0;
-        __syncwarp();
-        if (lane < 14 && lane > p) {
-#pragma unroll
-            for (int r = 0; r < 8; ++r) if (r != p) S[r][lane] -= f[r] * prow;     // Gauss-Jordan: eliminate above and below
-        }
-        __syncwarp();
-    }
-    // W[r][c] = S[r][8 + c] / S[r][r];  A = W'[:, 0:6] -> A[i][j] = W[j][i];  B[i][k] = W[6 + k][i]
-    double* out = abc + (size_t)b * 54;
-    for (int e = lane; e < 54; e += 32) {
-        double v = 0.0;
-        if (e < 36) { const int i = e / 6, j = e % 6; v = S[j][8 + i] / S[j][j]; }
-        else if (e < 48) { const int i = (e - 36) / 2, k = (e - 36) % 2; v = S[6 + k][8 + i] / S[6 + k][6 + k]; }
-        out[e] = v;
-    }
-    if (lane == 0 && !ok) atomicOr(&status[b], 1);
-}
-
-// Seed a controller from the closed-loop record the way main.py:99-110 does from the PID lap: the record is stored `copies`
-// times in the safe set (slots ss_slot0 ..) and in the regression model (slots model_slot0 ..), cost-to-go by computeCost,
-// the controller state from the record (seed_state_block), timeStep = 0, no previous prediction; the record restarts.  One CTA
-// per instance.  With reports the report table starts afresh.
-__global__ void __launch_bounds__(256) seed_from_record_kernel(int batch, LapPool ss, LapPool model, int copies, int ss_slot0, int model_slot0,
-                                                              const double* cl_x, const double* cl_u, int* cl_len, int Tcl, int N,
-                                                              double* xLin, double* uLin, double* zt, double* OldInput, int* timeStep,
-                                                              int* hasPred, int* done, Tracks trk, Shapes shp, LapReports rep) {
-    const int b = blockIdx.x;
-    if (b >= batch) return;
-    const int Trec = cl_len[b];
-    const double TrackLength = trk.of(b).TrackLength;
-    const double* cx = cl_x + (size_t)b * Tcl * 6;
-    const double* cu = cl_u + (size_t)b * Tcl * 2;
-    for (int c = 0; c < copies; ++c) {
-        copy_ss_lap_block(ss, ss.lap_index(b, ss_slot0 + c), cx, cu, Trec, TrackLength);
-        copy_lap_block(model, model.lap_index(b, model_slot0 + c), cx, cu, Trec);
-    }
-    seed_state_block(b, N, shp, cx, cu, xLin, uLin, zt, OldInput);
-    if (threadIdx.x == 0) {
-        timeStep[b] = 0; hasPred[b] = 0; cl_len[b] = 0; done[b] = 0;
-        if (rep.rows) report_restart(rep, b);
-    }
 }
 
 }  // namespace lmpc

@@ -1,4 +1,4 @@
-"""Numpy restatement of the state observer of the device closed loop (observe_kernel in csrc/safeset.cuh; DESIGN.md,
+"""Numpy restatement of the state observer of the device closed loop (observe_kernel in csrc/observer.cuh; DESIGN.md,
 "Per-controller state observers").
 
 For one step of a batch it forms x_hat from the state the controllers are given (y), the previous prediction's row 1 and

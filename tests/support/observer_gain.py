@@ -1,5 +1,5 @@
 """Numpy restatement of the observer's model gains (lmpc_rollout_set_observer_gains; observer_gain_kernel and
-observe_kernel<true, true> in csrc/safeset.cuh; DESIGN.md, "Observer gains"), for tests.
+observe_kernel<true, true> in csrc/observer.cuh; DESIGN.md, "Observer gains"), for tests.
 
   curvature       the device's curvature lookup in fp64 (wrap by subtraction, first segment with s0 <= s < s0 + len)
   zone_forces     a surface row's peak tyre forces at s: fl(mu_f Df), fl(mu_r Dr) in a zone, else Df, Dr

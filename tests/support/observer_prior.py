@@ -1,10 +1,10 @@
-"""Exact restatement of the observer's model prior (lmpc_rollout_set_observer_priors; observe_kernel<true> in csrc/safeset.cuh;
+"""Exact restatement of the observer's model prior (lmpc_rollout_set_observer_priors; observe_kernel<true> in csrc/observer.cuh;
 DESIGN.md, "Observer priors"), for tests.
 
   back_laps      how many laps before lap_n a source 2 prior reads its rows at: 1 when a hand-over came between the previous
                  step and this one (x_hat_{k-1}.s - y.s > TrackLength / 2), else 0
   scheduled_row  the row of a lap schedule [L] at lap lap_n - back, clamped to [0, L - 1]
-  prior_exact    Phi_car(x_prev, u): surface_exact.dyn_model with zero draws and no global frame, its curvilinear state (mpf)
+  prior_exact    Phi_car(x_prev, u): plant_exact.dyn_model with zero draws and no global frame, its curvilinear state (mpf)
   blend          the observer's lap-wrap fix and blend of one controller from a given prior (observer.observe_one)
 
 The device prior runs the simulator's own sub-step code, so with process noise off it equals the plant state bit for bit; against
@@ -15,7 +15,7 @@ from types import SimpleNamespace
 import numpy as np
 
 import observer as ob
-import surface_exact as se
+import plant_exact as pe
 
 NO_NOISE = SimpleNamespace(sim_sigma=(0.0, 0.0, 0.0), sim_clip=(0.0, 0.0, 0.0), sim_gain=0.0)
 
@@ -34,9 +34,9 @@ def scheduled_row(rows, lap_n, back):
 
 def prior_exact(vehicle, track, x_prev, u, dt=0.1, surface=None):
     """The exact noise-free control period of ``vehicle`` (an object with the ten vehicle fields) from the curvilinear state
-    x_prev under u = (delta, a), with ``surface`` (surface_exact.ExactSurface) or none, on ``track`` (plant_exact.ExactTrack).
+    x_prev under u = (delta, a), with ``surface`` (plant_exact.ExactSurface) or none, on ``track`` (plant_exact.ExactTrack).
     Returns the dyn_model result: x (six mpf), margin, failed (a sub-step's lookup failed) and, with a surface, zone_margin."""
-    return se.dyn_model(vehicle, track, x_prev, np.zeros(6), u, z=(0.0, 0.0, 0.0), noise=NO_NOISE, dt=dt, on_fail="zero",
+    return pe.dyn_model(vehicle, track, x_prev, np.zeros(6), u, z=(0.0, 0.0, 0.0), noise=NO_NOISE, dt=dt, on_fail="zero",
                         surface=surface)
 
 

@@ -1,7 +1,7 @@
 """Exact restatement of the plant kernels, for tests: the operations of the reference evaluated in multi-precision arithmetic
 (mpmath, DPS digits) from the fp64 inputs and constants the device actually used, with no rounding in between.
 
-  dyn_model     Simulator.dynModel (SysModel.py:56-147)        sim_step_kernel
+  dyn_model     Simulator.dynModel (SysModel.py:56-147)        sim_step_kernel, with or without a track surface (ExactSurface)
   pid_input     PID.solve (Utilities.py:42-68)                 pid_input_kernel
   regression    Regression (Utilities.py:5-28)                 ridge_sysid_kernel
   compute_cost  LMPC.computeCost (PC.py:447-464)               lap_cost_block (rollout_cost_kernel, lap hand-over, seeding)
@@ -12,7 +12,8 @@ each sub-step (Track.py:292-310) compares the exact s with the track table's fp6
 rounded to fp64, as both the reference and the device form it) and wraps by repeated exact subtraction of the fp64
 TrackLength.  A state a fp64 implementation could place on the other side of a boundary is one whose exact s lies within its
 rounding error of that boundary: ``dyn_model`` reports the smallest distance of any computed sub-step's s to a boundary, so a
-case can check its own margin.
+case can check its own margin.  A track surface (lmpc_rollout_set_surfaces, ExactSurface) sets each sub-step's peak tyre forces
+from the zone its s lies in; ``dyn_model`` reports the distance to a zone bound the same way.
 
 The variants of ``dyn_model`` and ``regression`` (keyword ``variant``) are the known-wrong implementations the tests' bounds
 must reject.
@@ -62,6 +63,32 @@ class ExactTrack:
         raise LookupFailed("s = %s has no segment" % mp.nstr(s, 20))
 
 
+class ExactSurface:
+    """A track-surface row (lmpc_rollout_set_surfaces): zones (s_start, s_end, mu_f, mu_r) as fp64 values.  ``at`` places the
+    exact s of a sub-step against the fp64 bounds, wrapped as ExactTrack.lookup wraps it, and returns the sub-step's peak forces
+    fl(mu_f Df), fl(mu_r Dr) (each product rounded once to fp64, as the device forms it) or Df, Dr exactly off every zone, with the
+    distance of the wrapped s to the nearest zone bound.  ``variant``: "closed_end" (s <= s_end matches), "unwrapped" (the zone
+    tested on the unwrapped s), "front_only" (mu_r ignored)."""
+
+    def __init__(self, zones):
+        self.zones = [tuple(float(v) for v in z) for z in zones]
+        self.bounds = sorted(set(_f(z[0]) for z in self.zones) | set(_f(z[1]) for z in self.zones))
+
+    def at(self, s, L, Df, Dr, variant=""):
+        dist = min((abs(s - b) for b in self.bounds), default=mp.inf) if mp.isfinite(s) else mp.inf
+        if not mp.isfinite(s) or s > 64 * L:
+            return _f(Df), _f(Dr), dist
+        if variant != "unwrapped":
+            while s > L:
+                s = s - L
+            dist = min((abs(s - b) for b in self.bounds), default=mp.inf)
+        for s0, s1, muf, mur in self.zones:
+            if _f(s0) <= s and (s <= _f(s1) if variant == "closed_end" else s < _f(s1)):
+                dr = _f(Dr) if variant == "front_only" else _f(np.float64(mur) * np.float64(Dr))
+                return _f(np.float64(muf) * np.float64(Df)), dr, dist
+        return _f(Df), _f(Dr), dist
+
+
 def _substeps(dt, h=0.001):
     """SysModel.py:83's loop count, in fp64 as the reference and the device evaluate it."""
     i = 0
@@ -70,16 +97,19 @@ def _substeps(dt, h=0.001):
     return i
 
 
-def dyn_model(vehicle, track, x, x_glob, u, z=(0.0, 0.0, 0.0), noise=None, dt=0.1, on_fail="raise", variant=None):
+def dyn_model(vehicle, track, x, x_glob, u, z=(0.0, 0.0, 0.0), noise=None, dt=0.1, on_fail="raise", variant=None, surface=None):
     """One control period of SysModel.py:56-147, exactly.  ``vehicle``: an object with the ten fields above; ``track``: an
-    ExactTrack; ``z``: the three standard-normal draws (vx, vy, wz); ``noise``: an object with sim_sigma, sim_clip, sim_gain
+    ExactTrack; ``surface``: an ExactSurface, whose zone each sub-step's peak tyre forces follow, or None; ``z``: the three
+    standard-normal draws (vx, vy, wz); ``noise``: an object with sim_sigma, sim_clip, sim_gain
     (None: the reference's constants).  ``on_fail``: "raise" (the reference) or "zero" (go on with curvature 0, as the device
     does, and report it).  Returns dict(x, x_glob: lists of 6 mpf, margin: smallest distance of the s of sub-steps 1.. to a
     segment boundary (sub-step 0's s is an fp64 input and is placed exactly by every implementation), failed: bool,
     done: s_next > TrackLength).
     ``variant`` (known-wrong implementations): "alpha_r_lr" (lr in place of lf in alpha_r), "curvature_at_next_s" (the epsi
     update reads the curvature at the updated s), "noise_global" (noise added to the global copy), "substeps_99",
-    "substeps_101"."""
+    "substeps_101"; with a ``surface`` (an ExactSurface) also "mu_at_start" (the zone of sub-step 0 for the whole period),
+    "mu_front_only", "zone_closed_end" and "zone_unwrapped" (ExactSurface's variants).  The result also holds zone_margin: the
+    smallest distance of the s of sub-steps 1.. to a zone bound (inf without a surface)."""
     variant = variant or ""
     with mp.workdps(DPS):
         m, lf, lr, Iz, Df, Cf, Bf, Dr, Cr, Br = (_f(getattr(vehicle, k)) for k in VEHICLE_FIELDS)
@@ -91,6 +121,9 @@ def dyn_model(vehicle, track, x, x_glob, u, z=(0.0, 0.0, 0.0), noise=None, dt=0.
         sd, cd = mp.sin(delta), mp.cos(delta)
         arm_r = lr if variant == "alpha_r_lr" else lf
         margin, failed = mp.inf, False
+        zone_margin = mp.inf
+        zvar = {"mu_front_only": "front_only", "zone_closed_end": "closed_end", "zone_unwrapped": "unwrapped"}.get(variant, "")
+        D0 = None
 
         # IEEE sign of an exactly zero atan2 argument (vy +- lf wz == 0 with vx <= 0: the branch cut at +-pi): taken from the
         # fp64 inputs at sub-step 0, where they can be signed zeros; later sub-steps produce +0
@@ -116,10 +149,19 @@ def dyn_model(vehicle, track, x, x_glob, u, z=(0.0, 0.0, 0.0), noise=None, dt=0.
             return c
 
         for i in range(n):
+            Dfi, Dri = Df, Dr
+            if surface is not None:
+                if variant == "mu_at_start" and D0 is not None:
+                    Dfi, Dri = D0
+                else:
+                    Dfi, Dri, d = surface.at(s, track.L, vehicle.Df, vehicle.Dr, zvar)
+                    D0 = (Dfi, Dri)
+                    if i > 0:
+                        zone_margin = min(zone_margin, d)
             af = delta - atan2(vy + lf * wz, vx, i, 0)
             ar = -atan2(vy - arm_r * wz, vx, i, 1)
-            Fyf = Df * mp.sin(Cf * mp.atan(Bf * af))
-            Fyr = Dr * mp.sin(Cr * mp.atan(Br * ar))
+            Fyf = Dfi * mp.sin(Cf * mp.atan(Bf * af))
+            Fyr = Dri * mp.sin(Cr * mp.atan(Br * ar))
             nvx = vx + h * (acc - 1 / m * Fyf * sd + wz * vy)
             nvy = vy + h * (1 / m * (Fyf * cd + Fyr) - wz * vx)
             nwz = wz + h * (1 / Iz * (lf * Fyf * cd - lr * Fyr))
@@ -145,7 +187,8 @@ def dyn_model(vehicle, track, x, x_glob, u, z=(0.0, 0.0, 0.0), noise=None, dt=0.
         tgt = gs if variant == "noise_global" else xs
         for j in range(3):
             tgt[j] = tgt[j] + gain * draw[j]
-        return dict(x=xs, x_glob=gs, margin=margin, failed=failed, done=bool(s > track.L), draw=[gain * d for d in draw])
+        return dict(x=xs, x_glob=gs, margin=margin, failed=failed, done=bool(s > track.L), draw=[gain * d for d in draw],
+                    zone_margin=zone_margin)
 
 
 def to_f64(v):

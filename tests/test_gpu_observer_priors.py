@@ -305,7 +305,7 @@ def test_prior_is_the_exact_map_and_x_est_its_blend_under_noise():
     idx = np.arange(Bs) % 2
     c = _controller(Bs, obs=gains, oidx=idx, pri=[ObserverPrior.plant()], surf=[WET], meas=(MeasurementParams.scaled(3, BASE),))
     _pid_lap_and_seed(c)
-    sfc = op.se.ExactSurface(WET.zones)
+    sfc = pe.ExactSurface(WET.zones)
     worst, n, resets = 0.0, 0, 0
     for k in range(260):
         hp = _read(c, "has_pred", Bs, np.int32)

@@ -4,7 +4,7 @@ No table, an all-dry table, a 16-zone table with every mu = 1 and a removed tabl
 lap, seeding, three LMPC laps, lap reports, records), also with an all-learned prediction table; under mode 2 a dry row and
 the 16 zones of mu = 1 drive one closed loop.  One zone over the whole lap is the
 vehicle row fl(mu_f Df), fl(mu_r Dr), in the closed loop and for mode 2 against mode 1.  The simulator meets the exact
-restatement (tests/support/surface_exact.py) within SIM_BOUND at zone bounds, per-axle, zero and large mu, across the finish line,
+restatement (tests/support/plant_exact.py, nominal_model.py) within SIM_BOUND at zone bounds, per-axle, zero and large mu, across the finish line,
 at s = TrackLength, s < 0 and a non-finite s; mode 2 rows 0..2 meet its nominal rows within NOMINAL_BOUND, a period
 crossing a zone bound included.  Interleaved rows equal one handle per row (with vehicles and tracks); a surface schedule equals
 host re-installs at every change of entry and drives mode 2 the same way; an identity schedule equals none; the PID lap ignores
@@ -21,7 +21,6 @@ pytestmark = pytest.mark.gpu
 import closed_loop as cl                                           # noqa: E402
 import nominal_model as nm                                         # noqa: E402
 import plant_exact as pe                                           # noqa: E402
-import surface_exact as se                                         # noqa: E402
 from racinglmpc_b200 import reference_params as rp                # noqa: E402
 from racinglmpc_b200 import _native as nat                        # noqa: E402
 from racinglmpc_b200.reference_params import (PredictionModelParams as P, SurfaceParams as S, TrackParams,   # noqa: E402
@@ -188,7 +187,7 @@ def test_simulator_with_zones_meets_the_exact_restatement():
     c.close()
     worst = 0.0
     for b, (name, xb, zones, boundary) in enumerate(SIM_CASES):
-        r = se.dyn_model(CAR, ET, xb, xb, u[b], noise=rp.NoiseParams.scaled(0, 0), on_fail="zero", surface=se.ExactSurface(zones))
+        r = pe.dyn_model(CAR, ET, xb, xb, u[b], noise=rp.NoiseParams.scaled(0, 0), on_fail="zero", surface=pe.ExactSurface(zones))
         e = max(pe.sim_error(st["x"][b], r["x"]), pe.sim_error(st["xglob"][b], r["x_glob"]))
         assert e <= pe.SIM_BOUND, (name, e)
         assert r["zone_margin"] >= 1e-9, (name, float(r["zone_margin"]))      # every case's own margin to the zone bounds
@@ -226,17 +225,17 @@ def test_mode_2_rows_under_a_surface_meet_the_exact_reference():
         rel = float(np.max(np.abs(abc[1] - dry[1]) / (1.0 + np.abs(dry[1]))))
     print("\nmode 2, dry row against no table: max |diff| / (1 + |no table|) = %.3e" % rel)
     assert rel <= nm.NOMINAL_BOUND and np.array_equal(dry[0], dry[1])
-    srf = se.ExactSurface(zones)
+    srf = pe.ExactSurface(zones)
     worst, crossed = 0.0, 0
     for i in range(12):
-        exact = se.rows(CAR, xs[i], us[i], surface=srf, track=ET)
-        crossed += se.phi_sens.zone_margin < 0.2
-        assert se.phi_sens.zone_margin >= 1e-9, i                          # the stage's own margin to the zone bounds
+        exact = nm.rows(CAR, xs[i], us[i], surface=srf, track=ET)
+        crossed += nm.phi_sens.zone_margin < 0.2
+        assert nm.phi_sens.zone_margin >= 1e-9, i                          # the stage's own margin to the zone bounds
         dev = nm.from_abc(abc[0, i])
         worst = max(worst, nm.deviation(dev, exact))
         assert np.all(dev[0][:, 3:] == 0)
         pred = dev[0] @ xs[i] + dev[1] @ us[i] + dev[2]
-        plant = se.dyn_model(CAR, ET, xs[i], [0.0] * 6, us[i], z=(0.0, 0.0, 0.0), on_fail="zero", surface=srf)
+        plant = pe.dyn_model(CAR, ET, xs[i], [0.0] * 6, us[i], z=(0.0, 0.0, 0.0), on_fail="zero", surface=srf)
         with mp.workdps(pe.DPS):
             err = max(float(abs(pe._f(p) - e) / (1 + abs(e))) for p, e in zip(pred, plant["x"][:3]))
         assert err <= nm.NOMINAL_BOUND, (i, err)

@@ -16,7 +16,6 @@ from racinglmpc_b200.reference_params import ObserverGains, VehicleParams
 import observer_gain as og
 import observer_prior as op
 import plant_exact as pe
-import surface_exact as se
 
 B = 8
 T0 = rp.TrackParams.l_shaped()
@@ -170,7 +169,7 @@ def test_tangent_against_central_differences(case):
     x, u, zones = CASES[case]
     if case == "join":
         x = _join_state()
-    surf = se.ExactSurface(zones) if zones else None
+    surf = pe.ExactSurface(zones) if zones else None
     p, A, ok = og.tangent_period(CAR, SEG, L, x, u, zones=zones)
     assert ok
     assert np.max(np.abs(p - _exact(x, u, surf))) <= 1e-12 * max(1.0, np.max(np.abs(p)))

@@ -1,6 +1,6 @@
 """CPU tier: observer priors (lmpc_rollout_set_observer_priors) -- the ABI size and packing of ObserverPriorParams, every refusal
 of make_observer_prior_sets before any native call, ObserverPrior's constructors, and the restatement the GPU tests compare
-against (tests/support/observer_prior.py): with zero draws its prior is surface_exact's plant state (plant_exact's without a
+against (tests/support/observer_prior.py): with zero draws its prior is plant_exact's plant state (with or without a
 surface) on the curvilinear channels, whatever the global frame, and the rule that picks the car and surface of the step before
 a hand-over."""
 import ctypes as C
@@ -15,7 +15,6 @@ from racinglmpc_b200 import reference_params as rp
 from racinglmpc_b200.reference_params import ObserverPrior, VehicleParams
 import observer_prior as op
 import plant_exact as pe
-import surface_exact as se
 
 B = 8
 T0 = rp.TrackParams.l_shaped()
@@ -100,11 +99,11 @@ def test_prior_without_surface_is_plant_exact_with_zero_draws(k):
 
 
 @pytest.mark.parametrize("k", range(len(STATES)))
-def test_prior_with_surface_is_surface_exact_with_zero_draws(k):
+def test_prior_with_surface_is_plant_exact_with_zero_draws(k):
     x, u = STATES[k], INPUTS[k]
-    surf = se.ExactSurface([(0.0, 2.0, 0.6, 0.5), (3.5, 5.0, 1.1, 0.9), (6.0, L, 0.4, 0.4)])
+    surf = pe.ExactSurface([(0.0, 2.0, 0.6, 0.5), (3.5, 5.0, 1.1, 0.9), (6.0, L, 0.4, 0.4)])
     got = op.prior_exact(CAR, TRACK, x, u, surface=surf)
-    ref = se.dyn_model(CAR, TRACK, x, np.array([0.0, 0.0, 0.0, -0.7, 2.0, 1.0]), u, z=(0.0, 0.0, 0.0), on_fail="zero",
+    ref = pe.dyn_model(CAR, TRACK, x, np.array([0.0, 0.0, 0.0, -0.7, 2.0, 1.0]), u, z=(0.0, 0.0, 0.0), on_fail="zero",
                        surface=surf)
     assert all(a == b for a, b in zip(got["x"], ref["x"]))
     plain = op.prior_exact(CAR, TRACK, x, u)

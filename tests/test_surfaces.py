@@ -1,7 +1,6 @@
 """CPU tier: track surfaces (lmpc_rollout_set_surfaces) -- the ABI record and its packing, every refusal of make_surface_sets,
-BatchedController and rollout_mc.run before any native call or device work, the surface rule of tests/support/surface_exact.py
-(without a surface it is plant_exact's plant and nominal_model's rows exactly; identities, sensitivities against numerical
-differentiation of the exact plant), and the simulator bound rejecting every known-wrong surface variant."""
+BatchedController and rollout_mc.run before any native call or device work, the surface rule of the exact plant and nominal model
+(tests/support/plant_exact.py, nominal_model.py: identities, sensitivities against numerical differentiation of the exact plant), and the simulator bound rejecting every known-wrong surface variant."""
 import ctypes as C
 import math
 import os
@@ -18,7 +17,6 @@ from racinglmpc_b200.controller import BatchedController
 from racinglmpc_b200.reference_params import SurfaceParams, VehicleParams
 import nominal_model as nm
 import plant_exact as pe
-import surface_exact as se
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "benchmarks"))
@@ -169,45 +167,33 @@ U0 = [0.1, 0.5]
 
 
 def _step(x, u=U0, surface=None, vehicle=CAR, variant=None):
-    return se.dyn_model(vehicle, TRACK, x, [0.0] * 6, u, dt=0.1, on_fail="zero", variant=variant, surface=surface)
+    return pe.dyn_model(vehicle, TRACK, x, [0.0] * 6, u, dt=0.1, on_fail="zero", variant=variant, surface=surface)
 
 
 def _eq(a, b):
     return all(p == q or (mp.isnan(p) and mp.isnan(q)) for p, q in zip(a["x"] + a["x_glob"], b["x"] + b["x_glob"]))
 
 
-@pytest.mark.parametrize("variant", [None, "alpha_r_lr", "curvature_at_next_s", "noise_global", "substeps_99"])
-def test_without_a_surface_the_restatement_is_plant_exact_and_nominal_model(variant):
-    for x in (X0, [1.0, 0.0, 0.0, 0.0, L - 0.05, 0.0], [0.8, 0.1, 0.2, 0.0, -0.01, 0.0]):
-        a = pe.dyn_model(CAR, TRACK, x, [0.0, 0.0, 0.0, 0.3, 1.0, -2.0], U0, z=(0.3, -1.2, 0.7), on_fail="zero", variant=variant)
-        b = se.dyn_model(CAR, TRACK, x, [0.0, 0.0, 0.0, 0.3, 1.0, -2.0], U0, z=(0.3, -1.2, 0.7), on_fail="zero", variant=variant)
-        assert _eq(a, b) and a["margin"] == b["margin"] and a["failed"] == b["failed"] and a["done"] == b["done"]
-    for v in (None,) + nm.VARIANTS:
-        got, want = se.rows(CAR, X0, U0, variant=v), nm.rows(CAR, X0, U0, variant=v)
-        assert all(p == q for g, w in zip(got, want) for gr, wr in zip(g, w) for p, q in zip(gr if isinstance(gr, list) else [gr],
-                                                                                             wr if isinstance(wr, list) else [wr]))
-
-
 def test_neutral_surfaces_are_the_plant_exactly():
-    ones = se.ExactSurface([(k, k + 0.9, 1.0, 1.0) for k in range(16)])
+    ones = pe.ExactSurface([(k, k + 0.9, 1.0, 1.0) for k in range(16)])
     for x in (X0, [1.0, 0.0, 0.0, 0.0, L - 0.05, 0.0], [0.8, 0.1, 0.2, 0.0, -0.01, 0.0]):
         ref = _step(x)
-        assert _eq(_step(x, surface=se.ExactSurface([])), ref)
+        assert _eq(_step(x, surface=pe.ExactSurface([])), ref)
         assert _eq(_step(x, surface=ones), ref)
 
 
 def test_one_zone_over_the_lap_is_the_scaled_vehicle_exactly():
     for muf, mur in ((0.75, 0.6), (0.0, 1.3), (1.0, 0.0)):
-        whole = se.ExactSurface([(0.0, 2 * L, muf, mur)])
+        whole = pe.ExactSurface([(0.0, 2 * L, muf, mur)])
         car = VehicleParams(CAR.m, CAR.lf, CAR.lr, CAR.Iz, muf * CAR.Df, CAR.Cf, CAR.Bf, mur * CAR.Dr, CAR.Cr, CAR.Br)
         for x in (X0, [1.0, 0.0, 0.0, 0.0, L - 0.05, 0.0]):                    # the second crosses the finish line
             assert _eq(_step(x, surface=whole), _step(x, vehicle=car))
 
 
 def test_zone_margin_and_dry_fallbacks():
-    r = _step(X0, surface=se.ExactSurface(WET.zones))
+    r = _step(X0, surface=pe.ExactSurface(WET.zones))
     assert 0 < r["zone_margin"] < 0.2                                      # 4.0 is crossed inside the period
-    wet = se.ExactSurface([(0.0, 2 * L, 0.5, 0.5)])
+    wet = pe.ExactSurface([(0.0, 2 * L, 0.5, 0.5)])
     for s in (math.nan, math.inf, 65 * L):                                 # not finite or beyond 64 laps: dry, as the device
         assert _eq(_step([1.0, 0.0, 0.1, 0.0, s, 0.0], surface=wet), _step([1.0, 0.0, 0.1, 0.0, s, 0.0]))
     assert not _eq(_step([1.0, 0.0, 0.1, 0.0, 40 * L + 1.0, 0.0], surface=wet), _step([1.0, 0.0, 0.1, 0.0, 40 * L + 1.0, 0.0]))
@@ -223,7 +209,7 @@ VARIANT_CASES = [
 
 @pytest.mark.parametrize("variant, zones, x", VARIANT_CASES)
 def test_every_known_wrong_variant_is_outside_the_bound(variant, zones, x):
-    srf = se.ExactSurface(zones)
+    srf = pe.ExactSurface(zones)
     exact = _step(x, surface=srf)
     wrong = _step(x, surface=srf, variant=variant)
     assert pe.sim_error(pe.to_f64(wrong["x"]), exact["x"]) > 1e3 * pe.SIM_BOUND
@@ -239,21 +225,21 @@ def _f64(rows):
 
 @pytest.mark.parametrize("x", [[1.3, 0.12, 0.6, 0.05, 3.0, 0.1], [2.0, -0.05, -0.4, 0.0, 10.0, -0.2]])
 def test_nominal_sensitivities_under_a_surface_equal_numerical_differentiation(x):
-    srf = se.ExactSurface(WET.zones)
-    phi, S = se.phi_sens(CAR, x, U0, surface=srf, track=TRACK)
-    assert se.phi_sens.zone_margin > 0.5                                   # no bound within the period
-    phn, Sn = se.numdiff(CAR, x, U0, surface=srf, track=TRACK)
+    srf = pe.ExactSurface(WET.zones)
+    phi, S = nm.phi_sens(CAR, x, U0, surface=srf, track=TRACK)
+    assert nm.phi_sens.zone_margin > 0.5                                   # no bound within the period
+    phn, Sn = nm.numdiff(CAR, x, U0, surface=srf, track=TRACK)
     assert max(abs(float(a - b)) for a, b in zip(phi, phn)) < 1e-50
     err = max(abs(float(S[r][c] - Sn[r][c])) / (1 + abs(float(S[r][c]))) for r in range(3) for c in range(5))
     assert err < 1e-15, err
     # and the surface is felt: the same state dry gives other rows
-    assert nm.deviation(_f64(se.rows(CAR, x, U0)), se.rows(CAR, x, U0, surface=srf, track=TRACK)) > 1e3 * nm.NOMINAL_BOUND
+    assert nm.deviation(_f64(nm.rows(CAR, x, U0)), nm.rows(CAR, x, U0, surface=srf, track=TRACK)) > 1e3 * nm.NOMINAL_BOUND
 
 
 def test_nominal_phi_across_a_zone_bound_is_the_plant_step():
-    srf = se.ExactSurface(WET.zones)
-    phi, _ = se.phi_sens(CAR, X0, U0, surface=srf, track=TRACK)
-    assert 0 < se.phi_sens.zone_margin < 0.2
+    srf = pe.ExactSurface(WET.zones)
+    phi, _ = nm.phi_sens(CAR, X0, U0, surface=srf, track=TRACK)
+    assert 0 < nm.phi_sens.zone_margin < 0.2
     plant = _step(X0, surface=srf)
     with mp.workdps(pe.DPS):
         assert max(abs(a - b) for a, b in zip(phi, plant["x"][:3])) < mp.mpf(10) ** -50
@@ -262,6 +248,6 @@ def test_nominal_phi_across_a_zone_bound_is_the_plant_step():
 def test_nominal_one_zone_over_the_lap_is_the_scaled_vehicle():
     muf, mur = 0.75, 0.6
     car = VehicleParams(CAR.m, CAR.lf, CAR.lr, CAR.Iz, muf * CAR.Df, CAR.Cf, CAR.Bf, mur * CAR.Dr, CAR.Cr, CAR.Br)
-    got = se.rows(CAR, X0, U0, surface=se.ExactSurface([(0.0, 2 * L, muf, mur)]), track=TRACK)
-    want = se.rows(car, X0, U0)
+    got = nm.rows(CAR, X0, U0, surface=pe.ExactSurface([(0.0, 2 * L, muf, mur)]), track=TRACK)
+    want = nm.rows(car, X0, U0)
     assert nm.deviation(_f64(got), want) <= 2.0 ** -52

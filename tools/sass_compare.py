@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""tools/sass_compare.py OLD NEW — compare the SASS of the QP kernels of two builds (cubins or liblmpc_b200.so).
+"""tools/sass_compare.py OLD NEW — compare the SASS of every kernel of two builds (cubins or liblmpc_b200.so).
 
 Kernels are matched by variant and (N, M) across their old and new names:
   uniform  ftocp_kernel<N, M, 2, 4>  or  ftocp_kernel<N, M, 2, 4, false>
@@ -17,6 +17,8 @@ to five `false` flags, so that the instantiation without a per-controller table 
            table (later builds have no such kernel: their sim_step_kernel<true> is the surface instantiation)
   surface  sim_step_kernel<true> and nominal_model_kernel<true>: the surface instantiations (builds with track surfaces)
   prior    observe_kernel<true, false> or <true>: an observer prior table without a gain table (builds with observer priors)
+  exact    every other kernel (observer_gain_kernel, observe_kernel<true, true>, K1's shaped and nominal instantiations, ...),
+           matched by its exact demangled name
 and compared by instruction text (cuobjdump -sass without addresses and encodings).  Each differing line pair is classified:
   dfma-swap   one DFMA with its two factors exchanged (a*b+c = b*a+c)
   lds-swap    LDS.128 loads of unchanged addresses whose destination registers are permuted among themselves
@@ -66,6 +68,8 @@ def kernels(path):
                 cur = out.setdefault(("surface", sf.group(1), 0), [])
             elif pr:
                 cur = out.setdefault(("prior", pr.group(1), 0), [])
+            else:
+                cur = out.setdefault(("exact", name, 0), [])
             continue
         m = re.match(r"\s+/\*[0-9a-f]{4,}\*/\s+(.*?)\s*;", line)
         if m and cur is not None:
@@ -111,7 +115,7 @@ def main(old, new):
     totals = collections.defaultdict(collections.Counter)
     for key in sorted(set(ko) | set(kn)):
         variant, n, m = key
-        label = ("%-24s" % n) if variant in ("default", "reports", "surface", "prior") else "<%2d,%2d>" % (n, m)
+        label = ("%-24s" % n) if variant in ("default", "reports", "surface", "prior", "exact") else "<%2d,%2d>" % (n, m)
         if key not in ko or key not in kn:
             print("%-7s %s  only in %s" % (variant, label, "new" if key in kn else "old"))
             totals[variant]["unmatched"] += 1
